@@ -74,16 +74,24 @@ __device__ __forceinline__ int az_bins_for(int nrings, int tab) {
   return tab / p2;
 }
 
+// Counting-sort counters / cursors, two 16-bit halves per 32-bit word (bucket b = half b & 1 of word b >> 1): every count
+// and every cursor is at most T < 65536, so a half never carries into its neighbour.  Half the scratch of 32-bit counters
+// keeps a CTA's shared memory under the 196 KB carve-out, which leaves the SM twice the L1 (see lins_kernels.cuh, CtaMem).
+__device__ __forceinline__ int cnt16_add1(unsigned* cnt, int b) {  // atomic ++ of half b; returns its old value
+  const int sh = (b & 1) * 16;
+  return (int)((atomicAdd(&cnt[b >> 1], 1u << sh) >> sh) & 0xffffu);
+}
 // counting sort of `src` (ring-sorted, rings validated by check_ring_sorted, T < 65536) into dst; bucket starts ->
-// table[0..TAB].  cnt (TAB + 1 ints) and scan_tmp (kThreads ints) are CTA scratch.  Block-wide.
+// table[0..TAB].  cnt (TAB / 2 + 1 packed words, cnt16_add1) and scan_tmp (kThreads ints) are CTA scratch.  Block-wide.
 template <int TAB>
-__device__ void az_build(const float4* __restrict__ src, int T, float4* dst, aztab_t* table, int* cnt, int* scan_tmp, int nb, int (*elev)[2]) {
-  for (int b = threadIdx.x; b <= TAB; b += kThreads) cnt[b] = 0;
+__device__ void az_build(const float4* __restrict__ src, int T, float4* dst, aztab_t* table, unsigned* cnt, int* scan_tmp, int nb, int (*elev)[2]) {
+  unsigned short* cnt16 = reinterpret_cast<unsigned short*>(cnt);  // (plain reads / writes of the halves between barriers)
+  for (int w = threadIdx.x; w <= TAB / 2; w += kThreads) cnt[w] = 0u;
   for (int r = threadIdx.x; r < kMaxRing; r += kThreads) { elev[r][0] = float_key(3.0e38f); elev[r][1] = float_key(-3.0e38f); }
   __syncthreads();
   for (int j = threadIdx.x; j < T; j += kThreads) {
     const float4 t = __ldg(&src[j]);
-    atomicAdd(&cnt[(int)t.w * nb + az_bin(t.x, t.y, nb)], 1);
+    cnt16_add1(cnt, (int)t.w * nb + az_bin(t.x, t.y, nb));
     const float e = slope_of(t.x, t.y, t.z);
     if (fabsf(e) < 1.0e30f) { const int k = float_key(e); atomicMin(&elev[(int)t.w][0], k); atomicMax(&elev[(int)t.w][1], k); }
     else { atomicMin(&elev[(int)t.w][0], float_key(-3.0e38f)); atomicMax(&elev[(int)t.w][1], float_key(3.0e38f)); }  // (on the z axis / NaN: never skip its ring)
@@ -94,7 +102,7 @@ __device__ void az_build(const float4* __restrict__ src, int T, float4* dst, azt
   int loc[PER];
   int sum = 0;
 #pragma unroll
-  for (int k = 0; k < PER; ++k) { loc[k] = cnt[threadIdx.x * PER + k]; sum += loc[k]; }
+  for (int k = 0; k < PER; ++k) { loc[k] = cnt16[threadIdx.x * PER + k]; sum += loc[k]; }
   scan_tmp[threadIdx.x] = sum;
   __syncthreads();
   if (threadIdx.x < 32) {
@@ -115,12 +123,12 @@ __device__ void az_build(const float4* __restrict__ src, int T, float4* dst, azt
   {
     int run = scan_tmp[threadIdx.x];
 #pragma unroll
-    for (int k = 0; k < PER; ++k) { cnt[threadIdx.x * PER + k] = run; table[threadIdx.x * PER + k] = (aztab_t)run; run += loc[k]; }
+    for (int k = 0; k < PER; ++k) { cnt16[threadIdx.x * PER + k] = (unsigned short)run; table[threadIdx.x * PER + k] = (aztab_t)run; run += loc[k]; }
   }
   __syncthreads();
   for (int j = threadIdx.x; j < T; j += kThreads) {  // scatter; the counters are the cursors now
     const float4 t = __ldg(&src[j]);
-    const int pos = atomicAdd(&cnt[(int)t.w * nb + az_bin(t.x, t.y, nb)], 1);
+    const int pos = cnt16_add1(cnt, (int)t.w * nb + az_bin(t.x, t.y, nb));
     dst[pos] = make_float4(t.x, t.y, t.z, __int_as_float(((int)t.w << 24) | j));  // ring (7 bits) | original index (24 bits)
   }
   __syncthreads();

@@ -5,14 +5,7 @@ minimum.  numpy's float32 arctan2 / arcsin differ from CUDA's by an ulp or two; 
 bin on each side for exactly that, so the property has to hold with either library."""
 import numpy as np
 
-F = np.float32
-PI = F(3.14159265358979)
-
-
-def az_bin(x, y, nb):
-    a = np.arctan2(y.astype(F), x.astype(F)).astype(F)
-    b = np.floor((a + PI) * (F(nb) * (F(0.5) / PI))).astype(np.int64)
-    return np.clip(b, 0, nb - 1)
+from scenes import PI, F, az_bin
 
 
 def az_halfwidth(U, rho):

@@ -10,108 +10,14 @@ pruning (lins_assoc_az.cuh) could get wrong and the synthetic benchmark data nev
   * random small scenes: any ring count, tiny / empty clouds, queries far outside the map.
 Reference: lins/include/StateEstimator.hpp:844-915, :970-1029 (search + walks), :465-600 (loop).
 """
-import concurrent.futures as cf
 import os
 
 import numpy as np
 import pytest
 
+from scenes import STATE_TOL, batch_from_units, compare_units, gpu_batch_run, mutate, oracle_runs, random_scene
+
 pytestmark = pytest.mark.gpu
-
-STATE_TOL = 1e-7
-
-
-def _batch_from_units(defs, units):
-    clouds, offsets = {}, {}
-    for k in defs.Batch.FIELDS:
-        parts = [u[k] for u in units]
-        clouds[k] = np.concatenate(parts) if parts else np.zeros(0, defs.POINT_DTYPE)
-        offsets[k] = np.concatenate([[0], np.cumsum([len(p) for p in parts])]).astype(np.int32)
-    return defs.Batch(clouds, offsets, np.stack([u["state"] for u in units]), np.stack([u["cov"] for u in units]))
-
-
-def _dup_targets(rng, cloud, frac):
-    """Insert exact copies of a fraction of the points right after the original (keeps the ring order)."""
-    n = len(cloud)
-    if n == 0:
-        return cloud
-    pick = np.sort(rng.choice(n, size=max(1, int(frac * n)), replace=False))
-    reps = np.ones(n, int)
-    reps[pick] += rng.integers(1, 3, len(pick))
-    return np.repeat(cloud, reps)
-
-
-def _mutate(rng, u, kind):
-    u = {k: (v.copy() if hasattr(v, "copy") else v) for k, v in u.items()}
-    if kind == "dup":
-        u["surf_less_flat"] = _dup_targets(rng, u["surf_less_flat"], 0.15)
-        u["corner_less_sharp"] = _dup_targets(rng, u["corner_less_sharp"], 0.3)
-    elif kind == "axis":  # queries at rho < 0.1 m and a few targets near the axis too
-        for k in ("surf_flat", "corner_sharp"):
-            q = u[k]
-            m = rng.random(len(q)) < 0.08
-            q["x"][m] = rng.uniform(-0.05, 0.05, m.sum()).astype(np.float32)
-            q["y"][m] = rng.uniform(-0.05, 0.05, m.sum()).astype(np.float32)
-            q["z"][m] = rng.uniform(-2.0, 2.0, m.sum()).astype(np.float32)
-        t = u["surf_less_flat"]
-        m = rng.random(len(t)) < 0.01
-        t["x"][m] = rng.uniform(-0.08, 0.08, m.sum()).astype(np.float32)
-        t["y"][m] = rng.uniform(-0.08, 0.08, m.sum()).astype(np.float32)
-    elif kind == "jump":  # prior 1-4 m / up to 0.1 rad off with a covariance that lets the update move that far
-        st = u["state"]
-        st[0:3] += rng.normal(0, 1.0, 3) * rng.uniform(1.0, 4.0)
-        ax = rng.normal(0, 0.03, 3)
-        th = np.linalg.norm(ax)
-        dq = np.r_[ax / th * np.sin(th / 2), np.cos(th / 2)]
-        x1, y1, z1, w1 = st[6:10]
-        x2, y2, z2, w2 = dq
-        st[6:10] = [w1 * x2 + x1 * w2 + y1 * z2 - z1 * y2, w1 * y2 - x1 * z2 + y1 * w2 + z1 * x2,
-                    w1 * z2 + x1 * y2 - y1 * x2 + z1 * w2, w1 * w2 - x1 * x2 - y1 * y2 - z1 * z2]
-        P = u["cov"].reshape(18, 18)
-        P[np.arange(3), np.arange(3)] += 4.0
-        P[np.arange(6, 9), np.arange(6, 9)] += 0.01
-    return u
-
-
-def _random_scene(rng, defs):
-    """A small random unit: ring-sorted targets on 1..40 rings (sometimes empty / tiny), queries near and far."""
-    nr = int(rng.integers(1, 41))
-
-    def cloud(n, spread):
-        ring = np.sort(rng.integers(0, nr, n))
-        az = rng.uniform(-np.pi, np.pi, n)
-        rho = rng.uniform(0.5, 30.0, n) * spread
-        xyz = np.stack([rho * np.cos(az), rho * np.sin(az), rng.uniform(-2, 2, n)], 1)
-        if n and rng.random() < 0.5:  # quantised coordinates: plenty of exact distance ties
-            xyz = np.round(xyz * 4) / 4
-        return defs.make_points(xyz, ring + 0.1 * rng.random(n) * 0.999)
-
-    ts = cloud(int(rng.choice([0, 3, 25, 300, 1500])), 1.0)
-    tc = cloud(int(rng.choice([0, 2, 6, 80, 400])), 1.0)
-
-    def queries(n, tgt):
-        if n == 0 or len(tgt) == 0:
-            return cloud(n, 1.0)
-        pick = tgt[rng.integers(0, len(tgt), n)].copy()
-        for ax in ("x", "y", "z"):
-            pick[ax] += rng.normal(0, 0.3, n).astype(np.float32)
-        far = rng.random(n) < 0.1
-        pick["x"][far] += 60.0
-        pick["intensity"] = (np.floor(pick["intensity"]) + 0.1 * rng.random(n) * 0.999).astype(np.float32)
-        return pick
-
-    qs = queries(int(rng.choice([0, 1, 40, 200])), ts)
-    qc = queries(int(rng.choice([0, 1, 20, 90])), tc)
-    st = np.zeros(19)
-    st[0:3] = rng.normal(0, 0.2, 3)
-    ax = rng.normal(0, 0.01, 3)
-    th = np.linalg.norm(ax)
-    st[6:9] = ax / th * np.sin(th / 2)
-    st[9] = np.cos(th / 2)
-    st[18] = -9.81
-    A = rng.normal(0, 1, (18, 18))
-    cov = (A @ A.T) * 1e-4 + np.diag(np.r_[np.full(3, 0.05), np.full(3, 0.01), np.full(3, 1e-3), np.full(9, 1e-4)])
-    return dict(surf_flat=qs, corner_sharp=qc, surf_less_flat=ts, corner_less_sharp=tc, state=st, cov=cov.T.reshape(-1))
 
 
 def test_fuzz_2000_units_against_bruteforce_oracle(gpu, ob, synth, defs):
@@ -122,77 +28,25 @@ def test_fuzz_2000_units_against_bruteforce_oracle(gpu, ob, synth, defs):
     units = []
     for i in range(base.n):
         u = base.unit(i)
-        units.append(_mutate(rng, u, "none"))
-        units.append(_mutate(rng, u, "dup"))
-        units.append(_mutate(rng, u, "axis"))
-        units.append(_mutate(rng, u, "jump"))
+        units.append(mutate(rng, u, "none"))
+        units.append(mutate(rng, u, "dup"))
+        units.append(mutate(rng, u, "axis"))
+        units.append(mutate(rng, u, "jump"))
     for _ in range(600):
-        units.append(_random_scene(rng, defs))
+        units.append(random_scene(rng, defs))
     assert len(units) >= 2000
-    batch = _batch_from_units(defs, units)
+    batch = batch_from_units(defs, units)
 
-    gpu.batch_upload(batch)
-    gpu.batch_run()
-    sg, cg, rg, reps = gpu.batch_download(states=True, covs=True, reports=True)
-    si, ci = gpu.batch_download_indices(batch)
+    g = gpu_batch_run(gpu, batch)
+    outs = oracle_runs(ob, prm, units, use_kdtree=False)  # brute-force exact 1-NN, lowest index among ties
 
-    def run_oracle(i):
-        u = units[i]
-        o = ob.Oracle(prm, use_kdtree=False)  # brute-force exact 1-NN, lowest index among ties
-        o.set_map(u["surf_less_flat"], u["corner_less_sharp"])
-        so, co, rep, tr = o.ieskf_trace(u["surf_flat"], u["corner_sharp"], u["state"], u["cov"])
-        out = dict(state=so, iters=rep.iters, flags=(rep.converged | (rep.diverged << 1) | (rep.has_nan << 2)),
-                   m_surf=list(rep.m_surf[: rep.iters]), m_corner=list(rep.m_corner[: rep.iters]),
-                   rnorm=np.array(rep.residual_norm[: rep.iters]),
-                   surf_ind=tr["surf_ind"][-1] if rep.iters else None, corner_ind=tr["corner_ind"][-1] if rep.iters else None)
-        o.close()
-        return out
+    def tag_of(i):
+        return f"unit {i} (kind {['none', 'dup', 'axis', 'jump'][i % 4] if i < 4 * base.n else 'random'})"
 
-    with cf.ThreadPoolExecutor(max_workers=min(32, os.cpu_count() or 4)) as ex:
-        outs = list(ex.map(run_oracle, range(len(units))))
-
-    so_off, co_off = batch.offsets["surf_flat"], batch.offsets["corner_sharp"]
-    n_div = n_jump = 0
-    worst = worst_nc = 0.0
-    bad = []
-    for i, o in enumerate(outs):
-        tag = f"unit {i} (kind {['none', 'dup', 'axis', 'jump'][i % 4] if i < 4 * base.n else 'random'})"
-        r = reps[i]
-        n_it = o["iters"]
-        if int(rg["iters"][i]) != n_it or int(rg["flags"][i]) != o["flags"]:
-            bad.append((tag, "iters / flags", int(rg["iters"][i]), n_it, int(rg["flags"][i]), o["flags"]))
-            continue
-        if list(r.m_surf[:n_it]) != o["m_surf"] or list(r.m_corner[:n_it]) != o["m_corner"]:
-            bad.append((tag, "accepted-measurement counts"))
-            continue
-        # residual norms: equal to f64 summation order while the iteration is contracting; a unit that never converges
-        # (random scenes, 30 iterations) amplifies the 1e-15 differences of the f64 algebra from pass to pass
-        rn_g, rn_o = np.array(r.residual_norm[:n_it]), o["rnorm"]
-        if not (np.allclose(rn_g[:3], rn_o[:3], rtol=1e-9, atol=1e-300, equal_nan=True) and np.allclose(rn_g, rn_o, rtol=1e-6, atol=1e-300, equal_nan=True)):
-            bad.append((tag, "residual norms", float(np.nanmax(np.abs(rn_g - rn_o) / np.maximum(np.abs(rn_o), 1e-300)))))
-            continue
-        if n_it and not (np.array_equal(si[so_off[i] : so_off[i + 1]], o["surf_ind"]) and np.array_equal(ci[co_off[i] : co_off[i + 1]], o["corner_ind"])):
-            bad.append((tag, "correspondence IDs of the last iteration"))
-            continue
-        if o["flags"] & 2:
-            n_div += 1
-            if not np.allclose(sg[i], units[i]["state"], equal_nan=True):
-                bad.append((tag, "diverged unit must return the prior"))
-        else:
-            d = float(np.abs(sg[i] - o["state"]).max())
-            conv = bool(o["flags"] & 1)
-            if conv:
-                worst = max(worst, d)
-            else:
-                worst_nc = max(worst_nc, d)
-            if d > (STATE_TOL if conv else 1e-5):  # (north_star: 1e-4)
-                bad.append((tag, "state", d, "converged" if conv else "not converged"))
-        un = np.array(r.update_norm[:n_it])
-        if len(un) and un.max() > 1.0:
-            n_jump += 1
-    print(f"fuzz: {len(units)} units, {n_div} diverged, {n_jump} with a > 1 m / rad update, worst state diff {worst:.3g} (converged) {worst_nc:.3g} (30 iterations, not converged)")
+    bad, st = compare_units(units, outs, g, batch, tag_of, STATE_TOL)
+    print(f"fuzz: {len(units)} units, {st['n_div']} diverged, {st['n_jump']} with a > 1 m / rad update, worst state diff {st['worst']:.3g} (converged) {st['worst_nc']:.3g} (30 iterations, not converged)")
     assert not bad, (len(bad), bad[:10])
-    assert n_jump >= 100, n_jump  # the stress really happened
+    assert st["n_jump"] >= 100, st["n_jump"]  # the stress really happened
 
 
 def test_associate_reuses_indices_across_calls_icp_freq2(gpu, ob, golden_batch):

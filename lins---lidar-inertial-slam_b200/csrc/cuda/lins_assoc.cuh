@@ -338,6 +338,7 @@ __device__ void association_pass(CtaMem& cta, Smem* slots, const BatchView& bv, 
 
   // ---- A5/A6 residuals + A7-A9 fold ------------------------------------------------------------------------------
   // tripod points: slots of the sorted copies after a fast-path search, otherwise original indices into the walk clouds.
+  double* const fold_stage = cta.u.fold[warp];
   for (int v0 = warp * 32; v0 < NQ; v0 += kThreads) {
     const int sl = slot_of(v0, Q), i0 = v0 - sl * Q;
     const Smem& sm = slots[sl];
@@ -372,11 +373,10 @@ __device__ void association_pass(CtaMem& cta, Smem* slots, const BatchView& bv, 
       if (MODE == MODE_ICP_REDUCE) jacobian_row_icp(pb.qpt[v], coeff, sm.phi, kp.scan_period, g, r);
       else jacobian_row(pb.qpt[v], coeff, sm.R, kp.lidar_scale, g, r);
     }
-    const double tot = warp_fold_row(g, r);
-    const unsigned mS = __ballot_sync(0xffffffffu, ok && surf), mC = __ballot_sync(0xffffffffu, ok && !surf);
     const int vw = sl * pb.nvw + (i0 >> 5);
-    if (lane < kNAcc) pb.wacc[vw * kNAcc + lane] = tot;
-    else if (lane == kNAcc) pb.wcnt[vw * 2] = __popc(mS);
+    warp_fold_mma(g, r, fold_stage, pb.wacc + vw * kNAcc);
+    const unsigned mS = __ballot_sync(0xffffffffu, ok && surf), mC = __ballot_sync(0xffffffffu, ok && !surf);
+    if (lane == kNAcc) pb.wcnt[vw * 2] = __popc(mS);
     else if (lane == kNAcc + 1) pb.wcnt[vw * 2 + 1] = __popc(mC);
     if (MODE == MODE_ASSOC && valid) {
       if (surf) {

@@ -30,9 +30,6 @@ constexpr int kJacRow = 12;             // doubles per staged row (8 used): 96-B
 #define LINS_JAC_MIN_CTAS 2
 #endif
 
-__device__ __forceinline__ void dmma_8x8x4(double& c0, double& c1, double a, double b) {
-  asm volatile("mma.sync.aligned.m8n8k4.row.col.f64.f64.f64.f64 {%0,%1}, {%2}, {%3}, {%0,%1};" : "+d"(c0), "+d"(c1) : "d"(a), "d"(b));
-}
 // sin / cos of a small angle (|x| < 0.125) to better than one ulp
 __device__ __forceinline__ void sincos_small(double x, double& sn, double& cs) {
   const double x2 = x * x;

@@ -149,6 +149,9 @@ struct CtaMem {
     // the residuals read
     unsigned build_tab[kAzTabS / 2 + 1];
     struct { double P[324], X[324], U[108], V[108], X6[72]; } ex;  // exit covariance of one finished unit
+    // the residual phase's tensor-core fold (warp_fold_mma): 8 staged rows of 8 doubles per warp, 16 x 512 B = 8192 B,
+    // inside the 8196 B of build_tab, so the CTA does not grow.  Free then: the index build and the exit run outside passes.
+    double fold[kWarps][64];
   } u;
   int scan_tmp[kThreads];
   int wl_n[2], wl_head[2];  // work lists of the closest-point / walk phases (entries, next entry to hand out)
@@ -159,6 +162,7 @@ struct CtaMem {
   unsigned int phase;
   long long tlast;
 };
+static_assert(sizeof(((CtaMem*)nullptr)->u.fold) <= sizeof(((CtaMem*)nullptr)->u.build_tab), "the fold stage must not grow the CTA");
 
 // phase timers (thread 0 of each CTA; compiled in, enabled when bv.timers != nullptr)
 #define LINS_TICK(k)                                                                   \
@@ -364,6 +368,46 @@ __device__ __forceinline__ double warp_fold_row(const double* g, double r) {
     }
   }
   return p[0];
+}
+
+__device__ __forceinline__ void dmma_8x8x4(double& c0, double& c1, double a, double b) {
+  asm volatile("mma.sync.aligned.m8n8k4.row.col.f64.f64.f64.f64 {%0,%1}, {%2}, {%3}, {%0,%1};" : "+d"(c0), "+d"(c1) : "d"(a), "d"(b));
+}
+
+// The same 28 sums on the FP64 tensor cores: they are entries of the 8 x 8 Gram matrix C = G^T G of the warp's 32 rows
+// G = [g0..g5, r, 0], which eight mma.sync m8n8k4 (four rows each) accumulate.  The A (8 x 4, row) and B (4 x 8, col)
+// fragments of lane L are both G[4c + L % 4][L / 4], i.e. entries of other lanes' rows, so the rows pass through the warp's
+// 512 B of shared memory `st`: four rounds of 8 rows (two MMAs each).  A staged row is four 16-B chunks, chunk k of row j
+// at chunk 4 j + (k ^ (j >> 1)): the 8 writing lanes hit 8 different bank groups and the 32 reads of an MMA one 256-B
+// block.  Lane L writes C[L / 4][2 (L % 4) + {0, 1}] to dst[entry] where that is one of the 28 sums (same entry order as
+// warp_fold_row).  Fixed order => deterministic.  Lanes without a measurement pass g = 0, r = 0.
+__device__ __forceinline__ void warp_fold_mma(const double* g, double r, double* st, double* dst) {
+  const int lane = threadIdx.x & 31;
+  const int wj = lane & 7, f = lane >> 2;
+  double c0 = 0.0, c1 = 0.0;
+#pragma unroll
+  for (int q = 0; q < 4; ++q) {
+    __syncwarp();
+    if ((lane >> 3) == q) {
+      double2* row = reinterpret_cast<double2*>(st) + 4 * wj;
+      const int sw = wj >> 1;
+      row[0 ^ sw] = make_double2(g[0], g[1]); row[1 ^ sw] = make_double2(g[2], g[3]);
+      row[2 ^ sw] = make_double2(g[4], g[5]); row[3 ^ sw] = make_double2(r, 0.0);
+    }
+    __syncwarp();
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const int j = 4 * h + (lane & 3);
+      const double v = st[2 * (4 * j + ((f >> 1) ^ (j >> 1))) + (f & 1)];
+      dmma_8x8x4(c0, c1, v, v);
+    }
+  }
+  const int ci = f;
+#pragma unroll
+  for (int u = 0; u < 2; ++u) {
+    const int cj = 2 * (lane & 3) + u;
+    if (ci <= cj && cj <= 6) dst[cj < 6 ? ci * 6 - (ci * (ci - 1)) / 2 + (cj - ci) : (ci < 6 ? 21 + ci : 27)] = u ? c1 : c0;
+  }
 }
 
 __device__ __forceinline__ int col6(int a) { return a < 3 ? a : a + 3; }  // {0,1,2,6,7,8}

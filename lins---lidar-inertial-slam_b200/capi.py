@@ -34,9 +34,10 @@ EXPORTS = [
 
 NVCC_ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]  # H100 (Hopper)
 NVCC_COMMON = NVCC_ARCH + ["-lineinfo", "-O3", "-std=c++17", "-Xcompiler", "-fPIC"]
-# translation units and their extra flags: lins_gpu.cu (C-ABI + the fused kernel: bit-exact association, no multiply-add
-# contraction), lins_jacobian.cu (the tolerance-checked split Jacobian kernel: contraction allowed)
-UNITS = [("lins_gpu.cu", ["-fmad=false"]), ("lins_jacobian.cu", [])]
+# translation units and their extra flags: lins_gpu.cu (the fused kernel and most of the C-ABI), lins_upload.cu (batch
+# upload), lins_map.cu (row F2's host side) — all bit-exact, so no multiply-add contraction: the association and the map
+# fits depend on it — and lins_jacobian.cu (the tolerance-checked split Jacobian kernel: contraction allowed)
+UNITS = [("lins_gpu.cu", ["-fmad=false"]), ("lins_upload.cu", ["-fmad=false"]), ("lins_map.cu", ["-fmad=false"]), ("lins_jacobian.cu", [])]
 NVCC_FLAGS = NVCC_COMMON + ["-fmad=false", "-shared"]  # (what tools/ scripts print)
 
 

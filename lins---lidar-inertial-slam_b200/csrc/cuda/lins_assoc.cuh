@@ -52,6 +52,58 @@ struct PassBuffers {           // per-query arrays, indexed by v = slot * qtile 
   int nvw;                   // warps per slot = qtile / 32
 };
 
+// The fused kernel's dynamic shared memory, in this order, every region starting 16-byte aligned:
+//   CtaMem | Smem x nslots | wacc | wcnt | per-query arrays
+// The per-query arrays hold NQ = nslots * qtile entries each, back to back in the order pass_layout carves them (qtile
+// is a multiple of 32, so each of them starts 16-byte aligned).  When even one slot's arrays do not fit shared memory,
+// they live in a per-CTA global scratch instead (BatchView::qscratch) and the launch asks only for fixed_bytes.
+struct PassLayout {
+  size_t slots;        // offset of slot 0 (CtaMem is at offset 0)
+  size_t fixed_bytes;  // CtaMem, slots, wacc, wcnt
+  size_t query_bytes;  // the per-query arrays
+};
+
+__host__ __device__ constexpr size_t align16(size_t b) { return (b + 15) & ~(size_t)15; }
+
+// The layout for nslots units of qtile queries.  With pb, also fills *pb for CTA `cta`, whose dynamic shared memory starts
+// at smem: its per-query arrays follow wcnt there or, when qscratch is not null, start at qscratch + cta * qscratch_stride.
+__host__ __device__ __forceinline__ PassLayout pass_layout(int nslots, int qtile, PassBuffers* pb = nullptr, unsigned char* smem = nullptr,
+                                                           unsigned char* qscratch = nullptr, unsigned cta = 0, size_t qscratch_stride = 0) {
+  static_assert(sizeof(Smem) % 16 == 0, "slots are indexed as an array");
+  const int NQ = nslots * qtile;
+  const size_t nvw_all = (size_t)nslots * (qtile / 32);
+  const size_t wacc_bytes = align16(nvw_all * kNAcc * sizeof(double)), wcnt_bytes = align16(nvw_all * 2 * sizeof(int));
+  PassLayout lay;
+  lay.slots = align16(sizeof(CtaMem));
+  lay.fixed_bytes = lay.slots + nslots * sizeof(Smem) + wacc_bytes + wcnt_bytes;
+  // one entry of every per-query array the carve below takes, in its order (pos holds three per query); the carve is a
+  // pointer chain so that the kernel's address set-up stays as before
+  lay.query_bytes = align16((size_t)NQ * (sizeof(*pb->qpt) + sizeof(*pb->sel) + sizeof(*pb->qa) + sizeof(*pb->qw) + sizeof(*pb->qref) +
+                                          sizeof(*pb->qref2) + sizeof(*pb->qext) + sizeof(*pb->key) + 3 * sizeof(*pb->pos) +
+                                          sizeof(*pb->qccr) + sizeof(*pb->wl)));
+  if (pb) {
+    PassBuffers& b = *pb;
+    b.nvw = qtile / 32;
+    unsigned char* p = smem + lay.slots;
+    p += nslots * sizeof(Smem);
+    b.wacc = reinterpret_cast<double*>(p); p += wacc_bytes;
+    b.wcnt = reinterpret_cast<int*>(p); p += wcnt_bytes;
+    if (qscratch) p = qscratch + (size_t)cta * qscratch_stride;
+    b.qpt = reinterpret_cast<float4*>(p); p = reinterpret_cast<unsigned char*>(b.qpt + NQ);
+    b.sel = reinterpret_cast<float4*>(p); p = reinterpret_cast<unsigned char*>(b.sel + NQ);
+    b.qa = reinterpret_cast<float4*>(p); p = reinterpret_cast<unsigned char*>(b.qa + NQ);
+    b.qw = reinterpret_cast<int4*>(p); p = reinterpret_cast<unsigned char*>(b.qw + NQ);
+    b.qref = reinterpret_cast<float4*>(p); p = reinterpret_cast<unsigned char*>(b.qref + NQ);
+    b.qref2 = reinterpret_cast<float4*>(p); p = reinterpret_cast<unsigned char*>(b.qref2 + NQ);
+    b.qext = reinterpret_cast<float4*>(p); p = reinterpret_cast<unsigned char*>(b.qext + NQ);
+    b.key = reinterpret_cast<unsigned long long*>(p); p = reinterpret_cast<unsigned char*>(b.key + NQ);
+    b.pos = reinterpret_cast<int*>(p); p = reinterpret_cast<unsigned char*>(b.pos + 3 * NQ);
+    b.qccr = reinterpret_cast<int*>(p); p = reinterpret_cast<unsigned char*>(b.qccr + NQ);
+    b.wl = reinterpret_cast<int*>(p);
+  }
+  return lay;
+}
+
 __device__ __forceinline__ AzIndex az_index_of(const Smem& sm, const BatchView& bv, bool surf) {
   AzIndex ix;
   if (surf) { ix.pts = bv.az_s + sm.ts0; ix.bstart = sm.azTabS; ix.elev = sm.elevS; ix.nb = sm.nbS; ix.nrings = sm.nringsS; ix.T = sm.Ts; }

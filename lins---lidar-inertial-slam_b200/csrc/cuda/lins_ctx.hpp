@@ -1,0 +1,225 @@
+// lins_ctx.hpp — host state of a C-ABI context (struct lins_ctx of include/lins_gpu.h) and the helpers the translation units
+// that implement the C-ABI share: lins_gpu.cu (fused kernel, single-scan and batched entry points, F1), lins_upload.cu
+// (batch upload), lins_map.cu (row F2).  Host code only: a header that defines kernels cannot be included here, because
+// every unit that includes this one would define them again.
+#pragma once
+#include <cuda_runtime.h>
+#if defined(__SSE2__)
+#include <emmintrin.h>
+#endif
+
+#include <algorithm>
+#include <cstddef>
+#include <cstdint>
+#include <string>
+#include <utility>
+
+#include "../../../include/lins_gpu.h"
+#include "../host/host_pool.hpp"
+
+namespace lins_dev { struct IcpState; }                       // lins_icp_step.cuh
+namespace lins_map { struct PassConsts; struct MapLoopState; }  // lins_map.cuh
+
+namespace lins_capi {
+
+constexpr bool kPinned = true;
+
+// Grow-only buffer that owns its memory: device memory, or pinned host memory when Pinned.  reserve() never shrinks; to
+// grow it frees first, then allocates at least 16 elements, so the contents do not survive growth.
+template <typename T, bool Pinned = false>
+struct Buf {
+  T* p = nullptr;
+  size_t cap = 0;
+  Buf() = default;
+  Buf(const Buf&) = delete;
+  Buf& operator=(const Buf&) = delete;
+  Buf(Buf&& o) noexcept : p(o.p), cap(o.cap) { o.p = nullptr; o.cap = 0; }
+  Buf& operator=(Buf&& o) noexcept { std::swap(p, o.p); std::swap(cap, o.cap); return *this; }
+  ~Buf() { deallocate(); }
+  cudaError_t reserve(size_t n) {
+    if (n <= cap) return cudaSuccess;
+    deallocate();
+    const size_t want = std::max<size_t>(n, 16);
+    const cudaError_t e = Pinned ? cudaMallocHost(&p, want * sizeof(T)) : cudaMalloc(&p, want * sizeof(T));
+    if (e == cudaSuccess) cap = want;
+    return e;
+  }
+
+ private:
+  void deallocate() {
+    if (p) { if (Pinned) cudaFreeHost(p); else cudaFree(p); }
+    p = nullptr; cap = 0;
+  }
+};
+
+struct Resident {  // one resident batch (device) + its pinned staging (host)
+  int n = 0;
+  size_t nqs = 0, nqc = 0, nts = 0, ntc = 0;
+  int max_q = 0;
+  Buf<float4> qs, qc, ts, tc, az_s, az_c;
+  Buf<float4> raw;              // raw 32-B records of clouds uploaded straight from caller-pinned memory (2 float4 per point)
+  Buf<unsigned char> qscratch;  // per-CTA per-query arrays of units too large for shared memory
+  Buf<int> qs_off, qc_off, ts_off, tc_off, ind_s, ind_c, counter;
+  Buf<long long> timers;
+  Buf<double> jac_part;         // split Jacobian kernel: per-(unit, part) sums and arrival counters
+  Buf<int> jac_cnt;
+  Buf<lins_dev::IcpState> icp;  // pose-update state of the ICP fallback loop (lins_gpu_estimate_transform)
+  Buf<lins_dev::IcpState, kPinned> h_icp;
+  Buf<double> state_in, cov_in, state_out, cov_out, accum;
+  Buf<lins_scan_result> results;
+  Buf<lins_report> reports;
+  Buf<float> sel_s, sel_c, coeff_s, coeff_c;
+  Buf<unsigned char> mask_s, mask_c;
+  Buf<float4, kPinned> h_pts;   // staging for all four clouds, back to back
+  Buf<int, kPinned> h_off;      // 4 x (n+1)
+  Buf<double, kPinned> h_state, h_cov, h_state_out, h_cov_out, h_accum;
+  Buf<lins_scan_result, kPinned> h_results;
+  Buf<lins_report, kPinned> h_reports;
+};
+
+}  // namespace lins_capi
+
+struct lins_ctx {
+  template <typename T, bool Pinned = false>
+  using Buf = lins_capi::Buf<T, Pinned>;
+  static constexpr bool kPinned = lins_capi::kPinned;
+
+  HostPool pool;
+  int device = 0;
+  cudaStream_t stream = nullptr;
+  bool own_stream = false;
+  lins_params prm;
+  std::string err;
+  int sm_count = 132;  // (replaced by the device's count in lins_gpu_create)
+  int max_smem_optin = 0;
+  int64_t launches = 0;
+  int64_t upload_raw_points = 0, upload_packed_points = 0;  // cumulative split of lins_gpu_batch_upload (raw DMA vs host pack)
+  lins_capi::Resident batch;   // lins_gpu_batch_* working set
+  lins_capi::Resident single;  // lins_gpu_ieskf / associate / estimate_transform (n = 1)
+  // the single-scan map: "last" clouds (walks + tripods) and the clouds the 1-NN index was built on
+  Buf<float4> map_s, map_c, tree_s, tree_c;
+  Buf<int> map_off;  // 4 x 2 ints: [0,ns][0,nc][0,tns][0,tnc]
+  int map_ns = -1, map_nc = -1, tree_ns = -1, tree_nc = -1;
+  bool tree_is_map = true;
+  bool timers_on = false;
+  bool verbose = false;  // LINS_VERBOSE: print the launch configuration
+  int force_slots = 0;  // tuning knob (LINS_SLOTS): resident units per CTA
+  Buf<lins_point> tmp_out;      // transformed clouds as full PointXYZI records (update_map read-back)
+  cudaEvent_t tmp_ev = nullptr; // recorded after the last H2D copies that read h_tmp
+  Buf<lins_point, kPinned> h_out;  // pinned staging of the update_map read-back
+  Buf<double> tmp_lin;
+  Buf<float4, kPinned> h_tmp;
+  // row F2 (scan-to-map refinement): the map clouds, the current feature clouds, search / reduction scratch
+  struct MapState {
+    Buf<float4> map_c, map_s, q_c, q_s;
+    int n_map_c = -1, n_map_s = -1;
+    struct Grid {  // hashed uniform grid of one map cloud (lins_map.cuh: GridIndex)
+      Buf<float4> sorted;
+      Buf<int> start, count, cursor;
+      unsigned mask = 0;                      // buckets - 1
+      float origin[3] = {0.f, 0.f, 0.f};
+      int n = 0;
+    } grid_c, grid_s;
+    Buf<lins_map::MapLoopState> loop;   // device-resident state of one scan2map call
+    Buf<lins_map::MapLoopState, kPinned> h_loop;
+    Buf<lins_map::PassConsts> consts;   // sin / cos + translation of the pass being run
+    Buf<float> part_d;
+    Buf<int> part_i;
+    Buf<double> partial;
+    Buf<double, kPinned> h_partial;
+    Buf<int32_t> knn_c, knn_s;
+    Buf<float> coeff_c, coeff_s;
+    Buf<uint8_t> mask_c, mask_s;
+  } mp;
+};
+
+namespace lins_capi {
+
+inline int fail(lins_ctx* c, int code, const char* what, cudaError_t e = cudaSuccess) {
+  if (c) {
+    c->err = what;
+    if (e != cudaSuccess) { c->err += ": "; c->err += cudaGetErrorString(e); }
+  }
+  return code;
+}
+#define CK(call)                                                                \
+  do {                                                                          \
+    cudaError_t _e = (call);                                                    \
+    if (_e != cudaSuccess) return lins_capi::fail(ctx, LINS_E_CUDA, #call, _e); \
+  } while (0)
+
+// pcl::PointXYZI (32 B) -> (x, y, z, intensity) (16 B).  The destination is pinned staging that the copy engine
+// reads next and the host never reads back: SSE2 (x86-64 baseline) with non-temporal stores.
+inline void pack_into(float4* dst, const lins_point* src, int n) {
+#if defined(__SSE2__)
+  if ((reinterpret_cast<uintptr_t>(dst) & 15u) == 0) {
+    for (int i = 0; i < n; ++i) {
+      const __m128 a = _mm_loadu_ps(&src[i].x);                         // x y z pad
+      const __m128 b = _mm_load_ss(&src[i].intensity);                  // i 0 0 0
+      const __m128 t = _mm_shuffle_ps(a, b, _MM_SHUFFLE(0, 0, 2, 2));   // z z i i
+      _mm_stream_ps(reinterpret_cast<float*>(dst + i), _mm_shuffle_ps(a, t, _MM_SHUFFLE(2, 0, 1, 0)));  // x y z i
+    }
+    _mm_sfence();
+    return;
+  }
+#endif
+  for (int i = 0; i < n; ++i) dst[i] = make_float4(src[i].x, src[i].y, src[i].z, src[i].intensity);
+}
+
+// allocate the per-batch outputs / scratch for n scans with the given query totals
+inline int reserve_outputs(lins_ctx* ctx, Resident& r, bool want_reports, bool want_trace) {
+  CK(r.state_out.reserve((size_t)r.n * 20));
+  CK(r.cov_out.reserve((size_t)r.n * 324));
+  CK(r.results.reserve(r.n));
+  CK(r.accum.reserve((size_t)r.n * 32));
+  CK(r.az_s.reserve(r.nts + 4));
+  CK(r.az_c.reserve(r.ntc + 4));
+  CK(r.ind_s.reserve(3 * r.nqs + 4));
+  CK(r.ind_c.reserve(2 * r.nqc + 4));
+  CK(r.counter.reserve(4));
+  if (want_reports) CK(r.reports.reserve(r.n));
+  if (want_trace) {
+    CK(r.sel_s.reserve(3 * r.nqs + 4)); CK(r.sel_c.reserve(3 * r.nqc + 4));
+    CK(r.coeff_s.reserve(4 * r.nqs + 4)); CK(r.coeff_c.reserve(4 * r.nqc + 4));
+    CK(r.mask_s.reserve(r.nqs + 4)); CK(r.mask_c.reserve(r.nqc + 4));
+  }
+  return LINS_OK;
+}
+
+// ---- two clouds through the context's pinned staging (ctx->h_tmp) ------------------------------------------------------
+// h_tmp is read by asynchronous H2D copies: before it is rewritten, wait for the event recorded after the last copies that
+// read it (already complete in steady state: no stream synchronisation).
+inline cudaError_t tmp_staging_wait(lins_ctx* ctx) {
+  if (!ctx->tmp_ev) return cudaSuccess;
+  return cudaEventSynchronize(ctx->tmp_ev);
+}
+inline cudaError_t tmp_staging_mark(lins_ctx* ctx) {
+  if (!ctx->tmp_ev) { cudaError_t e = cudaEventCreateWithFlags(&ctx->tmp_ev, cudaEventDisableTiming); if (e != cudaSuccess) return e; }
+  return cudaEventRecord(ctx->tmp_ev, ctx->stream);
+}
+
+// every allocation of an upload of na + nb points into dst_a / dst_b; waits until the staging is free
+inline int upload2_reserve(lins_ctx* ctx, Buf<float4>& dst_a, int na, Buf<float4>& dst_b, int nb) {
+  CK(dst_a.reserve((size_t)na + 1)); CK(dst_b.reserve((size_t)nb + 1));
+  if (na + nb == 0) return LINS_OK;
+  CK(tmp_staging_wait(ctx));
+  CK(ctx->h_tmp.reserve((size_t)na + nb + 1));
+  return LINS_OK;
+}
+// pack a and b into the staging and queue their H2D copies into dst_a / dst_b, reserved by upload2_reserve (no stream
+// synchronisation)
+inline int upload2_queue(lins_ctx* ctx, Buf<float4>& dst_a, const lins_point* a, int na, Buf<float4>& dst_b, const lins_point* b, int nb) {
+  if (na + nb == 0) return LINS_OK;
+  pack_into(ctx->h_tmp.p, a, na);
+  pack_into(ctx->h_tmp.p + na, b, nb);
+  if (na) CK(cudaMemcpyAsync(dst_a.p, ctx->h_tmp.p, sizeof(float4) * (size_t)na, cudaMemcpyHostToDevice, ctx->stream));
+  if (nb) CK(cudaMemcpyAsync(dst_b.p, ctx->h_tmp.p + na, sizeof(float4) * (size_t)nb, cudaMemcpyHostToDevice, ctx->stream));
+  CK(tmp_staging_mark(ctx));
+  return LINS_OK;
+}
+inline int upload2(lins_ctx* ctx, Buf<float4>& dst_a, const lins_point* a, int na, Buf<float4>& dst_b, const lins_point* b, int nb) {
+  const int rc = upload2_reserve(ctx, dst_a, na, dst_b, nb);
+  return rc != LINS_OK ? rc : upload2_queue(ctx, dst_a, a, na, dst_b, b, nb);
+}
+
+}  // namespace lins_capi

@@ -1,0 +1,211 @@
+// lins_map.cu — host side of row F2 (SURVEY.md §8(f)): the mapping node's scan-to-map refinement, whose kernels are in
+// lins_map.cuh.
+#include <cuda_runtime.h>
+
+#include <algorithm>
+#include <cmath>
+#include <cstddef>
+#include <cstdlib>
+#include <cstring>
+
+#include "lins_ctx.hpp"
+#include "lins_map.cuh"
+
+using namespace lins_capi;
+
+// ---- row F2: the mapping node's scan-to-map refinement (lidar_mapping_node.cpp:1635-1652) --------------------------------
+namespace {
+
+lins_map::PassConsts host_pass_consts(const float* T) {  // libm sin / cos in f32, like the reference (:579-592, :1527-1532)
+  lins_map::PassConsts pc;
+  pc.cRoll = std::cos(T[0]); pc.sRoll = std::sin(T[0]); pc.cPitch = std::cos(T[1]); pc.sPitch = std::sin(T[1]);
+  pc.cYaw = std::cos(T[2]); pc.sYaw = std::sin(T[2]); pc.tX = T[3]; pc.tY = T[4]; pc.tZ = T[5];
+  pc.srx = std::sin(T[0]); pc.crx = std::cos(T[0]); pc.sry = std::sin(T[1]); pc.cry = std::cos(T[1]);
+  pc.srz = std::sin(T[2]); pc.crz = std::cos(T[2]);
+  return pc;
+}
+
+// which 5-NN search a pass uses: the hashed grid (exact for every point that can be accepted) or the brute-force slices
+// (exact for every point).  LINS_MAP_KNN=grid|brute overrides the caller's default.
+bool map_use_grid(bool dflt) {
+  const char* e = std::getenv("LINS_MAP_KNN");  // (read per call: tests flip it between calls)
+  return !e || !*e ? dflt : std::strcmp(e, "grid") == 0;
+}
+
+// the kernels' view of a grid (lins_ctx.hpp keeps its parts: that header cannot include lins_map.cuh)
+lins_map::GridIndex grid_index(const lins_ctx::MapState::Grid& g) {
+  lins_map::GridIndex gi;
+  gi.pts = g.sorted.p; gi.start = g.start.p; gi.mask = g.mask; gi.ox = g.origin[0]; gi.oy = g.origin[1]; gi.oz = g.origin[2];
+  return gi;
+}
+
+// bucket-sort one map cloud into its grid (≙ kdtree*FromMap->setInputCloud, :1637-1638)
+int map_build_grid(lins_ctx* ctx, lins_ctx::MapState::Grid& g, const float4* map, int n, const lins_point* host_pts) {
+  using namespace lins_map;
+  g.n = n;
+  if (n <= 0) return LINS_OK;
+  float mn[3] = {3.0e38f, 3.0e38f, 3.0e38f};
+  for (int i = 0; i < n; ++i) {  // origin = the finite minimum (cells are addressed by hash: the extent does not matter)
+    const float v[3] = {host_pts[i].x, host_pts[i].y, host_pts[i].z};
+    for (int k = 0; k < 3; ++k) if (v[k] == v[k] && std::fabs(v[k]) < 1.0e30f && v[k] < mn[k]) mn[k] = v[k];
+  }
+  for (int k = 0; k < 3; ++k) if (!(mn[k] < 3.0e38f)) mn[k] = 0.f;
+  unsigned nb = 4096;
+  while (nb < 2u * (unsigned)n && nb < (1u << 24)) nb <<= 1;
+  CK(g.start.reserve((size_t)nb + 2)); CK(g.count.reserve((size_t)nb + 2)); CK(g.cursor.reserve((size_t)nb + 2)); CK(g.sorted.reserve((size_t)n + 1));
+  g.mask = nb - 1;
+  for (int k = 0; k < 3; ++k) g.origin[k] = mn[k];
+  const GridIndex gi = grid_index(g);
+  CK(cudaMemsetAsync(g.count.p, 0, sizeof(int) * nb, ctx->stream));
+  lins_grid_count_kernel<<<(n + 255) / 256, 256, 0, ctx->stream>>>(map, n, gi, g.count.p);
+  lins_grid_scan_kernel<<<1, 1024, 0, ctx->stream>>>(g.count.p, g.start.p, g.cursor.p, (int)nb);
+  lins_grid_scatter_kernel<<<(n + 255) / 256, 256, 0, ctx->stream>>>(map, n, gi, g.cursor.p, g.sorted.p);
+  CK(cudaGetLastError());
+  ctx->launches += 3;
+  return LINS_OK;
+}
+
+// queue one cornerOptimization + surfOptimization pass (5-NN, fits, block partials) that reads its constants from
+// m.consts (device); nothing is synchronised.  Returns the number of partial blocks.
+int map_queue_pass(lins_ctx* ctx, int nc, int ns, bool dense, bool grid, const int* done, int* nblocks_out) {
+  using namespace lins_map;
+  lins_ctx::MapState& m = ctx->mp;
+  const int qb[2] = {(nc + kKnnThreads - 1) / kKnnThreads, (ns + kKnnThreads - 1) / kKnnThreads};
+  const int nq[2] = {nc, ns}, nm[2] = {std::max(m.n_map_c, 0), std::max(m.n_map_s, 0)};
+  const float4* q[2] = {m.q_c.p, m.q_s.p};
+  const float4* mp[2] = {m.map_c.p, m.map_s.p};
+  const lins_ctx::MapState::Grid* gr[2] = {&m.grid_c, &m.grid_s};
+  int slices[2], slice_len[2];
+  size_t part = 0;
+  for (int k = 0; k < 2; ++k) {
+    // brute force: enough (query block, map slice) pairs for ~8 CTAs per SM (the scan is latency bound: profiles/r01_map_*);
+    // a slice is at least 256 map points.  grid: one list per query
+    int S = qb[k] > 0 ? (8 * ctx->sm_count + qb[k] - 1) / qb[k] : 1;
+    S = std::max(1, std::min(S, std::min(64, (nm[k] + 255) / 256)));
+    if (grid) S = 1;
+    slices[k] = S;
+    slice_len[k] = std::max(1, (nm[k] + S - 1) / S);
+    part = std::max(part, (size_t)nq[k] * S * 5);
+  }
+  CK(m.part_d.reserve(part + 1)); CK(m.part_i.reserve(part + 1));
+  const int nblocks = qb[0] + qb[1];
+  CK(m.partial.reserve((size_t)(nblocks + 1) * (kRowAcc + 1))); CK(m.h_partial.reserve((size_t)(nblocks + 1) * (kRowAcc + 1)));
+  if (dense) {
+    CK(m.knn_c.reserve(5 * (size_t)nc + 1)); CK(m.knn_s.reserve(5 * (size_t)ns + 1)); CK(m.coeff_c.reserve(4 * (size_t)nc + 1));
+    CK(m.coeff_s.reserve(4 * (size_t)ns + 1)); CK(m.mask_c.reserve((size_t)nc + 1)); CK(m.mask_s.reserve((size_t)ns + 1));
+  }
+  for (int k = 0; k < 2; ++k) {
+    if (nq[k] == 0) continue;
+    if (grid && nm[k] > 0)
+      lins_map_knn_grid_kernel<<<(nq[k] + kGridKnnWarps - 1) / kGridKnnWarps, kGridKnnWarps * 32, 0, ctx->stream>>>(q[k], nq[k], grid_index(*gr[k]), m.consts.p, done, m.part_d.p, m.part_i.p);
+    else
+      lins_map_knn_kernel<<<dim3(qb[k], slices[k]), kKnnThreads, 0, ctx->stream>>>(q[k], nq[k], mp[k], nm[k], slice_len[k], m.consts.p, done, m.part_d.p, m.part_i.p);
+    double* partial = m.partial.p + (size_t)(k == 0 ? 0 : qb[0]) * (kRowAcc + 1);
+    if (k == 0)
+      lins_map_fit_kernel<true><<<qb[k], kFitThreads, 0, ctx->stream>>>(q[k], nq[k], mp[k], slices[k], m.part_d.p, m.part_i.p, m.consts.p, done, dense ? m.knn_c.p : nullptr,
+                                                                       dense ? m.coeff_c.p : nullptr, dense ? m.mask_c.p : nullptr, partial);
+    else
+      lins_map_fit_kernel<false><<<qb[k], kFitThreads, 0, ctx->stream>>>(q[k], nq[k], mp[k], slices[k], m.part_d.p, m.part_i.p, m.consts.p, done, dense ? m.knn_s.p : nullptr,
+                                                                        dense ? m.coeff_s.p : nullptr, dense ? m.mask_s.p : nullptr, partial);
+    CK(cudaGetLastError());
+    ctx->launches += 2;
+  }
+  *nblocks_out = nblocks;
+  return LINS_OK;
+}
+
+int map_stage_queries(lins_ctx* ctx, const lins_point* corner, int nc, const lins_point* surf, int ns) {
+  if (nc < 0 || ns < 0 || (nc > 0 && !corner) || (ns > 0 && !surf)) return fail(ctx, LINS_E_INVALID, "bad feature clouds");
+  if (ctx->mp.n_map_c < 0) return fail(ctx, LINS_E_NOMAP, "lins_gpu_map_set has not been called");
+  return upload2(ctx, ctx->mp.q_c, corner, nc, ctx->mp.q_s, surf, ns);
+}
+
+}  // namespace
+
+extern "C" {
+
+int lins_gpu_map_set(lins_ctx* ctx, const lins_point* corner, int nc, const lins_point* surf, int ns) {
+  if (!ctx) return LINS_E_INVALID;
+  if (nc < 0 || ns < 0 || (nc > 0 && !corner) || (ns > 0 && !surf)) return fail(ctx, LINS_E_INVALID, "bad map clouds");
+  CK(cudaSetDevice(ctx->device));
+  int rc = upload2(ctx, ctx->mp.map_c, corner, nc, ctx->mp.map_s, surf, ns);
+  if (rc != LINS_OK) return rc;
+  ctx->mp.n_map_c = nc; ctx->mp.n_map_s = ns;
+  rc = map_build_grid(ctx, ctx->mp.grid_c, ctx->mp.map_c.p, nc, corner);
+  if (rc != LINS_OK) return rc;
+  return map_build_grid(ctx, ctx->mp.grid_s, ctx->mp.map_s.p, ns, surf);
+}
+
+int lins_gpu_scan2map(lins_ctx* ctx, const lins_point* corner, int nc, const lins_point* surf, int ns, float* T, lins_map_report* rep) {
+  if (!ctx) return LINS_E_INVALID;
+  if (!T) return fail(ctx, LINS_E_INVALID, "null transform");
+  CK(cudaSetDevice(ctx->device));
+  using namespace lins_map;
+  lins_map_report r;
+  std::memset(&r, 0, sizeof(r));
+  lins_ctx::MapState& m = ctx->mp;
+  if (m.n_map_c < 0) return fail(ctx, LINS_E_NOMAP, "lins_gpu_map_set has not been called");
+  if (!(m.n_map_c > 10 && m.n_map_s > 100)) {  // :1636
+    r.skipped = 1;
+    if (rep) *rep = r;
+    return LINS_OK;
+  }
+  int rc = map_stage_queries(ctx, corner, nc, surf, ns);
+  if (rc != LINS_OK) return rc;
+  // The whole iteration loop (:1640-1648) is queued up front: transformTobeMapped, matP / isDegenerate and the report live
+  // on the device (MapLoopState); the first pass uses libm sin / cos of the caller's transform (bit-identical to the
+  // reference's first pass), later ones the constants the LM kernel derived on the device.
+  if (!m.loop.p) {  // isDegenerate / matP are members of the reference's mapping node (:226-227, :395-396): they survive the
+    CK(m.loop.reserve(1));  // calls — a call whose first pass selects < 50 points keeps using the previous scan's values
+    CK(cudaMemsetAsync(m.loop.p, 0, sizeof(MapLoopState), ctx->stream));
+  }
+  CK(m.h_loop.reserve(1)); CK(m.consts.reserve(1));
+  const PassConsts pc0 = host_pass_consts(T);
+  CK(cudaMemcpyAsync(m.loop.p, T, sizeof(float) * 6, cudaMemcpyHostToDevice, ctx->stream));  // (pageable sources: staged before the call returns)
+  CK(cudaMemsetAsync(reinterpret_cast<char*>(m.loop.p) + offsetof(MapLoopState, done), 0, sizeof(MapLoopState) - offsetof(MapLoopState, done), ctx->stream));
+  CK(cudaMemcpyAsync(m.consts.p, &pc0, sizeof(pc0), cudaMemcpyHostToDevice, ctx->stream));
+  const bool grid = map_use_grid(true);
+  for (int iter = 0; iter < LINS_MAP_MAX_ITER; ++iter) {
+    int nblocks = 0;
+    rc = map_queue_pass(ctx, nc, ns, false, grid, &m.loop.p->done, &nblocks);
+    if (rc != LINS_OK) return rc;
+    lins_map_lm_kernel<<<1, 32, 0, ctx->stream>>>(m.partial.p, nblocks, iter, m.loop.p, m.consts.p);
+    CK(cudaGetLastError());
+    ctx->launches += 1;
+  }
+  CK(cudaMemcpyAsync(m.h_loop.p, m.loop.p, sizeof(MapLoopState), cudaMemcpyDeviceToHost, ctx->stream));
+  CK(cudaStreamSynchronize(ctx->stream));
+  const MapLoopState& st = *m.h_loop.p;
+  for (int i = 0; i < 6; ++i) T[i] = st.T[i];
+  r.iters = st.iters; r.converged = st.converged; r.degenerate = st.isDegenerate;
+  for (int i = 0; i < LINS_MAP_MAX_ITER; ++i) { r.n_sel[i] = st.n_sel[i]; r.delta_r[i] = st.delta_r[i]; r.delta_t[i] = st.delta_t[i]; }
+  if (rep) *rep = r;
+  return LINS_OK;
+}
+
+int lins_gpu_map_associate(lins_ctx* ctx, const lins_point* corner, int nc, const lins_point* surf, int ns, const float* T,
+                           int32_t* cknn, int32_t* sknn, float* ccoeff, float* scoeff, uint8_t* cmask, uint8_t* smask) {
+  if (!ctx) return LINS_E_INVALID;
+  if (!T) return fail(ctx, LINS_E_INVALID, "null transform");
+  CK(cudaSetDevice(ctx->device));
+  int rc = map_stage_queries(ctx, corner, nc, surf, ns);
+  if (rc != LINS_OK) return rc;
+  lins_ctx::MapState& m = ctx->mp;
+  CK(m.consts.reserve(1));
+  const lins_map::PassConsts pc = host_pass_consts(T);
+  CK(cudaMemcpyAsync(m.consts.p, &pc, sizeof(pc), cudaMemcpyHostToDevice, ctx->stream));
+  int nblocks = 0;
+  // the parity hook: brute force by default (exact neighbours for EVERY point, also those the 1 m gate rejects)
+  rc = map_queue_pass(ctx, nc, ns, true, map_use_grid(false), nullptr, &nblocks);
+  if (rc != LINS_OK) return rc;
+  if (cknn && nc) CK(cudaMemcpyAsync(cknn, m.knn_c.p, sizeof(int32_t) * 5 * (size_t)nc, cudaMemcpyDeviceToHost, ctx->stream));
+  if (sknn && ns) CK(cudaMemcpyAsync(sknn, m.knn_s.p, sizeof(int32_t) * 5 * (size_t)ns, cudaMemcpyDeviceToHost, ctx->stream));
+  if (ccoeff && nc) CK(cudaMemcpyAsync(ccoeff, m.coeff_c.p, sizeof(float) * 4 * (size_t)nc, cudaMemcpyDeviceToHost, ctx->stream));
+  if (scoeff && ns) CK(cudaMemcpyAsync(scoeff, m.coeff_s.p, sizeof(float) * 4 * (size_t)ns, cudaMemcpyDeviceToHost, ctx->stream));
+  if (cmask && nc) CK(cudaMemcpyAsync(cmask, m.mask_c.p, (size_t)nc, cudaMemcpyDeviceToHost, ctx->stream));
+  if (smask && ns) CK(cudaMemcpyAsync(smask, m.mask_s.p, (size_t)ns, cudaMemcpyDeviceToHost, ctx->stream));
+  CK(cudaStreamSynchronize(ctx->stream));
+  return LINS_OK;
+}
+
+}  // extern "C"

@@ -1,4 +1,4 @@
-"""build_variant.py NAME [extra nvcc flags...] -> variants/liblins_gpu_NAME.so (both translation units, same flags as the product)."""
+"""build_variant.py NAME [extra nvcc flags...] -> variants/liblins_gpu_NAME.so (every translation unit, same flags as the product)."""
 import importlib, os, sys
 root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, root)

@@ -14,6 +14,9 @@
  *   lins_gpu_update_map     <-> updatePointCloud() / transformToEnd()     StateEstimator.hpp:1083-1101, :1116-1161
  *   lins_gpu_batch_*        <-> the same performIESKF, for many independent (scan pair, prior) units
  *                               resident in HBM (offline / batched odometry; SURVEY.md §8(e))
+ *   lins_gpu_seq_*          <-> processImu + processScan (StateEstimator.hpp:242-270, :435-463) of many running
+ *                               sequences in lockstep: IMU propagation, IESKF, ICP fallback, reset(1), roll / pitch
+ *                               correction and the map refresh all on the device
  *
  * Conventions
  *   - extern "C", plain pointers and sizes; no Eigen / PCL / ROS / torch types.
@@ -138,6 +141,10 @@ int lins_gpu_ieskf(lins_ctx* ctx, const lins_point* surf_flat, int n_surf, const
    pointer may be NULL. ind: -1 = none. mask = the accept test (s > 0.1 && res != 0). coeff = (s*jac, s*res).
    sel = pointSel (the de-skewed query, f32). Indices persist inside the ctx between calls like
    pointSearchSurfInd1/2/3 do, so iter % icp_freq != 0 reuses them. */
+/* The correspondence IDs of the last lins_gpu_ieskf / lins_gpu_associate / lins_gpu_estimate_transform call's last search
+   iteration (3 per surf query, 2 per corner query, -1 = none; either pointer may be NULL). */
+int lins_gpu_download_indices(lins_ctx* ctx, int32_t* surf_ind, int32_t* corner_ind);
+
 int lins_gpu_associate(lins_ctx* ctx, const lins_point* surf_flat, int n_surf, const lins_point* corner_sharp,
                        int n_corner, const double* lin_state, int iter, int32_t* surf_ind /*3*n_surf*/,
                        int32_t* corner_ind /*2*n_corner*/, float* surf_coeff /*4*n_surf*/,
@@ -190,6 +197,81 @@ int lins_gpu_batch_results_device(lins_ctx* ctx, void** dev_ptr, int* n_scans);
    pinned staging first).  Unregister before freeing the buffer. */
 int lins_gpu_host_register(void* ptr, size_t bytes);
 int lins_gpu_host_unregister(void* ptr);
+
+/* ---- sequence mode: S running sequences advanced one scan per step, all on the device -------------------------------
+   Per present sequence one step runs what StateEstimator does between two scans once it is RUNNING
+   (lins/src/lib/Estimator.cpp:228-252 -> StateEstimator.hpp:242-270, :435-463): the processImu calls
+   (StatePredictor::predict, KalmanFilter.hpp:125-186), the processScan gate (:436-440), performIESKF (:465-600) with the
+   estimateTransform fallback (:585-592, :1163-1196), filter_->update (KalmanFilter.hpp:195-200), integrateTransformation
+   (:608-617), reset(1) (KalmanFilter.hpp:320-353), calculateRPfromGravity + correctRollPitch (:602-605, :427-431) and
+   updatePointCloud (:1116-1161).  Sequence initialisation (processFirstScan / processSecondScan, :331-425) stays with the
+   caller; lins_gpu_seq_begin takes its result. */
+
+/* the filter constants the device chain needs (exp_port.yaml:29-62) */
+typedef struct lins_seq_params {
+  double noise[4];         /* StatePredictor::noise_[0..3] (KalmanFilter.hpp:300-311), as kalman_filter.hpp setNoise() computes them */
+  double init_pos_std[3];  /* INIT_POS_STD, m: reset(1) installs their squares (KalmanFilter.hpp:330) */
+  double init_att_std[3];  /* INIT_ATT_STD, degrees (KalmanFilter.hpp:323-325) */
+} lins_seq_params;
+
+/* hand-over of S running sequences, each right after its processSecondScan (StateEstimator.hpp:379-425) */
+typedef struct lins_seq_begin_desc {
+  int32_t n_seq;
+  const double* filter_state;  /* S x 19 : filter_->state_ */
+  const double* filter_cov;    /* S x 324: filter_->covariance_ */
+  const double* global_state;  /* S x 19 : globalState_ */
+  const double* imu_last;      /* S x 6  : acc_last (3), gyr_last (3) of the StatePredictor */
+  const lins_point* surf_map;   const int32_t* surf_map_off;    /* scan_last_->surfPointsLessFlat_ (already at scan end) */
+  const lins_point* corner_map; const int32_t* corner_map_off;  /* scan_last_->cornerPointsLessSharp_ */
+  int32_t point_format;        /* LINS_POINTS_XYZI32 or LINS_POINTS_PACKED16, as in lins_batch_desc */
+} lins_seq_begin_desc;
+
+/* one scan per sequence; CSR like lins_batch_desc (every *_off has n_seq + 1 entries) */
+typedef struct lins_seq_step_desc {
+  int32_t n_seq;                 /* == the begin call's */
+  const uint8_t* present;        /* NULL = all; 0 = this sequence has no scan this step: its state is left untouched */
+  const double* imu; const int32_t* imu_off;  /* k x 7 (dt, acc[3], gyr[3]): the processImu calls before the scan */
+  const lins_point* surf_flat;  const int32_t* surf_flat_off;         /* queries: surfPointsFlat_ */
+  const lins_point* corner_sharp; const int32_t* corner_sharp_off;    /* queries: cornerPointsSharp_ */
+  const lins_point* surf_less_flat; const int32_t* surf_less_flat_off;        /* the new scan's, as extracted */
+  const lins_point* corner_less_sharp; const int32_t* corner_less_sharp_off;
+  int32_t point_format;
+} lins_seq_step_desc;
+
+#define LINS_SEQ_IDLE 0      /* not present this step */
+#define LINS_SEQ_SKIPPED 1   /* failed the processScan gate (cornerLessSharp <= 5 || surfLessFlat <= 10): predicted state, old map */
+#define LINS_SEQ_RAN 2       /* processScan ran */
+#define LINS_SEQ_ICP 3       /* processScan ran and the IESKF diverged: the pose is estimateTransform's */
+
+/* Uploads the hand-over; replaces any running sequences of this ctx (single-scan and batched state are untouched). */
+int lins_gpu_seq_begin(lins_ctx* ctx, const lins_seq_params* params, const lins_seq_begin_desc* desc);
+/* Advances every present sequence by one scan.  Returns LINS_E_NOMAP before lins_gpu_seq_begin.  One stream
+   synchronisation (the divergence check) per call; the rest is queued.  LINS_E_INVALID for a bad descriptor leaves the
+   sequences as they were; any other error ends the run (the sequences are dropped, the next step returns LINS_E_NOMAP
+   until a new lins_gpu_seq_begin), because the step may have advanced some of its phases already. */
+int lins_gpu_seq_step(lins_ctx* ctx, const lins_seq_step_desc* step);
+/* The sequences' state after the last step; any pointer may be NULL.  results / reports: the last step's performIESKF,
+   valid where scan_status is LINS_SEQ_RAN or LINS_SEQ_ICP and unspecified elsewhere (zero before the first step);
+   scan_status: LINS_SEQ_* of the last step. */
+int lins_gpu_seq_download(lins_ctx* ctx, double* global_state /*S x 19*/, double* filter_state /*S x 19*/,
+                          double* filter_cov /*S x 324*/, lins_scan_result* results /*S*/, lins_report* reports /*S*/,
+                          int32_t* scan_status /*S*/);
+/* CUDA-event times of the last lins_gpu_seq_step's phases, ms: ms[0] IMU propagation, ms[1] query compaction + IESKF,
+   ms[2] divergence check (D2H + synchronisation) + estimateTransform fallbacks, ms[3] post kernel + map refresh. */
+int lins_gpu_seq_phase_ms(lins_ctx* ctx, float* ms /*4*/);
+/* Parity hooks of sequence mode (any pointer may be NULL).  download_ieskf: the last step's IESKF prior (the filter state
+   and covariance after the IMU propagation, every sequence), its output (state_out / cov_out as lins_gpu_ieskf returns
+   them; valid where scan_status >= LINS_SEQ_RAN), and the correspondence IDs of its last search iteration
+   (pointSearchSurfInd1/2/3, pointSearchCornerInd1/2) for the sequences that ran, in sequence order: query_off holds the
+   2 x (S + 1) offsets of their surf / corner queries into surf_ind (3 per query) and corner_ind (2 per query).
+   download_maps: the maps the next step searches, as (x, y, z, intensity) float records, CSR with off = 4 x (S + 1)
+   (surf map, corner map, surf 1-NN cloud, corner 1-NN cloud), and stale[s] = 1 where the sequence's 1-NN cloud is not its
+   map (the last refresh failed the >= 5 && >= 20 guard; its 1-NN cloud is the tree range, else that range is empty). */
+int lins_gpu_seq_download_ieskf(lins_ctx* ctx, double* prior_state /*S x 19*/, double* prior_cov /*S x 324*/,
+                                double* state_out /*S x 19*/, double* cov_out /*S x 324*/, int32_t* query_off,
+                                int32_t* surf_ind, int32_t* corner_ind);
+int lins_gpu_seq_download_maps(lins_ctx* ctx, int32_t* off, float* surf_map, float* corner_map, float* surf_tree,
+                               float* corner_tree, uint8_t* stale /*S*/);
 
 /* Split "Jacobian kernel" (SURVEY.md §8(d) unit U1): residual + Jacobian row + 29-scalar reduction over the
    resident batch given the correspondence IDs of iteration `iter` of each scan's current linearisation

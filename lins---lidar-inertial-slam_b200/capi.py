@@ -13,8 +13,8 @@ import subprocess
 
 import numpy as np
 
-from .ctypes_defs import (Batch, COV_SIZE, LinsBatchDesc, LinsMapReport, LinsParams, LinsReport, LinsScanResult, POINT_DTYPE,
-                          SCAN_RESULT_DTYPE, STATE_DIM, as_points, ptr)
+from .ctypes_defs import (Batch, COV_SIZE, LinsBatchDesc, LinsMapReport, LinsParams, LinsReport, LinsScanResult, LinsSeqBeginDesc,
+                          LinsSeqParams, LinsSeqStepDesc, POINT_DTYPE, SCAN_RESULT_DTYPE, STATE_DIM, as_points, ptr)
 
 _PKG = os.path.dirname(os.path.abspath(__file__))
 _ROOT = os.path.dirname(_PKG)
@@ -29,15 +29,17 @@ EXPORTS = [
     "lins_gpu_batch_results_device", "lins_gpu_batch_jacobian_pass", "lins_gpu_launch_count", "lins_gpu_sync",
     "lins_gpu_debug_phase_cycles", "lins_gpu_map_set", "lins_gpu_scan2map", "lins_gpu_map_associate",
     "lins_gpu_host_register", "lins_gpu_host_unregister", "lins_gpu_batch_download_indices", "lins_gpu_update_map_ex",
-    "lins_gpu_batch_upload_stats",
+    "lins_gpu_batch_upload_stats", "lins_gpu_seq_begin", "lins_gpu_seq_step", "lins_gpu_seq_download",
+    "lins_gpu_seq_phase_ms", "lins_gpu_seq_download_ieskf", "lins_gpu_seq_download_maps", "lins_gpu_download_indices",
 ]
 
 NVCC_ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]  # H100 (Hopper)
 NVCC_COMMON = NVCC_ARCH + ["-lineinfo", "-O3", "-std=c++17", "-Xcompiler", "-fPIC"]
 # translation units and their extra flags: lins_gpu.cu (the fused kernel and most of the C-ABI), lins_upload.cu (batch
-# upload), lins_map.cu (row F2's host side) — all bit-exact, so no multiply-add contraction: the association and the map
+# upload), lins_map.cu (row F2's host side), lins_seq.cu (sequence mode) — all bit-exact, so no multiply-add contraction: the association and the map
 # fits depend on it — and lins_jacobian.cu (the tolerance-checked split Jacobian kernel: contraction allowed)
-UNITS = [("lins_gpu.cu", ["-fmad=false"]), ("lins_upload.cu", ["-fmad=false"]), ("lins_map.cu", ["-fmad=false"]), ("lins_jacobian.cu", [])]
+UNITS = [("lins_gpu.cu", ["-fmad=false"]), ("lins_upload.cu", ["-fmad=false"]), ("lins_map.cu", ["-fmad=false"]),
+         ("lins_seq.cu", ["-fmad=false"]), ("lins_jacobian.cu", [])]
 NVCC_FLAGS = NVCC_COMMON + ["-fmad=false", "-shared"]  # (what tools/ scripts print)
 
 
@@ -103,6 +105,13 @@ def lib():
         if hasattr(L, "lins_gpu_batch_upload_stats"):
             L.lins_gpu_batch_upload_stats.argtypes = [vp, C.POINTER(C.c_int64), C.POINTER(C.c_int64)]
         L.lins_gpu_host_unregister.argtypes = [vp]
+        L.lins_gpu_seq_begin.argtypes = [vp, C.POINTER(LinsSeqParams), C.POINTER(LinsSeqBeginDesc)]
+        L.lins_gpu_seq_step.argtypes = [vp, C.POINTER(LinsSeqStepDesc)]
+        L.lins_gpu_seq_download.argtypes = [vp, f64p, f64p, f64p, vp, vp, vp]
+        L.lins_gpu_seq_phase_ms.argtypes = [vp, vp]
+        L.lins_gpu_seq_download_ieskf.argtypes = [vp] + [vp] * 7
+        L.lins_gpu_seq_download_maps.argtypes = [vp] + [vp] * 6
+        L.lins_gpu_download_indices.argtypes = [vp, vp, vp]
         _LIB = L
     return _LIB
 
@@ -213,6 +222,12 @@ class LinsGpu:
                                            ptr(out["corner_sel"])))
         return out
 
+    def download_indices(self, n_surf, n_corner):
+        """(surf_ind (n_surf, 3), corner_ind (n_corner, 2)) of the last single-scan call's last search iteration."""
+        si, ci = np.full((n_surf, 3), -2, np.int32), np.full((n_corner, 2), -2, np.int32)
+        self._ck(self.L.lins_gpu_download_indices(self.h, ptr(si), ptr(ci)))
+        return si, ci
+
     def estimate_transform(self, surf_flat, corner_sharp, t, q_xyzw):
         s, c = as_points(surf_flat), as_points(corner_sharp)
         pose = np.ascontiguousarray(np.concatenate([np.asarray(t, float), np.asarray(q_xyzw, float)]))
@@ -312,3 +327,89 @@ class LinsGpu:
         acc = np.zeros((self._batch_n, 32)) if want_accum else None
         self._ck(self.L.lins_gpu_batch_jacobian_pass(self.h, ptr(acc)))
         return acc
+
+    # ---- sequence mode ---------------------------------------------------------------------------------------------
+    def seq_begin(self, params, handover):
+        """Hand over S running sequences (each right after its processSecondScan).  `handover`: dict with filter_state
+        (S x 19), filter_cov (S x 324), global_state (S x 19), imu_last (S x 6), surf_map / corner_map (POINT_DTYPE clouds)
+        and their (S + 1) offsets surf_map_off / corner_map_off."""
+        h = {k: np.ascontiguousarray(handover[k], dtype=np.float64) for k in ("filter_state", "filter_cov", "global_state", "imu_last")}
+        for k in ("surf_map", "corner_map"):
+            h[k] = as_points(handover[k])
+            h[k + "_off"] = np.ascontiguousarray(handover[k + "_off"], dtype=np.int32)
+        d = LinsSeqBeginDesc()
+        d.n_seq = len(h["surf_map_off"]) - 1
+        for k, v in h.items():
+            setattr(d, k, v.ctypes.data)
+        self._ck(self.L.lins_gpu_seq_begin(self.h, C.byref(params), C.byref(d)))
+        self._seq_n = d.n_seq
+
+    def seq_step(self, step):
+        """Advance every present sequence by one scan.  `step`: dict with imu (k x 7: dt, acc, gyr) + imu_off, the four
+        feature clouds (Batch.FIELDS) + their offsets (<name>_off), and optionally present (S, uint8)."""
+        keep = {"imu": np.ascontiguousarray(step["imu"], dtype=np.float64), "imu_off": np.ascontiguousarray(step["imu_off"], dtype=np.int32)}
+        for k in Batch.FIELDS:
+            keep[k] = as_points(step[k])
+            keep[k + "_off"] = np.ascontiguousarray(step[k + "_off"], dtype=np.int32)
+        d = LinsSeqStepDesc()
+        d.n_seq = len(keep["imu_off"]) - 1
+        d.point_format = int(step.get("point_format", 0))
+        if step.get("present") is not None:
+            keep["present"] = np.ascontiguousarray(step["present"], dtype=np.uint8)
+        for k, v in keep.items():
+            setattr(d, k, v.ctypes.data)
+        self._ck(self.L.lins_gpu_seq_step(self.h, C.byref(d)))
+
+    def seq_download(self, reports=False):
+        """dict: global_state, filter_state (S x 19), filter_cov (S x 324), results (SCAN_RESULT_DTYPE), status (S) and,
+        when asked for, reports (LinsReport array)."""
+        n = self._seq_n
+        out = dict(global_state=np.zeros((n, STATE_DIM)), filter_state=np.zeros((n, STATE_DIM)), filter_cov=np.zeros((n, COV_SIZE)),
+                   results=np.zeros(n, dtype=SCAN_RESULT_DTYPE), status=np.zeros(n, np.int32))
+        reps = (LinsReport * n)() if reports else None
+        self._ck(self.L.lins_gpu_seq_download(self.h, ptr(out["global_state"]), ptr(out["filter_state"]), ptr(out["filter_cov"]),
+                                              ptr(out["results"]), C.cast(reps, C.c_void_p) if reports else None, ptr(out["status"])))
+        if reports:
+            out["reports"] = reps
+        return out
+
+    def seq_phase_ms(self):
+        """CUDA-event times (ms) of the last seq_step's phases: predict, IESKF, divergence check + ICP fallback, post + map."""
+        ms = np.zeros(4, np.float32)
+        self._ck(self.L.lins_gpu_seq_phase_ms(self.h, ptr(ms)))
+        return ms
+
+    def seq_download_ieskf(self):
+        """The last step's IESKF: prior_state / prior_cov (every sequence), state_out / cov_out, and per sequence that ran its
+        last-iteration correspondence IDs: surf_ind[s] (ns, 3), corner_ind[s] (nc, 2) (None for a sequence that did not run)."""
+        n = self._seq_n
+        off = np.zeros(2 * (n + 1), np.int32)
+        self._ck(self.L.lins_gpu_seq_download_ieskf(self.h, None, None, None, None, ptr(off), None, None))
+        so, co = off[: n + 1], off[n + 1:]
+        out = dict(prior_state=np.zeros((n, STATE_DIM)), prior_cov=np.zeros((n, COV_SIZE)), state_out=np.zeros((n, STATE_DIM)),
+                   cov_out=np.zeros((n, COV_SIZE)))
+        si, ci = np.zeros((so[-1], 3), np.int32), np.zeros((co[-1], 2), np.int32)
+        ran = so[-1] + co[-1] > 0
+        self._ck(self.L.lins_gpu_seq_download_ieskf(self.h, ptr(out["prior_state"]), ptr(out["prior_cov"]),
+                                                    ptr(out["state_out"]) if ran else None, ptr(out["cov_out"]) if ran else None,
+                                                    None, ptr(si), ptr(ci)))
+        out["surf_ind"] = [si[so[s]:so[s + 1]] for s in range(n)]
+        out["corner_ind"] = [ci[co[s]:co[s + 1]] for s in range(n)]
+        return out
+
+    def seq_download_maps(self):
+        """The maps the next step searches: per sequence surf_map, corner_map, surf_tree, corner_tree (POINT_DTYPE clouds)
+        and stale (S,)."""
+        n = self._seq_n
+        off = np.zeros(4 * (n + 1), np.int32)
+        self._ck(self.L.lins_gpu_seq_download_maps(self.h, ptr(off), None, None, None, None, None))
+        o = off.reshape(4, n + 1)
+        bufs = [np.zeros((o[c, -1], 4), np.float32) for c in range(4)]
+        stale = np.zeros(n, np.uint8)
+        self._ck(self.L.lins_gpu_seq_download_maps(self.h, None, *[ptr(b) for b in bufs], ptr(stale)))
+        out = dict(stale=stale)
+        for c, name in enumerate(("surf_map", "corner_map", "surf_tree", "corner_tree")):
+            pts = np.zeros(o[c, -1], POINT_DTYPE)
+            pts["x"], pts["y"], pts["z"], pts["intensity"] = bufs[c][:, 0], bufs[c][:, 1], bufs[c][:, 2], bufs[c][:, 3]
+            out[name] = [pts[o[c, s]:o[c, s + 1]] for s in range(n)]
+        return out

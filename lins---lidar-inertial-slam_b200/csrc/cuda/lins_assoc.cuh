@@ -349,10 +349,11 @@ __device__ void association_pass(CtaMem& cta, Smem* slots, const BatchView& bv, 
     for (int sl = 0; sl < bv.nslots; ++sl) {
       const Smem& sm = slots[sl];
       if (!sm.run || sm.az_ok || (sm.iter % kp.icp_freq) != 0) continue;
-      const float4* __restrict__ nnS = bv.nn_s ? bv.nn_s + bv.nn_s_off[sm.scan] : bv.ts + sm.ts0;
-      const float4* __restrict__ nnC = bv.nn_c ? bv.nn_c + bv.nn_c_off[sm.scan] : bv.tc + sm.tc0;
-      const int TnS = bv.nn_s ? bv.nn_s_off[sm.scan + 1] - bv.nn_s_off[sm.scan] : sm.Ts;
-      const int TnC = bv.nn_c ? bv.nn_c_off[sm.scan + 1] - bv.nn_c_off[sm.scan] : sm.Tc;
+      const bool sep = nn_separate(bv, sm.scan);
+      const float4* __restrict__ nnS = sep ? bv.nn_s + bv.nn_s_off[sm.scan] : bv.ts + sm.ts0;
+      const float4* __restrict__ nnC = sep ? bv.nn_c + bv.nn_c_off[sm.scan] : bv.tc + sm.tc0;
+      const int TnS = sep ? bv.nn_s_off[sm.scan + 1] - bv.nn_s_off[sm.scan] : sm.Ts;
+      const int TnC = sep ? bv.nn_c_off[sm.scan + 1] - bv.nn_c_off[sm.scan] : sm.Tc;
       if (sm.ns > 0 && TnS > 0) nn_brute(pb.sel + sl * Q, pb.key + sl * Q, sm.ns, nnS, TnS);
       if (sm.nc > 0 && TnC > 0) nn_brute(pb.sel + sl * Q + sm.ns, pb.key + sl * Q + sm.ns, sm.nc, nnC, TnC);
     }

@@ -1,6 +1,6 @@
 // lins_ctx.hpp — host state of a C-ABI context (struct lins_ctx of include/lins_gpu.h) and the helpers the translation units
 // that implement the C-ABI share: lins_gpu.cu (fused kernel, single-scan and batched entry points, F1), lins_upload.cu
-// (batch upload), lins_map.cu (row F2).  Host code only: a header that defines kernels cannot be included here, because
+// (batch upload), lins_map.cu (row F2), lins_seq.cu (sequence mode).  Host code only: a header that defines kernels cannot be included here, because
 // every unit that includes this one would define them again.
 #pragma once
 #include <cuda_runtime.h>
@@ -13,11 +13,12 @@
 #include <cstdint>
 #include <string>
 #include <utility>
+#include <vector>
 
 #include "../../../include/lins_gpu.h"
 #include "../host/host_pool.hpp"
 
-namespace lins_dev { struct IcpState; }                       // lins_icp_step.cuh
+namespace lins_dev { struct IcpState; struct BatchView; }     // lins_icp_step.cuh, lins_kernels.cuh
 namespace lins_map { struct PassConsts; struct MapLoopState; }  // lins_map.cuh
 
 namespace lins_capi {
@@ -77,6 +78,40 @@ struct Resident {  // one resident batch (device) + its pinned staging (host)
   Buf<lins_report, kPinned> h_reports;
 };
 
+// One contiguous device-to-device copy of sequence mode (lins_seq.cu): query compaction and the map refresh
+struct SeqCopy { const float4* src; float4* dst; int n, pad; };
+
+// Sequence mode (lins_gpu_seq_*, lins_seq.cu): the running sequences' filter state and maps.  Maps are CSR over the
+// sequences in sequence order; `tree` holds the cloud a sequence's 1-NN index was last built on where that differs from
+// its map (stale[s] = 1, after a refresh that failed the >=5 && >=20 guard), and is empty elsewhere.
+struct SeqState {
+  int n = 0;                      // sequences (0 = lins_gpu_seq_begin has not run)
+  double consts[10];              // lins_seq::Consts
+  Buf<double> filt, cov, glob, lin, imu_last, icp_pose;  // n x 20, n x 324, n x 20, n x 20, n x 8, n x 20
+  Buf<double> prior_state, prior_cov;                  // the last step's IESKF prior (after the IMU propagation)
+  Buf<int> icp_ind_s, icp_ind_c;                       // correspondence IDs of the ICP fallback (the IESKF's stay in run)
+  Buf<unsigned char> icp;                              // n IcpState records (lins_icp_step.cuh; icp_state_bytes() each)
+  Buf<float4> map_s, map_c, tree_s, tree_c;            // current generation
+  Buf<float4> nmap_s, nmap_c, ntree_s, ntree_c;        // next generation (built by the step, then swapped in)
+  Buf<int> map_off;                                    // 4 x (n + 1): map_s, map_c, tree_s, tree_c
+  Buf<unsigned char> stale;
+  std::vector<int> h_map_off, h_nmap_off;              // host copies of map_off
+  std::vector<unsigned char> h_stale_v;
+  Resident up;                                         // the step's four uploaded clouds (qs, qc, ts = new less-flat, tc = new less-sharp)
+  Resident run;                                        // the IESKF batch: compacted queries of the sequences that run, outputs
+  Buf<double> imu; Buf<int> imu_off;
+  Buf<double, kPinned> h_imu; Buf<int, kPinned> h_imu_off;
+  Buf<unsigned char> status_d;                         // n: LINS_SEQ_* of the step (read by the post kernel)
+  Buf<unsigned char, kPinned> h_status;
+  Buf<SeqCopy> copies; Buf<SeqCopy, kPinned> h_copies;
+  std::vector<int32_t> status;                         // host copy of status_d
+  cudaEvent_t ev[5] = {nullptr, nullptr, nullptr, nullptr, nullptr};  // phase boundaries of the last step (lins_gpu_seq_phase_ms)
+  bool ev_valid = false;
+  bool has_step = false;                               // a step has run since lins_gpu_seq_begin
+  std::vector<int> h_run_off;                          // 2 x (n + 1): the last step's compacted query offsets (surf, corner)
+  ~SeqState() { for (cudaEvent_t e : ev) if (e) cudaEventDestroy(e); }
+};
+
 }  // namespace lins_capi
 
 struct lins_ctx {
@@ -96,6 +131,7 @@ struct lins_ctx {
   int64_t upload_raw_points = 0, upload_packed_points = 0;  // cumulative split of lins_gpu_batch_upload (raw DMA vs host pack)
   lins_capi::Resident batch;   // lins_gpu_batch_* working set
   lins_capi::Resident single;  // lins_gpu_ieskf / associate / estimate_transform (n = 1)
+  lins_capi::SeqState seq;     // lins_gpu_seq_*
   // the single-scan map: "last" clouds (walks + tripods) and the clouds the 1-NN index was built on
   Buf<float4> map_s, map_c, tree_s, tree_c;
   Buf<int> map_off;  // 4 x 2 ints: [0,ns][0,nc][0,tns][0,tnc]
@@ -221,5 +257,16 @@ inline int upload2(lins_ctx* ctx, Buf<float4>& dst_a, const lins_point* a, int n
   const int rc = upload2_reserve(ctx, dst_a, na, dst_b, nb);
   return rc != LINS_OK ? rc : upload2_queue(ctx, dst_a, a, na, dst_b, b, nb);
 }
+
+// lins_upload.cu: validate n units' four CSR clouds (the lins_batch_desc order: surf_flat, corner_sharp, surf_less_flat,
+// corner_less_sharp) and upload them with their offsets into r (qs, qc, ts, tc); sets r.n, the totals and r.max_q
+int upload_clouds(lins_ctx* ctx, Resident& r, int n, const lins_point* const pts[4], const int32_t* const offs[4], int point_format);
+// lins_gpu.cu: the fused kernel's IESKF launch over bv (with r's scratch), its query tile, the estimateTransform loop of
+// one device-resident unit, and the CSR transformToEnd of the units with run[u] != 0 (lin: 20 doubles per unit)
+int fused_ieskf_launch(lins_ctx* ctx, Resident& r, const lins_dev::BatchView& bv);
+int fused_qtile(int max_q);
+size_t icp_state_bytes();
+int icp_loop(lins_ctx* ctx, Resident& r, lins_dev::BatchView bv, double* pose, lins_dev::IcpState* icp, int icp_index = 0);
+int transform_to_end_csr(lins_ctx* ctx, float4* pts, const int* off, int n_units, const double* lin, const unsigned char* run);
 
 }  // namespace lins_capi

@@ -57,7 +57,7 @@ __device__ void unit_prologue(CtaMem& cta, Smem& sm, const BatchView& bv, const 
   check_ring_sorted(bv.tc + sm.tc0, sm.Tc, &sm.sortedC);
   if (tid == 0) {
     // slot payload = ring (7 bits) | index (24 bits); bucket tables hold 16-bit slots
-    const bool ok = sm.sortedS && sm.sortedC && bv.nn_s == nullptr && bv.nn_c == nullptr && sm.Ts < 65536 && sm.Tc < 65536;
+    const bool ok = sm.sortedS && sm.sortedC && !nn_separate(bv, scan) && sm.Ts < 65536 && sm.Tc < 65536;
     sm.az_ok = ok ? 1 : 0;
     sm.nringsS = ok && sm.Ts > 0 ? (int)bv.ts[sm.ts0 + sm.Ts - 1].w + 1 : 0;  // ring-sorted: the last point has the largest ring
     sm.nringsC = ok && sm.Tc > 0 ? (int)bv.tc[sm.tc0 + sm.Tc - 1].w + 1 : 0;
@@ -409,10 +409,9 @@ __global__ void __launch_bounds__(kJacThreads, kJacMinBlocks) lins_jacobian_kern
   }
 }
 
-// F1: transformToEnd (StateEstimator.hpp:1083-1101) of a packed cloud, in place on device.
-__global__ void lins_transform_to_end_kernel(float4* __restrict__ pts, int n, const double* __restrict__ lin,
-                                             double scan_period, lins_point* __restrict__ out32) {
-  __shared__ double sphi[3], srn[3], sq[4];
+// F1: transformToEnd (StateEstimator.hpp:1083-1101).  The per-scan constants (block-wide, into shared memory) and the
+// per-point body, shared by the single-cloud kernel and the CSR kernel of sequence mode.
+__device__ __forceinline__ void to_end_consts(const double* __restrict__ lin, double* sphi, double* srn, double* sq) {
   if (threadIdx.x == 0) {
     q4 q; q.x = lin[6]; q.y = lin[7]; q.z = lin[8]; q.w = lin[9];
     d3 phi = Quat2axis(q);
@@ -421,9 +420,8 @@ __global__ void lins_transform_to_end_kernel(float4* __restrict__ pts, int n, co
     sq[0] = q.x; sq[1] = q.y; sq[2] = q.z; sq[3] = q.w;
   }
   __syncthreads();
-  int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= n) return;
-  float4 p = pts[i];
+}
+__device__ __forceinline__ float4 to_end_point(float4 p, const double* sphi, const double* srn, const double* sq, double scan_period) {
   float fi = p.w - (float)((int)p.w);
   double s = (1.f / scan_period) * fi;
   q4 r = axis2Quat(mk3(s * sphi[0], s * sphi[1], s * sphi[2]));
@@ -431,6 +429,27 @@ __global__ void lins_transform_to_end_kernel(float4* __restrict__ pts, int n, co
   q4 q; q.x = sq[0]; q.y = sq[1]; q.z = sq[2]; q.w = sq[3];
   d3 P2 = qrot(qinverse(q), sub3(P1, mk3(srn[0], srn[1], srn[2])));
   p.x = (float)P2.x; p.y = (float)P2.y; p.z = (float)P2.z;
+  return p;
+}
+
+// CSR version: one block per unit u with run[u] != 0, its cloud pts[off[u], off[u+1]) with linState_ lin[20 u ..].
+__global__ void lins_transform_to_end_csr_kernel(float4* __restrict__ pts, const int* __restrict__ off, const double* __restrict__ lin,
+                                                 const unsigned char* __restrict__ run, double scan_period) {
+  __shared__ double sphi[3], srn[3], sq[4];
+  const int u = blockIdx.x;
+  if (!run[u]) return;
+  to_end_consts(lin + (size_t)u * 20, sphi, srn, sq);
+  for (int i = off[u] + threadIdx.x; i < off[u + 1]; i += blockDim.x) pts[i] = to_end_point(pts[i], sphi, srn, sq, scan_period);
+}
+
+// in place on a packed cloud; out32 (optional) receives full PointXYZI records
+__global__ void lins_transform_to_end_kernel(float4* __restrict__ pts, int n, const double* __restrict__ lin,
+                                             double scan_period, lins_point* __restrict__ out32) {
+  __shared__ double sphi[3], srn[3], sq[4];
+  to_end_consts(lin, sphi, srn, sq);
+  int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  float4 p = to_end_point(pts[i], sphi, srn, sq, scan_period);
   pts[i] = p;
   if (out32) {  // full pcl::PointXYZI records for a straight D2H into the caller's cloud
     float4* o = reinterpret_cast<float4*>(out32 + i);
@@ -580,6 +599,45 @@ int upload_map_offsets(lins_ctx* ctx) {
 
 }  // namespace
 
+// ---- what sequence mode (lins_seq.cu) runs of this unit: lins_ctx.hpp declares these ------------------------------------
+namespace lins_capi {
+
+int fused_ieskf_launch(lins_ctx* ctx, Resident& r, const BatchView& bv) {
+  return launch(ctx, r, bv, make_kparams(ctx->prm, MODE_IESKF, 0));
+}
+
+int fused_qtile(int max_q) { return choose_qtile(max_q); }
+
+size_t icp_state_bytes() { return sizeof(IcpState); }
+
+// the Gauss-Newton loop of estimateTransform on one unit whose queries, map and pose (state_in) are on the device: every
+// iteration is a reduction launch (MODE_ICP_REDUCE, linearised at bv.state_in) + the one-thread step kernel that updates
+// that pose; once the step kernel sets `done` the remaining queued launches return immediately.  No synchronisation.
+int icp_loop(lins_ctx* ctx, Resident& r, BatchView bv, double* pose, IcpState* icp, int icp_index) {
+  icp += icp_index;
+  CK(cudaMemsetAsync(icp, 0, sizeof(IcpState), ctx->stream));
+  bv.state_in = pose;
+  bv.icp_done = &icp->done;
+  for (int iter = 0; iter < ctx->prm.num_iter; ++iter) {
+    const int rc = launch(ctx, r, bv, make_kparams(ctx->prm, MODE_ICP_REDUCE, iter));
+    if (rc != LINS_OK) return rc;
+    lins_icp_step_kernel<<<1, 32, 0, ctx->stream>>>(bv.accum, pose, icp, iter);
+    CK(cudaGetLastError());
+    ctx->launches += 1;
+  }
+  return LINS_OK;
+}
+
+int transform_to_end_csr(lins_ctx* ctx, float4* pts, const int* off, int n_units, const double* lin, const unsigned char* run) {
+  if (n_units <= 0) return LINS_OK;
+  lins_transform_to_end_csr_kernel<<<n_units, 256, 0, ctx->stream>>>(pts, off, lin, run, ctx->prm.scan_period);
+  CK(cudaGetLastError());
+  ctx->launches += 1;
+  return LINS_OK;
+}
+
+}  // namespace lins_capi
+
 // =========================================================================================================
 // C-ABI
 // =========================================================================================================
@@ -664,6 +722,17 @@ int lins_gpu_ieskf(lins_ctx* ctx, const lins_point* surf_flat, int ns, const lin
   if (state_out) std::memcpy(state_out, r.h_state_out.p, sizeof(double) * 19);
   if (cov_out) std::memcpy(cov_out, r.h_cov_out.p, sizeof(double) * 324);
   if (rep) *rep = r.h_reports.p[0];
+  return LINS_OK;
+}
+
+int lins_gpu_download_indices(lins_ctx* ctx, int32_t* surf_ind, int32_t* corner_ind) {
+  if (!ctx) return LINS_E_INVALID;
+  Resident& r = ctx->single;
+  if (r.n != 1 || !r.ind_s.p) return fail(ctx, LINS_E_INVALID, "no single-scan call has run");
+  CK(cudaSetDevice(ctx->device));
+  if (surf_ind && r.nqs) CK(cudaMemcpyAsync(surf_ind, r.ind_s.p, sizeof(int32_t) * 3 * r.nqs, cudaMemcpyDeviceToHost, ctx->stream));
+  if (corner_ind && r.nqc) CK(cudaMemcpyAsync(corner_ind, r.ind_c.p, sizeof(int32_t) * 2 * r.nqc, cudaMemcpyDeviceToHost, ctx->stream));
+  CK(cudaStreamSynchronize(ctx->stream));
   return LINS_OK;
 }
 
@@ -908,9 +977,8 @@ int lins_gpu_estimate_transform(lins_ctx* ctx, const lins_point* surf_flat, int 
   if (!pose_io) return fail(ctx, LINS_E_INVALID, "null pose");
   CK(cudaSetDevice(ctx->device));
   if (std::getenv("LINS_ICP_HOST_LOOP")) return estimate_transform_host_loop(ctx, surf_flat, ns, corner_sharp, nc, pose_io, iters_out, converged_out);
-  // queries + initial pose are staged ONCE; every Gauss-Newton iteration is a reduction launch (MODE_ICP_REDUCE, linearised
-  // at the pose block on the device) + the one-thread step kernel that updates that block; once the step kernel sets
-  // `done` the remaining queued launches return immediately.  One D2H + one synchronisation at the end.
+  // queries + initial pose are staged ONCE, then the loop runs on the device (icp_loop).  One D2H + one synchronisation
+  // at the end.
   double lin[19];
   std::memset(lin, 0, sizeof(lin));
   lin[0] = pose_io[0]; lin[1] = pose_io[1]; lin[2] = pose_io[2];
@@ -919,16 +987,8 @@ int lins_gpu_estimate_transform(lins_ctx* ctx, const lins_point* surf_flat, int 
   if (rc != LINS_OK) return rc;
   Resident& r = ctx->single;
   CK(r.icp.reserve(1)); CK(r.h_icp.reserve(1)); CK(r.h_state_out.reserve(20));
-  CK(cudaMemsetAsync(r.icp.p, 0, sizeof(IcpState), ctx->stream));
-  for (int iter = 0; iter < ctx->prm.num_iter; ++iter) {
-    BatchView bv = single_view(ctx, false);
-    bv.icp_done = &r.icp.p->done;
-    rc = launch(ctx, r, bv, make_kparams(ctx->prm, MODE_ICP_REDUCE, iter));
-    if (rc != LINS_OK) return rc;
-    lins_icp_step_kernel<<<1, 32, 0, ctx->stream>>>(r.accum.p, r.state_in.p, r.icp.p, iter);
-    CK(cudaGetLastError());
-    ctx->launches += 1;
-  }
+  rc = icp_loop(ctx, r, single_view(ctx, false), r.state_in.p, r.icp.p);
+  if (rc != LINS_OK) return rc;
   CK(cudaMemcpyAsync(r.h_state_out.p, r.state_in.p, sizeof(double) * 20, cudaMemcpyDeviceToHost, ctx->stream));
   CK(cudaMemcpyAsync(r.h_icp.p, r.icp.p, sizeof(IcpState), cudaMemcpyDeviceToHost, ctx->stream));
   CK(cudaStreamSynchronize(ctx->stream));

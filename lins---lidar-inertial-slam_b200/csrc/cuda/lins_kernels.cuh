@@ -54,6 +54,7 @@ struct BatchView {
   // failed the >=5 && >=20 guard (StateEstimator.hpp:1156-1157): scan_last_ advanced, the kd-trees did not.
   const float4* nn_s; const int* nn_s_off;
   const float4* nn_c; const int* nn_c_off;
+  const unsigned char* nn_stale;         // per unit: 1 = nn_s / nn_c hold its 1-NN clouds; null = every unit's do (when nn_s is set)
   const double* state_in;                // n x 20 (19 used)
   const double* cov_in;                  // n x 324, column-major
   double* state_out;                     // n x 20
@@ -81,6 +82,11 @@ struct KParams {
   int num_iter, icp_freq, force_all_iters, mode, iter0;
   double nearest_sq, lidar_std, lidar_scale, scan_period;
 };
+
+// unit `scan` searches a 1-NN cloud of its own (a stale index: brute-force 1-NN over it, then walks over the map)
+__device__ __forceinline__ bool nn_separate(const BatchView& bv, int scan) {
+  return bv.nn_s != nullptr && (bv.nn_stale == nullptr || bv.nn_stale[scan] != 0);
+}
 
 __device__ __forceinline__ unsigned long long pack_key(float d, unsigned int lo) {
   return ((unsigned long long)__float_as_uint(d) << 32) | lo;

@@ -1,0 +1,482 @@
+// lins_seq.cu — sequence mode (include/lins_gpu.h: lins_gpu_seq_*): S running sequences advanced one scan per step with
+// the whole per-scan chain of StateEstimator on the device:
+//   predict x k (lins_seq_predict_kernel) -> processScan gate (host: it only reads cloud sizes) -> IESKF (the fused kernel,
+//   one launch) -> divergence check (one D2H) -> estimateTransform loop per diverged sequence (lins_gpu.cu: icp_loop) ->
+//   update / integrateTransformation / reset(1) / roll-pitch (lins_seq_post_kernel) -> transformToEnd (CSR kernel of
+//   lins_gpu.cu) + the guarded map swap (lins_seq_copy_kernel).
+// The filter algebra is lins_seq_step.cuh, shared with the CPU test.  Built with -fmad=false like the other bit-exact units.
+#include <cuda_runtime.h>
+
+#include <algorithm>
+#include <cmath>
+#include <cstring>
+#include <vector>
+
+#include "lins_ctx.hpp"
+#include "lins_kernels.cuh"
+#include "lins_seq_step.cuh"
+
+using namespace lins_capi;
+using lins_dev::BatchView;
+
+namespace {
+
+// One warp per sequence: the sequence's k StatePredictor::predict calls in order (kalman_filter.hpp:98-170).  The 18x18
+// matrices live in shared memory; lane l owns the entries e = l, l + 32, ... of every matrix phase, each entry summed in
+// the host's order.
+__global__ void __launch_bounds__(32) lins_seq_predict_kernel(double* __restrict__ filt, double* __restrict__ cov, double* __restrict__ imu_last,
+                                                             const double* __restrict__ imu, const int* __restrict__ imu_off,
+                                                             const unsigned char* __restrict__ status, const lins_seq::Consts k) {
+  const int s = blockIdx.x, lane = threadIdx.x;
+  if (status[s] == LINS_SEQ_IDLE) return;
+  const int m0 = imu_off[s], m1 = imu_off[s + 1];
+  if (m0 == m1) return;
+  __shared__ double P[324], Ft[324], F[324], FP[324], P2[324];
+  __shared__ double st[20], al[3], gl[3];
+  __shared__ lins_seq::PredictBlocks sb;  // R, va, aa of the sample being applied
+  double* S = filt + (size_t)s * 20;
+  double* C = cov + (size_t)s * 324;
+  for (int e = lane; e < 324; e += 32) P[e] = C[e];
+  if (lane < 20) st[lane] = S[lane];
+  if (lane < 3) { al[lane] = imu_last[(size_t)s * 8 + lane]; gl[lane] = imu_last[(size_t)s * 8 + 3 + lane]; }
+  __syncwarp();
+  for (int m = m0; m < m1; ++m) {
+    const double* smp = imu + (size_t)m * 7;
+    const double dt = smp[0];
+    if (lane == 0) {
+      sb = lins_seq::predict_state(st, al, gl, dt, smp + 1, smp + 4);
+      for (int i = 0; i < 3; ++i) { al[i] = smp[1 + i]; gl[i] = smp[4 + i]; }
+    }
+    __syncwarp();
+    const lins_seq::PredictBlocks& b = sb;
+    for (int e = lane; e < 324; e += 32) Ft[e] = lins_seq::ft_entry(b, e / 18, e % 18);
+    __syncwarp();
+    for (int e = lane; e < 324; e += 32) F[e] = lins_seq::f_entry(Ft, e / 18, e % 18, dt);
+    __syncwarp();
+    for (int e = lane; e < 324; e += 32) FP[e] = lins_seq::fp_entry(F, P, e / 18, e % 18);
+    __syncwarp();
+    for (int e = lane; e < 324; e += 32) {
+      const int i = e / 18, j = e % 18;
+      P2[e] = lins_seq::fpft_entry(FP, F, lins_seq::q_entry(b, k.noise, i, j, dt), i, j);
+    }
+    __syncwarp();
+    for (int e = lane; e < 324; e += 32) { const int i = e / 18, j = e % 18; P[j * 18 + i] = 0.5 * (P2[i * 18 + j] + P2[j * 18 + i]); }
+    __syncwarp();
+  }
+  for (int e = lane; e < 324; e += 32) C[e] = P[e];
+  if (lane < 20) S[lane] = st[lane];
+  if (lane < 3) { imu_last[(size_t)s * 8 + lane] = al[lane]; imu_last[(size_t)s * 8 + 3 + lane] = gl[lane]; }
+}
+
+// One thread per sequence that ran: filter_->update with the IESKF posterior (or, after divergence, the prior with
+// estimateTransform's pose and the prior covariance), integrateTransformation, reset(1), calculateRPfromGravity +
+// correctRollPitch (state_estimator.hpp:202-237).  lin receives linState_ (rn / qbn only after divergence, like the shim).
+__global__ void lins_seq_post_kernel(int n, const unsigned char* __restrict__ status, const double* __restrict__ state_out,
+                                     const double* __restrict__ cov_out, const double* __restrict__ icp_pose, double* __restrict__ filt,
+                                     double* __restrict__ cov, double* __restrict__ glob, double* __restrict__ lin, const lins_seq::Consts k) {
+  const int s = blockIdx.x * blockDim.x + threadIdx.x;
+  if (s >= n || status[s] < LINS_SEQ_RAN) return;
+  double f[20];
+  for (int i = 0; i < 20; ++i) f[i] = state_out[(size_t)s * 20 + i];
+  double* L = lin + (size_t)s * 20;
+  if (status[s] == LINS_SEQ_ICP) {
+    const double* p = icp_pose + (size_t)s * 20;
+    for (int i = 0; i < 10; ++i) if (i < 3 || i >= 6) { f[i] = p[i]; L[i] = p[i]; }
+  } else {
+    for (int i = 0; i < 20; ++i) L[i] = f[i];
+  }
+  double* P = cov + (size_t)s * 324;
+  for (int e = 0; e < 324; ++e) P[e] = cov_out[(size_t)s * 324 + e];
+  double* g = glob + (size_t)s * 20;
+  lins_seq::integrate(g, f);
+  lins_seq::reset1(f, P, k);
+  lins_seq::correct_roll_pitch(g, f);
+  for (int i = 0; i < 19; ++i) filt[(size_t)s * 20 + i] = f[i];
+}
+
+__global__ void lins_seq_copy_kernel(const SeqCopy* __restrict__ copies) {
+  const SeqCopy c = copies[blockIdx.x];
+  for (int i = threadIdx.x; i < c.n; i += blockDim.x) c.dst[i] = c.src[i];
+}
+
+lins_seq::Consts consts_of(const SeqState& q) {
+  lins_seq::Consts k;
+  std::memcpy(&k, q.consts, sizeof(k));
+  return k;
+}
+
+int check_csr(lins_ctx* ctx, const int32_t* off, int n, const void* data, const char* what) {
+  if (!off) return fail(ctx, LINS_E_INVALID, what);
+  if (off[0] != 0) return fail(ctx, LINS_E_INVALID, what);
+  for (int i = 0; i < n; ++i) if (off[i + 1] < off[i]) return fail(ctx, LINS_E_INVALID, what);
+  if (off[n] > 0 && !data) return fail(ctx, LINS_E_INVALID, what);
+  return LINS_OK;
+}
+
+int run_copies(lins_ctx* ctx, const SeqCopy* dev, int count) {
+  if (count <= 0) return LINS_OK;
+  lins_seq_copy_kernel<<<count, 256, 0, ctx->stream>>>(dev);
+  CK(cudaGetLastError());
+  ctx->launches += 1;
+  return LINS_OK;
+}
+
+}  // namespace
+
+static int seq_step_run(lins_ctx* ctx, const lins_seq_step_desc* d, const int32_t* const offs[4]);
+
+extern "C" {
+
+int lins_gpu_seq_begin(lins_ctx* ctx, const lins_seq_params* prm, const lins_seq_begin_desc* d) {
+  if (!ctx) return LINS_E_INVALID;
+  if (!prm || !d || d->n_seq < 1) return fail(ctx, LINS_E_INVALID, "bad sequence hand-over");
+  if (!d->filter_state || !d->filter_cov || !d->global_state || !d->imu_last) return fail(ctx, LINS_E_INVALID, "null hand-over state");
+  const int n = d->n_seq;
+  int rc = check_csr(ctx, d->surf_map_off, n, d->surf_map, "bad surf map offsets / cloud");
+  if (rc == LINS_OK) rc = check_csr(ctx, d->corner_map_off, n, d->corner_map, "bad corner map offsets / cloud");
+  if (rc != LINS_OK) return rc;
+  if (d->point_format != LINS_POINTS_XYZI32 && d->point_format != LINS_POINTS_PACKED16) return fail(ctx, LINS_E_INVALID, "bad point_format");
+  CK(cudaSetDevice(ctx->device));
+  SeqState& q = ctx->seq;
+  q.n = 0;  // (until the hand-over is in place)
+  // the maps go through the batch uploader as the target clouds of n units without queries
+  std::vector<int32_t> zeros(n + 1, 0);
+  const lins_point* pts[4] = {nullptr, nullptr, d->surf_map, d->corner_map};
+  const int32_t* offs[4] = {zeros.data(), zeros.data(), d->surf_map_off, d->corner_map_off};
+  rc = upload_clouds(ctx, q.up, n, pts, offs, d->point_format);
+  if (rc != LINS_OK) return rc;
+  const size_t ns = d->surf_map_off[n], nc = d->corner_map_off[n];
+  CK(q.filt.reserve((size_t)n * 20)); CK(q.cov.reserve((size_t)n * 324)); CK(q.glob.reserve((size_t)n * 20));
+  CK(q.lin.reserve((size_t)n * 20)); CK(q.imu_last.reserve((size_t)n * 8)); CK(q.icp_pose.reserve((size_t)n * 20)); CK(q.icp.reserve(icp_state_bytes() * n));
+  CK(q.map_s.reserve(ns + 1)); CK(q.map_c.reserve(nc + 1)); CK(q.tree_s.reserve(1)); CK(q.tree_c.reserve(1));
+  CK(q.map_off.reserve(4 * (size_t)(n + 1))); CK(q.stale.reserve(n));
+  if (ns) CK(cudaMemcpyAsync(q.map_s.p, q.up.ts.p, sizeof(float4) * ns, cudaMemcpyDeviceToDevice, ctx->stream));
+  if (nc) CK(cudaMemcpyAsync(q.map_c.p, q.up.tc.p, sizeof(float4) * nc, cudaMemcpyDeviceToDevice, ctx->stream));
+  std::vector<double> st((size_t)n * 20, 0.0), gl((size_t)n * 20, 0.0), il((size_t)n * 8, 0.0);
+  for (int s = 0; s < n; ++s) {
+    std::memcpy(&st[(size_t)s * 20], d->filter_state + (size_t)s * 19, sizeof(double) * 19);
+    std::memcpy(&gl[(size_t)s * 20], d->global_state + (size_t)s * 19, sizeof(double) * 19);
+    std::memcpy(&il[(size_t)s * 8], d->imu_last + (size_t)s * 6, sizeof(double) * 6);
+  }
+  q.h_map_off.assign(4 * (size_t)(n + 1), 0);
+  std::memcpy(&q.h_map_off[0], d->surf_map_off, sizeof(int) * (n + 1));
+  std::memcpy(&q.h_map_off[n + 1], d->corner_map_off, sizeof(int) * (n + 1));
+  q.h_stale_v.assign(n, 0);
+  CK(cudaMemcpyAsync(q.filt.p, st.data(), sizeof(double) * st.size(), cudaMemcpyHostToDevice, ctx->stream));
+  CK(cudaMemcpyAsync(q.lin.p, st.data(), sizeof(double) * st.size(), cudaMemcpyHostToDevice, ctx->stream));
+  CK(cudaMemcpyAsync(q.glob.p, gl.data(), sizeof(double) * gl.size(), cudaMemcpyHostToDevice, ctx->stream));
+  CK(cudaMemcpyAsync(q.imu_last.p, il.data(), sizeof(double) * il.size(), cudaMemcpyHostToDevice, ctx->stream));
+  CK(cudaMemcpyAsync(q.cov.p, d->filter_cov, sizeof(double) * 324 * (size_t)n, cudaMemcpyHostToDevice, ctx->stream));
+  CK(cudaMemcpyAsync(q.map_off.p, q.h_map_off.data(), sizeof(int) * q.h_map_off.size(), cudaMemcpyHostToDevice, ctx->stream));
+  CK(cudaMemcpyAsync(q.stale.p, q.h_stale_v.data(), n, cudaMemcpyHostToDevice, ctx->stream));
+  CK(cudaStreamSynchronize(ctx->stream));  // (the sources above are pageable host memory)
+  lins_seq::Consts k;
+  for (int i = 0; i < 4; ++i) k.noise[i] = prm->noise[i];
+  for (int i = 0; i < 3; ++i) {
+    k.pos_var[i] = prm->init_pos_std[i] * prm->init_pos_std[i];                 // sq(init_pos_std)
+    k.att_var[i] = std::pow(prm->init_att_std[i] * M_PI / 180.0, 2);            // pow(deg2rad(init_att_std), 2)
+  }
+  static_assert(sizeof(k) == sizeof(q.consts), "consts");
+  std::memcpy(q.consts, &k, sizeof(k));
+  // result records / reports read as zero until a step has run a sequence's IESKF
+  CK(q.run.results.reserve(n)); CK(q.run.reports.reserve(n));
+  CK(cudaMemsetAsync(q.run.results.p, 0, sizeof(lins_scan_result) * n, ctx->stream));
+  CK(cudaMemsetAsync(q.run.reports.p, 0, sizeof(lins_report) * n, ctx->stream));
+  q.ev_valid = false;
+  q.has_step = false;
+  q.status.assign(n, LINS_SEQ_IDLE);
+  q.n = n;
+  return LINS_OK;
+}
+
+int lins_gpu_seq_step(lins_ctx* ctx, const lins_seq_step_desc* d) {
+  if (!ctx) return LINS_E_INVALID;
+  SeqState& q = ctx->seq;
+  if (q.n == 0) return fail(ctx, LINS_E_NOMAP, "lins_gpu_seq_begin has not been called");
+  if (!d || d->n_seq != q.n) return fail(ctx, LINS_E_INVALID, "n_seq differs from the hand-over's");
+  const int n = q.n;
+  const int32_t* offs[4] = {d->surf_flat_off, d->corner_sharp_off, d->surf_less_flat_off, d->corner_less_sharp_off};
+  const lins_point* pts[4] = {d->surf_flat, d->corner_sharp, d->surf_less_flat, d->corner_less_sharp};
+  for (int k = 0; k < 4; ++k) { const int rc = check_csr(ctx, offs[k], n, pts[k], "bad cloud offsets / cloud"); if (rc != LINS_OK) return rc; }
+  if (d->imu_off) { const int rc = check_csr(ctx, d->imu_off, n, d->imu, "bad imu offsets / samples"); if (rc != LINS_OK) return rc; }
+  else if (d->imu) return fail(ctx, LINS_E_INVALID, "imu without imu_off");
+  CK(cudaSetDevice(ctx->device));
+  int rc = upload_clouds(ctx, q.up, n, pts, offs, d->point_format);  // (validates the rest; synchronises the stream first)
+  if (rc != LINS_OK) return rc;
+  // from here on the sequences' state changes: a failure ends the run (lins_gpu.h), the context stays usable
+  rc = seq_step_run(ctx, d, offs);
+  if (rc != LINS_OK) q.n = 0;
+  return rc;
+}
+
+}  // extern "C"
+
+// the part of lins_gpu_seq_step after its input is validated and uploaded
+static int seq_step_run(lins_ctx* ctx, const lins_seq_step_desc* d, const int32_t* const offs[4]) {
+  SeqState& q = ctx->seq;
+  const int n = q.n;
+  int rc = LINS_OK;
+
+  // ---- host bookkeeping: who runs, the compacted queries, the next maps (all from sizes the host knows) --------------
+  std::vector<int32_t>& status = q.status;
+  const int* mo = q.h_map_off.data();
+  const int N1 = n + 1;
+  std::vector<int> run_off(2 * (size_t)N1, 0);  // compacted query offsets: surf, corner
+  q.h_nmap_off.assign(4 * (size_t)N1, 0);
+  int* no = q.h_nmap_off.data();
+  std::vector<SeqCopy> qcopies, mcopies;
+  std::vector<std::pair<int, int>> qto, mto;  // destination of each copy: (cloud, offset), resolved once the buffers exist
+  std::vector<unsigned char> new_stale(q.h_stale_v);
+  int max_q = 0, n_run = 0;
+  for (int s = 0; s < n; ++s) {
+    const bool present = !d->present || d->present[s];
+    const int nsl = offs[2][s + 1] - offs[2][s], ncl = offs[3][s + 1] - offs[3][s];
+    status[s] = !present ? LINS_SEQ_IDLE : (ncl <= 5 || nsl <= 10) ? LINS_SEQ_SKIPPED : LINS_SEQ_RAN;  // :436-440
+    const bool ran = status[s] == LINS_SEQ_RAN;
+    const int nq[2] = {ran ? offs[0][s + 1] - offs[0][s] : 0, ran ? offs[1][s + 1] - offs[1][s] : 0};
+    for (int c = 0; c < 2; ++c) {
+      run_off[c * N1 + s + 1] = run_off[c * N1 + s] + nq[c];
+      if (nq[c]) { qcopies.push_back(SeqCopy{(c ? q.up.qc.p : q.up.qs.p) + offs[c][s], nullptr, nq[c], 0}); qto.emplace_back(c, run_off[c * N1 + s]); }
+    }
+    if (ran) { max_q = std::max(max_q, nq[0] + nq[1]); ++n_run; }
+    // map swap (:1151-1160): the new clouds become the map; the 1-NN index is rebuilt iff ncl >= 5 && nsl >= 20, else it
+    // stays on the cloud it was built on (the old map, or an older stale cloud)
+    int len[4];  // map_s, map_c, tree_s, tree_c
+    int src_kind[4];  // 0 new cloud, 1 old map, 2 old tree, -1 none
+    if (ran) {
+      const bool guard = ncl >= 5 && nsl >= 20;
+      len[0] = nsl; len[1] = ncl; src_kind[0] = src_kind[1] = 0;
+      if (guard) { len[2] = len[3] = 0; src_kind[2] = src_kind[3] = -1; new_stale[s] = 0; }
+      else if (!q.h_stale_v[s]) { len[2] = mo[s + 1] - mo[s]; len[3] = mo[N1 + s + 1] - mo[N1 + s]; src_kind[2] = src_kind[3] = 1; new_stale[s] = 1; }
+      else { len[2] = mo[2 * N1 + s + 1] - mo[2 * N1 + s]; len[3] = mo[3 * N1 + s + 1] - mo[3 * N1 + s]; src_kind[2] = src_kind[3] = 2; }
+    } else {
+      for (int c = 0; c < 4; ++c) { len[c] = mo[c * N1 + s + 1] - mo[c * N1 + s]; src_kind[c] = c < 2 ? 1 : 2; }
+    }
+    for (int c = 0; c < 4; ++c) {
+      no[c * N1 + s + 1] = no[c * N1 + s] + len[c];
+      if (!len[c] || src_kind[c] < 0) continue;
+      const int cc = c & 1;  // surf / corner
+      const float4* src = nullptr;
+      if (src_kind[c] == 0) src = (cc ? q.up.tc.p : q.up.ts.p) + offs[2 + cc][s];
+      else if (src_kind[c] == 1) src = (cc ? q.map_c.p : q.map_s.p) + mo[cc * N1 + s];
+      else src = (cc ? q.tree_c.p : q.tree_s.p) + mo[(2 + cc) * N1 + s];
+      mcopies.push_back(SeqCopy{src, nullptr, len[c], 0});
+      mto.emplace_back(c, no[c * N1 + s]);
+    }
+  }
+
+  // ---- allocations ------------------------------------------------------------------------------------------------
+  Resident& r = q.run;
+  r.n = n; r.nqs = run_off[N1 - 1]; r.nqc = run_off[2 * N1 - 1]; r.max_q = max_q;
+  r.nts = mo[N1 - 1]; r.ntc = mo[2 * N1 - 1];
+  CK(r.qs.reserve(r.nqs + 1)); CK(r.qc.reserve(r.nqc + 1)); CK(r.qs_off.reserve(N1)); CK(r.qc_off.reserve(N1));
+  rc = reserve_outputs(ctx, r, true, false);
+  if (rc != LINS_OK) return rc;
+  CK(r.h_off.reserve(2 * (size_t)N1));
+  CK(q.nmap_s.reserve((size_t)no[N1 - 1] + 1)); CK(q.nmap_c.reserve((size_t)no[2 * N1 - 1] + 1));
+  CK(q.ntree_s.reserve((size_t)no[3 * N1 - 1] + 1)); CK(q.ntree_c.reserve((size_t)no[4 * N1 - 1] + 1));
+  const size_t n_imu = d->imu_off ? (size_t)d->imu_off[n] : 0;
+  CK(q.imu.reserve(7 * n_imu + 1)); CK(q.imu_off.reserve(N1)); CK(q.h_imu.reserve(7 * n_imu + 1)); CK(q.h_imu_off.reserve(N1));
+  CK(q.status_d.reserve(2 * (size_t)n)); CK(q.h_status.reserve(2 * (size_t)n));
+  const size_t n_copies = qcopies.size() + mcopies.size();
+  CK(q.copies.reserve(n_copies + 1)); CK(q.h_copies.reserve(n_copies + 1));
+  CK(q.prior_state.reserve((size_t)n * 20)); CK(q.prior_cov.reserve((size_t)n * 324));
+  CK(q.icp_ind_s.reserve(3 * r.nqs + 4)); CK(q.icp_ind_c.reserve(2 * r.nqc + 4));
+  float4* qdst[2] = {r.qs.p, r.qc.p};
+  float4* mdst[4] = {q.nmap_s.p, q.nmap_c.p, q.ntree_s.p, q.ntree_c.p};
+  for (size_t i = 0; i < qcopies.size(); ++i) qcopies[i].dst = qdst[qto[i].first] + qto[i].second;
+  for (size_t i = 0; i < mcopies.size(); ++i) mcopies[i].dst = mdst[mto[i].first] + mto[i].second;
+
+  // ---- uploads: IMU, status, copy lists, compacted query offsets ---------------------------------------------------
+  if (d->imu_off) std::memcpy(q.h_imu_off.p, d->imu_off, sizeof(int) * N1);
+  else std::memset(q.h_imu_off.p, 0, sizeof(int) * N1);
+  if (n_imu) std::memcpy(q.h_imu.p, d->imu, sizeof(double) * 7 * n_imu);
+  for (int s = 0; s < n; ++s) q.h_status.p[s] = (unsigned char)status[s];
+  std::copy(qcopies.begin(), qcopies.end(), q.h_copies.p);
+  std::copy(mcopies.begin(), mcopies.end(), q.h_copies.p + qcopies.size());
+  std::memcpy(r.h_off.p, run_off.data(), sizeof(int) * 2 * N1);
+  if (n_imu) CK(cudaMemcpyAsync(q.imu.p, q.h_imu.p, sizeof(double) * 7 * n_imu, cudaMemcpyHostToDevice, ctx->stream));
+  CK(cudaMemcpyAsync(q.imu_off.p, q.h_imu_off.p, sizeof(int) * N1, cudaMemcpyHostToDevice, ctx->stream));
+  CK(cudaMemcpyAsync(q.status_d.p, q.h_status.p, n, cudaMemcpyHostToDevice, ctx->stream));
+  if (n_copies) CK(cudaMemcpyAsync(q.copies.p, q.h_copies.p, sizeof(SeqCopy) * n_copies, cudaMemcpyHostToDevice, ctx->stream));
+  CK(cudaMemcpyAsync(r.qs_off.p, r.h_off.p, sizeof(int) * N1, cudaMemcpyHostToDevice, ctx->stream));
+  CK(cudaMemcpyAsync(r.qc_off.p, r.h_off.p + N1, sizeof(int) * N1, cudaMemcpyHostToDevice, ctx->stream));
+
+  // ---- 1. IMU propagation -----------------------------------------------------------------------------------------
+  for (cudaEvent_t& e : q.ev) if (!e) CK(cudaEventCreate(&e));
+  q.ev_valid = false;
+  CK(cudaEventRecord(q.ev[0], ctx->stream));
+  const lins_seq::Consts k = consts_of(q);
+  if (n_imu) {
+    lins_seq_predict_kernel<<<n, 32, 0, ctx->stream>>>(q.filt.p, q.cov.p, q.imu_last.p, q.imu.p, q.imu_off.p, q.status_d.p, k);
+    CK(cudaGetLastError());
+    ctx->launches += 1;
+  }
+  // the prior of this step's IESKF (also what lins_gpu_seq_download_ieskf returns)
+  CK(cudaMemcpyAsync(q.prior_state.p, q.filt.p, sizeof(double) * 20 * (size_t)n, cudaMemcpyDeviceToDevice, ctx->stream));
+  CK(cudaMemcpyAsync(q.prior_cov.p, q.cov.p, sizeof(double) * 324 * (size_t)n, cudaMemcpyDeviceToDevice, ctx->stream));
+  CK(cudaEventRecord(q.ev[1], ctx->stream));
+  if (n_run == 0) {  // nothing passed the gate: the maps stay, nothing else to do
+    for (int e = 2; e < 5; ++e) CK(cudaEventRecord(q.ev[e], ctx->stream));
+    CK(cudaStreamSynchronize(ctx->stream));
+    q.ev_valid = true;
+    q.has_step = true;
+    q.h_run_off.swap(run_off);
+    return LINS_OK;
+  }
+
+  // ---- 2. IESKF over every sequence; those that do not run have no queries ------------------------------------------
+  rc = run_copies(ctx, q.copies.p, (int)qcopies.size());
+  if (rc != LINS_OK) return rc;
+  BatchView bv;
+  std::memset(&bv, 0, sizeof(bv));
+  bv.n_scans = n;
+  bv.qs = r.qs.p; bv.qs_off = r.qs_off.p; bv.qc = r.qc.p; bv.qc_off = r.qc_off.p;
+  bv.ts = q.map_s.p; bv.ts_off = q.map_off.p; bv.tc = q.map_c.p; bv.tc_off = q.map_off.p + N1;
+  bv.nn_s = q.tree_s.p; bv.nn_s_off = q.map_off.p + 2 * N1; bv.nn_c = q.tree_c.p; bv.nn_c_off = q.map_off.p + 3 * N1;
+  bv.nn_stale = q.stale.p;
+  bv.state_in = q.prior_state.p; bv.cov_in = q.prior_cov.p; bv.state_out = r.state_out.p; bv.cov_out = r.cov_out.p;
+  bv.results = r.results.p; bv.reports = r.reports.p;
+  bv.ind_s = r.ind_s.p; bv.ind_c = r.ind_c.p; bv.az_s = r.az_s.p; bv.az_c = r.az_c.p;
+  bv.accum = r.accum.p; bv.work_counter = r.counter.p;
+  bv.qtile = fused_qtile(r.max_q);
+  rc = fused_ieskf_launch(ctx, r, bv);
+  if (rc != LINS_OK) return rc;
+  CK(cudaEventRecord(q.ev[2], ctx->stream));
+
+  // ---- 3. divergence: one D2H of the result records -----------------------------------------------------------------
+  CK(r.h_results.reserve(n));
+  CK(cudaMemcpyAsync(r.h_results.p, r.results.p, sizeof(lins_scan_result) * n, cudaMemcpyDeviceToHost, ctx->stream));
+  CK(cudaStreamSynchronize(ctx->stream));
+  bool any_icp = false;
+  for (int s = 0; s < n; ++s) {
+    if (status[s] != LINS_SEQ_RAN || !(r.h_results.p[s].flags & 2u)) continue;
+    // estimateTransform from the prior's pose (performIESKF's "Using ICP Method" branch, StateEstimator.hpp:585-592)
+    status[s] = LINS_SEQ_ICP;
+    q.h_status.p[s] = LINS_SEQ_ICP;
+    any_icp = true;
+    CK(cudaMemcpyAsync(q.icp_pose.p + (size_t)s * 20, q.prior_state.p + (size_t)s * 20, sizeof(double) * 20, cudaMemcpyDeviceToDevice, ctx->stream));
+    BatchView u = bv;
+    u.n_scans = 1;
+    u.qs_off += s; u.qc_off += s; u.ts_off += s; u.tc_off += s; u.nn_s_off += s; u.nn_c_off += s; u.nn_stale += s;
+    u.cov_in += (size_t)s * 324; u.state_out += (size_t)s * 20; u.cov_out += (size_t)s * 324; u.results += s; u.reports = nullptr;
+    u.accum += (size_t)s * 32;
+    u.ind_s = q.icp_ind_s.p; u.ind_c = q.icp_ind_c.p;  // (the IESKF's IDs stay readable)
+    u.qtile = fused_qtile((run_off[s + 1] - run_off[s]) + (run_off[N1 + s + 1] - run_off[N1 + s]));
+    rc = icp_loop(ctx, r, u, q.icp_pose.p + (size_t)s * 20, reinterpret_cast<lins_dev::IcpState*>(q.icp.p), s);
+    if (rc != LINS_OK) return rc;
+  }
+  if (any_icp) CK(cudaMemcpyAsync(q.status_d.p, q.h_status.p, n, cudaMemcpyHostToDevice, ctx->stream));
+  CK(cudaEventRecord(q.ev[3], ctx->stream));
+
+  // ---- 4. update, integrateTransformation, reset(1), roll / pitch --------------------------------------------------
+  lins_seq_post_kernel<<<(n + 127) / 128, 128, 0, ctx->stream>>>(n, q.status_d.p, r.state_out.p, r.cov_out.p, q.icp_pose.p, q.filt.p, q.cov.p,
+                                                                   q.glob.p, q.lin.p, k);
+  CK(cudaGetLastError());
+  ctx->launches += 1;
+
+  // ---- 5. transformToEnd of the new less-* clouds + the guarded map swap --------------------------------------------
+  unsigned char* run_mask = q.status_d.p + n;
+  for (int s = 0; s < n; ++s) q.h_status.p[n + s] = status[s] >= LINS_SEQ_RAN ? 1 : 0;
+  CK(cudaMemcpyAsync(run_mask, q.h_status.p + n, n, cudaMemcpyHostToDevice, ctx->stream));
+  rc = transform_to_end_csr(ctx, q.up.ts.p, q.up.ts_off.p, n, q.lin.p, run_mask);
+  if (rc == LINS_OK) rc = transform_to_end_csr(ctx, q.up.tc.p, q.up.tc_off.p, n, q.lin.p, run_mask);
+  if (rc == LINS_OK) rc = run_copies(ctx, q.copies.p + qcopies.size(), (int)mcopies.size());
+  if (rc != LINS_OK) return rc;
+  std::swap(q.map_s, q.nmap_s); std::swap(q.map_c, q.nmap_c); std::swap(q.tree_s, q.ntree_s); std::swap(q.tree_c, q.ntree_c);
+  q.h_map_off.swap(q.h_nmap_off);
+  q.h_stale_v = new_stale;
+  CK(cudaMemcpyAsync(q.map_off.p, q.h_map_off.data(), sizeof(int) * 4 * N1, cudaMemcpyHostToDevice, ctx->stream));
+  CK(cudaMemcpyAsync(q.stale.p, q.h_stale_v.data(), n, cudaMemcpyHostToDevice, ctx->stream));
+  CK(cudaEventRecord(q.ev[4], ctx->stream));
+  CK(cudaStreamSynchronize(ctx->stream));  // (the two sources above are pageable and change with the next step)
+  q.ev_valid = true;
+  q.has_step = true;
+  q.h_run_off.swap(run_off);
+  return LINS_OK;
+}
+
+extern "C" {
+
+int lins_gpu_seq_phase_ms(lins_ctx* ctx, float* ms) {
+  if (!ctx || !ms) return LINS_E_INVALID;
+  SeqState& q = ctx->seq;
+  if (!q.ev_valid) return fail(ctx, LINS_E_INVALID, "no completed lins_gpu_seq_step");
+  CK(cudaSetDevice(ctx->device));
+  for (int i = 0; i < 4; ++i) CK(cudaEventElapsedTime(&ms[i], q.ev[i], q.ev[i + 1]));
+  return LINS_OK;
+}
+
+int lins_gpu_seq_download(lins_ctx* ctx, double* global_state, double* filter_state, double* filter_cov, lins_scan_result* results,
+                          lins_report* reports, int32_t* scan_status) {
+  if (!ctx) return LINS_E_INVALID;
+  SeqState& q = ctx->seq;
+  if (q.n == 0) return fail(ctx, LINS_E_NOMAP, "lins_gpu_seq_begin has not been called");
+  CK(cudaSetDevice(ctx->device));
+  const size_t n = q.n;
+  Resident& r = q.run;
+  if ((results || reports) && r.results.cap < n) return fail(ctx, LINS_E_INVALID, "no step has run an IESKF yet");
+  if (reports && r.reports.cap < n) return fail(ctx, LINS_E_INVALID, "no step has run an IESKF yet");
+  std::vector<double> g(global_state ? n * 20 : 0), f(filter_state ? n * 20 : 0);
+  if (global_state) CK(cudaMemcpyAsync(g.data(), q.glob.p, sizeof(double) * 20 * n, cudaMemcpyDeviceToHost, ctx->stream));
+  if (filter_state) CK(cudaMemcpyAsync(f.data(), q.filt.p, sizeof(double) * 20 * n, cudaMemcpyDeviceToHost, ctx->stream));
+  if (filter_cov) CK(cudaMemcpyAsync(filter_cov, q.cov.p, sizeof(double) * 324 * n, cudaMemcpyDeviceToHost, ctx->stream));
+  if (results) CK(cudaMemcpyAsync(results, r.results.p, sizeof(lins_scan_result) * n, cudaMemcpyDeviceToHost, ctx->stream));
+  if (reports) CK(cudaMemcpyAsync(reports, r.reports.p, sizeof(lins_report) * n, cudaMemcpyDeviceToHost, ctx->stream));
+  CK(cudaStreamSynchronize(ctx->stream));
+  for (size_t s = 0; s < n; ++s) {
+    if (global_state) std::memcpy(global_state + s * 19, &g[s * 20], sizeof(double) * 19);
+    if (filter_state) std::memcpy(filter_state + s * 19, &f[s * 20], sizeof(double) * 19);
+  }
+  if (scan_status) std::memcpy(scan_status, q.status.data(), sizeof(int32_t) * n);
+  return LINS_OK;
+}
+
+// ---- parity hooks: what the last step's IESKF saw and produced, and the maps the next step will use ---------------------
+int lins_gpu_seq_download_ieskf(lins_ctx* ctx, double* prior_state, double* prior_cov, double* state_out, double* cov_out,
+                                int32_t* query_off, int32_t* surf_ind, int32_t* corner_ind) {
+  if (!ctx) return LINS_E_INVALID;
+  SeqState& q = ctx->seq;
+  if (q.n == 0) return fail(ctx, LINS_E_NOMAP, "lins_gpu_seq_begin has not been called");
+  if (!q.has_step) return fail(ctx, LINS_E_INVALID, "no lins_gpu_seq_step since lins_gpu_seq_begin");
+  CK(cudaSetDevice(ctx->device));
+  const size_t n = q.n, N1 = n + 1;
+  Resident& r = q.run;
+  const int* ro = q.h_run_off.data();
+  const bool ran = ro[N1 - 1] + ro[2 * N1 - 1] > 0;  // (else the IESKF did not run and its outputs are not this step's)
+  if (!ran && (state_out || cov_out)) return fail(ctx, LINS_E_INVALID, "no sequence ran an IESKF in the last step");
+  std::vector<double> a(prior_state ? n * 20 : 0), b(state_out ? n * 20 : 0);
+  if (prior_state) CK(cudaMemcpyAsync(a.data(), q.prior_state.p, sizeof(double) * 20 * n, cudaMemcpyDeviceToHost, ctx->stream));
+  if (prior_cov) CK(cudaMemcpyAsync(prior_cov, q.prior_cov.p, sizeof(double) * 324 * n, cudaMemcpyDeviceToHost, ctx->stream));
+  if (state_out) CK(cudaMemcpyAsync(b.data(), r.state_out.p, sizeof(double) * 20 * n, cudaMemcpyDeviceToHost, ctx->stream));
+  if (cov_out) CK(cudaMemcpyAsync(cov_out, r.cov_out.p, sizeof(double) * 324 * n, cudaMemcpyDeviceToHost, ctx->stream));
+  if (surf_ind && ro[N1 - 1]) CK(cudaMemcpyAsync(surf_ind, r.ind_s.p, sizeof(int32_t) * 3 * ro[N1 - 1], cudaMemcpyDeviceToHost, ctx->stream));
+  if (corner_ind && ro[2 * N1 - 1]) CK(cudaMemcpyAsync(corner_ind, r.ind_c.p, sizeof(int32_t) * 2 * ro[2 * N1 - 1], cudaMemcpyDeviceToHost, ctx->stream));
+  CK(cudaStreamSynchronize(ctx->stream));
+  for (size_t s = 0; s < n; ++s) {
+    if (prior_state) std::memcpy(prior_state + s * 19, &a[s * 20], sizeof(double) * 19);
+    if (state_out) std::memcpy(state_out + s * 19, &b[s * 20], sizeof(double) * 19);
+  }
+  if (query_off) std::memcpy(query_off, ro, sizeof(int32_t) * 2 * N1);
+  return LINS_OK;
+}
+
+int lins_gpu_seq_download_maps(lins_ctx* ctx, int32_t* off, float* surf_map, float* corner_map, float* surf_tree, float* corner_tree,
+                               uint8_t* stale) {
+  if (!ctx) return LINS_E_INVALID;
+  SeqState& q = ctx->seq;
+  if (q.n == 0) return fail(ctx, LINS_E_NOMAP, "lins_gpu_seq_begin has not been called");
+  CK(cudaSetDevice(ctx->device));
+  const size_t N1 = q.n + 1;
+  const int* mo = q.h_map_off.data();
+  float* dst[4] = {surf_map, corner_map, surf_tree, corner_tree};
+  const float4* src[4] = {q.map_s.p, q.map_c.p, q.tree_s.p, q.tree_c.p};
+  for (int c = 0; c < 4; ++c)
+    if (dst[c] && mo[c * N1 + N1 - 1]) CK(cudaMemcpyAsync(dst[c], src[c], sizeof(float4) * mo[c * N1 + N1 - 1], cudaMemcpyDeviceToHost, ctx->stream));
+  CK(cudaStreamSynchronize(ctx->stream));
+  if (off) std::memcpy(off, mo, sizeof(int32_t) * 4 * N1);
+  if (stale) std::memcpy(stale, q.h_stale_v.data(), q.n);
+  return LINS_OK;
+}
+
+}  // extern "C"

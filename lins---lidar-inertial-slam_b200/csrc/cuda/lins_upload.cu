@@ -29,37 +29,27 @@ __global__ void lins_pack_points_kernel(const float4* __restrict__ raw, float4* 
 
 }  // namespace
 
-extern "C" {
+namespace lins_capi {
 
-int lins_gpu_batch_upload(lins_ctx* ctx, const lins_batch_desc* b) {
-  if (!ctx) return LINS_E_INVALID;
-  if (!b || b->n_scans < 0) return fail(ctx, LINS_E_INVALID, "bad batch");
-  CK(cudaSetDevice(ctx->device));
-  Resident& r = ctx->batch;
-  const int n = b->n_scans;
+int upload_clouds(lins_ctx* ctx, Resident& r, int n, const lins_point* const pts[4], const int32_t* const offs[4], int point_format) {
   CK(cudaStreamSynchronize(ctx->stream));  // the pinned staging of a previous upload may still be in flight
   r.n = n;
   if (n == 0) return LINS_OK;
-  const int32_t* offs[4] = {b->surf_flat_off, b->corner_sharp_off, b->surf_less_flat_off, b->corner_less_sharp_off};
-  const lins_point* pts[4] = {b->surf_flat, b->corner_sharp, b->surf_less_flat, b->corner_less_sharp};
   for (int k = 0; k < 4; ++k) {
     if (!offs[k]) return fail(ctx, LINS_E_INVALID, "null offsets");
     if (offs[k][0] != 0) return fail(ctx, LINS_E_INVALID, "offsets must start at 0");
     for (int i = 0; i < n; ++i) if (offs[k][i + 1] < offs[k][i]) return fail(ctx, LINS_E_INVALID, "offsets must be non-decreasing");
     if (offs[k][n] > 0 && !pts[k]) return fail(ctx, LINS_E_INVALID, "null cloud");
   }
-  if (!b->state_in || !b->cov_in) return fail(ctx, LINS_E_INVALID, "null prior");
-  if (b->point_format != LINS_POINTS_XYZI32 && b->point_format != LINS_POINTS_PACKED16) return fail(ctx, LINS_E_INVALID, "bad point_format");
-  const bool packed16 = b->point_format == LINS_POINTS_PACKED16;  // the clouds are already (x, y, z, intensity) float4 records
+  if (point_format != LINS_POINTS_XYZI32 && point_format != LINS_POINTS_PACKED16) return fail(ctx, LINS_E_INVALID, "bad point_format");
+  const bool packed16 = point_format == LINS_POINTS_PACKED16;  // the clouds are already (x, y, z, intensity) float4 records
   r.nqs = offs[0][n]; r.nqc = offs[1][n]; r.nts = offs[2][n]; r.ntc = offs[3][n];
   r.max_q = 0;
   for (int i = 0; i < n; ++i) r.max_q = std::max(r.max_q, (offs[0][i + 1] - offs[0][i]) + (offs[1][i + 1] - offs[1][i]));
   const size_t total = r.nqs + r.nqc + r.nts + r.ntc;
   CK(r.h_pts.reserve(total + 1)); CK(r.h_off.reserve(4 * (size_t)(n + 1)));
-  CK(r.h_state.reserve((size_t)n * 20)); CK(r.h_cov.reserve((size_t)n * 324));
   CK(r.qs.reserve(r.nqs + 1)); CK(r.qc.reserve(r.nqc + 1)); CK(r.ts.reserve(r.nts + 1)); CK(r.tc.reserve(r.ntc + 1));
   CK(r.qs_off.reserve(n + 1)); CK(r.qc_off.reserve(n + 1)); CK(r.ts_off.reserve(n + 1)); CK(r.tc_off.reserve(n + 1));
-  CK(r.state_in.reserve((size_t)n * 20)); CK(r.cov_in.reserve((size_t)n * 324));
   // pack 32-B PointXYZI -> 16-B float4 while copying into pinned staging (the copy is needed anyway: user
   // buffers are pageable), so PCIe moves half the bytes.  The pack is spread over host threads in 64 K-point
   // slices; each slice's H2D copy is queued as soon as the slice is packed, so packing and PCIe overlap.
@@ -85,7 +75,7 @@ int lins_gpu_batch_upload(lins_ctx* ctx, const lins_batch_desc* b) {
   const char* mode = std::getenv("LINS_UPLOAD");
   // default: host pack when this context has >= 8 pack threads to itself (measured, 2 GPUs x 3 contexts: 10 threads each
   // 6.1 M it/s per GPU; raw DMA 3.8 M whatever the threads; the two-ended split with 2-5 threads 3.3-3.6 M), raw DMA otherwise
-  const bool p16 = b->point_format == LINS_POINTS_PACKED16;  // (16-B records from pinned memory: always straight DMA)
+  const bool p16 = packed16;  // (16-B records from pinned memory: always straight DMA)
   const bool mode_pack = mode ? std::strcmp(mode, "pack") == 0 : (want_threads >= 8 && !p16);
   const bool mode_direct = mode ? (std::strcmp(mode, "direct") == 0 || std::strcmp(mode, "pinned") == 0) : (want_threads < 8 || p16);
   bool pinned[4] = {false, false, false, false};
@@ -174,13 +164,33 @@ int lins_gpu_batch_upload(lins_ctx* ctx, const lins_batch_desc* b) {
     ctx->upload_packed_points += (int64_t)(total - raw_pts);
   }
   for (int k = 0; k < 4; ++k) std::memcpy(r.h_off.p + (size_t)k * (n + 1), offs[k], sizeof(int) * (n + 1));
+  for (int k = 0; k < 4; ++k)
+    CK(cudaMemcpyAsync(doffs[k], r.h_off.p + (size_t)k * (n + 1), sizeof(int) * (n + 1), cudaMemcpyHostToDevice, ctx->stream));
+  return LINS_OK;
+}
+
+}  // namespace lins_capi
+
+extern "C" {
+
+int lins_gpu_batch_upload(lins_ctx* ctx, const lins_batch_desc* b) {
+  if (!ctx) return LINS_E_INVALID;
+  if (!b || b->n_scans < 0) return fail(ctx, LINS_E_INVALID, "bad batch");
+  CK(cudaSetDevice(ctx->device));
+  Resident& r = ctx->batch;
+  const int n = b->n_scans;
+  if (n > 0 && (!b->state_in || !b->cov_in)) return fail(ctx, LINS_E_INVALID, "null prior");
+  const int32_t* offs[4] = {b->surf_flat_off, b->corner_sharp_off, b->surf_less_flat_off, b->corner_less_sharp_off};
+  const lins_point* pts[4] = {b->surf_flat, b->corner_sharp, b->surf_less_flat, b->corner_less_sharp};
+  int rc = upload_clouds(ctx, r, n, pts, offs, b->point_format);
+  if (rc != LINS_OK || n == 0) return rc;
+  CK(r.h_state.reserve((size_t)n * 20)); CK(r.h_cov.reserve((size_t)n * 324));
+  CK(r.state_in.reserve((size_t)n * 20)); CK(r.cov_in.reserve((size_t)n * 324));
   for (int i = 0; i < n; ++i) {
     std::memcpy(r.h_state.p + (size_t)i * 20, b->state_in + (size_t)i * 19, sizeof(double) * 19);
     r.h_state.p[(size_t)i * 20 + 19] = 0.0;
   }
   std::memcpy(r.h_cov.p, b->cov_in, sizeof(double) * 324 * (size_t)n);
-  for (int k = 0; k < 4; ++k)
-    CK(cudaMemcpyAsync(doffs[k], r.h_off.p + (size_t)k * (n + 1), sizeof(int) * (n + 1), cudaMemcpyHostToDevice, ctx->stream));
   CK(cudaMemcpyAsync(r.state_in.p, r.h_state.p, sizeof(double) * 20 * (size_t)n, cudaMemcpyHostToDevice, ctx->stream));
   CK(cudaMemcpyAsync(r.cov_in.p, r.h_cov.p, sizeof(double) * 324 * (size_t)n, cudaMemcpyHostToDevice, ctx->stream));
   return reserve_outputs(ctx, r, true, false);

@@ -161,6 +161,27 @@ class StateEstimator {
     }
   }
 
+  // processPCL without the extractor: the same status machine on features extracted elsewhere (a replayed feature log)
+  void processFeatures(double time, const sensor_utils::Imu& imu, const ScanFeatures& f) {
+    scan_new_->time_ = time;
+    scan_new_->undistPointCloud_ = f.undistPointCloud;
+    scan_new_->cornerPointsSharp_ = f.cornerPointsSharp; scan_new_->cornerPointsLessSharp_ = f.cornerPointsLessSharp;
+    scan_new_->surfPointsFlat_ = f.surfPointsFlat; scan_new_->surfPointsLessFlat_ = f.surfPointsLessFlat;
+    imu_last_ = imu;
+    switch (status_) {
+      case STATUS_INIT:
+        if (processFirstScan()) status_ = STATUS_FIRST_SCAN;
+        break;
+      case STATUS_FIRST_SCAN:
+        if (processSecondScan()) status_ = STATUS_RUNNING; else status_ = STATUS_INIT;
+        break;
+      case STATUS_RUNNING:
+        if (!processScan()) status_ = STATUS_RUNNING;
+        break;
+      default: break;
+    }
+  }
+
   // StateEstimator.hpp:331-375
   bool processFirstScan() {
     if (scan_new_->cornerPointsLessSharp_.size() < 10 || scan_new_->surfPointsLessFlat_.size() < 100) {
@@ -284,6 +305,7 @@ class StateEstimator {
     check(lins_gpu_update_map(ctx_, pts(scan_new_->surfPointsLessFlat_), (int)scan_new_->surfPointsLessFlat_.size(),
                               pts(scan_new_->cornerPointsLessSharp_), (int)scan_new_->cornerPointsLessSharp_.size(), lin, &replaced),
           "lins_gpu_update_map");
+    last_map_replaced_ = replaced != 0;
     scan_new_->cornerPointsLessSharpYZX_.clear(); scan_new_->surfPointsLessFlatYZX_.clear(); scan_new_->outlierPointCloudYZX_.clear();
     for (const auto& p : scan_new_->cornerPointsLessSharp_.points) scan_new_->cornerPointsLessSharpYZX_.push_back(makePoint(p.y, p.z, p.x, p.intensity));
     for (const auto& p : scan_new_->surfPointsLessFlat_.points) scan_new_->surfPointsLessFlatYZX_.push_back(makePoint(p.y, p.z, p.x, p.intensity));
@@ -301,6 +323,7 @@ class StateEstimator {
   Q4D Q_yzx_to_xyz, Q_xyz_to_yzx;
   sensor_utils::Imu imu_last_;
   lins_report last_report_;
+  bool last_map_replaced_ = false;  // the last updatePointCloud rebuilt the 1-NN index (:1156-1157)
 
  private:
   FeatureExtractor extractor_;

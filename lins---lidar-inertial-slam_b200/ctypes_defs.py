@@ -92,6 +92,62 @@ class LinsBatchDesc(C.Structure):
     ]
 
 
+class LinsSeqParams(C.Structure):
+    """lins_seq_params (include/lins_gpu.h, sequence mode)."""
+    _fields_ = [("noise", C.c_double * 4), ("init_pos_std", C.c_double * 3), ("init_att_std", C.c_double * 3)]
+
+    @classmethod
+    def shipped(cls, acc_n=70000.0, gyr_n=0.1, acc_w=500.0, gyr_w=0.05, init_pos_std=(0.0, 0.0, 0.0), init_att_std=(0.0, 0.0, 0.0)):
+        """csrc/host/kalman_filter.hpp FilterParams defaults (exp_port.yaml:29-62); noise as StatePredictor::setNoise."""
+        import math
+        deg = math.pi / 180.0
+        dph, dpsh = deg / 3600.0, deg / math.sqrt(3600.0)
+        ug = (9.81 / 1000.0) / 1000.0
+        ugpshz = ug / math.sqrt(1.0)
+        p = cls()
+        for i, v in enumerate((math.pow(acc_n * ug, 2), math.pow(gyr_n * dph, 2), math.pow(acc_w * ugpshz, 2), math.pow(gyr_w * dpsh, 2))):
+            p.noise[i] = v
+        for i in range(3):
+            p.init_pos_std[i], p.init_att_std[i] = init_pos_std[i], init_att_std[i]
+        return p
+
+
+class LinsSeqBeginDesc(C.Structure):
+    _fields_ = [
+        ("n_seq", C.c_int32),
+        ("filter_state", C.c_void_p),
+        ("filter_cov", C.c_void_p),
+        ("global_state", C.c_void_p),
+        ("imu_last", C.c_void_p),
+        ("surf_map", C.c_void_p),
+        ("surf_map_off", C.c_void_p),
+        ("corner_map", C.c_void_p),
+        ("corner_map_off", C.c_void_p),
+        ("point_format", C.c_int32),
+    ]
+
+
+class LinsSeqStepDesc(C.Structure):
+    _fields_ = [
+        ("n_seq", C.c_int32),
+        ("present", C.c_void_p),
+        ("imu", C.c_void_p),
+        ("imu_off", C.c_void_p),
+        ("surf_flat", C.c_void_p),
+        ("surf_flat_off", C.c_void_p),
+        ("corner_sharp", C.c_void_p),
+        ("corner_sharp_off", C.c_void_p),
+        ("surf_less_flat", C.c_void_p),
+        ("surf_less_flat_off", C.c_void_p),
+        ("corner_less_sharp", C.c_void_p),
+        ("corner_less_sharp_off", C.c_void_p),
+        ("point_format", C.c_int32),
+    ]
+
+
+SEQ_IDLE, SEQ_SKIPPED, SEQ_RAN, SEQ_ICP = 0, 1, 2, 3  # lins_gpu_seq_download scan_status (LINS_SEQ_*)
+
+
 def ptr(a):
     """void* of a C-contiguous numpy array (None -> NULL)."""
     if a is None:

@@ -190,6 +190,125 @@ def run_sequence(config="config3", seed=1, n_scans=12, device=0, **overrides):
         L.lins_seq_destroy(h)
 
 
+# ---- feature logs (tools/synth/lins_sequence.cpp): per scan the IMU calls and the four feature clouds ----------------
+class FeatureLogDesc(C.Structure):
+    _fields_ = [("n_scans", C.c_int32), ("time", C.c_void_p), ("imu", C.c_void_p), ("imu_off", C.c_void_p),
+                ("imu_last", C.c_void_p), ("clouds", C.c_void_p * 4), ("offs", C.c_void_p * 4)]
+
+
+def _flog_lib():
+    L = seq_lib()
+    if not hasattr(L, "_flog"):
+        L.lins_flog_create.restype = C.c_void_p
+        L.lins_flog_create.argtypes = [C.POINTER(SynthCfg), C.c_uint64, C.c_int]
+        L.lins_flog_destroy.argtypes = [C.c_void_p]
+        L.lins_flog_desc.argtypes = [C.c_void_p, C.POINTER(FeatureLogDesc)]
+        L.lins_flog_replay.restype = C.c_void_p
+        L.lins_flog_replay.argtypes = [C.POINTER(FeatureLogDesc), C.c_int, C.c_int, C.c_void_p, C.c_void_p]
+        L.lins_host_predict.argtypes = [C.c_void_p] * 4 + [C.c_int]
+        L.lins_replay_destroy.argtypes = [C.c_void_p]
+        L.lins_replay_handover.argtypes = [C.c_void_p]
+        L.lins_replay_ints.restype = C.POINTER(C.c_int32)
+        L.lins_replay_ints.argtypes = [C.c_void_p, C.c_int]
+        L.lins_replay_doubles.restype = C.POINTER(C.c_double)
+        L.lins_replay_doubles.argtypes = [C.c_void_p, C.c_int]
+        L.lins_replay_handover_cloud.argtypes = [C.c_void_p, C.c_int, C.POINTER(C.c_void_p)]
+        L._flog = True
+    return L
+
+
+def feature_log(config="config3", seed=1, n_scans=12, **overrides):
+    """A simulated drive through the front end only (image projection + feature extraction; no GPU): dict with time (n),
+    imu (k x 7: dt, acc, gyr) + imu_off (n + 1), imu_last (n x 6) and the four feature clouds (Batch.FIELDS) with their
+    offsets (<name>_off).  Edit it freely, then replay it with replay_feature_log or sequence mode."""
+    L = _flog_lib()
+    kw = dict(CONFIGS[config])
+    kw.update(overrides)
+    cfg = SynthCfg(**kw)
+    h = L.lins_flog_create(C.byref(cfg), seed, n_scans)
+    try:
+        d = FeatureLogDesc()
+        L.lins_flog_desc(h, C.byref(d))
+        n = d.n_scans
+        log = dict(lidar=kw["lidar"], time=_copy(d.time, n, np.float64), imu_off=_copy(d.imu_off, n + 1, np.int32),
+                   imu_last=_copy(d.imu_last, n * 6, np.float64).reshape(n, 6))
+        log["imu"] = _copy(d.imu, int(log["imu_off"][-1]) * 7, np.float64).reshape(-1, 7)
+        for j, k in enumerate(Batch.FIELDS):
+            log[k + "_off"] = _copy(d.offs[j], n + 1, np.int32)
+            log[k] = _copy(d.clouds[j], int(log[k + "_off"][-1]), POINT_DTYPE)
+        return log
+    finally:
+        L.lins_flog_destroy(h)
+
+
+def log_scan(log, k):
+    """Scan k of a feature log: its IMU rows and its four clouds."""
+    o = log["imu_off"]
+    out = dict(imu=log["imu"][o[k]:o[k + 1]], imu_last=log["imu_last"][k], time=log["time"][k])
+    for f in Batch.FIELDS:
+        out[f] = log[f][log[f + "_off"][k]:log[f + "_off"][k + 1]]
+    return out
+
+
+def make_log(scans, lidar=0):
+    """Reassemble a feature log from a list of log_scan dicts (the way tests edit one)."""
+    log = dict(lidar=lidar, time=np.array([s["time"] for s in scans], np.float64), imu_last=np.array([s["imu_last"] for s in scans], np.float64).reshape(-1, 6))
+    log["imu"] = np.ascontiguousarray(np.concatenate([np.asarray(s["imu"], np.float64).reshape(-1, 7) for s in scans]))
+    log["imu_off"] = np.concatenate([[0], np.cumsum([len(s["imu"]) for s in scans])]).astype(np.int32)
+    for f in Batch.FIELDS:
+        log[f] = np.ascontiguousarray(np.concatenate([s[f] for s in scans])) if scans else np.zeros(0, POINT_DTYPE)
+        log[f + "_off"] = np.concatenate([[0], np.cumsum([len(s[f]) for s in scans])]).astype(np.int32)
+    return log
+
+
+def replay_feature_log(log, device=0, params=None, init_std=None):
+    """Replay a feature log through one C++ StateEstimator shim (processImu + processFeatures per scan).  Returns per scan
+    code (LINS_SEQ_*: 0 before the hand-over), iters, flags, map_replaced, est_status, global_state / filter_state /
+    lin_state (n x 19) and filter_cov (n x 324) after the scan, plus `handover`: the scan index after which the shim first
+    ran and its state then, as lins_gpu_seq_begin takes it.  params: the shim context's LinsParams (None = shipped);
+    init_std: INIT_POS_STD (3) + INIT_ATT_STD (3, degrees) of its filter (None = zero).  scan_s: wall seconds per scan."""
+    L = _flog_lib()
+    n = len(log["time"])
+    keep = {k: np.ascontiguousarray(log[k]) for k in ("time", "imu", "imu_off", "imu_last")}
+    d = FeatureLogDesc()
+    d.n_scans = n
+    for k, v in keep.items():
+        setattr(d, k, v.ctypes.data)
+    for j, k in enumerate(Batch.FIELDS):
+        keep[k], keep[k + "_off"] = np.ascontiguousarray(log[k]), np.ascontiguousarray(log[k + "_off"], dtype=np.int32)
+        d.clouds[j], d.offs[j] = keep[k].ctypes.data, keep[k + "_off"].ctypes.data
+    std = None if init_std is None else np.ascontiguousarray(init_std, dtype=np.float64)
+    h = L.lins_flog_replay(C.byref(d), int(log.get("lidar", 0)), device, C.cast(C.byref(params), C.c_void_p) if params is not None else None,
+                           None if std is None else std.ctypes.data)
+    try:
+        ints = lambda w: np.ctypeslib.as_array(L.lins_replay_ints(h, w), shape=(n,)).copy()  # noqa: E731
+        dbl = lambda w, cnt: np.ctypeslib.as_array(L.lins_replay_doubles(h, w), shape=(cnt,)).copy()  # noqa: E731
+        rec = dict(code=ints(0), iters=ints(1), flags=ints(2), map_replaced=ints(3), est_status=ints(4),
+                   global_state=dbl(0, n * 19).reshape(n, 19), filter_state=dbl(1, n * 19).reshape(n, 19),
+                   filter_cov=dbl(2, n * 324).reshape(n, 324), lin_state=dbl(3, n * 19).reshape(n, 19), scan_s=dbl(8, n))
+        k = L.lins_replay_handover(h)
+        rec["handover_index"] = k
+        if k >= 0:
+            ho = dict(filter_state=dbl(4, 19), global_state=dbl(5, 19), filter_cov=dbl(6, 324), imu_last=dbl(7, 6))
+            for which, name in ((0, "surf_map"), (1, "corner_map")):
+                p = C.c_void_p()
+                cnt = L.lins_replay_handover_cloud(h, which, C.byref(p))
+                ho[name] = _copy(p.value, cnt, POINT_DTYPE)
+            rec["handover"] = ho
+        return rec
+    finally:
+        L.lins_replay_destroy(h)
+
+
+def host_predict(state, cov, imu_last, rows):
+    """kalman_filter.hpp StatePredictor::predict over `rows` (k x 7) from (state, cov, imu_last): returns the three after."""
+    L = _flog_lib()
+    s, c, i = (np.array(a, np.float64).ravel().copy() for a in (state, cov, imu_last))
+    r = np.ascontiguousarray(rows, dtype=np.float64).reshape(-1, 7)
+    L.lins_host_predict(s.ctypes.data, c.ctypes.data, i.ctypes.data, r.ctypes.data, len(r))
+    return s, c, i
+
+
 # ---- row F2: scan-to-map units (tools/synth/lins_synth.cpp: lins_synth_map_unit_create) -------------------------------
 class MapUnit:
     """One scan2MapOptimization input: map clouds, the newest scan's (down-sampled) features, true / guessed transform."""

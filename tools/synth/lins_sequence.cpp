@@ -15,6 +15,7 @@
 #include "../../lins---lidar-inertial-slam_b200/csrc/host/state_estimator.hpp"
 #include "../../lins---lidar-inertial-slam_b200/csrc/host/rosbag_reader.hpp"
 #include <algorithm>
+#include <chrono>
 
 using lins::fusion::StateEstimator;
 
@@ -282,6 +283,180 @@ void* lins_seq_run_bag(const char* path, const char* lidar_topic, const char* im
     feed_scan(est, ip, rec, (int)k, ts, scans[k].second, dts, acc, gyr, nullptr, nullptr, verbose);
   }
   return rec;
+}
+
+// ---- feature logs: what the front end hands the estimator per scan, replayable through the shim or sequence mode ------
+// clouds[4] in lins_batch_desc order: surfPointsFlat_, cornerPointsSharp_, surfPointsLessFlat_, cornerPointsLessSharp_
+typedef struct lins_feature_log_desc {
+  int32_t n_scans;
+  const double* time;       /* n: scan stamps */
+  const double* imu;        /* k x 7 (dt, acc, gyr): the processImu calls before each scan */
+  const int32_t* imu_off;   /* n + 1 */
+  const double* imu_last;   /* n x 6: the acc / gyr processPCL receives with the scan */
+  const lins_point* clouds[4];
+  const int32_t* offs[4];   /* n + 1 each */
+} lins_feature_log_desc;
+
+struct FeatureLog {
+  std::vector<double> time, imu, imu_last;
+  std::vector<int32_t> imu_off{0};
+  std::vector<lins_point> c[4];
+  std::vector<int32_t> off[4] = {{0}, {0}, {0}, {0}};
+};
+
+// what the shim did with every scan of a replayed log, and its state right after it became RUNNING (the hand-over)
+struct ReplayRecord {
+  int handover = -1;  // index of the scan after which the shim was RUNNING for the first time
+  std::vector<int32_t> code, iters, flags, replaced, est_status;  // code: LINS_SEQ_* (0 before the hand-over)
+  std::vector<double> glob, filt, cov, lin;  // n x 19, n x 19, n x 324, n x 19 after each scan
+  std::vector<double> scan_s;                // wall time of each scan's processImu calls + processFeatures
+  double h_filt[19], h_glob[19], h_imu[6], h_cov[324];
+  std::vector<lins_point> h_surf, h_corner;
+};
+
+void* lins_flog_create(const lins_synth_cfg* cfg, uint64_t seed, int n_scans) {
+  FeatureLog* L = new FeatureLog();
+  SimDrive sim(cfg, seed);
+  ImageProjection ip(sim.lm);
+  FeatureExtractor ex(sim.lm, FeatureParams());
+  Sweep sw;
+  for (int k = 0; k < n_scans; ++k) {
+    sim.next(sw);
+    for (int i = 1; i <= SimDrive::nimu; ++i) {
+      const double row[7] = {sim.dt(), sw.accs[i].x(), sw.accs[i].y(), sw.accs[i].z(), sw.gyrs[i].x(), sw.gyrs[i].y(), sw.gyrs[i].z()};
+      L->imu.insert(L->imu.end(), row, row + 7);
+    }
+    L->imu_off.push_back((int32_t)(L->imu.size() / 7));
+    const double last[6] = {sw.accs.back().x(), sw.accs.back().y(), sw.accs.back().z(), sw.gyrs.back().x(), sw.gyrs.back().y(), sw.gyrs.back().z()};
+    L->imu_last.insert(L->imu_last.end(), last, last + 6);
+    L->time.push_back(sw.t_end);
+    ip.process(sw.raw);
+    ScanFeatures f;
+    ex.run(ip.segmentedCloud, ip.segMsg, f);
+    const Cloud* cl[4] = {&f.surfPointsFlat, &f.cornerPointsSharp, &f.surfPointsLessFlat, &f.cornerPointsLessSharp};
+    for (int j = 0; j < 4; ++j) append_cloud(L->c[j], L->off[j], *cl[j]);
+  }
+  return L;
+}
+void lins_flog_destroy(void* h) { delete static_cast<FeatureLog*>(h); }
+void lins_flog_desc(void* h, lins_feature_log_desc* d) {
+  FeatureLog* L = static_cast<FeatureLog*>(h);
+  d->n_scans = (int32_t)L->time.size();
+  d->time = L->time.data(); d->imu = L->imu.data(); d->imu_off = L->imu_off.data(); d->imu_last = L->imu_last.data();
+  for (int j = 0; j < 4; ++j) { d->clouds[j] = L->c[j].data(); d->offs[j] = L->off[j].data(); }
+}
+
+// Replay a (possibly edited) feature log through one shim: processImu for every IMU row, then processFeatures.
+// gpu: the C-ABI parameters of the shim's context (NULL = the shipped ones); init_std: INIT_POS_STD (3) + INIT_ATT_STD (3,
+// degrees) of its filter (NULL = zero)
+void* lins_flog_replay(const lins_feature_log_desc* d, int lidar_model, int device, const lins_params* gpu, const double* init_std) {
+  ReplayRecord* R = new ReplayRecord();
+  const LidarModel lm = lidar_model == 1 ? LidarModel::dense64() : LidarModel::vlp16();
+  lins::fusion::EstimatorParams ep = seq_params(lm);
+  if (gpu) ep.gpu = *gpu;
+  if (init_std) { ep.filter.init_pos_std = V3D(init_std[0], init_std[1], init_std[2]); ep.filter.init_att_std = V3D(init_std[3], init_std[4], init_std[5]); }
+  StateEstimator est(ep, device);
+  for (int k = 0; k < d->n_scans; ++k) {
+    const auto t0 = std::chrono::steady_clock::now();
+    for (int m = d->imu_off[k]; m < d->imu_off[k + 1]; ++m) {
+      const double* r = d->imu + (size_t)m * 7;
+      est.processImu(r[0], V3D(r[1], r[2], r[3]), V3D(r[4], r[5], r[6]));
+    }
+    ScanFeatures f;
+    Cloud* cl[4] = {&f.surfPointsFlat, &f.cornerPointsSharp, &f.surfPointsLessFlat, &f.cornerPointsLessSharp};
+    for (int j = 0; j < 4; ++j) cl[j]->points.assign(d->clouds[j] + d->offs[j][k], d->clouds[j] + d->offs[j][k + 1]);
+    const bool running = est.status_ == StateEstimator::STATUS_RUNNING;
+    est.last_report_ = lins_report();
+    const double* il = d->imu_last + (size_t)k * 6;
+    est.processFeatures(d->time[k], lins::sensor_utils::Imu(d->time[k], V3D(il[0], il[1], il[2]), V3D(il[3], il[4], il[5])), f);
+    R->scan_s.push_back(std::chrono::duration<double>(std::chrono::steady_clock::now() - t0).count());
+    int code = LINS_SEQ_IDLE;
+    if (running) {
+      const bool gate = f.cornerPointsLessSharp.size() <= 5 || f.surfPointsLessFlat.size() <= 10;  // processScan (:436-440)
+      code = gate ? LINS_SEQ_SKIPPED : est.last_report_.diverged ? LINS_SEQ_ICP : LINS_SEQ_RAN;
+    }
+    R->code.push_back(code);
+    R->iters.push_back(est.last_report_.iters);
+    R->flags.push_back((est.last_report_.converged ? 1 : 0) | (est.last_report_.diverged ? 2 : 0) | (est.last_report_.has_nan ? 4 : 0));
+    R->replaced.push_back(code >= LINS_SEQ_RAN && est.last_map_replaced_ ? 1 : 0);
+    R->est_status.push_back((int)est.status_);
+    double g[19], s[19], l[19];
+    est.globalState_.toArray(g); est.filter_->state_.toArray(s); est.linState_.toArray(l);
+    R->glob.insert(R->glob.end(), g, g + 19);
+    R->filt.insert(R->filt.end(), s, s + 19);
+    R->lin.insert(R->lin.end(), l, l + 19);
+    R->cov.insert(R->cov.end(), est.filter_->covariance_.data(), est.filter_->covariance_.data() + 324);
+    if (R->handover < 0 && est.status_ == StateEstimator::STATUS_RUNNING) {
+      R->handover = k;
+      std::memcpy(R->h_filt, s, sizeof(s)); std::memcpy(R->h_glob, g, sizeof(g));
+      std::memcpy(R->h_cov, est.filter_->covariance_.data(), sizeof(R->h_cov));
+      const V3D& a = est.filter_->acc_last; const V3D& w = est.filter_->gyr_last;
+      const double im[6] = {a.x(), a.y(), a.z(), w.x(), w.y(), w.z()};
+      std::memcpy(R->h_imu, im, sizeof(im));
+      R->h_surf = est.scan_last_->surfPointsLessFlat_.points;  // (already moved to the scan end by updatePointCloud)
+      R->h_corner = est.scan_last_->cornerPointsLessSharp_.points;
+    }
+  }
+  return R;
+}
+// k StatePredictor::predict calls (default FilterParams) from state / covariance / acc_last + gyr_last, in place: the
+// host side of the predict stage check
+void lins_host_predict(double* state, double* cov, double* imu_last, const double* rows, int k) {
+  filter::StatePredictor sp;
+  sp.initialization(0.0, V3D(), V3D(), V3D(), V3D(), V3D(imu_last[0], imu_last[1], imu_last[2]), V3D(imu_last[3], imu_last[4], imu_last[5]));
+  sp.state_ = filter::GlobalState::fromArray(state);
+  std::memcpy(sp.covariance_.data(), cov, sizeof(double) * 324);
+  for (int m = 0; m < k; ++m) {
+    const double* r = rows + 7 * m;
+    sp.predict(r[0], V3D(r[1], r[2], r[3]), V3D(r[4], r[5], r[6]), true);
+  }
+  sp.state_.toArray(state);
+  std::memcpy(cov, sp.covariance_.data(), sizeof(double) * 324);
+  const double il[6] = {sp.acc_last.x(), sp.acc_last.y(), sp.acc_last.z(), sp.gyr_last.x(), sp.gyr_last.y(), sp.gyr_last.z()};
+  std::memcpy(imu_last, il, sizeof(il));
+}
+
+// seconds per call of StatePredictor::predict (the host IMU propagation sequence mode replaces) over `rows` (k x 7)
+double lins_bench_host_predict(const double* rows, int k, int reps) {
+  filter::StatePredictor sp;
+  sp.initialization(0.0, V3D(), V3D(), V3D(), V3D(), V3D(0, 0, 9.81), V3D());
+  const auto t0 = std::chrono::steady_clock::now();
+  for (int r = 0; r < reps; ++r)
+    for (int m = 0; m < k; ++m) sp.predict(rows[7 * m], V3D(rows[7 * m + 1], rows[7 * m + 2], rows[7 * m + 3]), V3D(rows[7 * m + 4], rows[7 * m + 5], rows[7 * m + 6]), true);
+  const double s = std::chrono::duration<double>(std::chrono::steady_clock::now() - t0).count();
+  volatile double sink = sp.covariance_.a[0];
+  (void)sink;
+  return s / ((double)reps * (k > 0 ? k : 1));
+}
+
+void lins_replay_destroy(void* h) { delete static_cast<ReplayRecord*>(h); }
+int lins_replay_handover(void* h) { return static_cast<ReplayRecord*>(h)->handover; }
+const int32_t* lins_replay_ints(void* h, int which) {
+  ReplayRecord* R = static_cast<ReplayRecord*>(h);
+  const std::vector<int32_t>* v[5] = {&R->code, &R->iters, &R->flags, &R->replaced, &R->est_status};
+  return which >= 0 && which < 5 ? v[which]->data() : nullptr;
+}
+const double* lins_replay_doubles(void* h, int which) {
+  ReplayRecord* R = static_cast<ReplayRecord*>(h);
+  switch (which) {
+    case 0: return R->glob.data();
+    case 1: return R->filt.data();
+    case 2: return R->cov.data();
+    case 3: return R->lin.data();
+    case 4: return R->h_filt;
+    case 5: return R->h_glob;
+    case 6: return R->h_cov;
+    case 7: return R->h_imu;
+    case 8: return R->scan_s.data();
+  }
+  return nullptr;
+}
+// the hand-over's maps: which 0 = surf, 1 = corner; returns the point count
+int lins_replay_handover_cloud(void* h, int which, const lins_point** pts) {
+  ReplayRecord* R = static_cast<ReplayRecord*>(h);
+  const std::vector<lins_point>& c = which == 0 ? R->h_surf : R->h_corner;
+  *pts = c.data();
+  return (int)c.size();
 }
 
 void lins_seq_destroy(void* h) { delete static_cast<SeqRecord*>(h); }

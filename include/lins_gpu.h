@@ -204,8 +204,11 @@ int lins_gpu_host_unregister(void* ptr);
    (StatePredictor::predict, KalmanFilter.hpp:125-186), the processScan gate (:436-440), performIESKF (:465-600) with the
    estimateTransform fallback (:585-592, :1163-1196), filter_->update (KalmanFilter.hpp:195-200), integrateTransformation
    (:608-617), reset(1) (KalmanFilter.hpp:320-353), calculateRPfromGravity + correctRollPitch (:602-605, :427-431) and
-   updatePointCloud (:1116-1161).  Sequence initialisation (processFirstScan / processSecondScan, :331-425) stays with the
-   caller; lins_gpu_seq_begin takes its result. */
+   updatePointCloud (:1116-1161).  A run starts in one of two ways: lins_gpu_seq_begin takes S sequences the caller has
+   initialised itself (each right after processSecondScan), or lins_gpu_seq_open opens S empty slots that start from their
+   first scan: the step then also runs the status machine of processPCL (:294-307) — processFirstScan (:331-375), the IMU
+   pre-integration and processSecondScan (:379-425) with its estimateTransform — and lins_gpu_seq_restart hands a slot to
+   a new recording. */
 
 /* the filter constants the device chain needs (exp_port.yaml:29-62) */
 typedef struct lins_seq_params {
@@ -242,14 +245,48 @@ typedef struct lins_seq_step_desc {
 #define LINS_SEQ_SKIPPED 1   /* failed the processScan gate (cornerLessSharp <= 5 || surfLessFlat <= 10): predicted state, old map */
 #define LINS_SEQ_RAN 2       /* processScan ran */
 #define LINS_SEQ_ICP 3       /* processScan ran and the IESKF diverged: the pose is estimateTransform's */
+#define LINS_SEQ_INIT_WAIT 4 /* an initialising slot's scan failed the first / second scan gate (cornerLessSharp < 10 ||
+                                surfLessFlat < 100): the slot is (back) in STATUS_INIT */
+#define LINS_SEQ_FIRST 5     /* processFirstScan accepted the scan: the slot is in STATUS_FIRST_SCAN */
+#define LINS_SEQ_SECOND 6    /* processSecondScan ran (with its estimateTransform): the slot is RUNNING */
+
+/* the filter constants sequence initialisation reads (initializeCovariance, KalmanFilter.hpp:247-312; estimateInitialState,
+   StateEstimator.hpp:1408-1419); INIT_POS_STD / INIT_ATT_STD are lins_seq_params' */
+typedef struct lins_seq_init_params {
+  double init_vel_std[3];  /* INIT_VEL_STD, m/s */
+  double init_acc_std[3];  /* INIT_ACC_STD */
+  double init_gyr_std[3];  /* INIT_GYR_STD */
+  double init_ba[3];       /* INIT_BA: the accelerometer bias of the hand-over and the pre-integration's linearisation point */
+  double init_bw[3];       /* INIT_BW: the same for the gyroscope */
+} lins_seq_init_params;
 
 /* Uploads the hand-over; replaces any running sequences of this ctx (single-scan and batched state are untouched). */
 int lins_gpu_seq_begin(lins_ctx* ctx, const lins_seq_params* params, const lins_seq_begin_desc* desc);
-/* Advances every present sequence by one scan.  Returns LINS_E_NOMAP before lins_gpu_seq_begin.  One stream
-   synchronisation (the divergence check) per call; the rest is queued.  LINS_E_INVALID for a bad descriptor leaves the
-   sequences as they were; any other error ends the run (the sequences are dropped, the next step returns LINS_E_NOMAP
-   until a new lins_gpu_seq_begin), because the step may have advanced some of its phases already. */
+/* Opens a run of n_seq empty slots, each what a newly constructed StateEstimator holds: STATUS_INIT, globalState_ and the
+   filter state identity (gn = (0, 0, -9.81)), the covariance of initializeCovariance, no map.  Replaces any running
+   sequences of this ctx, like lins_gpu_seq_begin.  LINS_E_INVALID for n_seq < 1 or a NULL argument. */
+int lins_gpu_seq_open(lins_ctx* ctx, const lins_seq_params* params, const lins_seq_init_params* init, int32_t n_seq);
+/* Puts every slot with mask[s] != 0 back into the fresh state of lins_gpu_seq_open (its last scan_status reads
+   LINS_SEQ_IDLE); the other slots are untouched.  LINS_E_INVALID for a NULL mask or a run started by lins_gpu_seq_begin
+   (it has no init params); LINS_E_NOMAP without a run. */
+int lins_gpu_seq_restart(lins_ctx* ctx, const uint8_t* mask /*S*/);
+/* Advances every present sequence by one scan.  Returns LINS_E_NOMAP before lins_gpu_seq_begin / lins_gpu_seq_open.  One
+   stream synchronisation (the divergence check) per call; the rest is queued.  LINS_E_INVALID for a bad descriptor leaves
+   the sequences as they were; any other error ends the run (the sequences are dropped, the next step returns LINS_E_NOMAP
+   until a new lins_gpu_seq_begin / lins_gpu_seq_open), because the step may have advanced some of its phases already.
+   A present slot runs what processImu + processPCL do in its status: in STATUS_INIT its IMU rows are ignored and the scan
+   goes through processFirstScan; in STATUS_FIRST_SCAN its IMU rows are pre-integrated (IntegrationBase::propagate) and the
+   scan goes through processSecondScan; RUNNING is as above. */
 int lins_gpu_seq_step(lins_ctx* ctx, const lins_seq_step_desc* step);
+/* The same with the IMU sample processPCL receives with each scan (acc (3), gyr (3); Estimator.cpp:238-243): S x 6, read
+   for the present slots in STATUS_INIT or STATUS_FIRST_SCAN.  scan_imu may be NULL only when no present slot is
+   initialising (else LINS_E_INVALID, before anything changes).  lins_gpu_seq_step(ctx, d) = lins_gpu_seq_step_ex(ctx, d, NULL). */
+int lins_gpu_seq_step_ex(lins_ctx* ctx, const lins_seq_step_desc* step, const double* scan_imu /*S x 6 or NULL*/);
+/* Sequence initialisation read-back (any pointer may be NULL): fusion_status[s] = the slot's StateEstimator::status_
+   (0 STATUS_INIT, 1 STATUS_FIRST_SCAN, 3 STATUS_RUNNING); where the last step's scan_status is LINS_SEQ_SECOND, icp_pose
+   (t (3) + q (x,y,z,w)), icp_iters and icp_converged are that scan's estimateTransform result, elsewhere zero. */
+int lins_gpu_seq_download_init(lins_ctx* ctx, int32_t* fusion_status /*S*/, double* icp_pose /*S x 7*/, int32_t* icp_iters /*S*/,
+                               int32_t* icp_converged /*S*/);
 /* The sequences' state after the last step; any pointer may be NULL.  results / reports: the last step's performIESKF,
    valid where scan_status is LINS_SEQ_RAN or LINS_SEQ_ICP and unspecified elsewhere (zero before the first step);
    scan_status: LINS_SEQ_* of the last step. */
@@ -257,7 +294,8 @@ int lins_gpu_seq_download(lins_ctx* ctx, double* global_state /*S x 19*/, double
                           double* filter_cov /*S x 324*/, lins_scan_result* results /*S*/, lins_report* reports /*S*/,
                           int32_t* scan_status /*S*/);
 /* CUDA-event times of the last lins_gpu_seq_step's phases, ms: ms[0] IMU propagation, ms[1] query compaction + IESKF,
-   ms[2] divergence check (D2H + synchronisation) + estimateTransform fallbacks, ms[3] post kernel + map refresh. */
+   ms[2] divergence check (D2H + synchronisation) + estimateTransform fallbacks + the second scans' estimateTransform
+   (one batched loop), ms[3] post kernel + sequence initialisation + map refresh. */
 int lins_gpu_seq_phase_ms(lins_ctx* ctx, float* ms /*4*/);
 /* Parity hooks of sequence mode (any pointer may be NULL).  download_ieskf: the last step's IESKF prior (the filter state
    and covariance after the IMU propagation, every sequence), its output (state_out / cov_out as lins_gpu_ieskf returns

@@ -14,7 +14,7 @@ import subprocess
 import numpy as np
 
 from .ctypes_defs import (Batch, COV_SIZE, LinsBatchDesc, LinsMapReport, LinsParams, LinsReport, LinsScanResult, LinsSeqBeginDesc,
-                          LinsSeqParams, LinsSeqStepDesc, POINT_DTYPE, SCAN_RESULT_DTYPE, STATE_DIM, as_points, ptr)
+                          LinsSeqInitParams, LinsSeqParams, LinsSeqStepDesc, POINT_DTYPE, SCAN_RESULT_DTYPE, STATE_DIM, as_points, ptr)
 
 _PKG = os.path.dirname(os.path.abspath(__file__))
 _ROOT = os.path.dirname(_PKG)
@@ -31,6 +31,7 @@ EXPORTS = [
     "lins_gpu_host_register", "lins_gpu_host_unregister", "lins_gpu_batch_download_indices", "lins_gpu_update_map_ex",
     "lins_gpu_batch_upload_stats", "lins_gpu_seq_begin", "lins_gpu_seq_step", "lins_gpu_seq_download",
     "lins_gpu_seq_phase_ms", "lins_gpu_seq_download_ieskf", "lins_gpu_seq_download_maps", "lins_gpu_download_indices",
+    "lins_gpu_seq_open", "lins_gpu_seq_restart", "lins_gpu_seq_step_ex", "lins_gpu_seq_download_init",
 ]
 
 NVCC_ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]  # H100 (Hopper)
@@ -112,6 +113,11 @@ def lib():
         L.lins_gpu_seq_download_ieskf.argtypes = [vp] + [vp] * 7
         L.lins_gpu_seq_download_maps.argtypes = [vp] + [vp] * 6
         L.lins_gpu_download_indices.argtypes = [vp, vp, vp]
+        if hasattr(L, "lins_gpu_seq_open"):  # (absent from older libraries selected through LINS_GPU_LIB)
+            L.lins_gpu_seq_open.argtypes = [vp, C.POINTER(LinsSeqParams), C.POINTER(LinsSeqInitParams), C.c_int32]
+            L.lins_gpu_seq_restart.argtypes = [vp, vp]
+            L.lins_gpu_seq_step_ex.argtypes = [vp, C.POINTER(LinsSeqStepDesc), vp]
+            L.lins_gpu_seq_download_init.argtypes = [vp, vp, vp, vp, vp]
         _LIB = L
     return _LIB
 
@@ -344,9 +350,34 @@ class LinsGpu:
         self._ck(self.L.lins_gpu_seq_begin(self.h, C.byref(params), C.byref(d)))
         self._seq_n = d.n_seq
 
-    def seq_step(self, step):
+    def seq_open(self, params, init_params, n_seq):
+        """Open n_seq empty slots that start from their first scan (lins_gpu_seq_open).  params: LinsSeqParams,
+        init_params: LinsSeqInitParams."""
+        self._ck(self.L.lins_gpu_seq_open(self.h, C.byref(params), C.byref(init_params), int(n_seq)))
+        self._seq_n = int(n_seq)
+
+    def seq_restart(self, mask):
+        """Put the slots with mask[s] != 0 back into the fresh state of seq_open (their next scan is a first scan)."""
+        m = np.ascontiguousarray(mask, dtype=np.uint8)
+        if len(m) != self._seq_n:
+            raise ValueError(f"mask has {len(m)} entries, the run {self._seq_n}")
+        self._ck(self.L.lins_gpu_seq_restart(self.h, ptr(m)))
+
+    def seq_download_init(self):
+        """dict: fusion_status (S; StateEstimator::status_ of every slot) and, for the slots whose last scan was a second
+        scan (LINS_SEQ_SECOND), its estimateTransform result: icp_pose (S x 7: t, q xyzw), icp_iters, icp_converged (zero
+        elsewhere)."""
+        n = self._seq_n
+        out = dict(fusion_status=np.zeros(n, np.int32), icp_pose=np.zeros((n, 7)), icp_iters=np.zeros(n, np.int32),
+                   icp_converged=np.zeros(n, np.int32))
+        self._ck(self.L.lins_gpu_seq_download_init(self.h, ptr(out["fusion_status"]), ptr(out["icp_pose"]), ptr(out["icp_iters"]),
+                                                   ptr(out["icp_converged"])))
+        return out
+
+    def seq_step(self, step, scan_imu=None):
         """Advance every present sequence by one scan.  `step`: dict with imu (k x 7: dt, acc, gyr) + imu_off, the four
-        feature clouds (Batch.FIELDS) + their offsets (<name>_off), and optionally present (S, uint8)."""
+        feature clouds (Batch.FIELDS) + their offsets (<name>_off), and optionally present (S, uint8).  scan_imu (S x 6:
+        acc, gyr): the IMU sample that comes with each scan, needed while a present slot initialises."""
         keep = {"imu": np.ascontiguousarray(step["imu"], dtype=np.float64), "imu_off": np.ascontiguousarray(step["imu_off"], dtype=np.int32)}
         for k in Batch.FIELDS:
             keep[k] = as_points(step[k])
@@ -358,7 +389,13 @@ class LinsGpu:
             keep["present"] = np.ascontiguousarray(step["present"], dtype=np.uint8)
         for k, v in keep.items():
             setattr(d, k, v.ctypes.data)
-        self._ck(self.L.lins_gpu_seq_step(self.h, C.byref(d)))
+        if scan_imu is None:
+            self._ck(self.L.lins_gpu_seq_step(self.h, C.byref(d)))
+        else:
+            si = np.ascontiguousarray(scan_imu, dtype=np.float64).reshape(-1, 6)
+            if len(si) != d.n_seq:
+                raise ValueError(f"scan_imu has {len(si)} rows, the step {d.n_seq}")
+            self._ck(self.L.lins_gpu_seq_step_ex(self.h, C.byref(d), ptr(si)))
 
     def seq_download(self, reports=False):
         """dict: global_state, filter_state (S x 19), filter_cov (S x 324), results (SCAN_RESULT_DTYPE), status (S) and,

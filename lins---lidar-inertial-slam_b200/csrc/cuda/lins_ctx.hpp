@@ -18,7 +18,7 @@
 #include "../../../include/lins_gpu.h"
 #include "../host/host_pool.hpp"
 
-namespace lins_dev { struct IcpState; struct BatchView; }     // lins_icp_step.cuh, lins_kernels.cuh
+namespace lins_dev { struct IcpState; struct BatchView; }     // lins_kernels.cuh
 namespace lins_map { struct PassConsts; struct MapLoopState; }  // lins_map.cuh
 
 namespace lins_capi {
@@ -85,8 +85,19 @@ struct SeqCopy { const float4* src; float4* dst; int n, pad; };
 // sequences in sequence order; `tree` holds the cloud a sequence's 1-NN index was last built on where that differs from
 // its map (stale[s] = 1, after a refresh that failed the >=5 && >=20 guard), and is empty elsewhere.
 struct SeqState {
-  int n = 0;                      // sequences (0 = lins_gpu_seq_begin has not run)
+  int n = 0;                      // sequences (0 = lins_gpu_seq_begin / lins_gpu_seq_open has not run)
   double consts[10];              // lins_seq::Consts
+  // sequence initialisation (lins_gpu_seq_open runs only): init_consts = lins_seq::InitConsts, fusion = each slot's
+  // StateEstimator::status_ (every slot of a lins_gpu_seq_begin run is RUNNING), pre = the pre-integration (n x 20),
+  // init_icp = the second scans' estimateTransform loop state (n IcpState records), init_off = their compacted query
+  // offsets (2 x (n + 1), after the IESKF's), scan_imu = the step's processPCL IMU samples (n x 6)
+  bool has_init = false;
+  double init_consts[24];
+  std::vector<int32_t> fusion;
+  Buf<double> pre, scan_imu;
+  Buf<double, kPinned> h_scan_imu;
+  Buf<unsigned char> init_icp;
+  Buf<int> init_off;
   Buf<double> filt, cov, glob, lin, imu_last, icp_pose;  // n x 20, n x 324, n x 20, n x 20, n x 8, n x 20
   Buf<double> prior_state, prior_cov;                  // the last step's IESKF prior (after the IMU propagation)
   Buf<int> icp_ind_s, icp_ind_c;                       // correspondence IDs of the ICP fallback (the IESKF's stay in run)
@@ -101,7 +112,8 @@ struct SeqState {
   Resident run;                                        // the IESKF batch: compacted queries of the sequences that run, outputs
   Buf<double> imu; Buf<int> imu_off;
   Buf<double, kPinned> h_imu; Buf<int, kPinned> h_imu_off;
-  Buf<unsigned char> status_d;                         // n: LINS_SEQ_* of the step (read by the post kernel)
+  Buf<unsigned char> status_d;                         // 3 x n: LINS_SEQ_* of the step (read by the post kernel), the
+                                                       // transformToEnd mask, the IMU rows' use (lins_seq.cu: ImuUse)
   Buf<unsigned char, kPinned> h_status;
   Buf<SeqCopy> copies; Buf<SeqCopy, kPinned> h_copies;
   std::vector<int32_t> status;                         // host copy of status_d
@@ -262,11 +274,12 @@ inline int upload2(lins_ctx* ctx, Buf<float4>& dst_a, const lins_point* a, int n
 // corner_less_sharp) and upload them with their offsets into r (qs, qc, ts, tc); sets r.n, the totals and r.max_q
 int upload_clouds(lins_ctx* ctx, Resident& r, int n, const lins_point* const pts[4], const int32_t* const offs[4], int point_format);
 // lins_gpu.cu: the fused kernel's IESKF launch over bv (with r's scratch), its query tile, the estimateTransform loop of
-// one device-resident unit, and the CSR transformToEnd of the units with run[u] != 0 (lin: 20 doubles per unit)
+// bv's device-resident units (pose: 20 doubles, icp: one IcpState per unit, set by the caller), and the CSR transformToEnd
+// of the units with run[u] != 0 (lin: 20 doubles per unit)
 int fused_ieskf_launch(lins_ctx* ctx, Resident& r, const lins_dev::BatchView& bv);
 int fused_qtile(int max_q);
 size_t icp_state_bytes();
-int icp_loop(lins_ctx* ctx, Resident& r, lins_dev::BatchView bv, double* pose, lins_dev::IcpState* icp, int icp_index = 0);
+int icp_loop(lins_ctx* ctx, Resident& r, lins_dev::BatchView bv, double* pose, lins_dev::IcpState* icp);
 int transform_to_end_csr(lins_ctx* ctx, float4* pts, const int* off, int n_units, const double* lin, const unsigned char* run);
 
 }  // namespace lins_capi

@@ -236,7 +236,6 @@ __global__ void __launch_bounds__(kThreads, kMinCtas) lins_ieskf_kernel(const __
   Smem* slots = reinterpret_cast<Smem*>(smem_raw + lay.slots);
   const int tid = threadIdx.x, warp = tid >> 5;
   const double sig2 = kp.lidar_std * kp.lidar_std;
-  if (MODE == MODE_ICP_REDUCE && bv.icp_done && *bv.icp_done) return;  // the queued tail of a converged ICP loop (uniform)
 
   if (tid == 0) {
     mbar_init(&cta.mbar, 1);
@@ -256,7 +255,13 @@ __global__ void __launch_bounds__(kThreads, kMinCtas) lins_ieskf_kernel(const __
       int nact = 0, nfresh = 0;
       for (int s = 0; s < S; ++s) {
         Smem& sm = slots[s];
-        if (sm.scan < 0 && !cta.exhausted) {
+        if (MODE == MODE_ICP_REDUCE) {  // a unit whose Gauss-Newton loop has ended is passed over (the queued tail of its loop)
+          while (sm.scan < 0 && !cta.exhausted) {
+            const int u = atomicAdd(bv.work_counter, 1);
+            if (u >= bv.n_scans) cta.exhausted = 1;
+            else if (!bv.icp_done || !bv.icp_done[(size_t)u * kIcpDoneStride]) { sm.scan = u; sm.fresh = 1; }
+          }
+        } else if (sm.scan < 0 && !cta.exhausted) {
           const int u = atomicAdd(bv.work_counter, 1);
           if (u < bv.n_scans) { sm.scan = u; sm.fresh = 1; } else cta.exhausted = 1;
         }
@@ -610,18 +615,18 @@ int fused_qtile(int max_q) { return choose_qtile(max_q); }
 
 size_t icp_state_bytes() { return sizeof(IcpState); }
 
-// the Gauss-Newton loop of estimateTransform on one unit whose queries, map and pose (state_in) are on the device: every
-// iteration is a reduction launch (MODE_ICP_REDUCE, linearised at bv.state_in) + the one-thread step kernel that updates
-// that pose; once the step kernel sets `done` the remaining queued launches return immediately.  No synchronisation.
-int icp_loop(lins_ctx* ctx, Resident& r, BatchView bv, double* pose, IcpState* icp, int icp_index) {
-  icp += icp_index;
-  CK(cudaMemsetAsync(icp, 0, sizeof(IcpState), ctx->stream));
+// the Gauss-Newton loop of estimateTransform on the bv.n_scans units of bv, whose queries, maps and poses (pose: 20 doubles
+// per unit, the linearisation point) are on the device: every iteration is one reduction launch over all units
+// (MODE_ICP_REDUCE) + one step launch with a block per unit that updates the unit's pose.  icp holds one IcpState per unit,
+// set by the caller: zero = run, done = 1 = skip.  Once a unit's step sets `done`, the remaining queued launches pass it
+// over.  No synchronisation.
+int icp_loop(lins_ctx* ctx, Resident& r, BatchView bv, double* pose, IcpState* icp) {
   bv.state_in = pose;
   bv.icp_done = &icp->done;
   for (int iter = 0; iter < ctx->prm.num_iter; ++iter) {
     const int rc = launch(ctx, r, bv, make_kparams(ctx->prm, MODE_ICP_REDUCE, iter));
     if (rc != LINS_OK) return rc;
-    lins_icp_step_kernel<<<1, 32, 0, ctx->stream>>>(bv.accum, pose, icp, iter);
+    lins_icp_step_kernel<<<bv.n_scans, 32, 0, ctx->stream>>>(bv.accum, pose, icp, iter);
     CK(cudaGetLastError());
     ctx->launches += 1;
   }
@@ -987,6 +992,7 @@ int lins_gpu_estimate_transform(lins_ctx* ctx, const lins_point* surf_flat, int 
   if (rc != LINS_OK) return rc;
   Resident& r = ctx->single;
   CK(r.icp.reserve(1)); CK(r.h_icp.reserve(1)); CK(r.h_state_out.reserve(20));
+  CK(cudaMemsetAsync(r.icp.p, 0, sizeof(IcpState), ctx->stream));
   rc = icp_loop(ctx, r, single_view(ctx, false), r.state_in.p, r.icp.p);
   if (rc != LINS_OK) return rc;
   CK(cudaMemcpyAsync(r.h_state_out.p, r.state_in.p, sizeof(double) * 20, cudaMemcpyDeviceToHost, ctx->stream));

@@ -7,14 +7,10 @@
 // shim still uses elsewhere): Householder QR with column pivoting and Eigen's rank rule, cyclic Jacobi, Gauss-Jordan.
 #pragma once
 #include "lins_device_math.cuh"
+#include "lins_kernels.cuh"  // IcpState
 #include <cstdio>
 
 namespace lins_dev {
-
-struct IcpState {
-  double matP[36];
-  int iters, converged, done, pad;
-};
 
 __device__ inline void icp_qr_solve6(double A[6][6], double b[6], double x[6]) {
   int perm[6];
@@ -122,10 +118,15 @@ __device__ inline bool icp_inverse6(double A[6][6], double inv[6][6]) {
   return true;
 }
 
-// accum: the 28 sums + counts of one MODE_ICP_REDUCE pass (entries 0..20 = upper triangle of J^T J, 21..26 = J^T b, 28 / 29 =
-// matched surfs / corners); state: the 20-double pose block the next pass linearises at (t at 0..2, q xyzw at 6..9).
+// One 32-thread block per unit u = blockIdx.x, thread 0 working.  accum + 32 u: the 28 sums + counts of one MODE_ICP_REDUCE
+// pass (entries 0..20 = upper triangle of J^T J, 21..26 = J^T b, 28 / 29 = matched surfs / corners); state + 20 u: the
+// 20-double pose block the next pass linearises at (t at 0..2, q xyzw at 6..9); st + u: the unit's loop state.
 __global__ void lins_icp_step_kernel(const double* __restrict__ accum, double* __restrict__ state, IcpState* __restrict__ st, int iter) {
-  if (threadIdx.x != 0 || blockIdx.x != 0 || st->done) return;
+  const int u = blockIdx.x;
+  accum += (size_t)u * 32;
+  state += (size_t)u * 20;
+  st += u;
+  if (threadIdx.x != 0 || st->done) return;
   st->iters = iter + 1;
   const double* a = accum;
   if (a[28] < 10) return;  // "Insufficient matched surfs..." (:1175-1178)

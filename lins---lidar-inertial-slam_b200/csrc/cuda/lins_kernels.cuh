@@ -73,10 +73,20 @@ struct BatchView {
   long long* timers;                     // optional: per-phase SM cycles summed over CTAs (diagnostics), 64 slots
   int qtile;                             // per-slot capacity of the per-query arrays (>= the largest unit, multiple of 32)
   int nslots;                            // resident units per CTA
-  const int* icp_done;                   // MODE_ICP_REDUCE: non-zero = the Gauss-Newton loop has converged, return at once (or null)
+  const int* icp_done;                   // MODE_ICP_REDUCE: IcpState::done of unit 0, unit u's kIcpDoneStride ints further
+                                         // (lins_icp_step.cuh); non-zero = that unit's Gauss-Newton loop has ended, skip it (or null)
   unsigned char* qscratch;               // per-CTA global scratch for the per-query arrays when they do not fit shared
   size_t qscratch_stride;                // memory (null: they live in shared memory)
 };
+
+// loop state of one unit's estimateTransform (lins_icp_step.cuh)
+struct IcpState {
+  double matP[36];
+  int iters, converged, done, pad;
+};
+// BatchView::icp_done points at the `done` of unit 0's IcpState; unit u's is kIcpDoneStride ints further
+constexpr int kIcpDoneStride = (int)(sizeof(IcpState) / sizeof(int));
+static_assert(sizeof(IcpState) % sizeof(int) == 0, "IcpState stride");
 
 struct KParams {
   int num_iter, icp_freq, force_all_iters, mode, iter0;

@@ -4,6 +4,10 @@
 //   one launch) -> divergence check (one D2H) -> estimateTransform loop per diverged sequence (lins_gpu.cu: icp_loop) ->
 //   update / integrateTransformation / reset(1) / roll-pitch (lins_seq_post_kernel) -> transformToEnd (CSR kernel of
 //   lins_gpu.cu) + the guarded map swap (lins_seq_copy_kernel).
+// Slots of a lins_gpu_seq_open run also initialise on the device (processPCL's status machine): the predict kernel
+//   pre-integrates a slot's IMU rows between its first and second scan, the second scans' estimateTransform runs as ONE
+//   batched icp_loop over all of them (lins_seq_icp_start_kernel sets its start poses), and lins_seq_init_kernel installs
+//   the state of processFirstScan / processSecondScan.
 // The filter algebra is lins_seq_step.cuh, shared with the CPU test.  Built with -fmad=false like the other bit-exact units.
 #include <cuda_runtime.h>
 
@@ -21,16 +25,27 @@ using lins_dev::BatchView;
 
 namespace {
 
+// what processImu does with a sequence's IMU rows this step (StateEstimator.hpp:242-270)
+enum ImuUse : unsigned char { IMU_IGNORE = 0, IMU_PREDICT = 1, IMU_PREINTEGRATE = 2 };
+// StateEstimator::FusionStatus
+enum Fusion : int32_t { FUSION_INIT = 0, FUSION_FIRST_SCAN = 1, FUSION_RUNNING = 3 };
+
 // One warp per sequence: the sequence's k StatePredictor::predict calls in order (kalman_filter.hpp:98-170).  The 18x18
 // matrices live in shared memory; lane l owns the entries e = l, l + 32, ... of every matrix phase, each entry summed in
-// the host's order.
+// the host's order.  A sequence in STATUS_FIRST_SCAN pre-integrates its rows instead (IntegrationBase::propagate, lane 0).
 __global__ void __launch_bounds__(32) lins_seq_predict_kernel(double* __restrict__ filt, double* __restrict__ cov, double* __restrict__ imu_last,
                                                              const double* __restrict__ imu, const int* __restrict__ imu_off,
-                                                             const unsigned char* __restrict__ status, const lins_seq::Consts k) {
+                                                             const unsigned char* __restrict__ use, double* __restrict__ pre,
+                                                             const lins_seq::Consts k, const lins_seq::InitConsts ik) {
   const int s = blockIdx.x, lane = threadIdx.x;
-  if (status[s] == LINS_SEQ_IDLE) return;
+  if (use[s] == IMU_IGNORE) return;
   const int m0 = imu_off[s], m1 = imu_off[s + 1];
   if (m0 == m1) return;
+  if (use[s] == IMU_PREINTEGRATE) {
+    if (lane == 0)
+      for (int m = m0; m < m1; ++m) lins_seq::preint_propagate(pre + (size_t)s * 20, ik, imu[(size_t)m * 7], imu + (size_t)m * 7 + 1, imu + (size_t)m * 7 + 4);
+    return;
+  }
   __shared__ double P[324], Ft[324], F[324], FP[324], P2[324];
   __shared__ double st[20], al[3], gl[3];
   __shared__ lins_seq::PredictBlocks sb;  // R, va, aa of the sample being applied
@@ -75,7 +90,7 @@ __global__ void lins_seq_post_kernel(int n, const unsigned char* __restrict__ st
                                      const double* __restrict__ cov_out, const double* __restrict__ icp_pose, double* __restrict__ filt,
                                      double* __restrict__ cov, double* __restrict__ glob, double* __restrict__ lin, const lins_seq::Consts k) {
   const int s = blockIdx.x * blockDim.x + threadIdx.x;
-  if (s >= n || status[s] < LINS_SEQ_RAN) return;
+  if (s >= n || (status[s] != LINS_SEQ_RAN && status[s] != LINS_SEQ_ICP)) return;
   double f[20];
   for (int i = 0; i < 20; ++i) f[i] = state_out[(size_t)s * 20 + i];
   double* L = lin + (size_t)s * 20;
@@ -94,6 +109,45 @@ __global__ void lins_seq_post_kernel(int n, const unsigned char* __restrict__ st
   for (int i = 0; i < 19; ++i) filt[(size_t)s * 20 + i] = f[i];
 }
 
+// One thread per second scan: the start pose of its estimateTransform (processSecondScan's pl / ql) and a fresh loop state;
+// every other sequence's loop state reads done, so the batched loop passes it over.
+__global__ void lins_seq_icp_start_kernel(int n, const unsigned char* __restrict__ status, const double* __restrict__ pre,
+                                          double* __restrict__ icp_pose, lins_dev::IcpState* __restrict__ icp) {
+  const int s = blockIdx.x * blockDim.x + threadIdx.x;
+  if (s >= n) return;
+  const bool second = status[s] == LINS_SEQ_SECOND;
+  lins_dev::IcpState& st = icp[s];
+  for (int i = 0; i < 36; ++i) st.matP[i] = 0.0;
+  st.iters = 0; st.converged = 0; st.pad = 0;
+  st.done = second ? 0 : 1;
+  if (second) lins_seq::second_scan_start(pre + (size_t)s * 20, icp_pose + (size_t)s * 20);
+}
+
+// One thread per sequence that initialised this step: processFirstScan (LINS_SEQ_FIRST) or the rest of processSecondScan
+// after its estimateTransform (LINS_SEQ_SECOND; icp_pose holds the result).  imu: the step's processPCL samples, 6 per
+// sequence.
+__global__ void lins_seq_init_kernel(int n, const unsigned char* __restrict__ status, const double* __restrict__ imu,
+                                     const double* __restrict__ icp_pose, double* __restrict__ pre, double* __restrict__ glob,
+                                     double* __restrict__ filt, double* __restrict__ cov, double* __restrict__ lin,
+                                     double* __restrict__ imu_last, const lins_seq::InitConsts k) {
+  const int s = blockIdx.x * blockDim.x + threadIdx.x;
+  if (s >= n) return;
+  const size_t o = (size_t)s * 20;
+  double* il = imu_last + (size_t)s * 8;
+  if (status[s] == LINS_SEQ_FIRST)
+    lins_seq::first_scan(filt + o, cov + (size_t)s * 324, lin + o, pre + o, il, imu + (size_t)s * 6, k);
+  else if (status[s] == LINS_SEQ_SECOND)
+    lins_seq::second_scan(glob + o, filt + o, cov + (size_t)s * 324, lin + o, il, pre + o, icp_pose + o, imu + (size_t)s * 6, k);
+}
+
+// One thread per sequence with mask[s] != 0 (every sequence for a null mask): the state of a new StateEstimator
+__global__ void lins_seq_fresh_kernel(int n, const unsigned char* __restrict__ mask, double* __restrict__ glob, double* __restrict__ filt,
+                                      double* __restrict__ cov, const lins_seq::InitConsts k) {
+  const int s = blockIdx.x * blockDim.x + threadIdx.x;
+  if (s >= n || (mask && !mask[s])) return;
+  lins_seq::fresh_slot(glob + (size_t)s * 20, filt + (size_t)s * 20, cov + (size_t)s * 324, k);
+}
+
 __global__ void lins_seq_copy_kernel(const SeqCopy* __restrict__ copies) {
   const SeqCopy c = copies[blockIdx.x];
   for (int i = threadIdx.x; i < c.n; i += blockDim.x) c.dst[i] = c.src[i];
@@ -103,6 +157,47 @@ lins_seq::Consts consts_of(const SeqState& q) {
   lins_seq::Consts k;
   std::memcpy(&k, q.consts, sizeof(k));
   return k;
+}
+lins_seq::InitConsts init_consts_of(const SeqState& q) {
+  lins_seq::InitConsts k;
+  static_assert(sizeof(k) == sizeof(q.init_consts), "init consts");
+  std::memcpy(&k, q.init_consts, sizeof(k));
+  return k;
+}
+
+// noise, sq(init_pos_std) and pow(deg2rad(init_att_std), 2) of lins_seq_params (kalman_filter.hpp setNoise / reset(1))
+void set_consts(SeqState& q, const lins_seq_params* prm) {
+  lins_seq::Consts k;
+  for (int i = 0; i < 4; ++i) k.noise[i] = prm->noise[i];
+  for (int i = 0; i < 3; ++i) {
+    k.pos_var[i] = prm->init_pos_std[i] * prm->init_pos_std[i];                 // sq(init_pos_std)
+    k.att_var[i] = std::pow(prm->init_att_std[i] * M_PI / 180.0, 2);            // pow(deg2rad(init_att_std), 2)
+  }
+  static_assert(sizeof(k) == sizeof(q.consts), "consts");
+  std::memcpy(q.consts, &k, sizeof(k));
+}
+
+// the diagonal initializeCovariance installs (kalman_filter.hpp:197-209) and init_ba / init_bw
+void set_init_consts(SeqState& q, const lins_seq_params* prm, const lins_seq_init_params* ip) {
+  lins_seq::InitConsts k;
+  for (int i = 0; i < 3; ++i) {
+    k.var[lins_seq::kPos + i] = prm->init_pos_std[i] * prm->init_pos_std[i];
+    k.var[lins_seq::kVel + i] = ip->init_vel_std[i] * ip->init_vel_std[i];
+    k.var[lins_seq::kAtt + i] = std::pow(prm->init_att_std[i] * M_PI / 180.0, 2);
+    k.var[lins_seq::kAcc + i] = ip->init_acc_std[i] * ip->init_acc_std[i];
+    k.var[lins_seq::kGyr + i] = ip->init_gyr_std[i] * ip->init_gyr_std[i];
+    k.var[lins_seq::kGra + i] = 0.01;
+    k.ba[i] = ip->init_ba[i];
+    k.bw[i] = ip->init_bw[i];
+  }
+  std::memcpy(q.init_consts, &k, sizeof(k));
+}
+
+int launch_fresh(lins_ctx* ctx, SeqState& q, int n, const unsigned char* mask_dev) {
+  lins_seq_fresh_kernel<<<(n + 127) / 128, 128, 0, ctx->stream>>>(n, mask_dev, q.glob.p, q.filt.p, q.cov.p, init_consts_of(q));
+  CK(cudaGetLastError());
+  ctx->launches += 1;
+  return LINS_OK;
 }
 
 int check_csr(lins_ctx* ctx, const int32_t* off, int n, const void* data, const char* what) {
@@ -123,7 +218,7 @@ int run_copies(lins_ctx* ctx, const SeqCopy* dev, int count) {
 
 }  // namespace
 
-static int seq_step_run(lins_ctx* ctx, const lins_seq_step_desc* d, const int32_t* const offs[4]);
+static int seq_step_run(lins_ctx* ctx, const lins_seq_step_desc* d, const int32_t* const offs[4], const double* scan_imu);
 
 extern "C" {
 
@@ -170,14 +265,7 @@ int lins_gpu_seq_begin(lins_ctx* ctx, const lins_seq_params* prm, const lins_seq
   CK(cudaMemcpyAsync(q.map_off.p, q.h_map_off.data(), sizeof(int) * q.h_map_off.size(), cudaMemcpyHostToDevice, ctx->stream));
   CK(cudaMemcpyAsync(q.stale.p, q.h_stale_v.data(), n, cudaMemcpyHostToDevice, ctx->stream));
   CK(cudaStreamSynchronize(ctx->stream));  // (the sources above are pageable host memory)
-  lins_seq::Consts k;
-  for (int i = 0; i < 4; ++i) k.noise[i] = prm->noise[i];
-  for (int i = 0; i < 3; ++i) {
-    k.pos_var[i] = prm->init_pos_std[i] * prm->init_pos_std[i];                 // sq(init_pos_std)
-    k.att_var[i] = std::pow(prm->init_att_std[i] * M_PI / 180.0, 2);            // pow(deg2rad(init_att_std), 2)
-  }
-  static_assert(sizeof(k) == sizeof(q.consts), "consts");
-  std::memcpy(q.consts, &k, sizeof(k));
+  set_consts(q, prm);
   // result records / reports read as zero until a step has run a sequence's IESKF
   CK(q.run.results.reserve(n)); CK(q.run.reports.reserve(n));
   CK(cudaMemsetAsync(q.run.results.p, 0, sizeof(lins_scan_result) * n, ctx->stream));
@@ -185,11 +273,96 @@ int lins_gpu_seq_begin(lins_ctx* ctx, const lins_seq_params* prm, const lins_seq
   q.ev_valid = false;
   q.has_step = false;
   q.status.assign(n, LINS_SEQ_IDLE);
+  q.has_init = false;
+  q.fusion.assign(n, FUSION_RUNNING);
   q.n = n;
   return LINS_OK;
 }
 
-int lins_gpu_seq_step(lins_ctx* ctx, const lins_seq_step_desc* d) {
+int lins_gpu_seq_open(lins_ctx* ctx, const lins_seq_params* prm, const lins_seq_init_params* ip, int32_t n_seq) {
+  if (!ctx) return LINS_E_INVALID;
+  if (!prm || !ip || n_seq < 1) return fail(ctx, LINS_E_INVALID, "bad lins_gpu_seq_open arguments");
+  CK(cudaSetDevice(ctx->device));
+  SeqState& q = ctx->seq;
+  q.n = 0;  // (until the slots are in place)
+  const int n = n_seq;
+  CK(q.filt.reserve((size_t)n * 20)); CK(q.cov.reserve((size_t)n * 324)); CK(q.glob.reserve((size_t)n * 20));
+  CK(q.lin.reserve((size_t)n * 20)); CK(q.imu_last.reserve((size_t)n * 8)); CK(q.icp_pose.reserve((size_t)n * 20)); CK(q.icp.reserve(icp_state_bytes() * n));
+  CK(q.pre.reserve((size_t)n * 20)); CK(q.init_icp.reserve(icp_state_bytes() * n));
+  CK(q.map_s.reserve(1)); CK(q.map_c.reserve(1)); CK(q.tree_s.reserve(1)); CK(q.tree_c.reserve(1));
+  CK(q.map_off.reserve(4 * (size_t)(n + 1))); CK(q.stale.reserve(n));
+  CK(q.run.results.reserve(n)); CK(q.run.reports.reserve(n));
+  set_consts(q, prm);
+  set_init_consts(q, prm, ip);
+  q.h_map_off.assign(4 * (size_t)(n + 1), 0);  // no maps
+  q.h_stale_v.assign(n, 0);
+  CK(cudaMemsetAsync(q.lin.p, 0, sizeof(double) * 20 * (size_t)n, ctx->stream));
+  CK(cudaMemsetAsync(q.imu_last.p, 0, sizeof(double) * 8 * (size_t)n, ctx->stream));
+  CK(cudaMemsetAsync(q.pre.p, 0, sizeof(double) * 20 * (size_t)n, ctx->stream));
+  CK(cudaMemsetAsync(q.icp_pose.p, 0, sizeof(double) * 20 * (size_t)n, ctx->stream));
+  CK(cudaMemsetAsync(q.init_icp.p, 0, icp_state_bytes() * n, ctx->stream));
+  CK(cudaMemsetAsync(q.run.results.p, 0, sizeof(lins_scan_result) * n, ctx->stream));
+  CK(cudaMemsetAsync(q.run.reports.p, 0, sizeof(lins_report) * n, ctx->stream));
+  CK(cudaMemcpyAsync(q.map_off.p, q.h_map_off.data(), sizeof(int) * q.h_map_off.size(), cudaMemcpyHostToDevice, ctx->stream));
+  CK(cudaMemcpyAsync(q.stale.p, q.h_stale_v.data(), n, cudaMemcpyHostToDevice, ctx->stream));
+  const int rc = launch_fresh(ctx, q, n, nullptr);
+  if (rc != LINS_OK) return rc;
+  CK(cudaStreamSynchronize(ctx->stream));  // (the sources above are pageable host memory)
+  q.ev_valid = false;
+  q.has_step = false;
+  q.status.assign(n, LINS_SEQ_IDLE);
+  q.has_init = true;
+  q.fusion.assign(n, FUSION_INIT);
+  q.n = n;
+  return LINS_OK;
+}
+
+int lins_gpu_seq_restart(lins_ctx* ctx, const uint8_t* mask) {
+  if (!ctx) return LINS_E_INVALID;
+  SeqState& q = ctx->seq;
+  if (q.n == 0) return fail(ctx, LINS_E_NOMAP, "no sequence run: call lins_gpu_seq_open");
+  if (!mask) return fail(ctx, LINS_E_INVALID, "null restart mask");
+  if (!q.has_init) return fail(ctx, LINS_E_INVALID, "lins_gpu_seq_restart needs a run opened by lins_gpu_seq_open");
+  CK(cudaSetDevice(ctx->device));
+  const int n = q.n, N1 = n + 1;
+  // the restarted slots' maps go: the other slots' ranges are copied into the next generation, which is swapped in
+  const int* mo = q.h_map_off.data();
+  q.h_nmap_off.assign(4 * (size_t)N1, 0);
+  int* no = q.h_nmap_off.data();
+  std::vector<SeqCopy> copies;
+  std::vector<std::pair<int, int>> to;
+  const float4* srcs[4] = {q.map_s.p, q.map_c.p, q.tree_s.p, q.tree_c.p};
+  for (int c = 0; c < 4; ++c)
+    for (int s = 0; s < n; ++s) {
+      const int len = mask[s] ? 0 : mo[c * N1 + s + 1] - mo[c * N1 + s];
+      no[c * N1 + s + 1] = no[c * N1 + s] + len;
+      if (len) { copies.push_back(SeqCopy{srcs[c] + mo[c * N1 + s], nullptr, len, 0}); to.emplace_back(c, no[c * N1 + s]); }
+    }
+  CK(q.nmap_s.reserve((size_t)no[N1 - 1] + 1)); CK(q.nmap_c.reserve((size_t)no[2 * N1 - 1] + 1));
+  CK(q.ntree_s.reserve((size_t)no[3 * N1 - 1] + 1)); CK(q.ntree_c.reserve((size_t)no[4 * N1 - 1] + 1));
+  CK(q.copies.reserve(copies.size() + 1)); CK(q.h_copies.reserve(copies.size() + 1));
+  CK(q.status_d.reserve(3 * (size_t)n)); CK(q.h_status.reserve(3 * (size_t)n));
+  float4* dst[4] = {q.nmap_s.p, q.nmap_c.p, q.ntree_s.p, q.ntree_c.p};
+  for (size_t i = 0; i < copies.size(); ++i) copies[i].dst = dst[to[i].first] + to[i].second;
+  // (the last step ended with a stream synchronisation: the pinned staging is free)
+  std::copy(copies.begin(), copies.end(), q.h_copies.p);
+  for (int s = 0; s < n; ++s) q.h_status.p[s] = mask[s] ? 1 : 0;
+  if (!copies.empty()) CK(cudaMemcpyAsync(q.copies.p, q.h_copies.p, sizeof(SeqCopy) * copies.size(), cudaMemcpyHostToDevice, ctx->stream));
+  CK(cudaMemcpyAsync(q.status_d.p, q.h_status.p, n, cudaMemcpyHostToDevice, ctx->stream));
+  int rc = run_copies(ctx, q.copies.p, (int)copies.size());
+  if (rc == LINS_OK) rc = launch_fresh(ctx, q, n, q.status_d.p);
+  if (rc != LINS_OK) { q.n = 0; return rc; }  // (some slots may have changed: the run ends, as after a failed step)
+  std::swap(q.map_s, q.nmap_s); std::swap(q.map_c, q.nmap_c); std::swap(q.tree_s, q.ntree_s); std::swap(q.tree_c, q.ntree_c);
+  q.h_map_off.swap(q.h_nmap_off);
+  for (int s = 0; s < n; ++s)
+    if (mask[s]) { q.h_stale_v[s] = 0; q.fusion[s] = FUSION_INIT; q.status[s] = LINS_SEQ_IDLE; }
+  CK(cudaMemcpyAsync(q.map_off.p, q.h_map_off.data(), sizeof(int) * 4 * N1, cudaMemcpyHostToDevice, ctx->stream));
+  CK(cudaMemcpyAsync(q.stale.p, q.h_stale_v.data(), n, cudaMemcpyHostToDevice, ctx->stream));
+  CK(cudaStreamSynchronize(ctx->stream));  // (the two sources above are pageable)
+  return LINS_OK;
+}
+
+int lins_gpu_seq_step_ex(lins_ctx* ctx, const lins_seq_step_desc* d, const double* scan_imu) {
   if (!ctx) return LINS_E_INVALID;
   SeqState& q = ctx->seq;
   if (q.n == 0) return fail(ctx, LINS_E_NOMAP, "lins_gpu_seq_begin has not been called");
@@ -200,19 +373,25 @@ int lins_gpu_seq_step(lins_ctx* ctx, const lins_seq_step_desc* d) {
   for (int k = 0; k < 4; ++k) { const int rc = check_csr(ctx, offs[k], n, pts[k], "bad cloud offsets / cloud"); if (rc != LINS_OK) return rc; }
   if (d->imu_off) { const int rc = check_csr(ctx, d->imu_off, n, d->imu, "bad imu offsets / samples"); if (rc != LINS_OK) return rc; }
   else if (d->imu) return fail(ctx, LINS_E_INVALID, "imu without imu_off");
+  if (!scan_imu)
+    for (int s = 0; s < n; ++s)
+      if ((!d->present || d->present[s]) && q.fusion[s] != FUSION_RUNNING)
+        return fail(ctx, LINS_E_INVALID, "scan_imu is required while a present slot is initialising");
   CK(cudaSetDevice(ctx->device));
   int rc = upload_clouds(ctx, q.up, n, pts, offs, d->point_format);  // (validates the rest; synchronises the stream first)
   if (rc != LINS_OK) return rc;
   // from here on the sequences' state changes: a failure ends the run (lins_gpu.h), the context stays usable
-  rc = seq_step_run(ctx, d, offs);
+  rc = seq_step_run(ctx, d, offs, scan_imu);
   if (rc != LINS_OK) q.n = 0;
   return rc;
 }
 
+int lins_gpu_seq_step(lins_ctx* ctx, const lins_seq_step_desc* d) { return lins_gpu_seq_step_ex(ctx, d, nullptr); }
+
 }  // extern "C"
 
 // the part of lins_gpu_seq_step after its input is validated and uploaded
-static int seq_step_run(lins_ctx* ctx, const lins_seq_step_desc* d, const int32_t* const offs[4]) {
+static int seq_step_run(lins_ctx* ctx, const lins_seq_step_desc* d, const int32_t* const offs[4], const double* scan_imu) {
   SeqState& q = ctx->seq;
   const int n = q.n;
   int rc = LINS_OK;
@@ -227,12 +406,21 @@ static int seq_step_run(lins_ctx* ctx, const lins_seq_step_desc* d, const int32_
   std::vector<SeqCopy> qcopies, mcopies;
   std::vector<std::pair<int, int>> qto, mto;  // destination of each copy: (cloud, offset), resolved once the buffers exist
   std::vector<unsigned char> new_stale(q.h_stale_v);
-  int max_q = 0, n_run = 0;
+  std::vector<unsigned char> imu_use(n, IMU_IGNORE);
+  int max_q = 0, n_run = 0, n_init = 0, n_second = 0;
   for (int s = 0; s < n; ++s) {
     const bool present = !d->present || d->present[s];
     const int nsl = offs[2][s + 1] - offs[2][s], ncl = offs[3][s + 1] - offs[3][s];
-    status[s] = !present ? LINS_SEQ_IDLE : (ncl <= 5 || nsl <= 10) ? LINS_SEQ_SKIPPED : LINS_SEQ_RAN;  // :436-440
+    const int32_t fs = q.fusion[s];
+    if (!present) status[s] = LINS_SEQ_IDLE;
+    else if (fs == FUSION_RUNNING) status[s] = (ncl <= 5 || nsl <= 10) ? LINS_SEQ_SKIPPED : LINS_SEQ_RAN;  // :436-440
+    else if (ncl < 10 || nsl < 100) status[s] = LINS_SEQ_INIT_WAIT;  // processFirstScan / processSecondScan (:331-336, :379-384)
+    else status[s] = fs == FUSION_INIT ? LINS_SEQ_FIRST : LINS_SEQ_SECOND;
+    if (present) imu_use[s] = fs == FUSION_RUNNING ? IMU_PREDICT : fs == FUSION_FIRST_SCAN ? IMU_PREINTEGRATE : IMU_IGNORE;
     const bool ran = status[s] == LINS_SEQ_RAN;
+    const bool init = status[s] == LINS_SEQ_FIRST || status[s] == LINS_SEQ_SECOND;
+    n_init += init;
+    n_second += status[s] == LINS_SEQ_SECOND;
     const int nq[2] = {ran ? offs[0][s + 1] - offs[0][s] : 0, ran ? offs[1][s + 1] - offs[1][s] : 0};
     for (int c = 0; c < 2; ++c) {
       run_off[c * N1 + s + 1] = run_off[c * N1 + s] + nq[c];
@@ -240,10 +428,11 @@ static int seq_step_run(lins_ctx* ctx, const lins_seq_step_desc* d, const int32_
     }
     if (ran) { max_q = std::max(max_q, nq[0] + nq[1]); ++n_run; }
     // map swap (:1151-1160): the new clouds become the map; the 1-NN index is rebuilt iff ncl >= 5 && nsl >= 20, else it
-    // stays on the cloud it was built on (the old map, or an older stale cloud)
+    // stays on the cloud it was built on (the old map, or an older stale cloud).  A first scan's clouds become the map
+    // as they are (setInputCloud, :363-364) and a second scan's like a running one's: both pass the guard after the init gate.
     int len[4];  // map_s, map_c, tree_s, tree_c
     int src_kind[4];  // 0 new cloud, 1 old map, 2 old tree, -1 none
-    if (ran) {
+    if (ran || init) {
       const bool guard = ncl >= 5 && nsl >= 20;
       len[0] = nsl; len[1] = ncl; src_kind[0] = src_kind[1] = 0;
       if (guard) { len[2] = len[3] = 0; src_kind[2] = src_kind[3] = -1; new_stale[s] = 0; }
@@ -264,20 +453,36 @@ static int seq_step_run(lins_ctx* ctx, const lins_seq_step_desc* d, const int32_
       mto.emplace_back(c, no[c * N1 + s]);
     }
   }
+  // the second scans' queries follow the IESKF's in the compacted buffers, with offsets of their own (init_off): the IESKF
+  // launch sees no query of theirs, the estimateTransform loop none of the IESKF's
+  std::vector<int> init_off(2 * (size_t)N1, 0);
+  int max_init_q = 0;
+  for (int c = 0; c < 2; ++c) init_off[c * N1] = run_off[c * N1 + N1 - 1];
+  for (int s = 0; s < n; ++s) {
+    const bool second = status[s] == LINS_SEQ_SECOND;
+    const int nq[2] = {second ? offs[0][s + 1] - offs[0][s] : 0, second ? offs[1][s + 1] - offs[1][s] : 0};
+    for (int c = 0; c < 2; ++c) {
+      init_off[c * N1 + s + 1] = init_off[c * N1 + s] + nq[c];
+      if (nq[c]) { qcopies.push_back(SeqCopy{(c ? q.up.qc.p : q.up.qs.p) + offs[c][s], nullptr, nq[c], 0}); qto.emplace_back(c, init_off[c * N1 + s]); }
+    }
+    if (second) max_init_q = std::max(max_init_q, nq[0] + nq[1]);
+  }
 
   // ---- allocations ------------------------------------------------------------------------------------------------
   Resident& r = q.run;
-  r.n = n; r.nqs = run_off[N1 - 1]; r.nqc = run_off[2 * N1 - 1]; r.max_q = max_q;
+  r.n = n; r.nqs = init_off[N1 - 1]; r.nqc = init_off[2 * N1 - 1]; r.max_q = max_q;
   r.nts = mo[N1 - 1]; r.ntc = mo[2 * N1 - 1];
   CK(r.qs.reserve(r.nqs + 1)); CK(r.qc.reserve(r.nqc + 1)); CK(r.qs_off.reserve(N1)); CK(r.qc_off.reserve(N1));
   rc = reserve_outputs(ctx, r, true, false);
   if (rc != LINS_OK) return rc;
-  CK(r.h_off.reserve(2 * (size_t)N1));
+  CK(r.h_off.reserve(4 * (size_t)N1));
+  if (n_init) { CK(q.init_off.reserve(2 * (size_t)N1)); CK(q.scan_imu.reserve((size_t)n * 6)); CK(q.h_scan_imu.reserve((size_t)n * 6)); }
+  // (pre and init_icp are lins_gpu_seq_open's: they keep their contents from step to step)
   CK(q.nmap_s.reserve((size_t)no[N1 - 1] + 1)); CK(q.nmap_c.reserve((size_t)no[2 * N1 - 1] + 1));
   CK(q.ntree_s.reserve((size_t)no[3 * N1 - 1] + 1)); CK(q.ntree_c.reserve((size_t)no[4 * N1 - 1] + 1));
   const size_t n_imu = d->imu_off ? (size_t)d->imu_off[n] : 0;
   CK(q.imu.reserve(7 * n_imu + 1)); CK(q.imu_off.reserve(N1)); CK(q.h_imu.reserve(7 * n_imu + 1)); CK(q.h_imu_off.reserve(N1));
-  CK(q.status_d.reserve(2 * (size_t)n)); CK(q.h_status.reserve(2 * (size_t)n));
+  CK(q.status_d.reserve(3 * (size_t)n)); CK(q.h_status.reserve(3 * (size_t)n));
   const size_t n_copies = qcopies.size() + mcopies.size();
   CK(q.copies.reserve(n_copies + 1)); CK(q.h_copies.reserve(n_copies + 1));
   CK(q.prior_state.reserve((size_t)n * 20)); CK(q.prior_cov.reserve((size_t)n * 324));
@@ -291,24 +496,32 @@ static int seq_step_run(lins_ctx* ctx, const lins_seq_step_desc* d, const int32_
   if (d->imu_off) std::memcpy(q.h_imu_off.p, d->imu_off, sizeof(int) * N1);
   else std::memset(q.h_imu_off.p, 0, sizeof(int) * N1);
   if (n_imu) std::memcpy(q.h_imu.p, d->imu, sizeof(double) * 7 * n_imu);
-  for (int s = 0; s < n; ++s) q.h_status.p[s] = (unsigned char)status[s];
+  for (int s = 0; s < n; ++s) { q.h_status.p[s] = (unsigned char)status[s]; q.h_status.p[2 * n + s] = imu_use[s]; }
   std::copy(qcopies.begin(), qcopies.end(), q.h_copies.p);
   std::copy(mcopies.begin(), mcopies.end(), q.h_copies.p + qcopies.size());
   std::memcpy(r.h_off.p, run_off.data(), sizeof(int) * 2 * N1);
+  std::memcpy(r.h_off.p + 2 * N1, init_off.data(), sizeof(int) * 2 * N1);
   if (n_imu) CK(cudaMemcpyAsync(q.imu.p, q.h_imu.p, sizeof(double) * 7 * n_imu, cudaMemcpyHostToDevice, ctx->stream));
   CK(cudaMemcpyAsync(q.imu_off.p, q.h_imu_off.p, sizeof(int) * N1, cudaMemcpyHostToDevice, ctx->stream));
   CK(cudaMemcpyAsync(q.status_d.p, q.h_status.p, n, cudaMemcpyHostToDevice, ctx->stream));
+  CK(cudaMemcpyAsync(q.status_d.p + 2 * n, q.h_status.p + 2 * n, n, cudaMemcpyHostToDevice, ctx->stream));
   if (n_copies) CK(cudaMemcpyAsync(q.copies.p, q.h_copies.p, sizeof(SeqCopy) * n_copies, cudaMemcpyHostToDevice, ctx->stream));
   CK(cudaMemcpyAsync(r.qs_off.p, r.h_off.p, sizeof(int) * N1, cudaMemcpyHostToDevice, ctx->stream));
   CK(cudaMemcpyAsync(r.qc_off.p, r.h_off.p + N1, sizeof(int) * N1, cudaMemcpyHostToDevice, ctx->stream));
+  if (n_init) {
+    std::memcpy(q.h_scan_imu.p, scan_imu, sizeof(double) * 6 * (size_t)n);  // (validated: non-null when a slot initialises)
+    CK(cudaMemcpyAsync(q.scan_imu.p, q.h_scan_imu.p, sizeof(double) * 6 * (size_t)n, cudaMemcpyHostToDevice, ctx->stream));
+    CK(cudaMemcpyAsync(q.init_off.p, r.h_off.p + 2 * N1, sizeof(int) * 2 * N1, cudaMemcpyHostToDevice, ctx->stream));
+  }
 
-  // ---- 1. IMU propagation -----------------------------------------------------------------------------------------
+  // ---- 1. IMU propagation (StatePredictor::predict; the pre-integration of a slot between its first and second scan) --
   for (cudaEvent_t& e : q.ev) if (!e) CK(cudaEventCreate(&e));
   q.ev_valid = false;
   CK(cudaEventRecord(q.ev[0], ctx->stream));
   const lins_seq::Consts k = consts_of(q);
+  const lins_seq::InitConsts ik = init_consts_of(q);
   if (n_imu) {
-    lins_seq_predict_kernel<<<n, 32, 0, ctx->stream>>>(q.filt.p, q.cov.p, q.imu_last.p, q.imu.p, q.imu_off.p, q.status_d.p, k);
+    lins_seq_predict_kernel<<<n, 32, 0, ctx->stream>>>(q.filt.p, q.cov.p, q.imu_last.p, q.imu.p, q.imu_off.p, q.status_d.p + 2 * n, q.pre.p, k, ik);
     CK(cudaGetLastError());
     ctx->launches += 1;
   }
@@ -316,9 +529,10 @@ static int seq_step_run(lins_ctx* ctx, const lins_seq_step_desc* d, const int32_
   CK(cudaMemcpyAsync(q.prior_state.p, q.filt.p, sizeof(double) * 20 * (size_t)n, cudaMemcpyDeviceToDevice, ctx->stream));
   CK(cudaMemcpyAsync(q.prior_cov.p, q.cov.p, sizeof(double) * 324 * (size_t)n, cudaMemcpyDeviceToDevice, ctx->stream));
   CK(cudaEventRecord(q.ev[1], ctx->stream));
-  if (n_run == 0) {  // nothing passed the gate: the maps stay, nothing else to do
+  if (n_run == 0 && n_init == 0) {  // nothing passed the gate: the maps stay, nothing else to do
     for (int e = 2; e < 5; ++e) CK(cudaEventRecord(q.ev[e], ctx->stream));
     CK(cudaStreamSynchronize(ctx->stream));
+    for (int s = 0; s < n; ++s) if (status[s] == LINS_SEQ_INIT_WAIT) q.fusion[s] = FUSION_INIT;
     q.ev_valid = true;
     q.has_step = true;
     q.h_run_off.swap(run_off);
@@ -340,16 +554,20 @@ static int seq_step_run(lins_ctx* ctx, const lins_seq_step_desc* d, const int32_
   bv.ind_s = r.ind_s.p; bv.ind_c = r.ind_c.p; bv.az_s = r.az_s.p; bv.az_c = r.az_c.p;
   bv.accum = r.accum.p; bv.work_counter = r.counter.p;
   bv.qtile = fused_qtile(r.max_q);
-  rc = fused_ieskf_launch(ctx, r, bv);
-  if (rc != LINS_OK) return rc;
+  if (n_run) {
+    rc = fused_ieskf_launch(ctx, r, bv);
+    if (rc != LINS_OK) return rc;
+  }
   CK(cudaEventRecord(q.ev[2], ctx->stream));
 
   // ---- 3. divergence: one D2H of the result records -----------------------------------------------------------------
-  CK(r.h_results.reserve(n));
-  CK(cudaMemcpyAsync(r.h_results.p, r.results.p, sizeof(lins_scan_result) * n, cudaMemcpyDeviceToHost, ctx->stream));
-  CK(cudaStreamSynchronize(ctx->stream));
   bool any_icp = false;
-  for (int s = 0; s < n; ++s) {
+  if (n_run) {
+    CK(r.h_results.reserve(n));
+    CK(cudaMemcpyAsync(r.h_results.p, r.results.p, sizeof(lins_scan_result) * n, cudaMemcpyDeviceToHost, ctx->stream));
+    CK(cudaStreamSynchronize(ctx->stream));
+  }
+  for (int s = 0; s < n && n_run; ++s) {
     if (status[s] != LINS_SEQ_RAN || !(r.h_results.p[s].flags & 2u)) continue;
     // estimateTransform from the prior's pose (performIESKF's "Using ICP Method" branch, StateEstimator.hpp:585-592)
     status[s] = LINS_SEQ_ICP;
@@ -363,21 +581,48 @@ static int seq_step_run(lins_ctx* ctx, const lins_seq_step_desc* d, const int32_
     u.accum += (size_t)s * 32;
     u.ind_s = q.icp_ind_s.p; u.ind_c = q.icp_ind_c.p;  // (the IESKF's IDs stay readable)
     u.qtile = fused_qtile((run_off[s + 1] - run_off[s]) + (run_off[N1 + s + 1] - run_off[N1 + s]));
-    rc = icp_loop(ctx, r, u, q.icp_pose.p + (size_t)s * 20, reinterpret_cast<lins_dev::IcpState*>(q.icp.p), s);
+    lins_dev::IcpState* icp = reinterpret_cast<lins_dev::IcpState*>(q.icp.p) + s;
+    CK(cudaMemsetAsync(icp, 0, icp_state_bytes(), ctx->stream));
+    rc = icp_loop(ctx, r, u, q.icp_pose.p + (size_t)s * 20, icp);
     if (rc != LINS_OK) return rc;
   }
   if (any_icp) CK(cudaMemcpyAsync(q.status_d.p, q.h_status.p, n, cudaMemcpyHostToDevice, ctx->stream));
+
+  // ---- 3b. the second scans' estimateTransform (processSecondScan), all in one loop: each from its pre-integrated pose
+  // against its first scan's map; the IESKF's sequences read done and are passed over --------------------------------
+  lins_dev::IcpState* init_icp = reinterpret_cast<lins_dev::IcpState*>(q.init_icp.p);
+  if (n_second) {
+    lins_seq_icp_start_kernel<<<(n + 127) / 128, 128, 0, ctx->stream>>>(n, q.status_d.p, q.pre.p, q.icp_pose.p, init_icp);
+    CK(cudaGetLastError());
+    ctx->launches += 1;
+    BatchView u = bv;
+    u.qs_off = q.init_off.p; u.qc_off = q.init_off.p + N1;
+    u.reports = nullptr;
+    u.ind_s = q.icp_ind_s.p; u.ind_c = q.icp_ind_c.p;
+    u.qtile = fused_qtile(max_init_q);
+    rc = icp_loop(ctx, r, u, q.icp_pose.p, init_icp);
+    if (rc != LINS_OK) return rc;
+  }
   CK(cudaEventRecord(q.ev[3], ctx->stream));
 
-  // ---- 4. update, integrateTransformation, reset(1), roll / pitch --------------------------------------------------
-  lins_seq_post_kernel<<<(n + 127) / 128, 128, 0, ctx->stream>>>(n, q.status_d.p, r.state_out.p, r.cov_out.p, q.icp_pose.p, q.filt.p, q.cov.p,
-                                                                   q.glob.p, q.lin.p, k);
-  CK(cudaGetLastError());
-  ctx->launches += 1;
+  // ---- 4. update, integrateTransformation, reset(1), roll / pitch; processFirstScan / the rest of processSecondScan ---
+  if (n_run) {
+    lins_seq_post_kernel<<<(n + 127) / 128, 128, 0, ctx->stream>>>(n, q.status_d.p, r.state_out.p, r.cov_out.p, q.icp_pose.p, q.filt.p, q.cov.p,
+                                                                     q.glob.p, q.lin.p, k);
+    CK(cudaGetLastError());
+    ctx->launches += 1;
+  }
+  if (n_init) {
+    lins_seq_init_kernel<<<(n + 127) / 128, 128, 0, ctx->stream>>>(n, q.status_d.p, q.scan_imu.p, q.icp_pose.p, q.pre.p, q.glob.p, q.filt.p,
+                                                                     q.cov.p, q.lin.p, q.imu_last.p, ik);
+    CK(cudaGetLastError());
+    ctx->launches += 1;
+  }
 
-  // ---- 5. transformToEnd of the new less-* clouds + the guarded map swap --------------------------------------------
+  // ---- 5. transformToEnd of the new less-* clouds + the guarded map swap (a first scan's clouds stay as they are) ------
   unsigned char* run_mask = q.status_d.p + n;
-  for (int s = 0; s < n; ++s) q.h_status.p[n + s] = status[s] >= LINS_SEQ_RAN ? 1 : 0;
+  for (int s = 0; s < n; ++s)
+    q.h_status.p[n + s] = status[s] == LINS_SEQ_RAN || status[s] == LINS_SEQ_ICP || status[s] == LINS_SEQ_SECOND ? 1 : 0;
   CK(cudaMemcpyAsync(run_mask, q.h_status.p + n, n, cudaMemcpyHostToDevice, ctx->stream));
   rc = transform_to_end_csr(ctx, q.up.ts.p, q.up.ts_off.p, n, q.lin.p, run_mask);
   if (rc == LINS_OK) rc = transform_to_end_csr(ctx, q.up.tc.p, q.up.tc_off.p, n, q.lin.p, run_mask);
@@ -390,6 +635,11 @@ static int seq_step_run(lins_ctx* ctx, const lins_seq_step_desc* d, const int32_
   CK(cudaMemcpyAsync(q.stale.p, q.h_stale_v.data(), n, cudaMemcpyHostToDevice, ctx->stream));
   CK(cudaEventRecord(q.ev[4], ctx->stream));
   CK(cudaStreamSynchronize(ctx->stream));  // (the two sources above are pageable and change with the next step)
+  for (int s = 0; s < n; ++s) {  // processPCL's status transitions (:294-307)
+    if (status[s] == LINS_SEQ_INIT_WAIT) q.fusion[s] = FUSION_INIT;
+    else if (status[s] == LINS_SEQ_FIRST) q.fusion[s] = FUSION_FIRST_SCAN;
+    else if (status[s] == LINS_SEQ_SECOND) q.fusion[s] = FUSION_RUNNING;
+  }
   q.ev_valid = true;
   q.has_step = true;
   q.h_run_off.swap(run_off);
@@ -429,6 +679,35 @@ int lins_gpu_seq_download(lins_ctx* ctx, double* global_state, double* filter_st
     if (filter_state) std::memcpy(filter_state + s * 19, &f[s * 20], sizeof(double) * 19);
   }
   if (scan_status) std::memcpy(scan_status, q.status.data(), sizeof(int32_t) * n);
+  return LINS_OK;
+}
+
+int lins_gpu_seq_download_init(lins_ctx* ctx, int32_t* fusion_status, double* icp_pose, int32_t* icp_iters, int32_t* icp_converged) {
+  if (!ctx) return LINS_E_INVALID;
+  SeqState& q = ctx->seq;
+  if (q.n == 0) return fail(ctx, LINS_E_NOMAP, "lins_gpu_seq_begin has not been called");
+  const size_t n = q.n;
+  if (fusion_status) std::memcpy(fusion_status, q.fusion.data(), sizeof(int32_t) * n);
+  if (!icp_pose && !icp_iters && !icp_converged) return LINS_OK;
+  if (icp_pose) std::memset(icp_pose, 0, sizeof(double) * 7 * n);
+  if (icp_iters) std::memset(icp_iters, 0, sizeof(int32_t) * n);
+  if (icp_converged) std::memset(icp_converged, 0, sizeof(int32_t) * n);
+  bool any = false;
+  for (size_t s = 0; s < n; ++s) any |= q.status[s] == LINS_SEQ_SECOND;
+  if (!any) return LINS_OK;
+  CK(cudaSetDevice(ctx->device));
+  std::vector<double> pose(n * 20);
+  std::vector<lins_dev::IcpState> st(n);
+  CK(cudaMemcpyAsync(pose.data(), q.icp_pose.p, sizeof(double) * 20 * n, cudaMemcpyDeviceToHost, ctx->stream));
+  CK(cudaMemcpyAsync(st.data(), q.init_icp.p, sizeof(lins_dev::IcpState) * n, cudaMemcpyDeviceToHost, ctx->stream));
+  CK(cudaStreamSynchronize(ctx->stream));
+  for (size_t s = 0; s < n; ++s) {
+    if (q.status[s] != LINS_SEQ_SECOND) continue;
+    const double* p = &pose[s * 20];
+    if (icp_pose) { double* o = icp_pose + s * 7; o[0] = p[0]; o[1] = p[1]; o[2] = p[2]; o[3] = p[6]; o[4] = p[7]; o[5] = p[8]; o[6] = p[9]; }
+    if (icp_iters) icp_iters[s] = st[s].iters;
+    if (icp_converged) icp_converged[s] = st[s].converged;
+  }
   return LINS_OK;
 }
 

@@ -251,4 +251,110 @@ LSQ_HD void correct_roll_pitch(double* g, const double* fs) {
   stq(g, rpy2Quat(v3(roll, pitch, rpy.d[2])));
 }
 
+// ---- sequence initialisation: processFirstScan / processSecondScan (state_estimator.hpp:186-220) ---------------------
+// The constants they read.  var = the diagonal initializeCovariance installs (kalman_filter.hpp:197-209), in error-state
+// order: sq(init_pos_std), sq(init_vel_std), pow(deg2rad(init_att_std), 2), sq(init_acc_std), sq(init_gyr_std), 0.01 —
+// computed on the host once, like Consts; ba / bw = init_ba / init_bw.
+struct InitConsts {
+  double var[18];
+  double ba[3], bw[3];
+};
+
+// The pre-integration between the first and the second scan (state_estimator.hpp:41-62): 20 doubles per sequence,
+// acc_0[0..2] gyr_0[3..5] delta_p[6..8] delta_v[9..11] delta_q(x,y,z,w)[12..15] sum_dt[16]; linearized_ba / bg are init_ba /
+// init_bw.
+constexpr int pAcc = 0, pGyr = 3, pDp = 6, pDv = 9, pDq = 12, pSum = 16;
+LSQ_HD Q4 ldq_at(const double* s, int o) { return q4(s[o + 3], s[o], s[o + 1], s[o + 2]); }
+LSQ_HD void stq_at(double* s, int o, Q4 q) { s[o] = q.x; s[o + 1] = q.y; s[o + 2] = q.z; s[o + 3] = q.w; }
+
+// IntegrationBase(acc0, gyr0, ba, bg): delta_p = delta_v = 0, delta_q = identity, sum_dt = 0
+LSQ_HD void preint_begin(double* pre, const double* imu) {
+  for (int i = 0; i < 20; ++i) pre[i] = 0.0;
+  for (int i = 0; i < 3; ++i) { pre[pAcc + i] = imu[i]; pre[pGyr + i] = imu[3 + i]; }
+  stq_at(pre, pDq, qident());
+}
+// IntegrationBase::propagate
+LSQ_HD void preint_propagate(double* pre, const InitConsts& k, double dt, const double* acc, const double* gyr) {
+  const V3 ba = ld3(k.ba, 0), bg = ld3(k.bw, 0), a0 = ld3(pre, pAcc), g0 = ld3(pre, pGyr), a1 = ld3(acc, 0), g1 = ld3(gyr, 0);
+  const V3 dp = ld3(pre, pDp), dv = ld3(pre, pDv);
+  const Q4 dq = ldq_at(pre, pDq);
+  const V3 un_acc_0 = qrot(dq, vsub(a0, ba));
+  const V3 un_gyr = vsub(vscl(0.5, vadd(g0, g1)), bg);
+  const Q4 rq = qmul(dq, q4(1.0, un_gyr.d[0] * dt / 2, un_gyr.d[1] * dt / 2, un_gyr.d[2] * dt / 2));
+  const V3 un_acc_1 = qrot(rq, vsub(a1, ba));
+  const V3 un_acc = vscl(0.5, vadd(un_acc_0, un_acc_1));
+  st3(pre, pDp, vadd(vadd(dp, vscl(dt, dv)), vscl(0.5 * dt * dt, un_acc)));
+  st3(pre, pDv, vadd(dv, vscl(dt, un_acc)));
+  stq_at(pre, pDq, qnormalized(rq));
+  pre[pSum] += dt;
+  st3(pre, pAcc, a1);
+  st3(pre, pGyr, g1);
+}
+
+// GlobalState::setIdentity (19 doubles + the device's pad)
+LSQ_HD void state_identity(double* s) {
+  for (int i = 0; i < 20; ++i) s[i] = 0.0;
+  stq(s, qident());
+  s[sGn + 2] = -kG0;
+}
+// GlobalState(rn, vn, qbn, ba, bw)
+LSQ_HD void state_set(double* s, V3 rn, V3 vn, Q4 q, V3 ba, V3 bw) {
+  state_identity(s);
+  st3(s, sRn, rn); st3(s, sVn, vn); stq(s, q); st3(s, sBa, ba); st3(s, sBw, bw);
+}
+// StatePredictor::initializeCovariance (P column-major; only the diagonal is non-zero)
+LSQ_HD void initialize_covariance(double* P, const InitConsts& k) {
+  for (int e = 0; e < 324; ++e) P[e] = 0.0;
+  for (int i = 0; i < 18; ++i) P[i * 18 + i] = k.var[i];
+}
+
+// What a newly constructed StateEstimator holds: globalState_ and the filter state identity, initializeCovariance
+LSQ_HD void fresh_slot(double* glob, double* filt, double* P, const InitConsts& k) {
+  state_identity(glob);
+  state_identity(filt);
+  initialize_covariance(P, k);
+}
+
+// processFirstScan once its gate has passed: linState_ identity, a new pre-integration from the scan's IMU sample, and
+// filter_->initialization(time, 0, 0, 0, 0, acc, gyr).  imu: acc (3) + gyr (3) of the scan; imu_last: acc_last / gyr_last.
+LSQ_HD void first_scan(double* filt, double* P, double* lin, double* pre, double* imu_last, const double* imu, const InitConsts& k) {
+  const V3 z = v3(0.0, 0.0, 0.0);
+  state_identity(lin);
+  preint_begin(pre, imu);
+  state_set(filt, z, z, rpy2Quat(v3(0.0, 0.0, 0.0)), z, z);
+  for (int i = 0; i < 6; ++i) imu_last[i] = imu[i];
+  initialize_covariance(P, k);
+}
+
+// processSecondScan, before estimateTransform: the ICP's start pose pl = delta_p + 0.5 sum_dt^2 gn (linState_.gn_ is
+// the identity's), ql = delta_q, as the 20-double pose block the ICP linearises at (t at 0..2, q at 6..9, the rest 0)
+LSQ_HD void second_scan_start(const double* pre, double* pose) {
+  const double sum_dt = pre[pSum];
+  const V3 gn = v3(0.0, 0.0, -kG0);
+  for (int i = 0; i < 20; ++i) pose[i] = 0.0;
+  st3(pose, sRn, vadd(ld3(pre, pDp), vscl(0.5 * sum_dt * sum_dt, gn)));
+  stq(pose, ldq_at(pre, pDq));
+}
+
+// processSecondScan after estimateTransform (pose: its result): linState_ = (t, q) over the identity,
+// estimateInitialState (v = p / sum_dt: no guard, like the reference), filter_->initialization(time, pl, v1, ba0, bw0, acc,
+// gyr), calculateRPfromGravity(acc - ba0) and the hand-over to globalState_.
+LSQ_HD void second_scan(double* glob, double* filt, double* P, double* lin, double* imu_last, const double* pre, const double* pose,
+                        const double* imu, const InitConsts& k) {
+  const V3 pl = ld3(pose, sRn);
+  const Q4 ql = ldq(pose);
+  state_identity(lin);
+  st3(lin, sRn, pl);
+  stq(lin, ql);
+  const V3 v1 = vdiv(pl, pre[pSum]);
+  const V3 ba0 = ld3(k.ba, 0), bw0 = ld3(k.bw, 0);
+  state_set(filt, pl, v1, rpy2Quat(v3(0.0, 0.0, 0.0)), ba0, bw0);
+  for (int i = 0; i < 6; ++i) imu_last[i] = imu[i];
+  initialize_covariance(P, k);
+  const V3 f = vsub(ld3(imu, 0), ba0);
+  const double pitch = -sign(f.d[2]) * asin(f.d[0] / kG0);
+  const double roll = sign(f.d[2]) * asin(f.d[1] / kG0);
+  state_set(glob, pl, v1, rpy2Quat(v3(roll, pitch, 0.0)), ba0, bw0);
+}
+
 }  // namespace lins_seq

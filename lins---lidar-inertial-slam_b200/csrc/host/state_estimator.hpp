@@ -268,6 +268,7 @@ class StateEstimator {
     t = V3D(pose[0], pose[1], pose[2]);
     q = Q4D(pose[6], pose[3], pose[4], pose[5]);
     linState_.rn_ = t; linState_.qbn_ = q;
+    last_icp_iters_ = iters; last_icp_converged_ = conv;
   }
 
   // StateEstimator.hpp:602-605
@@ -324,6 +325,7 @@ class StateEstimator {
   sensor_utils::Imu imu_last_;
   lins_report last_report_;
   bool last_map_replaced_ = false;  // the last updatePointCloud rebuilt the 1-NN index (:1156-1157)
+  int last_icp_iters_ = 0, last_icp_converged_ = 0;  // the last estimateTransform's iterations and converged flag
 
  private:
   FeatureExtractor extractor_;

@@ -112,6 +112,23 @@ class LinsSeqParams(C.Structure):
         return p
 
 
+class LinsSeqInitParams(C.Structure):
+    """lins_seq_init_params (include/lins_gpu.h): the filter constants sequence initialisation reads."""
+    _fields_ = [("init_vel_std", C.c_double * 3), ("init_acc_std", C.c_double * 3), ("init_gyr_std", C.c_double * 3),
+                ("init_ba", C.c_double * 3), ("init_bw", C.c_double * 3)]
+
+    @classmethod
+    def shipped(cls, init_vel_std=(0.0, 0.0, 0.0), init_acc_std=(0.01, 0.01, 0.02), init_gyr_std=(0.002, 0.002, 0.002),
+                init_ba=(-0.015774, 0.143237, -0.0263845), init_bw=(-0.00275058, -0.000165954, 0.00262913)):
+        """csrc/host/kalman_filter.hpp FilterParams defaults (exp_port.yaml:29-62)."""
+        p = cls()
+        for name, v in (("init_vel_std", init_vel_std), ("init_acc_std", init_acc_std), ("init_gyr_std", init_gyr_std),
+                        ("init_ba", init_ba), ("init_bw", init_bw)):
+            for i in range(3):
+                getattr(p, name)[i] = v[i]
+        return p
+
+
 class LinsSeqBeginDesc(C.Structure):
     _fields_ = [
         ("n_seq", C.c_int32),
@@ -146,6 +163,8 @@ class LinsSeqStepDesc(C.Structure):
 
 
 SEQ_IDLE, SEQ_SKIPPED, SEQ_RAN, SEQ_ICP = 0, 1, 2, 3  # lins_gpu_seq_download scan_status (LINS_SEQ_*)
+SEQ_INIT_WAIT, SEQ_FIRST, SEQ_SECOND = 4, 5, 6        # ... of a slot that initialises (lins_gpu_seq_open runs)
+FUSION_INIT, FUSION_FIRST_SCAN, FUSION_RUNNING = 0, 1, 3  # lins_gpu_seq_download_init fusion_status (StateEstimator::status_)
 
 
 def ptr(a):

@@ -265,7 +265,9 @@ def replay_feature_log(log, device=0, params=None, init_std=None):
     """Replay a feature log through one C++ StateEstimator shim (processImu + processFeatures per scan).  Returns per scan
     code (LINS_SEQ_*: 0 before the hand-over), iters, flags, map_replaced, est_status, global_state / filter_state /
     lin_state (n x 19) and filter_cov (n x 324) after the scan, plus `handover`: the scan index after which the shim first
-    ran and its state then, as lins_gpu_seq_begin takes it.  params: the shim context's LinsParams (None = shipped);
+    ran and its state then, as lins_gpu_seq_begin takes it.  init_code: the code an opened sequence-mode slot gets for
+    the scan (LINS_SEQ_INIT_WAIT / FIRST / SECOND while initialising, else code); icp_pose (n x 7: t, q xyzw), icp_iters,
+    icp_converged: the second scan's estimateTransform result where init_code is LINS_SEQ_SECOND, else zero.  params: the shim context's LinsParams (None = shipped);
     init_std: INIT_POS_STD (3) + INIT_ATT_STD (3, degrees) of its filter (None = zero).  scan_s: wall seconds per scan."""
     L = _flog_lib()
     n = len(log["time"])
@@ -285,7 +287,8 @@ def replay_feature_log(log, device=0, params=None, init_std=None):
         dbl = lambda w, cnt: np.ctypeslib.as_array(L.lins_replay_doubles(h, w), shape=(cnt,)).copy()  # noqa: E731
         rec = dict(code=ints(0), iters=ints(1), flags=ints(2), map_replaced=ints(3), est_status=ints(4),
                    global_state=dbl(0, n * 19).reshape(n, 19), filter_state=dbl(1, n * 19).reshape(n, 19),
-                   filter_cov=dbl(2, n * 324).reshape(n, 324), lin_state=dbl(3, n * 19).reshape(n, 19), scan_s=dbl(8, n))
+                   filter_cov=dbl(2, n * 324).reshape(n, 324), lin_state=dbl(3, n * 19).reshape(n, 19), scan_s=dbl(8, n),
+                   init_code=ints(5), icp_pose=dbl(9, n * 7).reshape(n, 7), icp_iters=ints(6), icp_converged=ints(7))
         k = L.lins_replay_handover(h)
         rec["handover_index"] = k
         if k >= 0:

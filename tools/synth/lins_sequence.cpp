@@ -310,6 +310,10 @@ struct ReplayRecord {
   std::vector<int32_t> code, iters, flags, replaced, est_status;  // code: LINS_SEQ_* (0 before the hand-over)
   std::vector<double> glob, filt, cov, lin;  // n x 19, n x 19, n x 324, n x 19 after each scan
   std::vector<double> scan_s;                // wall time of each scan's processImu calls + processFeatures
+  // sequence initialisation: init_code = the code lins_gpu_seq_step_ex gives an opened slot (LINS_SEQ_INIT_WAIT / FIRST /
+  // SECOND while initialising, else `code`); where it is LINS_SEQ_SECOND, the scan's estimateTransform result
+  std::vector<int32_t> init_code, icp_iters, icp_converged;
+  std::vector<double> icp_pose;              // n x 7: t (3) + q (x,y,z,w)
   double h_filt[19], h_glob[19], h_imu[6], h_cov[324];
   std::vector<lins_point> h_surf, h_corner;
 };
@@ -366,6 +370,7 @@ void* lins_flog_replay(const lins_feature_log_desc* d, int lidar_model, int devi
     Cloud* cl[4] = {&f.surfPointsFlat, &f.cornerPointsSharp, &f.surfPointsLessFlat, &f.cornerPointsLessSharp};
     for (int j = 0; j < 4; ++j) cl[j]->points.assign(d->clouds[j] + d->offs[j][k], d->clouds[j] + d->offs[j][k + 1]);
     const bool running = est.status_ == StateEstimator::STATUS_RUNNING;
+    const StateEstimator::FusionStatus before = est.status_;
     est.last_report_ = lins_report();
     const double* il = d->imu_last + (size_t)k * 6;
     est.processFeatures(d->time[k], lins::sensor_utils::Imu(d->time[k], V3D(il[0], il[1], il[2]), V3D(il[3], il[4], il[5])), f);
@@ -376,6 +381,19 @@ void* lins_flog_replay(const lins_feature_log_desc* d, int lidar_model, int devi
       code = gate ? LINS_SEQ_SKIPPED : est.last_report_.diverged ? LINS_SEQ_ICP : LINS_SEQ_RAN;
     }
     R->code.push_back(code);
+    int icode = code;
+    if (before == StateEstimator::STATUS_INIT) icode = est.status_ == StateEstimator::STATUS_FIRST_SCAN ? LINS_SEQ_FIRST : LINS_SEQ_INIT_WAIT;
+    else if (before == StateEstimator::STATUS_FIRST_SCAN) icode = est.status_ == StateEstimator::STATUS_RUNNING ? LINS_SEQ_SECOND : LINS_SEQ_INIT_WAIT;
+    R->init_code.push_back(icode);
+    double ip[7] = {0, 0, 0, 0, 0, 0, 0};
+    if (icode == LINS_SEQ_SECOND) {
+      const double v[7] = {est.linState_.rn_.x(), est.linState_.rn_.y(), est.linState_.rn_.z(), est.linState_.qbn_.x(),
+                           est.linState_.qbn_.y(), est.linState_.qbn_.z(), est.linState_.qbn_.w()};
+      std::memcpy(ip, v, sizeof(v));
+    }
+    R->icp_pose.insert(R->icp_pose.end(), ip, ip + 7);
+    R->icp_iters.push_back(icode == LINS_SEQ_SECOND ? est.last_icp_iters_ : 0);
+    R->icp_converged.push_back(icode == LINS_SEQ_SECOND ? est.last_icp_converged_ : 0);
     R->iters.push_back(est.last_report_.iters);
     R->flags.push_back((est.last_report_.converged ? 1 : 0) | (est.last_report_.diverged ? 2 : 0) | (est.last_report_.has_nan ? 4 : 0));
     R->replaced.push_back(code >= LINS_SEQ_RAN && est.last_map_replaced_ ? 1 : 0);
@@ -433,8 +451,8 @@ void lins_replay_destroy(void* h) { delete static_cast<ReplayRecord*>(h); }
 int lins_replay_handover(void* h) { return static_cast<ReplayRecord*>(h)->handover; }
 const int32_t* lins_replay_ints(void* h, int which) {
   ReplayRecord* R = static_cast<ReplayRecord*>(h);
-  const std::vector<int32_t>* v[5] = {&R->code, &R->iters, &R->flags, &R->replaced, &R->est_status};
-  return which >= 0 && which < 5 ? v[which]->data() : nullptr;
+  const std::vector<int32_t>* v[8] = {&R->code, &R->iters, &R->flags, &R->replaced, &R->est_status, &R->init_code, &R->icp_iters, &R->icp_converged};
+  return which >= 0 && which < 8 ? v[which]->data() : nullptr;
 }
 const double* lins_replay_doubles(void* h, int which) {
   ReplayRecord* R = static_cast<ReplayRecord*>(h);
@@ -448,6 +466,7 @@ const double* lins_replay_doubles(void* h, int which) {
     case 6: return R->h_cov;
     case 7: return R->h_imu;
     case 8: return R->scan_s.data();
+    case 9: return R->icp_pose.data();
   }
   return nullptr;
 }

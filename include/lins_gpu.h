@@ -311,6 +311,69 @@ int lins_gpu_seq_download_ieskf(lins_ctx* ctx, double* prior_state /*S x 19*/, d
 int lins_gpu_seq_download_maps(lins_ctx* ctx, int32_t* off, float* surf_map, float* corner_map, float* surf_tree,
                                float* corner_tree, uint8_t* stale /*S*/);
 
+/* ---- feature extraction: StateEstimator.hpp:619-827 (undistortPcl, calculateSmoothness, markOccludedPoints,
+   extractFeatures with the per-ring pcl::VoxelGrid, leaf 0.2 m) on the device, from what processPCL receives: the
+   segmented cloud and cloud_info of image projection (cloud_msgs/msg/cloud_info.msg).  Bit-identical to the host
+   restatement csrc/host/feature_extraction.hpp except where equal curvatures decide a pick: the reference's std::sort
+   leaves their order unspecified; the device keeps them in array order (DESIGN.md §4.6). */
+
+/* n segmented scans, CSR: scan i's points are cloud[cloud_off[i] .. cloud_off[i + 1]) and its per-point cloud_info
+   arrays share those offsets */
+typedef struct lins_pcl_desc {
+  int32_t n_scans;
+  int32_t line_num;                    /* LINE_NUM, 1..128: the entries of start/end_ring_index per scan */
+  const lins_point* cloud; const int32_t* cloud_off;  /* segmentedCloud; n_scans + 1 offsets */
+  const uint8_t* ground_flag;          /* segmentedCloudGroundFlag */
+  const uint32_t* col_ind;             /* segmentedCloudColInd */
+  const float* range;                  /* segmentedCloudRange */
+  const int32_t* start_ring_index;     /* n_scans x line_num: startRingIndex */
+  const int32_t* end_ring_index;       /* n_scans x line_num: endRingIndex */
+  const float* orientation;            /* n_scans x 3: startOrientation, endOrientation, orientationDiff */
+  int32_t point_format;                /* LINS_POINTS_XYZI32 or LINS_POINTS_PACKED16, as in lins_batch_desc */
+} lins_pcl_desc;
+
+/* the extraction's constants (exp_port.yaml:7, :12-13; shipped 0.5 / 0.5 / 0); SCAN_PERIOD is lins_params.scan_period */
+typedef struct lins_feature_params {
+  double edge_threshold;
+  double surf_threshold;
+  double imu_lidar_extrinsic_angle;    /* degrees */
+} lins_feature_params;
+
+/* the largest ring span (endRingIndex - startRingIndex) of a ring with a visited sextant that the on-chip sorts take;
+   a scan with a longer ring returns LINS_E_TOOBIG (VLP-16 rings hold at most 1800 points, 64 x 1024 rings 1024) */
+#define LINS_FEAT_RING_CAP 2048
+
+/* ≙ the four extraction stages of processPCL (StateEstimator.hpp:619-827) for every scan of d.  Scan i's clouds are
+   written at its own input offsets (none is larger than the input): surf_flat (surfPointsFlat), corner_sharp
+   (cornerPointsSharp), surf_less_flat (surfPointsLessFlat), corner_less_sharp (cornerPointsLessSharp) and, unless
+   undist is NULL, the de-skewed cloud (intensity = ring + SCAN_PERIOD * relTime), all in d->point_format (XYZI32
+   records carry pad0 = 1 and zero pads).  counts: n_scans x 4 in that order.  LINS_E_INVALID, before anything is
+   written, for bad offsets, a NULL array, line_num outside 1..128, a non-finite point, range or orientation, or a
+   visited sextant (sp < ep) outside the scan's [0, n), or rings whose visited ranges overlap or come out of order (LeGO-LOAM's
+   rings are 10 points apart; abutting rings are fine); LINS_E_TOOBIG for a ring span above LINS_FEAT_RING_CAP. */
+int lins_gpu_extract_features(lins_ctx* ctx, const lins_feature_params* fp, const lins_pcl_desc* d, lins_point* surf_flat,
+                              lins_point* corner_sharp, lins_point* surf_less_flat, lins_point* corner_less_sharp,
+                              lins_point* undist, int32_t* counts /*n_scans x 4*/);
+/* CUDA-event time of the last extraction kernel (lins_gpu_extract_features or lins_gpu_seq_step_pcl), ms */
+int lins_gpu_extract_ms(lins_ctx* ctx, float* ms);
+
+/* one processPCL-shaped scan per sequence: the IMU rows as in lins_seq_step_desc, the scans as a lins_pcl_desc with
+   n_scans == n_seq (a slot that is not present should have an empty scan; its features are not used) */
+typedef struct lins_seq_pcl_desc {
+  int32_t n_seq;
+  const uint8_t* present;              /* NULL = all */
+  const double* imu; const int32_t* imu_off;
+  lins_pcl_desc pcl;
+} lins_seq_pcl_desc;
+
+/* ≙ processPCL (StateEstimator.hpp:279-307) with its feature extraction (:619-827) on the device: extracts every
+   slot's scan, reads the counts back (one D2H + synchronisation: the gates and the map plan are made from sizes), packs
+   the features into the step's buffers and runs lins_gpu_seq_step_ex.  Bit-identical to lins_gpu_extract_features
+   followed by lins_gpu_seq_step_ex with those clouds; may alternate with lins_gpu_seq_step_ex in one run.  Invalid
+   input (as lins_gpu_extract_features, or as lins_gpu_seq_step_ex) returns before the sequences change. */
+int lins_gpu_seq_step_pcl(lins_ctx* ctx, const lins_seq_pcl_desc* step, const lins_feature_params* fp,
+                          const double* scan_imu /*S x 6 or NULL*/);
+
 /* Split "Jacobian kernel" (SURVEY.md §8(d) unit U1): residual + Jacobian row + 29-scalar reduction over the
    resident batch given the correspondence IDs of iteration `iter` of each scan's current linearisation
    point. Used for the HBM-roofline measurement; results land in an internal n x 29 accumulator array. */

@@ -13,8 +13,9 @@ import subprocess
 
 import numpy as np
 
-from .ctypes_defs import (Batch, COV_SIZE, LinsBatchDesc, LinsMapReport, LinsParams, LinsReport, LinsScanResult, LinsSeqBeginDesc,
-                          LinsSeqInitParams, LinsSeqParams, LinsSeqStepDesc, POINT_DTYPE, SCAN_RESULT_DTYPE, STATE_DIM, as_points, ptr)
+from .ctypes_defs import (Batch, COV_SIZE, LinsBatchDesc, LinsFeatureParams, LinsMapReport, LinsParams, LinsPclDesc, LinsReport,
+                          LinsScanResult, LinsSeqBeginDesc, LinsSeqInitParams, LinsSeqParams, LinsSeqPclDesc, LinsSeqStepDesc, POINT_DTYPE,
+                          SCAN_RESULT_DTYPE, STATE_DIM, as_points, ptr)
 
 _PKG = os.path.dirname(os.path.abspath(__file__))
 _ROOT = os.path.dirname(_PKG)
@@ -32,15 +33,16 @@ EXPORTS = [
     "lins_gpu_batch_upload_stats", "lins_gpu_seq_begin", "lins_gpu_seq_step", "lins_gpu_seq_download",
     "lins_gpu_seq_phase_ms", "lins_gpu_seq_download_ieskf", "lins_gpu_seq_download_maps", "lins_gpu_download_indices",
     "lins_gpu_seq_open", "lins_gpu_seq_restart", "lins_gpu_seq_step_ex", "lins_gpu_seq_download_init",
+    "lins_gpu_extract_features", "lins_gpu_extract_ms", "lins_gpu_seq_step_pcl",
 ]
 
 NVCC_ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]  # H100 (Hopper)
 NVCC_COMMON = NVCC_ARCH + ["-lineinfo", "-O3", "-std=c++17", "-Xcompiler", "-fPIC"]
 # translation units and their extra flags: lins_gpu.cu (the fused kernel and most of the C-ABI), lins_upload.cu (batch
-# upload), lins_map.cu (row F2's host side), lins_seq.cu (sequence mode) — all bit-exact, so no multiply-add contraction: the association and the map
+# upload), lins_map.cu (row F2's host side), lins_seq.cu (sequence mode), lins_features.cu (feature extraction) — all bit-exact, so no multiply-add contraction: the association and the map
 # fits depend on it — and lins_jacobian.cu (the tolerance-checked split Jacobian kernel: contraction allowed)
 UNITS = [("lins_gpu.cu", ["-fmad=false"]), ("lins_upload.cu", ["-fmad=false"]), ("lins_map.cu", ["-fmad=false"]),
-         ("lins_seq.cu", ["-fmad=false"]), ("lins_jacobian.cu", [])]
+         ("lins_seq.cu", ["-fmad=false"]), ("lins_features.cu", ["-fmad=false"]), ("lins_jacobian.cu", [])]
 NVCC_FLAGS = NVCC_COMMON + ["-fmad=false", "-shared"]  # (what tools/ scripts print)
 
 
@@ -118,12 +120,25 @@ def lib():
             L.lins_gpu_seq_restart.argtypes = [vp, vp]
             L.lins_gpu_seq_step_ex.argtypes = [vp, C.POINTER(LinsSeqStepDesc), vp]
             L.lins_gpu_seq_download_init.argtypes = [vp, vp, vp, vp, vp]
+        if hasattr(L, "lins_gpu_extract_features"):
+            L.lins_gpu_extract_features.argtypes = [vp, C.POINTER(LinsFeatureParams), C.POINTER(LinsPclDesc)] + [vp] * 6
+            L.lins_gpu_extract_ms.argtypes = [vp, vp]
+            L.lins_gpu_seq_step_pcl.argtypes = [vp, C.POINTER(LinsSeqPclDesc), C.POINTER(LinsFeatureParams), vp]
         _LIB = L
     return _LIB
 
 
 class LinsError(RuntimeError):
     pass
+
+
+def _points_from_xyzi(a):
+    """POINT_DTYPE records of an (m x 4) float32 (x, y, z, intensity) array (pad0 = 1, as pcl's PointXYZI)."""
+    a = np.asarray(a, np.float32).reshape(-1, 4)
+    out = np.zeros(len(a), POINT_DTYPE)
+    out["x"], out["y"], out["z"], out["intensity"] = a[:, 0], a[:, 1], a[:, 2], a[:, 3]
+    out["pad0"] = 1.0
+    return out
 
 
 def pin_batch(batch):
@@ -396,6 +411,76 @@ class LinsGpu:
             if len(si) != d.n_seq:
                 raise ValueError(f"scan_imu has {len(si)} rows, the step {d.n_seq}")
             self._ck(self.L.lins_gpu_seq_step_ex(self.h, C.byref(d), ptr(si)))
+
+    @staticmethod
+    def _pcl_desc(scans, line_num, keep):
+        """LinsPclDesc of a list of segmented scans (dicts: seg (m x 4 float32 x, y, z, intensity, or POINT_DTYPE), ground,
+        col, range, start_ring, end_ring, ori (3)); the arrays it points at are added to `keep`."""
+        n = len(scans)
+        segs = [as_points(s["seg"]) if np.asarray(s["seg"]).dtype == POINT_DTYPE else _points_from_xyzi(s["seg"]) for s in scans]
+        off = np.zeros(n + 1, np.int32)
+        off[1:] = np.cumsum([len(a) for a in segs])
+        cat = lambda k, t: np.ascontiguousarray(np.concatenate([np.asarray(s[k], t).reshape(-1) for s in scans]) if n else np.zeros(0, t))  # noqa: E731
+        keep.update(cloud=np.ascontiguousarray(np.concatenate(segs)) if n else np.zeros(0, POINT_DTYPE), cloud_off=off,
+                    ground_flag=cat("ground", np.uint8), col_ind=cat("col", np.uint32), range=cat("range", np.float32),
+                    start_ring_index=cat("start_ring", np.int32), end_ring_index=cat("end_ring", np.int32), orientation=cat("ori", np.float32))
+        for k in ("start_ring_index", "end_ring_index"):
+            if len(keep[k]) != n * line_num:
+                raise ValueError(f"{k}: {len(keep[k])} entries for {n} scans of {line_num} rings")
+        d = LinsPclDesc()
+        d.n_scans, d.line_num, d.point_format = n, int(line_num), 0
+        for k in ("cloud", "cloud_off", "ground_flag", "col_ind", "range", "start_ring_index", "end_ring_index", "orientation"):
+            setattr(d, k, keep[k].ctypes.data)
+        return d
+
+    def extract_features(self, scans, line_num=16, params=None, undist=False):
+        """Feature extraction of segmented scans on the device (lins_gpu_extract_features).  Returns one dict per scan with
+        surf_flat, corner_sharp, surf_less_flat, corner_less_sharp (and undist when asked for) as (k x 4) float32
+        (x, y, z, intensity) arrays."""
+        keep = {}
+        d = self._pcl_desc(scans, line_num, keep)
+        n, total = d.n_scans, int(keep["cloud_off"][-1])
+        outs = [np.zeros(max(total, 1), POINT_DTYPE) for _ in range(5)]
+        counts = np.zeros((max(n, 1), 4), np.int32)
+        fp = params or LinsFeatureParams.shipped()
+        self._ck(self.L.lins_gpu_extract_features(self.h, C.byref(fp), C.byref(d), *[ptr(o) for o in outs[:4]],
+                                                  ptr(outs[4]) if undist else None, ptr(counts)))
+        x4 = lambda a: np.stack([a["x"], a["y"], a["z"], a["intensity"]], 1).astype(np.float32)  # noqa: E731
+        names = ("surf_flat", "corner_sharp", "surf_less_flat", "corner_less_sharp")
+        res = []
+        off = keep["cloud_off"]
+        for i in range(n):
+            r = {k: x4(outs[c][off[i]: off[i] + counts[i, c]]) for c, k in enumerate(names)}
+            if undist:
+                r["undist"] = x4(outs[4][off[i]: off[i + 1]])
+            res.append(r)
+        return res
+
+    def extract_ms(self):
+        """CUDA-event time (ms) of the last extraction kernel."""
+        ms = np.zeros(1, np.float32)
+        self._ck(self.L.lins_gpu_extract_ms(self.h, ptr(ms)))
+        return float(ms[0])
+
+    def seq_step_pcl(self, step, fp=None, scan_imu=None, line_num=16):
+        """Advance every present sequence by one processPCL-shaped scan (lins_gpu_seq_step_pcl): `step` has imu + imu_off as
+        in seq_step, scans (one segmented scan per slot, as extract_features takes them; an absent slot's may be empty) and
+        optionally present."""
+        keep = {"imu": np.ascontiguousarray(step["imu"], dtype=np.float64), "imu_off": np.ascontiguousarray(step["imu_off"], dtype=np.int32)}
+        d = LinsSeqPclDesc()
+        d.pcl = self._pcl_desc(step["scans"], line_num, keep)
+        d.n_seq = len(keep["imu_off"]) - 1
+        d.imu, d.imu_off = keep["imu"].ctypes.data, keep["imu_off"].ctypes.data
+        if step.get("present") is not None:
+            keep["present"] = np.ascontiguousarray(step["present"], dtype=np.uint8)
+            d.present = keep["present"].ctypes.data
+        fp = fp or LinsFeatureParams.shipped()
+        si = None
+        if scan_imu is not None:
+            si = np.ascontiguousarray(scan_imu, dtype=np.float64).reshape(-1, 6)
+            if len(si) != d.n_seq:
+                raise ValueError(f"scan_imu has {len(si)} rows, the step {d.n_seq}")
+        self._ck(self.L.lins_gpu_seq_step_pcl(self.h, C.byref(d), C.byref(fp), ptr(si)))
 
     def seq_download(self, reports=False):
         """dict: global_state, filter_state (S x 19), filter_cov (S x 324), results (SCAN_RESULT_DTYPE), status (S) and,

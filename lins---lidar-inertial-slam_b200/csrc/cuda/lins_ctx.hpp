@@ -124,6 +124,25 @@ struct SeqState {
   ~SeqState() { for (cudaEvent_t e : ev) if (e) cudaEventDestroy(e); }
 };
 
+// Feature extraction (lins_features.cu): the uploaded segmented scans (cloud in up.qs, CSR in up.qs_off) with their
+// cloud_info, the extracted clouds at the input offsets, per-point scratch, and the counts read back (n x 5: the four
+// counts in lins_seq_step_desc order, then the scan's status)
+struct FeatState {
+  Resident up;
+  Buf<unsigned char> ground, picked, label;
+  Buf<unsigned> col;
+  Buf<float> range, ori;
+  Buf<int> ring, counts, sind;
+  Buf<double> curv;
+  Buf<float4> und, out[4];
+  Buf<int, kPinned> h_counts;
+  std::vector<int32_t> h_ring;
+  Buf<SeqCopy> copies; Buf<SeqCopy, kPinned> h_copies;  // the pack into sequence mode's feature buffers
+  cudaEvent_t ev[2] = {nullptr, nullptr};               // around the last extraction kernel (lins_gpu_extract_ms)
+  bool ev_valid = false;
+  ~FeatState() { for (cudaEvent_t e : ev) if (e) cudaEventDestroy(e); }
+};
+
 }  // namespace lins_capi
 
 struct lins_ctx {
@@ -144,6 +163,7 @@ struct lins_ctx {
   lins_capi::Resident batch;   // lins_gpu_batch_* working set
   lins_capi::Resident single;  // lins_gpu_ieskf / associate / estimate_transform (n = 1)
   lins_capi::SeqState seq;     // lins_gpu_seq_*
+  lins_capi::FeatState feat;   // lins_gpu_extract_features, lins_gpu_seq_step_pcl
   // the single-scan map: "last" clouds (walks + tripods) and the clouds the 1-NN index was built on
   Buf<float4> map_s, map_c, tree_s, tree_c;
   Buf<int> map_off;  // 4 x 2 ints: [0,ns][0,nc][0,tns][0,tnc]
@@ -281,5 +301,7 @@ int fused_qtile(int max_q);
 size_t icp_state_bytes();
 int icp_loop(lins_ctx* ctx, Resident& r, lins_dev::BatchView bv, double* pose, lins_dev::IcpState* icp);
 int transform_to_end_csr(lins_ctx* ctx, float4* pts, const int* off, int n_units, const double* lin, const unsigned char* run);
+// lins_features.cu: validate, upload and extract the scans of d into ctx->feat; reads the counts back (one synchronisation)
+int features_run(lins_ctx* ctx, const lins_feature_params* fp, const lins_pcl_desc* d);
 
 }  // namespace lins_capi

@@ -388,6 +388,60 @@ int lins_gpu_seq_step_ex(lins_ctx* ctx, const lins_seq_step_desc* d, const doubl
 
 int lins_gpu_seq_step(lins_ctx* ctx, const lins_seq_step_desc* d) { return lins_gpu_seq_step_ex(ctx, d, nullptr); }
 
+int lins_gpu_seq_step_pcl(lins_ctx* ctx, const lins_seq_pcl_desc* d, const lins_feature_params* fp, const double* scan_imu) {
+  if (!ctx) return LINS_E_INVALID;
+  SeqState& q = ctx->seq;
+  if (q.n == 0) return fail(ctx, LINS_E_NOMAP, "lins_gpu_seq_begin has not been called");
+  if (!d || d->n_seq != q.n || d->pcl.n_scans != q.n) return fail(ctx, LINS_E_INVALID, "n_seq differs from the hand-over's");
+  const int n = q.n, N1 = n + 1;
+  if (d->imu_off) { const int rc = check_csr(ctx, d->imu_off, n, d->imu, "bad imu offsets / samples"); if (rc != LINS_OK) return rc; }
+  else if (d->imu) return fail(ctx, LINS_E_INVALID, "imu without imu_off");
+  if (!scan_imu)
+    for (int s = 0; s < n; ++s)
+      if ((!d->present || d->present[s]) && q.fusion[s] != FUSION_RUNNING)
+        return fail(ctx, LINS_E_INVALID, "scan_imu is required while a present slot is initialising");
+  // extraction, validation of the scans and the counts' read-back: nothing of the sequences has changed yet
+  int rc = features_run(ctx, fp, &d->pcl);
+  if (rc != LINS_OK) return rc;
+  // the present slots' features -> the step's four clouds (q.up, lins_seq_step_desc order), dense in slot order
+  FeatState& f = ctx->feat;
+  Resident& r = q.up;
+  std::vector<int32_t> off(4 * (size_t)N1, 0);
+  r.max_q = 0;
+  for (int s = 0; s < n; ++s) {
+    const bool present = !d->present || d->present[s];
+    for (int k = 0; k < 4; ++k) off[k * N1 + s + 1] = off[k * N1 + s] + (present ? f.h_counts.p[5 * s + k] : 0);
+    r.max_q = std::max(r.max_q, (off[s + 1] - off[s]) + (off[N1 + s + 1] - off[N1 + s]));
+  }
+  r.n = n; r.nqs = off[N1 - 1]; r.nqc = off[2 * N1 - 1]; r.nts = off[3 * N1 - 1]; r.ntc = off[4 * N1 - 1];
+  CK(r.qs.reserve(r.nqs + 1)); CK(r.qc.reserve(r.nqc + 1)); CK(r.ts.reserve(r.nts + 1)); CK(r.tc.reserve(r.ntc + 1));
+  CK(r.qs_off.reserve(N1)); CK(r.qc_off.reserve(N1)); CK(r.ts_off.reserve(N1)); CK(r.tc_off.reserve(N1));
+  CK(r.h_off.reserve(4 * (size_t)N1));
+  float4* dst[4] = {r.qs.p, r.qc.p, r.ts.p, r.tc.p};
+  int* doff[4] = {r.qs_off.p, r.qc_off.p, r.ts_off.p, r.tc_off.p};
+  std::vector<SeqCopy> copies;
+  for (int k = 0; k < 4; ++k)
+    for (int s = 0; s < n; ++s) {
+      const int len = off[k * N1 + s + 1] - off[k * N1 + s];
+      if (len) copies.push_back(SeqCopy{f.out[k].p + d->pcl.cloud_off[s], dst[k] + off[k * N1 + s], len, 0});
+    }
+  CK(f.copies.reserve(copies.size() + 1)); CK(f.h_copies.reserve(copies.size() + 1));
+  std::copy(copies.begin(), copies.end(), f.h_copies.p);
+  std::memcpy(r.h_off.p, off.data(), sizeof(int) * off.size());
+  if (!copies.empty()) CK(cudaMemcpyAsync(f.copies.p, f.h_copies.p, sizeof(SeqCopy) * copies.size(), cudaMemcpyHostToDevice, ctx->stream));
+  for (int k = 0; k < 4; ++k) CK(cudaMemcpyAsync(doff[k], r.h_off.p + (size_t)k * N1, sizeof(int) * N1, cudaMemcpyHostToDevice, ctx->stream));
+  rc = run_copies(ctx, f.copies.p, (int)copies.size());
+  if (rc != LINS_OK) return rc;
+  lins_seq_step_desc sd;
+  std::memset(&sd, 0, sizeof(sd));
+  sd.n_seq = n; sd.present = d->present; sd.imu = d->imu; sd.imu_off = d->imu_off; sd.point_format = LINS_POINTS_XYZI32;
+  const int32_t* offs[4] = {&off[0], &off[N1], &off[2 * N1], &off[3 * N1]};
+  // from here on the sequences' state changes, as in lins_gpu_seq_step_ex
+  rc = seq_step_run(ctx, &sd, offs, scan_imu);
+  if (rc != LINS_OK) q.n = 0;
+  return rc;
+}
+
 }  // extern "C"
 
 // the part of lins_gpu_seq_step after its input is validated and uploaded

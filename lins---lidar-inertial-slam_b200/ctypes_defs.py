@@ -144,6 +144,31 @@ class LinsSeqBeginDesc(C.Structure):
     ]
 
 
+class LinsFeatureParams(C.Structure):
+    """lins_feature_params (include/lins_gpu.h): the feature extraction's constants."""
+    _fields_ = [("edge_threshold", C.c_double), ("surf_threshold", C.c_double), ("imu_lidar_extrinsic_angle", C.c_double)]
+
+    @classmethod
+    def shipped(cls, edge_threshold=0.5, surf_threshold=0.5, imu_lidar_extrinsic_angle=0.0):
+        """exp_port.yaml:7, :12-13 (csrc/host/feature_extraction.hpp FeatureParams defaults)."""
+        return cls(edge_threshold, surf_threshold, imu_lidar_extrinsic_angle)
+
+
+class LinsPclDesc(C.Structure):
+    """lins_pcl_desc: n segmented scans with their cloud_info, CSR."""
+    _fields_ = [("n_scans", C.c_int32), ("line_num", C.c_int32), ("cloud", C.c_void_p), ("cloud_off", C.c_void_p),
+                ("ground_flag", C.c_void_p), ("col_ind", C.c_void_p), ("range", C.c_void_p), ("start_ring_index", C.c_void_p),
+                ("end_ring_index", C.c_void_p), ("orientation", C.c_void_p), ("point_format", C.c_int32)]
+
+
+class LinsSeqPclDesc(C.Structure):
+    """lins_seq_pcl_desc: one processPCL-shaped scan per sequence."""
+    _fields_ = [("n_seq", C.c_int32), ("present", C.c_void_p), ("imu", C.c_void_p), ("imu_off", C.c_void_p), ("pcl", LinsPclDesc)]
+
+
+FEAT_RING_CAP = 2048  # LINS_FEAT_RING_CAP
+
+
 class LinsSeqStepDesc(C.Structure):
     _fields_ = [
         ("n_seq", C.c_int32),

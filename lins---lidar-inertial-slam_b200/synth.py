@@ -10,7 +10,7 @@ import subprocess
 
 import numpy as np
 
-from .ctypes_defs import Batch, LinsBatchDesc, POINT_DTYPE
+from .ctypes_defs import Batch, LinsBatchDesc, LinsPclDesc, POINT_DTYPE
 
 _ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 _DIR = os.path.join(_ROOT, "tools", "synth")
@@ -282,6 +282,11 @@ def replay_feature_log(log, device=0, params=None, init_std=None):
     std = None if init_std is None else np.ascontiguousarray(init_std, dtype=np.float64)
     h = L.lins_flog_replay(C.byref(d), int(log.get("lidar", 0)), device, C.cast(C.byref(params), C.c_void_p) if params is not None else None,
                            None if std is None else std.ctypes.data)
+    return _replay_record(L, h, n)
+
+
+def _replay_record(L, h, n):
+    """Read (and free) a replay record of lins_flog_replay / lins_plog_replay."""
     try:
         ints = lambda w: np.ctypeslib.as_array(L.lins_replay_ints(h, w), shape=(n,)).copy()  # noqa: E731
         dbl = lambda w, cnt: np.ctypeslib.as_array(L.lins_replay_doubles(h, w), shape=(cnt,)).copy()  # noqa: E731
@@ -301,6 +306,84 @@ def replay_feature_log(log, device=0, params=None, init_std=None):
         return rec
     finally:
         L.lins_replay_destroy(h)
+
+
+# ---- pcl logs: the same drives as processPCL receives them (segmented cloud + cloud_info per scan) ---------------------
+class PclLogDesc(C.Structure):
+    _fields_ = [("n_scans", C.c_int32), ("time", C.c_void_p), ("imu", C.c_void_p), ("imu_off", C.c_void_p),
+                ("imu_last", C.c_void_p), ("pcl", LinsPclDesc)]
+
+
+def _plog_lib():
+    L = _flog_lib()
+    if not hasattr(L, "_plog"):
+        L.lins_plog_desc.argtypes = [C.c_void_p, C.POINTER(PclLogDesc)]
+        L.lins_plog_replay.restype = C.c_void_p
+        L.lins_plog_replay.argtypes = [C.POINTER(PclLogDesc), C.c_int, C.c_int, C.c_void_p, C.c_void_p]
+        L._plog = True
+    return L
+
+
+def pcl_log(config="config3", seed=1, n_scans=12, **overrides):
+    """The drive of feature_log(config, seed, n_scans) as processPCL receives it: dict with lidar, line_num, time, imu +
+    imu_off, imu_last (as in a feature log) and scans: one dict per scan with seg (m x 4 float32 x, y, z, intensity), ground,
+    col, range, start_ring / end_ring (line_num) and ori (start, end, diff).  Edit the scans freely, then replay the log
+    with replay_pcl_log or sequence mode (LinsGpu.seq_step_pcl)."""
+    L = _plog_lib()
+    kw = dict(CONFIGS[config])
+    kw.update(overrides)
+    cfg = SynthCfg(**kw)
+    h = L.lins_flog_create(C.byref(cfg), seed, n_scans)
+    try:
+        d = PclLogDesc()
+        L.lins_plog_desc(h, C.byref(d))
+        n, p = d.n_scans, d.pcl
+        ln = p.line_num
+        log = dict(lidar=kw["lidar"], line_num=ln, time=_copy(d.time, n, np.float64), imu_off=_copy(d.imu_off, n + 1, np.int32),
+                   imu_last=_copy(d.imu_last, n * 6, np.float64).reshape(n, 6))
+        log["imu"] = _copy(d.imu, int(log["imu_off"][-1]) * 7, np.float64).reshape(-1, 7)
+        off = _copy(p.cloud_off, n + 1, np.int32)
+        tot = int(off[-1])
+        pts = _copy(p.cloud, tot, POINT_DTYPE)
+        xyzi = np.stack([pts["x"], pts["y"], pts["z"], pts["intensity"]], 1).astype(np.float32)
+        ground, col, rng = _copy(p.ground_flag, tot, np.uint8), _copy(p.col_ind, tot, np.uint32), _copy(p.range, tot, np.float32)
+        sr, er = _copy(p.start_ring_index, n * ln, np.int32).reshape(n, ln), _copy(p.end_ring_index, n * ln, np.int32).reshape(n, ln)
+        ori = _copy(p.orientation, n * 3, np.float32).reshape(n, 3)
+        log["scans"] = [dict(seg=xyzi[off[k]:off[k + 1]].copy(), ground=ground[off[k]:off[k + 1]].copy(), col=col[off[k]:off[k + 1]].copy(),
+                             range=rng[off[k]:off[k + 1]].copy(), start_ring=sr[k].copy(), end_ring=er[k].copy(), ori=ori[k].copy()) for k in range(n)]
+        return log
+    finally:
+        L.lins_flog_destroy(h)
+
+
+def replay_pcl_log(log, device=0, params=None, init_std=None):
+    """Replay a pcl log through one C++ StateEstimator shim: processImu for every IMU row, then processPCL with the scan's
+    segmented cloud and cloud_info (the shim's host FeatureExtractor runs).  The record of replay_feature_log."""
+    L = _plog_lib()
+    n = len(log["time"])
+    scans = log["scans"]
+    keep = {k: np.ascontiguousarray(log[k]) for k in ("time", "imu", "imu_off", "imu_last")}
+    d = PclLogDesc()
+    d.n_scans = n
+    for k, v in keep.items():
+        setattr(d, k, v.ctypes.data)
+    off = np.concatenate([[0], np.cumsum([len(s["seg"]) for s in scans])]).astype(np.int32)
+    pts = np.zeros(max(int(off[-1]), 1), POINT_DTYPE)
+    xyzi = np.concatenate([np.asarray(s["seg"], np.float32).reshape(-1, 4) for s in scans])
+    pts["x"][:len(xyzi)], pts["y"][:len(xyzi)], pts["z"][:len(xyzi)], pts["intensity"][:len(xyzi)] = xyzi.T
+    pts["pad0"] = 1.0
+    cat = lambda k, t: np.ascontiguousarray(np.concatenate([np.asarray(s[k], t).reshape(-1) for s in scans] + [np.zeros(1, t)]))  # noqa: E731
+    keep.update(cloud=pts, cloud_off=off, ground=cat("ground", np.uint8), col=cat("col", np.uint32), range=cat("range", np.float32),
+                sr=cat("start_ring", np.int32), er=cat("end_ring", np.int32), ori=cat("ori", np.float32))
+    p = d.pcl
+    p.n_scans, p.line_num, p.point_format = n, int(log["line_num"]), 0
+    p.cloud, p.cloud_off, p.ground_flag, p.col_ind, p.range = (keep[k].ctypes.data for k in ("cloud", "cloud_off", "ground", "col", "range"))
+    p.start_ring_index, p.end_ring_index, p.orientation = keep["sr"].ctypes.data, keep["er"].ctypes.data, keep["ori"].ctypes.data
+    d.pcl = p
+    std = None if init_std is None else np.ascontiguousarray(init_std, dtype=np.float64)
+    h = L.lins_plog_replay(C.byref(d), int(log.get("lidar", 0)), device, C.cast(C.byref(params), C.c_void_p) if params is not None else None,
+                           None if std is None else std.ctypes.data)
+    return _replay_record(L, h, n)
 
 
 def host_predict(state, cov, imu_last, rows):

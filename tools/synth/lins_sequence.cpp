@@ -302,7 +302,21 @@ struct FeatureLog {
   std::vector<int32_t> imu_off{0};
   std::vector<lins_point> c[4];
   std::vector<int32_t> off[4] = {{0}, {0}, {0}, {0}};
+  // the same scans as processPCL receives them (a "pcl log"): segmented cloud + cloud_info, CSR like lins_pcl_desc
+  int line_num = 0;
+  std::vector<lins_point> seg;
+  std::vector<int32_t> seg_off{0}, start_ring, end_ring;
+  std::vector<uint8_t> ground;
+  std::vector<uint32_t> col;
+  std::vector<float> range, ori;
 };
+
+// a pcl log: per scan the IMU calls and processPCL's segmented cloud + cloud_info (lins_pcl_desc, n_scans == n)
+typedef struct lins_pcl_log_desc {
+  int32_t n_scans;
+  const double* time; const double* imu; const int32_t* imu_off; const double* imu_last;
+  lins_pcl_desc pcl;
+} lins_pcl_log_desc;
 
 // what the shim did with every scan of a replayed log, and its state right after it became RUNNING (the hand-over)
 struct ReplayRecord {
@@ -339,8 +353,31 @@ void* lins_flog_create(const lins_synth_cfg* cfg, uint64_t seed, int n_scans) {
     ex.run(ip.segmentedCloud, ip.segMsg, f);
     const Cloud* cl[4] = {&f.surfPointsFlat, &f.cornerPointsSharp, &f.surfPointsLessFlat, &f.cornerPointsLessSharp};
     for (int j = 0; j < 4; ++j) append_cloud(L->c[j], L->off[j], *cl[j]);
+    const CloudInfo& ci = ip.segMsg;
+    L->line_num = sim.lm.line_num;
+    append_cloud(L->seg, L->seg_off, ip.segmentedCloud);
+    const size_t m = ip.segmentedCloud.size();
+    L->ground.insert(L->ground.end(), ci.segmentedCloudGroundFlag.begin(), ci.segmentedCloudGroundFlag.begin() + m);
+    L->col.insert(L->col.end(), ci.segmentedCloudColInd.begin(), ci.segmentedCloudColInd.begin() + m);
+    L->range.insert(L->range.end(), ci.segmentedCloudRange.begin(), ci.segmentedCloudRange.begin() + m);
+    L->start_ring.insert(L->start_ring.end(), ci.startRingIndex.begin(), ci.startRingIndex.end());
+    L->end_ring.insert(L->end_ring.end(), ci.endRingIndex.begin(), ci.endRingIndex.end());
+    const float o3[3] = {ci.startOrientation, ci.endOrientation, ci.orientationDiff};
+    L->ori.insert(L->ori.end(), o3, o3 + 3);
   }
   return L;
+}
+// the pcl-log view of a feature log made by lins_flog_create (valid while the log lives)
+void lins_plog_desc(void* h, lins_pcl_log_desc* d) {
+  FeatureLog* L = static_cast<FeatureLog*>(h);
+  d->n_scans = (int32_t)L->time.size();
+  d->time = L->time.data(); d->imu = L->imu.data(); d->imu_off = L->imu_off.data(); d->imu_last = L->imu_last.data();
+  lins_pcl_desc& p = d->pcl;
+  p.n_scans = d->n_scans; p.line_num = L->line_num;
+  p.cloud = L->seg.data(); p.cloud_off = L->seg_off.data();
+  p.ground_flag = L->ground.data(); p.col_ind = L->col.data(); p.range = L->range.data();
+  p.start_ring_index = L->start_ring.data(); p.end_ring_index = L->end_ring.data(); p.orientation = L->ori.data();
+  p.point_format = LINS_POINTS_XYZI32;
 }
 void lins_flog_destroy(void* h) { delete static_cast<FeatureLog*>(h); }
 void lins_flog_desc(void* h, lins_feature_log_desc* d) {
@@ -353,27 +390,70 @@ void lins_flog_desc(void* h, lins_feature_log_desc* d) {
 // Replay a (possibly edited) feature log through one shim: processImu for every IMU row, then processFeatures.
 // gpu: the C-ABI parameters of the shim's context (NULL = the shipped ones); init_std: INIT_POS_STD (3) + INIT_ATT_STD (3,
 // degrees) of its filter (NULL = zero)
+// One shim over n scans: processImu for every IMU row of scan k, then feed(est, k, f), which hands the scan to the
+// estimator and leaves its four feature clouds in f (for the record's gate and code)
+}  // extern "C"
+template <typename Feed>
+static ReplayRecord* replay_scans(int n_scans, const double* time, const double* imu, const int32_t* imu_off, const double* imu_last,
+                                  int lidar_model, int device, const lins_params* gpu, const double* init_std, Feed feed);
+extern "C" {
+
 void* lins_flog_replay(const lins_feature_log_desc* d, int lidar_model, int device, const lins_params* gpu, const double* init_std) {
+  return replay_scans(d->n_scans, d->time, d->imu, d->imu_off, d->imu_last, lidar_model, device, gpu, init_std,
+                      [d](StateEstimator& est, int k, const lins::sensor_utils::Imu& im, ScanFeatures& f) {
+                        Cloud* cl[4] = {&f.surfPointsFlat, &f.cornerPointsSharp, &f.surfPointsLessFlat, &f.cornerPointsLessSharp};
+                        for (int j = 0; j < 4; ++j) cl[j]->points.assign(d->clouds[j] + d->offs[j][k], d->clouds[j] + d->offs[j][k + 1]);
+                        est.processFeatures(d->time[k], im, f);
+                      });
+}
+
+// Replay a (possibly edited) pcl log through one shim: processImu for every IMU row, then processPCL with the scan's
+// segmented cloud and cloud_info (the shim's own FeatureExtractor runs; the outlier cloud is empty: the odometry never
+// reads it).  Same record as lins_flog_replay.
+void* lins_plog_replay(const lins_pcl_log_desc* d, int lidar_model, int device, const lins_params* gpu, const double* init_std) {
+  const LidarModel lm0 = lidar_model == 1 ? LidarModel::dense64() : LidarModel::vlp16();
+  return replay_scans(d->n_scans, d->time, d->imu, d->imu_off, d->imu_last, lidar_model, device, gpu, init_std,
+                      [d, lm0](StateEstimator& est, int k, const lins::sensor_utils::Imu& im, ScanFeatures& f) {
+                        const lins_pcl_desc& p = d->pcl;
+                        const int a = p.cloud_off[k], b = p.cloud_off[k + 1], L = p.line_num;
+                        Cloud cloud, outlier;
+                        cloud.points.assign(p.cloud + a, p.cloud + b);
+                        CloudInfo info;
+                        info.resize(L, b - a);
+                        for (int i = 0; i < L; ++i) { info.startRingIndex[i] = p.start_ring_index[(size_t)k * L + i]; info.endRingIndex[i] = p.end_ring_index[(size_t)k * L + i]; }
+                        info.startOrientation = p.orientation[3 * k]; info.endOrientation = p.orientation[3 * k + 1]; info.orientationDiff = p.orientation[3 * k + 2];
+                        for (int i = a; i < b; ++i) {
+                          info.segmentedCloudGroundFlag[i - a] = p.ground_flag[i]; info.segmentedCloudColInd[i - a] = p.col_ind[i]; info.segmentedCloudRange[i - a] = p.range[i];
+                        }
+                        LidarModel lm = lm0;
+                        lm.line_num = L;
+                        FeatureExtractor(lm, FeatureParams()).run(cloud, info, f);  // (what processPCL extracts: the record's sizes)
+                        est.processPCL(d->time[k], im, cloud, info, outlier);
+                      });
+}
+
+}  // extern "C"
+template <typename Feed>
+static ReplayRecord* replay_scans(int n_scans, const double* time, const double* imu, const int32_t* imu_off, const double* imu_last,
+                                  int lidar_model, int device, const lins_params* gpu, const double* init_std, Feed feed) {
   ReplayRecord* R = new ReplayRecord();
   const LidarModel lm = lidar_model == 1 ? LidarModel::dense64() : LidarModel::vlp16();
   lins::fusion::EstimatorParams ep = seq_params(lm);
   if (gpu) ep.gpu = *gpu;
   if (init_std) { ep.filter.init_pos_std = V3D(init_std[0], init_std[1], init_std[2]); ep.filter.init_att_std = V3D(init_std[3], init_std[4], init_std[5]); }
   StateEstimator est(ep, device);
-  for (int k = 0; k < d->n_scans; ++k) {
+  for (int k = 0; k < n_scans; ++k) {
     const auto t0 = std::chrono::steady_clock::now();
-    for (int m = d->imu_off[k]; m < d->imu_off[k + 1]; ++m) {
-      const double* r = d->imu + (size_t)m * 7;
+    for (int m = imu_off[k]; m < imu_off[k + 1]; ++m) {
+      const double* r = imu + (size_t)m * 7;
       est.processImu(r[0], V3D(r[1], r[2], r[3]), V3D(r[4], r[5], r[6]));
     }
     ScanFeatures f;
-    Cloud* cl[4] = {&f.surfPointsFlat, &f.cornerPointsSharp, &f.surfPointsLessFlat, &f.cornerPointsLessSharp};
-    for (int j = 0; j < 4; ++j) cl[j]->points.assign(d->clouds[j] + d->offs[j][k], d->clouds[j] + d->offs[j][k + 1]);
     const bool running = est.status_ == StateEstimator::STATUS_RUNNING;
     const StateEstimator::FusionStatus before = est.status_;
     est.last_report_ = lins_report();
-    const double* il = d->imu_last + (size_t)k * 6;
-    est.processFeatures(d->time[k], lins::sensor_utils::Imu(d->time[k], V3D(il[0], il[1], il[2]), V3D(il[3], il[4], il[5])), f);
+    const double* il = imu_last + (size_t)k * 6;
+    feed(est, k, lins::sensor_utils::Imu(time[k], V3D(il[0], il[1], il[2]), V3D(il[3], il[4], il[5])), f);
     R->scan_s.push_back(std::chrono::duration<double>(std::chrono::steady_clock::now() - t0).count());
     int code = LINS_SEQ_IDLE;
     if (running) {
@@ -417,6 +497,7 @@ void* lins_flog_replay(const lins_feature_log_desc* d, int lidar_model, int devi
   }
   return R;
 }
+extern "C" {
 // k StatePredictor::predict calls (default FilterParams) from state / covariance / acc_last + gyr_last, in place: the
 // host side of the predict stage check
 void lins_host_predict(double* state, double* cov, double* imu_last, const double* rows, int k) {

@@ -12,6 +12,7 @@
 //   unit   : (scan A -> targets in A's end frame, scan B -> queries, prior state + covariance from 40 IMU steps)
 // Never includes anything from oracle/.
 #include <atomic>
+#include <chrono>
 #include <cmath>
 #include <cstdint>
 #include <cstring>
@@ -473,6 +474,70 @@ int lins_frontend_run(const lins_point* raw, int n_raw, int lidar_model, int cap
   ori3[0] = ip.segMsg.startOrientation; ori3[1] = ip.segMsg.endOrientation; ori3[2] = ip.segMsg.orientationDiff;
   for (int i = 0; i < std::min(n[0], cap); ++i) { ground[i] = ip.segMsg.segmentedCloudGroundFlag[i]; col[i] = ip.segMsg.segmentedCloudColInd[i]; range[i] = ip.segMsg.segmentedCloudRange[i]; }
   return 0;
+}
+
+// FeatureExtractor::run (csrc/host/feature_extraction.hpp) on a given segmented cloud and cloud_info: the host side of
+// lins_gpu_extract_features for hand-built scans.  counts: surfPointsFlat, cornerPointsSharp, surfPointsLessFlat,
+// cornerPointsLessSharp (lins_gpu_extract_features' order); every output holds up to n points.
+int lins_features_host(const lins_point* seg, int n, int line_num, const int32_t* start_ring, const int32_t* end_ring,
+                       const float* ori3, const uint8_t* ground, const uint32_t* col, const float* range, const double* prm4,
+                       lins_point* undist, lins_point* surf_flat, lins_point* corner_sharp, lins_point* surf_less_flat,
+                       lins_point* corner_less_sharp, int32_t* counts) {
+  LidarModel lm;
+  lm.line_num = line_num;
+  lm.scan_period = prm4[3];
+  FeatureParams fp;
+  fp.edge_threshold = prm4[0]; fp.surf_threshold = prm4[1]; fp.imu_lidar_extrinsic_angle = prm4[2];
+  Cloud in;
+  in.points.assign(seg, seg + n);
+  CloudInfo info;
+  info.resize(line_num, n);
+  for (int i = 0; i < line_num; ++i) { info.startRingIndex[i] = start_ring[i]; info.endRingIndex[i] = end_ring[i]; }
+  info.startOrientation = ori3[0]; info.endOrientation = ori3[1]; info.orientationDiff = ori3[2];
+  for (int i = 0; i < n; ++i) { info.segmentedCloudGroundFlag[i] = ground[i]; info.segmentedCloudColInd[i] = col[i]; info.segmentedCloudRange[i] = range[i]; }
+  FeatureExtractor fe(lm, fp);
+  ScanFeatures f;
+  fe.run(in, info, f);
+  const Cloud* outs[4] = {&f.surfPointsFlat, &f.cornerPointsSharp, &f.surfPointsLessFlat, &f.cornerPointsLessSharp};
+  lins_point* dst[4] = {surf_flat, corner_sharp, surf_less_flat, corner_less_sharp};
+  for (int k = 0; k < 4; ++k) {
+    counts[k] = (int32_t)outs[k]->size();
+    std::memcpy(dst[k], outs[k]->points.data(), sizeof(lins_point) * std::min<size_t>(outs[k]->size(), (size_t)n));
+  }
+  std::memcpy(undist, f.undistPointCloud.points.data(), sizeof(lins_point) * (size_t)n);
+  return 0;
+}
+
+// Wall seconds of `reps` passes of FeatureExtractor::run (shipped parameters, SCAN_PERIOD 0.1) over every scan of d, the
+// scans handed out to `threads` std::threads one at a time: the host throughput lins_gpu_extract_features replaces.
+// Inputs are converted to Cloud / CloudInfo before the clock starts.
+double lins_features_host_bench(const lins_pcl_desc* d, int threads, int reps) {
+  const int n = d->n_scans, L = d->line_num;
+  std::vector<Cloud> clouds(n);
+  std::vector<CloudInfo> infos(n);
+  for (int k = 0; k < n; ++k) {
+    const int a = d->cloud_off[k], b = d->cloud_off[k + 1];
+    clouds[k].points.assign(d->cloud + a, d->cloud + b);
+    CloudInfo& info = infos[k];
+    info.resize(L, b - a);
+    for (int i = 0; i < L; ++i) { info.startRingIndex[i] = d->start_ring_index[(size_t)k * L + i]; info.endRingIndex[i] = d->end_ring_index[(size_t)k * L + i]; }
+    info.startOrientation = d->orientation[3 * k]; info.endOrientation = d->orientation[3 * k + 1]; info.orientationDiff = d->orientation[3 * k + 2];
+    for (int i = a; i < b; ++i) { info.segmentedCloudGroundFlag[i - a] = d->ground_flag[i]; info.segmentedCloudColInd[i - a] = d->col_ind[i]; info.segmentedCloudRange[i - a] = d->range[i]; }
+  }
+  LidarModel lm;
+  lm.line_num = L;
+  std::atomic<long> next(0);
+  const long total = (long)n * std::max(reps, 1);
+  auto work = [&]() {
+    FeatureExtractor fe(lm, FeatureParams());
+    ScanFeatures f;
+    for (long i; (i = next.fetch_add(1)) < total;) fe.run(clouds[i % n], infos[i % n], f);
+  };
+  const auto t0 = std::chrono::steady_clock::now();
+  std::vector<std::thread> pool;
+  for (int t = 0; t < std::max(threads, 1); ++t) pool.emplace_back(work);
+  for (auto& t : pool) t.join();
+  return std::chrono::duration<double>(std::chrono::steady_clock::now() - t0).count();
 }
 
 // one simulated raw sweep of the seeded world (an input for lins_frontend_run): returns the number of points written

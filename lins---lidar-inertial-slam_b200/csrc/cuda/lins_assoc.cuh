@@ -34,6 +34,23 @@ constexpr int kGroupLanes = LINS_GROUP_LANES;
 #endif
 constexpr int kThreadScanBins = LINS_THREAD_SCAN_BINS, kThreadWalkBins = LINS_THREAD_WALK_BINS;
 
+// Certificate and pass counters of the phase timers (bv.timers, read by lins_gpu_debug_phase_cycles; tools/phase_profile.py
+// prints them).  Slots kCertSlots + k, k = 0..7, count the certificates of seeded queries: checked, accepted, failed because
+// the runner-up now beats the winner (and the bound does not certify it), because winner + moved + slack >= bound, because
+// the answer left the gate, because a rejected search's slack is used up, failed although the fresh search returned one of
+// the stored front-runners, accepted by a swap.  Each slot holds two 32-bit counts: the closest point's certificates in
+// the low half, the walks' (one per query: Ind2 and, for surf, Ind3) in the high half.  Slots kPassSlots + 0..13: later
+// passes (no unit in its first pass) by their number of closest-point searches (0 / 1-16 / > 16: 3 counts, then the P2
+// cycles of each) and of walk searches (0 / 1-16 / 17-32 / > 32: 4 counts, then the P3 + P4 cycles of each).
+constexpr int kCertSlots = 40, kPassSlots = 48;
+__device__ __forceinline__ void count_cert_events(long long* timers, unsigned ev) {  // warp-wide; ev: bit k / 8 + k
+#pragma unroll
+  for (int k = 0; k < 8; ++k) {
+    const unsigned n1 = __popc(__ballot_sync(0xffffffffu, (ev >> k) & 1u)), n2 = __popc(__ballot_sync(0xffffffffu, (ev >> (8 + k)) & 1u));
+    if ((threadIdx.x & 31) == 0 && (n1 | n2)) atomicAdd((unsigned long long*)&timers[kCertSlots + k], ((unsigned long long)n2 << 32) | n1);
+  }
+}
+
 struct PassBuffers {           // per-query arrays, indexed by v = slot * qtile + i (shared memory, or the CTA's global scratch)
   float4* qpt;               // staged queries (x, y, z, intensity)
   float4* sel;               // de-skewed queries (pointSel)
@@ -119,12 +136,14 @@ __device__ void association_pass(CtaMem& cta, Smem* slots, const BatchView& bv, 
   const int Q = bv.qtile, NQ = bv.nslots * Q;
   const float nearf = (float)kp.nearest_sq;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int toff = cta.pass_first ? 32 : 0;  // diagnostics: passes that contain a unit's first pass are clocked separately
 
   // ---- A2: de-skew, fused with phase P1 of the association (same thread-per-query mapping; P1 touches only its own
   // query's state and the read-only index): per-query level -2 everything certified, -3 closest point certified (walks
-  // only), >= 0 full search (= window), -1 cannot match.  The work-list counters were reset after the previous pass.
-  for (int v = threadIdx.x; v < NQ; v += kThreads) {
+  // only), -4 closest point certified by a swap (walks only, around the new closest point), >= 0 full search (= window),
+  // -1 cannot match.  The work-list counters were reset after the previous pass.
+  for (int v = threadIdx.x; v < NQ; v += kThreads) {  // (NQ is a multiple of 32: every lane of a warp runs every trip)
+    unsigned ev = 0u;  // diagnostics: certificate events of this query (bit k: closest point, slot 40 + k; bit 8 + k: walks)
+    do {  // (a `continue` below leaves this block, not the loop: the events of every query are counted after it)
     const int sl = slot_of(v, Q), i = v - sl * Q;
     Smem& sm = slots[sl];
     if (!sm.run || i >= sm.ns + sm.nc) continue;
@@ -146,7 +165,7 @@ __device__ void association_pass(CtaMem& cta, Smem* slots, const BatchView& bv, 
     const bool seeded = !sm.first_pass;
     const AzIndex ixq = az_index_of(sm, bv, surf);
     float4 qa = make_float4(0.f, 0.f, -1.f, 0.f);
-    if (seeded) {  // certificates (lins_assoc_az.cuh: cert_accepted / cert_rejected): the stored answers still hold
+    if (seeded) {  // certificates (lins_assoc_az.cuh: cert_check / cert_rejected): the stored answers still hold
       const float4 r1 = pb.qref[v], r2 = pb.qref2[v], ex = pb.qext[v];
       const unsigned nearbits = __float_as_uint(nearf);
       const int w1s = pb.pos[3 * v], w2s = pb.pos[3 * v + 1], w3s = pb.pos[3 * v + 2];
@@ -163,15 +182,27 @@ __device__ void association_pass(CtaMem& cta, Smem* slots, const BatchView& bv, 
       const float4 tw2 = entry(w2s, walks), tr2 = entry(r2s, walks && w2s >= 0);
       const float4 tw3 = entry(w3s, walks && surf), tr3 = entry(r3s, walks && surf && w3s >= 0);
       const float moved1 = sqrtf(sqdist_f32(s.x, s.y, s.z, r1.x, r1.y, r1.z));
-      const bool ok1 = w1s >= 0 ? cert_accepted<false>(tw1, tr1, s, r1s, r1.w, moved1, nearbits, 0) : cert_rejected(r1.w, moved1);
+      const int c1 = w1s >= 0 ? cert_check<false>(tw1, tr1, s, r1s, r1.w, moved1, nearbits, 0)
+                              : (cert_rejected(r1.w, moved1) ? kCertKeep : kCertFailSlack);
+      const bool ok1 = c1 <= kCertSwap;
+      ev = 1u | (1u << (ok1 ? 1 : c1)) | (c1 == kCertSwap ? 1u << 7 : 0u);
+      // (a swap's write-back runs in P3, where a thread holds far fewer values than here)
+      if (c1 == kCertSwap) { az_polar(s, qa); pb.qa[v] = qa; pb.qw[v] = make_int4(-4, 0, 0, 0); continue; }
       bool ok2 = false;
+      int c2 = kCertKeep, c3 = kCertKeep;
       if (ok1 && walks) {  // (the walks' candidate sets are defined by the closest point: only meaningful while it stands)
         const int c0 = ccr0 & 0x00ffffff;
         const float moved2 = sqrtf(sqdist_f32(s.x, s.y, s.z, r2.x, r2.y, r2.z));
-        ok2 = w2s >= 0 ? cert_accepted<true>(tw2, tr2, s, r2s, r2.w, moved2, nearbits, c0) : cert_rejected(r2.w, moved2);
-        if (ok2 && surf) ok2 = w3s >= 0 ? cert_accepted<true>(tw3, tr3, s, r3s, ex.x, moved2, nearbits, c0) : cert_rejected(ex.x, moved2);
+        c2 = w2s >= 0 ? cert_check<true>(tw2, tr2, s, r2s, r2.w, moved2, nearbits, c0) : (cert_rejected(r2.w, moved2) ? kCertKeep : kCertFailSlack);
+        ok2 = c2 <= kCertSwap;
+        if (ok2 && surf) {
+          c3 = w3s >= 0 ? cert_check<true>(tw3, tr3, s, r3s, ex.x, moved2, nearbits, c0) : (cert_rejected(ex.x, moved2) ? kCertKeep : kCertFailSlack);
+          ok2 = c3 <= kCertSwap;
+        }
+        ev |= (1u << 8) | (1u << (8 + (ok2 ? 1 : c2 <= kCertSwap ? c3 : c2))) |  // (the first that failed)
+              (ok2 && (c2 == kCertSwap || c3 == kCertSwap) ? 1u << 15 : 0u);
       }
-      if (ok1 && (ok2 || ccr0 < 0)) { pb.qw[v] = make_int4(-2, 0, 0, 0); continue; }
+      if (ok1 && (ok2 || ccr0 < 0)) { pb.qw[v] = make_int4(-2, (c2 == kCertSwap ? 1 : 0) | (c3 == kCertSwap ? 2 : 0), 0, 0); continue; }
       if (ok1) { az_polar(s, qa); pb.qa[v] = qa; pb.qw[v] = make_int4(-3, 0, 0, 0); continue; }
     }
     const int w1 = az_prepare_nn(ixq, s, nearf, seeded ? pb.pos[3 * v] : -1, (int)pb.qpt[v].w, qa);
@@ -184,9 +215,11 @@ __device__ void association_pass(CtaMem& cta, Smem* slots, const BatchView& bv, 
     if (sm.first_pass && w1 >= 0 && (w1 & 0xffff) <= kThreadScanBins) pb.wl[NQ - 1 - atomicAdd(&cta.wl_tn[0], 1)] = v;
     else pb.wl[atomicAdd(&cta.wl_n[0], 1)] = v;
     if (bv.timers && w1 >= 0) atomicAdd(&cta.dbg[0], w1 & 0xffff);
+    } while (false);
+    if (bv.timers) count_cert_events(bv.timers, ev);
   }
   __syncthreads();
-  LINS_TICK(3 + toff);
+  LINS_TICK_PASS(3);
 
   if (cta.any_indexed) {
     // ---- A3/A4 fast path.  Scalar preparation (certificates, atan2f, asinf, bounds: P1 above, P3 below) runs one
@@ -202,6 +235,9 @@ __device__ void association_pass(CtaMem& cta, Smem* slots, const BatchView& bv, 
       const int p1 = top.p1;
       const float d1 = __uint_as_float((unsigned)(k1 >> 32));
       const bool acc1 = k1 != kKeyMax && p1 >= 0 && (double)d1 < kp.nearest_sq;
+      // (diagnostics read what they need from shared memory, so that nothing extra stays live across the scan)
+      if (bv.timers && !slots[slot_of(v, Q)].first_pass && pb.pos[3 * v] >= 0 && acc1 && (p1 == pb.pos[3 * v] || p1 == __float_as_int(pb.qext[v].y)))
+        atomicAdd((unsigned long long*)&bv.timers[kCertSlots + 6], 1ull);  // a failed certificate whose stored front-runners held the answer
       // accepted: what everything but the two front-runners exceeded; else the slack of "nothing within the gate"
       const float bound1 = w1 < 0 ? -1.f : acc1 ? cert_bound(top.d3, Bout) : rejected_slack((unsigned)(k1 >> 32), Bout, gate);
       pb.qref[v] = make_float4(s.x, s.y, s.z, bound1);
@@ -259,14 +295,38 @@ __device__ void association_pass(CtaMem& cta, Smem* slots, const BatchView& bv, 
       if (lane == 0) nn_finish(v, ix, s, top, w1, qa.w);
     }
     __syncthreads();
-    LINS_TICK(4 + toff);
+    if (bv.timers && threadIdx.x == 0 && !cta.pass_first) {  // later passes by their number of closest-point searches
+      const int n = cta.wl_n[0] + cta.wl_tn[0], b = n == 0 ? 0 : n <= 16 ? 1 : 2;
+      atomicAdd((unsigned long long*)&bv.timers[kPassSlots + b], 1ull);
+      atomicAdd((unsigned long long*)&bv.timers[kPassSlots + 3 + b], (unsigned long long)(clock64() - cta.tlast));
+    }
+    LINS_TICK_PASS(4);
     for (int v = threadIdx.x; v < NQ; v += kThreads) {  // P3
       const int sl = slot_of(v, Q), i = v - sl * Q;
       const Smem& sm = slots[sl];
       if (!sm.run || !sm.az_ok || i >= sm.ns + sm.nc || (sm.iter % kp.icp_freq) != 0) continue;
-      const int lvl = pb.qw[v].x;
-      if (lvl == -2) continue;
+      const int2 lq = *reinterpret_cast<const int2*>(&pb.qw[v]);  // (level, walk swaps)
+      const int lvl = lq.x;
       const bool surf = i < sm.ns;
+      // swaps certified in P1: winner and runner-up change places, the IDs follow; the search position and bound stay
+      auto swap_front = [&](int k, float* runner_up) {  // k = 0 closest point, 1 Ind2, 2 Ind3; returns the new winner's entry
+        const int w = pb.pos[3 * v + k], r = __float_as_int(*runner_up);
+        pb.pos[3 * v + k] = r;
+        *runner_up = __int_as_float(w);
+        return az_index_of(sm, bv, surf).pts[r].w;
+      };
+      if (lvl == -2) {
+        if (lq.y) {
+          int* const o = surf ? bv.ind_s + 3 * (size_t)(sm.qs0 + i) : bv.ind_c + 2 * (size_t)(sm.qc0 + i - sm.ns);
+          if (lq.y & 1) o[1] = slot_index(swap_front(1, &pb.qext[v].z));
+          if (lq.y & 2) o[2] = slot_index(swap_front(2, &pb.qext[v].w));
+        }
+        continue;
+      }
+      if (lvl == -4) {  // a new closest point: its walks are searched below (their candidate sets are defined by it)
+        const float tw = swap_front(0, &pb.qext[v].y);
+        pb.qccr[v] = (slot_ring(tw) << 24) | slot_index(tw);
+      }
       const int ccr = pb.qccr[v];
       if (ccr < 0) {  // no closest point within the gate: nothing to walk
         pb.pos[3 * v + 1] = -1; pb.pos[3 * v + 2] = -1;
@@ -284,7 +344,7 @@ __device__ void association_pass(CtaMem& cta, Smem* slots, const BatchView& bv, 
       const int p1 = pb.pos[3 * v];
       if (surf) az_prepare_walk<true>(ix, pb.sel[v], pb.qa[v], p1, c, cr, sd2, sd3, min(sm.ns, sm.Ts), nearf, w2, w3, B2, B3);
       else az_prepare_walk<false>(ix, pb.sel[v], pb.qa[v], p1, c, cr, sd2, sd3, min(sm.nc, sm.Tc), nearf, w2, w3, B2, B3);
-      pb.qw[v] = make_int4(1, w2, w3, ccr);
+      pb.qw[v] = make_int4(lvl == -3 ? 2 : 1, w2, w3, ccr);  // (.x = 2: the walks' certificate failed; diagnostics only)
       reinterpret_cast<float2*>(pb.key)[v] = make_float2(B2, B3);
       if (sm.first_pass && (w2 & 0xffff) <= kThreadWalkBins && (w3 & 0xffff) <= kThreadWalkBins) pb.wl[NQ - 1 - atomicAdd(&cta.wl_tn[1], 1)] = v;
       else pb.wl[atomicAdd(&cta.wl_n[1], 1)] = v;
@@ -297,9 +357,14 @@ __device__ void association_pass(CtaMem& cta, Smem* slots, const BatchView& bv, 
     }
     // result of a query's walks -> its state + the correspondence IDs (one thread)
     auto walk_finish = [&](int v, const Smem& sm, int i, bool surf, const float4 s, int ccr, const WalkOut& wo) {
+      float4 ex = pb.qext[v];  // (.y = the closest point's runner-up, written by P2 or kept from an earlier pass)
+      if (bv.timers && pb.qw[v].x == 2) {  // did the stored front-runners hold every answer of the failed certificate?
+        auto held = [](int w, int r, int now) { return w >= 0 ? now == w || now == r : now < 0; };
+        if (held(pb.pos[3 * v + 1], __float_as_int(ex.z), wo.pos2) && (!surf || held(pb.pos[3 * v + 2], __float_as_int(ex.w), wo.pos3)))
+          atomicAdd((unsigned long long*)&bv.timers[kCertSlots + 6], 1ull << 32);
+      }
       pb.pos[3 * v + 1] = wo.pos2; pb.pos[3 * v + 2] = wo.pos3;
       pb.qref2[v] = make_float4(s.x, s.y, s.z, wo.bound2);
-      float4 ex = pb.qext[v];  // (.y = the closest point's runner-up, written by P2 or kept from an earlier pass)
       ex.x = wo.bound3; ex.z = __int_as_float(wo.run2); ex.w = __int_as_float(wo.run3);
       pb.qext[v] = ex;
       const int i1 = ccr & 0x00ffffff;
@@ -385,7 +450,12 @@ __device__ void association_pass(CtaMem& cta, Smem* slots, const BatchView& bv, 
     }
   }
   __syncthreads();
-  LINS_TICK(5 + toff);
+  if (bv.timers && threadIdx.x == 0 && !cta.pass_first) {  // later passes by their number of walk searches
+    const int n = cta.wl_n[1] + cta.wl_tn[1], b = n == 0 ? 0 : n <= 16 ? 1 : n <= 32 ? 2 : 3;
+    atomicAdd((unsigned long long*)&bv.timers[kPassSlots + 6 + b], 1ull);
+    atomicAdd((unsigned long long*)&bv.timers[kPassSlots + 10 + b], (unsigned long long)(clock64() - cta.tlast));
+  }
+  LINS_TICK_PASS(5);
   // the searches of this pass are over: reset the work lists for the next pass
   if (threadIdx.x == kThreads - 1) { cta.wl_n[0] = 0; cta.wl_n[1] = 0; cta.wl_tn[0] = 0; cta.wl_tn[1] = 0; cta.wl_head[0] = 0; cta.wl_head[1] = 0; cta.wl_thead[0] = 0; cta.wl_thead[1] = 0; cta.dbg[0] = 0; cta.dbg[1] = 0; }
 
@@ -446,7 +516,7 @@ __device__ void association_pass(CtaMem& cta, Smem* slots, const BatchView& bv, 
     }
   }
   __syncthreads();
-  LINS_TICK(6 + toff);
+  LINS_TICK_PASS(6);
 }
 
 }  // namespace lins_dev

@@ -22,11 +22,11 @@
 // Certificates.  Every search also returns its two front-runners (winner and runner-up slots) and a bound: the
 // distance every OTHER candidate exceeded at the search position (the third best distance, or the distance bound of
 // everything outside the window, whichever is smaller).  Later, one thread re-evaluates the two front-runners exactly;
-// if the winner still beats the runner-up (exact keys), is still inside the gate, and is closer than
-// bound - displacement (true distances change by at most the displacement), nothing else can have overtaken it: the
-// stored answer is reused and the search is skipped (cert_accepted).  A plain winner / runner-up margin cannot certify a
-// query that sits almost midway between two neighbouring points of a ring — the common case; this can.  Three-way
-// exact ties fail the test and are re-searched.  A search that found nothing within the gate keeps a plain slack
+// if the better of them (exact keys) is inside the gate and closer than bound - displacement (true distances change by
+// at most the displacement), nothing else can have overtaken it: it is the answer — the stored winner, or the runner-up
+// when the two swapped — and the search is skipped (cert_check).  A plain winner / runner-up margin cannot certify a
+// query that sits almost midway between two neighbouring points of a ring — the common case; this can, on either side
+// of the midpoint.  Three-way exact ties fail the test and are re-searched.  A search that found nothing within the gate keeps a plain slack
 // (cert_rejected).  Windows are built for sqrt(U) + kCertMargin so the "outside" bound is not vacuous.  The closest
 // point and the walks are certified separately (a new closest point always forces new walks).
 #pragma once
@@ -590,29 +590,33 @@ __device__ __forceinline__ WalkOut az_scan_walk_group(const AzIndex& ix, const f
 }
 
 // ---- certificates (phase P1, one THREAD per query) ------------------------------------------------------------------
-// An accepted answer (winner slot w >= 0) is still the answer at the query's new position s if
-//   * the winner re-evaluated exactly is still inside the gate and still beats the re-evaluated runner-up (exact keys,
-//     so ties fall like in a full search), and
-//   * it is closer than everything else can have become: bound - moved, where `bound` is what every other candidate
-//     exceeded at the search position and `moved` the displacement since (distances change by at most that much);
-//     2e-4 m absorbs the f32 rounding of the distances involved.
+// Of the two stored front-runners (winner w >= 0, runner-up r), re-evaluated exactly at the query's new position s, the
+// one with the smaller key (exact keys, so ties fall like in a full search) is the answer of a search at s if it is
+// closer than everything else can have become: bound - moved, where `bound` is what every other candidate exceeded at
+// the search position and `moved` the displacement since (distances change by at most that much); 2e-4 m absorbs the
+// f32 rounding of the distances involved.  Nothing else can then beat it or tie with it, whether it is the old winner
+// or the runner-up: a query sliding along a ring past the midpoint of two neighbouring points swaps them and keeps its
+// certificate.  That answer must also be inside the gate (an answer beyond it would mean "no match", which is searched).
 // WALK: keys carry the visiting order relative to the closest point c instead of the original index.
 // tw / tr = the winner's / runner-up's entry of the sorted copy, loaded by the caller (all of a query's front-runners are
 // fetched in one batch: one L2 round trip instead of up to six dependent ones); r < 0 = no runner-up.
+// Returns kCertKeep / kCertSwap (certified; on a swap the runner-up is the answer now) or the reason it failed.
+enum : int { kCertKeep = 0, kCertSwap = 1, kCertFailRunnerUp = 2, kCertFailBound = 3, kCertFailGate = 4, kCertFailSlack = 5 };
 template <bool WALK>
-__device__ __forceinline__ bool cert_accepted(const float4 tw, const float4 tr, const float4 s, int r, float bound, float moved, unsigned nearbits,
-                                              int c) {
+__device__ __forceinline__ int cert_check(const float4 tw, const float4 tr, const float4 s, int r, float bound, float moved, unsigned nearbits,
+                                          int c) {
   auto key_of = [&](const float4 t) -> unsigned long long {
     const unsigned d = __float_as_uint(sqdist_f32(t.x, t.y, t.z, s.x, s.y, s.z));
     const int j = slot_index(t.w);
     const unsigned lo = WALK ? (j > c ? order_fwd(j) : order_bwd(j)) : (unsigned)j;
     return ((unsigned long long)d << 32) | lo;
   };
-  const unsigned long long kw = key_of(tw);
-  const unsigned dw = (unsigned)(kw >> 32);
-  if (!(dw < nearbits)) return false;
-  if (r >= 0 && !(kw < key_of(tr))) return false;
-  return sqrtf(__uint_as_float(dw)) + moved + 2.0e-4f < bound;
+  const unsigned long long kw = key_of(tw), kr = r >= 0 ? key_of(tr) : kKeyMax;
+  const bool swap = kr < kw;
+  const unsigned dm = (unsigned)((swap ? kr : kw) >> 32);
+  if (!(dm < nearbits)) return kCertFailGate;
+  if (!(sqrtf(__uint_as_float(dm)) + moved + 2.0e-4f < bound)) return swap ? kCertFailRunnerUp : kCertFailBound;
+  return swap ? kCertSwap : kCertKeep;
 }
 // a search that found nothing within the gate: stays that way while the query moved less than half the slack
 __device__ __forceinline__ bool cert_rejected(float slack, float moved) { return slack > 0.f && 2.0f * moved + 2.0e-4f < slack; }

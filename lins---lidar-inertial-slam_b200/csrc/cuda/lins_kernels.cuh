@@ -189,6 +189,9 @@ static_assert(sizeof(((CtaMem*)nullptr)->u.fold) <= sizeof(((CtaMem*)nullptr)->u
       cta.tlast = _t;                                                                   \
     }                                                                                  \
   } while (0)
+// a tick of the association pass: passes that contain a unit's first pass are clocked separately, in slot k + 32
+// (cta.pass_first is read when the tick is taken, so no register is held across the pass for it)
+#define LINS_TICK_PASS(k) LINS_TICK((k) + (cta.pass_first ? 32 : 0))
 
 // ---------------------------------------------------------------------------------------------------------
 // A2 transformToStart (StateEstimator.hpp:1066-1080) -------------------------------------------------------

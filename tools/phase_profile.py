@@ -34,3 +34,16 @@ print("passes with a first-pass unit: %d (%.2f units resident), cycles per pass:
     t[62], t[63]/max(t[62],1), t[35]/max(t[62],1), t[36]/max(t[62],1), t[37]/max(t[62],1), t[38]/max(t[62],1)))
 print("other passes:                   %d (%.2f units resident), cycles per pass: P1 %.0f  P2 %.0f  P3+P4 %.0f  residual %.0f" % (
     t[30], t[31]/max(t[30],1), (t[3]-t[35])/max(t[30],1), (t[4]-t[36])/max(t[30],1), (t[5]-t[37])/max(t[30],1), (t[6]-t[38])/max(t[30],1)))
+# certificates of seeded queries (lins_assoc.cuh, kCertSlots = 40): two 32-bit counts per slot, closest point low, walks high
+cert = [[(int(t[40 + k]) >> (32 * h)) & 0xffffffff for k in range(8)] for h in (0, 1)]
+for h, nm in ((0, "closest point"), (1, "walks")):
+    c = cert[h]
+    print(f"certificates, {nm:13s}: checked {c[0]}  accepted {c[1]} ({100*c[1]/max(c[0],1):.1f}%, by a swap {c[7]})  failed: runner-up wins {c[2]}"
+          f"  bound {c[3]}  left the gate {c[4]}  slack used up {c[5]};  failed but a stored front-runner was the answer {c[6]}")
+print(f"  checked = accepted + failed: {all(c[0] == c[1] + sum(c[2:6]) for c in cert)}")
+# later passes by their number of searches (kPassSlots = 48)
+later = max(int(t[30]), 1)
+for nm, base, labels, ph in (("closest-point", 48, ("0", "1-16", ">16"), "P2"), ("walk", 54, ("0", "1-16", "17-32", ">32"), "P3+P4")):
+    nb = len(labels)
+    print(f"later passes by {nm} searches: " + "  ".join(
+        f"{lab}: {100*t[base+b]/later:.1f}% ({t[base+nb+b]/max(t[base+b],1):.0f} {ph} cycles)" for b, lab in enumerate(labels)))

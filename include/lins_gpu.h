@@ -374,6 +374,44 @@ typedef struct lins_seq_pcl_desc {
 int lins_gpu_seq_step_pcl(lins_ctx* ctx, const lins_seq_pcl_desc* step, const lins_feature_params* fp,
                           const double* scan_imu /*S x 6 or NULL*/);
 
+/* ---- image projection: lins/src/image_projection_node.cpp:191-415 (findStartEndAngle, projectPointCloud,
+   groundRemoval, cloudSegmentation with labelComponents) on the device, from the raw sweep the LiDAR driver publishes to
+   the segmented cloud, cloud_info and outlier cloud (cloudHandler :177-189 without ROS).  Bit-identical to a fresh host
+   restatement csrc/host/image_projection.hpp per scan (DESIGN.md §4.7). */
+
+/* the lidar geometry image projection reads; the reference hard-wires VLP-16 (parameters.h:82-92: N_SCAN 16, Horizon_SCAN
+   1800, ang_res_x 0.2, ang_res_y 2.0, ang_bottom 15.1, groundScanInd 5) */
+typedef struct lins_lidar_model {
+  int32_t line_num;         /* N_SCAN: rows of the range image, 1..128 */
+  int32_t scan_num;         /* Horizon_SCAN: columns, 2..LINS_FEAT_RING_CAP */
+  float ang_res_x;          /* degrees per column, finite and > 0 */
+  float ang_res_y;          /* degrees per row, finite and > 0 */
+  float ang_bottom;         /* degrees, finite */
+  int32_t ground_scan_ind;  /* groundScanInd: 0..line_num - 1 */
+} lins_lidar_model;
+
+/* n raw sweeps, CSR: sweep i's points (firing order; NaN no-returns allowed) are cloud[cloud_off[i] .. cloud_off[i + 1]).
+   The points' own intensity is not read. */
+typedef struct lins_raw_desc {
+  int32_t n_scans;
+  const lins_point* cloud; const int32_t* cloud_off;  /* n_scans + 1 offsets */
+  int32_t point_format;                /* LINS_POINTS_XYZI32 or LINS_POINTS_PACKED16, as in lins_batch_desc */
+} lins_raw_desc;
+
+/* ≙ cloudHandler (image_projection_node.cpp:177-189) for every sweep of d, each on a fresh ImageProjection.  Sweep i's
+   segmented cloud (seg) with its per-point cloud_info (ground_flag, col_ind, range) and its outlier cloud are written at
+   its own input offsets (each pixel holds at most one point, so neither is longer than the sweep), in d->point_format
+   (XYZI32 records carry pad0 = 1 and zero pads): the layout lins_pcl_desc takes.  start_ring / end_ring: n x line_num;
+   ori: n x 3 (startOrientation, endOrientation, orientationDiff; NaN where the first or last point is NaN, and (0, 0, 0)
+   for a sweep of fewer than 2 points, as a fresh ImageProjection holds — the host object keeps its previous scan's);
+   counts: n x 2 (segmented, outlier).  LINS_E_INVALID, before anything is written, for bad offsets, a NULL array, or a
+   model outside the limits of lins_lidar_model. */
+int lins_gpu_project_scans(lins_ctx* ctx, const lins_lidar_model* model, const lins_raw_desc* raw, lins_point* seg,
+                           uint8_t* ground_flag, uint32_t* col_ind, float* range, lins_point* outlier, int32_t* start_ring,
+                           int32_t* end_ring, float* ori /*n x 3*/, int32_t* counts /*n x 2*/);
+/* CUDA-event time of the last projection kernel (lins_gpu_project_scans), ms */
+int lins_gpu_project_ms(lins_ctx* ctx, float* ms);
+
 /* Split "Jacobian kernel" (SURVEY.md §8(d) unit U1): residual + Jacobian row + 29-scalar reduction over the
    resident batch given the correspondence IDs of iteration `iter` of each scan's current linearisation
    point. Used for the HBM-roofline measurement; results land in an internal n x 29 accumulator array. */

@@ -13,9 +13,9 @@ import subprocess
 
 import numpy as np
 
-from .ctypes_defs import (Batch, COV_SIZE, LinsBatchDesc, LinsFeatureParams, LinsMapReport, LinsParams, LinsPclDesc, LinsReport,
-                          LinsScanResult, LinsSeqBeginDesc, LinsSeqInitParams, LinsSeqParams, LinsSeqPclDesc, LinsSeqStepDesc, POINT_DTYPE,
-                          SCAN_RESULT_DTYPE, STATE_DIM, as_points, ptr)
+from .ctypes_defs import (Batch, COV_SIZE, LinsBatchDesc, LinsFeatureParams, LinsLidarModel, LinsMapReport, LinsParams, LinsPclDesc,
+                          LinsRawDesc, LinsReport, LinsScanResult, LinsSeqBeginDesc, LinsSeqInitParams, LinsSeqParams, LinsSeqPclDesc,
+                          LinsSeqStepDesc, POINT_DTYPE, SCAN_RESULT_DTYPE, STATE_DIM, as_points, make_points, ptr)
 
 _PKG = os.path.dirname(os.path.abspath(__file__))
 _ROOT = os.path.dirname(_PKG)
@@ -33,16 +33,18 @@ EXPORTS = [
     "lins_gpu_batch_upload_stats", "lins_gpu_seq_begin", "lins_gpu_seq_step", "lins_gpu_seq_download",
     "lins_gpu_seq_phase_ms", "lins_gpu_seq_download_ieskf", "lins_gpu_seq_download_maps", "lins_gpu_download_indices",
     "lins_gpu_seq_open", "lins_gpu_seq_restart", "lins_gpu_seq_step_ex", "lins_gpu_seq_download_init",
-    "lins_gpu_extract_features", "lins_gpu_extract_ms", "lins_gpu_seq_step_pcl",
+    "lins_gpu_extract_features", "lins_gpu_extract_ms", "lins_gpu_seq_step_pcl", "lins_gpu_project_scans", "lins_gpu_project_ms",
 ]
 
 NVCC_ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]  # H100 (Hopper)
 NVCC_COMMON = NVCC_ARCH + ["-lineinfo", "-O3", "-std=c++17", "-Xcompiler", "-fPIC"]
 # translation units and their extra flags: lins_gpu.cu (the fused kernel and most of the C-ABI), lins_upload.cu (batch
-# upload), lins_map.cu (row F2's host side), lins_seq.cu (sequence mode), lins_features.cu (feature extraction) — all bit-exact, so no multiply-add contraction: the association and the map
+# upload), lins_map.cu (row F2's host side), lins_seq.cu (sequence mode), lins_features.cu (feature extraction),
+# lins_projection.cu (image projection) — all bit-exact, so no multiply-add contraction: the association and the map
 # fits depend on it — and lins_jacobian.cu (the tolerance-checked split Jacobian kernel: contraction allowed)
 UNITS = [("lins_gpu.cu", ["-fmad=false"]), ("lins_upload.cu", ["-fmad=false"]), ("lins_map.cu", ["-fmad=false"]),
-         ("lins_seq.cu", ["-fmad=false"]), ("lins_features.cu", ["-fmad=false"]), ("lins_jacobian.cu", [])]
+         ("lins_seq.cu", ["-fmad=false"]), ("lins_features.cu", ["-fmad=false"]), ("lins_projection.cu", ["-fmad=false"]),
+         ("lins_jacobian.cu", [])]
 NVCC_FLAGS = NVCC_COMMON + ["-fmad=false", "-shared"]  # (what tools/ scripts print)
 
 
@@ -124,6 +126,9 @@ def lib():
             L.lins_gpu_extract_features.argtypes = [vp, C.POINTER(LinsFeatureParams), C.POINTER(LinsPclDesc)] + [vp] * 6
             L.lins_gpu_extract_ms.argtypes = [vp, vp]
             L.lins_gpu_seq_step_pcl.argtypes = [vp, C.POINTER(LinsSeqPclDesc), C.POINTER(LinsFeatureParams), vp]
+        if hasattr(L, "lins_gpu_project_scans"):
+            L.lins_gpu_project_scans.argtypes = [vp, C.POINTER(LinsLidarModel), C.POINTER(LinsRawDesc)] + [vp] * 9
+            L.lins_gpu_project_ms.argtypes = [vp, vp]
         _LIB = L
     return _LIB
 
@@ -460,6 +465,63 @@ class LinsGpu:
         """CUDA-event time (ms) of the last extraction kernel."""
         ms = np.zeros(1, np.float32)
         self._ck(self.L.lins_gpu_extract_ms(self.h, ptr(ms)))
+        return float(ms[0])
+
+    @staticmethod
+    def _raw_desc(sweeps, point_format, keep):
+        """LinsRawDesc of a list of raw sweeps (POINT_DTYPE arrays, or (m x 3 / m x 4) float32 x, y, z[, intensity]);
+        point_format 1 sends them as packed 16-B records.  The arrays it points at are added to `keep`."""
+        n = len(sweeps)
+
+        def points(s):
+            a = np.asarray(s)
+            if a.dtype == POINT_DTYPE:
+                return as_points(a)
+            a = np.asarray(a, np.float32).reshape(len(a), -1)
+            return make_points(a[:, :3], a[:, 3] if a.shape[1] > 3 else np.zeros(len(a), np.float32))
+
+        pts = [points(s) for s in sweeps]
+        off = np.zeros(n + 1, np.int32)
+        off[1:] = np.cumsum([len(a) for a in pts])
+        cloud = np.ascontiguousarray(np.concatenate(pts)) if n else np.zeros(0, POINT_DTYPE)
+        if point_format == 1:
+            cloud = np.ascontiguousarray(np.stack([cloud["x"], cloud["y"], cloud["z"], cloud["intensity"]], 1).astype(np.float32))
+        keep.update(cloud=cloud, cloud_off=off)
+        d = LinsRawDesc()
+        d.n_scans, d.point_format = n, int(point_format)
+        d.cloud, d.cloud_off = cloud.ctypes.data, off.ctypes.data
+        return d
+
+    def project_scans(self, sweeps, model=None, point_format=0):
+        """Image projection of raw sweeps on the device (lins_gpu_project_scans).  Returns one dict per sweep in the form
+        extract_features takes: seg (m x 4 float32 x, y, z, intensity), ground, col, range, start_ring, end_ring, ori (3),
+        plus outlier (k x 4)."""
+        model = model or LinsLidarModel.vlp16()
+        keep = {}
+        d = self._raw_desc(sweeps, point_format, keep)
+        n, total, L = d.n_scans, int(keep["cloud_off"][-1]), model.line_num
+        rec = np.float32 if point_format == 1 else POINT_DTYPE
+        shape = (max(total, 1), 4) if point_format == 1 else max(total, 1)
+        seg, outl = np.zeros(shape, rec), np.zeros(shape, rec)
+        ground, col, rng = np.zeros(max(total, 1), np.uint8), np.zeros(max(total, 1), np.uint32), np.zeros(max(total, 1), np.float32)
+        sr, er = np.zeros((max(n, 1), max(L, 1)), np.int32), np.zeros((max(n, 1), max(L, 1)), np.int32)
+        ori, counts = np.zeros((max(n, 1), 3), np.float32), np.zeros((max(n, 1), 2), np.int32)
+        self._ck(self.L.lins_gpu_project_scans(self.h, C.byref(model), C.byref(d), ptr(seg), ptr(ground), ptr(col), ptr(rng), ptr(outl),
+                                               ptr(sr), ptr(er), ptr(ori), ptr(counts)))
+        x4 = (lambda a: a.astype(np.float32)) if point_format == 1 else (  # noqa: E731
+            lambda a: np.stack([a["x"], a["y"], a["z"], a["intensity"]], 1).astype(np.float32).reshape(-1, 4))
+        off = keep["cloud_off"]
+        res = []
+        for i in range(n):
+            o, m, k = off[i], counts[i, 0], counts[i, 1]
+            res.append(dict(seg=x4(seg[o: o + m]), ground=ground[o: o + m].copy(), col=col[o: o + m].copy(), range=rng[o: o + m].copy(),
+                            start_ring=sr[i].copy(), end_ring=er[i].copy(), ori=ori[i].copy(), outlier=x4(outl[o: o + k])))
+        return res
+
+    def project_ms(self):
+        """CUDA-event time (ms) of the last projection kernel."""
+        ms = np.zeros(1, np.float32)
+        self._ck(self.L.lins_gpu_project_ms(self.h, ptr(ms)))
         return float(ms[0])
 
     def seq_step_pcl(self, step, fp=None, scan_imu=None, line_num=16):

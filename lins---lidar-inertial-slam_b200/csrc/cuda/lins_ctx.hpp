@@ -143,6 +143,37 @@ struct FeatState {
   ~FeatState() { for (cudaEvent_t e : ev) if (e) cudaEventDestroy(e); }
 };
 
+// Image projection (lins_projection.cu): the uploaded raw sweeps (up.qs, CSR in up.qs_off), each resident CTA's range-image
+// scratch (line_num x scan_num entries: winning point, range, ground, label, out-edges, owner counts, owner row extents),
+// the projected clouds and per-point cloud_info at the raw offsets, ring indices (n x 2 x line_num: start, end),
+// orientations (n x 3) and counts (n x 2: segmented, outlier); for lins_gpu_project_scans' read-back, the clouds packed
+// to dense offsets (d*) and their pinned staging (h_*)
+struct ProjState {
+  Resident up;
+  Buf<int> idx, lab, cnt, rlo, rhi;
+  Buf<float> rng;
+  Buf<unsigned char> gnd, edg;
+  Buf<float4> seg, outl;
+  Buf<unsigned char> ground;
+  Buf<unsigned> col;
+  Buf<float> range, ori;
+  Buf<int> ring, counts;
+  Buf<int, kPinned> h_counts;
+  Buf<float4> dseg, doutl;
+  Buf<unsigned char> dground;
+  Buf<unsigned> dcol;
+  Buf<float> drange;
+  Buf<int> doff;
+  Buf<float4, kPinned> h_seg, h_outl;
+  Buf<unsigned char, kPinned> h_ground;
+  Buf<unsigned, kPinned> h_col;
+  Buf<float, kPinned> h_range, h_ori;
+  Buf<int, kPinned> h_doff, h_ring;
+  cudaEvent_t ev[2] = {nullptr, nullptr};  // around the last projection kernel (lins_gpu_project_ms)
+  bool ev_valid = false;
+  ~ProjState() { for (cudaEvent_t e : ev) if (e) cudaEventDestroy(e); }
+};
+
 }  // namespace lins_capi
 
 struct lins_ctx {
@@ -164,6 +195,7 @@ struct lins_ctx {
   lins_capi::Resident single;  // lins_gpu_ieskf / associate / estimate_transform (n = 1)
   lins_capi::SeqState seq;     // lins_gpu_seq_*
   lins_capi::FeatState feat;   // lins_gpu_extract_features, lins_gpu_seq_step_pcl
+  lins_capi::ProjState proj;   // lins_gpu_project_scans
   // the single-scan map: "last" clouds (walks + tripods) and the clouds the 1-NN index was built on
   Buf<float4> map_s, map_c, tree_s, tree_c;
   Buf<int> map_off;  // 4 x 2 ints: [0,ns][0,nc][0,tns][0,tnc]
@@ -303,5 +335,8 @@ int icp_loop(lins_ctx* ctx, Resident& r, lins_dev::BatchView bv, double* pose, l
 int transform_to_end_csr(lins_ctx* ctx, float4* pts, const int* off, int n_units, const double* lin, const unsigned char* run);
 // lins_features.cu: validate, upload and extract the scans of d into ctx->feat; reads the counts back (one synchronisation)
 int features_run(lins_ctx* ctx, const lins_feature_params* fp, const lins_pcl_desc* d);
+// lins_projection.cu: validate the model and the sweeps of d, upload them and queue their projection into ctx->proj (no
+// synchronisation)
+int projection_run(lins_ctx* ctx, const lins_lidar_model* m, const lins_raw_desc* d);
 
 }  // namespace lins_capi

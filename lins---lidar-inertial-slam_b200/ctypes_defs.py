@@ -169,6 +169,30 @@ class LinsSeqPclDesc(C.Structure):
 FEAT_RING_CAP = 2048  # LINS_FEAT_RING_CAP
 
 
+class LinsLidarModel(C.Structure):
+    """lins_lidar_model: the lidar geometry image projection reads (csrc/host/cloud.hpp LidarModel)."""
+    _fields_ = [("line_num", C.c_int32), ("scan_num", C.c_int32), ("ang_res_x", C.c_float), ("ang_res_y", C.c_float),
+                ("ang_bottom", C.c_float), ("ground_scan_ind", C.c_int32)]
+
+    # (the C++ LidarModel's constants are float expressions: evaluated in float32 here too)
+    @classmethod
+    def vlp16(cls):
+        """The reference's hard-wired VLP-16 (parameters.h:82-92)."""
+        f = np.float32
+        return cls(16, 1800, f(0.2), f(2.0), f(15.0) + f(0.1), 5)
+
+    @classmethod
+    def dense64(cls):
+        """The 64 x 1024 stress shape (LidarModel::dense64)."""
+        f = np.float32
+        return cls(64, 1024, f(360.0) / f(1024.0), f(45.0) / f(63.0), f(22.5) + f(0.1), 24)
+
+
+class LinsRawDesc(C.Structure):
+    """lins_raw_desc: n raw sweeps, CSR."""
+    _fields_ = [("n_scans", C.c_int32), ("cloud", C.c_void_p), ("cloud_off", C.c_void_p), ("point_format", C.c_int32)]
+
+
 class LinsSeqStepDesc(C.Structure):
     _fields_ = [
         ("n_seq", C.c_int32),

@@ -540,6 +540,56 @@ double lins_features_host_bench(const lins_pcl_desc* d, int threads, int reps) {
   return std::chrono::duration<double>(std::chrono::steady_clock::now() - t0).count();
 }
 
+static LidarModel model_of(const lins_lidar_model* m) {
+  LidarModel lm;
+  lm.line_num = m->line_num; lm.scan_num = m->scan_num; lm.ang_res_x = m->ang_res_x; lm.ang_res_y = m->ang_res_y;
+  lm.ang_bottom = m->ang_bottom; lm.ground_scan_ind = m->ground_scan_ind;
+  return lm;
+}
+
+// ImageProjection::process (csrc/host/image_projection.hpp) of one raw sweep on a fresh object with the given model: the
+// host side of lins_gpu_project_scans.  seg / ground / col / range / outlier hold up to max(n, 1) entries; counts:
+// segmented, outlier.
+int lins_projection_host(const lins_point* raw, int n, const lins_lidar_model* m, lins_point* seg, uint8_t* ground, uint32_t* col,
+                         float* range, lins_point* outlier, int32_t* start_ring, int32_t* end_ring, float* ori3, int32_t* counts) {
+  const LidarModel lm = model_of(m);
+  Cloud in;
+  in.points.assign(raw, raw + n);
+  ImageProjection ip(lm);
+  ip.process(in);
+  const size_t ns = ip.segmentedCloud.size(), no = ip.outlierCloud.size();
+  counts[0] = (int32_t)ns; counts[1] = (int32_t)no;
+  std::memcpy(seg, ip.segmentedCloud.points.data(), sizeof(lins_point) * ns);
+  std::memcpy(outlier, ip.outlierCloud.points.data(), sizeof(lins_point) * no);
+  for (size_t i = 0; i < ns; ++i) { ground[i] = ip.segMsg.segmentedCloudGroundFlag[i]; col[i] = ip.segMsg.segmentedCloudColInd[i]; range[i] = ip.segMsg.segmentedCloudRange[i]; }
+  for (int i = 0; i < lm.line_num; ++i) { start_ring[i] = ip.segMsg.startRingIndex[i]; end_ring[i] = ip.segMsg.endRingIndex[i]; }
+  ori3[0] = ip.segMsg.startOrientation; ori3[1] = ip.segMsg.endOrientation; ori3[2] = ip.segMsg.orientationDiff;
+  return 0;
+}
+
+// Wall seconds of `reps` passes of ImageProjection::process over every sweep of d with model m, the sweeps handed out to
+// `threads` std::threads one at a time (one ImageProjection per thread, as a node keeps one): the host throughput
+// lins_gpu_project_scans replaces.  Inputs are converted to Clouds before the clock starts.
+double lins_projection_host_bench(const lins_raw_desc* d, const lins_lidar_model* m, int threads, int reps) {
+  const int n = d->n_scans;
+  std::vector<Cloud> clouds(n);
+  for (int k = 0; k < n; ++k) {
+    clouds[k].points.assign(d->cloud + d->cloud_off[k], d->cloud + d->cloud_off[k + 1]);
+  }
+  const LidarModel lm = model_of(m);
+  std::atomic<long> next(0);
+  const long total = (long)n * std::max(reps, 1);
+  auto work = [&]() {
+    ImageProjection ip(lm);
+    for (long i; (i = next.fetch_add(1)) < total;) ip.process(clouds[i % n]);
+  };
+  const auto t0 = std::chrono::steady_clock::now();
+  std::vector<std::thread> pool;
+  for (int t = 0; t < std::max(threads, 1); ++t) pool.emplace_back(work);
+  for (auto& t : pool) t.join();
+  return std::chrono::duration<double>(std::chrono::steady_clock::now() - t0).count();
+}
+
 // one simulated raw sweep of the seeded world (an input for lins_frontend_run): returns the number of points written
 int lins_synth_raw_sweep(const lins_synth_cfg* cfg, uint64_t seed, lins_point* out, int cap) {
   Rng rng(seed);

@@ -19,7 +19,7 @@ from .ctypes_defs import (Batch, COV_SIZE, LinsBatchDesc, LinsFeatureParams, Lin
 
 _PKG = os.path.dirname(os.path.abspath(__file__))
 _ROOT = os.path.dirname(_PKG)
-LIB_PATH = os.environ.get("LINS_GPU_LIB") or os.path.join(_PKG, "liblins_gpu.so")  # override only for A/B experiments
+LIB_PATH = os.path.join(_PKG, "liblins_gpu.so")
 CUDA_DIR = os.path.join(_PKG, "csrc", "cuda")
 
 # every symbol include/lins_gpu.h declares
@@ -45,28 +45,25 @@ NVCC_COMMON = NVCC_ARCH + ["-lineinfo", "-O3", "-std=c++17", "-Xcompiler", "-fPI
 UNITS = [("lins_gpu.cu", ["-fmad=false"]), ("lins_upload.cu", ["-fmad=false"]), ("lins_map.cu", ["-fmad=false"]),
          ("lins_seq.cu", ["-fmad=false"]), ("lins_features.cu", ["-fmad=false"]), ("lins_projection.cu", ["-fmad=false"]),
          ("lins_jacobian.cu", [])]
-NVCC_FLAGS = NVCC_COMMON + ["-fmad=false", "-shared"]  # (what tools/ scripts print)
 
 
-def build(force=False, verbose=False, out=None, extra=()):
+def build(force=False, verbose=False):
     """Compile csrc/cuda/*.cu -> liblins_gpu.so for sm_90a (nvcc cross-compiles without a GPU)."""
-    out = out or LIB_PATH
     # (this file too: a library built with other flags, e.g. for another architecture, is stale)
     deps = [os.path.join(CUDA_DIR, u) for u, _ in UNITS] + [os.path.join(_ROOT, "include", "lins_gpu.h"), os.path.abspath(__file__)]
     for d in (CUDA_DIR, os.path.join(os.path.dirname(CUDA_DIR), "host")):  # every header the translation units include
         deps += [os.path.join(d, f) for f in sorted(os.listdir(d)) if f.endswith((".cuh", ".hpp", ".h"))]
-    if not force and os.path.exists(out) and all(os.path.getmtime(out) >= os.path.getmtime(s) for s in deps):
-        return out
+    if not force and os.path.exists(LIB_PATH) and all(os.path.getmtime(LIB_PATH) >= os.path.getmtime(s) for s in deps):
+        return LIB_PATH
     objdir = os.path.join(_PKG, "build")
     os.makedirs(objdir, exist_ok=True)
-    tag = os.path.splitext(os.path.basename(out))[0]
     objs = []
     for unit, flags in UNITS:
-        obj = os.path.join(objdir, f"{tag}_{os.path.splitext(unit)[0]}.o")
-        subprocess.check_call(["nvcc"] + NVCC_COMMON + flags + list(extra) + (["-Xptxas", "-v"] if verbose else []) + ["-c", "-o", obj, os.path.join(CUDA_DIR, unit)])
+        obj = os.path.join(objdir, os.path.splitext(unit)[0] + ".o")
+        subprocess.check_call(["nvcc"] + NVCC_COMMON + flags + (["-Xptxas", "-v"] if verbose else []) + ["-c", "-o", obj, os.path.join(CUDA_DIR, unit)])
         objs.append(obj)
-    subprocess.check_call(["nvcc"] + NVCC_ARCH + ["-shared", "-o", out] + objs)
-    return out
+    subprocess.check_call(["nvcc"] + NVCC_ARCH + ["-shared", "-o", LIB_PATH] + objs)
+    return LIB_PATH
 
 
 _LIB = None
@@ -90,8 +87,7 @@ def lib():
         L.lins_gpu_associate.argtypes = [vp, vp, C.c_int, vp, C.c_int, f64p, C.c_int, i32p, i32p, f32p, f32p, u8p, u8p, f32p, f32p]
         L.lins_gpu_estimate_transform.argtypes = [vp, vp, C.c_int, vp, C.c_int, f64p, C.POINTER(C.c_int), C.POINTER(C.c_int)]
         L.lins_gpu_update_map.argtypes = [vp, vp, C.c_int, vp, C.c_int, f64p, C.POINTER(C.c_int)]
-        if hasattr(L, "lins_gpu_update_map_ex"):  # (absent from older A/B variant libraries selected through LINS_GPU_LIB)
-            L.lins_gpu_update_map_ex.argtypes = [vp, vp, C.c_int, vp, C.c_int, f64p, vp, vp, C.POINTER(C.c_int)]
+        L.lins_gpu_update_map_ex.argtypes = [vp, vp, C.c_int, vp, C.c_int, f64p, vp, vp, C.POINTER(C.c_int)]
         L.lins_gpu_batch_upload.argtypes = [vp, C.POINTER(LinsBatchDesc)]
         L.lins_gpu_batch_run.argtypes = [vp]
         L.lins_gpu_batch_download.argtypes = [vp, f64p, f64p, vp, vp]
@@ -107,8 +103,7 @@ def lib():
         L.lins_gpu_map_associate.argtypes = [vp, vp, C.c_int, vp, C.c_int, vp] + [vp] * 6
         L.lins_gpu_host_register.argtypes = [vp, C.c_size_t]
         L.lins_gpu_batch_download_indices.argtypes = [vp, vp, vp]
-        if hasattr(L, "lins_gpu_batch_upload_stats"):
-            L.lins_gpu_batch_upload_stats.argtypes = [vp, C.POINTER(C.c_int64), C.POINTER(C.c_int64)]
+        L.lins_gpu_batch_upload_stats.argtypes = [vp, C.POINTER(C.c_int64), C.POINTER(C.c_int64)]
         L.lins_gpu_host_unregister.argtypes = [vp]
         L.lins_gpu_seq_begin.argtypes = [vp, C.POINTER(LinsSeqParams), C.POINTER(LinsSeqBeginDesc)]
         L.lins_gpu_seq_step.argtypes = [vp, C.POINTER(LinsSeqStepDesc)]
@@ -117,18 +112,15 @@ def lib():
         L.lins_gpu_seq_download_ieskf.argtypes = [vp] + [vp] * 7
         L.lins_gpu_seq_download_maps.argtypes = [vp] + [vp] * 6
         L.lins_gpu_download_indices.argtypes = [vp, vp, vp]
-        if hasattr(L, "lins_gpu_seq_open"):  # (absent from older libraries selected through LINS_GPU_LIB)
-            L.lins_gpu_seq_open.argtypes = [vp, C.POINTER(LinsSeqParams), C.POINTER(LinsSeqInitParams), C.c_int32]
-            L.lins_gpu_seq_restart.argtypes = [vp, vp]
-            L.lins_gpu_seq_step_ex.argtypes = [vp, C.POINTER(LinsSeqStepDesc), vp]
-            L.lins_gpu_seq_download_init.argtypes = [vp, vp, vp, vp, vp]
-        if hasattr(L, "lins_gpu_extract_features"):
-            L.lins_gpu_extract_features.argtypes = [vp, C.POINTER(LinsFeatureParams), C.POINTER(LinsPclDesc)] + [vp] * 6
-            L.lins_gpu_extract_ms.argtypes = [vp, vp]
-            L.lins_gpu_seq_step_pcl.argtypes = [vp, C.POINTER(LinsSeqPclDesc), C.POINTER(LinsFeatureParams), vp]
-        if hasattr(L, "lins_gpu_project_scans"):
-            L.lins_gpu_project_scans.argtypes = [vp, C.POINTER(LinsLidarModel), C.POINTER(LinsRawDesc)] + [vp] * 9
-            L.lins_gpu_project_ms.argtypes = [vp, vp]
+        L.lins_gpu_seq_open.argtypes = [vp, C.POINTER(LinsSeqParams), C.POINTER(LinsSeqInitParams), C.c_int32]
+        L.lins_gpu_seq_restart.argtypes = [vp, vp]
+        L.lins_gpu_seq_step_ex.argtypes = [vp, C.POINTER(LinsSeqStepDesc), vp]
+        L.lins_gpu_seq_download_init.argtypes = [vp, vp, vp, vp, vp]
+        L.lins_gpu_extract_features.argtypes = [vp, C.POINTER(LinsFeatureParams), C.POINTER(LinsPclDesc)] + [vp] * 6
+        L.lins_gpu_extract_ms.argtypes = [vp, vp]
+        L.lins_gpu_seq_step_pcl.argtypes = [vp, C.POINTER(LinsSeqPclDesc), C.POINTER(LinsFeatureParams), vp]
+        L.lins_gpu_project_scans.argtypes = [vp, C.POINTER(LinsLidarModel), C.POINTER(LinsRawDesc)] + [vp] * 9
+        L.lins_gpu_project_ms.argtypes = [vp, vp]
         _LIB = L
     return _LIB
 

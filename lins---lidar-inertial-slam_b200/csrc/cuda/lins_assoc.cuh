@@ -17,22 +17,9 @@ namespace lins_dev {
 // Probe-first search (lins_assoc_az.cuh: az_probe_window) is used for the closest-point search of a unit's FIRST pass
 // only: there every query is unseeded and the gate-wide window is much larger than the neighbourhood that holds the
 // answer.
-#ifndef LINS_SEARCH_DIAG
-#define LINS_SEARCH_DIAG 0
-#endif
-constexpr bool kSearchDiag = LINS_SEARCH_DIAG != 0;  // per-search cycle counters for tools/phase_profile.py
 // widest windows (azimuth bins per ring) a group of kGroupLanes lanes scans; wider ones go to a whole warp
-#ifndef LINS_GROUP_LANES
-#define LINS_GROUP_LANES 4
-#endif
-constexpr int kGroupLanes = LINS_GROUP_LANES;
-#ifndef LINS_THREAD_SCAN_BINS
-#define LINS_THREAD_SCAN_BINS 16
-#endif
-#ifndef LINS_THREAD_WALK_BINS
-#define LINS_THREAD_WALK_BINS 48
-#endif
-constexpr int kThreadScanBins = LINS_THREAD_SCAN_BINS, kThreadWalkBins = LINS_THREAD_WALK_BINS;
+constexpr int kGroupLanes = 4;
+constexpr int kThreadScanBins = 16, kThreadWalkBins = 48;
 
 // Certificate and pass counters of the phase timers (bv.timers, read by lins_gpu_debug_phase_cycles; tools/phase_profile.py
 // prints them).  Slots kCertSlots + k, k = 0..7, count the certificates of seeded queries: checked, accepted, failed because

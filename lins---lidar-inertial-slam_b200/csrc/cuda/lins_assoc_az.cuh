@@ -154,10 +154,7 @@ __device__ __forceinline__ void az_window(int nb, float aq, float th, int& blo, 
 __device__ __forceinline__ int slot_index(float w) { return __float_as_int(w) & 0x00ffffff; }
 __device__ __forceinline__ int slot_ring(float w) { return (int)((unsigned)__float_as_int(w) >> 24); }
 __device__ __forceinline__ int pack_window(int blo, int nbins) { return (blo << 16) | nbins; }
-#ifndef LINS_CERT_MARGIN
-#define LINS_CERT_MARGIN 0.1f
-#endif
-constexpr float kCertMargin = LINS_CERT_MARGIN;  // metres added to every search radius so that certificates have room
+constexpr float kCertMargin = 0.1f;  // metres added to every search radius so that certificates have room
 // bound used to build a window: (sqrt(U) + margin)^2
 __device__ __forceinline__ float widen(float U) { const float r = sqrtf(U) + kCertMargin; return r * r; }
 // slack (metres) of a search that found nothing within the gate: how far its best candidate (f32 squared-distance
@@ -456,14 +453,8 @@ __device__ __forceinline__ void az_prepare_walk(const AzIndex& ix, const float4 
 // ---- phase P4 (one WARP per query): the ring walks inside their windows -------------------------------------------
 // SURF: Ind2 over ring cr (window w2), Ind3 over rings cr-2, cr-1, cr+1, cr+2 (window w3).  Corner: Ind2 over rings
 // cr-2, cr-1, cr+1, cr+2 (window w2).  Forward candidates (original index j > c) count only while j < fwdBound.
-#ifndef LINS_WALK_IN_FLIGHT
-#define LINS_WALK_IN_FLIGHT 4
-#endif
-constexpr int kWalkInFlight = LINS_WALK_IN_FLIGHT;
-#ifndef LINS_GROUP_WALK_IN_FLIGHT
-#define LINS_GROUP_WALK_IN_FLIGHT 4
-#endif
-constexpr int kGroupWalkInFlight = LINS_GROUP_WALK_IN_FLIGHT;
+constexpr int kWalkInFlight = 4;
+constexpr int kGroupWalkInFlight = 4;
 struct WalkOut {  // per class: original index (-1 = none within the gate), slot, certificate bound, runner-up slot
   int i2, i3, pos2, pos3, run2, run3;
   float bound2, bound3;

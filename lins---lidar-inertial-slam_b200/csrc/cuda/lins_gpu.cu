@@ -9,12 +9,9 @@
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
-#include <limits>
 #include <new>
 #include <utility>
 
-#include "../host/math_utils.hpp"
-#include "../host/small_linalg.hpp"
 #include "lins_assoc.cuh"
 #include "lins_ctx.hpp"
 #include "lins_icp_step.cuh"
@@ -333,86 +330,6 @@ __global__ void __launch_bounds__(kThreads, kMinCtas) lins_ieskf_kernel(const __
   }
 }
 
-
-// Split "Jacobian kernel", shuffle-fold version (kept for A/B runs, LINS_JAC_VARIANT=2; the default is the tensor-core fold
-// of lins_jacobian.cu).  SURVEY.md §8(d) unit U1; rows A5-A9 form B given the correspondence IDs.
-// One warp per scan: streams the scan's queries (16 B each, coalesced) and IDs (12 / 8 B, coalesced), gathers
-// the 3 / 2 matched targets (16 B each), recomputes de-skew, residual, weight and Jacobian row.  Every trip of 32
-// queries is folded across the warp straight away (warp_fold_row: lane e owns sum e), so a lane carries ONE running
-// sum instead of 28 accumulators: few registers, many resident warps to hide the dependent ID -> target gathers; the
-// next trip's query and IDs are loaded before the current trip's arithmetic.  Nothing is staged in shared memory: with
-// >= 4096 resident scans the working set exceeds L2 and the kernel is bound by HBM traffic + f64 issue.
-template <int kJacThreads, int kJacMinBlocks>
-__global__ void __launch_bounds__(kJacThreads, kJacMinBlocks) lins_jacobian_kernel(const __grid_constant__ BatchView bv,
-                                                                                const __grid_constant__ KParams kp) {
-  const int lane = threadIdx.x & 31;
-  const int warps_per_grid = (gridDim.x * kJacThreads) >> 5;
-  for (int scan = (blockIdx.x * kJacThreads + threadIdx.x) >> 5; scan < bv.n_scans; scan += warps_per_grid) {
-    // per-scan constants (every lane computes the same values)
-    const double* st = bv.state_in + (size_t)scan * 20;
-    const double rn0 = st[0], rn1 = st[1], rn2 = st[2];
-    q4 q; q.x = st[6]; q.y = st[7]; q.z = st[8]; q.w = st[9];
-    const d3 phi = Quat2axis(q);
-    const m3 R = qtoR(q);
-    const int qs0 = bv.qs_off[scan], ns = bv.qs_off[scan + 1] - qs0;
-    const int qc0 = bv.qc_off[scan], nc = bv.qc_off[scan + 1] - qc0;
-    const float4* __restrict__ tgtS = bv.ts + bv.ts_off[scan];
-    const float4* __restrict__ tgtC = bv.tc + bv.tc_off[scan];
-    const int Ts = bv.ts_off[scan + 1] - bv.ts_off[scan], Tc = bv.tc_off[scan + 1] - bv.tc_off[scan];
-    const bool weighted = kp.iter0 >= kp.icp_freq;
-    double total = 0.0;  // lane e: running sum of entry e
-    int cs = 0, cc = 0;
-    auto fetch = [&](int i, float4& p, int& i1, int& i2, int& i3) {
-      p = make_float4(0.f, 0.f, 0.f, 0.f); i1 = -1; i2 = -1; i3 = -1;
-      if (i < ns) {
-        p = __ldg(bv.qs + qs0 + i);
-        const int* id = bv.ind_s + 3 * (size_t)(qs0 + i);
-        i1 = __ldg(id); i2 = __ldg(id + 1); i3 = __ldg(id + 2);
-      } else if (i < ns + nc) {
-        p = __ldg(bv.qc + qc0 + (i - ns));
-        const int* id = bv.ind_c + 2 * (size_t)(qc0 + (i - ns));
-        i1 = __ldg(id); i2 = __ldg(id + 1);
-      }
-    };
-    float4 pn; int n1, n2, n3;
-    fetch(lane, pn, n1, n2, n3);
-    for (int i0 = 0; i0 < ns + nc; i0 += 32) {
-      const int i = i0 + lane;
-      const float4 p = pn;
-      const int i1 = n1, i2 = n2, i3 = n3;
-      const bool surf = i < ns;
-      // gathers of this trip, then the next trip's streaming loads: both in flight during the arithmetic below
-      float4 t1 = make_float4(0.f, 0.f, 0.f, 0.f), t2 = t1, t3 = t1;
-      bool have = false;
-      if (surf) {
-        if (i2 >= 0 && i3 >= 0 && i1 >= 0 && i1 < Ts && i2 < Ts && i3 < Ts) { t1 = __ldg(&tgtS[i1]); t2 = __ldg(&tgtS[i2]); t3 = __ldg(&tgtS[i3]); have = true; }
-      } else if (i < ns + nc) {
-        if (i2 >= 0 && i1 >= 0 && i1 < Tc && i2 < Tc) { t1 = __ldg(&tgtC[i1]); t2 = __ldg(&tgtC[i2]); have = true; }
-      }
-      fetch(i + 32, pn, n1, n2, n3);
-      double g[6] = {0.0, 0.0, 0.0, 0.0, 0.0, 0.0}, r = 0.0;
-      bool ok = false;
-      if (have) {
-        // A2 de-skew
-        const float fi = p.w - (float)((int)p.w);
-        const double s = (1.f / kp.scan_period) * fi;
-        const q4 rq = axis2Quat(mk3(s * phi.x, s * phi.y, s * phi.z));
-        const d3 rp = qrot(rq, mk3(p.x, p.y, p.z));
-        float4 sel;
-        sel.x = (float)(rp.x + s * rn0); sel.y = (float)(rp.y + s * rn1); sel.z = (float)(rp.z + s * rn2); sel.w = p.w;
-        float4 coeff = make_float4(0.f, 0.f, 0.f, 0.f);
-        ok = surf ? plane_residual(sel, t1, t2, t3, weighted, coeff) : line_residual(sel, t1, t2, weighted, coeff);
-        if (ok) jacobian_row(p, coeff, R.m, kp.lidar_scale, g, r);
-      }
-      total += warp_fold_row(g, r);
-      cs += __popc(__ballot_sync(0xffffffffu, ok && surf));
-      cc += __popc(__ballot_sync(0xffffffffu, ok && !surf));
-    }
-    if (lane < kNAcc) bv.accum[(size_t)scan * 32 + lane] = total;
-    if (lane == 28) bv.accum[(size_t)scan * 32 + 28] = (double)cs;
-    if (lane == 29) bv.accum[(size_t)scan * 32 + 29] = (double)cc;
-  }
-}
 
 // F1: transformToEnd (StateEstimator.hpp:1083-1101).  The per-scan constants (block-wide, into shared memory) and the
 // per-point body, shared by the single-cloud kernel and the CSR kernel of sequence mode.
@@ -877,20 +794,11 @@ int lins_gpu_batch_jacobian_pass(lins_ctx* ctx, double* accum_out) {
   BatchView bv = view_of(r, false, false);
   bv.state_in = r.state_out.p;  // linearise at the updated state; IDs = the last iteration's
   KParams kp = make_kparams(ctx->prm, MODE_JACOBIAN, 1);
-  // default: lins_jacobian.cu (FP64 tensor-core fold, multiply-add contraction); LINS_JAC_VARIANT=2: the shuffle-fold
-  // kernel above (this TU, -fmad=false)
-  static const int variant = [] { const char* e = std::getenv("LINS_JAC_VARIANT"); return e ? std::atoi(e) : 0; }();
-  if (variant == 2) {
-    const int wpb = 128 / 32;
-    int grid = std::min((r.n + wpb - 1) / wpb, ctx->sm_count * 5);
-    if (grid < 1) grid = 1;
-    lins_jacobian_kernel<128, 5><<<grid, 128, 0, ctx->stream>>>(bv, kp);  // measured: 83 us per 5000 units (96 registers, 20 warps per SM)
-  } else {
-    const int P = lins_jacobian_parts(r.n, ctx->sm_count);
-    if (P > 1) { CK(r.jac_part.reserve((size_t)r.n * P * 32)); CK(r.jac_cnt.reserve((size_t)r.n)); }
-    const int e = lins_launch_jacobian_mma(&bv, &kp, r.n, ctx->sm_count, P, r.jac_part.p, r.jac_cnt.p, ctx->stream);
-    if (e != 0) return fail(ctx, LINS_E_CUDA, "jacobian kernel launch", (cudaError_t)e);
-  }
+  // lins_jacobian.cu: FP64 tensor-core fold, multiply-add contraction
+  const int P = lins_jacobian_parts(r.n, ctx->sm_count);
+  if (P > 1) { CK(r.jac_part.reserve((size_t)r.n * P * 32)); CK(r.jac_cnt.reserve((size_t)r.n)); }
+  const int e = lins_launch_jacobian_mma(&bv, &kp, r.n, ctx->sm_count, P, r.jac_part.p, r.jac_cnt.p, ctx->stream);
+  if (e != 0) return fail(ctx, LINS_E_CUDA, "jacobian kernel launch", (cudaError_t)e);
   CK(cudaGetLastError());
   ctx->launches += 1;
   if (accum_out) {
@@ -902,77 +810,6 @@ int lins_gpu_batch_jacobian_pass(lins_ctx* ctx, double* accum_out) {
   return LINS_OK;
 }
 
-// (A/B only, LINS_ICP_HOST_LOOP=1: the round-1 flow — one reduction launch, D2H and host 6x6 step per iteration)
-static int estimate_transform_host_loop(lins_ctx* ctx, const lins_point* surf_flat, int ns, const lins_point* corner_sharp,
-                                int nc, double* pose_io, int* iters_out, int* converged_out) {
-  if (!ctx) return LINS_E_INVALID;
-  if (!pose_io) return fail(ctx, LINS_E_INVALID, "null pose");
-  CK(cudaSetDevice(ctx->device));
-  using namespace lins;
-  V3D t(pose_io[0], pose_io[1], pose_io[2]);
-  Q4D q(pose_io[6], pose_io[3], pose_io[4], pose_io[5]);
-  double lin[19];
-  std::memset(lin, 0, sizeof(lin));
-  linalg::Mat<6> matP{};
-  bool conv = false;
-  int it = 0;
-  Resident& r = ctx->single;
-  for (int iter = 0; iter < ctx->prm.num_iter; ++iter) {
-    it = iter + 1;
-    lin[0] = t.x(); lin[1] = t.y(); lin[2] = t.z();
-    lin[6] = q.x(); lin[7] = q.y(); lin[8] = q.z(); lin[9] = q.w();
-    int rc = stage_single(ctx, surf_flat, ns, corner_sharp, nc, lin, nullptr, false);
-    if (rc != LINS_OK) return rc;
-    BatchView bv = single_view(ctx, false);
-    rc = launch(ctx, r, bv, make_kparams(ctx->prm, MODE_ICP_REDUCE, iter));
-    if (rc != LINS_OK) return rc;
-    CK(r.h_accum.reserve(32));
-    CK(cudaMemcpyAsync(r.h_accum.p, r.accum.p, sizeof(double) * 32, cudaMemcpyDeviceToHost, ctx->stream));
-    CK(cudaStreamSynchronize(ctx->stream));
-    const double* a = r.h_accum.p;
-    if (ctx->verbose) { std::fprintf(stderr, "[lins_gpu] icp iter %d:", iter); for (int k = 0; k < 30; ++k) std::fprintf(stderr, " %.6g", a[k]); std::fprintf(stderr, "\n"); }
-    if (a[28] < 10) continue;  // "Insufficient matched surfs..." (:1175-1178)
-    if (a[29] < 5) continue;   // "Insufficient matched corners..." (:1181-1184)
-    linalg::Mat<6> JTJ;
-    linalg::Vec<6> JTb;
-    int k = 0;
-    for (int i = 0; i < 6; ++i) for (int j = i; j < 6; ++j) { JTJ[i][j] = a[k]; JTJ[j][i] = a[k]; ++k; }
-    for (int i = 0; i < 6; ++i) JTb[i] = a[21 + i];
-    linalg::Vec<6> x = linalg::colPivQrSolve<6>(JTJ, JTb);
-    if (ctx->verbose) std::fprintf(stderr, "[lins_gpu] icp iter %d x (before projection): %.12g %.12g %.12g %.12g %.12g %.12g\n", iter, x[0], x[1], x[2], x[3], x[4], x[5]);
-    bool isDegenerate = false;
-    if (iter == 0) {  // :1269-1296
-      linalg::Vec<6> matE;
-      linalg::Mat<6> matV, matV2, Vinv;
-      linalg::symmetricEigen<6>(JTJ, matE, matV);
-      if (ctx->verbose) std::fprintf(stderr, "[lins_gpu] icp E: %.9g %.9g %.9g %.9g %.9g %.9g\n", matE[0], matE[1], matE[2], matE[3], matE[4], matE[5]);
-      matV2 = matV;
-      for (int i = 0; i < 6; ++i) {
-        if (matE[i] < 10.) { for (int j = 0; j < 6; ++j) matV2[i][j] = 0; isDegenerate = true; }
-        else break;
-      }
-      if (!linalg::inverse<6>(matV, Vinv)) for (auto& row : Vinv) for (auto& e : row) e = std::numeric_limits<double>::quiet_NaN();
-      for (int i = 0; i < 6; ++i) for (int j = 0; j < 6; ++j) { double sacc = 0; for (int m = 0; m < 6; ++m) sacc += Vinv[i][m] * matV2[m][j]; matP[i][j] = sacc; }
-    }
-    if (ctx->verbose) std::fprintf(stderr, "[lins_gpu] icp iter %d degenerate %d\n", iter, (int)isDegenerate);
-    if (isDegenerate) {
-      linalg::Vec<6> x2 = x;
-      for (int i = 0; i < 6; ++i) { double sacc = 0; for (int j = 0; j < 6; ++j) sacc += matP[i][j] * x2[j]; x[i] = sacc; }
-    }
-    Q4D dq = math_utils::rpy2Quat(V3D(x[0], x[1], x[2]));
-    q = (q * dq).normalized();
-    t = t + V3D(x[3], x[4], x[5]);
-    double deltaR = V3D(math_utils::rad2deg(x[0]), math_utils::rad2deg(x[1]), math_utils::rad2deg(x[2])).norm();
-    double deltaT = V3D(100 * x[3], 100 * x[4], 100 * x[5]).norm();
-    if (deltaR < 0.1 && deltaT < 0.1) { conv = true; break; }
-  }
-  pose_io[0] = t.x(); pose_io[1] = t.y(); pose_io[2] = t.z();
-  pose_io[3] = q.x(); pose_io[4] = q.y(); pose_io[5] = q.z(); pose_io[6] = q.w();
-  if (iters_out) *iters_out = it;
-  if (converged_out) *converged_out = conv ? 1 : 0;
-  return LINS_OK;
-}
-
 // ≙ estimateTransform (StateEstimator.hpp:1163-1196): the association + J^T J / J^T b reduction of every
 // Gauss-Newton step runs on device (MODE_ICP_REDUCE), and so do the 6x6 solve / degeneracy projection / pose update of
 // calculateTransformation (:1260-1320): lins_icp_step.cuh.
@@ -981,7 +818,6 @@ int lins_gpu_estimate_transform(lins_ctx* ctx, const lins_point* surf_flat, int 
   if (!ctx) return LINS_E_INVALID;
   if (!pose_io) return fail(ctx, LINS_E_INVALID, "null pose");
   CK(cudaSetDevice(ctx->device));
-  if (std::getenv("LINS_ICP_HOST_LOOP")) return estimate_transform_host_loop(ctx, surf_flat, ns, corner_sharp, nc, pose_io, iters_out, converged_out);
   // queries + initial pose are staged ONCE, then the loop runs on the device (icp_loop).  One D2H + one synchronisation
   // at the end.
   double lin[19];

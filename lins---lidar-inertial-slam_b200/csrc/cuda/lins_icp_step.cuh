@@ -8,7 +8,6 @@
 #pragma once
 #include "lins_device_math.cuh"
 #include "lins_kernels.cuh"  // IcpState
-#include <cstdio>
 
 namespace lins_dev {
 
@@ -148,9 +147,6 @@ __global__ void lins_icp_step_kernel(const double* __restrict__ accum, double* _
       if (E[i] < 10.) { for (int j = 0; j < 6; ++j) V2[i][j] = 0; degenerate = true; }
       else break;
     }
-#ifdef LINS_ICP_DEBUG
-    printf("[icp dev] E: %.9g %.9g %.9g %.9g %.9g %.9g\n", E[0], E[1], E[2], E[3], E[4], E[5]);
-#endif
     if (!icp_inverse6(Vc, Vinv)) for (int i = 0; i < 6; ++i) for (int j = 0; j < 6; ++j) Vinv[i][j] = __longlong_as_double(0x7ff8000000000000ll);
     for (int i = 0; i < 6; ++i) for (int j = 0; j < 6; ++j) { double s = 0; for (int m = 0; m < 6; ++m) s += Vinv[i][m] * V2[m][j]; st->matP[i * 6 + j] = s; }
     st->pad = degenerate ? 1 : 0;
@@ -161,9 +157,6 @@ __global__ void lins_icp_step_kernel(const double* __restrict__ accum, double* _
     for (int i = 0; i < 6; ++i) x2[i] = x[i];
     for (int i = 0; i < 6; ++i) { double s = 0; for (int j = 0; j < 6; ++j) s += st->matP[i * 6 + j] * x2[j]; x[i] = s; }
   }
-#ifdef LINS_ICP_DEBUG
-  printf("[icp dev] iter %d acc:", iter); for (int i = 0; i < 30; ++i) printf(" %.9g", a[i]); printf("\n[icp dev] degenerate %d x: %.12g %.12g %.12g %.12g %.12g %.12g\n", (int)degenerate, x[0], x[1], x[2], x[3], x[4], x[5]);
-#endif
   // q <- (q * rpy2Quat(x[0:3])).normalized(), t += x[3:6]   (math_utils.h:131-149)
   const double hy = x[2] * 0.5, hp = x[1] * 0.5, hr = x[0] * 0.5;
   const double cy = cos(hy), sy = sin(hy), cp = cos(hp), sp = sin(hp), cr = cos(hr), sr = sin(hr);

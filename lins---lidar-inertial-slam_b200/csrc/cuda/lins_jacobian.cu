@@ -16,8 +16,6 @@
 //   * one warp per unit in a two-deep software pipeline: while trip k is computed, the gathers of trip k + 1 and the
 //     query / ID loads of trip k + 2 are in flight (a unit's ~16 trips are a serial chain: its memory latency, not the
 //     SM's issue rate, is what one warp per unit has to hide).
-#include <cstdlib>
-
 #include "lins_kernels.cuh"
 
 namespace lins_dev {
@@ -26,9 +24,7 @@ constexpr int kJacWarps = 8;            // warps per CTA
 constexpr int kJacRow = 12;             // doubles per staged row (8 used): 96-B stride -> conflict-free 8-B reads
 // resident CTAs per SM the register budget is set for.  Measured on an H100 SXM (400 W limit; 5000 units, 408 MB working
 // set): 1 98 us, 2 (128 registers, no spills, 16 warps per SM) 76.6 us, 3 (80 registers) 101 us
-#ifndef LINS_JAC_MIN_CTAS
-#define LINS_JAC_MIN_CTAS 2
-#endif
+constexpr int kJacMinCtas = 2;
 
 // sin / cos of a small angle (|x| < 0.125) to better than one ulp
 __device__ __forceinline__ void sincos_small(double x, double& sn, double& cs) {
@@ -40,7 +36,7 @@ __device__ __forceinline__ void sincos_small(double x, double& sn, double& cs) {
 // P = parts a unit is cut into (trips dealt round-robin to P warps): with one warp per unit and only a few units per warp the
 // grid's last round is nearly empty; cutting units keeps every warp busy to the end.  The parts' sums meet in part_acc and
 // the warp that arrives last adds them in part order (deterministic).
-__global__ void __launch_bounds__(kJacWarps * 32, LINS_JAC_MIN_CTAS) lins_jacobian_mma_kernel(const __grid_constant__ BatchView bv,
+__global__ void __launch_bounds__(kJacWarps * 32, kJacMinCtas) lins_jacobian_mma_kernel(const __grid_constant__ BatchView bv,
                                                                                              const __grid_constant__ KParams kp, int P,
                                                                                              double* __restrict__ part_acc, int* __restrict__ part_cnt) {
   __shared__ __align__(16) double stage[kJacWarps][32 * kJacRow];
@@ -66,9 +62,6 @@ __global__ void __launch_bounds__(kJacWarps * 32, LINS_JAC_MIN_CTAS) lins_jacobi
     const float4* __restrict__ tgtC = bv.tc + bv.tc_off[scan];
     const int Ts = bv.ts_off[scan + 1] - bv.ts_off[scan], Tc = bv.tc_off[scan + 1] - bv.tc_off[scan];
     double c0 = 0.0, c1 = 0.0;  // this lane's two entries of the 8 x 8 Gram matrix
-#ifdef LINS_JAC_FOLD_SHUFFLE
-    double shuffle_total = 0.0;
-#endif
     int cs = 0, cc = 0;
     auto fetch = [&](int i, float4& p, int& i1, int& i2, int& i3) {
       p = make_float4(0.f, 0.f, 0.f, 0.f); i1 = -1; i2 = -1; i3 = -1;
@@ -136,9 +129,6 @@ __global__ void __launch_bounds__(kJacWarps * 32, LINS_JAC_MIN_CTAS) lins_jacobi
       }
       // stage the row [g0..g5, r, 0] and fold the warp's 32 rows: C += G^T G, four queries per MMA.
       // A (8 x 4, row) and B (4 x 8, col) fragments of lane L are both G[4c + L % 4][L / 4].
-#ifdef LINS_JAC_FOLD_SHUFFLE
-      shuffle_total += warp_fold_row(g, r);
-#endif
       __syncwarp();
       double2* row = reinterpret_cast<double2*>(my + lane * kJacRow);
       row[0] = make_double2(g[0], g[1]); row[1] = make_double2(g[2], g[3]); row[2] = make_double2(g[4], g[5]); row[3] = make_double2(r, 0.0);
@@ -167,10 +157,6 @@ __global__ void __launch_bounds__(kJacWarps * 32, LINS_JAC_MIN_CTAS) lins_jacobi
         dst[e] = v;
       }
     }
-#ifdef LINS_JAC_FOLD_SHUFFLE
-    __syncwarp();
-    if (lane < kNAcc) dst[lane] = shuffle_total;
-#endif
     if (lane == 28) dst[28] = (double)cs;
     if (lane == 29) dst[29] = (double)cc;
     if (P > 1) {
@@ -195,14 +181,13 @@ __global__ void __launch_bounds__(kJacWarps * 32, LINS_JAC_MIN_CTAS) lins_jacobi
 
 // launched from lins_gpu.cu (lins_gpu_batch_jacobian_pass)
 // parts per unit.  The kernel is bound by its scattered 32-B sector gathers, not by the emptiness of the grid's last round,
-// and cutting units only adds per-unit set-up and spoils locality.  One part unless the batch cannot even fill the resident warps (LINS_JAC_PARTS: A/B).
+// and cutting units only adds per-unit set-up and spoils locality.  One part unless the batch cannot even fill the resident warps.
 extern "C" int lins_jacobian_parts(int n_units, int sm_count) {
   using namespace lins_dev;
   int per_sm = 1;
   if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, lins_jacobian_mma_kernel, kJacWarps * 32, 0) != cudaSuccess || per_sm < 1) per_sm = 1;
   const long warps = (long)sm_count * per_sm * kJacWarps;
-  long P = n_units > 0 && n_units < warps / 2 ? warps / n_units : 1;
-  if (const char* e = std::getenv("LINS_JAC_PARTS")) P = std::atoi(e);
+  const long P = n_units > 0 && n_units < warps / 2 ? warps / n_units : 1;
   return (int)(P < 1 ? 1 : (P > 4 ? 4 : P));
 }
 extern "C" int lins_launch_jacobian_mma(const lins_dev::BatchView* bv, const lins_dev::KParams* kp, int n_units, int sm_count, int P, double* part_acc,

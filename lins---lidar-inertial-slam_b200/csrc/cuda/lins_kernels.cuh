@@ -23,14 +23,8 @@
 
 namespace lins_dev {
 
-#ifndef LINS_THREADS
-#define LINS_THREADS 512
-#endif
-#ifndef LINS_MIN_CTAS
-#define LINS_MIN_CTAS 1
-#endif
-constexpr int kThreads = LINS_THREADS;   // threads per CTA (one unit per CTA); LINS_MIN_CTAS = resident CTAs per SM the register budget is set for
-constexpr int kMinCtas = LINS_MIN_CTAS;
+constexpr int kThreads = 512;   // threads per CTA
+constexpr int kMinCtas = 1;     // resident CTAs per SM the register budget is set for
 constexpr int kWarps = kThreads / 32;
 constexpr int kMaxSlots = 4;    // resident units per CTA (<= kWarps: warp w runs the serial tail of slot w)
 constexpr int kMaxRing = 128;   // rings outside [0, kMaxRing) or unsorted clouds take the brute-force search + sequential walk
@@ -358,48 +352,18 @@ __device__ __forceinline__ void jacobian_row_icp(const float4 kp, const float4 c
   g[3] = cx; g[4] = cy; g[5] = cz;
 }
 
-// Warp fold of one row per lane into the 28 sums of the information form: entries 0..20 = upper triangle of g g^T
-// (row-major), 21..26 = g r, 27 = r r.  Reduce-scatter: the 32 (28 + 4 zero) products of every lane are halved five
-// times, each half travelling to the partner lane that owns it, so 31 shuffles replace 28 x 5; lane e ends up with the
-// total of entry e.  Fixed tree => deterministic.  Lanes without a measurement pass g = 0, r = 0.
-__device__ __forceinline__ double warp_fold_row(const double* g, double r) {
-  const int lane = threadIdx.x & 31;
-  double p[32];
-  {
-    int k = 0;
-#pragma unroll
-    for (int a = 0; a < 6; ++a)
-#pragma unroll
-      for (int b = a; b < 6; ++b) p[k++] = g[a] * g[b];
-#pragma unroll
-    for (int a = 0; a < 6; ++a) p[21 + a] = g[a] * r;
-    p[27] = r * r;
-    p[28] = p[29] = p[30] = p[31] = 0.0;
-  }
-#pragma unroll
-  for (int h = 16; h >= 1; h >>= 1) {
-    const bool up = (lane & h) != 0;
-#pragma unroll
-    for (int i = 0; i < h; ++i) {
-      const double send = up ? p[i] : p[i + h];
-      const double keep = up ? p[i + h] : p[i];
-      p[i] = keep + __shfl_xor_sync(0xffffffffu, send, h);
-    }
-  }
-  return p[0];
-}
-
 __device__ __forceinline__ void dmma_8x8x4(double& c0, double& c1, double a, double b) {
   asm volatile("mma.sync.aligned.m8n8k4.row.col.f64.f64.f64.f64 {%0,%1}, {%2}, {%3}, {%0,%1};" : "+d"(c0), "+d"(c1) : "d"(a), "d"(b));
 }
 
-// The same 28 sums on the FP64 tensor cores: they are entries of the 8 x 8 Gram matrix C = G^T G of the warp's 32 rows
-// G = [g0..g5, r, 0], which eight mma.sync m8n8k4 (four rows each) accumulate.  The A (8 x 4, row) and B (4 x 8, col)
-// fragments of lane L are both G[4c + L % 4][L / 4], i.e. entries of other lanes' rows, so the rows pass through the warp's
-// 512 B of shared memory `st`: four rounds of 8 rows (two MMAs each).  A staged row is four 16-B chunks, chunk k of row j
-// at chunk 4 j + (k ^ (j >> 1)): the 8 writing lanes hit 8 different bank groups and the 32 reads of an MMA one 256-B
-// block.  Lane L writes C[L / 4][2 (L % 4) + {0, 1}] to dst[entry] where that is one of the 28 sums (same entry order as
-// warp_fold_row).  Fixed order => deterministic.  Lanes without a measurement pass g = 0, r = 0.
+// Warp fold of one row per lane into the 28 sums of the information form: entries 0..20 = upper triangle of g g^T
+// (row-major), 21..26 = g r, 27 = r r.  They are entries of the 8 x 8 Gram matrix C = G^T G of the warp's 32 rows
+// G = [g0..g5, r, 0], which eight FP64 tensor-core mma.sync m8n8k4 (four rows each) accumulate.  The A (8 x 4, row) and
+// B (4 x 8, col) fragments of lane L are both G[4c + L % 4][L / 4], i.e. entries of other lanes' rows, so the rows pass
+// through the warp's 512 B of shared memory `st`: four rounds of 8 rows (two MMAs each).  A staged row is four 16-B
+// chunks, chunk k of row j at chunk 4 j + (k ^ (j >> 1)): the 8 writing lanes hit 8 different bank groups and the 32
+// reads of an MMA one 256-B block.  Lane L writes C[L / 4][2 (L % 4) + {0, 1}] to dst[entry] where that is one of the
+// 28 sums.  Fixed order => deterministic.  Lanes without a measurement pass g = 0, r = 0.
 __device__ __forceinline__ void warp_fold_mma(const double* g, double r, double* st, double* dst) {
   const int lane = threadIdx.x & 31;
   const int wj = lane & 7, f = lane >> 2;

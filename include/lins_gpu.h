@@ -354,7 +354,8 @@ typedef struct lins_feature_params {
 int lins_gpu_extract_features(lins_ctx* ctx, const lins_feature_params* fp, const lins_pcl_desc* d, lins_point* surf_flat,
                               lins_point* corner_sharp, lins_point* surf_less_flat, lins_point* corner_less_sharp,
                               lins_point* undist, int32_t* counts /*n_scans x 4*/);
-/* CUDA-event time of the last extraction kernel (lins_gpu_extract_features or lins_gpu_seq_step_pcl), ms */
+/* CUDA-event time of the last extraction kernel (lins_gpu_extract_features, lins_gpu_seq_step_pcl or
+   lins_gpu_seq_step_raw), ms */
 int lins_gpu_extract_ms(lins_ctx* ctx, float* ms);
 
 /* one processPCL-shaped scan per sequence: the IMU rows as in lins_seq_step_desc, the scans as a lins_pcl_desc with
@@ -409,8 +410,32 @@ typedef struct lins_raw_desc {
 int lins_gpu_project_scans(lins_ctx* ctx, const lins_lidar_model* model, const lins_raw_desc* raw, lins_point* seg,
                            uint8_t* ground_flag, uint32_t* col_ind, float* range, lins_point* outlier, int32_t* start_ring,
                            int32_t* end_ring, float* ori /*n x 3*/, int32_t* counts /*n x 2*/);
-/* CUDA-event time of the last projection kernel (lins_gpu_project_scans), ms */
+/* CUDA-event time of the last projection kernel (lins_gpu_project_scans or lins_gpu_seq_step_raw), ms */
 int lins_gpu_project_ms(lins_ctx* ctx, float* ms);
+
+/* one raw sweep per sequence: the IMU rows as in lins_seq_step_desc, the sweeps as a lins_raw_desc with n_scans == n_seq
+   (a slot that is not present is neither projected nor extracted; its sweep may be empty) */
+typedef struct lins_seq_raw_desc {
+  int32_t n_seq;
+  const uint8_t* present;              /* NULL = all */
+  const double* imu; const int32_t* imu_off;
+  lins_raw_desc raw;
+} lins_seq_raw_desc;
+
+/* ≙ cloudHandler (image_projection_node.cpp:177-189, including copyPointCloud's pcl::removeNaNFromPointCloud) followed
+   by processPCL (StateEstimator.hpp:279-307, with the feature extraction of :619-827) for every present slot, all on the
+   device: nothing goes from device to host but the feature counts (one D2H + synchronisation).  Bit-identical to: drop
+   every point whose x, y or z is not finite (keeping the firing order), lins_gpu_project_scans, compact each segmented
+   cloud to dense CSR, lins_gpu_seq_step_pcl.  Unlike PCL, which skips the removal when the message claims is_dense, the
+   device always drops non-finite points (for an honest dense cloud the two agree).  All slots share one lidar model (a
+   run that mixes sensors uses a context per model, or lins_gpu_seq_step_pcl with padded rings).  May alternate with
+   lins_gpu_seq_step_ex and lins_gpu_seq_step_pcl in one run.  LINS_E_INVALID before anything changes for a bad
+   descriptor, model (as lins_gpu_project_scans), offsets, point format, NULL array or fp, or a NULL scan_imu while a
+   present slot is initialising; a segmented scan the extraction rejects (as lins_gpu_extract_features:
+   LINS_E_INVALID / LINS_E_TOOBIG) returns before the sequences change; any later failure ends the run.  Afterwards
+   lins_gpu_project_ms and lins_gpu_extract_ms report the step's two kernels. */
+int lins_gpu_seq_step_raw(lins_ctx* ctx, const lins_seq_raw_desc* step, const lins_lidar_model* model,
+                          const lins_feature_params* fp, const double* scan_imu /*S x 6 or NULL*/);
 
 /* Split "Jacobian kernel" (SURVEY.md §8(d) unit U1): residual + Jacobian row + 29-scalar reduction over the
    resident batch given the correspondence IDs of iteration `iter` of each scan's current linearisation

@@ -15,7 +15,7 @@ import numpy as np
 
 from .ctypes_defs import (Batch, COV_SIZE, LinsBatchDesc, LinsFeatureParams, LinsLidarModel, LinsMapReport, LinsParams, LinsPclDesc,
                           LinsRawDesc, LinsReport, LinsScanResult, LinsSeqBeginDesc, LinsSeqInitParams, LinsSeqParams, LinsSeqPclDesc,
-                          LinsSeqStepDesc, POINT_DTYPE, SCAN_RESULT_DTYPE, STATE_DIM, as_points, make_points, ptr)
+                          LinsSeqRawDesc, LinsSeqStepDesc, POINT_DTYPE, SCAN_RESULT_DTYPE, STATE_DIM, as_points, make_points, ptr)
 
 _PKG = os.path.dirname(os.path.abspath(__file__))
 _ROOT = os.path.dirname(_PKG)
@@ -34,6 +34,7 @@ EXPORTS = [
     "lins_gpu_seq_phase_ms", "lins_gpu_seq_download_ieskf", "lins_gpu_seq_download_maps", "lins_gpu_download_indices",
     "lins_gpu_seq_open", "lins_gpu_seq_restart", "lins_gpu_seq_step_ex", "lins_gpu_seq_download_init",
     "lins_gpu_extract_features", "lins_gpu_extract_ms", "lins_gpu_seq_step_pcl", "lins_gpu_project_scans", "lins_gpu_project_ms",
+    "lins_gpu_seq_step_raw",
 ]
 
 NVCC_ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]  # H100 (Hopper)
@@ -121,6 +122,7 @@ def lib():
         L.lins_gpu_seq_step_pcl.argtypes = [vp, C.POINTER(LinsSeqPclDesc), C.POINTER(LinsFeatureParams), vp]
         L.lins_gpu_project_scans.argtypes = [vp, C.POINTER(LinsLidarModel), C.POINTER(LinsRawDesc)] + [vp] * 9
         L.lins_gpu_project_ms.argtypes = [vp, vp]
+        L.lins_gpu_seq_step_raw.argtypes = [vp, C.POINTER(LinsSeqRawDesc), C.POINTER(LinsLidarModel), C.POINTER(LinsFeatureParams), vp]
         _LIB = L
     return _LIB
 
@@ -469,7 +471,8 @@ class LinsGpu:
             a = np.asarray(s)
             if a.dtype == POINT_DTYPE:
                 return as_points(a)
-            a = np.asarray(a, np.float32).reshape(len(a), -1)
+            a = np.asarray(a, np.float32)
+            a = a.reshape(len(a), -1) if a.size else a.reshape(0, 4)  # (an empty sweep)
             return make_points(a[:, :3], a[:, 3] if a.shape[1] > 3 else np.zeros(len(a), np.float32))
 
         pts = [points(s) for s in sweeps]
@@ -535,6 +538,28 @@ class LinsGpu:
             if len(si) != d.n_seq:
                 raise ValueError(f"scan_imu has {len(si)} rows, the step {d.n_seq}")
         self._ck(self.L.lins_gpu_seq_step_pcl(self.h, C.byref(d), C.byref(fp), ptr(si)))
+
+    def seq_step_raw(self, step, model=None, fp=None, scan_imu=None, point_format=0):
+        """Advance every present sequence by one raw sweep (lins_gpu_seq_step_raw: image projection with copyPointCloud's NaN
+        removal, feature extraction and the filter step on the device): `step` has imu + imu_off as in seq_step, sweeps (one
+        raw sweep per slot, as project_scans takes them; an absent slot's may be empty) and optionally present.  model: the
+        LinsLidarModel every slot shares (None = VLP-16)."""
+        keep = {"imu": np.ascontiguousarray(step["imu"], dtype=np.float64), "imu_off": np.ascontiguousarray(step["imu_off"], dtype=np.int32)}
+        d = LinsSeqRawDesc()
+        d.raw = self._raw_desc(step["sweeps"], point_format, keep)
+        d.n_seq = len(keep["imu_off"]) - 1
+        d.imu, d.imu_off = keep["imu"].ctypes.data, keep["imu_off"].ctypes.data
+        if step.get("present") is not None:
+            keep["present"] = np.ascontiguousarray(step["present"], dtype=np.uint8)
+            d.present = keep["present"].ctypes.data
+        model = model or LinsLidarModel.vlp16()
+        fp = fp or LinsFeatureParams.shipped()
+        si = None
+        if scan_imu is not None:
+            si = np.ascontiguousarray(scan_imu, dtype=np.float64).reshape(-1, 6)
+            if len(si) != d.n_seq:
+                raise ValueError(f"scan_imu has {len(si)} rows, the step {d.n_seq}")
+        self._ck(self.L.lins_gpu_seq_step_raw(self.h, C.byref(d), C.byref(model), C.byref(fp), ptr(si)))
 
     def seq_download(self, reports=False):
         """dict: global_state, filter_state (S x 19), filter_cov (S x 324), results (SCAN_RESULT_DTYPE), status (S) and,

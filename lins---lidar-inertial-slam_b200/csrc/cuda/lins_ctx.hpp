@@ -169,6 +169,8 @@ struct ProjState {
   Buf<unsigned, kPinned> h_col;
   Buf<float, kPinned> h_range, h_ori;
   Buf<int, kPinned> h_doff, h_ring;
+  Buf<unsigned char> present;              // lins_gpu_seq_step_raw's present flags (n)
+  Buf<unsigned char, kPinned> h_present;
   cudaEvent_t ev[2] = {nullptr, nullptr};  // around the last projection kernel (lins_gpu_project_ms)
   bool ev_valid = false;
   ~ProjState() { for (cudaEvent_t e : ev) if (e) cudaEventDestroy(e); }
@@ -194,8 +196,8 @@ struct lins_ctx {
   lins_capi::Resident batch;   // lins_gpu_batch_* working set
   lins_capi::Resident single;  // lins_gpu_ieskf / associate / estimate_transform (n = 1)
   lins_capi::SeqState seq;     // lins_gpu_seq_*
-  lins_capi::FeatState feat;   // lins_gpu_extract_features, lins_gpu_seq_step_pcl
-  lins_capi::ProjState proj;   // lins_gpu_project_scans
+  lins_capi::FeatState feat;   // lins_gpu_extract_features, lins_gpu_seq_step_pcl, lins_gpu_seq_step_raw
+  lins_capi::ProjState proj;   // lins_gpu_project_scans, lins_gpu_seq_step_raw
   // the single-scan map: "last" clouds (walks + tripods) and the clouds the 1-NN index was built on
   Buf<float4> map_s, map_c, tree_s, tree_c;
   Buf<int> map_off;  // 4 x 2 ints: [0,ns][0,nc][0,tns][0,tnc]
@@ -333,10 +335,24 @@ int fused_qtile(int max_q);
 size_t icp_state_bytes();
 int icp_loop(lins_ctx* ctx, Resident& r, lins_dev::BatchView bv, double* pose, lins_dev::IcpState* icp);
 int transform_to_end_csr(lins_ctx* ctx, float4* pts, const int* off, int n_units, const double* lin, const unsigned char* run);
+// device-resident input of one feature extraction: n scans of line_num rings; scan i's points are pts[off[i] ..
+// off[i] + count[count_stride * i]) (off[i] .. off[i + 1] when count is null), its per-point cloud_info at the same
+// offsets; ring: n x 2 x line_num (start, end), ori: n x 3; total = off[n], the length of the per-point outputs
+struct FeatInputs {
+  int n = 0, line_num = 0, total = 0;
+  const float4* pts = nullptr; const int* off = nullptr;
+  const int* count = nullptr; int count_stride = 0;
+  const unsigned char* ground = nullptr; const unsigned* col = nullptr; const float* range = nullptr;
+  const int* ring = nullptr; const float* ori = nullptr;
+};
 // lins_features.cu: validate, upload and extract the scans of d into ctx->feat; reads the counts back (one synchronisation)
 int features_run(lins_ctx* ctx, const lins_feature_params* fp, const lins_pcl_desc* d);
+// lins_features.cu: extract the scans of `in` into ctx->feat (clouds at the input offsets) and read the counts back (one
+// D2H + synchronisation; a scan's device-side status returns LINS_E_INVALID / LINS_E_TOOBIG)
+int features_launch(lins_ctx* ctx, const lins_feature_params* fp, const FeatInputs& in);
 // lins_projection.cu: validate the model and the sweeps of d, upload them and queue their projection into ctx->proj (no
-// synchronisation)
-int projection_run(lins_ctx* ctx, const lins_lidar_model* m, const lins_raw_desc* d);
+// synchronisation); drop_nonfinite: copyPointCloud's NaN removal first; present (host, n; null = all): a scan whose flag is
+// 0 is projected as an empty sweep
+int projection_run(lins_ctx* ctx, const lins_lidar_model* m, const lins_raw_desc* d, bool drop_nonfinite, const uint8_t* present);
 
 }  // namespace lins_capi

@@ -35,6 +35,7 @@ static_assert(kThreads * kSextantItems >= lins_feat::kRingCap / 6 + 2, "sextant 
 struct FeatArgs {
   int line_num;
   const float4* pts;  const int* off;
+  const int* count; int count_stride;  // scan i: [off[i], off[i] + count[count_stride * i]); null: [off[i], off[i + 1])
   const unsigned char* ground; const unsigned* col; const float* range;
   const int* ring;    // n x 2 x line_num: startRingIndex, endRingIndex
   const float* ori;   // n x 3: startOrientation, endOrientation, orientationDiff
@@ -79,7 +80,7 @@ __global__ void __launch_bounds__(kThreads) lins_features_kernel(const FeatArgs 
   __shared__ int s_half, s_bad, s_m, s_cnt[4];
 
   const int sc = blockIdx.x, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-  const int base = a.off[sc], np = a.off[sc + 1] - base;
+  const int base = a.off[sc], np = a.count ? a.count[(size_t)a.count_stride * sc] : a.off[sc + 1] - base;
   const int L = a.line_num;
   const int* rs = a.ring + (size_t)sc * 2 * L;
   const int* re = rs + L;
@@ -338,10 +339,11 @@ __global__ void __launch_bounds__(kThreads) lins_features_kernel(const FeatArgs 
 
 namespace lins_capi {
 
-// Validate the descriptor on the host (offsets, arrays, line_num), upload it, extract on the device and read the counts
-// back (one D2H and one stream synchronisation).  The device checks what needs the points (finite input, sextants inside
-// the cloud, ring spans) and reports it in the same read-back.  On return f.h_counts holds n x 5 (counts, status) and the
-// clouds are in f.out / f.und at the input offsets.
+// features_run: validate the descriptor on the host (offsets, arrays, line_num), upload it, then features_launch.
+// features_launch: extract on the device and read the counts back (one D2H and one stream synchronisation).  The device
+// checks what needs the points (finite input, sextants inside the cloud, ring spans) and reports it in the same
+// read-back.  On return f.h_counts holds n x 5 (counts, status) and the clouds are in f.out / f.und at the input offsets.
+// lins_gpu_seq_step_raw calls features_launch on the projection's output where it lies (ctx->proj, raw offsets).
 int features_run(lins_ctx* ctx, const lins_feature_params* fp, const lins_pcl_desc* d) {
   if (!fp || !d || d->n_scans < 0) return fail(ctx, LINS_E_INVALID, "bad feature extraction arguments");
   if (d->line_num < 1 || d->line_num > lins_feat::kMaxLines) return fail(ctx, LINS_E_INVALID, "line_num outside 1..128");
@@ -360,12 +362,9 @@ int features_run(lins_ctx* ctx, const lins_feature_params* fp, const lins_pcl_de
   const int32_t* offs[4] = {d->cloud_off, zeros.data(), zeros.data(), zeros.data()};
   int rc = upload_clouds(ctx, f.up, n, pts, offs, d->point_format);  // (synchronises the stream first)
   if (rc != LINS_OK) return rc;
-  CK(f.h_counts.reserve(5 * (size_t)n + 1));
-  if (n == 0) return LINS_OK;
+  if (n == 0) return features_launch(ctx, fp, FeatInputs());
   const size_t N = (size_t)total + 1;
   CK(f.ground.reserve(N)); CK(f.col.reserve(N)); CK(f.range.reserve(N)); CK(f.ring.reserve(2 * (size_t)n * L)); CK(f.ori.reserve(3 * (size_t)n));
-  CK(f.und.reserve(N)); for (auto& o : f.out) CK(o.reserve(N));
-  CK(f.counts.reserve(5 * (size_t)n)); CK(f.curv.reserve(N)); CK(f.sind.reserve(N)); CK(f.picked.reserve(N)); CK(f.label.reserve(N));
   f.h_ring.resize(2 * (size_t)n * L);
   for (int i = 0; i < n; ++i) {
     std::memcpy(&f.h_ring[(size_t)i * 2 * L], d->start_ring_index + (size_t)i * L, sizeof(int32_t) * L);
@@ -378,10 +377,25 @@ int features_run(lins_ctx* ctx, const lins_feature_params* fp, const lins_pcl_de
   }
   CK(cudaMemcpyAsync(f.ring.p, f.h_ring.data(), sizeof(int) * f.h_ring.size(), cudaMemcpyHostToDevice, ctx->stream));
   CK(cudaMemcpyAsync(f.ori.p, d->orientation, sizeof(float) * 3 * n, cudaMemcpyHostToDevice, ctx->stream));
+  FeatInputs in;
+  in.n = n; in.line_num = L; in.total = total;
+  in.pts = f.up.qs.p; in.off = f.up.qs_off.p;
+  in.ground = f.ground.p; in.col = f.col.p; in.range = f.range.p; in.ring = f.ring.p; in.ori = f.ori.p;
+  return features_launch(ctx, fp, in);
+}
+
+int features_launch(lins_ctx* ctx, const lins_feature_params* fp, const FeatInputs& in) {
+  FeatState& f = ctx->feat;
+  const int n = in.n;
+  CK(f.h_counts.reserve(5 * (size_t)n + 1));
+  if (n == 0) return LINS_OK;
+  const size_t N = (size_t)in.total + 1;
+  CK(f.und.reserve(N)); for (auto& o : f.out) CK(o.reserve(N));
+  CK(f.counts.reserve(5 * (size_t)n)); CK(f.curv.reserve(N)); CK(f.sind.reserve(N)); CK(f.picked.reserve(N)); CK(f.label.reserve(N));
   FeatArgs a;
-  a.line_num = L;
-  a.pts = f.up.qs.p; a.off = f.up.qs_off.p;
-  a.ground = f.ground.p; a.col = f.col.p; a.range = f.range.p; a.ring = f.ring.p; a.ori = f.ori.p;
+  a.line_num = in.line_num;
+  a.pts = in.pts; a.off = in.off; a.count = in.count; a.count_stride = in.count_stride;
+  a.ground = in.ground; a.col = in.col; a.range = in.range; a.ring = in.ring; a.ori = in.ori;
   const double y = fp->imu_lidar_extrinsic_angle * M_PI / 180.0;  // math_utils::deg2rad
   a.c = std::cos(y); a.s = std::sin(y);
   a.edge = fp->edge_threshold; a.surf = fp->surf_threshold; a.scan_period = ctx->prm.scan_period;

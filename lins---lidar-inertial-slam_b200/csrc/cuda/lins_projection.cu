@@ -15,6 +15,11 @@
 //    along the jump, wrap and down edges, until a round changes nothing;
 //  - feasibility from per-owner counts and row extents (the seed's own row is not counted), then cloudSegmentation's
 //    compaction in raster order with a block scan.
+// lins_gpu_seq_step_raw runs the kernel with drop_nonfinite: copyPointCloud's pcl::removeNaNFromPointCloud
+// (image_projection_node.cpp:172-177) without a compaction pass.  A non-finite point is never projected, and
+// findStartEndAngle reads the first, last and second-to-last finite points; the removal keeps the order, so the highest
+// index of a pixel is still the point the filtered sweep's overwrite would leave.  A scan whose present flag is 0 is
+// projected as an empty sweep.
 #include <cuda_runtime.h>
 
 #include <cfloat>
@@ -41,6 +46,8 @@ struct ProjArgs {
   float res_x, res_y, bottom;
   float sin_x, cos_x, sin_y, cos_y;  // sinf / cosf of segmentAlphaX / Y (host libm)
   const float4* pts; const int* off;
+  const unsigned char* present;  // n, or null = all (lins_gpu_seq_step_raw)
+  int drop_nonfinite;            // copyPointCloud's NaN removal (lins_gpu_seq_step_raw)
   // per-CTA scratch, L * S entries each
   int* idx; float* rng; signed char* gnd; int* lab; unsigned char* edg; int* cnt; int* rlo; int* rhi;
   // outputs at the raw offsets
@@ -54,9 +61,13 @@ __device__ __forceinline__ bool push_label(int* lab, int t, int v) {
   return lab[t] > v && atomicMin(&lab[t], v) > v;
 }
 
+// pcl::removeNaNFromPointCloud keeps a point iff its x, y and z are finite
+__device__ __forceinline__ bool finite_xyz(const float4& q) { return isfinite(q.x) && isfinite(q.y) && isfinite(q.z); }
+
 __global__ void __launch_bounds__(kThreads) lins_projection_kernel(const ProjArgs a) {
   using Scan = cub::BlockScan<unsigned long long, kThreads>;
   __shared__ typename Scan::TempStorage tmp;
+  __shared__ int s_fin[3];  // drop_nonfinite: the first, last and second-to-last finite point (-1: none)
   const unsigned FULL = 0xffffffffu;
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   const int L = a.L, S = a.S, P = L * S;
@@ -72,14 +83,39 @@ __global__ void __launch_bounds__(kThreads) lins_projection_kernel(const ProjArg
   auto blocked = [&](int p) { return gnd[p] == 1 || rng[p] == FLT_MAX; };
 
   for (int sc = blockIdx.x; sc < a.n; sc += gridDim.x) {
-    const int base = a.off[sc], np = a.off[sc + 1] - base;
+    const int base = a.off[sc], np = a.present && !a.present[sc] ? 0 : a.off[sc + 1] - base;
     const float4* pt = a.pts + base;
     for (int p = tid; p < P; p += kThreads) {
       idx[p] = -1; gnd[p] = 0; cnt[p] = 0; rlo[p] = INT_MAX; rhi[p] = -1;
     }
-    if (tid == 0) {  // findStartEndAngle; a scan of fewer than 2 points keeps a fresh cloud_info's zeros
+    if (a.drop_nonfinite) {  // the filtered sweep's ends: warp 0 from the front, warp 1 from the back, 32 points a round
+      if (warp == 0) {
+        int f = -1;
+        for (int i0 = 0; i0 < np && f < 0; i0 += 32) {
+          const unsigned b = __ballot_sync(FULL, i0 + lane < np && finite_xyz(pt[i0 + lane]));
+          if (b) f = i0 + __ffs(b) - 1;
+        }
+        if (lane == 0) s_fin[0] = f;
+      } else if (warp == 1) {
+        int l1 = -1, l2 = -1;
+        for (int i0 = np - 1; i0 >= 0 && l2 < 0; i0 -= 32) {
+          unsigned b = __ballot_sync(FULL, i0 - lane >= 0 && finite_xyz(pt[i0 - lane]));
+          for (; b && l2 < 0; b &= b - 1) {
+            const int k = i0 - (__ffs(b) - 1);
+            if (l1 < 0) l1 = k; else l2 = k;
+          }
+        }
+        if (lane == 0) { s_fin[1] = l1; s_fin[2] = l2; }
+      }
+      __syncthreads();
+    }
+    if (tid == 0) {  // findStartEndAngle; a scan of fewer than 2 (finite) points keeps a fresh cloud_info's zeros
       float o[3] = {0.f, 0.f, 0.f};
-      if (np >= 2) lins_proj::start_end_angle(pt[0].x, pt[0].y, pt[np - 1].y, pt[np - 2].x, o);
+      if (a.drop_nonfinite) {
+        if (s_fin[2] >= 0) lins_proj::start_end_angle(pt[s_fin[0]].x, pt[s_fin[0]].y, pt[s_fin[1]].y, pt[s_fin[2]].x, o);
+      } else if (np >= 2) {
+        lins_proj::start_end_angle(pt[0].x, pt[0].y, pt[np - 1].y, pt[np - 2].x, o);
+      }
       for (int k = 0; k < 3; ++k) a.ori[3 * sc + k] = o[k];
     }
     __syncthreads();
@@ -88,7 +124,8 @@ __global__ void __launch_bounds__(kThreads) lins_projection_kernel(const ProjArg
     for (int i = tid; i < np; i += kThreads) {
       const float4 q = pt[i];
       int r, c;
-      if (lins_proj::project(q.x, q.y, q.z, L, S, a.res_x, a.res_y, a.bottom, r, c)) atomicMax(&idx[r * S + c], i);
+      if ((!a.drop_nonfinite || finite_xyz(q)) && lins_proj::project(q.x, q.y, q.z, L, S, a.res_x, a.res_y, a.bottom, r, c))
+        atomicMax(&idx[r * S + c], i);
     }
     __syncthreads();
     for (int p = tid; p < P; p += kThreads) {
@@ -263,8 +300,8 @@ namespace lins_capi {
 
 // Validate the model and the descriptor on the host, upload the sweeps and queue the projection kernel (no
 // synchronisation).  Afterwards ctx->proj holds the projected clouds at the raw offsets, n x 2 x L ring indices, n x 3
-// orientations and n x 2 counts, all on the device.
-int projection_run(lins_ctx* ctx, const lins_lidar_model* m, const lins_raw_desc* d) {
+// orientations and n x 2 counts, all on the device.  drop_nonfinite / present: see ProjArgs.
+int projection_run(lins_ctx* ctx, const lins_lidar_model* m, const lins_raw_desc* d, bool drop_nonfinite, const uint8_t* present) {
   int rc = check_model(ctx, m);
   if (rc != LINS_OK) return rc;
   if (!d || d->n_scans < 0) return fail(ctx, LINS_E_INVALID, "bad raw sweep descriptor");
@@ -288,8 +325,15 @@ int projection_run(lins_ctx* ctx, const lins_lidar_model* m, const lins_raw_desc
   CK(pr.cnt.reserve(G)); CK(pr.rlo.reserve(G)); CK(pr.rhi.reserve(G));
   CK(pr.seg.reserve(N)); CK(pr.outl.reserve(N)); CK(pr.ground.reserve(N)); CK(pr.col.reserve(N)); CK(pr.range.reserve(N));
   CK(pr.ring.reserve(2 * (size_t)n * L)); CK(pr.ori.reserve(3 * (size_t)n)); CK(pr.counts.reserve(2 * (size_t)n));
+  if (present) {  // (upload_clouds synchronised the stream: the staging is free)
+    CK(pr.present.reserve(n)); CK(pr.h_present.reserve(n));
+    std::memcpy(pr.h_present.p, present, n);
+    CK(cudaMemcpyAsync(pr.present.p, pr.h_present.p, n, cudaMemcpyHostToDevice, ctx->stream));
+  }
   ProjArgs a;
   a.n = n; a.L = L; a.S = S; a.gsi = m->ground_scan_ind;
+  a.present = present ? pr.present.p : nullptr;
+  a.drop_nonfinite = drop_nonfinite;
   a.res_x = m->ang_res_x; a.res_y = m->ang_res_y; a.bottom = m->ang_bottom;
   const float ax = lins_proj::segment_alpha(m->ang_res_x), ay = lins_proj::segment_alpha(m->ang_res_y);
   a.sin_x = std::sin(ax); a.cos_x = std::cos(ax); a.sin_y = std::sin(ay); a.cos_y = std::cos(ay);  // (float overloads: sinf / cosf)
@@ -321,7 +365,7 @@ int lins_gpu_project_scans(lins_ctx* ctx, const lins_lidar_model* m, const lins_
     if (d->cloud_off && d->cloud_off[d->n_scans] > 0 && (!seg || !ground_flag || !col_ind || !range || !outlier))
       return fail(ctx, LINS_E_INVALID, "null output cloud");
   }
-  const int rc = projection_run(ctx, m, d);
+  const int rc = projection_run(ctx, m, d, false, nullptr);
   if (rc != LINS_OK) return rc;
   const int n = d->n_scans;
   if (n == 0) return LINS_OK;

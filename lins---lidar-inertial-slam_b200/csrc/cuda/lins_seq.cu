@@ -388,28 +388,36 @@ int lins_gpu_seq_step_ex(lins_ctx* ctx, const lins_seq_step_desc* d, const doubl
 
 int lins_gpu_seq_step(lins_ctx* ctx, const lins_seq_step_desc* d) { return lins_gpu_seq_step_ex(ctx, d, nullptr); }
 
-int lins_gpu_seq_step_pcl(lins_ctx* ctx, const lins_seq_pcl_desc* d, const lins_feature_params* fp, const double* scan_imu) {
-  if (!ctx) return LINS_E_INVALID;
+}  // extern "C"
+
+namespace {
+
+// the IMU rows and scan_imu of a step from sweeps / segmented scans, checked before anything runs
+int check_step_imu(lins_ctx* ctx, const uint8_t* present, const double* imu, const int32_t* imu_off, const double* scan_imu) {
   SeqState& q = ctx->seq;
-  if (q.n == 0) return fail(ctx, LINS_E_NOMAP, "lins_gpu_seq_begin has not been called");
-  if (!d || d->n_seq != q.n || d->pcl.n_scans != q.n) return fail(ctx, LINS_E_INVALID, "n_seq differs from the hand-over's");
-  const int n = q.n, N1 = n + 1;
-  if (d->imu_off) { const int rc = check_csr(ctx, d->imu_off, n, d->imu, "bad imu offsets / samples"); if (rc != LINS_OK) return rc; }
-  else if (d->imu) return fail(ctx, LINS_E_INVALID, "imu without imu_off");
+  const int n = q.n;
+  if (imu_off) { const int rc = check_csr(ctx, imu_off, n, imu, "bad imu offsets / samples"); if (rc != LINS_OK) return rc; }
+  else if (imu) return fail(ctx, LINS_E_INVALID, "imu without imu_off");
   if (!scan_imu)
     for (int s = 0; s < n; ++s)
-      if ((!d->present || d->present[s]) && q.fusion[s] != FUSION_RUNNING)
+      if ((!present || present[s]) && q.fusion[s] != FUSION_RUNNING)
         return fail(ctx, LINS_E_INVALID, "scan_imu is required while a present slot is initialising");
-  // extraction, validation of the scans and the counts' read-back: nothing of the sequences has changed yet
-  int rc = features_run(ctx, fp, &d->pcl);
-  if (rc != LINS_OK) return rc;
-  // the present slots' features -> the step's four clouds (q.up, lins_seq_step_desc order), dense in slot order
+  return LINS_OK;
+}
+
+// The rest of a step whose features were extracted into ctx->feat (scan s's clouds at f.out[k] + src_off[s], counts read
+// back): the present slots' features -> the step's four clouds (q.up, lins_seq_step_desc order), dense in slot order,
+// then the sequence step.  A failure ends the run.
+int step_from_features(lins_ctx* ctx, const uint8_t* pres, const double* imu, const int32_t* imu_off, const int32_t* src_off,
+                       const double* scan_imu) {
+  SeqState& q = ctx->seq;
+  const int n = q.n, N1 = n + 1;
   FeatState& f = ctx->feat;
   Resident& r = q.up;
   std::vector<int32_t> off(4 * (size_t)N1, 0);
   r.max_q = 0;
   for (int s = 0; s < n; ++s) {
-    const bool present = !d->present || d->present[s];
+    const bool present = !pres || pres[s];
     for (int k = 0; k < 4; ++k) off[k * N1 + s + 1] = off[k * N1 + s] + (present ? f.h_counts.p[5 * s + k] : 0);
     r.max_q = std::max(r.max_q, (off[s + 1] - off[s]) + (off[N1 + s + 1] - off[N1 + s]));
   }
@@ -423,23 +431,63 @@ int lins_gpu_seq_step_pcl(lins_ctx* ctx, const lins_seq_pcl_desc* d, const lins_
   for (int k = 0; k < 4; ++k)
     for (int s = 0; s < n; ++s) {
       const int len = off[k * N1 + s + 1] - off[k * N1 + s];
-      if (len) copies.push_back(SeqCopy{f.out[k].p + d->pcl.cloud_off[s], dst[k] + off[k * N1 + s], len, 0});
+      if (len) copies.push_back(SeqCopy{f.out[k].p + src_off[s], dst[k] + off[k * N1 + s], len, 0});
     }
   CK(f.copies.reserve(copies.size() + 1)); CK(f.h_copies.reserve(copies.size() + 1));
   std::copy(copies.begin(), copies.end(), f.h_copies.p);
   std::memcpy(r.h_off.p, off.data(), sizeof(int) * off.size());
   if (!copies.empty()) CK(cudaMemcpyAsync(f.copies.p, f.h_copies.p, sizeof(SeqCopy) * copies.size(), cudaMemcpyHostToDevice, ctx->stream));
   for (int k = 0; k < 4; ++k) CK(cudaMemcpyAsync(doff[k], r.h_off.p + (size_t)k * N1, sizeof(int) * N1, cudaMemcpyHostToDevice, ctx->stream));
-  rc = run_copies(ctx, f.copies.p, (int)copies.size());
+  int rc = run_copies(ctx, f.copies.p, (int)copies.size());
   if (rc != LINS_OK) return rc;
   lins_seq_step_desc sd;
   std::memset(&sd, 0, sizeof(sd));
-  sd.n_seq = n; sd.present = d->present; sd.imu = d->imu; sd.imu_off = d->imu_off; sd.point_format = LINS_POINTS_XYZI32;
+  sd.n_seq = n; sd.present = pres; sd.imu = imu; sd.imu_off = imu_off; sd.point_format = LINS_POINTS_XYZI32;
   const int32_t* offs[4] = {&off[0], &off[N1], &off[2 * N1], &off[3 * N1]};
   // from here on the sequences' state changes, as in lins_gpu_seq_step_ex
   rc = seq_step_run(ctx, &sd, offs, scan_imu);
   if (rc != LINS_OK) q.n = 0;
   return rc;
+}
+
+}  // namespace
+
+extern "C" {
+
+int lins_gpu_seq_step_pcl(lins_ctx* ctx, const lins_seq_pcl_desc* d, const lins_feature_params* fp, const double* scan_imu) {
+  if (!ctx) return LINS_E_INVALID;
+  SeqState& q = ctx->seq;
+  if (q.n == 0) return fail(ctx, LINS_E_NOMAP, "lins_gpu_seq_begin has not been called");
+  if (!d || d->n_seq != q.n || d->pcl.n_scans != q.n) return fail(ctx, LINS_E_INVALID, "n_seq differs from the hand-over's");
+  int rc = check_step_imu(ctx, d->present, d->imu, d->imu_off, scan_imu);
+  if (rc != LINS_OK) return rc;
+  // extraction, validation of the scans and the counts' read-back: nothing of the sequences has changed yet
+  rc = features_run(ctx, fp, &d->pcl);
+  if (rc != LINS_OK) return rc;
+  return step_from_features(ctx, d->present, d->imu, d->imu_off, d->pcl.cloud_off, scan_imu);
+}
+
+int lins_gpu_seq_step_raw(lins_ctx* ctx, const lins_seq_raw_desc* d, const lins_lidar_model* m, const lins_feature_params* fp,
+                          const double* scan_imu) {
+  if (!ctx) return LINS_E_INVALID;
+  SeqState& q = ctx->seq;
+  if (q.n == 0) return fail(ctx, LINS_E_NOMAP, "lins_gpu_seq_begin has not been called");
+  if (!d || d->n_seq != q.n || d->raw.n_scans != q.n) return fail(ctx, LINS_E_INVALID, "n_seq differs from the hand-over's");
+  if (!fp) return fail(ctx, LINS_E_INVALID, "null feature params");
+  int rc = check_step_imu(ctx, d->present, d->imu, d->imu_off, scan_imu);
+  if (rc != LINS_OK) return rc;
+  // projection with copyPointCloud's NaN removal, then the extraction on its output where it lies (the raw offsets, each
+  // scan's segmented count as its extent): one D2H + synchronisation for the counts, before the sequences change
+  rc = projection_run(ctx, m, &d->raw, true, d->present);
+  if (rc != LINS_OK) return rc;
+  ProjState& pr = ctx->proj;
+  FeatInputs in;
+  in.n = q.n; in.line_num = m->line_num; in.total = d->raw.cloud_off[q.n];
+  in.pts = pr.seg.p; in.off = pr.up.qs_off.p; in.count = pr.counts.p; in.count_stride = 2;
+  in.ground = pr.ground.p; in.col = pr.col.p; in.range = pr.range.p; in.ring = pr.ring.p; in.ori = pr.ori.p;
+  rc = features_launch(ctx, fp, in);
+  if (rc != LINS_OK) return rc;
+  return step_from_features(ctx, d->present, d->imu, d->imu_off, d->raw.cloud_off, scan_imu);
 }
 
 }  // extern "C"

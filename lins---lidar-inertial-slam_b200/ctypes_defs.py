@@ -193,6 +193,11 @@ class LinsRawDesc(C.Structure):
     _fields_ = [("n_scans", C.c_int32), ("cloud", C.c_void_p), ("cloud_off", C.c_void_p), ("point_format", C.c_int32)]
 
 
+class LinsSeqRawDesc(C.Structure):
+    """lins_seq_raw_desc: one raw sweep per sequence."""
+    _fields_ = [("n_seq", C.c_int32), ("present", C.c_void_p), ("imu", C.c_void_p), ("imu_off", C.c_void_p), ("raw", LinsRawDesc)]
+
+
 class LinsSeqStepDesc(C.Structure):
     _fields_ = [
         ("n_seq", C.c_int32),

@@ -10,7 +10,7 @@ import subprocess
 
 import numpy as np
 
-from .ctypes_defs import Batch, LinsBatchDesc, LinsPclDesc, POINT_DTYPE
+from .ctypes_defs import Batch, LinsBatchDesc, LinsPclDesc, LinsRawDesc, POINT_DTYPE
 
 _ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 _DIR = os.path.join(_ROOT, "tools", "synth")
@@ -351,6 +351,37 @@ def pcl_log(config="config3", seed=1, n_scans=12, **overrides):
         ori = _copy(p.orientation, n * 3, np.float32).reshape(n, 3)
         log["scans"] = [dict(seg=xyzi[off[k]:off[k + 1]].copy(), ground=ground[off[k]:off[k + 1]].copy(), col=col[off[k]:off[k + 1]].copy(),
                              range=rng[off[k]:off[k + 1]].copy(), start_ring=sr[k].copy(), end_ring=er[k].copy(), ori=ori[k].copy()) for k in range(n)]
+        return log
+    finally:
+        L.lins_flog_destroy(h)
+
+
+def raw_log(config="config3", seed=1, n_scans=12, **overrides):
+    """The drive of feature_log(config, seed, n_scans) as the LiDAR driver publishes it: dict with lidar, line_num, time,
+    imu + imu_off, imu_last (as in a feature log) and sweeps: one raw sweep per scan (m x 4 float32 x, y, z, intensity,
+    firing order).  Run through sequence mode with LinsGpu.seq_step_raw; the host reference projects each sweep (after
+    dropping its non-finite points) into a pcl log for replay_pcl_log."""
+    L = _plog_lib()
+    if not hasattr(L, "_rlog"):
+        L.lins_flog_raw.argtypes = [C.c_void_p, C.c_void_p]
+        L._rlog = True
+    kw = dict(CONFIGS[config])
+    kw.update(overrides)
+    cfg = SynthCfg(**kw)
+    h = L.lins_flog_create(C.byref(cfg), seed, n_scans)
+    try:
+        d = PclLogDesc()
+        L.lins_plog_desc(h, C.byref(d))
+        r = LinsRawDesc()
+        L.lins_flog_raw(h, C.byref(r))
+        n = d.n_scans
+        log = dict(lidar=kw["lidar"], line_num=d.pcl.line_num, time=_copy(d.time, n, np.float64), imu_off=_copy(d.imu_off, n + 1, np.int32),
+                   imu_last=_copy(d.imu_last, n * 6, np.float64).reshape(n, 6))
+        log["imu"] = _copy(d.imu, int(log["imu_off"][-1]) * 7, np.float64).reshape(-1, 7)
+        off = _copy(r.cloud_off, n + 1, np.int32)
+        pts = _copy(r.cloud, int(off[-1]), POINT_DTYPE)
+        xyzi = np.stack([pts["x"], pts["y"], pts["z"], pts["intensity"]], 1).astype(np.float32)
+        log["sweeps"] = [xyzi[off[k]:off[k + 1]].copy() for k in range(n)]
         return log
     finally:
         L.lins_flog_destroy(h)

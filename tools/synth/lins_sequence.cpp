@@ -309,6 +309,9 @@ struct FeatureLog {
   std::vector<uint8_t> ground;
   std::vector<uint32_t> col;
   std::vector<float> range, ori;
+  // ... and as the LiDAR driver publishes them (a "raw log"): the raw sweeps, CSR like lins_raw_desc
+  std::vector<lins_point> raw;
+  std::vector<int32_t> raw_off{0};
 };
 
 // a pcl log: per scan the IMU calls and processPCL's segmented cloud + cloud_info (lins_pcl_desc, n_scans == n)
@@ -348,6 +351,7 @@ void* lins_flog_create(const lins_synth_cfg* cfg, uint64_t seed, int n_scans) {
     const double last[6] = {sw.accs.back().x(), sw.accs.back().y(), sw.accs.back().z(), sw.gyrs.back().x(), sw.gyrs.back().y(), sw.gyrs.back().z()};
     L->imu_last.insert(L->imu_last.end(), last, last + 6);
     L->time.push_back(sw.t_end);
+    append_cloud(L->raw, L->raw_off, sw.raw);
     ip.process(sw.raw);
     ScanFeatures f;
     ex.run(ip.segmentedCloud, ip.segMsg, f);
@@ -378,6 +382,13 @@ void lins_plog_desc(void* h, lins_pcl_log_desc* d) {
   p.ground_flag = L->ground.data(); p.col_ind = L->col.data(); p.range = L->range.data();
   p.start_ring_index = L->start_ring.data(); p.end_ring_index = L->end_ring.data(); p.orientation = L->ori.data();
   p.point_format = LINS_POINTS_XYZI32;
+}
+// the raw sweeps of a feature log made by lins_flog_create (valid while the log lives)
+void lins_flog_raw(void* h, lins_raw_desc* d) {
+  FeatureLog* L = static_cast<FeatureLog*>(h);
+  d->n_scans = (int32_t)L->time.size();
+  d->cloud = L->raw.data(); d->cloud_off = L->raw_off.data();
+  d->point_format = LINS_POINTS_XYZI32;
 }
 void lins_flog_destroy(void* h) { delete static_cast<FeatureLog*>(h); }
 void lins_flog_desc(void* h, lins_feature_log_desc* d) {

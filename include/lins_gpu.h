@@ -437,6 +437,64 @@ typedef struct lins_seq_raw_desc {
 int lins_gpu_seq_step_raw(lins_ctx* ctx, const lins_seq_raw_desc* step, const lins_lidar_model* model,
                           const lins_feature_params* fp, const double* scan_imu /*S x 6 or NULL*/);
 
+/* ---- sensor_msgs/PointCloud2 on the device: pcl::fromROSMsg<pcl::PointXYZI> of copyPointCloud
+   (image_projection_node.cpp:172-177), from the message's bytes as the driver publishes them (a ROS callback's
+   msg->data, or a message's data field inside a bag chunk).  Bit-identical to the host decoder
+   csrc/host/rosbag_reader.hpp decode_pointcloud2 (DESIGN.md §4.8). */
+
+/* what fromROSMsg<PointXYZI> reads of one message: its geometry and the x, y, z and intensity PointFields */
+typedef struct lins_cloud2_layout {
+  uint32_t height, width;       /* the message has width * height points, read row-major */
+  uint32_t point_step, row_step;  /* bytes; point (r, c) starts at r * row_step + c * point_step */
+  uint32_t offset[4];           /* x, y, z, intensity: byte offset inside a point */
+  uint8_t datatype[4];          /* x, y, z, intensity: sensor_msgs/PointField datatype 1..8 (INT8 .. FLOAT64); intensity may
+                                   be 0 = the message has no intensity field (it then reads as 0).  A field named intensity
+                                   whose own datatype is 0 makes the message malformed (decode_pointcloud2 rejects it):
+                                   give it a datatype outside 0..8 so that the call rejects it too (INTEGRATION.md) */
+  uint8_t is_bigendian;         /* must be 0 */
+  uint8_t pad_[3];
+} lins_cloud2_layout;           /* 40 bytes */
+
+/* n messages: message i's data field is data[data_off[i] .. data_off[i + 1]) (data_off non-decreasing, data_off[0] may be
+   > 0), its layout layouts[i].  The blob may start at any address and the fields at any offset: nothing is assumed aligned. */
+typedef struct lins_cloud2_desc {
+  int32_t n_scans;
+  const uint8_t* data;
+  const int64_t* data_off;                /* n_scans + 1 */
+  const lins_cloud2_layout* layouts;      /* n_scans */
+} lins_cloud2_desc;
+
+/* ≙ pcl::fromROSMsg<pcl::PointXYZI> of every message of d (as decode_pointcloud2 reads it: each field through
+   read_scalar, then (float); a field the layout does not name is not read).  Message i's width * height records are
+   written in row-major order at out + the prefix sum of the earlier messages' width * height, with pad0 = 1 and zero
+   pads; counts[i] = width * height (counts may be NULL).  NaN no-returns are kept.  LINS_E_INVALID, before anything is
+   uploaded or written, for a NULL array, bad data_off, a total above INT32_MAX points, or a message decode_pointcloud2
+   rejects: big-endian, a datatype outside 1..8 (0 allowed for intensity only), a field with offset + size > point_step,
+   or a point past its message's data ((h - 1) * row_step + (w - 1) * point_step + point_step > length, in 64-bit
+   arithmetic).  The blob is uploaded as lins_gpu_batch_upload uploads clouds: through pinned staging, or in one DMA
+   when the caller registered it with lins_gpu_host_register. */
+int lins_gpu_decode_cloud2(lins_ctx* ctx, const lins_cloud2_desc* d, lins_point* out, int32_t* counts /*n or NULL*/);
+/* CUDA-event time of the last decode kernel (lins_gpu_decode_cloud2 or lins_gpu_seq_step_cloud2), ms */
+int lins_gpu_decode_ms(lins_ctx* ctx, float* ms);
+
+/* one sensor_msgs/PointCloud2 message per sequence: the IMU rows as in lins_seq_step_desc, the messages as a
+   lins_cloud2_desc with n_scans == n_seq (a slot that is not present is not decoded; its message may be empty) */
+typedef struct lins_seq_cloud2_desc {
+  int32_t n_seq;
+  const uint8_t* present;              /* NULL = all */
+  const double* imu; const int32_t* imu_off;
+  lins_cloud2_desc cloud2;
+} lins_seq_cloud2_desc;
+
+/* ≙ cloudHandler from the PointCloud2 message (fromROSMsg, removeNaNFromPointCloud, image projection) followed by
+   processPCL for every present slot, all on the device: lins_gpu_seq_step_raw with the decode in front.  Bit-identical to
+   lins_gpu_decode_cloud2 (or the host decode_pointcloud2) followed by lins_gpu_seq_step_raw on the decoded sweeps; may
+   alternate with lins_gpu_seq_step_ex / _pcl / _raw in one run.  LINS_E_INVALID before anything changes for a descriptor
+   lins_gpu_decode_cloud2 rejects, and otherwise as lins_gpu_seq_step_raw.  Afterwards lins_gpu_decode_ms,
+   lins_gpu_project_ms and lins_gpu_extract_ms report the step's three front-end kernels. */
+int lins_gpu_seq_step_cloud2(lins_ctx* ctx, const lins_seq_cloud2_desc* step, const lins_lidar_model* model,
+                             const lins_feature_params* fp, const double* scan_imu /*S x 6 or NULL*/);
+
 /* Split "Jacobian kernel" (SURVEY.md §8(d) unit U1): residual + Jacobian row + 29-scalar reduction over the
    resident batch given the correspondence IDs of iteration `iter` of each scan's current linearisation
    point. Used for the HBM-roofline measurement; results land in an internal n x 29 accumulator array. */

@@ -1,0 +1,179 @@
+"""Replay many ROS1 bags (sensor_msgs/PointCloud2 + sensor_msgs/Imu) through sequence mode in lockstep.
+
+Each bag is one recording, scheduled exactly as tools/synth/lins_sequence.cpp lins_seq_run_bag (synth.run_bag) feeds
+one StateEstimator, so that run_bag is each bag's contract (LinsFusion, Estimator.cpp:204-252):
+  - IMU samples and scans are stably sorted by header stamp;
+  - the estimator clock starts one scan_period before the first scan;
+  - before each scan, samples are taken from the upper_bound of the estimator time, each with
+    dt = min(t_imu, t_scan) - t_est (a sample past the scan is used up to the scan and kept for the next);
+  - processPCL's IMU sample is the last propagated one, or (0, 0, G0) / 0 when there is none.
+The bags are queued through S slots (lins_gpu_seq_open, lins_gpu_seq_restart when a slot's bag has ended), and every
+step hands each present slot's PointCloud2 data field to lins_gpu_seq_step_cloud2 as it is: the decode runs on the
+device.  A step's data fields are gathered into one host buffer that is page-locked once (re-registered only when it
+grows), so each step's bytes go to the device in one DMA.
+"""
+import ctypes as C
+import importlib.util
+import os
+
+import numpy as np
+
+from . import capi as _capi
+from .ctypes_defs import LinsCloud2Desc, LinsCloud2Layout, LinsLidarModel, LinsSeqInitParams, LinsSeqParams, SEQ_ICP, SEQ_RAN
+
+G0 = 9.81  # filter::G0 (parameters.h:62)
+_ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+
+
+def _bag_tool():
+    spec = importlib.util.spec_from_file_location("bag_tool", os.path.join(_ROOT, "tools", "bag_tool.py"))
+    m = importlib.util.module_from_spec(spec)
+    spec.loader.exec_module(m)
+    return m
+
+
+def layout(ix):
+    """LinsCloud2Layout of a bag_tool.index_pointcloud2 dict."""
+    lay = LinsCloud2Layout()
+    lay.height, lay.width, lay.point_step, lay.row_step, lay.is_bigendian = ix["height"], ix["width"], ix["point_step"], ix["row_step"], ix["is_bigendian"]
+    for k in range(4):
+        lay.offset[k], lay.datatype[k] = ix["offset"][k], ix["datatype"][k]
+    return lay
+
+
+class Recording:
+    """One bag: its scans (stamp, layout, data field) and, per scan, the processImu rows (dt, acc, gyr) and processPCL's
+    IMU sample."""
+
+    def __init__(self, path, lidar_topic="/velodyne_points", imu_topic="/imu/data", max_scans=0, scan_period=0.1):
+        bt = _bag_tool()
+        conns, msgs = bt.read_bag(path)
+        topic = {cid: c["topic"] for cid, c in conns.items()}
+        imus, scans = [], []
+        for cid, _, b in msgs:
+            if topic.get(cid) == imu_topic:
+                m = bt.decode_imu(b)
+                imus.append((m["header"]["stamp"], m["linear_acceleration"], m["angular_velocity"]))
+            elif topic.get(cid) == lidar_topic and (max_scans <= 0 or len(scans) < max_scans):
+                ix = bt.index_pointcloud2(b)
+                if ix is None:
+                    raise ValueError(f"{path}: a PointCloud2 message the decoder rejects")
+                scans.append((ix["stamp"], layout(ix), np.frombuffer(b, np.uint8, ix["data_len"], ix["data_start"])))
+        imus = [imus[i] for i in np.argsort([t for t, _, _ in imus], kind="stable")]
+        scans = [scans[i] for i in np.argsort([t for t, _, _ in scans], kind="stable")]
+        self.path = path
+        self.stamps = np.array([s[0] for s in scans])
+        self.layouts = [s[1] for s in scans]
+        self.data = [s[2] for s in scans]
+        self.imu, self.imu_last = [], np.zeros((len(scans), 6))
+        nxt, t_est = 0, (self.stamps[0] - scan_period) if len(scans) else 0.0
+        for k, ts in enumerate(self.stamps):
+            rows = []
+            while t_est < ts and nxt < len(imus):
+                ti, a, g = imus[nxt]
+                if ti <= t_est:
+                    nxt += 1
+                    continue
+                dt = min(ti, ts) - t_est
+                rows.append((dt, *a, *g))
+                t_est += dt
+                if ti <= ts:
+                    nxt += 1
+            t_est = ts
+            self.imu.append(np.array(rows, np.float64).reshape(-1, 7))
+            self.imu_last[k] = rows[-1][1:] if rows else (0.0, 0.0, G0, 0.0, 0.0, 0.0)
+
+    def __len__(self):
+        return len(self.stamps)
+
+
+class _PinnedBlob:
+    """A host byte buffer page-locked once with lins_gpu_host_register (grown, and registered again, when a step needs
+    more)."""
+
+    def __init__(self):
+        self.a = None
+
+    def get(self, n):
+        if self.a is None or len(self.a) < n:
+            size = max(n, 1 << 20, 0 if self.a is None else 2 * len(self.a))
+            self.release()
+            self.a = np.empty(size, np.uint8)
+            if _capi.lib().lins_gpu_host_register(self.a.ctypes.data, self.a.nbytes) != 0:
+                raise _capi.LinsError("lins_gpu_host_register failed")
+        return self.a
+
+    def release(self):
+        if self.a is not None:
+            _capi.lib().lins_gpu_host_unregister(self.a.ctypes.data)
+            self.a = None
+
+
+def shim_init_params():
+    """The filter constants run_bag's StateEstimator uses (lins_sequence.cpp seq_params: zero INIT_BA / INIT_BW)."""
+    return LinsSeqInitParams.shipped(init_ba=(0.0, 0.0, 0.0), init_bw=(0.0, 0.0, 0.0))
+
+
+def replay(recordings, slots, model=None, device=0, gpu=None):
+    """Run the recordings through `slots` slots of one context.  Returns per recording a dict of per-scan arrays: stamps,
+    status (StateEstimator::status_ after the scan), scan_status (LINS_SEQ_*), global_est (n x 7: rn, qbn x y z w),
+    global_state (n x 19), iters and flags (-1 where the scan ran no IESKF)."""
+    model = model or LinsLidarModel.vlp16()
+    g = gpu or _capi.LinsGpu(device=device)
+    g.seq_open(LinsSeqParams.shipped(), shim_init_params(), slots)
+    out = [dict(stamps=r.stamps.copy(), status=np.zeros(len(r), np.int32), scan_status=np.zeros(len(r), np.int32),
+                global_est=np.zeros((len(r), 7)), global_state=np.zeros((len(r), 19)), iters=np.full(len(r), -1, np.int32),
+                flags=np.full(len(r), -1, np.int32)) for r in recordings]
+    cur, used, nxt = [None] * slots, [False] * slots, 0
+    blob = _PinnedBlob()
+    try:
+        while True:
+            restart = np.zeros(slots, np.uint8)
+            for j in range(slots):
+                if cur[j] is not None and cur[j][1] >= len(recordings[cur[j][0]]):
+                    cur[j] = None
+                while cur[j] is None and nxt < len(recordings):
+                    if len(recordings[nxt]):
+                        restart[j] = used[j]
+                        cur[j], used[j] = [nxt, 0], True
+                    nxt += 1
+            if all(c is None for c in cur):
+                break
+            if restart.any():
+                g.seq_restart(restart)
+            who = [(c[0], c[1]) if c is not None else None for c in cur]
+            present = np.array([w is not None for w in who], np.uint8)
+            imus = [recordings[w[0]].imu[w[1]] if w else np.zeros((0, 7)) for w in who]
+            imu_off = np.concatenate([[0], np.cumsum([len(r) for r in imus])]).astype(np.int32)
+            scan_imu = np.array([recordings[w[0]].imu_last[w[1]] if w else np.zeros(6) for w in who])
+            datas = [recordings[w[0]].data[w[1]] if w else np.zeros(0, np.uint8) for w in who]
+            data_off = np.concatenate([[0], np.cumsum([len(d) for d in datas])]).astype(np.int64)
+            buf = blob.get(int(data_off[-1]))
+            for d, o in zip(datas, data_off):
+                buf[o: o + len(d)] = d
+            lays = (LinsCloud2Layout * slots)(*[recordings[w[0]].layouts[w[1]] if w else LinsCloud2Layout() for w in who])
+            desc = LinsCloud2Desc()
+            desc.n_scans, desc.data, desc.data_off, desc.layouts = slots, buf.ctypes.data, data_off.ctypes.data, C.cast(lays, C.c_void_p)
+            g.seq_step_cloud2(dict(imu=np.concatenate(imus), imu_off=imu_off, present=present), model=model, scan_imu=scan_imu, desc=desc)
+            d, di = g.seq_download(), g.seq_download_init()
+            for j, w in enumerate(who):
+                if w is None:
+                    continue
+                o, k = out[w[0]], w[1]
+                o["status"][k], o["scan_status"][k] = di["fusion_status"][j], d["status"][j]
+                gs = d["global_state"][j]
+                o["global_state"][k] = gs
+                o["global_est"][k] = np.concatenate([gs[0:3], gs[6:10]])
+                if d["status"][j] in (SEQ_RAN, SEQ_ICP):
+                    o["iters"][k], o["flags"][k] = d["results"]["iters"][j], d["results"]["flags"][j]
+                cur[j][1] += 1
+    finally:
+        blob.release()
+    return out
+
+
+def summary(o):
+    """A line like tools/run_bag.py's."""
+    it = o["iters"][o["iters"] >= 0]
+    return "scans %d IESKF updates %d mean iterations %.2f diverged %d" % (
+        len(o["stamps"]), len(it), it.mean() if len(it) else 0.0, int(((o["flags"][o["flags"] >= 0] & 2) != 0).sum()))

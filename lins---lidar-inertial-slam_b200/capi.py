@@ -13,9 +13,9 @@ import subprocess
 
 import numpy as np
 
-from .ctypes_defs import (Batch, COV_SIZE, LinsBatchDesc, LinsFeatureParams, LinsLidarModel, LinsMapReport, LinsParams, LinsPclDesc,
+from .ctypes_defs import (Batch, COV_SIZE, LinsBatchDesc, LinsCloud2Desc, LinsCloud2Layout, LinsFeatureParams, LinsLidarModel, LinsMapReport, LinsParams, LinsPclDesc,
                           LinsRawDesc, LinsReport, LinsScanResult, LinsSeqBeginDesc, LinsSeqInitParams, LinsSeqParams, LinsSeqPclDesc,
-                          LinsSeqRawDesc, LinsSeqStepDesc, POINT_DTYPE, SCAN_RESULT_DTYPE, STATE_DIM, as_points, make_points, ptr)
+                          LinsSeqCloud2Desc, LinsSeqRawDesc, LinsSeqStepDesc, POINT_DTYPE, SCAN_RESULT_DTYPE, STATE_DIM, as_points, make_points, ptr)
 
 _PKG = os.path.dirname(os.path.abspath(__file__))
 _ROOT = os.path.dirname(_PKG)
@@ -34,18 +34,18 @@ EXPORTS = [
     "lins_gpu_seq_phase_ms", "lins_gpu_seq_download_ieskf", "lins_gpu_seq_download_maps", "lins_gpu_download_indices",
     "lins_gpu_seq_open", "lins_gpu_seq_restart", "lins_gpu_seq_step_ex", "lins_gpu_seq_download_init",
     "lins_gpu_extract_features", "lins_gpu_extract_ms", "lins_gpu_seq_step_pcl", "lins_gpu_project_scans", "lins_gpu_project_ms",
-    "lins_gpu_seq_step_raw",
+    "lins_gpu_seq_step_raw", "lins_gpu_decode_cloud2", "lins_gpu_decode_ms", "lins_gpu_seq_step_cloud2",
 ]
 
 NVCC_ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]  # H100 (Hopper)
 NVCC_COMMON = NVCC_ARCH + ["-lineinfo", "-O3", "-std=c++17", "-Xcompiler", "-fPIC"]
 # translation units and their extra flags: lins_gpu.cu (the fused kernel and most of the C-ABI), lins_upload.cu (batch
 # upload), lins_map.cu (row F2's host side), lins_seq.cu (sequence mode), lins_features.cu (feature extraction),
-# lins_projection.cu (image projection) — all bit-exact, so no multiply-add contraction: the association and the map
+# lins_projection.cu (image projection), lins_cloud2.cu (PointCloud2 decoding) — all bit-exact, so no multiply-add contraction: the association and the map
 # fits depend on it — and lins_jacobian.cu (the tolerance-checked split Jacobian kernel: contraction allowed)
 UNITS = [("lins_gpu.cu", ["-fmad=false"]), ("lins_upload.cu", ["-fmad=false"]), ("lins_map.cu", ["-fmad=false"]),
          ("lins_seq.cu", ["-fmad=false"]), ("lins_features.cu", ["-fmad=false"]), ("lins_projection.cu", ["-fmad=false"]),
-         ("lins_jacobian.cu", [])]
+         ("lins_cloud2.cu", ["-fmad=false"]), ("lins_jacobian.cu", [])]
 
 
 def build(force=False, verbose=False):
@@ -123,6 +123,9 @@ def lib():
         L.lins_gpu_project_scans.argtypes = [vp, C.POINTER(LinsLidarModel), C.POINTER(LinsRawDesc)] + [vp] * 9
         L.lins_gpu_project_ms.argtypes = [vp, vp]
         L.lins_gpu_seq_step_raw.argtypes = [vp, C.POINTER(LinsSeqRawDesc), C.POINTER(LinsLidarModel), C.POINTER(LinsFeatureParams), vp]
+        L.lins_gpu_decode_cloud2.argtypes = [vp, C.POINTER(LinsCloud2Desc), vp, vp]
+        L.lins_gpu_decode_ms.argtypes = [vp, vp]
+        L.lins_gpu_seq_step_cloud2.argtypes = [vp, C.POINTER(LinsSeqCloud2Desc), C.POINTER(LinsLidarModel), C.POINTER(LinsFeatureParams), vp]
         _LIB = L
     return _LIB
 
@@ -560,6 +563,64 @@ class LinsGpu:
             if len(si) != d.n_seq:
                 raise ValueError(f"scan_imu has {len(si)} rows, the step {d.n_seq}")
         self._ck(self.L.lins_gpu_seq_step_raw(self.h, C.byref(d), C.byref(model), C.byref(fp), ptr(si)))
+
+    @staticmethod
+    def cloud2_desc(msgs, keep, gap=0, base=0):
+        """LinsCloud2Desc of PointCloud2 messages [(LinsCloud2Layout, data field bytes)], their data fields back to back in
+        one blob.  gap: bytes after each data field (inside its range, as the rest of a message record in a bag chunk), so
+        the fields start at any alignment; base: bytes before the first.  The arrays it points at are added to `keep`."""
+        n = len(msgs)
+        parts, off, pos = [np.zeros(base, np.uint8)], np.zeros(n + 1, np.int64), base
+        off[0] = base
+        for i, (_, data) in enumerate(msgs):
+            a = np.frombuffer(bytes(data), np.uint8)
+            parts += [a, np.full(gap, 0xA5, np.uint8)]
+            pos += len(a) + gap
+            off[i + 1] = pos
+        blob = np.ascontiguousarray(np.concatenate(parts)) if parts else np.zeros(0, np.uint8)
+        lays = (LinsCloud2Layout * max(n, 1))(*[m[0] for m in msgs])
+        keep.update(blob=blob, data_off=off, layouts=lays)
+        d = LinsCloud2Desc()
+        d.n_scans, d.data, d.data_off, d.layouts = n, blob.ctypes.data, off.ctypes.data, C.cast(lays, C.c_void_p)
+        return d
+
+    def decode_cloud2(self, msgs=None, desc=None, gap=0, base=0):
+        """pcl::fromROSMsg<PointXYZI> of PointCloud2 messages on the device (lins_gpu_decode_cloud2): msgs as cloud2_desc takes
+        them, or a prepared LinsCloud2Desc.  Returns (POINT_DTYPE records of every message back to back, counts)."""
+        keep = {}
+        d = desc if desc is not None else self.cloud2_desc(msgs, keep, gap, base)
+        lays = C.cast(d.layouts, C.POINTER(LinsCloud2Layout)) if d.n_scans else None
+        total = sum(int(lays[i].width) * int(lays[i].height) for i in range(d.n_scans))
+        out, counts = np.zeros(max(total, 1), POINT_DTYPE), np.zeros(max(d.n_scans, 1), np.int32)
+        self._ck(self.L.lins_gpu_decode_cloud2(self.h, C.byref(d), ptr(out), ptr(counts)))
+        return out[:total], counts[: d.n_scans]
+
+    def decode_ms(self):
+        """CUDA-event time (ms) of the last PointCloud2 decode kernel."""
+        ms = np.zeros(1, np.float32)
+        self._ck(self.L.lins_gpu_decode_ms(self.h, ptr(ms)))
+        return float(ms[0])
+
+    def seq_step_cloud2(self, step, model=None, fp=None, scan_imu=None, desc=None, gap=0):
+        """Advance every present sequence by one sensor_msgs/PointCloud2 message (lins_gpu_seq_step_cloud2: the decode, then
+        what seq_step_raw runs): `step` has imu + imu_off as in seq_step, msgs (one (layout, data) per slot, as cloud2_desc
+        takes them; an absent slot's is not read) or desc (a prepared LinsCloud2Desc), and optionally present."""
+        keep = {"imu": np.ascontiguousarray(step["imu"], dtype=np.float64), "imu_off": np.ascontiguousarray(step["imu_off"], dtype=np.int32)}
+        d = LinsSeqCloud2Desc()
+        d.cloud2 = desc if desc is not None else self.cloud2_desc(step["msgs"], keep, gap)
+        d.n_seq = len(keep["imu_off"]) - 1
+        d.imu, d.imu_off = keep["imu"].ctypes.data, keep["imu_off"].ctypes.data
+        if step.get("present") is not None:
+            keep["present"] = np.ascontiguousarray(step["present"], dtype=np.uint8)
+            d.present = keep["present"].ctypes.data
+        model = model or LinsLidarModel.vlp16()
+        fp = fp or LinsFeatureParams.shipped()
+        si = None
+        if scan_imu is not None:
+            si = np.ascontiguousarray(scan_imu, dtype=np.float64).reshape(-1, 6)
+            if len(si) != d.n_seq:
+                raise ValueError(f"scan_imu has {len(si)} rows, the step {d.n_seq}")
+        self._ck(self.L.lins_gpu_seq_step_cloud2(self.h, C.byref(d), C.byref(model), C.byref(fp), ptr(si)))
 
     def seq_download(self, reports=False):
         """dict: global_state, filter_state (S x 19), filter_cov (S x 324), results (SCAN_RESULT_DTYPE), status (S) and,

@@ -176,6 +176,30 @@ struct ProjState {
   ~ProjState() { for (cudaEvent_t e : ev) if (e) cudaEventDestroy(e); }
 };
 
+// One decode record per PointCloud2 message (lins_cloud2.cu): where its data field starts in the uploaded blob, where its
+// points go, and its layout
+struct Cloud2Scan {
+  long long base;                 // byte offset of the data field in blob
+  int out;                        // first output point
+  unsigned width, point_step, row_step;
+  unsigned offset[4];
+  unsigned char datatype[4];
+};
+
+// PointCloud2 decoding (lins_cloud2.cu): the uploaded message bytes (as 32-bit words: the decode reads aligned words), their
+// pinned staging, the per-message records and, for lins_gpu_decode_cloud2's read-back, the decoded points' staging.  The
+// decoded points themselves go to ctx->proj.up (qs, qs_off), where the projection reads raw sweeps.
+struct Cloud2State {
+  Buf<unsigned> blob;
+  Buf<unsigned char, kPinned> h_blob;
+  Buf<Cloud2Scan> scans; Buf<Cloud2Scan, kPinned> h_scans;
+  Buf<int> prefix; Buf<int, kPinned> h_prefix;  // n + 1: the first output point of each message (what qs_off holds)
+  Buf<float4, kPinned> h_out;
+  cudaEvent_t ev[2] = {nullptr, nullptr};  // around the last decode kernel (lins_gpu_decode_ms)
+  bool ev_valid = false;
+  ~Cloud2State() { for (cudaEvent_t e : ev) if (e) cudaEventDestroy(e); }
+};
+
 }  // namespace lins_capi
 
 struct lins_ctx {
@@ -197,7 +221,8 @@ struct lins_ctx {
   lins_capi::Resident single;  // lins_gpu_ieskf / associate / estimate_transform (n = 1)
   lins_capi::SeqState seq;     // lins_gpu_seq_*
   lins_capi::FeatState feat;   // lins_gpu_extract_features, lins_gpu_seq_step_pcl, lins_gpu_seq_step_raw
-  lins_capi::ProjState proj;   // lins_gpu_project_scans, lins_gpu_seq_step_raw
+  lins_capi::ProjState proj;   // lins_gpu_project_scans, lins_gpu_seq_step_raw, lins_gpu_seq_step_cloud2
+  lins_capi::Cloud2State c2;   // lins_gpu_decode_cloud2, lins_gpu_seq_step_cloud2
   // the single-scan map: "last" clouds (walks + tripods) and the clouds the 1-NN index was built on
   Buf<float4> map_s, map_c, tree_s, tree_c;
   Buf<int> map_off;  // 4 x 2 ints: [0,ns][0,nc][0,tns][0,tnc]
@@ -354,5 +379,17 @@ int features_launch(lins_ctx* ctx, const lins_feature_params* fp, const FeatInpu
 // synchronisation); drop_nonfinite: copyPointCloud's NaN removal first; present (host, n; null = all): a scan whose flag is
 // 0 is projected as an empty sweep
 int projection_run(lins_ctx* ctx, const lins_lidar_model* m, const lins_raw_desc* d, bool drop_nonfinite, const uint8_t* present);
+// lins_projection.cu: the model's limits (LINS_E_INVALID otherwise), and the part of projection_run after the upload: the
+// n sweeps (total points) are in ctx->proj.up (qs, CSR in qs_off), the model has been checked
+int check_model(lins_ctx* ctx, const lins_lidar_model* m);
+int projection_launch(lins_ctx* ctx, const lins_lidar_model* m, int n, size_t total, bool drop_nonfinite, const uint8_t* present);
+// lins_upload.cu: n bytes from the caller's src to the device at dst, as upload_clouds moves clouds: a host thread pool copies
+// 1 MiB slices into the pinned staging and queues each slice's H2D as soon as it is staged; a src in caller-pinned memory
+// goes in one DMA with no host pass.  Synchronises the stream first (the staging may still be read by an earlier copy).
+int upload_bytes(lins_ctx* ctx, void* dst, Buf<unsigned char, kPinned>& staging, const uint8_t* src, size_t n);
+// lins_cloud2.cu: validate the messages of d (present: host, n; null = all; an absent message is neither checked nor
+// decoded and has no points), upload them and queue their decode into ctx->proj.up (qs, qs_off; no synchronisation).
+// off (n + 1) receives the host copy of qs_off.
+int cloud2_run(lins_ctx* ctx, const lins_cloud2_desc* d, const uint8_t* present, std::vector<int32_t>& off);
 
 }  // namespace lins_capi

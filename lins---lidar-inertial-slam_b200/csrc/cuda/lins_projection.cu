@@ -283,6 +283,10 @@ __global__ void lins_projection_pack_kernel(const PackArgs a) {
   for (int t = threadIdx.x; t < no; t += blockDim.x) a.doutl[dq + t] = a.outl[o + t];
 }
 
+}  // namespace
+
+namespace lins_capi {
+
 int check_model(lins_ctx* ctx, const lins_lidar_model* m) {
   if (!m) return fail(ctx, LINS_E_INVALID, "null lidar model");
   if (m->line_num < 1 || m->line_num > lins_feat::kMaxLines) return fail(ctx, LINS_E_INVALID, "line_num outside 1..128");
@@ -293,10 +297,6 @@ int check_model(lins_ctx* ctx, const lins_lidar_model* m) {
   if (m->ground_scan_ind < 0 || m->ground_scan_ind > m->line_num - 1) return fail(ctx, LINS_E_INVALID, "ground_scan_ind outside 0..line_num-1");
   return LINS_OK;
 }
-
-}  // namespace
-
-namespace lins_capi {
 
 // Validate the model and the descriptor on the host, upload the sweeps and queue the projection kernel (no
 // synchronisation).  Afterwards ctx->proj holds the projected clouds at the raw offsets, n x 2 x L ring indices, n x 3
@@ -315,8 +315,13 @@ int projection_run(lins_ctx* ctx, const lins_lidar_model* m, const lins_raw_desc
   rc = upload_clouds(ctx, pr.up, n, pts, offs, d->point_format);  // (validates the offsets and the format; synchronises first)
   if (rc != LINS_OK) return rc;
   if (n == 0) return LINS_OK;
+  return projection_launch(ctx, m, n, (size_t)d->cloud_off[n], drop_nonfinite, present);
+}
+
+int projection_launch(lins_ctx* ctx, const lins_lidar_model* m, int n, size_t total, bool drop_nonfinite, const uint8_t* present) {
+  ProjState& pr = ctx->proj;
   const int L = m->line_num, S = m->scan_num;
-  const size_t P = (size_t)L * S, N = (size_t)d->cloud_off[n] + 1;
+  const size_t P = (size_t)L * S, N = total + 1;
   int per_sm = 0;
   CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, lins_projection_kernel, kThreads, 0));
   const int grid = std::max(1, std::min(n, per_sm * ctx->sm_count));
@@ -325,7 +330,7 @@ int projection_run(lins_ctx* ctx, const lins_lidar_model* m, const lins_raw_desc
   CK(pr.cnt.reserve(G)); CK(pr.rlo.reserve(G)); CK(pr.rhi.reserve(G));
   CK(pr.seg.reserve(N)); CK(pr.outl.reserve(N)); CK(pr.ground.reserve(N)); CK(pr.col.reserve(N)); CK(pr.range.reserve(N));
   CK(pr.ring.reserve(2 * (size_t)n * L)); CK(pr.ori.reserve(3 * (size_t)n)); CK(pr.counts.reserve(2 * (size_t)n));
-  if (present) {  // (upload_clouds synchronised the stream: the staging is free)
+  if (present) {  // (the upload synchronised the stream: the staging is free)
     CK(pr.present.reserve(n)); CK(pr.h_present.reserve(n));
     std::memcpy(pr.h_present.p, present, n);
     CK(cudaMemcpyAsync(pr.present.p, pr.h_present.p, n, cudaMemcpyHostToDevice, ctx->stream));

@@ -450,6 +450,22 @@ int step_from_features(lins_ctx* ctx, const uint8_t* pres, const double* imu, co
   return rc;
 }
 
+// The rest of a step whose sweeps' projection (with the NaN removal) is queued in ctx->proj at the raw offsets src_off:
+// the extraction on the projection's output where it lies (each scan's segmented count as its extent), one D2H +
+// synchronisation for the counts before the sequences change, then step_from_features.
+int step_from_projection(lins_ctx* ctx, const uint8_t* pres, const double* imu, const int32_t* imu_off, const lins_lidar_model* m,
+                         const lins_feature_params* fp, const int32_t* src_off, const double* scan_imu) {
+  const int n = ctx->seq.n;
+  ProjState& pr = ctx->proj;
+  FeatInputs in;
+  in.n = n; in.line_num = m->line_num; in.total = src_off[n];
+  in.pts = pr.seg.p; in.off = pr.up.qs_off.p; in.count = pr.counts.p; in.count_stride = 2;
+  in.ground = pr.ground.p; in.col = pr.col.p; in.range = pr.range.p; in.ring = pr.ring.p; in.ori = pr.ori.p;
+  const int rc = features_launch(ctx, fp, in);
+  if (rc != LINS_OK) return rc;
+  return step_from_features(ctx, pres, imu, imu_off, src_off, scan_imu);
+}
+
 }  // namespace
 
 extern "C" {
@@ -476,18 +492,30 @@ int lins_gpu_seq_step_raw(lins_ctx* ctx, const lins_seq_raw_desc* d, const lins_
   if (!fp) return fail(ctx, LINS_E_INVALID, "null feature params");
   int rc = check_step_imu(ctx, d->present, d->imu, d->imu_off, scan_imu);
   if (rc != LINS_OK) return rc;
-  // projection with copyPointCloud's NaN removal, then the extraction on its output where it lies (the raw offsets, each
-  // scan's segmented count as its extent): one D2H + synchronisation for the counts, before the sequences change
+  // projection with copyPointCloud's NaN removal, then the rest of the step
   rc = projection_run(ctx, m, &d->raw, true, d->present);
   if (rc != LINS_OK) return rc;
-  ProjState& pr = ctx->proj;
-  FeatInputs in;
-  in.n = q.n; in.line_num = m->line_num; in.total = d->raw.cloud_off[q.n];
-  in.pts = pr.seg.p; in.off = pr.up.qs_off.p; in.count = pr.counts.p; in.count_stride = 2;
-  in.ground = pr.ground.p; in.col = pr.col.p; in.range = pr.range.p; in.ring = pr.ring.p; in.ori = pr.ori.p;
-  rc = features_launch(ctx, fp, in);
+  return step_from_projection(ctx, d->present, d->imu, d->imu_off, m, fp, d->raw.cloud_off, scan_imu);
+}
+
+int lins_gpu_seq_step_cloud2(lins_ctx* ctx, const lins_seq_cloud2_desc* d, const lins_lidar_model* m, const lins_feature_params* fp,
+                             const double* scan_imu) {
+  if (!ctx) return LINS_E_INVALID;
+  SeqState& q = ctx->seq;
+  if (q.n == 0) return fail(ctx, LINS_E_NOMAP, "lins_gpu_seq_begin has not been called");
+  if (!d || d->n_seq != q.n || d->cloud2.n_scans != q.n) return fail(ctx, LINS_E_INVALID, "n_seq differs from the hand-over's");
+  if (!fp) return fail(ctx, LINS_E_INVALID, "null feature params");
+  int rc = check_step_imu(ctx, d->present, d->imu, d->imu_off, scan_imu);
   if (rc != LINS_OK) return rc;
-  return step_from_features(ctx, d->present, d->imu, d->imu_off, d->raw.cloud_off, scan_imu);
+  rc = check_model(ctx, m);
+  if (rc != LINS_OK) return rc;
+  // the messages decoded into the projection's input (the present slots' only), then step_raw's projection and the rest
+  std::vector<int32_t> off;
+  rc = cloud2_run(ctx, &d->cloud2, d->present, off);
+  if (rc != LINS_OK) return rc;
+  rc = projection_launch(ctx, m, q.n, (size_t)off[q.n], true, d->present);
+  if (rc != LINS_OK) return rc;
+  return step_from_projection(ctx, d->present, d->imu, d->imu_off, m, fp, off.data(), scan_imu);
 }
 
 }  // extern "C"

@@ -169,6 +169,42 @@ int upload_clouds(lins_ctx* ctx, Resident& r, int n, const lins_point* const pts
   return LINS_OK;
 }
 
+int upload_bytes(lins_ctx* ctx, void* dst, Buf<unsigned char, kPinned>& staging, const uint8_t* src, size_t n) {
+  CK(cudaStreamSynchronize(ctx->stream));  // the pinned staging of a previous upload may still be in flight
+  if (n == 0) return LINS_OK;
+  cudaPointerAttributes at;
+  if (cudaPointerGetAttributes(&at, src) == cudaSuccess && at.type == cudaMemoryTypeHost) {  // caller-pinned: one DMA
+    CK(cudaMemcpyAsync(dst, src, n, cudaMemcpyHostToDevice, ctx->stream));
+    return LINS_OK;
+  }
+  cudaGetLastError();
+  CK(staging.reserve(n));
+  // pool threads as upload_clouds counts them: LINS_PACK_THREADS, else half the hardware threads, at most 32
+  int want_threads;
+  {
+    unsigned hw = std::thread::hardware_concurrency();
+    want_threads = (int)std::min<unsigned>(hw ? hw / 2 : 4, 32);
+    if (const char* e = std::getenv("LINS_PACK_THREADS")) { const int v = std::atoi(e); if (v >= 1) want_threads = std::min(v, 64); }
+  }
+  const size_t SL = 1u << 20, n_slices = (n + SL - 1) / SL;
+  std::atomic<size_t> next(0);
+  std::atomic<int> cuda_err(0);
+  const int device = ctx->device;
+  cudaStream_t stream = ctx->stream;
+  unsigned char* hp = staging.p;
+  ctx->pool.run((int)std::min<size_t>((size_t)want_threads, n_slices), [&]() {
+    cudaSetDevice(device);
+    for (size_t i; (i = next.fetch_add(1)) < n_slices;) {
+      const size_t a = i * SL, len = std::min(SL, n - a);
+      std::memcpy(hp + a, src + a, len);
+      const cudaError_t e = cudaMemcpyAsync(static_cast<unsigned char*>(dst) + a, hp + a, len, cudaMemcpyHostToDevice, stream);
+      if (e != cudaSuccess) cuda_err.store((int)e);
+    }
+  });
+  if (cuda_err.load() != 0) return fail(ctx, LINS_E_CUDA, "H2D copy of a slice", (cudaError_t)cuda_err.load());
+  return LINS_OK;
+}
+
 }  // namespace lins_capi
 
 extern "C" {

@@ -198,6 +198,23 @@ class LinsSeqRawDesc(C.Structure):
     _fields_ = [("n_seq", C.c_int32), ("present", C.c_void_p), ("imu", C.c_void_p), ("imu_off", C.c_void_p), ("raw", LinsRawDesc)]
 
 
+class LinsCloud2Layout(C.Structure):
+    """lins_cloud2_layout: what fromROSMsg<PointXYZI> reads of one sensor_msgs/PointCloud2 (x, y, z, intensity in
+    offset / datatype order; intensity datatype 0 = absent)."""
+    _fields_ = [("height", C.c_uint32), ("width", C.c_uint32), ("point_step", C.c_uint32), ("row_step", C.c_uint32),
+                ("offset", C.c_uint32 * 4), ("datatype", C.c_uint8 * 4), ("is_bigendian", C.c_uint8), ("pad_", C.c_uint8 * 3)]
+
+
+class LinsCloud2Desc(C.Structure):
+    """lins_cloud2_desc: n messages' data fields, CSR over one byte blob (int64 offsets), one layout each."""
+    _fields_ = [("n_scans", C.c_int32), ("data", C.c_void_p), ("data_off", C.c_void_p), ("layouts", C.c_void_p)]
+
+
+class LinsSeqCloud2Desc(C.Structure):
+    """lins_seq_cloud2_desc: one PointCloud2 message per sequence."""
+    _fields_ = [("n_seq", C.c_int32), ("present", C.c_void_p), ("imu", C.c_void_p), ("imu_off", C.c_void_p), ("cloud2", LinsCloud2Desc)]
+
+
 class LinsSeqStepDesc(C.Structure):
     _fields_ = [
         ("n_seq", C.c_int32),

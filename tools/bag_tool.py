@@ -253,20 +253,76 @@ def decode_imu(b):
 VELODYNE_FIELDS = [("x", 0, 7, 1), ("y", 4, 7, 1), ("z", 8, 7, 1), ("intensity", 16, 7, 1), ("ring", 20, 4, 1)]  # the velodyne driver's PointXYZIR, 32-byte step
 
 
-def encode_pointcloud2(seq, stamp, xyz, intensity, ring=None, frame="velodyne", fields=VELODYNE_FIELDS, point_step=32):
+_NPT = {1: np.int8, 2: np.uint8, 3: np.int16, 4: np.uint16, 5: np.int32, 6: np.uint32, 7: np.float32, 8: np.float64}
+
+
+def encode_pointcloud2(seq, stamp, xyz, intensity, ring=None, frame="velodyne", fields=VELODYNE_FIELDS, point_step=32, height=1,
+                       row_pad=0, extra=None):
+    """A sensor_msgs/PointCloud2 of len(xyz) points, row-major in `height` rows of row_step = width * point_step + row_pad
+    bytes.  fields: (name, offset, datatype, count); x, y, z, intensity, ring and the columns of `extra` ({name: values})
+    are written with numpy's casts to the field's datatype, any other field stays zero."""
     n = len(xyz)
-    buf = np.zeros((n, point_step), np.uint8)
+    width = n // height if height else 0
+    assert width * height == n
+    row_step = width * point_step + row_pad
+    buf = np.zeros((height, row_step), np.uint8)
+    pts = buf[:, : width * point_step].reshape(height, width, point_step)
     cols = {"x": xyz[:, 0], "y": xyz[:, 1], "z": xyz[:, 2], "intensity": intensity, "ring": ring}
-    npt = {7: np.float32, 4: np.uint16, 8: np.float64, 2: np.uint8}
-    out = _hdr(seq, stamp, frame) + struct.pack("<III", 1, n, len(fields))
+    cols.update(extra or {})
+    out = _hdr(seq, stamp, frame) + struct.pack("<III", height, width, len(fields))
     for name, off, dt, cnt in fields:
         nb = name.encode()
         out += struct.pack("<I", len(nb)) + nb + struct.pack("<IBI", off, dt, cnt)
-        if cols.get(name) is not None:
-            a = np.ascontiguousarray(np.asarray(cols[name]).astype(npt[dt]))
-            buf[:, off : off + a.itemsize] = a.view(np.uint8).reshape(n, a.itemsize)
+        if cols.get(name) is not None and n and dt in _NPT and off + np.dtype(_NPT[dt]).itemsize <= point_step:
+            a = np.ascontiguousarray(np.asarray(cols[name]).astype(_NPT[dt]))
+            pts[:, :, off : off + a.itemsize] = a.view(np.uint8).reshape(height, width, a.itemsize)
     data = buf.tobytes()
-    return out + struct.pack("<BII", 0, point_step, point_step * n) + struct.pack("<I", len(data)) + data + struct.pack("<B", 1)
+    return out + struct.pack("<BII", 0, point_step, row_step) + struct.pack("<I", len(data)) + data + struct.pack("<B", 1)
+
+
+_TSIZE = {1: 1, 2: 1, 3: 2, 4: 2, 5: 4, 6: 4, 7: 4, 8: 8}
+
+
+def index_pointcloud2(b):
+    """What fromROSMsg<PointXYZI> reads of a sensor_msgs/PointCloud2 message, without decoding a point: dict(stamp, height,
+    width, point_step, row_step, is_bigendian, offset (x, y, z, intensity), datatype (the same; intensity 0 = absent),
+    data_start, data_len: the data field's byte range inside the message), or None where the C++ decode_pointcloud2
+    (csrc/host/rosbag_reader.hpp) rejects the message.  Field names match as there (the last field of a name wins);
+    extents are checked without 32-bit wrap-around."""
+    try:
+        seq, s, ns, fl = struct.unpack_from("<IIII", b, 0)
+        i = 16 + fl
+        height, width, nf = struct.unpack_from("<III", b, i)
+        i += 12
+        if nf > 64:
+            return None
+        found = {}
+        for _ in range(nf):
+            (nl,) = struct.unpack_from("<I", b, i)
+            name = bytes(b[i + 4 : i + 4 + nl])
+            if len(name) < nl:
+                return None
+            off, dt, cnt = struct.unpack_from("<IBI", b, i + 4 + nl)
+            i += 4 + nl + 9
+            if name in (b"x", b"y", b"z", b"intensity"):
+                found[name.decode()] = (off, dt)
+        big, step, row, dlen = struct.unpack_from("<BIII", b, i)
+        i += 13
+        if i + dlen + 1 > len(b):  # the data field and is_dense
+            return None
+    except struct.error:
+        return None
+    if big or not all(k in found for k in "xyz"):
+        return None
+    for off, dt in found.values():
+        if dt < 1 or dt > 8 or off + _TSIZE[dt] > step:
+            return None
+    if width * height and (height - 1) * row + (width - 1) * step + step > dlen:
+        return None
+    names = ("x", "y", "z", "intensity")
+    return dict(stamp=s + 1e-9 * ns, height=height, width=width, point_step=step, row_step=row, is_bigendian=big,
+                offset=[found.get(k, (0, 0))[0] for k in names], datatype=[found.get(k, (0, 0))[1] for k in names],
+                data_start=i, data_len=dlen)
 
 
 def decode_pointcloud2(b):
@@ -284,7 +340,7 @@ def decode_pointcloud2(b):
     i += 9
     (dl,) = struct.unpack_from("<I", b, i)
     data = np.frombuffer(b, np.uint8, dl, i + 4).reshape(height * width, step)
-    npt = {1: np.int8, 2: np.uint8, 3: np.int16, 4: np.uint16, 5: np.int32, 6: np.uint32, 7: np.float32, 8: np.float64}
+    npt = _NPT
     cols = {}
     for name, off, dt, cnt in fields:
         t = np.dtype(npt[dt])

@@ -2,10 +2,14 @@
 // summary of a ROS1 bag, decoded sensor_msgs/Imu, sensor_msgs/PointCloud2 and cloud_msgs/cloud_info messages, and a
 // writer of small bags.  No ROS, no PCL, no GPU.
 #include <algorithm>
+#include <atomic>
 #include <cstdio>
 #include <cstring>
 #include <string>
+#include <thread>
+#include <vector>
 
+#include "../../lins---lidar-inertial-slam_b200/csrc/cuda/lins_cloud2.cuh"
 #include "../../lins---lidar-inertial-slam_b200/csrc/host/rosbag_reader.hpp"
 
 using namespace lins;
@@ -107,6 +111,78 @@ int lins_bag_read_cloud_info(const char* path, const char* topic, int index, int
   });
   if (rc != LINS_BAG_OK) return rc;
   return bad ? LINS_BAG_E_FORMAT : (found ? LINS_BAG_OK : LINS_BAG_E_IO);
+}
+
+// One sensor_msgs/PointCloud2 message's bytes (b, n) -> what fromROSMsg<PointXYZI> reads of it, without decoding a point:
+// the layout lins_gpu_decode_cloud2 takes, the data field's byte range inside the message (*data_start, *data_len) and the
+// header stamp.  LINS_BAG_E_FORMAT exactly where decode_pointcloud2 rejects the message (extents without 32-bit wrap).
+int lins_bag_index_cloud2_msg(const uint8_t* b, size_t n, lins_cloud2_layout* lay, int64_t* data_start, int64_t* data_len, double* stamp) {
+  Cursor c(b, n);
+  const Header h = read_header(c);
+  const uint32_t height = c.get<uint32_t>(), width = c.get<uint32_t>(), nf = c.get<uint32_t>();
+  if (!c.ok || nf > 64) return LINS_BAG_E_FORMAT;
+  lins_cloud2_layout l;
+  std::memset(&l, 0, sizeof(l));
+  bool seen[4] = {false, false, false, false};
+  for (uint32_t k = 0; k < nf; ++k) {
+    const std::string name = c.str();
+    const uint32_t off = c.get<uint32_t>();
+    const uint8_t dt = c.get<uint8_t>();
+    c.get<uint32_t>();  // count
+    const int f = name == "x" ? 0 : name == "y" ? 1 : name == "z" ? 2 : name == "intensity" ? 3 : -1;
+    if (f >= 0) { l.offset[f] = off; l.datatype[f] = dt; seen[f] = true; }  // (the last field of a name wins, as there)
+  }
+  l.is_bigendian = c.get<uint8_t>();
+  l.point_step = c.get<uint32_t>(); l.row_step = c.get<uint32_t>();
+  const uint32_t dlen = c.get<uint32_t>();
+  const uint8_t* d = c.bytes(dlen);
+  c.get<uint8_t>();  // is_dense
+  if (!c.ok || (dlen && !d)) return LINS_BAG_E_FORMAT;
+  l.height = height; l.width = width;
+  if (!seen[0] || !seen[1] || !seen[2]) return LINS_BAG_E_FORMAT;
+  if (seen[3] && l.datatype[3] == 0) return LINS_BAG_E_FORMAT;  // (a named intensity of datatype 0 is rejected there)
+  if (lins_cloud2::check_layout(l, dlen)) return LINS_BAG_E_FORMAT;
+  *lay = l;
+  *data_start = d ? (int64_t)(d - b) : (int64_t)(c.p - b) - 1;
+  *data_len = dlen;
+  *stamp = h.stamp;
+  return LINS_BAG_OK;
+}
+
+// decode_pointcloud2 of one message's bytes: *n = its point count (also when cap is too small); LINS_BAG_E_FORMAT where it
+// rejects the message.  The host reference of lins_gpu_decode_cloud2.
+int lins_bag_decode_cloud2_msg(const uint8_t* b, size_t n, lins_point* out, int cap, int* npts) {
+  Header h;
+  Cloud cl;
+  if (!decode_pointcloud2(b, n, h, cl)) return LINS_BAG_E_FORMAT;
+  *npts = (int)cl.size();
+  std::memcpy(out, cl.points.data(), sizeof(lins_point) * std::min<size_t>(cl.size(), (size_t)std::max(cap, 0)));
+  return LINS_BAG_OK;
+}
+
+// decode_pointcloud2 of n whole messages (message i = buf[msg_off[i] .. msg_off[i + 1])) on `threads` std::threads, message
+// i's points as packed (x, y, z, intensity) float records at out + 4 * out_off[i] (LINS_POINTS_PACKED16, what
+// lins_gpu_seq_step_raw takes with the least upload): the host arm of tools/cloud2_bench.py.  LINS_BAG_E_FORMAT if a message
+// is rejected or its point count differs from out_off's.
+int lins_bag_decode_cloud2_many(const uint8_t* buf, const int64_t* msg_off, int n, float* out, const int32_t* out_off, int threads) {
+  std::atomic<int> next(0), bad(0);
+  auto work = [&]() {
+    Header h;
+    Cloud c;
+    for (int i; (i = next.fetch_add(1)) < n;) {
+      if (!decode_pointcloud2(buf + msg_off[i], (size_t)(msg_off[i + 1] - msg_off[i]), h, c) || (int)c.size() != out_off[i + 1] - out_off[i]) { bad = 1; continue; }
+      float* o = out + 4 * (size_t)out_off[i];
+      for (size_t k = 0; k < c.size(); ++k) {
+        const lins_point& p = c.points[k];
+        o[4 * k] = p.x; o[4 * k + 1] = p.y; o[4 * k + 2] = p.z; o[4 * k + 3] = p.intensity;
+      }
+    }
+  };
+  std::vector<std::thread> th;
+  for (int t = 1; t < std::max(threads, 1); ++t) th.emplace_back(work);
+  work();
+  for (auto& t : th) t.join();
+  return bad ? LINS_BAG_E_FORMAT : LINS_BAG_OK;
 }
 
 // Writer test hook: a bag with n_scans clouds of n_pts points on `lidar_topic` (deterministic contents: point i of scan k

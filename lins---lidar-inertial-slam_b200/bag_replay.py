@@ -114,6 +114,30 @@ def shim_init_params():
     return LinsSeqInitParams.shipped(init_ba=(0.0, 0.0, 0.0), init_bw=(0.0, 0.0, 0.0))
 
 
+def slot_queue(lengths, n_slots):
+    """Schedule jobs of the given lengths (steps) through n_slots slots, as sequence mode queues recordings: a free slot takes
+    the next job on the same step, and a job of length 0 is skipped.  Yields one (restart, who) per step until every job
+    has run: restart (n_slots, uint8) flags the slots that take a new job after an earlier one (lins_gpu_seq_restart's
+    mask), who[j] is (job, index of the step within the job) or None for a slot without a job."""
+    cur, used, nxt = [None] * n_slots, [False] * n_slots, 0
+    while True:
+        restart = np.zeros(n_slots, np.uint8)
+        for j in range(n_slots):
+            if cur[j] is not None and cur[j][1] >= lengths[cur[j][0]]:
+                cur[j] = None
+            while cur[j] is None and nxt < len(lengths):
+                if lengths[nxt]:
+                    restart[j] = used[j]
+                    cur[j], used[j] = [nxt, 0], True
+                nxt += 1
+        if all(c is None for c in cur):
+            return
+        yield restart, [(c[0], c[1]) if c is not None else None for c in cur]
+        for c in cur:
+            if c is not None:
+                c[1] += 1
+
+
 def replay(recordings, slots, model=None, device=0, gpu=None):
     """Run the recordings through `slots` slots of one context.  Returns per recording a dict of per-scan arrays: stamps,
     status (StateEstimator::status_ after the scan), scan_status (LINS_SEQ_*), global_est (n x 7: rn, qbn x y z w),
@@ -124,24 +148,11 @@ def replay(recordings, slots, model=None, device=0, gpu=None):
     out = [dict(stamps=r.stamps.copy(), status=np.zeros(len(r), np.int32), scan_status=np.zeros(len(r), np.int32),
                 global_est=np.zeros((len(r), 7)), global_state=np.zeros((len(r), 19)), iters=np.full(len(r), -1, np.int32),
                 flags=np.full(len(r), -1, np.int32)) for r in recordings]
-    cur, used, nxt = [None] * slots, [False] * slots, 0
     blob = _PinnedBlob()
     try:
-        while True:
-            restart = np.zeros(slots, np.uint8)
-            for j in range(slots):
-                if cur[j] is not None and cur[j][1] >= len(recordings[cur[j][0]]):
-                    cur[j] = None
-                while cur[j] is None and nxt < len(recordings):
-                    if len(recordings[nxt]):
-                        restart[j] = used[j]
-                        cur[j], used[j] = [nxt, 0], True
-                    nxt += 1
-            if all(c is None for c in cur):
-                break
+        for restart, who in slot_queue([len(r) for r in recordings], slots):
             if restart.any():
                 g.seq_restart(restart)
-            who = [(c[0], c[1]) if c is not None else None for c in cur]
             present = np.array([w is not None for w in who], np.uint8)
             imus = [recordings[w[0]].imu[w[1]] if w else np.zeros((0, 7)) for w in who]
             imu_off = np.concatenate([[0], np.cumsum([len(r) for r in imus])]).astype(np.int32)
@@ -166,7 +177,6 @@ def replay(recordings, slots, model=None, device=0, gpu=None):
                 o["global_est"][k] = np.concatenate([gs[0:3], gs[6:10]])
                 if d["status"][j] in (SEQ_RAN, SEQ_ICP):
                     o["iters"][k], o["flags"][k] = d["results"]["iters"][j], d["results"]["flags"][j]
-                cur[j][1] += 1
     finally:
         blob.release()
     return out

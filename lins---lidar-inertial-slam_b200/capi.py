@@ -395,24 +395,36 @@ class LinsGpu:
         """Advance every present sequence by one scan.  `step`: dict with imu (k x 7: dt, acc, gyr) + imu_off, the four
         feature clouds (Batch.FIELDS) + their offsets (<name>_off), and optionally present (S, uint8).  scan_imu (S x 6:
         acc, gyr): the IMU sample that comes with each scan, needed while a present slot initialises."""
-        keep = {"imu": np.ascontiguousarray(step["imu"], dtype=np.float64), "imu_off": np.ascontiguousarray(step["imu_off"], dtype=np.int32)}
+        keep, d = {}, LinsSeqStepDesc()
+        si = self._seq_step_common(d, step, scan_imu, keep)
         for k in Batch.FIELDS:
             keep[k] = as_points(step[k])
             keep[k + "_off"] = np.ascontiguousarray(step[k + "_off"], dtype=np.int32)
-        d = LinsSeqStepDesc()
-        d.n_seq = len(keep["imu_off"]) - 1
+            setattr(d, k, keep[k].ctypes.data)
+            setattr(d, k + "_off", keep[k + "_off"].ctypes.data)
         d.point_format = int(step.get("point_format", 0))
-        if step.get("present") is not None:
-            keep["present"] = np.ascontiguousarray(step["present"], dtype=np.uint8)
-        for k, v in keep.items():
-            setattr(d, k, v.ctypes.data)
-        if scan_imu is None:
+        if si is None:
             self._ck(self.L.lins_gpu_seq_step(self.h, C.byref(d)))
         else:
-            si = np.ascontiguousarray(scan_imu, dtype=np.float64).reshape(-1, 6)
-            if len(si) != d.n_seq:
-                raise ValueError(f"scan_imu has {len(si)} rows, the step {d.n_seq}")
             self._ck(self.L.lins_gpu_seq_step_ex(self.h, C.byref(d), ptr(si)))
+
+    @staticmethod
+    def _seq_step_common(d, step, scan_imu, keep):
+        """Fill what every seq_step* descriptor d shares from `step` (n_seq, imu, imu_off and, when given, present) and check
+        scan_imu against n_seq.  The arrays d points at are added to `keep`.  Returns scan_imu as an (S x 6) array, or None."""
+        keep["imu"] = np.ascontiguousarray(step["imu"], dtype=np.float64)
+        keep["imu_off"] = np.ascontiguousarray(step["imu_off"], dtype=np.int32)
+        d.n_seq = len(keep["imu_off"]) - 1
+        d.imu, d.imu_off = keep["imu"].ctypes.data, keep["imu_off"].ctypes.data
+        if step.get("present") is not None:
+            keep["present"] = np.ascontiguousarray(step["present"], dtype=np.uint8)
+            d.present = keep["present"].ctypes.data
+        if scan_imu is None:
+            return None
+        si = keep["scan_imu"] = np.ascontiguousarray(scan_imu, dtype=np.float64).reshape(-1, 6)
+        if len(si) != d.n_seq:
+            raise ValueError(f"scan_imu has {len(si)} rows, the step {d.n_seq}")
+        return si
 
     @staticmethod
     def _pcl_desc(scans, line_num, keep):
@@ -526,20 +538,10 @@ class LinsGpu:
         """Advance every present sequence by one processPCL-shaped scan (lins_gpu_seq_step_pcl): `step` has imu + imu_off as
         in seq_step, scans (one segmented scan per slot, as extract_features takes them; an absent slot's may be empty) and
         optionally present."""
-        keep = {"imu": np.ascontiguousarray(step["imu"], dtype=np.float64), "imu_off": np.ascontiguousarray(step["imu_off"], dtype=np.int32)}
-        d = LinsSeqPclDesc()
+        keep, d = {}, LinsSeqPclDesc()
+        si = self._seq_step_common(d, step, scan_imu, keep)
         d.pcl = self._pcl_desc(step["scans"], line_num, keep)
-        d.n_seq = len(keep["imu_off"]) - 1
-        d.imu, d.imu_off = keep["imu"].ctypes.data, keep["imu_off"].ctypes.data
-        if step.get("present") is not None:
-            keep["present"] = np.ascontiguousarray(step["present"], dtype=np.uint8)
-            d.present = keep["present"].ctypes.data
         fp = fp or LinsFeatureParams.shipped()
-        si = None
-        if scan_imu is not None:
-            si = np.ascontiguousarray(scan_imu, dtype=np.float64).reshape(-1, 6)
-            if len(si) != d.n_seq:
-                raise ValueError(f"scan_imu has {len(si)} rows, the step {d.n_seq}")
         self._ck(self.L.lins_gpu_seq_step_pcl(self.h, C.byref(d), C.byref(fp), ptr(si)))
 
     def seq_step_raw(self, step, model=None, fp=None, scan_imu=None, point_format=0):
@@ -547,21 +549,11 @@ class LinsGpu:
         removal, feature extraction and the filter step on the device): `step` has imu + imu_off as in seq_step, sweeps (one
         raw sweep per slot, as project_scans takes them; an absent slot's may be empty) and optionally present.  model: the
         LinsLidarModel every slot shares (None = VLP-16)."""
-        keep = {"imu": np.ascontiguousarray(step["imu"], dtype=np.float64), "imu_off": np.ascontiguousarray(step["imu_off"], dtype=np.int32)}
-        d = LinsSeqRawDesc()
+        keep, d = {}, LinsSeqRawDesc()
+        si = self._seq_step_common(d, step, scan_imu, keep)
         d.raw = self._raw_desc(step["sweeps"], point_format, keep)
-        d.n_seq = len(keep["imu_off"]) - 1
-        d.imu, d.imu_off = keep["imu"].ctypes.data, keep["imu_off"].ctypes.data
-        if step.get("present") is not None:
-            keep["present"] = np.ascontiguousarray(step["present"], dtype=np.uint8)
-            d.present = keep["present"].ctypes.data
         model = model or LinsLidarModel.vlp16()
         fp = fp or LinsFeatureParams.shipped()
-        si = None
-        if scan_imu is not None:
-            si = np.ascontiguousarray(scan_imu, dtype=np.float64).reshape(-1, 6)
-            if len(si) != d.n_seq:
-                raise ValueError(f"scan_imu has {len(si)} rows, the step {d.n_seq}")
         self._ck(self.L.lins_gpu_seq_step_raw(self.h, C.byref(d), C.byref(model), C.byref(fp), ptr(si)))
 
     @staticmethod
@@ -605,21 +597,11 @@ class LinsGpu:
         """Advance every present sequence by one sensor_msgs/PointCloud2 message (lins_gpu_seq_step_cloud2: the decode, then
         what seq_step_raw runs): `step` has imu + imu_off as in seq_step, msgs (one (layout, data) per slot, as cloud2_desc
         takes them; an absent slot's is not read) or desc (a prepared LinsCloud2Desc), and optionally present."""
-        keep = {"imu": np.ascontiguousarray(step["imu"], dtype=np.float64), "imu_off": np.ascontiguousarray(step["imu_off"], dtype=np.int32)}
-        d = LinsSeqCloud2Desc()
+        keep, d = {}, LinsSeqCloud2Desc()
+        si = self._seq_step_common(d, step, scan_imu, keep)
         d.cloud2 = desc if desc is not None else self.cloud2_desc(step["msgs"], keep, gap)
-        d.n_seq = len(keep["imu_off"]) - 1
-        d.imu, d.imu_off = keep["imu"].ctypes.data, keep["imu_off"].ctypes.data
-        if step.get("present") is not None:
-            keep["present"] = np.ascontiguousarray(step["present"], dtype=np.uint8)
-            d.present = keep["present"].ctypes.data
         model = model or LinsLidarModel.vlp16()
         fp = fp or LinsFeatureParams.shipped()
-        si = None
-        if scan_imu is not None:
-            si = np.ascontiguousarray(scan_imu, dtype=np.float64).reshape(-1, 6)
-            if len(si) != d.n_seq:
-                raise ValueError(f"scan_imu has {len(si)} rows, the step {d.n_seq}")
         self._ck(self.L.lins_gpu_seq_step_cloud2(self.h, C.byref(d), C.byref(model), C.byref(fp), ptr(si)))
 
     def seq_download(self, reports=False):

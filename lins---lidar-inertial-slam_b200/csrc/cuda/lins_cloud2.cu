@@ -108,16 +108,14 @@ int cloud2_launch(lins_ctx* ctx, const lins_cloud2_desc* d, const std::vector<in
   CK(cudaMemcpyAsync(c.scans.p, c.h_scans.p, sizeof(Cloud2Scan) * sc.size(), cudaMemcpyHostToDevice, ctx->stream));
   CK(cudaMemcpyAsync(c.prefix.p, c.h_prefix.p, sizeof(int32_t) * off.size(), cudaMemcpyHostToDevice, ctx->stream));
   CK(cudaMemcpyAsync(up.qs_off.p, c.prefix.p, sizeof(int32_t) * off.size(), cudaMemcpyDeviceToDevice, ctx->stream));
-  if (!c.ev[0]) for (auto& e : c.ev) CK(cudaEventCreate(&e));
-  CK(cudaEventRecord(c.ev[0], ctx->stream));
+  CK(c.ev.start(ctx->stream));
   if (total > 0) {
     const int blocks = (int)std::min<int64_t>((total + kThreads - 1) / kThreads, (int64_t)ctx->sm_count * 16);
     lins_cloud2_decode_kernel<<<blocks, kThreads, 0, ctx->stream>>>(c.blob.p, c.scans.p, c.prefix.p, n, (int)total, up.qs.p);
     CK(cudaGetLastError());
     ctx->launches += 1;
   }
-  CK(cudaEventRecord(c.ev[1], ctx->stream));
-  c.ev_valid = true;
+  CK(c.ev.stop(ctx->stream));
   return LINS_OK;
 }
 
@@ -150,21 +148,14 @@ int lins_gpu_decode_cloud2(lins_ctx* ctx, const lins_cloud2_desc* d, lins_point*
   CK(c.h_out.reserve(total + 1));
   if (total) CK(cudaMemcpyAsync(c.h_out.p, ctx->proj.up.qs.p, sizeof(float4) * total, cudaMemcpyDeviceToHost, ctx->stream));
   CK(cudaStreamSynchronize(ctx->stream));
-  for (size_t i = 0; i < total; ++i) {
-    const float4 p = c.h_out.p[i];
-    lins_point& q = out[i];
-    q.x = p.x; q.y = p.y; q.z = p.z; q.pad0 = 1.0f; q.intensity = p.w; q.pad1 = q.pad2 = q.pad3 = 0.f;
-  }
+  for (size_t i = 0; i < total; ++i) out[i] = unpack_point(c.h_out.p[i]);
   if (counts) for (int i = 0; i < n; ++i) counts[i] = off[i + 1] - off[i];
   return LINS_OK;
 }
 
 int lins_gpu_decode_ms(lins_ctx* ctx, float* ms) {
   if (!ctx) return LINS_E_INVALID;
-  if (!ms) return fail(ctx, LINS_E_INVALID, "null ms");
-  if (!ctx->c2.ev_valid) return fail(ctx, LINS_E_NOMAP, "no decode has run");
-  CK(cudaEventElapsedTime(ms, ctx->c2.ev[0], ctx->c2.ev[1]));
-  return LINS_OK;
+  return event_ms(ctx, ctx->c2.ev, ms, "no decode has run");
 }
 
 }  // extern "C"

@@ -78,6 +78,28 @@ struct Resident {  // one resident batch (device) + its pinned staging (host)
   Buf<lins_report, kPinned> h_reports;
 };
 
+// A start / stop pair of CUDA events around device work on a stream, created on first use; valid once the stop has been
+// recorded (what lins_gpu_extract_ms, lins_gpu_project_ms and lins_gpu_decode_ms read)
+struct EventPair {
+  cudaEvent_t ev[2] = {nullptr, nullptr};
+  bool valid = false;
+  EventPair() = default;
+  EventPair(const EventPair&) = delete;
+  EventPair& operator=(const EventPair&) = delete;
+  ~EventPair() { for (cudaEvent_t e : ev) if (e) cudaEventDestroy(e); }
+  cudaError_t start(cudaStream_t s) {
+    if (!ev[0])
+      for (cudaEvent_t& e : ev) { const cudaError_t r = cudaEventCreate(&e); if (r != cudaSuccess) return r; }
+    return cudaEventRecord(ev[0], s);
+  }
+  cudaError_t stop(cudaStream_t s) {
+    const cudaError_t r = cudaEventRecord(ev[1], s);
+    if (r == cudaSuccess) valid = true;
+    return r;
+  }
+  cudaError_t elapsed_ms(float* ms) const { return cudaEventElapsedTime(ms, ev[0], ev[1]); }
+};
+
 // One contiguous device-to-device copy of sequence mode (lins_seq.cu): query compaction and the map refresh
 struct SeqCopy { const float4* src; float4* dst; int n, pad; };
 
@@ -138,9 +160,7 @@ struct FeatState {
   Buf<int, kPinned> h_counts;
   std::vector<int32_t> h_ring;
   Buf<SeqCopy> copies; Buf<SeqCopy, kPinned> h_copies;  // the pack into sequence mode's feature buffers
-  cudaEvent_t ev[2] = {nullptr, nullptr};               // around the last extraction kernel (lins_gpu_extract_ms)
-  bool ev_valid = false;
-  ~FeatState() { for (cudaEvent_t e : ev) if (e) cudaEventDestroy(e); }
+  EventPair ev;                                         // around the last extraction kernel (lins_gpu_extract_ms)
 };
 
 // Image projection (lins_projection.cu): the uploaded raw sweeps (up.qs, CSR in up.qs_off), each resident CTA's range-image
@@ -171,9 +191,7 @@ struct ProjState {
   Buf<int, kPinned> h_doff, h_ring;
   Buf<unsigned char> present;              // lins_gpu_seq_step_raw's present flags (n)
   Buf<unsigned char, kPinned> h_present;
-  cudaEvent_t ev[2] = {nullptr, nullptr};  // around the last projection kernel (lins_gpu_project_ms)
-  bool ev_valid = false;
-  ~ProjState() { for (cudaEvent_t e : ev) if (e) cudaEventDestroy(e); }
+  EventPair ev;                            // around the last projection kernel (lins_gpu_project_ms)
 };
 
 // One decode record per PointCloud2 message (lins_cloud2.cu): where its data field starts in the uploaded blob, where its
@@ -195,9 +213,7 @@ struct Cloud2State {
   Buf<Cloud2Scan> scans; Buf<Cloud2Scan, kPinned> h_scans;
   Buf<int> prefix; Buf<int, kPinned> h_prefix;  // n + 1: the first output point of each message (what qs_off holds)
   Buf<float4, kPinned> h_out;
-  cudaEvent_t ev[2] = {nullptr, nullptr};  // around the last decode kernel (lins_gpu_decode_ms)
-  bool ev_valid = false;
-  ~Cloud2State() { for (cudaEvent_t e : ev) if (e) cudaEventDestroy(e); }
+  EventPair ev;                            // around the last decode kernel (lins_gpu_decode_ms)
 };
 
 }  // namespace lins_capi
@@ -291,6 +307,21 @@ inline void pack_into(float4* dst, const lins_point* src, int n) {
   }
 #endif
   for (int i = 0; i < n; ++i) dst[i] = make_float4(src[i].x, src[i].y, src[i].z, src[i].intensity);
+}
+// (x, y, z, intensity) -> pcl::PointXYZI, the read-back of pack_into: pad0 = 1 as PCL_ADD_POINT4D sets it, the rest 0
+inline lins_point unpack_point(const float4& p) {
+  lins_point q;
+  q.x = p.x; q.y = p.y; q.z = p.z; q.pad0 = 1.0f; q.intensity = p.w; q.pad1 = q.pad2 = q.pad3 = 0.f;
+  return q;
+}
+
+// lins_gpu_extract_ms / lins_gpu_project_ms / lins_gpu_decode_ms: the CUDA-event time of e (none: the error when it has
+// not run)
+inline int event_ms(lins_ctx* ctx, const EventPair& e, float* ms, const char* none) {
+  if (!ms) return fail(ctx, LINS_E_INVALID, "null ms");
+  if (!e.valid) return fail(ctx, LINS_E_NOMAP, none);
+  CK(e.elapsed_ms(ms));
+  return LINS_OK;
 }
 
 // allocate the per-batch outputs / scratch for n scans with the given query totals

@@ -403,13 +403,11 @@ int features_launch(lins_ctx* ctx, const lins_feature_params* fp, const FeatInpu
   for (int k = 0; k < 4; ++k) a.out[k] = f.out[k].p;
   a.counts = f.counts.p;
   a.curv = f.curv.p; a.sind = f.sind.p; a.picked = f.picked.p; a.label = reinterpret_cast<signed char*>(f.label.p);
-  if (!f.ev[0]) for (auto& e : f.ev) CK(cudaEventCreate(&e));
-  CK(cudaEventRecord(f.ev[0], ctx->stream));
+  CK(f.ev.start(ctx->stream));
   lins_features_kernel<<<n, kThreads, 0, ctx->stream>>>(a);
   CK(cudaGetLastError());
   ctx->launches += 1;
-  CK(cudaEventRecord(f.ev[1], ctx->stream));
-  f.ev_valid = true;
+  CK(f.ev.stop(ctx->stream));
   CK(cudaMemcpyAsync(f.h_counts.p, f.counts.p, sizeof(int) * 5 * n, cudaMemcpyDeviceToHost, ctx->stream));
   CK(cudaStreamSynchronize(ctx->stream));
   for (int i = 0; i < n; ++i) {
@@ -448,7 +446,7 @@ int lins_gpu_extract_features(lins_ctx* ctx, const lins_feature_params* fp, cons
       for (int t = o; t < o + cnt; ++t) {
         const float4 p = h[t];
         if (d->point_format == LINS_POINTS_PACKED16) reinterpret_cast<float4*>(dst[k])[t] = p;
-        else { lins_point& q = dst[k][t]; q.x = p.x; q.y = p.y; q.z = p.z; q.pad0 = 1.0f; q.intensity = p.w; q.pad1 = q.pad2 = q.pad3 = 0.f; }
+        else dst[k][t] = unpack_point(p);
       }
     }
   }
@@ -458,10 +456,7 @@ int lins_gpu_extract_features(lins_ctx* ctx, const lins_feature_params* fp, cons
 
 int lins_gpu_extract_ms(lins_ctx* ctx, float* ms) {
   if (!ctx) return LINS_E_INVALID;
-  if (!ms) return fail(ctx, LINS_E_INVALID, "null ms");
-  if (!ctx->feat.ev_valid) return fail(ctx, LINS_E_NOMAP, "no extraction has run");
-  CK(cudaEventElapsedTime(ms, ctx->feat.ev[0], ctx->feat.ev[1]));
-  return LINS_OK;
+  return event_ms(ctx, ctx->feat.ev, ms, "no extraction has run");
 }
 
 }  // extern "C"

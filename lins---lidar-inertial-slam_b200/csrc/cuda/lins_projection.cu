@@ -347,13 +347,11 @@ int projection_launch(lins_ctx* ctx, const lins_lidar_model* m, int n, size_t to
   a.cnt = pr.cnt.p; a.rlo = pr.rlo.p; a.rhi = pr.rhi.p;
   a.seg = pr.seg.p; a.ground = pr.ground.p; a.col = pr.col.p; a.range = pr.range.p; a.outl = pr.outl.p;
   a.ring = pr.ring.p; a.ori = pr.ori.p; a.counts = pr.counts.p;
-  if (!pr.ev[0]) for (auto& e : pr.ev) CK(cudaEventCreate(&e));
-  CK(cudaEventRecord(pr.ev[0], ctx->stream));
+  CK(pr.ev.start(ctx->stream));
   lins_projection_kernel<<<grid, kThreads, 0, ctx->stream>>>(a);
   CK(cudaGetLastError());
   ctx->launches += 1;
-  CK(cudaEventRecord(pr.ev[1], ctx->stream));
-  pr.ev_valid = true;
+  CK(pr.ev.stop(ctx->stream));
   return LINS_OK;
 }
 
@@ -415,9 +413,8 @@ int lins_gpu_project_scans(lins_ctx* ctx, const lins_lidar_model* m, const lins_
   CK(cudaStreamSynchronize(ctx->stream));
   const bool p16 = d->point_format == LINS_POINTS_PACKED16;
   auto put = [&](lins_point* dst, int t, const float4& p) {
-    if (p16) { reinterpret_cast<float4*>(dst)[t] = p; return; }
-    lins_point& q = dst[t];
-    q.x = p.x; q.y = p.y; q.z = p.z; q.pad0 = 1.0f; q.intensity = p.w; q.pad1 = q.pad2 = q.pad3 = 0.f;
+    if (p16) reinterpret_cast<float4*>(dst)[t] = p;
+    else dst[t] = unpack_point(p);
   };
   for (int i = 0; i < n; ++i) {
     const int o = d->cloud_off[i], ns = pr.h_counts.p[2 * i], no = pr.h_counts.p[2 * i + 1], ds = doff[i], dq = doff[n + 1 + i];
@@ -437,10 +434,7 @@ int lins_gpu_project_scans(lins_ctx* ctx, const lins_lidar_model* m, const lins_
 
 int lins_gpu_project_ms(lins_ctx* ctx, float* ms) {
   if (!ctx) return LINS_E_INVALID;
-  if (!ms) return fail(ctx, LINS_E_INVALID, "null ms");
-  if (!ctx->proj.ev_valid) return fail(ctx, LINS_E_NOMAP, "no projection has run");
-  CK(cudaEventElapsedTime(ms, ctx->proj.ev[0], ctx->proj.ev[1]));
-  return LINS_OK;
+  return event_ms(ctx, ctx->proj.ev, ms, "no projection has run");
 }
 
 }  // extern "C"

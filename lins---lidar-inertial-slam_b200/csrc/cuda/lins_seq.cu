@@ -216,328 +216,121 @@ int run_copies(lins_ctx* ctx, const SeqCopy* dev, int count) {
   return LINS_OK;
 }
 
-}  // namespace
-
-static int seq_step_run(lins_ctx* ctx, const lins_seq_step_desc* d, const int32_t* const offs[4], const double* scan_imu);
-
-extern "C" {
-
-int lins_gpu_seq_begin(lins_ctx* ctx, const lins_seq_params* prm, const lins_seq_begin_desc* d) {
-  if (!ctx) return LINS_E_INVALID;
-  if (!prm || !d || d->n_seq < 1) return fail(ctx, LINS_E_INVALID, "bad sequence hand-over");
-  if (!d->filter_state || !d->filter_cov || !d->global_state || !d->imu_last) return fail(ctx, LINS_E_INVALID, "null hand-over state");
-  const int n = d->n_seq;
-  int rc = check_csr(ctx, d->surf_map_off, n, d->surf_map, "bad surf map offsets / cloud");
-  if (rc == LINS_OK) rc = check_csr(ctx, d->corner_map_off, n, d->corner_map, "bad corner map offsets / cloud");
-  if (rc != LINS_OK) return rc;
-  if (d->point_format != LINS_POINTS_XYZI32 && d->point_format != LINS_POINTS_PACKED16) return fail(ctx, LINS_E_INVALID, "bad point_format");
-  CK(cudaSetDevice(ctx->device));
-  SeqState& q = ctx->seq;
-  q.n = 0;  // (until the hand-over is in place)
-  // the maps go through the batch uploader as the target clouds of n units without queries
-  std::vector<int32_t> zeros(n + 1, 0);
-  const lins_point* pts[4] = {nullptr, nullptr, d->surf_map, d->corner_map};
-  const int32_t* offs[4] = {zeros.data(), zeros.data(), d->surf_map_off, d->corner_map_off};
-  rc = upload_clouds(ctx, q.up, n, pts, offs, d->point_format);
-  if (rc != LINS_OK) return rc;
-  const size_t ns = d->surf_map_off[n], nc = d->corner_map_off[n];
+// ---- slot lifecycle ------------------------------------------------------------------------------------------------------
+// every per-slot buffer of a run of n slots; ns / nc: the surf / corner maps it starts with
+int reserve_run(lins_ctx* ctx, SeqState& q, int n, size_t ns, size_t nc) {
   CK(q.filt.reserve((size_t)n * 20)); CK(q.cov.reserve((size_t)n * 324)); CK(q.glob.reserve((size_t)n * 20));
   CK(q.lin.reserve((size_t)n * 20)); CK(q.imu_last.reserve((size_t)n * 8)); CK(q.icp_pose.reserve((size_t)n * 20)); CK(q.icp.reserve(icp_state_bytes() * n));
   CK(q.map_s.reserve(ns + 1)); CK(q.map_c.reserve(nc + 1)); CK(q.tree_s.reserve(1)); CK(q.tree_c.reserve(1));
   CK(q.map_off.reserve(4 * (size_t)(n + 1))); CK(q.stale.reserve(n));
-  if (ns) CK(cudaMemcpyAsync(q.map_s.p, q.up.ts.p, sizeof(float4) * ns, cudaMemcpyDeviceToDevice, ctx->stream));
-  if (nc) CK(cudaMemcpyAsync(q.map_c.p, q.up.tc.p, sizeof(float4) * nc, cudaMemcpyDeviceToDevice, ctx->stream));
-  std::vector<double> st((size_t)n * 20, 0.0), gl((size_t)n * 20, 0.0), il((size_t)n * 8, 0.0);
-  for (int s = 0; s < n; ++s) {
-    std::memcpy(&st[(size_t)s * 20], d->filter_state + (size_t)s * 19, sizeof(double) * 19);
-    std::memcpy(&gl[(size_t)s * 20], d->global_state + (size_t)s * 19, sizeof(double) * 19);
-    std::memcpy(&il[(size_t)s * 8], d->imu_last + (size_t)s * 6, sizeof(double) * 6);
-  }
-  q.h_map_off.assign(4 * (size_t)(n + 1), 0);
-  std::memcpy(&q.h_map_off[0], d->surf_map_off, sizeof(int) * (n + 1));
-  std::memcpy(&q.h_map_off[n + 1], d->corner_map_off, sizeof(int) * (n + 1));
-  q.h_stale_v.assign(n, 0);
-  CK(cudaMemcpyAsync(q.filt.p, st.data(), sizeof(double) * st.size(), cudaMemcpyHostToDevice, ctx->stream));
-  CK(cudaMemcpyAsync(q.lin.p, st.data(), sizeof(double) * st.size(), cudaMemcpyHostToDevice, ctx->stream));
-  CK(cudaMemcpyAsync(q.glob.p, gl.data(), sizeof(double) * gl.size(), cudaMemcpyHostToDevice, ctx->stream));
-  CK(cudaMemcpyAsync(q.imu_last.p, il.data(), sizeof(double) * il.size(), cudaMemcpyHostToDevice, ctx->stream));
-  CK(cudaMemcpyAsync(q.cov.p, d->filter_cov, sizeof(double) * 324 * (size_t)n, cudaMemcpyHostToDevice, ctx->stream));
-  CK(cudaMemcpyAsync(q.map_off.p, q.h_map_off.data(), sizeof(int) * q.h_map_off.size(), cudaMemcpyHostToDevice, ctx->stream));
-  CK(cudaMemcpyAsync(q.stale.p, q.h_stale_v.data(), n, cudaMemcpyHostToDevice, ctx->stream));
-  CK(cudaStreamSynchronize(ctx->stream));  // (the sources above are pageable host memory)
-  set_consts(q, prm);
-  // result records / reports read as zero until a step has run a sequence's IESKF
   CK(q.run.results.reserve(n)); CK(q.run.reports.reserve(n));
-  CK(cudaMemsetAsync(q.run.results.p, 0, sizeof(lins_scan_result) * n, ctx->stream));
-  CK(cudaMemsetAsync(q.run.reports.p, 0, sizeof(lins_report) * n, ctx->stream));
-  q.ev_valid = false;
-  q.has_step = false;
-  q.status.assign(n, LINS_SEQ_IDLE);
-  q.has_init = false;
-  q.fusion.assign(n, FUSION_RUNNING);
-  q.n = n;
   return LINS_OK;
 }
 
-int lins_gpu_seq_open(lins_ctx* ctx, const lins_seq_params* prm, const lins_seq_init_params* ip, int32_t n_seq) {
-  if (!ctx) return LINS_E_INVALID;
-  if (!prm || !ip || n_seq < 1) return fail(ctx, LINS_E_INVALID, "bad lins_gpu_seq_open arguments");
-  CK(cudaSetDevice(ctx->device));
-  SeqState& q = ctx->seq;
-  q.n = 0;  // (until the slots are in place)
-  const int n = n_seq;
-  CK(q.filt.reserve((size_t)n * 20)); CK(q.cov.reserve((size_t)n * 324)); CK(q.glob.reserve((size_t)n * 20));
-  CK(q.lin.reserve((size_t)n * 20)); CK(q.imu_last.reserve((size_t)n * 8)); CK(q.icp_pose.reserve((size_t)n * 20)); CK(q.icp.reserve(icp_state_bytes() * n));
-  CK(q.pre.reserve((size_t)n * 20)); CK(q.init_icp.reserve(icp_state_bytes() * n));
-  CK(q.map_s.reserve(1)); CK(q.map_c.reserve(1)); CK(q.tree_s.reserve(1)); CK(q.tree_c.reserve(1));
-  CK(q.map_off.reserve(4 * (size_t)(n + 1))); CK(q.stale.reserve(n));
-  CK(q.run.results.reserve(n)); CK(q.run.reports.reserve(n));
-  set_consts(q, prm);
-  set_init_consts(q, prm, ip);
-  q.h_map_off.assign(4 * (size_t)(n + 1), 0);  // no maps
-  q.h_stale_v.assign(n, 0);
-  CK(cudaMemsetAsync(q.lin.p, 0, sizeof(double) * 20 * (size_t)n, ctx->stream));
-  CK(cudaMemsetAsync(q.imu_last.p, 0, sizeof(double) * 8 * (size_t)n, ctx->stream));
-  CK(cudaMemsetAsync(q.pre.p, 0, sizeof(double) * 20 * (size_t)n, ctx->stream));
-  CK(cudaMemsetAsync(q.icp_pose.p, 0, sizeof(double) * 20 * (size_t)n, ctx->stream));
-  CK(cudaMemsetAsync(q.init_icp.p, 0, icp_state_bytes() * n, ctx->stream));
-  CK(cudaMemsetAsync(q.run.results.p, 0, sizeof(lins_scan_result) * n, ctx->stream));
-  CK(cudaMemsetAsync(q.run.reports.p, 0, sizeof(lins_report) * n, ctx->stream));
-  CK(cudaMemcpyAsync(q.map_off.p, q.h_map_off.data(), sizeof(int) * q.h_map_off.size(), cudaMemcpyHostToDevice, ctx->stream));
-  CK(cudaMemcpyAsync(q.stale.p, q.h_stale_v.data(), n, cudaMemcpyHostToDevice, ctx->stream));
-  const int rc = launch_fresh(ctx, q, n, nullptr);
-  if (rc != LINS_OK) return rc;
-  CK(cudaStreamSynchronize(ctx->stream));  // (the sources above are pageable host memory)
+// the host side of a run whose slots are in place: no step yet, every slot idle in the given fusion status
+void install_run(SeqState& q, int n, bool has_init) {
   q.ev_valid = false;
   q.has_step = false;
   q.status.assign(n, LINS_SEQ_IDLE);
-  q.has_init = true;
-  q.fusion.assign(n, FUSION_INIT);
+  q.has_init = has_init;
+  q.fusion.assign(n, has_init ? FUSION_INIT : FUSION_RUNNING);
   q.n = n;
-  return LINS_OK;
 }
 
-int lins_gpu_seq_restart(lins_ctx* ctx, const uint8_t* mask) {
-  if (!ctx) return LINS_E_INVALID;
-  SeqState& q = ctx->seq;
-  if (q.n == 0) return fail(ctx, LINS_E_NOMAP, "no sequence run: call lins_gpu_seq_open");
-  if (!mask) return fail(ctx, LINS_E_INVALID, "null restart mask");
-  if (!q.has_init) return fail(ctx, LINS_E_INVALID, "lins_gpu_seq_restart needs a run opened by lins_gpu_seq_open");
-  CK(cudaSetDevice(ctx->device));
-  const int n = q.n, N1 = n + 1;
-  // the restarted slots' maps go: the other slots' ranges are copied into the next generation, which is swapped in
+// queue the upload of the host copies of map_off and stale (pageable: the caller synchronises before they change)
+cudaError_t queue_map_state(lins_ctx* ctx, SeqState& q) {
+  const cudaError_t e = cudaMemcpyAsync(q.map_off.p, q.h_map_off.data(), sizeof(int) * q.h_map_off.size(), cudaMemcpyHostToDevice, ctx->stream);
+  return e != cudaSuccess ? e : cudaMemcpyAsync(q.stale.p, q.h_stale_v.data(), q.h_stale_v.size(), cudaMemcpyHostToDevice, ctx->stream);
+}
+
+// ---- map generations -----------------------------------------------------------------------------------------------------
+// Where one (cloud, slot) range of the next generation comes from: len points at src
+struct MapPiece { const float4* src = nullptr; int len = 0; };
+
+// cloud c (map_s, map_c, tree_s, tree_c) of slot s in the current generation
+MapPiece current_piece(const SeqState& q, int c, int s) {
+  const int N1 = q.n + 1;
   const int* mo = q.h_map_off.data();
+  const float4* srcs[4] = {q.map_s.p, q.map_c.p, q.tree_s.p, q.tree_c.p};
+  return MapPiece{srcs[c] + mo[c * N1 + s], mo[c * N1 + s + 1] - mo[c * N1 + s]};
+}
+
+// The next generation from next[4 * s + c], slot s's cloud c: fills h_nmap_off, reserves nmap_* / ntree_* and appends the
+// copies that fill them, in slot order, to `copies`
+int build_next_maps(lins_ctx* ctx, SeqState& q, const std::vector<MapPiece>& next, std::vector<SeqCopy>& copies) {
+  const int n = q.n, N1 = n + 1;
   q.h_nmap_off.assign(4 * (size_t)N1, 0);
   int* no = q.h_nmap_off.data();
-  std::vector<SeqCopy> copies;
-  std::vector<std::pair<int, int>> to;
-  const float4* srcs[4] = {q.map_s.p, q.map_c.p, q.tree_s.p, q.tree_c.p};
-  for (int c = 0; c < 4; ++c)
-    for (int s = 0; s < n; ++s) {
-      const int len = mask[s] ? 0 : mo[c * N1 + s + 1] - mo[c * N1 + s];
-      no[c * N1 + s + 1] = no[c * N1 + s] + len;
-      if (len) { copies.push_back(SeqCopy{srcs[c] + mo[c * N1 + s], nullptr, len, 0}); to.emplace_back(c, no[c * N1 + s]); }
-    }
+  for (int s = 0; s < n; ++s)
+    for (int c = 0; c < 4; ++c) no[c * N1 + s + 1] = no[c * N1 + s] + next[4 * (size_t)s + c].len;
   CK(q.nmap_s.reserve((size_t)no[N1 - 1] + 1)); CK(q.nmap_c.reserve((size_t)no[2 * N1 - 1] + 1));
   CK(q.ntree_s.reserve((size_t)no[3 * N1 - 1] + 1)); CK(q.ntree_c.reserve((size_t)no[4 * N1 - 1] + 1));
-  CK(q.copies.reserve(copies.size() + 1)); CK(q.h_copies.reserve(copies.size() + 1));
-  CK(q.status_d.reserve(3 * (size_t)n)); CK(q.h_status.reserve(3 * (size_t)n));
   float4* dst[4] = {q.nmap_s.p, q.nmap_c.p, q.ntree_s.p, q.ntree_c.p};
-  for (size_t i = 0; i < copies.size(); ++i) copies[i].dst = dst[to[i].first] + to[i].second;
-  // (the last step ended with a stream synchronisation: the pinned staging is free)
-  std::copy(copies.begin(), copies.end(), q.h_copies.p);
-  for (int s = 0; s < n; ++s) q.h_status.p[s] = mask[s] ? 1 : 0;
-  if (!copies.empty()) CK(cudaMemcpyAsync(q.copies.p, q.h_copies.p, sizeof(SeqCopy) * copies.size(), cudaMemcpyHostToDevice, ctx->stream));
-  CK(cudaMemcpyAsync(q.status_d.p, q.h_status.p, n, cudaMemcpyHostToDevice, ctx->stream));
-  int rc = run_copies(ctx, q.copies.p, (int)copies.size());
-  if (rc == LINS_OK) rc = launch_fresh(ctx, q, n, q.status_d.p);
-  if (rc != LINS_OK) { q.n = 0; return rc; }  // (some slots may have changed: the run ends, as after a failed step)
-  std::swap(q.map_s, q.nmap_s); std::swap(q.map_c, q.nmap_c); std::swap(q.tree_s, q.ntree_s); std::swap(q.tree_c, q.ntree_c);
-  q.h_map_off.swap(q.h_nmap_off);
   for (int s = 0; s < n; ++s)
-    if (mask[s]) { q.h_stale_v[s] = 0; q.fusion[s] = FUSION_INIT; q.status[s] = LINS_SEQ_IDLE; }
-  CK(cudaMemcpyAsync(q.map_off.p, q.h_map_off.data(), sizeof(int) * 4 * N1, cudaMemcpyHostToDevice, ctx->stream));
-  CK(cudaMemcpyAsync(q.stale.p, q.h_stale_v.data(), n, cudaMemcpyHostToDevice, ctx->stream));
-  CK(cudaStreamSynchronize(ctx->stream));  // (the two sources above are pageable)
+    for (int c = 0; c < 4; ++c) {
+      const MapPiece& p = next[4 * (size_t)s + c];
+      if (p.len) copies.push_back(SeqCopy{p.src, dst[c] + no[c * N1 + s], p.len, 0});
+    }
   return LINS_OK;
 }
 
-int lins_gpu_seq_step_ex(lins_ctx* ctx, const lins_seq_step_desc* d, const double* scan_imu) {
+// the next generation becomes the current one (its copies have been queued)
+void swap_maps(SeqState& q) {
+  std::swap(q.map_s, q.nmap_s); std::swap(q.map_c, q.nmap_c); std::swap(q.tree_s, q.ntree_s); std::swap(q.tree_c, q.ntree_c);
+  q.h_map_off.swap(q.h_nmap_off);
+}
+
+// ---- a step ----------------------------------------------------------------------------------------------------------------
+// What every step entry checks before anything runs: the run, n_seq and n_scans (the number of scans d carries), the IMU
+// rows, and scan_imu while a present slot initialises
+template <typename Desc>
+int check_step(lins_ctx* ctx, const Desc* d, int n_scans, const double* scan_imu) {
   if (!ctx) return LINS_E_INVALID;
   SeqState& q = ctx->seq;
-  if (q.n == 0) return fail(ctx, LINS_E_NOMAP, "lins_gpu_seq_begin has not been called");
-  if (!d || d->n_seq != q.n) return fail(ctx, LINS_E_INVALID, "n_seq differs from the hand-over's");
   const int n = q.n;
-  const int32_t* offs[4] = {d->surf_flat_off, d->corner_sharp_off, d->surf_less_flat_off, d->corner_less_sharp_off};
-  const lins_point* pts[4] = {d->surf_flat, d->corner_sharp, d->surf_less_flat, d->corner_less_sharp};
-  for (int k = 0; k < 4; ++k) { const int rc = check_csr(ctx, offs[k], n, pts[k], "bad cloud offsets / cloud"); if (rc != LINS_OK) return rc; }
+  if (n == 0) return fail(ctx, LINS_E_NOMAP, "lins_gpu_seq_begin has not been called");
+  if (!d || d->n_seq != n || n_scans != n) return fail(ctx, LINS_E_INVALID, "n_seq differs from the hand-over's");
   if (d->imu_off) { const int rc = check_csr(ctx, d->imu_off, n, d->imu, "bad imu offsets / samples"); if (rc != LINS_OK) return rc; }
   else if (d->imu) return fail(ctx, LINS_E_INVALID, "imu without imu_off");
   if (!scan_imu)
     for (int s = 0; s < n; ++s)
       if ((!d->present || d->present[s]) && q.fusion[s] != FUSION_RUNNING)
         return fail(ctx, LINS_E_INVALID, "scan_imu is required while a present slot is initialising");
-  CK(cudaSetDevice(ctx->device));
-  int rc = upload_clouds(ctx, q.up, n, pts, offs, d->point_format);  // (validates the rest; synchronises the stream first)
-  if (rc != LINS_OK) return rc;
-  // from here on the sequences' state changes: a failure ends the run (lins_gpu.h), the context stays usable
-  rc = seq_step_run(ctx, d, offs, scan_imu);
-  if (rc != LINS_OK) q.n = 0;
-  return rc;
-}
-
-int lins_gpu_seq_step(lins_ctx* ctx, const lins_seq_step_desc* d) { return lins_gpu_seq_step_ex(ctx, d, nullptr); }
-
-}  // extern "C"
-
-namespace {
-
-// the IMU rows and scan_imu of a step from sweeps / segmented scans, checked before anything runs
-int check_step_imu(lins_ctx* ctx, const uint8_t* present, const double* imu, const int32_t* imu_off, const double* scan_imu) {
-  SeqState& q = ctx->seq;
-  const int n = q.n;
-  if (imu_off) { const int rc = check_csr(ctx, imu_off, n, imu, "bad imu offsets / samples"); if (rc != LINS_OK) return rc; }
-  else if (imu) return fail(ctx, LINS_E_INVALID, "imu without imu_off");
-  if (!scan_imu)
-    for (int s = 0; s < n; ++s)
-      if ((!present || present[s]) && q.fusion[s] != FUSION_RUNNING)
-        return fail(ctx, LINS_E_INVALID, "scan_imu is required while a present slot is initialising");
   return LINS_OK;
 }
 
-// The rest of a step whose features were extracted into ctx->feat (scan s's clouds at f.out[k] + src_off[s], counts read
-// back): the present slots' features -> the step's four clouds (q.up, lins_seq_step_desc order), dense in slot order,
-// then the sequence step.  A failure ends the run.
-int step_from_features(lins_ctx* ctx, const uint8_t* pres, const double* imu, const int32_t* imu_off, const int32_t* src_off,
-                       const double* scan_imu) {
-  SeqState& q = ctx->seq;
+// Query compaction: the surf / corner queries of the step's clouds (q.up.qs / qc at offs[0] / offs[1]) of the slots whose
+// status is `code`, packed from off[0] / off[N1] on (set by the caller).  Fills the rest of off (2 x (n + 1)), appends
+// their copies to `copies` with each destination (cloud, offset) in `to`, and returns the largest per-slot total.
+int compact_queries(const SeqState& q, const int32_t* const offs[4], int32_t code, std::vector<int>& off, std::vector<SeqCopy>& copies,
+                    std::vector<std::pair<int, int>>& to) {
   const int n = q.n, N1 = n + 1;
-  FeatState& f = ctx->feat;
-  Resident& r = q.up;
-  std::vector<int32_t> off(4 * (size_t)N1, 0);
-  r.max_q = 0;
+  int max_q = 0;
   for (int s = 0; s < n; ++s) {
-    const bool present = !pres || pres[s];
-    for (int k = 0; k < 4; ++k) off[k * N1 + s + 1] = off[k * N1 + s] + (present ? f.h_counts.p[5 * s + k] : 0);
-    r.max_q = std::max(r.max_q, (off[s + 1] - off[s]) + (off[N1 + s + 1] - off[N1 + s]));
-  }
-  r.n = n; r.nqs = off[N1 - 1]; r.nqc = off[2 * N1 - 1]; r.nts = off[3 * N1 - 1]; r.ntc = off[4 * N1 - 1];
-  CK(r.qs.reserve(r.nqs + 1)); CK(r.qc.reserve(r.nqc + 1)); CK(r.ts.reserve(r.nts + 1)); CK(r.tc.reserve(r.ntc + 1));
-  CK(r.qs_off.reserve(N1)); CK(r.qc_off.reserve(N1)); CK(r.ts_off.reserve(N1)); CK(r.tc_off.reserve(N1));
-  CK(r.h_off.reserve(4 * (size_t)N1));
-  float4* dst[4] = {r.qs.p, r.qc.p, r.ts.p, r.tc.p};
-  int* doff[4] = {r.qs_off.p, r.qc_off.p, r.ts_off.p, r.tc_off.p};
-  std::vector<SeqCopy> copies;
-  for (int k = 0; k < 4; ++k)
-    for (int s = 0; s < n; ++s) {
-      const int len = off[k * N1 + s + 1] - off[k * N1 + s];
-      if (len) copies.push_back(SeqCopy{f.out[k].p + src_off[s], dst[k] + off[k * N1 + s], len, 0});
+    const bool take = q.status[s] == code;
+    const int nq[2] = {take ? offs[0][s + 1] - offs[0][s] : 0, take ? offs[1][s + 1] - offs[1][s] : 0};
+    for (int c = 0; c < 2; ++c) {
+      off[c * N1 + s + 1] = off[c * N1 + s] + nq[c];
+      if (nq[c]) { copies.push_back(SeqCopy{(c ? q.up.qc.p : q.up.qs.p) + offs[c][s], nullptr, nq[c], 0}); to.emplace_back(c, off[c * N1 + s]); }
     }
-  CK(f.copies.reserve(copies.size() + 1)); CK(f.h_copies.reserve(copies.size() + 1));
-  std::copy(copies.begin(), copies.end(), f.h_copies.p);
-  std::memcpy(r.h_off.p, off.data(), sizeof(int) * off.size());
-  if (!copies.empty()) CK(cudaMemcpyAsync(f.copies.p, f.h_copies.p, sizeof(SeqCopy) * copies.size(), cudaMemcpyHostToDevice, ctx->stream));
-  for (int k = 0; k < 4; ++k) CK(cudaMemcpyAsync(doff[k], r.h_off.p + (size_t)k * N1, sizeof(int) * N1, cudaMemcpyHostToDevice, ctx->stream));
-  int rc = run_copies(ctx, f.copies.p, (int)copies.size());
-  if (rc != LINS_OK) return rc;
-  lins_seq_step_desc sd;
-  std::memset(&sd, 0, sizeof(sd));
-  sd.n_seq = n; sd.present = pres; sd.imu = imu; sd.imu_off = imu_off; sd.point_format = LINS_POINTS_XYZI32;
-  const int32_t* offs[4] = {&off[0], &off[N1], &off[2 * N1], &off[3 * N1]};
-  // from here on the sequences' state changes, as in lins_gpu_seq_step_ex
-  rc = seq_step_run(ctx, &sd, offs, scan_imu);
-  if (rc != LINS_OK) q.n = 0;
-  return rc;
+    max_q = std::max(max_q, nq[0] + nq[1]);
+  }
+  return max_q;
 }
 
-// The rest of a step whose sweeps' projection (with the NaN removal) is queued in ctx->proj at the raw offsets src_off:
-// the extraction on the projection's output where it lies (each scan's segmented count as its extent), one D2H +
-// synchronisation for the counts before the sequences change, then step_from_features.
-int step_from_projection(lins_ctx* ctx, const uint8_t* pres, const double* imu, const int32_t* imu_off, const lins_lidar_model* m,
-                         const lins_feature_params* fp, const int32_t* src_off, const double* scan_imu) {
-  const int n = ctx->seq.n;
-  ProjState& pr = ctx->proj;
-  FeatInputs in;
-  in.n = n; in.line_num = m->line_num; in.total = src_off[n];
-  in.pts = pr.seg.p; in.off = pr.up.qs_off.p; in.count = pr.counts.p; in.count_stride = 2;
-  in.ground = pr.ground.p; in.col = pr.col.p; in.range = pr.range.p; in.ring = pr.ring.p; in.ori = pr.ori.p;
-  const int rc = features_launch(ctx, fp, in);
-  if (rc != LINS_OK) return rc;
-  return step_from_features(ctx, pres, imu, imu_off, src_off, scan_imu);
-}
-
-}  // namespace
-
-extern "C" {
-
-int lins_gpu_seq_step_pcl(lins_ctx* ctx, const lins_seq_pcl_desc* d, const lins_feature_params* fp, const double* scan_imu) {
-  if (!ctx) return LINS_E_INVALID;
-  SeqState& q = ctx->seq;
-  if (q.n == 0) return fail(ctx, LINS_E_NOMAP, "lins_gpu_seq_begin has not been called");
-  if (!d || d->n_seq != q.n || d->pcl.n_scans != q.n) return fail(ctx, LINS_E_INVALID, "n_seq differs from the hand-over's");
-  int rc = check_step_imu(ctx, d->present, d->imu, d->imu_off, scan_imu);
-  if (rc != LINS_OK) return rc;
-  // extraction, validation of the scans and the counts' read-back: nothing of the sequences has changed yet
-  rc = features_run(ctx, fp, &d->pcl);
-  if (rc != LINS_OK) return rc;
-  return step_from_features(ctx, d->present, d->imu, d->imu_off, d->pcl.cloud_off, scan_imu);
-}
-
-int lins_gpu_seq_step_raw(lins_ctx* ctx, const lins_seq_raw_desc* d, const lins_lidar_model* m, const lins_feature_params* fp,
-                          const double* scan_imu) {
-  if (!ctx) return LINS_E_INVALID;
-  SeqState& q = ctx->seq;
-  if (q.n == 0) return fail(ctx, LINS_E_NOMAP, "lins_gpu_seq_begin has not been called");
-  if (!d || d->n_seq != q.n || d->raw.n_scans != q.n) return fail(ctx, LINS_E_INVALID, "n_seq differs from the hand-over's");
-  if (!fp) return fail(ctx, LINS_E_INVALID, "null feature params");
-  int rc = check_step_imu(ctx, d->present, d->imu, d->imu_off, scan_imu);
-  if (rc != LINS_OK) return rc;
-  // projection with copyPointCloud's NaN removal, then the rest of the step
-  rc = projection_run(ctx, m, &d->raw, true, d->present);
-  if (rc != LINS_OK) return rc;
-  return step_from_projection(ctx, d->present, d->imu, d->imu_off, m, fp, d->raw.cloud_off, scan_imu);
-}
-
-int lins_gpu_seq_step_cloud2(lins_ctx* ctx, const lins_seq_cloud2_desc* d, const lins_lidar_model* m, const lins_feature_params* fp,
-                             const double* scan_imu) {
-  if (!ctx) return LINS_E_INVALID;
-  SeqState& q = ctx->seq;
-  if (q.n == 0) return fail(ctx, LINS_E_NOMAP, "lins_gpu_seq_begin has not been called");
-  if (!d || d->n_seq != q.n || d->cloud2.n_scans != q.n) return fail(ctx, LINS_E_INVALID, "n_seq differs from the hand-over's");
-  if (!fp) return fail(ctx, LINS_E_INVALID, "null feature params");
-  int rc = check_step_imu(ctx, d->present, d->imu, d->imu_off, scan_imu);
-  if (rc != LINS_OK) return rc;
-  rc = check_model(ctx, m);
-  if (rc != LINS_OK) return rc;
-  // the messages decoded into the projection's input (the present slots' only), then step_raw's projection and the rest
-  std::vector<int32_t> off;
-  rc = cloud2_run(ctx, &d->cloud2, d->present, off);
-  if (rc != LINS_OK) return rc;
-  rc = projection_launch(ctx, m, q.n, (size_t)off[q.n], true, d->present);
-  if (rc != LINS_OK) return rc;
-  return step_from_projection(ctx, d->present, d->imu, d->imu_off, m, fp, off.data(), scan_imu);
-}
-
-}  // extern "C"
-
-// the part of lins_gpu_seq_step after its input is validated and uploaded
-static int seq_step_run(lins_ctx* ctx, const lins_seq_step_desc* d, const int32_t* const offs[4], const double* scan_imu) {
+// the phases of a step after its input is validated and uploaded (seq_step_run)
+int seq_step_phases(lins_ctx* ctx, const lins_seq_step_desc* d, const int32_t* const offs[4], const double* scan_imu) {
   SeqState& q = ctx->seq;
   const int n = q.n;
   int rc = LINS_OK;
 
   // ---- host bookkeeping: who runs, the compacted queries, the next maps (all from sizes the host knows) --------------
   std::vector<int32_t>& status = q.status;
-  const int* mo = q.h_map_off.data();
   const int N1 = n + 1;
-  std::vector<int> run_off(2 * (size_t)N1, 0);  // compacted query offsets: surf, corner
-  q.h_nmap_off.assign(4 * (size_t)N1, 0);
-  int* no = q.h_nmap_off.data();
-  std::vector<SeqCopy> qcopies, mcopies;
-  std::vector<std::pair<int, int>> qto, mto;  // destination of each copy: (cloud, offset), resolved once the buffers exist
+  std::vector<MapPiece> next(4 * (size_t)n);
   std::vector<unsigned char> new_stale(q.h_stale_v);
   std::vector<unsigned char> imu_use(n, IMU_IGNORE);
-  int max_q = 0, n_run = 0, n_init = 0, n_second = 0;
+  int n_run = 0, n_init = 0, n_second = 0;
   for (int s = 0; s < n; ++s) {
     const bool present = !d->present || d->present[s];
     const int nsl = offs[2][s + 1] - offs[2][s], ncl = offs[3][s + 1] - offs[3][s];
@@ -549,67 +342,44 @@ static int seq_step_run(lins_ctx* ctx, const lins_seq_step_desc* d, const int32_
     if (present) imu_use[s] = fs == FUSION_RUNNING ? IMU_PREDICT : fs == FUSION_FIRST_SCAN ? IMU_PREINTEGRATE : IMU_IGNORE;
     const bool ran = status[s] == LINS_SEQ_RAN;
     const bool init = status[s] == LINS_SEQ_FIRST || status[s] == LINS_SEQ_SECOND;
+    n_run += ran;
     n_init += init;
     n_second += status[s] == LINS_SEQ_SECOND;
-    const int nq[2] = {ran ? offs[0][s + 1] - offs[0][s] : 0, ran ? offs[1][s + 1] - offs[1][s] : 0};
-    for (int c = 0; c < 2; ++c) {
-      run_off[c * N1 + s + 1] = run_off[c * N1 + s] + nq[c];
-      if (nq[c]) { qcopies.push_back(SeqCopy{(c ? q.up.qc.p : q.up.qs.p) + offs[c][s], nullptr, nq[c], 0}); qto.emplace_back(c, run_off[c * N1 + s]); }
-    }
-    if (ran) { max_q = std::max(max_q, nq[0] + nq[1]); ++n_run; }
     // map swap (:1151-1160): the new clouds become the map; the 1-NN index is rebuilt iff ncl >= 5 && nsl >= 20, else it
     // stays on the cloud it was built on (the old map, or an older stale cloud).  A first scan's clouds become the map
     // as they are (setInputCloud, :363-364) and a second scan's like a running one's: both pass the guard after the init gate.
-    int len[4];  // map_s, map_c, tree_s, tree_c
-    int src_kind[4];  // 0 new cloud, 1 old map, 2 old tree, -1 none
+    MapPiece* p = &next[4 * (size_t)s];  // map_s, map_c, tree_s, tree_c
     if (ran || init) {
-      const bool guard = ncl >= 5 && nsl >= 20;
-      len[0] = nsl; len[1] = ncl; src_kind[0] = src_kind[1] = 0;
-      if (guard) { len[2] = len[3] = 0; src_kind[2] = src_kind[3] = -1; new_stale[s] = 0; }
-      else if (!q.h_stale_v[s]) { len[2] = mo[s + 1] - mo[s]; len[3] = mo[N1 + s + 1] - mo[N1 + s]; src_kind[2] = src_kind[3] = 1; new_stale[s] = 1; }
-      else { len[2] = mo[2 * N1 + s + 1] - mo[2 * N1 + s]; len[3] = mo[3 * N1 + s + 1] - mo[3 * N1 + s]; src_kind[2] = src_kind[3] = 2; }
+      p[0] = MapPiece{q.up.ts.p + offs[2][s], nsl};
+      p[1] = MapPiece{q.up.tc.p + offs[3][s], ncl};
+      if (ncl >= 5 && nsl >= 20) new_stale[s] = 0;
+      else if (!q.h_stale_v[s]) { p[2] = current_piece(q, 0, s); p[3] = current_piece(q, 1, s); new_stale[s] = 1; }
+      else { p[2] = current_piece(q, 2, s); p[3] = current_piece(q, 3, s); }
     } else {
-      for (int c = 0; c < 4; ++c) { len[c] = mo[c * N1 + s + 1] - mo[c * N1 + s]; src_kind[c] = c < 2 ? 1 : 2; }
-    }
-    for (int c = 0; c < 4; ++c) {
-      no[c * N1 + s + 1] = no[c * N1 + s] + len[c];
-      if (!len[c] || src_kind[c] < 0) continue;
-      const int cc = c & 1;  // surf / corner
-      const float4* src = nullptr;
-      if (src_kind[c] == 0) src = (cc ? q.up.tc.p : q.up.ts.p) + offs[2 + cc][s];
-      else if (src_kind[c] == 1) src = (cc ? q.map_c.p : q.map_s.p) + mo[cc * N1 + s];
-      else src = (cc ? q.tree_c.p : q.tree_s.p) + mo[(2 + cc) * N1 + s];
-      mcopies.push_back(SeqCopy{src, nullptr, len[c], 0});
-      mto.emplace_back(c, no[c * N1 + s]);
+      for (int c = 0; c < 4; ++c) p[c] = current_piece(q, c, s);
     }
   }
-  // the second scans' queries follow the IESKF's in the compacted buffers, with offsets of their own (init_off): the IESKF
-  // launch sees no query of theirs, the estimateTransform loop none of the IESKF's
-  std::vector<int> init_off(2 * (size_t)N1, 0);
-  int max_init_q = 0;
+  // the IESKF's queries, then the second scans' after them in the compacted buffers, with offsets of their own (init_off):
+  // the IESKF launch sees no query of theirs, the estimateTransform loop none of the IESKF's
+  std::vector<SeqCopy> qcopies, mcopies;
+  std::vector<std::pair<int, int>> qto;  // destination of each query copy: (cloud, offset), resolved once the buffers exist
+  std::vector<int> run_off(2 * (size_t)N1, 0), init_off(2 * (size_t)N1, 0);
+  const int max_q = compact_queries(q, offs, LINS_SEQ_RAN, run_off, qcopies, qto);
   for (int c = 0; c < 2; ++c) init_off[c * N1] = run_off[c * N1 + N1 - 1];
-  for (int s = 0; s < n; ++s) {
-    const bool second = status[s] == LINS_SEQ_SECOND;
-    const int nq[2] = {second ? offs[0][s + 1] - offs[0][s] : 0, second ? offs[1][s + 1] - offs[1][s] : 0};
-    for (int c = 0; c < 2; ++c) {
-      init_off[c * N1 + s + 1] = init_off[c * N1 + s] + nq[c];
-      if (nq[c]) { qcopies.push_back(SeqCopy{(c ? q.up.qc.p : q.up.qs.p) + offs[c][s], nullptr, nq[c], 0}); qto.emplace_back(c, init_off[c * N1 + s]); }
-    }
-    if (second) max_init_q = std::max(max_init_q, nq[0] + nq[1]);
-  }
+  const int max_init_q = compact_queries(q, offs, LINS_SEQ_SECOND, init_off, qcopies, qto);
 
   // ---- allocations ------------------------------------------------------------------------------------------------
   Resident& r = q.run;
   r.n = n; r.nqs = init_off[N1 - 1]; r.nqc = init_off[2 * N1 - 1]; r.max_q = max_q;
-  r.nts = mo[N1 - 1]; r.ntc = mo[2 * N1 - 1];
+  r.nts = q.h_map_off[N1 - 1]; r.ntc = q.h_map_off[2 * N1 - 1];
   CK(r.qs.reserve(r.nqs + 1)); CK(r.qc.reserve(r.nqc + 1)); CK(r.qs_off.reserve(N1)); CK(r.qc_off.reserve(N1));
   rc = reserve_outputs(ctx, r, true, false);
   if (rc != LINS_OK) return rc;
   CK(r.h_off.reserve(4 * (size_t)N1));
   if (n_init) { CK(q.init_off.reserve(2 * (size_t)N1)); CK(q.scan_imu.reserve((size_t)n * 6)); CK(q.h_scan_imu.reserve((size_t)n * 6)); }
   // (pre and init_icp are lins_gpu_seq_open's: they keep their contents from step to step)
-  CK(q.nmap_s.reserve((size_t)no[N1 - 1] + 1)); CK(q.nmap_c.reserve((size_t)no[2 * N1 - 1] + 1));
-  CK(q.ntree_s.reserve((size_t)no[3 * N1 - 1] + 1)); CK(q.ntree_c.reserve((size_t)no[4 * N1 - 1] + 1));
+  rc = build_next_maps(ctx, q, next, mcopies);
+  if (rc != LINS_OK) return rc;
   const size_t n_imu = d->imu_off ? (size_t)d->imu_off[n] : 0;
   CK(q.imu.reserve(7 * n_imu + 1)); CK(q.imu_off.reserve(N1)); CK(q.h_imu.reserve(7 * n_imu + 1)); CK(q.h_imu_off.reserve(N1));
   CK(q.status_d.reserve(3 * (size_t)n)); CK(q.h_status.reserve(3 * (size_t)n));
@@ -618,9 +388,7 @@ static int seq_step_run(lins_ctx* ctx, const lins_seq_step_desc* d, const int32_
   CK(q.prior_state.reserve((size_t)n * 20)); CK(q.prior_cov.reserve((size_t)n * 324));
   CK(q.icp_ind_s.reserve(3 * r.nqs + 4)); CK(q.icp_ind_c.reserve(2 * r.nqc + 4));
   float4* qdst[2] = {r.qs.p, r.qc.p};
-  float4* mdst[4] = {q.nmap_s.p, q.nmap_c.p, q.ntree_s.p, q.ntree_c.p};
   for (size_t i = 0; i < qcopies.size(); ++i) qcopies[i].dst = qdst[qto[i].first] + qto[i].second;
-  for (size_t i = 0; i < mcopies.size(); ++i) mcopies[i].dst = mdst[mto[i].first] + mto[i].second;
 
   // ---- uploads: IMU, status, copy lists, compacted query offsets ---------------------------------------------------
   if (d->imu_off) std::memcpy(q.h_imu_off.p, d->imu_off, sizeof(int) * N1);
@@ -758,11 +526,9 @@ static int seq_step_run(lins_ctx* ctx, const lins_seq_step_desc* d, const int32_
   if (rc == LINS_OK) rc = transform_to_end_csr(ctx, q.up.tc.p, q.up.tc_off.p, n, q.lin.p, run_mask);
   if (rc == LINS_OK) rc = run_copies(ctx, q.copies.p + qcopies.size(), (int)mcopies.size());
   if (rc != LINS_OK) return rc;
-  std::swap(q.map_s, q.nmap_s); std::swap(q.map_c, q.nmap_c); std::swap(q.tree_s, q.ntree_s); std::swap(q.tree_c, q.ntree_c);
-  q.h_map_off.swap(q.h_nmap_off);
+  swap_maps(q);
   q.h_stale_v = new_stale;
-  CK(cudaMemcpyAsync(q.map_off.p, q.h_map_off.data(), sizeof(int) * 4 * N1, cudaMemcpyHostToDevice, ctx->stream));
-  CK(cudaMemcpyAsync(q.stale.p, q.h_stale_v.data(), n, cudaMemcpyHostToDevice, ctx->stream));
+  CK(queue_map_state(ctx, q));
   CK(cudaEventRecord(q.ev[4], ctx->stream));
   CK(cudaStreamSynchronize(ctx->stream));  // (the two sources above are pageable and change with the next step)
   for (int s = 0; s < n; ++s) {  // processPCL's status transitions (:294-307)
@@ -776,7 +542,237 @@ static int seq_step_run(lins_ctx* ctx, const lins_seq_step_desc* d, const int32_
   return LINS_OK;
 }
 
+// The part of a step after its input is validated and uploaded.  From here on the sequences' state changes: a failure ends
+// the run (lins_gpu.h), the context stays usable.
+int seq_step_run(lins_ctx* ctx, const lins_seq_step_desc* d, const int32_t* const offs[4], const double* scan_imu) {
+  const int rc = seq_step_phases(ctx, d, offs, scan_imu);
+  if (rc != LINS_OK) ctx->seq.n = 0;
+  return rc;
+}
+
+// The rest of a step whose features were extracted into ctx->feat (scan s's clouds at f.out[k] + src_off[s], counts read
+// back): the present slots' features -> the step's four clouds (q.up, lins_seq_step_desc order), dense in slot order,
+// then the sequence step.
+int step_from_features(lins_ctx* ctx, const uint8_t* pres, const double* imu, const int32_t* imu_off, const int32_t* src_off,
+                       const double* scan_imu) {
+  SeqState& q = ctx->seq;
+  const int n = q.n, N1 = n + 1;
+  FeatState& f = ctx->feat;
+  Resident& r = q.up;
+  std::vector<int32_t> off(4 * (size_t)N1, 0);
+  r.max_q = 0;
+  for (int s = 0; s < n; ++s) {
+    const bool present = !pres || pres[s];
+    for (int k = 0; k < 4; ++k) off[k * N1 + s + 1] = off[k * N1 + s] + (present ? f.h_counts.p[5 * s + k] : 0);
+    r.max_q = std::max(r.max_q, (off[s + 1] - off[s]) + (off[N1 + s + 1] - off[N1 + s]));
+  }
+  r.n = n; r.nqs = off[N1 - 1]; r.nqc = off[2 * N1 - 1]; r.nts = off[3 * N1 - 1]; r.ntc = off[4 * N1 - 1];
+  CK(r.qs.reserve(r.nqs + 1)); CK(r.qc.reserve(r.nqc + 1)); CK(r.ts.reserve(r.nts + 1)); CK(r.tc.reserve(r.ntc + 1));
+  CK(r.qs_off.reserve(N1)); CK(r.qc_off.reserve(N1)); CK(r.ts_off.reserve(N1)); CK(r.tc_off.reserve(N1));
+  CK(r.h_off.reserve(4 * (size_t)N1));
+  float4* dst[4] = {r.qs.p, r.qc.p, r.ts.p, r.tc.p};
+  int* doff[4] = {r.qs_off.p, r.qc_off.p, r.ts_off.p, r.tc_off.p};
+  std::vector<SeqCopy> copies;
+  for (int k = 0; k < 4; ++k)
+    for (int s = 0; s < n; ++s) {
+      const int len = off[k * N1 + s + 1] - off[k * N1 + s];
+      if (len) copies.push_back(SeqCopy{f.out[k].p + src_off[s], dst[k] + off[k * N1 + s], len, 0});
+    }
+  CK(f.copies.reserve(copies.size() + 1)); CK(f.h_copies.reserve(copies.size() + 1));
+  std::copy(copies.begin(), copies.end(), f.h_copies.p);
+  std::memcpy(r.h_off.p, off.data(), sizeof(int) * off.size());
+  if (!copies.empty()) CK(cudaMemcpyAsync(f.copies.p, f.h_copies.p, sizeof(SeqCopy) * copies.size(), cudaMemcpyHostToDevice, ctx->stream));
+  for (int k = 0; k < 4; ++k) CK(cudaMemcpyAsync(doff[k], r.h_off.p + (size_t)k * N1, sizeof(int) * N1, cudaMemcpyHostToDevice, ctx->stream));
+  int rc = run_copies(ctx, f.copies.p, (int)copies.size());
+  if (rc != LINS_OK) return rc;
+  lins_seq_step_desc sd;
+  std::memset(&sd, 0, sizeof(sd));
+  sd.n_seq = n; sd.present = pres; sd.imu = imu; sd.imu_off = imu_off; sd.point_format = LINS_POINTS_XYZI32;
+  const int32_t* offs[4] = {&off[0], &off[N1], &off[2 * N1], &off[3 * N1]};
+  return seq_step_run(ctx, &sd, offs, scan_imu);
+}
+
+// The rest of a step whose sweeps' projection (with the NaN removal) is queued in ctx->proj at the raw offsets src_off:
+// the extraction on the projection's output where it lies (each scan's segmented count as its extent), one D2H +
+// synchronisation for the counts before the sequences change, then step_from_features.
+int step_from_projection(lins_ctx* ctx, const uint8_t* pres, const double* imu, const int32_t* imu_off, const lins_lidar_model* m,
+                         const lins_feature_params* fp, const int32_t* src_off, const double* scan_imu) {
+  const int n = ctx->seq.n;
+  ProjState& pr = ctx->proj;
+  FeatInputs in;
+  in.n = n; in.line_num = m->line_num; in.total = src_off[n];
+  in.pts = pr.seg.p; in.off = pr.up.qs_off.p; in.count = pr.counts.p; in.count_stride = 2;
+  in.ground = pr.ground.p; in.col = pr.col.p; in.range = pr.range.p; in.ring = pr.ring.p; in.ori = pr.ori.p;
+  const int rc = features_launch(ctx, fp, in);
+  if (rc != LINS_OK) return rc;
+  return step_from_features(ctx, pres, imu, imu_off, src_off, scan_imu);
+}
+
+}  // namespace
+
 extern "C" {
+
+int lins_gpu_seq_begin(lins_ctx* ctx, const lins_seq_params* prm, const lins_seq_begin_desc* d) {
+  if (!ctx) return LINS_E_INVALID;
+  if (!prm || !d || d->n_seq < 1) return fail(ctx, LINS_E_INVALID, "bad sequence hand-over");
+  if (!d->filter_state || !d->filter_cov || !d->global_state || !d->imu_last) return fail(ctx, LINS_E_INVALID, "null hand-over state");
+  const int n = d->n_seq;
+  int rc = check_csr(ctx, d->surf_map_off, n, d->surf_map, "bad surf map offsets / cloud");
+  if (rc == LINS_OK) rc = check_csr(ctx, d->corner_map_off, n, d->corner_map, "bad corner map offsets / cloud");
+  if (rc != LINS_OK) return rc;
+  if (d->point_format != LINS_POINTS_XYZI32 && d->point_format != LINS_POINTS_PACKED16) return fail(ctx, LINS_E_INVALID, "bad point_format");
+  CK(cudaSetDevice(ctx->device));
+  SeqState& q = ctx->seq;
+  q.n = 0;  // (until the hand-over is in place)
+  // the maps go through the batch uploader as the target clouds of n units without queries
+  std::vector<int32_t> zeros(n + 1, 0);
+  const lins_point* pts[4] = {nullptr, nullptr, d->surf_map, d->corner_map};
+  const int32_t* offs[4] = {zeros.data(), zeros.data(), d->surf_map_off, d->corner_map_off};
+  rc = upload_clouds(ctx, q.up, n, pts, offs, d->point_format);
+  if (rc != LINS_OK) return rc;
+  const size_t ns = d->surf_map_off[n], nc = d->corner_map_off[n];
+  rc = reserve_run(ctx, q, n, ns, nc);
+  if (rc != LINS_OK) return rc;
+  if (ns) CK(cudaMemcpyAsync(q.map_s.p, q.up.ts.p, sizeof(float4) * ns, cudaMemcpyDeviceToDevice, ctx->stream));
+  if (nc) CK(cudaMemcpyAsync(q.map_c.p, q.up.tc.p, sizeof(float4) * nc, cudaMemcpyDeviceToDevice, ctx->stream));
+  std::vector<double> st((size_t)n * 20, 0.0), gl((size_t)n * 20, 0.0), il((size_t)n * 8, 0.0);
+  for (int s = 0; s < n; ++s) {
+    std::memcpy(&st[(size_t)s * 20], d->filter_state + (size_t)s * 19, sizeof(double) * 19);
+    std::memcpy(&gl[(size_t)s * 20], d->global_state + (size_t)s * 19, sizeof(double) * 19);
+    std::memcpy(&il[(size_t)s * 8], d->imu_last + (size_t)s * 6, sizeof(double) * 6);
+  }
+  q.h_map_off.assign(4 * (size_t)(n + 1), 0);
+  std::memcpy(&q.h_map_off[0], d->surf_map_off, sizeof(int) * (n + 1));
+  std::memcpy(&q.h_map_off[n + 1], d->corner_map_off, sizeof(int) * (n + 1));
+  q.h_stale_v.assign(n, 0);
+  CK(cudaMemcpyAsync(q.filt.p, st.data(), sizeof(double) * st.size(), cudaMemcpyHostToDevice, ctx->stream));
+  CK(cudaMemcpyAsync(q.lin.p, st.data(), sizeof(double) * st.size(), cudaMemcpyHostToDevice, ctx->stream));
+  CK(cudaMemcpyAsync(q.glob.p, gl.data(), sizeof(double) * gl.size(), cudaMemcpyHostToDevice, ctx->stream));
+  CK(cudaMemcpyAsync(q.imu_last.p, il.data(), sizeof(double) * il.size(), cudaMemcpyHostToDevice, ctx->stream));
+  CK(cudaMemcpyAsync(q.cov.p, d->filter_cov, sizeof(double) * 324 * (size_t)n, cudaMemcpyHostToDevice, ctx->stream));
+  CK(queue_map_state(ctx, q));
+  CK(cudaStreamSynchronize(ctx->stream));  // (the sources above are pageable host memory)
+  set_consts(q, prm);
+  // result records / reports read as zero until a step has run a sequence's IESKF
+  CK(cudaMemsetAsync(q.run.results.p, 0, sizeof(lins_scan_result) * n, ctx->stream));
+  CK(cudaMemsetAsync(q.run.reports.p, 0, sizeof(lins_report) * n, ctx->stream));
+  install_run(q, n, false);
+  return LINS_OK;
+}
+
+int lins_gpu_seq_open(lins_ctx* ctx, const lins_seq_params* prm, const lins_seq_init_params* ip, int32_t n_seq) {
+  if (!ctx) return LINS_E_INVALID;
+  if (!prm || !ip || n_seq < 1) return fail(ctx, LINS_E_INVALID, "bad lins_gpu_seq_open arguments");
+  CK(cudaSetDevice(ctx->device));
+  SeqState& q = ctx->seq;
+  q.n = 0;  // (until the slots are in place)
+  const int n = n_seq;
+  int rc = reserve_run(ctx, q, n, 0, 0);  // (no maps)
+  if (rc != LINS_OK) return rc;
+  CK(q.pre.reserve((size_t)n * 20)); CK(q.init_icp.reserve(icp_state_bytes() * n));
+  set_consts(q, prm);
+  set_init_consts(q, prm, ip);
+  q.h_map_off.assign(4 * (size_t)(n + 1), 0);
+  q.h_stale_v.assign(n, 0);
+  CK(cudaMemsetAsync(q.lin.p, 0, sizeof(double) * 20 * (size_t)n, ctx->stream));
+  CK(cudaMemsetAsync(q.imu_last.p, 0, sizeof(double) * 8 * (size_t)n, ctx->stream));
+  CK(cudaMemsetAsync(q.pre.p, 0, sizeof(double) * 20 * (size_t)n, ctx->stream));
+  CK(cudaMemsetAsync(q.icp_pose.p, 0, sizeof(double) * 20 * (size_t)n, ctx->stream));
+  CK(cudaMemsetAsync(q.init_icp.p, 0, icp_state_bytes() * n, ctx->stream));
+  CK(cudaMemsetAsync(q.run.results.p, 0, sizeof(lins_scan_result) * n, ctx->stream));
+  CK(cudaMemsetAsync(q.run.reports.p, 0, sizeof(lins_report) * n, ctx->stream));
+  CK(queue_map_state(ctx, q));
+  rc = launch_fresh(ctx, q, n, nullptr);
+  if (rc != LINS_OK) return rc;
+  CK(cudaStreamSynchronize(ctx->stream));  // (the sources above are pageable host memory)
+  install_run(q, n, true);
+  return LINS_OK;
+}
+
+int lins_gpu_seq_restart(lins_ctx* ctx, const uint8_t* mask) {
+  if (!ctx) return LINS_E_INVALID;
+  SeqState& q = ctx->seq;
+  if (q.n == 0) return fail(ctx, LINS_E_NOMAP, "no sequence run: call lins_gpu_seq_open");
+  if (!mask) return fail(ctx, LINS_E_INVALID, "null restart mask");
+  if (!q.has_init) return fail(ctx, LINS_E_INVALID, "lins_gpu_seq_restart needs a run opened by lins_gpu_seq_open");
+  CK(cudaSetDevice(ctx->device));
+  const int n = q.n;
+  // the restarted slots' maps go: the other slots' ranges are copied into the next generation, which is swapped in
+  std::vector<MapPiece> next(4 * (size_t)n);
+  for (int s = 0; s < n; ++s)
+    if (!mask[s]) for (int c = 0; c < 4; ++c) next[4 * (size_t)s + c] = current_piece(q, c, s);
+  std::vector<SeqCopy> copies;
+  int rc = build_next_maps(ctx, q, next, copies);
+  if (rc != LINS_OK) return rc;
+  CK(q.copies.reserve(copies.size() + 1)); CK(q.h_copies.reserve(copies.size() + 1));
+  CK(q.status_d.reserve(3 * (size_t)n)); CK(q.h_status.reserve(3 * (size_t)n));
+  // (the last step ended with a stream synchronisation: the pinned staging is free)
+  std::copy(copies.begin(), copies.end(), q.h_copies.p);
+  for (int s = 0; s < n; ++s) q.h_status.p[s] = mask[s] ? 1 : 0;
+  if (!copies.empty()) CK(cudaMemcpyAsync(q.copies.p, q.h_copies.p, sizeof(SeqCopy) * copies.size(), cudaMemcpyHostToDevice, ctx->stream));
+  CK(cudaMemcpyAsync(q.status_d.p, q.h_status.p, n, cudaMemcpyHostToDevice, ctx->stream));
+  rc = run_copies(ctx, q.copies.p, (int)copies.size());
+  if (rc == LINS_OK) rc = launch_fresh(ctx, q, n, q.status_d.p);
+  if (rc != LINS_OK) { q.n = 0; return rc; }  // (some slots may have changed: the run ends, as after a failed step)
+  swap_maps(q);
+  for (int s = 0; s < n; ++s)
+    if (mask[s]) { q.h_stale_v[s] = 0; q.fusion[s] = FUSION_INIT; q.status[s] = LINS_SEQ_IDLE; }
+  CK(queue_map_state(ctx, q));
+  CK(cudaStreamSynchronize(ctx->stream));  // (the two sources above are pageable)
+  return LINS_OK;
+}
+
+int lins_gpu_seq_step_ex(lins_ctx* ctx, const lins_seq_step_desc* d, const double* scan_imu) {
+  int rc = check_step(ctx, d, d ? d->n_seq : 0, scan_imu);
+  if (rc != LINS_OK) return rc;
+  const int n = ctx->seq.n;
+  const int32_t* offs[4] = {d->surf_flat_off, d->corner_sharp_off, d->surf_less_flat_off, d->corner_less_sharp_off};
+  const lins_point* pts[4] = {d->surf_flat, d->corner_sharp, d->surf_less_flat, d->corner_less_sharp};
+  for (int k = 0; k < 4; ++k) { rc = check_csr(ctx, offs[k], n, pts[k], "bad cloud offsets / cloud"); if (rc != LINS_OK) return rc; }
+  CK(cudaSetDevice(ctx->device));
+  rc = upload_clouds(ctx, ctx->seq.up, n, pts, offs, d->point_format);  // (validates the rest; synchronises the stream first)
+  if (rc != LINS_OK) return rc;
+  return seq_step_run(ctx, d, offs, scan_imu);
+}
+
+int lins_gpu_seq_step(lins_ctx* ctx, const lins_seq_step_desc* d) { return lins_gpu_seq_step_ex(ctx, d, nullptr); }
+
+int lins_gpu_seq_step_pcl(lins_ctx* ctx, const lins_seq_pcl_desc* d, const lins_feature_params* fp, const double* scan_imu) {
+  int rc = check_step(ctx, d, d ? d->pcl.n_scans : 0, scan_imu);
+  if (rc != LINS_OK) return rc;
+  // extraction, validation of the scans and the counts' read-back: nothing of the sequences has changed yet
+  rc = features_run(ctx, fp, &d->pcl);
+  if (rc != LINS_OK) return rc;
+  return step_from_features(ctx, d->present, d->imu, d->imu_off, d->pcl.cloud_off, scan_imu);
+}
+
+int lins_gpu_seq_step_raw(lins_ctx* ctx, const lins_seq_raw_desc* d, const lins_lidar_model* m, const lins_feature_params* fp,
+                          const double* scan_imu) {
+  int rc = check_step(ctx, d, d ? d->raw.n_scans : 0, scan_imu);
+  if (rc != LINS_OK) return rc;
+  if (!fp) return fail(ctx, LINS_E_INVALID, "null feature params");
+  // projection with copyPointCloud's NaN removal, then the rest of the step
+  rc = projection_run(ctx, m, &d->raw, true, d->present);
+  if (rc != LINS_OK) return rc;
+  return step_from_projection(ctx, d->present, d->imu, d->imu_off, m, fp, d->raw.cloud_off, scan_imu);
+}
+
+int lins_gpu_seq_step_cloud2(lins_ctx* ctx, const lins_seq_cloud2_desc* d, const lins_lidar_model* m, const lins_feature_params* fp,
+                             const double* scan_imu) {
+  int rc = check_step(ctx, d, d ? d->cloud2.n_scans : 0, scan_imu);
+  if (rc != LINS_OK) return rc;
+  if (!fp) return fail(ctx, LINS_E_INVALID, "null feature params");
+  rc = check_model(ctx, m);
+  if (rc != LINS_OK) return rc;
+  // the messages decoded into the projection's input (the present slots' only), then step_raw's projection and the rest
+  const int n = ctx->seq.n;
+  std::vector<int32_t> off;
+  rc = cloud2_run(ctx, &d->cloud2, d->present, off);
+  if (rc != LINS_OK) return rc;
+  rc = projection_launch(ctx, m, n, (size_t)off[n], true, d->present);
+  if (rc != LINS_OK) return rc;
+  return step_from_projection(ctx, d->present, d->imu, d->imu_off, m, fp, off.data(), scan_imu);
+}
 
 int lins_gpu_seq_phase_ms(lins_ctx* ctx, float* ms) {
   if (!ctx || !ms) return LINS_E_INVALID;

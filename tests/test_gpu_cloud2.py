@@ -196,22 +196,12 @@ def drive(capi, defs, baglib, logs, n_slots, jobs, layout, alt=False, gap=3):
         g.seq_open(defs.LinsSeqParams.shipped(), init_params(defs), n_slots)
         ctxs.append(g)
     g, tw = ctxs
-    cur, used, nxt, t = [None] * n_slots, [False] * n_slots, 0, 0
+    t = 0
     rows = [[] for _ in jobs]
-    while True:
-        restart = np.zeros(n_slots, np.uint8)
-        for j in range(n_slots):
-            if cur[j] is not None and cur[j][1] >= len(logs[jobs[cur[j][0]]]["time"]):
-                cur[j] = None
-            if cur[j] is None and nxt < len(jobs):
-                restart[j], cur[j], used[j] = used[j], [nxt, 0], True
-                nxt += 1
-        if all(c is None for c in cur):
-            break
+    for restart, who in pkg("bag_replay").slot_queue([len(logs[i]["time"]) for i in jobs], n_slots):
         if restart.any():
             for c in ctxs:
                 c.seq_restart(restart)
-        who = [(c[0], c[1]) if c is not None else None for c in cur]
         imus, si, ins, sweeps = [], np.zeros((n_slots, 6)), [], []
         for j, w in enumerate(who):
             if w is None:
@@ -221,7 +211,6 @@ def drive(capi, defs, baglib, logs, n_slots, jobs, layout, alt=False, gap=3):
             o = l["imu_off"]
             imus.append(l["imu"][o[k]:o[k + 1]]); si[j] = l["imu_last"][k]
             ins.append(cc.as_input(defs, msgs[jobs[w[0]]][k])); sweeps.append(host[jobs[w[0]]][k])
-            cur[j][1] += 1
         imu = np.concatenate(imus).reshape(-1, 7)
         imu_off = np.concatenate([[0], np.cumsum([len(r) for r in imus])]).astype(np.int32)
         pres = np.array([w is not None for w in who], np.uint8)

@@ -34,36 +34,19 @@ def drive(capi, defs, logs, n_slots, jobs, params=None):
     synth = pkg("synth")
     g = capi.LinsGpu(params)
     g.seq_open(defs.LinsSeqParams.shipped(), init_params(defs), n_slots)
-    cur = [None] * n_slots  # [job index, next event]
-    used = [False] * n_slots
-    nxt = 0
     rows, steps = [[] for _ in jobs], []
     empty = {c: logs[0][c][:0] for c in defs.Batch.FIELDS}
-    while True:
-        restart = np.zeros(n_slots, np.uint8)
-        for j in range(n_slots):
-            if cur[j] is not None and cur[j][1] >= len(jobs[cur[j][0]][1]):
-                cur[j] = None
-            if cur[j] is None and nxt < len(jobs):
-                restart[j] = used[j]
-                cur[j], used[j] = [nxt, 0], True
-                nxt += 1
-        if all(c is None for c in cur):
-            break
+    for restart, slots in pkg("bag_replay").slot_queue([len(ev) for _, ev in jobs], n_slots):
         if restart.any():
             g.seq_restart(restart)
         scans, present, who, scan_imu = [], [], [], np.zeros((n_slots, 6))
-        for j in range(n_slots):
-            k = None
-            if cur[j] is not None:
-                i, e = cur[j]
-                k = jobs[i][1][e]
-                cur[j][1] += 1
+        for j, w in enumerate(slots):
+            k = jobs[w[0]][1][w[1]] if w is not None else None
             if k is None:
                 scans.append(dict(imu=np.zeros((0, 7)), **empty)); present.append(0); who.append(None)
             else:
-                s = synth.log_scan(logs[jobs[cur[j][0]][0]], k)
-                scans.append(s); present.append(1); who.append((cur[j][0], k)); scan_imu[j] = s["imu_last"]
+                s = synth.log_scan(logs[jobs[w[0]][0]], k)
+                scans.append(s); present.append(1); who.append((w[0], k)); scan_imu[j] = s["imu_last"]
         step = dict(present=np.array(present, np.uint8), imu=np.concatenate([np.asarray(s["imu"]).reshape(-1, 7) for s in scans]),
                     imu_off=np.concatenate([[0], np.cumsum([len(s["imu"]) for s in scans])]))
         for c in defs.Batch.FIELDS:

@@ -5,6 +5,7 @@ import numpy as np
 import pytest
 
 import featcases as fc
+from conftest import pkg
 
 pytestmark = pytest.mark.gpu
 
@@ -167,32 +168,20 @@ def drive_pcl(capi, defs, logs, flogs, n_slots, jobs, twin=True):
     if twin:
         g2 = capi.LinsGpu()
         g2.seq_open(defs.LinsSeqParams.shipped(), init_params(defs), n_slots)
-    cur, used, nxt = [None] * n_slots, [False] * n_slots, 0
     rows = [[] for _ in jobs]
     empty = {c: flogs[0][c][:0] for c in defs.Batch.FIELDS}
-    while True:
-        restart = np.zeros(n_slots, np.uint8)
-        for j in range(n_slots):
-            if cur[j] is not None and cur[j][1] >= len(jobs[cur[j][0]][1]):
-                cur[j] = None
-            if cur[j] is None and nxt < len(jobs):
-                restart[j] = used[j]
-                cur[j], used[j] = [nxt, 0], True
-                nxt += 1
-        if all(c is None for c in cur):
-            break
+    for restart, slots in pkg("bag_replay").slot_queue([len(ev) for _, ev in jobs], n_slots):
         if restart.any():
             g.seq_restart(restart)
             if g2:
                 g2.seq_restart(restart)
         scans, fscans, present, who, scan_imu = [], [], [], [], np.zeros((n_slots, 6))
-        for j in range(n_slots):
-            if cur[j] is None:
+        for j, w in enumerate(slots):
+            if w is None:
                 scans.append(_empty_scan64()); fscans.append(dict(imu=np.zeros((0, 7)), **empty)); present.append(0); who.append(None)
                 continue
-            i, e = cur[j]
+            i, e = w
             k = jobs[i][1][e]
-            cur[j][1] += 1
             li = jobs[i][0]
             scans.append(logs[li]["scans"][k]); fscans.append(synth.log_scan(flogs[li], k)); present.append(1); who.append((i, k))
             scan_imu[j] = logs[li]["imu_last"][k]

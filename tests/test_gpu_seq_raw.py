@@ -92,37 +92,22 @@ def drive(capi, defs, cases, n_slots, jobs, twins=(), point_format=0, hooks=Fals
         g.seq_open(defs.LinsSeqParams.shipped(), init_params(defs), n_slots)
         ctxs.append(g)
     g = ctxs[0]
-    cur, used, nxt = [None] * n_slots, [False] * n_slots, 0
     rows = [[] for _ in jobs]
     t = 0
-    while True:
-        restart = np.zeros(n_slots, np.uint8)
-        for j in range(n_slots):
-            if cur[j] is not None and cur[j][1] >= len(jobs[cur[j][0]][1]):
-                cur[j] = None
-            if cur[j] is None and nxt < len(jobs):
-                restart[j] = used[j]
-                cur[j], used[j] = [nxt, 0], True
-                nxt += 1
-        if all(c is None for c in cur):
-            break
+    for restart, slots in pkg("bag_replay").slot_queue([len(ev) for _, ev in jobs], n_slots):
         if restart.any():
             for c in ctxs:
                 c.seq_restart(restart)
         sweeps, scans, present, who, imus, scan_imu = [], [], [], [], [], np.zeros((n_slots, 6))
-        for j in range(n_slots):
-            k = None
-            if cur[j] is not None:
-                i, e = cur[j]
-                k = jobs[i][1][e]
-                cur[j][1] += 1
+        for j, w in enumerate(slots):
+            k = jobs[w[0]][1][w[1]] if w is not None else None
             if k is None:
                 sweeps.append(np.zeros((0, 4), np.float32)); scans.append(_empty_scan(L)); present.append(0); who.append(None)
                 imus.append(np.zeros((0, 7)))
                 continue
-            li = jobs[cur[j][0]][0]
+            li = jobs[w[0]][0]
             o = logs[li]["imu_off"]
-            sweeps.append(logs[li]["sweeps"][k]); scans.append(pcls[li]["scans"][k]); present.append(1); who.append((cur[j][0], k))
+            sweeps.append(logs[li]["sweeps"][k]); scans.append(pcls[li]["scans"][k]); present.append(1); who.append((w[0], k))
             imus.append(logs[li]["imu"][o[k]:o[k + 1]])
             scan_imu[j] = logs[li]["imu_last"][k]
         imu = np.concatenate(imus).reshape(-1, 7)

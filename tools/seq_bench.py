@@ -29,7 +29,7 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 import __graft_entry__ as ge  # noqa: E402
 
-capi, defs, synth = ge._pkg("capi"), ge._pkg("ctypes_defs"), ge._pkg("synth")
+capi, defs, synth, bag_replay = ge._pkg("capi"), ge._pkg("ctypes_defs"), ge._pkg("synth"), ge._pkg("bag_replay")
 
 
 def gpu_info():
@@ -88,25 +88,14 @@ def queue_open(logs, jobs, S):
     """(a): every recording from its first scan in S opened slots, freed slots restarted with the next recording."""
     g = capi.LinsGpu()
     g.seq_open(defs.LinsSeqParams.shipped(), defs.LinsSeqInitParams.shipped(init_ba=(0.0, 0.0, 0.0), init_bw=(0.0, 0.0, 0.0)), S)
-    cur, used, nxt = [None] * S, [False] * S, 0
     wall, phases, steps, scans, n_first, n_second = 0.0, np.zeros(4), 0, 0, 0, 0
-    while True:
-        restart = np.zeros(S, np.uint8)
-        for j in range(S):
-            if cur[j] is not None and cur[j][1] >= jobs[cur[j][0]][1]:
-                cur[j] = None
-            if cur[j] is None and nxt < len(jobs):
-                restart[j], cur[j], used[j] = used[j], [nxt, 0], True
-                nxt += 1
-        if all(c is None for c in cur):
-            break
+    for restart, who in bag_replay.slot_queue([n for _, n in jobs], S):
         sl, present, imu = [], [], np.zeros((S, 6))
-        for j in range(S):
-            if cur[j] is None:
+        for j, w in enumerate(who):
+            if w is None:
                 sl.append(empty_scan(logs[0])); present.append(0)
                 continue
-            s = synth.log_scan(logs[jobs[cur[j][0]][0]], cur[j][1])
-            cur[j][1] += 1
+            s = synth.log_scan(logs[jobs[w[0]][0]], w[1])
             sl.append(s); present.append(1); imu[j] = s["imu_last"]
         sd = cat_step(sl, present)
         t0 = time.perf_counter()

@@ -427,8 +427,8 @@ typedef struct lins_seq_raw_desc {
    device: nothing goes from device to host but the feature counts (one D2H + synchronisation).  Bit-identical to: drop
    every point whose x, y or z is not finite (keeping the firing order), lins_gpu_project_scans, compact each segmented
    cloud to dense CSR, lins_gpu_seq_step_pcl.  Unlike PCL, which skips the removal when the message claims is_dense, the
-   device always drops non-finite points (for an honest dense cloud the two agree).  All slots share one lidar model (a
-   run that mixes sensors uses a context per model, or lins_gpu_seq_step_pcl with padded rings).  May alternate with
+   device always drops non-finite points (for an honest dense cloud the two agree).  All slots share one lidar model; a
+   run that mixes sensors gives each slot its own with lins_gpu_seq_step_raw_mixed.  May alternate with
    lins_gpu_seq_step_ex and lins_gpu_seq_step_pcl in one run.  LINS_E_INVALID before anything changes for a bad
    descriptor, model (as lins_gpu_project_scans), offsets, point format, NULL array or fp, or a NULL scan_imu while a
    present slot is initialising; a segmented scan the extraction rejects (as lins_gpu_extract_features:
@@ -494,6 +494,37 @@ typedef struct lins_seq_cloud2_desc {
    lins_gpu_project_ms and lins_gpu_extract_ms report the step's three front-end kernels. */
 int lins_gpu_seq_step_cloud2(lins_ctx* ctx, const lins_seq_cloud2_desc* step, const lins_lidar_model* model,
                              const lins_feature_params* fp, const double* scan_imu /*S x 6 or NULL*/);
+
+/* ---- mixed sensors: one lidar model per scan, so sweeps of different sensors (a VLP-16 next to a 64-ring lidar) are
+   projected in one call and their sequences run in one context (DESIGN.md §4.7). */
+
+/* a table of lidar models and each scan's entry in it */
+typedef struct lins_lidar_models {
+  int32_t n_models;                /* >= 1 */
+  const lins_lidar_model* models;  /* n_models, each within the limits of lins_lidar_model */
+  const int32_t* model_of;         /* one entry per scan (absent slots included) in 0..n_models-1; NULL only if
+                                      n_models == 1 (every scan uses models[0]) */
+} lins_lidar_models;
+
+/* lins_gpu_project_scans with scan i projected by models->models[model_of[i]]: per scan bit-identical to
+   lins_gpu_project_scans with that model.  start_ring / end_ring are n x L_max, L_max the table's largest line_num: scan
+   i's first line_num entries are its ring indices, the rest 0 (the padded layout lins_gpu_extract_features takes with
+   line_num = L_max).  LINS_E_INVALID, before anything is uploaded or written, as lins_gpu_project_scans and for a NULL
+   table or models, n_models < 1, a listed model outside its limits, a NULL model_of with n_models > 1, or a model_of
+   entry outside 0..n_models-1. */
+int lins_gpu_project_scans_mixed(lins_ctx* ctx, const lins_lidar_models* models, const lins_raw_desc* raw, lins_point* seg,
+                                 uint8_t* ground_flag, uint32_t* col_ind, float* range, lins_point* outlier,
+                                 int32_t* start_ring /*n x L_max*/, int32_t* end_ring /*n x L_max*/, float* ori /*n x 3*/,
+                                 int32_t* counts /*n x 2*/);
+/* lins_gpu_seq_step_raw / lins_gpu_seq_step_cloud2 with slot s's sweep projected by models->models[model_of[s]]: each
+   slot bit-identical to the same slot stepped through the single-model entry with that model.  Each may alternate with
+   every other step entry in one run, and a slot may change sensor when lins_gpu_seq_restart hands it a new recording.
+   LINS_E_INVALID before anything changes for a table lins_gpu_project_scans_mixed rejects, and otherwise as the
+   single-model entry. */
+int lins_gpu_seq_step_raw_mixed(lins_ctx* ctx, const lins_seq_raw_desc* step, const lins_lidar_models* models,
+                                const lins_feature_params* fp, const double* scan_imu /*S x 6 or NULL*/);
+int lins_gpu_seq_step_cloud2_mixed(lins_ctx* ctx, const lins_seq_cloud2_desc* step, const lins_lidar_models* models,
+                                   const lins_feature_params* fp, const double* scan_imu /*S x 6 or NULL*/);
 
 /* Split "Jacobian kernel" (SURVEY.md §8(d) unit U1): residual + Jacobian row + 29-scalar reduction over the
    resident batch given the correspondence IDs of iteration `iter` of each scan's current linearisation

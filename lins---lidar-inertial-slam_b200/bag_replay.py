@@ -9,7 +9,8 @@ one StateEstimator, so that run_bag is each bag's contract (LinsFusion, Estimato
   - processPCL's IMU sample is the last propagated one, or (0, 0, G0) / 0 when there is none.
 The bags are queued through S slots (lins_gpu_seq_open, lins_gpu_seq_restart when a slot's bag has ended), and every
 step hands each present slot's PointCloud2 data field to lins_gpu_seq_step_cloud2 as it is: the decode runs on the
-device.  A step's data fields are gathered into one host buffer that is page-locked once (re-registered only when it
+device.  Bags of different sensors run together: each bag names its lidar model, and a step whose slots hold bags of more
+than one model goes through lins_gpu_seq_step_cloud2_mixed, each slot projected with its bag's model.  A step's data fields are gathered into one host buffer that is page-locked once (re-registered only when it
 grows), so each step's bytes go to the device in one DMA.
 """
 import ctypes as C
@@ -138,11 +139,30 @@ def slot_queue(lengths, n_slots):
                 c[1] += 1
 
 
+def model_table(recordings, model):
+    """(models, model_of): the distinct lidar models of the recordings (a list, in first-use order) and each recording's
+    index in it.  model: one LinsLidarModel for every recording, a list with one per recording, or None (VLP-16)."""
+    if model is None or isinstance(model, LinsLidarModel):
+        return [model or LinsLidarModel.vlp16()], [0] * len(recordings)
+    model = list(model)
+    if len(model) != len(recordings):
+        raise ValueError(f"{len(model)} lidar models for {len(recordings)} recordings")
+    models, keys, of = [], [], []
+    for m in model:
+        k = bytes(m)
+        if k not in keys:
+            keys.append(k)
+            models.append(m)
+        of.append(keys.index(k))
+    return models, of
+
+
 def replay(recordings, slots, model=None, device=0, gpu=None):
-    """Run the recordings through `slots` slots of one context.  Returns per recording a dict of per-scan arrays: stamps,
-    status (StateEstimator::status_ after the scan), scan_status (LINS_SEQ_*), global_est (n x 7: rn, qbn x y z w),
-    global_state (n x 19), iters and flags (-1 where the scan ran no IESKF)."""
-    model = model or LinsLidarModel.vlp16()
+    """Run the recordings through `slots` slots of one context.  model: one LinsLidarModel for every recording (None =
+    VLP-16) or a list with one per recording; a slot is projected with the model of the recording it holds.  Returns per
+    recording a dict of per-scan arrays: stamps, status (StateEstimator::status_ after the scan), scan_status (LINS_SEQ_*),
+    global_est (n x 7: rn, qbn x y z w), global_state (n x 19), iters and flags (-1 where the scan ran no IESKF)."""
+    models, rec_model = model_table(recordings, model)
     g = gpu or _capi.LinsGpu(device=device)
     g.seq_open(LinsSeqParams.shipped(), shim_init_params(), slots)
     out = [dict(stamps=r.stamps.copy(), status=np.zeros(len(r), np.int32), scan_status=np.zeros(len(r), np.int32),
@@ -165,7 +185,12 @@ def replay(recordings, slots, model=None, device=0, gpu=None):
             lays = (LinsCloud2Layout * slots)(*[recordings[w[0]].layouts[w[1]] if w else LinsCloud2Layout() for w in who])
             desc = LinsCloud2Desc()
             desc.n_scans, desc.data, desc.data_off, desc.layouts = slots, buf.ctypes.data, data_off.ctypes.data, C.cast(lays, C.c_void_p)
-            g.seq_step_cloud2(dict(imu=np.concatenate(imus), imu_off=imu_off, present=present), model=model, scan_imu=scan_imu, desc=desc)
+            step = dict(imu=np.concatenate(imus), imu_off=imu_off, present=present)
+            if len(models) == 1:
+                g.seq_step_cloud2(step, model=models[0], scan_imu=scan_imu, desc=desc)
+            else:  # (an absent slot is projected as an empty sweep: any entry in range will do)
+                model_of = np.array([rec_model[w[0]] if w else 0 for w in who], np.int32)
+                g.seq_step_cloud2_mixed(step, models, model_of, scan_imu=scan_imu, desc=desc)
             d, di = g.seq_download(), g.seq_download_init()
             for j, w in enumerate(who):
                 if w is None:

@@ -13,7 +13,7 @@ import subprocess
 
 import numpy as np
 
-from .ctypes_defs import (Batch, COV_SIZE, LinsBatchDesc, LinsCloud2Desc, LinsCloud2Layout, LinsFeatureParams, LinsLidarModel, LinsMapReport, LinsParams, LinsPclDesc,
+from .ctypes_defs import (Batch, COV_SIZE, LinsBatchDesc, LinsCloud2Desc, LinsCloud2Layout, LinsFeatureParams, LinsLidarModel, LinsLidarModels, LinsMapReport, LinsParams, LinsPclDesc,
                           LinsRawDesc, LinsReport, LinsScanResult, LinsSeqBeginDesc, LinsSeqInitParams, LinsSeqParams, LinsSeqPclDesc,
                           LinsSeqCloud2Desc, LinsSeqRawDesc, LinsSeqStepDesc, POINT_DTYPE, SCAN_RESULT_DTYPE, STATE_DIM, as_points, make_points, ptr)
 
@@ -35,6 +35,7 @@ EXPORTS = [
     "lins_gpu_seq_open", "lins_gpu_seq_restart", "lins_gpu_seq_step_ex", "lins_gpu_seq_download_init",
     "lins_gpu_extract_features", "lins_gpu_extract_ms", "lins_gpu_seq_step_pcl", "lins_gpu_project_scans", "lins_gpu_project_ms",
     "lins_gpu_seq_step_raw", "lins_gpu_decode_cloud2", "lins_gpu_decode_ms", "lins_gpu_seq_step_cloud2",
+    "lins_gpu_project_scans_mixed", "lins_gpu_seq_step_raw_mixed", "lins_gpu_seq_step_cloud2_mixed",
 ]
 
 NVCC_ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]  # H100 (Hopper)
@@ -126,6 +127,9 @@ def lib():
         L.lins_gpu_decode_cloud2.argtypes = [vp, C.POINTER(LinsCloud2Desc), vp, vp]
         L.lins_gpu_decode_ms.argtypes = [vp, vp]
         L.lins_gpu_seq_step_cloud2.argtypes = [vp, C.POINTER(LinsSeqCloud2Desc), C.POINTER(LinsLidarModel), C.POINTER(LinsFeatureParams), vp]
+        L.lins_gpu_project_scans_mixed.argtypes = [vp, C.POINTER(LinsLidarModels), C.POINTER(LinsRawDesc)] + [vp] * 9
+        L.lins_gpu_seq_step_raw_mixed.argtypes = [vp, C.POINTER(LinsSeqRawDesc), C.POINTER(LinsLidarModels), C.POINTER(LinsFeatureParams), vp]
+        L.lins_gpu_seq_step_cloud2_mixed.argtypes = [vp, C.POINTER(LinsSeqCloud2Desc), C.POINTER(LinsLidarModels), C.POINTER(LinsFeatureParams), vp]
         _LIB = L
     return _LIB
 
@@ -507,17 +511,42 @@ class LinsGpu:
         extract_features takes: seg (m x 4 float32 x, y, z, intensity), ground, col, range, start_ring, end_ring, ori (3),
         plus outlier (k x 4)."""
         model = model or LinsLidarModel.vlp16()
+        return self._project(sweeps, point_format, model.line_num,
+                             lambda d, *out: self.L.lins_gpu_project_scans(self.h, C.byref(model), C.byref(d), *out))
+
+    def project_scans_mixed(self, sweeps, models, model_of, point_format=0):
+        """project_scans with sweep i projected by models[model_of[i]] (lins_gpu_project_scans_mixed); model_of may be None
+        with one model.  start_ring / end_ring hold max(line_num) entries per sweep, those past its own model's line_num 0."""
+        keep = {}
+        t = self.models_table(models, model_of, keep)
+        return self._project(sweeps, point_format, max(m.line_num for m in models),
+                             lambda d, *out: self.L.lins_gpu_project_scans_mixed(self.h, C.byref(t), C.byref(d), *out))
+
+    @staticmethod
+    def models_table(models, model_of, keep):
+        """LinsLidarModels of a list of LinsLidarModel and one entry per scan (or None); the arrays it points at are added
+        to `keep`."""
+        keep["models"] = (LinsLidarModel * max(len(models), 1))(*models)
+        t = LinsLidarModels()
+        t.n_models, t.models = len(models), C.cast(keep["models"], C.c_void_p)
+        if model_of is not None:
+            keep["model_of"] = np.ascontiguousarray(model_of, dtype=np.int32)
+            t.model_of = keep["model_of"].ctypes.data
+        return t
+
+    def _project(self, sweeps, point_format, L, call):
+        """project_scans / project_scans_mixed: the outputs of `call(raw desc, *9 output pointers)` with L ring entries per
+        sweep."""
         keep = {}
         d = self._raw_desc(sweeps, point_format, keep)
-        n, total, L = d.n_scans, int(keep["cloud_off"][-1]), model.line_num
+        n, total = d.n_scans, int(keep["cloud_off"][-1])
         rec = np.float32 if point_format == 1 else POINT_DTYPE
         shape = (max(total, 1), 4) if point_format == 1 else max(total, 1)
         seg, outl = np.zeros(shape, rec), np.zeros(shape, rec)
         ground, col, rng = np.zeros(max(total, 1), np.uint8), np.zeros(max(total, 1), np.uint32), np.zeros(max(total, 1), np.float32)
         sr, er = np.zeros((max(n, 1), max(L, 1)), np.int32), np.zeros((max(n, 1), max(L, 1)), np.int32)
         ori, counts = np.zeros((max(n, 1), 3), np.float32), np.zeros((max(n, 1), 2), np.int32)
-        self._ck(self.L.lins_gpu_project_scans(self.h, C.byref(model), C.byref(d), ptr(seg), ptr(ground), ptr(col), ptr(rng), ptr(outl),
-                                               ptr(sr), ptr(er), ptr(ori), ptr(counts)))
+        self._ck(call(d, ptr(seg), ptr(ground), ptr(col), ptr(rng), ptr(outl), ptr(sr), ptr(er), ptr(ori), ptr(counts)))
         x4 = (lambda a: a.astype(np.float32)) if point_format == 1 else (  # noqa: E731
             lambda a: np.stack([a["x"], a["y"], a["z"], a["intensity"]], 1).astype(np.float32).reshape(-1, 4))
         off = keep["cloud_off"]
@@ -555,6 +584,16 @@ class LinsGpu:
         model = model or LinsLidarModel.vlp16()
         fp = fp or LinsFeatureParams.shipped()
         self._ck(self.L.lins_gpu_seq_step_raw(self.h, C.byref(d), C.byref(model), C.byref(fp), ptr(si)))
+
+    def seq_step_raw_mixed(self, step, models, model_of, fp=None, scan_imu=None, point_format=0):
+        """seq_step_raw with slot s's sweep projected by models[model_of[s]] (lins_gpu_seq_step_raw_mixed): models is a list
+        of LinsLidarModel, model_of one entry per slot, absent slots included (None with one model)."""
+        keep, d = {}, LinsSeqRawDesc()
+        si = self._seq_step_common(d, step, scan_imu, keep)
+        d.raw = self._raw_desc(step["sweeps"], point_format, keep)
+        t = self.models_table(models, model_of, keep)
+        fp = fp or LinsFeatureParams.shipped()
+        self._ck(self.L.lins_gpu_seq_step_raw_mixed(self.h, C.byref(d), C.byref(t), C.byref(fp), ptr(si)))
 
     @staticmethod
     def cloud2_desc(msgs, keep, gap=0, base=0):
@@ -603,6 +642,16 @@ class LinsGpu:
         model = model or LinsLidarModel.vlp16()
         fp = fp or LinsFeatureParams.shipped()
         self._ck(self.L.lins_gpu_seq_step_cloud2(self.h, C.byref(d), C.byref(model), C.byref(fp), ptr(si)))
+
+    def seq_step_cloud2_mixed(self, step, models, model_of, fp=None, scan_imu=None, desc=None, gap=0):
+        """seq_step_cloud2 with slot s's message projected by models[model_of[s]] (lins_gpu_seq_step_cloud2_mixed): models
+        and model_of as seq_step_raw_mixed takes them."""
+        keep, d = {}, LinsSeqCloud2Desc()
+        si = self._seq_step_common(d, step, scan_imu, keep)
+        d.cloud2 = desc if desc is not None else self.cloud2_desc(step["msgs"], keep, gap)
+        t = self.models_table(models, model_of, keep)
+        fp = fp or LinsFeatureParams.shipped()
+        self._ck(self.L.lins_gpu_seq_step_cloud2_mixed(self.h, C.byref(d), C.byref(t), C.byref(fp), ptr(si)))
 
     def seq_download(self, reports=False):
         """dict: global_state, filter_state (S x 19), filter_cov (S x 324), results (SCAN_RESULT_DTYPE), status (S) and,

@@ -163,9 +163,18 @@ struct FeatState {
   EventPair ev;                                         // around the last extraction kernel (lins_gpu_extract_ms)
 };
 
+// One lidar model as the projection kernel reads it: the range image's rows and columns, groundScanInd, the angular
+// resolutions and ang_bottom, and sinf / cosf of segmentAlphaX / Y (host libm)
+struct ProjModel {
+  int L, S, gsi;
+  float res_x, res_y, bottom;
+  float sin_x, cos_x, sin_y, cos_y;
+};
+
 // Image projection (lins_projection.cu): the uploaded raw sweeps (up.qs, CSR in up.qs_off), each resident CTA's range-image
-// scratch (line_num x scan_num entries: winning point, range, ground, label, out-edges, owner counts, owner row extents),
-// the projected clouds and per-point cloud_info at the raw offsets, ring indices (n x 2 x line_num: start, end),
+// scratch (the largest listed model's line_num x scan_num entries: winning point, range, ground, label, out-edges, owner
+// counts, owner row extents), the projected clouds and per-point cloud_info at the raw offsets, ring indices (n x 2 x the
+// largest line_num: start, end),
 // orientations (n x 3) and counts (n x 2: segmented, outlier); for lins_gpu_project_scans' read-back, the clouds packed
 // to dense offsets (d*) and their pinned staging (h_*)
 struct ProjState {
@@ -191,6 +200,10 @@ struct ProjState {
   Buf<int, kPinned> h_doff, h_ring;
   Buf<unsigned char> present;              // lins_gpu_seq_step_raw's present flags (n)
   Buf<unsigned char, kPinned> h_present;
+  Buf<ProjModel> models;                   // the model table
+  Buf<ProjModel, kPinned> h_models;
+  Buf<int> model_of;                       // each scan's entry in the table (n; not uploaded for a one-model call)
+  Buf<int, kPinned> h_model_of;
   EventPair ev;                            // around the last projection kernel (lins_gpu_project_ms)
 };
 
@@ -406,14 +419,20 @@ int features_run(lins_ctx* ctx, const lins_feature_params* fp, const lins_pcl_de
 // lins_features.cu: extract the scans of `in` into ctx->feat (clouds at the input offsets) and read the counts back (one
 // D2H + synchronisation; a scan's device-side status returns LINS_E_INVALID / LINS_E_TOOBIG)
 int features_launch(lins_ctx* ctx, const lins_feature_params* fp, const FeatInputs& in);
-// lins_projection.cu: validate the model and the sweeps of d, upload them and queue their projection into ctx->proj (no
-// synchronisation); drop_nonfinite: copyPointCloud's NaN removal first; present (host, n; null = all): a scan whose flag is
-// 0 is projected as an empty sweep
-int projection_run(lins_ctx* ctx, const lins_lidar_model* m, const lins_raw_desc* d, bool drop_nonfinite, const uint8_t* present);
-// lins_projection.cu: the model's limits (LINS_E_INVALID otherwise), and the part of projection_run after the upload: the
-// n sweeps (total points) are in ctx->proj.up (qs, CSR in qs_off), the model has been checked
+// lins_projection.cu: validate the model table and the sweeps of d, upload them and queue their projection into ctx->proj
+// (no synchronisation); drop_nonfinite: copyPointCloud's NaN removal first; present (host, n; null = all): a scan whose
+// flag is 0 is projected as an empty sweep.  A single-model entry passes the table {1, m, NULL}.
+int projection_run(lins_ctx* ctx, const lins_lidar_models* t, const lins_raw_desc* d, bool drop_nonfinite, const uint8_t* present);
+// lins_projection.cu: one model's limits; the table's (a table, n_models >= 1, every model within its limits, model_of
+// given when n_models > 1); model_of's n entries within 0..n_models-1 (each LINS_E_INVALID otherwise); the table's largest
+// line_num (the ring stride of the projection's output)
 int check_model(lins_ctx* ctx, const lins_lidar_model* m);
-int projection_launch(lins_ctx* ctx, const lins_lidar_model* m, int n, size_t total, bool drop_nonfinite, const uint8_t* present);
+int check_models(lins_ctx* ctx, const lins_lidar_models* t);
+int check_model_of(lins_ctx* ctx, const lins_lidar_models* t, int n);
+int max_line_num(const lins_lidar_models* t);
+// lins_projection.cu: the part of projection_run after the upload: the n sweeps (total points) are in ctx->proj.up (qs,
+// CSR in qs_off), the table and model_of have been checked
+int projection_launch(lins_ctx* ctx, const lins_lidar_models* t, int n, size_t total, bool drop_nonfinite, const uint8_t* present);
 // lins_upload.cu: n bytes from the caller's src to the device at dst, as upload_clouds moves clouds: a host thread pool copies
 // 1 MiB slices into the pinned staging and queues each slice's H2D as soon as it is staged; a src in caller-pinned memory
 // goes in one DMA with no host pass.  Synchronises the stream first (the staging may still be read by an earlier copy).

@@ -20,6 +20,9 @@
 // findStartEndAngle reads the first, last and second-to-last finite points; the removal keeps the order, so the highest
 // index of a pixel is still the point the filtered sweep's overwrite would leave.  A scan whose present flag is 0 is
 // projected as an empty sweep.
+// Each scan reads its lidar model from a device-resident table (lins_gpu_project_scans_mixed and the _mixed step
+// entries; the single-model entries pass a table of one), so sweeps of different sensors share a call.  Ring indices use
+// the table's largest line_num as their stride; a scan's rings past its own line_num are written as 0.
 #include <cuda_runtime.h>
 
 #include <cfloat>
@@ -42,17 +45,19 @@ constexpr int kMidRow = 1 << 30;   // (owner counts stay below 2^18 = 128 x 2048
 enum : unsigned char { E_RIGHT = 1, E_JUMP = 2, E_DOWN = 4, FEASIBLE = 0x80 };
 
 struct ProjArgs {
-  int n, L, S, gsi;
-  float res_x, res_y, bottom;
-  float sin_x, cos_x, sin_y, cos_y;  // sinf / cosf of segmentAlphaX / Y (host libm)
+  int n;
+  int L_max;                     // the ring stride: the largest line_num in the table
+  size_t P_max;                  // the per-CTA scratch stride: the largest line_num x scan_num in the table
+  const ProjModel* models;       // the model table (device)
+  const int* model_of;           // n: each scan's entry in models, or null = every scan uses models[0]
   const float4* pts; const int* off;
   const unsigned char* present;  // n, or null = all (lins_gpu_seq_step_raw)
   int drop_nonfinite;            // copyPointCloud's NaN removal (lins_gpu_seq_step_raw)
-  // per-CTA scratch, L * S entries each
+  // per-CTA scratch, P_max entries each
   int* idx; float* rng; signed char* gnd; int* lab; unsigned char* edg; int* cnt; int* rlo; int* rhi;
   // outputs at the raw offsets
   float4* seg; unsigned char* ground; unsigned* col; float* range; float4* outl;
-  int* ring;    // n x 2 x L: startRingIndex, endRingIndex
+  int* ring;    // n x 2 x L_max: startRingIndex, endRingIndex; a scan's rings past its own line_num are 0
   float* ori;   // n x 3
   int* counts;  // n x 2: segmented, outlier
 };
@@ -68,10 +73,10 @@ __global__ void __launch_bounds__(kThreads) lins_projection_kernel(const ProjArg
   using Scan = cub::BlockScan<unsigned long long, kThreads>;
   __shared__ typename Scan::TempStorage tmp;
   __shared__ int s_fin[3];  // drop_nonfinite: the first, last and second-to-last finite point (-1: none)
+  __shared__ ProjModel s_m; // the current scan's model
   const unsigned FULL = 0xffffffffu;
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-  const int L = a.L, S = a.S, P = L * S;
-  const size_t so = (size_t)blockIdx.x * P;
+  const size_t so = (size_t)blockIdx.x * a.P_max;
   int* idx = a.idx + so;
   float* rng = a.rng + so;
   signed char* gnd = a.gnd + so;
@@ -83,6 +88,9 @@ __global__ void __launch_bounds__(kThreads) lins_projection_kernel(const ProjArg
   auto blocked = [&](int p) { return gnd[p] == 1 || rng[p] == FLT_MAX; };
 
   for (int sc = blockIdx.x; sc < a.n; sc += gridDim.x) {
+    if (tid == 0) s_m = a.models[a.model_of ? a.model_of[sc] : 0];
+    __syncthreads();  // (the previous scan's last reads of s_m are behind its final barrier)
+    const int L = s_m.L, S = s_m.S, P = L * S;
     const int base = a.off[sc], np = a.present && !a.present[sc] ? 0 : a.off[sc + 1] - base;
     const float4* pt = a.pts + base;
     for (int p = tid; p < P; p += kThreads) {
@@ -124,7 +132,7 @@ __global__ void __launch_bounds__(kThreads) lins_projection_kernel(const ProjArg
     for (int i = tid; i < np; i += kThreads) {
       const float4 q = pt[i];
       int r, c;
-      if ((!a.drop_nonfinite || finite_xyz(q)) && lins_proj::project(q.x, q.y, q.z, L, S, a.res_x, a.res_y, a.bottom, r, c))
+      if ((!a.drop_nonfinite || finite_xyz(q)) && lins_proj::project(q.x, q.y, q.z, L, S, s_m.res_x, s_m.res_y, s_m.bottom, r, c))
         atomicMax(&idx[r * S + c], i);
     }
     __syncthreads();
@@ -134,7 +142,7 @@ __global__ void __launch_bounds__(kThreads) lins_projection_kernel(const ProjArg
     }
     // ---- groundRemoval: each column's rows in order ------------------------------------------------------------------
     for (int j = tid; j < S; j += kThreads)
-      for (int i = 0; i < a.gsi; ++i) {
+      for (int i = 0; i < s_m.gsi; ++i) {
         const int lo = idx[i * S + j], up = idx[(i + 1) * S + j];
         if (lo < 0 || up < 0) { gnd[i * S + j] = -1; continue; }
         const float4 l = pt[lo], u = pt[up];
@@ -151,9 +159,9 @@ __global__ void __launch_bounds__(kThreads) lins_projection_kernel(const ProjArg
       if (!blk) {
         const float rp = rng[p];
         const int t1 = r * S + (c + 1 < S ? c + 1 : 0), t2 = r * S + (c + 255 < S ? c + 255 : 0);
-        if (!blocked(t1) && lins_proj::edge(rp, rng[t1], a.sin_x, a.cos_x)) e |= E_RIGHT;
-        if (!blocked(t2) && lins_proj::edge(rp, rng[t2], a.sin_x, a.cos_x)) e |= E_JUMP;
-        if (r + 1 < L && !blocked(p + S) && lins_proj::edge(rp, rng[p + S], a.sin_y, a.cos_y)) e |= E_DOWN;
+        if (!blocked(t1) && lins_proj::edge(rp, rng[t1], s_m.sin_x, s_m.cos_x)) e |= E_RIGHT;
+        if (!blocked(t2) && lins_proj::edge(rp, rng[t2], s_m.sin_x, s_m.cos_x)) e |= E_JUMP;
+        if (r + 1 < L && !blocked(p + S) && lins_proj::edge(rp, rng[p + S], s_m.sin_y, s_m.cos_y)) e |= E_DOWN;
       }
       edg[p] = e;
     }
@@ -216,7 +224,9 @@ __global__ void __launch_bounds__(kThreads) lins_projection_kernel(const ProjArg
     __syncthreads();
 
     // ---- cloudSegmentation's compaction in raster order ----------------------------------------------------------------
-    int* ring = a.ring + (size_t)sc * 2 * L;
+    const int LM = a.L_max;
+    int* ring = a.ring + (size_t)sc * 2 * LM;  // start: ring[0 .. L), end: ring[LM .. LM + L)
+    for (int r = L + tid; r < LM; r += kThreads) { ring[r] = 0; ring[LM + r] = 0; }  // (the buffer is reused)
     int n_seg = 0, n_out = 0;
     for (int q0 = 0; q0 < P; q0 += kThreads) {
       const int p = q0 + tid;
@@ -230,7 +240,7 @@ __global__ void __launch_bounds__(kThreads) lins_projection_kernel(const ProjArg
         } else if (ow != kBlocked) {
           const bool feasible = edg[ow] & FEASIBLE;
           s = feasible;
-          o = !feasible && r > a.gsi && c % 5 == 0;  // label 999999
+          o = !feasible && r > s_m.gsi && c % 5 == 0;  // label 999999
         }
       }
       unsigned long long pre, tot;
@@ -250,14 +260,14 @@ __global__ void __launch_bounds__(kThreads) lins_projection_kernel(const ProjArg
       }
       if (p < P && c == 0) {
         ring[r] = ps - 1 + 5;
-        if (r > 0) ring[L + r - 1] = ps - 1 - 5;
+        if (r > 0) ring[LM + r - 1] = ps - 1 - 5;
       }
       n_seg += (int)(tot & 0xffffffffu);
       n_out += (int)(tot >> 32);
       __syncthreads();  // (tmp is reused)
     }
     if (tid == 0) {
-      ring[2 * L - 1] = n_seg - 1 - 5;
+      ring[LM + L - 1] = n_seg - 1 - 5;
       a.counts[2 * sc] = n_seg;
       a.counts[2 * sc + 1] = n_out;
     }
@@ -298,15 +308,42 @@ int check_model(lins_ctx* ctx, const lins_lidar_model* m) {
   return LINS_OK;
 }
 
-// Validate the model and the descriptor on the host, upload the sweeps and queue the projection kernel (no
-// synchronisation).  Afterwards ctx->proj holds the projected clouds at the raw offsets, n x 2 x L ring indices, n x 3
-// orientations and n x 2 counts, all on the device.  drop_nonfinite / present: see ProjArgs.
-int projection_run(lins_ctx* ctx, const lins_lidar_model* m, const lins_raw_desc* d, bool drop_nonfinite, const uint8_t* present) {
-  int rc = check_model(ctx, m);
+int check_models(lins_ctx* ctx, const lins_lidar_models* t) {
+  if (!t) return fail(ctx, LINS_E_INVALID, "null lidar model table");
+  if (t->n_models < 1) return fail(ctx, LINS_E_INVALID, "n_models < 1");
+  if (!t->models) return fail(ctx, LINS_E_INVALID, "null lidar model");
+  for (int i = 0; i < t->n_models; ++i) {
+    const int rc = check_model(ctx, &t->models[i]);
+    if (rc != LINS_OK) return rc;
+  }
+  if (!t->model_of && t->n_models > 1) return fail(ctx, LINS_E_INVALID, "null model_of with more than one lidar model");
+  return LINS_OK;
+}
+
+int check_model_of(lins_ctx* ctx, const lins_lidar_models* t, int n) {
+  if (t->model_of)
+    for (int i = 0; i < n; ++i)
+      if (t->model_of[i] < 0 || t->model_of[i] >= t->n_models) return fail(ctx, LINS_E_INVALID, "model_of entry outside 0..n_models-1");
+  return LINS_OK;
+}
+
+int max_line_num(const lins_lidar_models* t) {
+  int L = 0;
+  for (int i = 0; i < t->n_models; ++i) L = std::max(L, (int)t->models[i].line_num);
+  return L;
+}
+
+// Validate the model table and the descriptor on the host, upload the sweeps and queue the projection kernel (no
+// synchronisation).  Afterwards ctx->proj holds the projected clouds at the raw offsets, n x 2 x L_max ring indices (L_max
+// = max_line_num(t)), n x 3 orientations and n x 2 counts, all on the device.  drop_nonfinite / present: see ProjArgs.
+int projection_run(lins_ctx* ctx, const lins_lidar_models* t, const lins_raw_desc* d, bool drop_nonfinite, const uint8_t* present) {
+  int rc = check_models(ctx, t);
   if (rc != LINS_OK) return rc;
   if (!d || d->n_scans < 0) return fail(ctx, LINS_E_INVALID, "bad raw sweep descriptor");
   const int n = d->n_scans;
   if (!d->cloud_off) return fail(ctx, LINS_E_INVALID, "null cloud offsets");
+  rc = check_model_of(ctx, t, n);
+  if (rc != LINS_OK) return rc;
   CK(cudaSetDevice(ctx->device));
   ProjState& pr = ctx->proj;
   std::vector<int32_t> zeros(n + 1, 0);
@@ -315,33 +352,49 @@ int projection_run(lins_ctx* ctx, const lins_lidar_model* m, const lins_raw_desc
   rc = upload_clouds(ctx, pr.up, n, pts, offs, d->point_format);  // (validates the offsets and the format; synchronises first)
   if (rc != LINS_OK) return rc;
   if (n == 0) return LINS_OK;
-  return projection_launch(ctx, m, n, (size_t)d->cloud_off[n], drop_nonfinite, present);
+  return projection_launch(ctx, t, n, (size_t)d->cloud_off[n], drop_nonfinite, present);
 }
 
-int projection_launch(lins_ctx* ctx, const lins_lidar_model* m, int n, size_t total, bool drop_nonfinite, const uint8_t* present) {
+int projection_launch(lins_ctx* ctx, const lins_lidar_models* t, int n, size_t total, bool drop_nonfinite, const uint8_t* present) {
   ProjState& pr = ctx->proj;
-  const int L = m->line_num, S = m->scan_num;
-  const size_t P = (size_t)L * S, N = total + 1;
+  const int nm = t->n_models, L_max = max_line_num(t);
+  size_t P_max = 0;
+  for (int i = 0; i < nm; ++i) P_max = std::max(P_max, (size_t)t->models[i].line_num * t->models[i].scan_num);
+  const size_t N = total + 1;
   int per_sm = 0;
   CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, lins_projection_kernel, kThreads, 0));
   const int grid = std::max(1, std::min(n, per_sm * ctx->sm_count));
-  const size_t G = (size_t)grid * P;
+  const size_t G = (size_t)grid * P_max;
   CK(pr.idx.reserve(G)); CK(pr.rng.reserve(G)); CK(pr.gnd.reserve(G)); CK(pr.lab.reserve(G)); CK(pr.edg.reserve(G));
   CK(pr.cnt.reserve(G)); CK(pr.rlo.reserve(G)); CK(pr.rhi.reserve(G));
   CK(pr.seg.reserve(N)); CK(pr.outl.reserve(N)); CK(pr.ground.reserve(N)); CK(pr.col.reserve(N)); CK(pr.range.reserve(N));
-  CK(pr.ring.reserve(2 * (size_t)n * L)); CK(pr.ori.reserve(3 * (size_t)n)); CK(pr.counts.reserve(2 * (size_t)n));
-  if (present) {  // (the upload synchronised the stream: the staging is free)
+  CK(pr.ring.reserve(2 * (size_t)n * L_max)); CK(pr.ori.reserve(3 * (size_t)n)); CK(pr.counts.reserve(2 * (size_t)n));
+  // (the upload synchronised the stream: the staging is free)
+  CK(pr.models.reserve(nm)); CK(pr.h_models.reserve(nm));
+  for (int i = 0; i < nm; ++i) {
+    const lins_lidar_model& m = t->models[i];
+    ProjModel& q = pr.h_models.p[i];
+    q.L = m.line_num; q.S = m.scan_num; q.gsi = m.ground_scan_ind;
+    q.res_x = m.ang_res_x; q.res_y = m.ang_res_y; q.bottom = m.ang_bottom;
+    const float ax = lins_proj::segment_alpha(m.ang_res_x), ay = lins_proj::segment_alpha(m.ang_res_y);
+    q.sin_x = std::sin(ax); q.cos_x = std::cos(ax); q.sin_y = std::sin(ay); q.cos_y = std::cos(ay);  // (float overloads: sinf / cosf)
+  }
+  CK(cudaMemcpyAsync(pr.models.p, pr.h_models.p, sizeof(ProjModel) * nm, cudaMemcpyHostToDevice, ctx->stream));
+  if (t->model_of) {
+    CK(pr.model_of.reserve(n)); CK(pr.h_model_of.reserve(n));
+    std::memcpy(pr.h_model_of.p, t->model_of, sizeof(int32_t) * n);
+    CK(cudaMemcpyAsync(pr.model_of.p, pr.h_model_of.p, sizeof(int32_t) * n, cudaMemcpyHostToDevice, ctx->stream));
+  }
+  if (present) {
     CK(pr.present.reserve(n)); CK(pr.h_present.reserve(n));
     std::memcpy(pr.h_present.p, present, n);
     CK(cudaMemcpyAsync(pr.present.p, pr.h_present.p, n, cudaMemcpyHostToDevice, ctx->stream));
   }
   ProjArgs a;
-  a.n = n; a.L = L; a.S = S; a.gsi = m->ground_scan_ind;
+  a.n = n; a.L_max = L_max; a.P_max = P_max;
+  a.models = pr.models.p; a.model_of = t->model_of ? pr.model_of.p : nullptr;
   a.present = present ? pr.present.p : nullptr;
   a.drop_nonfinite = drop_nonfinite;
-  a.res_x = m->ang_res_x; a.res_y = m->ang_res_y; a.bottom = m->ang_bottom;
-  const float ax = lins_proj::segment_alpha(m->ang_res_x), ay = lins_proj::segment_alpha(m->ang_res_y);
-  a.sin_x = std::sin(ax); a.cos_x = std::cos(ax); a.sin_y = std::sin(ay); a.cos_y = std::cos(ay);  // (float overloads: sinf / cosf)
   a.pts = pr.up.qs.p; a.off = pr.up.qs_off.p;
   a.idx = pr.idx.p; a.rng = pr.rng.p; a.gnd = reinterpret_cast<signed char*>(pr.gnd.p); a.lab = pr.lab.p; a.edg = pr.edg.p;
   a.cnt = pr.cnt.p; a.rlo = pr.rlo.p; a.rhi = pr.rhi.p;
@@ -359,21 +412,21 @@ int projection_launch(lins_ctx* ctx, const lins_lidar_model* m, int n, size_t to
 
 extern "C" {
 
-int lins_gpu_project_scans(lins_ctx* ctx, const lins_lidar_model* m, const lins_raw_desc* d, lins_point* seg, uint8_t* ground_flag,
-                           uint32_t* col_ind, float* range, lins_point* outlier, int32_t* start_ring, int32_t* end_ring, float* ori,
-                           int32_t* counts) {
+int lins_gpu_project_scans_mixed(lins_ctx* ctx, const lins_lidar_models* t, const lins_raw_desc* d, lins_point* seg, uint8_t* ground_flag,
+                                 uint32_t* col_ind, float* range, lins_point* outlier, int32_t* start_ring, int32_t* end_ring, float* ori,
+                                 int32_t* counts) {
   if (!ctx) return LINS_E_INVALID;
   if (d && d->n_scans > 0) {
     if (!start_ring || !end_ring || !ori || !counts) return fail(ctx, LINS_E_INVALID, "null cloud_info output");
     if (d->cloud_off && d->cloud_off[d->n_scans] > 0 && (!seg || !ground_flag || !col_ind || !range || !outlier))
       return fail(ctx, LINS_E_INVALID, "null output cloud");
   }
-  const int rc = projection_run(ctx, m, d, false, nullptr);
+  const int rc = projection_run(ctx, t, d, false, nullptr);
   if (rc != LINS_OK) return rc;
   const int n = d->n_scans;
   if (n == 0) return LINS_OK;
   ProjState& pr = ctx->proj;
-  const int L = m->line_num;
+  const int L = max_line_num(t);
   // the counts first (one synchronisation), then only the clouds' used prefixes: packed to dense offsets on the device
   // and read back through pinned staging (a second synchronisation)
   CK(pr.h_counts.reserve(2 * (size_t)n)); CK(pr.h_ring.reserve(2 * (size_t)n * L)); CK(pr.h_ori.reserve(3 * (size_t)n));
@@ -430,6 +483,13 @@ int lins_gpu_project_scans(lins_ctx* ctx, const lins_lidar_model* m, const lins_
     counts[2 * i + 1] = no;
   }
   return LINS_OK;
+}
+
+int lins_gpu_project_scans(lins_ctx* ctx, const lins_lidar_model* m, const lins_raw_desc* d, lins_point* seg, uint8_t* ground_flag,
+                           uint32_t* col_ind, float* range, lins_point* outlier, int32_t* start_ring, int32_t* end_ring, float* ori,
+                           int32_t* counts) {
+  const lins_lidar_models t = {1, m, nullptr};
+  return lins_gpu_project_scans_mixed(ctx, &t, d, seg, ground_flag, col_ind, range, outlier, start_ring, end_ring, ori, counts);
 }
 
 int lins_gpu_project_ms(lins_ctx* ctx, float* ms) {

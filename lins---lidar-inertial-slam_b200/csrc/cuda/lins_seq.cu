@@ -593,14 +593,15 @@ int step_from_features(lins_ctx* ctx, const uint8_t* pres, const double* imu, co
 }
 
 // The rest of a step whose sweeps' projection (with the NaN removal) is queued in ctx->proj at the raw offsets src_off:
-// the extraction on the projection's output where it lies (each scan's segmented count as its extent), one D2H +
-// synchronisation for the counts before the sequences change, then step_from_features.
-int step_from_projection(lins_ctx* ctx, const uint8_t* pres, const double* imu, const int32_t* imu_off, const lins_lidar_model* m,
+// the extraction on the projection's output where it lies (each scan's segmented count as its extent; line_num: the
+// ring stride, the table's largest line_num, whose extra rings are empty), one D2H + synchronisation for the counts before
+// the sequences change, then step_from_features.
+int step_from_projection(lins_ctx* ctx, const uint8_t* pres, const double* imu, const int32_t* imu_off, int line_num,
                          const lins_feature_params* fp, const int32_t* src_off, const double* scan_imu) {
   const int n = ctx->seq.n;
   ProjState& pr = ctx->proj;
   FeatInputs in;
-  in.n = n; in.line_num = m->line_num; in.total = src_off[n];
+  in.n = n; in.line_num = line_num; in.total = src_off[n];
   in.pts = pr.seg.p; in.off = pr.up.qs_off.p; in.count = pr.counts.p; in.count_stride = 2;
   in.ground = pr.ground.p; in.col = pr.col.p; in.range = pr.range.p; in.ring = pr.ring.p; in.ori = pr.ori.p;
   const int rc = features_launch(ctx, fp, in);
@@ -746,32 +747,45 @@ int lins_gpu_seq_step_pcl(lins_ctx* ctx, const lins_seq_pcl_desc* d, const lins_
   return step_from_features(ctx, d->present, d->imu, d->imu_off, d->pcl.cloud_off, scan_imu);
 }
 
-int lins_gpu_seq_step_raw(lins_ctx* ctx, const lins_seq_raw_desc* d, const lins_lidar_model* m, const lins_feature_params* fp,
-                          const double* scan_imu) {
+int lins_gpu_seq_step_raw_mixed(lins_ctx* ctx, const lins_seq_raw_desc* d, const lins_lidar_models* t, const lins_feature_params* fp,
+                                const double* scan_imu) {
   int rc = check_step(ctx, d, d ? d->raw.n_scans : 0, scan_imu);
   if (rc != LINS_OK) return rc;
   if (!fp) return fail(ctx, LINS_E_INVALID, "null feature params");
   // projection with copyPointCloud's NaN removal, then the rest of the step
-  rc = projection_run(ctx, m, &d->raw, true, d->present);
+  rc = projection_run(ctx, t, &d->raw, true, d->present);
   if (rc != LINS_OK) return rc;
-  return step_from_projection(ctx, d->present, d->imu, d->imu_off, m, fp, d->raw.cloud_off, scan_imu);
+  return step_from_projection(ctx, d->present, d->imu, d->imu_off, max_line_num(t), fp, d->raw.cloud_off, scan_imu);
+}
+
+int lins_gpu_seq_step_raw(lins_ctx* ctx, const lins_seq_raw_desc* d, const lins_lidar_model* m, const lins_feature_params* fp,
+                          const double* scan_imu) {
+  const lins_lidar_models t = {1, m, nullptr};
+  return lins_gpu_seq_step_raw_mixed(ctx, d, &t, fp, scan_imu);
+}
+
+int lins_gpu_seq_step_cloud2_mixed(lins_ctx* ctx, const lins_seq_cloud2_desc* d, const lins_lidar_models* t, const lins_feature_params* fp,
+                                   const double* scan_imu) {
+  int rc = check_step(ctx, d, d ? d->cloud2.n_scans : 0, scan_imu);
+  if (rc != LINS_OK) return rc;
+  if (!fp) return fail(ctx, LINS_E_INVALID, "null feature params");
+  const int n = ctx->seq.n;
+  rc = check_models(ctx, t);
+  if (rc == LINS_OK) rc = check_model_of(ctx, t, n);
+  if (rc != LINS_OK) return rc;
+  // the messages decoded into the projection's input (the present slots' only), then step_raw's projection and the rest
+  std::vector<int32_t> off;
+  rc = cloud2_run(ctx, &d->cloud2, d->present, off);
+  if (rc != LINS_OK) return rc;
+  rc = projection_launch(ctx, t, n, (size_t)off[n], true, d->present);
+  if (rc != LINS_OK) return rc;
+  return step_from_projection(ctx, d->present, d->imu, d->imu_off, max_line_num(t), fp, off.data(), scan_imu);
 }
 
 int lins_gpu_seq_step_cloud2(lins_ctx* ctx, const lins_seq_cloud2_desc* d, const lins_lidar_model* m, const lins_feature_params* fp,
                              const double* scan_imu) {
-  int rc = check_step(ctx, d, d ? d->cloud2.n_scans : 0, scan_imu);
-  if (rc != LINS_OK) return rc;
-  if (!fp) return fail(ctx, LINS_E_INVALID, "null feature params");
-  rc = check_model(ctx, m);
-  if (rc != LINS_OK) return rc;
-  // the messages decoded into the projection's input (the present slots' only), then step_raw's projection and the rest
-  const int n = ctx->seq.n;
-  std::vector<int32_t> off;
-  rc = cloud2_run(ctx, &d->cloud2, d->present, off);
-  if (rc != LINS_OK) return rc;
-  rc = projection_launch(ctx, m, n, (size_t)off[n], true, d->present);
-  if (rc != LINS_OK) return rc;
-  return step_from_projection(ctx, d->present, d->imu, d->imu_off, m, fp, off.data(), scan_imu);
+  const lins_lidar_models t = {1, m, nullptr};
+  return lins_gpu_seq_step_cloud2_mixed(ctx, d, &t, fp, scan_imu);
 }
 
 int lins_gpu_seq_phase_ms(lins_ctx* ctx, float* ms) {

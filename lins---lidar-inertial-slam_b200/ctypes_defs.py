@@ -188,6 +188,11 @@ class LinsLidarModel(C.Structure):
         return cls(64, 1024, f(360.0) / f(1024.0), f(45.0) / f(63.0), f(22.5) + f(0.1), 24)
 
 
+class LinsLidarModels(C.Structure):
+    """lins_lidar_models: a table of lidar models and each scan's entry in it (model_of NULL only with one model)."""
+    _fields_ = [("n_models", C.c_int32), ("models", C.c_void_p), ("model_of", C.c_void_p)]
+
+
 class LinsRawDesc(C.Structure):
     """lins_raw_desc: n raw sweeps, CSR."""
     _fields_ = [("n_scans", C.c_int32), ("cloud", C.c_void_p), ("cloud_off", C.c_void_p), ("point_format", C.c_int32)]

@@ -540,7 +540,8 @@ int lins_gpu_batch_jacobian_pass(lins_ctx* ctx, double* accum_out /*n x 29 or NU
 typedef struct lins_map_report {
   int32_t iters;       /* LM iterations executed (<= 10) */
   int32_t converged;   /* deltaR < 0.05 deg && deltaT < 0.05 cm reached (:1628) */
-  int32_t degenerate;  /* isDegenerate of iteration 0 (:1606-1617) */
+  int32_t degenerate;  /* isDegenerate of iteration 0 (:1606-1617); 0 when that pass selects < 50 points and no LM step
+                          runs.  matP / isDegenerate themselves persist across calls, like the reference's members */
   int32_t skipped;     /* map too small: cornerFromMapDSNum <= 10 || surfFromMapDSNum <= 100 (:1636) */
   int32_t n_sel[LINS_MAP_MAX_ITER];   /* laserCloudSelNum per iteration (< 50 => that LM step is skipped, :1535) */
   float delta_r[LINS_MAP_MAX_ITER];   /* deg */

@@ -177,7 +177,9 @@ int lins_gpu_scan2map(lins_ctx* ctx, const lins_point* corner, int nc, const lin
   CK(cudaStreamSynchronize(ctx->stream));
   const MapLoopState& st = *m.h_loop.p;
   for (int i = 0; i < 6; ++i) T[i] = st.T[i];
-  r.iters = st.iters; r.converged = st.converged; r.degenerate = st.isDegenerate;
+  // a call whose first pass selects < 50 points takes no LM step (its later passes see the same transform), so nothing
+  // was projected: it reports 0, like the reference's LMOptimization, while matP / isDegenerate persist for later calls
+  r.iters = st.iters; r.converged = st.converged; r.degenerate = st.n_sel[0] >= 50 ? st.isDegenerate : 0;
   for (int i = 0; i < LINS_MAP_MAX_ITER; ++i) { r.n_sel[i] = st.n_sel[i]; r.delta_r[i] = st.delta_r[i]; r.delta_t[i] = st.delta_t[i]; }
   if (rep) *rep = r;
   return LINS_OK;

@@ -267,7 +267,8 @@ __global__ void __launch_bounds__(kFitThreads) lins_map_fit_kernel(const float4*
 //
 // Grid.  The reference accepts a feature point only if its FIFTH neighbour lies within 1 m (pointSearchSqDis[4] < 1.0,
 // lidar_mapping_node.cpp:1374, :1481), so the only neighbours that matter are those within 1 m, and every map point
-// within 1 m of a query lies in the 3 x 3 x 3 block of 1 m cells around the query's cell.  lins_gpu_map_set bucket-sorts
+// whose f32 distance is < 1 lies in the 3 x 3 x 3 block of 1 m cells around the query's cell (cells of the exact
+// difference: grid_cell, DESIGN.md §4.4).  lins_gpu_map_set bucket-sorts
 // the map by hash(cell) (the role of kdtree*FromMap->setInputCloud, :1637-1638); a query warp gives one cell of the
 // block to each of 27 lanes (cells that hash to the same bucket are visited once), every lane keeps the five smallest
 // (distance, index) keys of its bucket — points of other cells that share the bucket are just extra candidates — and a
@@ -288,18 +289,27 @@ struct GridIndex {
   unsigned mask;          // n_buckets - 1 (power of two)
   float ox, oy, oz;       // grid origin
 };
-__device__ __forceinline__ unsigned grid_hash(int ix, int iy, int iz) {
-  return ((unsigned)ix * 73856093u) ^ ((unsigned)iy * 19349663u) ^ ((unsigned)iz * 83492791u);
+// Cell indices are taken as unsigned so that the block's neighbour arithmetic (cx - 1, cx + 1) wraps instead of
+// overflowing at a saturated cell; the hash sees the same bits either way.
+__device__ __forceinline__ unsigned grid_hash(unsigned ix, unsigned iy, unsigned iz) {
+  return (ix * 73856093u) ^ (iy * 19349663u) ^ (iz * 83492791u);
 }
-__device__ __forceinline__ void grid_cell(const GridIndex& g, float x, float y, float z, int& ix, int& iy, int& iz) {
-  ix = (int)floorf((x - g.ox) * (1.0f / kGridCell)); iy = (int)floorf((y - g.oy) * (1.0f / kGridCell)); iz = (int)floorf((z - g.oz) * (1.0f / kGridCell));
+// floor(x - ox) of the EXACT difference: f32 operands subtract exactly in f64 unless their exponents are ~29 apart, and
+// then the f64 rounding is far below the 2^-25 margin the block rule needs (DESIGN.md §4.4).  An f32 x - ox would round
+// near a power of two from the origin and could put a neighbour whose f32 distance is < 1 two cells away.  The
+// conversion floors and saturates (NaN -> 0), so far and non-finite coordinates land in the edge cells.
+__device__ __forceinline__ void grid_cell(const GridIndex& g, float x, float y, float z, unsigned& ix, unsigned& iy, unsigned& iz) {
+  static_assert(kGridCell == 1.0f, "grid_cell assumes 1 m cells");
+  ix = (unsigned)__double2int_rd((double)x - (double)g.ox);
+  iy = (unsigned)__double2int_rd((double)y - (double)g.oy);
+  iz = (unsigned)__double2int_rd((double)z - (double)g.oz);
 }
 // counting sort of the map by bucket: count, (host-launched) scan, scatter
 __global__ void lins_grid_count_kernel(const float4* __restrict__ map, int n, GridIndex g, int* __restrict__ count) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n) return;
   const float4 p = __ldg(&map[i]);
-  int ix, iy, iz;
+  unsigned ix, iy, iz;
   grid_cell(g, p.x, p.y, p.z, ix, iy, iz);
   atomicAdd(&count[grid_hash(ix, iy, iz) & g.mask], 1);
 }
@@ -320,7 +330,7 @@ __global__ void lins_grid_scatter_kernel(const float4* __restrict__ map, int n, 
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n) return;
   const float4 p = __ldg(&map[i]);
-  int ix, iy, iz;
+  unsigned ix, iy, iz;
   grid_cell(g, p.x, p.y, p.z, ix, iy, iz);
   const int pos = atomicAdd(&cursor[grid_hash(ix, iy, iz) & g.mask], 1);
   sorted[pos] = make_float4(p.x, p.y, p.z, __int_as_float(i));
@@ -351,10 +361,10 @@ __global__ void __launch_bounds__(kGridKnnWarps * 32) lins_map_knn_grid_kernel(c
   if (qi >= n_q) return;
   const PassConsts pc = *pcp;
   const float3 s = associate_to_map(__ldg(&q[qi]), pc);
-  int cx, cy, cz;
+  unsigned cx, cy, cz;
   grid_cell(g, s.x, s.y, s.z, cx, cy, cz);
   unsigned b = 0xFFFFFF00u + (unsigned)lane;  // lanes 27..31: a bucket id nobody shares, never scanned
-  if (lane < 27) b = grid_hash(cx + lane % 3 - 1, cy + (lane / 3) % 3 - 1, cz + lane / 9 - 1) & g.mask;
+  if (lane < 27) b = grid_hash(cx + lane % 3 - 1u, cy + (lane / 3) % 3 - 1u, cz + lane / 9 - 1u) & g.mask;
   const unsigned same = __match_any_sync(0xffffffffu, b);
   const bool mine = lane < 27 && (__ffs(same) - 1) == lane;  // cells of the block that share a bucket are visited once
   Top5K t;
@@ -365,7 +375,8 @@ __global__ void __launch_bounds__(kGridKnnWarps * 32) lins_map_knn_grid_kernel(c
       const float4 m = __ldg(&g.pts[p]);
       const float dx = __fsub_rn(s.x, m.x), dy = __fsub_rn(s.y, m.y), dz = __fsub_rn(s.z, m.z);
       const float dist = __fadd_rn(__fadd_rn(__fmul_rn(dx, dx), __fmul_rn(dy, dy)), __fmul_rn(dz, dz));
-      if (dist == dist) t.insert(((unsigned long long)__float_as_uint(dist) << 32) | (unsigned)__float_as_int(m.w));
+      // never a NaN or +inf distance, like the brute-force scan
+      if (dist < __int_as_float(0x7f800000)) t.insert(((unsigned long long)__float_as_uint(dist) << 32) | (unsigned)__float_as_int(m.w));
     }
   }
   // five rounds: the smallest head among the lanes' ascending lists

@@ -566,6 +566,69 @@ int lins_gpu_map_associate(lins_ctx* ctx, const lins_point* corner_last, int n_c
                            int32_t* surf_knn /*5*n_surf*/, float* corner_coeff /*4*n_corner*/, float* surf_coeff /*4*n_surf*/,
                            uint8_t* corner_mask, uint8_t* surf_mask);
 
+/* ---- the mapping node's cycle: lidar_mapping_node.cpp run() :1806-1855 behind one call per mapping cycle ------------
+   One mapper per context.  Per processed cycle: transformAssociateToMap (:411-536), extractSurroundingKeyFrames in the
+   branch the reference compiles (loopClosureEnableFlag = true, parameters.h:80: the window of the 50 most recent key
+   frames, :1204-1246), the local map's pcl::VoxelGrid (corner 0.2 m, surf + outlier 0.4 m, :1317-1323),
+   downsampleCurrentScan (:1326-1349), scan2MapOptimization with its 10 / 100 gate and transformUpdate (:1635-1652,
+   :538-577) and saveKeyFramesAndFactor (:1654-1765).  The clouds, the key-frame store, the VoxelGrids and the scan-to-map
+   loop are on the device; transformAssociateToMap, transformUpdate, the key-frame test and the pose bookkeeping run on
+   the host in the reference's f32 / f64 types.  Loop closure (loopClosureThread, performLoopClosure) is not performed:
+   without a loop factor the iSAM2 estimate of a new key frame is the pose inserted for it up to f32 rounding (DESIGN.md §4.9), and
+   correctPoses is a no-op.  The reference's constants are fixed: mappingProcessInterval 0.3 s, window 50, key-frame
+   distance 0.3 m, loop search 5 m / 30 s; SCAN_PERIOD is the context's lins_params.scan_period.
+   All clouds are in the mapping node's YZX frame convention, like lins_gpu_scan2map's.
+   A context has one scan-to-map state, and the mapper uses it: a processed cycle replaces the map lins_gpu_map_set
+   installed, the cycles and lins_gpu_scan2map calls share the persistent matP / isDegenerate, and lins_gpu_mapper_reset
+   clears them.  Use a context of its own for the mapper when both are needed.  One device-to-host synchronisation per
+   processed cycle. */
+#define LINS_MAPPER_WINDOW 50     /* surroundingKeyframeSearchNum (parameters.h) */
+#define LINS_MAPPER_IMU_QUEUE 200 /* imuQueLength_ (:55) */
+typedef struct lins_mapper_desc {
+  double time;                    /* timeLaserOdometry: header stamp of the odometry and of the three clouds */
+  double quat[4];                 /* odometry pose.orientation x, y, z, w; converted as laserOdometryHandler (:711-724) */
+  double pos[3];                  /* odometry pose.position x, y, z */
+  const lins_point* corner;       /* laserCloudCornerLast (the estimator's less-sharp corners) */
+  const lins_point* surf;         /* laserCloudSurfLast (less-flat surfs) */
+  const lins_point* outlier;      /* laserCloudOutlierLast */
+  int32_t n_corner, n_surf, n_outlier, pad;
+} lins_mapper_desc;
+typedef struct lins_mapper_report {
+  int32_t processed;              /* the cycle ran (timeLaserOdometry - timeLastProcessing >= 0.3, :1821) */
+  int32_t skipped_interval;       /* the 0.3 s gate skipped it: nothing else changed */
+  int32_t n_map_corner_ds, n_map_surf_ds;    /* laserCloudCornerFromMapDSNum / SurfFromMapDSNum (0 without key frames) */
+  int32_t n_corner_ds, n_surf_ds, n_outlier_ds, n_surf_total_ds;  /* laserCloud{CornerLast,SurfLast,OutlierLast,SurfTotalLast}DSNum */
+  int32_t keyframe_saved;         /* saveKeyFramesAndFactor stored a key frame */
+  int32_t n_keyframes;            /* cloudKeyPoses3D->points.size() after the cycle */
+  int32_t window_len;             /* recentCornerCloudKeyFrames.size() used by this cycle's local map */
+  int32_t loop_candidate;         /* after a saved key frame: the key pose detectLoopClosure (:1043-1067) would pick (the
+                                     nearest within 5 m whose time differs by > 30 s), else -1.  From such a cycle on the
+                                     reference may close a loop this library does not */
+  float transform_guess[6];       /* transformTobeMapped after transformAssociateToMap (the scan-to-map start) */
+  float transform_aft_mapped[6];  /* transformAftMapped after the cycle */
+  lins_map_report map;            /* the scan-to-map loop (map.skipped = 1: the 10 / 100 gate failed, :1636, and
+                                     transformUpdate did not run) */
+} lins_mapper_report;
+/* forget every key frame, the IMU queue and the transforms: the state of a freshly constructed mapping node */
+int lins_gpu_mapper_reset(lins_ctx* ctx);
+/* ≙ imuHandler (:726-735) for n messages: time = header stamp, roll / pitch = what getRPY of the orientation gave
+   (stored to f32 like imuRoll / imuPitch); the library keeps the 200-entry ring */
+int lins_gpu_mapper_imu(lins_ctx* ctx, const double* time, const double* roll, const double* pitch, int n);
+/* ≙ laserOdometryHandler (:711-724) + the cloud handlers + one pass of run() (:1806-1855).  LINS_E_TOOBIG when a
+   VoxelGrid's div_x * div_y * div_z exceeds INT32_MAX (the leaf is too small for the cloud's extent); the mapper's state
+   (transforms, key frames, window, IMU queue) is then unchanged, and lins_gpu_mapper_download returns no clouds until
+   the next cycle completes.  rep may be NULL. */
+int lins_gpu_mapper_step(lins_ctx* ctx, const lins_mapper_desc* desc, lins_mapper_report* rep);
+/* the key poses (cloudKeyPoses6D: n_keyframes x 7 doubles x, y, z, roll, pitch, yaw, time; the first six are the f32
+   PointTypePose fields), the window (window_len key-frame ids, oldest first, as used by the last processed cycle) and that
+   cycle's clouds (x, y, z, intensity float records; sizes in its report): the local map after down-sampling, and the
+   scan's corner, surf, outlier and surf-total DS clouds.  NULL skips. */
+int lins_gpu_mapper_download(lins_ctx* ctx, double* key_poses, int32_t* window, float* map_corner_ds, float* map_surf_ds,
+                             float* corner_ds, float* surf_ds, float* outlier_ds, float* surf_total_ds);
+/* pcl::VoxelGrid<PointXYZI> on one cloud of n points (leaf > 0): the filter the mapper runs, as a call of its own.  out
+   has room for n records (x, y, z, intensity floats); *n_out receives the voxel count.  LINS_E_TOOBIG as above. */
+int lins_gpu_voxel_grid(lins_ctx* ctx, const lins_point* in, int n, float leaf, float* out, int* n_out);
+
 /* block until everything queued on the ctx stream has finished */
 int lins_gpu_sync(lins_ctx* ctx);
 

@@ -13,7 +13,7 @@ import subprocess
 
 import numpy as np
 
-from .ctypes_defs import (Batch, COV_SIZE, LinsBatchDesc, LinsCloud2Desc, LinsCloud2Layout, LinsFeatureParams, LinsLidarModel, LinsLidarModels, LinsMapReport, LinsParams, LinsPclDesc,
+from .ctypes_defs import (Batch, COV_SIZE, LinsBatchDesc, LinsCloud2Desc, LinsCloud2Layout, LinsFeatureParams, LinsLidarModel, LinsLidarModels, LinsMapperDesc, LinsMapperReport, LinsMapReport, LinsParams, LinsPclDesc,
                           LinsRawDesc, LinsReport, LinsScanResult, LinsSeqBeginDesc, LinsSeqInitParams, LinsSeqParams, LinsSeqPclDesc,
                           LinsSeqCloud2Desc, LinsSeqRawDesc, LinsSeqStepDesc, POINT_DTYPE, SCAN_RESULT_DTYPE, STATE_DIM, as_points, make_points, ptr)
 
@@ -36,17 +36,18 @@ EXPORTS = [
     "lins_gpu_extract_features", "lins_gpu_extract_ms", "lins_gpu_seq_step_pcl", "lins_gpu_project_scans", "lins_gpu_project_ms",
     "lins_gpu_seq_step_raw", "lins_gpu_decode_cloud2", "lins_gpu_decode_ms", "lins_gpu_seq_step_cloud2",
     "lins_gpu_project_scans_mixed", "lins_gpu_seq_step_raw_mixed", "lins_gpu_seq_step_cloud2_mixed",
+    "lins_gpu_mapper_reset", "lins_gpu_mapper_imu", "lins_gpu_mapper_step", "lins_gpu_mapper_download", "lins_gpu_voxel_grid",
 ]
 
 NVCC_ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]  # H100 (Hopper)
 NVCC_COMMON = NVCC_ARCH + ["-lineinfo", "-O3", "-std=c++17", "-Xcompiler", "-fPIC"]
 # translation units and their extra flags: lins_gpu.cu (the fused kernel and most of the C-ABI), lins_upload.cu (batch
 # upload), lins_map.cu (row F2's host side), lins_seq.cu (sequence mode), lins_features.cu (feature extraction),
-# lins_projection.cu (image projection), lins_cloud2.cu (PointCloud2 decoding) — all bit-exact, so no multiply-add contraction: the association and the map
+# lins_projection.cu (image projection), lins_cloud2.cu (PointCloud2 decoding), lins_mapper.cu (the mapping node's cycle) — all bit-exact, so no multiply-add contraction: the association and the map
 # fits depend on it — and lins_jacobian.cu (the tolerance-checked split Jacobian kernel: contraction allowed)
 UNITS = [("lins_gpu.cu", ["-fmad=false"]), ("lins_upload.cu", ["-fmad=false"]), ("lins_map.cu", ["-fmad=false"]),
          ("lins_seq.cu", ["-fmad=false"]), ("lins_features.cu", ["-fmad=false"]), ("lins_projection.cu", ["-fmad=false"]),
-         ("lins_cloud2.cu", ["-fmad=false"]), ("lins_jacobian.cu", [])]
+         ("lins_cloud2.cu", ["-fmad=false"]), ("lins_mapper.cu", ["-fmad=false"]), ("lins_jacobian.cu", [])]
 
 
 def build(force=False, verbose=False):
@@ -130,6 +131,11 @@ def lib():
         L.lins_gpu_project_scans_mixed.argtypes = [vp, C.POINTER(LinsLidarModels), C.POINTER(LinsRawDesc)] + [vp] * 9
         L.lins_gpu_seq_step_raw_mixed.argtypes = [vp, C.POINTER(LinsSeqRawDesc), C.POINTER(LinsLidarModels), C.POINTER(LinsFeatureParams), vp]
         L.lins_gpu_seq_step_cloud2_mixed.argtypes = [vp, C.POINTER(LinsSeqCloud2Desc), C.POINTER(LinsLidarModels), C.POINTER(LinsFeatureParams), vp]
+        L.lins_gpu_mapper_reset.argtypes = [vp]
+        L.lins_gpu_mapper_imu.argtypes = [vp, vp, vp, vp, C.c_int]
+        L.lins_gpu_mapper_step.argtypes = [vp, C.POINTER(LinsMapperDesc), C.POINTER(LinsMapperReport)]
+        L.lins_gpu_mapper_download.argtypes = [vp] + [vp] * 8
+        L.lins_gpu_voxel_grid.argtypes = [vp, vp, C.c_int, C.c_float, vp, C.POINTER(C.c_int)]
         _LIB = L
     return _LIB
 
@@ -301,6 +307,46 @@ class LinsGpu:
         self._ck(self.L.lins_gpu_map_associate(self.h, ptr(c), len(c), ptr(s), len(s), ptr(t), ptr(out["corner_knn"]), ptr(out["surf_knn"]),
                                                ptr(out["corner_coeff"]), ptr(out["surf_coeff"]), ptr(out["corner_mask"]), ptr(out["surf_mask"])))
         return out
+
+    # ---- the mapping node's cycle (lins_gpu_mapper_*) ---------------------------------------------------------------
+    def mapper_reset(self):
+        self._ck(self.L.lins_gpu_mapper_reset(self.h))
+
+    def mapper_imu(self, time, roll, pitch):
+        """imuHandler for each (stamp, roll, pitch) (the roll / pitch getRPY gave for the message's orientation)."""
+        t, r, p = (np.ascontiguousarray(np.atleast_1d(a), np.float64) for a in (time, roll, pitch))
+        self._ck(self.L.lins_gpu_mapper_imu(self.h, ptr(t), ptr(r), ptr(p), len(t)))
+
+    def mapper_step(self, time, quat_xyzw, pos, corner, surf, outlier):
+        """One mapping cycle from the odometry message (stamp, orientation, position) and the three YZX clouds;
+        returns the LinsMapperReport."""
+        c, s, o = as_points(corner), as_points(surf), as_points(outlier)
+        d = LinsMapperDesc(time=float(time), quat=(C.c_double * 4)(*[float(v) for v in quat_xyzw]),
+                           pos=(C.c_double * 3)(*[float(v) for v in pos]), corner=ptr(c), surf=ptr(s), outlier=ptr(o),
+                           n_corner=len(c), n_surf=len(s), n_outlier=len(o))
+        rep = LinsMapperReport()
+        self._ck(self.L.lins_gpu_mapper_step(self.h, C.byref(d), C.byref(rep)))
+        return rep
+
+    def mapper_download(self, rep):
+        """Key poses (n x 7: x, y, z, roll, pitch, yaw, time), the window's ids, and the last processed cycle's clouds
+        ((n, 4) float32: map_corner_ds, map_surf_ds, corner_ds, surf_ds, outlier_ds, surf_total_ds) whose sizes `rep`,
+        that cycle's report, gives."""
+        poses = np.zeros((rep.n_keyframes, 7))
+        window = np.zeros(rep.window_len, np.int32)
+        names = ("map_corner_ds", "map_surf_ds", "corner_ds", "surf_ds", "outlier_ds", "surf_total_ds")
+        sizes = (rep.n_map_corner_ds, rep.n_map_surf_ds, rep.n_corner_ds, rep.n_surf_ds, rep.n_outlier_ds, rep.n_surf_total_ds)
+        clouds = {k: np.zeros((n, 4), np.float32) for k, n in zip(names, sizes)}
+        self._ck(self.L.lins_gpu_mapper_download(self.h, ptr(poses), ptr(window), *[ptr(clouds[k]) for k in names]))
+        return poses, window, clouds
+
+    def voxel_grid(self, cloud, leaf):
+        """pcl::VoxelGrid<PointXYZI> on the device: (n_voxels, 4) float32 (x, y, z, intensity) centroids."""
+        p = as_points(cloud)
+        out = np.zeros((max(len(p), 1), 4), np.float32)
+        n = C.c_int(0)
+        self._ck(self.L.lins_gpu_voxel_grid(self.h, ptr(p), len(p), float(leaf), ptr(out), C.byref(n)))
+        return out[:n.value].copy()
 
     # ---- batched mode ------------------------------------------------------------------------------------------
     def batch_upload(self, batch):

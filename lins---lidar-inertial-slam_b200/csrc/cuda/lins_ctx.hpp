@@ -11,7 +11,9 @@
 #include <algorithm>
 #include <cstddef>
 #include <cstdint>
+#include <deque>
 #include <string>
+#include <unordered_map>
 #include <utility>
 #include <vector>
 
@@ -229,6 +231,52 @@ struct Cloud2State {
   EventPair ev;                            // around the last decode kernel (lins_gpu_decode_ms)
 };
 
+// The mapper (lins_mapper.cu): one VoxelGrid call's device record — the ordered-integer encodings of the finite points'
+// f32 min / max, the box, the voxel count
+struct VgInfo {
+  unsigned enc[6];   // min x y z, max x y z
+  int min_b[3], mul[3];
+  float inv;
+  int any;           // at least one finite point
+  int toobig;        // div_x * div_y * div_z > INT32_MAX
+  int count;         // voxels
+};
+constexpr int kMapperGrids = 6;  // per cycle: map corner, map surf, scan corner, surf, outlier, surf total
+// PointTypePose (:57-65): the f32 pose fields and the f64 time
+struct MapperKeyPose { float x, y, z, roll, pitch, yaw; double time; };
+// one stored key frame: its corner, surf and outlier DS clouds in the map frame
+struct MapperKeyFrame { Buf<float4> c[3]; int n[3] = {0, 0, 0}; };
+// the mapping node's scalar members the cycle reads and writes (lidar_mapping_node.cpp:198-214, :356-408)
+struct MapperScalars {
+  float transformLast[6] = {}, transformSum[6] = {}, transformIncre[6] = {}, transformTobeMapped[6] = {}, transformBefMapped[6] = {},
+        transformAftMapped[6] = {};
+  double imuTime[LINS_MAPPER_IMU_QUEUE] = {};
+  float imuRoll[LINS_MAPPER_IMU_QUEUE] = {}, imuPitch[LINS_MAPPER_IMU_QUEUE] = {};
+  int imuPointerFront = 0, imuPointerLast = -1;
+  double timeLastProcessing = -1;
+  int latestFrameID = 0;
+  float previousRobotPos[3] = {0.f, 0.f, 0.f};
+  std::deque<int> window;  // recent*CloudKeyFrames as key-frame ids, oldest first
+};
+struct MapperLast { bool valid = false; int n[6] = {0, 0, 0, 0, 0, 0}; };  // the last processed cycle's DS sizes
+struct MapperState {
+  MapperScalars s;
+  std::vector<MapperKeyPose> poses;          // cloudKeyPoses6D
+  std::vector<MapperKeyFrame> slots;         // the key-frame store: the window and the newest key frame
+  std::unordered_map<int, int> slot_of;      // key-frame id -> slot
+  std::vector<int> free_slots;
+  MapperLast last;
+  Buf<float4> in[3], ds[4], cat[3], map_ds[2];  // scan clouds, their DS (corner, surf, outlier, surf total), concatenations
+  Buf<float4> vg_in, vg_out;                 // lins_gpu_voxel_grid
+  Buf<float4, kPinned> h_in;
+  Buf<unsigned> key[2];
+  Buf<int> idx[2], head, vid;
+  Buf<unsigned char> temp;                   // CUB scratch
+  Buf<VgInfo> vg_info;
+  Buf<VgInfo, kPinned> h_vg_info, h_vg_init;
+  Buf<SeqCopy> copies; Buf<SeqCopy, kPinned> h_copies;
+};
+
 }  // namespace lins_capi
 
 struct lins_ctx {
@@ -287,6 +335,7 @@ struct lins_ctx {
     Buf<float> coeff_c, coeff_s;
     Buf<uint8_t> mask_c, mask_s;
   } mp;
+  lins_capi::MapperState mapper;  // lins_gpu_mapper_*, lins_gpu_voxel_grid
 };
 
 namespace lins_capi {
@@ -441,5 +490,18 @@ int upload_bytes(lins_ctx* ctx, void* dst, Buf<unsigned char, kPinned>& staging,
 // decoded and has no points), upload them and queue their decode into ctx->proj.up (qs, qs_off; no synchronisation).
 // off (n + 1) receives the host copy of qs_off.
 int cloud2_run(lins_ctx* ctx, const lins_cloud2_desc* d, const uint8_t* present, std::vector<int32_t>& off);
+// lins_map.cu: the grid origin of a host cloud; bucket-sort n device map points into g (n_dev: the device-resident
+// count of the first n that are real); queue the scan-to-map loop on the
+// queries in ctx->mp.q_c / q_s (nc, ns) from transform T, with the loop state's D2H into mp.h_loop (no synchronisation;
+// with gate_nc / gate_ns, device counts, the loop stops before its first pass unless *gate_nc > 10 && *gate_ns > 100);
+// read that state into T and a report; zero the persistent loop state (matP, isDegenerate)
+void map_grid_origin(const lins_point* host_pts, int n, float origin[3]);
+int map_build_grid(lins_ctx* ctx, lins_ctx::MapState::Grid& g, const float4* map, int n, const float origin[3], const int* n_dev = nullptr);
+int map_queue_loop(lins_ctx* ctx, int nc, int ns, const float* T, const int* gate_nc = nullptr, const int* gate_ns = nullptr);
+void map_loop_report(const lins_ctx* ctx, float* T, lins_map_report* rep);
+int map_reset_loop(lins_ctx* ctx);
+// lins_mapper.cu: queue pcl::VoxelGrid of n device points into out (room for n) with its record at info (device)
+int voxel_grid_queue(lins_ctx* ctx, const float4* in, int n, float leaf, float4* out, VgInfo* info);
+int voxel_grid_reserve(lins_ctx* ctx, int n);
 
 }  // namespace lins_capi

@@ -158,11 +158,11 @@ LINS_FHD void sextant(int64_t s, int64_t e, int j, int64_t& sp, int64_t& ep) {
   ep = b / 6 - 1;
 }
 
-// pcl::VoxelGrid, leaf 0.2 m: inverse leaf, the box bounds, and a point's voxel index
-LINS_FHD float voxel_inv() { return 1.0f / 0.2f; }
-LINS_FHD int voxel_bound(float v) { return (int)floorf(v * voxel_inv()); }
-LINS_FHD uint32_t voxel_key(float x, float y, float z, const int min_b[3], const int mul[3]) {
-  const float inv = voxel_inv();
+// pcl::VoxelGrid: inverse leaf (1.0f / leaf in f32, as setLeafSize takes it), the box bounds, and a point's voxel index.
+// The leaf defaults to the 0.2 m of feature extraction; the mapping node's filters pass 0.2 / 0.4.
+LINS_FHD float voxel_inv(float leaf = 0.2f) { return 1.0f / leaf; }
+LINS_FHD int voxel_bound(float v, float inv = voxel_inv()) { return (int)floorf(v * inv); }
+LINS_FHD uint32_t voxel_key(float x, float y, float z, const int min_b[3], const int mul[3], float inv = voxel_inv()) {
   const int i0 = (int)(floorf(x * inv) - (float)min_b[0]);
   const int i1 = (int)(floorf(y * inv) - (float)min_b[1]);
   const int i2 = (int)(floorf(z * inv) - (float)min_b[2]);

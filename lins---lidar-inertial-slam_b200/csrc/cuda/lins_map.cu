@@ -39,31 +39,44 @@ lins_map::GridIndex grid_index(const lins_ctx::MapState::Grid& g) {
   return gi;
 }
 
-// bucket-sort one map cloud into its grid (≙ kdtree*FromMap->setInputCloud, :1637-1638)
-int map_build_grid(lins_ctx* ctx, lins_ctx::MapState::Grid& g, const float4* map, int n, const lins_point* host_pts) {
-  using namespace lins_map;
-  g.n = n;
-  if (n <= 0) return LINS_OK;
+}  // namespace
+
+namespace lins_capi {
+
+// the grid origin of a host cloud: its finite minimum (cells are addressed by hash: the extent does not matter)
+void map_grid_origin(const lins_point* host_pts, int n, float origin[3]) {
   float mn[3] = {3.0e38f, 3.0e38f, 3.0e38f};
-  for (int i = 0; i < n; ++i) {  // origin = the finite minimum (cells are addressed by hash: the extent does not matter)
+  for (int i = 0; i < n; ++i) {
     const float v[3] = {host_pts[i].x, host_pts[i].y, host_pts[i].z};
     for (int k = 0; k < 3; ++k) if (v[k] == v[k] && std::fabs(v[k]) < 1.0e30f && v[k] < mn[k]) mn[k] = v[k];
   }
-  for (int k = 0; k < 3; ++k) if (!(mn[k] < 3.0e38f)) mn[k] = 0.f;
+  for (int k = 0; k < 3; ++k) origin[k] = mn[k] < 3.0e38f ? mn[k] : 0.f;
+}
+
+// bucket-sort one device-resident map cloud into its grid (≙ kdtree*FromMap->setInputCloud, :1637-1638).  Any finite
+// origin gives the same 5-NN: the cells are exact (lins_map.cuh: grid_cell) and addressed by hash.
+int map_build_grid(lins_ctx* ctx, lins_ctx::MapState::Grid& g, const float4* map, int n, const float origin[3], const int* n_dev) {
+  using namespace lins_map;
+  g.n = n;
+  if (n <= 0) return LINS_OK;
   unsigned nb = 4096;
   while (nb < 2u * (unsigned)n && nb < (1u << 24)) nb <<= 1;
   CK(g.start.reserve((size_t)nb + 2)); CK(g.count.reserve((size_t)nb + 2)); CK(g.cursor.reserve((size_t)nb + 2)); CK(g.sorted.reserve((size_t)n + 1));
   g.mask = nb - 1;
-  for (int k = 0; k < 3; ++k) g.origin[k] = mn[k];
+  for (int k = 0; k < 3; ++k) g.origin[k] = origin[k];
   const GridIndex gi = grid_index(g);
   CK(cudaMemsetAsync(g.count.p, 0, sizeof(int) * nb, ctx->stream));
-  lins_grid_count_kernel<<<(n + 255) / 256, 256, 0, ctx->stream>>>(map, n, gi, g.count.p);
+  lins_grid_count_kernel<<<(n + 255) / 256, 256, 0, ctx->stream>>>(map, n, n_dev, gi, g.count.p);
   lins_grid_scan_kernel<<<1, 1024, 0, ctx->stream>>>(g.count.p, g.start.p, g.cursor.p, (int)nb);
-  lins_grid_scatter_kernel<<<(n + 255) / 256, 256, 0, ctx->stream>>>(map, n, gi, g.cursor.p, g.sorted.p);
+  lins_grid_scatter_kernel<<<(n + 255) / 256, 256, 0, ctx->stream>>>(map, n, n_dev, gi, g.cursor.p, g.sorted.p);
   CK(cudaGetLastError());
   ctx->launches += 3;
   return LINS_OK;
 }
+
+}  // namespace lins_capi
+
+namespace {
 
 // queue one cornerOptimization + surfOptimization pass (5-NN, fits, block partials) that reads its constants from
 // m.consts (device); nothing is synchronised.  Returns the number of partial blocks.
@@ -122,36 +135,18 @@ int map_stage_queries(lins_ctx* ctx, const lins_point* corner, int nc, const lin
 
 }  // namespace
 
-extern "C" {
-
-int lins_gpu_map_set(lins_ctx* ctx, const lins_point* corner, int nc, const lins_point* surf, int ns) {
-  if (!ctx) return LINS_E_INVALID;
-  if (nc < 0 || ns < 0 || (nc > 0 && !corner) || (ns > 0 && !surf)) return fail(ctx, LINS_E_INVALID, "bad map clouds");
-  CK(cudaSetDevice(ctx->device));
-  int rc = upload2(ctx, ctx->mp.map_c, corner, nc, ctx->mp.map_s, surf, ns);
-  if (rc != LINS_OK) return rc;
-  ctx->mp.n_map_c = nc; ctx->mp.n_map_s = ns;
-  rc = map_build_grid(ctx, ctx->mp.grid_c, ctx->mp.map_c.p, nc, corner);
-  if (rc != LINS_OK) return rc;
-  return map_build_grid(ctx, ctx->mp.grid_s, ctx->mp.map_s.p, ns, surf);
+// scan2MapOptimization's gate (:1636) on device-resident map sizes: a failing map marks the loop done before its first pass
+__global__ void lins_map_gate_kernel(const int* __restrict__ nc, const int* __restrict__ ns, lins_map::MapLoopState* __restrict__ st) {
+  if (!(*nc > 10 && *ns > 100)) st->done = 1;
 }
 
-int lins_gpu_scan2map(lins_ctx* ctx, const lins_point* corner, int nc, const lins_point* surf, int ns, float* T, lins_map_report* rep) {
-  if (!ctx) return LINS_E_INVALID;
-  if (!T) return fail(ctx, LINS_E_INVALID, "null transform");
-  CK(cudaSetDevice(ctx->device));
+namespace lins_capi {
+
+// the iteration loop of scan2MapOptimization (:1640-1648) on the queries in ctx->mp.q_c / q_s and the map set up
+// in ctx->mp, queued up front with the loop state's D2H into mp.h_loop; nothing is synchronised
+int map_queue_loop(lins_ctx* ctx, int nc, int ns, const float* T, const int* gate_nc, const int* gate_ns) {
   using namespace lins_map;
-  lins_map_report r;
-  std::memset(&r, 0, sizeof(r));
   lins_ctx::MapState& m = ctx->mp;
-  if (m.n_map_c < 0) return fail(ctx, LINS_E_NOMAP, "lins_gpu_map_set has not been called");
-  if (!(m.n_map_c > 10 && m.n_map_s > 100)) {  // :1636
-    r.skipped = 1;
-    if (rep) *rep = r;
-    return LINS_OK;
-  }
-  int rc = map_stage_queries(ctx, corner, nc, surf, ns);
-  if (rc != LINS_OK) return rc;
   // The whole iteration loop (:1640-1648) is queued up front: transformTobeMapped, matP / isDegenerate and the report live
   // on the device (MapLoopState); the first pass uses libm sin / cos of the caller's transform (bit-identical to the
   // reference's first pass), later ones the constants the LM kernel derived on the device.
@@ -164,23 +159,80 @@ int lins_gpu_scan2map(lins_ctx* ctx, const lins_point* corner, int nc, const lin
   CK(cudaMemcpyAsync(m.loop.p, T, sizeof(float) * 6, cudaMemcpyHostToDevice, ctx->stream));  // (pageable sources: staged before the call returns)
   CK(cudaMemsetAsync(reinterpret_cast<char*>(m.loop.p) + offsetof(MapLoopState, done), 0, sizeof(MapLoopState) - offsetof(MapLoopState, done), ctx->stream));
   CK(cudaMemcpyAsync(m.consts.p, &pc0, sizeof(pc0), cudaMemcpyHostToDevice, ctx->stream));
+  if (gate_nc) {
+    lins_map_gate_kernel<<<1, 1, 0, ctx->stream>>>(gate_nc, gate_ns, m.loop.p);
+    CK(cudaGetLastError());
+    ctx->launches += 1;
+  }
   const bool grid = map_use_grid(true);
   for (int iter = 0; iter < LINS_MAP_MAX_ITER; ++iter) {
     int nblocks = 0;
-    rc = map_queue_pass(ctx, nc, ns, false, grid, &m.loop.p->done, &nblocks);
+    const int rc = map_queue_pass(ctx, nc, ns, false, grid, &m.loop.p->done, &nblocks);
     if (rc != LINS_OK) return rc;
     lins_map_lm_kernel<<<1, 32, 0, ctx->stream>>>(m.partial.p, nblocks, iter, m.loop.p, m.consts.p);
     CK(cudaGetLastError());
     ctx->launches += 1;
   }
   CK(cudaMemcpyAsync(m.h_loop.p, m.loop.p, sizeof(MapLoopState), cudaMemcpyDeviceToHost, ctx->stream));
-  CK(cudaStreamSynchronize(ctx->stream));
-  const MapLoopState& st = *m.h_loop.p;
+  return LINS_OK;
+}
+
+int map_reset_loop(lins_ctx* ctx) {
+  if (ctx->mp.loop.p) CK(cudaMemsetAsync(ctx->mp.loop.p, 0, sizeof(lins_map::MapLoopState), ctx->stream));
+  return LINS_OK;
+}
+
+// the report of the loop whose state mp.h_loop holds
+void map_loop_report(const lins_ctx* ctx, float* T, lins_map_report* rep) {
+  const lins_map::MapLoopState& st = *ctx->mp.h_loop.p;
+  lins_map_report r;
+  std::memset(&r, 0, sizeof(r));
   for (int i = 0; i < 6; ++i) T[i] = st.T[i];
   // a call whose first pass selects < 50 points takes no LM step (its later passes see the same transform), so nothing
   // was projected: it reports 0, like the reference's LMOptimization, while matP / isDegenerate persist for later calls
   r.iters = st.iters; r.converged = st.converged; r.degenerate = st.n_sel[0] >= 50 ? st.isDegenerate : 0;
   for (int i = 0; i < LINS_MAP_MAX_ITER; ++i) { r.n_sel[i] = st.n_sel[i]; r.delta_r[i] = st.delta_r[i]; r.delta_t[i] = st.delta_t[i]; }
+  *rep = r;
+}
+
+}  // namespace lins_capi
+
+extern "C" {
+
+int lins_gpu_map_set(lins_ctx* ctx, const lins_point* corner, int nc, const lins_point* surf, int ns) {
+  if (!ctx) return LINS_E_INVALID;
+  if (nc < 0 || ns < 0 || (nc > 0 && !corner) || (ns > 0 && !surf)) return fail(ctx, LINS_E_INVALID, "bad map clouds");
+  CK(cudaSetDevice(ctx->device));
+  int rc = upload2(ctx, ctx->mp.map_c, corner, nc, ctx->mp.map_s, surf, ns);
+  if (rc != LINS_OK) return rc;
+  ctx->mp.n_map_c = nc; ctx->mp.n_map_s = ns;
+  float oc[3], os[3];
+  map_grid_origin(corner, nc, oc);
+  map_grid_origin(surf, ns, os);
+  rc = map_build_grid(ctx, ctx->mp.grid_c, ctx->mp.map_c.p, nc, oc);
+  if (rc != LINS_OK) return rc;
+  return map_build_grid(ctx, ctx->mp.grid_s, ctx->mp.map_s.p, ns, os);
+}
+
+int lins_gpu_scan2map(lins_ctx* ctx, const lins_point* corner, int nc, const lins_point* surf, int ns, float* T, lins_map_report* rep) {
+  if (!ctx) return LINS_E_INVALID;
+  if (!T) return fail(ctx, LINS_E_INVALID, "null transform");
+  CK(cudaSetDevice(ctx->device));
+  lins_map_report r;
+  std::memset(&r, 0, sizeof(r));
+  lins_ctx::MapState& m = ctx->mp;
+  if (m.n_map_c < 0) return fail(ctx, LINS_E_NOMAP, "lins_gpu_map_set has not been called");
+  if (!(m.n_map_c > 10 && m.n_map_s > 100)) {  // :1636
+    r.skipped = 1;
+    if (rep) *rep = r;
+    return LINS_OK;
+  }
+  int rc = map_stage_queries(ctx, corner, nc, surf, ns);
+  if (rc != LINS_OK) return rc;
+  rc = map_queue_loop(ctx, nc, ns, T);
+  if (rc != LINS_OK) return rc;
+  CK(cudaStreamSynchronize(ctx->stream));
+  map_loop_report(ctx, T, &r);
   if (rep) *rep = r;
   return LINS_OK;
 }

@@ -304,10 +304,11 @@ __device__ __forceinline__ void grid_cell(const GridIndex& g, float x, float y, 
   iy = (unsigned)__double2int_rd((double)y - (double)g.oy);
   iz = (unsigned)__double2int_rd((double)z - (double)g.oz);
 }
-// counting sort of the map by bucket: count, (host-launched) scan, scatter
-__global__ void lins_grid_count_kernel(const float4* __restrict__ map, int n, GridIndex g, int* __restrict__ count) {
+// counting sort of the map by bucket: count, (host-launched) scan, scatter.  n_dev (optional): the device-resident
+// number of points, <= n, when the host only knows the capacity n
+__global__ void lins_grid_count_kernel(const float4* __restrict__ map, int n, const int* __restrict__ n_dev, GridIndex g, int* __restrict__ count) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= n) return;
+  if (i >= n || (n_dev && i >= *n_dev)) return;
   const float4 p = __ldg(&map[i]);
   unsigned ix, iy, iz;
   grid_cell(g, p.x, p.y, p.z, ix, iy, iz);
@@ -326,9 +327,10 @@ __global__ void __launch_bounds__(1024) lins_grid_scan_kernel(const int* __restr
   int run = part[threadIdx.x];
   for (int i = lo; i < hi; ++i) { start[i] = run; cursor[i] = run; run += count[i]; }
 }
-__global__ void lins_grid_scatter_kernel(const float4* __restrict__ map, int n, GridIndex g, int* __restrict__ cursor, float4* __restrict__ sorted) {
+__global__ void lins_grid_scatter_kernel(const float4* __restrict__ map, int n, const int* __restrict__ n_dev, GridIndex g, int* __restrict__ cursor,
+                                         float4* __restrict__ sorted) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= n) return;
+  if (i >= n || (n_dev && i >= *n_dev)) return;
   const float4 p = __ldg(&map[i]);
   unsigned ix, iy, iz;
   grid_cell(g, p.x, p.y, p.z, ix, iy, iz);

@@ -1,0 +1,647 @@
+// lins_mapper.cu — the mapping node's cycle (lidar_mapping_node.cpp run() :1806-1855, without loop closure) behind
+// lins_gpu_mapper_step, and the device pcl::VoxelGrid it runs (lins_gpu_voxel_grid).
+//
+// Device: the scan's three clouds, the key-frame store (each key frame's DS clouds transformed into the map frame once,
+// at save time, with its PointTypePose), the local map of the window (one gather launch), six VoxelGrids per cycle and
+// the scan-to-map loop of lins_map.cu.  Host: transformAssociateToMap, the window's deque of key-frame ids,
+// transformUpdate with the IMU ring, the 0.3 m key-frame test, the pose's round trip through gtsam's Rot3 and the
+// loop-candidate search, in the reference's f32 / f64 types (no multiply-add contraction: this unit is built with
+// -fmad=false and g++ does not contract on x86-64 without -mfma).
+//
+// VoxelGrid (csrc/host/feature_extraction.hpp restates PCL's applyFilter): the finite points' min / max (ordered-integer
+// atomics: min / max are exact in any order), min_b = floor(min * inv), the key floor(p * inv) - (float)min_b per axis
+// (lins_features.cuh: voxel_key), a stable CUB radix sort of (key, index), and one centroid per voxel, its points summed
+// in f32 in input order (the sort is stable), output in ascending key order.  Non-finite points and every point of a
+// call whose div_x * div_y * div_z exceeds INT32_MAX get the key 0xffffffff, which no voxel can have, and are dropped.
+//
+// Synchronisation: one per processed cycle.  The VoxelGrids' outputs are sized by their inputs and padded with NaN, the
+// later launches take those capacities, a device-side gate stops the scan-to-map loop when the map is too small, and
+// the six VoxelGrid records come back with the loop's state.
+#include <cuda_runtime.h>
+#include <cub/device/device_radix_sort.cuh>
+#include <cub/device/device_scan.cuh>
+
+#include <algorithm>
+#include <climits>
+#include <cmath>
+#include <cstdint>
+#include <cstring>
+
+#include "lins_ctx.hpp"
+#include "lins_features.cuh"
+
+using namespace lins_capi;
+
+namespace {
+
+constexpr unsigned kInvalidKey = 0xffffffffu;
+constexpr int kVgThreads = 256;
+
+__device__ __forceinline__ unsigned f2ord(float f) {
+  const unsigned u = __float_as_uint(f);
+  return (u & 0x80000000u) ? ~u : (u | 0x80000000u);
+}
+__device__ __forceinline__ float ord2f(unsigned u) { return __uint_as_float((u & 0x80000000u) ? (u & 0x7fffffffu) : ~u); }
+__device__ __forceinline__ bool finite3(const float4 p) { return isfinite(p.x) && isfinite(p.y) && isfinite(p.z); }
+
+__global__ void __launch_bounds__(kVgThreads) lins_vg_bounds_kernel(const float4* __restrict__ p, int n, VgInfo* __restrict__ info) {
+  unsigned e[6] = {0xffffffffu, 0xffffffffu, 0xffffffffu, 0u, 0u, 0u};
+  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
+    const float4 q = p[i];
+    if (!finite3(q)) continue;
+    const unsigned a[3] = {f2ord(q.x), f2ord(q.y), f2ord(q.z)};
+    for (int k = 0; k < 3; ++k) { e[k] = min(e[k], a[k]); e[3 + k] = max(e[3 + k], a[k]); }
+  }
+  for (int off = 16; off > 0; off >>= 1)
+    for (int k = 0; k < 6; ++k) {
+      const unsigned o = __shfl_xor_sync(0xffffffffu, e[k], off);
+      e[k] = k < 3 ? min(e[k], o) : max(e[k], o);
+    }
+  if ((threadIdx.x & 31) == 0) {
+    for (int k = 0; k < 3; ++k) { atomicMin(&info->enc[k], e[k]); atomicMax(&info->enc[3 + k], e[3 + k]); }
+  }
+}
+
+// getMinMax3D -> min_b, div_b, divb_mul (feature_extraction.hpp VoxelGrid::filter)
+__global__ void lins_vg_box_kernel(VgInfo* __restrict__ info) {
+  VgInfo& v = *info;
+  v.any = v.enc[0] != 0xffffffffu;
+  v.toobig = 0;
+  if (!v.any) return;
+  long long div[3];
+  for (int k = 0; k < 3; ++k) {
+    v.min_b[k] = lins_feat::voxel_bound(ord2f(v.enc[k]), v.inv);
+    div[k] = (long long)lins_feat::voxel_bound(ord2f(v.enc[3 + k]), v.inv) - v.min_b[k] + 1;
+  }
+  v.toobig = (double)div[0] * (double)div[1] * (double)div[2] > (double)INT_MAX;  // (exact below 2^53; no overflow)
+  v.mul[0] = 1; v.mul[1] = (int)div[0]; v.mul[2] = v.toobig ? 0 : (int)(div[0] * div[1]);
+}
+
+__global__ void __launch_bounds__(kVgThreads) lins_vg_key_kernel(const float4* __restrict__ p, int n, const VgInfo* __restrict__ info,
+                                                                 unsigned* __restrict__ key, int* __restrict__ idx) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  const VgInfo& v = *info;
+  const float4 q = p[i];
+  key[i] = v.any && !v.toobig && finite3(q) ? lins_feat::voxel_key(q.x, q.y, q.z, v.min_b, v.mul, v.inv) : kInvalidKey;
+  idx[i] = i;
+}
+
+__global__ void __launch_bounds__(kVgThreads) lins_vg_head_kernel(const unsigned* __restrict__ key, int n, int* __restrict__ head) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  head[i] = key[i] != kInvalidKey && (i == 0 || key[i] != key[i - 1]);
+}
+
+// one thread per voxel head: the f32 sums of its points in sorted (= input) order, divided by the count
+__global__ void __launch_bounds__(kVgThreads) lins_vg_centroid_kernel(const unsigned* __restrict__ key, const int* __restrict__ idx,
+                                                                      const int* __restrict__ vid, int n, const float4* __restrict__ p,
+                                                                      float4* __restrict__ out, VgInfo* __restrict__ info) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  const unsigned k = key[i];
+  if (k == kInvalidKey) return;
+  if (i + 1 == n || key[i + 1] == kInvalidKey) info->count = vid[i];
+  if (i > 0 && key[i - 1] == k) return;
+  float cx = 0.f, cy = 0.f, cz = 0.f, ci = 0.f;
+  int j = i;
+  for (; j < n && key[j] == k; ++j) {
+    const float4 q = p[idx[j]];
+    cx += q.x; cy += q.y; cz += q.z; ci += q.w;
+  }
+  const float c = (float)(j - i);
+  out[vid[i] - 1] = make_float4(cx / c, cy / c, cz / c, ci / c);
+}
+
+// transformPointCloud (:624-652) with the constants of updateTransformPointCloudSinCos (:609-622)
+struct TfConsts { float cr, sr, cp, sp, cy, sy, tx, ty, tz; };
+__global__ void __launch_bounds__(256) lins_mapper_transform_kernel(const float4* __restrict__ in, float4* __restrict__ out, int n, TfConsts c) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  const float4 p = in[i];
+  const float x1 = c.cy * p.x - c.sy * p.y;
+  const float y1 = c.sy * p.x + c.cy * p.y;
+  const float z1 = p.z;
+  const float x2 = x1;
+  const float y2 = c.cr * y1 - c.sr * z1;
+  const float z2 = c.sr * y1 + c.cr * z1;
+  out[i] = make_float4(c.cp * x2 + c.sp * z2 + c.tx, y2 + c.ty, -c.sp * x2 + c.cp * z2 + c.tz, p.w);
+}
+
+// one block per contiguous copy (the local map's concatenation, the surf-total concatenation)
+__global__ void lins_mapper_gather_kernel(const SeqCopy* __restrict__ copies) {
+  const SeqCopy c = copies[blockIdx.x];
+  for (int i = threadIdx.x; i < c.n; i += blockDim.x) c.dst[i] = c.src[i];
+}
+
+}  // namespace
+
+namespace lins_capi {
+
+// the scratch of VoxelGrids of up to n points (grow-only; call before queuing work that a growth could free under)
+int voxel_grid_reserve(lins_ctx* ctx, int n) {
+  MapperState& M = ctx->mapper;
+  if (n <= 0) return LINS_OK;
+  CK(M.key[0].reserve((size_t)n)); CK(M.key[1].reserve((size_t)n)); CK(M.idx[0].reserve((size_t)n)); CK(M.idx[1].reserve((size_t)n));
+  CK(M.head.reserve((size_t)n)); CK(M.vid.reserve((size_t)n));
+  size_t b_sort = 0, b_scan = 0;
+  CK(cub::DeviceRadixSort::SortPairs(nullptr, b_sort, M.key[0].p, M.key[1].p, M.idx[0].p, M.idx[1].p, n, 0, 32, ctx->stream));
+  CK(cub::DeviceScan::InclusiveSum(nullptr, b_scan, M.head.p, M.vid.p, n, ctx->stream));
+  CK(M.temp.reserve(std::max(b_sort, b_scan) + 16));
+  return LINS_OK;
+}
+
+// queue one VoxelGrid of the n device points `in` into `out` (room for n: the centroids, then NaN records), with its
+// record at info (device); the count and the flags are read back by the caller
+int voxel_grid_queue(lins_ctx* ctx, const float4* in, int n, float leaf, float4* out, VgInfo* info) {
+  MapperState& M = ctx->mapper;
+  VgInfo init;
+  std::memset(&init, 0, sizeof(init));
+  for (int k = 0; k < 3; ++k) { init.enc[k] = 0xffffffffu; init.enc[3 + k] = 0u; }
+  init.inv = lins_feat::voxel_inv(leaf);
+  CK(M.h_vg_init.reserve(kMapperGrids));
+  // (pinned: a pageable H2D could complete before the copy engine reads it, but the staging is per-record and rewritten
+  // only after the cycle's read-back)
+  const int slot = (int)(info - M.vg_info.p);
+  M.h_vg_init.p[slot] = init;
+  CK(cudaMemcpyAsync(info, &M.h_vg_init.p[slot], sizeof(VgInfo), cudaMemcpyHostToDevice, ctx->stream));
+  if (n <= 0) return LINS_OK;
+  int rc = voxel_grid_reserve(ctx, n);
+  if (rc != LINS_OK) return rc;
+  CK(cudaMemsetAsync(out, 0xff, sizeof(float4) * (size_t)n, ctx->stream));  // NaN past the voxel count
+  size_t bytes;
+  const int blocks = (n + kVgThreads - 1) / kVgThreads;
+  lins_vg_bounds_kernel<<<std::min(blocks, 8 * ctx->sm_count), kVgThreads, 0, ctx->stream>>>(in, n, info);
+  lins_vg_box_kernel<<<1, 1, 0, ctx->stream>>>(info);
+  lins_vg_key_kernel<<<blocks, kVgThreads, 0, ctx->stream>>>(in, n, info, M.key[0].p, M.idx[0].p);
+  CK(cudaGetLastError());
+  bytes = M.temp.cap;
+  CK(cub::DeviceRadixSort::SortPairs(M.temp.p, bytes, M.key[0].p, M.key[1].p, M.idx[0].p, M.idx[1].p, n, 0, 32, ctx->stream));
+  lins_vg_head_kernel<<<blocks, kVgThreads, 0, ctx->stream>>>(M.key[1].p, n, M.head.p);
+  bytes = M.temp.cap;
+  CK(cub::DeviceScan::InclusiveSum(M.temp.p, bytes, M.head.p, M.vid.p, n, ctx->stream));
+  lins_vg_centroid_kernel<<<blocks, kVgThreads, 0, ctx->stream>>>(M.key[1].p, M.idx[1].p, M.vid.p, n, in, out, info);
+  CK(cudaGetLastError());
+  ctx->launches += 7;
+  return LINS_OK;
+}
+
+}  // namespace lins_capi
+
+namespace {
+
+// ---- host scalar code, typed as the reference types it ---------------------------------------------------------------
+// tf::Matrix3x3(q).getRPY(roll, pitch, yaw) (tf/LinearMath/Matrix3x3.h: setRotation, getEulerYPR with solution 1)
+void tf_get_rpy(double qx, double qy, double qz, double qw, double& roll, double& pitch, double& yaw) {
+  const double d = qx * qx + qy * qy + qz * qz + qw * qw;
+  const double s = 2.0 / d;
+  const double xs = qx * s, ys = qy * s, zs = qz * s;
+  const double wx = qw * xs, wy = qw * ys, wz = qw * zs;
+  const double xx = qx * xs, xy = qx * ys, xz = qx * zs;
+  const double yy = qy * ys, yz = qy * zs, zz = qz * zs;
+  const double m00 = 1.0 - (yy + zz), m10 = xy + wz, m20 = xz - wy, m21 = yz + wx, m22 = 1.0 - (xx + yy);
+  if (std::fabs(m20) >= 1) {
+    yaw = 0;
+    const double delta = std::atan2(m21, m22);
+    if (m20 < 0) { pitch = M_PI / 2.0; roll = delta; }
+    else { pitch = -M_PI / 2.0; roll = delta; }
+  } else {
+    pitch = -std::asin(m20);
+    roll = std::atan2(m21 / std::cos(pitch), m22 / std::cos(pitch));
+    yaw = std::atan2(m10 / std::cos(pitch), m00 / std::cos(pitch));
+  }
+}
+
+// gtsam Rot3::RzRyRx(x, y, z) (the matrix representation) and Rot3::xyz() through RQ; ypr = (z, y, x):
+// roll() = x, pitch() = y, yaw() = z
+void rot3_rzryrx(double x, double y, double z, double R[3][3]) {
+  const double cx = std::cos(x), sx = std::sin(x), cy = std::cos(y), sy = std::sin(y), cz = std::cos(z), sz = std::sin(z);
+  const double ss_ = sx * sy, cs_ = cx * sy, sc_ = sx * cy, cc_ = cx * cy, c_s = cx * sz, s_s = sx * sz, _cs = cy * sz, _cc = cy * cz,
+               s_c = sx * cz, c_c = cx * cz, ssc = ss_ * cz, csc = cs_ * cz, sss = ss_ * sz, css = cs_ * sz;
+  const double M[3][3] = {{_cc, -c_s + ssc, s_s + csc}, {_cs, c_c + sss, -s_c + css}, {-sy, sc_, cc_}};
+  std::memcpy(R, M, sizeof(M));
+}
+void mat_mul3(const double A[3][3], const double B[3][3], double C[3][3]) {
+  for (int i = 0; i < 3; ++i)
+    for (int j = 0; j < 3; ++j) C[i][j] = A[i][0] * B[0][j] + A[i][1] * B[1][j] + A[i][2] * B[2][j];
+}
+void rot3_xyz(const double A[3][3], double xyz[3]) {
+  const double x = -std::atan2(-A[2][1], A[2][2]);
+  const double cqx = std::cos(-x), sqx = std::sin(-x);
+  const double Qx[3][3] = {{1, 0, 0}, {0, cqx, -sqx}, {0, sqx, cqx}};
+  double B[3][3];
+  mat_mul3(A, Qx, B);
+  const double y = -std::atan2(B[2][0], B[2][2]);
+  const double cqy = std::cos(-y), sqy = std::sin(-y);
+  const double Qy[3][3] = {{cqy, 0, sqy}, {0, 1, 0}, {-sqy, 0, cqy}};
+  double Cm[3][3];
+  mat_mul3(B, Qy, Cm);
+  const double z = -std::atan2(-Cm[1][0], Cm[1][1]);
+  xyz[0] = x; xyz[1] = y; xyz[2] = z;
+}
+
+// transformAssociateToMap (:411-536); cos / sin / asin / atan2 of floats are the f32 overloads (DESIGN.md §4.4)
+void transform_associate_to_map(MapperScalars& s) {
+  const float* Sum = s.transformSum;
+  const float* Bef = s.transformBefMapped;
+  const float* Aft = s.transformAftMapped;
+  float* Inc = s.transformIncre;
+  float* T = s.transformTobeMapped;
+  using std::cos; using std::sin;
+  float x1 = cos(Sum[1]) * (Bef[3] - Sum[3]) - sin(Sum[1]) * (Bef[5] - Sum[5]);
+  float y1 = Bef[4] - Sum[4];
+  float z1 = sin(Sum[1]) * (Bef[3] - Sum[3]) + cos(Sum[1]) * (Bef[5] - Sum[5]);
+  float x2 = x1;
+  float y2 = cos(Sum[0]) * y1 + sin(Sum[0]) * z1;
+  float z2 = -sin(Sum[0]) * y1 + cos(Sum[0]) * z1;
+  Inc[3] = cos(Sum[2]) * x2 + sin(Sum[2]) * y2;
+  Inc[4] = -sin(Sum[2]) * x2 + cos(Sum[2]) * y2;
+  Inc[5] = z2;
+  const float sbcx = sin(Sum[0]), cbcx = cos(Sum[0]), sbcy = sin(Sum[1]), cbcy = cos(Sum[1]), sbcz = sin(Sum[2]), cbcz = cos(Sum[2]);
+  const float sblx = sin(Bef[0]), cblx = cos(Bef[0]), sbly = sin(Bef[1]), cbly = cos(Bef[1]), sblz = sin(Bef[2]), cblz = cos(Bef[2]);
+  const float salx = sin(Aft[0]), calx = cos(Aft[0]), saly = sin(Aft[1]), caly = cos(Aft[1]), salz = sin(Aft[2]), calz = cos(Aft[2]);
+  const float srx = -sbcx * (salx * sblx + calx * cblx * salz * sblz + calx * calz * cblx * cblz) -
+                    cbcx * sbcy * (calx * calz * (cbly * sblz - cblz * sblx * sbly) - calx * salz * (cbly * cblz + sblx * sbly * sblz) + cblx * salx * sbly) -
+                    cbcx * cbcy * (calx * salz * (cblz * sbly - cbly * sblx * sblz) - calx * calz * (sbly * sblz + cbly * cblz * sblx) + cblx * cbly * salx);
+  T[0] = -std::asin(srx);
+  const float srycrx = sbcx * (cblx * cblz * (caly * salz - calz * salx * saly) - cblx * sblz * (caly * calz + salx * saly * salz) + calx * saly * sblx) -
+                       cbcx * cbcy * ((caly * calz + salx * saly * salz) * (cblz * sbly - cbly * sblx * sblz) +
+                                      (caly * salz - calz * salx * saly) * (sbly * sblz + cbly * cblz * sblx) - calx * cblx * cbly * saly) +
+                       cbcx * sbcy * ((caly * calz + salx * saly * salz) * (cbly * cblz + sblx * sbly * sblz) +
+                                      (caly * salz - calz * salx * saly) * (cbly * sblz - cblz * sblx * sbly) + calx * cblx * saly * sbly);
+  const float crycrx = sbcx * (cblx * sblz * (calz * saly - caly * salx * salz) - cblx * cblz * (saly * salz + caly * calz * salx) + calx * caly * sblx) +
+                       cbcx * cbcy * ((saly * salz + caly * calz * salx) * (sbly * sblz + cbly * cblz * sblx) +
+                                      (calz * saly - caly * salx * salz) * (cblz * sbly - cbly * sblx * sblz) + calx * caly * cblx * cbly) -
+                       cbcx * sbcy * ((saly * salz + caly * calz * salx) * (cbly * sblz - cblz * sblx * sbly) +
+                                      (calz * saly - caly * salx * salz) * (cbly * cblz + sblx * sbly * sblz) - calx * caly * cblx * sbly);
+  T[1] = std::atan2(srycrx / cos(T[0]), crycrx / cos(T[0]));
+  const float srzcrx = (cbcz * sbcy - cbcy * sbcx * sbcz) * (calx * salz * (cblz * sbly - cbly * sblx * sblz) - calx * calz * (sbly * sblz + cbly * cblz * sblx) + cblx * cbly * salx) -
+                       (cbcy * cbcz + sbcx * sbcy * sbcz) * (calx * calz * (cbly * sblz - cblz * sblx * sbly) - calx * salz * (cbly * cblz + sblx * sbly * sblz) + cblx * salx * sbly) +
+                       cbcx * sbcz * (salx * sblx + calx * cblx * salz * sblz + calx * calz * cblx * cblz);
+  const float crzcrx = (cbcy * sbcz - cbcz * sbcx * sbcy) * (calx * calz * (cbly * sblz - cblz * sblx * sbly) - calx * salz * (cbly * cblz + sblx * sbly * sblz) + cblx * salx * sbly) -
+                       (sbcy * sbcz + cbcy * cbcz * sbcx) * (calx * salz * (cblz * sbly - cbly * sblx * sblz) - calx * calz * (sbly * sblz + cbly * cblz * sblx) + cblx * cbly * salx) +
+                       cbcx * cbcz * (salx * sblx + calx * cblx * salz * sblz + calx * calz * cblx * cblz);
+  T[2] = std::atan2(srzcrx / cos(T[0]), crzcrx / cos(T[0]));
+  x1 = cos(T[2]) * Inc[3] - sin(T[2]) * Inc[4];
+  y1 = sin(T[2]) * Inc[3] + cos(T[2]) * Inc[4];
+  z1 = Inc[5];
+  x2 = x1;
+  y2 = cos(T[0]) * y1 - sin(T[0]) * z1;
+  z2 = sin(T[0]) * y1 + cos(T[0]) * z1;
+  T[3] = Aft[3] - (cos(T[1]) * x2 + sin(T[1]) * z2);
+  T[4] = Aft[4] - y2;
+  T[5] = Aft[5] - (-sin(T[1]) * x2 + cos(T[1]) * z2);
+}
+
+// transformUpdate (:538-577)
+void transform_update(MapperScalars& s, double timeLaserOdometry, double SCAN_PERIOD) {
+  float* T = s.transformTobeMapped;
+  if (s.imuPointerLast >= 0) {
+    float imuRollLast = 0, imuPitchLast = 0;
+    while (s.imuPointerFront != s.imuPointerLast) {
+      if (timeLaserOdometry + SCAN_PERIOD < s.imuTime[s.imuPointerFront]) break;
+      s.imuPointerFront = (s.imuPointerFront + 1) % LINS_MAPPER_IMU_QUEUE;
+    }
+    const int f = s.imuPointerFront;
+    if (timeLaserOdometry + SCAN_PERIOD > s.imuTime[f]) {
+      imuRollLast = s.imuRoll[f];
+      imuPitchLast = s.imuPitch[f];
+    } else {
+      const int b = (f + LINS_MAPPER_IMU_QUEUE - 1) % LINS_MAPPER_IMU_QUEUE;
+      const float ratioFront = (timeLaserOdometry + SCAN_PERIOD - s.imuTime[b]) / (s.imuTime[f] - s.imuTime[b]);
+      const float ratioBack = (s.imuTime[f] - timeLaserOdometry - SCAN_PERIOD) / (s.imuTime[f] - s.imuTime[b]);
+      imuRollLast = s.imuRoll[f] * ratioFront + s.imuRoll[b] * ratioBack;
+      imuPitchLast = s.imuPitch[f] * ratioFront + s.imuPitch[b] * ratioBack;
+    }
+    T[0] = 0.998 * T[0] + 0.002 * imuPitchLast;
+    T[2] = 0.998 * T[2] + 0.002 * imuRollLast;
+  }
+  for (int i = 0; i < 6; i++) {
+    s.transformBefMapped[i] = s.transformSum[i];
+    s.transformAftMapped[i] = T[i];
+  }
+}
+
+TfConsts tf_consts(const MapperKeyPose& k) {  // updateTransformPointCloudSinCos: libm's f32 sin / cos of the f32 fields
+  TfConsts c;
+  c.cr = std::cos(k.roll); c.sr = std::sin(k.roll); c.cp = std::cos(k.pitch); c.sp = std::sin(k.pitch);
+  c.cy = std::cos(k.yaw); c.sy = std::sin(k.yaw); c.tx = k.x; c.ty = k.y; c.tz = k.z;
+  return c;
+}
+
+int upload3(lins_ctx* ctx, const lins_mapper_desc* d) {
+  MapperState& M = ctx->mapper;
+  const int n[3] = {d->n_corner, d->n_surf, d->n_outlier};
+  const lins_point* src[3] = {d->corner, d->surf, d->outlier};
+  Buf<float4>* dst[3] = {&M.in[0], &M.in[1], &M.in[2]};
+  CK(M.h_in.reserve((size_t)n[0] + n[1] + n[2] + 1));
+  size_t o = 0;
+  for (int k = 0; k < 3; ++k) {
+    CK(dst[k]->reserve((size_t)n[k] + 1));
+    pack_into(M.h_in.p + o, src[k], n[k]);
+    if (n[k]) CK(cudaMemcpyAsync(dst[k]->p, M.h_in.p + o, sizeof(float4) * n[k], cudaMemcpyHostToDevice, ctx->stream));
+    o += n[k];
+  }
+  return LINS_OK;
+}
+
+// the copies go to entries base.. of the (reserved) staging and device lists: two batches of one cycle do not overlap
+int queue_copies(lins_ctx* ctx, const std::vector<SeqCopy>& copies, int base) {
+  MapperState& M = ctx->mapper;
+  int m = 0;
+  for (const SeqCopy& c : copies) if (c.n > 0) M.h_copies.p[base + m++] = c;
+  if (!m) return LINS_OK;
+  CK(cudaMemcpyAsync(M.copies.p + base, M.h_copies.p + base, sizeof(SeqCopy) * m, cudaMemcpyHostToDevice, ctx->stream));
+  lins_mapper_gather_kernel<<<m, 256, 0, ctx->stream>>>(M.copies.p + base);
+  CK(cudaGetLastError());
+  ctx->launches += 1;
+  return LINS_OK;
+}
+
+// the slot of key frame id (a free one, or a new one)
+MapperKeyFrame& keyframe_slot(MapperState& M, int id) {
+  auto it = M.slot_of.find(id);
+  if (it != M.slot_of.end()) return M.slots[it->second];
+  int s;
+  if (!M.free_slots.empty()) { s = M.free_slots.back(); M.free_slots.pop_back(); }
+  else { s = (int)M.slots.size(); M.slots.emplace_back(); }
+  M.slot_of[id] = s;
+  return M.slots[s];
+}
+
+}  // namespace
+
+extern "C" {
+
+int lins_gpu_mapper_reset(lins_ctx* ctx) {
+  if (!ctx) return LINS_E_INVALID;
+  CK(cudaSetDevice(ctx->device));
+  MapperState& M = ctx->mapper;
+  M.s = MapperScalars();
+  M.poses.clear();
+  for (auto& kv : M.slot_of) M.free_slots.push_back(kv.second);
+  M.slot_of.clear();
+  M.last = MapperLast();
+  return map_reset_loop(ctx);  // isDegenerate, matP
+}
+
+int lins_gpu_mapper_imu(lins_ctx* ctx, const double* time, const double* roll, const double* pitch, int n) {
+  if (!ctx) return LINS_E_INVALID;
+  if (n < 0 || (n > 0 && (!time || !roll || !pitch))) return fail(ctx, LINS_E_INVALID, "bad IMU arrays");
+  MapperScalars& s = ctx->mapper.s;
+  for (int i = 0; i < n; ++i) {  // imuHandler :731-734
+    s.imuPointerLast = (s.imuPointerLast + 1) % LINS_MAPPER_IMU_QUEUE;
+    s.imuTime[s.imuPointerLast] = time[i];
+    s.imuRoll[s.imuPointerLast] = (float)roll[i];
+    s.imuPitch[s.imuPointerLast] = (float)pitch[i];
+  }
+  return LINS_OK;
+}
+
+int lins_gpu_mapper_step(lins_ctx* ctx, const lins_mapper_desc* d, lins_mapper_report* rep) {
+  if (!ctx) return LINS_E_INVALID;
+  if (!d) return fail(ctx, LINS_E_INVALID, "null desc");
+  if (d->n_corner < 0 || d->n_surf < 0 || d->n_outlier < 0 || (d->n_corner && !d->corner) || (d->n_surf && !d->surf) ||
+      (d->n_outlier && !d->outlier))
+    return fail(ctx, LINS_E_INVALID, "bad mapper clouds");
+  CK(cudaSetDevice(ctx->device));
+  MapperState& M = ctx->mapper;
+  lins_mapper_report r;
+  std::memset(&r, 0, sizeof(r));
+  r.loop_candidate = -1;
+  MapperScalars s = M.s;  // committed only when the cycle completes
+  const double timeLaserOdometry = d->time;
+  {  // laserOdometryHandler :713-722
+    double roll, pitch, yaw;
+    tf_get_rpy(d->quat[2], -d->quat[0], -d->quat[1], d->quat[3], roll, pitch, yaw);
+    s.transformSum[0] = -pitch; s.transformSum[1] = -yaw; s.transformSum[2] = roll;
+    s.transformSum[3] = d->pos[0]; s.transformSum[4] = d->pos[1]; s.transformSum[5] = d->pos[2];
+  }
+  if (!(timeLaserOdometry - s.timeLastProcessing >= 0.3)) {  // :1821 (the odometry still replaces transformSum)
+    r.skipped_interval = 1;
+    r.n_keyframes = (int)M.poses.size();
+    r.window_len = (int)s.window.size();
+    for (int i = 0; i < 6; ++i) { r.transform_guess[i] = s.transformTobeMapped[i]; r.transform_aft_mapped[i] = s.transformAftMapped[i]; }
+    M.s = s;
+    if (rep) *rep = r;
+    return LINS_OK;
+  }
+  s.timeLastProcessing = timeLaserOdometry;
+  transform_associate_to_map(s);
+  for (int i = 0; i < 6; ++i) r.transform_guess[i] = s.transformTobeMapped[i];
+
+  // extractSurroundingKeyFrames :1201-1246 (the deque of ids)
+  const int numPoses = (int)M.poses.size();
+  if (numPoses > 0) {
+    if ((int)s.window.size() < LINS_MAPPER_WINDOW) {
+      s.window.clear();
+      for (int i = numPoses - 1; i >= 0; --i) {
+        s.window.push_front(i);
+        if ((int)s.window.size() >= LINS_MAPPER_WINDOW) break;
+      }
+    } else if (s.latestFrameID != numPoses - 1) {
+      s.window.pop_front();
+      s.latestFrameID = numPoses - 1;
+      s.window.push_back(s.latestFrameID);
+    }
+  }
+  // Everything up to the scan-to-map loop is queued without reading anything back: the VoxelGrids' outputs are sized
+  // by their inputs and filled with NaN past their counts, and the later stages take those capacities.  A NaN point is
+  // dropped by a VoxelGrid, is never a neighbour and never selects a query, and the block partials it leaves are zero,
+  // so the results equal those of the exact sizes.  The counts come back with the loop's state: one synchronisation.
+  const int n_in[3] = {d->n_corner, d->n_surf, d->n_outlier};
+  int n_cat[3] = {0, 0, d->n_surf + d->n_outlier};
+  for (int id : s.window) {
+    const MapperKeyFrame& kf = M.slots[M.slot_of.at(id)];
+    n_cat[0] += kf.n[0]; n_cat[1] += kf.n[1] + kf.n[2];
+  }
+  // every buffer of the cycle first (a growth frees memory queued work may still read)
+  const int n_max = std::max({n_cat[0], n_cat[1], n_cat[2]});
+  int rc = voxel_grid_reserve(ctx, n_max);
+  if (rc != LINS_OK) return rc;
+  CK(M.vg_info.reserve(kMapperGrids)); CK(M.h_vg_info.reserve(kMapperGrids));
+  for (int k = 0; k < 3; ++k) { CK(M.cat[k].reserve((size_t)n_cat[k] + 1)); CK(M.ds[k].reserve((size_t)n_in[k] + 1)); }
+  CK(M.ds[3].reserve((size_t)n_cat[2] + 1));
+  CK(M.map_ds[0].reserve((size_t)n_cat[0] + 1)); CK(M.map_ds[1].reserve((size_t)n_cat[1] + 1));
+  const size_t n_copies = 3 * s.window.size() + 2;
+  CK(M.h_copies.reserve(n_copies + 1)); CK(M.copies.reserve(n_copies + 1));
+  VgInfo* info = M.vg_info.p;
+  // the local map: corner_i ..., and surf_i, outlier_i interleaved (:1242-1246)
+  std::vector<SeqCopy> copies;
+  {
+    int oc = 0, os = 0;
+    for (int id : s.window) {
+      const MapperKeyFrame& kf = M.slots[M.slot_of.at(id)];
+      copies.push_back(SeqCopy{kf.c[0].p, M.cat[0].p + oc, kf.n[0], 0}); oc += kf.n[0];
+      copies.push_back(SeqCopy{kf.c[1].p, M.cat[1].p + os, kf.n[1], 0}); os += kf.n[1];
+      copies.push_back(SeqCopy{kf.c[2].p, M.cat[1].p + os, kf.n[2], 0}); os += kf.n[2];
+    }
+  }
+  if ((rc = queue_copies(ctx, copies, 0)) != LINS_OK) return rc;
+  const bool have_map = numPoses > 0;
+  if ((rc = voxel_grid_queue(ctx, M.cat[0].p, have_map ? n_cat[0] : 0, 0.2f, M.map_ds[0].p, info + 0)) != LINS_OK) return rc;
+  if ((rc = voxel_grid_queue(ctx, M.cat[1].p, have_map ? n_cat[1] : 0, 0.4f, M.map_ds[1].p, info + 1)) != LINS_OK) return rc;
+  // downsampleCurrentScan :1326-1349
+  if ((rc = upload3(ctx, d)) != LINS_OK) return rc;
+  const float leaf[3] = {0.2f, 0.4f, 0.4f};
+  for (int k = 0; k < 3; ++k)
+    if ((rc = voxel_grid_queue(ctx, M.in[k].p, n_in[k], leaf[k], M.ds[k].p, info + 2 + k)) != LINS_OK) return rc;
+  // laserCloudSurfTotalLast = surf DS + outlier DS: their NaN tails ride along and are dropped by the filter
+  copies.assign({SeqCopy{M.ds[1].p, M.cat[2].p, n_in[1], 0}, SeqCopy{M.ds[2].p, M.cat[2].p + n_in[1], n_in[2], 0}});
+  if ((rc = queue_copies(ctx, copies, (int)n_copies - 2)) != LINS_OK) return rc;
+  if ((rc = voxel_grid_queue(ctx, M.cat[2].p, n_cat[2], 0.4f, M.ds[3].p, info + 5)) != LINS_OK) return rc;
+
+  // scan2MapOptimization :1635-1652: without key poses the map is empty and the gate fails on the host; otherwise the
+  // loop is queued on the capacities and a device-side gate on the two map counts stops it before its first pass
+  lins_ctx::MapState& mp = ctx->mp;
+  if (have_map) {
+    CK(mp.map_c.reserve((size_t)n_cat[0] + 1)); CK(mp.map_s.reserve((size_t)n_cat[1] + 1));
+    CK(mp.q_c.reserve((size_t)n_in[0] + 1)); CK(mp.q_s.reserve((size_t)n_cat[2] + 1));
+    if (n_cat[0]) CK(cudaMemcpyAsync(mp.map_c.p, M.map_ds[0].p, sizeof(float4) * n_cat[0], cudaMemcpyDeviceToDevice, ctx->stream));
+    if (n_cat[1]) CK(cudaMemcpyAsync(mp.map_s.p, M.map_ds[1].p, sizeof(float4) * n_cat[1], cudaMemcpyDeviceToDevice, ctx->stream));
+    if (n_in[0]) CK(cudaMemcpyAsync(mp.q_c.p, M.ds[0].p, sizeof(float4) * n_in[0], cudaMemcpyDeviceToDevice, ctx->stream));
+    if (n_cat[2]) CK(cudaMemcpyAsync(mp.q_s.p, M.ds[3].p, sizeof(float4) * n_cat[2], cudaMemcpyDeviceToDevice, ctx->stream));
+    // the grids hold the real points only (a NaN tail would crowd one bucket); the searches take the capacities
+    const float origin[3] = {0.f, 0.f, 0.f};  // (any finite origin gives the same 5-NN)
+    if ((rc = map_build_grid(ctx, mp.grid_c, mp.map_c.p, n_cat[0], origin, &info[0].count)) != LINS_OK) return rc;
+    if ((rc = map_build_grid(ctx, mp.grid_s, mp.map_s.p, n_cat[1], origin, &info[1].count)) != LINS_OK) return rc;
+    mp.n_map_c = n_cat[0]; mp.n_map_s = n_cat[1];
+    if ((rc = map_queue_loop(ctx, n_in[0], n_cat[2], s.transformTobeMapped, &info[0].count, &info[1].count)) != LINS_OK) return rc;
+  }
+  CK(cudaMemcpyAsync(M.h_vg_info.p, info, sizeof(VgInfo) * kMapperGrids, cudaMemcpyDeviceToHost, ctx->stream));
+  CK(cudaStreamSynchronize(ctx->stream));  // the cycle's one read-back
+  M.last.valid = false;  // (a failed cycle has overwritten the previous one's clouds)
+  const VgInfo* hi = M.h_vg_info.p;
+  for (int i = 0; i < kMapperGrids; ++i)
+    if (hi[i].toobig) return fail(ctx, LINS_E_TOOBIG, "VoxelGrid: the leaf is too small for the cloud's extent (div_x * div_y * div_z > INT32_MAX)");
+  // (without key poses the reference returns before the filters and keeps the previous sizes, which are 0 then)
+  const int nmc = have_map ? hi[0].count : 0, nms = have_map ? hi[1].count : 0;
+  const int ndc = hi[2].count, nds = hi[3].count, ndo = hi[4].count, ndt = hi[5].count;
+  if (have_map) { mp.n_map_c = nmc; mp.n_map_s = nms; }
+  if (nmc > 10 && nms > 100) {
+    map_loop_report(ctx, s.transformTobeMapped, &r.map);
+    transform_update(s, timeLaserOdometry, ctx->prm.scan_period);
+  } else {
+    r.map.skipped = 1;
+  }
+
+  // saveKeyFramesAndFactor :1654-1765
+  const float cur[3] = {s.transformAftMapped[3], s.transformAftMapped[4], s.transformAftMapped[5]};  // currentRobotPosPoint
+  bool save = true;
+  {
+    const float dx = s.previousRobotPos[0] - cur[0], dy = s.previousRobotPos[1] - cur[1], dz = s.previousRobotPos[2] - cur[2];
+    if (std::sqrt(dx * dx + dy * dy + dz * dz) < 0.3) save = false;
+  }
+  if (save || M.poses.empty()) {
+    for (int k = 0; k < 3; ++k) s.previousRobotPos[k] = cur[k];
+    // the pose inserted into iSAM2, and (no loop factor: DESIGN.md §4.9) its estimate
+    const float* P = M.poses.empty() ? s.transformTobeMapped : s.transformAftMapped;
+    if (M.poses.empty()) for (int i = 0; i < 6; ++i) s.transformLast[i] = s.transformTobeMapped[i];
+    double R[3][3], xyz[3];
+    rot3_rzryrx(P[2], P[0], P[1], R);
+    rot3_xyz(R, xyz);  // roll() = xyz[0], pitch() = xyz[1], yaw() = xyz[2]
+    const double t[3] = {P[5], P[3], P[4]};  // Point3(x = T[5], y = T[3], z = T[4])
+    MapperKeyPose kp;
+    kp.x = (float)t[1]; kp.y = (float)t[2]; kp.z = (float)t[0];
+    kp.roll = (float)xyz[1]; kp.pitch = (float)xyz[2]; kp.yaw = (float)xyz[0];
+    kp.time = timeLaserOdometry;
+    const int id = (int)M.poses.size();
+    M.poses.push_back(kp);
+    if (M.poses.size() > 1) {
+      s.transformAftMapped[0] = (float)xyz[1]; s.transformAftMapped[1] = (float)xyz[2]; s.transformAftMapped[2] = (float)xyz[0];
+      s.transformAftMapped[3] = (float)t[1]; s.transformAftMapped[4] = (float)t[2]; s.transformAftMapped[5] = (float)t[0];
+      for (int i = 0; i < 6; ++i) { s.transformLast[i] = s.transformAftMapped[i]; s.transformTobeMapped[i] = s.transformAftMapped[i]; }
+    }
+    // the key frame's clouds, in the map frame once (its pose never changes without a loop closure)
+    MapperKeyFrame& kf = keyframe_slot(M, id);
+    const int nk[3] = {ndc, nds, ndo};
+    const TfConsts tc = tf_consts(kp);
+    for (int k = 0; k < 3; ++k) {
+      CK(kf.c[k].reserve((size_t)nk[k] + 1));
+      kf.n[k] = nk[k];
+      if (nk[k]) {
+        lins_mapper_transform_kernel<<<(nk[k] + 255) / 256, 256, 0, ctx->stream>>>(M.ds[k].p, kf.c[k].p, nk[k], tc);
+        CK(cudaGetLastError());
+        ctx->launches += 1;
+      }
+    }
+    r.keyframe_saved = 1;
+    // detectLoopClosure's candidate (:1050-1064): radius 5 m around currentRobotPosPoint, nearest first, |dt| > 30 s
+    float best = 0.f;
+    for (int i = 0; i < (int)M.poses.size(); ++i) {
+      const MapperKeyPose& q = M.poses[i];
+      const float ex = q.x - cur[0], ey = q.y - cur[1], ez = q.z - cur[2];
+      const float d2 = ex * ex + ey * ey + ez * ez;
+      if (!(d2 < 25.0f) || !(std::fabs(q.time - timeLaserOdometry) > 30.0)) continue;
+      if (r.loop_candidate < 0 || d2 < best) { r.loop_candidate = i; best = d2; }
+    }
+    // the store keeps the window and the newest key frame: nothing else can enter a later window
+    for (auto it = M.slot_of.begin(); it != M.slot_of.end();) {
+      const int kid = it->first;
+      if (kid != id && std::find(s.window.begin(), s.window.end(), kid) == s.window.end()) { M.free_slots.push_back(it->second); it = M.slot_of.erase(it); }
+      else ++it;
+    }
+  }
+  M.s = s;
+  M.last.valid = true;
+  M.last.n[0] = nmc; M.last.n[1] = nms; M.last.n[2] = ndc; M.last.n[3] = nds; M.last.n[4] = ndo; M.last.n[5] = ndt;
+  r.processed = 1;
+  r.n_map_corner_ds = nmc; r.n_map_surf_ds = nms;
+  r.n_corner_ds = ndc; r.n_surf_ds = nds; r.n_outlier_ds = ndo; r.n_surf_total_ds = ndt;
+  r.n_keyframes = (int)M.poses.size();
+  r.window_len = (int)s.window.size();
+  for (int i = 0; i < 6; ++i) r.transform_aft_mapped[i] = s.transformAftMapped[i];
+  if (rep) *rep = r;
+  return LINS_OK;
+}
+
+int lins_gpu_mapper_download(lins_ctx* ctx, double* key_poses, int32_t* window, float* map_corner_ds, float* map_surf_ds,
+                             float* corner_ds, float* surf_ds, float* outlier_ds, float* surf_total_ds) {
+  if (!ctx) return LINS_E_INVALID;
+  CK(cudaSetDevice(ctx->device));
+  MapperState& M = ctx->mapper;
+  if (key_poses)
+    for (size_t i = 0; i < M.poses.size(); ++i) {
+      const MapperKeyPose& k = M.poses[i];
+      const double v[7] = {k.x, k.y, k.z, k.roll, k.pitch, k.yaw, k.time};
+      std::memcpy(key_poses + 7 * i, v, sizeof(v));
+    }
+  if (window) { int i = 0; for (int id : M.s.window) window[i++] = id; }
+  float* dst[6] = {map_corner_ds, map_surf_ds, corner_ds, surf_ds, outlier_ds, surf_total_ds};
+  const float4* src[6] = {M.map_ds[0].p, M.map_ds[1].p, M.ds[0].p, M.ds[1].p, M.ds[2].p, M.ds[3].p};
+  bool any = false;
+  for (int k = 0; k < 6; ++k) {
+    if (!dst[k] || !M.last.valid || M.last.n[k] == 0) continue;
+    CK(cudaMemcpyAsync(dst[k], src[k], sizeof(float4) * M.last.n[k], cudaMemcpyDeviceToHost, ctx->stream));
+    any = true;
+  }
+  if (any) CK(cudaStreamSynchronize(ctx->stream));
+  return LINS_OK;
+}
+
+int lins_gpu_voxel_grid(lins_ctx* ctx, const lins_point* in, int n, float leaf, float* out, int* n_out) {
+  if (!ctx) return LINS_E_INVALID;
+  if (n < 0 || (n > 0 && (!in || !out)) || !n_out || !(leaf > 0.f) || !std::isfinite(leaf)) return fail(ctx, LINS_E_INVALID, "bad VoxelGrid arguments");
+  CK(cudaSetDevice(ctx->device));
+  MapperState& M = ctx->mapper;
+  CK(M.vg_info.reserve(kMapperGrids));
+  CK(M.vg_in.reserve((size_t)n + 1)); CK(M.vg_out.reserve((size_t)n + 1));
+  CK(M.h_in.reserve((size_t)n + 1));
+  pack_into(M.h_in.p, in, n);
+  if (n) CK(cudaMemcpyAsync(M.vg_in.p, M.h_in.p, sizeof(float4) * n, cudaMemcpyHostToDevice, ctx->stream));
+  int rc = voxel_grid_queue(ctx, M.vg_in.p, n, leaf, M.vg_out.p, M.vg_info.p);
+  if (rc != LINS_OK) return rc;
+  CK(M.h_vg_info.reserve(kMapperGrids));
+  CK(cudaMemcpyAsync(M.h_vg_info.p, M.vg_info.p, sizeof(VgInfo), cudaMemcpyDeviceToHost, ctx->stream));
+  CK(cudaStreamSynchronize(ctx->stream));
+  if (M.h_vg_info.p[0].toobig) return fail(ctx, LINS_E_TOOBIG, "VoxelGrid: the leaf is too small for the cloud's extent (div_x * div_y * div_z > INT32_MAX)");
+  const int c = n > 0 ? M.h_vg_info.p[0].count : 0;
+  if (c) {
+    CK(cudaMemcpyAsync(out, M.vg_out.p, sizeof(float4) * c, cudaMemcpyDeviceToHost, ctx->stream));
+    CK(cudaStreamSynchronize(ctx->stream));
+  }
+  *n_out = c;
+  return LINS_OK;
+}
+
+}  // extern "C"

@@ -60,6 +60,22 @@ class LinsMapReport(C.Structure):
                 ("n_sel", C.c_int32 * 10), ("delta_r", C.c_float * 10), ("delta_t", C.c_float * 10)]
 
 
+class LinsMapperDesc(C.Structure):
+    """lins_mapper_desc (include/lins_gpu.h): one mapping cycle's odometry and clouds."""
+    _fields_ = [("time", C.c_double), ("quat", C.c_double * 4), ("pos", C.c_double * 3), ("corner", C.c_void_p),
+                ("surf", C.c_void_p), ("outlier", C.c_void_p), ("n_corner", C.c_int32), ("n_surf", C.c_int32),
+                ("n_outlier", C.c_int32), ("pad", C.c_int32)]
+
+
+class LinsMapperReport(C.Structure):
+    """lins_mapper_report (include/lins_gpu.h)."""
+    _fields_ = [("processed", C.c_int32), ("skipped_interval", C.c_int32), ("n_map_corner_ds", C.c_int32),
+                ("n_map_surf_ds", C.c_int32), ("n_corner_ds", C.c_int32), ("n_surf_ds", C.c_int32), ("n_outlier_ds", C.c_int32),
+                ("n_surf_total_ds", C.c_int32), ("keyframe_saved", C.c_int32), ("n_keyframes", C.c_int32),
+                ("window_len", C.c_int32), ("loop_candidate", C.c_int32), ("transform_guess", C.c_float * 6),
+                ("transform_aft_mapped", C.c_float * 6), ("map", LinsMapReport)]
+
+
 class LinsScanResult(C.Structure):
     _fields_ = [
         ("scan_id", C.c_int32),

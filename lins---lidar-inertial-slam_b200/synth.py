@@ -131,6 +131,11 @@ def seq_lib():
         L.lins_seq_write_bag.argtypes = [C.POINTER(SynthCfg), C.c_uint64, C.c_int, C.c_char_p, C.c_char_p, C.c_char_p]
         L.lins_seq_run_bag.restype = C.c_void_p
         L.lins_seq_run_bag.argtypes = [C.c_char_p, C.c_char_p, C.c_char_p, C.c_int, C.c_int, C.c_int, C.POINTER(C.c_int)]
+        L.lins_seq_map_count.argtypes = [C.c_void_p]
+        L.lins_seq_map_array.restype = C.POINTER(C.c_double)
+        L.lins_seq_map_array.argtypes = [C.c_void_p, C.c_int]
+        L.lins_seq_map_cloud.restype = C.c_void_p
+        L.lins_seq_map_cloud.argtypes = [C.c_void_p, C.c_int, C.POINTER(C.c_void_p)]
         _SEQ = L
     return _SEQ
 
@@ -148,7 +153,26 @@ def _seq_record(L, h):
     ints = lambda which, cnt: np.ctypeslib.as_array(L.lins_seq_ints(h, which), shape=(cnt,)).copy() if cnt else np.zeros(0, np.int32)  # noqa: E731
     units = Batch(clouds, offsets, _copy(d.state_in, n * 19, np.float64), _copy(d.cov_in, n * 324, np.float64), arr(1, n * 7)) if n else None
     return dict(units=units, state_out=arr(0, n * 19).reshape(-1, 19), iters=ints(0, n), flags=ints(1, n), scan_index=ints(2, n),
-                status=ints(3, ns), global_est=arr(2, ns * 7).reshape(-1, 7), global_true=arr(3, ns * 7).reshape(-1, 7))
+                status=ints(3, ns), global_est=arr(2, ns * 7).reshape(-1, 7), global_true=arr(3, ns * 7).reshape(-1, 7),
+                map_inputs=_map_inputs(L, h))
+
+
+def _map_inputs(L, h):
+    """What the estimator published for the mapping node after each scan (LinsFusion::publishTopics): per published scan
+    the stamp, the odometry (YZX position + quaternion x, y, z, w of globalStateYZX_) and the YZX less-sharp, less-flat and
+    outlier clouds."""
+    m = L.lins_seq_map_count(h)
+    time = _copy(C.cast(L.lins_seq_map_array(h, 0), C.c_void_p).value, m, np.float64)
+    odom = _copy(C.cast(L.lins_seq_map_array(h, 1), C.c_void_p).value, 7 * m, np.float64).reshape(-1, 7)
+    clouds = []
+    for which in range(3):
+        o = C.c_void_p()
+        p = L.lins_seq_map_cloud(h, which, C.byref(o))
+        off = _copy(o.value, m + 1, np.int32)
+        pts = _copy(p, int(off[-1]), POINT_DTYPE)
+        clouds.append([pts[off[k]:off[k + 1]] for k in range(m)])
+    return [dict(time=float(time[k]), quat=odom[k, 3:], pos=odom[k, :3], corner=clouds[0][k], surf=clouds[1][k], outlier=clouds[2][k])
+            for k in range(m)]
 
 
 def write_sequence_bag(path, config="config3", seed=1, n_scans=12, lidar_topic="/velodyne_points", imu_topic="/imu/data", **overrides):
@@ -457,3 +481,35 @@ def generate_map_unit(config="config3", seed=1, n_keyframes=20, sigma_t=0.1, sig
         return MapUnit(*clouds, truth, guess)
     finally:
         L.lins_synth_map_unit_destroy(h)
+
+
+# ---- the mapping node's input along a drive (tools/synth/lins_synth.cpp: lins_synth_map_drive_create) ----------------
+def generate_map_drive(poses_xyzyaw, config="config3", seed=1, **overrides):
+    """One sweep at each sensor pose (rows x, y, z, yaw in the world) through the product's CPU front end: per scan the YZX
+    less-sharp corners, less-flat surfs and outliers the estimator publishes, and the true pose as the mapping node's
+    transform (rx, ry, rz, tx, ty, tz).  Returns (list of (corner, surf, outlier) POINT_DTYPE triples, truth (n, 6) f32)."""
+    L = lib()
+    L.lins_synth_map_drive_create.restype = C.c_void_p
+    L.lins_synth_map_drive_create.argtypes = [C.POINTER(SynthCfg), C.c_uint64, C.c_int, C.c_void_p]
+    L.lins_synth_map_drive_destroy.argtypes = [C.c_void_p]
+    L.lins_synth_map_drive_cloud.argtypes = [C.c_void_p, C.c_int, C.c_int, C.POINTER(C.c_void_p)]
+    L.lins_synth_map_drive_truth.argtypes = [C.c_void_p, C.c_void_p]
+    kw = dict(CONFIGS[config])
+    kw.update(overrides)
+    cfg = SynthCfg(**kw)
+    P = np.ascontiguousarray(poses_xyzyaw, np.float64).reshape(-1, 4)
+    h = L.lins_synth_map_drive_create(C.byref(cfg), seed, len(P), P.ctypes.data_as(C.c_void_p))
+    try:
+        scans = []
+        for k in range(len(P)):
+            trip = []
+            for which in range(3):
+                p = C.c_void_p()
+                n = L.lins_synth_map_drive_cloud(h, k, which, C.byref(p))
+                trip.append(_copy(p.value, n, POINT_DTYPE))
+            scans.append(tuple(trip))
+        truth = np.zeros((len(P), 6), np.float32)
+        L.lins_synth_map_drive_truth(h, truth.ctypes.data_as(C.c_void_p))
+        return scans, truth
+    finally:
+        L.lins_synth_map_drive_destroy(h)

@@ -1,8 +1,13 @@
 #!/usr/bin/env python
-"""tools/run_bag.py BAG [--lidar /velodyne_points] [--imu /imu/data] [--max-scans N] [--lidar-model 0|1]
+"""tools/run_bag.py BAG [--lidar /velodyne_points] [--imu /imu/data] [--max-scans N] [--lidar-model 0|1] [--map [--out DIR]]
 
 BASELINE.json configs[1] runner (GPU box): replays a ROS1 bag through the restated front end (image projection, feature
-extraction, IMU propagation) and the GPU IESKF update, prints the trajectory.  Uncompressed and lz4-compressed bags
+extraction, IMU propagation) and the GPU IESKF update, prints the trajectory.  With --map, every odometry output (what
+LinsFusion::publishTopics hands the mapping node: globalStateYZX_ and the YZX clouds) also runs one cycle of the device
+mapper (lins_gpu_mapper_step), and DIR/odometry.txt and DIR/mapped.txt receive the two trajectories, one line per
+published scan: stamp, then x y z qx qy qz qw of the odometry, resp. the processed flag and transformAftMapped (rx ry rz
+tx ty tz, the mapping node's YZX frame).  The replayed IMU messages are not fed to the mapper's roll / pitch queue (the
+front end reads their rates and accelerations only), so transformUpdate runs without the IMU blend.  Uncompressed and lz4-compressed bags
 are read directly; for bz2 run `python tools/bag_tool.py decompress IN.bag OUT.bag` first."""
 import argparse, importlib, os, sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
@@ -10,6 +15,8 @@ import numpy as np
 ap = argparse.ArgumentParser()
 ap.add_argument("bag"); ap.add_argument("--lidar", default="/velodyne_points"); ap.add_argument("--imu", default="/imu/data")
 ap.add_argument("--max-scans", type=int, default=0); ap.add_argument("--lidar-model", type=int, default=0)
+ap.add_argument("--map", action="store_true", help="run the mapping node's cycle after every odometry output")
+ap.add_argument("--out", default=".", help="with --map: directory for odometry.txt and mapped.txt")
 a = ap.parse_args()
 synth = importlib.import_module("lins---lidar-inertial-slam_b200.synth")
 out = synth.run_bag(a.bag, a.lidar, a.imu, a.max_scans, a.lidar_model)
@@ -17,3 +24,16 @@ print("scans", len(out["status"]), "IESKF updates", len(out["iters"]), "mean ite
 np.set_printoptions(precision=4, suppress=True)
 for k, (st, g) in enumerate(zip(out["status"], out["global_est"])):
     print(k, int(st), g)
+if a.map:
+    capi = importlib.import_module("lins---lidar-inertial-slam_b200.capi")
+    g = capi.LinsGpu()
+    g.mapper_reset()
+    os.makedirs(a.out, exist_ok=True)
+    with open(os.path.join(a.out, "odometry.txt"), "w") as fo, open(os.path.join(a.out, "mapped.txt"), "w") as fm:
+        for m in out["map_inputs"]:
+            rep = g.mapper_step(m["time"], m["quat"], m["pos"], m["corner"], m["surf"], m["outlier"])
+            fo.write("%.9f %s\n" % (m["time"], " ".join("%.9g" % v for v in list(m["pos"]) + list(m["quat"]))))
+            fm.write("%.9f %d %s\n" % (m["time"], rep.processed, " ".join("%.9g" % v for v in rep.transform_aft_mapped)))
+            last = rep
+    print("mapper:", len(out["map_inputs"]), "odometry outputs,", last.n_keyframes if out["map_inputs"] else 0, "key frames;",
+          "trajectories in", os.path.join(a.out, "odometry.txt"), "and", os.path.join(a.out, "mapped.txt"))

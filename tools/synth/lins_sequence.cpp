@@ -30,6 +30,12 @@ struct SeqRecord {
   std::vector<double> rel_true;  // true relative pose of that scan: t (3) + q (x,y,z,w)
   std::vector<int32_t> status;   // estimator status after each scan
   std::vector<double> global_est, global_true;  // per scan: position (3) + quaternion (x,y,z,w)
+  // what LinsFusion::publishTopics hands the mapping node after each scan of an initialised estimator
+  // (Estimator.cpp:177-318): the stamp, globalStateYZX_ (rn (3) + qbn (x,y,z,w)) and scan_last_'s YZX less-sharp,
+  // less-flat and outlier clouds
+  std::vector<double> map_time, map_odom;
+  std::vector<lins_point> map_cloud[3];
+  std::vector<int32_t> map_off[3] = {{0}, {0}, {0}};
 };
 
 void append_cloud(std::vector<lins_point>& dst, std::vector<int32_t>& off, const Cloud& c) {
@@ -132,9 +138,19 @@ void feed_scan(StateEstimator& est, ImageProjection& ip, SeqRecord* rec, int k, 
     mapC = est.scan_last_->cornerPointsLessSharp_.points;
   }
   est.last_report_.iters = 0;
+  const bool publishes = est.isInitialized();  // performStateEstimation publishes after every scan but the first
   const V3D a_last = acc.empty() ? V3D(0, 0, filter::G0) : acc.back(), g_last = gyr.empty() ? V3D() : gyr.back();
   est.processPCL(scan_time, lins::sensor_utils::Imu(scan_time, a_last, g_last), ip.segmentedCloud, ip.segMsg, ip.outlierCloud);
   rec->status.push_back((int)est.status_);
+  if (publishes) {
+    const auto& g = est.globalStateYZX_;
+    const double o[7] = {g.rn_.x(), g.rn_.y(), g.rn_.z(), g.qbn_.x(), g.qbn_.y(), g.qbn_.z(), g.qbn_.w()};
+    rec->map_time.push_back(scan_time);
+    rec->map_odom.insert(rec->map_odom.end(), o, o + 7);
+    append_cloud(rec->map_cloud[0], rec->map_off[0], est.scan_last_->cornerPointsLessSharpYZX_);
+    append_cloud(rec->map_cloud[1], rec->map_off[1], est.scan_last_->surfPointsLessFlatYZX_);
+    append_cloud(rec->map_cloud[2], rec->map_off[2], est.scan_last_->outlierPointCloudYZX_);
+  }
   if (verbose) std::fprintf(stderr, "[lins_seq] scan %d: status %d, IESKF iterations %d, %zu segmented points\n", k, (int)est.status_, (int)est.last_report_.iters, ip.segmentedCloud.size());
   if (will_run && est.last_report_.iters > 0) {
     // processScan swapped the scans: scan_last_ now IS the scan whose features were the queries
@@ -571,6 +587,18 @@ int lins_replay_handover_cloud(void* h, int which, const lins_point** pts) {
 }
 
 void lins_seq_destroy(void* h) { delete static_cast<SeqRecord*>(h); }
+// the mapping node's inputs of a record: n published scans; time (n), odom (n x 7: YZX position, quaternion x y z w), and
+// the YZX clouds (which: 0 less-sharp, 1 less-flat, 2 outlier) with their CSR offsets (n + 1)
+int lins_seq_map_count(void* h) { return (int)static_cast<SeqRecord*>(h)->map_time.size(); }
+const double* lins_seq_map_array(void* h, int which) {
+  SeqRecord* r = static_cast<SeqRecord*>(h);
+  return which == 0 ? r->map_time.data() : r->map_odom.data();
+}
+const lins_point* lins_seq_map_cloud(void* h, int which, const int32_t** off) {
+  SeqRecord* r = static_cast<SeqRecord*>(h);
+  *off = r->map_off[which].data();
+  return r->map_cloud[which].data();
+}
 int lins_seq_num_units(void* h) { return (int)static_cast<SeqRecord*>(h)->iters.size(); }
 int lins_seq_num_scans(void* h) { return (int)static_cast<SeqRecord*>(h)->status.size(); }
 void lins_seq_desc(void* h, lins_batch_desc* d) {

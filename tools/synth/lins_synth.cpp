@@ -446,6 +446,54 @@ void lins_synth_map_unit_transforms(void* h, float* truth, float* guess) {
   std::memcpy(guess, u->guess, sizeof(u->guess));
 }
 
+// ---- the mapping node's input along a drive: what the estimator publishes per scan ------------------------------------
+// One VLP-16 / 64-ring sweep at each given sensor pose (world x, y, z, yaw; roll = pitch = 0) of a seeded world, run through
+// the product's CPU front end: the less-sharp corners, less-flat surfs and outliers in the YZX frame the estimator
+// publishes them in (StateEstimator.hpp:1125-1150), and the pose as the mapping node's transform (rx, ry, rz, tx, ty, tz).
+struct MapDrive {
+  std::vector<std::vector<lins_point>> clouds[3];
+  std::vector<float> truth;
+};
+void* lins_synth_map_drive_create(const lins_synth_cfg* cfg, uint64_t seed, int n, const double* xyzyaw) {
+  MapDrive* d = new MapDrive();
+  Rng rng(seed);
+  LidarModel lm = cfg->lidar == 1 ? LidarModel::dense64() : LidarModel::vlp16();
+  World w = make_world(rng, cfg->world);
+  ImageProjection ip(lm);
+  FeatureExtractor fe(lm);
+  Twist still{V3D(0, 0, 0), V3D(0, 0, 0)};
+  d->truth.resize(6 * (size_t)n);
+  for (int k = 0; k < n; ++k) {
+    Pose T;
+    T.p = V3D(xyzyaw[4 * k], xyzyaw[4 * k + 1], xyzyaw[4 * k + 2]);
+    T.R = math_utils::rpy2Quat(V3D(0, 0, xyzyaw[4 * k + 3])).toRotationMatrix();
+    Cloud raw;
+    simulate_scan(w, lm, T, still, cfg->range_noise, rng, raw);
+    ip.process(raw);
+    ScanFeatures f;
+    fe.run(ip.segmentedCloud, ip.segMsg, f);
+    const Cloud* src[3] = {&f.cornerPointsLessSharp, &f.surfPointsLessFlat, &ip.outlierCloud};
+    for (int c = 0; c < 3; ++c) {
+      std::vector<lins_point> v;
+      for (const auto& p : src[c]->points) v.push_back(yzx(p));
+      d->clouds[c].push_back(std::move(v));
+    }
+    euler_of(T.R, T.p, &d->truth[6 * (size_t)k]);
+  }
+  return d;
+}
+void lins_synth_map_drive_destroy(void* h) { delete static_cast<MapDrive*>(h); }
+// which: 0 less-sharp corners, 1 less-flat surfs, 2 outliers
+int lins_synth_map_drive_cloud(void* h, int scan, int which, const lins_point** pts) {
+  const std::vector<lins_point>& v = static_cast<MapDrive*>(h)->clouds[which][scan];
+  *pts = v.data();
+  return (int)v.size();
+}
+void lins_synth_map_drive_truth(void* h, float* out) {
+  const MapDrive* d = static_cast<MapDrive*>(h);
+  std::memcpy(out, d->truth.data(), sizeof(float) * d->truth.size());
+}
+
 // The product's CPU front end alone (csrc/host/image_projection.hpp + feature_extraction.hpp) on one raw sweep, for the
 // tests that check these restatements against an independent Python one (tests/pyfront.py).  Every output array has room
 // for `cap` entries (>= line_num * scan_num); counts: n[0] segmented, n[1] outlier, n[2] sharp, n[3] less sharp, n[4] flat,

@@ -557,16 +557,14 @@ class LinsGpu:
         extract_features takes: seg (m x 4 float32 x, y, z, intensity), ground, col, range, start_ring, end_ring, ori (3),
         plus outlier (k x 4)."""
         model = model or LinsLidarModel.vlp16()
-        return self._project(sweeps, point_format, model.line_num,
-                             lambda d, *out: self.L.lins_gpu_project_scans(self.h, C.byref(model), C.byref(d), *out))
+        return self._project(sweeps, point_format, model.line_num, self.L.lins_gpu_project_scans, model)
 
     def project_scans_mixed(self, sweeps, models, model_of, point_format=0):
         """project_scans with sweep i projected by models[model_of[i]] (lins_gpu_project_scans_mixed); model_of may be None
         with one model.  start_ring / end_ring hold max(line_num) entries per sweep, those past its own model's line_num 0."""
         keep = {}
         t = self.models_table(models, model_of, keep)
-        return self._project(sweeps, point_format, max(m.line_num for m in models),
-                             lambda d, *out: self.L.lins_gpu_project_scans_mixed(self.h, C.byref(t), C.byref(d), *out))
+        return self._project(sweeps, point_format, max(m.line_num for m in models), self.L.lins_gpu_project_scans_mixed, t)
 
     @staticmethod
     def models_table(models, model_of, keep):
@@ -580,9 +578,9 @@ class LinsGpu:
             t.model_of = keep["model_of"].ctypes.data
         return t
 
-    def _project(self, sweeps, point_format, L, call):
-        """project_scans / project_scans_mixed: the outputs of `call(raw desc, *9 output pointers)` with L ring entries per
-        sweep."""
+    def _project(self, sweeps, point_format, L, entry, model):
+        """project_scans / project_scans_mixed: the outputs of the C entry `entry` called with `model` (a LinsLidarModel or
+        a LinsLidarModels table), with L ring entries per sweep."""
         keep = {}
         d = self._raw_desc(sweeps, point_format, keep)
         n, total = d.n_scans, int(keep["cloud_off"][-1])
@@ -592,7 +590,7 @@ class LinsGpu:
         ground, col, rng = np.zeros(max(total, 1), np.uint8), np.zeros(max(total, 1), np.uint32), np.zeros(max(total, 1), np.float32)
         sr, er = np.zeros((max(n, 1), max(L, 1)), np.int32), np.zeros((max(n, 1), max(L, 1)), np.int32)
         ori, counts = np.zeros((max(n, 1), 3), np.float32), np.zeros((max(n, 1), 2), np.int32)
-        self._ck(call(d, ptr(seg), ptr(ground), ptr(col), ptr(rng), ptr(outl), ptr(sr), ptr(er), ptr(ori), ptr(counts)))
+        self._ck(entry(self.h, C.byref(model), C.byref(d), ptr(seg), ptr(ground), ptr(col), ptr(rng), ptr(outl), ptr(sr), ptr(er), ptr(ori), ptr(counts)))
         x4 = (lambda a: a.astype(np.float32)) if point_format == 1 else (  # noqa: E731
             lambda a: np.stack([a["x"], a["y"], a["z"], a["intensity"]], 1).astype(np.float32).reshape(-1, 4))
         off = keep["cloud_off"]
@@ -624,22 +622,23 @@ class LinsGpu:
         removal, feature extraction and the filter step on the device): `step` has imu + imu_off as in seq_step, sweeps (one
         raw sweep per slot, as project_scans takes them; an absent slot's may be empty) and optionally present.  model: the
         LinsLidarModel every slot shares (None = VLP-16)."""
-        keep, d = {}, LinsSeqRawDesc()
-        si = self._seq_step_common(d, step, scan_imu, keep)
-        d.raw = self._raw_desc(step["sweeps"], point_format, keep)
-        model = model or LinsLidarModel.vlp16()
-        fp = fp or LinsFeatureParams.shipped()
-        self._ck(self.L.lins_gpu_seq_step_raw(self.h, C.byref(d), C.byref(model), C.byref(fp), ptr(si)))
+        self._seq_step_sweeps(self.L.lins_gpu_seq_step_raw, model or LinsLidarModel.vlp16(), {}, step, fp, scan_imu, point_format)
 
     def seq_step_raw_mixed(self, step, models, model_of, fp=None, scan_imu=None, point_format=0):
         """seq_step_raw with slot s's sweep projected by models[model_of[s]] (lins_gpu_seq_step_raw_mixed): models is a list
         of LinsLidarModel, model_of one entry per slot, absent slots included (None with one model)."""
-        keep, d = {}, LinsSeqRawDesc()
+        keep = {}
+        t = self.models_table(models, model_of, keep)
+        self._seq_step_sweeps(self.L.lins_gpu_seq_step_raw_mixed, t, keep, step, fp, scan_imu, point_format)
+
+    def _seq_step_sweeps(self, entry, model, keep, step, fp, scan_imu, point_format):
+        """seq_step_raw / seq_step_raw_mixed: the C entry `entry` called with `model` (a LinsLidarModel or a LinsLidarModels
+        table); `keep` holds what model points at."""
+        d = LinsSeqRawDesc()
         si = self._seq_step_common(d, step, scan_imu, keep)
         d.raw = self._raw_desc(step["sweeps"], point_format, keep)
-        t = self.models_table(models, model_of, keep)
         fp = fp or LinsFeatureParams.shipped()
-        self._ck(self.L.lins_gpu_seq_step_raw_mixed(self.h, C.byref(d), C.byref(t), C.byref(fp), ptr(si)))
+        self._ck(entry(self.h, C.byref(d), C.byref(model), C.byref(fp), ptr(si)))
 
     @staticmethod
     def cloud2_desc(msgs, keep, gap=0, base=0):
@@ -682,22 +681,23 @@ class LinsGpu:
         """Advance every present sequence by one sensor_msgs/PointCloud2 message (lins_gpu_seq_step_cloud2: the decode, then
         what seq_step_raw runs): `step` has imu + imu_off as in seq_step, msgs (one (layout, data) per slot, as cloud2_desc
         takes them; an absent slot's is not read) or desc (a prepared LinsCloud2Desc), and optionally present."""
-        keep, d = {}, LinsSeqCloud2Desc()
-        si = self._seq_step_common(d, step, scan_imu, keep)
-        d.cloud2 = desc if desc is not None else self.cloud2_desc(step["msgs"], keep, gap)
-        model = model or LinsLidarModel.vlp16()
-        fp = fp or LinsFeatureParams.shipped()
-        self._ck(self.L.lins_gpu_seq_step_cloud2(self.h, C.byref(d), C.byref(model), C.byref(fp), ptr(si)))
+        self._seq_step_msgs(self.L.lins_gpu_seq_step_cloud2, model or LinsLidarModel.vlp16(), {}, step, fp, scan_imu, desc, gap)
 
     def seq_step_cloud2_mixed(self, step, models, model_of, fp=None, scan_imu=None, desc=None, gap=0):
         """seq_step_cloud2 with slot s's message projected by models[model_of[s]] (lins_gpu_seq_step_cloud2_mixed): models
         and model_of as seq_step_raw_mixed takes them."""
-        keep, d = {}, LinsSeqCloud2Desc()
+        keep = {}
+        t = self.models_table(models, model_of, keep)
+        self._seq_step_msgs(self.L.lins_gpu_seq_step_cloud2_mixed, t, keep, step, fp, scan_imu, desc, gap)
+
+    def _seq_step_msgs(self, entry, model, keep, step, fp, scan_imu, desc, gap):
+        """seq_step_cloud2 / seq_step_cloud2_mixed: the C entry `entry` called with `model` (a LinsLidarModel or a
+        LinsLidarModels table); `keep` holds what model points at."""
+        d = LinsSeqCloud2Desc()
         si = self._seq_step_common(d, step, scan_imu, keep)
         d.cloud2 = desc if desc is not None else self.cloud2_desc(step["msgs"], keep, gap)
-        t = self.models_table(models, model_of, keep)
         fp = fp or LinsFeatureParams.shipped()
-        self._ck(self.L.lins_gpu_seq_step_cloud2_mixed(self.h, C.byref(d), C.byref(t), C.byref(fp), ptr(si)))
+        self._ck(entry(self.h, C.byref(d), C.byref(model), C.byref(fp), ptr(si)))
 
     def seq_download(self, reports=False):
         """dict: global_state, filter_state (S x 19), filter_cov (S x 324), results (SCAN_RESULT_DTYPE), status (S) and,

@@ -1,7 +1,8 @@
 // lins_ctx.hpp — host state of a C-ABI context (struct lins_ctx of include/lins_gpu.h) and the helpers the translation units
 // that implement the C-ABI share: lins_gpu.cu (fused kernel, single-scan and batched entry points, F1), lins_upload.cu
-// (batch upload), lins_map.cu (row F2), lins_seq.cu (sequence mode).  Host code only: a header that defines kernels cannot be included here, because
-// every unit that includes this one would define them again.
+// (batch upload, gather lists), lins_map.cu (row F2), lins_seq.cu (sequence mode), lins_mapper.cu (the mapping node) and
+// the front-end units.  Host code only: a header that defines kernels cannot be included here, because every unit that
+// includes this one would define them again.
 #pragma once
 #include <cuda_runtime.h>
 #if defined(__SSE2__)
@@ -102,8 +103,18 @@ struct EventPair {
   cudaError_t elapsed_ms(float* ms) const { return cudaEventElapsedTime(ms, ev[0], ev[1]); }
 };
 
-// One contiguous device-to-device copy of sequence mode (lins_seq.cu): query compaction and the map refresh
-struct SeqCopy { const float4* src; float4* dst; int n, pad; };
+// A gather list: contiguous device-to-device copies of float4 records, staged in pinned memory, copied to the device in
+// one H2D and run by one launch of a block per copy (lins_upload.cu).  Each user keeps its own list: a list's staging may
+// still be read by a queued H2D when another list is written.
+struct DevCopy { const float4* src; float4* dst; int n, pad; };
+struct CopyList {
+  Buf<DevCopy> dev; Buf<DevCopy, kPinned> host;
+  // room for n records (before any work is queued: growth frees the old buffers); records [base, base + n) from src into
+  // the staging and one H2D of them (none for n = 0); one launch of the staged records [base, base + n) (none for n = 0)
+  int reserve(lins_ctx* ctx, size_t n);
+  int stage(lins_ctx* ctx, const DevCopy* src, int n, int base);
+  int launch(lins_ctx* ctx, int base, int n);
+};
 
 // Sequence mode (lins_gpu_seq_*, lins_seq.cu): the running sequences' filter state and maps.  Maps are CSR over the
 // sequences in sequence order; `tree` holds the cloud a sequence's 1-NN index was last built on where that differs from
@@ -139,7 +150,7 @@ struct SeqState {
   Buf<unsigned char> status_d;                         // 3 x n: LINS_SEQ_* of the step (read by the post kernel), the
                                                        // transformToEnd mask, the IMU rows' use (lins_seq.cu: ImuUse)
   Buf<unsigned char, kPinned> h_status;
-  Buf<SeqCopy> copies; Buf<SeqCopy, kPinned> h_copies;
+  CopyList copies;                                     // query compaction, then the map refresh
   std::vector<int32_t> status;                         // host copy of status_d
   cudaEvent_t ev[5] = {nullptr, nullptr, nullptr, nullptr, nullptr};  // phase boundaries of the last step (lins_gpu_seq_phase_ms)
   bool ev_valid = false;
@@ -161,7 +172,7 @@ struct FeatState {
   Buf<float4> und, out[4];
   Buf<int, kPinned> h_counts;
   std::vector<int32_t> h_ring;
-  Buf<SeqCopy> copies; Buf<SeqCopy, kPinned> h_copies;  // the pack into sequence mode's feature buffers
+  CopyList copies;                                      // the pack into sequence mode's feature buffers
   EventPair ev;                                         // around the last extraction kernel (lins_gpu_extract_ms)
 };
 
@@ -274,7 +285,7 @@ struct MapperState {
   Buf<unsigned char> temp;                   // CUB scratch
   Buf<VgInfo> vg_info;
   Buf<VgInfo, kPinned> h_vg_info, h_vg_init;
-  Buf<SeqCopy> copies; Buf<SeqCopy, kPinned> h_copies;
+  CopyList copies;                           // the local map's concatenation, then the surf-total one
 };
 
 }  // namespace lins_capi
@@ -352,6 +363,34 @@ inline int fail(lins_ctx* c, int code, const char* what, cudaError_t e = cudaSuc
     cudaError_t _e = (call);                                                    \
     if (_e != cudaSuccess) return lins_capi::fail(ctx, LINS_E_CUDA, #call, _e); \
   } while (0)
+
+// CSR offsets of n ranges over data: off[0] = 0, non-decreasing, data non-null when off[n] > 0 (LINS_E_INVALID: what)
+inline int check_csr(lins_ctx* ctx, const int32_t* off, int n, const void* data, const char* what) {
+  if (!off || off[0] != 0) return fail(ctx, LINS_E_INVALID, what);
+  for (int i = 0; i < n; ++i) if (off[i + 1] < off[i]) return fail(ctx, LINS_E_INVALID, what);
+  if (off[n] > 0 && !data) return fail(ctx, LINS_E_INVALID, what);
+  return LINS_OK;
+}
+// a caller's cloud of n points: n >= 0, p non-null when n > 0 (LINS_E_INVALID: what)
+inline int check_cloud(lins_ctx* ctx, const void* p, int n, const char* what) {
+  return n < 0 || (n > 0 && !p) ? fail(ctx, LINS_E_INVALID, what) : LINS_OK;
+}
+
+// State rows: the C ABI passes 19 doubles per state, the device keeps 20 (the last one 0); a pose (t, q xyzw) is
+// state[0..2], state[6..9].  copy_rows: n rows of src_w doubles into rows of dst_w, a wider row's tail 0.
+inline void copy_rows(double* dst, size_t dst_w, const double* src, size_t src_w, size_t n) {
+  for (size_t i = 0; i < n; ++i)
+    for (size_t k = 0; k < dst_w; ++k) dst[i * dst_w + k] = k < src_w ? src[i * src_w + k] : 0.0;
+}
+inline void pad_states(double* dev, const double* abi, size_t n) { copy_rows(dev, 20, abi, 19, n); }
+inline void strip_states(double* abi, const double* dev, size_t n) { copy_rows(abi, 19, dev, 20, n); }
+inline void pose_to_state(const double* pose, double* state) { std::copy(pose, pose + 3, state); std::copy(pose + 3, pose + 7, state + 6); }
+inline void state_to_pose(const double* state, double* pose) { std::copy(state, state + 3, pose); std::copy(state + 6, state + 10, pose + 3); }
+
+// a D2H copy on the context's stream, skipped for a null destination or nothing to copy
+inline cudaError_t d2h(lins_ctx* ctx, void* dst, const void* src, size_t bytes) {
+  return dst && bytes ? cudaMemcpyAsync(dst, src, bytes, cudaMemcpyDeviceToHost, ctx->stream) : cudaSuccess;
+}
 
 // pcl::PointXYZI (32 B) -> (x, y, z, intensity) (16 B).  The destination is pinned staging that the copy engine
 // reads next and the host never reads back: SSE2 (x86-64 baseline) with non-temporal stores.

@@ -348,11 +348,10 @@ int features_run(lins_ctx* ctx, const lins_feature_params* fp, const lins_pcl_de
   if (!fp || !d || d->n_scans < 0) return fail(ctx, LINS_E_INVALID, "bad feature extraction arguments");
   if (d->line_num < 1 || d->line_num > lins_feat::kMaxLines) return fail(ctx, LINS_E_INVALID, "line_num outside 1..128");
   const int n = d->n_scans, L = d->line_num;
-  if (!d->cloud_off) return fail(ctx, LINS_E_INVALID, "null cloud offsets");
-  if (d->cloud_off[0] != 0) return fail(ctx, LINS_E_INVALID, "cloud offsets must start at 0");
-  for (int i = 0; i < n; ++i) if (d->cloud_off[i + 1] < d->cloud_off[i]) return fail(ctx, LINS_E_INVALID, "cloud offsets must be non-decreasing");
+  int rc = check_csr(ctx, d->cloud_off, n, d->cloud, "bad cloud offsets / cloud");
+  if (rc != LINS_OK) return rc;
   const int total = d->cloud_off[n];
-  if (total > 0 && (!d->cloud || !d->ground_flag || !d->col_ind || !d->range)) return fail(ctx, LINS_E_INVALID, "null per-point array");
+  if (total > 0 && (!d->ground_flag || !d->col_ind || !d->range)) return fail(ctx, LINS_E_INVALID, "null per-point array");
   if (n > 0 && (!d->start_ring_index || !d->end_ring_index || !d->orientation)) return fail(ctx, LINS_E_INVALID, "null cloud_info array");
   if (d->point_format != LINS_POINTS_XYZI32 && d->point_format != LINS_POINTS_PACKED16) return fail(ctx, LINS_E_INVALID, "bad point_format");
   CK(cudaSetDevice(ctx->device));
@@ -360,7 +359,7 @@ int features_run(lins_ctx* ctx, const lins_feature_params* fp, const lins_pcl_de
   std::vector<int32_t> zeros(n + 1, 0);
   const lins_point* pts[4] = {d->cloud, nullptr, nullptr, nullptr};
   const int32_t* offs[4] = {d->cloud_off, zeros.data(), zeros.data(), zeros.data()};
-  int rc = upload_clouds(ctx, f.up, n, pts, offs, d->point_format);  // (synchronises the stream first)
+  rc = upload_clouds(ctx, f.up, n, pts, offs, d->point_format);  // (synchronises the stream first)
   if (rc != LINS_OK) return rc;
   if (n == 0) return features_launch(ctx, fp, FeatInputs());
   const size_t N = (size_t)total + 1;

@@ -476,7 +476,8 @@ BatchView view_of(const Resident& r, bool reports, bool trace) {
 int stage_single(lins_ctx* ctx, const lins_point* surf_flat, int ns, const lins_point* corner_sharp, int nc,
                  const double* state_in, const double* cov_in, bool trace) {
   if (ctx->map_ns < 0) return fail(ctx, LINS_E_NOMAP, "lins_gpu_set_map has not been called");
-  if (ns < 0 || nc < 0 || (ns > 0 && !surf_flat) || (nc > 0 && !corner_sharp)) return fail(ctx, LINS_E_INVALID, "bad query cloud");
+  if (check_cloud(ctx, surf_flat, ns, "bad surf_flat cloud") != LINS_OK || check_cloud(ctx, corner_sharp, nc, "bad corner_sharp cloud") != LINS_OK)
+    return LINS_E_INVALID;
   Resident& r = ctx->single;
   r.n = 1; r.nqs = ns; r.nqc = nc; r.max_q = ns + nc;
   CK(r.qs.reserve(ns + 1)); CK(r.qc.reserve(nc + 1));
@@ -486,8 +487,7 @@ int stage_single(lins_ctx* ctx, const lins_point* surf_flat, int ns, const lins_
   pack_into(r.h_pts.p, surf_flat, ns);
   pack_into(r.h_pts.p + ns, corner_sharp, nc);
   r.h_off.p[0] = 0; r.h_off.p[1] = ns; r.h_off.p[2] = 0; r.h_off.p[3] = nc;
-  for (int i = 0; i < 19; ++i) r.h_state.p[i] = state_in[i];
-  r.h_state.p[19] = 0.0;
+  pad_states(r.h_state.p, state_in, 1);
   if (cov_in) std::memcpy(r.h_cov.p, cov_in, sizeof(double) * 324); else std::memset(r.h_cov.p, 0, sizeof(double) * 324);
   if (ns) CK(cudaMemcpyAsync(r.qs.p, r.h_pts.p, sizeof(float4) * ns, cudaMemcpyHostToDevice, ctx->stream));
   if (nc) CK(cudaMemcpyAsync(r.qc.p, r.h_pts.p + ns, sizeof(float4) * nc, cudaMemcpyHostToDevice, ctx->stream));
@@ -516,6 +516,30 @@ int upload_map_offsets(lins_ctx* ctx) {
   int h[8] = {0, ctx->map_ns, 0, ctx->map_nc, 0, ctx->tree_ns, 0, ctx->tree_nc};
   // (h is pageable stack memory: cudaMemcpyAsync returns once it has been copied to the driver's staging buffer)
   CK(cudaMemcpyAsync(ctx->map_off.p, h, sizeof(h), cudaMemcpyHostToDevice, ctx->stream));
+  return LINS_OK;
+}
+
+// r's outputs into the caller's arrays (each may be null; states as ABI rows) through r's pinned staging: one synchronisation
+int download_outputs(lins_ctx* ctx, Resident& r, double* state_out, double* cov_out, lins_scan_result* results, lins_report* reports) {
+  const size_t n = r.n;
+  if (state_out) { CK(r.h_state_out.reserve(n * 20)); CK(cudaMemcpyAsync(r.h_state_out.p, r.state_out.p, sizeof(double) * 20 * n, cudaMemcpyDeviceToHost, ctx->stream)); }
+  if (cov_out) { CK(r.h_cov_out.reserve(n * 324)); CK(cudaMemcpyAsync(r.h_cov_out.p, r.cov_out.p, sizeof(double) * 324 * n, cudaMemcpyDeviceToHost, ctx->stream)); }
+  if (results) { CK(r.h_results.reserve(n)); CK(cudaMemcpyAsync(r.h_results.p, r.results.p, sizeof(lins_scan_result) * n, cudaMemcpyDeviceToHost, ctx->stream)); }
+  if (reports) { CK(r.h_reports.reserve(n)); CK(cudaMemcpyAsync(r.h_reports.p, r.reports.p, sizeof(lins_report) * n, cudaMemcpyDeviceToHost, ctx->stream)); }
+  CK(cudaStreamSynchronize(ctx->stream));
+  if (state_out) strip_states(state_out, r.h_state_out.p, n);
+  if (cov_out) std::memcpy(cov_out, r.h_cov_out.p, sizeof(double) * 324 * n);
+  if (results) std::memcpy(results, r.h_results.p, sizeof(lins_scan_result) * n);
+  if (reports) std::memcpy(reports, r.h_reports.p, sizeof(lins_report) * n);
+  return LINS_OK;
+}
+
+// the correspondence IDs of r's last IESKF / association (each destination may be null); one stream synchronisation
+int download_indices(lins_ctx* ctx, const Resident& r, int32_t* surf_ind, int32_t* corner_ind) {
+  CK(cudaSetDevice(ctx->device));
+  CK(d2h(ctx, surf_ind, r.ind_s.p, sizeof(int32_t) * 3 * r.nqs));
+  CK(d2h(ctx, corner_ind, r.ind_c.p, sizeof(int32_t) * 2 * r.nqc));
+  CK(cudaStreamSynchronize(ctx->stream));
   return LINS_OK;
 }
 
@@ -616,7 +640,8 @@ int64_t lins_gpu_launch_count(const lins_ctx* ctx) { return ctx ? ctx->launches 
 
 int lins_gpu_set_map(lins_ctx* ctx, const lins_point* surf, int ns, const lins_point* corner, int nc) {
   if (!ctx) return LINS_E_INVALID;
-  if (ns < 0 || nc < 0 || (ns > 0 && !surf) || (nc > 0 && !corner)) return fail(ctx, LINS_E_INVALID, "bad map cloud");
+  if (check_cloud(ctx, surf, ns, "bad surf map cloud") != LINS_OK || check_cloud(ctx, corner, nc, "bad corner map cloud") != LINS_OK)
+    return LINS_E_INVALID;
   CK(cudaSetDevice(ctx->device));
   const int rc = upload2(ctx, ctx->map_s, surf, ns, ctx->map_c, corner, nc);
   if (rc != LINS_OK) return rc;
@@ -636,26 +661,13 @@ int lins_gpu_ieskf(lins_ctx* ctx, const lins_point* surf_flat, int ns, const lin
   CK(cudaMemsetAsync(r.reports.p, 0, sizeof(lins_report), ctx->stream));
   rc = launch(ctx, r, bv, make_kparams(ctx->prm, MODE_IESKF, 0));
   if (rc != LINS_OK) return rc;
-  CK(r.h_state_out.reserve(20)); CK(r.h_cov_out.reserve(324)); CK(r.h_reports.reserve(1));
-  CK(cudaMemcpyAsync(r.h_state_out.p, r.state_out.p, sizeof(double) * 20, cudaMemcpyDeviceToHost, ctx->stream));
-  CK(cudaMemcpyAsync(r.h_cov_out.p, r.cov_out.p, sizeof(double) * 324, cudaMemcpyDeviceToHost, ctx->stream));
-  CK(cudaMemcpyAsync(r.h_reports.p, r.reports.p, sizeof(lins_report), cudaMemcpyDeviceToHost, ctx->stream));
-  CK(cudaStreamSynchronize(ctx->stream));
-  if (state_out) std::memcpy(state_out, r.h_state_out.p, sizeof(double) * 19);
-  if (cov_out) std::memcpy(cov_out, r.h_cov_out.p, sizeof(double) * 324);
-  if (rep) *rep = r.h_reports.p[0];
-  return LINS_OK;
+  return download_outputs(ctx, r, state_out, cov_out, nullptr, rep);
 }
 
 int lins_gpu_download_indices(lins_ctx* ctx, int32_t* surf_ind, int32_t* corner_ind) {
   if (!ctx) return LINS_E_INVALID;
-  Resident& r = ctx->single;
-  if (r.n != 1 || !r.ind_s.p) return fail(ctx, LINS_E_INVALID, "no single-scan call has run");
-  CK(cudaSetDevice(ctx->device));
-  if (surf_ind && r.nqs) CK(cudaMemcpyAsync(surf_ind, r.ind_s.p, sizeof(int32_t) * 3 * r.nqs, cudaMemcpyDeviceToHost, ctx->stream));
-  if (corner_ind && r.nqc) CK(cudaMemcpyAsync(corner_ind, r.ind_c.p, sizeof(int32_t) * 2 * r.nqc, cudaMemcpyDeviceToHost, ctx->stream));
-  CK(cudaStreamSynchronize(ctx->stream));
-  return LINS_OK;
+  if (ctx->single.n != 1 || !ctx->single.ind_s.p) return fail(ctx, LINS_E_INVALID, "no single-scan call has run");
+  return download_indices(ctx, ctx->single, surf_ind, corner_ind);
 }
 
 int lins_gpu_associate(lins_ctx* ctx, const lins_point* surf_flat, int ns, const lins_point* corner_sharp, int nc,
@@ -671,18 +683,14 @@ int lins_gpu_associate(lins_ctx* ctx, const lins_point* surf_flat, int ns, const
   BatchView bv = single_view(ctx, true);
   rc = launch(ctx, r, bv, make_kparams(ctx->prm, MODE_ASSOC, iter));
   if (rc != LINS_OK) return rc;
-  auto d2h = [&](void* dst, const void* src, size_t bytes) -> cudaError_t {
-    if (!dst || bytes == 0) return cudaSuccess;
-    return cudaMemcpyAsync(dst, src, bytes, cudaMemcpyDeviceToHost, ctx->stream);
-  };
-  CK(d2h(surf_ind, r.ind_s.p, sizeof(int) * 3 * ns));
-  CK(d2h(corner_ind, r.ind_c.p, sizeof(int) * 2 * nc));
-  CK(d2h(surf_coeff, r.coeff_s.p, sizeof(float) * 4 * ns));
-  CK(d2h(corner_coeff, r.coeff_c.p, sizeof(float) * 4 * nc));
-  CK(d2h(surf_mask, r.mask_s.p, ns));
-  CK(d2h(corner_mask, r.mask_c.p, nc));
-  CK(d2h(surf_sel, r.sel_s.p, sizeof(float) * 3 * ns));
-  CK(d2h(corner_sel, r.sel_c.p, sizeof(float) * 3 * nc));
+  CK(d2h(ctx, surf_ind, r.ind_s.p, sizeof(int) * 3 * ns));
+  CK(d2h(ctx, corner_ind, r.ind_c.p, sizeof(int) * 2 * nc));
+  CK(d2h(ctx, surf_coeff, r.coeff_s.p, sizeof(float) * 4 * ns));
+  CK(d2h(ctx, corner_coeff, r.coeff_c.p, sizeof(float) * 4 * nc));
+  CK(d2h(ctx, surf_mask, r.mask_s.p, ns));
+  CK(d2h(ctx, corner_mask, r.mask_c.p, nc));
+  CK(d2h(ctx, surf_sel, r.sel_s.p, sizeof(float) * 3 * ns));
+  CK(d2h(ctx, corner_sel, r.sel_c.p, sizeof(float) * 3 * nc));
   CK(cudaStreamSynchronize(ctx->stream));
   return LINS_OK;
 }
@@ -706,31 +714,15 @@ int lins_gpu_batch_run(lins_ctx* ctx) {
 int lins_gpu_batch_download(lins_ctx* ctx, double* state_out, double* cov_out, lins_scan_result* results,
                             lins_report* reports) {
   if (!ctx) return LINS_E_INVALID;
-  Resident& r = ctx->batch;
-  if (r.n <= 0) return fail(ctx, LINS_E_INVALID, "no resident batch");
+  if (ctx->batch.n <= 0) return fail(ctx, LINS_E_INVALID, "no resident batch");
   CK(cudaSetDevice(ctx->device));
-  const size_t n = r.n;
-  if (state_out) { CK(r.h_state_out.reserve(n * 20)); CK(cudaMemcpyAsync(r.h_state_out.p, r.state_out.p, sizeof(double) * 20 * n, cudaMemcpyDeviceToHost, ctx->stream)); }
-  if (cov_out) { CK(r.h_cov_out.reserve(n * 324)); CK(cudaMemcpyAsync(r.h_cov_out.p, r.cov_out.p, sizeof(double) * 324 * n, cudaMemcpyDeviceToHost, ctx->stream)); }
-  if (results) { CK(r.h_results.reserve(n)); CK(cudaMemcpyAsync(r.h_results.p, r.results.p, sizeof(lins_scan_result) * n, cudaMemcpyDeviceToHost, ctx->stream)); }
-  if (reports) { CK(r.h_reports.reserve(n)); CK(cudaMemcpyAsync(r.h_reports.p, r.reports.p, sizeof(lins_report) * n, cudaMemcpyDeviceToHost, ctx->stream)); }
-  CK(cudaStreamSynchronize(ctx->stream));
-  if (state_out) for (size_t i = 0; i < n; ++i) std::memcpy(state_out + i * 19, r.h_state_out.p + i * 20, sizeof(double) * 19);
-  if (cov_out) std::memcpy(cov_out, r.h_cov_out.p, sizeof(double) * 324 * n);
-  if (results) std::memcpy(results, r.h_results.p, sizeof(lins_scan_result) * n);
-  if (reports) std::memcpy(reports, r.h_reports.p, sizeof(lins_report) * n);
-  return LINS_OK;
+  return download_outputs(ctx, ctx->batch, state_out, cov_out, results, reports);
 }
 
 int lins_gpu_batch_download_indices(lins_ctx* ctx, int32_t* surf_ind, int32_t* corner_ind) {
   if (!ctx) return LINS_E_INVALID;
-  Resident& r = ctx->batch;
-  if (r.n <= 0) return fail(ctx, LINS_E_INVALID, "no resident batch");
-  CK(cudaSetDevice(ctx->device));
-  if (surf_ind && r.nqs) CK(cudaMemcpyAsync(surf_ind, r.ind_s.p, sizeof(int32_t) * 3 * r.nqs, cudaMemcpyDeviceToHost, ctx->stream));
-  if (corner_ind && r.nqc) CK(cudaMemcpyAsync(corner_ind, r.ind_c.p, sizeof(int32_t) * 2 * r.nqc, cudaMemcpyDeviceToHost, ctx->stream));
-  CK(cudaStreamSynchronize(ctx->stream));
-  return LINS_OK;
+  if (ctx->batch.n <= 0) return fail(ctx, LINS_E_INVALID, "no resident batch");
+  return download_indices(ctx, ctx->batch, surf_ind, corner_ind);
 }
 
 int lins_gpu_ieskf_batch(lins_ctx* ctx, const lins_batch_desc* batch, double* state_out, double* cov_out,
@@ -820,10 +812,8 @@ int lins_gpu_estimate_transform(lins_ctx* ctx, const lins_point* surf_flat, int 
   CK(cudaSetDevice(ctx->device));
   // queries + initial pose are staged ONCE, then the loop runs on the device (icp_loop).  One D2H + one synchronisation
   // at the end.
-  double lin[19];
-  std::memset(lin, 0, sizeof(lin));
-  lin[0] = pose_io[0]; lin[1] = pose_io[1]; lin[2] = pose_io[2];
-  lin[6] = pose_io[3]; lin[7] = pose_io[4]; lin[8] = pose_io[5]; lin[9] = pose_io[6];
+  double lin[19] = {};
+  pose_to_state(pose_io, lin);
   int rc = stage_single(ctx, surf_flat, ns, corner_sharp, nc, lin, nullptr, false);
   if (rc != LINS_OK) return rc;
   Resident& r = ctx->single;
@@ -834,9 +824,7 @@ int lins_gpu_estimate_transform(lins_ctx* ctx, const lins_point* surf_flat, int 
   CK(cudaMemcpyAsync(r.h_state_out.p, r.state_in.p, sizeof(double) * 20, cudaMemcpyDeviceToHost, ctx->stream));
   CK(cudaMemcpyAsync(r.h_icp.p, r.icp.p, sizeof(IcpState), cudaMemcpyDeviceToHost, ctx->stream));
   CK(cudaStreamSynchronize(ctx->stream));
-  const double* so = r.h_state_out.p;
-  pose_io[0] = so[0]; pose_io[1] = so[1]; pose_io[2] = so[2];
-  pose_io[3] = so[6]; pose_io[4] = so[7]; pose_io[5] = so[8]; pose_io[6] = so[9];
+  state_to_pose(r.h_state_out.p, pose_io);
   if (iters_out) *iters_out = r.h_icp.p->iters;
   if (converged_out) *converged_out = r.h_icp.p->converged;
   return LINS_OK;
@@ -849,7 +837,8 @@ int lins_gpu_estimate_transform(lins_ctx* ctx, const lins_point* surf_flat, int 
 int lins_gpu_update_map_ex(lins_ctx* ctx, const lins_point* surf, int ns, const lins_point* corner, int nc, const double* lin_state,
                            lins_point* surf_out, lins_point* corner_out, int* map_replaced) {
   if (!ctx) return LINS_E_INVALID;
-  if (ns < 0 || nc < 0 || (ns > 0 && !surf) || (nc > 0 && !corner)) return fail(ctx, LINS_E_INVALID, "bad update_map args");
+  if (check_cloud(ctx, surf, ns, "bad update_map surf cloud") != LINS_OK || check_cloud(ctx, corner, nc, "bad update_map corner cloud") != LINS_OK)
+    return LINS_E_INVALID;
   CK(cudaSetDevice(ctx->device));
   const double* lin_dev = nullptr;
   if (!lin_state) {  // the posterior the last lins_gpu_ieskf left on the device (linState_ of a run that did not diverge)
@@ -874,8 +863,7 @@ int lins_gpu_update_map_ex(lins_ctx* ctx, const lins_point* surf, int ns, const 
   }
   if (lin_state) {
     double lin[20];
-    std::memcpy(lin, lin_state, sizeof(double) * 19);
-    lin[19] = 0;
+    pad_states(lin, lin_state, 1);
     CK(cudaMemcpyAsync(ctx->tmp_lin.p, lin, sizeof(lin), cudaMemcpyHostToDevice, ctx->stream));  // (pageable source: staged before the call returns)
     lin_dev = ctx->tmp_lin.p;
   }

@@ -128,7 +128,8 @@ int map_queue_pass(lins_ctx* ctx, int nc, int ns, bool dense, bool grid, const i
 }
 
 int map_stage_queries(lins_ctx* ctx, const lins_point* corner, int nc, const lins_point* surf, int ns) {
-  if (nc < 0 || ns < 0 || (nc > 0 && !corner) || (ns > 0 && !surf)) return fail(ctx, LINS_E_INVALID, "bad feature clouds");
+  if (check_cloud(ctx, corner, nc, "bad corner feature cloud") != LINS_OK || check_cloud(ctx, surf, ns, "bad surf feature cloud") != LINS_OK)
+    return LINS_E_INVALID;
   if (ctx->mp.n_map_c < 0) return fail(ctx, LINS_E_NOMAP, "lins_gpu_map_set has not been called");
   return upload2(ctx, ctx->mp.q_c, corner, nc, ctx->mp.q_s, surf, ns);
 }
@@ -201,7 +202,8 @@ extern "C" {
 
 int lins_gpu_map_set(lins_ctx* ctx, const lins_point* corner, int nc, const lins_point* surf, int ns) {
   if (!ctx) return LINS_E_INVALID;
-  if (nc < 0 || ns < 0 || (nc > 0 && !corner) || (ns > 0 && !surf)) return fail(ctx, LINS_E_INVALID, "bad map clouds");
+  if (check_cloud(ctx, corner, nc, "bad corner map cloud") != LINS_OK || check_cloud(ctx, surf, ns, "bad surf map cloud") != LINS_OK)
+    return LINS_E_INVALID;
   CK(cudaSetDevice(ctx->device));
   int rc = upload2(ctx, ctx->mp.map_c, corner, nc, ctx->mp.map_s, surf, ns);
   if (rc != LINS_OK) return rc;
@@ -252,12 +254,12 @@ int lins_gpu_map_associate(lins_ctx* ctx, const lins_point* corner, int nc, cons
   // the parity hook: brute force by default (exact neighbours for EVERY point, also those the 1 m gate rejects)
   rc = map_queue_pass(ctx, nc, ns, true, map_use_grid(false), nullptr, &nblocks);
   if (rc != LINS_OK) return rc;
-  if (cknn && nc) CK(cudaMemcpyAsync(cknn, m.knn_c.p, sizeof(int32_t) * 5 * (size_t)nc, cudaMemcpyDeviceToHost, ctx->stream));
-  if (sknn && ns) CK(cudaMemcpyAsync(sknn, m.knn_s.p, sizeof(int32_t) * 5 * (size_t)ns, cudaMemcpyDeviceToHost, ctx->stream));
-  if (ccoeff && nc) CK(cudaMemcpyAsync(ccoeff, m.coeff_c.p, sizeof(float) * 4 * (size_t)nc, cudaMemcpyDeviceToHost, ctx->stream));
-  if (scoeff && ns) CK(cudaMemcpyAsync(scoeff, m.coeff_s.p, sizeof(float) * 4 * (size_t)ns, cudaMemcpyDeviceToHost, ctx->stream));
-  if (cmask && nc) CK(cudaMemcpyAsync(cmask, m.mask_c.p, (size_t)nc, cudaMemcpyDeviceToHost, ctx->stream));
-  if (smask && ns) CK(cudaMemcpyAsync(smask, m.mask_s.p, (size_t)ns, cudaMemcpyDeviceToHost, ctx->stream));
+  CK(d2h(ctx, cknn, m.knn_c.p, sizeof(int32_t) * 5 * (size_t)nc));
+  CK(d2h(ctx, sknn, m.knn_s.p, sizeof(int32_t) * 5 * (size_t)ns));
+  CK(d2h(ctx, ccoeff, m.coeff_c.p, sizeof(float) * 4 * (size_t)nc));
+  CK(d2h(ctx, scoeff, m.coeff_s.p, sizeof(float) * 4 * (size_t)ns));
+  CK(d2h(ctx, cmask, m.mask_c.p, (size_t)nc));
+  CK(d2h(ctx, smask, m.mask_s.p, (size_t)ns));
   CK(cudaStreamSynchronize(ctx->stream));
   return LINS_OK;
 }

@@ -128,12 +128,6 @@ __global__ void __launch_bounds__(256) lins_mapper_transform_kernel(const float4
   out[i] = make_float4(c.cp * x2 + c.sp * z2 + c.tx, y2 + c.ty, -c.sp * x2 + c.cp * z2 + c.tz, p.w);
 }
 
-// one block per contiguous copy (the local map's concatenation, the surf-total concatenation)
-__global__ void lins_mapper_gather_kernel(const SeqCopy* __restrict__ copies) {
-  const SeqCopy c = copies[blockIdx.x];
-  for (int i = threadIdx.x; i < c.n; i += blockDim.x) c.dst[i] = c.src[i];
-}
-
 }  // namespace
 
 namespace lins_capi {
@@ -345,17 +339,11 @@ int upload3(lins_ctx* ctx, const lins_mapper_desc* d) {
   return LINS_OK;
 }
 
-// the copies go to entries base.. of the (reserved) staging and device lists: two batches of one cycle do not overlap
-int queue_copies(lins_ctx* ctx, const std::vector<SeqCopy>& copies, int base) {
-  MapperState& M = ctx->mapper;
-  int m = 0;
-  for (const SeqCopy& c : copies) if (c.n > 0) M.h_copies.p[base + m++] = c;
-  if (!m) return LINS_OK;
-  CK(cudaMemcpyAsync(M.copies.p + base, M.h_copies.p + base, sizeof(SeqCopy) * m, cudaMemcpyHostToDevice, ctx->stream));
-  lins_mapper_gather_kernel<<<m, 256, 0, ctx->stream>>>(M.copies.p + base);
-  CK(cudaGetLastError());
-  ctx->launches += 1;
-  return LINS_OK;
+// the non-empty copies of a batch through the gather list, at entries base.. (two batches of one cycle do not overlap)
+int queue_copies(lins_ctx* ctx, std::vector<DevCopy> v, int base) {
+  v.erase(std::remove_if(v.begin(), v.end(), [](const DevCopy& c) { return c.n <= 0; }), v.end());
+  const int rc = ctx->mapper.copies.stage(ctx, v.data(), (int)v.size(), base);
+  return rc != LINS_OK ? rc : ctx->mapper.copies.launch(ctx, base, (int)v.size());
 }
 
 // the slot of key frame id (a free one, or a new one)
@@ -401,9 +389,9 @@ int lins_gpu_mapper_imu(lins_ctx* ctx, const double* time, const double* roll, c
 int lins_gpu_mapper_step(lins_ctx* ctx, const lins_mapper_desc* d, lins_mapper_report* rep) {
   if (!ctx) return LINS_E_INVALID;
   if (!d) return fail(ctx, LINS_E_INVALID, "null desc");
-  if (d->n_corner < 0 || d->n_surf < 0 || d->n_outlier < 0 || (d->n_corner && !d->corner) || (d->n_surf && !d->surf) ||
-      (d->n_outlier && !d->outlier))
-    return fail(ctx, LINS_E_INVALID, "bad mapper clouds");
+  if (check_cloud(ctx, d->corner, d->n_corner, "bad mapper corner cloud") != LINS_OK || check_cloud(ctx, d->surf, d->n_surf, "bad mapper surf cloud") != LINS_OK ||
+      check_cloud(ctx, d->outlier, d->n_outlier, "bad mapper outlier cloud") != LINS_OK)
+    return LINS_E_INVALID;
   CK(cudaSetDevice(ctx->device));
   MapperState& M = ctx->mapper;
   lins_mapper_report r;
@@ -464,17 +452,17 @@ int lins_gpu_mapper_step(lins_ctx* ctx, const lins_mapper_desc* d, lins_mapper_r
   CK(M.ds[3].reserve((size_t)n_cat[2] + 1));
   CK(M.map_ds[0].reserve((size_t)n_cat[0] + 1)); CK(M.map_ds[1].reserve((size_t)n_cat[1] + 1));
   const size_t n_copies = 3 * s.window.size() + 2;
-  CK(M.h_copies.reserve(n_copies + 1)); CK(M.copies.reserve(n_copies + 1));
+  if ((rc = M.copies.reserve(ctx, n_copies)) != LINS_OK) return rc;
   VgInfo* info = M.vg_info.p;
   // the local map: corner_i ..., and surf_i, outlier_i interleaved (:1242-1246)
-  std::vector<SeqCopy> copies;
+  std::vector<DevCopy> copies;
   {
     int oc = 0, os = 0;
     for (int id : s.window) {
       const MapperKeyFrame& kf = M.slots[M.slot_of.at(id)];
-      copies.push_back(SeqCopy{kf.c[0].p, M.cat[0].p + oc, kf.n[0], 0}); oc += kf.n[0];
-      copies.push_back(SeqCopy{kf.c[1].p, M.cat[1].p + os, kf.n[1], 0}); os += kf.n[1];
-      copies.push_back(SeqCopy{kf.c[2].p, M.cat[1].p + os, kf.n[2], 0}); os += kf.n[2];
+      copies.push_back(DevCopy{kf.c[0].p, M.cat[0].p + oc, kf.n[0], 0}); oc += kf.n[0];
+      copies.push_back(DevCopy{kf.c[1].p, M.cat[1].p + os, kf.n[1], 0}); os += kf.n[1];
+      copies.push_back(DevCopy{kf.c[2].p, M.cat[1].p + os, kf.n[2], 0}); os += kf.n[2];
     }
   }
   if ((rc = queue_copies(ctx, copies, 0)) != LINS_OK) return rc;
@@ -487,7 +475,7 @@ int lins_gpu_mapper_step(lins_ctx* ctx, const lins_mapper_desc* d, lins_mapper_r
   for (int k = 0; k < 3; ++k)
     if ((rc = voxel_grid_queue(ctx, M.in[k].p, n_in[k], leaf[k], M.ds[k].p, info + 2 + k)) != LINS_OK) return rc;
   // laserCloudSurfTotalLast = surf DS + outlier DS: their NaN tails ride along and are dropped by the filter
-  copies.assign({SeqCopy{M.ds[1].p, M.cat[2].p, n_in[1], 0}, SeqCopy{M.ds[2].p, M.cat[2].p + n_in[1], n_in[2], 0}});
+  copies.assign({DevCopy{M.ds[1].p, M.cat[2].p, n_in[1], 0}, DevCopy{M.ds[2].p, M.cat[2].p + n_in[1], n_in[2], 0}});
   if ((rc = queue_copies(ctx, copies, (int)n_copies - 2)) != LINS_OK) return rc;
   if ((rc = voxel_grid_queue(ctx, M.cat[2].p, n_cat[2], 0.4f, M.ds[3].p, info + 5)) != LINS_OK) return rc;
 
@@ -609,19 +597,16 @@ int lins_gpu_mapper_download(lins_ctx* ctx, double* key_poses, int32_t* window, 
   if (window) { int i = 0; for (int id : M.s.window) window[i++] = id; }
   float* dst[6] = {map_corner_ds, map_surf_ds, corner_ds, surf_ds, outlier_ds, surf_total_ds};
   const float4* src[6] = {M.map_ds[0].p, M.map_ds[1].p, M.ds[0].p, M.ds[1].p, M.ds[2].p, M.ds[3].p};
-  bool any = false;
-  for (int k = 0; k < 6; ++k) {
-    if (!dst[k] || !M.last.valid || M.last.n[k] == 0) continue;
-    CK(cudaMemcpyAsync(dst[k], src[k], sizeof(float4) * M.last.n[k], cudaMemcpyDeviceToHost, ctx->stream));
-    any = true;
-  }
-  if (any) CK(cudaStreamSynchronize(ctx->stream));
+  for (int k = 0; k < 6 && M.last.valid; ++k) CK(d2h(ctx, dst[k], src[k], sizeof(float4) * M.last.n[k]));
+  CK(cudaStreamSynchronize(ctx->stream));
   return LINS_OK;
 }
 
 int lins_gpu_voxel_grid(lins_ctx* ctx, const lins_point* in, int n, float leaf, float* out, int* n_out) {
   if (!ctx) return LINS_E_INVALID;
-  if (n < 0 || (n > 0 && (!in || !out)) || !n_out || !(leaf > 0.f) || !std::isfinite(leaf)) return fail(ctx, LINS_E_INVALID, "bad VoxelGrid arguments");
+  if (check_cloud(ctx, in, n, "bad VoxelGrid input cloud") != LINS_OK || check_cloud(ctx, out, n, "bad VoxelGrid output cloud") != LINS_OK)
+    return LINS_E_INVALID;
+  if (!n_out || !(leaf > 0.f) || !std::isfinite(leaf)) return fail(ctx, LINS_E_INVALID, "bad VoxelGrid n_out / leaf");
   CK(cudaSetDevice(ctx->device));
   MapperState& M = ctx->mapper;
   CK(M.vg_info.reserve(kMapperGrids));
@@ -636,10 +621,8 @@ int lins_gpu_voxel_grid(lins_ctx* ctx, const lins_point* in, int n, float leaf, 
   CK(cudaStreamSynchronize(ctx->stream));
   if (M.h_vg_info.p[0].toobig) return fail(ctx, LINS_E_TOOBIG, "VoxelGrid: the leaf is too small for the cloud's extent (div_x * div_y * div_z > INT32_MAX)");
   const int c = n > 0 ? M.h_vg_info.p[0].count : 0;
-  if (c) {
-    CK(cudaMemcpyAsync(out, M.vg_out.p, sizeof(float4) * c, cudaMemcpyDeviceToHost, ctx->stream));
-    CK(cudaStreamSynchronize(ctx->stream));
-  }
+  CK(d2h(ctx, out, M.vg_out.p, sizeof(float4) * c));
+  CK(cudaStreamSynchronize(ctx->stream));
   *n_out = c;
   return LINS_OK;
 }

@@ -3,7 +3,7 @@
 //   predict x k (lins_seq_predict_kernel) -> processScan gate (host: it only reads cloud sizes) -> IESKF (the fused kernel,
 //   one launch) -> divergence check (one D2H) -> estimateTransform loop per diverged sequence (lins_gpu.cu: icp_loop) ->
 //   update / integrateTransformation / reset(1) / roll-pitch (lins_seq_post_kernel) -> transformToEnd (CSR kernel of
-//   lins_gpu.cu) + the guarded map swap (lins_seq_copy_kernel).
+//   lins_gpu.cu) + the guarded map swap (a gather list: lins_ctx.hpp CopyList).
 // Slots of a lins_gpu_seq_open run also initialise on the device (processPCL's status machine): the predict kernel
 //   pre-integrates a slot's IMU rows between its first and second scan, the second scans' estimateTransform runs as ONE
 //   batched icp_loop over all of them (lins_seq_icp_start_kernel sets its start poses), and lins_seq_init_kernel installs
@@ -148,11 +148,6 @@ __global__ void lins_seq_fresh_kernel(int n, const unsigned char* __restrict__ m
   lins_seq::fresh_slot(glob + (size_t)s * 20, filt + (size_t)s * 20, cov + (size_t)s * 324, k);
 }
 
-__global__ void lins_seq_copy_kernel(const SeqCopy* __restrict__ copies) {
-  const SeqCopy c = copies[blockIdx.x];
-  for (int i = threadIdx.x; i < c.n; i += blockDim.x) c.dst[i] = c.src[i];
-}
-
 lins_seq::Consts consts_of(const SeqState& q) {
   lins_seq::Consts k;
   std::memcpy(&k, q.consts, sizeof(k));
@@ -200,22 +195,6 @@ int launch_fresh(lins_ctx* ctx, SeqState& q, int n, const unsigned char* mask_de
   return LINS_OK;
 }
 
-int check_csr(lins_ctx* ctx, const int32_t* off, int n, const void* data, const char* what) {
-  if (!off) return fail(ctx, LINS_E_INVALID, what);
-  if (off[0] != 0) return fail(ctx, LINS_E_INVALID, what);
-  for (int i = 0; i < n; ++i) if (off[i + 1] < off[i]) return fail(ctx, LINS_E_INVALID, what);
-  if (off[n] > 0 && !data) return fail(ctx, LINS_E_INVALID, what);
-  return LINS_OK;
-}
-
-int run_copies(lins_ctx* ctx, const SeqCopy* dev, int count) {
-  if (count <= 0) return LINS_OK;
-  lins_seq_copy_kernel<<<count, 256, 0, ctx->stream>>>(dev);
-  CK(cudaGetLastError());
-  ctx->launches += 1;
-  return LINS_OK;
-}
-
 // ---- slot lifecycle ------------------------------------------------------------------------------------------------------
 // every per-slot buffer of a run of n slots; ns / nc: the surf / corner maps it starts with
 int reserve_run(lins_ctx* ctx, SeqState& q, int n, size_t ns, size_t nc) {
@@ -257,7 +236,7 @@ MapPiece current_piece(const SeqState& q, int c, int s) {
 
 // The next generation from next[4 * s + c], slot s's cloud c: fills h_nmap_off, reserves nmap_* / ntree_* and appends the
 // copies that fill them, in slot order, to `copies`
-int build_next_maps(lins_ctx* ctx, SeqState& q, const std::vector<MapPiece>& next, std::vector<SeqCopy>& copies) {
+int build_next_maps(lins_ctx* ctx, SeqState& q, const std::vector<MapPiece>& next, std::vector<DevCopy>& copies) {
   const int n = q.n, N1 = n + 1;
   q.h_nmap_off.assign(4 * (size_t)N1, 0);
   int* no = q.h_nmap_off.data();
@@ -269,7 +248,7 @@ int build_next_maps(lins_ctx* ctx, SeqState& q, const std::vector<MapPiece>& nex
   for (int s = 0; s < n; ++s)
     for (int c = 0; c < 4; ++c) {
       const MapPiece& p = next[4 * (size_t)s + c];
-      if (p.len) copies.push_back(SeqCopy{p.src, dst[c] + no[c * N1 + s], p.len, 0});
+      if (p.len) copies.push_back(DevCopy{p.src, dst[c] + no[c * N1 + s], p.len, 0});
     }
   return LINS_OK;
 }
@@ -302,7 +281,7 @@ int check_step(lins_ctx* ctx, const Desc* d, int n_scans, const double* scan_imu
 // Query compaction: the surf / corner queries of the step's clouds (q.up.qs / qc at offs[0] / offs[1]) of the slots whose
 // status is `code`, packed from off[0] / off[N1] on (set by the caller).  Fills the rest of off (2 x (n + 1)), appends
 // their copies to `copies` with each destination (cloud, offset) in `to`, and returns the largest per-slot total.
-int compact_queries(const SeqState& q, const int32_t* const offs[4], int32_t code, std::vector<int>& off, std::vector<SeqCopy>& copies,
+int compact_queries(const SeqState& q, const int32_t* const offs[4], int32_t code, std::vector<int>& off, std::vector<DevCopy>& copies,
                     std::vector<std::pair<int, int>>& to) {
   const int n = q.n, N1 = n + 1;
   int max_q = 0;
@@ -311,7 +290,7 @@ int compact_queries(const SeqState& q, const int32_t* const offs[4], int32_t cod
     const int nq[2] = {take ? offs[0][s + 1] - offs[0][s] : 0, take ? offs[1][s + 1] - offs[1][s] : 0};
     for (int c = 0; c < 2; ++c) {
       off[c * N1 + s + 1] = off[c * N1 + s] + nq[c];
-      if (nq[c]) { copies.push_back(SeqCopy{(c ? q.up.qc.p : q.up.qs.p) + offs[c][s], nullptr, nq[c], 0}); to.emplace_back(c, off[c * N1 + s]); }
+      if (nq[c]) { copies.push_back(DevCopy{(c ? q.up.qc.p : q.up.qs.p) + offs[c][s], nullptr, nq[c], 0}); to.emplace_back(c, off[c * N1 + s]); }
     }
     max_q = std::max(max_q, nq[0] + nq[1]);
   }
@@ -360,13 +339,15 @@ int seq_step_phases(lins_ctx* ctx, const lins_seq_step_desc* d, const int32_t* c
     }
   }
   // the IESKF's queries, then the second scans' after them in the compacted buffers, with offsets of their own (init_off):
-  // the IESKF launch sees no query of theirs, the estimateTransform loop none of the IESKF's
-  std::vector<SeqCopy> qcopies, mcopies;
+  // the IESKF launch sees no query of theirs, the estimateTransform loop none of the IESKF's.  One gather list: the
+  // query copies (the first n_qcopies), then the map refresh's.
+  std::vector<DevCopy> copies;
   std::vector<std::pair<int, int>> qto;  // destination of each query copy: (cloud, offset), resolved once the buffers exist
   std::vector<int> run_off(2 * (size_t)N1, 0), init_off(2 * (size_t)N1, 0);
-  const int max_q = compact_queries(q, offs, LINS_SEQ_RAN, run_off, qcopies, qto);
+  const int max_q = compact_queries(q, offs, LINS_SEQ_RAN, run_off, copies, qto);
   for (int c = 0; c < 2; ++c) init_off[c * N1] = run_off[c * N1 + N1 - 1];
-  const int max_init_q = compact_queries(q, offs, LINS_SEQ_SECOND, init_off, qcopies, qto);
+  const int max_init_q = compact_queries(q, offs, LINS_SEQ_SECOND, init_off, copies, qto);
+  const int n_qcopies = (int)copies.size();
 
   // ---- allocations ------------------------------------------------------------------------------------------------
   Resident& r = q.run;
@@ -378,32 +359,30 @@ int seq_step_phases(lins_ctx* ctx, const lins_seq_step_desc* d, const int32_t* c
   CK(r.h_off.reserve(4 * (size_t)N1));
   if (n_init) { CK(q.init_off.reserve(2 * (size_t)N1)); CK(q.scan_imu.reserve((size_t)n * 6)); CK(q.h_scan_imu.reserve((size_t)n * 6)); }
   // (pre and init_icp are lins_gpu_seq_open's: they keep their contents from step to step)
-  rc = build_next_maps(ctx, q, next, mcopies);
+  rc = build_next_maps(ctx, q, next, copies);
   if (rc != LINS_OK) return rc;
   const size_t n_imu = d->imu_off ? (size_t)d->imu_off[n] : 0;
   CK(q.imu.reserve(7 * n_imu + 1)); CK(q.imu_off.reserve(N1)); CK(q.h_imu.reserve(7 * n_imu + 1)); CK(q.h_imu_off.reserve(N1));
   CK(q.status_d.reserve(3 * (size_t)n)); CK(q.h_status.reserve(3 * (size_t)n));
-  const size_t n_copies = qcopies.size() + mcopies.size();
-  CK(q.copies.reserve(n_copies + 1)); CK(q.h_copies.reserve(n_copies + 1));
+  const int n_copies = (int)copies.size();
+  if ((rc = q.copies.reserve(ctx, n_copies)) != LINS_OK) return rc;
   CK(q.prior_state.reserve((size_t)n * 20)); CK(q.prior_cov.reserve((size_t)n * 324));
   CK(q.icp_ind_s.reserve(3 * r.nqs + 4)); CK(q.icp_ind_c.reserve(2 * r.nqc + 4));
   float4* qdst[2] = {r.qs.p, r.qc.p};
-  for (size_t i = 0; i < qcopies.size(); ++i) qcopies[i].dst = qdst[qto[i].first] + qto[i].second;
+  for (int i = 0; i < n_qcopies; ++i) copies[i].dst = qdst[qto[i].first] + qto[i].second;
 
   // ---- uploads: IMU, status, copy lists, compacted query offsets ---------------------------------------------------
   if (d->imu_off) std::memcpy(q.h_imu_off.p, d->imu_off, sizeof(int) * N1);
   else std::memset(q.h_imu_off.p, 0, sizeof(int) * N1);
   if (n_imu) std::memcpy(q.h_imu.p, d->imu, sizeof(double) * 7 * n_imu);
   for (int s = 0; s < n; ++s) { q.h_status.p[s] = (unsigned char)status[s]; q.h_status.p[2 * n + s] = imu_use[s]; }
-  std::copy(qcopies.begin(), qcopies.end(), q.h_copies.p);
-  std::copy(mcopies.begin(), mcopies.end(), q.h_copies.p + qcopies.size());
   std::memcpy(r.h_off.p, run_off.data(), sizeof(int) * 2 * N1);
   std::memcpy(r.h_off.p + 2 * N1, init_off.data(), sizeof(int) * 2 * N1);
   if (n_imu) CK(cudaMemcpyAsync(q.imu.p, q.h_imu.p, sizeof(double) * 7 * n_imu, cudaMemcpyHostToDevice, ctx->stream));
   CK(cudaMemcpyAsync(q.imu_off.p, q.h_imu_off.p, sizeof(int) * N1, cudaMemcpyHostToDevice, ctx->stream));
   CK(cudaMemcpyAsync(q.status_d.p, q.h_status.p, n, cudaMemcpyHostToDevice, ctx->stream));
   CK(cudaMemcpyAsync(q.status_d.p + 2 * n, q.h_status.p + 2 * n, n, cudaMemcpyHostToDevice, ctx->stream));
-  if (n_copies) CK(cudaMemcpyAsync(q.copies.p, q.h_copies.p, sizeof(SeqCopy) * n_copies, cudaMemcpyHostToDevice, ctx->stream));
+  if ((rc = q.copies.stage(ctx, copies.data(), n_copies, 0)) != LINS_OK) return rc;
   CK(cudaMemcpyAsync(r.qs_off.p, r.h_off.p, sizeof(int) * N1, cudaMemcpyHostToDevice, ctx->stream));
   CK(cudaMemcpyAsync(r.qc_off.p, r.h_off.p + N1, sizeof(int) * N1, cudaMemcpyHostToDevice, ctx->stream));
   if (n_init) {
@@ -438,8 +417,7 @@ int seq_step_phases(lins_ctx* ctx, const lins_seq_step_desc* d, const int32_t* c
   }
 
   // ---- 2. IESKF over every sequence; those that do not run have no queries ------------------------------------------
-  rc = run_copies(ctx, q.copies.p, (int)qcopies.size());
-  if (rc != LINS_OK) return rc;
+  if ((rc = q.copies.launch(ctx, 0, n_qcopies)) != LINS_OK) return rc;
   BatchView bv;
   std::memset(&bv, 0, sizeof(bv));
   bv.n_scans = n;
@@ -524,7 +502,7 @@ int seq_step_phases(lins_ctx* ctx, const lins_seq_step_desc* d, const int32_t* c
   CK(cudaMemcpyAsync(run_mask, q.h_status.p + n, n, cudaMemcpyHostToDevice, ctx->stream));
   rc = transform_to_end_csr(ctx, q.up.ts.p, q.up.ts_off.p, n, q.lin.p, run_mask);
   if (rc == LINS_OK) rc = transform_to_end_csr(ctx, q.up.tc.p, q.up.tc_off.p, n, q.lin.p, run_mask);
-  if (rc == LINS_OK) rc = run_copies(ctx, q.copies.p + qcopies.size(), (int)mcopies.size());
+  if (rc == LINS_OK) rc = q.copies.launch(ctx, n_qcopies, n_copies - n_qcopies);
   if (rc != LINS_OK) return rc;
   swap_maps(q);
   q.h_stale_v = new_stale;
@@ -572,19 +550,18 @@ int step_from_features(lins_ctx* ctx, const uint8_t* pres, const double* imu, co
   CK(r.h_off.reserve(4 * (size_t)N1));
   float4* dst[4] = {r.qs.p, r.qc.p, r.ts.p, r.tc.p};
   int* doff[4] = {r.qs_off.p, r.qc_off.p, r.ts_off.p, r.tc_off.p};
-  std::vector<SeqCopy> copies;
+  std::vector<DevCopy> copies;
   for (int k = 0; k < 4; ++k)
     for (int s = 0; s < n; ++s) {
       const int len = off[k * N1 + s + 1] - off[k * N1 + s];
-      if (len) copies.push_back(SeqCopy{f.out[k].p + src_off[s], dst[k] + off[k * N1 + s], len, 0});
+      if (len) copies.push_back(DevCopy{f.out[k].p + src_off[s], dst[k] + off[k * N1 + s], len, 0});
     }
-  CK(f.copies.reserve(copies.size() + 1)); CK(f.h_copies.reserve(copies.size() + 1));
-  std::copy(copies.begin(), copies.end(), f.h_copies.p);
-  std::memcpy(r.h_off.p, off.data(), sizeof(int) * off.size());
-  if (!copies.empty()) CK(cudaMemcpyAsync(f.copies.p, f.h_copies.p, sizeof(SeqCopy) * copies.size(), cudaMemcpyHostToDevice, ctx->stream));
-  for (int k = 0; k < 4; ++k) CK(cudaMemcpyAsync(doff[k], r.h_off.p + (size_t)k * N1, sizeof(int) * N1, cudaMemcpyHostToDevice, ctx->stream));
-  int rc = run_copies(ctx, f.copies.p, (int)copies.size());
+  int rc = f.copies.reserve(ctx, copies.size());
+  if (rc == LINS_OK) rc = f.copies.stage(ctx, copies.data(), (int)copies.size(), 0);
   if (rc != LINS_OK) return rc;
+  std::memcpy(r.h_off.p, off.data(), sizeof(int) * off.size());
+  for (int k = 0; k < 4; ++k) CK(cudaMemcpyAsync(doff[k], r.h_off.p + (size_t)k * N1, sizeof(int) * N1, cudaMemcpyHostToDevice, ctx->stream));
+  if ((rc = f.copies.launch(ctx, 0, (int)copies.size())) != LINS_OK) return rc;
   lins_seq_step_desc sd;
   std::memset(&sd, 0, sizeof(sd));
   sd.n_seq = n; sd.present = pres; sd.imu = imu; sd.imu_off = imu_off; sd.point_format = LINS_POINTS_XYZI32;
@@ -636,12 +613,10 @@ int lins_gpu_seq_begin(lins_ctx* ctx, const lins_seq_params* prm, const lins_seq
   if (rc != LINS_OK) return rc;
   if (ns) CK(cudaMemcpyAsync(q.map_s.p, q.up.ts.p, sizeof(float4) * ns, cudaMemcpyDeviceToDevice, ctx->stream));
   if (nc) CK(cudaMemcpyAsync(q.map_c.p, q.up.tc.p, sizeof(float4) * nc, cudaMemcpyDeviceToDevice, ctx->stream));
-  std::vector<double> st((size_t)n * 20, 0.0), gl((size_t)n * 20, 0.0), il((size_t)n * 8, 0.0);
-  for (int s = 0; s < n; ++s) {
-    std::memcpy(&st[(size_t)s * 20], d->filter_state + (size_t)s * 19, sizeof(double) * 19);
-    std::memcpy(&gl[(size_t)s * 20], d->global_state + (size_t)s * 19, sizeof(double) * 19);
-    std::memcpy(&il[(size_t)s * 8], d->imu_last + (size_t)s * 6, sizeof(double) * 6);
-  }
+  std::vector<double> st((size_t)n * 20), gl((size_t)n * 20), il((size_t)n * 8);
+  pad_states(st.data(), d->filter_state, n);
+  pad_states(gl.data(), d->global_state, n);
+  copy_rows(il.data(), 8, d->imu_last, 6, n);
   q.h_map_off.assign(4 * (size_t)(n + 1), 0);
   std::memcpy(&q.h_map_off[0], d->surf_map_off, sizeof(int) * (n + 1));
   std::memcpy(&q.h_map_off[n + 1], d->corner_map_off, sizeof(int) * (n + 1));
@@ -702,17 +677,16 @@ int lins_gpu_seq_restart(lins_ctx* ctx, const uint8_t* mask) {
   std::vector<MapPiece> next(4 * (size_t)n);
   for (int s = 0; s < n; ++s)
     if (!mask[s]) for (int c = 0; c < 4; ++c) next[4 * (size_t)s + c] = current_piece(q, c, s);
-  std::vector<SeqCopy> copies;
+  std::vector<DevCopy> copies;
   int rc = build_next_maps(ctx, q, next, copies);
+  if (rc == LINS_OK) rc = q.copies.reserve(ctx, copies.size());
   if (rc != LINS_OK) return rc;
-  CK(q.copies.reserve(copies.size() + 1)); CK(q.h_copies.reserve(copies.size() + 1));
   CK(q.status_d.reserve(3 * (size_t)n)); CK(q.h_status.reserve(3 * (size_t)n));
   // (the last step ended with a stream synchronisation: the pinned staging is free)
-  std::copy(copies.begin(), copies.end(), q.h_copies.p);
+  if ((rc = q.copies.stage(ctx, copies.data(), (int)copies.size(), 0)) != LINS_OK) return rc;
   for (int s = 0; s < n; ++s) q.h_status.p[s] = mask[s] ? 1 : 0;
-  if (!copies.empty()) CK(cudaMemcpyAsync(q.copies.p, q.h_copies.p, sizeof(SeqCopy) * copies.size(), cudaMemcpyHostToDevice, ctx->stream));
   CK(cudaMemcpyAsync(q.status_d.p, q.h_status.p, n, cudaMemcpyHostToDevice, ctx->stream));
-  rc = run_copies(ctx, q.copies.p, (int)copies.size());
+  rc = q.copies.launch(ctx, 0, (int)copies.size());
   if (rc == LINS_OK) rc = launch_fresh(ctx, q, n, q.status_d.p);
   if (rc != LINS_OK) { q.n = 0; return rc; }  // (some slots may have changed: the run ends, as after a failed step)
   swap_maps(q);
@@ -729,9 +703,8 @@ int lins_gpu_seq_step_ex(lins_ctx* ctx, const lins_seq_step_desc* d, const doubl
   const int n = ctx->seq.n;
   const int32_t* offs[4] = {d->surf_flat_off, d->corner_sharp_off, d->surf_less_flat_off, d->corner_less_sharp_off};
   const lins_point* pts[4] = {d->surf_flat, d->corner_sharp, d->surf_less_flat, d->corner_less_sharp};
-  for (int k = 0; k < 4; ++k) { rc = check_csr(ctx, offs[k], n, pts[k], "bad cloud offsets / cloud"); if (rc != LINS_OK) return rc; }
   CK(cudaSetDevice(ctx->device));
-  rc = upload_clouds(ctx, ctx->seq.up, n, pts, offs, d->point_format);  // (validates the rest; synchronises the stream first)
+  rc = upload_clouds(ctx, ctx->seq.up, n, pts, offs, d->point_format);  // (validates the clouds; synchronises the stream first)
   if (rc != LINS_OK) return rc;
   return seq_step_run(ctx, d, offs, scan_imu);
 }
@@ -810,14 +783,12 @@ int lins_gpu_seq_download(lins_ctx* ctx, double* global_state, double* filter_st
   std::vector<double> g(global_state ? n * 20 : 0), f(filter_state ? n * 20 : 0);
   if (global_state) CK(cudaMemcpyAsync(g.data(), q.glob.p, sizeof(double) * 20 * n, cudaMemcpyDeviceToHost, ctx->stream));
   if (filter_state) CK(cudaMemcpyAsync(f.data(), q.filt.p, sizeof(double) * 20 * n, cudaMemcpyDeviceToHost, ctx->stream));
-  if (filter_cov) CK(cudaMemcpyAsync(filter_cov, q.cov.p, sizeof(double) * 324 * n, cudaMemcpyDeviceToHost, ctx->stream));
-  if (results) CK(cudaMemcpyAsync(results, r.results.p, sizeof(lins_scan_result) * n, cudaMemcpyDeviceToHost, ctx->stream));
-  if (reports) CK(cudaMemcpyAsync(reports, r.reports.p, sizeof(lins_report) * n, cudaMemcpyDeviceToHost, ctx->stream));
+  CK(d2h(ctx, filter_cov, q.cov.p, sizeof(double) * 324 * n));
+  CK(d2h(ctx, results, r.results.p, sizeof(lins_scan_result) * n));
+  CK(d2h(ctx, reports, r.reports.p, sizeof(lins_report) * n));
   CK(cudaStreamSynchronize(ctx->stream));
-  for (size_t s = 0; s < n; ++s) {
-    if (global_state) std::memcpy(global_state + s * 19, &g[s * 20], sizeof(double) * 19);
-    if (filter_state) std::memcpy(filter_state + s * 19, &f[s * 20], sizeof(double) * 19);
-  }
+  if (global_state) strip_states(global_state, g.data(), n);
+  if (filter_state) strip_states(filter_state, f.data(), n);
   if (scan_status) std::memcpy(scan_status, q.status.data(), sizeof(int32_t) * n);
   return LINS_OK;
 }
@@ -843,8 +814,7 @@ int lins_gpu_seq_download_init(lins_ctx* ctx, int32_t* fusion_status, double* ic
   CK(cudaStreamSynchronize(ctx->stream));
   for (size_t s = 0; s < n; ++s) {
     if (q.status[s] != LINS_SEQ_SECOND) continue;
-    const double* p = &pose[s * 20];
-    if (icp_pose) { double* o = icp_pose + s * 7; o[0] = p[0]; o[1] = p[1]; o[2] = p[2]; o[3] = p[6]; o[4] = p[7]; o[5] = p[8]; o[6] = p[9]; }
+    if (icp_pose) state_to_pose(&pose[s * 20], icp_pose + s * 7);
     if (icp_iters) icp_iters[s] = st[s].iters;
     if (icp_converged) icp_converged[s] = st[s].converged;
   }
@@ -866,16 +836,14 @@ int lins_gpu_seq_download_ieskf(lins_ctx* ctx, double* prior_state, double* prio
   if (!ran && (state_out || cov_out)) return fail(ctx, LINS_E_INVALID, "no sequence ran an IESKF in the last step");
   std::vector<double> a(prior_state ? n * 20 : 0), b(state_out ? n * 20 : 0);
   if (prior_state) CK(cudaMemcpyAsync(a.data(), q.prior_state.p, sizeof(double) * 20 * n, cudaMemcpyDeviceToHost, ctx->stream));
-  if (prior_cov) CK(cudaMemcpyAsync(prior_cov, q.prior_cov.p, sizeof(double) * 324 * n, cudaMemcpyDeviceToHost, ctx->stream));
+  CK(d2h(ctx, prior_cov, q.prior_cov.p, sizeof(double) * 324 * n));
   if (state_out) CK(cudaMemcpyAsync(b.data(), r.state_out.p, sizeof(double) * 20 * n, cudaMemcpyDeviceToHost, ctx->stream));
-  if (cov_out) CK(cudaMemcpyAsync(cov_out, r.cov_out.p, sizeof(double) * 324 * n, cudaMemcpyDeviceToHost, ctx->stream));
-  if (surf_ind && ro[N1 - 1]) CK(cudaMemcpyAsync(surf_ind, r.ind_s.p, sizeof(int32_t) * 3 * ro[N1 - 1], cudaMemcpyDeviceToHost, ctx->stream));
-  if (corner_ind && ro[2 * N1 - 1]) CK(cudaMemcpyAsync(corner_ind, r.ind_c.p, sizeof(int32_t) * 2 * ro[2 * N1 - 1], cudaMemcpyDeviceToHost, ctx->stream));
+  CK(d2h(ctx, cov_out, r.cov_out.p, sizeof(double) * 324 * n));
+  CK(d2h(ctx, surf_ind, r.ind_s.p, sizeof(int32_t) * 3 * ro[N1 - 1]));
+  CK(d2h(ctx, corner_ind, r.ind_c.p, sizeof(int32_t) * 2 * ro[2 * N1 - 1]));
   CK(cudaStreamSynchronize(ctx->stream));
-  for (size_t s = 0; s < n; ++s) {
-    if (prior_state) std::memcpy(prior_state + s * 19, &a[s * 20], sizeof(double) * 19);
-    if (state_out) std::memcpy(state_out + s * 19, &b[s * 20], sizeof(double) * 19);
-  }
+  if (prior_state) strip_states(prior_state, a.data(), n);
+  if (state_out) strip_states(state_out, b.data(), n);
   if (query_off) std::memcpy(query_off, ro, sizeof(int32_t) * 2 * N1);
   return LINS_OK;
 }
@@ -890,8 +858,7 @@ int lins_gpu_seq_download_maps(lins_ctx* ctx, int32_t* off, float* surf_map, flo
   const int* mo = q.h_map_off.data();
   float* dst[4] = {surf_map, corner_map, surf_tree, corner_tree};
   const float4* src[4] = {q.map_s.p, q.map_c.p, q.tree_s.p, q.tree_c.p};
-  for (int c = 0; c < 4; ++c)
-    if (dst[c] && mo[c * N1 + N1 - 1]) CK(cudaMemcpyAsync(dst[c], src[c], sizeof(float4) * mo[c * N1 + N1 - 1], cudaMemcpyDeviceToHost, ctx->stream));
+  for (int c = 0; c < 4; ++c) CK(d2h(ctx, dst[c], src[c], sizeof(float4) * mo[c * N1 + N1 - 1]));
   CK(cudaStreamSynchronize(ctx->stream));
   if (off) std::memcpy(off, mo, sizeof(int32_t) * 4 * N1);
   if (stale) std::memcpy(stale, q.h_stale_v.data(), q.n);

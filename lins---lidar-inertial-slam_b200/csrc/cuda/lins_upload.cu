@@ -1,6 +1,7 @@
 // lins_upload.cu — lins_gpu_batch_upload: the four clouds, offsets and priors of a batch from host memory into the
 // context's resident batch (lins_ctx.hpp: Resident), packing 32-B PointXYZI records into 16-B (x, y, z, intensity)
-// records on host threads or, for clouds in pinned host memory, on the device.
+// records on host threads or, for clouds in pinned host memory, on the device.  Also the gather lists' staging and copy
+// kernel (lins_ctx.hpp: CopyList).
 #include <cuda_runtime.h>
 
 #include <algorithm>
@@ -27,21 +28,41 @@ __global__ void lins_pack_points_kernel(const float4* __restrict__ raw, float4* 
   }
 }
 
+// one block per record of a gather list (lins_ctx.hpp: CopyList)
+__global__ void lins_copy_kernel(const DevCopy* __restrict__ copies) {
+  const DevCopy c = copies[blockIdx.x];
+  for (int i = threadIdx.x; i < c.n; i += blockDim.x) c.dst[i] = c.src[i];
+}
+
 }  // namespace
 
 namespace lins_capi {
 
+int CopyList::reserve(lins_ctx* ctx, size_t n) { CK(dev.reserve(n + 1)); CK(host.reserve(n + 1)); return LINS_OK; }
+
+int CopyList::stage(lins_ctx* ctx, const DevCopy* src, int n, int base) {
+  if (n <= 0) return LINS_OK;
+  std::copy(src, src + n, host.p + base);
+  CK(cudaMemcpyAsync(dev.p + base, host.p + base, sizeof(DevCopy) * n, cudaMemcpyHostToDevice, ctx->stream));
+  return LINS_OK;
+}
+
+int CopyList::launch(lins_ctx* ctx, int base, int n) {
+  if (n <= 0) return LINS_OK;
+  lins_copy_kernel<<<n, 256, 0, ctx->stream>>>(dev.p + base);
+  CK(cudaGetLastError());
+  ctx->launches += 1;
+  return LINS_OK;
+}
+
 int upload_clouds(lins_ctx* ctx, Resident& r, int n, const lins_point* const pts[4], const int32_t* const offs[4], int point_format) {
   CK(cudaStreamSynchronize(ctx->stream));  // the pinned staging of a previous upload may still be in flight
-  r.n = n;
-  if (n == 0) return LINS_OK;
-  for (int k = 0; k < 4; ++k) {
-    if (!offs[k]) return fail(ctx, LINS_E_INVALID, "null offsets");
-    if (offs[k][0] != 0) return fail(ctx, LINS_E_INVALID, "offsets must start at 0");
-    for (int i = 0; i < n; ++i) if (offs[k][i + 1] < offs[k][i]) return fail(ctx, LINS_E_INVALID, "offsets must be non-decreasing");
-    if (offs[k][n] > 0 && !pts[k]) return fail(ctx, LINS_E_INVALID, "null cloud");
-  }
+  if (n == 0) { r.n = 0; return LINS_OK; }
+  static const char* const what[4] = {"bad surf_flat (or raw sweep) offsets / cloud", "bad corner_sharp offsets / cloud",
+                                      "bad surf_less_flat offsets / cloud", "bad corner_less_sharp offsets / cloud"};
+  for (int k = 0; k < 4; ++k) { const int rc = check_csr(ctx, offs[k], n, pts[k], what[k]); if (rc != LINS_OK) return rc; }
   if (point_format != LINS_POINTS_XYZI32 && point_format != LINS_POINTS_PACKED16) return fail(ctx, LINS_E_INVALID, "bad point_format");
+  r.n = n;
   const bool packed16 = point_format == LINS_POINTS_PACKED16;  // the clouds are already (x, y, z, intensity) float4 records
   r.nqs = offs[0][n]; r.nqc = offs[1][n]; r.nts = offs[2][n]; r.ntc = offs[3][n];
   r.max_q = 0;
@@ -222,10 +243,7 @@ int lins_gpu_batch_upload(lins_ctx* ctx, const lins_batch_desc* b) {
   if (rc != LINS_OK || n == 0) return rc;
   CK(r.h_state.reserve((size_t)n * 20)); CK(r.h_cov.reserve((size_t)n * 324));
   CK(r.state_in.reserve((size_t)n * 20)); CK(r.cov_in.reserve((size_t)n * 324));
-  for (int i = 0; i < n; ++i) {
-    std::memcpy(r.h_state.p + (size_t)i * 20, b->state_in + (size_t)i * 19, sizeof(double) * 19);
-    r.h_state.p[(size_t)i * 20 + 19] = 0.0;
-  }
+  pad_states(r.h_state.p, b->state_in, n);
   std::memcpy(r.h_cov.p, b->cov_in, sizeof(double) * 324 * (size_t)n);
   CK(cudaMemcpyAsync(r.state_in.p, r.h_state.p, sizeof(double) * 20 * (size_t)n, cudaMemcpyHostToDevice, ctx->stream));
   CK(cudaMemcpyAsync(r.cov_in.p, r.h_cov.p, sizeof(double) * 324 * (size_t)n, cudaMemcpyHostToDevice, ctx->stream));

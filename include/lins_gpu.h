@@ -567,7 +567,7 @@ int lins_gpu_map_associate(lins_ctx* ctx, const lins_point* corner_last, int n_c
                            uint8_t* corner_mask, uint8_t* surf_mask);
 
 /* ---- the mapping node's cycle: lidar_mapping_node.cpp run() :1806-1855 behind one call per mapping cycle ------------
-   One mapper per context.  Per processed cycle: transformAssociateToMap (:411-536), extractSurroundingKeyFrames in the
+   One mapper per context (lins_gpu_mappers_* below run many in lockstep).  Per processed cycle: transformAssociateToMap (:411-536), extractSurroundingKeyFrames in the
    branch the reference compiles (loopClosureEnableFlag = true, parameters.h:80: the window of the 50 most recent key
    frames, :1204-1246), the local map's pcl::VoxelGrid (corner 0.2 m, surf + outlier 0.4 m, :1317-1323),
    downsampleCurrentScan (:1326-1349), scan2MapOptimization with its 10 / 100 gate and transformUpdate (:1635-1652,
@@ -628,6 +628,42 @@ int lins_gpu_mapper_download(lins_ctx* ctx, double* key_poses, int32_t* window, 
 /* pcl::VoxelGrid<PointXYZI> on one cloud of n points (leaf > 0): the filter the mapper runs, as a call of its own.  out
    has room for n records (x, y, z, intensity floats); *n_out receives the voxel count.  LINS_E_TOOBIG as above. */
 int lins_gpu_voxel_grid(lins_ctx* ctx, const lins_point* in, int n, float leaf, float* out, int* n_out);
+
+/* ---- the mapping node's cycle for many drives in lockstep ----------------------------------------------------------
+   M mapper slots on one context, each a mapping node of its own (one drive's), stepped together: one call runs the
+   lins_gpu_mapper_step cycle of every present slot with one device-to-host synchronisation, whatever M is.  Per present
+   slot, the report, the key poses, the window and the six clouds are bit-identical to lins_gpu_mapper_step /
+   lins_gpu_mapper_download on a context of its own given the same event sequence (the interval gate, the 10 / 100 gate
+   with its stale transformAftMapped, and the duplicated key frame when the window first fills included).  The slots'
+   state is a member of the context of its own: lins_gpu_mapper_*, lins_gpu_map_set, lins_gpu_scan2map and
+   lins_gpu_voxel_grid on the same context neither see nor change it.  Loop closure is not performed, as in the single
+   mapper.  A call before lins_gpu_mappers_open returns LINS_E_NOMAP. */
+/* opens M mapper slots, each a freshly constructed mapping node (as after lins_gpu_mapper_reset); replaces any open run */
+int lins_gpu_mappers_open(lins_ctx* ctx, int32_t n_slots);
+/* slots with mask[s] != 0 back to the fresh state (hand a slot to a new drive); others untouched */
+int lins_gpu_mappers_reset(lins_ctx* ctx, const uint8_t* mask /*M*/);
+/* imuHandler for every slot: slot s's rows are [off[s], off[s+1]) of time / roll / pitch (as lins_gpu_mapper_imu) */
+int lins_gpu_mappers_imu(lins_ctx* ctx, const int32_t* off /*M+1*/, const double* time, const double* roll, const double* pitch);
+typedef struct lins_mappers_desc {
+  int32_t n_slots;                       /* == M */
+  int32_t pad;
+  const uint8_t* present;                /* M flags; NULL = all.  An absent slot is neither read nor changed */
+  const double* time;                    /* M: timeLaserOdometry */
+  const double* quat;                    /* M x 4 (x, y, z, w) */
+  const double* pos;                     /* M x 3 */
+  const lins_point* corner;  const int32_t* corner_off;   /* M + 1, CSR as lins_batch_desc: slot s's cloud is */
+  const lins_point* surf;    const int32_t* surf_off;     /* [off[s], off[s+1]) (an absent slot's range is ignored) */
+  const lins_point* outlier; const int32_t* outlier_off;
+} lins_mappers_desc;
+/* lins_gpu_mapper_step for every present slot; reps[s] written for present slots only (reps may be NULL).
+   LINS_E_INVALID before anything changes for a bad descriptor (n_slots != M, null time / quat / pos, bad offsets, a
+   NULL cloud with points).  LINS_E_TOOBIG when any slot's VoxelGrid overflows: then no slot's state changes (transforms,
+   key frames, windows, IMU queues), and lins_gpu_mappers_download returns no clouds for the slots the step processed
+   until their next completed cycle. */
+int lins_gpu_mappers_step(lins_ctx* ctx, const lins_mappers_desc* d, lins_mapper_report* reps /*M or NULL*/);
+/* lins_gpu_mapper_download of one slot */
+int lins_gpu_mappers_download(lins_ctx* ctx, int32_t slot, double* key_poses, int32_t* window, float* map_corner_ds,
+                              float* map_surf_ds, float* corner_ds, float* surf_ds, float* outlier_ds, float* surf_total_ds);
 
 /* block until everything queued on the ctx stream has finished */
 int lins_gpu_sync(lins_ctx* ctx);

@@ -13,7 +13,7 @@ import subprocess
 
 import numpy as np
 
-from .ctypes_defs import (Batch, COV_SIZE, LinsBatchDesc, LinsCloud2Desc, LinsCloud2Layout, LinsFeatureParams, LinsLidarModel, LinsLidarModels, LinsMapperDesc, LinsMapperReport, LinsMapReport, LinsParams, LinsPclDesc,
+from .ctypes_defs import (Batch, COV_SIZE, LinsBatchDesc, LinsCloud2Desc, LinsCloud2Layout, LinsFeatureParams, LinsLidarModel, LinsLidarModels, LinsMapperDesc, LinsMapperReport, LinsMappersDesc, LinsMapReport, LinsParams, LinsPclDesc,
                           LinsRawDesc, LinsReport, LinsScanResult, LinsSeqBeginDesc, LinsSeqInitParams, LinsSeqParams, LinsSeqPclDesc,
                           LinsSeqCloud2Desc, LinsSeqRawDesc, LinsSeqStepDesc, POINT_DTYPE, SCAN_RESULT_DTYPE, STATE_DIM, as_points, make_points, ptr)
 
@@ -37,17 +37,19 @@ EXPORTS = [
     "lins_gpu_seq_step_raw", "lins_gpu_decode_cloud2", "lins_gpu_decode_ms", "lins_gpu_seq_step_cloud2",
     "lins_gpu_project_scans_mixed", "lins_gpu_seq_step_raw_mixed", "lins_gpu_seq_step_cloud2_mixed",
     "lins_gpu_mapper_reset", "lins_gpu_mapper_imu", "lins_gpu_mapper_step", "lins_gpu_mapper_download", "lins_gpu_voxel_grid",
+    "lins_gpu_mappers_open", "lins_gpu_mappers_reset", "lins_gpu_mappers_imu", "lins_gpu_mappers_step", "lins_gpu_mappers_download",
 ]
 
 NVCC_ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]  # H100 (Hopper)
 NVCC_COMMON = NVCC_ARCH + ["-lineinfo", "-O3", "-std=c++17", "-Xcompiler", "-fPIC"]
 # translation units and their extra flags: lins_gpu.cu (the fused kernel and most of the C-ABI), lins_upload.cu (batch
 # upload), lins_map.cu (row F2's host side), lins_seq.cu (sequence mode), lins_features.cu (feature extraction),
-# lins_projection.cu (image projection), lins_cloud2.cu (PointCloud2 decoding), lins_mapper.cu (the mapping node's cycle) — all bit-exact, so no multiply-add contraction: the association and the map
+# lins_projection.cu (image projection), lins_cloud2.cu (PointCloud2 decoding), lins_mapper.cu (the mapping node's cycle), lins_mappers.cu (many mapping nodes in lockstep) — all bit-exact, so no multiply-add contraction: the association and the map
 # fits depend on it — and lins_jacobian.cu (the tolerance-checked split Jacobian kernel: contraction allowed)
 UNITS = [("lins_gpu.cu", ["-fmad=false"]), ("lins_upload.cu", ["-fmad=false"]), ("lins_map.cu", ["-fmad=false"]),
          ("lins_seq.cu", ["-fmad=false"]), ("lins_features.cu", ["-fmad=false"]), ("lins_projection.cu", ["-fmad=false"]),
-         ("lins_cloud2.cu", ["-fmad=false"]), ("lins_mapper.cu", ["-fmad=false"]), ("lins_jacobian.cu", [])]
+         ("lins_cloud2.cu", ["-fmad=false"]), ("lins_mapper.cu", ["-fmad=false"]), ("lins_mappers.cu", ["-fmad=false"]),
+         ("lins_jacobian.cu", [])]
 
 
 def build(force=False, verbose=False):
@@ -136,6 +138,11 @@ def lib():
         L.lins_gpu_mapper_step.argtypes = [vp, C.POINTER(LinsMapperDesc), C.POINTER(LinsMapperReport)]
         L.lins_gpu_mapper_download.argtypes = [vp] + [vp] * 8
         L.lins_gpu_voxel_grid.argtypes = [vp, vp, C.c_int, C.c_float, vp, C.POINTER(C.c_int)]
+        L.lins_gpu_mappers_open.argtypes = [vp, C.c_int32]
+        L.lins_gpu_mappers_reset.argtypes = [vp, vp]
+        L.lins_gpu_mappers_imu.argtypes = [vp, vp, vp, vp, vp]
+        L.lins_gpu_mappers_step.argtypes = [vp, C.POINTER(LinsMappersDesc), vp]
+        L.lins_gpu_mappers_download.argtypes = [vp, C.c_int32] + [vp] * 8
         _LIB = L
     return _LIB
 
@@ -180,6 +187,17 @@ def unpin_arrays(arrays):
 def unpin_batch(batch):
     unpin_arrays(getattr(batch, "_pinned", []))
     batch._pinned = []
+
+
+def pack_csr(clouds):
+    """Per-slot clouds (point arrays, or None for none) -> (one POINT_DTYPE array, int32 offsets of len(clouds) + 1):
+    slot s's points are [off[s], off[s + 1])."""
+    parts = [as_points(c) if c is not None else np.zeros(0, POINT_DTYPE) for c in clouds]
+    off = np.zeros(len(parts) + 1, np.int32)
+    off[1:] = np.cumsum([len(p) for p in parts])
+    # (joined as plain float32 rows: numpy concatenates structured records far more slowly)
+    pts = np.concatenate([p.view(np.float32).reshape(-1, 8) for p in parts]).view(POINT_DTYPE).reshape(-1) if parts else np.zeros(0, POINT_DTYPE)
+    return pts, off
 
 
 class LinsGpu:
@@ -347,6 +365,50 @@ class LinsGpu:
         n = C.c_int(0)
         self._ck(self.L.lins_gpu_voxel_grid(self.h, ptr(p), len(p), float(leaf), ptr(out), C.byref(n)))
         return out[:n.value].copy()
+
+    # ---- many mapping nodes in lockstep (lins_gpu_mappers_*) ------------------------------------------------------
+    def mappers_open(self, n_slots):
+        self._ck(self.L.lins_gpu_mappers_open(self.h, int(n_slots)))
+        self._mappers_n = int(n_slots)
+
+    def mappers_reset(self, mask):
+        m = np.ascontiguousarray(mask, np.uint8).reshape(-1)
+        assert len(m) == self._mappers_n
+        self._ck(self.L.lins_gpu_mappers_reset(self.h, ptr(m)))
+
+    def mappers_imu(self, rows):
+        """imuHandler per slot: rows[s] = (times, rolls, pitches) of slot s (None or empty: no message)."""
+        per = [[np.atleast_1d(np.asarray(a, np.float64)) for a in (r if r is not None else ((), (), ()))] for r in rows]
+        off = np.zeros(len(per) + 1, np.int32)
+        off[1:] = np.cumsum([len(t) for t, _, _ in per])
+        t, r, p = (np.ascontiguousarray(np.concatenate([x[k] for x in per]) if per else np.zeros(0)) for k in range(3))
+        self._ck(self.L.lins_gpu_mappers_imu(self.h, ptr(off), ptr(t), ptr(r), ptr(p)))
+
+    def mappers_step(self, steps):
+        """One lockstep step: steps[s] = (time, quat_xyzw, pos, corner, surf, outlier) of slot s, or None for an absent
+        slot.  Returns the list of LinsMapperReport (None for absent slots)."""
+        M = len(steps)
+        present = np.array([st is not None for st in steps], np.uint8)
+        time = np.array([float(st[0]) if st is not None else 0.0 for st in steps], np.float64)
+        quat = np.array([[float(v) for v in st[1]] if st is not None else [0.0, 0.0, 0.0, 1.0] for st in steps], np.float64).reshape(M, 4)
+        pos = np.array([[float(v) for v in st[2]] if st is not None else [0.0] * 3 for st in steps], np.float64).reshape(M, 3)
+        clouds = [pack_csr([st[3 + k] if st is not None else None for st in steps]) for k in range(3)]
+        d = LinsMappersDesc(n_slots=M, present=ptr(present), time=ptr(time), quat=ptr(quat), pos=ptr(pos),
+                            corner=ptr(clouds[0][0]), corner_off=ptr(clouds[0][1]), surf=ptr(clouds[1][0]), surf_off=ptr(clouds[1][1]),
+                            outlier=ptr(clouds[2][0]), outlier_off=ptr(clouds[2][1]))
+        reps = (LinsMapperReport * M)()
+        self._ck(self.L.lins_gpu_mappers_step(self.h, C.byref(d), C.cast(reps, C.c_void_p)))
+        return [reps[s] if present[s] else None for s in range(M)]
+
+    def mappers_download(self, slot, rep):
+        """mapper_download of one slot: (key poses, window, clouds) with the sizes its last processed cycle's report gives."""
+        poses = np.zeros((rep.n_keyframes, 7))
+        window = np.zeros(rep.window_len, np.int32)
+        names = ("map_corner_ds", "map_surf_ds", "corner_ds", "surf_ds", "outlier_ds", "surf_total_ds")
+        sizes = (rep.n_map_corner_ds, rep.n_map_surf_ds, rep.n_corner_ds, rep.n_surf_ds, rep.n_outlier_ds, rep.n_surf_total_ds)
+        clouds = {k: np.zeros((n, 4), np.float32) for k, n in zip(names, sizes)}
+        self._ck(self.L.lins_gpu_mappers_download(self.h, int(slot), ptr(poses), ptr(window), *[ptr(clouds[k]) for k in names]))
+        return poses, window, clouds
 
     # ---- batched mode ------------------------------------------------------------------------------------------
     def batch_upload(self, batch):

@@ -1,7 +1,7 @@
 // lins_ctx.hpp — host state of a C-ABI context (struct lins_ctx of include/lins_gpu.h) and the helpers the translation units
 // that implement the C-ABI share: lins_gpu.cu (fused kernel, single-scan and batched entry points, F1), lins_upload.cu
-// (batch upload, gather lists), lins_map.cu (row F2), lins_seq.cu (sequence mode), lins_mapper.cu (the mapping node) and
-// the front-end units.  Host code only: a header that defines kernels cannot be included here, because every unit that
+// (batch upload, gather lists), lins_map.cu (row F2), lins_seq.cu (sequence mode), lins_mapper.cu (the mapping node),
+// lins_mappers.cu (mapping nodes in lockstep) and the front-end units.  Host code only: a header that defines kernels cannot be included here, because every unit that
 // includes this one would define them again.
 #pragma once
 #include <cuda_runtime.h>
@@ -10,6 +10,7 @@
 #endif
 
 #include <algorithm>
+#include <array>
 #include <cstddef>
 #include <cstdint>
 #include <deque>
@@ -22,7 +23,7 @@
 #include "../host/host_pool.hpp"
 
 namespace lins_dev { struct IcpState; struct BatchView; }     // lins_kernels.cuh
-namespace lins_map { struct PassConsts; struct MapLoopState; }  // lins_map.cuh
+namespace lins_map { struct PassConsts; struct MapLoopState; struct MapSlot; }  // lins_map.cuh
 
 namespace lins_capi {
 
@@ -48,6 +49,9 @@ struct Buf {
     if (e == cudaSuccess) cap = want;
     return e;
   }
+  // reserve with a quarter of headroom when it has to grow: buffers whose sizes drift from call to call (a key frame's
+  // clouds, the lockstep mappers' per-slot clouds) settle after a few calls instead of reallocating on most of them
+  cudaError_t grow(size_t n) { return n <= cap ? cudaSuccess : reserve(n + n / 4); }
 
  private:
   void deallocate() {
@@ -270,22 +274,59 @@ struct MapperScalars {
   std::deque<int> window;  // recent*CloudKeyFrames as key-frame ids, oldest first
 };
 struct MapperLast { bool valid = false; int n[6] = {0, 0, 0, 0, 0, 0}; };  // the last processed cycle's DS sizes
-struct MapperState {
+// one mapping node's host state: its scalars, its key poses, the key-frame store (the window and the newest key frame,
+// each key frame's DS clouds in the map frame) and the sizes of its last processed cycle's clouds
+struct MapperNode {
   MapperScalars s;
   std::vector<MapperKeyPose> poses;          // cloudKeyPoses6D
-  std::vector<MapperKeyFrame> slots;         // the key-frame store: the window and the newest key frame
+  std::vector<MapperKeyFrame> slots;         // the key-frame store
   std::unordered_map<int, int> slot_of;      // key-frame id -> slot
   std::vector<int> free_slots;
   MapperLast last;
+};
+// the scratch of segmented VoxelGrids (lins_mapper.cu): 32-bit keys for one segment, (segment, key) 64-bit keys for more
+struct VgScratch {
+  Buf<unsigned> key[2];
+  Buf<unsigned long long> key64[2];
+  Buf<int> idx[2], head, vid;
+  Buf<unsigned char> temp;                   // CUB scratch
+};
+struct MapperState {
+  MapperNode n;
   Buf<float4> in[3], ds[4], cat[3], map_ds[2];  // scan clouds, their DS (corner, surf, outlier, surf total), concatenations
   Buf<float4> vg_in, vg_out;                 // lins_gpu_voxel_grid
   Buf<float4, kPinned> h_in;
-  Buf<unsigned> key[2];
-  Buf<int> idx[2], head, vid;
-  Buf<unsigned char> temp;                   // CUB scratch
+  VgScratch vg;
   Buf<VgInfo> vg_info;
   Buf<VgInfo, kPinned> h_vg_info, h_vg_init;
+  Buf<unsigned char> tf; Buf<unsigned char, kPinned> h_tf;  // the key frame's transform job
   CopyList copies;                           // the local map's concatenation, then the surf-total one
+};
+// Lockstep mappers (lins_gpu_mappers_*, lins_mappers.cu): one MapperNode per slot with its six DS clouds of the last
+// processed cycle (map corner, map surf, corner, surf, outlier, surf total), and the step's shared device buffers
+struct MappersState {
+  int n = 0;                                 // slots (0 = lins_gpu_mappers_open has not run)
+  std::vector<MapperNode> node;
+  std::vector<std::array<Buf<float4>, 6>> ds;
+  Buf<lins_map::MapLoopState> loop;          // per slot: the scan-to-map loop state (matP / isDegenerate persist)
+  Buf<lins_map::MapLoopState, kPinned> h_loop;
+  Buf<lins_map::PassConsts> consts;          // per slot
+  Buf<lins_map::PassConsts, kPinned> h_consts;
+  Buf<lins_map::MapSlot> mslot;              // per slot: the step's scan-to-map view
+  Buf<lins_map::MapSlot, kPinned> h_mslot;
+  Buf<int> blk_slot; Buf<int, kPinned> h_blk_slot;  // per fit block: its slot
+  Buf<float4> vin[2];                        // the VoxelGrids' inputs: round 1 (maps and scans), round 2 (surf total)
+  Buf<float4, kPinned> h_in;
+  VgScratch vg;
+  Buf<VgInfo> vg_info; Buf<VgInfo, kPinned> h_vg_info, h_vg_init;
+  Buf<int> vg_off; Buf<int, kPinned> h_vg_off;      // per round: S + 1 segment offsets
+  Buf<float4*> vg_out; Buf<float4*, kPinned> h_vg_out;  // per round: S output clouds
+  Buf<int> grid_start, grid_count, grid_cursor;      // every slot's corner and surf buckets
+  Buf<float4> grid_sorted;
+  Buf<unsigned char> scan_temp;              // CUB scratch of the buckets' scan
+  Buf<float> part_d; Buf<int> part_i; Buf<double> partial;
+  Buf<unsigned char> tf; Buf<unsigned char, kPinned> h_tf;  // the key frames' transform jobs
+  CopyList copies;                           // the local maps' concatenation, then the surf-total one
 };
 
 }  // namespace lins_capi
@@ -347,6 +388,7 @@ struct lins_ctx {
     Buf<uint8_t> mask_c, mask_s;
   } mp;
   lins_capi::MapperState mapper;  // lins_gpu_mapper_*, lins_gpu_voxel_grid
+  lins_capi::MappersState mappers;  // lins_gpu_mappers_*
 };
 
 namespace lins_capi {
@@ -537,10 +579,42 @@ int cloud2_run(lins_ctx* ctx, const lins_cloud2_desc* d, const uint8_t* present,
 void map_grid_origin(const lins_point* host_pts, int n, float origin[3]);
 int map_build_grid(lins_ctx* ctx, lins_ctx::MapState::Grid& g, const float4* map, int n, const float origin[3], const int* n_dev = nullptr);
 int map_queue_loop(lins_ctx* ctx, int nc, int ns, const float* T, const int* gate_nc = nullptr, const int* gate_ns = nullptr);
-void map_loop_report(const lins_ctx* ctx, float* T, lins_map_report* rep);
+void map_loop_report(const lins_map::MapLoopState& st, float* T, lins_map_report* rep);
 int map_reset_loop(lins_ctx* ctx);
-// lins_mapper.cu: queue pcl::VoxelGrid of n device points into out (room for n) with its record at info (device)
-int voxel_grid_queue(lins_ctx* ctx, const float4* in, int n, float leaf, float4* out, VgInfo* info);
-int voxel_grid_reserve(lins_ctx* ctx, int n);
+// lins_map.cu: the scan-to-map loops of many slots in one queue (lins_gpu_mappers_step).  ms.h_mslot (pinned, n_slots)
+// holds each slot's map and query clouds, capacities, device map counts, start transform and run flag; the rest of the
+// table is filled here.  Queued: every slot's two grids in one bucket array (one count, one CUB scan, one scatter), the
+// start / gate kernel (a slot with run = 0 starts done), and LINS_MAP_MAX_ITER passes of one 5-NN and one fit launch per
+// kind over all slots and one LM launch with a warp per slot; then the loop states' D2H into ms.h_loop.  Nothing is
+// synchronised; ms.loop (n_slots) keeps each slot's matP / isDegenerate.
+int map_queue_slots(lins_ctx* ctx, MappersState& ms, int n_slots);
+// lins_mapper.cu: queue pcl::VoxelGrid of n_seg segments of the device points `in` (segment k: [h_off[k], h_off[k + 1]),
+// leaf[k]) into outputs with room for each segment's points (out for one segment; else the device table d_out, with
+// d_off the device copy of h_off), the records at info (device, n_seg; their initial values staged through h_init, pinned,
+// n_seg records).  The counts and flags are read back by the caller.  voxel_grid_reserve: the scratch for n points in
+// n_seg segments (grow-only; call before queuing work that a growth could free under).
+int voxel_grid_queue(lins_ctx* ctx, VgScratch& w, const float4* in, int n_seg, const int* h_off, const int* d_off, const float* leaf,
+                     float4* out, float4* const* d_out, VgInfo* h_init, VgInfo* info);
+int voxel_grid_reserve(lins_ctx* ctx, VgScratch& w, int n, int n_seg);
+// lins_mapper.cu: the mapping node's host logic, one copy for lins_gpu_mapper_* and lins_gpu_mappers_*.
+// mapper_node_reset: a freshly constructed node (the store's buffers are kept for reuse); mapper_node_imu: imuHandler.
+// mapper_cycle_begin: laserOdometryHandler into s (a copy of m.s, committed by the caller) and, unless the 0.3 s gate
+// skips the cycle (false; r reports it), transformAssociateToMap and the window; window_sizes: the local map's corner and
+// surf + outlier point counts.  mapper_cycle_end, after the read-back of the DS counts cnt (map corner, map surf, corner,
+// surf, outlier, surf total) and of the loop state st (null: no key frames, or the 10 / 100 gate failed): transformUpdate,
+// saveKeyFramesAndFactor and the loop candidate; commits s into m and fills r.  A saved key frame is left in *save for
+// keyframes_queue, which transforms every listed key frame's DS clouds into its store slot in one launch.
+struct KfSave { MapperKeyFrame* kf; MapperKeyPose kp; const float4* ds[3]; };
+void mapper_node_reset(MapperNode& m);
+void mapper_node_imu(MapperScalars& s, const double* time, const double* roll, const double* pitch, int n);
+bool mapper_cycle_begin(const MapperNode& m, MapperScalars& s, double time, const double quat[4], const double pos[3], lins_mapper_report& r);
+void mapper_window_sizes(const MapperNode& m, const MapperScalars& s, int& n_corner, int& n_surf);
+void mapper_cycle_end(MapperNode& m, MapperScalars& s, double time, double scan_period, const int cnt[6], const lins_map::MapLoopState* st,
+                      lins_mapper_report& r, KfSave* save, bool* saved);
+int keyframes_queue(lins_ctx* ctx, const KfSave* saves, int n, Buf<unsigned char>& dev, Buf<unsigned char, kPinned>& host);
+// lins_mapper.cu: a node's key poses, window and last cycle's clouds (src: its six DS clouds on the device; NULL skips)
+int mapper_node_download(lins_ctx* ctx, const MapperNode& m, const float4* const src[6], double* key_poses, int32_t* window, float* const dst[6]);
+// lins_mapper.cu: the non-empty copies of v through the gather list l, staged at entries base.. and run in one launch
+int queue_copies(lins_ctx* ctx, CopyList& l, std::vector<DevCopy> v, int base);
 
 }  // namespace lins_capi

@@ -1,6 +1,7 @@
 // lins_map.cu — host side of row F2 (SURVEY.md §8(f)): the mapping node's scan-to-map refinement, whose kernels are in
 // lins_map.cuh.
 #include <cuda_runtime.h>
+#include <cub/device/device_scan.cuh>
 
 #include <algorithm>
 #include <cmath>
@@ -66,9 +67,9 @@ int map_build_grid(lins_ctx* ctx, lins_ctx::MapState::Grid& g, const float4* map
   for (int k = 0; k < 3; ++k) g.origin[k] = origin[k];
   const GridIndex gi = grid_index(g);
   CK(cudaMemsetAsync(g.count.p, 0, sizeof(int) * nb, ctx->stream));
-  lins_grid_count_kernel<<<(n + 255) / 256, 256, 0, ctx->stream>>>(map, n, n_dev, gi, g.count.p);
+  lins_grid_count_kernel<<<(n + 255) / 256, 256, 0, ctx->stream>>>(map, n, n_dev, gi, g.count.p, nullptr, 0);
   lins_grid_scan_kernel<<<1, 1024, 0, ctx->stream>>>(g.count.p, g.start.p, g.cursor.p, (int)nb);
-  lins_grid_scatter_kernel<<<(n + 255) / 256, 256, 0, ctx->stream>>>(map, n, n_dev, gi, g.cursor.p, g.sorted.p);
+  lins_grid_scatter_kernel<<<(n + 255) / 256, 256, 0, ctx->stream>>>(map, n, n_dev, gi, g.cursor.p, g.sorted.p, nullptr, 0);
   CK(cudaGetLastError());
   ctx->launches += 3;
   return LINS_OK;
@@ -80,7 +81,7 @@ namespace {
 
 // queue one cornerOptimization + surfOptimization pass (5-NN, fits, block partials) that reads its constants from
 // m.consts (device); nothing is synchronised.  Returns the number of partial blocks.
-int map_queue_pass(lins_ctx* ctx, int nc, int ns, bool dense, bool grid, const int* done, int* nblocks_out) {
+int map_queue_pass(lins_ctx* ctx, int nc, int ns, bool dense, bool grid, const lins_map::MapLoopState* st, int* nblocks_out) {
   using namespace lins_map;
   lins_ctx::MapState& m = ctx->mp;
   const int qb[2] = {(nc + kKnnThreads - 1) / kKnnThreads, (ns + kKnnThreads - 1) / kKnnThreads};
@@ -110,16 +111,16 @@ int map_queue_pass(lins_ctx* ctx, int nc, int ns, bool dense, bool grid, const i
   for (int k = 0; k < 2; ++k) {
     if (nq[k] == 0) continue;
     if (grid && nm[k] > 0)
-      lins_map_knn_grid_kernel<<<(nq[k] + kGridKnnWarps - 1) / kGridKnnWarps, kGridKnnWarps * 32, 0, ctx->stream>>>(q[k], nq[k], grid_index(*gr[k]), m.consts.p, done, m.part_d.p, m.part_i.p);
+      lins_map_knn_grid_kernel<<<(nq[k] + kGridKnnWarps - 1) / kGridKnnWarps, kGridKnnWarps * 32, 0, ctx->stream>>>(q[k], nq[k], grid_index(*gr[k]), m.consts.p, st, m.part_d.p, m.part_i.p, nullptr, nullptr, k);
     else
-      lins_map_knn_kernel<<<dim3(qb[k], slices[k]), kKnnThreads, 0, ctx->stream>>>(q[k], nq[k], mp[k], nm[k], slice_len[k], m.consts.p, done, m.part_d.p, m.part_i.p);
+      lins_map_knn_kernel<<<dim3(qb[k], slices[k]), kKnnThreads, 0, ctx->stream>>>(q[k], nq[k], mp[k], nm[k], slice_len[k], m.consts.p, st, m.part_d.p, m.part_i.p);
     double* partial = m.partial.p + (size_t)(k == 0 ? 0 : qb[0]) * (kRowAcc + 1);
     if (k == 0)
-      lins_map_fit_kernel<true><<<qb[k], kFitThreads, 0, ctx->stream>>>(q[k], nq[k], mp[k], slices[k], m.part_d.p, m.part_i.p, m.consts.p, done, dense ? m.knn_c.p : nullptr,
-                                                                       dense ? m.coeff_c.p : nullptr, dense ? m.mask_c.p : nullptr, partial);
+      lins_map_fit_kernel<true><<<qb[k], kFitThreads, 0, ctx->stream>>>(q[k], nq[k], mp[k], slices[k], m.part_d.p, m.part_i.p, m.consts.p, st, dense ? m.knn_c.p : nullptr,
+                                                                       dense ? m.coeff_c.p : nullptr, dense ? m.mask_c.p : nullptr, partial, nullptr, nullptr);
     else
-      lins_map_fit_kernel<false><<<qb[k], kFitThreads, 0, ctx->stream>>>(q[k], nq[k], mp[k], slices[k], m.part_d.p, m.part_i.p, m.consts.p, done, dense ? m.knn_s.p : nullptr,
-                                                                        dense ? m.coeff_s.p : nullptr, dense ? m.mask_s.p : nullptr, partial);
+      lins_map_fit_kernel<false><<<qb[k], kFitThreads, 0, ctx->stream>>>(q[k], nq[k], mp[k], slices[k], m.part_d.p, m.part_i.p, m.consts.p, st, dense ? m.knn_s.p : nullptr,
+                                                                        dense ? m.coeff_s.p : nullptr, dense ? m.mask_s.p : nullptr, partial, nullptr, nullptr);
     CK(cudaGetLastError());
     ctx->launches += 2;
   }
@@ -136,9 +137,23 @@ int map_stage_queries(lins_ctx* ctx, const lins_point* corner, int nc, const lin
 
 }  // namespace
 
-// scan2MapOptimization's gate (:1636) on device-resident map sizes: a failing map marks the loop done before its first pass
-__global__ void lins_map_gate_kernel(const int* __restrict__ nc, const int* __restrict__ ns, lins_map::MapLoopState* __restrict__ st) {
-  if (!(*nc > 10 && *ns > 100)) st->done = 1;
+// scan2MapOptimization's gate (:1636) on device-resident map sizes: a failing map marks the loop done before its first
+// pass.  Many slots (sl non-null, n of them): slot s's loop state first takes its start transform and a cleared report
+// (matP / isDegenerate persist), and a slot without a map (run = 0) starts done.
+__global__ void lins_map_gate_kernel(const int* __restrict__ nc, const int* __restrict__ ns, lins_map::MapLoopState* __restrict__ st,
+                                     const lins_map::MapSlot* __restrict__ sl, int n) {
+  const int s = blockIdx.x * blockDim.x + threadIdx.x;
+  if (s >= n) return;
+  if (sl) {
+    const lins_map::MapSlot& v = sl[s];
+    lins_map::MapLoopState& m = st[s];
+    for (int i = 0; i < 6; ++i) m.T[i] = v.T[i];
+    m.done = m.iters = m.converged = 0;
+    for (int i = 0; i < LINS_MAP_MAX_ITER; ++i) { m.n_sel[i] = 0; m.delta_r[i] = 0.f; m.delta_t[i] = 0.f; }
+    if (!v.run) { m.done = 1; return; }
+    nc = v.n_map[0]; ns = v.n_map[1];
+  }
+  if (!(*nc > 10 && *ns > 100)) st[s].done = 1;
 }
 
 namespace lins_capi {
@@ -161,20 +176,96 @@ int map_queue_loop(lins_ctx* ctx, int nc, int ns, const float* T, const int* gat
   CK(cudaMemsetAsync(reinterpret_cast<char*>(m.loop.p) + offsetof(MapLoopState, done), 0, sizeof(MapLoopState) - offsetof(MapLoopState, done), ctx->stream));
   CK(cudaMemcpyAsync(m.consts.p, &pc0, sizeof(pc0), cudaMemcpyHostToDevice, ctx->stream));
   if (gate_nc) {
-    lins_map_gate_kernel<<<1, 1, 0, ctx->stream>>>(gate_nc, gate_ns, m.loop.p);
+    lins_map_gate_kernel<<<1, 1, 0, ctx->stream>>>(gate_nc, gate_ns, m.loop.p, nullptr, 1);
     CK(cudaGetLastError());
     ctx->launches += 1;
   }
   const bool grid = map_use_grid(true);
   for (int iter = 0; iter < LINS_MAP_MAX_ITER; ++iter) {
     int nblocks = 0;
-    const int rc = map_queue_pass(ctx, nc, ns, false, grid, &m.loop.p->done, &nblocks);
+    const int rc = map_queue_pass(ctx, nc, ns, false, grid, m.loop.p, &nblocks);
     if (rc != LINS_OK) return rc;
-    lins_map_lm_kernel<<<1, 32, 0, ctx->stream>>>(m.partial.p, nblocks, iter, m.loop.p, m.consts.p);
+    lins_map_lm_kernel<<<1, 32, 0, ctx->stream>>>(m.partial.p, nblocks, iter, m.loop.p, m.consts.p, nullptr);
     CK(cudaGetLastError());
     ctx->launches += 1;
   }
   CK(cudaMemcpyAsync(m.h_loop.p, m.loop.p, sizeof(MapLoopState), cudaMemcpyDeviceToHost, ctx->stream));
+  return LINS_OK;
+}
+
+int map_queue_slots(lins_ctx* ctx, MappersState& ms, int n_slots) {
+  using namespace lins_map;
+  MapSlot* h = ms.h_mslot.p;
+  // per slot: map_build_grid's bucket rule for each map, fit blocks that start with the slot's queries
+  int nb_tot = 0, pts = 0, blocks[2] = {0, 0};
+  std::vector<int> blk_slot[2];
+  for (int s = 0; s < n_slots; ++s) {
+    MapSlot& v = h[s];
+    for (int k = 0; k < 2; ++k) {
+      unsigned nb = v.run ? 4096 : 1;  // (a slot that does not run searches nothing)
+      while (v.run && nb < 2u * (unsigned)v.cap[k] && nb < (1u << 24)) nb <<= 1;
+      v.g[k].mask = nb - 1; v.g[k].ox = v.g[k].oy = v.g[k].oz = 0.f;  // (any finite origin gives the same 5-NN)
+      v.bucket0[k] = nb_tot; nb_tot += (int)nb;
+      v.m0[k] = pts; pts += v.cap[k];
+      v.blk[k] = blocks[k];
+      v.nblk[k] = v.run ? (v.nq[k] + kFitThreads - 1) / kFitThreads : 0;
+      blocks[k] += v.nblk[k];
+      blk_slot[k].insert(blk_slot[k].end(), v.nblk[k], s);
+    }
+  }
+  size_t scan_bytes = 0;
+  CK(cub::DeviceScan::ExclusiveSum(nullptr, scan_bytes, ms.grid_count.p, ms.grid_start.p, nb_tot + 1, ctx->stream));
+  CK(ms.scan_temp.grow(scan_bytes + 16));
+  CK(ms.grid_start.grow((size_t)nb_tot + 2)); CK(ms.grid_count.grow((size_t)nb_tot + 2)); CK(ms.grid_cursor.grow((size_t)nb_tot + 2));
+  CK(ms.grid_sorted.grow((size_t)pts + 1));
+  const size_t rows = (size_t)std::max(blocks[0], blocks[1]) * kFitThreads;
+  CK(ms.part_d.grow(5 * rows + 1)); CK(ms.part_i.grow(5 * rows + 1));
+  CK(ms.partial.grow((size_t)(blocks[0] + blocks[1] + 1) * (kRowAcc + 1)));
+  CK(ms.blk_slot.grow((size_t)blocks[0] + blocks[1] + 1)); CK(ms.h_blk_slot.grow((size_t)blocks[0] + blocks[1] + 1));
+  CK(ms.consts.grow(n_slots)); CK(ms.h_consts.grow(n_slots)); CK(ms.mslot.grow(n_slots));
+  for (int s = 0; s < n_slots; ++s) {
+    for (int k = 0; k < 2; ++k) { h[s].g[k].pts = ms.grid_sorted.p; h[s].g[k].start = ms.grid_start.p + h[s].bucket0[k]; }
+    ms.h_consts.p[s] = host_pass_consts(h[s].T);
+  }
+  std::copy(blk_slot[0].begin(), blk_slot[0].end(), ms.h_blk_slot.p);
+  std::copy(blk_slot[1].begin(), blk_slot[1].end(), ms.h_blk_slot.p + blocks[0]);
+  CK(cudaMemcpyAsync(ms.mslot.p, h, sizeof(MapSlot) * n_slots, cudaMemcpyHostToDevice, ctx->stream));
+  CK(cudaMemcpyAsync(ms.consts.p, ms.h_consts.p, sizeof(PassConsts) * n_slots, cudaMemcpyHostToDevice, ctx->stream));
+  if (blocks[0] + blocks[1])
+    CK(cudaMemcpyAsync(ms.blk_slot.p, ms.h_blk_slot.p, sizeof(int) * (blocks[0] + blocks[1]), cudaMemcpyHostToDevice, ctx->stream));
+  // every slot's two grids: one count, one scan of all buckets, one scatter
+  CK(cudaMemsetAsync(ms.grid_count.p, 0, sizeof(int) * ((size_t)nb_tot + 1), ctx->stream));
+  const GridIndex g0{};
+  if (pts) lins_grid_count_kernel<<<(pts + 255) / 256, 256, 0, ctx->stream>>>(nullptr, pts, nullptr, g0, ms.grid_count.p, ms.mslot.p, n_slots);
+  size_t bytes = ms.scan_temp.cap;
+  CK(cub::DeviceScan::ExclusiveSum(ms.scan_temp.p, bytes, ms.grid_count.p, ms.grid_start.p, nb_tot + 1, ctx->stream));
+  CK(cudaMemcpyAsync(ms.grid_cursor.p, ms.grid_start.p, sizeof(int) * nb_tot, cudaMemcpyDeviceToDevice, ctx->stream));
+  if (pts) lins_grid_scatter_kernel<<<(pts + 255) / 256, 256, 0, ctx->stream>>>(nullptr, pts, nullptr, g0, ms.grid_cursor.p, ms.grid_sorted.p, ms.mslot.p, n_slots);
+  lins_map_gate_kernel<<<(n_slots + 127) / 128, 128, 0, ctx->stream>>>(nullptr, nullptr, ms.loop.p, ms.mslot.p, n_slots);
+  CK(cudaGetLastError());
+  ctx->launches += pts ? 4 : 2;
+  // the loop: per pass one 5-NN and one fit launch per kind over every slot, one LM launch of a warp per slot
+  double* partial_s = ms.partial.p + (size_t)blocks[0] * (kRowAcc + 1);
+  for (int iter = 0; iter < LINS_MAP_MAX_ITER; ++iter) {
+    if (blocks[0]) {
+      lins_map_knn_grid_kernel<<<blocks[0] * kFitThreads / kGridKnnWarps, kGridKnnWarps * 32, 0, ctx->stream>>>(
+          nullptr, blocks[0] * kFitThreads, g0, ms.consts.p, ms.loop.p, ms.part_d.p, ms.part_i.p, ms.mslot.p, ms.blk_slot.p, 0);
+      lins_map_fit_kernel<true><<<blocks[0], kFitThreads, 0, ctx->stream>>>(nullptr, 0, nullptr, 1, ms.part_d.p, ms.part_i.p, ms.consts.p, ms.loop.p,
+                                                                            nullptr, nullptr, nullptr, ms.partial.p, ms.mslot.p, ms.blk_slot.p);
+      ctx->launches += 2;
+    }
+    if (blocks[1]) {
+      lins_map_knn_grid_kernel<<<blocks[1] * kFitThreads / kGridKnnWarps, kGridKnnWarps * 32, 0, ctx->stream>>>(
+          nullptr, blocks[1] * kFitThreads, g0, ms.consts.p, ms.loop.p, ms.part_d.p, ms.part_i.p, ms.mslot.p, ms.blk_slot.p + blocks[0], 1);
+      lins_map_fit_kernel<false><<<blocks[1], kFitThreads, 0, ctx->stream>>>(nullptr, 0, nullptr, 1, ms.part_d.p, ms.part_i.p, ms.consts.p, ms.loop.p,
+                                                                             nullptr, nullptr, nullptr, partial_s, ms.mslot.p, ms.blk_slot.p + blocks[0]);
+      ctx->launches += 2;
+    }
+    lins_map_lm_kernel<<<n_slots, 32, 0, ctx->stream>>>(ms.partial.p, blocks[0], iter, ms.loop.p, ms.consts.p, ms.mslot.p);
+    CK(cudaGetLastError());
+    ctx->launches += 1;
+  }
+  CK(cudaMemcpyAsync(ms.h_loop.p, ms.loop.p, sizeof(MapLoopState) * n_slots, cudaMemcpyDeviceToHost, ctx->stream));
   return LINS_OK;
 }
 
@@ -183,9 +274,8 @@ int map_reset_loop(lins_ctx* ctx) {
   return LINS_OK;
 }
 
-// the report of the loop whose state mp.h_loop holds
-void map_loop_report(const lins_ctx* ctx, float* T, lins_map_report* rep) {
-  const lins_map::MapLoopState& st = *ctx->mp.h_loop.p;
+// the report of the loop whose state st holds
+void map_loop_report(const lins_map::MapLoopState& st, float* T, lins_map_report* rep) {
   lins_map_report r;
   std::memset(&r, 0, sizeof(r));
   for (int i = 0; i < 6; ++i) T[i] = st.T[i];
@@ -234,7 +324,7 @@ int lins_gpu_scan2map(lins_ctx* ctx, const lins_point* corner, int nc, const lin
   rc = map_queue_loop(ctx, nc, ns, T);
   if (rc != LINS_OK) return rc;
   CK(cudaStreamSynchronize(ctx->stream));
-  map_loop_report(ctx, T, &r);
+  map_loop_report(*m.h_loop.p, T, &r);
   if (rep) *rep = r;
   return LINS_OK;
 }

@@ -20,6 +20,7 @@
 #include <stdint.h>
 
 #include "../host/lins_cv_small.hpp"
+#include "lins_map_types.cuh"
 
 namespace lins_map {
 
@@ -27,11 +28,6 @@ constexpr int kKnnThreads = 128;
 constexpr int kTile = 2048;      // map points per shared-memory tile (32 KB)
 constexpr int kFitThreads = 128;
 constexpr int kRowAcc = 27;      // 21 (upper triangle of A^T A) + 6 (A^T B)
-
-struct PassConsts {
-  float cRoll, sRoll, cPitch, sPitch, cYaw, sYaw, tX, tY, tZ;  // updatePointAssociateToMapSinCos :579-592
-  float srx, crx, sry, cry, srz, crz;                          // LMOptimization :1527-1532
-};
 
 __device__ __forceinline__ float3 associate_to_map(const float4 pi, const PassConsts& c) {  // :594-608
   const float x1 = c.cYaw * pi.x - c.sYaw * pi.y;
@@ -63,9 +59,9 @@ struct Top5 {
 
 // grid (query blocks, slices).  part_d / part_i: [n_q][n_slices][5]
 __global__ void __launch_bounds__(kKnnThreads) lins_map_knn_kernel(const float4* __restrict__ q, int n_q, const float4* __restrict__ map, int n_map,
-                                                                   int slice_len, const PassConsts* __restrict__ pcp, const int* __restrict__ done,
+                                                                   int slice_len, const PassConsts* __restrict__ pcp, const MapLoopState* __restrict__ st,
                                                                    float* __restrict__ part_d, int* __restrict__ part_i) {
-  if (done && *done) return;  // (the queued tail of a converged scan2map loop)
+  if (st && st->done) return;  // (the queued tail of a converged scan2map loop)
   const PassConsts pc = *pcp;
   __shared__ float4 tile[kTile];
   const int qi = blockIdx.x * kKnnThreads + threadIdx.x;
@@ -180,16 +176,27 @@ __device__ __forceinline__ void lm_row(const float4 po, const float* c, const Pa
 }
 
 // One thread per feature point.  partial: [gridDim.x][kRowAcc + 1] (the last entry = selected points of the block).
+// Many slots (sl non-null): block b serves slot blk_slot[b], whose queries q[CORNER ? 0 : 1] start at its block
+// blk[...]; a block never straddles two slots, so each slot's partials are those of its own single call.
 template <bool CORNER>
 __global__ void __launch_bounds__(kFitThreads) lins_map_fit_kernel(const float4* __restrict__ q, int n_q, const float4* __restrict__ map,
                                                                    int n_slices, const float* __restrict__ part_d,
                                                                    const int* __restrict__ part_i, const PassConsts* __restrict__ pcp,
-                                                                   const int* __restrict__ done, int32_t* __restrict__ knn_out,
+                                                                   const MapLoopState* __restrict__ st, int32_t* __restrict__ knn_out,
                                                                    float* __restrict__ coeff_out, uint8_t* __restrict__ mask_out,
-                                                                   double* __restrict__ partial) {
-  if (done && *done) return;
-  const PassConsts pc = *pcp;
-  const int qi = blockIdx.x * kFitThreads + threadIdx.x;
+                                                                   double* __restrict__ partial, const MapSlot* __restrict__ sl,
+                                                                   const int* __restrict__ blk_slot) {
+  const int row = blockIdx.x * kFitThreads + threadIdx.x;
+  int slot = 0, qi = row;
+  if (sl) {
+    constexpr int K = CORNER ? 0 : 1;
+    slot = blk_slot[blockIdx.x];
+    const MapSlot& v = sl[slot];
+    q = v.q[K]; n_q = v.nq[K]; map = v.map[K];
+    qi = (blockIdx.x - v.blk[K]) * kFitThreads + threadIdx.x;
+  }
+  if (st && st[slot].done) return;
+  const PassConsts pc = pcp[slot];
   double acc[kRowAcc];
 #pragma unroll
   for (int k = 0; k < kRowAcc; ++k) acc[k] = 0.0;
@@ -201,7 +208,7 @@ __global__ void __launch_bounds__(kFitThreads) lins_map_fit_kernel(const float4*
     Top5 t;
     t.init();
     for (int s = 0; s < n_slices; ++s) {
-      const size_t o = ((size_t)qi * n_slices + s) * 5;
+      const size_t o = ((size_t)row * n_slices + s) * 5;
       for (int k = 0; k < 5; ++k) {
         const int idx = part_i[o + k];
         const float dk = part_d[o + k];
@@ -283,12 +290,7 @@ __global__ void __launch_bounds__(kFitThreads) lins_map_fit_kernel(const float4*
 constexpr float kGridCell = 1.0f;  // >= the 1 m acceptance radius
 constexpr int kGridKnnWarps = 4;   // query warps per CTA
 
-struct GridIndex {
-  const float4* pts;      // map points bucket-sorted: (x, y, z, original index as int bits)
-  const int* start;       // [n_buckets + 1]
-  unsigned mask;          // n_buckets - 1 (power of two)
-  float ox, oy, oz;       // grid origin
-};
+
 // Cell indices are taken as unsigned so that the block's neighbour arithmetic (cx - 1, cx + 1) wraps instead of
 // overflowing at a saturated cell; the hash sees the same bits either way.
 __device__ __forceinline__ unsigned grid_hash(unsigned ix, unsigned iy, unsigned iz) {
@@ -305,14 +307,27 @@ __device__ __forceinline__ void grid_cell(const GridIndex& g, float x, float y, 
   iz = (unsigned)__double2int_rd((double)z - (double)g.oz);
 }
 // counting sort of the map by bucket: count, (host-launched) scan, scatter.  n_dev (optional): the device-resident
-// number of points, <= n, when the host only knows the capacity n
-__global__ void lins_grid_count_kernel(const float4* __restrict__ map, int n, const int* __restrict__ n_dev, GridIndex g, int* __restrict__ count) {
-  const int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= n || (n_dev && i >= *n_dev)) return;
-  const float4 p = __ldg(&map[i]);
+// number of points, <= n, when the host only knows the capacity n.  Many slots (sl non-null, n_sl slots): point i of
+// the n is point i - m0[k] of slot s's map k, with the slot's grid and its buckets from bucket0[k] on.
+struct GridPoint { const float4* map; int i; const int* n_dev; GridIndex g; int b0; };
+__device__ __forceinline__ GridPoint grid_point(const float4* map, int i, const int* n_dev, const GridIndex& g, const MapSlot* sl, int n_sl) {
+  if (!sl) return GridPoint{map, i, n_dev, g, 0};
+  int lo = 0, hi = n_sl - 1;  // the last slot whose maps start at or before i
+  while (lo < hi) { const int m = (lo + hi + 1) >> 1; if (sl[m].m0[0] <= i) lo = m; else hi = m - 1; }
+  const MapSlot& v = sl[lo];
+  const int k = i >= v.m0[1];
+  return GridPoint{v.map[k], i - v.m0[k], v.n_map[k], v.g[k], v.bucket0[k]};
+}
+__global__ void lins_grid_count_kernel(const float4* __restrict__ map, int n, const int* __restrict__ n_dev, GridIndex g, int* __restrict__ count,
+                                       const MapSlot* __restrict__ sl, int n_sl) {
+  const int i0 = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i0 >= n) return;
+  const GridPoint gp = grid_point(map, i0, n_dev, g, sl, n_sl);
+  if (gp.n_dev && gp.i >= *gp.n_dev) return;
+  const float4 p = __ldg(&gp.map[gp.i]);
   unsigned ix, iy, iz;
-  grid_cell(g, p.x, p.y, p.z, ix, iy, iz);
-  atomicAdd(&count[grid_hash(ix, iy, iz) & g.mask], 1);
+  grid_cell(gp.g, p.x, p.y, p.z, ix, iy, iz);
+  atomicAdd(&count[gp.b0 + (grid_hash(ix, iy, iz) & gp.g.mask)], 1);
 }
 // exclusive scan of count[0..n) -> start[0..n], one CTA (runs once per lins_gpu_map_set)
 __global__ void __launch_bounds__(1024) lins_grid_scan_kernel(const int* __restrict__ count, int* __restrict__ start, int* __restrict__ cursor, int n) {
@@ -328,14 +343,16 @@ __global__ void __launch_bounds__(1024) lins_grid_scan_kernel(const int* __restr
   for (int i = lo; i < hi; ++i) { start[i] = run; cursor[i] = run; run += count[i]; }
 }
 __global__ void lins_grid_scatter_kernel(const float4* __restrict__ map, int n, const int* __restrict__ n_dev, GridIndex g, int* __restrict__ cursor,
-                                         float4* __restrict__ sorted) {
-  const int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= n || (n_dev && i >= *n_dev)) return;
-  const float4 p = __ldg(&map[i]);
+                                         float4* __restrict__ sorted, const MapSlot* __restrict__ sl, int n_sl) {
+  const int i0 = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i0 >= n) return;
+  const GridPoint gp = grid_point(map, i0, n_dev, g, sl, n_sl);
+  if (gp.n_dev && gp.i >= *gp.n_dev) return;
+  const float4 p = __ldg(&gp.map[gp.i]);
   unsigned ix, iy, iz;
-  grid_cell(g, p.x, p.y, p.z, ix, iy, iz);
-  const int pos = atomicAdd(&cursor[grid_hash(ix, iy, iz) & g.mask], 1);
-  sorted[pos] = make_float4(p.x, p.y, p.z, __int_as_float(i));
+  grid_cell(gp.g, p.x, p.y, p.z, ix, iy, iz);
+  const int pos = atomicAdd(&cursor[gp.b0 + (grid_hash(ix, iy, iz) & gp.g.mask)], 1);
+  sorted[pos] = make_float4(p.x, p.y, p.z, __int_as_float(gp.i));
 }
 
 struct Top5K {  // five smallest (distance bits, index) keys, ascending
@@ -353,15 +370,26 @@ struct Top5K {  // five smallest (distance bits, index) keys, ascending
   }
 };
 
-// one warp per query; part_d / part_i: [n_q][1][5] (a single "slice" for lins_map_fit_kernel)
+// one warp per query; part_d / part_i: [n_q][1][5] (a single "slice" for lins_map_fit_kernel).  Many slots (sl
+// non-null): n_q rows in lins_map_fit_kernel's blocks, row r in block r / kFitThreads of slot blk_slot[that block], map
+// `kind` (0 corner, 1 surf).
 __global__ void __launch_bounds__(kGridKnnWarps * 32) lins_map_knn_grid_kernel(const float4* __restrict__ q, int n_q, GridIndex g,
-                                                                               const PassConsts* __restrict__ pcp, const int* __restrict__ done,
-                                                                               float* __restrict__ part_d, int* __restrict__ part_i) {
-  if (done && *done) return;
+                                                                               const PassConsts* __restrict__ pcp, const MapLoopState* __restrict__ st,
+                                                                               float* __restrict__ part_d, int* __restrict__ part_i,
+                                                                               const MapSlot* __restrict__ sl, const int* __restrict__ blk_slot, int kind) {
   const int lane = threadIdx.x & 31;
-  const int qi = blockIdx.x * kGridKnnWarps + (threadIdx.x >> 5);
-  if (qi >= n_q) return;
-  const PassConsts pc = *pcp;
+  const int row = blockIdx.x * kGridKnnWarps + (threadIdx.x >> 5);
+  if (row >= n_q) return;
+  int slot = 0, qi = row;
+  if (sl) {
+    slot = blk_slot[row / kFitThreads];
+    const MapSlot& v = sl[slot];
+    qi = row - v.blk[kind] * kFitThreads;
+    if (qi >= v.nq[kind]) return;
+    q = v.q[kind]; g = v.g[kind];
+  }
+  if (st && st[slot].done) return;
+  const PassConsts pc = pcp[slot];
   const float3 s = associate_to_map(__ldg(&q[qi]), pc);
   unsigned cx, cy, cz;
   grid_cell(g, s.x, s.y, s.z, cx, cy, cz);
@@ -383,7 +411,7 @@ __global__ void __launch_bounds__(kGridKnnWarps * 32) lins_map_knn_grid_kernel(c
   }
   // five rounds: the smallest head among the lanes' ascending lists
   int head = 0;
-  const size_t o = (size_t)qi * 5;
+  const size_t o = (size_t)row * 5;
 #pragma unroll
   for (int r = 0; r < 5; ++r) {
     const unsigned long long mykey = head < 5 ? t.k[0] : 0xFFFFFFFFFFFFFFFFull;
@@ -404,15 +432,6 @@ __global__ void __launch_bounds__(kGridKnnWarps * 32) lins_map_knn_grid_kernel(c
   }
 }
 
-// state of one scan2MapOptimization call on the device
-struct MapLoopState {
-  float T[6];            // transformTobeMapped
-  float matP[36];
-  int isDegenerate, done, iters, converged;
-  int n_sel[10];
-  float delta_r[10], delta_t[10];
-};
-
 __device__ __forceinline__ void pass_consts_from(const float* T, PassConsts& pc) {  // :579-592, :1527-1532 (f32 like the reference)
   pc.cRoll = (float)cos((double)T[0]); pc.sRoll = (float)sin((double)T[0]);
   pc.cPitch = (float)cos((double)T[1]); pc.sPitch = (float)sin((double)T[1]);
@@ -421,16 +440,22 @@ __device__ __forceinline__ void pass_consts_from(const float* T, PassConsts& pc)
   pc.srx = pc.sRoll; pc.crx = pc.cRoll; pc.sry = pc.sPitch; pc.cry = pc.cPitch; pc.srz = pc.sYaw; pc.crz = pc.cYaw;
 }
 
-// one warp (the 6 x 6 step itself is one thread): block partials -> matAtA / matAtB (f32), the LM step, the next iteration's constants.  Every matrix lives
-// in shared memory (plain dynamically indexed loads / stores).
+// one warp per slot, one block each (the 6 x 6 step itself is one thread): block partials -> matAtA / matAtB (f32), the LM
+// step, the next iteration's constants.  Every matrix lives in shared memory (plain dynamically indexed loads / stores).
+// One slot: partial blocks [0, nblocks).  Many slots (sl non-null): slot s sums its corner blocks [blk[0], blk[0] +
+// nblk[0]) and then its surf blocks, which start at nblocks (the corner launch's block count) + blk[1].
 __global__ void lins_map_lm_kernel(const double* __restrict__ partial, int nblocks, int iter, MapLoopState* __restrict__ st,
-                                   PassConsts* __restrict__ pc_next) {
-  if (blockIdx.x != 0 || st->done) return;
+                                   PassConsts* __restrict__ pc_next, const MapSlot* __restrict__ sl) {
+  st += blockIdx.x; pc_next += blockIdx.x;
+  if (st->done) return;
   __shared__ double acc[kRowAcc + 1];
   __shared__ float AtA[36], AtB[6], Aw[36], X[6], Ae[36], E[6], V[36], V2[36], Vc[36], Vinv[36], X2[6];
   if (threadIdx.x <= kRowAcc) {  // lane k sums column k of the block partials, in a fixed order: corner blocks, then surf
     double v = 0.0;               // blocks (laserCloudOri's order)
-    for (int b = 0; b < nblocks; ++b) v += partial[(size_t)b * (kRowAcc + 1) + threadIdx.x];
+    int r[4] = {0, nblocks, 0, 0};
+    if (sl) { const MapSlot& m = sl[blockIdx.x]; r[0] = m.blk[0]; r[1] = m.blk[0] + m.nblk[0]; r[2] = nblocks + m.blk[1]; r[3] = r[2] + m.nblk[1]; }
+    for (int b = r[0]; b < r[1]; ++b) v += partial[(size_t)b * (kRowAcc + 1) + threadIdx.x];
+    for (int b = r[2]; b < r[3]; ++b) v += partial[(size_t)b * (kRowAcc + 1) + threadIdx.x];
     acc[threadIdx.x] = v;
   }
   __syncwarp();

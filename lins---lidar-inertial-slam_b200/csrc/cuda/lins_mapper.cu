@@ -8,11 +8,14 @@
 // loop-candidate search, in the reference's f32 / f64 types (no multiply-add contraction: this unit is built with
 // -fmad=false and g++ does not contract on x86-64 without -mfma).
 //
-// VoxelGrid (csrc/host/feature_extraction.hpp restates PCL's applyFilter): the finite points' min / max (ordered-integer
-// atomics: min / max are exact in any order), min_b = floor(min * inv), the key floor(p * inv) - (float)min_b per axis
-// (lins_features.cuh: voxel_key), a stable CUB radix sort of (key, index), and one centroid per voxel, its points summed
-// in f32 in input order (the sort is stable), output in ascending key order.  Non-finite points and every point of a
-// call whose div_x * div_y * div_z exceeds INT32_MAX get the key 0xffffffff, which no voxel can have, and are dropped.
+// VoxelGrid (csrc/host/feature_extraction.hpp restates PCL's applyFilter), on one or many clouds (segments) in one pass:
+// each segment's finite points' min / max (ordered-integer atomics: min / max are exact in any order), its min_b =
+// floor(min * inv), the key floor(p * inv) - (float)min_b per axis (lins_features.cuh: voxel_key), a stable CUB radix
+// sort of (key, index) — with more than one segment of ((segment, key), index) on 32 + ceil(log2 segments) bits, so
+// the segments stay in their input ranges — and one centroid per voxel, its points summed in f32 in input order (the
+// sort is stable), output in ascending key order at the segment's own offset.  Non-finite points and every point of a
+// segment whose div_x * div_y * div_z exceeds INT32_MAX get the key 0xffffffff, which no voxel can have, and are
+// dropped; each output has room for its segment's points and is NaN past the voxel count.
 //
 // Synchronisation: one per processed cycle.  The VoxelGrids' outputs are sized by their inputs and padded with NaN, the
 // later launches take those capacities, a device-side gate stops the scan-to-map loop when the map is too small, and
@@ -44,27 +47,70 @@ __device__ __forceinline__ unsigned f2ord(float f) {
 __device__ __forceinline__ float ord2f(unsigned u) { return __uint_as_float((u & 0x80000000u) ? (u & 0x7fffffffu) : ~u); }
 __device__ __forceinline__ bool finite3(const float4 p) { return isfinite(p.x) && isfinite(p.y) && isfinite(p.z); }
 
-__global__ void __launch_bounds__(kVgThreads) lins_vg_bounds_kernel(const float4* __restrict__ p, int n, VgInfo* __restrict__ info) {
+// the segments of one VoxelGrid call: off (n + 1) and out (n) on the device; n == 1 needs neither (out is a kernel argument)
+struct VgSegs { const int* off; float4* const* out; int n; };
+__device__ __forceinline__ int seg_of(const VgSegs& sg, int i) {  // the segment of input point i
+  if (sg.n == 1) return 0;
+  int lo = 0, hi = sg.n - 1;
+  while (lo < hi) { const int m = (lo + hi + 1) >> 1; if (__ldg(&sg.off[m]) <= i) lo = m; else hi = m - 1; }
+  return lo;
+}
+__device__ __forceinline__ void vg_flush(VgInfo* info, const unsigned e[6]) {
+  for (int k = 0; k < 3; ++k) { atomicMin(&info->enc[k], e[k]); atomicMax(&info->enc[3 + k], e[3 + k]); }
+}
+// 32-bit keys: one segment; 64-bit keys: (segment, voxel key)
+template <typename Key> __device__ __forceinline__ Key make_key(int sgi, unsigned k) {
+  if constexpr (sizeof(Key) == 8) return ((Key)sgi << 32) | k;
+  else return k;
+}
+template <typename Key> __device__ __forceinline__ int key_seg(Key k) {
+  if constexpr (sizeof(Key) == 8) return (int)(k >> 32);
+  else return 0;
+}
+template <typename Key> __device__ __forceinline__ unsigned key_low(Key k) { return (unsigned)k; }
+
+// per segment: the finite points' min / max.  Each warp scans one contiguous run of points, its lanes interleaved
+// (coalesced loads); a lane looks its segment up only when it passes the end of the last one, and accumulates while the
+// segment stays the same.  A warp whose lanes all end in one segment reduces before its one set of atomics.
+__global__ void __launch_bounds__(kVgThreads) lins_vg_bounds_kernel(const float4* __restrict__ p, int n, VgSegs sg, VgInfo* __restrict__ info) {
   unsigned e[6] = {0xffffffffu, 0xffffffffu, 0xffffffffu, 0u, 0u, 0u};
-  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
+  int cur = -1, seg_end = 0;
+  const long long n_warps = ((long long)gridDim.x * blockDim.x) >> 5, warp = ((long long)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+  const long long per = ((n + n_warps - 1) / n_warps + 31) & ~31ll;
+  const int i1 = (int)min((long long)n, (warp + 1) * per);
+  for (int i = (int)min((long long)n, warp * per) + (threadIdx.x & 31); i < i1; i += 32) {
     const float4 q = p[i];
     if (!finite3(q)) continue;
+    if (i >= seg_end) {
+      const int sgi = seg_of(sg, i);
+      seg_end = sg.n == 1 ? n : __ldg(&sg.off[sgi + 1]);
+      if (sgi != cur) {
+        if (cur >= 0) vg_flush(info + cur, e);
+        cur = sgi;
+        for (int k = 0; k < 3; ++k) { e[k] = 0xffffffffu; e[3 + k] = 0u; }
+      }
+    }
     const unsigned a[3] = {f2ord(q.x), f2ord(q.y), f2ord(q.z)};
     for (int k = 0; k < 3; ++k) { e[k] = min(e[k], a[k]); e[3 + k] = max(e[3 + k], a[k]); }
   }
-  for (int off = 16; off > 0; off >>= 1)
-    for (int k = 0; k < 6; ++k) {
-      const unsigned o = __shfl_xor_sync(0xffffffffu, e[k], off);
-      e[k] = k < 3 ? min(e[k], o) : max(e[k], o);
-    }
-  if ((threadIdx.x & 31) == 0) {
-    for (int k = 0; k < 3; ++k) { atomicMin(&info->enc[k], e[k]); atomicMax(&info->enc[3 + k], e[3 + k]); }
+  const int c0 = __reduce_max_sync(0xffffffffu, cur);
+  if (__all_sync(0xffffffffu, cur == c0 || cur < 0)) {
+    for (int off = 16; off > 0; off >>= 1)
+      for (int k = 0; k < 6; ++k) {
+        const unsigned o = __shfl_xor_sync(0xffffffffu, e[k], off);
+        e[k] = k < 3 ? min(e[k], o) : max(e[k], o);
+      }
+    if ((threadIdx.x & 31) == 0 && c0 >= 0) vg_flush(info + c0, e);
+  } else if (cur >= 0) {
+    vg_flush(info + cur, e);
   }
 }
 
-// getMinMax3D -> min_b, div_b, divb_mul (feature_extraction.hpp VoxelGrid::filter)
-__global__ void lins_vg_box_kernel(VgInfo* __restrict__ info) {
-  VgInfo& v = *info;
+// getMinMax3D -> min_b, div_b, divb_mul (feature_extraction.hpp VoxelGrid::filter), one thread per segment
+__global__ void lins_vg_box_kernel(VgInfo* __restrict__ infos, int n_seg) {
+  const int sgi = blockIdx.x * blockDim.x + threadIdx.x;
+  if (sgi >= n_seg) return;
+  VgInfo& v = infos[sgi];
   v.any = v.enc[0] != 0xffffffffu;
   v.toobig = 0;
   if (!v.any) return;
@@ -77,31 +123,43 @@ __global__ void lins_vg_box_kernel(VgInfo* __restrict__ info) {
   v.mul[0] = 1; v.mul[1] = (int)div[0]; v.mul[2] = v.toobig ? 0 : (int)(div[0] * div[1]);
 }
 
-__global__ void __launch_bounds__(kVgThreads) lins_vg_key_kernel(const float4* __restrict__ p, int n, const VgInfo* __restrict__ info,
-                                                                 unsigned* __restrict__ key, int* __restrict__ idx) {
+// the keys, and NaN in every output record (the centroids then overwrite a segment's first `count`)
+template <typename Key>
+__global__ void __launch_bounds__(kVgThreads) lins_vg_key_kernel(const float4* __restrict__ p, int n, VgSegs sg, const VgInfo* __restrict__ info,
+                                                                 float4* __restrict__ out, Key* __restrict__ key, int* __restrict__ idx) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n) return;
-  const VgInfo& v = *info;
+  const int sgi = seg_of(sg, i);
+  const VgInfo& v = info[sgi];
   const float4 q = p[i];
-  key[i] = v.any && !v.toobig && finite3(q) ? lins_feat::voxel_key(q.x, q.y, q.z, v.min_b, v.mul, v.inv) : kInvalidKey;
+  key[i] = make_key<Key>(sgi, v.any && !v.toobig && finite3(q) ? lins_feat::voxel_key(q.x, q.y, q.z, v.min_b, v.mul, v.inv) : kInvalidKey);
   idx[i] = i;
+  const float nan = __int_as_float(0xffffffff);
+  if (sg.n == 1) out[i] = make_float4(nan, nan, nan, nan);
+  else sg.out[sgi][i - __ldg(&sg.off[sgi])] = make_float4(nan, nan, nan, nan);
 }
 
-__global__ void __launch_bounds__(kVgThreads) lins_vg_head_kernel(const unsigned* __restrict__ key, int n, int* __restrict__ head) {
+template <typename Key>
+__global__ void __launch_bounds__(kVgThreads) lins_vg_head_kernel(const Key* __restrict__ key, int n, int* __restrict__ head) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n) return;
-  head[i] = key[i] != kInvalidKey && (i == 0 || key[i] != key[i - 1]);
+  head[i] = key_low(key[i]) != kInvalidKey && (i == 0 || key[i] != key[i - 1]);
 }
 
-// one thread per voxel head: the f32 sums of its points in sorted (= input) order, divided by the count
-__global__ void __launch_bounds__(kVgThreads) lins_vg_centroid_kernel(const unsigned* __restrict__ key, const int* __restrict__ idx,
-                                                                      const int* __restrict__ vid, int n, const float4* __restrict__ p,
+// one thread per voxel head: the f32 sums of its points in sorted (= input) order, divided by the count.  The sort keeps
+// each segment in its input range, so a segment's voxel ids count from the inclusive scan just before that range.
+template <typename Key>
+__global__ void __launch_bounds__(kVgThreads) lins_vg_centroid_kernel(const Key* __restrict__ key, const int* __restrict__ idx,
+                                                                      const int* __restrict__ vid, int n, VgSegs sg, const float4* __restrict__ p,
                                                                       float4* __restrict__ out, VgInfo* __restrict__ info) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n) return;
-  const unsigned k = key[i];
-  if (k == kInvalidKey) return;
-  if (i + 1 == n || key[i + 1] == kInvalidKey) info->count = vid[i];
+  const Key k = key[i];
+  if (key_low(k) == kInvalidKey) return;
+  const int sgi = key_seg(k);
+  const int b0 = sg.n == 1 ? 0 : __ldg(&sg.off[sgi]), b1 = sg.n == 1 ? n : __ldg(&sg.off[sgi + 1]);
+  const int base = b0 > 0 ? vid[b0 - 1] : 0;
+  if (i + 1 == b1 || key_low(key[i + 1]) == kInvalidKey) info[sgi].count = vid[i] - base;
   if (i > 0 && key[i - 1] == k) return;
   float cx = 0.f, cy = 0.f, cz = 0.f, ci = 0.f;
   int j = i;
@@ -110,73 +168,113 @@ __global__ void __launch_bounds__(kVgThreads) lins_vg_centroid_kernel(const unsi
     cx += q.x; cy += q.y; cz += q.z; ci += q.w;
   }
   const float c = (float)(j - i);
-  out[vid[i] - 1] = make_float4(cx / c, cy / c, cz / c, ci / c);
+  float4* o = sg.n == 1 ? out : sg.out[sgi];
+  o[vid[i] - base - 1] = make_float4(cx / c, cy / c, cz / c, ci / c);
 }
 
-// transformPointCloud (:624-652) with the constants of updateTransformPointCloudSinCos (:609-622)
+// transformPointCloud (:624-652) with the constants of updateTransformPointCloudSinCos (:609-622), one block per job
 struct TfConsts { float cr, sr, cp, sp, cy, sy, tx, ty, tz; };
-__global__ void __launch_bounds__(256) lins_mapper_transform_kernel(const float4* __restrict__ in, float4* __restrict__ out, int n, TfConsts c) {
-  const int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= n) return;
-  const float4 p = in[i];
-  const float x1 = c.cy * p.x - c.sy * p.y;
-  const float y1 = c.sy * p.x + c.cy * p.y;
-  const float z1 = p.z;
-  const float x2 = x1;
-  const float y2 = c.cr * y1 - c.sr * z1;
-  const float z2 = c.sr * y1 + c.cr * z1;
-  out[i] = make_float4(c.cp * x2 + c.sp * z2 + c.tx, y2 + c.ty, -c.sp * x2 + c.cp * z2 + c.tz, p.w);
+struct TfJob { const float4* in; float4* out; int n, pad; TfConsts c; };
+__global__ void __launch_bounds__(256) lins_mapper_transform_kernel(const TfJob* __restrict__ jobs) {
+  const TfJob& jb = jobs[blockIdx.x];
+  const TfConsts c = jb.c;
+  for (int i = threadIdx.x; i < jb.n; i += blockDim.x) {
+    const float4 p = jb.in[i];
+    const float x1 = c.cy * p.x - c.sy * p.y;
+    const float y1 = c.sy * p.x + c.cy * p.y;
+    const float z1 = p.z;
+    const float x2 = x1;
+    const float y2 = c.cr * y1 - c.sr * z1;
+    const float z2 = c.sr * y1 + c.cr * z1;
+    jb.out[i] = make_float4(c.cp * x2 + c.sp * z2 + c.tx, y2 + c.ty, -c.sp * x2 + c.cp * z2 + c.tz, p.w);
+  }
+}
+
+int ceil_log2(int n) { int b = 0; while ((1 << b) < n) ++b; return b; }
+
+template <typename Key>
+int vg_queue(lins_ctx* ctx, VgScratch& w, Key* const k[2], const float4* in, int n, const VgSegs& sg, float4* out, VgInfo* info) {
+  const int blocks = (n + kVgThreads - 1) / kVgThreads;
+  lins_vg_bounds_kernel<<<std::min(blocks, 8 * ctx->sm_count), kVgThreads, 0, ctx->stream>>>(in, n, sg, info);
+  lins_vg_box_kernel<<<(sg.n + 127) / 128, 128, 0, ctx->stream>>>(info, sg.n);
+  lins_vg_key_kernel<Key><<<blocks, kVgThreads, 0, ctx->stream>>>(in, n, sg, info, out, k[0], w.idx[0].p);
+  CK(cudaGetLastError());
+  size_t bytes = w.temp.cap;
+  CK(cub::DeviceRadixSort::SortPairs(w.temp.p, bytes, k[0], k[1], w.idx[0].p, w.idx[1].p, n, 0, 32 + ceil_log2(sg.n), ctx->stream));
+  lins_vg_head_kernel<Key><<<blocks, kVgThreads, 0, ctx->stream>>>(k[1], n, w.head.p);
+  bytes = w.temp.cap;
+  CK(cub::DeviceScan::InclusiveSum(w.temp.p, bytes, w.head.p, w.vid.p, n, ctx->stream));
+  lins_vg_centroid_kernel<Key><<<blocks, kVgThreads, 0, ctx->stream>>>(k[1], w.idx[1].p, w.vid.p, n, sg, in, out, info);
+  CK(cudaGetLastError());
+  ctx->launches += 7;
+  return LINS_OK;
 }
 
 }  // namespace
 
 namespace lins_capi {
 
-// the scratch of VoxelGrids of up to n points (grow-only; call before queuing work that a growth could free under)
-int voxel_grid_reserve(lins_ctx* ctx, int n) {
-  MapperState& M = ctx->mapper;
+int voxel_grid_reserve(lins_ctx* ctx, VgScratch& w, int n, int n_seg) {
   if (n <= 0) return LINS_OK;
-  CK(M.key[0].reserve((size_t)n)); CK(M.key[1].reserve((size_t)n)); CK(M.idx[0].reserve((size_t)n)); CK(M.idx[1].reserve((size_t)n));
-  CK(M.head.reserve((size_t)n)); CK(M.vid.reserve((size_t)n));
+  CK(w.idx[0].grow((size_t)n)); CK(w.idx[1].grow((size_t)n)); CK(w.head.grow((size_t)n)); CK(w.vid.grow((size_t)n));
   size_t b_sort = 0, b_scan = 0;
-  CK(cub::DeviceRadixSort::SortPairs(nullptr, b_sort, M.key[0].p, M.key[1].p, M.idx[0].p, M.idx[1].p, n, 0, 32, ctx->stream));
-  CK(cub::DeviceScan::InclusiveSum(nullptr, b_scan, M.head.p, M.vid.p, n, ctx->stream));
-  CK(M.temp.reserve(std::max(b_sort, b_scan) + 16));
+  const int bits = 32 + ceil_log2(n_seg);
+  if (n_seg == 1) {
+    CK(w.key[0].grow((size_t)n)); CK(w.key[1].grow((size_t)n));
+    CK(cub::DeviceRadixSort::SortPairs(nullptr, b_sort, w.key[0].p, w.key[1].p, w.idx[0].p, w.idx[1].p, n, 0, bits, ctx->stream));
+  } else {
+    CK(w.key64[0].grow((size_t)n)); CK(w.key64[1].grow((size_t)n));
+    CK(cub::DeviceRadixSort::SortPairs(nullptr, b_sort, w.key64[0].p, w.key64[1].p, w.idx[0].p, w.idx[1].p, n, 0, bits, ctx->stream));
+  }
+  CK(cub::DeviceScan::InclusiveSum(nullptr, b_scan, w.head.p, w.vid.p, n, ctx->stream));
+  CK(w.temp.grow(std::max(b_sort, b_scan) + 16));
   return LINS_OK;
 }
 
-// queue one VoxelGrid of the n device points `in` into `out` (room for n: the centroids, then NaN records), with its
-// record at info (device); the count and the flags are read back by the caller
-int voxel_grid_queue(lins_ctx* ctx, const float4* in, int n, float leaf, float4* out, VgInfo* info) {
-  MapperState& M = ctx->mapper;
-  VgInfo init;
-  std::memset(&init, 0, sizeof(init));
-  for (int k = 0; k < 3; ++k) { init.enc[k] = 0xffffffffu; init.enc[3 + k] = 0u; }
-  init.inv = lins_feat::voxel_inv(leaf);
-  CK(M.h_vg_init.reserve(kMapperGrids));
-  // (pinned: a pageable H2D could complete before the copy engine reads it, but the staging is per-record and rewritten
-  // only after the cycle's read-back)
-  const int slot = (int)(info - M.vg_info.p);
-  M.h_vg_init.p[slot] = init;
-  CK(cudaMemcpyAsync(info, &M.h_vg_init.p[slot], sizeof(VgInfo), cudaMemcpyHostToDevice, ctx->stream));
+int voxel_grid_queue(lins_ctx* ctx, VgScratch& w, const float4* in, int n_seg, const int* h_off, const int* d_off, const float* leaf,
+                     float4* out, float4* const* d_out, VgInfo* h_init, VgInfo* info) {
+  // (pinned staging: a pageable H2D could complete before the copy engine reads it; the callers rewrite it only after
+  // the cycle's read-back)
+  for (int k = 0; k < n_seg; ++k) {
+    VgInfo& v = h_init[k];
+    std::memset(&v, 0, sizeof(v));
+    for (int a = 0; a < 3; ++a) { v.enc[a] = 0xffffffffu; v.enc[3 + a] = 0u; }
+    v.inv = lins_feat::voxel_inv(leaf[k]);
+  }
+  CK(cudaMemcpyAsync(info, h_init, sizeof(VgInfo) * n_seg, cudaMemcpyHostToDevice, ctx->stream));
+  const int n = h_off[n_seg];
   if (n <= 0) return LINS_OK;
-  int rc = voxel_grid_reserve(ctx, n);
+  const int rc = voxel_grid_reserve(ctx, w, n, n_seg);
   if (rc != LINS_OK) return rc;
-  CK(cudaMemsetAsync(out, 0xff, sizeof(float4) * (size_t)n, ctx->stream));  // NaN past the voxel count
-  size_t bytes;
-  const int blocks = (n + kVgThreads - 1) / kVgThreads;
-  lins_vg_bounds_kernel<<<std::min(blocks, 8 * ctx->sm_count), kVgThreads, 0, ctx->stream>>>(in, n, info);
-  lins_vg_box_kernel<<<1, 1, 0, ctx->stream>>>(info);
-  lins_vg_key_kernel<<<blocks, kVgThreads, 0, ctx->stream>>>(in, n, info, M.key[0].p, M.idx[0].p);
+  if (n_seg == 1) {
+    unsigned* const k[2] = {w.key[0].p, w.key[1].p};
+    return vg_queue(ctx, w, k, in, n, VgSegs{nullptr, nullptr, 1}, out, info);
+  }
+  unsigned long long* const k[2] = {w.key64[0].p, w.key64[1].p};
+  return vg_queue(ctx, w, k, in, n, VgSegs{d_off, d_out, n_seg}, nullptr, info);
+}
+
+int keyframes_queue(lins_ctx* ctx, const KfSave* saves, int n, Buf<unsigned char>& dev, Buf<unsigned char, kPinned>& host) {
+  std::vector<TfJob> jobs;
+  for (int i = 0; i < n; ++i) {
+    const KfSave& sv = saves[i];
+    const MapperKeyPose& k = sv.kp;
+    TfConsts c;  // updateTransformPointCloudSinCos: libm's f32 sin / cos of the f32 fields
+    c.cr = std::cos(k.roll); c.sr = std::sin(k.roll); c.cp = std::cos(k.pitch); c.sp = std::sin(k.pitch);
+    c.cy = std::cos(k.yaw); c.sy = std::sin(k.yaw); c.tx = k.x; c.ty = k.y; c.tz = k.z;
+    for (int a = 0; a < 3; ++a) {
+      CK(sv.kf->c[a].grow((size_t)sv.kf->n[a] + 1));
+      if (sv.kf->n[a]) jobs.push_back(TfJob{sv.ds[a], sv.kf->c[a].p, sv.kf->n[a], 0, c});
+    }
+  }
+  if (jobs.empty()) return LINS_OK;
+  const size_t bytes = sizeof(TfJob) * jobs.size();
+  CK(dev.reserve(bytes)); CK(host.reserve(bytes));
+  std::memcpy(host.p, jobs.data(), bytes);
+  CK(cudaMemcpyAsync(dev.p, host.p, bytes, cudaMemcpyHostToDevice, ctx->stream));
+  lins_mapper_transform_kernel<<<(int)jobs.size(), 256, 0, ctx->stream>>>(reinterpret_cast<const TfJob*>(dev.p));
   CK(cudaGetLastError());
-  bytes = M.temp.cap;
-  CK(cub::DeviceRadixSort::SortPairs(M.temp.p, bytes, M.key[0].p, M.key[1].p, M.idx[0].p, M.idx[1].p, n, 0, 32, ctx->stream));
-  lins_vg_head_kernel<<<blocks, kVgThreads, 0, ctx->stream>>>(M.key[1].p, n, M.head.p);
-  bytes = M.temp.cap;
-  CK(cub::DeviceScan::InclusiveSum(M.temp.p, bytes, M.head.p, M.vid.p, n, ctx->stream));
-  lins_vg_centroid_kernel<<<blocks, kVgThreads, 0, ctx->stream>>>(M.key[1].p, M.idx[1].p, M.vid.p, n, in, out, info);
-  CK(cudaGetLastError());
-  ctx->launches += 7;
+  ctx->launches += 1;
   return LINS_OK;
 }
 
@@ -316,13 +414,6 @@ void transform_update(MapperScalars& s, double timeLaserOdometry, double SCAN_PE
   }
 }
 
-TfConsts tf_consts(const MapperKeyPose& k) {  // updateTransformPointCloudSinCos: libm's f32 sin / cos of the f32 fields
-  TfConsts c;
-  c.cr = std::cos(k.roll); c.sr = std::sin(k.roll); c.cp = std::cos(k.pitch); c.sp = std::sin(k.pitch);
-  c.cy = std::cos(k.yaw); c.sy = std::sin(k.yaw); c.tx = k.x; c.ty = k.y; c.tz = k.z;
-  return c;
-}
-
 int upload3(lins_ctx* ctx, const lins_mapper_desc* d) {
   MapperState& M = ctx->mapper;
   const int n[3] = {d->n_corner, d->n_surf, d->n_outlier};
@@ -339,15 +430,8 @@ int upload3(lins_ctx* ctx, const lins_mapper_desc* d) {
   return LINS_OK;
 }
 
-// the non-empty copies of a batch through the gather list, at entries base.. (two batches of one cycle do not overlap)
-int queue_copies(lins_ctx* ctx, std::vector<DevCopy> v, int base) {
-  v.erase(std::remove_if(v.begin(), v.end(), [](const DevCopy& c) { return c.n <= 0; }), v.end());
-  const int rc = ctx->mapper.copies.stage(ctx, v.data(), (int)v.size(), base);
-  return rc != LINS_OK ? rc : ctx->mapper.copies.launch(ctx, base, (int)v.size());
-}
-
 // the slot of key frame id (a free one, or a new one)
-MapperKeyFrame& keyframe_slot(MapperState& M, int id) {
+MapperKeyFrame& keyframe_slot(MapperNode& M, int id) {
   auto it = M.slot_of.find(id);
   if (it != M.slot_of.end()) return M.slots[it->second];
   int s;
@@ -357,69 +441,63 @@ MapperKeyFrame& keyframe_slot(MapperState& M, int id) {
   return M.slots[s];
 }
 
-}  // namespace
-
-extern "C" {
-
-int lins_gpu_mapper_reset(lins_ctx* ctx) {
-  if (!ctx) return LINS_E_INVALID;
-  CK(cudaSetDevice(ctx->device));
+// one VoxelGrid record per segment at info, staged at h_init
+int voxel_grid_one(lins_ctx* ctx, const float4* in, int n, float leaf, float4* out, VgInfo* info) {
   MapperState& M = ctx->mapper;
-  M.s = MapperScalars();
-  M.poses.clear();
-  for (auto& kv : M.slot_of) M.free_slots.push_back(kv.second);
-  M.slot_of.clear();
-  M.last = MapperLast();
-  return map_reset_loop(ctx);  // isDegenerate, matP
+  CK(M.h_vg_init.reserve(kMapperGrids));
+  const int off[2] = {0, std::max(n, 0)};
+  return voxel_grid_queue(ctx, M.vg, in, 1, off, nullptr, &leaf, out, nullptr, M.h_vg_init.p + (info - M.vg_info.p), info);
 }
 
-int lins_gpu_mapper_imu(lins_ctx* ctx, const double* time, const double* roll, const double* pitch, int n) {
-  if (!ctx) return LINS_E_INVALID;
-  if (n < 0 || (n > 0 && (!time || !roll || !pitch))) return fail(ctx, LINS_E_INVALID, "bad IMU arrays");
-  MapperScalars& s = ctx->mapper.s;
+}  // namespace
+
+namespace lins_capi {
+
+// the non-empty copies of a batch through the gather list, at entries base.. (two batches of one cycle do not overlap)
+int queue_copies(lins_ctx* ctx, CopyList& l, std::vector<DevCopy> v, int base) {
+  v.erase(std::remove_if(v.begin(), v.end(), [](const DevCopy& c) { return c.n <= 0; }), v.end());
+  const int rc = l.stage(ctx, v.data(), (int)v.size(), base);
+  return rc != LINS_OK ? rc : l.launch(ctx, base, (int)v.size());
+}
+
+void mapper_node_reset(MapperNode& m) {
+  m.s = MapperScalars();
+  m.poses.clear();
+  for (auto& kv : m.slot_of) m.free_slots.push_back(kv.second);
+  m.slot_of.clear();
+  m.last = MapperLast();
+}
+
+void mapper_node_imu(MapperScalars& s, const double* time, const double* roll, const double* pitch, int n) {
   for (int i = 0; i < n; ++i) {  // imuHandler :731-734
     s.imuPointerLast = (s.imuPointerLast + 1) % LINS_MAPPER_IMU_QUEUE;
     s.imuTime[s.imuPointerLast] = time[i];
     s.imuRoll[s.imuPointerLast] = (float)roll[i];
     s.imuPitch[s.imuPointerLast] = (float)pitch[i];
   }
-  return LINS_OK;
 }
 
-int lins_gpu_mapper_step(lins_ctx* ctx, const lins_mapper_desc* d, lins_mapper_report* rep) {
-  if (!ctx) return LINS_E_INVALID;
-  if (!d) return fail(ctx, LINS_E_INVALID, "null desc");
-  if (check_cloud(ctx, d->corner, d->n_corner, "bad mapper corner cloud") != LINS_OK || check_cloud(ctx, d->surf, d->n_surf, "bad mapper surf cloud") != LINS_OK ||
-      check_cloud(ctx, d->outlier, d->n_outlier, "bad mapper outlier cloud") != LINS_OK)
-    return LINS_E_INVALID;
-  CK(cudaSetDevice(ctx->device));
-  MapperState& M = ctx->mapper;
-  lins_mapper_report r;
+bool mapper_cycle_begin(const MapperNode& m, MapperScalars& s, double timeLaserOdometry, const double quat[4], const double pos[3], lins_mapper_report& r) {
   std::memset(&r, 0, sizeof(r));
   r.loop_candidate = -1;
-  MapperScalars s = M.s;  // committed only when the cycle completes
-  const double timeLaserOdometry = d->time;
   {  // laserOdometryHandler :713-722
     double roll, pitch, yaw;
-    tf_get_rpy(d->quat[2], -d->quat[0], -d->quat[1], d->quat[3], roll, pitch, yaw);
+    tf_get_rpy(quat[2], -quat[0], -quat[1], quat[3], roll, pitch, yaw);
     s.transformSum[0] = -pitch; s.transformSum[1] = -yaw; s.transformSum[2] = roll;
-    s.transformSum[3] = d->pos[0]; s.transformSum[4] = d->pos[1]; s.transformSum[5] = d->pos[2];
+    s.transformSum[3] = pos[0]; s.transformSum[4] = pos[1]; s.transformSum[5] = pos[2];
   }
   if (!(timeLaserOdometry - s.timeLastProcessing >= 0.3)) {  // :1821 (the odometry still replaces transformSum)
     r.skipped_interval = 1;
-    r.n_keyframes = (int)M.poses.size();
+    r.n_keyframes = (int)m.poses.size();
     r.window_len = (int)s.window.size();
     for (int i = 0; i < 6; ++i) { r.transform_guess[i] = s.transformTobeMapped[i]; r.transform_aft_mapped[i] = s.transformAftMapped[i]; }
-    M.s = s;
-    if (rep) *rep = r;
-    return LINS_OK;
+    return false;
   }
   s.timeLastProcessing = timeLaserOdometry;
   transform_associate_to_map(s);
   for (int i = 0; i < 6; ++i) r.transform_guess[i] = s.transformTobeMapped[i];
-
   // extractSurroundingKeyFrames :1201-1246 (the deque of ids)
-  const int numPoses = (int)M.poses.size();
+  const int numPoses = (int)m.poses.size();
   if (numPoses > 0) {
     if ((int)s.window.size() < LINS_MAPPER_WINDOW) {
       s.window.clear();
@@ -433,94 +511,36 @@ int lins_gpu_mapper_step(lins_ctx* ctx, const lins_mapper_desc* d, lins_mapper_r
       s.window.push_back(s.latestFrameID);
     }
   }
-  // Everything up to the scan-to-map loop is queued without reading anything back: the VoxelGrids' outputs are sized
-  // by their inputs and filled with NaN past their counts, and the later stages take those capacities.  A NaN point is
-  // dropped by a VoxelGrid, is never a neighbour and never selects a query, and the block partials it leaves are zero,
-  // so the results equal those of the exact sizes.  The counts come back with the loop's state: one synchronisation.
-  const int n_in[3] = {d->n_corner, d->n_surf, d->n_outlier};
-  int n_cat[3] = {0, 0, d->n_surf + d->n_outlier};
-  for (int id : s.window) {
-    const MapperKeyFrame& kf = M.slots[M.slot_of.at(id)];
-    n_cat[0] += kf.n[0]; n_cat[1] += kf.n[1] + kf.n[2];
-  }
-  // every buffer of the cycle first (a growth frees memory queued work may still read)
-  const int n_max = std::max({n_cat[0], n_cat[1], n_cat[2]});
-  int rc = voxel_grid_reserve(ctx, n_max);
-  if (rc != LINS_OK) return rc;
-  CK(M.vg_info.reserve(kMapperGrids)); CK(M.h_vg_info.reserve(kMapperGrids));
-  for (int k = 0; k < 3; ++k) { CK(M.cat[k].reserve((size_t)n_cat[k] + 1)); CK(M.ds[k].reserve((size_t)n_in[k] + 1)); }
-  CK(M.ds[3].reserve((size_t)n_cat[2] + 1));
-  CK(M.map_ds[0].reserve((size_t)n_cat[0] + 1)); CK(M.map_ds[1].reserve((size_t)n_cat[1] + 1));
-  const size_t n_copies = 3 * s.window.size() + 2;
-  if ((rc = M.copies.reserve(ctx, n_copies)) != LINS_OK) return rc;
-  VgInfo* info = M.vg_info.p;
-  // the local map: corner_i ..., and surf_i, outlier_i interleaved (:1242-1246)
-  std::vector<DevCopy> copies;
-  {
-    int oc = 0, os = 0;
-    for (int id : s.window) {
-      const MapperKeyFrame& kf = M.slots[M.slot_of.at(id)];
-      copies.push_back(DevCopy{kf.c[0].p, M.cat[0].p + oc, kf.n[0], 0}); oc += kf.n[0];
-      copies.push_back(DevCopy{kf.c[1].p, M.cat[1].p + os, kf.n[1], 0}); os += kf.n[1];
-      copies.push_back(DevCopy{kf.c[2].p, M.cat[1].p + os, kf.n[2], 0}); os += kf.n[2];
-    }
-  }
-  if ((rc = queue_copies(ctx, copies, 0)) != LINS_OK) return rc;
-  const bool have_map = numPoses > 0;
-  if ((rc = voxel_grid_queue(ctx, M.cat[0].p, have_map ? n_cat[0] : 0, 0.2f, M.map_ds[0].p, info + 0)) != LINS_OK) return rc;
-  if ((rc = voxel_grid_queue(ctx, M.cat[1].p, have_map ? n_cat[1] : 0, 0.4f, M.map_ds[1].p, info + 1)) != LINS_OK) return rc;
-  // downsampleCurrentScan :1326-1349
-  if ((rc = upload3(ctx, d)) != LINS_OK) return rc;
-  const float leaf[3] = {0.2f, 0.4f, 0.4f};
-  for (int k = 0; k < 3; ++k)
-    if ((rc = voxel_grid_queue(ctx, M.in[k].p, n_in[k], leaf[k], M.ds[k].p, info + 2 + k)) != LINS_OK) return rc;
-  // laserCloudSurfTotalLast = surf DS + outlier DS: their NaN tails ride along and are dropped by the filter
-  copies.assign({DevCopy{M.ds[1].p, M.cat[2].p, n_in[1], 0}, DevCopy{M.ds[2].p, M.cat[2].p + n_in[1], n_in[2], 0}});
-  if ((rc = queue_copies(ctx, copies, (int)n_copies - 2)) != LINS_OK) return rc;
-  if ((rc = voxel_grid_queue(ctx, M.cat[2].p, n_cat[2], 0.4f, M.ds[3].p, info + 5)) != LINS_OK) return rc;
+  return true;
+}
 
-  // scan2MapOptimization :1635-1652: without key poses the map is empty and the gate fails on the host; otherwise the
-  // loop is queued on the capacities and a device-side gate on the two map counts stops it before its first pass
-  lins_ctx::MapState& mp = ctx->mp;
-  if (have_map) {
-    CK(mp.map_c.reserve((size_t)n_cat[0] + 1)); CK(mp.map_s.reserve((size_t)n_cat[1] + 1));
-    CK(mp.q_c.reserve((size_t)n_in[0] + 1)); CK(mp.q_s.reserve((size_t)n_cat[2] + 1));
-    if (n_cat[0]) CK(cudaMemcpyAsync(mp.map_c.p, M.map_ds[0].p, sizeof(float4) * n_cat[0], cudaMemcpyDeviceToDevice, ctx->stream));
-    if (n_cat[1]) CK(cudaMemcpyAsync(mp.map_s.p, M.map_ds[1].p, sizeof(float4) * n_cat[1], cudaMemcpyDeviceToDevice, ctx->stream));
-    if (n_in[0]) CK(cudaMemcpyAsync(mp.q_c.p, M.ds[0].p, sizeof(float4) * n_in[0], cudaMemcpyDeviceToDevice, ctx->stream));
-    if (n_cat[2]) CK(cudaMemcpyAsync(mp.q_s.p, M.ds[3].p, sizeof(float4) * n_cat[2], cudaMemcpyDeviceToDevice, ctx->stream));
-    // the grids hold the real points only (a NaN tail would crowd one bucket); the searches take the capacities
-    const float origin[3] = {0.f, 0.f, 0.f};  // (any finite origin gives the same 5-NN)
-    if ((rc = map_build_grid(ctx, mp.grid_c, mp.map_c.p, n_cat[0], origin, &info[0].count)) != LINS_OK) return rc;
-    if ((rc = map_build_grid(ctx, mp.grid_s, mp.map_s.p, n_cat[1], origin, &info[1].count)) != LINS_OK) return rc;
-    mp.n_map_c = n_cat[0]; mp.n_map_s = n_cat[1];
-    if ((rc = map_queue_loop(ctx, n_in[0], n_cat[2], s.transformTobeMapped, &info[0].count, &info[1].count)) != LINS_OK) return rc;
+void mapper_window_sizes(const MapperNode& m, const MapperScalars& s, int& n_corner, int& n_surf) {
+  n_corner = n_surf = 0;
+  for (int id : s.window) {
+    const MapperKeyFrame& kf = m.slots[m.slot_of.at(id)];
+    n_corner += kf.n[0]; n_surf += kf.n[1] + kf.n[2];
   }
-  CK(cudaMemcpyAsync(M.h_vg_info.p, info, sizeof(VgInfo) * kMapperGrids, cudaMemcpyDeviceToHost, ctx->stream));
-  CK(cudaStreamSynchronize(ctx->stream));  // the cycle's one read-back
-  M.last.valid = false;  // (a failed cycle has overwritten the previous one's clouds)
-  const VgInfo* hi = M.h_vg_info.p;
-  for (int i = 0; i < kMapperGrids; ++i)
-    if (hi[i].toobig) return fail(ctx, LINS_E_TOOBIG, "VoxelGrid: the leaf is too small for the cloud's extent (div_x * div_y * div_z > INT32_MAX)");
+}
+
+void mapper_cycle_end(MapperNode& M, MapperScalars& s, double timeLaserOdometry, double scan_period, const int cnt[6], const lins_map::MapLoopState* st,
+                      lins_mapper_report& r, KfSave* save, bool* saved) {
   // (without key poses the reference returns before the filters and keeps the previous sizes, which are 0 then)
-  const int nmc = have_map ? hi[0].count : 0, nms = have_map ? hi[1].count : 0;
-  const int ndc = hi[2].count, nds = hi[3].count, ndo = hi[4].count, ndt = hi[5].count;
-  if (have_map) { mp.n_map_c = nmc; mp.n_map_s = nms; }
-  if (nmc > 10 && nms > 100) {
-    map_loop_report(ctx, s.transformTobeMapped, &r.map);
-    transform_update(s, timeLaserOdometry, ctx->prm.scan_period);
+  const int nmc = cnt[0], nms = cnt[1], ndc = cnt[2], nds = cnt[3], ndo = cnt[4], ndt = cnt[5];
+  if (st) {
+    map_loop_report(*st, s.transformTobeMapped, &r.map);
+    transform_update(s, timeLaserOdometry, scan_period);
   } else {
     r.map.skipped = 1;
   }
-
+  *saved = false;
   // saveKeyFramesAndFactor :1654-1765
   const float cur[3] = {s.transformAftMapped[3], s.transformAftMapped[4], s.transformAftMapped[5]};  // currentRobotPosPoint
-  bool save = true;
+  bool save_kf = true;
   {
     const float dx = s.previousRobotPos[0] - cur[0], dy = s.previousRobotPos[1] - cur[1], dz = s.previousRobotPos[2] - cur[2];
-    if (std::sqrt(dx * dx + dy * dy + dz * dz) < 0.3) save = false;
+    if (std::sqrt(dx * dx + dy * dy + dz * dz) < 0.3) save_kf = false;
   }
-  if (save || M.poses.empty()) {
+  if (save_kf || M.poses.empty()) {
     for (int k = 0; k < 3; ++k) s.previousRobotPos[k] = cur[k];
     // the pose inserted into iSAM2, and (no loop factor: DESIGN.md §4.9) its estimate
     const float* P = M.poses.empty() ? s.transformTobeMapped : s.transformAftMapped;
@@ -542,17 +562,10 @@ int lins_gpu_mapper_step(lins_ctx* ctx, const lins_mapper_desc* d, lins_mapper_r
     }
     // the key frame's clouds, in the map frame once (its pose never changes without a loop closure)
     MapperKeyFrame& kf = keyframe_slot(M, id);
-    const int nk[3] = {ndc, nds, ndo};
-    const TfConsts tc = tf_consts(kp);
-    for (int k = 0; k < 3; ++k) {
-      CK(kf.c[k].reserve((size_t)nk[k] + 1));
-      kf.n[k] = nk[k];
-      if (nk[k]) {
-        lins_mapper_transform_kernel<<<(nk[k] + 255) / 256, 256, 0, ctx->stream>>>(M.ds[k].p, kf.c[k].p, nk[k], tc);
-        CK(cudaGetLastError());
-        ctx->launches += 1;
-      }
-    }
+    kf.n[0] = ndc; kf.n[1] = nds; kf.n[2] = ndo;
+    save->kf = &kf;
+    save->kp = kp;
+    *saved = true;
     r.keyframe_saved = 1;
     // detectLoopClosure's candidate (:1050-1064): radius 5 m around currentRobotPosPoint, nearest first, |dt| > 30 s
     float best = 0.f;
@@ -572,13 +585,139 @@ int lins_gpu_mapper_step(lins_ctx* ctx, const lins_mapper_desc* d, lins_mapper_r
   }
   M.s = s;
   M.last.valid = true;
-  M.last.n[0] = nmc; M.last.n[1] = nms; M.last.n[2] = ndc; M.last.n[3] = nds; M.last.n[4] = ndo; M.last.n[5] = ndt;
+  for (int k = 0; k < 6; ++k) M.last.n[k] = cnt[k];
   r.processed = 1;
   r.n_map_corner_ds = nmc; r.n_map_surf_ds = nms;
   r.n_corner_ds = ndc; r.n_surf_ds = nds; r.n_outlier_ds = ndo; r.n_surf_total_ds = ndt;
   r.n_keyframes = (int)M.poses.size();
   r.window_len = (int)s.window.size();
   for (int i = 0; i < 6; ++i) r.transform_aft_mapped[i] = s.transformAftMapped[i];
+}
+
+int mapper_node_download(lins_ctx* ctx, const MapperNode& M, const float4* const src[6], double* key_poses, int32_t* window, float* const dst[6]) {
+  if (key_poses)
+    for (size_t i = 0; i < M.poses.size(); ++i) {
+      const MapperKeyPose& k = M.poses[i];
+      const double v[7] = {k.x, k.y, k.z, k.roll, k.pitch, k.yaw, k.time};
+      std::memcpy(key_poses + 7 * i, v, sizeof(v));
+    }
+  if (window) { int i = 0; for (int id : M.s.window) window[i++] = id; }
+  for (int k = 0; k < 6 && M.last.valid; ++k) CK(d2h(ctx, dst[k], src[k], sizeof(float4) * M.last.n[k]));
+  CK(cudaStreamSynchronize(ctx->stream));
+  return LINS_OK;
+}
+
+}  // namespace lins_capi
+
+extern "C" {
+
+int lins_gpu_mapper_reset(lins_ctx* ctx) {
+  if (!ctx) return LINS_E_INVALID;
+  CK(cudaSetDevice(ctx->device));
+  mapper_node_reset(ctx->mapper.n);
+  return map_reset_loop(ctx);  // isDegenerate, matP
+}
+
+int lins_gpu_mapper_imu(lins_ctx* ctx, const double* time, const double* roll, const double* pitch, int n) {
+  if (!ctx) return LINS_E_INVALID;
+  if (n < 0 || (n > 0 && (!time || !roll || !pitch))) return fail(ctx, LINS_E_INVALID, "bad IMU arrays");
+  mapper_node_imu(ctx->mapper.n.s, time, roll, pitch, n);
+  return LINS_OK;
+}
+
+int lins_gpu_mapper_step(lins_ctx* ctx, const lins_mapper_desc* d, lins_mapper_report* rep) {
+  if (!ctx) return LINS_E_INVALID;
+  if (!d) return fail(ctx, LINS_E_INVALID, "null desc");
+  if (check_cloud(ctx, d->corner, d->n_corner, "bad mapper corner cloud") != LINS_OK || check_cloud(ctx, d->surf, d->n_surf, "bad mapper surf cloud") != LINS_OK ||
+      check_cloud(ctx, d->outlier, d->n_outlier, "bad mapper outlier cloud") != LINS_OK)
+    return LINS_E_INVALID;
+  CK(cudaSetDevice(ctx->device));
+  MapperState& M = ctx->mapper;
+  lins_mapper_report r;
+  MapperScalars s = M.n.s;  // committed only when the cycle completes
+  const double timeLaserOdometry = d->time;
+  if (!mapper_cycle_begin(M.n, s, timeLaserOdometry, d->quat, d->pos, r)) {
+    M.n.s = s;
+    if (rep) *rep = r;
+    return LINS_OK;
+  }
+  const int numPoses = (int)M.n.poses.size();
+  // Everything up to the scan-to-map loop is queued without reading anything back: the VoxelGrids' outputs are sized
+  // by their inputs and filled with NaN past their counts, and the later stages take those capacities.  A NaN point is
+  // dropped by a VoxelGrid, is never a neighbour and never selects a query, and the block partials it leaves are zero,
+  // so the results equal those of the exact sizes.  The counts come back with the loop's state: one synchronisation.
+  const int n_in[3] = {d->n_corner, d->n_surf, d->n_outlier};
+  int n_cat[3] = {0, 0, d->n_surf + d->n_outlier};
+  mapper_window_sizes(M.n, s, n_cat[0], n_cat[1]);
+  // every buffer of the cycle first (a growth frees memory queued work may still read)
+  const int n_max = std::max({n_cat[0], n_cat[1], n_cat[2]});
+  int rc = voxel_grid_reserve(ctx, M.vg, n_max, 1);
+  if (rc != LINS_OK) return rc;
+  CK(M.vg_info.reserve(kMapperGrids)); CK(M.h_vg_info.reserve(kMapperGrids));
+  for (int k = 0; k < 3; ++k) { CK(M.cat[k].reserve((size_t)n_cat[k] + 1)); CK(M.ds[k].reserve((size_t)n_in[k] + 1)); }
+  CK(M.ds[3].reserve((size_t)n_cat[2] + 1));
+  CK(M.map_ds[0].reserve((size_t)n_cat[0] + 1)); CK(M.map_ds[1].reserve((size_t)n_cat[1] + 1));
+  const size_t n_copies = 3 * s.window.size() + 2;
+  if ((rc = M.copies.reserve(ctx, n_copies)) != LINS_OK) return rc;
+  VgInfo* info = M.vg_info.p;
+  // the local map: corner_i ..., and surf_i, outlier_i interleaved (:1242-1246)
+  std::vector<DevCopy> copies;
+  {
+    int oc = 0, os = 0;
+    for (int id : s.window) {
+      const MapperKeyFrame& kf = M.n.slots[M.n.slot_of.at(id)];
+      copies.push_back(DevCopy{kf.c[0].p, M.cat[0].p + oc, kf.n[0], 0}); oc += kf.n[0];
+      copies.push_back(DevCopy{kf.c[1].p, M.cat[1].p + os, kf.n[1], 0}); os += kf.n[1];
+      copies.push_back(DevCopy{kf.c[2].p, M.cat[1].p + os, kf.n[2], 0}); os += kf.n[2];
+    }
+  }
+  if ((rc = queue_copies(ctx, M.copies, copies, 0)) != LINS_OK) return rc;
+  const bool have_map = numPoses > 0;
+  if ((rc = voxel_grid_one(ctx, M.cat[0].p, have_map ? n_cat[0] : 0, 0.2f, M.map_ds[0].p, info + 0)) != LINS_OK) return rc;
+  if ((rc = voxel_grid_one(ctx, M.cat[1].p, have_map ? n_cat[1] : 0, 0.4f, M.map_ds[1].p, info + 1)) != LINS_OK) return rc;
+  // downsampleCurrentScan :1326-1349
+  if ((rc = upload3(ctx, d)) != LINS_OK) return rc;
+  const float leaf[3] = {0.2f, 0.4f, 0.4f};
+  for (int k = 0; k < 3; ++k)
+    if ((rc = voxel_grid_one(ctx, M.in[k].p, n_in[k], leaf[k], M.ds[k].p, info + 2 + k)) != LINS_OK) return rc;
+  // laserCloudSurfTotalLast = surf DS + outlier DS: their NaN tails ride along and are dropped by the filter
+  copies.assign({DevCopy{M.ds[1].p, M.cat[2].p, n_in[1], 0}, DevCopy{M.ds[2].p, M.cat[2].p + n_in[1], n_in[2], 0}});
+  if ((rc = queue_copies(ctx, M.copies, copies, (int)n_copies - 2)) != LINS_OK) return rc;
+  if ((rc = voxel_grid_one(ctx, M.cat[2].p, n_cat[2], 0.4f, M.ds[3].p, info + 5)) != LINS_OK) return rc;
+
+  // scan2MapOptimization :1635-1652: without key poses the map is empty and the gate fails on the host; otherwise the
+  // loop is queued on the capacities and a device-side gate on the two map counts stops it before its first pass
+  lins_ctx::MapState& mp = ctx->mp;
+  if (have_map) {
+    CK(mp.map_c.reserve((size_t)n_cat[0] + 1)); CK(mp.map_s.reserve((size_t)n_cat[1] + 1));
+    CK(mp.q_c.reserve((size_t)n_in[0] + 1)); CK(mp.q_s.reserve((size_t)n_cat[2] + 1));
+    if (n_cat[0]) CK(cudaMemcpyAsync(mp.map_c.p, M.map_ds[0].p, sizeof(float4) * n_cat[0], cudaMemcpyDeviceToDevice, ctx->stream));
+    if (n_cat[1]) CK(cudaMemcpyAsync(mp.map_s.p, M.map_ds[1].p, sizeof(float4) * n_cat[1], cudaMemcpyDeviceToDevice, ctx->stream));
+    if (n_in[0]) CK(cudaMemcpyAsync(mp.q_c.p, M.ds[0].p, sizeof(float4) * n_in[0], cudaMemcpyDeviceToDevice, ctx->stream));
+    if (n_cat[2]) CK(cudaMemcpyAsync(mp.q_s.p, M.ds[3].p, sizeof(float4) * n_cat[2], cudaMemcpyDeviceToDevice, ctx->stream));
+    // the grids hold the real points only (a NaN tail would crowd one bucket); the searches take the capacities
+    const float origin[3] = {0.f, 0.f, 0.f};  // (any finite origin gives the same 5-NN)
+    if ((rc = map_build_grid(ctx, mp.grid_c, mp.map_c.p, n_cat[0], origin, &info[0].count)) != LINS_OK) return rc;
+    if ((rc = map_build_grid(ctx, mp.grid_s, mp.map_s.p, n_cat[1], origin, &info[1].count)) != LINS_OK) return rc;
+    mp.n_map_c = n_cat[0]; mp.n_map_s = n_cat[1];
+    if ((rc = map_queue_loop(ctx, n_in[0], n_cat[2], s.transformTobeMapped, &info[0].count, &info[1].count)) != LINS_OK) return rc;
+  }
+  CK(cudaMemcpyAsync(M.h_vg_info.p, info, sizeof(VgInfo) * kMapperGrids, cudaMemcpyDeviceToHost, ctx->stream));
+  CK(cudaStreamSynchronize(ctx->stream));  // the cycle's one read-back
+  M.n.last.valid = false;  // (a failed cycle has overwritten the previous one's clouds)
+  const VgInfo* hi = M.h_vg_info.p;
+  for (int i = 0; i < kMapperGrids; ++i)
+    if (hi[i].toobig) return fail(ctx, LINS_E_TOOBIG, "VoxelGrid: the leaf is too small for the cloud's extent (div_x * div_y * div_z > INT32_MAX)");
+  const int cnt[6] = {have_map ? hi[0].count : 0, have_map ? hi[1].count : 0, hi[2].count, hi[3].count, hi[4].count, hi[5].count};
+  if (have_map) { mp.n_map_c = cnt[0]; mp.n_map_s = cnt[1]; }
+  const bool gate = cnt[0] > 10 && cnt[1] > 100;
+  KfSave sv;
+  bool saved = false;
+  mapper_cycle_end(M.n, s, timeLaserOdometry, ctx->prm.scan_period, cnt, gate ? ctx->mp.h_loop.p : nullptr, r, &sv, &saved);
+  if (saved) {
+    for (int k = 0; k < 3; ++k) sv.ds[k] = M.ds[k].p;
+    if ((rc = keyframes_queue(ctx, &sv, 1, M.tf, M.h_tf)) != LINS_OK) return rc;
+  }
   if (rep) *rep = r;
   return LINS_OK;
 }
@@ -588,18 +727,9 @@ int lins_gpu_mapper_download(lins_ctx* ctx, double* key_poses, int32_t* window, 
   if (!ctx) return LINS_E_INVALID;
   CK(cudaSetDevice(ctx->device));
   MapperState& M = ctx->mapper;
-  if (key_poses)
-    for (size_t i = 0; i < M.poses.size(); ++i) {
-      const MapperKeyPose& k = M.poses[i];
-      const double v[7] = {k.x, k.y, k.z, k.roll, k.pitch, k.yaw, k.time};
-      std::memcpy(key_poses + 7 * i, v, sizeof(v));
-    }
-  if (window) { int i = 0; for (int id : M.s.window) window[i++] = id; }
   float* dst[6] = {map_corner_ds, map_surf_ds, corner_ds, surf_ds, outlier_ds, surf_total_ds};
   const float4* src[6] = {M.map_ds[0].p, M.map_ds[1].p, M.ds[0].p, M.ds[1].p, M.ds[2].p, M.ds[3].p};
-  for (int k = 0; k < 6 && M.last.valid; ++k) CK(d2h(ctx, dst[k], src[k], sizeof(float4) * M.last.n[k]));
-  CK(cudaStreamSynchronize(ctx->stream));
-  return LINS_OK;
+  return mapper_node_download(ctx, M.n, src, key_poses, window, dst);
 }
 
 int lins_gpu_voxel_grid(lins_ctx* ctx, const lins_point* in, int n, float leaf, float* out, int* n_out) {
@@ -614,7 +744,7 @@ int lins_gpu_voxel_grid(lins_ctx* ctx, const lins_point* in, int n, float leaf, 
   CK(M.h_in.reserve((size_t)n + 1));
   pack_into(M.h_in.p, in, n);
   if (n) CK(cudaMemcpyAsync(M.vg_in.p, M.h_in.p, sizeof(float4) * n, cudaMemcpyHostToDevice, ctx->stream));
-  int rc = voxel_grid_queue(ctx, M.vg_in.p, n, leaf, M.vg_out.p, M.vg_info.p);
+  int rc = voxel_grid_one(ctx, M.vg_in.p, n, leaf, M.vg_out.p, M.vg_info.p);
   if (rc != LINS_OK) return rc;
   CK(M.h_vg_info.reserve(kMapperGrids));
   CK(cudaMemcpyAsync(M.h_vg_info.p, M.vg_info.p, sizeof(VgInfo), cudaMemcpyDeviceToHost, ctx->stream));

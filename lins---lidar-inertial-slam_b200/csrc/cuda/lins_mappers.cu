@@ -1,0 +1,249 @@
+// lins_mappers.cu — the mapping node's cycle for many drives in lockstep (lins_gpu_mappers_*): one MapperNode per slot,
+// each stepped by the host logic of lins_mapper.cu, with one queue of device work per step for every processed slot.
+//
+// Per step (one synchronisation): the scans of the processed slots in one H2D; one gather launch of every slot's window
+// into its local-map clouds; one segmented VoxelGrid over the five clouds of every slot (map corner 0.2 m, map surf
+// 0.4 m, corner 0.2 m, surf 0.4 m, outlier 0.4 m), one gather of each slot's surf DS + outlier DS and one segmented
+// VoxelGrid of those (0.4 m); every slot's grids and scan-to-map loop (lins_map.cu: map_queue_slots); the read-back of
+// the VoxelGrid records and loop states.  After it, the host tail of each slot and one transform launch for every key
+// frame saved.  The segments of a VoxelGrid keep their input ranges and each slot's fit blocks cover its own queries
+// only, so every slot's clouds, sums and steps are those of a lins_gpu_mapper_step on a context of its own.
+#include <cuda_runtime.h>
+
+#include <algorithm>
+#include <cstdint>
+#include <cstring>
+#include <vector>
+
+#include "lins_ctx.hpp"
+#include "lins_map_types.cuh"
+
+using namespace lins_capi;
+
+namespace {
+
+int need_open(lins_ctx* ctx) {
+  return ctx->mappers.n > 0 ? LINS_OK : fail(ctx, LINS_E_NOMAP, "lins_gpu_mappers_open has not been called");
+}
+
+const char* const kBad = "VoxelGrid: the leaf is too small for the cloud's extent (div_x * div_y * div_z > INT32_MAX)";
+
+}  // namespace
+
+extern "C" {
+
+int lins_gpu_mappers_open(lins_ctx* ctx, int32_t n_slots) {
+  if (!ctx) return LINS_E_INVALID;
+  if (n_slots < 1) return fail(ctx, LINS_E_INVALID, "n_slots < 1");
+  CK(cudaSetDevice(ctx->device));
+  MappersState& ms = ctx->mappers;
+  ms.n = 0;
+  ms.node = std::vector<MapperNode>(n_slots);  // (constructed in place: a node is not copyable)
+  ms.ds = std::vector<std::array<Buf<float4>, 6>>(n_slots);
+  CK(ms.loop.reserve(n_slots)); CK(ms.h_loop.reserve(n_slots)); CK(ms.h_mslot.reserve(n_slots));
+  CK(cudaMemsetAsync(ms.loop.p, 0, sizeof(lins_map::MapLoopState) * n_slots, ctx->stream));  // matP, isDegenerate
+  ms.n = n_slots;
+  return LINS_OK;
+}
+
+int lins_gpu_mappers_reset(lins_ctx* ctx, const uint8_t* mask) {
+  if (!ctx) return LINS_E_INVALID;
+  if (need_open(ctx) != LINS_OK) return LINS_E_NOMAP;
+  if (!mask) return fail(ctx, LINS_E_INVALID, "null mask");
+  CK(cudaSetDevice(ctx->device));
+  MappersState& ms = ctx->mappers;
+  for (int s = 0; s < ms.n; ++s)
+    if (mask[s]) {
+      mapper_node_reset(ms.node[s]);
+      CK(cudaMemsetAsync(ms.loop.p + s, 0, sizeof(lins_map::MapLoopState), ctx->stream));
+    }
+  return LINS_OK;
+}
+
+int lins_gpu_mappers_imu(lins_ctx* ctx, const int32_t* off, const double* time, const double* roll, const double* pitch) {
+  if (!ctx) return LINS_E_INVALID;
+  if (need_open(ctx) != LINS_OK) return LINS_E_NOMAP;
+  MappersState& ms = ctx->mappers;
+  if (check_csr(ctx, off, ms.n, time, "bad IMU offsets / arrays") != LINS_OK) return LINS_E_INVALID;
+  if (off[ms.n] > 0 && (!roll || !pitch)) return fail(ctx, LINS_E_INVALID, "bad IMU offsets / arrays");
+  for (int s = 0; s < ms.n; ++s) mapper_node_imu(ms.node[s].s, time + off[s], roll + off[s], pitch + off[s], off[s + 1] - off[s]);
+  return LINS_OK;
+}
+
+int lins_gpu_mappers_step(lins_ctx* ctx, const lins_mappers_desc* d, lins_mapper_report* reps) {
+  if (!ctx) return LINS_E_INVALID;
+  if (!d) return fail(ctx, LINS_E_INVALID, "null desc");
+  if (need_open(ctx) != LINS_OK) return LINS_E_NOMAP;
+  MappersState& ms = ctx->mappers;
+  const int M = ms.n;
+  if (d->n_slots != M) return fail(ctx, LINS_E_INVALID, "n_slots differs from the open run's");
+  if (!d->time || !d->quat || !d->pos) return fail(ctx, LINS_E_INVALID, "null time / quat / pos");
+  const lins_point* src[3] = {d->corner, d->surf, d->outlier};
+  const int32_t* off[3] = {d->corner_off, d->surf_off, d->outlier_off};
+  static const char* const what[3] = {"bad corner offsets / cloud", "bad surf offsets / cloud", "bad outlier offsets / cloud"};
+  for (int k = 0; k < 3; ++k) if (check_csr(ctx, off[k], M, src[k], what[k]) != LINS_OK) return LINS_E_INVALID;
+  CK(cudaSetDevice(ctx->device));
+
+  // the host head of every present slot's cycle, on copies of its scalars (committed after the read-back)
+  std::vector<MapperScalars> sc(M);
+  std::vector<lins_mapper_report> rr(M);
+  std::vector<int> proc, skipped;  // processed slots; interval-skipped slots
+  for (int s = 0; s < M; ++s) {
+    if (d->present && !d->present[s]) continue;
+    sc[s] = ms.node[s].s;
+    (mapper_cycle_begin(ms.node[s], sc[s], d->time[s], d->quat + 4 * s, d->pos + 3 * s, rr[s]) ? proc : skipped).push_back(s);
+  }
+  const int P = (int)proc.size();
+  auto finish = [&]() {
+    for (int s : skipped) ms.node[s].s = sc[s];
+    if (reps) for (int s = 0; s < M; ++s) if (!d->present || d->present[s]) reps[s] = rr[s];
+    return LINS_OK;
+  };
+  if (P == 0) return finish();
+
+  // round 1: segment 3p + k = scan cloud k of processed slot p (one H2D), 3P + 2p + k = its local map k; round 2:
+  // segment p = its surf DS + outlier DS.  Every capacity is known here: the outputs are sized by the inputs.
+  std::vector<int> h_off1(5 * P + 1), h_off2(P + 1), mapc(2 * P);
+  std::vector<float> leaf1(5 * P), leaf2(P, 0.4f);
+  std::vector<float4*> out(6 * P);
+  int n_scan = 0;
+  for (int p = 0; p < P; ++p) {
+    const int s = proc[p];
+    for (int k = 0; k < 3; ++k) { h_off1[3 * p + k] = n_scan; n_scan += off[k][s + 1] - off[k][s]; leaf1[3 * p + k] = k == 0 ? 0.2f : 0.4f; }
+    int nc = 0, nsf = 0;
+    if (!ms.node[s].poses.empty()) mapper_window_sizes(ms.node[s], sc[s], nc, nsf);
+    mapc[2 * p] = nc; mapc[2 * p + 1] = nsf;
+  }
+  int n1 = n_scan;
+  for (int p = 0; p < P; ++p)
+    for (int k = 0; k < 2; ++k) { h_off1[3 * P + 2 * p + k] = n1; n1 += mapc[2 * p + k]; leaf1[3 * P + 2 * p + k] = k == 0 ? 0.2f : 0.4f; }
+  h_off1[5 * P] = n1;
+  int n2 = 0;
+  for (int p = 0; p < P; ++p) { h_off2[p] = n2; n2 += (h_off1[3 * p + 3] - h_off1[3 * p + 1]); }
+  h_off2[P] = n2;
+
+  // every buffer of the step first (a growth frees memory queued work may still read)
+  int rc;
+  if ((rc = voxel_grid_reserve(ctx, ms.vg, std::max(n1, n2), 5 * P)) != LINS_OK) return rc;
+  if ((rc = voxel_grid_reserve(ctx, ms.vg, std::max(n1, n2), P)) != LINS_OK) return rc;
+  CK(ms.vin[0].grow((size_t)n1 + 1)); CK(ms.vin[1].grow((size_t)n2 + 1)); CK(ms.h_in.grow((size_t)n_scan + 1));
+  CK(ms.vg_info.reserve(6 * (size_t)P)); CK(ms.h_vg_info.reserve(6 * (size_t)P)); CK(ms.h_vg_init.reserve(6 * (size_t)P));
+  CK(ms.vg_off.reserve(6 * (size_t)P + 2)); CK(ms.h_vg_off.reserve(6 * (size_t)P + 2));
+  CK(ms.vg_out.reserve(6 * (size_t)P)); CK(ms.h_vg_out.reserve(6 * (size_t)P));
+  size_t n_copies = 2 * (size_t)P;
+  for (int p = 0; p < P; ++p) {
+    const int s = proc[p];
+    auto& ds = ms.ds[s];
+    const int cap[6] = {mapc[2 * p], mapc[2 * p + 1], h_off1[3 * p + 1] - h_off1[3 * p], h_off1[3 * p + 2] - h_off1[3 * p + 1],
+                        h_off1[3 * p + 3] - h_off1[3 * p + 2], h_off2[p + 1] - h_off2[p]};
+    for (int k = 0; k < 6; ++k) CK(ds[k].grow((size_t)cap[k] + 1));
+    out[3 * p + 0] = ds[2].p; out[3 * p + 1] = ds[3].p; out[3 * p + 2] = ds[4].p;
+    out[3 * P + 2 * p] = ds[0].p; out[3 * P + 2 * p + 1] = ds[1].p;
+    out[5 * P + p] = ds[5].p;
+    if (!ms.node[s].poses.empty()) n_copies += 3 * sc[s].window.size();
+  }
+  if ((rc = ms.copies.reserve(ctx, n_copies)) != LINS_OK) return rc;
+
+  // the scans (one H2D) and the segment tables (outputs: the slots' own DS clouds, which persist for the download)
+  {
+    size_t o = 0;
+    for (int p = 0; p < P; ++p)
+      for (int k = 0; k < 3; ++k) {
+        const int s = proc[p], n = off[k][s + 1] - off[k][s];
+        pack_into(ms.h_in.p + o, src[k] + off[k][s], n);
+        o += n;
+      }
+    if (n_scan) CK(cudaMemcpyAsync(ms.vin[0].p, ms.h_in.p, sizeof(float4) * n_scan, cudaMemcpyHostToDevice, ctx->stream));
+  }
+  std::copy(h_off1.begin(), h_off1.end(), ms.h_vg_off.p);
+  std::copy(h_off2.begin(), h_off2.end(), ms.h_vg_off.p + 5 * P + 1);
+  std::copy(out.begin(), out.end(), ms.h_vg_out.p);
+  CK(cudaMemcpyAsync(ms.vg_off.p, ms.h_vg_off.p, sizeof(int) * (6 * (size_t)P + 2), cudaMemcpyHostToDevice, ctx->stream));
+  CK(cudaMemcpyAsync(ms.vg_out.p, ms.h_vg_out.p, sizeof(float4*) * 6 * (size_t)P, cudaMemcpyHostToDevice, ctx->stream));
+
+  // every slot's local map: corner_i ..., and surf_i, outlier_i interleaved (:1242-1246), one gather launch
+  std::vector<DevCopy> copies;
+  for (int p = 0; p < P; ++p) {
+    const MapperNode& m = ms.node[proc[p]];
+    if (m.poses.empty()) continue;
+    float4* oc = ms.vin[0].p + h_off1[3 * P + 2 * p];
+    float4* os = ms.vin[0].p + h_off1[3 * P + 2 * p + 1];
+    for (int id : sc[proc[p]].window) {
+      const MapperKeyFrame& kf = m.slots[m.slot_of.at(id)];
+      copies.push_back(DevCopy{kf.c[0].p, oc, kf.n[0], 0}); oc += kf.n[0];
+      copies.push_back(DevCopy{kf.c[1].p, os, kf.n[1], 0}); os += kf.n[1];
+      copies.push_back(DevCopy{kf.c[2].p, os, kf.n[2], 0}); os += kf.n[2];
+    }
+  }
+  if ((rc = queue_copies(ctx, ms.copies, copies, 0)) != LINS_OK) return rc;
+  VgInfo* info = ms.vg_info.p;
+  if ((rc = voxel_grid_queue(ctx, ms.vg, ms.vin[0].p, 5 * P, h_off1.data(), ms.vg_off.p, leaf1.data(), nullptr, ms.vg_out.p, ms.h_vg_init.p,
+                             info)) != LINS_OK)
+    return rc;
+  // laserCloudSurfTotalLast = surf DS + outlier DS: their NaN tails ride along and are dropped by the filter
+  copies.clear();
+  for (int p = 0; p < P; ++p) {
+    const int s = proc[p], ns = h_off1[3 * p + 2] - h_off1[3 * p + 1], no = h_off1[3 * p + 3] - h_off1[3 * p + 2];
+    copies.push_back(DevCopy{ms.ds[s][3].p, ms.vin[1].p + h_off2[p], ns, 0});
+    copies.push_back(DevCopy{ms.ds[s][4].p, ms.vin[1].p + h_off2[p] + ns, no, 0});
+  }
+  if ((rc = queue_copies(ctx, ms.copies, copies, (int)(n_copies - 2 * P))) != LINS_OK) return rc;
+  if ((rc = voxel_grid_queue(ctx, ms.vg, ms.vin[1].p, P, h_off2.data(), ms.vg_off.p + 5 * P + 1, leaf2.data(), out[5 * P],
+                             ms.vg_out.p + 5 * P, ms.h_vg_init.p + 5 * P, info + 5 * P)) != LINS_OK)
+    return rc;
+
+  // scan2MapOptimization of every slot with key frames (a slot without runs no pass, like the single mapper's host gate)
+  bool any_map = false;
+  for (int s = 0; s < M; ++s) std::memset(&ms.h_mslot.p[s], 0, sizeof(lins_map::MapSlot));
+  for (int p = 0; p < P; ++p) {
+    const int s = proc[p];
+    if (ms.node[s].poses.empty()) continue;
+    lins_map::MapSlot& v = ms.h_mslot.p[s];
+    v.run = 1; any_map = true;
+    for (int k = 0; k < 2; ++k) { v.map[k] = ms.ds[s][k].p; v.cap[k] = mapc[2 * p + k]; v.n_map[k] = &info[3 * P + 2 * p + k].count; }
+    v.q[0] = ms.ds[s][2].p; v.nq[0] = h_off1[3 * p + 1] - h_off1[3 * p];
+    v.q[1] = ms.ds[s][5].p; v.nq[1] = h_off2[p + 1] - h_off2[p];
+    for (int i = 0; i < 6; ++i) v.T[i] = sc[s].transformTobeMapped[i];
+  }
+  if (any_map && (rc = map_queue_slots(ctx, ms, M)) != LINS_OK) return rc;
+  CK(cudaMemcpyAsync(ms.h_vg_info.p, info, sizeof(VgInfo) * 6 * (size_t)P, cudaMemcpyDeviceToHost, ctx->stream));
+  CK(cudaStreamSynchronize(ctx->stream));  // the step's one read-back
+  for (int s : proc) ms.node[s].last.valid = false;  // (a failed step has overwritten their previous clouds)
+  const VgInfo* hi = ms.h_vg_info.p;
+  for (int i = 0; i < 6 * P; ++i)
+    if (hi[i].toobig) return fail(ctx, LINS_E_TOOBIG, kBad);
+
+  // the host tail of every processed slot, then one transform launch for the key frames saved
+  std::vector<KfSave> saves;
+  for (int p = 0; p < P; ++p) {
+    const int s = proc[p];
+    const bool have_map = !ms.node[s].poses.empty();
+    const int cnt[6] = {have_map ? hi[3 * P + 2 * p].count : 0, have_map ? hi[3 * P + 2 * p + 1].count : 0, hi[3 * p].count, hi[3 * p + 1].count,
+                        hi[3 * p + 2].count, hi[5 * P + p].count};
+    const bool gate = cnt[0] > 10 && cnt[1] > 100;
+    KfSave sv;
+    bool saved = false;
+    mapper_cycle_end(ms.node[s], sc[s], d->time[s], ctx->prm.scan_period, cnt, gate ? &ms.h_loop.p[s] : nullptr, rr[s], &sv, &saved);
+    if (saved) {
+      for (int k = 0; k < 3; ++k) sv.ds[k] = ms.ds[s][2 + k].p;
+      saves.push_back(sv);
+    }
+  }
+  if ((rc = keyframes_queue(ctx, saves.data(), (int)saves.size(), ms.tf, ms.h_tf)) != LINS_OK) return rc;
+  return finish();
+}
+
+int lins_gpu_mappers_download(lins_ctx* ctx, int32_t slot, double* key_poses, int32_t* window, float* map_corner_ds, float* map_surf_ds,
+                              float* corner_ds, float* surf_ds, float* outlier_ds, float* surf_total_ds) {
+  if (!ctx) return LINS_E_INVALID;
+  if (need_open(ctx) != LINS_OK) return LINS_E_NOMAP;
+  MappersState& ms = ctx->mappers;
+  if (slot < 0 || slot >= ms.n) return fail(ctx, LINS_E_INVALID, "slot out of range");
+  CK(cudaSetDevice(ctx->device));
+  float* const dst[6] = {map_corner_ds, map_surf_ds, corner_ds, surf_ds, outlier_ds, surf_total_ds};
+  const float4* src[6];
+  for (int k = 0; k < 6; ++k) src[k] = ms.ds[slot][k].p;
+  return mapper_node_download(ctx, ms.node[slot], src, key_poses, window, dst);
+}
+
+}  // extern "C"

@@ -67,6 +67,13 @@ class LinsMapperDesc(C.Structure):
                 ("n_outlier", C.c_int32), ("pad", C.c_int32)]
 
 
+class LinsMappersDesc(C.Structure):
+    """lins_mappers_desc (include/lins_gpu.h): one lockstep step of M mapper slots (CSR clouds as lins_batch_desc)."""
+    _fields_ = [("n_slots", C.c_int32), ("pad", C.c_int32), ("present", C.c_void_p), ("time", C.c_void_p), ("quat", C.c_void_p),
+                ("pos", C.c_void_p), ("corner", C.c_void_p), ("corner_off", C.c_void_p), ("surf", C.c_void_p), ("surf_off", C.c_void_p),
+                ("outlier", C.c_void_p), ("outlier_off", C.c_void_p)]
+
+
 class LinsMapperReport(C.Structure):
     """lins_mapper_report (include/lins_gpu.h)."""
     _fields_ = [("processed", C.c_int32), ("skipped_interval", C.c_int32), ("n_map_corner_ds", C.c_int32),

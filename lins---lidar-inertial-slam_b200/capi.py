@@ -350,12 +350,16 @@ class LinsGpu:
         """Key poses (n x 7: x, y, z, roll, pitch, yaw, time), the window's ids, and the last processed cycle's clouds
         ((n, 4) float32: map_corner_ds, map_surf_ds, corner_ds, surf_ds, outlier_ds, surf_total_ds) whose sizes `rep`,
         that cycle's report, gives."""
+        return self._download_node(lambda *out: self.L.lins_gpu_mapper_download(self.h, *out), rep)
+
+    def _download_node(self, call, rep):
+        """A mapping node's download through call(key_poses, window, six clouds), sized by its last cycle's report."""
         poses = np.zeros((rep.n_keyframes, 7))
         window = np.zeros(rep.window_len, np.int32)
         names = ("map_corner_ds", "map_surf_ds", "corner_ds", "surf_ds", "outlier_ds", "surf_total_ds")
         sizes = (rep.n_map_corner_ds, rep.n_map_surf_ds, rep.n_corner_ds, rep.n_surf_ds, rep.n_outlier_ds, rep.n_surf_total_ds)
         clouds = {k: np.zeros((n, 4), np.float32) for k, n in zip(names, sizes)}
-        self._ck(self.L.lins_gpu_mapper_download(self.h, ptr(poses), ptr(window), *[ptr(clouds[k]) for k in names]))
+        self._ck(call(ptr(poses), ptr(window), *[ptr(clouds[k]) for k in names]))
         return poses, window, clouds
 
     def voxel_grid(self, cloud, leaf):
@@ -402,13 +406,7 @@ class LinsGpu:
 
     def mappers_download(self, slot, rep):
         """mapper_download of one slot: (key poses, window, clouds) with the sizes its last processed cycle's report gives."""
-        poses = np.zeros((rep.n_keyframes, 7))
-        window = np.zeros(rep.window_len, np.int32)
-        names = ("map_corner_ds", "map_surf_ds", "corner_ds", "surf_ds", "outlier_ds", "surf_total_ds")
-        sizes = (rep.n_map_corner_ds, rep.n_map_surf_ds, rep.n_corner_ds, rep.n_surf_ds, rep.n_outlier_ds, rep.n_surf_total_ds)
-        clouds = {k: np.zeros((n, 4), np.float32) for k, n in zip(names, sizes)}
-        self._ck(self.L.lins_gpu_mappers_download(self.h, int(slot), ptr(poses), ptr(window), *[ptr(clouds[k]) for k in names]))
-        return poses, window, clouds
+        return self._download_node(lambda *out: self.L.lins_gpu_mappers_download(self.h, int(slot), *out), rep)
 
     # ---- batched mode ------------------------------------------------------------------------------------------
     def batch_upload(self, batch):

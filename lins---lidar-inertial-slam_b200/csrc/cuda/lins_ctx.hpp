@@ -1,8 +1,9 @@
 // lins_ctx.hpp — host state of a C-ABI context (struct lins_ctx of include/lins_gpu.h) and the helpers the translation units
 // that implement the C-ABI share: lins_gpu.cu (fused kernel, single-scan and batched entry points, F1), lins_upload.cu
-// (batch upload, gather lists), lins_map.cu (row F2), lins_seq.cu (sequence mode), lins_mapper.cu (the mapping node),
-// lins_mappers.cu (mapping nodes in lockstep) and the front-end units.  Host code only: a header that defines kernels cannot be included here, because every unit that
-// includes this one would define them again.
+// (batch upload, gather lists), lins_map.cu (row F2), lins_seq.cu (sequence mode), lins_mapper.cu (the mapping node's
+// host logic and VoxelGrid), lins_mappers.cu (the mapping node's cycle for one or many drives) and the front-end units.
+// Host code only: a header that defines kernels cannot be included here, because every unit that includes this one
+// would define them again.
 #pragma once
 #include <cuda_runtime.h>
 #if defined(__SSE2__)
@@ -246,8 +247,8 @@ struct Cloud2State {
   EventPair ev;                            // around the last decode kernel (lins_gpu_decode_ms)
 };
 
-// The mapper (lins_mapper.cu): one VoxelGrid call's device record — the ordered-integer encodings of the finite points'
-// f32 min / max, the box, the voxel count
+// The mapper (lins_mapper.cu): one VoxelGrid segment's device record — the ordered-integer encodings of the finite
+// points' f32 min / max, the box, the voxel count
 struct VgInfo {
   unsigned enc[6];   // min x y z, max x y z
   int min_b[3], mul[3];
@@ -256,7 +257,6 @@ struct VgInfo {
   int toobig;        // div_x * div_y * div_z > INT32_MAX
   int count;         // voxels
 };
-constexpr int kMapperGrids = 6;  // per cycle: map corner, map surf, scan corner, surf, outlier, surf total
 // PointTypePose (:57-65): the f32 pose fields and the f64 time
 struct MapperKeyPose { float x, y, z, roll, pitch, yaw; double time; };
 // one stored key frame: its corner, surf and outlier DS clouds in the map frame
@@ -291,21 +291,19 @@ struct VgScratch {
   Buf<int> idx[2], head, vid;
   Buf<unsigned char> temp;                   // CUB scratch
 };
-struct MapperState {
-  MapperNode n;
-  Buf<float4> in[3], ds[4], cat[3], map_ds[2];  // scan clouds, their DS (corner, surf, outlier, surf total), concatenations
-  Buf<float4> vg_in, vg_out;                 // lins_gpu_voxel_grid
+// lins_gpu_voxel_grid: its input and output cloud, the input's pinned staging, the VoxelGrid scratch and the record
+// (h_info stages its initial value, then receives it back: the stream orders the two copies)
+struct VoxelGridState {
+  Buf<float4> in, out;
   Buf<float4, kPinned> h_in;
-  VgScratch vg;
-  Buf<VgInfo> vg_info;
-  Buf<VgInfo, kPinned> h_vg_info, h_vg_init;
-  Buf<unsigned char> tf; Buf<unsigned char, kPinned> h_tf;  // the key frame's transform job
-  CopyList copies;                           // the local map's concatenation, then the surf-total one
+  VgScratch w;
+  Buf<VgInfo> info; Buf<VgInfo, kPinned> h_info;
 };
-// Lockstep mappers (lins_gpu_mappers_*, lins_mappers.cu): one MapperNode per slot with its six DS clouds of the last
+// A run of mapping nodes in lockstep (lins_mappers.cu): the lockstep mappers (lins_gpu_mappers_*), or the single
+// mapper (lins_gpu_mapper_*) as a run of one slot.  One MapperNode per slot with its six DS clouds of the last
 // processed cycle (map corner, map surf, corner, surf, outlier, surf total), and the step's shared device buffers
 struct MappersState {
-  int n = 0;                                 // slots (0 = lins_gpu_mappers_open has not run)
+  int n = 0;                                 // slots (0 = not opened)
   std::vector<MapperNode> node;
   std::vector<std::array<Buf<float4>, 6>> ds;
   Buf<lins_map::MapLoopState> loop;          // per slot: the scan-to-map loop state (matP / isDegenerate persist)
@@ -387,8 +385,9 @@ struct lins_ctx {
     Buf<float> coeff_c, coeff_s;
     Buf<uint8_t> mask_c, mask_s;
   } mp;
-  lins_capi::MapperState mapper;  // lins_gpu_mapper_*, lins_gpu_voxel_grid
+  lins_capi::MappersState mapper;   // lins_gpu_mapper_*: one slot, opened by the first call
   lins_capi::MappersState mappers;  // lins_gpu_mappers_*
+  lins_capi::VoxelGridState vg;     // lins_gpu_voxel_grid
 };
 
 namespace lins_capi {
@@ -571,17 +570,14 @@ int upload_bytes(lins_ctx* ctx, void* dst, Buf<unsigned char, kPinned>& staging,
 // decoded and has no points), upload them and queue their decode into ctx->proj.up (qs, qs_off; no synchronisation).
 // off (n + 1) receives the host copy of qs_off.
 int cloud2_run(lins_ctx* ctx, const lins_cloud2_desc* d, const uint8_t* present, std::vector<int32_t>& off);
-// lins_map.cu: the grid origin of a host cloud; bucket-sort n device map points into g (n_dev: the device-resident
-// count of the first n that are real); queue the scan-to-map loop on the
-// queries in ctx->mp.q_c / q_s (nc, ns) from transform T, with the loop state's D2H into mp.h_loop (no synchronisation;
-// with gate_nc / gate_ns, device counts, the loop stops before its first pass unless *gate_nc > 10 && *gate_ns > 100);
-// read that state into T and a report; zero the persistent loop state (matP, isDegenerate)
+// lins_map.cu: the grid origin of a host cloud; bucket-sort n device map points into g; queue the scan-to-map loop on
+// the queries in ctx->mp.q_c / q_s (nc, ns) from transform T, with the loop state's D2H into mp.h_loop (no
+// synchronisation); read a loop state into T and a report
 void map_grid_origin(const lins_point* host_pts, int n, float origin[3]);
-int map_build_grid(lins_ctx* ctx, lins_ctx::MapState::Grid& g, const float4* map, int n, const float origin[3], const int* n_dev = nullptr);
-int map_queue_loop(lins_ctx* ctx, int nc, int ns, const float* T, const int* gate_nc = nullptr, const int* gate_ns = nullptr);
+int map_build_grid(lins_ctx* ctx, lins_ctx::MapState::Grid& g, const float4* map, int n, const float origin[3]);
+int map_queue_loop(lins_ctx* ctx, int nc, int ns, const float* T);
 void map_loop_report(const lins_map::MapLoopState& st, float* T, lins_map_report* rep);
-int map_reset_loop(lins_ctx* ctx);
-// lins_map.cu: the scan-to-map loops of many slots in one queue (lins_gpu_mappers_step).  ms.h_mslot (pinned, n_slots)
+// lins_map.cu: the scan-to-map loops of many slots in one queue (the mapping nodes' step).  ms.h_mslot (pinned, n_slots)
 // holds each slot's map and query clouds, capacities, device map counts, start transform and run flag; the rest of the
 // table is filled here.  Queued: every slot's two grids in one bucket array (one count, one CUB scan, one scatter), the
 // start / gate kernel (a slot with run = 0 starts done), and LINS_MAP_MAX_ITER passes of one 5-NN and one fit launch per
@@ -596,7 +592,7 @@ int map_queue_slots(lins_ctx* ctx, MappersState& ms, int n_slots);
 int voxel_grid_queue(lins_ctx* ctx, VgScratch& w, const float4* in, int n_seg, const int* h_off, const int* d_off, const float* leaf,
                      float4* out, float4* const* d_out, VgInfo* h_init, VgInfo* info);
 int voxel_grid_reserve(lins_ctx* ctx, VgScratch& w, int n, int n_seg);
-// lins_mapper.cu: the mapping node's host logic, one copy for lins_gpu_mapper_* and lins_gpu_mappers_*.
+// lins_mapper.cu: the mapping node's host logic, which lins_mappers.cu runs for every slot.
 // mapper_node_reset: a freshly constructed node (the store's buffers are kept for reuse); mapper_node_imu: imuHandler.
 // mapper_cycle_begin: laserOdometryHandler into s (a copy of m.s, committed by the caller) and, unless the 0.3 s gate
 // skips the cycle (false; r reports it), transformAssociateToMap and the window; window_sizes: the local map's corner and

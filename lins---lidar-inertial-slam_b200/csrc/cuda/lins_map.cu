@@ -56,7 +56,7 @@ void map_grid_origin(const lins_point* host_pts, int n, float origin[3]) {
 
 // bucket-sort one device-resident map cloud into its grid (≙ kdtree*FromMap->setInputCloud, :1637-1638).  Any finite
 // origin gives the same 5-NN: the cells are exact (lins_map.cuh: grid_cell) and addressed by hash.
-int map_build_grid(lins_ctx* ctx, lins_ctx::MapState::Grid& g, const float4* map, int n, const float origin[3], const int* n_dev) {
+int map_build_grid(lins_ctx* ctx, lins_ctx::MapState::Grid& g, const float4* map, int n, const float origin[3]) {
   using namespace lins_map;
   g.n = n;
   if (n <= 0) return LINS_OK;
@@ -67,9 +67,9 @@ int map_build_grid(lins_ctx* ctx, lins_ctx::MapState::Grid& g, const float4* map
   for (int k = 0; k < 3; ++k) g.origin[k] = origin[k];
   const GridIndex gi = grid_index(g);
   CK(cudaMemsetAsync(g.count.p, 0, sizeof(int) * nb, ctx->stream));
-  lins_grid_count_kernel<<<(n + 255) / 256, 256, 0, ctx->stream>>>(map, n, n_dev, gi, g.count.p, nullptr, 0);
+  lins_grid_count_kernel<<<(n + 255) / 256, 256, 0, ctx->stream>>>(map, n, gi, g.count.p, nullptr, 0);
   lins_grid_scan_kernel<<<1, 1024, 0, ctx->stream>>>(g.count.p, g.start.p, g.cursor.p, (int)nb);
-  lins_grid_scatter_kernel<<<(n + 255) / 256, 256, 0, ctx->stream>>>(map, n, n_dev, gi, g.cursor.p, g.sorted.p, nullptr, 0);
+  lins_grid_scatter_kernel<<<(n + 255) / 256, 256, 0, ctx->stream>>>(map, n, gi, g.cursor.p, g.sorted.p, nullptr, 0);
   CK(cudaGetLastError());
   ctx->launches += 3;
   return LINS_OK;
@@ -137,30 +137,26 @@ int map_stage_queries(lins_ctx* ctx, const lins_point* corner, int nc, const lin
 
 }  // namespace
 
-// scan2MapOptimization's gate (:1636) on device-resident map sizes: a failing map marks the loop done before its first
-// pass.  Many slots (sl non-null, n of them): slot s's loop state first takes its start transform and a cleared report
-// (matP / isDegenerate persist), and a slot without a map (run = 0) starts done.
-__global__ void lins_map_gate_kernel(const int* __restrict__ nc, const int* __restrict__ ns, lins_map::MapLoopState* __restrict__ st,
-                                     const lins_map::MapSlot* __restrict__ sl, int n) {
+// the start of every slot's loop (n slots): its loop state takes the start transform and a cleared report (matP /
+// isDegenerate persist), and scan2MapOptimization's gate (:1636) on the device-resident map sizes marks a slot done
+// before its first pass when its map fails, or when it has none (run = 0)
+__global__ void lins_map_gate_kernel(lins_map::MapLoopState* __restrict__ st, const lins_map::MapSlot* __restrict__ sl, int n) {
   const int s = blockIdx.x * blockDim.x + threadIdx.x;
   if (s >= n) return;
-  if (sl) {
-    const lins_map::MapSlot& v = sl[s];
-    lins_map::MapLoopState& m = st[s];
-    for (int i = 0; i < 6; ++i) m.T[i] = v.T[i];
-    m.done = m.iters = m.converged = 0;
-    for (int i = 0; i < LINS_MAP_MAX_ITER; ++i) { m.n_sel[i] = 0; m.delta_r[i] = 0.f; m.delta_t[i] = 0.f; }
-    if (!v.run) { m.done = 1; return; }
-    nc = v.n_map[0]; ns = v.n_map[1];
-  }
-  if (!(*nc > 10 && *ns > 100)) st[s].done = 1;
+  const lins_map::MapSlot& v = sl[s];
+  lins_map::MapLoopState& m = st[s];
+  for (int i = 0; i < 6; ++i) m.T[i] = v.T[i];
+  m.done = m.iters = m.converged = 0;
+  for (int i = 0; i < LINS_MAP_MAX_ITER; ++i) { m.n_sel[i] = 0; m.delta_r[i] = 0.f; m.delta_t[i] = 0.f; }
+  if (!v.run) { m.done = 1; return; }
+  if (!(*v.n_map[0] > 10 && *v.n_map[1] > 100)) m.done = 1;
 }
 
 namespace lins_capi {
 
 // the iteration loop of scan2MapOptimization (:1640-1648) on the queries in ctx->mp.q_c / q_s and the map set up
 // in ctx->mp, queued up front with the loop state's D2H into mp.h_loop; nothing is synchronised
-int map_queue_loop(lins_ctx* ctx, int nc, int ns, const float* T, const int* gate_nc, const int* gate_ns) {
+int map_queue_loop(lins_ctx* ctx, int nc, int ns, const float* T) {
   using namespace lins_map;
   lins_ctx::MapState& m = ctx->mp;
   // The whole iteration loop (:1640-1648) is queued up front: transformTobeMapped, matP / isDegenerate and the report live
@@ -175,11 +171,6 @@ int map_queue_loop(lins_ctx* ctx, int nc, int ns, const float* T, const int* gat
   CK(cudaMemcpyAsync(m.loop.p, T, sizeof(float) * 6, cudaMemcpyHostToDevice, ctx->stream));  // (pageable sources: staged before the call returns)
   CK(cudaMemsetAsync(reinterpret_cast<char*>(m.loop.p) + offsetof(MapLoopState, done), 0, sizeof(MapLoopState) - offsetof(MapLoopState, done), ctx->stream));
   CK(cudaMemcpyAsync(m.consts.p, &pc0, sizeof(pc0), cudaMemcpyHostToDevice, ctx->stream));
-  if (gate_nc) {
-    lins_map_gate_kernel<<<1, 1, 0, ctx->stream>>>(gate_nc, gate_ns, m.loop.p, nullptr, 1);
-    CK(cudaGetLastError());
-    ctx->launches += 1;
-  }
   const bool grid = map_use_grid(true);
   for (int iter = 0; iter < LINS_MAP_MAX_ITER; ++iter) {
     int nblocks = 0;
@@ -236,12 +227,12 @@ int map_queue_slots(lins_ctx* ctx, MappersState& ms, int n_slots) {
   // every slot's two grids: one count, one scan of all buckets, one scatter
   CK(cudaMemsetAsync(ms.grid_count.p, 0, sizeof(int) * ((size_t)nb_tot + 1), ctx->stream));
   const GridIndex g0{};
-  if (pts) lins_grid_count_kernel<<<(pts + 255) / 256, 256, 0, ctx->stream>>>(nullptr, pts, nullptr, g0, ms.grid_count.p, ms.mslot.p, n_slots);
+  if (pts) lins_grid_count_kernel<<<(pts + 255) / 256, 256, 0, ctx->stream>>>(nullptr, pts, g0, ms.grid_count.p, ms.mslot.p, n_slots);
   size_t bytes = ms.scan_temp.cap;
   CK(cub::DeviceScan::ExclusiveSum(ms.scan_temp.p, bytes, ms.grid_count.p, ms.grid_start.p, nb_tot + 1, ctx->stream));
   CK(cudaMemcpyAsync(ms.grid_cursor.p, ms.grid_start.p, sizeof(int) * nb_tot, cudaMemcpyDeviceToDevice, ctx->stream));
-  if (pts) lins_grid_scatter_kernel<<<(pts + 255) / 256, 256, 0, ctx->stream>>>(nullptr, pts, nullptr, g0, ms.grid_cursor.p, ms.grid_sorted.p, ms.mslot.p, n_slots);
-  lins_map_gate_kernel<<<(n_slots + 127) / 128, 128, 0, ctx->stream>>>(nullptr, nullptr, ms.loop.p, ms.mslot.p, n_slots);
+  if (pts) lins_grid_scatter_kernel<<<(pts + 255) / 256, 256, 0, ctx->stream>>>(nullptr, pts, g0, ms.grid_cursor.p, ms.grid_sorted.p, ms.mslot.p, n_slots);
+  lins_map_gate_kernel<<<(n_slots + 127) / 128, 128, 0, ctx->stream>>>(ms.loop.p, ms.mslot.p, n_slots);
   CK(cudaGetLastError());
   ctx->launches += pts ? 4 : 2;
   // the loop: per pass one 5-NN and one fit launch per kind over every slot, one LM launch of a warp per slot
@@ -266,11 +257,6 @@ int map_queue_slots(lins_ctx* ctx, MappersState& ms, int n_slots) {
     ctx->launches += 1;
   }
   CK(cudaMemcpyAsync(ms.h_loop.p, ms.loop.p, sizeof(MapLoopState) * n_slots, cudaMemcpyDeviceToHost, ctx->stream));
-  return LINS_OK;
-}
-
-int map_reset_loop(lins_ctx* ctx) {
-  if (ctx->mp.loop.p) CK(cudaMemsetAsync(ctx->mp.loop.p, 0, sizeof(lins_map::MapLoopState), ctx->stream));
   return LINS_OK;
 }
 

@@ -306,23 +306,23 @@ __device__ __forceinline__ void grid_cell(const GridIndex& g, float x, float y, 
   iy = (unsigned)__double2int_rd((double)y - (double)g.oy);
   iz = (unsigned)__double2int_rd((double)z - (double)g.oz);
 }
-// counting sort of the map by bucket: count, (host-launched) scan, scatter.  n_dev (optional): the device-resident
-// number of points, <= n, when the host only knows the capacity n.  Many slots (sl non-null, n_sl slots): point i of
-// the n is point i - m0[k] of slot s's map k, with the slot's grid and its buckets from bucket0[k] on.
+// counting sort of the map by bucket: count, (host-launched) scan, scatter.  Many slots (sl non-null, n_sl slots): point
+// i of the n is point i - m0[k] of slot s's map k, with the slot's grid and its buckets from bucket0[k] on; n counts the
+// maps' capacities, and n_dev points at the device-resident number of a map's real points.
 struct GridPoint { const float4* map; int i; const int* n_dev; GridIndex g; int b0; };
-__device__ __forceinline__ GridPoint grid_point(const float4* map, int i, const int* n_dev, const GridIndex& g, const MapSlot* sl, int n_sl) {
-  if (!sl) return GridPoint{map, i, n_dev, g, 0};
+__device__ __forceinline__ GridPoint grid_point(const float4* map, int i, const GridIndex& g, const MapSlot* sl, int n_sl) {
+  if (!sl) return GridPoint{map, i, nullptr, g, 0};
   int lo = 0, hi = n_sl - 1;  // the last slot whose maps start at or before i
   while (lo < hi) { const int m = (lo + hi + 1) >> 1; if (sl[m].m0[0] <= i) lo = m; else hi = m - 1; }
   const MapSlot& v = sl[lo];
   const int k = i >= v.m0[1];
   return GridPoint{v.map[k], i - v.m0[k], v.n_map[k], v.g[k], v.bucket0[k]};
 }
-__global__ void lins_grid_count_kernel(const float4* __restrict__ map, int n, const int* __restrict__ n_dev, GridIndex g, int* __restrict__ count,
+__global__ void lins_grid_count_kernel(const float4* __restrict__ map, int n, GridIndex g, int* __restrict__ count,
                                        const MapSlot* __restrict__ sl, int n_sl) {
   const int i0 = blockIdx.x * blockDim.x + threadIdx.x;
   if (i0 >= n) return;
-  const GridPoint gp = grid_point(map, i0, n_dev, g, sl, n_sl);
+  const GridPoint gp = grid_point(map, i0, g, sl, n_sl);
   if (gp.n_dev && gp.i >= *gp.n_dev) return;
   const float4 p = __ldg(&gp.map[gp.i]);
   unsigned ix, iy, iz;
@@ -342,11 +342,11 @@ __global__ void __launch_bounds__(1024) lins_grid_scan_kernel(const int* __restr
   int run = part[threadIdx.x];
   for (int i = lo; i < hi; ++i) { start[i] = run; cursor[i] = run; run += count[i]; }
 }
-__global__ void lins_grid_scatter_kernel(const float4* __restrict__ map, int n, const int* __restrict__ n_dev, GridIndex g, int* __restrict__ cursor,
+__global__ void lins_grid_scatter_kernel(const float4* __restrict__ map, int n, GridIndex g, int* __restrict__ cursor,
                                          float4* __restrict__ sorted, const MapSlot* __restrict__ sl, int n_sl) {
   const int i0 = blockIdx.x * blockDim.x + threadIdx.x;
   if (i0 >= n) return;
-  const GridPoint gp = grid_point(map, i0, n_dev, g, sl, n_sl);
+  const GridPoint gp = grid_point(map, i0, g, sl, n_sl);
   if (gp.n_dev && gp.i >= *gp.n_dev) return;
   const float4 p = __ldg(&gp.map[gp.i]);
   unsigned ix, iy, iz;

@@ -1,12 +1,12 @@
-// lins_mapper.cu — the mapping node's cycle (lidar_mapping_node.cpp run() :1806-1855, without loop closure) behind
-// lins_gpu_mapper_step, and the device pcl::VoxelGrid it runs (lins_gpu_voxel_grid).
+// lins_mapper.cu — the mapping node (lidar_mapping_node.cpp run() :1806-1855, without loop closure) whose cycle
+// lins_mappers.cu runs for one or many drives: a node's host logic, its key-frame store's transform, and the device
+// pcl::VoxelGrid the cycle runs (also behind lins_gpu_voxel_grid).
 //
-// Device: the scan's three clouds, the key-frame store (each key frame's DS clouds transformed into the map frame once,
-// at save time, with its PointTypePose), the local map of the window (one gather launch), six VoxelGrids per cycle and
-// the scan-to-map loop of lins_map.cu.  Host: transformAssociateToMap, the window's deque of key-frame ids,
-// transformUpdate with the IMU ring, the 0.3 m key-frame test, the pose's round trip through gtsam's Rot3 and the
-// loop-candidate search, in the reference's f32 / f64 types (no multiply-add contraction: this unit is built with
-// -fmad=false and g++ does not contract on x86-64 without -mfma).
+// Host, per node (MapperNode): transformAssociateToMap, the window's deque of key-frame ids, transformUpdate with the IMU
+// ring, the 0.3 m key-frame test, the pose's round trip through gtsam's Rot3 and the loop-candidate search, in the
+// reference's f32 / f64 types (no multiply-add contraction: this unit is built with -fmad=false and g++ does not
+// contract on x86-64 without -mfma).  Device: the key-frame store, each key frame's DS clouds transformed into the map
+// frame once, at save time, with its PointTypePose (one launch for the key frames a step saves).
 //
 // VoxelGrid (csrc/host/feature_extraction.hpp restates PCL's applyFilter), on one or many clouds (segments) in one pass:
 // each segment's finite points' min / max (ordered-integer atomics: min / max are exact in any order), its min_b =
@@ -16,10 +16,6 @@
 // sort is stable), output in ascending key order at the segment's own offset.  Non-finite points and every point of a
 // segment whose div_x * div_y * div_z exceeds INT32_MAX get the key 0xffffffff, which no voxel can have, and are
 // dropped; each output has room for its segment's points and is NaN past the voxel count.
-//
-// Synchronisation: one per processed cycle.  The VoxelGrids' outputs are sized by their inputs and padded with NaN, the
-// later launches take those capacities, a device-side gate stops the scan-to-map loop when the map is too small, and
-// the six VoxelGrid records come back with the loop's state.
 #include <cuda_runtime.h>
 #include <cub/device/device_radix_sort.cuh>
 #include <cub/device/device_scan.cuh>
@@ -414,22 +410,6 @@ void transform_update(MapperScalars& s, double timeLaserOdometry, double SCAN_PE
   }
 }
 
-int upload3(lins_ctx* ctx, const lins_mapper_desc* d) {
-  MapperState& M = ctx->mapper;
-  const int n[3] = {d->n_corner, d->n_surf, d->n_outlier};
-  const lins_point* src[3] = {d->corner, d->surf, d->outlier};
-  Buf<float4>* dst[3] = {&M.in[0], &M.in[1], &M.in[2]};
-  CK(M.h_in.reserve((size_t)n[0] + n[1] + n[2] + 1));
-  size_t o = 0;
-  for (int k = 0; k < 3; ++k) {
-    CK(dst[k]->reserve((size_t)n[k] + 1));
-    pack_into(M.h_in.p + o, src[k], n[k]);
-    if (n[k]) CK(cudaMemcpyAsync(dst[k]->p, M.h_in.p + o, sizeof(float4) * n[k], cudaMemcpyHostToDevice, ctx->stream));
-    o += n[k];
-  }
-  return LINS_OK;
-}
-
 // the slot of key frame id (a free one, or a new one)
 MapperKeyFrame& keyframe_slot(MapperNode& M, int id) {
   auto it = M.slot_of.find(id);
@@ -439,14 +419,6 @@ MapperKeyFrame& keyframe_slot(MapperNode& M, int id) {
   else { s = (int)M.slots.size(); M.slots.emplace_back(); }
   M.slot_of[id] = s;
   return M.slots[s];
-}
-
-// one VoxelGrid record per segment at info, staged at h_init
-int voxel_grid_one(lins_ctx* ctx, const float4* in, int n, float leaf, float4* out, VgInfo* info) {
-  MapperState& M = ctx->mapper;
-  CK(M.h_vg_init.reserve(kMapperGrids));
-  const int off[2] = {0, std::max(n, 0)};
-  return voxel_grid_queue(ctx, M.vg, in, 1, off, nullptr, &leaf, out, nullptr, M.h_vg_init.p + (info - M.vg_info.p), info);
 }
 
 }  // namespace
@@ -611,147 +583,25 @@ int mapper_node_download(lins_ctx* ctx, const MapperNode& M, const float4* const
 
 extern "C" {
 
-int lins_gpu_mapper_reset(lins_ctx* ctx) {
-  if (!ctx) return LINS_E_INVALID;
-  CK(cudaSetDevice(ctx->device));
-  mapper_node_reset(ctx->mapper.n);
-  return map_reset_loop(ctx);  // isDegenerate, matP
-}
-
-int lins_gpu_mapper_imu(lins_ctx* ctx, const double* time, const double* roll, const double* pitch, int n) {
-  if (!ctx) return LINS_E_INVALID;
-  if (n < 0 || (n > 0 && (!time || !roll || !pitch))) return fail(ctx, LINS_E_INVALID, "bad IMU arrays");
-  mapper_node_imu(ctx->mapper.n.s, time, roll, pitch, n);
-  return LINS_OK;
-}
-
-int lins_gpu_mapper_step(lins_ctx* ctx, const lins_mapper_desc* d, lins_mapper_report* rep) {
-  if (!ctx) return LINS_E_INVALID;
-  if (!d) return fail(ctx, LINS_E_INVALID, "null desc");
-  if (check_cloud(ctx, d->corner, d->n_corner, "bad mapper corner cloud") != LINS_OK || check_cloud(ctx, d->surf, d->n_surf, "bad mapper surf cloud") != LINS_OK ||
-      check_cloud(ctx, d->outlier, d->n_outlier, "bad mapper outlier cloud") != LINS_OK)
-    return LINS_E_INVALID;
-  CK(cudaSetDevice(ctx->device));
-  MapperState& M = ctx->mapper;
-  lins_mapper_report r;
-  MapperScalars s = M.n.s;  // committed only when the cycle completes
-  const double timeLaserOdometry = d->time;
-  if (!mapper_cycle_begin(M.n, s, timeLaserOdometry, d->quat, d->pos, r)) {
-    M.n.s = s;
-    if (rep) *rep = r;
-    return LINS_OK;
-  }
-  const int numPoses = (int)M.n.poses.size();
-  // Everything up to the scan-to-map loop is queued without reading anything back: the VoxelGrids' outputs are sized
-  // by their inputs and filled with NaN past their counts, and the later stages take those capacities.  A NaN point is
-  // dropped by a VoxelGrid, is never a neighbour and never selects a query, and the block partials it leaves are zero,
-  // so the results equal those of the exact sizes.  The counts come back with the loop's state: one synchronisation.
-  const int n_in[3] = {d->n_corner, d->n_surf, d->n_outlier};
-  int n_cat[3] = {0, 0, d->n_surf + d->n_outlier};
-  mapper_window_sizes(M.n, s, n_cat[0], n_cat[1]);
-  // every buffer of the cycle first (a growth frees memory queued work may still read)
-  const int n_max = std::max({n_cat[0], n_cat[1], n_cat[2]});
-  int rc = voxel_grid_reserve(ctx, M.vg, n_max, 1);
-  if (rc != LINS_OK) return rc;
-  CK(M.vg_info.reserve(kMapperGrids)); CK(M.h_vg_info.reserve(kMapperGrids));
-  for (int k = 0; k < 3; ++k) { CK(M.cat[k].reserve((size_t)n_cat[k] + 1)); CK(M.ds[k].reserve((size_t)n_in[k] + 1)); }
-  CK(M.ds[3].reserve((size_t)n_cat[2] + 1));
-  CK(M.map_ds[0].reserve((size_t)n_cat[0] + 1)); CK(M.map_ds[1].reserve((size_t)n_cat[1] + 1));
-  const size_t n_copies = 3 * s.window.size() + 2;
-  if ((rc = M.copies.reserve(ctx, n_copies)) != LINS_OK) return rc;
-  VgInfo* info = M.vg_info.p;
-  // the local map: corner_i ..., and surf_i, outlier_i interleaved (:1242-1246)
-  std::vector<DevCopy> copies;
-  {
-    int oc = 0, os = 0;
-    for (int id : s.window) {
-      const MapperKeyFrame& kf = M.n.slots[M.n.slot_of.at(id)];
-      copies.push_back(DevCopy{kf.c[0].p, M.cat[0].p + oc, kf.n[0], 0}); oc += kf.n[0];
-      copies.push_back(DevCopy{kf.c[1].p, M.cat[1].p + os, kf.n[1], 0}); os += kf.n[1];
-      copies.push_back(DevCopy{kf.c[2].p, M.cat[1].p + os, kf.n[2], 0}); os += kf.n[2];
-    }
-  }
-  if ((rc = queue_copies(ctx, M.copies, copies, 0)) != LINS_OK) return rc;
-  const bool have_map = numPoses > 0;
-  if ((rc = voxel_grid_one(ctx, M.cat[0].p, have_map ? n_cat[0] : 0, 0.2f, M.map_ds[0].p, info + 0)) != LINS_OK) return rc;
-  if ((rc = voxel_grid_one(ctx, M.cat[1].p, have_map ? n_cat[1] : 0, 0.4f, M.map_ds[1].p, info + 1)) != LINS_OK) return rc;
-  // downsampleCurrentScan :1326-1349
-  if ((rc = upload3(ctx, d)) != LINS_OK) return rc;
-  const float leaf[3] = {0.2f, 0.4f, 0.4f};
-  for (int k = 0; k < 3; ++k)
-    if ((rc = voxel_grid_one(ctx, M.in[k].p, n_in[k], leaf[k], M.ds[k].p, info + 2 + k)) != LINS_OK) return rc;
-  // laserCloudSurfTotalLast = surf DS + outlier DS: their NaN tails ride along and are dropped by the filter
-  copies.assign({DevCopy{M.ds[1].p, M.cat[2].p, n_in[1], 0}, DevCopy{M.ds[2].p, M.cat[2].p + n_in[1], n_in[2], 0}});
-  if ((rc = queue_copies(ctx, M.copies, copies, (int)n_copies - 2)) != LINS_OK) return rc;
-  if ((rc = voxel_grid_one(ctx, M.cat[2].p, n_cat[2], 0.4f, M.ds[3].p, info + 5)) != LINS_OK) return rc;
-
-  // scan2MapOptimization :1635-1652: without key poses the map is empty and the gate fails on the host; otherwise the
-  // loop is queued on the capacities and a device-side gate on the two map counts stops it before its first pass
-  lins_ctx::MapState& mp = ctx->mp;
-  if (have_map) {
-    CK(mp.map_c.reserve((size_t)n_cat[0] + 1)); CK(mp.map_s.reserve((size_t)n_cat[1] + 1));
-    CK(mp.q_c.reserve((size_t)n_in[0] + 1)); CK(mp.q_s.reserve((size_t)n_cat[2] + 1));
-    if (n_cat[0]) CK(cudaMemcpyAsync(mp.map_c.p, M.map_ds[0].p, sizeof(float4) * n_cat[0], cudaMemcpyDeviceToDevice, ctx->stream));
-    if (n_cat[1]) CK(cudaMemcpyAsync(mp.map_s.p, M.map_ds[1].p, sizeof(float4) * n_cat[1], cudaMemcpyDeviceToDevice, ctx->stream));
-    if (n_in[0]) CK(cudaMemcpyAsync(mp.q_c.p, M.ds[0].p, sizeof(float4) * n_in[0], cudaMemcpyDeviceToDevice, ctx->stream));
-    if (n_cat[2]) CK(cudaMemcpyAsync(mp.q_s.p, M.ds[3].p, sizeof(float4) * n_cat[2], cudaMemcpyDeviceToDevice, ctx->stream));
-    // the grids hold the real points only (a NaN tail would crowd one bucket); the searches take the capacities
-    const float origin[3] = {0.f, 0.f, 0.f};  // (any finite origin gives the same 5-NN)
-    if ((rc = map_build_grid(ctx, mp.grid_c, mp.map_c.p, n_cat[0], origin, &info[0].count)) != LINS_OK) return rc;
-    if ((rc = map_build_grid(ctx, mp.grid_s, mp.map_s.p, n_cat[1], origin, &info[1].count)) != LINS_OK) return rc;
-    mp.n_map_c = n_cat[0]; mp.n_map_s = n_cat[1];
-    if ((rc = map_queue_loop(ctx, n_in[0], n_cat[2], s.transformTobeMapped, &info[0].count, &info[1].count)) != LINS_OK) return rc;
-  }
-  CK(cudaMemcpyAsync(M.h_vg_info.p, info, sizeof(VgInfo) * kMapperGrids, cudaMemcpyDeviceToHost, ctx->stream));
-  CK(cudaStreamSynchronize(ctx->stream));  // the cycle's one read-back
-  M.n.last.valid = false;  // (a failed cycle has overwritten the previous one's clouds)
-  const VgInfo* hi = M.h_vg_info.p;
-  for (int i = 0; i < kMapperGrids; ++i)
-    if (hi[i].toobig) return fail(ctx, LINS_E_TOOBIG, "VoxelGrid: the leaf is too small for the cloud's extent (div_x * div_y * div_z > INT32_MAX)");
-  const int cnt[6] = {have_map ? hi[0].count : 0, have_map ? hi[1].count : 0, hi[2].count, hi[3].count, hi[4].count, hi[5].count};
-  if (have_map) { mp.n_map_c = cnt[0]; mp.n_map_s = cnt[1]; }
-  const bool gate = cnt[0] > 10 && cnt[1] > 100;
-  KfSave sv;
-  bool saved = false;
-  mapper_cycle_end(M.n, s, timeLaserOdometry, ctx->prm.scan_period, cnt, gate ? ctx->mp.h_loop.p : nullptr, r, &sv, &saved);
-  if (saved) {
-    for (int k = 0; k < 3; ++k) sv.ds[k] = M.ds[k].p;
-    if ((rc = keyframes_queue(ctx, &sv, 1, M.tf, M.h_tf)) != LINS_OK) return rc;
-  }
-  if (rep) *rep = r;
-  return LINS_OK;
-}
-
-int lins_gpu_mapper_download(lins_ctx* ctx, double* key_poses, int32_t* window, float* map_corner_ds, float* map_surf_ds,
-                             float* corner_ds, float* surf_ds, float* outlier_ds, float* surf_total_ds) {
-  if (!ctx) return LINS_E_INVALID;
-  CK(cudaSetDevice(ctx->device));
-  MapperState& M = ctx->mapper;
-  float* dst[6] = {map_corner_ds, map_surf_ds, corner_ds, surf_ds, outlier_ds, surf_total_ds};
-  const float4* src[6] = {M.map_ds[0].p, M.map_ds[1].p, M.ds[0].p, M.ds[1].p, M.ds[2].p, M.ds[3].p};
-  return mapper_node_download(ctx, M.n, src, key_poses, window, dst);
-}
-
 int lins_gpu_voxel_grid(lins_ctx* ctx, const lins_point* in, int n, float leaf, float* out, int* n_out) {
   if (!ctx) return LINS_E_INVALID;
   if (check_cloud(ctx, in, n, "bad VoxelGrid input cloud") != LINS_OK || check_cloud(ctx, out, n, "bad VoxelGrid output cloud") != LINS_OK)
     return LINS_E_INVALID;
   if (!n_out || !(leaf > 0.f) || !std::isfinite(leaf)) return fail(ctx, LINS_E_INVALID, "bad VoxelGrid n_out / leaf");
   CK(cudaSetDevice(ctx->device));
-  MapperState& M = ctx->mapper;
-  CK(M.vg_info.reserve(kMapperGrids));
-  CK(M.vg_in.reserve((size_t)n + 1)); CK(M.vg_out.reserve((size_t)n + 1));
-  CK(M.h_in.reserve((size_t)n + 1));
-  pack_into(M.h_in.p, in, n);
-  if (n) CK(cudaMemcpyAsync(M.vg_in.p, M.h_in.p, sizeof(float4) * n, cudaMemcpyHostToDevice, ctx->stream));
-  int rc = voxel_grid_one(ctx, M.vg_in.p, n, leaf, M.vg_out.p, M.vg_info.p);
+  VoxelGridState& v = ctx->vg;
+  CK(v.in.reserve((size_t)n + 1)); CK(v.out.reserve((size_t)n + 1)); CK(v.h_in.reserve((size_t)n + 1));
+  CK(v.info.reserve(1)); CK(v.h_info.reserve(1));
+  pack_into(v.h_in.p, in, n);
+  if (n) CK(cudaMemcpyAsync(v.in.p, v.h_in.p, sizeof(float4) * n, cudaMemcpyHostToDevice, ctx->stream));
+  const int off[2] = {0, n};
+  const int rc = voxel_grid_queue(ctx, v.w, v.in.p, 1, off, nullptr, &leaf, v.out.p, nullptr, v.h_info.p, v.info.p);
   if (rc != LINS_OK) return rc;
-  CK(M.h_vg_info.reserve(kMapperGrids));
-  CK(cudaMemcpyAsync(M.h_vg_info.p, M.vg_info.p, sizeof(VgInfo), cudaMemcpyDeviceToHost, ctx->stream));
+  CK(cudaMemcpyAsync(v.h_info.p, v.info.p, sizeof(VgInfo), cudaMemcpyDeviceToHost, ctx->stream));
   CK(cudaStreamSynchronize(ctx->stream));
-  if (M.h_vg_info.p[0].toobig) return fail(ctx, LINS_E_TOOBIG, "VoxelGrid: the leaf is too small for the cloud's extent (div_x * div_y * div_z > INT32_MAX)");
-  const int c = n > 0 ? M.h_vg_info.p[0].count : 0;
-  CK(d2h(ctx, out, M.vg_out.p, sizeof(float4) * c));
+  if (v.h_info.p->toobig) return fail(ctx, LINS_E_TOOBIG, "VoxelGrid: the leaf is too small for the cloud's extent (div_x * div_y * div_z > INT32_MAX)");
+  const int c = n > 0 ? v.h_info.p->count : 0;
+  CK(d2h(ctx, out, v.out.p, sizeof(float4) * c));
   CK(cudaStreamSynchronize(ctx->stream));
   *n_out = c;
   return LINS_OK;

@@ -1,13 +1,15 @@
-// lins_mappers.cu — the mapping node's cycle for many drives in lockstep (lins_gpu_mappers_*): one MapperNode per slot,
-// each stepped by the host logic of lins_mapper.cu, with one queue of device work per step for every processed slot.
+// lins_mappers.cu — the mapping node's cycle for many drives in lockstep (lins_gpu_mappers_*) and for one
+// (lins_gpu_mapper_*, a run of one slot of its own): one MapperNode per slot, each stepped by the host logic of
+// lins_mapper.cu, with one queue of device work per step for every processed slot.
 //
 // Per step (one synchronisation): the scans of the processed slots in one H2D; one gather launch of every slot's window
 // into its local-map clouds; one segmented VoxelGrid over the five clouds of every slot (map corner 0.2 m, map surf
 // 0.4 m, corner 0.2 m, surf 0.4 m, outlier 0.4 m), one gather of each slot's surf DS + outlier DS and one segmented
 // VoxelGrid of those (0.4 m); every slot's grids and scan-to-map loop (lins_map.cu: map_queue_slots); the read-back of
 // the VoxelGrid records and loop states.  After it, the host tail of each slot and one transform launch for every key
-// frame saved.  The segments of a VoxelGrid keep their input ranges and each slot's fit blocks cover its own queries
-// only, so every slot's clouds, sums and steps are those of a lins_gpu_mapper_step on a context of its own.
+// frame saved.  The VoxelGrids' outputs are sized by their inputs and padded with NaN, and the later launches take those
+// capacities.  The segments of a VoxelGrid keep their input ranges and each slot's fit blocks cover its own queries
+// only, so every slot's clouds, sums and steps are those of a run of one slot.
 #include <cuda_runtime.h>
 
 #include <algorithm>
@@ -28,15 +30,9 @@ int need_open(lins_ctx* ctx) {
 
 const char* const kBad = "VoxelGrid: the leaf is too small for the cloud's extent (div_x * div_y * div_z > INT32_MAX)";
 
-}  // namespace
-
-extern "C" {
-
-int lins_gpu_mappers_open(lins_ctx* ctx, int32_t n_slots) {
-  if (!ctx) return LINS_E_INVALID;
-  if (n_slots < 1) return fail(ctx, LINS_E_INVALID, "n_slots < 1");
+// n_slots fresh mapping nodes in ms, replacing any open run
+int mappers_open(lins_ctx* ctx, MappersState& ms, int n_slots) {
   CK(cudaSetDevice(ctx->device));
-  MappersState& ms = ctx->mappers;
   ms.n = 0;
   ms.node = std::vector<MapperNode>(n_slots);  // (constructed in place: a node is not copyable)
   ms.ds = std::vector<std::array<Buf<float4>, 6>>(n_slots);
@@ -46,12 +42,9 @@ int lins_gpu_mappers_open(lins_ctx* ctx, int32_t n_slots) {
   return LINS_OK;
 }
 
-int lins_gpu_mappers_reset(lins_ctx* ctx, const uint8_t* mask) {
-  if (!ctx) return LINS_E_INVALID;
-  if (need_open(ctx) != LINS_OK) return LINS_E_NOMAP;
-  if (!mask) return fail(ctx, LINS_E_INVALID, "null mask");
+// the slots with mask[s] != 0 back to the fresh state
+int mappers_reset(lins_ctx* ctx, MappersState& ms, const uint8_t* mask) {
   CK(cudaSetDevice(ctx->device));
-  MappersState& ms = ctx->mappers;
   for (int s = 0; s < ms.n; ++s)
     if (mask[s]) {
       mapper_node_reset(ms.node[s]);
@@ -60,28 +53,16 @@ int lins_gpu_mappers_reset(lins_ctx* ctx, const uint8_t* mask) {
   return LINS_OK;
 }
 
-int lins_gpu_mappers_imu(lins_ctx* ctx, const int32_t* off, const double* time, const double* roll, const double* pitch) {
-  if (!ctx) return LINS_E_INVALID;
-  if (need_open(ctx) != LINS_OK) return LINS_E_NOMAP;
-  MappersState& ms = ctx->mappers;
-  if (check_csr(ctx, off, ms.n, time, "bad IMU offsets / arrays") != LINS_OK) return LINS_E_INVALID;
-  if (off[ms.n] > 0 && (!roll || !pitch)) return fail(ctx, LINS_E_INVALID, "bad IMU offsets / arrays");
+// imuHandler for every slot: slot s's rows are [off[s], off[s + 1])
+void mappers_imu(MappersState& ms, const int32_t* off, const double* time, const double* roll, const double* pitch) {
   for (int s = 0; s < ms.n; ++s) mapper_node_imu(ms.node[s].s, time + off[s], roll + off[s], pitch + off[s], off[s + 1] - off[s]);
-  return LINS_OK;
 }
 
-int lins_gpu_mappers_step(lins_ctx* ctx, const lins_mappers_desc* d, lins_mapper_report* reps) {
-  if (!ctx) return LINS_E_INVALID;
-  if (!d) return fail(ctx, LINS_E_INVALID, "null desc");
-  if (need_open(ctx) != LINS_OK) return LINS_E_NOMAP;
-  MappersState& ms = ctx->mappers;
+// one step of every present slot of ms on a checked descriptor (d->n_slots == ms.n, valid offsets and arrays)
+int mappers_step(lins_ctx* ctx, MappersState& ms, const lins_mappers_desc* d, lins_mapper_report* reps) {
   const int M = ms.n;
-  if (d->n_slots != M) return fail(ctx, LINS_E_INVALID, "n_slots differs from the open run's");
-  if (!d->time || !d->quat || !d->pos) return fail(ctx, LINS_E_INVALID, "null time / quat / pos");
   const lins_point* src[3] = {d->corner, d->surf, d->outlier};
   const int32_t* off[3] = {d->corner_off, d->surf_off, d->outlier_off};
-  static const char* const what[3] = {"bad corner offsets / cloud", "bad surf offsets / cloud", "bad outlier offsets / cloud"};
-  for (int k = 0; k < 3; ++k) if (check_csr(ctx, off[k], M, src[k], what[k]) != LINS_OK) return LINS_E_INVALID;
   CK(cudaSetDevice(ctx->device));
 
   // the host head of every present slot's cycle, on copies of its scalars (committed after the read-back)
@@ -233,17 +214,112 @@ int lins_gpu_mappers_step(lins_ctx* ctx, const lins_mappers_desc* d, lins_mapper
   return finish();
 }
 
+// the key poses, window and last cycle's clouds of one slot (dst: NULL skips)
+int mappers_download(lins_ctx* ctx, MappersState& ms, int slot, double* key_poses, int32_t* window, float* const dst[6]) {
+  CK(cudaSetDevice(ctx->device));
+  const float4* src[6];
+  for (int k = 0; k < 6; ++k) src[k] = ms.ds[slot][k].p;
+  return mapper_node_download(ctx, ms.node[slot], src, key_poses, window, dst);
+}
+
+// the single mapper: a run of one slot of its own, opened by the first lins_gpu_mapper_* call on the context
+int mapper_open(lins_ctx* ctx) {
+  return ctx->mapper.n > 0 ? LINS_OK : mappers_open(ctx, ctx->mapper, 1);
+}
+
+}  // namespace
+
+extern "C" {
+
+int lins_gpu_mappers_open(lins_ctx* ctx, int32_t n_slots) {
+  if (!ctx) return LINS_E_INVALID;
+  if (n_slots < 1) return fail(ctx, LINS_E_INVALID, "n_slots < 1");
+  return mappers_open(ctx, ctx->mappers, n_slots);
+}
+
+int lins_gpu_mappers_reset(lins_ctx* ctx, const uint8_t* mask) {
+  if (!ctx) return LINS_E_INVALID;
+  if (need_open(ctx) != LINS_OK) return LINS_E_NOMAP;
+  if (!mask) return fail(ctx, LINS_E_INVALID, "null mask");
+  return mappers_reset(ctx, ctx->mappers, mask);
+}
+
+int lins_gpu_mappers_imu(lins_ctx* ctx, const int32_t* off, const double* time, const double* roll, const double* pitch) {
+  if (!ctx) return LINS_E_INVALID;
+  if (need_open(ctx) != LINS_OK) return LINS_E_NOMAP;
+  MappersState& ms = ctx->mappers;
+  if (check_csr(ctx, off, ms.n, time, "bad IMU offsets / arrays") != LINS_OK) return LINS_E_INVALID;
+  if (off[ms.n] > 0 && (!roll || !pitch)) return fail(ctx, LINS_E_INVALID, "bad IMU offsets / arrays");
+  mappers_imu(ms, off, time, roll, pitch);
+  return LINS_OK;
+}
+
+int lins_gpu_mappers_step(lins_ctx* ctx, const lins_mappers_desc* d, lins_mapper_report* reps) {
+  if (!ctx) return LINS_E_INVALID;
+  if (!d) return fail(ctx, LINS_E_INVALID, "null desc");
+  if (need_open(ctx) != LINS_OK) return LINS_E_NOMAP;
+  const int M = ctx->mappers.n;
+  if (d->n_slots != M) return fail(ctx, LINS_E_INVALID, "n_slots differs from the open run's");
+  if (!d->time || !d->quat || !d->pos) return fail(ctx, LINS_E_INVALID, "null time / quat / pos");
+  const lins_point* src[3] = {d->corner, d->surf, d->outlier};
+  const int32_t* off[3] = {d->corner_off, d->surf_off, d->outlier_off};
+  static const char* const what[3] = {"bad corner offsets / cloud", "bad surf offsets / cloud", "bad outlier offsets / cloud"};
+  for (int k = 0; k < 3; ++k) if (check_csr(ctx, off[k], M, src[k], what[k]) != LINS_OK) return LINS_E_INVALID;
+  return mappers_step(ctx, ctx->mappers, d, reps);
+}
+
 int lins_gpu_mappers_download(lins_ctx* ctx, int32_t slot, double* key_poses, int32_t* window, float* map_corner_ds, float* map_surf_ds,
                               float* corner_ds, float* surf_ds, float* outlier_ds, float* surf_total_ds) {
   if (!ctx) return LINS_E_INVALID;
   if (need_open(ctx) != LINS_OK) return LINS_E_NOMAP;
-  MappersState& ms = ctx->mappers;
-  if (slot < 0 || slot >= ms.n) return fail(ctx, LINS_E_INVALID, "slot out of range");
-  CK(cudaSetDevice(ctx->device));
+  if (slot < 0 || slot >= ctx->mappers.n) return fail(ctx, LINS_E_INVALID, "slot out of range");
   float* const dst[6] = {map_corner_ds, map_surf_ds, corner_ds, surf_ds, outlier_ds, surf_total_ds};
-  const float4* src[6];
-  for (int k = 0; k < 6; ++k) src[k] = ms.ds[slot][k].p;
-  return mapper_node_download(ctx, ms.node[slot], src, key_poses, window, dst);
+  return mappers_download(ctx, ctx->mappers, slot, key_poses, window, dst);
+}
+
+int lins_gpu_mapper_reset(lins_ctx* ctx) {
+  if (!ctx) return LINS_E_INVALID;
+  const int rc = mapper_open(ctx);
+  if (rc != LINS_OK) return rc;
+  const uint8_t all = 1;
+  return mappers_reset(ctx, ctx->mapper, &all);
+}
+
+int lins_gpu_mapper_imu(lins_ctx* ctx, const double* time, const double* roll, const double* pitch, int n) {
+  if (!ctx) return LINS_E_INVALID;
+  if (n < 0 || (n > 0 && (!time || !roll || !pitch))) return fail(ctx, LINS_E_INVALID, "bad IMU arrays");
+  const int rc = mapper_open(ctx);
+  if (rc != LINS_OK) return rc;
+  const int32_t off[2] = {0, n};
+  mappers_imu(ctx->mapper, off, time, roll, pitch);
+  return LINS_OK;
+}
+
+int lins_gpu_mapper_step(lins_ctx* ctx, const lins_mapper_desc* d, lins_mapper_report* rep) {
+  if (!ctx) return LINS_E_INVALID;
+  if (!d) return fail(ctx, LINS_E_INVALID, "null desc");
+  if (check_cloud(ctx, d->corner, d->n_corner, "bad mapper corner cloud") != LINS_OK || check_cloud(ctx, d->surf, d->n_surf, "bad mapper surf cloud") != LINS_OK ||
+      check_cloud(ctx, d->outlier, d->n_outlier, "bad mapper outlier cloud") != LINS_OK)
+    return LINS_E_INVALID;
+  const int rc = mapper_open(ctx);
+  if (rc != LINS_OK) return rc;
+  const int32_t off[3][2] = {{0, d->n_corner}, {0, d->n_surf}, {0, d->n_outlier}};
+  lins_mappers_desc one = {};
+  one.n_slots = 1;
+  one.time = &d->time; one.quat = d->quat; one.pos = d->pos;
+  one.corner = d->corner; one.corner_off = off[0];
+  one.surf = d->surf; one.surf_off = off[1];
+  one.outlier = d->outlier; one.outlier_off = off[2];
+  return mappers_step(ctx, ctx->mapper, &one, rep);
+}
+
+int lins_gpu_mapper_download(lins_ctx* ctx, double* key_poses, int32_t* window, float* map_corner_ds, float* map_surf_ds,
+                             float* corner_ds, float* surf_ds, float* outlier_ds, float* surf_total_ds) {
+  if (!ctx) return LINS_E_INVALID;
+  const int rc = mapper_open(ctx);
+  if (rc != LINS_OK) return rc;
+  float* const dst[6] = {map_corner_ds, map_surf_ds, corner_ds, surf_ds, outlier_ds, surf_total_ds};
+  return mappers_download(ctx, ctx->mapper, 0, key_poses, window, dst);
 }
 
 }  // extern "C"

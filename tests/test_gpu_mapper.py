@@ -8,6 +8,7 @@ transformAftMapped and newest key pose, so every cycle starts from bit-identical
 import numpy as np
 import pytest
 
+import mapcases
 import mapper_drive
 import mapperref
 import pyfront
@@ -110,6 +111,25 @@ def test_mapper_gate_failure_keeps_stale_transform(capi, ob, defs, synth):
     reps = [r for _, r, _ in log if r.processed]
     assert all(r.map.skipped for r in reps) and reps[-1].n_keyframes == 1
     assert all(list(r.transform_aft_mapped) == [0.0] * 6 for r in reps)
+
+
+def test_mapper_leaves_the_scan2map_state_alone(capi, synth):
+    """map_set + scan2map, then mapper cycles that run scan-to-map, a mapper_reset and scan2map again without map_set:
+    the transform and report equal those of a context that never ran the mapper (the map, matP and isDegenerate of
+    map_set / scan2map are not the mapper's)."""
+    c = mapcases.corridor_scene()
+    shared, alone = capi.LinsGpu(), capi.LinsGpu()
+    for g in (shared, alone):
+        g.map_set(c.corner_map, c.surf_map)
+        g.scan2map(c.corner_q, c.surf_q, c.T)
+    ev = [e for e in mapper_drive.make_drive(synth, n_out=8, seed=9, stall_at=-1) if e[0] == "odom"]
+    reps = [shared.mapper_step(*e[1:7]) for e in ev]
+    assert sum(1 for r in reps if r.processed and not r.map.skipped) >= 3
+    shared.mapper_reset()
+    (t1, m1), (t2, m2) = (g.scan2map(c.corner_q, c.surf_q, c.T) for g in (shared, alone))
+    assert m2.degenerate == 1 and not m2.skipped
+    assert np.array_equal(t1.view(np.uint32), t2.view(np.uint32)) and bytes(m1) == bytes(m2)
+    shared.close(); alone.close()
 
 
 def test_voxel_grid_million_points(gpu):

@@ -251,10 +251,11 @@ struct Cloud2State {
 // points' f32 min / max, the box, the voxel count
 struct VgInfo {
   unsigned enc[6];   // min x y z, max x y z
-  int min_b[3], mul[3];
+  float base[3];     // floor(min * inv) in f32 (an integer value; |base| < 2^62 unless toobig)
+  int mul[3];
   float inv;
   int any;           // at least one finite point
-  int toobig;        // div_x * div_y * div_z > INT32_MAX
+  int toobig;        // div_x * div_y * div_z > INT32_MAX, or a floor of min / max * inv of magnitude 2^62 or more
   int count;         // voxels
 };
 // PointTypePose (:57-65): the f32 pose fields and the f64 time

@@ -10,7 +10,7 @@
 //
 // VoxelGrid (csrc/host/feature_extraction.hpp restates PCL's applyFilter), on one or many clouds (segments) in one pass:
 // each segment's finite points' min / max (ordered-integer atomics: min / max are exact in any order), its min_b =
-// floor(min * inv), the key floor(p * inv) - (float)min_b per axis (lins_features.cuh: voxel_key), a stable CUB radix
+// floor(min * inv) as int64, the key floor(p * inv) - (float)min_b per axis (vg_key), a stable CUB radix
 // sort of (key, index) — with more than one segment of ((segment, key), index) on 32 + ceil(log2 segments) bits, so
 // the segments stay in their input ranges — and one centroid per voxel, its points summed in f32 in input order (the
 // sort is stable), output in ascending key order at the segment's own offset.  Non-finite points and every point of a
@@ -102,7 +102,10 @@ __global__ void __launch_bounds__(kVgThreads) lins_vg_bounds_kernel(const float4
   }
 }
 
-// getMinMax3D -> min_b, div_b, divb_mul (feature_extraction.hpp VoxelGrid::filter), one thread per segment
+// getMinMax3D -> min_b, div_b, divb_mul (feature_extraction.hpp VoxelGrid::filter), one thread per segment.  The bounds
+// are int64 of the f32 floors: an int cast clamps beyond 2^31 voxels from the origin, and a box there would get div = 1
+// on that axis and merge distinct voxels.  A floor at or beyond 2^62 in magnitude (an overflow of min / max * inv to
+// inf included) has no exact int64 difference and makes the segment toobig.
 __global__ void lins_vg_box_kernel(VgInfo* __restrict__ infos, int n_seg) {
   const int sgi = blockIdx.x * blockDim.x + threadIdx.x;
   if (sgi >= n_seg) return;
@@ -112,11 +115,23 @@ __global__ void lins_vg_box_kernel(VgInfo* __restrict__ infos, int n_seg) {
   if (!v.any) return;
   long long div[3];
   for (int k = 0; k < 3; ++k) {
-    v.min_b[k] = lins_feat::voxel_bound(ord2f(v.enc[k]), v.inv);
-    div[k] = (long long)lins_feat::voxel_bound(ord2f(v.enc[3 + k]), v.inv) - v.min_b[k] + 1;
+    const float lo = floorf(ord2f(v.enc[k]) * v.inv), hi = floorf(ord2f(v.enc[3 + k]) * v.inv);
+    if (!(fabsf(lo) < 0x1p62f && fabsf(hi) < 0x1p62f)) { v.toobig = 1; return; }
+    v.base[k] = lo;
+    div[k] = (long long)hi - (long long)lo + 1;
   }
   v.toobig = (double)div[0] * (double)div[1] * (double)div[2] > (double)INT_MAX;  // (exact below 2^53; no overflow)
   v.mul[0] = 1; v.mul[1] = (int)div[0]; v.mul[2] = v.toobig ? 0 : (int)(div[0] * div[1]);
+}
+
+// a point's voxel key (feature_extraction.hpp: (int)(floor(p * inv) - (float)min_b) per axis): the f32 differences to
+// the box's f32 floor as int64, combined in 64 bits.  In a box of at most INT32_MAX voxels a difference rounds to at
+// most 2^31, and the key stays below 0xffffffff.
+__device__ __forceinline__ unsigned vg_key(const float4 q, const VgInfo& v) {
+  const long long i0 = (long long)(floorf(q.x * v.inv) - v.base[0]);
+  const long long i1 = (long long)(floorf(q.y * v.inv) - v.base[1]);
+  const long long i2 = (long long)(floorf(q.z * v.inv) - v.base[2]);
+  return (unsigned)(i0 + i1 * v.mul[1] + i2 * v.mul[2]);
 }
 
 // the keys, and NaN in every output record (the centroids then overwrite a segment's first `count`)
@@ -128,7 +143,7 @@ __global__ void __launch_bounds__(kVgThreads) lins_vg_key_kernel(const float4* _
   const int sgi = seg_of(sg, i);
   const VgInfo& v = info[sgi];
   const float4 q = p[i];
-  key[i] = make_key<Key>(sgi, v.any && !v.toobig && finite3(q) ? lins_feat::voxel_key(q.x, q.y, q.z, v.min_b, v.mul, v.inv) : kInvalidKey);
+  key[i] = make_key<Key>(sgi, v.any && !v.toobig && finite3(q) ? vg_key(q, v) : kInvalidKey);
   idx[i] = i;
   const float nan = __int_as_float(0xffffffff);
   if (sg.n == 1) out[i] = make_float4(nan, nan, nan, nan);

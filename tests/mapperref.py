@@ -33,22 +33,28 @@ def atan2f(y, x): return F(_libm.atan2f(float(F(y)), float(F(x))))
 
 
 class TooBig(Exception):
-    """div_x * div_y * div_z > INT32_MAX (PCL's 'Leaf size is too small' case)."""
+    """div_x * div_y * div_z > INT32_MAX (PCL's 'Leaf size is too small' case), or a box bound floor(min / max * inv)
+    at or beyond 2^62 in magnitude, inf included."""
 
 
 def voxel_grid(pts, leaf):
     """pcl::VoxelGrid<PointXYZI>: (n, >=4) float32 rows (x, y, z, intensity) -> (m, 4) centroids.  Same semantics as
     tests/pyfront.voxel_grid (f32 sums in input order per voxel, ascending voxel index), vectorised by rank within the
     voxel so that 10^6 points stay fast: the k-th points of all voxels are added in one step, in order k = 0, 1, ..."""
-    p = np.asarray(pts, F).reshape(len(pts), -1)[:, :4]
+    p = np.asarray(pts, F)
+    if p.size == 0:
+        return np.zeros((0, 4), F)
+    p = p.reshape(len(p), -1)[:, :4]
     fin = np.isfinite(p[:, :3]).all(1)
     if not fin.any():
         return np.zeros((0, 4), F)
     inv = F(1.0) / F(leaf)
     q = p[fin]
     with np.errstate(over="ignore"):
-        min_b = np.floor(q[:, :3].min(0) * inv).astype(np.int64)
-        max_b = np.floor(q[:, :3].max(0) * inv).astype(np.int64)
+        lo, hi = np.floor(q[:, :3].min(0) * inv), np.floor(q[:, :3].max(0) * inv)
+    if not (np.abs(lo) < F(2.0 ** 62)).all() or not (np.abs(hi) < F(2.0 ** 62)).all():
+        raise TooBig((lo, hi))  # (no exact int64 box: an overflow to inf, or 2^62 voxels from the origin)
+    min_b, max_b = lo.astype(np.int64), hi.astype(np.int64)
     div = max_b - min_b + 1
     if float(div[0]) * float(div[1]) * float(div[2]) > INT32_MAX:
         raise TooBig(div)

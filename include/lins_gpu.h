@@ -665,6 +665,47 @@ int lins_gpu_mappers_step(lins_ctx* ctx, const lins_mappers_desc* d, lins_mapper
 int lins_gpu_mappers_download(lins_ctx* ctx, int32_t slot, double* key_poses, int32_t* window, float* map_corner_ds,
                               float* map_surf_ds, float* corner_ds, float* surf_ds, float* outlier_ds, float* surf_total_ds);
 
+/* ---- sequence mode feeding its mapping nodes: LinsFusion::publishTopics (Estimator.cpp:177-202, :254-320) on the device ---
+   A run opened by lins_gpu_seq_open can be bound to the context's lockstep mappers: slot s of the sequence run feeds
+   mapper slot s.  After every sequence step (lins_gpu_seq_step, _ex, _pcl, _raw, _cloud2 and the _mixed forms) the run
+   takes exactly one lins_gpu_seq_map_step, which publishes what each slot's estimator would and runs those slots'
+   mapping cycles in one lins_gpu_mappers_step on the device clouds, with no host copy of a cloud.  A slot publishes
+   after every scan of an estimator that was initialised before the scan (status_ != STATUS_INIT): its stamp,
+   globalStateYZX_ and scan_last_'s YZX less-sharp, less-flat and outlier clouds, which only an accepted scan
+   (LINS_SEQ_SECOND / RAN / ICP) replaces; a first scan (LINS_SEQ_FIRST) leaves them empty, a skipped scan publishes the
+   previous ones again, an absent slot or an estimator still in STATUS_INIT publishes nothing.  Per slot the mapper's
+   reports and downloads are bit-identical to lins_gpu_mappers_step fed the same clouds from the host.
+   lins_gpu_mappers_imu, _download and _reset work on the bound run as on any lockstep run.  An unbound run is unchanged. */
+typedef struct lins_seq_map_desc {
+  int32_t n_seq;                 /* == S */
+  int32_t pad;
+  const double* time;            /* S: scan_time_ of each present slot's scan in the last step */
+  const lins_point* outlier; const int32_t* outlier_off;  /* S + 1 CSR: the outlier clouds processPCL received with the
+                                    last step's scans.  NULL after a _raw / _cloud2 step (the projection made them on the
+                                    device), required after a lins_gpu_seq_step / _ex / _pcl step */
+} lins_seq_map_desc;
+/* Binds the open sequence run to the lockstep mappers, opened with M = S fresh slots (replacing any open lockstep run, as
+   lins_gpu_mappers_open does).  LINS_E_NOMAP without a run; LINS_E_INVALID for a run of lins_gpu_seq_begin (a hand-over
+   carries no outlier cloud and no publish state) or after the run's first step.  lins_gpu_seq_open, lins_gpu_seq_begin,
+   lins_gpu_mappers_open and a step error that drops the run end the binding.  On a bound run lins_gpu_seq_restart also
+   resets the restarted slots' mappers and publish state (a new recording is a new LinsFusion with a new mapping node). */
+int lins_gpu_seq_map_open(lins_ctx* ctx);
+/* publishTopics for every slot of the last step, then one lins_gpu_mappers_step of the slots that published: published[s]
+   receives the decision, reps[s] the report of a published slot (either may be NULL).  At most one stream
+   synchronisation (the mapper step's; none when no slot's cycle passes the 0.3 s gate), whatever S is.
+   LINS_E_NOMAP on an unbound run.  LINS_E_INVALID before anything changes with no step since the last call, a wrong
+   n_seq, a NULL time, bad outlier offsets, or outliers given after a _raw / _cloud2 step or missing after another step;
+   a sequence step of a bound run whose publish is still pending returns LINS_E_INVALID before anything changes.
+   LINS_E_TOOBIG as lins_gpu_mappers_step: no mapper slot changes, but the estimator side of the publish is committed
+   and the next sequence step may run. */
+int lins_gpu_seq_map_step(lins_ctx* ctx, const lins_seq_map_desc* d, lins_mapper_report* reps /*S or NULL*/,
+                          uint8_t* published /*S or NULL*/);
+/* what each slot's estimator publishes (what the last lins_gpu_seq_map_step fed a published slot's mapper): pose =
+   globalStateYZX_ (S x 7: position, quaternion x y z w; the identity before the slot's first accepted scan since open /
+   restart), sizes = the points of its less-sharp, less-flat and outlier YZX clouds (S x 3).  Either may be NULL.
+   LINS_E_NOMAP on an unbound run. */
+int lins_gpu_seq_map_published(lins_ctx* ctx, double* pose /*S x 7*/, int32_t* sizes /*S x 3*/);
+
 /* block until everything queued on the ctx stream has finished */
 int lins_gpu_sync(lins_ctx* ctx);
 

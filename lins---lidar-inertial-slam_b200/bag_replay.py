@@ -12,6 +12,9 @@ step hands each present slot's PointCloud2 data field to lins_gpu_seq_step_cloud
 device.  Bags of different sensors run together: each bag names its lidar model, and a step whose slots hold bags of more
 than one model goes through lins_gpu_seq_step_cloud2_mixed, each slot projected with its bag's model.  A step's data fields are gathered into one host buffer that is page-locked once (re-registered only when it
 grows), so each step's bytes go to the device in one DMA.
+With map=True the run is bound to the context's lockstep mappers (lins_gpu_seq_map_open): after every step
+lins_gpu_seq_map_step publishes what each slot's LinsFusion::publishTopics would and runs the mapping cycles of the slots
+that published, on the device clouds.
 """
 import ctypes as C
 import importlib.util
@@ -157,20 +160,43 @@ def model_table(recordings, model):
     return models, of
 
 
-def replay(recordings, slots, model=None, device=0, gpu=None):
+def replay(recordings, slots, model=None, device=0, gpu=None, map=False):
     """Run the recordings through `slots` slots of one context.  model: one LinsLidarModel for every recording (None =
     VLP-16) or a list with one per recording; a slot is projected with the model of the recording it holds.  Returns per
     recording a dict of per-scan arrays: stamps, status (StateEstimator::status_ after the scan), scan_status (LINS_SEQ_*),
-    global_est (n x 7: rn, qbn x y z w), global_state (n x 19), iters and flags (-1 where the scan ran no IESKF)."""
+    global_est (n x 7: rn, qbn x y z w), global_state (n x 19), iters and flags (-1 where the scan ran no IESKF).
+    map=True also runs each recording's mapping node on what its estimator publishes (the IMU orientation is not fed to
+    the mappers, as tools/run_bag.py --map does not), and adds per published scan: map_time, map_odom (m x 7: the
+    odometry, YZX position + quaternion x y z w of globalStateYZX_, as fed to the mapper), map_sizes (m x 3: the
+    less-sharp, less-flat and outlier cloud sizes), map_processed, map_aft_mapped (m x 6: transformAftMapped) and
+    map_keyframes (n_keyframes after the cycle); and key_poses (the mapper's cloudKeyPoses6D, k x
+    7, downloaded when the recording ends)."""
     models, rec_model = model_table(recordings, model)
     g = gpu or _capi.LinsGpu(device=device)
     g.seq_open(LinsSeqParams.shipped(), shim_init_params(), slots)
     out = [dict(stamps=r.stamps.copy(), status=np.zeros(len(r), np.int32), scan_status=np.zeros(len(r), np.int32),
                 global_est=np.zeros((len(r), 7)), global_state=np.zeros((len(r), 19)), iters=np.full(len(r), -1, np.int32),
                 flags=np.full(len(r), -1, np.int32)) for r in recordings]
+    if map:
+        g.seq_map_open()
+        for o in out:
+            o.update(map_time=[], map_odom=[], map_processed=[], map_aft_mapped=[], map_keyframes=[], map_sizes=[], key_poses=np.zeros((0, 7)))
+        held = [None] * slots  # (recording, last published report) of each slot
     blob = _PinnedBlob()
+
+    def finish(j):  # the key poses of the recording slot j held, before the slot is handed on
+        if held[j] is not None and held[j][1] is not None:
+            kp = np.zeros((held[j][1].n_keyframes, 7))
+            g._ck(g.L.lins_gpu_mappers_download(g.h, j, _capi.ptr(kp), *[None] * 7))
+            out[held[j][0]]["key_poses"] = kp
+        held[j] = None
+
     try:
         for restart, who in slot_queue([len(r) for r in recordings], slots):
+            if map:
+                for j in range(slots):
+                    if held[j] is not None and (who[j] is None or who[j][0] != held[j][0]):
+                        finish(j)
             if restart.any():
                 g.seq_restart(restart)
             present = np.array([w is not None for w in who], np.uint8)
@@ -202,6 +228,31 @@ def replay(recordings, slots, model=None, device=0, gpu=None):
                 o["global_est"][k] = np.concatenate([gs[0:3], gs[6:10]])
                 if d["status"][j] in (SEQ_RAN, SEQ_ICP):
                     o["iters"][k], o["flags"][k] = d["results"]["iters"][j], d["results"]["flags"][j]
+            if map:
+                time = np.array([recordings[w[0]].stamps[w[1]] if w else 0.0 for w in who])
+                reps, pub = g.seq_map_step(time)
+                pose, sizes = g.seq_map_published()  # (the odometry and cloud sizes each slot's mapper was fed)
+                for j, w in enumerate(who):
+                    if w is None:
+                        continue
+                    if held[j] is None:
+                        held[j] = (w[0], None)
+                    if not pub[j]:
+                        continue
+                    o, r = out[w[0]], reps[j]
+                    held[j] = (w[0], r)
+                    o["map_time"].append(time[j]); o["map_odom"].append(pose[j].copy()); o["map_processed"].append(r.processed)
+                    o["map_aft_mapped"].append(list(r.transform_aft_mapped)); o["map_keyframes"].append(r.n_keyframes)
+                    o["map_sizes"].append(sizes[j].copy())
+        if map:
+            for j in range(slots):
+                finish(j)
+            for o in out:
+                o["map_time"] = np.array(o["map_time"]); o["map_odom"] = np.array(o["map_odom"]).reshape(-1, 7)
+                o["map_processed"] = np.array(o["map_processed"], np.int32)
+                o["map_aft_mapped"] = np.array(o["map_aft_mapped"], np.float32).reshape(-1, 6)
+                o["map_keyframes"] = np.array(o["map_keyframes"], np.int32)
+                o["map_sizes"] = np.array(o["map_sizes"], np.int32).reshape(-1, 3)
     finally:
         blob.release()
     return out

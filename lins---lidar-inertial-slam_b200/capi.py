@@ -15,7 +15,7 @@ import numpy as np
 
 from .ctypes_defs import (Batch, COV_SIZE, LinsBatchDesc, LinsCloud2Desc, LinsCloud2Layout, LinsFeatureParams, LinsLidarModel, LinsLidarModels, LinsMapperDesc, LinsMapperReport, LinsMappersDesc, LinsMapReport, LinsParams, LinsPclDesc,
                           LinsRawDesc, LinsReport, LinsScanResult, LinsSeqBeginDesc, LinsSeqInitParams, LinsSeqParams, LinsSeqPclDesc,
-                          LinsSeqCloud2Desc, LinsSeqRawDesc, LinsSeqStepDesc, POINT_DTYPE, SCAN_RESULT_DTYPE, STATE_DIM, as_points, make_points, ptr)
+                          LinsSeqCloud2Desc, LinsSeqMapDesc, LinsSeqRawDesc, LinsSeqStepDesc, POINT_DTYPE, SCAN_RESULT_DTYPE, STATE_DIM, as_points, make_points, ptr)
 
 _PKG = os.path.dirname(os.path.abspath(__file__))
 _ROOT = os.path.dirname(_PKG)
@@ -38,6 +38,7 @@ EXPORTS = [
     "lins_gpu_project_scans_mixed", "lins_gpu_seq_step_raw_mixed", "lins_gpu_seq_step_cloud2_mixed",
     "lins_gpu_mapper_reset", "lins_gpu_mapper_imu", "lins_gpu_mapper_step", "lins_gpu_mapper_download", "lins_gpu_voxel_grid",
     "lins_gpu_mappers_open", "lins_gpu_mappers_reset", "lins_gpu_mappers_imu", "lins_gpu_mappers_step", "lins_gpu_mappers_download",
+    "lins_gpu_seq_map_open", "lins_gpu_seq_map_step", "lins_gpu_seq_map_published",
 ]
 
 NVCC_ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]  # H100 (Hopper)
@@ -143,6 +144,9 @@ def lib():
         L.lins_gpu_mappers_imu.argtypes = [vp, vp, vp, vp, vp]
         L.lins_gpu_mappers_step.argtypes = [vp, C.POINTER(LinsMappersDesc), vp]
         L.lins_gpu_mappers_download.argtypes = [vp, C.c_int32] + [vp] * 8
+        L.lins_gpu_seq_map_open.argtypes = [vp]
+        L.lins_gpu_seq_map_step.argtypes = [vp, C.POINTER(LinsSeqMapDesc), vp, vp]
+        L.lins_gpu_seq_map_published.argtypes = [vp, vp, vp]
         _LIB = L
     return _LIB
 
@@ -407,6 +411,37 @@ class LinsGpu:
     def mappers_download(self, slot, rep):
         """mapper_download of one slot: (key poses, window, clouds) with the sizes its last processed cycle's report gives."""
         return self._download_node(lambda *out: self.L.lins_gpu_mappers_download(self.h, int(slot), *out), rep)
+
+    # ---- sequence mode feeding its mapping nodes (lins_gpu_seq_map_*) ---------------------------------------------
+    def seq_map_open(self):
+        """Bind the open sequence run (seq_open, before its first step) to S fresh lockstep mapper slots: slot s feeds
+        mapper slot s."""
+        self._ck(self.L.lins_gpu_seq_map_open(self.h))
+        self._mappers_n = self._seq_n
+
+    def seq_map_step(self, time, outlier=None):
+        """publishTopics after the last sequence step and the published slots' mapping cycles.  time: S scan stamps;
+        outlier: after a seq_step / seq_step_pcl step, the S outlier clouds its scans came with (None after seq_step_raw /
+        seq_step_cloud2).  Returns (reports: a LinsMapperReport per published slot, None elsewhere; published: S uint8)."""
+        n = self._seq_n
+        t = np.ascontiguousarray(time, np.float64).reshape(-1)
+        if len(t) != n:
+            raise ValueError(f"time has {len(t)} entries, the run {n}")
+        d = LinsSeqMapDesc(n_seq=n, time=ptr(t))
+        if outlier is not None:
+            pts, off = pack_csr(outlier)
+            d.outlier, d.outlier_off = ptr(pts), ptr(off)
+        reps = (LinsMapperReport * n)()
+        published = np.zeros(n, np.uint8)
+        self._ck(self.L.lins_gpu_seq_map_step(self.h, C.byref(d), C.cast(reps, C.c_void_p), ptr(published)))
+        return [reps[s] if published[s] else None for s in range(n)], published
+
+    def seq_map_published(self):
+        """What each slot publishes, as the last seq_map_step fed a published slot's mapper: (pose (S, 7): globalStateYZX_,
+        position + quaternion x y z w; sizes (S, 3): points of the less-sharp, less-flat and outlier YZX clouds)."""
+        pose, sizes = np.zeros((self._seq_n, 7)), np.zeros((self._seq_n, 3), np.int32)
+        self._ck(self.L.lins_gpu_seq_map_published(self.h, ptr(pose), ptr(sizes)))
+        return pose, sizes
 
     # ---- batched mode ------------------------------------------------------------------------------------------
     def batch_upload(self, batch):

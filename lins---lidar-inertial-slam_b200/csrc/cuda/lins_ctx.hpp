@@ -110,8 +110,9 @@ struct EventPair {
 
 // A gather list: contiguous device-to-device copies of float4 records, staged in pinned memory, copied to the device in
 // one H2D and run by one launch of a block per copy (lins_upload.cu).  Each user keeps its own list: a list's staging may
-// still be read by a queued H2D when another list is written.
-struct DevCopy { const float4* src; float4* dst; int n, pad; };
+// still be read by a queued H2D when another list is written.  yzx != 0: the copy writes (y, z, x, w) of each record, the
+// mapping node's axis order (sequence mode's publish step); 0: the record as it is.
+struct DevCopy { const float4* src; float4* dst; int n, yzx; };
 struct CopyList {
   Buf<DevCopy> dev; Buf<DevCopy, kPinned> host;
   // room for n records (before any work is queued: growth frees the old buffers); records [base, base + n) from src into
@@ -119,6 +120,29 @@ struct CopyList {
   int reserve(lins_ctx* ctx, size_t n);
   int stage(lins_ctx* ctx, const DevCopy* src, int n, int base);
   int launch(lins_ctx* ctx, int base, int n);
+};
+// one device range of float4 records: len points at src
+struct MapPiece { const float4* src = nullptr; int len = 0; };
+
+// Sequence mode's publish step (lins_gpu_seq_map_*, lins_seq.cu): what LinsFusion::publishTopics hands each slot's
+// mapping node (scan_last_'s YZX clouds, globalStateYZX_), kept for a run bound to the lockstep mappers.  Maps and the
+// kept outlier clouds are in XYZ order; the mapper step's gather writes them YZX.
+struct SeqPubState {
+  bool bound = false;                  // lins_gpu_seq_map_open bound the run (ends with seq_open / seq_begin / mappers_open)
+  bool pending = false;                // a step has run whose lins_gpu_seq_map_step has not
+  bool dev_outliers = false;           // the last step projected its scans on the device (_raw / _cloud2): the stash holds
+                                       // their outlier clouds
+  std::vector<int32_t> fusion_before;  // each slot's StateEstimator::status_ before the last step
+  std::vector<unsigned char> yzx;      // the slot's YZX clouds exist (false after open, restart and a first scan)
+  std::vector<double> pose;            // n x 7: the slot's globalStateYZX_ (pos, quat x y z w)
+  Buf<float4> stash;                   // the last step's outlier clouds, dense in slot order at h_stash_off (n + 1)
+  std::vector<int> h_stash_off;
+  Buf<float4, kPinned> h_stash;        // staging of a caller's outlier clouds
+  Buf<float4> outl, noutl;             // the published outlier cloud of each slot: current and next generation
+  std::vector<int> h_outl_off, h_noutl_off;
+  Buf<double, kPinned> h_glob;         // n x 20: the global states after the last step
+  Buf<int, kPinned> h_proj_counts;     // n x 2: the last projection's counts (segmented, outlier)
+  CopyList copies;                     // the outlier stash, then the next outlier generation
 };
 
 // Sequence mode (lins_gpu_seq_*, lins_seq.cu): the running sequences' filter state and maps.  Maps are CSR over the
@@ -161,6 +185,7 @@ struct SeqState {
   bool ev_valid = false;
   bool has_step = false;                               // a step has run since lins_gpu_seq_begin
   std::vector<int> h_run_off;                          // 2 x (n + 1): the last step's compacted query offsets (surf, corner)
+  SeqPubState pub;                                     // the publish step of a run bound to the lockstep mappers
   ~SeqState() { for (cudaEvent_t e : ev) if (e) cudaEventDestroy(e); }
 };
 
@@ -613,5 +638,11 @@ int keyframes_queue(lins_ctx* ctx, const KfSave* saves, int n, Buf<unsigned char
 int mapper_node_download(lins_ctx* ctx, const MapperNode& m, const float4* const src[6], double* key_poses, int32_t* window, float* const dst[6]);
 // lins_mapper.cu: the non-empty copies of v through the gather list l, staged at entries base.. and run in one launch
 int queue_copies(lins_ctx* ctx, CopyList& l, std::vector<DevCopy> v, int base);
+// lins_mappers.cu: n_slots fresh mapping nodes in ms (replacing any open run); the slots with mask[s] != 0 back to the
+// fresh state; one lockstep step of ms's present slots on a checked descriptor, from d's host clouds or, with dev
+// (n_slots x 3: corner, surf, outlier), from device ranges in XYZ order that the step's gather writes YZX
+int mappers_open(lins_ctx* ctx, MappersState& ms, int n_slots);
+int mappers_reset(lins_ctx* ctx, MappersState& ms, const uint8_t* mask);
+int mappers_step(lins_ctx* ctx, MappersState& ms, const lins_mappers_desc* d, lins_mapper_report* reps, const MapPiece* dev);
 
 }  // namespace lins_capi

@@ -2,7 +2,8 @@
 // (lins_gpu_mapper_*, a run of one slot of its own): one MapperNode per slot, each stepped by the host logic of
 // lins_mapper.cu, with one queue of device work per step for every processed slot.
 //
-// Per step (one synchronisation): the scans of the processed slots in one H2D; one gather launch of every slot's window
+// Per step (one synchronisation): the scans of the processed slots in one H2D (or, from device clouds, in the gather
+// launch that follows: sequence mode's publish step, lins_seq.cu); one gather launch of every slot's window
 // into its local-map clouds; one segmented VoxelGrid over the five clouds of every slot (map corner 0.2 m, map surf
 // 0.4 m, corner 0.2 m, surf 0.4 m, outlier 0.4 m), one gather of each slot's surf DS + outlier DS and one segmented
 // VoxelGrid of those (0.4 m); every slot's grids and scan-to-map loop (lins_map.cu: map_queue_slots); the read-back of
@@ -30,6 +31,10 @@ int need_open(lins_ctx* ctx) {
 
 const char* const kBad = "VoxelGrid: the leaf is too small for the cloud's extent (div_x * div_y * div_z > INT32_MAX)";
 
+}  // namespace
+
+namespace lins_capi {
+
 // n_slots fresh mapping nodes in ms, replacing any open run
 int mappers_open(lins_ctx* ctx, MappersState& ms, int n_slots) {
   CK(cudaSetDevice(ctx->device));
@@ -53,16 +58,27 @@ int mappers_reset(lins_ctx* ctx, MappersState& ms, const uint8_t* mask) {
   return LINS_OK;
 }
 
+}  // namespace lins_capi
+
+namespace {
+
 // imuHandler for every slot: slot s's rows are [off[s], off[s + 1])
 void mappers_imu(MappersState& ms, const int32_t* off, const double* time, const double* roll, const double* pitch) {
   for (int s = 0; s < ms.n; ++s) mapper_node_imu(ms.node[s].s, time + off[s], roll + off[s], pitch + off[s], off[s + 1] - off[s]);
 }
 
-// one step of every present slot of ms on a checked descriptor (d->n_slots == ms.n, valid offsets and arrays)
-int mappers_step(lins_ctx* ctx, MappersState& ms, const lins_mappers_desc* d, lins_mapper_report* reps) {
+}  // namespace
+
+namespace lins_capi {
+
+// one step of every present slot of ms on a checked descriptor (d->n_slots == ms.n, valid offsets and arrays).  dev
+// (M x 3: corner, surf, outlier, or null): the slots' clouds are device ranges in XYZ order, copied YZX-permuted into the
+// VoxelGrids' input by the local maps' gather launch; d's clouds are then not read.
+int mappers_step(lins_ctx* ctx, MappersState& ms, const lins_mappers_desc* d, lins_mapper_report* reps, const MapPiece* dev) {
   const int M = ms.n;
   const lins_point* src[3] = {d->corner, d->surf, d->outlier};
   const int32_t* off[3] = {d->corner_off, d->surf_off, d->outlier_off};
+  auto count = [&](int k, int s) { return dev ? dev[3 * s + k].len : off[k][s + 1] - off[k][s]; };
   CK(cudaSetDevice(ctx->device));
 
   // the host head of every present slot's cycle, on copies of its scalars (committed after the read-back)
@@ -82,7 +98,7 @@ int mappers_step(lins_ctx* ctx, MappersState& ms, const lins_mappers_desc* d, li
   };
   if (P == 0) return finish();
 
-  // round 1: segment 3p + k = scan cloud k of processed slot p (one H2D), 3P + 2p + k = its local map k; round 2:
+  // round 1: segment 3p + k = scan cloud k of processed slot p (one H2D, or gathered), 3P + 2p + k = its local map k; round 2:
   // segment p = its surf DS + outlier DS.  Every capacity is known here: the outputs are sized by the inputs.
   std::vector<int> h_off1(5 * P + 1), h_off2(P + 1), mapc(2 * P);
   std::vector<float> leaf1(5 * P), leaf2(P, 0.4f);
@@ -90,7 +106,7 @@ int mappers_step(lins_ctx* ctx, MappersState& ms, const lins_mappers_desc* d, li
   int n_scan = 0;
   for (int p = 0; p < P; ++p) {
     const int s = proc[p];
-    for (int k = 0; k < 3; ++k) { h_off1[3 * p + k] = n_scan; n_scan += off[k][s + 1] - off[k][s]; leaf1[3 * p + k] = k == 0 ? 0.2f : 0.4f; }
+    for (int k = 0; k < 3; ++k) { h_off1[3 * p + k] = n_scan; n_scan += count(k, s); leaf1[3 * p + k] = k == 0 ? 0.2f : 0.4f; }
     int nc = 0, nsf = 0;
     if (!ms.node[s].poses.empty()) mapper_window_sizes(ms.node[s], sc[s], nc, nsf);
     mapc[2 * p] = nc; mapc[2 * p + 1] = nsf;
@@ -107,11 +123,11 @@ int mappers_step(lins_ctx* ctx, MappersState& ms, const lins_mappers_desc* d, li
   int rc;
   if ((rc = voxel_grid_reserve(ctx, ms.vg, std::max(n1, n2), 5 * P)) != LINS_OK) return rc;
   if ((rc = voxel_grid_reserve(ctx, ms.vg, std::max(n1, n2), P)) != LINS_OK) return rc;
-  CK(ms.vin[0].grow((size_t)n1 + 1)); CK(ms.vin[1].grow((size_t)n2 + 1)); CK(ms.h_in.grow((size_t)n_scan + 1));
+  CK(ms.vin[0].grow((size_t)n1 + 1)); CK(ms.vin[1].grow((size_t)n2 + 1)); if (!dev) CK(ms.h_in.grow((size_t)n_scan + 1));
   CK(ms.vg_info.reserve(6 * (size_t)P)); CK(ms.h_vg_info.reserve(6 * (size_t)P)); CK(ms.h_vg_init.reserve(6 * (size_t)P));
   CK(ms.vg_off.reserve(6 * (size_t)P + 2)); CK(ms.h_vg_off.reserve(6 * (size_t)P + 2));
   CK(ms.vg_out.reserve(6 * (size_t)P)); CK(ms.h_vg_out.reserve(6 * (size_t)P));
-  size_t n_copies = 2 * (size_t)P;
+  size_t n_copies = (dev ? 5 : 2) * (size_t)P;
   for (int p = 0; p < P; ++p) {
     const int s = proc[p];
     auto& ds = ms.ds[s];
@@ -125,8 +141,16 @@ int mappers_step(lins_ctx* ctx, MappersState& ms, const lins_mappers_desc* d, li
   }
   if ((rc = ms.copies.reserve(ctx, n_copies)) != LINS_OK) return rc;
 
-  // the scans (one H2D) and the segment tables (outputs: the slots' own DS clouds, which persist for the download)
-  {
+  // the scans (one H2D; device clouds join the gather below) and the segment tables (outputs: the slots' own DS clouds,
+  // which persist for the download)
+  std::vector<DevCopy> copies;
+  if (dev) {
+    for (int p = 0; p < P; ++p)
+      for (int k = 0; k < 3; ++k) {
+        const MapPiece& c = dev[3 * proc[p] + k];
+        copies.push_back(DevCopy{c.src, ms.vin[0].p + h_off1[3 * p + k], c.len, 1});
+      }
+  } else {
     size_t o = 0;
     for (int p = 0; p < P; ++p)
       for (int k = 0; k < 3; ++k) {
@@ -143,7 +167,6 @@ int mappers_step(lins_ctx* ctx, MappersState& ms, const lins_mappers_desc* d, li
   CK(cudaMemcpyAsync(ms.vg_out.p, ms.h_vg_out.p, sizeof(float4*) * 6 * (size_t)P, cudaMemcpyHostToDevice, ctx->stream));
 
   // every slot's local map: corner_i ..., and surf_i, outlier_i interleaved (:1242-1246), one gather launch
-  std::vector<DevCopy> copies;
   for (int p = 0; p < P; ++p) {
     const MapperNode& m = ms.node[proc[p]];
     if (m.poses.empty()) continue;
@@ -214,6 +237,10 @@ int mappers_step(lins_ctx* ctx, MappersState& ms, const lins_mappers_desc* d, li
   return finish();
 }
 
+}  // namespace lins_capi
+
+namespace {
+
 // the key poses, window and last cycle's clouds of one slot (dst: NULL skips)
 int mappers_download(lins_ctx* ctx, MappersState& ms, int slot, double* key_poses, int32_t* window, float* const dst[6]) {
   CK(cudaSetDevice(ctx->device));
@@ -234,6 +261,7 @@ extern "C" {
 int lins_gpu_mappers_open(lins_ctx* ctx, int32_t n_slots) {
   if (!ctx) return LINS_E_INVALID;
   if (n_slots < 1) return fail(ctx, LINS_E_INVALID, "n_slots < 1");
+  ctx->seq.pub.bound = false;  // (a sequence run's mapping nodes are replaced)
   return mappers_open(ctx, ctx->mappers, n_slots);
 }
 
@@ -265,7 +293,7 @@ int lins_gpu_mappers_step(lins_ctx* ctx, const lins_mappers_desc* d, lins_mapper
   const int32_t* off[3] = {d->corner_off, d->surf_off, d->outlier_off};
   static const char* const what[3] = {"bad corner offsets / cloud", "bad surf offsets / cloud", "bad outlier offsets / cloud"};
   for (int k = 0; k < 3; ++k) if (check_csr(ctx, off[k], M, src[k], what[k]) != LINS_OK) return LINS_E_INVALID;
-  return mappers_step(ctx, ctx->mappers, d, reps);
+  return mappers_step(ctx, ctx->mappers, d, reps, nullptr);
 }
 
 int lins_gpu_mappers_download(lins_ctx* ctx, int32_t slot, double* key_poses, int32_t* window, float* map_corner_ds, float* map_surf_ds,
@@ -310,7 +338,7 @@ int lins_gpu_mapper_step(lins_ctx* ctx, const lins_mapper_desc* d, lins_mapper_r
   one.corner = d->corner; one.corner_off = off[0];
   one.surf = d->surf; one.surf_off = off[1];
   one.outlier = d->outlier; one.outlier_off = off[2];
-  return mappers_step(ctx, ctx->mapper, &one, rep);
+  return mappers_step(ctx, ctx->mapper, &one, rep, nullptr);
 }
 
 int lins_gpu_mapper_download(lins_ctx* ctx, double* key_poses, int32_t* window, float* map_corner_ds, float* map_surf_ds,

@@ -8,6 +8,10 @@
 //   pre-integrates a slot's IMU rows between its first and second scan, the second scans' estimateTransform runs as ONE
 //   batched icp_loop over all of them (lins_seq_icp_start_kernel sets its start poses), and lins_seq_init_kernel installs
 //   the state of processFirstScan / processSecondScan.
+// A run bound to the lockstep mappers (lins_gpu_seq_map_*) also keeps what each slot's scan_last_ would publish: the
+//   outlier clouds of the step's scans (a stash), the published outlier cloud (a generation, like the maps), whether the
+//   YZX clouds exist, and the global states (read back with the step's last synchronisation); lins_gpu_seq_map_step then
+//   runs publishTopics and one lockstep mapper step on the device clouds.
 // The filter algebra is lins_seq_step.cuh, shared with the CPU test.  Built with -fmad=false like the other bit-exact units.
 #include <cuda_runtime.h>
 
@@ -16,6 +20,7 @@
 #include <cstring>
 #include <vector>
 
+#include "../host/global_state_yzx.hpp"
 #include "lins_ctx.hpp"
 #include "lins_kernels.cuh"
 #include "lins_seq_step.cuh"
@@ -223,8 +228,7 @@ cudaError_t queue_map_state(lins_ctx* ctx, SeqState& q) {
 }
 
 // ---- map generations -----------------------------------------------------------------------------------------------------
-// Where one (cloud, slot) range of the next generation comes from: len points at src
-struct MapPiece { const float4* src = nullptr; int len = 0; };
+// Where one (cloud, slot) range of the next generation comes from: a MapPiece (lins_ctx.hpp)
 
 // cloud c (map_s, map_c, tree_s, tree_c) of slot s in the current generation
 MapPiece current_piece(const SeqState& q, int c, int s) {
@@ -269,6 +273,8 @@ int check_step(lins_ctx* ctx, const Desc* d, int n_scans, const double* scan_imu
   const int n = q.n;
   if (n == 0) return fail(ctx, LINS_E_NOMAP, "lins_gpu_seq_begin has not been called");
   if (!d || d->n_seq != n || n_scans != n) return fail(ctx, LINS_E_INVALID, "n_seq differs from the hand-over's");
+  if (q.pub.bound && q.pub.pending) return fail(ctx, LINS_E_INVALID, "the last step's lins_gpu_seq_map_step has not run");
+  q.pub.dev_outliers = false;  // (until a projection stashes them)
   if (d->imu_off) { const int rc = check_csr(ctx, d->imu_off, n, d->imu, "bad imu offsets / samples"); if (rc != LINS_OK) return rc; }
   else if (d->imu) return fail(ctx, LINS_E_INVALID, "imu without imu_off");
   if (!scan_imu)
@@ -306,6 +312,7 @@ int seq_step_phases(lins_ctx* ctx, const lins_seq_step_desc* d, const int32_t* c
   // ---- host bookkeeping: who runs, the compacted queries, the next maps (all from sizes the host knows) --------------
   std::vector<int32_t>& status = q.status;
   const int N1 = n + 1;
+  if (q.pub.bound) q.pub.fusion_before = q.fusion;  // (publishTopics' rule reads the status before the scan)
   std::vector<MapPiece> next(4 * (size_t)n);
   std::vector<unsigned char> new_stale(q.h_stale_v);
   std::vector<unsigned char> imu_use(n, IMU_IGNORE);
@@ -508,6 +515,7 @@ int seq_step_phases(lins_ctx* ctx, const lins_seq_step_desc* d, const int32_t* c
   q.h_stale_v = new_stale;
   CK(queue_map_state(ctx, q));
   CK(cudaEventRecord(q.ev[4], ctx->stream));
+  if (q.pub.bound) CK(cudaMemcpyAsync(q.pub.h_glob.p, q.glob.p, sizeof(double) * 20 * (size_t)n, cudaMemcpyDeviceToHost, ctx->stream));
   CK(cudaStreamSynchronize(ctx->stream));  // (the two sources above are pageable and change with the next step)
   for (int s = 0; s < n; ++s) {  // processPCL's status transitions (:294-307)
     if (status[s] == LINS_SEQ_INIT_WAIT) q.fusion[s] = FUSION_INIT;
@@ -525,6 +533,7 @@ int seq_step_phases(lins_ctx* ctx, const lins_seq_step_desc* d, const int32_t* c
 int seq_step_run(lins_ctx* ctx, const lins_seq_step_desc* d, const int32_t* const offs[4], const double* scan_imu) {
   const int rc = seq_step_phases(ctx, d, offs, scan_imu);
   if (rc != LINS_OK) ctx->seq.n = 0;
+  else if (ctx->seq.pub.bound) ctx->seq.pub.pending = true;
   return rc;
 }
 
@@ -575,15 +584,119 @@ int step_from_features(lins_ctx* ctx, const uint8_t* pres, const double* imu, co
 // the sequences change, then step_from_features.
 int step_from_projection(lins_ctx* ctx, const uint8_t* pres, const double* imu, const int32_t* imu_off, int line_num,
                          const lins_feature_params* fp, const int32_t* src_off, const double* scan_imu) {
-  const int n = ctx->seq.n;
+  SeqState& q = ctx->seq;
+  const int n = q.n;
   ProjState& pr = ctx->proj;
+  SeqPubState& pb = q.pub;
+  // a bound run keeps the outlier clouds: their counts join the extraction's read-back
+  if (pb.bound) CK(cudaMemcpyAsync(pb.h_proj_counts.p, pr.counts.p, sizeof(int) * 2 * (size_t)n, cudaMemcpyDeviceToHost, ctx->stream));
   FeatInputs in;
   in.n = n; in.line_num = line_num; in.total = src_off[n];
   in.pts = pr.seg.p; in.off = pr.up.qs_off.p; in.count = pr.counts.p; in.count_stride = 2;
   in.ground = pr.ground.p; in.col = pr.col.p; in.range = pr.range.p; in.ring = pr.ring.p; in.ori = pr.ori.p;
-  const int rc = features_launch(ctx, fp, in);
+  int rc = features_launch(ctx, fp, in);
   if (rc != LINS_OK) return rc;
+  if (pb.bound) {  // the stash: every slot's outlier cloud, device to device (an absent slot's sweep projected empty)
+    pb.h_stash_off.assign((size_t)n + 1, 0);
+    for (int s = 0; s < n; ++s) pb.h_stash_off[s + 1] = pb.h_stash_off[s] + pb.h_proj_counts.p[2 * s + 1];
+    CK(pb.stash.reserve((size_t)pb.h_stash_off[n] + 1));
+    std::vector<DevCopy> copies;
+    for (int s = 0; s < n; ++s) {
+      const int no = pb.h_stash_off[s + 1] - pb.h_stash_off[s];
+      if (no) copies.push_back(DevCopy{pr.outl.p + src_off[s], pb.stash.p + pb.h_stash_off[s], no, 0});
+    }
+    if ((rc = pb.copies.reserve(ctx, copies.size())) != LINS_OK) return rc;
+    if ((rc = pb.copies.stage(ctx, copies.data(), (int)copies.size(), 0)) != LINS_OK) return rc;
+    if ((rc = pb.copies.launch(ctx, 0, (int)copies.size())) != LINS_OK) return rc;
+    pb.dev_outliers = true;
+  }
   return step_from_features(ctx, pres, imu, imu_off, src_off, scan_imu);
+}
+
+// ---- the publish step of a bound run ---------------------------------------------------------------------------------
+// publishTopics' rule (Estimator.cpp:254-284): a slot publishes after every scan of an estimator that was initialised
+// before it, i.e. present with a status other than STATUS_INIT before the step
+bool publishes(int32_t status, int32_t fusion_before) {
+  return status != LINS_SEQ_IDLE && fusion_before != FUSION_INIT;
+}
+// updatePointCloud ran: the scan was accepted (SECOND / RAN / ICP)
+bool accepted(int32_t status) { return status == LINS_SEQ_SECOND || status == LINS_SEQ_RAN || status == LINS_SEQ_ICP; }
+
+// the state of a slot whose estimator is new: no YZX clouds, globalStateYZX_ the identity
+void pub_fresh(SeqPubState& pb, int s) {
+  pb.yzx[s] = 0;
+  static const double id[7] = {0, 0, 0, 0, 0, 0, 1};
+  std::copy(id, id + 7, &pb.pose[7 * (size_t)s]);
+}
+
+// lins_gpu_seq_map_step on a checked call: the estimator side (outlier stash and generation, YZX flags, poses) is
+// committed, then one lockstep mapper step of the publishing slots on the device clouds
+int seq_map_run(lins_ctx* ctx, const lins_seq_map_desc* d, lins_mapper_report* reps, uint8_t* published) {
+  SeqState& q = ctx->seq;
+  SeqPubState& pb = q.pub;
+  const int n = q.n;
+  CK(cudaSetDevice(ctx->device));
+  std::vector<uint8_t> pub(n, 0);
+  for (int s = 0; s < n; ++s) pub[s] = publishes(q.status[s], pb.fusion_before[s]) ? 1 : 0;
+  // a caller's outlier clouds into the stash (the last step ended with a synchronisation: the staging is free)
+  if (!pb.dev_outliers) {
+    const int total = d->outlier_off[n];
+    pb.h_stash_off.assign(d->outlier_off, d->outlier_off + n + 1);
+    CK(pb.stash.reserve((size_t)total + 1)); CK(pb.h_stash.reserve((size_t)total + 1));
+    if (total) {
+      pack_into(pb.h_stash.p, d->outlier, total);
+      CK(cudaMemcpyAsync(pb.stash.p, pb.h_stash.p, sizeof(float4) * total, cudaMemcpyHostToDevice, ctx->stream));
+    }
+  }
+  // updatePointCloud of the accepted scans (their YZX clouds and pose); processFirstScan's fresh scan_last_
+  for (int s = 0; s < n; ++s) {
+    const int32_t st = q.status[s];
+    if (st == LINS_SEQ_FIRST) pb.yzx[s] = 0;
+    if (!accepted(st)) continue;
+    pb.yzx[s] = 1;
+    const double* g = pb.h_glob.p + 20 * (size_t)s;  // rn = g[0..2], qbn = g[6..9]
+    lins::global_state_yzx(g, g + 6, &pb.pose[7 * (size_t)s], &pb.pose[7 * (size_t)s + 3]);
+  }
+  // the next outlier generation: an accepted scan's outliers, a slot without YZX clouds none, else the kept ones
+  const int N1 = n + 1;
+  pb.h_noutl_off.assign(N1, 0);
+  std::vector<MapPiece> next(n);
+  for (int s = 0; s < n; ++s) {
+    if (!pb.yzx[s]) next[s] = MapPiece{};
+    else if (accepted(q.status[s])) next[s] = MapPiece{pb.stash.p + pb.h_stash_off[s], pb.h_stash_off[s + 1] - pb.h_stash_off[s]};
+    else next[s] = MapPiece{pb.outl.p + pb.h_outl_off[s], pb.h_outl_off[s + 1] - pb.h_outl_off[s]};
+    pb.h_noutl_off[s + 1] = pb.h_noutl_off[s] + next[s].len;
+  }
+  CK(pb.noutl.reserve((size_t)pb.h_noutl_off[n] + 1));
+  std::vector<DevCopy> copies;
+  for (int s = 0; s < n; ++s)
+    if (next[s].len) copies.push_back(DevCopy{next[s].src, pb.noutl.p + pb.h_noutl_off[s], next[s].len, 0});
+  int rc = pb.copies.reserve(ctx, copies.size());
+  if (rc == LINS_OK) rc = pb.copies.stage(ctx, copies.data(), (int)copies.size(), 0);
+  if (rc == LINS_OK) rc = pb.copies.launch(ctx, 0, (int)copies.size());
+  if (rc != LINS_OK) return rc;
+  std::swap(pb.outl, pb.noutl);
+  pb.h_outl_off.swap(pb.h_noutl_off);
+  pb.pending = false;
+  if (published) std::copy(pub.begin(), pub.end(), published);
+
+  // the mapping nodes' inputs: scan_last_'s less-sharp / less-flat clouds are the slot's current maps, in XYZ order
+  std::vector<MapPiece> dev(3 * (size_t)n);
+  std::vector<double> quat(4 * (size_t)n), pos(3 * (size_t)n);
+  for (int s = 0; s < n; ++s) {
+    if (!pub[s]) continue;
+    if (pb.yzx[s]) {
+      dev[3 * s + 0] = current_piece(q, 1, s);
+      dev[3 * s + 1] = current_piece(q, 0, s);
+      dev[3 * s + 2] = MapPiece{pb.outl.p + pb.h_outl_off[s], pb.h_outl_off[s + 1] - pb.h_outl_off[s]};
+    }
+    std::copy(&pb.pose[7 * (size_t)s], &pb.pose[7 * (size_t)s] + 3, &pos[3 * (size_t)s]);
+    std::copy(&pb.pose[7 * (size_t)s] + 3, &pb.pose[7 * (size_t)s] + 7, &quat[4 * (size_t)s]);
+  }
+  lins_mappers_desc md;
+  std::memset(&md, 0, sizeof(md));
+  md.n_slots = n; md.present = pub.data(); md.time = d->time; md.quat = quat.data(); md.pos = pos.data();
+  return mappers_step(ctx, ctx->mappers, &md, reps, dev.data());
 }
 
 }  // namespace
@@ -602,6 +715,7 @@ int lins_gpu_seq_begin(lins_ctx* ctx, const lins_seq_params* prm, const lins_seq
   CK(cudaSetDevice(ctx->device));
   SeqState& q = ctx->seq;
   q.n = 0;  // (until the hand-over is in place)
+  q.pub.bound = false;
   // the maps go through the batch uploader as the target clouds of n units without queries
   std::vector<int32_t> zeros(n + 1, 0);
   const lins_point* pts[4] = {nullptr, nullptr, d->surf_map, d->corner_map};
@@ -642,6 +756,7 @@ int lins_gpu_seq_open(lins_ctx* ctx, const lins_seq_params* prm, const lins_seq_
   CK(cudaSetDevice(ctx->device));
   SeqState& q = ctx->seq;
   q.n = 0;  // (until the slots are in place)
+  q.pub.bound = false;
   const int n = n_seq;
   int rc = reserve_run(ctx, q, n, 0, 0);  // (no maps)
   if (rc != LINS_OK) return rc;
@@ -692,6 +807,10 @@ int lins_gpu_seq_restart(lins_ctx* ctx, const uint8_t* mask) {
   swap_maps(q);
   for (int s = 0; s < n; ++s)
     if (mask[s]) { q.h_stale_v[s] = 0; q.fusion[s] = FUSION_INIT; q.status[s] = LINS_SEQ_IDLE; }
+  if (q.pub.bound) {  // a new recording is a new LinsFusion with a new mapping node
+    for (int s = 0; s < n; ++s) if (mask[s]) pub_fresh(q.pub, s);
+    if ((rc = mappers_reset(ctx, ctx->mappers, mask)) != LINS_OK) return rc;
+  }
   CK(queue_map_state(ctx, q));
   CK(cudaStreamSynchronize(ctx->stream));  // (the two sources above are pageable)
   return LINS_OK;
@@ -759,6 +878,62 @@ int lins_gpu_seq_step_cloud2(lins_ctx* ctx, const lins_seq_cloud2_desc* d, const
                              const double* scan_imu) {
   const lins_lidar_models t = {1, m, nullptr};
   return lins_gpu_seq_step_cloud2_mixed(ctx, d, &t, fp, scan_imu);
+}
+
+int lins_gpu_seq_map_open(lins_ctx* ctx) {
+  if (!ctx) return LINS_E_INVALID;
+  SeqState& q = ctx->seq;
+  if (q.n == 0) return fail(ctx, LINS_E_NOMAP, "no sequence run: call lins_gpu_seq_open");
+  if (!q.has_init) return fail(ctx, LINS_E_INVALID, "lins_gpu_seq_map_open needs a run opened by lins_gpu_seq_open");
+  if (q.has_step) return fail(ctx, LINS_E_INVALID, "lins_gpu_seq_map_open after the run's first step");
+  const int n = q.n;
+  SeqPubState& pb = q.pub;
+  CK(cudaSetDevice(ctx->device));
+  CK(pb.h_glob.reserve(20 * (size_t)n)); CK(pb.h_proj_counts.reserve(2 * (size_t)n)); CK(pb.outl.reserve(1));
+  int rc = mappers_open(ctx, ctx->mappers, n);
+  if (rc != LINS_OK) return rc;
+  pb.yzx.assign(n, 0);
+  pb.pose.assign(7 * (size_t)n, 0.0);
+  for (int s = 0; s < n; ++s) pub_fresh(pb, s);
+  pb.h_outl_off.assign((size_t)n + 1, 0);
+  pb.fusion_before.assign(n, FUSION_INIT);
+  pb.pending = false;
+  pb.dev_outliers = false;
+  pb.bound = true;
+  return LINS_OK;
+}
+
+int lins_gpu_seq_map_step(lins_ctx* ctx, const lins_seq_map_desc* d, lins_mapper_report* reps, uint8_t* published) {
+  if (!ctx) return LINS_E_INVALID;
+  SeqState& q = ctx->seq;
+  if (q.n == 0 || !q.pub.bound) return fail(ctx, LINS_E_NOMAP, "no sequence run bound by lins_gpu_seq_map_open");
+  const int n = q.n;
+  if (!d) return fail(ctx, LINS_E_INVALID, "null desc");
+  if (!q.pub.pending) return fail(ctx, LINS_E_INVALID, "no sequence step since the last lins_gpu_seq_map_step");
+  if (d->n_seq != n) return fail(ctx, LINS_E_INVALID, "n_seq differs from the run's");
+  if (!d->time) return fail(ctx, LINS_E_INVALID, "null time");
+  const bool given = d->outlier || d->outlier_off;
+  if (q.pub.dev_outliers && given) return fail(ctx, LINS_E_INVALID, "outliers after a step that projected its scans on the device");
+  if (!q.pub.dev_outliers) {
+    if (!given) return fail(ctx, LINS_E_INVALID, "the last step's outlier clouds are required after a _ex / _pcl step");
+    if (check_csr(ctx, d->outlier_off, n, d->outlier, "bad outlier offsets / cloud") != LINS_OK) return LINS_E_INVALID;
+  }
+  return seq_map_run(ctx, d, reps, published);
+}
+
+int lins_gpu_seq_map_published(lins_ctx* ctx, double* pose, int32_t* sizes) {
+  if (!ctx) return LINS_E_INVALID;
+  SeqState& q = ctx->seq;
+  if (q.n == 0 || !q.pub.bound) return fail(ctx, LINS_E_NOMAP, "no sequence run bound by lins_gpu_seq_map_open");
+  const SeqPubState& pb = q.pub;
+  if (pose) std::copy(pb.pose.begin(), pb.pose.end(), pose);
+  for (int s = 0; s < q.n && sizes; ++s) {
+    const bool y = pb.yzx[s];
+    sizes[3 * s + 0] = y ? current_piece(q, 1, s).len : 0;
+    sizes[3 * s + 1] = y ? current_piece(q, 0, s).len : 0;
+    sizes[3 * s + 2] = y ? pb.h_outl_off[s + 1] - pb.h_outl_off[s] : 0;
+  }
+  return LINS_OK;
 }
 
 int lins_gpu_seq_phase_ms(lins_ctx* ctx, float* ms) {

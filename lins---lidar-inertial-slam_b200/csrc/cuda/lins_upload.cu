@@ -28,10 +28,13 @@ __global__ void lins_pack_points_kernel(const float4* __restrict__ raw, float4* 
   }
 }
 
-// one block per record of a gather list (lins_ctx.hpp: CopyList)
+// one block per record of a gather list (lins_ctx.hpp: CopyList); a record flagged yzx permutes each point to (y, z, x, w)
 __global__ void lins_copy_kernel(const DevCopy* __restrict__ copies) {
   const DevCopy c = copies[blockIdx.x];
-  for (int i = threadIdx.x; i < c.n; i += blockDim.x) c.dst[i] = c.src[i];
+  if (c.yzx)
+    for (int i = threadIdx.x; i < c.n; i += blockDim.x) { const float4 p = c.src[i]; c.dst[i] = make_float4(p.y, p.z, p.x, p.w); }
+  else
+    for (int i = threadIdx.x; i < c.n; i += blockDim.x) c.dst[i] = c.src[i];
 }
 
 }  // namespace

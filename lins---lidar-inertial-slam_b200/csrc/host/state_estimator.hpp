@@ -22,6 +22,7 @@
 #include "../../../include/lins_gpu.h"
 #include "cloud.hpp"
 #include "feature_extraction.hpp"
+#include "global_state_yzx.hpp"
 #include "kalman_filter.hpp"
 
 namespace lins {
@@ -311,8 +312,7 @@ class StateEstimator {
     for (const auto& p : scan_new_->cornerPointsLessSharp_.points) scan_new_->cornerPointsLessSharpYZX_.push_back(makePoint(p.y, p.z, p.x, p.intensity));
     for (const auto& p : scan_new_->surfPointsLessFlat_.points) scan_new_->surfPointsLessFlatYZX_.push_back(makePoint(p.y, p.z, p.x, p.intensity));
     for (const auto& p : scan_new_->outlierPointCloud_.points) scan_new_->outlierPointCloudYZX_.push_back(makePoint(p.y, p.z, p.x, p.intensity));
-    globalStateYZX_.rn_ = Q_xyz_to_yzx * globalState_.rn_;
-    globalStateYZX_.qbn_ = Q_xyz_to_yzx * globalState_.qbn_ * Q_xyz_to_yzx.inverse();
+    global_state_yzx(globalState_.rn_.d.data(), globalState_.qbn_.c.data(), globalStateYZX_.rn_.d.data(), globalStateYZX_.qbn_.c.data());
   }
 
  public:

@@ -74,6 +74,12 @@ class LinsMappersDesc(C.Structure):
                 ("outlier", C.c_void_p), ("outlier_off", C.c_void_p)]
 
 
+class LinsSeqMapDesc(C.Structure):
+    """lins_seq_map_desc (include/lins_gpu.h): the publish step after a sequence step: the scans' stamps and, after a step
+    whose scans did not come through the device projection, their outlier clouds (CSR)."""
+    _fields_ = [("n_seq", C.c_int32), ("pad", C.c_int32), ("time", C.c_void_p), ("outlier", C.c_void_p), ("outlier_off", C.c_void_p)]
+
+
 class LinsMapperReport(C.Structure):
     """lins_mapper_report (include/lins_gpu.h)."""
     _fields_ = [("processed", C.c_int32), ("skipped_interval", C.c_int32), ("n_map_corner_ds", C.c_int32),

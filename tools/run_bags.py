@@ -1,12 +1,15 @@
 #!/usr/bin/env python
-"""tools/run_bags.py BAG... [--slots S] [--lidar /velodyne_points] [--imu /imu/data] [--max-scans N] [--lidar-model M] [--out DIR]
+"""tools/run_bags.py BAG... [--slots S] [--lidar /velodyne_points] [--imu /imu/data] [--max-scans N] [--lidar-model M] [--map] [--out DIR]
 
 Replays many ROS1 bags through sequence mode in lockstep (bag_replay.py): every bag is scheduled as tools/run_bag.py
 schedules one, the bags are queued through S slots, and each scan's sensor_msgs/PointCloud2 message is decoded on the
 device (lins_gpu_seq_step_cloud2).  --lidar-model is 0 (VLP-16) or 1 (64 x 1024) for every bag, or a comma-separated list
 with one value per bag (e.g. 0,1,1,0): bags of different sensors then run in one context, each slot projected with its
 bag's model (lins_gpu_seq_step_cloud2_mixed).  Prints a summary line and the trajectory per bag, like run_bag.py; with
---out, writes DIR/<bag name>.npz (stamps, status, scan_status, global_est, iters, flags per scan)."""
+--out, writes DIR/<bag name>.npz (stamps, status, scan_status, global_est, iters, flags per scan).  With --map, each
+bag's mapping node runs on what its estimator publishes, in lockstep on the device (lins_gpu_seq_map_step), and
+DIR/<bag name>.odometry.txt and DIR/<bag name>.mapped.txt (DIR: --out, default .) receive the two trajectories in
+tools/run_bag.py --map's line format; like run_bag.py --map, the bags' IMU orientation is not fed to the mappers."""
 import argparse, importlib, os, sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import numpy as np
@@ -28,12 +31,26 @@ def lidar_models(spec, n_bags):
     return [presets[v]() for v in vals]
 
 
+def write_map(o, out_dir, name):
+    """<name>.odometry.txt and <name>.mapped.txt of one replayed bag, one line per published scan as tools/run_bag.py --map
+    writes odometry.txt and mapped.txt: stamp, then x y z qx qy qz qw of the odometry, resp. the processed flag and
+    transformAftMapped."""
+    os.makedirs(out_dir, exist_ok=True)
+    with open(os.path.join(out_dir, name + ".odometry.txt"), "w") as fo, open(os.path.join(out_dir, name + ".mapped.txt"), "w") as fm:
+        for t, od, pr, aft in zip(o["map_time"], o["map_odom"], o["map_processed"], o["map_aft_mapped"]):
+            fo.write("%.9f %s\n" % (t, " ".join("%.9g" % v for v in od)))
+            fm.write("%.9f %d %s\n" % (t, pr, " ".join("%.9g" % v for v in aft)))
+    print("mapper:", len(o["map_time"]), "odometry outputs,", len(o["key_poses"]), "key frames;", "trajectories in",
+          os.path.join(out_dir, name + ".odometry.txt"), "and", os.path.join(out_dir, name + ".mapped.txt"))
+
+
 def main(argv=None):
     ap = argparse.ArgumentParser()
     ap.add_argument("bags", nargs="+"); ap.add_argument("--slots", type=int, default=0, help="slots (0 = one per bag)")
     ap.add_argument("--lidar", default="/velodyne_points"); ap.add_argument("--imu", default="/imu/data")
     ap.add_argument("--max-scans", type=int, default=0)
     ap.add_argument("--lidar-model", default="0", help="0 | 1 for every bag, or one per bag: 0,1,...")
+    ap.add_argument("--map", action="store_true", help="run each bag's mapping node on what its estimator publishes")
     ap.add_argument("--out")
     a = ap.parse_args(argv)
     try:
@@ -42,12 +59,14 @@ def main(argv=None):
         ap.error(str(e))
     br = importlib.import_module("lins---lidar-inertial-slam_b200.bag_replay")
     recs = [br.Recording(p, a.lidar, a.imu, a.max_scans) for p in a.bags]
-    outs = br.replay(recs, a.slots or len(recs), model=model)
+    outs = br.replay(recs, a.slots or len(recs), model=model, map=a.map)
     np.set_printoptions(precision=4, suppress=True)
     for p, o in zip(a.bags, outs):
         print(p, br.summary(o))
         for k, (st, g) in enumerate(zip(o["status"], o["global_est"])):
             print(k, int(st), g)
+        if a.map:
+            write_map(o, a.out or ".", os.path.splitext(os.path.basename(p))[0])
         if a.out:
             os.makedirs(a.out, exist_ok=True)
             np.savez(os.path.join(a.out, os.path.splitext(os.path.basename(p))[0] + ".npz"),

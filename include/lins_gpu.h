@@ -526,10 +526,20 @@ int lins_gpu_seq_step_raw_mixed(lins_ctx* ctx, const lins_seq_raw_desc* step, co
 int lins_gpu_seq_step_cloud2_mixed(lins_ctx* ctx, const lins_seq_cloud2_desc* step, const lins_lidar_models* models,
                                    const lins_feature_params* fp, const double* scan_imu /*S x 6 or NULL*/);
 
-/* Split "Jacobian kernel" (SURVEY.md §8(d) unit U1): residual + Jacobian row + 29-scalar reduction over the
-   resident batch given the correspondence IDs of iteration `iter` of each scan's current linearisation
-   point. Used for the HBM-roofline measurement; results land in an internal n x 29 accumulator array. */
-int lins_gpu_batch_jacobian_pass(lins_ctx* ctx, double* accum_out /*n x 29 or NULL*/);
+/* Split "Jacobian kernel" (SURVEY.md §8(d) unit U1): de-skew, residual, robust weight and the factored Jacobian row
+   g = [c ; p x (R^T c)], r = lidar_scale * coeff.w of every query of the resident batch, reduced per unit.  The
+   linearisation point is each unit's posterior (what lins_gpu_batch_download returns as state_out, R its rotation) and the
+   correspondences are the IDs of each unit's last search iteration (lins_gpu_batch_download_indices).  The rows are
+   weighted iff the parameters' icp_freq == 1 (the weight of a search iteration >= 1).  Call it after lins_gpu_batch_run;
+   lins_gpu_set_params in between changes the pass's scan_period, lidar_scale and weighting.
+   accum_out (NULL = keep the sums on the device): n x 30 doubles, row i = unit i:
+     0..20   the upper triangle of sum g g^T, row-major (g0 g0, g0 g1, .., g0 g5, g1 g1, .., g5 g5)
+     21..26  sum g r
+     27      sum r r
+     28, 29  the accepted surf and corner rows (as doubles)
+   Each sum is deterministic from run to run; it matches an exact sum of the same rows to a few f64 ulps of its
+   condition scale (DESIGN.md §4.2). */
+int lins_gpu_batch_jacobian_pass(lins_ctx* ctx, double* accum_out /*n x 30 or NULL*/);
 
 /* ---- row F2 (SURVEY.md §8(f)): the mapping node's scan-to-map refinement -------------------------------------
    lins/src/lidar_mapping_node.cpp: scan2MapOptimization :1635-1652, cornerOptimization :1351-1461,

@@ -492,7 +492,8 @@ class LinsGpu:
         return p.value, n.value
 
     def batch_jacobian_pass(self, want_accum=False):
-        acc = np.zeros((self._batch_n, 32)) if want_accum else None
+        """The split Jacobian pass over the resident batch; with want_accum its (n, 30) sums (include/lins_gpu.h)."""
+        acc = np.zeros((self._batch_n, 30)) if want_accum else None
         self._ck(self.L.lins_gpu_batch_jacobian_pass(self.h, ptr(acc)))
         return acc
 

@@ -794,10 +794,12 @@ int lins_gpu_batch_jacobian_pass(lins_ctx* ctx, double* accum_out) {
   CK(cudaGetLastError());
   ctx->launches += 1;
   if (accum_out) {
+    // the device rows are 32 doubles apart; the caller's are the 30 the header documents
     CK(r.h_accum.reserve((size_t)r.n * 32));
-    CK(cudaMemcpyAsync(r.h_accum.p, r.accum.p, sizeof(double) * 32 * (size_t)r.n, cudaMemcpyDeviceToHost, ctx->stream));
+    CK(cudaMemcpy2DAsync(r.h_accum.p, sizeof(double) * 30, r.accum.p, sizeof(double) * 32, sizeof(double) * 30, (size_t)r.n,
+                         cudaMemcpyDeviceToHost, ctx->stream));
     CK(cudaStreamSynchronize(ctx->stream));
-    std::memcpy(accum_out, r.h_accum.p, sizeof(double) * 32 * (size_t)r.n);
+    std::memcpy(accum_out, r.h_accum.p, sizeof(double) * 30 * (size_t)r.n);
   }
   return LINS_OK;
 }

@@ -5,7 +5,8 @@
 // M x M products folded into the 6 x 6 information form).  This is the kernel whose achieved HBM bandwidth the north_star
 // asks about; the product path is the fused kernel in lins_gpu.cu, which never calls this one.
 //
-// Its own translation unit because it is tolerance-checked (1e-9 on the sums), not bit-checked, and is built for speed:
+// Its own translation unit because it is tolerance-checked (tests/test_gpu_jacobian.py: each sum within a few f64 ulps of
+// its condition scale of an exact-sum reference), not bit-checked, and is built for speed:
 //   * compiled WITH multiply-add contraction (lins_gpu.cu is -fmad=false for the bit-exact association); the per-unit
 //     constants of the de-skew (|phi|, phi / |phi|) are hoisted and sin / cos of the small half angle come from their
 //     Taylor polynomials (|x| < 1/8: remainder < 1e-19) — differences to the fused kernel's values are a few f64 ulps;
@@ -117,7 +118,7 @@ __global__ void __launch_bounds__(kJacWarps * 32, kJacMinCtas) lins_jacobian_mma
         q4 rq;
         {
           double sn, csn;
-          if (half < 0.125) sincos_small(half, sn, csn); else sincos(half, &sn, &csn);
+          if (fabs(half) < 0.125) sincos_small(half, sn, csn); else sincos(half, &sn, &csn);
           rq.w = csn; rq.x = ax.x * sn; rq.y = ax.y * sn; rq.z = ax.z * sn;
         }
         const d3 rp = qrot(rq, mk3(p.x, p.y, p.z));

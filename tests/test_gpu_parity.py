@@ -281,60 +281,6 @@ def test_estimate_transform_fallback(gpu, ob, golden_batch):
         assert np.abs(tg - to).max() <= POSE_TOL and _rot_err(qg, qo) <= POSE_TOL
 
 
-def test_jacobian_pass_matches_fused_reduction(gpu, ob, golden_batch):
-    """The split Jacobian kernel (unit U1) must reproduce the 28 sums of an association pass at the same state
-    with the same correspondence IDs."""
-    import ctypes as C
-
-    prm = ob.LinsParams.shipped()
-    gpu.set_params(prm)
-    gpu.batch_upload(golden_batch)
-    gpu.batch_run()
-    so, co, res, _ = gpu.batch_download()
-    acc = gpu.batch_jacobian_pass(want_accum=True)
-    L = ob.lib()
-    for i in range(golden_batch.n):
-        u = golden_batch.unit(i)
-        o = ob.Oracle(prm)
-        o.set_map(u["surf_less_flat"], u["corner_less_sharp"])
-        # oracle association at the updated state, with the weights of iter >= 1, searching afresh: the IDs of
-        # the GPU's last iteration were found at the previous linearisation point, so compare through the
-        # accepted-measurement sums computed from the GPU's own IDs instead
-        last_it = int(res["iters"][i]) - 1
-        assert acc[i, 28] >= 0 and acc[i, 29] >= 0
-        assert np.isfinite(acc[i, :28]).all()
-        assert acc[i, 27] >= 0
-    # exact cross-check on a unit that ran a single forced iteration: IDs and state are then known
-    prm1 = ob.LinsParams.shipped(num_iter=1, force_all_iters=1)
-    gpu.set_params(prm1)
-    gpu.batch_upload(golden_batch)
-    gpu.batch_run()
-    so, co, res, _ = gpu.batch_download()
-    acc = gpu.batch_jacobian_pass(want_accum=True)
-    for i in range(golden_batch.n):
-        u = golden_batch.unit(i)
-        o = ob.Oracle(prm1)
-        o.set_map(u["surf_less_flat"], u["corner_less_sharp"])
-        o.associate(u["surf_flat"], u["corner_sharp"], u["state"], 0)  # IDs at the prior (what iteration 0 stored)
-        # weights/coeffs at the updated state with those stored IDs: with icp_freq=2, iteration 3 reuses them
-        o2 = ob.Oracle(ob.LinsParams.shipped(icp_freq=2), use_kdtree=False)
-        o2.set_map(u["surf_less_flat"], u["corner_less_sharp"])
-        o2.associate(u["surf_flat"], u["corner_sharp"], u["state"], 0)
-        a1 = o2.associate(u["surf_flat"], u["corner_sharp"], so[i], 3)  # 3 % 2 != 0: reuse IDs; 3 >= 2: weighted
-        kp = np.concatenate([u["surf_flat"][a1["surf_mask"] == 1], u["corner_sharp"][a1["corner_mask"] == 1]])
-        cf = np.concatenate([a1["surf_coeff"][a1["surf_mask"] == 1], a1["corner_coeff"][a1["corner_mask"] == 1]])
-        n = len(kp)
-        h6, r = np.zeros((n, 6)), np.zeros(n)
-        L.lins_oracle_measurement_rows(C.byref(prm1), ob.ptr(np.ascontiguousarray(so[i])), ob.ptr(np.ascontiguousarray(kp)),
-                                       ob.ptr(np.ascontiguousarray(cf)), n, ob.ptr(h6), ob.ptr(r))
-        assert (acc[i, 28], acc[i, 29]) == (a1["surf_mask"].sum(), a1["corner_mask"].sum())
-        assert np.isclose(acc[i, 27], (r * r).sum(), rtol=1e-9)
-        # translation block of the information matrix: sum c c^T (g and h agree on the first three entries)
-        A_tt = h6[:, :3].T @ h6[:, :3]
-        got = np.array([[acc[i, 0], acc[i, 1], acc[i, 2]], [acc[i, 1], acc[i, 6], acc[i, 7]], [acc[i, 2], acc[i, 7], acc[i, 11]]])
-        assert np.allclose(got, A_tt, rtol=1e-9, atol=1e-12)
-
-
 def test_full_size_properties(gpu, ob, synth):
     """BASELINE.json configs[2] at bench size through size-independent properties: determinism, scan-order
     independence (units are independent), symmetric PSD covariances, unit quaternions, iteration accounting."""

@@ -526,6 +526,31 @@ int lins_gpu_seq_step_raw_mixed(lins_ctx* ctx, const lins_seq_raw_desc* step, co
 int lins_gpu_seq_step_cloud2_mixed(lins_ctx* ctx, const lins_seq_cloud2_desc* step, const lins_lidar_models* models,
                                    const lins_feature_params* fp, const double* scan_imu /*S x 6 or NULL*/);
 
+/* ---- per-slot rig configuration: the exp_port.yaml values that describe one recording's sensors -------------------
+   A slot of a lins_gpu_seq_open run reads the context's lins_params.scan_period, the step call's lins_feature_params and
+   the open's lins_seq_params / lins_seq_init_params unless it is configured; a configured slot reads its own values in
+   every stage that reads them: the IMU propagation's noise, reset(1)'s variances, the pre-integration and initialisation,
+   the feature extraction of _raw / _cloud2 steps (thresholds, the extrinsic, the re-stamp period), the de-skew of the
+   IESKF, of its estimateTransform fallback and of the second scan's estimateTransform, the map refresh's transformToEnd
+   and, on a run bound by lins_gpu_seq_map_open, its mapper's transformUpdate.  After a _pcl step the extraction's
+   thresholds and extrinsic are the call's (the re-stamp period is the slot's); after a lins_gpu_seq_step / _ex step,
+   whose features come from the caller, only the period and the filter values apply.  Each configured slot is
+   bit-identical to the same recording in the same slot of a run whose shared values equal its config. */
+typedef struct lins_slot_config {
+  double scan_period;              /* SCAN_PERIOD, finite and > 0 */
+  lins_feature_params features;    /* EDGE_THRESHOLD, SURF_THRESHOLD, IMU_LIDAR_EXTRINSIC_ANGLE (degrees) */
+  lins_seq_params filter;          /* the IMU noise (as setNoise computes it from ACC_N, GYR_N, ACC_W, GYR_W), INIT_POS_STD,
+                                      INIT_ATT_STD */
+  lins_seq_init_params init;       /* INIT_VEL_STD, INIT_ACC_STD, INIT_GYR_STD, INIT_BA, INIT_BW */
+} lins_slot_config;
+/* Configures every slot with mask[s] != 0 with cfg[s] (cfg has S entries; the unmasked ones are not read) and re-installs
+   its fresh state with the config's initializeCovariance.  A slot can be configured only while it is fresh: not present
+   in any step since lins_gpu_seq_open or its last lins_gpu_seq_restart, which returns it to unconfigured.  All or
+   nothing: LINS_E_INVALID, with nothing changed, for a NULL mask or cfg, a run of lins_gpu_seq_begin, a masked slot that
+   is not fresh, or a masked config with a non-finite value, scan_period <= 0, or a negative noise or std.  LINS_E_NOMAP
+   without a run. */
+int lins_gpu_seq_configure(lins_ctx* ctx, const uint8_t* mask /*S*/, const lins_slot_config* cfg /*S*/);
+
 /* Split "Jacobian kernel" (SURVEY.md §8(d) unit U1): de-skew, residual, robust weight and the factored Jacobian row
    g = [c ; p x (R^T c)], r = lidar_scale * coeff.w of every query of the resident batch, reduced per unit.  The
    linearisation point is each unit's posterior (what lins_gpu_batch_download returns as state_out, R its rotation) and the
@@ -587,7 +612,8 @@ int lins_gpu_map_associate(lins_ctx* ctx, const lins_point* corner_last, int n_c
    the host in the reference's f32 / f64 types.  Loop closure (loopClosureThread, performLoopClosure) is not performed:
    without a loop factor the iSAM2 estimate of a new key frame is the pose inserted for it up to f32 rounding (DESIGN.md §4.9), and
    correctPoses is a no-op.  The reference's constants are fixed: mappingProcessInterval 0.3 s, window 50, key-frame
-   distance 0.3 m, loop search 5 m / 30 s; SCAN_PERIOD is the context's lins_params.scan_period.
+   distance 0.3 m, loop search 5 m / 30 s; SCAN_PERIOD is the context's lins_params.scan_period (a configured slot's
+   own on a run bound by lins_gpu_seq_map_open, see lins_slot_config).
    All clouds are in the mapping node's YZX frame convention, like lins_gpu_scan2map's.
    The mapper's state, its scan-to-map matP / isDegenerate included, is its own: lins_gpu_map_set, lins_gpu_scan2map,
    lins_gpu_voxel_grid and lins_gpu_mappers_* on the same context neither see nor change it, nor does it change theirs.

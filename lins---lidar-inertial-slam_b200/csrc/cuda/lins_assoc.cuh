@@ -134,7 +134,7 @@ __device__ void association_pass(CtaMem& cta, Smem* slots, const BatchView& bv, 
     const int sl = slot_of(v, Q), i = v - sl * Q;
     Smem& sm = slots[sl];
     if (!sm.run || i >= sm.ns + sm.nc) continue;
-    const float4 s = transform_to_start(pb.qpt[v], sm, kp.scan_period);
+    const float4 s = transform_to_start(pb.qpt[v], sm, sm.period);
     pb.sel[v] = s;
     pb.key[v] = kKeyMax;
     const bool search = (sm.iter % kp.icp_freq) == 0;
@@ -480,7 +480,7 @@ __device__ void association_pass(CtaMem& cta, Smem* slots, const BatchView& bv, 
     }
     double g[6] = {0.0, 0.0, 0.0, 0.0, 0.0, 0.0}, r = 0.0;
     if (ok) {
-      if (MODE == MODE_ICP_REDUCE) jacobian_row_icp(pb.qpt[v], coeff, sm.phi, kp.scan_period, g, r);
+      if (MODE == MODE_ICP_REDUCE) jacobian_row_icp(pb.qpt[v], coeff, sm.phi, sm.period, g, r);
       else jacobian_row(pb.qpt[v], coeff, sm.R, kp.lidar_scale, g, r);
     }
     const int vw = sl * pb.nvw + (i0 >> 5);

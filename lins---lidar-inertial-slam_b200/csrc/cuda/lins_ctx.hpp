@@ -150,13 +150,21 @@ struct SeqPubState {
 // its map (stale[s] = 1, after a refresh that failed the >=5 && >=20 guard), and is empty elsewhere.
 struct SeqState {
   int n = 0;                      // sequences (0 = lins_gpu_seq_begin / lins_gpu_seq_open has not run)
-  double consts[10];              // lins_seq::Consts
+  double consts[10];              // lins_seq::Consts of the run's params
   // sequence initialisation (lins_gpu_seq_open runs only): init_consts = lins_seq::InitConsts, fusion = each slot's
   // StateEstimator::status_ (every slot of a lins_gpu_seq_begin run is RUNNING), pre = the pre-integration (n x 20),
   // init_icp = the second scans' estimateTransform loop state (n IcpState records), init_off = their compacted query
   // offsets (2 x (n + 1), after the IESKF's), scan_imu = the step's processPCL IMU samples (n x 6)
   bool has_init = false;
   double init_consts[24];
+  // per-slot rig configuration (lins_gpu_seq_configure): every slot's Consts / InitConsts on the device (n x 10, n x 24;
+  // the run's for an unconfigured slot, so every slot takes one path), the step's de-skew period of each slot (n), and on
+  // the host each slot's config, whether it is configured and whether it is fresh (not present in a step since open /
+  // restart: only a fresh slot can be configured)
+  Buf<double> slot_consts, slot_init_consts, period;
+  Buf<double, kPinned> h_period;
+  std::vector<lins_slot_config> cfg;
+  std::vector<unsigned char> configured, fresh;
   std::vector<int32_t> fusion;
   Buf<double> pre, scan_imu;
   Buf<double, kPinned> h_scan_imu;
@@ -189,6 +197,10 @@ struct SeqState {
   ~SeqState() { for (cudaEvent_t e : ev) if (e) cudaEventDestroy(e); }
 };
 
+// One scan's feature extraction constants: cos / sin of imu_lidar_extrinsic_angle (host libm), the edge / surf thresholds
+// and the re-stamp's SCAN_PERIOD
+struct FeatConsts { double c, s, edge, surf, scan_period; };
+
 // Feature extraction (lins_features.cu): the uploaded segmented scans (cloud in up.qs, CSR in up.qs_off) with their
 // cloud_info, the extracted clouds at the input offsets, per-point scratch, and the counts read back (n x 5: the four
 // counts in lins_seq_step_desc order, then the scan's status)
@@ -201,6 +213,7 @@ struct FeatState {
   Buf<double> curv;
   Buf<float4> und, out[4];
   Buf<int, kPinned> h_counts;
+  Buf<FeatConsts> consts; Buf<FeatConsts, kPinned> h_consts;  // each scan's constants
   std::vector<int32_t> h_ring;
   CopyList copies;                                      // the pack into sequence mode's feature buffers
   EventPair ev;                                         // around the last extraction kernel (lins_gpu_extract_ms)
@@ -553,12 +566,13 @@ inline int upload2(lins_ctx* ctx, Buf<float4>& dst_a, const lins_point* a, int n
 int upload_clouds(lins_ctx* ctx, Resident& r, int n, const lins_point* const pts[4], const int32_t* const offs[4], int point_format);
 // lins_gpu.cu: the fused kernel's IESKF launch over bv (with r's scratch), its query tile, the estimateTransform loop of
 // bv's device-resident units (pose: 20 doubles, icp: one IcpState per unit, set by the caller), and the CSR transformToEnd
-// of the units with run[u] != 0 (lin: 20 doubles per unit)
+// of the units with run[u] != 0 (lin: 20 doubles per unit, period: one SCAN_PERIOD per unit, both on the device)
 int fused_ieskf_launch(lins_ctx* ctx, Resident& r, const lins_dev::BatchView& bv);
 int fused_qtile(int max_q);
 size_t icp_state_bytes();
 int icp_loop(lins_ctx* ctx, Resident& r, lins_dev::BatchView bv, double* pose, lins_dev::IcpState* icp);
-int transform_to_end_csr(lins_ctx* ctx, float4* pts, const int* off, int n_units, const double* lin, const unsigned char* run);
+int transform_to_end_csr(lins_ctx* ctx, float4* pts, const int* off, int n_units, const double* lin, const unsigned char* run,
+                         const double* period);
 // device-resident input of one feature extraction: n scans of line_num rings; scan i's points are pts[off[i] ..
 // off[i] + count[count_stride * i]) (off[i] .. off[i + 1] when count is null), its per-point cloud_info at the same
 // offsets; ring: n x 2 x line_num (start, end), ori: n x 3; total = off[n], the length of the per-point outputs
@@ -569,11 +583,15 @@ struct FeatInputs {
   const unsigned char* ground = nullptr; const unsigned* col = nullptr; const float* range = nullptr;
   const int* ring = nullptr; const float* ori = nullptr;
 };
-// lins_features.cu: validate, upload and extract the scans of d into ctx->feat; reads the counts back (one synchronisation)
-int features_run(lins_ctx* ctx, const lins_feature_params* fp, const lins_pcl_desc* d);
-// lins_features.cu: extract the scans of `in` into ctx->feat (clouds at the input offsets) and read the counts back (one
-// D2H + synchronisation; a scan's device-side status returns LINS_E_INVALID / LINS_E_TOOBIG)
-int features_launch(lins_ctx* ctx, const lins_feature_params* fp, const FeatInputs& in);
+// lins_features.cu: one scan's constants from fp and its SCAN_PERIOD
+FeatConsts feat_consts(const lins_feature_params& fp, double scan_period);
+// lins_features.cu: validate, upload and extract the scans of d into ctx->feat with fp and SCAN_PERIOD period[i] (host, n;
+// null = the context's) for scan i; reads the counts back (one synchronisation)
+int features_run(lins_ctx* ctx, const lins_feature_params* fp, const lins_pcl_desc* d, const double* period = nullptr);
+// lins_features.cu: extract the scans of `in` into ctx->feat (clouds at the input offsets) with scan i's constants k[i]
+// (host, in.n) and read the counts back (one D2H + synchronisation; a scan's device-side status returns LINS_E_INVALID /
+// LINS_E_TOOBIG)
+int features_launch(lins_ctx* ctx, const FeatConsts* k, const FeatInputs& in);
 // lins_projection.cu: validate the model table and the sweeps of d, upload them and queue their projection into ctx->proj
 // (no synchronisation); drop_nonfinite: copyPointCloud's NaN removal first; present (host, n; null = all): a scan whose
 // flag is 0 is projected as an empty sweep.  A single-model entry passes the table {1, m, NULL}.
@@ -640,9 +658,11 @@ int mapper_node_download(lins_ctx* ctx, const MapperNode& m, const float4* const
 int queue_copies(lins_ctx* ctx, CopyList& l, std::vector<DevCopy> v, int base);
 // lins_mappers.cu: n_slots fresh mapping nodes in ms (replacing any open run); the slots with mask[s] != 0 back to the
 // fresh state; one lockstep step of ms's present slots on a checked descriptor, from d's host clouds or, with dev
-// (n_slots x 3: corner, surf, outlier), from device ranges in XYZ order that the step's gather writes YZX
+// (n_slots x 3: corner, surf, outlier), from device ranges in XYZ order that the step's gather writes YZX; period (host,
+// n_slots; null = the context's): each slot's SCAN_PERIOD in transformUpdate
 int mappers_open(lins_ctx* ctx, MappersState& ms, int n_slots);
 int mappers_reset(lins_ctx* ctx, MappersState& ms, const uint8_t* mask);
-int mappers_step(lins_ctx* ctx, MappersState& ms, const lins_mappers_desc* d, lins_mapper_report* reps, const MapPiece* dev);
+int mappers_step(lins_ctx* ctx, MappersState& ms, const lins_mappers_desc* d, lins_mapper_report* reps, const MapPiece* dev,
+                 const double* period);
 
 }  // namespace lins_capi

@@ -39,7 +39,7 @@ struct FeatArgs {
   const unsigned char* ground; const unsigned* col; const float* range;
   const int* ring;    // n x 2 x line_num: startRingIndex, endRingIndex
   const float* ori;   // n x 3: startOrientation, endOrientation, orientationDiff
-  double c, s, edge, surf, scan_period;
+  const FeatConsts* k;  // n: each scan's constants
   float4* und;        // de-skewed cloud, at the input offsets
   float4* out[4];     // surf_flat, corner_sharp, surf_less_flat, corner_less_sharp, at the input offsets
   int* counts;        // n x 5: the four counts, then the scan's status (FEAT_*)
@@ -85,6 +85,7 @@ __global__ void __launch_bounds__(kThreads) lins_features_kernel(const FeatArgs 
   const int* rs = a.ring + (size_t)sc * 2 * L;
   const int* re = rs + L;
   const float start = a.ori[3 * sc], end = a.ori[3 * sc + 1], diff = a.ori[3 * sc + 2];
+  const FeatConsts kc = a.k[sc];
   const float4* P = a.pts + base;
   const float* R = a.range + base;
   const unsigned* C = a.col + base;
@@ -143,7 +144,7 @@ __global__ void __launch_bounds__(kThreads) lins_features_kernel(const FeatArgs 
   for (int i = tid; i < np; i += kThreads) {
     const float4 p = P[i];
     float x, y;
-    lins_feat::rotate_xy(a.c, a.s, p.x, p.y, x, y);
+    lins_feat::rotate_xy(kc.c, kc.s, p.x, p.y, x, y);
     bool flips;
     lins_feat::ori_not_passed(x, y, start, flips);
     if (flips) atomicMin(&s_half, i);
@@ -153,10 +154,10 @@ __global__ void __launch_bounds__(kThreads) lins_features_kernel(const FeatArgs 
   for (int i = tid; i < np; i += kThreads) {
     const float4 p = P[i];
     float x, y;
-    lins_feat::rotate_xy(a.c, a.s, p.x, p.y, x, y);
+    lins_feat::rotate_xy(kc.c, kc.s, p.x, p.y, x, y);
     bool flips;
     const double ori = i <= half ? lins_feat::ori_not_passed(x, y, start, flips) : lins_feat::ori_passed(x, y, end);
-    U[i] = make_float4(x, y, p.z, lins_feat::stamp(p.w, ori, start, diff, a.scan_period));
+    U[i] = make_float4(x, y, p.z, lins_feat::stamp(p.w, ori, start, diff, kc.scan_period));
     // calculateSmoothness on [5, n - 5); elsewhere the fresh arrays' defaults (curvature 0, entry (0, ind 0))
     const bool inner = i >= 5 && i < np - 5;
     curv[i] = inner ? lins_feat::curvature(R + i - 5) : 0.0;
@@ -215,7 +216,7 @@ __global__ void __launch_bounds__(kThreads) lins_features_kernel(const FeatArgs 
           const int kk = k - lane;
           int ind = 0;
           bool ok = false;
-          if (kk >= sp) { ind = s_ind[kk - sp]; ok = picked[ind] == 0 && curv[ind] > a.edge && G[ind] == 0; }
+          if (kk >= sp) { ind = s_ind[kk - sp]; ok = picked[ind] == 0 && curv[ind] > kc.edge && G[ind] == 0; }
           const unsigned b = __ballot_sync(FULL, ok);
           if (!b) { k -= 32; continue; }
           const int l = __ffs(b) - 1;
@@ -237,7 +238,7 @@ __global__ void __launch_bounds__(kThreads) lins_features_kernel(const FeatArgs 
           const int kk = k + lane;
           int ind = 0;
           bool ok = false;
-          if (kk <= ep) { ind = s_ind[kk - sp]; ok = picked[ind] == 0 && curv[ind] < a.surf && G[ind] == 1; }
+          if (kk <= ep) { ind = s_ind[kk - sp]; ok = picked[ind] == 0 && curv[ind] < kc.surf && G[ind] == 1; }
           const unsigned b = __ballot_sync(FULL, ok);
           if (!b) { k += 32; continue; }
           const int l = __ffs(b) - 1;
@@ -344,7 +345,15 @@ namespace lins_capi {
 // checks what needs the points (finite input, sextants inside the cloud, ring spans) and reports it in the same
 // read-back.  On return f.h_counts holds n x 5 (counts, status) and the clouds are in f.out / f.und at the input offsets.
 // lins_gpu_seq_step_raw calls features_launch on the projection's output where it lies (ctx->proj, raw offsets).
-int features_run(lins_ctx* ctx, const lins_feature_params* fp, const lins_pcl_desc* d) {
+FeatConsts feat_consts(const lins_feature_params& fp, double scan_period) {
+  FeatConsts k;
+  const double y = fp.imu_lidar_extrinsic_angle * M_PI / 180.0;  // math_utils::deg2rad
+  k.c = std::cos(y); k.s = std::sin(y);
+  k.edge = fp.edge_threshold; k.surf = fp.surf_threshold; k.scan_period = scan_period;
+  return k;
+}
+
+int features_run(lins_ctx* ctx, const lins_feature_params* fp, const lins_pcl_desc* d, const double* period) {
   if (!fp || !d || d->n_scans < 0) return fail(ctx, LINS_E_INVALID, "bad feature extraction arguments");
   if (d->line_num < 1 || d->line_num > lins_feat::kMaxLines) return fail(ctx, LINS_E_INVALID, "line_num outside 1..128");
   const int n = d->n_scans, L = d->line_num;
@@ -361,7 +370,9 @@ int features_run(lins_ctx* ctx, const lins_feature_params* fp, const lins_pcl_de
   const int32_t* offs[4] = {d->cloud_off, zeros.data(), zeros.data(), zeros.data()};
   rc = upload_clouds(ctx, f.up, n, pts, offs, d->point_format);  // (synchronises the stream first)
   if (rc != LINS_OK) return rc;
-  if (n == 0) return features_launch(ctx, fp, FeatInputs());
+  std::vector<FeatConsts> k(n);
+  for (int i = 0; i < n; ++i) k[i] = feat_consts(*fp, period ? period[i] : ctx->prm.scan_period);
+  if (n == 0) return features_launch(ctx, k.data(), FeatInputs());
   const size_t N = (size_t)total + 1;
   CK(f.ground.reserve(N)); CK(f.col.reserve(N)); CK(f.range.reserve(N)); CK(f.ring.reserve(2 * (size_t)n * L)); CK(f.ori.reserve(3 * (size_t)n));
   f.h_ring.resize(2 * (size_t)n * L);
@@ -380,24 +391,25 @@ int features_run(lins_ctx* ctx, const lins_feature_params* fp, const lins_pcl_de
   in.n = n; in.line_num = L; in.total = total;
   in.pts = f.up.qs.p; in.off = f.up.qs_off.p;
   in.ground = f.ground.p; in.col = f.col.p; in.range = f.range.p; in.ring = f.ring.p; in.ori = f.ori.p;
-  return features_launch(ctx, fp, in);
+  return features_launch(ctx, k.data(), in);
 }
 
-int features_launch(lins_ctx* ctx, const lins_feature_params* fp, const FeatInputs& in) {
+int features_launch(lins_ctx* ctx, const FeatConsts* k, const FeatInputs& in) {
   FeatState& f = ctx->feat;
   const int n = in.n;
   CK(f.h_counts.reserve(5 * (size_t)n + 1));
   if (n == 0) return LINS_OK;
   const size_t N = (size_t)in.total + 1;
   CK(f.und.reserve(N)); for (auto& o : f.out) CK(o.reserve(N));
+  CK(f.consts.reserve(n)); CK(f.h_consts.reserve(n));
   CK(f.counts.reserve(5 * (size_t)n)); CK(f.curv.reserve(N)); CK(f.sind.reserve(N)); CK(f.picked.reserve(N)); CK(f.label.reserve(N));
   FeatArgs a;
   a.line_num = in.line_num;
   a.pts = in.pts; a.off = in.off; a.count = in.count; a.count_stride = in.count_stride;
   a.ground = in.ground; a.col = in.col; a.range = in.range; a.ring = in.ring; a.ori = in.ori;
-  const double y = fp->imu_lidar_extrinsic_angle * M_PI / 180.0;  // math_utils::deg2rad
-  a.c = std::cos(y); a.s = std::sin(y);
-  a.edge = fp->edge_threshold; a.surf = fp->surf_threshold; a.scan_period = ctx->prm.scan_period;
+  std::memcpy(f.h_consts.p, k, sizeof(FeatConsts) * n);  // (the last extraction ended with a synchronisation)
+  CK(cudaMemcpyAsync(f.consts.p, f.h_consts.p, sizeof(FeatConsts) * n, cudaMemcpyHostToDevice, ctx->stream));
+  a.k = f.consts.p;
   a.und = f.und.p;
   for (int k = 0; k < 4; ++k) a.out[k] = f.out[k].p;
   a.counts = f.counts.p;

@@ -39,6 +39,7 @@ __device__ void unit_prologue(CtaMem& cta, Smem& sm, const BatchView& bv, const 
   }
   if (tid == 32) {
     sm.flags[0] = sm.flags[1] = sm.flags[2] = sm.flags[3] = 0; sm.residualNorm = 1e6;
+    sm.period = bv.unit_period ? bv.unit_period[scan] : kp.scan_period;
     sm.cnt[0] = sm.cnt[1] = 0;
     sm.iter = MODE == MODE_IESKF ? 0 : kp.iter0;
     sm.fresh = 0; sm.finished = 0; sm.first_pass = 1; sm.pos_valid = 0; sm.pos_is_slot = 0;
@@ -354,13 +355,15 @@ __device__ __forceinline__ float4 to_end_point(float4 p, const double* sphi, con
   return p;
 }
 
-// CSR version: one block per unit u with run[u] != 0, its cloud pts[off[u], off[u+1]) with linState_ lin[20 u ..].
+// CSR version: one block per unit u with run[u] != 0, its cloud pts[off[u], off[u+1]) with linState_ lin[20 u ..] and
+// SCAN_PERIOD period[u].
 __global__ void lins_transform_to_end_csr_kernel(float4* __restrict__ pts, const int* __restrict__ off, const double* __restrict__ lin,
-                                                 const unsigned char* __restrict__ run, double scan_period) {
+                                                 const unsigned char* __restrict__ run, const double* __restrict__ period) {
   __shared__ double sphi[3], srn[3], sq[4];
   const int u = blockIdx.x;
   if (!run[u]) return;
   to_end_consts(lin + (size_t)u * 20, sphi, srn, sq);
+  const double scan_period = period[u];
   for (int i = off[u] + threadIdx.x; i < off[u + 1]; i += blockDim.x) pts[i] = to_end_point(pts[i], sphi, srn, sq, scan_period);
 }
 
@@ -574,9 +577,10 @@ int icp_loop(lins_ctx* ctx, Resident& r, BatchView bv, double* pose, IcpState* i
   return LINS_OK;
 }
 
-int transform_to_end_csr(lins_ctx* ctx, float4* pts, const int* off, int n_units, const double* lin, const unsigned char* run) {
+int transform_to_end_csr(lins_ctx* ctx, float4* pts, const int* off, int n_units, const double* lin, const unsigned char* run,
+                         const double* period) {
   if (n_units <= 0) return LINS_OK;
-  lins_transform_to_end_csr_kernel<<<n_units, 256, 0, ctx->stream>>>(pts, off, lin, run, ctx->prm.scan_period);
+  lins_transform_to_end_csr_kernel<<<n_units, 256, 0, ctx->stream>>>(pts, off, lin, run, period);
   CK(cudaGetLastError());
   ctx->launches += 1;
   return LINS_OK;

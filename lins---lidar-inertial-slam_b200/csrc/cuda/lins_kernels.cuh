@@ -71,6 +71,8 @@ struct BatchView {
                                          // (lins_icp_step.cuh); non-zero = that unit's Gauss-Newton loop has ended, skip it (or null)
   unsigned char* qscratch;               // per-CTA global scratch for the per-query arrays when they do not fit shared
   size_t qscratch_stride;                // memory (null: they live in shared memory)
+  const double* unit_period;             // per unit: the SCAN_PERIOD of its de-skew (sequence mode's per-slot rigs); null =
+                                         // every unit's is KParams::scan_period
 };
 
 // loop state of one unit's estimateTransform (lins_icp_step.cuh)
@@ -128,6 +130,7 @@ struct alignas(16) Smem {
   double X6[6];         // right-hand side / solution of the gain system
   double upd[18];
   double residualNorm;
+  double period;        // SCAN_PERIOD of the unit's de-skew (transformToStart, the ICP fallback's rows)
   int flags[4];         // 0 converged 1 diverged 2 has_nan 3 stop
   int cnt[2];
   // bookkeeping
@@ -154,7 +157,7 @@ struct alignas(16) Smem {
 struct CtaMem {
   union {
     // counting-sort counters / cursors while a unit's index is built, 16 bits each (lins_assoc_az.cuh: cnt16_add1): 8 kB
-    // instead of 16 kB brings the CTA (three slots of 320 queries) from 204 880 B to 196 688 B of shared memory, under the
+    // instead of 16 kB brings the CTA (three slots of 320 queries) from 204 928 B to 196 736 B of shared memory, under the
     // 196 KB carve-out, so the SM keeps about 60 KB of L1 instead of 28 KB for the sorted target copies the searches and
     // the residuals read
     unsigned build_tab[kAzTabS / 2 + 1];

@@ -74,7 +74,8 @@ namespace lins_capi {
 // one step of every present slot of ms on a checked descriptor (d->n_slots == ms.n, valid offsets and arrays).  dev
 // (M x 3: corner, surf, outlier, or null): the slots' clouds are device ranges in XYZ order, copied YZX-permuted into the
 // VoxelGrids' input by the local maps' gather launch; d's clouds are then not read.
-int mappers_step(lins_ctx* ctx, MappersState& ms, const lins_mappers_desc* d, lins_mapper_report* reps, const MapPiece* dev) {
+int mappers_step(lins_ctx* ctx, MappersState& ms, const lins_mappers_desc* d, lins_mapper_report* reps, const MapPiece* dev,
+                 const double* period) {
   const int M = ms.n;
   const lins_point* src[3] = {d->corner, d->surf, d->outlier};
   const int32_t* off[3] = {d->corner_off, d->surf_off, d->outlier_off};
@@ -227,7 +228,7 @@ int mappers_step(lins_ctx* ctx, MappersState& ms, const lins_mappers_desc* d, li
     const bool gate = cnt[0] > 10 && cnt[1] > 100;
     KfSave sv;
     bool saved = false;
-    mapper_cycle_end(ms.node[s], sc[s], d->time[s], ctx->prm.scan_period, cnt, gate ? &ms.h_loop.p[s] : nullptr, rr[s], &sv, &saved);
+    mapper_cycle_end(ms.node[s], sc[s], d->time[s], period ? period[s] : ctx->prm.scan_period, cnt, gate ? &ms.h_loop.p[s] : nullptr, rr[s], &sv, &saved);
     if (saved) {
       for (int k = 0; k < 3; ++k) sv.ds[k] = ms.ds[s][2 + k].p;
       saves.push_back(sv);
@@ -293,7 +294,7 @@ int lins_gpu_mappers_step(lins_ctx* ctx, const lins_mappers_desc* d, lins_mapper
   const int32_t* off[3] = {d->corner_off, d->surf_off, d->outlier_off};
   static const char* const what[3] = {"bad corner offsets / cloud", "bad surf offsets / cloud", "bad outlier offsets / cloud"};
   for (int k = 0; k < 3; ++k) if (check_csr(ctx, off[k], M, src[k], what[k]) != LINS_OK) return LINS_E_INVALID;
-  return mappers_step(ctx, ctx->mappers, d, reps, nullptr);
+  return mappers_step(ctx, ctx->mappers, d, reps, nullptr, nullptr);
 }
 
 int lins_gpu_mappers_download(lins_ctx* ctx, int32_t slot, double* key_poses, int32_t* window, float* map_corner_ds, float* map_surf_ds,
@@ -338,7 +339,7 @@ int lins_gpu_mapper_step(lins_ctx* ctx, const lins_mapper_desc* d, lins_mapper_r
   one.corner = d->corner; one.corner_off = off[0];
   one.surf = d->surf; one.surf_off = off[1];
   one.outlier = d->outlier; one.outlier_off = off[2];
-  return mappers_step(ctx, ctx->mapper, &one, rep, nullptr);
+  return mappers_step(ctx, ctx->mapper, &one, rep, nullptr, nullptr);
 }
 
 int lins_gpu_mapper_download(lins_ctx* ctx, double* key_poses, int32_t* window, float* map_corner_ds, float* map_surf_ds,

@@ -35,20 +35,21 @@ enum ImuUse : unsigned char { IMU_IGNORE = 0, IMU_PREDICT = 1, IMU_PREINTEGRATE 
 // StateEstimator::FusionStatus
 enum Fusion : int32_t { FUSION_INIT = 0, FUSION_FIRST_SCAN = 1, FUSION_RUNNING = 3 };
 
-// One warp per sequence: the sequence's k StatePredictor::predict calls in order (kalman_filter.hpp:98-170).  The 18x18
+// One warp per sequence: the sequence's k StatePredictor::predict calls in order (kalman_filter.hpp:98-170), with its own
+// constants k[s] / ik[s] (here and in the kernels below: the run's, or the slot's config).  The 18x18
 // matrices live in shared memory; lane l owns the entries e = l, l + 32, ... of every matrix phase, each entry summed in
 // the host's order.  A sequence in STATUS_FIRST_SCAN pre-integrates its rows instead (IntegrationBase::propagate, lane 0).
 __global__ void __launch_bounds__(32) lins_seq_predict_kernel(double* __restrict__ filt, double* __restrict__ cov, double* __restrict__ imu_last,
                                                              const double* __restrict__ imu, const int* __restrict__ imu_off,
                                                              const unsigned char* __restrict__ use, double* __restrict__ pre,
-                                                             const lins_seq::Consts k, const lins_seq::InitConsts ik) {
+                                                             const lins_seq::Consts* __restrict__ k, const lins_seq::InitConsts* __restrict__ ik) {
   const int s = blockIdx.x, lane = threadIdx.x;
   if (use[s] == IMU_IGNORE) return;
   const int m0 = imu_off[s], m1 = imu_off[s + 1];
   if (m0 == m1) return;
   if (use[s] == IMU_PREINTEGRATE) {
     if (lane == 0)
-      for (int m = m0; m < m1; ++m) lins_seq::preint_propagate(pre + (size_t)s * 20, ik, imu[(size_t)m * 7], imu + (size_t)m * 7 + 1, imu + (size_t)m * 7 + 4);
+      for (int m = m0; m < m1; ++m) lins_seq::preint_propagate(pre + (size_t)s * 20, ik[s], imu[(size_t)m * 7], imu + (size_t)m * 7 + 1, imu + (size_t)m * 7 + 4);
     return;
   }
   __shared__ double P[324], Ft[324], F[324], FP[324], P2[324];
@@ -77,7 +78,7 @@ __global__ void __launch_bounds__(32) lins_seq_predict_kernel(double* __restrict
     __syncwarp();
     for (int e = lane; e < 324; e += 32) {
       const int i = e / 18, j = e % 18;
-      P2[e] = lins_seq::fpft_entry(FP, F, lins_seq::q_entry(b, k.noise, i, j, dt), i, j);
+      P2[e] = lins_seq::fpft_entry(FP, F, lins_seq::q_entry(b, k[s].noise, i, j, dt), i, j);
     }
     __syncwarp();
     for (int e = lane; e < 324; e += 32) { const int i = e / 18, j = e % 18; P[j * 18 + i] = 0.5 * (P2[i * 18 + j] + P2[j * 18 + i]); }
@@ -93,7 +94,8 @@ __global__ void __launch_bounds__(32) lins_seq_predict_kernel(double* __restrict
 // correctRollPitch (state_estimator.hpp:202-237).  lin receives linState_ (rn / qbn only after divergence, like the shim).
 __global__ void lins_seq_post_kernel(int n, const unsigned char* __restrict__ status, const double* __restrict__ state_out,
                                      const double* __restrict__ cov_out, const double* __restrict__ icp_pose, double* __restrict__ filt,
-                                     double* __restrict__ cov, double* __restrict__ glob, double* __restrict__ lin, const lins_seq::Consts k) {
+                                     double* __restrict__ cov, double* __restrict__ glob, double* __restrict__ lin,
+                                     const lins_seq::Consts* __restrict__ k) {
   const int s = blockIdx.x * blockDim.x + threadIdx.x;
   if (s >= n || (status[s] != LINS_SEQ_RAN && status[s] != LINS_SEQ_ICP)) return;
   double f[20];
@@ -109,7 +111,7 @@ __global__ void lins_seq_post_kernel(int n, const unsigned char* __restrict__ st
   for (int e = 0; e < 324; ++e) P[e] = cov_out[(size_t)s * 324 + e];
   double* g = glob + (size_t)s * 20;
   lins_seq::integrate(g, f);
-  lins_seq::reset1(f, P, k);
+  lins_seq::reset1(f, P, k[s]);
   lins_seq::correct_roll_pitch(g, f);
   for (int i = 0; i < 19; ++i) filt[(size_t)s * 20 + i] = f[i];
 }
@@ -134,51 +136,41 @@ __global__ void lins_seq_icp_start_kernel(int n, const unsigned char* __restrict
 __global__ void lins_seq_init_kernel(int n, const unsigned char* __restrict__ status, const double* __restrict__ imu,
                                      const double* __restrict__ icp_pose, double* __restrict__ pre, double* __restrict__ glob,
                                      double* __restrict__ filt, double* __restrict__ cov, double* __restrict__ lin,
-                                     double* __restrict__ imu_last, const lins_seq::InitConsts k) {
+                                     double* __restrict__ imu_last, const lins_seq::InitConsts* __restrict__ k) {
   const int s = blockIdx.x * blockDim.x + threadIdx.x;
   if (s >= n) return;
   const size_t o = (size_t)s * 20;
   double* il = imu_last + (size_t)s * 8;
   if (status[s] == LINS_SEQ_FIRST)
-    lins_seq::first_scan(filt + o, cov + (size_t)s * 324, lin + o, pre + o, il, imu + (size_t)s * 6, k);
+    lins_seq::first_scan(filt + o, cov + (size_t)s * 324, lin + o, pre + o, il, imu + (size_t)s * 6, k[s]);
   else if (status[s] == LINS_SEQ_SECOND)
-    lins_seq::second_scan(glob + o, filt + o, cov + (size_t)s * 324, lin + o, il, pre + o, icp_pose + o, imu + (size_t)s * 6, k);
+    lins_seq::second_scan(glob + o, filt + o, cov + (size_t)s * 324, lin + o, il, pre + o, icp_pose + o, imu + (size_t)s * 6, k[s]);
 }
 
 // One thread per sequence with mask[s] != 0 (every sequence for a null mask): the state of a new StateEstimator
 __global__ void lins_seq_fresh_kernel(int n, const unsigned char* __restrict__ mask, double* __restrict__ glob, double* __restrict__ filt,
-                                      double* __restrict__ cov, const lins_seq::InitConsts k) {
+                                      double* __restrict__ cov, const lins_seq::InitConsts* __restrict__ k) {
   const int s = blockIdx.x * blockDim.x + threadIdx.x;
   if (s >= n || (mask && !mask[s])) return;
-  lins_seq::fresh_slot(glob + (size_t)s * 20, filt + (size_t)s * 20, cov + (size_t)s * 324, k);
+  lins_seq::fresh_slot(glob + (size_t)s * 20, filt + (size_t)s * 20, cov + (size_t)s * 324, k[s]);
 }
 
-lins_seq::Consts consts_of(const SeqState& q) {
-  lins_seq::Consts k;
-  std::memcpy(&k, q.consts, sizeof(k));
-  return k;
-}
-lins_seq::InitConsts init_consts_of(const SeqState& q) {
-  lins_seq::InitConsts k;
-  static_assert(sizeof(k) == sizeof(q.init_consts), "init consts");
-  std::memcpy(&k, q.init_consts, sizeof(k));
-  return k;
-}
+static_assert(sizeof(lins_seq::Consts) == sizeof(SeqState::consts), "consts");
+static_assert(sizeof(lins_seq::InitConsts) == sizeof(SeqState::init_consts), "init consts");
 
 // noise, sq(init_pos_std) and pow(deg2rad(init_att_std), 2) of lins_seq_params (kalman_filter.hpp setNoise / reset(1))
-void set_consts(SeqState& q, const lins_seq_params* prm) {
+void consts_of(double* out, const lins_seq_params* prm) {
   lins_seq::Consts k;
   for (int i = 0; i < 4; ++i) k.noise[i] = prm->noise[i];
   for (int i = 0; i < 3; ++i) {
     k.pos_var[i] = prm->init_pos_std[i] * prm->init_pos_std[i];                 // sq(init_pos_std)
     k.att_var[i] = std::pow(prm->init_att_std[i] * M_PI / 180.0, 2);            // pow(deg2rad(init_att_std), 2)
   }
-  static_assert(sizeof(k) == sizeof(q.consts), "consts");
-  std::memcpy(q.consts, &k, sizeof(k));
+  std::memcpy(out, &k, sizeof(k));
 }
 
 // the diagonal initializeCovariance installs (kalman_filter.hpp:197-209) and init_ba / init_bw
-void set_init_consts(SeqState& q, const lins_seq_params* prm, const lins_seq_init_params* ip) {
+void init_consts_of(double* out, const lins_seq_params* prm, const lins_seq_init_params* ip) {
   lins_seq::InitConsts k;
   for (int i = 0; i < 3; ++i) {
     k.var[lins_seq::kPos + i] = prm->init_pos_std[i] * prm->init_pos_std[i];
@@ -190,11 +182,50 @@ void set_init_consts(SeqState& q, const lins_seq_params* prm, const lins_seq_ini
     k.ba[i] = ip->init_ba[i];
     k.bw[i] = ip->init_bw[i];
   }
-  std::memcpy(q.init_consts, &k, sizeof(k));
+  std::memcpy(out, &k, sizeof(k));
+}
+
+constexpr size_t kNConsts = sizeof(SeqState::consts) / sizeof(double), kNInit = sizeof(SeqState::init_consts) / sizeof(double);
+
+// every slot's device constants: a configured slot's from its config, the others the run's; then a synchronisation (the
+// sources are pageable)
+int upload_slot_consts(lins_ctx* ctx, SeqState& q, int n) {
+  std::vector<double> k(kNConsts * n), ik(kNInit * n);
+  for (int s = 0; s < n; ++s) {
+    double* ks = &k[kNConsts * s];
+    double* iks = &ik[kNInit * s];
+    if (q.configured[s]) {
+      consts_of(ks, &q.cfg[s].filter);
+      init_consts_of(iks, &q.cfg[s].filter, &q.cfg[s].init);
+    } else {
+      std::copy(q.consts, q.consts + kNConsts, ks);
+      std::copy(q.init_consts, q.init_consts + kNInit, iks);
+    }
+  }
+  CK(q.slot_consts.reserve(k.size())); CK(q.slot_init_consts.reserve(ik.size()));
+  CK(cudaMemcpyAsync(q.slot_consts.p, k.data(), sizeof(double) * k.size(), cudaMemcpyHostToDevice, ctx->stream));
+  CK(cudaMemcpyAsync(q.slot_init_consts.p, ik.data(), sizeof(double) * ik.size(), cudaMemcpyHostToDevice, ctx->stream));
+  CK(cudaStreamSynchronize(ctx->stream));
+  return LINS_OK;
+}
+const lins_seq::Consts* slot_consts(const SeqState& q) { return reinterpret_cast<const lins_seq::Consts*>(q.slot_consts.p); }
+const lins_seq::InitConsts* slot_init_consts(const SeqState& q) { return reinterpret_cast<const lins_seq::InitConsts*>(q.slot_init_consts.p); }
+
+// the SCAN_PERIOD slot s reads: its config's, else the context's
+double slot_period(const lins_ctx* ctx, int s) {
+  const SeqState& q = ctx->seq;
+  return q.configured[s] ? q.cfg[s].scan_period : ctx->prm.scan_period;
+}
+
+// the host side of a run's slot configuration: every slot unconfigured and fresh
+void reset_slot_configs(SeqState& q, int n) {
+  q.cfg.assign(n, lins_slot_config());
+  q.configured.assign(n, 0);
+  q.fresh.assign(n, 1);
 }
 
 int launch_fresh(lins_ctx* ctx, SeqState& q, int n, const unsigned char* mask_dev) {
-  lins_seq_fresh_kernel<<<(n + 127) / 128, 128, 0, ctx->stream>>>(n, mask_dev, q.glob.p, q.filt.p, q.cov.p, init_consts_of(q));
+  lins_seq_fresh_kernel<<<(n + 127) / 128, 128, 0, ctx->stream>>>(n, mask_dev, q.glob.p, q.filt.p, q.cov.p, slot_init_consts(q));
   CK(cudaGetLastError());
   ctx->launches += 1;
   return LINS_OK;
@@ -321,6 +352,7 @@ int seq_step_phases(lins_ctx* ctx, const lins_seq_step_desc* d, const int32_t* c
     const bool present = !d->present || d->present[s];
     const int nsl = offs[2][s + 1] - offs[2][s], ncl = offs[3][s + 1] - offs[3][s];
     const int32_t fs = q.fusion[s];
+    if (present) q.fresh[s] = 0;
     if (!present) status[s] = LINS_SEQ_IDLE;
     else if (fs == FUSION_RUNNING) status[s] = (ncl <= 5 || nsl <= 10) ? LINS_SEQ_SKIPPED : LINS_SEQ_RAN;  // :436-440
     else if (ncl < 10 || nsl < 100) status[s] = LINS_SEQ_INIT_WAIT;  // processFirstScan / processSecondScan (:331-336, :379-384)
@@ -371,6 +403,7 @@ int seq_step_phases(lins_ctx* ctx, const lins_seq_step_desc* d, const int32_t* c
   const size_t n_imu = d->imu_off ? (size_t)d->imu_off[n] : 0;
   CK(q.imu.reserve(7 * n_imu + 1)); CK(q.imu_off.reserve(N1)); CK(q.h_imu.reserve(7 * n_imu + 1)); CK(q.h_imu_off.reserve(N1));
   CK(q.status_d.reserve(3 * (size_t)n)); CK(q.h_status.reserve(3 * (size_t)n));
+  CK(q.period.reserve(n)); CK(q.h_period.reserve(n));
   const int n_copies = (int)copies.size();
   if ((rc = q.copies.reserve(ctx, n_copies)) != LINS_OK) return rc;
   CK(q.prior_state.reserve((size_t)n * 20)); CK(q.prior_cov.reserve((size_t)n * 324));
@@ -382,13 +415,14 @@ int seq_step_phases(lins_ctx* ctx, const lins_seq_step_desc* d, const int32_t* c
   if (d->imu_off) std::memcpy(q.h_imu_off.p, d->imu_off, sizeof(int) * N1);
   else std::memset(q.h_imu_off.p, 0, sizeof(int) * N1);
   if (n_imu) std::memcpy(q.h_imu.p, d->imu, sizeof(double) * 7 * n_imu);
-  for (int s = 0; s < n; ++s) { q.h_status.p[s] = (unsigned char)status[s]; q.h_status.p[2 * n + s] = imu_use[s]; }
+  for (int s = 0; s < n; ++s) { q.h_status.p[s] = (unsigned char)status[s]; q.h_status.p[2 * n + s] = imu_use[s]; q.h_period.p[s] = slot_period(ctx, s); }
   std::memcpy(r.h_off.p, run_off.data(), sizeof(int) * 2 * N1);
   std::memcpy(r.h_off.p + 2 * N1, init_off.data(), sizeof(int) * 2 * N1);
   if (n_imu) CK(cudaMemcpyAsync(q.imu.p, q.h_imu.p, sizeof(double) * 7 * n_imu, cudaMemcpyHostToDevice, ctx->stream));
   CK(cudaMemcpyAsync(q.imu_off.p, q.h_imu_off.p, sizeof(int) * N1, cudaMemcpyHostToDevice, ctx->stream));
   CK(cudaMemcpyAsync(q.status_d.p, q.h_status.p, n, cudaMemcpyHostToDevice, ctx->stream));
   CK(cudaMemcpyAsync(q.status_d.p + 2 * n, q.h_status.p + 2 * n, n, cudaMemcpyHostToDevice, ctx->stream));
+  CK(cudaMemcpyAsync(q.period.p, q.h_period.p, sizeof(double) * n, cudaMemcpyHostToDevice, ctx->stream));
   if ((rc = q.copies.stage(ctx, copies.data(), n_copies, 0)) != LINS_OK) return rc;
   CK(cudaMemcpyAsync(r.qs_off.p, r.h_off.p, sizeof(int) * N1, cudaMemcpyHostToDevice, ctx->stream));
   CK(cudaMemcpyAsync(r.qc_off.p, r.h_off.p + N1, sizeof(int) * N1, cudaMemcpyHostToDevice, ctx->stream));
@@ -402,8 +436,8 @@ int seq_step_phases(lins_ctx* ctx, const lins_seq_step_desc* d, const int32_t* c
   for (cudaEvent_t& e : q.ev) if (!e) CK(cudaEventCreate(&e));
   q.ev_valid = false;
   CK(cudaEventRecord(q.ev[0], ctx->stream));
-  const lins_seq::Consts k = consts_of(q);
-  const lins_seq::InitConsts ik = init_consts_of(q);
+  const lins_seq::Consts* k = slot_consts(q);
+  const lins_seq::InitConsts* ik = slot_init_consts(q);
   if (n_imu) {
     lins_seq_predict_kernel<<<n, 32, 0, ctx->stream>>>(q.filt.p, q.cov.p, q.imu_last.p, q.imu.p, q.imu_off.p, q.status_d.p + 2 * n, q.pre.p, k, ik);
     CK(cudaGetLastError());
@@ -432,6 +466,7 @@ int seq_step_phases(lins_ctx* ctx, const lins_seq_step_desc* d, const int32_t* c
   bv.ts = q.map_s.p; bv.ts_off = q.map_off.p; bv.tc = q.map_c.p; bv.tc_off = q.map_off.p + N1;
   bv.nn_s = q.tree_s.p; bv.nn_s_off = q.map_off.p + 2 * N1; bv.nn_c = q.tree_c.p; bv.nn_c_off = q.map_off.p + 3 * N1;
   bv.nn_stale = q.stale.p;
+  bv.unit_period = q.period.p;
   bv.state_in = q.prior_state.p; bv.cov_in = q.prior_cov.p; bv.state_out = r.state_out.p; bv.cov_out = r.cov_out.p;
   bv.results = r.results.p; bv.reports = r.reports.p;
   bv.ind_s = r.ind_s.p; bv.ind_c = r.ind_c.p; bv.az_s = r.az_s.p; bv.az_c = r.az_c.p;
@@ -459,7 +494,7 @@ int seq_step_phases(lins_ctx* ctx, const lins_seq_step_desc* d, const int32_t* c
     CK(cudaMemcpyAsync(q.icp_pose.p + (size_t)s * 20, q.prior_state.p + (size_t)s * 20, sizeof(double) * 20, cudaMemcpyDeviceToDevice, ctx->stream));
     BatchView u = bv;
     u.n_scans = 1;
-    u.qs_off += s; u.qc_off += s; u.ts_off += s; u.tc_off += s; u.nn_s_off += s; u.nn_c_off += s; u.nn_stale += s;
+    u.qs_off += s; u.qc_off += s; u.ts_off += s; u.tc_off += s; u.nn_s_off += s; u.nn_c_off += s; u.nn_stale += s; u.unit_period += s;
     u.cov_in += (size_t)s * 324; u.state_out += (size_t)s * 20; u.cov_out += (size_t)s * 324; u.results += s; u.reports = nullptr;
     u.accum += (size_t)s * 32;
     u.ind_s = q.icp_ind_s.p; u.ind_c = q.icp_ind_c.p;  // (the IESKF's IDs stay readable)
@@ -507,8 +542,8 @@ int seq_step_phases(lins_ctx* ctx, const lins_seq_step_desc* d, const int32_t* c
   for (int s = 0; s < n; ++s)
     q.h_status.p[n + s] = status[s] == LINS_SEQ_RAN || status[s] == LINS_SEQ_ICP || status[s] == LINS_SEQ_SECOND ? 1 : 0;
   CK(cudaMemcpyAsync(run_mask, q.h_status.p + n, n, cudaMemcpyHostToDevice, ctx->stream));
-  rc = transform_to_end_csr(ctx, q.up.ts.p, q.up.ts_off.p, n, q.lin.p, run_mask);
-  if (rc == LINS_OK) rc = transform_to_end_csr(ctx, q.up.tc.p, q.up.tc_off.p, n, q.lin.p, run_mask);
+  rc = transform_to_end_csr(ctx, q.up.ts.p, q.up.ts_off.p, n, q.lin.p, run_mask, q.period.p);
+  if (rc == LINS_OK) rc = transform_to_end_csr(ctx, q.up.tc.p, q.up.tc_off.p, n, q.lin.p, run_mask, q.period.p);
   if (rc == LINS_OK) rc = q.copies.launch(ctx, n_qcopies, n_copies - n_qcopies);
   if (rc != LINS_OK) return rc;
   swap_maps(q);
@@ -594,7 +629,9 @@ int step_from_projection(lins_ctx* ctx, const uint8_t* pres, const double* imu, 
   in.n = n; in.line_num = line_num; in.total = src_off[n];
   in.pts = pr.seg.p; in.off = pr.up.qs_off.p; in.count = pr.counts.p; in.count_stride = 2;
   in.ground = pr.ground.p; in.col = pr.col.p; in.range = pr.range.p; in.ring = pr.ring.p; in.ori = pr.ori.p;
-  int rc = features_launch(ctx, fp, in);
+  std::vector<FeatConsts> k(n);  // each slot's config, else the call's fp and the context's period
+  for (int s = 0; s < n; ++s) k[s] = feat_consts(q.configured[s] ? q.cfg[s].features : *fp, slot_period(ctx, s));
+  int rc = features_launch(ctx, k.data(), in);
   if (rc != LINS_OK) return rc;
   if (pb.bound) {  // the stash: every slot's outlier cloud, device to device (an absent slot's sweep projected empty)
     pb.h_stash_off.assign((size_t)n + 1, 0);
@@ -696,7 +733,9 @@ int seq_map_run(lins_ctx* ctx, const lins_seq_map_desc* d, lins_mapper_report* r
   lins_mappers_desc md;
   std::memset(&md, 0, sizeof(md));
   md.n_slots = n; md.present = pub.data(); md.time = d->time; md.quat = quat.data(); md.pos = pos.data();
-  return mappers_step(ctx, ctx->mappers, &md, reps, dev.data());
+  std::vector<double> period(n);
+  for (int s = 0; s < n; ++s) period[s] = slot_period(ctx, s);
+  return mappers_step(ctx, ctx->mappers, &md, reps, dev.data(), period.data());
 }
 
 }  // namespace
@@ -742,7 +781,10 @@ int lins_gpu_seq_begin(lins_ctx* ctx, const lins_seq_params* prm, const lins_seq
   CK(cudaMemcpyAsync(q.cov.p, d->filter_cov, sizeof(double) * 324 * (size_t)n, cudaMemcpyHostToDevice, ctx->stream));
   CK(queue_map_state(ctx, q));
   CK(cudaStreamSynchronize(ctx->stream));  // (the sources above are pageable host memory)
-  set_consts(q, prm);
+  consts_of(q.consts, prm);
+  std::fill(q.init_consts, q.init_consts + kNInit, 0.0);  // (a hand-over does not initialise)
+  reset_slot_configs(q, n);
+  if ((rc = upload_slot_consts(ctx, q, n)) != LINS_OK) return rc;
   // result records / reports read as zero until a step has run a sequence's IESKF
   CK(cudaMemsetAsync(q.run.results.p, 0, sizeof(lins_scan_result) * n, ctx->stream));
   CK(cudaMemsetAsync(q.run.reports.p, 0, sizeof(lins_report) * n, ctx->stream));
@@ -761,8 +803,10 @@ int lins_gpu_seq_open(lins_ctx* ctx, const lins_seq_params* prm, const lins_seq_
   int rc = reserve_run(ctx, q, n, 0, 0);  // (no maps)
   if (rc != LINS_OK) return rc;
   CK(q.pre.reserve((size_t)n * 20)); CK(q.init_icp.reserve(icp_state_bytes() * n));
-  set_consts(q, prm);
-  set_init_consts(q, prm, ip);
+  consts_of(q.consts, prm);
+  init_consts_of(q.init_consts, prm, ip);
+  reset_slot_configs(q, n);
+  if ((rc = upload_slot_consts(ctx, q, n)) != LINS_OK) return rc;
   q.h_map_off.assign(4 * (size_t)(n + 1), 0);
   q.h_stale_v.assign(n, 0);
   CK(cudaMemsetAsync(q.lin.p, 0, sizeof(double) * 20 * (size_t)n, ctx->stream));
@@ -798,6 +842,10 @@ int lins_gpu_seq_restart(lins_ctx* ctx, const uint8_t* mask) {
   if (rc != LINS_OK) return rc;
   CK(q.status_d.reserve(3 * (size_t)n)); CK(q.h_status.reserve(3 * (size_t)n));
   // (the last step ended with a stream synchronisation: the pinned staging is free)
+  // the restarted slots are unconfigured again: their constants go back to the run's before the fresh state reads them
+  bool any_configured = false;
+  for (int s = 0; s < n; ++s) if (mask[s] && q.configured[s]) { q.configured[s] = 0; any_configured = true; }
+  if (any_configured && (rc = upload_slot_consts(ctx, q, n)) != LINS_OK) { q.n = 0; return rc; }
   if ((rc = q.copies.stage(ctx, copies.data(), (int)copies.size(), 0)) != LINS_OK) return rc;
   for (int s = 0; s < n; ++s) q.h_status.p[s] = mask[s] ? 1 : 0;
   CK(cudaMemcpyAsync(q.status_d.p, q.h_status.p, n, cudaMemcpyHostToDevice, ctx->stream));
@@ -806,7 +854,7 @@ int lins_gpu_seq_restart(lins_ctx* ctx, const uint8_t* mask) {
   if (rc != LINS_OK) { q.n = 0; return rc; }  // (some slots may have changed: the run ends, as after a failed step)
   swap_maps(q);
   for (int s = 0; s < n; ++s)
-    if (mask[s]) { q.h_stale_v[s] = 0; q.fusion[s] = FUSION_INIT; q.status[s] = LINS_SEQ_IDLE; }
+    if (mask[s]) { q.h_stale_v[s] = 0; q.fusion[s] = FUSION_INIT; q.status[s] = LINS_SEQ_IDLE; q.fresh[s] = 1; }
   if (q.pub.bound) {  // a new recording is a new LinsFusion with a new mapping node
     for (int s = 0; s < n; ++s) if (mask[s]) pub_fresh(q.pub, s);
     if ((rc = mappers_reset(ctx, ctx->mappers, mask)) != LINS_OK) return rc;
@@ -814,6 +862,43 @@ int lins_gpu_seq_restart(lins_ctx* ctx, const uint8_t* mask) {
   CK(queue_map_state(ctx, q));
   CK(cudaStreamSynchronize(ctx->stream));  // (the two sources above are pageable)
   return LINS_OK;
+}
+
+int lins_gpu_seq_configure(lins_ctx* ctx, const uint8_t* mask, const lins_slot_config* cfg) {
+  if (!ctx) return LINS_E_INVALID;
+  SeqState& q = ctx->seq;
+  if (q.n == 0) return fail(ctx, LINS_E_NOMAP, "no sequence run: call lins_gpu_seq_open");
+  if (!mask || !cfg) return fail(ctx, LINS_E_INVALID, "null configure mask / configs");
+  if (!q.has_init) return fail(ctx, LINS_E_INVALID, "lins_gpu_seq_configure needs a run opened by lins_gpu_seq_open");
+  const int n = q.n;
+  for (int s = 0; s < n; ++s) {
+    if (!mask[s]) continue;
+    if (!q.fresh[s]) return fail(ctx, LINS_E_INVALID, "a configured slot must be fresh (no step since open / restart)");
+    const lins_slot_config& c = cfg[s];
+    const lins_seq_params& f = c.filter;
+    const lins_seq_init_params& i = c.init;
+    bool ok = std::isfinite(c.scan_period) && c.scan_period > 0 && std::isfinite(c.features.edge_threshold) &&
+              std::isfinite(c.features.surf_threshold) && std::isfinite(c.features.imu_lidar_extrinsic_angle);
+    auto nonneg = [&](const double* v, int m) { for (int k = 0; k < m; ++k) ok = ok && std::isfinite(v[k]) && v[k] >= 0; };
+    auto finite = [&](const double* v, int m) { for (int k = 0; k < m; ++k) ok = ok && std::isfinite(v[k]); };
+    nonneg(f.noise, 4); nonneg(f.init_pos_std, 3); nonneg(f.init_att_std, 3);
+    nonneg(i.init_vel_std, 3); nonneg(i.init_acc_std, 3); nonneg(i.init_gyr_std, 3);
+    finite(i.init_ba, 3); finite(i.init_bw, 3);
+    if (!ok) return fail(ctx, LINS_E_INVALID, "bad slot config (non-finite value, scan_period <= 0, or a negative noise / std)");
+  }
+  CK(cudaSetDevice(ctx->device));
+  CK(q.status_d.reserve(3 * (size_t)n)); CK(q.h_status.reserve(3 * (size_t)n));
+  // from here on the slots change: a failure ends the run, as a failed restart does
+  for (int s = 0; s < n; ++s) if (mask[s]) { q.cfg[s] = cfg[s]; q.configured[s] = 1; }
+  int rc = upload_slot_consts(ctx, q, n);
+  if (rc == LINS_OK) {
+    for (int s = 0; s < n; ++s) q.h_status.p[s] = mask[s] ? 1 : 0;
+    if (cudaMemcpyAsync(q.status_d.p, q.h_status.p, n, cudaMemcpyHostToDevice, ctx->stream) != cudaSuccess) rc = fail(ctx, LINS_E_CUDA, "configure mask upload");
+  }
+  if (rc == LINS_OK) rc = launch_fresh(ctx, q, n, q.status_d.p);  // initializeCovariance with the config's stds
+  if (rc == LINS_OK && cudaStreamSynchronize(ctx->stream) != cudaSuccess) rc = fail(ctx, LINS_E_CUDA, "configure");
+  if (rc != LINS_OK) q.n = 0;
+  return rc;
 }
 
 int lins_gpu_seq_step_ex(lins_ctx* ctx, const lins_seq_step_desc* d, const double* scan_imu) {
@@ -834,7 +919,9 @@ int lins_gpu_seq_step_pcl(lins_ctx* ctx, const lins_seq_pcl_desc* d, const lins_
   int rc = check_step(ctx, d, d ? d->pcl.n_scans : 0, scan_imu);
   if (rc != LINS_OK) return rc;
   // extraction, validation of the scans and the counts' read-back: nothing of the sequences has changed yet
-  rc = features_run(ctx, fp, &d->pcl);
+  std::vector<double> period(ctx->seq.n);  // (the re-stamp: each slot's period; the thresholds and extrinsic are fp's)
+  for (int s = 0; s < ctx->seq.n; ++s) period[s] = slot_period(ctx, s);
+  rc = features_run(ctx, fp, &d->pcl, period.data());
   if (rc != LINS_OK) return rc;
   return step_from_features(ctx, d->present, d->imu, d->imu_off, d->pcl.cloud_off, scan_imu);
 }

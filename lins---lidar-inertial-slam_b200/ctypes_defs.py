@@ -183,6 +183,24 @@ class LinsFeatureParams(C.Structure):
         return cls(edge_threshold, surf_threshold, imu_lidar_extrinsic_angle)
 
 
+class LinsSlotConfig(C.Structure):
+    """lins_slot_config (include/lins_gpu.h): one recording's rig, the exp_port.yaml values that describe its sensors."""
+    _fields_ = [("scan_period", C.c_double), ("features", LinsFeatureParams), ("filter", LinsSeqParams), ("init", LinsSeqInitParams)]
+
+    @classmethod
+    def shipped(cls, scan_period=0.1, **kw):
+        """The shipped rig (LinsFeatureParams / LinsSeqParams / LinsSeqInitParams.shipped) with any of their keyword
+        arguments overridden, e.g. shipped(scan_period=0.05, edge_threshold=1.0, acc_n=5e4, init_ba=(0, 0, 0))."""
+        import inspect
+        parts = []
+        for sub in (LinsFeatureParams, LinsSeqParams, LinsSeqInitParams):
+            names = inspect.signature(sub.shipped).parameters
+            parts.append(sub.shipped(**{k: kw.pop(k) for k in list(kw) if k in names}))
+        if kw:
+            raise TypeError(f"unknown slot config keys: {sorted(kw)}")
+        return cls(scan_period, *parts)
+
+
 class LinsPclDesc(C.Structure):
     """lins_pcl_desc: n segmented scans with their cloud_info, CSR."""
     _fields_ = [("n_scans", C.c_int32), ("line_num", C.c_int32), ("cloud", C.c_void_p), ("cloud_off", C.c_void_p),

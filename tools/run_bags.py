@@ -9,7 +9,11 @@ bag's model (lins_gpu_seq_step_cloud2_mixed).  Prints a summary line and the tra
 --out, writes DIR/<bag name>.npz (stamps, status, scan_status, global_est, iters, flags per scan).  With --map, each
 bag's mapping node runs on what its estimator publishes, in lockstep on the device (lins_gpu_seq_map_step), and
 DIR/<bag name>.odometry.txt and DIR/<bag name>.mapped.txt (DIR: --out, default .) receive the two trajectories in
-tools/run_bag.py --map's line format; like run_bag.py --map, the bags' IMU orientation is not fed to the mappers."""
+tools/run_bag.py --map's line format; like run_bag.py --map, the bags' IMU orientation is not fed to the mappers.
+--config a.yaml[,b.yaml,...] takes LINS config files (exp_port.yaml, OpenCV YAML): one for every bag or one per bag.
+Each bag's slot is configured with its file's rig (scan period, feature thresholds, extrinsic, IMU noise, init stds and
+biases); the files must agree on the keys every slot shares (num_iter, icp_freq, nearest_feature_search_sq_dist,
+lidar_std, lidar_scale), which set the context's parameters."""
 import argparse, importlib, os, sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import numpy as np
@@ -29,6 +33,25 @@ def lidar_models(spec, n_bags):
     if len(vals) != n_bags:
         raise ValueError(f"--lidar-model lists {len(vals)} models for {n_bags} bags")
     return [presets[v]() for v in vals]
+
+
+def bag_configs(spec, n_bags):
+    """(LinsParams of the context, one LinsSlotConfig per bag) from the --config value: one file for every bag or a
+    comma-separated list with one per bag.  ValueError for a count mismatch or files whose shared keys disagree."""
+    rc = importlib.import_module("lins---lidar-inertial-slam_b200.rig_config")
+    paths = [v.strip() for v in str(spec).split(",")]
+    if len(paths) not in (1, n_bags):
+        raise ValueError(f"--config lists {len(paths)} files for {n_bags} bags")
+    loaded = [rc.load_rig(p) for p in paths]
+    shared = loaded[0][1]
+    for p, (_, sh) in zip(paths, loaded):
+        bad = [k for k in rc.SHARED_KEYS if sh[k] != shared[k]]
+        if bad:
+            raise ValueError(f"--config: {p} and {paths[0]} disagree on {', '.join(bad)}, which every slot of a run shares")
+    cfgs = [rc.slot_config(r) for r, _ in loaded]
+    if len(cfgs) == 1:
+        cfgs = cfgs * n_bags
+    return rc.lins_params(shared), cfgs
 
 
 def write_map(o, out_dir, name):
@@ -51,15 +74,18 @@ def main(argv=None):
     ap.add_argument("--max-scans", type=int, default=0)
     ap.add_argument("--lidar-model", default="0", help="0 | 1 for every bag, or one per bag: 0,1,...")
     ap.add_argument("--map", action="store_true", help="run each bag's mapping node on what its estimator publishes")
+    ap.add_argument("--config", help="LINS config file(s): one for every bag, or one per bag: a.yaml,b.yaml,...")
     ap.add_argument("--out")
     a = ap.parse_args(argv)
     try:
         model = lidar_models(a.lidar_model, len(a.bags))
+        prm, cfgs = bag_configs(a.config, len(a.bags)) if a.config else (None, [None] * len(a.bags))
     except ValueError as e:
         ap.error(str(e))
     br = importlib.import_module("lins---lidar-inertial-slam_b200.bag_replay")
-    recs = [br.Recording(p, a.lidar, a.imu, a.max_scans) for p in a.bags]
-    outs = br.replay(recs, a.slots or len(recs), model=model, map=a.map)
+    capi = importlib.import_module("lins---lidar-inertial-slam_b200.capi")
+    recs = [br.Recording(p, a.lidar, a.imu, a.max_scans, config=c) for p, c in zip(a.bags, cfgs)]
+    outs = br.replay(recs, a.slots or len(recs), model=model, map=a.map, gpu=capi.LinsGpu(prm) if prm is not None else None)
     np.set_printoptions(precision=4, suppress=True)
     for p, o in zip(a.bags, outs):
         print(p, br.summary(o))

@@ -68,8 +68,10 @@ struct SimDrive {
   Pose P;
   double t = 0.0;
   static constexpr int nimu = 40;
-  SimDrive(const lins_synth_cfg* c, uint64_t seed) : cfg(c), rng(seed) {
+  // scan_period > 0: the sweep lasts that long (the IMU rate follows: nimu samples per sweep); else the model's SCAN_PERIOD
+  SimDrive(const lins_synth_cfg* c, uint64_t seed, double scan_period = 0.0) : cfg(c), rng(seed) {
     lm = cfg->lidar == 1 ? LidarModel::dense64() : LidarModel::vlp16();
+    if (scan_period > 0) lm.scan_period = scan_period;
     w = make_world(rng, cfg->world);
     tr = Traj{rng.uni(1.0, 0.6 * cfg->v_max), rng.uni(0.2, 1.0), rng.uni(0.5, 1.5), rng.uni(-0.5, 0.5) * cfg->w_max, 0.5 * cfg->w_max, rng.uni(0.3, 1.0)};
     P.R = math_utils::rpy2Quat(V3D(0.0, 0.0, rng.uni(-M_PI, M_PI))).toRotationMatrix();
@@ -223,9 +225,11 @@ void* lins_seq_run(const lins_synth_cfg* cfg, uint64_t seed, int n_scans, int de
 
 // The same simulated drive written as a ROS1 bag (csrc/host/rosbag_reader.hpp): the raw sweeps on `lidar_topic`
 // (sensor_msgs/PointCloud2, stamped at the sweep's end like LinsFusion uses them) and the IMU samples on `imu_topic`.
-int lins_seq_write_bag(const lins_synth_cfg* cfg, uint64_t seed, int n_scans, const char* path, const char* lidar_topic, const char* imu_topic) {
+// scan_period: the sweep's duration (lins_seq_write_bag_period; 0 = the model's SCAN_PERIOD, 0.1 s)
+int lins_seq_write_bag_period(const lins_synth_cfg* cfg, uint64_t seed, int n_scans, const char* path, const char* lidar_topic, const char* imu_topic,
+                              double scan_period) {
   using namespace lins::rosbag;
-  SimDrive sim(cfg, seed);
+  SimDrive sim(cfg, seed, scan_period);
   Writer w;
   if (w.open(path) != LINS_BAG_OK) return LINS_BAG_E_IO;
   const uint32_t cl = w.add_connection(lidar_topic, "sensor_msgs/PointCloud2", "1158d486dd51d683ce2f1be655c3c181", "(sensor_msgs/PointCloud2)");
@@ -245,12 +249,19 @@ int lins_seq_write_bag(const lins_synth_cfg* cfg, uint64_t seed, int n_scans, co
   }
   return w.close();
 }
+int lins_seq_write_bag(const lins_synth_cfg* cfg, uint64_t seed, int n_scans, const char* path, const char* lidar_topic, const char* imu_topic) {
+  return lins_seq_write_bag_period(cfg, seed, n_scans, path, lidar_topic, imu_topic, 0.0);
+}
 
 // BASELINE.json configs[1] runner: replay a bag the way LinsFusion does (Estimator.cpp:123-284): IMU messages are buffered,
 // every lidar message is a scan at its header stamp; between two scans the buffered IMU samples are propagated with
 // dt = min(imu stamp, scan stamp) - estimator time (:230-236); the raw cloud goes through the restated image projection.
 // Returns a record handle like lins_seq_run (status / pose per scan, one recorded unit per performIESKF call) or null.
-void* lins_seq_run_bag(const char* path, const char* lidar_topic, const char* imu_topic, int max_scans, int lidar_model, int device, int* error) {
+// rig (lins_seq_run_bag_rig; null = seq_params' defaults): the exp_port.yaml values of one robot, 29 doubles in the order
+// scan_period, edge_threshold, surf_threshold, imu_lidar_extrinsic_angle, acc_n, gyr_n, acc_w, gyr_w, then init_pos_std,
+// init_vel_std, init_att_std, init_acc_std, init_gyr_std, init_ba, init_bw (3 each)
+void* lins_seq_run_bag_rig(const char* path, const char* lidar_topic, const char* imu_topic, int max_scans, int lidar_model, int device,
+                           const double* rig, int* error) {
   using namespace lins::rosbag;
   if (error) *error = 0;
   Reader rd;
@@ -277,8 +288,19 @@ void* lins_seq_run_bag(const char* path, const char* lidar_topic, const char* im
   std::stable_sort(imus.begin(), imus.end(), [](const ImuS& x, const ImuS& y) { return x.t < y.t; });
   std::stable_sort(scans.begin(), scans.end(), [](const std::pair<double, Cloud>& x, const std::pair<double, Cloud>& y) { return x.first < y.first; });
   SeqRecord* rec = new SeqRecord();
-  const LidarModel lm = lidar_model == 1 ? LidarModel::dense64() : LidarModel::vlp16();
-  StateEstimator est(seq_params(lm), device);
+  LidarModel lm = lidar_model == 1 ? LidarModel::dense64() : LidarModel::vlp16();
+  lins::fusion::EstimatorParams ep = seq_params(lm);
+  if (rig) {
+    lm.scan_period = rig[0];
+    ep = seq_params(lm);
+    ep.gpu.scan_period = rig[0];
+    ep.feature.edge_threshold = rig[1]; ep.feature.surf_threshold = rig[2]; ep.feature.imu_lidar_extrinsic_angle = rig[3];
+    ep.filter.acc_n = rig[4]; ep.filter.gyr_n = rig[5]; ep.filter.acc_w = rig[6]; ep.filter.gyr_w = rig[7];
+    V3D* v[7] = {&ep.filter.init_pos_std, &ep.filter.init_vel_std, &ep.filter.init_att_std, &ep.filter.init_acc_std, &ep.filter.init_gyr_std,
+                 &ep.filter.init_ba, &ep.filter.init_bw};
+    for (int k = 0; k < 7; ++k) *v[k] = V3D(rig[8 + 3 * k], rig[9 + 3 * k], rig[10 + 3 * k]);
+  }
+  StateEstimator est(ep, device);
   ImageProjection ip(lm);
   const bool verbose = std::getenv("LINS_SEQ_VERBOSE") != nullptr;
   size_t next_imu = 0;
@@ -299,6 +321,10 @@ void* lins_seq_run_bag(const char* path, const char* lidar_topic, const char* im
     feed_scan(est, ip, rec, (int)k, ts, scans[k].second, dts, acc, gyr, nullptr, nullptr, verbose);
   }
   return rec;
+}
+
+void* lins_seq_run_bag(const char* path, const char* lidar_topic, const char* imu_topic, int max_scans, int lidar_model, int device, int* error) {
+  return lins_seq_run_bag_rig(path, lidar_topic, imu_topic, max_scans, lidar_model, device, nullptr, error);
 }
 
 // ---- feature logs: what the front end hands the estimator per scan, replayable through the shim or sequence mode ------

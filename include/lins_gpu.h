@@ -551,6 +551,31 @@ typedef struct lins_slot_config {
    without a run. */
 int lins_gpu_seq_configure(lins_ctx* ctx, const uint8_t* mask /*S*/, const lins_slot_config* cfg /*S*/);
 
+/* ---- per-slot estimator tuning: the rest of exp_port.yaml the odometry reads -----------------------------------------
+   A slot of a lins_gpu_seq_open run reads the context's current lins_params (num_iter, icp_freq, the 1-NN gate, lidar_std,
+   lidar_scale) at every step and takes its IMU values as they come, unless it is tuned.  A tuned slot reads its own
+   values everywhere the reference reads them: performIESKF's pass count and exit, its iter % ICP_FREQ searches, the
+   iter >= ICP_FREQ weighting, the 1-NN gate, LIDAR_STD^2 in the gain and LIDAR_SCALE in the residual; NUM_ITER caps its
+   estimateTransform fallback and its second scan's estimateTransform, whose association uses its gate and ICP_FREQ.  And
+   it runs alignIMUtoVehicle (Estimator.cpp:286-292) on every IMU value it receives: acc and gyr of the step's IMU rows
+   (dt unchanged) and of its scan_imu sample become R^T v, R = rpy2R((0, 0, deg2rad(imu_misalign_angle))), in f64 with
+   cos / sin from the host's libm, even when the angle is 0.  force_all_iters and verbose stay per context.  Tuning and
+   configuring (lins_gpu_seq_configure) are independent and either can come first.  Each tuned slot is bit-identical to
+   the same recording, its IMU values rotated the same way, in a context whose lins_params equal its tuning. */
+typedef struct lins_slot_tuning {
+  int32_t num_iter;                        /* NUM_ITER, 0 .. LINS_MAX_ITER */
+  int32_t icp_freq;                        /* ICP_FREQ, >= 1 */
+  double nearest_feature_search_sq_dist;   /* NEAREST_FEATURE_SEARCH_SQ_DIST */
+  double lidar_std, lidar_scale;           /* LIDAR_STD, LIDAR_SCALE */
+  double imu_misalign_angle;               /* IMU_MISALIGN_ANGLE, degrees: alignIMUtoVehicle's yaw */
+} lins_slot_tuning;
+/* Tunes every slot with mask[s] != 0 with t[s] (t has S entries; the unmasked ones are not read).  A slot can be tuned
+   only while it is fresh, like lins_gpu_seq_configure; lins_gpu_seq_restart returns it to untuned.  All or nothing:
+   LINS_E_INVALID, with nothing changed, for a NULL mask or t, a run of lins_gpu_seq_begin, a masked slot that is not
+   fresh, or a masked tuning with num_iter outside 0..LINS_MAX_ITER, icp_freq < 1 or a non-finite double.  LINS_E_NOMAP
+   without a run. */
+int lins_gpu_seq_tune(lins_ctx* ctx, const uint8_t* mask /*S*/, const lins_slot_tuning* t /*S*/);
+
 /* Split "Jacobian kernel" (SURVEY.md §8(d) unit U1): de-skew, residual, robust weight and the factored Jacobian row
    g = [c ; p x (R^T c)], r = lidar_scale * coeff.w of every query of the resident batch, reduced per unit.  The
    linearisation point is each unit's posterior (what lins_gpu_batch_download returns as state_out, R its rotation) and the

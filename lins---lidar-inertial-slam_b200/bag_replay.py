@@ -17,7 +17,9 @@ lins_gpu_seq_map_step publishes what each slot's LinsFusion::publishTopics would
 that published, on the device clouds.
 A recording may carry its rig (a LinsSlotConfig: scan period, feature thresholds, extrinsic, IMU noise and biases, as a
 LINS exp_port.yaml gives them): its slot is configured with it (lins_gpu_seq_configure) when it takes the recording, and
-its IMU schedule uses that scan period.  Recordings without one use the run's values.
+its IMU schedule uses that scan period.  Recordings without one use the run's values.  A recording may also carry its
+tuning (a LinsSlotTuning: NUM_ITER, ICP_FREQ, the 1-NN gate, LIDAR_STD, LIDAR_SCALE and imu_misalign_angle): its slot is
+tuned with it (lins_gpu_seq_tune) where it is configured, and the device rotates its IMU rows, which stay raw here.
 """
 import ctypes as C
 import importlib.util
@@ -51,13 +53,16 @@ def layout(ix):
 class Recording:
     """One bag: its scans (stamp, layout, data field) and, per scan, the processImu rows (dt, acc, gyr) and processPCL's
     IMU sample.  config: the bag's rig (LinsSlotConfig; None = the run's values); its scan_period is the schedule's, and a
-    scan_period given as well must equal it."""
+    scan_period given as well must equal it.  tuning: the bag's estimator tuning and IMU misalignment (LinsSlotTuning;
+    None = the context's lins_params and no rotation)."""
 
-    def __init__(self, path, lidar_topic="/velodyne_points", imu_topic="/imu/data", max_scans=0, scan_period=None, config=None):
+    def __init__(self, path, lidar_topic="/velodyne_points", imu_topic="/imu/data", max_scans=0, scan_period=None, config=None,
+                 tuning=None):
         if config is not None and scan_period is not None and scan_period != config.scan_period:
             raise ValueError(f"scan_period {scan_period} differs from the config's {config.scan_period}")
         scan_period = config.scan_period if config is not None else (0.1 if scan_period is None else scan_period)
         self.config = config
+        self.tuning = tuning
         bt = _bag_tool()
         conns, msgs = bt.read_bag(path)
         topic = {cid: c["topic"] for cid, c in conns.items()}
@@ -210,6 +215,9 @@ def replay(recordings, slots, model=None, device=0, gpu=None, map=False):
             fresh = [w is not None and w[1] == 0 and getattr(recordings[w[0]], "config", None) is not None for w in who]
             if any(fresh):  # a slot taking a recording with a rig of its own (after open or its restart)
                 g.seq_configure(np.array(fresh, np.uint8), [recordings[w[0]].config if f else None for w, f in zip(who, fresh)])
+            tuned = [w is not None and w[1] == 0 and getattr(recordings[w[0]], "tuning", None) is not None for w in who]
+            if any(tuned):  # ... and one with a tuning of its own
+                g.seq_tune(np.array(tuned, np.uint8), [recordings[w[0]].tuning if f else None for w, f in zip(who, tuned)])
             present = np.array([w is not None for w in who], np.uint8)
             imus = [recordings[w[0]].imu[w[1]] if w else np.zeros((0, 7)) for w in who]
             imu_off = np.concatenate([[0], np.cumsum([len(r) for r in imus])]).astype(np.int32)

@@ -15,7 +15,7 @@ import numpy as np
 
 from .ctypes_defs import (Batch, COV_SIZE, LinsBatchDesc, LinsCloud2Desc, LinsCloud2Layout, LinsFeatureParams, LinsLidarModel, LinsLidarModels, LinsMapperDesc, LinsMapperReport, LinsMappersDesc, LinsMapReport, LinsParams, LinsPclDesc,
                           LinsRawDesc, LinsReport, LinsScanResult, LinsSeqBeginDesc, LinsSeqInitParams, LinsSeqParams, LinsSeqPclDesc,
-                          LinsSeqCloud2Desc, LinsSeqMapDesc, LinsSeqRawDesc, LinsSeqStepDesc, LinsSlotConfig, POINT_DTYPE, SCAN_RESULT_DTYPE, STATE_DIM, as_points, make_points, ptr)
+                          LinsSeqCloud2Desc, LinsSeqMapDesc, LinsSeqRawDesc, LinsSeqStepDesc, LinsSlotConfig, LinsSlotTuning, POINT_DTYPE, SCAN_RESULT_DTYPE, STATE_DIM, as_points, make_points, ptr)
 
 _PKG = os.path.dirname(os.path.abspath(__file__))
 _ROOT = os.path.dirname(_PKG)
@@ -38,7 +38,7 @@ EXPORTS = [
     "lins_gpu_project_scans_mixed", "lins_gpu_seq_step_raw_mixed", "lins_gpu_seq_step_cloud2_mixed",
     "lins_gpu_mapper_reset", "lins_gpu_mapper_imu", "lins_gpu_mapper_step", "lins_gpu_mapper_download", "lins_gpu_voxel_grid",
     "lins_gpu_mappers_open", "lins_gpu_mappers_reset", "lins_gpu_mappers_imu", "lins_gpu_mappers_step", "lins_gpu_mappers_download",
-    "lins_gpu_seq_map_open", "lins_gpu_seq_map_step", "lins_gpu_seq_map_published", "lins_gpu_seq_configure",
+    "lins_gpu_seq_map_open", "lins_gpu_seq_map_step", "lins_gpu_seq_map_published", "lins_gpu_seq_configure", "lins_gpu_seq_tune",
 ]
 
 NVCC_ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]  # H100 (Hopper)
@@ -121,6 +121,7 @@ def lib():
         L.lins_gpu_seq_open.argtypes = [vp, C.POINTER(LinsSeqParams), C.POINTER(LinsSeqInitParams), C.c_int32]
         L.lins_gpu_seq_restart.argtypes = [vp, vp]
         L.lins_gpu_seq_configure.argtypes = [vp, vp, vp]
+        L.lins_gpu_seq_tune.argtypes = [vp, vp, vp]
         L.lins_gpu_seq_step_ex.argtypes = [vp, C.POINTER(LinsSeqStepDesc), vp]
         L.lins_gpu_seq_download_init.argtypes = [vp, vp, vp, vp, vp]
         L.lins_gpu_extract_features.argtypes = [vp, C.POINTER(LinsFeatureParams), C.POINTER(LinsPclDesc)] + [vp] * 6
@@ -536,6 +537,15 @@ class LinsGpu:
             raise ValueError(f"mask / configs have {len(m)} / {len(configs)} entries, the run {self._seq_n}")
         arr = (LinsSlotConfig * self._seq_n)(*[c if c is not None else LinsSlotConfig() for c in configs])
         self._ck(self.L.lins_gpu_seq_configure(self.h, ptr(m), C.cast(arr, C.c_void_p)))
+
+    def seq_tune(self, mask, tunings):
+        """Tune the slots with mask[s] != 0, each still fresh, with their own estimator tuning and IMU misalignment:
+        tunings is a LinsSlotTuning per slot (S entries; None where the mask is 0).  A restart returns a slot to untuned."""
+        m = np.ascontiguousarray(mask, dtype=np.uint8)
+        if len(m) != self._seq_n or len(tunings) != self._seq_n:
+            raise ValueError(f"mask / tunings have {len(m)} / {len(tunings)} entries, the run {self._seq_n}")
+        arr = (LinsSlotTuning * self._seq_n)(*[t if t is not None else LinsSlotTuning() for t in tunings])
+        self._ck(self.L.lins_gpu_seq_tune(self.h, ptr(m), C.cast(arr, C.c_void_p)))
 
     def seq_download_init(self):
         """dict: fusion_status (S; StateEstimator::status_ of every slot) and, for the slots whose last scan was a second

@@ -121,7 +121,6 @@ __device__ __forceinline__ int slot_of(int v, int Q) { return (v >= Q) + (v >= 2
 template <int MODE>
 __device__ void association_pass(CtaMem& cta, Smem* slots, const BatchView& bv, const KParams& kp, const PassBuffers& pb) {
   const int Q = bv.qtile, NQ = bv.nslots * Q;
-  const float nearf = (float)kp.nearest_sq;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
 
   // ---- A2: de-skew, fused with phase P1 of the association (same thread-per-query mapping; P1 touches only its own
@@ -137,8 +136,7 @@ __device__ void association_pass(CtaMem& cta, Smem* slots, const BatchView& bv, 
     const float4 s = transform_to_start(pb.qpt[v], sm, sm.period);
     pb.sel[v] = s;
     pb.key[v] = kKeyMax;
-    const bool search = (sm.iter % kp.icp_freq) == 0;
-    if (!search) {
+    if (!sm.search) {
       // iter % ICP_FREQ != 0: reuse pointSearch*Ind (StateEstimator.hpp:844, :970); a unit that has not searched in this
       // launch takes them from global memory (they persist between calls like the reference's arrays)
       if (!sm.pos_valid) {
@@ -154,7 +152,7 @@ __device__ void association_pass(CtaMem& cta, Smem* slots, const BatchView& bv, 
     float4 qa = make_float4(0.f, 0.f, -1.f, 0.f);
     if (seeded) {  // certificates (lins_assoc_az.cuh: cert_check / cert_rejected): the stored answers still hold
       const float4 r1 = pb.qref[v], r2 = pb.qref2[v], ex = pb.qext[v];
-      const unsigned nearbits = __float_as_uint(nearf);
+      const unsigned nearbits = __float_as_uint(sm.nearf);
       const int w1s = pb.pos[3 * v], w2s = pb.pos[3 * v + 1], w3s = pb.pos[3 * v + 2];
       const int r1s = __float_as_int(ex.y), r2s = __float_as_int(ex.z), r3s = __float_as_int(ex.w);
       // every front-runner of the query in one batch of independent (predicated) loads; a slot is read only where the
@@ -192,7 +190,7 @@ __device__ void association_pass(CtaMem& cta, Smem* slots, const BatchView& bv, 
       if (ok1 && (ok2 || ccr0 < 0)) { pb.qw[v] = make_int4(-2, (c2 == kCertSwap ? 1 : 0) | (c3 == kCertSwap ? 2 : 0), 0, 0); continue; }
       if (ok1) { az_polar(s, qa); pb.qa[v] = qa; pb.qw[v] = make_int4(-3, 0, 0, 0); continue; }
     }
-    const int w1 = az_prepare_nn(ixq, s, nearf, seeded ? pb.pos[3 * v] : -1, (int)pb.qpt[v].w, qa);
+    const int w1 = az_prepare_nn(ixq, s, sm.nearf, seeded ? pb.pos[3 * v] : -1, (int)pb.qpt[v].w, qa);
     pb.qa[v] = qa;
     pb.qw[v] = make_int4(w1, 0, 0, 0);
     // (list order does not matter: every query's result goes to its own slot.)  Two lists share pb.wl: searches run by a
@@ -215,18 +213,18 @@ __device__ void association_pass(CtaMem& cta, Smem* slots, const BatchView& bv, 
       atomicAdd((unsigned long long*)&bv.timers[10], (unsigned long long)cta.wl_n[0]);
       atomicAdd((unsigned long long*)&bv.timers[12], (unsigned long long)cta.dbg[0]);
     }
-    const float gate = sqrtf(nearf);
     // result of a closest-point search -> the query's state (one thread)
     auto nn_finish = [&](int v, const AzIndex& ix, const float4 s, const Top3& top, int w1, float Bout) {
       const unsigned long long k1 = top.k1;
       const int p1 = top.p1;
       const float d1 = __uint_as_float((unsigned)(k1 >> 32));
-      const bool acc1 = k1 != kKeyMax && p1 >= 0 && (double)d1 < kp.nearest_sq;
+      const Smem& sq = slots[slot_of(v, Q)];
+      const bool acc1 = k1 != kKeyMax && p1 >= 0 && (double)d1 < sq.nearest_sq;
       // (diagnostics read what they need from shared memory, so that nothing extra stays live across the scan)
-      if (bv.timers && !slots[slot_of(v, Q)].first_pass && pb.pos[3 * v] >= 0 && acc1 && (p1 == pb.pos[3 * v] || p1 == __float_as_int(pb.qext[v].y)))
+      if (bv.timers && !sq.first_pass && pb.pos[3 * v] >= 0 && acc1 && (p1 == pb.pos[3 * v] || p1 == __float_as_int(pb.qext[v].y)))
         atomicAdd((unsigned long long*)&bv.timers[kCertSlots + 6], 1ull);  // a failed certificate whose stored front-runners held the answer
       // accepted: what everything but the two front-runners exceeded; else the slack of "nothing within the gate"
-      const float bound1 = w1 < 0 ? -1.f : acc1 ? cert_bound(top.d3, Bout) : rejected_slack((unsigned)(k1 >> 32), Bout, gate);
+      const float bound1 = w1 < 0 ? -1.f : acc1 ? cert_bound(top.d3, Bout) : rejected_slack((unsigned)(k1 >> 32), Bout, sq.gate);
       pb.qref[v] = make_float4(s.x, s.y, s.z, bound1);
       pb.qext[v].y = __int_as_float(acc1 ? top.p2 : -1);
       pb.pos[3 * v] = acc1 ? p1 : -1;
@@ -273,7 +271,7 @@ __device__ void association_pass(CtaMem& cta, Smem* slots, const BatchView& bv, 
         if (wp >= 0) {  // wide window (no usable previous answer): probe first, then search inside the implied window
           const Top3 pr = az_scan_nn(ix, s, wp, qa.y, sqrtf(widen(kProbeSq)));  // (a probe needs no exactness: anything it finds is an upper bound)
           if (pr.p1 >= 0) {
-            w1 = az_nn_window(ix, az_seed_bound(ix, s, pr.p1, nearf), qa);
+            w1 = az_nn_window(ix, az_seed_bound(ix, s, pr.p1, sm.nearf), qa);
             if (lane == 0) pb.qa[v] = qa;
           }
         }
@@ -291,7 +289,7 @@ __device__ void association_pass(CtaMem& cta, Smem* slots, const BatchView& bv, 
     for (int v = threadIdx.x; v < NQ; v += kThreads) {  // P3
       const int sl = slot_of(v, Q), i = v - sl * Q;
       const Smem& sm = slots[sl];
-      if (!sm.run || !sm.az_ok || i >= sm.ns + sm.nc || (sm.iter % kp.icp_freq) != 0) continue;
+      if (!sm.run || !sm.az_ok || i >= sm.ns + sm.nc || !sm.search) continue;
       const int2 lq = *reinterpret_cast<const int2*>(&pb.qw[v]);  // (level, walk swaps)
       const int lvl = lq.x;
       const bool surf = i < sm.ns;
@@ -329,8 +327,8 @@ __device__ void association_pass(CtaMem& cta, Smem* slots, const BatchView& bv, 
       const int c = ccr & 0x00ffffff, cr = (int)((unsigned)ccr >> 24);
       const AzIndex ix = az_index_of(sm, bv, surf);
       const int p1 = pb.pos[3 * v];
-      if (surf) az_prepare_walk<true>(ix, pb.sel[v], pb.qa[v], p1, c, cr, sd2, sd3, min(sm.ns, sm.Ts), nearf, w2, w3, B2, B3);
-      else az_prepare_walk<false>(ix, pb.sel[v], pb.qa[v], p1, c, cr, sd2, sd3, min(sm.nc, sm.Tc), nearf, w2, w3, B2, B3);
+      if (surf) az_prepare_walk<true>(ix, pb.sel[v], pb.qa[v], p1, c, cr, sd2, sd3, min(sm.ns, sm.Ts), sm.nearf, w2, w3, B2, B3);
+      else az_prepare_walk<false>(ix, pb.sel[v], pb.qa[v], p1, c, cr, sd2, sd3, min(sm.nc, sm.Tc), sm.nearf, w2, w3, B2, B3);
       pb.qw[v] = make_int4(lvl == -3 ? 2 : 1, w2, w3, ccr);  // (.x = 2: the walks' certificate failed; diagnostics only)
       reinterpret_cast<float2*>(pb.key)[v] = make_float2(B2, B3);
       if (sm.first_pass && (w2 & 0xffff) <= kThreadWalkBins && (w3 & 0xffff) <= kThreadWalkBins) pb.wl[NQ - 1 - atomicAdd(&cta.wl_tn[1], 1)] = v;
@@ -373,8 +371,8 @@ __device__ void association_pass(CtaMem& cta, Smem* slots, const BatchView& bv, 
       const float2 B = reinterpret_cast<const float2*>(pb.key)[v];
       const float4 s = pb.sel[v];
       const AzIndex ix = az_index_of(sm, bv, surf);
-      const WalkOut wo = surf ? az_scan_walk_group<true, G>(ix, s, w.w, w.y, w.z, min(sm.ns, sm.Ts), nearf, B.x, B.y, sub, gmask)
-                              : az_scan_walk_group<false, G>(ix, s, w.w, w.y, w.z, min(sm.nc, sm.Tc), nearf, B.x, B.y, sub, gmask);
+      const WalkOut wo = surf ? az_scan_walk_group<true, G>(ix, s, w.w, w.y, w.z, min(sm.ns, sm.Ts), sm.nearf, B.x, B.y, sub, gmask)
+                              : az_scan_walk_group<false, G>(ix, s, w.w, w.y, w.z, min(sm.nc, sm.Tc), sm.nearf, B.x, B.y, sub, gmask);
       if (sub == 0) walk_finish(v, sm, i, surf, s, w.w, wo);
     }
     for (;;) {  // P4: same work-list scheme
@@ -391,8 +389,8 @@ __device__ void association_pass(CtaMem& cta, Smem* slots, const BatchView& bv, 
       const int w2 = w.y, w3 = w.z;
       const float4 s = pb.sel[v];
       const AzIndex ix = az_index_of(sm, bv, surf);
-      const WalkOut wo = surf ? az_scan_walk<true>(ix, s, w.w, w2, w3, min(sm.ns, sm.Ts), nearf, B.x, B.y)
-                              : az_scan_walk<false>(ix, s, w.w, w2, w3, min(sm.nc, sm.Tc), nearf, B.x, B.y);
+      const WalkOut wo = surf ? az_scan_walk<true>(ix, s, w.w, w2, w3, min(sm.ns, sm.Ts), sm.nearf, B.x, B.y)
+                              : az_scan_walk<false>(ix, s, w.w, w2, w3, min(sm.nc, sm.Tc), sm.nearf, B.x, B.y);
       if (lane == 0) walk_finish(v, sm, i, surf, s, w.w, wo);
     }
   }
@@ -400,7 +398,7 @@ __device__ void association_pass(CtaMem& cta, Smem* slots, const BatchView& bv, 
     // ---- legacy: brute-force exact 1-NN + literal sequential walks, unit by unit ----------------------------------
     for (int sl = 0; sl < bv.nslots; ++sl) {
       const Smem& sm = slots[sl];
-      if (!sm.run || sm.az_ok || (sm.iter % kp.icp_freq) != 0) continue;
+      if (!sm.run || sm.az_ok || !sm.search) continue;
       const bool sep = nn_separate(bv, sm.scan);
       const float4* __restrict__ nnS = sep ? bv.nn_s + bv.nn_s_off[sm.scan] : bv.ts + sm.ts0;
       const float4* __restrict__ nnC = sep ? bv.nn_c + bv.nn_c_off[sm.scan] : bv.tc + sm.tc0;
@@ -412,7 +410,7 @@ __device__ void association_pass(CtaMem& cta, Smem* slots, const BatchView& bv, 
     __syncthreads();
     for (int sl = 0; sl < bv.nslots; ++sl) {
       const Smem& sm = slots[sl];
-      if (!sm.run || sm.az_ok || (sm.iter % kp.icp_freq) != 0) continue;
+      if (!sm.run || sm.az_ok || !sm.search) continue;
       const float4* __restrict__ tgtS = bv.ts + sm.ts0;
       const float4* __restrict__ tgtC = bv.tc + sm.tc0;
       const int fwdS = min(sm.ns, sm.Ts), fwdC = min(sm.nc, sm.Tc);
@@ -422,13 +420,13 @@ __device__ void association_pass(CtaMem& cta, Smem* slots, const BatchView& bv, 
         const unsigned long long k1 = pb.key[v];
         const float d1 = __uint_as_float((unsigned)(k1 >> 32));
         const int c = (int)(unsigned)(k1 & 0xffffffffu);
-        const bool found = (k1 != kKeyMax) && ((double)d1 < kp.nearest_sq) && c < (surf ? sm.Ts : sm.Tc);
+        const bool found = (k1 != kKeyMax) && ((double)d1 < sm.nearest_sq) && c < (surf ? sm.Ts : sm.Tc);
         int i1 = -1, i2 = -1, i3 = -1;
         if (found) {
           i1 = c;
           const float4 s = pb.sel[v];
-          if (surf) walk_seq<true>(s, c, tgtS, sm.Ts, fwdS, nearf, i2, i3);
-          else walk_seq<false>(s, c, tgtC, sm.Tc, fwdC, nearf, i2, i3);
+          if (surf) walk_seq<true>(s, c, tgtS, sm.Ts, fwdS, sm.nearf, i2, i3);
+          else walk_seq<false>(s, c, tgtC, sm.Tc, fwdC, sm.nearf, i2, i3);
         }
         pb.pos[3 * v] = i1; pb.pos[3 * v + 1] = i2; pb.pos[3 * v + 2] = i3;
         if (surf) { int* o = bv.ind_s + 3 * (size_t)(sm.qs0 + i); o[0] = i1; o[1] = i2; o[2] = i3; }
@@ -457,9 +455,8 @@ __device__ void association_pass(CtaMem& cta, Smem* slots, const BatchView& bv, 
     const int v = v0 + lane, i = i0 + lane;
     const bool valid = i < ntot;
     const bool surf = i < sm.ns;
-    const bool search = (sm.iter % kp.icp_freq) == 0;
-    const bool weighted = sm.iter >= kp.icp_freq;
-    const bool by_slot = search ? (sm.az_ok != 0) : (sm.pos_valid && sm.pos_is_slot);
+    const bool weighted = sm.weighted != 0;
+    const bool by_slot = sm.search ? (sm.az_ok != 0) : (sm.pos_valid && sm.pos_is_slot);
     float4 coeff = make_float4(0.f, 0.f, 0.f, 0.f);
     float4 s = make_float4(0.f, 0.f, 0.f, 0.f);
     bool ok = false;
@@ -481,7 +478,7 @@ __device__ void association_pass(CtaMem& cta, Smem* slots, const BatchView& bv, 
     double g[6] = {0.0, 0.0, 0.0, 0.0, 0.0, 0.0}, r = 0.0;
     if (ok) {
       if (MODE == MODE_ICP_REDUCE) jacobian_row_icp(pb.qpt[v], coeff, sm.phi, sm.period, g, r);
-      else jacobian_row(pb.qpt[v], coeff, sm.R, kp.lidar_scale, g, r);
+      else jacobian_row(pb.qpt[v], coeff, sm.R, sm.lidar_scale, g, r);
     }
     const int vw = sl * pb.nvw + (i0 >> 5);
     warp_fold_mma(g, r, fold_stage, pb.wacc + vw * kNAcc);

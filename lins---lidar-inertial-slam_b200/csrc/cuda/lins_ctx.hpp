@@ -23,7 +23,7 @@
 #include "../../../include/lins_gpu.h"
 #include "../host/host_pool.hpp"
 
-namespace lins_dev { struct IcpState; struct BatchView; }     // lins_kernels.cuh
+namespace lins_dev { struct IcpState; struct BatchView; struct UnitTuning; }  // lins_kernels.cuh
 namespace lins_map { struct PassConsts; struct MapLoopState; struct MapSlot; }  // lins_map.cuh
 
 namespace lins_capi {
@@ -165,6 +165,15 @@ struct SeqState {
   Buf<double, kPinned> h_period;
   std::vector<lins_slot_config> cfg;
   std::vector<unsigned char> configured, fresh;
+  // per-slot estimator tuning (lins_gpu_seq_tune): on the host each slot's tuning, whether it is tuned and its
+  // alignIMUtoVehicle rotation (n x 9, row-major, built with the host's libm when the slot is tuned); per step the device
+  // table of every slot's tuning (the context's lins_params for an untuned slot) and, while a slot is tuned, the rotations
+  // (n x 10: R, then 1 = rotate the slot's IMU values)
+  std::vector<lins_slot_tuning> tune;
+  std::vector<unsigned char> tuned;
+  std::vector<double> align_R;
+  Buf<lins_dev::UnitTuning> unit_tune; Buf<lins_dev::UnitTuning, kPinned> h_unit_tune;
+  Buf<double> align; Buf<double, kPinned> h_align;
   std::vector<int32_t> fusion;
   Buf<double> pre, scan_imu;
   Buf<double, kPinned> h_scan_imu;
@@ -565,12 +574,13 @@ inline int upload2(lins_ctx* ctx, Buf<float4>& dst_a, const lins_point* a, int n
 // corner_less_sharp) and upload them with their offsets into r (qs, qc, ts, tc); sets r.n, the totals and r.max_q
 int upload_clouds(lins_ctx* ctx, Resident& r, int n, const lins_point* const pts[4], const int32_t* const offs[4], int point_format);
 // lins_gpu.cu: the fused kernel's IESKF launch over bv (with r's scratch), its query tile, the estimateTransform loop of
-// bv's device-resident units (pose: 20 doubles, icp: one IcpState per unit, set by the caller), and the CSR transformToEnd
+// bv's device-resident units (pose: 20 doubles, icp: one IcpState per unit, set by the caller; n_iter launches, the largest
+// NUM_ITER of the units), and the CSR transformToEnd
 // of the units with run[u] != 0 (lin: 20 doubles per unit, period: one SCAN_PERIOD per unit, both on the device)
 int fused_ieskf_launch(lins_ctx* ctx, Resident& r, const lins_dev::BatchView& bv);
 int fused_qtile(int max_q);
 size_t icp_state_bytes();
-int icp_loop(lins_ctx* ctx, Resident& r, lins_dev::BatchView bv, double* pose, lins_dev::IcpState* icp);
+int icp_loop(lins_ctx* ctx, Resident& r, lins_dev::BatchView bv, double* pose, lins_dev::IcpState* icp, int n_iter);
 int transform_to_end_csr(lins_ctx* ctx, float4* pts, const int* off, int n_units, const double* lin, const unsigned char* run,
                          const double* period);
 // device-resident input of one feature extraction: n scans of line_num rings; scan i's points are pts[off[i] ..

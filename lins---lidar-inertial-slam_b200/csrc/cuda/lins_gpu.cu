@@ -40,11 +40,22 @@ __device__ void unit_prologue(CtaMem& cta, Smem& sm, const BatchView& bv, const 
   if (tid == 32) {
     sm.flags[0] = sm.flags[1] = sm.flags[2] = sm.flags[3] = 0; sm.residualNorm = 1e6;
     sm.period = bv.unit_period ? bv.unit_period[scan] : kp.scan_period;
+    if (bv.unit_tune) {
+      const UnitTuning t = bv.unit_tune[scan];
+      sm.num_iter = t.num_iter; sm.icp_freq = t.icp_freq; sm.nearest_sq = t.nearest_sq; sm.sig2 = t.lidar_std * t.lidar_std;
+      sm.lidar_scale = t.lidar_scale;
+    } else {
+      sm.num_iter = kp.num_iter; sm.icp_freq = kp.icp_freq; sm.nearest_sq = kp.nearest_sq; sm.sig2 = kp.lidar_std * kp.lidar_std;
+      sm.lidar_scale = kp.lidar_scale;
+    }
+    sm.nearf = (float)sm.nearest_sq;
+    sm.gate = sqrtf(sm.nearf);
     sm.cnt[0] = sm.cnt[1] = 0;
     sm.iter = MODE == MODE_IESKF ? 0 : kp.iter0;
+    sm.search = (sm.iter % sm.icp_freq) == 0; sm.weighted = sm.iter >= sm.icp_freq;
     sm.fresh = 0; sm.finished = 0; sm.first_pass = 1; sm.pos_valid = 0; sm.pos_is_slot = 0;
     sm.run = 1;
-    if (MODE == MODE_IESKF && kp.num_iter <= 0) { sm.run = 0; sm.finished = 1; cta.any_finished = 1; }
+    if (MODE == MODE_IESKF && sm.num_iter <= 0) { sm.run = 0; sm.finished = 1; cta.any_finished = 1; }
     sm.qs0 = bv.qs_off[scan]; sm.ns = bv.qs_off[scan + 1] - sm.qs0;
     sm.qc0 = bv.qc_off[scan]; sm.nc = bv.qc_off[scan + 1] - sm.qc0;
     sm.ts0 = bv.ts_off[scan]; sm.Ts = bv.ts_off[scan + 1] - sm.ts0;
@@ -93,7 +104,7 @@ __device__ void unit_prologue(CtaMem& cta, Smem& sm, const BatchView& bv, const 
 // The serial tail of one unit's iteration (StateEstimator.hpp:535-580), run by ONE warp: finish the reduction, 6x6 gain
 // system, update, convergence logic, and the constants of the unit's NEXT iteration.  The tails of the resident units
 // run side by side on different warps.
-__device__ void unit_tail(CtaMem& cta, Smem& sm, const BatchView& bv, const KParams& kp, const PassBuffers& pb, int slot, double sig2) {
+__device__ void unit_tail(CtaMem& cta, Smem& sm, const BatchView& bv, const KParams& kp, const PassBuffers& pb, int slot) {
   const int lane = threadIdx.x & 31;
   const int iter = sm.iter;
   lins_report* rep = bv.reports ? bv.reports + sm.scan : nullptr;
@@ -106,7 +117,7 @@ __device__ void unit_tail(CtaMem& cta, Smem& sm, const BatchView& bv, const KPar
     for (int c = 0; c < 6; ++c) y += sm.A6[lane * 6 + c] * sm.dvec[col6(c)];
     sm.X6[lane] = y;
   }
-  form_M6(sm, sig2, lane, 32);
+  form_M6(sm, sm.sig2, lane, 32);
   __syncwarp();
   const bool ok = warp_lu_cols<6>(sm.M6, sm.X6, 1);  // z = M^-1 (b6 + A6 d_c)
   __syncwarp();
@@ -141,12 +152,12 @@ __device__ void unit_tail(CtaMem& cta, Smem& sm, const BatchView& bv, const KPar
       if (un <= 1e-2 && !kp.force_all_iters) { sm.flags[0] = 1; sm.flags[3] = 1; }  // :576-578
       sm.residualNorm = rnorm;
     }
-    const bool search = (iter % kp.icp_freq) == 0;
-    if (search) sm.pos_is_slot = sm.az_ok; else if (!sm.pos_valid) sm.pos_is_slot = 0;
+    if (sm.search) sm.pos_is_slot = sm.az_ok; else if (!sm.pos_valid) sm.pos_is_slot = 0;
     sm.pos_valid = 1;
     sm.first_pass = 0;
     sm.iter = iter + 1;
-    if (sm.flags[3] || iter + 1 >= kp.num_iter) { sm.finished = 1; sm.run = 0; cta.any_finished = 1; }
+    sm.search = ((iter + 1) % sm.icp_freq) == 0; sm.weighted = iter + 1 >= sm.icp_freq;
+    if (sm.flags[3] || iter + 1 >= sm.num_iter) { sm.finished = 1; sm.run = 0; cta.any_finished = 1; }
   }
   __syncwarp();
   if (slot == 0) LINS_TICK(23);
@@ -155,10 +166,11 @@ __device__ void unit_tail(CtaMem& cta, Smem& sm, const BatchView& bv, const KPar
 }
 
 // exit of one finished unit: covariance + outputs (StateEstimator.hpp:585-599).  Block-wide.
-__device__ void unit_exit(CtaMem& cta, Smem& sm, const BatchView& bv, double sig2) {
+__device__ void unit_exit(CtaMem& cta, Smem& sm, const BatchView& bv) {
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int scan = sm.scan, iters = sm.iter;
   const bool diverged = sm.flags[1] != 0;
+  const double sig2 = sm.sig2;
   auto& ex = cta.u.ex;
   if (!diverged && iters > 0) {
     // Joseph form with the LAST iteration's K, H, R (:595-596), all through the 6x6 system:
@@ -233,7 +245,6 @@ __global__ void __launch_bounds__(kThreads, kMinCtas) lins_ieskf_kernel(const __
   CtaMem& cta = *reinterpret_cast<CtaMem*>(smem_raw);
   Smem* slots = reinterpret_cast<Smem*>(smem_raw + lay.slots);
   const int tid = threadIdx.x, warp = tid >> 5;
-  const double sig2 = kp.lidar_std * kp.lidar_std;
 
   if (tid == 0) {
     mbar_init(&cta.mbar, 1);
@@ -300,7 +311,7 @@ __global__ void __launch_bounds__(kThreads, kMinCtas) lins_ieskf_kernel(const __
     // ---- one pass of every resident unit (StateEstimator.hpp:475-581) -----------------------------------------------
     association_pass<MODE>(cta, slots, bv, kp, pb);
     if (MODE == MODE_IESKF) {
-      if (warp < S && slots[warp].run) unit_tail(cta, slots[warp], bv, kp, pb, warp, sig2);
+      if (warp < S && slots[warp].run) unit_tail(cta, slots[warp], bv, kp, pb, warp);
     } else {
       if (warp < S && slots[warp].run) {  // single-pass modes: the 28 sums + counts are the result
         Smem& sm = slots[warp];
@@ -321,7 +332,7 @@ __global__ void __launch_bounds__(kThreads, kMinCtas) lins_ieskf_kernel(const __
     if (MODE == MODE_IESKF && cta.any_finished) {
       for (int s = 0; s < S; ++s) {
         if (!slots[s].finished) continue;  // (uniform: shared flag)
-        unit_exit(cta, slots[s], bv, sig2);
+        unit_exit(cta, slots[s], bv);
         if (tid == 0) { slots[s].scan = -1; slots[s].finished = 0; slots[s].run = 0; }
       }
       if (tid == 0) cta.any_finished = 0;
@@ -563,14 +574,15 @@ size_t icp_state_bytes() { return sizeof(IcpState); }
 // per unit, the linearisation point) are on the device: every iteration is one reduction launch over all units
 // (MODE_ICP_REDUCE) + one step launch with a block per unit that updates the unit's pose.  icp holds one IcpState per unit,
 // set by the caller: zero = run, done = 1 = skip.  Once a unit's step sets `done`, the remaining queued launches pass it
-// over.  No synchronisation.
-int icp_loop(lins_ctx* ctx, Resident& r, BatchView bv, double* pose, IcpState* icp) {
+// over.  n_iter launches: the largest NUM_ITER of the units (each unit's is bv.unit_tune's, else the context's, and its
+// step sets done at it).  No synchronisation.
+int icp_loop(lins_ctx* ctx, Resident& r, BatchView bv, double* pose, IcpState* icp, int n_iter) {
   bv.state_in = pose;
   bv.icp_done = &icp->done;
-  for (int iter = 0; iter < ctx->prm.num_iter; ++iter) {
+  for (int iter = 0; iter < n_iter; ++iter) {
     const int rc = launch(ctx, r, bv, make_kparams(ctx->prm, MODE_ICP_REDUCE, iter));
     if (rc != LINS_OK) return rc;
-    lins_icp_step_kernel<<<bv.n_scans, 32, 0, ctx->stream>>>(bv.accum, pose, icp, iter);
+    lins_icp_step_kernel<<<bv.n_scans, 32, 0, ctx->stream>>>(bv.accum, pose, icp, iter, bv.unit_tune, ctx->prm.num_iter);
     CK(cudaGetLastError());
     ctx->launches += 1;
   }
@@ -825,7 +837,7 @@ int lins_gpu_estimate_transform(lins_ctx* ctx, const lins_point* surf_flat, int 
   Resident& r = ctx->single;
   CK(r.icp.reserve(1)); CK(r.h_icp.reserve(1)); CK(r.h_state_out.reserve(20));
   CK(cudaMemsetAsync(r.icp.p, 0, sizeof(IcpState), ctx->stream));
-  rc = icp_loop(ctx, r, single_view(ctx, false), r.state_in.p, r.icp.p);
+  rc = icp_loop(ctx, r, single_view(ctx, false), r.state_in.p, r.icp.p, ctx->prm.num_iter);
   if (rc != LINS_OK) return rc;
   CK(cudaMemcpyAsync(r.h_state_out.p, r.state_in.p, sizeof(double) * 20, cudaMemcpyDeviceToHost, ctx->stream));
   CK(cudaMemcpyAsync(r.h_icp.p, r.icp.p, sizeof(IcpState), cudaMemcpyDeviceToHost, ctx->stream));

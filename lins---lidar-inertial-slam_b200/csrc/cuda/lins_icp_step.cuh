@@ -119,14 +119,20 @@ __device__ inline bool icp_inverse6(double A[6][6], double inv[6][6]) {
 
 // One 32-thread block per unit u = blockIdx.x, thread 0 working.  accum + 32 u: the 28 sums + counts of one MODE_ICP_REDUCE
 // pass (entries 0..20 = upper triangle of J^T J, 21..26 = J^T b, 28 / 29 = matched surfs / corners); state + 20 u: the
-// 20-double pose block the next pass linearises at (t at 0..2, q xyzw at 6..9); st + u: the unit's loop state.
-__global__ void lins_icp_step_kernel(const double* __restrict__ accum, double* __restrict__ state, IcpState* __restrict__ st, int iter) {
+// 20-double pose block the next pass linearises at (t at 0..2, q xyzw at 6..9); st + u: the unit's loop state.  The loop
+// ends at the unit's own NUM_ITER, tune[u].num_iter (null tune: num_iter): the step of its last iteration sets done, and a
+// unit whose cap the launch is past (NUM_ITER 0, where its caller did not start it done) is done without an iteration.
+__global__ void lins_icp_step_kernel(const double* __restrict__ accum, double* __restrict__ state, IcpState* __restrict__ st, int iter,
+                                     const UnitTuning* __restrict__ tune, int num_iter) {
   const int u = blockIdx.x;
   accum += (size_t)u * 32;
   state += (size_t)u * 20;
   st += u;
   if (threadIdx.x != 0 || st->done) return;
+  const int cap = tune ? tune[u].num_iter : num_iter;
+  if (iter >= cap) { st->done = 1; return; }
   st->iters = iter + 1;
+  if (iter + 1 >= cap) st->done = 1;  // (the loop's last iteration: converged or not, nothing reads the unit again)
   const double* a = accum;
   if (a[28] < 10) return;  // "Insufficient matched surfs..." (:1175-1178)
   if (a[29] < 5) return;   // "Insufficient matched corners..." (:1181-1184)

@@ -38,6 +38,13 @@ constexpr unsigned long long kKeyMax = 0xFFFFFFFFFFFFFFFFull;
 
 enum KernelMode { MODE_IESKF = 0, MODE_ASSOC = 1, MODE_ICP_REDUCE = 2, MODE_JACOBIAN = 3 };
 
+// one unit's estimator tuning (lins_slot_tuning without the IMU misalignment): NUM_ITER, ICP_FREQ (>= 1),
+// NEAREST_FEATURE_SEARCH_SQ_DIST, LIDAR_STD, LIDAR_SCALE
+struct UnitTuning {
+  int num_iter, icp_freq;
+  double nearest_sq, lidar_std, lidar_scale;
+};
+
 struct BatchView {
   int n_scans;
   const float4* qs; const int* qs_off;   // surf queries   (surfPointsFlat_)
@@ -73,6 +80,8 @@ struct BatchView {
   size_t qscratch_stride;                // memory (null: they live in shared memory)
   const double* unit_period;             // per unit: the SCAN_PERIOD of its de-skew (sequence mode's per-slot rigs); null =
                                          // every unit's is KParams::scan_period
+  const UnitTuning* unit_tune;           // per unit: its estimator tuning (sequence mode's per-slot tuning); null = every
+                                         // unit's is KParams'
 };
 
 // loop state of one unit's estimateTransform (lins_icp_step.cuh)
@@ -131,6 +140,16 @@ struct alignas(16) Smem {
   double upd[18];
   double residualNorm;
   double period;        // SCAN_PERIOD of the unit's de-skew (transformToStart, the ICP fallback's rows)
+  // the unit's tuning (BatchView::unit_tune or KParams): a pass mixes the queries of every resident unit, so each query
+  // reads its own unit's gate, ICP_FREQ and LIDAR_SCALE here
+  double nearest_sq;    // the 1-NN gate, compared in f64 ...
+  double lidar_scale;
+  double sig2;          // LIDAR_STD^2 of the gain
+  float nearf;          // ... and in f32 by the windows, walks and certificates
+  float gate;           // sqrtf(nearf)
+  int num_iter, icp_freq;
+  int search, weighted; // of the pass at `iter`: iter % ICP_FREQ == 0 (a closest-point search), iter >= ICP_FREQ (the
+                        // residual's weight); set with iter, so a pass reads two flags instead of dividing per query
   int flags[4];         // 0 converged 1 diverged 2 has_nan 3 stop
   int cnt[2];
   // bookkeeping
@@ -157,7 +176,7 @@ struct alignas(16) Smem {
 struct CtaMem {
   union {
     // counting-sort counters / cursors while a unit's index is built, 16 bits each (lins_assoc_az.cuh: cnt16_add1): 8 kB
-    // instead of 16 kB brings the CTA (three slots of 320 queries) from 204 928 B to 196 736 B of shared memory, under the
+    // instead of 16 kB brings the CTA (three slots of 320 queries) from 205 072 B to 196 880 B of shared memory, under the
     // 196 KB carve-out, so the SM keeps about 60 KB of L1 instead of 28 KB for the sorted target copies the searches and
     // the residuals read
     unsigned build_tab[kAzTabS / 2 + 1];

@@ -117,16 +117,18 @@ __global__ void lins_seq_post_kernel(int n, const unsigned char* __restrict__ st
 }
 
 // One thread per second scan: the start pose of its estimateTransform (processSecondScan's pl / ql) and a fresh loop state;
-// every other sequence's loop state reads done, so the batched loop passes it over.
+// every other sequence's loop state reads done, so the batched loop passes it over, and so does a second scan whose
+// NUM_ITER (tune[s]) is 0: its loop runs no iteration.
 __global__ void lins_seq_icp_start_kernel(int n, const unsigned char* __restrict__ status, const double* __restrict__ pre,
-                                          double* __restrict__ icp_pose, lins_dev::IcpState* __restrict__ icp) {
+                                          double* __restrict__ icp_pose, lins_dev::IcpState* __restrict__ icp,
+                                          const lins_dev::UnitTuning* __restrict__ tune) {
   const int s = blockIdx.x * blockDim.x + threadIdx.x;
   if (s >= n) return;
   const bool second = status[s] == LINS_SEQ_SECOND;
   lins_dev::IcpState& st = icp[s];
   for (int i = 0; i < 36; ++i) st.matP[i] = 0.0;
   st.iters = 0; st.converged = 0; st.pad = 0;
-  st.done = second ? 0 : 1;
+  st.done = second && tune[s].num_iter > 0 ? 0 : 1;
   if (second) lins_seq::second_scan_start(pre + (size_t)s * 20, icp_pose + (size_t)s * 20);
 }
 
@@ -145,6 +147,23 @@ __global__ void lins_seq_init_kernel(int n, const unsigned char* __restrict__ st
     lins_seq::first_scan(filt + o, cov + (size_t)s * 324, lin + o, pre + o, il, imu + (size_t)s * 6, k[s]);
   else if (status[s] == LINS_SEQ_SECOND)
     lins_seq::second_scan(glob + o, filt + o, cov + (size_t)s * 324, lin + o, il, pre + o, icp_pose + o, imu + (size_t)s * 6, k[s]);
+}
+
+// One warp per sequence s whose align[10 s + 9] != 0 (a tuned slot): alignIMUtoVehicle (Estimator.cpp:286-292) in place on
+// its IMU values, acc_out = R^T acc and gyr_out = R^T gyr with R = align[10 s ..] (row-major, rpy2R(0, 0, yaw)): its rows
+// imu[imu_off[s] .. imu_off[s + 1]) (dt, acc, gyr; dt stays) and, when scan_imu is set, its processPCL sample
+// scan_imu[6 s ..] (acc, gyr).  out_j = (R_0j v_0 + R_1j v_1) + R_2j v_2, unfused (-fmad=false).
+__global__ void __launch_bounds__(32) lins_seq_align_kernel(double* __restrict__ imu, const int* __restrict__ imu_off,
+                                                            double* __restrict__ scan_imu, const double* __restrict__ align) {
+  const int s = blockIdx.x, lane = threadIdx.x;
+  const double* R = align + (size_t)s * 10;
+  if (R[9] == 0.0) return;
+  auto rot = [R](double* v) {
+    const double x = v[0], y = v[1], z = v[2];
+    for (int j = 0; j < 3; ++j) v[j] = (R[j] * x + R[3 + j] * y) + R[6 + j] * z;
+  };
+  for (int m = imu_off[s] + lane; m < imu_off[s + 1]; m += 32) { rot(imu + (size_t)m * 7 + 1); rot(imu + (size_t)m * 7 + 4); }
+  if (scan_imu && lane == 0) { rot(scan_imu + (size_t)s * 6); rot(scan_imu + (size_t)s * 6 + 3); }
 }
 
 // One thread per sequence with mask[s] != 0 (every sequence for a null mask): the state of a new StateEstimator
@@ -217,11 +236,45 @@ double slot_period(const lins_ctx* ctx, int s) {
   return q.configured[s] ? q.cfg[s].scan_period : ctx->prm.scan_period;
 }
 
-// the host side of a run's slot configuration: every slot unconfigured and fresh
+// alignIMUtoVehicle's R = rpy2R((0, 0, deg2rad(angle))) = Rz Ry Rx (math_utils.h:164-182), row-major, with the host's libm
+void misalign_R(double angle, double* R) {
+  const double y = angle * M_PI / 180.0, p = 0.0, r = 0.0;  // math_utils::deg2rad of (0, 0, angle)
+  const double Rz[9] = {std::cos(y), -std::sin(y), 0, std::sin(y), std::cos(y), 0, 0, 0, 1};
+  const double Ry[9] = {std::cos(p), 0., std::sin(p), 0., 1., 0., -std::sin(p), 0., std::cos(p)};
+  const double Rx[9] = {1., 0., 0., 0., std::cos(r), -std::sin(r), 0., std::sin(r), std::cos(r)};
+  auto mul = [](const double* A, const double* B, double* C) {
+    for (int i = 0; i < 3; ++i)
+      for (int j = 0; j < 3; ++j) C[3 * i + j] = (A[3 * i] * B[j] + A[3 * i + 1] * B[3 + j]) + A[3 * i + 2] * B[6 + j];
+  };
+  double T[9];
+  mul(Rz, Ry, T);
+  mul(T, Rx, R);
+}
+
+// the host side of a run's slot configuration and tuning: every slot unconfigured, untuned and fresh
 void reset_slot_configs(SeqState& q, int n) {
   q.cfg.assign(n, lins_slot_config());
   q.configured.assign(n, 0);
   q.fresh.assign(n, 1);
+  q.tune.assign(n, lins_slot_tuning());
+  q.tuned.assign(n, 0);
+  q.align_R.assign(9 * (size_t)n, 0.0);
+}
+
+// the tuning slot s reads: its own, else the context's lins_params
+lins_dev::UnitTuning slot_tuning(const lins_ctx* ctx, int s) {
+  const SeqState& q = ctx->seq;
+  lins_dev::UnitTuning t;
+  if (q.tuned[s]) {
+    const lins_slot_tuning& u = q.tune[s];
+    t.num_iter = u.num_iter; t.icp_freq = u.icp_freq; t.nearest_sq = u.nearest_feature_search_sq_dist;
+    t.lidar_std = u.lidar_std; t.lidar_scale = u.lidar_scale;
+  } else {
+    const lins_params& p = ctx->prm;
+    t.num_iter = p.num_iter; t.icp_freq = p.icp_freq < 1 ? 1 : p.icp_freq; t.nearest_sq = p.nearest_feature_search_sq_dist;
+    t.lidar_std = p.lidar_std; t.lidar_scale = p.lidar_scale;
+  }
+  return t;
 }
 
 int launch_fresh(lins_ctx* ctx, SeqState& q, int n, const unsigned char* mask_dev) {
@@ -404,6 +457,10 @@ int seq_step_phases(lins_ctx* ctx, const lins_seq_step_desc* d, const int32_t* c
   CK(q.imu.reserve(7 * n_imu + 1)); CK(q.imu_off.reserve(N1)); CK(q.h_imu.reserve(7 * n_imu + 1)); CK(q.h_imu_off.reserve(N1));
   CK(q.status_d.reserve(3 * (size_t)n)); CK(q.h_status.reserve(3 * (size_t)n));
   CK(q.period.reserve(n)); CK(q.h_period.reserve(n));
+  CK(q.unit_tune.reserve(n)); CK(q.h_unit_tune.reserve(n));
+  const bool any_tuned = std::find(q.tuned.begin(), q.tuned.end(), 1) != q.tuned.end();
+  const bool align = any_tuned && (n_imu || n_init);  // (a run without a tuned slot launches what it launched before)
+  if (align) { CK(q.align.reserve(10 * (size_t)n)); CK(q.h_align.reserve(10 * (size_t)n)); }
   const int n_copies = (int)copies.size();
   if ((rc = q.copies.reserve(ctx, n_copies)) != LINS_OK) return rc;
   CK(q.prior_state.reserve((size_t)n * 20)); CK(q.prior_cov.reserve((size_t)n * 324));
@@ -415,7 +472,13 @@ int seq_step_phases(lins_ctx* ctx, const lins_seq_step_desc* d, const int32_t* c
   if (d->imu_off) std::memcpy(q.h_imu_off.p, d->imu_off, sizeof(int) * N1);
   else std::memset(q.h_imu_off.p, 0, sizeof(int) * N1);
   if (n_imu) std::memcpy(q.h_imu.p, d->imu, sizeof(double) * 7 * n_imu);
-  for (int s = 0; s < n; ++s) { q.h_status.p[s] = (unsigned char)status[s]; q.h_status.p[2 * n + s] = imu_use[s]; q.h_period.p[s] = slot_period(ctx, s); }
+  for (int s = 0; s < n; ++s) { q.h_status.p[s] = (unsigned char)status[s]; q.h_status.p[2 * n + s] = imu_use[s]; q.h_period.p[s] = slot_period(ctx, s); q.h_unit_tune.p[s] = slot_tuning(ctx, s); }
+  if (align)
+    for (int s = 0; s < n; ++s) {
+      double* a = q.h_align.p + 10 * (size_t)s;
+      std::copy(q.align_R.begin() + 9 * (size_t)s, q.align_R.begin() + 9 * (size_t)s + 9, a);
+      a[9] = q.tuned[s] ? 1.0 : 0.0;
+    }
   std::memcpy(r.h_off.p, run_off.data(), sizeof(int) * 2 * N1);
   std::memcpy(r.h_off.p + 2 * N1, init_off.data(), sizeof(int) * 2 * N1);
   if (n_imu) CK(cudaMemcpyAsync(q.imu.p, q.h_imu.p, sizeof(double) * 7 * n_imu, cudaMemcpyHostToDevice, ctx->stream));
@@ -423,6 +486,8 @@ int seq_step_phases(lins_ctx* ctx, const lins_seq_step_desc* d, const int32_t* c
   CK(cudaMemcpyAsync(q.status_d.p, q.h_status.p, n, cudaMemcpyHostToDevice, ctx->stream));
   CK(cudaMemcpyAsync(q.status_d.p + 2 * n, q.h_status.p + 2 * n, n, cudaMemcpyHostToDevice, ctx->stream));
   CK(cudaMemcpyAsync(q.period.p, q.h_period.p, sizeof(double) * n, cudaMemcpyHostToDevice, ctx->stream));
+  CK(cudaMemcpyAsync(q.unit_tune.p, q.h_unit_tune.p, sizeof(lins_dev::UnitTuning) * n, cudaMemcpyHostToDevice, ctx->stream));
+  if (align) CK(cudaMemcpyAsync(q.align.p, q.h_align.p, sizeof(double) * 10 * (size_t)n, cudaMemcpyHostToDevice, ctx->stream));
   if ((rc = q.copies.stage(ctx, copies.data(), n_copies, 0)) != LINS_OK) return rc;
   CK(cudaMemcpyAsync(r.qs_off.p, r.h_off.p, sizeof(int) * N1, cudaMemcpyHostToDevice, ctx->stream));
   CK(cudaMemcpyAsync(r.qc_off.p, r.h_off.p + N1, sizeof(int) * N1, cudaMemcpyHostToDevice, ctx->stream));
@@ -438,6 +503,11 @@ int seq_step_phases(lins_ctx* ctx, const lins_seq_step_desc* d, const int32_t* c
   CK(cudaEventRecord(q.ev[0], ctx->stream));
   const lins_seq::Consts* k = slot_consts(q);
   const lins_seq::InitConsts* ik = slot_init_consts(q);
+  if (align) {  // the tuned slots' IMU values into the vehicle frame (imuCallback) before anything reads them
+    lins_seq_align_kernel<<<n, 32, 0, ctx->stream>>>(q.imu.p, q.imu_off.p, n_init ? q.scan_imu.p : nullptr, q.align.p);
+    CK(cudaGetLastError());
+    ctx->launches += 1;
+  }
   if (n_imu) {
     lins_seq_predict_kernel<<<n, 32, 0, ctx->stream>>>(q.filt.p, q.cov.p, q.imu_last.p, q.imu.p, q.imu_off.p, q.status_d.p + 2 * n, q.pre.p, k, ik);
     CK(cudaGetLastError());
@@ -467,6 +537,7 @@ int seq_step_phases(lins_ctx* ctx, const lins_seq_step_desc* d, const int32_t* c
   bv.nn_s = q.tree_s.p; bv.nn_s_off = q.map_off.p + 2 * N1; bv.nn_c = q.tree_c.p; bv.nn_c_off = q.map_off.p + 3 * N1;
   bv.nn_stale = q.stale.p;
   bv.unit_period = q.period.p;
+  bv.unit_tune = q.unit_tune.p;
   bv.state_in = q.prior_state.p; bv.cov_in = q.prior_cov.p; bv.state_out = r.state_out.p; bv.cov_out = r.cov_out.p;
   bv.results = r.results.p; bv.reports = r.reports.p;
   bv.ind_s = r.ind_s.p; bv.ind_c = r.ind_c.p; bv.az_s = r.az_s.p; bv.az_c = r.az_c.p;
@@ -494,14 +565,14 @@ int seq_step_phases(lins_ctx* ctx, const lins_seq_step_desc* d, const int32_t* c
     CK(cudaMemcpyAsync(q.icp_pose.p + (size_t)s * 20, q.prior_state.p + (size_t)s * 20, sizeof(double) * 20, cudaMemcpyDeviceToDevice, ctx->stream));
     BatchView u = bv;
     u.n_scans = 1;
-    u.qs_off += s; u.qc_off += s; u.ts_off += s; u.tc_off += s; u.nn_s_off += s; u.nn_c_off += s; u.nn_stale += s; u.unit_period += s;
+    u.qs_off += s; u.qc_off += s; u.ts_off += s; u.tc_off += s; u.nn_s_off += s; u.nn_c_off += s; u.nn_stale += s; u.unit_period += s; u.unit_tune += s;
     u.cov_in += (size_t)s * 324; u.state_out += (size_t)s * 20; u.cov_out += (size_t)s * 324; u.results += s; u.reports = nullptr;
     u.accum += (size_t)s * 32;
     u.ind_s = q.icp_ind_s.p; u.ind_c = q.icp_ind_c.p;  // (the IESKF's IDs stay readable)
     u.qtile = fused_qtile((run_off[s + 1] - run_off[s]) + (run_off[N1 + s + 1] - run_off[N1 + s]));
     lins_dev::IcpState* icp = reinterpret_cast<lins_dev::IcpState*>(q.icp.p) + s;
     CK(cudaMemsetAsync(icp, 0, icp_state_bytes(), ctx->stream));
-    rc = icp_loop(ctx, r, u, q.icp_pose.p + (size_t)s * 20, icp);
+    rc = icp_loop(ctx, r, u, q.icp_pose.p + (size_t)s * 20, icp, q.h_unit_tune.p[s].num_iter);
     if (rc != LINS_OK) return rc;
   }
   if (any_icp) CK(cudaMemcpyAsync(q.status_d.p, q.h_status.p, n, cudaMemcpyHostToDevice, ctx->stream));
@@ -510,7 +581,7 @@ int seq_step_phases(lins_ctx* ctx, const lins_seq_step_desc* d, const int32_t* c
   // against its first scan's map; the IESKF's sequences read done and are passed over --------------------------------
   lins_dev::IcpState* init_icp = reinterpret_cast<lins_dev::IcpState*>(q.init_icp.p);
   if (n_second) {
-    lins_seq_icp_start_kernel<<<(n + 127) / 128, 128, 0, ctx->stream>>>(n, q.status_d.p, q.pre.p, q.icp_pose.p, init_icp);
+    lins_seq_icp_start_kernel<<<(n + 127) / 128, 128, 0, ctx->stream>>>(n, q.status_d.p, q.pre.p, q.icp_pose.p, init_icp, q.unit_tune.p);
     CK(cudaGetLastError());
     ctx->launches += 1;
     BatchView u = bv;
@@ -518,7 +589,9 @@ int seq_step_phases(lins_ctx* ctx, const lins_seq_step_desc* d, const int32_t* c
     u.reports = nullptr;
     u.ind_s = q.icp_ind_s.p; u.ind_c = q.icp_ind_c.p;
     u.qtile = fused_qtile(max_init_q);
-    rc = icp_loop(ctx, r, u, q.icp_pose.p, init_icp);
+    int n_iter = 0;  // (the largest NUM_ITER of the second scans)
+    for (int s = 0; s < n; ++s) if (status[s] == LINS_SEQ_SECOND) n_iter = std::max(n_iter, q.h_unit_tune.p[s].num_iter);
+    rc = icp_loop(ctx, r, u, q.icp_pose.p, init_icp, n_iter);
     if (rc != LINS_OK) return rc;
   }
   CK(cudaEventRecord(q.ev[3], ctx->stream));
@@ -846,6 +919,7 @@ int lins_gpu_seq_restart(lins_ctx* ctx, const uint8_t* mask) {
   bool any_configured = false;
   for (int s = 0; s < n; ++s) if (mask[s] && q.configured[s]) { q.configured[s] = 0; any_configured = true; }
   if (any_configured && (rc = upload_slot_consts(ctx, q, n)) != LINS_OK) { q.n = 0; return rc; }
+  for (int s = 0; s < n; ++s) if (mask[s]) q.tuned[s] = 0;  // (and untuned: the next step's tables read the context's)
   if ((rc = q.copies.stage(ctx, copies.data(), (int)copies.size(), 0)) != LINS_OK) return rc;
   for (int s = 0; s < n; ++s) q.h_status.p[s] = mask[s] ? 1 : 0;
   CK(cudaMemcpyAsync(q.status_d.p, q.h_status.p, n, cudaMemcpyHostToDevice, ctx->stream));
@@ -899,6 +973,31 @@ int lins_gpu_seq_configure(lins_ctx* ctx, const uint8_t* mask, const lins_slot_c
   if (rc == LINS_OK && cudaStreamSynchronize(ctx->stream) != cudaSuccess) rc = fail(ctx, LINS_E_CUDA, "configure");
   if (rc != LINS_OK) q.n = 0;
   return rc;
+}
+
+int lins_gpu_seq_tune(lins_ctx* ctx, const uint8_t* mask, const lins_slot_tuning* t) {
+  if (!ctx) return LINS_E_INVALID;
+  SeqState& q = ctx->seq;
+  if (q.n == 0) return fail(ctx, LINS_E_NOMAP, "no sequence run: call lins_gpu_seq_open");
+  if (!mask || !t) return fail(ctx, LINS_E_INVALID, "null tune mask / tunings");
+  if (!q.has_init) return fail(ctx, LINS_E_INVALID, "lins_gpu_seq_tune needs a run opened by lins_gpu_seq_open");
+  const int n = q.n;
+  for (int s = 0; s < n; ++s) {
+    if (!mask[s]) continue;
+    if (!q.fresh[s]) return fail(ctx, LINS_E_INVALID, "a tuned slot must be fresh (no step since open / restart)");
+    const lins_slot_tuning& u = t[s];
+    const bool ok = u.num_iter >= 0 && u.num_iter <= LINS_MAX_ITER && u.icp_freq >= 1 && std::isfinite(u.nearest_feature_search_sq_dist) &&
+                    std::isfinite(u.lidar_std) && std::isfinite(u.lidar_scale) && std::isfinite(u.imu_misalign_angle);
+    if (!ok) return fail(ctx, LINS_E_INVALID, "bad slot tuning (num_iter outside 0..LINS_MAX_ITER, icp_freq < 1, or a non-finite value)");
+  }
+  // (host state only: the step uploads the tables)
+  for (int s = 0; s < n; ++s)
+    if (mask[s]) {
+      q.tune[s] = t[s];
+      q.tuned[s] = 1;
+      misalign_R(t[s].imu_misalign_angle, &q.align_R[9 * (size_t)s]);
+    }
+  return LINS_OK;
 }
 
 int lins_gpu_seq_step_ex(lins_ctx* ctx, const lins_seq_step_desc* d, const double* scan_imu) {

@@ -201,6 +201,23 @@ class LinsSlotConfig(C.Structure):
         return cls(scan_period, *parts)
 
 
+class LinsSlotTuning(C.Structure):
+    """lins_slot_tuning (include/lins_gpu.h): one recording's estimator tuning and IMU misalignment."""
+    _fields_ = [("num_iter", C.c_int32), ("icp_freq", C.c_int32), ("nearest_feature_search_sq_dist", C.c_double),
+                ("lidar_std", C.c_double), ("lidar_scale", C.c_double), ("imu_misalign_angle", C.c_double)]
+
+    @classmethod
+    def shipped(cls, **kw):
+        """exp_port.yaml's values (NUM_ITER 30, ICP_FREQ 1, the 25 m^2 gate, LIDAR_STD 0.01, LIDAR_SCALE 1, a 3 degree
+        imu_misalign_angle) with any field overridden, e.g. shipped(num_iter=12, imu_misalign_angle=0.0)."""
+        t = cls(30, 1, 25.0, 0.01, 1.0, 3.0)
+        for k, v in kw.items():
+            if k not in dict(cls._fields_):
+                raise TypeError(f"unknown slot tuning key: {k}")
+            setattr(t, k, v)
+        return t
+
+
 class LinsPclDesc(C.Structure):
     """lins_pcl_desc: n segmented scans with their cloud_info, CSR."""
     _fields_ = [("n_scans", C.c_int32), ("line_num", C.c_int32), ("cloud", C.c_void_p), ("cloud_off", C.c_void_p),

@@ -134,6 +134,9 @@ def seq_lib():
         L.lins_seq_write_bag_period.argtypes = [C.POINTER(SynthCfg), C.c_uint64, C.c_int, C.c_char_p, C.c_char_p, C.c_char_p, C.c_double]
         L.lins_seq_run_bag_rig.restype = C.c_void_p
         L.lins_seq_run_bag_rig.argtypes = [C.c_char_p, C.c_char_p, C.c_char_p, C.c_int, C.c_int, C.c_int, C.c_void_p, C.POINTER(C.c_int)]
+        L.lins_seq_run_bag_tuned.restype = C.c_void_p
+        L.lins_seq_run_bag_tuned.argtypes = [C.c_char_p, C.c_char_p, C.c_char_p, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.POINTER(C.c_int)]
+        L.lins_host_align_imu.argtypes = [C.c_double, C.c_void_p, C.c_void_p]
         L.lins_seq_map_count.argtypes = [C.c_void_p]
         L.lins_seq_map_array.restype = C.POINTER(C.c_double)
         L.lins_seq_map_array.argtypes = [C.c_void_p, C.c_int]
@@ -201,24 +204,38 @@ def rig_array(rig):
     return np.array([v for k in RIG_ORDER for v in np.atleast_1d(np.asarray(rig[k], np.float64))], np.float64)
 
 
-def run_bag(path, lidar_topic="/velodyne_points", imu_topic="/imu/data", max_scans=0, lidar_model=0, device=0, rig=None):
+TUNING_ORDER = ("num_iter", "icp_freq", "nearest_feature_search_sq_dist", "lidar_std", "lidar_scale", "imu_misalign_angle")
+
+
+def run_bag(path, lidar_topic="/velodyne_points", imu_topic="/imu/data", max_scans=0, lidar_model=0, device=0, rig=None, tuning=None):
     """BASELINE.json configs[1] runner: replay a ROS1 bag (sensor_msgs/PointCloud2 + sensor_msgs/Imu) through image
     projection, feature extraction and the GPU IESKF update, the way LinsFusion does (Estimator.cpp:123-284).  rig: the
     robot's exp_port.yaml values (a dict as rig_config.load_rig returns) for the StateEstimator's EstimatorParams; None =
-    the shipped values with zero INIT_BA / INIT_BW."""
+    the shipped values with zero INIT_BA / INIT_BW.  tuning: the estimator's tuning and IMU misalignment (a dict as
+    rig_config.load_config returns): EstimatorParams::gpu takes the tuning, and every IMU sample is rotated by
+    alignIMUtoVehicle as imuCallback does; None = the shipped tuning and no rotation."""
     L = seq_lib()
     err = C.c_int(0)
     r = rig_array(rig) if rig is not None else None
     if r is not None and len(r) != 29:
         raise ValueError(f"a rig has 29 values, got {len(r)}")
-    h = L.lins_seq_run_bag_rig(path.encode(), lidar_topic.encode(), imu_topic.encode(), max_scans, lidar_model, device,
-                               None if r is None else r.ctypes.data, C.byref(err))
+    t = np.array([float(tuning[k]) for k in TUNING_ORDER], np.float64) if tuning is not None else None
+    h = L.lins_seq_run_bag_tuned(path.encode(), lidar_topic.encode(), imu_topic.encode(), max_scans, lidar_model, device,
+                                 None if r is None else r.ctypes.data, None if t is None else t.ctypes.data, C.byref(err))
     if not h:
         raise RuntimeError(f"lins_seq_run_bag failed with {err.value}")
     try:
         return _seq_record(L, h)
     finally:
         L.lins_seq_destroy(h)
+
+
+def host_align_imu(angle, v):
+    """The shim's alignIMUtoVehicle of one 3-vector (lins_host_align_imu): R^T v, R = rpy2R((0, 0, deg2rad(angle)))."""
+    a = np.ascontiguousarray(v, np.float64)
+    out = np.zeros(3)
+    seq_lib().lins_host_align_imu(float(angle), a.ctypes.data, out.ctypes.data)
+    return out
 
 
 def run_sequence(config="config3", seed=1, n_scans=12, device=0, **overrides):

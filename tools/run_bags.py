@@ -1,5 +1,6 @@
 #!/usr/bin/env python
-"""tools/run_bags.py BAG... [--slots S] [--lidar /velodyne_points] [--imu /imu/data] [--max-scans N] [--lidar-model M] [--map] [--out DIR]
+"""tools/run_bags.py BAG... [--slots S] [--lidar /velodyne_points] [--imu /imu/data] [--max-scans N] [--lidar-model M] [--map]
+                   [--config a.yaml[,b.yaml,...] [--tune]] [--out DIR]
 
 Replays many ROS1 bags through sequence mode in lockstep (bag_replay.py): every bag is scheduled as tools/run_bag.py
 schedules one, the bags are queued through S slots, and each scan's sensor_msgs/PointCloud2 message is decoded on the
@@ -13,7 +14,9 @@ tools/run_bag.py --map's line format; like run_bag.py --map, the bags' IMU orien
 --config a.yaml[,b.yaml,...] takes LINS config files (exp_port.yaml, OpenCV YAML): one for every bag or one per bag.
 Each bag's slot is configured with its file's rig (scan period, feature thresholds, extrinsic, IMU noise, init stds and
 biases); the files must agree on the keys every slot shares (num_iter, icp_freq, nearest_feature_search_sq_dist,
-lidar_std, lidar_scale), which set the context's parameters."""
+lidar_std, lidar_scale), which set the context's parameters.  With --tune as well, each bag's slot also takes its file's
+tuning (those shared keys) and imu_misalign_angle (lins_gpu_seq_tune: its IMU values are rotated into the vehicle frame as
+LinsFusion::imuCallback does), so the files may differ in any key; the first file's tuning sets the context's parameters."""
 import argparse, importlib, os, sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import numpy as np
@@ -54,6 +57,20 @@ def bag_configs(spec, n_bags):
     return rc.lins_params(shared), cfgs
 
 
+def bag_tunings(spec, n_bags):
+    """(LinsParams of the context, one LinsSlotConfig and one LinsSlotTuning per bag) from the --config value with --tune:
+    each file gives its bag's rig and tuning (rig_config.load_config), and the files may differ in any key.  ValueError
+    for a count mismatch."""
+    rc = importlib.import_module("lins---lidar-inertial-slam_b200.rig_config")
+    paths = [v.strip() for v in str(spec).split(",")]
+    if len(paths) not in (1, n_bags):
+        raise ValueError(f"--config lists {len(paths)} files for {n_bags} bags")
+    loaded = [rc.load_config(p) for p in paths]
+    if len(loaded) == 1:
+        loaded = loaded * n_bags
+    return rc.lins_params(loaded[0][1]), [rc.slot_config(r) for r, _ in loaded], [rc.slot_tuning(t) for _, t in loaded]
+
+
 def write_map(o, out_dir, name):
     """<name>.odometry.txt and <name>.mapped.txt of one replayed bag, one line per published scan as tools/run_bag.py --map
     writes odometry.txt and mapped.txt: stamp, then x y z qx qy qz qw of the odometry, resp. the processed flag and
@@ -75,16 +92,23 @@ def main(argv=None):
     ap.add_argument("--lidar-model", default="0", help="0 | 1 for every bag, or one per bag: 0,1,...")
     ap.add_argument("--map", action="store_true", help="run each bag's mapping node on what its estimator publishes")
     ap.add_argument("--config", help="LINS config file(s): one for every bag, or one per bag: a.yaml,b.yaml,...")
+    ap.add_argument("--tune", action="store_true", help="with --config: each bag also takes its file's tuning and IMU misalignment")
     ap.add_argument("--out")
     a = ap.parse_args(argv)
     try:
         model = lidar_models(a.lidar_model, len(a.bags))
-        prm, cfgs = bag_configs(a.config, len(a.bags)) if a.config else (None, [None] * len(a.bags))
+        if a.tune and not a.config:
+            raise ValueError("--tune takes the tuning from the --config files")
+        tunes = [None] * len(a.bags)
+        if a.tune:
+            prm, cfgs, tunes = bag_tunings(a.config, len(a.bags))
+        else:
+            prm, cfgs = bag_configs(a.config, len(a.bags)) if a.config else (None, [None] * len(a.bags))
     except ValueError as e:
         ap.error(str(e))
     br = importlib.import_module("lins---lidar-inertial-slam_b200.bag_replay")
     capi = importlib.import_module("lins---lidar-inertial-slam_b200.capi")
-    recs = [br.Recording(p, a.lidar, a.imu, a.max_scans, config=c) for p, c in zip(a.bags, cfgs)]
+    recs = [br.Recording(p, a.lidar, a.imu, a.max_scans, config=c, tuning=t) for p, c, t in zip(a.bags, cfgs, tunes)]
     outs = br.replay(recs, a.slots or len(recs), model=model, map=a.map, gpu=capi.LinsGpu(prm) if prm is not None else None)
     np.set_printoptions(precision=4, suppress=True)
     for p, o in zip(a.bags, outs):

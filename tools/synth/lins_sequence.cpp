@@ -260,8 +260,37 @@ int lins_seq_write_bag(const lins_synth_cfg* cfg, uint64_t seed, int n_scans, co
 // rig (lins_seq_run_bag_rig; null = seq_params' defaults): the exp_port.yaml values of one robot, 29 doubles in the order
 // scan_period, edge_threshold, surf_threshold, imu_lidar_extrinsic_angle, acc_n, gyr_n, acc_w, gyr_w, then init_pos_std,
 // init_vel_std, init_att_std, init_acc_std, init_gyr_std, init_ba, init_bw (3 each)
+// tuning (lins_seq_run_bag_tuned; null = the rig's run): the slot tuning of include/lins_gpu.h as 6 doubles, num_iter,
+// icp_freq, nearest_feature_search_sq_dist, lidar_std, lidar_scale, imu_misalign_angle (degrees).  EstimatorParams::gpu
+// takes the first five, and every decoded IMU sample goes through alignIMUtoVehicle with the angle, as imuCallback does
+// (Estimator.cpp:124-135, :286-292).
+void* lins_seq_run_bag_tuned(const char* path, const char* lidar_topic, const char* imu_topic, int max_scans, int lidar_model, int device,
+                             const double* rig, const double* tuning, int* error);
 void* lins_seq_run_bag_rig(const char* path, const char* lidar_topic, const char* imu_topic, int max_scans, int lidar_model, int device,
                            const double* rig, int* error) {
+  return lins_seq_run_bag_tuned(path, lidar_topic, imu_topic, max_scans, lidar_model, device, rig, nullptr, error);
+}
+
+// alignIMUtoVehicle (Estimator.cpp:286-292) of one vector: R^T v with R = rpy2R((0, 0, deg2rad(angle))) = Rz Ry Rx
+// (math_utils.h:164-182), every product entry and output summed (a0 b0 + a1 b1) + a2 b2, in f64
+void lins_host_align_imu(double angle, const double* v, double* out) {
+  const double y = angle * M_PI / 180.0, p = 0.0, r = 0.0;
+  const double Rz[9] = {std::cos(y), -std::sin(y), 0, std::sin(y), std::cos(y), 0, 0, 0, 1};
+  const double Ry[9] = {std::cos(p), 0., std::sin(p), 0., 1., 0., -std::sin(p), 0., std::cos(p)};
+  const double Rx[9] = {1., 0., 0., 0., std::cos(r), -std::sin(r), 0., std::sin(r), std::cos(r)};
+  auto mul = [](const double* A, const double* B, double* C) {
+    for (int i = 0; i < 3; ++i)
+      for (int j = 0; j < 3; ++j) C[3 * i + j] = (A[3 * i] * B[j] + A[3 * i + 1] * B[3 + j]) + A[3 * i + 2] * B[6 + j];
+  };
+  double T[9], R[9];
+  mul(Rz, Ry, T);
+  mul(T, Rx, R);
+  const double x = v[0], yy = v[1], z = v[2];
+  for (int j = 0; j < 3; ++j) out[j] = (R[j] * x + R[3 + j] * yy) + R[6 + j] * z;
+}
+
+void* lins_seq_run_bag_tuned(const char* path, const char* lidar_topic, const char* imu_topic, int max_scans, int lidar_model, int device,
+                             const double* rig, const double* tuning, int* error) {
   using namespace lins::rosbag;
   if (error) *error = 0;
   Reader rd;
@@ -275,8 +304,10 @@ void* lins_seq_run_bag_rig(const char* path, const char* lidar_topic, const char
     if (m.conn->topic == imu_topic) {
       ImuMsg im;
       if (!decode_imu(m.data, m.size, im)) { bad = true; return; }
-      imus.push_back(ImuS{im.header.stamp, V3D(im.linear_acceleration[0], im.linear_acceleration[1], im.linear_acceleration[2]),
-                          V3D(im.angular_velocity[0], im.angular_velocity[1], im.angular_velocity[2])});
+      double a[3] = {im.linear_acceleration[0], im.linear_acceleration[1], im.linear_acceleration[2]};
+      double g[3] = {im.angular_velocity[0], im.angular_velocity[1], im.angular_velocity[2]};
+      if (tuning) { const double a0[3] = {a[0], a[1], a[2]}, g0[3] = {g[0], g[1], g[2]}; lins_host_align_imu(tuning[5], a0, a); lins_host_align_imu(tuning[5], g0, g); }
+      imus.push_back(ImuS{im.header.stamp, V3D(a[0], a[1], a[2]), V3D(g[0], g[1], g[2])});
     } else if (m.conn->topic == lidar_topic && (max_scans <= 0 || (int)scans.size() < max_scans)) {
       Header h;
       Cloud c;
@@ -299,6 +330,10 @@ void* lins_seq_run_bag_rig(const char* path, const char* lidar_topic, const char
     V3D* v[7] = {&ep.filter.init_pos_std, &ep.filter.init_vel_std, &ep.filter.init_att_std, &ep.filter.init_acc_std, &ep.filter.init_gyr_std,
                  &ep.filter.init_ba, &ep.filter.init_bw};
     for (int k = 0; k < 7; ++k) *v[k] = V3D(rig[8 + 3 * k], rig[9 + 3 * k], rig[10 + 3 * k]);
+  }
+  if (tuning) {
+    ep.gpu.num_iter = (int)tuning[0]; ep.gpu.icp_freq = (int)tuning[1]; ep.gpu.nearest_feature_search_sq_dist = tuning[2];
+    ep.gpu.lidar_std = tuning[3]; ep.gpu.lidar_scale = tuning[4];
   }
   StateEstimator est(ep, device);
   ImageProjection ip(lm);

@@ -767,6 +767,37 @@ int lins_gpu_seq_map_step(lins_ctx* ctx, const lins_seq_map_desc* d, lins_mapper
    LINS_E_NOMAP on an unbound run. */
 int lins_gpu_seq_map_published(lins_ctx* ctx, double* pose /*S x 7*/, int32_t* sizes /*S x 3*/);
 
+/* ---- saving and loading slots: checkpoint, resume and move recordings between runs ---------------------------------
+   A slot of a lins_gpu_seq_open run is saved as a self-contained byte blob and loaded into a fresh slot of any
+   lins_gpu_seq_open run of the same library build, at any slot index, on the same GPU or another; the loaded slot then
+   continues bit-identically to the slot it was saved from.  A blob carries what a later step, publish or download reads:
+   the filter, global, linearisation and pre-integration rows and the covariance, imu_last, the fusion status, the maps
+   and the stale 1-NN cloud, the slot's config and tuning, and on a run bound by lins_gpu_seq_map_open its published
+   YZX flag, pose and outlier cloud and its mapping node (scalars and IMU queue, window, key poses, the stored key frames'
+   clouds, the scan-to-map loop state).  It does not carry the last step's outputs: until the slot's next step, results,
+   reports, the IESKF prior and the fallback's correspondence IDs read as after a restart, scan_status reads LINS_SEQ_IDLE,
+   and the mapper download returns key poses and window but no DS clouds until the slot's next processed cycle.  A
+   configured or tuned blob carries its own values; an unconfigured blob records the source run's lins_seq_params /
+   lins_seq_init_params and loads only into a run opened with bit-equal ones.  What each call takes stays the caller's,
+   as for any slot: lins_params, the step's lins_feature_params and lidar models.  A loaded slot is not fresh: it cannot
+   be configured or tuned.  Runs of lins_gpu_seq_begin cannot save or load.
+   Every call takes a slot mask (S entries); slot s's blob is the byte range [off[s], off[s + 1]) of one buffer. */
+/* The offsets of each masked slot's blob in one buffer (off: S + 1; an unmasked slot's range is empty).  Host bookkeeping
+   only, no synchronisation.  LINS_E_INVALID for a NULL argument, a run of lins_gpu_seq_begin or a bound run whose
+   lins_gpu_seq_map_step is pending; LINS_E_NOMAP without a run. */
+int lins_gpu_seq_save_size(lins_ctx* ctx, const uint8_t* mask /*S*/, uint64_t* off /*S+1*/);
+/* Writes every masked slot's blob at blob + off[s], off as lins_gpu_seq_save_size returned it.  One gather launch, one
+   D2H and one synchronisation whatever the mask; the run is unchanged.  LINS_E_INVALID as lins_gpu_seq_save_size and for
+   other offsets or a NULL blob; a CUDA error ends the run. */
+int lins_gpu_seq_save(lins_ctx* ctx, const uint8_t* mask /*S*/, void* blob, const uint64_t* off /*S+1*/);
+/* Loads the blob at [off[s], off[s + 1]) of blob into every masked slot, each of which must be fresh (not present in a
+   step since lins_gpu_seq_open or its last lins_gpu_seq_restart).  Every masked blob is validated in full first (format,
+   record sizes of the build, lengths, section bounds, counts, status values, the window's key frames, the binding: a
+   bound blob loads only into a bound run and an unbound one only into an unbound run; the constants rule above): all or
+   nothing, LINS_E_INVALID with nothing changed for any rejection, a NULL argument, a pending lins_gpu_seq_map_step or a
+   run of lins_gpu_seq_begin.  A CUDA error after the validation ends the run.  LINS_E_NOMAP without a run. */
+int lins_gpu_seq_load(lins_ctx* ctx, const uint8_t* mask /*S*/, const void* blob, const uint64_t* off /*S+1*/);
+
 /* block until everything queued on the ctx stream has finished */
 int lins_gpu_sync(lins_ctx* ctx);
 

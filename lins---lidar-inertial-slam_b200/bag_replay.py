@@ -20,9 +20,15 @@ LINS exp_port.yaml gives them): its slot is configured with it (lins_gpu_seq_con
 its IMU schedule uses that scan period.  Recordings without one use the run's values.  A recording may also carry its
 tuning (a LinsSlotTuning: NUM_ITER, ICP_FREQ, the 1-NN gate, LIDAR_STD, LIDAR_SCALE and imu_misalign_angle): its slot is
 tuned with it (lins_gpu_seq_tune) where it is configured, and the device rotates its IMU rows, which stay raw here.
+A replay can stop and continue: replay(..., checkpoint=dir, stop_after=k) ends after k steps and writes a checkpoint
+directory (every occupied slot saved by lins_gpu_seq_save, and the driver's state), and replay(..., resume=dir) opens a
+new context with the same slot count, loads the slots into it (lins_gpu_seq_load) and continues from step k.  The
+outputs equal those of a replay that never stopped, byte for byte.
 """
 import ctypes as C
+import glob
 import importlib.util
+import itertools
 import os
 
 import numpy as np
@@ -173,7 +179,87 @@ def model_table(recordings, model):
     return models, of
 
 
-def replay(recordings, slots, model=None, device=0, gpu=None, map=False):
+# the per-scan lists of a map=True replay and the arrays they become: (dtype, row shape)
+_MAP_LISTS = dict(map_time=(np.float64, ()), map_odom=(np.float64, (7,)), map_processed=(np.int32, ()),
+                  map_aft_mapped=(np.float32, (6,)), map_keyframes=(np.int32, ()), map_sizes=(np.int32, (3,)))
+
+
+def _map_arrays(o):
+    """o with its per-published-scan lists as the arrays a finished replay returns."""
+    o = dict(o)
+    for k, (dt, row) in _MAP_LISTS.items():
+        if k in o:
+            o[k] = np.array(o[k], dt).reshape((-1,) + row)
+    return o
+
+
+def save_driver_state(path, step, slots, lengths, map, held, out, blob_files):
+    """Write a replay's driver state to the file path (an .npz): the number of steps run, the slot count, the recording
+    lengths, map, each slot's held recording (-1: none) and its last report's key-frame count (-1: none yet), the output
+    dicts so far, and the file of each slot's blob ('' for an unsaved slot).  Written to a temporary file first, then
+    renamed over path, so that a reader sees the old state or the new one."""
+    a = dict(step=np.int64(step), slots=np.int64(slots), lengths=np.asarray(lengths, np.int64), map=np.int64(bool(map)),
+             held_rec=np.array([h[0] if h is not None else -1 for h in held], np.int64),
+             held_kf=np.array([h[1] if h is not None and h[1] is not None else -1 for h in held], np.int64),
+             blob_files=np.array(blob_files, dtype=np.str_), n_out=np.int64(len(out)))
+    for i, o in enumerate(out):
+        for k, v in _map_arrays(o).items():
+            a[f"out{i}.{k}"] = np.asarray(v)
+    tmp = path + ".tmp.npz"
+    np.savez(tmp, **a)
+    os.replace(tmp, path)
+
+
+def load_driver_state(path):
+    """The driver state save_driver_state wrote: a dict of step, slots, lengths, map, held, out and blob_files, with out
+    and held as replay() keeps them while it runs."""
+    with np.load(path, allow_pickle=False) as z:
+        out = [dict() for _ in range(int(z["n_out"]))]
+        for name in z.files:
+            if name.startswith("out"):
+                i, k = name[3:].split(".", 1)
+                v = z[name]
+                out[int(i)][k] = list(v) if k in _MAP_LISTS else v
+        held = [None if r < 0 else (int(r), None if kf < 0 else int(kf)) for r, kf in zip(z["held_rec"], z["held_kf"])]
+        return dict(step=int(z["step"]), slots=int(z["slots"]), lengths=[int(x) for x in z["lengths"]], map=bool(z["map"]),
+                    held=held, out=out, blob_files=[str(f) for f in z["blob_files"]])
+
+
+def write_checkpoint(g, directory, step, who, lengths, map, held, out):
+    """Save every slot that holds a recording after `step` steps (lins_gpu_seq_save) and the driver state into directory.
+    Each checkpoint's blobs have files of their own, named by step; the driver state names them and is written last, and
+    the older blobs go after it."""
+    os.makedirs(directory, exist_ok=True)
+    blobs = g.seq_save(np.array([w is not None for w in who], np.uint8))
+    files = []
+    for j, b in enumerate(blobs):
+        if b is None:
+            files.append("")
+            continue
+        files.append(f"slot{j}_step{step}.bin")
+        with open(os.path.join(directory, files[-1]), "wb") as f:
+            f.write(b)
+    save_driver_state(os.path.join(directory, "driver.npz"), step, len(who), lengths, map, held, out, files)
+    for f in glob.glob(os.path.join(directory, "slot*_step*.bin")):
+        if os.path.basename(f) not in files:
+            os.remove(f)
+
+
+def read_checkpoint(directory):
+    """The driver state of a checkpoint directory and its slot blobs (bytes, or None for a slot without one)."""
+    st = load_driver_state(os.path.join(directory, "driver.npz"))
+    blobs = []
+    for f in st["blob_files"]:
+        if not f:
+            blobs.append(None)
+            continue
+        with open(os.path.join(directory, f), "rb") as fh:
+            blobs.append(fh.read())
+    return st, blobs
+
+
+def replay(recordings, slots, model=None, device=0, gpu=None, map=False, checkpoint=None, checkpoint_every=None, stop_after=None,
+           resume=None):
     """Run the recordings through `slots` slots of one context.  model: one LinsLidarModel for every recording (None =
     VLP-16) or a list with one per recording; a slot is projected with the model of the recording it holds.  Returns per
     recording a dict of per-scan arrays: stamps, status (StateEstimator::status_ after the scan), scan_status (LINS_SEQ_*),
@@ -183,29 +269,46 @@ def replay(recordings, slots, model=None, device=0, gpu=None, map=False):
     odometry, YZX position + quaternion x y z w of globalStateYZX_, as fed to the mapper), map_sizes (m x 3: the
     less-sharp, less-flat and outlier cloud sizes), map_processed, map_aft_mapped (m x 6: transformAftMapped) and
     map_keyframes (n_keyframes after the cycle); and key_poses (the mapper's cloudKeyPoses6D, k x
-    7, downloaded when the recording ends)."""
+    7, downloaded when the recording ends).
+    checkpoint: a directory.  With stop_after=k the replay ends after its first k steps, writes a checkpoint there and
+    returns None (it returns the outputs as usual when it has fewer steps); with checkpoint_every=N it writes one after
+    every N-th step and runs on.  resume: a checkpoint directory written for the same recordings, slot count and map:
+    the replay continues from its step in a new context (gpu: one to open it on) and returns what a replay that never
+    stopped returns."""
     models, rec_model = model_table(recordings, model)
+    lengths = [len(r) for r in recordings]
+    if (stop_after is not None or checkpoint_every) and checkpoint is None:
+        raise ValueError("stop_after / checkpoint_every need a checkpoint directory")
+    start, blobs = 0, None
+    if resume is not None:
+        st, blobs = read_checkpoint(resume)
+        if st["lengths"] != lengths or st["slots"] != slots or st["map"] != bool(map):
+            raise ValueError(f"{resume}: a checkpoint of other recordings, slot count or map setting")
+        start = st["step"]
     g = gpu or _capi.LinsGpu(device=device)
     g.seq_open(LinsSeqParams.shipped(), shim_init_params(), slots)
     out = [dict(stamps=r.stamps.copy(), status=np.zeros(len(r), np.int32), scan_status=np.zeros(len(r), np.int32),
                 global_est=np.zeros((len(r), 7)), global_state=np.zeros((len(r), 19)), iters=np.full(len(r), -1, np.int32),
                 flags=np.full(len(r), -1, np.int32)) for r in recordings]
+    held = [None] * slots  # (recording, n_keyframes of its last published report or None) of each slot (map=True)
     if map:
         g.seq_map_open()
         for o in out:
             o.update(map_time=[], map_odom=[], map_processed=[], map_aft_mapped=[], map_keyframes=[], map_sizes=[], key_poses=np.zeros((0, 7)))
-        held = [None] * slots  # (recording, last published report) of each slot
+    if resume is not None:
+        out, held = st["out"], st["held"]
+        g.seq_load(np.array([b is not None for b in blobs], np.uint8), blobs)
     blob = _PinnedBlob()
 
     def finish(j):  # the key poses of the recording slot j held, before the slot is handed on
         if held[j] is not None and held[j][1] is not None:
-            kp = np.zeros((held[j][1].n_keyframes, 7))
+            kp = np.zeros((held[j][1], 7))
             g._ck(g.L.lins_gpu_mappers_download(g.h, j, _capi.ptr(kp), *[None] * 7))
             out[held[j][0]]["key_poses"] = kp
         held[j] = None
 
     try:
-        for restart, who in slot_queue([len(r) for r in recordings], slots):
+        for t, (restart, who) in enumerate(itertools.islice(slot_queue(lengths, slots), start, None), start):
             if map:
                 for j in range(slots):
                     if held[j] is not None and (who[j] is None or who[j][0] != held[j][0]):
@@ -259,19 +362,20 @@ def replay(recordings, slots, model=None, device=0, gpu=None, map=False):
                     if not pub[j]:
                         continue
                     o, r = out[w[0]], reps[j]
-                    held[j] = (w[0], r)
+                    held[j] = (w[0], r.n_keyframes)
                     o["map_time"].append(time[j]); o["map_odom"].append(pose[j].copy()); o["map_processed"].append(r.processed)
                     o["map_aft_mapped"].append(list(r.transform_aft_mapped)); o["map_keyframes"].append(r.n_keyframes)
                     o["map_sizes"].append(sizes[j].copy())
+            done = t + 1
+            if stop_after is not None and done == stop_after:
+                write_checkpoint(g, checkpoint, done, who, lengths, map, held, out)
+                return None
+            if checkpoint_every and done % checkpoint_every == 0:
+                write_checkpoint(g, checkpoint, done, who, lengths, map, held, out)
         if map:
             for j in range(slots):
                 finish(j)
-            for o in out:
-                o["map_time"] = np.array(o["map_time"]); o["map_odom"] = np.array(o["map_odom"]).reshape(-1, 7)
-                o["map_processed"] = np.array(o["map_processed"], np.int32)
-                o["map_aft_mapped"] = np.array(o["map_aft_mapped"], np.float32).reshape(-1, 6)
-                o["map_keyframes"] = np.array(o["map_keyframes"], np.int32)
-                o["map_sizes"] = np.array(o["map_sizes"], np.int32).reshape(-1, 3)
+            out = [_map_arrays(o) for o in out]
     finally:
         blob.release()
     return out

@@ -39,18 +39,19 @@ EXPORTS = [
     "lins_gpu_mapper_reset", "lins_gpu_mapper_imu", "lins_gpu_mapper_step", "lins_gpu_mapper_download", "lins_gpu_voxel_grid",
     "lins_gpu_mappers_open", "lins_gpu_mappers_reset", "lins_gpu_mappers_imu", "lins_gpu_mappers_step", "lins_gpu_mappers_download",
     "lins_gpu_seq_map_open", "lins_gpu_seq_map_step", "lins_gpu_seq_map_published", "lins_gpu_seq_configure", "lins_gpu_seq_tune",
+    "lins_gpu_seq_save_size", "lins_gpu_seq_save", "lins_gpu_seq_load",
 ]
 
 NVCC_ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]  # H100 (Hopper)
 NVCC_COMMON = NVCC_ARCH + ["-lineinfo", "-O3", "-std=c++17", "-Xcompiler", "-fPIC"]
 # translation units and their extra flags: lins_gpu.cu (the fused kernel and most of the C-ABI), lins_upload.cu (batch
 # upload), lins_map.cu (row F2's host side), lins_seq.cu (sequence mode), lins_features.cu (feature extraction),
-# lins_projection.cu (image projection), lins_cloud2.cu (PointCloud2 decoding), lins_mapper.cu (the mapping node's cycle), lins_mappers.cu (many mapping nodes in lockstep) — all bit-exact, so no multiply-add contraction: the association and the map
+# lins_projection.cu (image projection), lins_cloud2.cu (PointCloud2 decoding), lins_mapper.cu (the mapping node's cycle), lins_mappers.cu (many mapping nodes in lockstep), lins_seq_save.cu (saving and loading slots) — all bit-exact, so no multiply-add contraction: the association and the map
 # fits depend on it — and lins_jacobian.cu (the tolerance-checked split Jacobian kernel: contraction allowed)
 UNITS = [("lins_gpu.cu", ["-fmad=false"]), ("lins_upload.cu", ["-fmad=false"]), ("lins_map.cu", ["-fmad=false"]),
          ("lins_seq.cu", ["-fmad=false"]), ("lins_features.cu", ["-fmad=false"]), ("lins_projection.cu", ["-fmad=false"]),
          ("lins_cloud2.cu", ["-fmad=false"]), ("lins_mapper.cu", ["-fmad=false"]), ("lins_mappers.cu", ["-fmad=false"]),
-         ("lins_jacobian.cu", [])]
+         ("lins_seq_save.cu", ["-fmad=false"]), ("lins_jacobian.cu", [])]
 
 
 def build(force=False, verbose=False):
@@ -149,6 +150,9 @@ def lib():
         L.lins_gpu_seq_map_open.argtypes = [vp]
         L.lins_gpu_seq_map_step.argtypes = [vp, C.POINTER(LinsSeqMapDesc), vp, vp]
         L.lins_gpu_seq_map_published.argtypes = [vp, vp, vp]
+        L.lins_gpu_seq_save_size.argtypes = [vp, vp, vp]
+        L.lins_gpu_seq_save.argtypes = [vp, vp, vp, vp]
+        L.lins_gpu_seq_load.argtypes = [vp, vp, vp, vp]
         _LIB = L
     return _LIB
 
@@ -546,6 +550,35 @@ class LinsGpu:
             raise ValueError(f"mask / tunings have {len(m)} / {len(tunings)} entries, the run {self._seq_n}")
         arr = (LinsSlotTuning * self._seq_n)(*[t if t is not None else LinsSlotTuning() for t in tunings])
         self._ck(self.L.lins_gpu_seq_tune(self.h, ptr(m), C.cast(arr, C.c_void_p)))
+
+    def seq_save(self, mask):
+        """Save the slots with mask[s] != 0: a list of S entries, each slot's blob (bytes, self-contained: it can be
+        written to a file alone and loaded into a fresh slot of any seq_open run of this library build) or None where the
+        mask is 0.  The run is unchanged."""
+        m = self._slot_mask(mask)
+        off = np.zeros(self._seq_n + 1, np.uint64)
+        self._ck(self.L.lins_gpu_seq_save_size(self.h, ptr(m), ptr(off)))
+        buf = np.zeros(max(int(off[-1]), 1), np.uint8)
+        self._ck(self.L.lins_gpu_seq_save(self.h, ptr(m), ptr(buf), ptr(off)))
+        return [buf[int(off[s]): int(off[s + 1])].tobytes() if m[s] else None for s in range(self._seq_n)]
+
+    def seq_load(self, mask, blobs):
+        """Load blobs[s] (bytes, as seq_save returned it) into every slot with mask[s] != 0, each still fresh (no step
+        since seq_open / its last seq_restart); blobs has S entries (None where the mask is 0).  All or nothing."""
+        m = self._slot_mask(mask)
+        if len(blobs) != self._seq_n:
+            raise ValueError(f"{len(blobs)} blobs, the run has {self._seq_n} slots")
+        parts = [bytes(blobs[s]) if m[s] else b"" for s in range(self._seq_n)]
+        off = np.zeros(self._seq_n + 1, np.uint64)
+        off[1:] = np.cumsum([len(p) for p in parts])
+        buf = np.frombuffer(b"".join(parts) or b"\0", np.uint8)
+        self._ck(self.L.lins_gpu_seq_load(self.h, ptr(m), ptr(buf), ptr(off)))
+
+    def _slot_mask(self, mask):
+        m = np.ascontiguousarray(mask, dtype=np.uint8)
+        if len(m) != self._seq_n:
+            raise ValueError(f"mask has {len(m)} entries, the run {self._seq_n}")
+        return m
 
     def seq_download_init(self):
         """dict: fusion_status (S; StateEstimator::status_ of every slot) and, for the slots whose last scan was a second

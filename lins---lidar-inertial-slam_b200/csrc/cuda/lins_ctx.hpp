@@ -203,6 +203,8 @@ struct SeqState {
   bool has_step = false;                               // a step has run since lins_gpu_seq_begin
   std::vector<int> h_run_off;                          // 2 x (n + 1): the last step's compacted query offsets (surf, corner)
   SeqPubState pub;                                     // the publish step of a run bound to the lockstep mappers
+  Buf<float4> blob; Buf<float4, kPinned> h_blob;       // lins_gpu_seq_save / _load: the slot blobs on the device and
+                                                       // their pinned staging (lins_seq_save.cu)
   ~SeqState() { for (cudaEvent_t e : ev) if (e) cudaEventDestroy(e); }
 };
 
@@ -674,5 +676,16 @@ int mappers_open(lins_ctx* ctx, MappersState& ms, int n_slots);
 int mappers_reset(lins_ctx* ctx, MappersState& ms, const uint8_t* mask);
 int mappers_step(lins_ctx* ctx, MappersState& ms, const lins_mappers_desc* d, lins_mapper_report* reps, const MapPiece* dev,
                  const double* period);
+// lins_seq.cu: the map generations and slot constants a step, a restart and a load share.  upload_slot_consts: every
+// slot's device constants (its config's, else the run's), then a synchronisation; queue_map_state: the upload of the
+// host copies of map_off and stale (pageable: the caller synchronises before they change); current_piece: cloud c
+// (map_s, map_c, tree_s, tree_c) of slot s in the current generation; build_next_maps: the next generation from
+// next[4 * s + c] (fills h_nmap_off, reserves nmap_* / ntree_* and appends the copies that fill them to `copies`);
+// swap_maps: the next generation becomes the current one (its copies have been queued)
+int upload_slot_consts(lins_ctx* ctx, SeqState& q, int n);
+cudaError_t queue_map_state(lins_ctx* ctx, SeqState& q);
+MapPiece current_piece(const SeqState& q, int c, int s);
+int build_next_maps(lins_ctx* ctx, SeqState& q, const std::vector<MapPiece>& next, std::vector<DevCopy>& copies);
+void swap_maps(SeqState& q);
 
 }  // namespace lins_capi

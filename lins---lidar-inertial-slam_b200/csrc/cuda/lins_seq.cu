@@ -206,6 +206,10 @@ void init_consts_of(double* out, const lins_seq_params* prm, const lins_seq_init
 
 constexpr size_t kNConsts = sizeof(SeqState::consts) / sizeof(double), kNInit = sizeof(SeqState::init_consts) / sizeof(double);
 
+}  // namespace
+
+namespace lins_capi {
+
 // every slot's device constants: a configured slot's from its config, the others the run's; then a synchronisation (the
 // sources are pageable)
 int upload_slot_consts(lins_ctx* ctx, SeqState& q, int n) {
@@ -227,6 +231,11 @@ int upload_slot_consts(lins_ctx* ctx, SeqState& q, int n) {
   CK(cudaStreamSynchronize(ctx->stream));
   return LINS_OK;
 }
+
+}  // namespace lins_capi
+
+namespace {
+
 const lins_seq::Consts* slot_consts(const SeqState& q) { return reinterpret_cast<const lins_seq::Consts*>(q.slot_consts.p); }
 const lins_seq::InitConsts* slot_init_consts(const SeqState& q) { return reinterpret_cast<const lins_seq::InitConsts*>(q.slot_init_consts.p); }
 
@@ -305,6 +314,10 @@ void install_run(SeqState& q, int n, bool has_init) {
   q.n = n;
 }
 
+}  // namespace
+
+namespace lins_capi {
+
 // queue the upload of the host copies of map_off and stale (pageable: the caller synchronises before they change)
 cudaError_t queue_map_state(lins_ctx* ctx, SeqState& q) {
   const cudaError_t e = cudaMemcpyAsync(q.map_off.p, q.h_map_off.data(), sizeof(int) * q.h_map_off.size(), cudaMemcpyHostToDevice, ctx->stream);
@@ -346,6 +359,10 @@ void swap_maps(SeqState& q) {
   std::swap(q.map_s, q.nmap_s); std::swap(q.map_c, q.nmap_c); std::swap(q.tree_s, q.ntree_s); std::swap(q.tree_c, q.ntree_c);
   q.h_map_off.swap(q.h_nmap_off);
 }
+
+}  // namespace lins_capi
+
+namespace {
 
 // ---- a step ----------------------------------------------------------------------------------------------------------------
 // What every step entry checks before anything runs: the run, n_seq and n_scans (the number of scans d carries), the IMU

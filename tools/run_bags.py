@@ -1,6 +1,6 @@
 #!/usr/bin/env python
 """tools/run_bags.py BAG... [--slots S] [--lidar /velodyne_points] [--imu /imu/data] [--max-scans N] [--lidar-model M] [--map]
-                   [--config a.yaml[,b.yaml,...] [--tune]] [--out DIR]
+                   [--config a.yaml[,b.yaml,...] [--tune]] [--checkpoint-every N DIR] [--resume DIR] [--out DIR]
 
 Replays many ROS1 bags through sequence mode in lockstep (bag_replay.py): every bag is scheduled as tools/run_bag.py
 schedules one, the bags are queued through S slots, and each scan's sensor_msgs/PointCloud2 message is decoded on the
@@ -16,7 +16,10 @@ Each bag's slot is configured with its file's rig (scan period, feature threshol
 biases); the files must agree on the keys every slot shares (num_iter, icp_freq, nearest_feature_search_sq_dist,
 lidar_std, lidar_scale), which set the context's parameters.  With --tune as well, each bag's slot also takes its file's
 tuning (those shared keys) and imu_misalign_angle (lins_gpu_seq_tune: its IMU values are rotated into the vehicle frame as
-LinsFusion::imuCallback does), so the files may differ in any key; the first file's tuning sets the context's parameters."""
+LinsFusion::imuCallback does), so the files may differ in any key; the first file's tuning sets the context's parameters.
+--checkpoint-every N DIR writes a checkpoint of the replay into DIR after every N-th step (every occupied slot saved by
+lins_gpu_seq_save, and the driver's state); --resume DIR continues a replay of the same bags and options from the
+checkpoint in DIR, in a new context, with the outputs an uninterrupted replay would give."""
 import argparse, importlib, os, sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import numpy as np
@@ -93,9 +96,16 @@ def main(argv=None):
     ap.add_argument("--map", action="store_true", help="run each bag's mapping node on what its estimator publishes")
     ap.add_argument("--config", help="LINS config file(s): one for every bag, or one per bag: a.yaml,b.yaml,...")
     ap.add_argument("--tune", action="store_true", help="with --config: each bag also takes its file's tuning and IMU misalignment")
+    ap.add_argument("--checkpoint-every", nargs=2, metavar=("N", "DIR"), help="write a checkpoint into DIR after every N-th step")
+    ap.add_argument("--resume", metavar="DIR", help="continue from the checkpoint in DIR")
     ap.add_argument("--out")
     a = ap.parse_args(argv)
     try:
+        every, ck_dir = (None, None)
+        if a.checkpoint_every:
+            if not a.checkpoint_every[0].isdigit() or int(a.checkpoint_every[0]) < 1:
+                raise ValueError(f"--checkpoint-every: {a.checkpoint_every[0]!r} is not a step count >= 1")
+            every, ck_dir = int(a.checkpoint_every[0]), a.checkpoint_every[1]
         model = lidar_models(a.lidar_model, len(a.bags))
         if a.tune and not a.config:
             raise ValueError("--tune takes the tuning from the --config files")
@@ -109,7 +119,8 @@ def main(argv=None):
     br = importlib.import_module("lins---lidar-inertial-slam_b200.bag_replay")
     capi = importlib.import_module("lins---lidar-inertial-slam_b200.capi")
     recs = [br.Recording(p, a.lidar, a.imu, a.max_scans, config=c, tuning=t) for p, c, t in zip(a.bags, cfgs, tunes)]
-    outs = br.replay(recs, a.slots or len(recs), model=model, map=a.map, gpu=capi.LinsGpu(prm) if prm is not None else None)
+    outs = br.replay(recs, a.slots or len(recs), model=model, map=a.map, gpu=capi.LinsGpu(prm) if prm is not None else None,
+                     checkpoint=ck_dir, checkpoint_every=every, resume=a.resume)
     np.set_printoptions(precision=4, suppress=True)
     for p, o in zip(a.bags, outs):
         print(p, br.summary(o))

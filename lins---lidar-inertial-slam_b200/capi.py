@@ -527,27 +527,24 @@ class LinsGpu:
 
     def seq_restart(self, mask):
         """Put the slots with mask[s] != 0 back into the fresh state of seq_open (their next scan is a first scan)."""
-        m = np.ascontiguousarray(mask, dtype=np.uint8)
-        if len(m) != self._seq_n:
-            raise ValueError(f"mask has {len(m)} entries, the run {self._seq_n}")
-        self._ck(self.L.lins_gpu_seq_restart(self.h, ptr(m)))
+        self._ck(self.L.lins_gpu_seq_restart(self.h, ptr(self._slot_mask(mask))))
 
     def seq_configure(self, mask, configs):
         """Configure the slots with mask[s] != 0, each still fresh (no step since seq_open / its last seq_restart), with
         their own rig: configs is a LinsSlotConfig per slot (S entries; None where the mask is 0).  A restart returns a slot
         to the run's values."""
-        m = np.ascontiguousarray(mask, dtype=np.uint8)
-        if len(m) != self._seq_n or len(configs) != self._seq_n:
-            raise ValueError(f"mask / configs have {len(m)} / {len(configs)} entries, the run {self._seq_n}")
+        m = self._slot_mask(mask)
+        if len(configs) != self._seq_n:
+            raise ValueError(f"{len(configs)} configs, the run has {self._seq_n} slots")
         arr = (LinsSlotConfig * self._seq_n)(*[c if c is not None else LinsSlotConfig() for c in configs])
         self._ck(self.L.lins_gpu_seq_configure(self.h, ptr(m), C.cast(arr, C.c_void_p)))
 
     def seq_tune(self, mask, tunings):
         """Tune the slots with mask[s] != 0, each still fresh, with their own estimator tuning and IMU misalignment:
         tunings is a LinsSlotTuning per slot (S entries; None where the mask is 0).  A restart returns a slot to untuned."""
-        m = np.ascontiguousarray(mask, dtype=np.uint8)
-        if len(m) != self._seq_n or len(tunings) != self._seq_n:
-            raise ValueError(f"mask / tunings have {len(m)} / {len(tunings)} entries, the run {self._seq_n}")
+        m = self._slot_mask(mask)
+        if len(tunings) != self._seq_n:
+            raise ValueError(f"{len(tunings)} tunings, the run has {self._seq_n} slots")
         arr = (LinsSlotTuning * self._seq_n)(*[t if t is not None else LinsSlotTuning() for t in tunings])
         self._ck(self.L.lins_gpu_seq_tune(self.h, ptr(m), C.cast(arr, C.c_void_p)))
 

@@ -206,24 +206,71 @@ void init_consts_of(double* out, const lins_seq_params* prm, const lins_seq_init
 
 constexpr size_t kNConsts = sizeof(SeqState::consts) / sizeof(double), kNInit = sizeof(SeqState::init_consts) / sizeof(double);
 
+// Everything slot s reads: its config's and its tuning's values, else the run's open constants, the context's current
+// lins_params (lins_gpu_set_params can change them between steps) and the call's feature params fp (null: feat is not
+// filled).  Resolved again at every use, so an untuned slot follows the context.
+struct SlotParams {
+  double consts[kNConsts], init_consts[kNInit];  // lins_seq::Consts, InitConsts
+  double period;                                  // SCAN_PERIOD
+  FeatConsts feat;                                // the extraction of a _raw / _cloud2 step
+  lins_dev::UnitTuning tune;
+  double align[10];                               // alignIMUtoVehicle's R (row-major), then 1 = rotate the slot's IMU values
+};
+
+SlotParams slot_params(const lins_ctx* ctx, int s, const lins_feature_params* fp = nullptr) {
+  const SeqState& q = ctx->seq;
+  const SeqSlot& r = q.slot[s];
+  const lins_params& p = ctx->prm;
+  SlotParams o;
+  if (r.cfg) {
+    consts_of(o.consts, &r.cfg->filter);
+    init_consts_of(o.init_consts, &r.cfg->filter, &r.cfg->init);
+  } else {
+    std::copy(q.consts, q.consts + kNConsts, o.consts);
+    std::copy(q.init_consts, q.init_consts + kNInit, o.init_consts);
+  }
+  o.period = r.cfg ? r.cfg->scan_period : p.scan_period;
+  if (fp) o.feat = feat_consts(r.cfg ? r.cfg->features : *fp, o.period);
+  lins_dev::UnitTuning& t = o.tune;
+  if (r.tune) {
+    const lins_slot_tuning& u = r.tune->t;
+    t.num_iter = u.num_iter; t.icp_freq = u.icp_freq; t.nearest_sq = u.nearest_feature_search_sq_dist;
+    t.lidar_std = u.lidar_std; t.lidar_scale = u.lidar_scale;
+  } else {
+    t.num_iter = p.num_iter; t.icp_freq = p.icp_freq < 1 ? 1 : p.icp_freq; t.nearest_sq = p.nearest_feature_search_sq_dist;
+    t.lidar_std = p.lidar_std; t.lidar_scale = p.lidar_scale;
+  }
+  std::fill(o.align, o.align + 10, 0.0);
+  if (r.tune) { std::copy(r.tune->R, r.tune->R + 9, o.align); o.align[9] = 1.0; }
+  return o;
+}
+
 }  // namespace
 
 namespace lins_capi {
 
-// every slot's device constants: a configured slot's from its config, the others the run's; then a synchronisation (the
-// sources are pageable)
-int upload_slot_consts(lins_ctx* ctx, SeqState& q, int n) {
+int check_open_run(lins_ctx* ctx, const char* entry, bool args_ok) {
+  if (!ctx) return LINS_E_INVALID;
+  const std::string e(entry);
+  if (ctx->seq.n == 0) return fail(ctx, LINS_E_NOMAP, (e + ": no sequence run: call lins_gpu_seq_open").c_str());
+  if (!args_ok) return fail(ctx, LINS_E_INVALID, (e + ": null argument").c_str());
+  if (!ctx->seq.has_init) return fail(ctx, LINS_E_INVALID, (e + " needs a run opened by lins_gpu_seq_open").c_str());
+  return LINS_OK;
+}
+
+int check_fresh(lins_ctx* ctx, int s, const char* entry) {
+  if (ctx->seq.slot[s].fresh) return LINS_OK;
+  return fail(ctx, LINS_E_INVALID, (std::string(entry) + ": a masked slot is not fresh (no step since open / restart)").c_str());
+}
+
+// every slot's device constants; then a synchronisation (the sources are pageable)
+int upload_slot_consts(lins_ctx* ctx, int n) {
+  SeqState& q = ctx->seq;
   std::vector<double> k(kNConsts * n), ik(kNInit * n);
   for (int s = 0; s < n; ++s) {
-    double* ks = &k[kNConsts * s];
-    double* iks = &ik[kNInit * s];
-    if (q.configured[s]) {
-      consts_of(ks, &q.cfg[s].filter);
-      init_consts_of(iks, &q.cfg[s].filter, &q.cfg[s].init);
-    } else {
-      std::copy(q.consts, q.consts + kNConsts, ks);
-      std::copy(q.init_consts, q.init_consts + kNInit, iks);
-    }
+    const SlotParams p = slot_params(ctx, s);
+    std::copy(p.consts, p.consts + kNConsts, &k[kNConsts * s]);
+    std::copy(p.init_consts, p.init_consts + kNInit, &ik[kNInit * s]);
   }
   CK(q.slot_consts.reserve(k.size())); CK(q.slot_init_consts.reserve(ik.size()));
   CK(cudaMemcpyAsync(q.slot_consts.p, k.data(), sizeof(double) * k.size(), cudaMemcpyHostToDevice, ctx->stream));
@@ -239,12 +286,6 @@ namespace {
 const lins_seq::Consts* slot_consts(const SeqState& q) { return reinterpret_cast<const lins_seq::Consts*>(q.slot_consts.p); }
 const lins_seq::InitConsts* slot_init_consts(const SeqState& q) { return reinterpret_cast<const lins_seq::InitConsts*>(q.slot_init_consts.p); }
 
-// the SCAN_PERIOD slot s reads: its config's, else the context's
-double slot_period(const lins_ctx* ctx, int s) {
-  const SeqState& q = ctx->seq;
-  return q.configured[s] ? q.cfg[s].scan_period : ctx->prm.scan_period;
-}
-
 // alignIMUtoVehicle's R = rpy2R((0, 0, deg2rad(angle))) = Rz Ry Rx (math_utils.h:164-182), row-major, with the host's libm
 void misalign_R(double angle, double* R) {
   const double y = angle * M_PI / 180.0, p = 0.0, r = 0.0;  // math_utils::deg2rad of (0, 0, angle)
@@ -258,32 +299,6 @@ void misalign_R(double angle, double* R) {
   double T[9];
   mul(Rz, Ry, T);
   mul(T, Rx, R);
-}
-
-// the host side of a run's slot configuration and tuning: every slot unconfigured, untuned and fresh
-void reset_slot_configs(SeqState& q, int n) {
-  q.cfg.assign(n, lins_slot_config());
-  q.configured.assign(n, 0);
-  q.fresh.assign(n, 1);
-  q.tune.assign(n, lins_slot_tuning());
-  q.tuned.assign(n, 0);
-  q.align_R.assign(9 * (size_t)n, 0.0);
-}
-
-// the tuning slot s reads: its own, else the context's lins_params
-lins_dev::UnitTuning slot_tuning(const lins_ctx* ctx, int s) {
-  const SeqState& q = ctx->seq;
-  lins_dev::UnitTuning t;
-  if (q.tuned[s]) {
-    const lins_slot_tuning& u = q.tune[s];
-    t.num_iter = u.num_iter; t.icp_freq = u.icp_freq; t.nearest_sq = u.nearest_feature_search_sq_dist;
-    t.lidar_std = u.lidar_std; t.lidar_scale = u.lidar_scale;
-  } else {
-    const lins_params& p = ctx->prm;
-    t.num_iter = p.num_iter; t.icp_freq = p.icp_freq < 1 ? 1 : p.icp_freq; t.nearest_sq = p.nearest_feature_search_sq_dist;
-    t.lidar_std = p.lidar_std; t.lidar_scale = p.lidar_scale;
-  }
-  return t;
 }
 
 int launch_fresh(lins_ctx* ctx, SeqState& q, int n, const unsigned char* mask_dev) {
@@ -422,7 +437,7 @@ int seq_step_phases(lins_ctx* ctx, const lins_seq_step_desc* d, const int32_t* c
     const bool present = !d->present || d->present[s];
     const int nsl = offs[2][s + 1] - offs[2][s], ncl = offs[3][s + 1] - offs[3][s];
     const int32_t fs = q.fusion[s];
-    if (present) q.fresh[s] = 0;
+    if (present) q.slot[s].fresh = false;
     if (!present) status[s] = LINS_SEQ_IDLE;
     else if (fs == FUSION_RUNNING) status[s] = (ncl <= 5 || nsl <= 10) ? LINS_SEQ_SKIPPED : LINS_SEQ_RAN;  // :436-440
     else if (ncl < 10 || nsl < 100) status[s] = LINS_SEQ_INIT_WAIT;  // processFirstScan / processSecondScan (:331-336, :379-384)
@@ -475,7 +490,7 @@ int seq_step_phases(lins_ctx* ctx, const lins_seq_step_desc* d, const int32_t* c
   CK(q.status_d.reserve(3 * (size_t)n)); CK(q.h_status.reserve(3 * (size_t)n));
   CK(q.period.reserve(n)); CK(q.h_period.reserve(n));
   CK(q.unit_tune.reserve(n)); CK(q.h_unit_tune.reserve(n));
-  const bool any_tuned = std::find(q.tuned.begin(), q.tuned.end(), 1) != q.tuned.end();
+  const bool any_tuned = std::any_of(q.slot.begin(), q.slot.end(), [](const SeqSlot& x) { return x.tune.has_value(); });
   const bool align = any_tuned && (n_imu || n_init);  // (a run without a tuned slot launches what it launched before)
   if (align) { CK(q.align.reserve(10 * (size_t)n)); CK(q.h_align.reserve(10 * (size_t)n)); }
   const int n_copies = (int)copies.size();
@@ -489,13 +504,11 @@ int seq_step_phases(lins_ctx* ctx, const lins_seq_step_desc* d, const int32_t* c
   if (d->imu_off) std::memcpy(q.h_imu_off.p, d->imu_off, sizeof(int) * N1);
   else std::memset(q.h_imu_off.p, 0, sizeof(int) * N1);
   if (n_imu) std::memcpy(q.h_imu.p, d->imu, sizeof(double) * 7 * n_imu);
-  for (int s = 0; s < n; ++s) { q.h_status.p[s] = (unsigned char)status[s]; q.h_status.p[2 * n + s] = imu_use[s]; q.h_period.p[s] = slot_period(ctx, s); q.h_unit_tune.p[s] = slot_tuning(ctx, s); }
-  if (align)
-    for (int s = 0; s < n; ++s) {
-      double* a = q.h_align.p + 10 * (size_t)s;
-      std::copy(q.align_R.begin() + 9 * (size_t)s, q.align_R.begin() + 9 * (size_t)s + 9, a);
-      a[9] = q.tuned[s] ? 1.0 : 0.0;
-    }
+  for (int s = 0; s < n; ++s) {
+    const SlotParams p = slot_params(ctx, s);
+    q.h_status.p[s] = (unsigned char)status[s]; q.h_status.p[2 * n + s] = imu_use[s]; q.h_period.p[s] = p.period; q.h_unit_tune.p[s] = p.tune;
+    if (align) std::copy(p.align, p.align + 10, q.h_align.p + 10 * (size_t)s);
+  }
   std::memcpy(r.h_off.p, run_off.data(), sizeof(int) * 2 * N1);
   std::memcpy(r.h_off.p + 2 * N1, init_off.data(), sizeof(int) * 2 * N1);
   if (n_imu) CK(cudaMemcpyAsync(q.imu.p, q.h_imu.p, sizeof(double) * 7 * n_imu, cudaMemcpyHostToDevice, ctx->stream));
@@ -719,8 +732,8 @@ int step_from_projection(lins_ctx* ctx, const uint8_t* pres, const double* imu, 
   in.n = n; in.line_num = line_num; in.total = src_off[n];
   in.pts = pr.seg.p; in.off = pr.up.qs_off.p; in.count = pr.counts.p; in.count_stride = 2;
   in.ground = pr.ground.p; in.col = pr.col.p; in.range = pr.range.p; in.ring = pr.ring.p; in.ori = pr.ori.p;
-  std::vector<FeatConsts> k(n);  // each slot's config, else the call's fp and the context's period
-  for (int s = 0; s < n; ++s) k[s] = feat_consts(q.configured[s] ? q.cfg[s].features : *fp, slot_period(ctx, s));
+  std::vector<FeatConsts> k(n);
+  for (int s = 0; s < n; ++s) k[s] = slot_params(ctx, s, fp).feat;
   int rc = features_launch(ctx, k.data(), in);
   if (rc != LINS_OK) return rc;
   if (pb.bound) {  // the stash: every slot's outlier cloud, device to device (an absent slot's sweep projected empty)
@@ -749,13 +762,6 @@ bool publishes(int32_t status, int32_t fusion_before) {
 // updatePointCloud ran: the scan was accepted (SECOND / RAN / ICP)
 bool accepted(int32_t status) { return status == LINS_SEQ_SECOND || status == LINS_SEQ_RAN || status == LINS_SEQ_ICP; }
 
-// the state of a slot whose estimator is new: no YZX clouds, globalStateYZX_ the identity
-void pub_fresh(SeqPubState& pb, int s) {
-  pb.yzx[s] = 0;
-  static const double id[7] = {0, 0, 0, 0, 0, 0, 1};
-  std::copy(id, id + 7, &pb.pose[7 * (size_t)s]);
-}
-
 // lins_gpu_seq_map_step on a checked call: the estimator side (outlier stash and generation, YZX flags, poses) is
 // committed, then one lockstep mapper step of the publishing slots on the device clouds
 int seq_map_run(lins_ctx* ctx, const lins_seq_map_desc* d, lins_mapper_report* reps, uint8_t* published) {
@@ -778,18 +784,19 @@ int seq_map_run(lins_ctx* ctx, const lins_seq_map_desc* d, lins_mapper_report* r
   // updatePointCloud of the accepted scans (their YZX clouds and pose); processFirstScan's fresh scan_last_
   for (int s = 0; s < n; ++s) {
     const int32_t st = q.status[s];
-    if (st == LINS_SEQ_FIRST) pb.yzx[s] = 0;
+    SeqSlot& r = q.slot[s];
+    if (st == LINS_SEQ_FIRST) r.yzx = false;
     if (!accepted(st)) continue;
-    pb.yzx[s] = 1;
+    r.yzx = true;
     const double* g = pb.h_glob.p + 20 * (size_t)s;  // rn = g[0..2], qbn = g[6..9]
-    lins::global_state_yzx(g, g + 6, &pb.pose[7 * (size_t)s], &pb.pose[7 * (size_t)s + 3]);
+    lins::global_state_yzx(g, g + 6, r.pose, r.pose + 3);
   }
   // the next outlier generation: an accepted scan's outliers, a slot without YZX clouds none, else the kept ones
   const int N1 = n + 1;
   pb.h_noutl_off.assign(N1, 0);
   std::vector<MapPiece> next(n);
   for (int s = 0; s < n; ++s) {
-    if (!pb.yzx[s]) next[s] = MapPiece{};
+    if (!q.slot[s].yzx) next[s] = MapPiece{};
     else if (accepted(q.status[s])) next[s] = MapPiece{pb.stash.p + pb.h_stash_off[s], pb.h_stash_off[s + 1] - pb.h_stash_off[s]};
     else next[s] = MapPiece{pb.outl.p + pb.h_outl_off[s], pb.h_outl_off[s + 1] - pb.h_outl_off[s]};
     pb.h_noutl_off[s + 1] = pb.h_noutl_off[s] + next[s].len;
@@ -812,19 +819,20 @@ int seq_map_run(lins_ctx* ctx, const lins_seq_map_desc* d, lins_mapper_report* r
   std::vector<double> quat(4 * (size_t)n), pos(3 * (size_t)n);
   for (int s = 0; s < n; ++s) {
     if (!pub[s]) continue;
-    if (pb.yzx[s]) {
+    const SeqSlot& r = q.slot[s];
+    if (r.yzx) {
       dev[3 * s + 0] = current_piece(q, 1, s);
       dev[3 * s + 1] = current_piece(q, 0, s);
       dev[3 * s + 2] = MapPiece{pb.outl.p + pb.h_outl_off[s], pb.h_outl_off[s + 1] - pb.h_outl_off[s]};
     }
-    std::copy(&pb.pose[7 * (size_t)s], &pb.pose[7 * (size_t)s] + 3, &pos[3 * (size_t)s]);
-    std::copy(&pb.pose[7 * (size_t)s] + 3, &pb.pose[7 * (size_t)s] + 7, &quat[4 * (size_t)s]);
+    std::copy(r.pose, r.pose + 3, &pos[3 * (size_t)s]);
+    std::copy(r.pose + 3, r.pose + 7, &quat[4 * (size_t)s]);
   }
   lins_mappers_desc md;
   std::memset(&md, 0, sizeof(md));
   md.n_slots = n; md.present = pub.data(); md.time = d->time; md.quat = quat.data(); md.pos = pos.data();
   std::vector<double> period(n);
-  for (int s = 0; s < n; ++s) period[s] = slot_period(ctx, s);
+  for (int s = 0; s < n; ++s) period[s] = slot_params(ctx, s).period;
   return mappers_step(ctx, ctx->mappers, &md, reps, dev.data(), period.data());
 }
 
@@ -873,8 +881,8 @@ int lins_gpu_seq_begin(lins_ctx* ctx, const lins_seq_params* prm, const lins_seq
   CK(cudaStreamSynchronize(ctx->stream));  // (the sources above are pageable host memory)
   consts_of(q.consts, prm);
   std::fill(q.init_consts, q.init_consts + kNInit, 0.0);  // (a hand-over does not initialise)
-  reset_slot_configs(q, n);
-  if ((rc = upload_slot_consts(ctx, q, n)) != LINS_OK) return rc;
+  q.slot.assign(n, SeqSlot());
+  if ((rc = upload_slot_consts(ctx, n)) != LINS_OK) return rc;
   // result records / reports read as zero until a step has run a sequence's IESKF
   CK(cudaMemsetAsync(q.run.results.p, 0, sizeof(lins_scan_result) * n, ctx->stream));
   CK(cudaMemsetAsync(q.run.reports.p, 0, sizeof(lins_report) * n, ctx->stream));
@@ -895,8 +903,8 @@ int lins_gpu_seq_open(lins_ctx* ctx, const lins_seq_params* prm, const lins_seq_
   CK(q.pre.reserve((size_t)n * 20)); CK(q.init_icp.reserve(icp_state_bytes() * n));
   consts_of(q.consts, prm);
   init_consts_of(q.init_consts, prm, ip);
-  reset_slot_configs(q, n);
-  if ((rc = upload_slot_consts(ctx, q, n)) != LINS_OK) return rc;
+  q.slot.assign(n, SeqSlot());
+  if ((rc = upload_slot_consts(ctx, n)) != LINS_OK) return rc;
   q.h_map_off.assign(4 * (size_t)(n + 1), 0);
   q.h_stale_v.assign(n, 0);
   CK(cudaMemsetAsync(q.lin.p, 0, sizeof(double) * 20 * (size_t)n, ctx->stream));
@@ -915,11 +923,9 @@ int lins_gpu_seq_open(lins_ctx* ctx, const lins_seq_params* prm, const lins_seq_
 }
 
 int lins_gpu_seq_restart(lins_ctx* ctx, const uint8_t* mask) {
-  if (!ctx) return LINS_E_INVALID;
+  int rc = check_open_run(ctx, "lins_gpu_seq_restart", mask != nullptr);
+  if (rc != LINS_OK) return rc;
   SeqState& q = ctx->seq;
-  if (q.n == 0) return fail(ctx, LINS_E_NOMAP, "no sequence run: call lins_gpu_seq_open");
-  if (!mask) return fail(ctx, LINS_E_INVALID, "null restart mask");
-  if (!q.has_init) return fail(ctx, LINS_E_INVALID, "lins_gpu_seq_restart needs a run opened by lins_gpu_seq_open");
   CK(cudaSetDevice(ctx->device));
   const int n = q.n;
   // the restarted slots' maps go: the other slots' ranges are copied into the next generation, which is swapped in
@@ -927,16 +933,17 @@ int lins_gpu_seq_restart(lins_ctx* ctx, const uint8_t* mask) {
   for (int s = 0; s < n; ++s)
     if (!mask[s]) for (int c = 0; c < 4; ++c) next[4 * (size_t)s + c] = current_piece(q, c, s);
   std::vector<DevCopy> copies;
-  int rc = build_next_maps(ctx, q, next, copies);
+  rc = build_next_maps(ctx, q, next, copies);
   if (rc == LINS_OK) rc = q.copies.reserve(ctx, copies.size());
   if (rc != LINS_OK) return rc;
   CK(q.status_d.reserve(3 * (size_t)n)); CK(q.h_status.reserve(3 * (size_t)n));
   // (the last step ended with a stream synchronisation: the pinned staging is free)
-  // the restarted slots are unconfigured again: their constants go back to the run's before the fresh state reads them
+  // the restarted slots are new slots: unconfigured (their constants go back to the run's before the fresh state reads
+  // them), untuned (the next step's tables read the context's), fresh, without YZX clouds
   bool any_configured = false;
-  for (int s = 0; s < n; ++s) if (mask[s] && q.configured[s]) { q.configured[s] = 0; any_configured = true; }
-  if (any_configured && (rc = upload_slot_consts(ctx, q, n)) != LINS_OK) { q.n = 0; return rc; }
-  for (int s = 0; s < n; ++s) if (mask[s]) q.tuned[s] = 0;  // (and untuned: the next step's tables read the context's)
+  for (int s = 0; s < n; ++s)
+    if (mask[s]) { any_configured |= q.slot[s].cfg.has_value(); q.slot[s] = SeqSlot(); }
+  if (any_configured && (rc = upload_slot_consts(ctx, n)) != LINS_OK) { q.n = 0; return rc; }
   if ((rc = q.copies.stage(ctx, copies.data(), (int)copies.size(), 0)) != LINS_OK) return rc;
   for (int s = 0; s < n; ++s) q.h_status.p[s] = mask[s] ? 1 : 0;
   CK(cudaMemcpyAsync(q.status_d.p, q.h_status.p, n, cudaMemcpyHostToDevice, ctx->stream));
@@ -945,43 +952,31 @@ int lins_gpu_seq_restart(lins_ctx* ctx, const uint8_t* mask) {
   if (rc != LINS_OK) { q.n = 0; return rc; }  // (some slots may have changed: the run ends, as after a failed step)
   swap_maps(q);
   for (int s = 0; s < n; ++s)
-    if (mask[s]) { q.h_stale_v[s] = 0; q.fusion[s] = FUSION_INIT; q.status[s] = LINS_SEQ_IDLE; q.fresh[s] = 1; }
-  if (q.pub.bound) {  // a new recording is a new LinsFusion with a new mapping node
-    for (int s = 0; s < n; ++s) if (mask[s]) pub_fresh(q.pub, s);
-    if ((rc = mappers_reset(ctx, ctx->mappers, mask)) != LINS_OK) return rc;
-  }
+    if (mask[s]) { q.h_stale_v[s] = 0; q.fusion[s] = FUSION_INIT; q.status[s] = LINS_SEQ_IDLE; }
+  // a new recording is a new LinsFusion with a new mapping node
+  if (q.pub.bound && (rc = mappers_reset(ctx, ctx->mappers, mask)) != LINS_OK) return rc;
   CK(queue_map_state(ctx, q));
   CK(cudaStreamSynchronize(ctx->stream));  // (the two sources above are pageable)
   return LINS_OK;
 }
 
 int lins_gpu_seq_configure(lins_ctx* ctx, const uint8_t* mask, const lins_slot_config* cfg) {
-  if (!ctx) return LINS_E_INVALID;
+  const char* entry = "lins_gpu_seq_configure";
+  int rc = check_open_run(ctx, entry, mask && cfg);
+  if (rc != LINS_OK) return rc;
   SeqState& q = ctx->seq;
-  if (q.n == 0) return fail(ctx, LINS_E_NOMAP, "no sequence run: call lins_gpu_seq_open");
-  if (!mask || !cfg) return fail(ctx, LINS_E_INVALID, "null configure mask / configs");
-  if (!q.has_init) return fail(ctx, LINS_E_INVALID, "lins_gpu_seq_configure needs a run opened by lins_gpu_seq_open");
   const int n = q.n;
   for (int s = 0; s < n; ++s) {
     if (!mask[s]) continue;
-    if (!q.fresh[s]) return fail(ctx, LINS_E_INVALID, "a configured slot must be fresh (no step since open / restart)");
-    const lins_slot_config& c = cfg[s];
-    const lins_seq_params& f = c.filter;
-    const lins_seq_init_params& i = c.init;
-    bool ok = std::isfinite(c.scan_period) && c.scan_period > 0 && std::isfinite(c.features.edge_threshold) &&
-              std::isfinite(c.features.surf_threshold) && std::isfinite(c.features.imu_lidar_extrinsic_angle);
-    auto nonneg = [&](const double* v, int m) { for (int k = 0; k < m; ++k) ok = ok && std::isfinite(v[k]) && v[k] >= 0; };
-    auto finite = [&](const double* v, int m) { for (int k = 0; k < m; ++k) ok = ok && std::isfinite(v[k]); };
-    nonneg(f.noise, 4); nonneg(f.init_pos_std, 3); nonneg(f.init_att_std, 3);
-    nonneg(i.init_vel_std, 3); nonneg(i.init_acc_std, 3); nonneg(i.init_gyr_std, 3);
-    finite(i.init_ba, 3); finite(i.init_bw, 3);
-    if (!ok) return fail(ctx, LINS_E_INVALID, "bad slot config (non-finite value, scan_period <= 0, or a negative noise / std)");
+    if ((rc = check_fresh(ctx, s, entry)) != LINS_OK) return rc;
+    if (!lins_blob::config_ok(cfg[s]))
+      return fail(ctx, LINS_E_INVALID, "lins_gpu_seq_configure: bad slot config (non-finite value, scan_period <= 0, or a negative noise / std)");
   }
   CK(cudaSetDevice(ctx->device));
   CK(q.status_d.reserve(3 * (size_t)n)); CK(q.h_status.reserve(3 * (size_t)n));
   // from here on the slots change: a failure ends the run, as a failed restart does
-  for (int s = 0; s < n; ++s) if (mask[s]) { q.cfg[s] = cfg[s]; q.configured[s] = 1; }
-  int rc = upload_slot_consts(ctx, q, n);
+  for (int s = 0; s < n; ++s) if (mask[s]) q.slot[s].cfg = cfg[s];
+  rc = upload_slot_consts(ctx, n);
   if (rc == LINS_OK) {
     for (int s = 0; s < n; ++s) q.h_status.p[s] = mask[s] ? 1 : 0;
     if (cudaMemcpyAsync(q.status_d.p, q.h_status.p, n, cudaMemcpyHostToDevice, ctx->stream) != cudaSuccess) rc = fail(ctx, LINS_E_CUDA, "configure mask upload");
@@ -993,26 +988,23 @@ int lins_gpu_seq_configure(lins_ctx* ctx, const uint8_t* mask, const lins_slot_c
 }
 
 int lins_gpu_seq_tune(lins_ctx* ctx, const uint8_t* mask, const lins_slot_tuning* t) {
-  if (!ctx) return LINS_E_INVALID;
+  const char* entry = "lins_gpu_seq_tune";
+  int rc = check_open_run(ctx, entry, mask && t);
+  if (rc != LINS_OK) return rc;
   SeqState& q = ctx->seq;
-  if (q.n == 0) return fail(ctx, LINS_E_NOMAP, "no sequence run: call lins_gpu_seq_open");
-  if (!mask || !t) return fail(ctx, LINS_E_INVALID, "null tune mask / tunings");
-  if (!q.has_init) return fail(ctx, LINS_E_INVALID, "lins_gpu_seq_tune needs a run opened by lins_gpu_seq_open");
   const int n = q.n;
   for (int s = 0; s < n; ++s) {
     if (!mask[s]) continue;
-    if (!q.fresh[s]) return fail(ctx, LINS_E_INVALID, "a tuned slot must be fresh (no step since open / restart)");
-    const lins_slot_tuning& u = t[s];
-    const bool ok = u.num_iter >= 0 && u.num_iter <= LINS_MAX_ITER && u.icp_freq >= 1 && std::isfinite(u.nearest_feature_search_sq_dist) &&
-                    std::isfinite(u.lidar_std) && std::isfinite(u.lidar_scale) && std::isfinite(u.imu_misalign_angle);
-    if (!ok) return fail(ctx, LINS_E_INVALID, "bad slot tuning (num_iter outside 0..LINS_MAX_ITER, icp_freq < 1, or a non-finite value)");
+    if ((rc = check_fresh(ctx, s, entry)) != LINS_OK) return rc;
+    if (!lins_blob::tuning_ok(t[s]))
+      return fail(ctx, LINS_E_INVALID, "lins_gpu_seq_tune: bad slot tuning (num_iter outside 0..LINS_MAX_ITER, icp_freq < 1, or a non-finite value)");
   }
   // (host state only: the step uploads the tables)
   for (int s = 0; s < n; ++s)
     if (mask[s]) {
-      q.tune[s] = t[s];
-      q.tuned[s] = 1;
-      misalign_R(t[s].imu_misalign_angle, &q.align_R[9 * (size_t)s]);
+      SeqSlot::Tuning u{t[s], {}};
+      misalign_R(t[s].imu_misalign_angle, u.R);
+      q.slot[s].tune = u;
     }
   return LINS_OK;
 }
@@ -1036,7 +1028,7 @@ int lins_gpu_seq_step_pcl(lins_ctx* ctx, const lins_seq_pcl_desc* d, const lins_
   if (rc != LINS_OK) return rc;
   // extraction, validation of the scans and the counts' read-back: nothing of the sequences has changed yet
   std::vector<double> period(ctx->seq.n);  // (the re-stamp: each slot's period; the thresholds and extrinsic are fp's)
-  for (int s = 0; s < ctx->seq.n; ++s) period[s] = slot_period(ctx, s);
+  for (int s = 0; s < ctx->seq.n; ++s) period[s] = slot_params(ctx, s).period;
   rc = features_run(ctx, fp, &d->pcl, period.data());
   if (rc != LINS_OK) return rc;
   return step_from_features(ctx, d->present, d->imu, d->imu_off, d->pcl.cloud_off, scan_imu);
@@ -1084,20 +1076,18 @@ int lins_gpu_seq_step_cloud2(lins_ctx* ctx, const lins_seq_cloud2_desc* d, const
 }
 
 int lins_gpu_seq_map_open(lins_ctx* ctx) {
-  if (!ctx) return LINS_E_INVALID;
+  int rc = check_open_run(ctx, "lins_gpu_seq_map_open", true);
+  if (rc != LINS_OK) return rc;
   SeqState& q = ctx->seq;
-  if (q.n == 0) return fail(ctx, LINS_E_NOMAP, "no sequence run: call lins_gpu_seq_open");
-  if (!q.has_init) return fail(ctx, LINS_E_INVALID, "lins_gpu_seq_map_open needs a run opened by lins_gpu_seq_open");
   if (q.has_step) return fail(ctx, LINS_E_INVALID, "lins_gpu_seq_map_open after the run's first step");
   const int n = q.n;
   SeqPubState& pb = q.pub;
   CK(cudaSetDevice(ctx->device));
   CK(pb.h_glob.reserve(20 * (size_t)n)); CK(pb.h_proj_counts.reserve(2 * (size_t)n)); CK(pb.outl.reserve(1));
-  int rc = mappers_open(ctx, ctx->mappers, n);
+  rc = mappers_open(ctx, ctx->mappers, n);
   if (rc != LINS_OK) return rc;
-  pb.yzx.assign(n, 0);
-  pb.pose.assign(7 * (size_t)n, 0.0);
-  for (int s = 0; s < n; ++s) pub_fresh(pb, s);
+  const SeqSlot fresh;  // every estimator is new: no YZX clouds, globalStateYZX_ the identity
+  for (SeqSlot& r : q.slot) { r.yzx = fresh.yzx; std::copy(fresh.pose, fresh.pose + 7, r.pose); }
   pb.h_outl_off.assign((size_t)n + 1, 0);
   pb.fusion_before.assign(n, FUSION_INIT);
   pb.pending = false;
@@ -1129,9 +1119,10 @@ int lins_gpu_seq_map_published(lins_ctx* ctx, double* pose, int32_t* sizes) {
   SeqState& q = ctx->seq;
   if (q.n == 0 || !q.pub.bound) return fail(ctx, LINS_E_NOMAP, "no sequence run bound by lins_gpu_seq_map_open");
   const SeqPubState& pb = q.pub;
-  if (pose) std::copy(pb.pose.begin(), pb.pose.end(), pose);
-  for (int s = 0; s < q.n && sizes; ++s) {
-    const bool y = pb.yzx[s];
+  for (int s = 0; s < q.n; ++s) {
+    const bool y = q.slot[s].yzx;
+    if (pose) std::copy(q.slot[s].pose, q.slot[s].pose + 7, pose + 7 * (size_t)s);
+    if (!sizes) continue;
     sizes[3 * s + 0] = y ? current_piece(q, 1, s).len : 0;
     sizes[3 * s + 1] = y ? current_piece(q, 0, s).len : 0;
     sizes[3 * s + 2] = y ? pb.h_outl_off[s + 1] - pb.h_outl_off[s] : 0;

@@ -59,14 +59,12 @@ B::Counts slot_counts(const lins_ctx* ctx, int s) {
   return c;
 }
 
-// what save_size and save check: a lins_gpu_seq_open run, a mask, no pending publish
-int check_run(lins_ctx* ctx, const uint8_t* mask) {
-  if (!ctx) return LINS_E_INVALID;
-  const SeqState& q = ctx->seq;
-  if (q.n == 0) return fail(ctx, LINS_E_NOMAP, "no sequence run: call lins_gpu_seq_open");
-  if (!q.has_init) return fail(ctx, LINS_E_INVALID, "saving and loading slots needs a run opened by lins_gpu_seq_open");
+// what save_size, save and load check: a lins_gpu_seq_open run, a mask, no pending publish
+int check_run(lins_ctx* ctx, const uint8_t* mask, const char* entry) {
+  const int rc = check_open_run(ctx, entry, true);
+  if (rc != LINS_OK) return rc;
   if (!mask) return fail(ctx, LINS_E_INVALID, "null mask");
-  if (q.pub.bound && q.pub.pending) return fail(ctx, LINS_E_INVALID, "the last step's lins_gpu_seq_map_step has not run");
+  if (ctx->seq.pub.bound && ctx->seq.pub.pending) return fail(ctx, LINS_E_INVALID, "the last step's lins_gpu_seq_map_step has not run");
   return LINS_OK;
 }
 
@@ -111,9 +109,10 @@ void save_copies(lins_ctx* ctx, int s, const B::Header& h, float4* dst, const st
 // the host records of slot s's blob into img (its first byte in the pinned image)
 void save_host(lins_ctx* ctx, int s, const B::Counts& c, B::Header h, uint8_t* img, const std::vector<std::pair<int, int>>& kf) {
   const SeqState& q = ctx->seq;
+  const SeqSlot& r = q.slot[s];
   h.magic = B::kMagic;
   h.version = B::kVersion;
-  h.flags = (q.pub.bound ? B::kBound : 0u) | (q.configured[s] ? B::kConfigured : 0u) | (q.tuned[s] ? B::kTuned : 0u);
+  h.flags = (q.pub.bound ? B::kBound : 0u) | (r.cfg ? B::kConfigured : 0u) | (r.tune ? B::kTuned : 0u);
   h.sizes = build_sizes();
   h.n_sections = B::kNumSections;
   put(img, &h, sizeof(h));
@@ -125,29 +124,15 @@ void save_host(lins_ctx* ctx, int s, const B::Counts& c, B::Header h, uint8_t* i
   sc.n_outlier = (int32_t)c.n_outlier; sc.n_poses = (int32_t)c.n_poses; sc.n_window = (int32_t)c.n_window; sc.n_keyframes = (int32_t)c.n_keyframes;
   std::copy(q.consts, q.consts + 10, sc.consts);
   std::copy(q.init_consts, q.init_consts + 24, sc.init_consts);
-  if (q.configured[s]) sc.cfg = q.cfg[s];
-  if (q.tuned[s]) { sc.tune = q.tune[s]; std::copy(&q.align_R[9 * (size_t)s], &q.align_R[9 * (size_t)s] + 9, sc.align_R); }
-  if (q.pub.bound) { sc.yzx = q.pub.yzx[s]; std::copy(&q.pub.pose[7 * (size_t)s], &q.pub.pose[7 * (size_t)s] + 7, sc.pose); }
+  if (r.cfg) sc.cfg = *r.cfg;
+  if (r.tune) { sc.tune = r.tune->t; std::copy(r.tune->R, r.tune->R + 9, sc.align_R); }
+  if (q.pub.bound) { sc.yzx = r.yzx; std::copy(r.pose, r.pose + 7, sc.pose); }
   put(img + h.sec[B::kScalars].off, &sc, sizeof(sc));
   if (!q.pub.bound) return;
   const MapperNode& m = ctx->mappers.node[s];
-  const MapperScalars& ms = m.s;
-  B::MapperRec r;
-  std::memset(&r, 0, sizeof(r));
-  std::copy(ms.transformLast, ms.transformLast + 6, r.transformLast); std::copy(ms.transformSum, ms.transformSum + 6, r.transformSum);
-  std::copy(ms.transformIncre, ms.transformIncre + 6, r.transformIncre);
-  std::copy(ms.transformTobeMapped, ms.transformTobeMapped + 6, r.transformTobeMapped);
-  std::copy(ms.transformBefMapped, ms.transformBefMapped + 6, r.transformBefMapped);
-  std::copy(ms.transformAftMapped, ms.transformAftMapped + 6, r.transformAftMapped);
-  std::copy(ms.imuTime, ms.imuTime + LINS_MAPPER_IMU_QUEUE, r.imuTime);
-  std::copy(ms.imuRoll, ms.imuRoll + LINS_MAPPER_IMU_QUEUE, r.imuRoll); std::copy(ms.imuPitch, ms.imuPitch + LINS_MAPPER_IMU_QUEUE, r.imuPitch);
-  r.imuPointerFront = ms.imuPointerFront; r.imuPointerLast = ms.imuPointerLast;
-  r.timeLastProcessing = ms.timeLastProcessing;
-  r.latestFrameID = ms.latestFrameID;
-  std::copy(ms.previousRobotPos, ms.previousRobotPos + 3, r.previousRobotPos);
-  put(img + h.sec[B::kMapper].off, &r, sizeof(r));
+  put(img + h.sec[B::kMapper].off, static_cast<const B::MapperRec*>(&m.s), sizeof(B::MapperRec));
   put(img + h.sec[B::kPoses].off, m.poses.data(), sizeof(B::PoseRec) * m.poses.size());
-  const std::vector<int32_t> win(ms.window.begin(), ms.window.end());
+  const std::vector<int32_t> win(m.s.window.begin(), m.s.window.end());
   put(img + h.sec[B::kWindow].off, win.data(), sizeof(int32_t) * win.size());
   std::vector<B::KeyframeRec> tab;
   for (const auto& k : kf) {
@@ -273,42 +258,30 @@ int load_run(lins_ctx* ctx, const uint8_t* mask, const std::vector<B::View>& v) 
     q.h_stale_v[s] = (unsigned char)sc.stale;
     q.fusion[s] = sc.fusion;
     q.status[s] = LINS_SEQ_IDLE;
-    q.fresh[s] = 0;
-    // the device constants are uploaded again when the slot is configured now or was before (a fresh slot can have been
-    // configured: an unconfigured blob then takes the run's constants back, as lins_gpu_seq_restart does)
-    any_configured |= q.configured[s] != 0;
-    q.configured[s] = (b.h.flags & B::kConfigured) ? 1 : 0;
-    q.cfg[s] = q.configured[s] ? sc.cfg : lins_slot_config();
-    any_configured |= q.configured[s] != 0;
-    q.tuned[s] = (b.h.flags & B::kTuned) ? 1 : 0;
-    q.tune[s] = q.tuned[s] ? sc.tune : lins_slot_tuning();
-    std::copy(sc.align_R, sc.align_R + 9, &q.align_R[9 * (size_t)s]);
+    // the slot's record is the blob's.  The device constants are uploaded again when the slot is configured now or was
+    // before (a fresh slot can have been configured: an unconfigured blob then takes the run's constants back, as
+    // lins_gpu_seq_restart does)
+    SeqSlot& r = q.slot[s];
+    any_configured |= r.cfg.has_value();
+    r = SeqSlot();
+    r.fresh = false;
+    if (b.h.flags & B::kConfigured) r.cfg = sc.cfg;
+    if (b.h.flags & B::kTuned) { r.tune = SeqSlot::Tuning{sc.tune, {}}; std::copy(sc.align_R, sc.align_R + 9, r.tune->R); }
+    any_configured |= r.cfg.has_value();
     if (!pb.bound) continue;
-    pb.yzx[s] = (unsigned char)sc.yzx;
-    std::copy(sc.pose, sc.pose + 7, &pb.pose[7 * (size_t)s]);
+    r.yzx = sc.yzx != 0;
+    std::copy(sc.pose, sc.pose + 7, r.pose);
     MapperNode& m = ms.node[s];
-    MapperScalars& t = m.s;
-    const B::MapperRec& r = b.m;
-    std::copy(r.transformLast, r.transformLast + 6, t.transformLast); std::copy(r.transformSum, r.transformSum + 6, t.transformSum);
-    std::copy(r.transformIncre, r.transformIncre + 6, t.transformIncre);
-    std::copy(r.transformTobeMapped, r.transformTobeMapped + 6, t.transformTobeMapped);
-    std::copy(r.transformBefMapped, r.transformBefMapped + 6, t.transformBefMapped);
-    std::copy(r.transformAftMapped, r.transformAftMapped + 6, t.transformAftMapped);
-    std::copy(r.imuTime, r.imuTime + LINS_MAPPER_IMU_QUEUE, t.imuTime);
-    std::copy(r.imuRoll, r.imuRoll + LINS_MAPPER_IMU_QUEUE, t.imuRoll); std::copy(r.imuPitch, r.imuPitch + LINS_MAPPER_IMU_QUEUE, t.imuPitch);
-    t.imuPointerFront = r.imuPointerFront; t.imuPointerLast = r.imuPointerLast;
-    t.timeLastProcessing = r.timeLastProcessing;
-    t.latestFrameID = r.latestFrameID;
-    std::copy(r.previousRobotPos, r.previousRobotPos + 3, t.previousRobotPos);
-    t.window.clear();
-    for (int i = 0; i < sc.n_window; ++i) t.window.push_back(b.window(i));
+    static_cast<B::MapperRec&>(m.s) = b.m;
+    m.s.window.clear();
+    for (int i = 0; i < sc.n_window; ++i) m.s.window.push_back(b.window(i));
     m.poses.resize(sc.n_poses);
     for (int i = 0; i < sc.n_poses; ++i) { const B::PoseRec p = b.pose(i); std::memcpy(&m.poses[i], &p, sizeof(p)); }
     m.last = MapperLast();  // (no DS clouds until the slot's next processed cycle)
   }
   CK(queue_map_state(ctx, q));
   // (upload_slot_consts ends with a synchronisation; the sources above are pageable)
-  if (any_configured) return upload_slot_consts(ctx, q, n);
+  if (any_configured) return upload_slot_consts(ctx, n);
   CK(cudaStreamSynchronize(ctx->stream));
   return LINS_OK;
 }
@@ -318,7 +291,7 @@ int load_run(lins_ctx* ctx, const uint8_t* mask, const std::vector<B::View>& v) 
 extern "C" {
 
 int lins_gpu_seq_save_size(lins_ctx* ctx, const uint8_t* mask, uint64_t* off) {
-  const int rc = check_run(ctx, mask);
+  const int rc = check_run(ctx, mask, "lins_gpu_seq_save_size");
   if (rc != LINS_OK) return rc;
   if (!off) return fail(ctx, LINS_E_INVALID, "null offsets");
   offsets(ctx, mask, off);
@@ -326,7 +299,7 @@ int lins_gpu_seq_save_size(lins_ctx* ctx, const uint8_t* mask, uint64_t* off) {
 }
 
 int lins_gpu_seq_save(lins_ctx* ctx, const uint8_t* mask, void* blob, const uint64_t* off) {
-  int rc = check_run(ctx, mask);
+  int rc = check_run(ctx, mask, "lins_gpu_seq_save");
   if (rc != LINS_OK) return rc;
   if (!off) return fail(ctx, LINS_E_INVALID, "null offsets");
   const int n = ctx->seq.n;
@@ -341,7 +314,8 @@ int lins_gpu_seq_save(lins_ctx* ctx, const uint8_t* mask, void* blob, const uint
 }
 
 int lins_gpu_seq_load(lins_ctx* ctx, const uint8_t* mask, const void* blob, const uint64_t* off) {
-  int rc = check_run(ctx, mask);
+  const char* entry = "lins_gpu_seq_load";
+  int rc = check_run(ctx, mask, entry);
   if (rc != LINS_OK) return rc;
   if (!off) return fail(ctx, LINS_E_INVALID, "null offsets");
   SeqState& q = ctx->seq;
@@ -354,7 +328,7 @@ int lins_gpu_seq_load(lins_ctx* ctx, const uint8_t* mask, const void* blob, cons
     any = true;
     if (!p) return fail(ctx, LINS_E_INVALID, "null blob");
     if (off[s + 1] < off[s]) return fail(ctx, LINS_E_INVALID, "blob offsets decrease");
-    if (!q.fresh[s]) return fail(ctx, LINS_E_INVALID, "a loaded slot must be fresh (no step since open / restart)");
+    if ((rc = check_fresh(ctx, s, entry)) != LINS_OK) return rc;
     const char* bad = B::parse(p + off[s], off[s + 1] - off[s], build_sizes(), v[s]);
     if (bad) return fail(ctx, LINS_E_INVALID, bad);
     const bool bound = v[s].h.flags & B::kBound;

@@ -61,7 +61,7 @@ struct Scalars {
   double align_R[9];                   // the tuning's alignIMUtoVehicle rotation
   double pose[7];                      // globalStateYZX_ (bound runs)
 };
-// the mapping node's scalar members (lins_ctx.hpp MapperScalars without its window)
+// the mapping node's scalar members (the base of lins_ctx.hpp's MapperScalars, which adds the window)
 struct MapperRec {
   float transformLast[6], transformSum[6], transformIncre[6], transformTobeMapped[6], transformBefMapped[6], transformAftMapped[6];
   double imuTime[LINS_MAPPER_IMU_QUEUE];
@@ -71,6 +71,10 @@ struct MapperRec {
   int32_t latestFrameID;
   float previousRobotPos[3];
 };
+// a saved node's record is copied into the blob as it is: it must have no padding bytes, which would not be zero
+static_assert(sizeof(MapperRec) == sizeof(float) * (36 + 2 * LINS_MAPPER_IMU_QUEUE + 3) + sizeof(double) * (LINS_MAPPER_IMU_QUEUE + 1) +
+                                       sizeof(int32_t) * 3,
+              "MapperRec without padding");
 struct PoseRec { float x, y, z, roll, pitch, yaw; double time; };  // PointTypePose
 struct KeyframeRec { int32_t id, n[3]; };                           // corner, surf, outlier points
 
@@ -122,7 +126,7 @@ inline bool finite_all(const double* v, int n, bool nonneg) {
   for (int i = 0; i < n; ++i) if (!std::isfinite(v[i]) || (nonneg && v[i] < 0)) return false;
   return true;
 }
-// lins_gpu_seq_configure's and lins_gpu_seq_tune's value checks
+// the value checks of a config and a tuning, in a blob and in lins_gpu_seq_configure / lins_gpu_seq_tune
 inline bool config_ok(const lins_slot_config& c) {
   const lins_seq_params& f = c.filter;
   const lins_seq_init_params& i = c.init;

@@ -1,16 +1,17 @@
 """GPU suite: saving sequence-mode slots and loading them into fresh slots (lins_gpu_seq_save_size / _save / _load).
 
 Drives of tests/rawcases.py (one edited so that a running scan fails the map refresh guard) run through a context A
-(one slot configured, two tuned; bound runs also feed their mappers IMU rows), through seq_step_raw or seq_step_cloud2.
-Every slot of A is saved at every step.  At each step where A first holds a state a load must carry (a slot in INIT, one
-in FIRST_SCAN part-way through its pre-integration, a SKIPPED scan, a stale 1-NN index; and at fixed steps), the blobs
-are loaded into a fresh context B with more slots at a permutation of the slot indices, one of the destination slots
-configured before the load with a config its blob does not have.  A and B then step on the same inputs to the end, and
-every slot of B equals its slot of A byte for byte: the rows, statuses and maps, the IESKF results of the slots that ran,
-the published poses and sizes, the mapper reports, key poses, window and clouds of processed cycles.  A twin of A that
-never saves equals A (save is read-only).  Long bound drives (240 scans) reach a mapper window of 50 key frames with the
-duplicate id and a first key frame whose clouds fail the 10 / 100 gate, and are loaded there.  A saved slot loaded into
-a spare slot of its own run continues as its source does.  Rejected loads change nothing.  bag_replay.replay stopped with
+(two slots configured, two tuned, one of them both; bound runs also feed their mappers IMU rows), through seq_step_raw
+or seq_step_cloud2.  Every slot of A is saved at every step.  At each step where A first holds a state a load must carry
+(a slot in INIT, one in FIRST_SCAN part-way through its pre-integration, a SKIPPED scan, a stale 1-NN index; and at
+fixed steps), the blobs are loaded into a fresh context B with more slots at a permutation of the slot indices, one of
+the destination slots configured and tuned before the load with a config and a tuning its blob does not have.  A and B
+then step on the same inputs to the end, and every slot of B equals its slot of A byte for byte: the rows, statuses and
+maps, the IESKF results of the slots that ran, the published poses and sizes, the mapper reports, key poses, window and
+clouds of processed cycles.  A twin of A that never saves equals A (save is read-only).  A configured and tuned slot's
+blob, loaded and then restarted, replays a drive as a slot that was never configured or tuned does.  Long bound drives
+(240 scans) reach a mapper window of 50 key frames with the duplicate id and a first key frame whose clouds fail the
+10 / 100 gate, and are loaded there.  A saved slot loaded into a spare slot of its own run continues as its source does.  Rejected loads change nothing.  bag_replay.replay stopped with
 a checkpoint and resumed in a new context (seq_step_cloud2) returns what an uninterrupted replay returns, with map=True
 and map=False."""
 import os
@@ -63,14 +64,17 @@ def _cfg(defs):
     return defs.LinsSlotConfig.shipped(init_ba=(0.0, 0.0, 0.0), init_bw=(0.0, 0.0, 0.0), init_vel_std=(0.5, 0.5, 0.5), acc_n=60000.0)
 
 
+def _tun(defs):
+    return defs.LinsSlotTuning.shipped(num_iter=12, nearest_feature_search_sq_dist=16.0, imu_misalign_angle=1.5)
+
+
 def _rig(defs, g, slots_cfg, slots_tune, n):
-    """slot slots_cfg configured (a rig of other init stds and noise), slots slots_tune tuned (fewer iterations, another
+    """slots slots_cfg configured (a rig of other init stds and noise), slots slots_tune tuned (fewer iterations, another
     gate, a misalignment)"""
-    tun = defs.LinsSlotTuning.shipped(num_iter=12, nearest_feature_search_sq_dist=16.0, imu_misalign_angle=1.5)
     m = np.zeros(n, np.uint8); m[slots_cfg] = 1
     g.seq_configure(m, [_cfg(defs) if x else None for x in m])
     m = np.zeros(n, np.uint8); m[slots_tune] = 1
-    g.seq_tune(m, [tun if x else None for x in m])
+    g.seq_tune(m, [_tun(defs) if x else None for x in m])
 
 
 def _inputs(logs, t, slot_log, n, empty=()):
@@ -147,12 +151,13 @@ def _diff(sa, sb):
 
 def _load_into_new(capi, defs, blobs, n, bound, rng, configure=None):
     """the blobs of n slots loaded into a fresh run of n + 3 slots at a permutation; `configure` (a source slot): its
-    destination is configured before the load with a config its blob does not carry"""
+    destination is configured and tuned before the load with a config and a tuning its blob does not carry"""
     perm = rng.permutation(n + 3)[:n]
     b = _open(capi, defs, n + 3, bound)
     if configure is not None:
         m = np.zeros(n + 3, np.uint8); m[perm[configure]] = 1
         b.seq_configure(m, [_cfg(defs) if x else None for x in m])
+        b.seq_tune(m, [_tun(defs) if x else None for x in m])
     mask = np.zeros(n + 3, np.uint8); mask[perm] = 1
     bl = [None] * (n + 3)
     for j in range(n):
@@ -171,14 +176,16 @@ def test_continuation_bit_identical(capi, defs, logs, bound, entry):
     slot_log = {j: j for j in range(n)}
     a, twin = _open(capi, defs, n, bound), _open(capi, defs, n, bound)
     for g in (a, twin):
-        _rig(defs, g, 0, [1, 4], n)
+        _rig(defs, g, [0, 1], [1, 4], n)
     resumed = []  # (B, perm, its slot -> log map)
     loaded_states = set()
+    history = []  # A's state after each step
     rng = np.random.default_rng(7)
     for t in range(T):
         ra, pa = _step(a, logs, t, slot_log, n, model, bound, entry, defs)
         rt, pt = _step(twin, logs, t, slot_log, n, model, bound, entry, defs)
         sa = _state(a, range(n), ra, pa, bound)
+        history.append(sa)
         assert sa == _state(twin, range(n), rt, pt, bound), t  # save is read-only
         for b, perm, blog in resumed:
             rb, pbb = _step(b, logs, t, blog, n + 3, model, bound, entry, defs)
@@ -195,6 +202,16 @@ def test_continuation_bit_identical(capi, defs, logs, bound, entry):
     # way), RUNNING, a SKIPPED scan, a stale index; the configured and tuned slots are in every one
     assert REQUIRED <= loaded_states, REQUIRED - loaded_states
     assert len(resumed) >= 3
+    # slot 1's last blob (configured and tuned) loaded into a fresh run and restarted: the slot then replays log 2 with
+    # the run's values, as A's slot 2, never configured or tuned, did
+    c = _open(capi, defs, n, bound)
+    m = np.eye(n, dtype=np.uint8)[1]
+    c.seq_load(m, [blobs[1] if x else None for x in m])
+    c.seq_restart(m)
+    for t in range(T):
+        rc_, pc_ = _step(c, logs, t, {1: 2}, n, model, bound, entry, defs)
+        sc = _state(c, [1], rc_, pc_, bound)
+        assert sc == [history[t][2]], (t, _diff([history[t][2]], sc))
 
 
 REQUIRED = {("fusion", 0), ("fusion", 1), ("fusion", 3), ("status", SEQ_SKIPPED), ("stale", 1)}

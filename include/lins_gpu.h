@@ -686,6 +686,27 @@ int lins_gpu_mapper_step(lins_ctx* ctx, const lins_mapper_desc* desc, lins_mappe
    scan's corner, surf, outlier and surf-total DS clouds.  NULL skips. */
 int lins_gpu_mapper_download(lins_ctx* ctx, double* key_poses, int32_t* window, float* map_corner_ds, float* map_surf_ds,
                              float* corner_ds, float* surf_ds, float* outlier_ds, float* surf_total_ds);
+/* ---- transform fusion: transform_fusion_node.cpp's laserOdometryHandler (:217-254), the pose on /integrated_to_init ---
+   The odometry of a scan corrected by the mapping node's latest scan-to-map result, at scan rate: transformSum from the
+   odometry message, transformAssociateToMap (:91-215) against the (transformAftMapped, transformBefMapped) pair the
+   mapping node published (publishTF, lidar_mapping_node.cpp:737-777, after every processed cycle: NaN replaced by 0, the
+   angles of transformAftMapped round-tripped through the published quaternion and getRPY), and the pose the node
+   publishes.  Ordering: scan k's fused pose uses the pair of the last processed cycle of an earlier scan (zeros before the
+   first one), as on a machine whose mapping cycle for a scan ends before the next scan's odometry arrives.  Host f32 / f64
+   arithmetic with libm's trigonometry, as the mapper's own host algebra; no kernel, no synchronisation, nothing changes. */
+typedef struct lins_fused_pose {
+  double time;                    /* the odometry message's stamp */
+  double pos[3];                  /* position x, y, z (= transform_mapped[3..5]) in the /camera_init frame */
+  double quat[4];                 /* orientation x, y, z, w: (-q.y, -q.z, q.x, q.w) of createQuaternionMsgFromRollPitchYaw(
+                                     T[2], -T[0], -T[1]) with T = transform_mapped */
+  float transform_mapped[6];      /* transformMapped (rx, ry, rz, tx, ty, tz) */
+  int32_t valid;                  /* 1: a fused pose; 0: none (the struct is zero) */
+  int32_t pad;
+} lins_fused_pose;
+/* The single mapper's fused pose for the odometry message of desc (time, quat, pos; nothing else is read), against the
+   mapper's state now.  Call it with the descriptor of the next lins_gpu_mapper_step, before that step, for the
+   reference's order.  LINS_E_INVALID for a NULL desc or out. */
+int lins_gpu_mapper_fuse(lins_ctx* ctx, const lins_mapper_desc* desc, lins_fused_pose* out);
 /* pcl::VoxelGrid<PointXYZI> on one cloud of n points (leaf > 0): the filter the mapper runs, as a call of its own.  out
    has room for n records (x, y, z, intensity floats); *n_out receives the voxel count.  LINS_E_TOOBIG as above. */
 int lins_gpu_voxel_grid(lins_ctx* ctx, const lins_point* in, int n, float leaf, float* out, int* n_out);
@@ -725,6 +746,10 @@ int lins_gpu_mappers_step(lins_ctx* ctx, const lins_mappers_desc* d, lins_mapper
 /* lins_gpu_mapper_download of one slot */
 int lins_gpu_mappers_download(lins_ctx* ctx, int32_t slot, double* key_poses, int32_t* window, float* map_corner_ds,
                               float* map_surf_ds, float* corner_ds, float* surf_ds, float* outlier_ds, float* surf_total_ds);
+/* lins_gpu_mapper_fuse for every present slot of d (present, time, quat and pos are read), against each slot's state now;
+   out[s].valid = 0 for an absent slot.  Call it with the descriptor of the next lins_gpu_mappers_step, before that step.
+   LINS_E_INVALID for a NULL d or out, n_slots != M or a NULL time / quat / pos; LINS_E_NOMAP without a run. */
+int lins_gpu_mappers_fuse(lins_ctx* ctx, const lins_mappers_desc* d, lins_fused_pose* out /*M*/);
 
 /* ---- sequence mode feeding its mapping nodes: LinsFusion::publishTopics (Estimator.cpp:177-202, :254-320) on the device ---
    A run opened by lins_gpu_seq_open can be bound to the context's lockstep mappers: slot s of the sequence run feeds
@@ -766,6 +791,11 @@ int lins_gpu_seq_map_step(lins_ctx* ctx, const lins_seq_map_desc* d, lins_mapper
    restart), sizes = the points of its less-sharp, less-flat and outlier YZX clouds (S x 3).  Either may be NULL.
    LINS_E_NOMAP on an unbound run. */
 int lins_gpu_seq_map_published(lins_ctx* ctx, double* pose /*S x 7*/, int32_t* sizes /*S x 3*/);
+/* each slot's fused pose (lins_gpu_mapper_fuse) of the last lins_gpu_seq_map_step, which computes it for every published
+   slot after the publish decision and before the mapping cycles, from the stamp and the pose the slot published
+   (lins_gpu_seq_map_published).  valid = 0 for a slot that did not publish in that step, and for a slot restarted or
+   loaded since.  Host copies only.  LINS_E_INVALID for a NULL out; LINS_E_NOMAP on an unbound run. */
+int lins_gpu_seq_map_fused(lins_ctx* ctx, lins_fused_pose* out /*S*/);
 
 /* ---- saving and loading slots: checkpoint, resume and move recordings between runs ---------------------------------
    A slot of a lins_gpu_seq_open run is saved as a self-contained byte blob and loaded into a fresh slot of any

@@ -181,7 +181,8 @@ def model_table(recordings, model):
 
 # the per-scan lists of a map=True replay and the arrays they become: (dtype, row shape)
 _MAP_LISTS = dict(map_time=(np.float64, ()), map_odom=(np.float64, (7,)), map_processed=(np.int32, ()),
-                  map_aft_mapped=(np.float32, (6,)), map_keyframes=(np.int32, ()), map_sizes=(np.int32, (3,)))
+                  map_aft_mapped=(np.float32, (6,)), map_keyframes=(np.int32, ()), map_sizes=(np.int32, (3,)),
+                  map_fused=(np.float64, (7,)))
 
 
 def _map_arrays(o):
@@ -268,8 +269,9 @@ def replay(recordings, slots, model=None, device=0, gpu=None, map=False, checkpo
     the mappers, as tools/run_bag.py --map does not), and adds per published scan: map_time, map_odom (m x 7: the
     odometry, YZX position + quaternion x y z w of globalStateYZX_, as fed to the mapper), map_sizes (m x 3: the
     less-sharp, less-flat and outlier cloud sizes), map_processed, map_aft_mapped (m x 6: transformAftMapped) and
-    map_keyframes (n_keyframes after the cycle); and key_poses (the mapper's cloudKeyPoses6D, k x
-    7, downloaded when the recording ends).
+    map_keyframes (n_keyframes after the cycle), map_fused (m x 7: transform_fusion_node's pose of the scan, x y z qx qy
+    qz qw in /camera_init, lins_gpu_seq_map_fused); and key_poses (the mapper's cloudKeyPoses6D, k x 7, downloaded when
+    the recording ends).
     checkpoint: a directory.  With stop_after=k the replay ends after its first k steps, writes a checkpoint there and
     returns None (it returns the outputs as usual when it has fewer steps); with checkpoint_every=N it writes one after
     every N-th step and runs on.  resume: a checkpoint directory written for the same recordings, slot count and map:
@@ -294,7 +296,8 @@ def replay(recordings, slots, model=None, device=0, gpu=None, map=False, checkpo
     if map:
         g.seq_map_open()
         for o in out:
-            o.update(map_time=[], map_odom=[], map_processed=[], map_aft_mapped=[], map_keyframes=[], map_sizes=[], key_poses=np.zeros((0, 7)))
+            o.update(map_time=[], map_odom=[], map_processed=[], map_aft_mapped=[], map_keyframes=[], map_sizes=[], map_fused=[],
+                     key_poses=np.zeros((0, 7)))
     if resume is not None:
         out, held = st["out"], st["held"]
         g.seq_load(np.array([b is not None for b in blobs], np.uint8), blobs)
@@ -354,6 +357,7 @@ def replay(recordings, slots, model=None, device=0, gpu=None, map=False, checkpo
                 time = np.array([recordings[w[0]].stamps[w[1]] if w else 0.0 for w in who])
                 reps, pub = g.seq_map_step(time)
                 pose, sizes = g.seq_map_published()  # (the odometry and cloud sizes each slot's mapper was fed)
+                fused = g.seq_map_fused()
                 for j, w in enumerate(who):
                     if w is None:
                         continue
@@ -366,6 +370,7 @@ def replay(recordings, slots, model=None, device=0, gpu=None, map=False, checkpo
                     o["map_time"].append(time[j]); o["map_odom"].append(pose[j].copy()); o["map_processed"].append(r.processed)
                     o["map_aft_mapped"].append(list(r.transform_aft_mapped)); o["map_keyframes"].append(r.n_keyframes)
                     o["map_sizes"].append(sizes[j].copy())
+                    o["map_fused"].append(fused[j].row())
             done = t + 1
             if stop_after is not None and done == stop_after:
                 write_checkpoint(g, checkpoint, done, who, lengths, map, held, out)

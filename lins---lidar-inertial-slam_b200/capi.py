@@ -13,7 +13,7 @@ import subprocess
 
 import numpy as np
 
-from .ctypes_defs import (Batch, COV_SIZE, LinsBatchDesc, LinsCloud2Desc, LinsCloud2Layout, LinsFeatureParams, LinsLidarModel, LinsLidarModels, LinsMapperDesc, LinsMapperReport, LinsMappersDesc, LinsMapReport, LinsParams, LinsPclDesc,
+from .ctypes_defs import (Batch, COV_SIZE, LinsBatchDesc, LinsCloud2Desc, LinsCloud2Layout, LinsFeatureParams, LinsLidarModel, LinsLidarModels, LinsFusedPose, LinsMapperDesc, LinsMapperReport, LinsMappersDesc, LinsMapReport, LinsParams, LinsPclDesc,
                           LinsRawDesc, LinsReport, LinsScanResult, LinsSeqBeginDesc, LinsSeqInitParams, LinsSeqParams, LinsSeqPclDesc,
                           LinsSeqCloud2Desc, LinsSeqMapDesc, LinsSeqRawDesc, LinsSeqStepDesc, LinsSlotConfig, LinsSlotTuning, POINT_DTYPE, SCAN_RESULT_DTYPE, STATE_DIM, as_points, make_points, ptr)
 
@@ -39,7 +39,8 @@ EXPORTS = [
     "lins_gpu_mapper_reset", "lins_gpu_mapper_imu", "lins_gpu_mapper_step", "lins_gpu_mapper_download", "lins_gpu_voxel_grid",
     "lins_gpu_mappers_open", "lins_gpu_mappers_reset", "lins_gpu_mappers_imu", "lins_gpu_mappers_step", "lins_gpu_mappers_download",
     "lins_gpu_seq_map_open", "lins_gpu_seq_map_step", "lins_gpu_seq_map_published", "lins_gpu_seq_configure", "lins_gpu_seq_tune",
-    "lins_gpu_seq_save_size", "lins_gpu_seq_save", "lins_gpu_seq_load",
+    "lins_gpu_seq_save_size", "lins_gpu_seq_save", "lins_gpu_seq_load", "lins_gpu_mapper_fuse", "lins_gpu_mappers_fuse",
+    "lins_gpu_seq_map_fused",
 ]
 
 NVCC_ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]  # H100 (Hopper)
@@ -153,6 +154,9 @@ def lib():
         L.lins_gpu_seq_save_size.argtypes = [vp, vp, vp]
         L.lins_gpu_seq_save.argtypes = [vp, vp, vp, vp]
         L.lins_gpu_seq_load.argtypes = [vp, vp, vp, vp]
+        L.lins_gpu_mapper_fuse.argtypes = [vp, C.POINTER(LinsMapperDesc), C.POINTER(LinsFusedPose)]
+        L.lins_gpu_mappers_fuse.argtypes = [vp, C.POINTER(LinsMappersDesc), vp]
+        L.lins_gpu_seq_map_fused.argtypes = [vp, vp]
         _LIB = L
     return _LIB
 
@@ -208,6 +212,17 @@ def pack_csr(clouds):
     # (joined as plain float32 rows: numpy concatenates structured records far more slowly)
     pts = np.concatenate([p.view(np.float32).reshape(-1, 8) for p in parts]).view(POINT_DTYPE).reshape(-1) if parts else np.zeros(0, POINT_DTYPE)
     return pts, off
+
+
+def _odometry_arrays(steps):
+    """The present flags, stamps, quaternions (M x 4) and positions (M x 3) of lockstep steps[s] = (time, quat_xyzw, pos,
+    ...) or None (an absent slot: identity odometry)."""
+    M = len(steps)
+    present = np.array([st is not None for st in steps], np.uint8)
+    time = np.array([float(st[0]) if st is not None else 0.0 for st in steps], np.float64)
+    quat = np.array([[float(v) for v in st[1]] if st is not None else [0.0, 0.0, 0.0, 1.0] for st in steps], np.float64).reshape(M, 4)
+    pos = np.array([[float(v) for v in st[2]] if st is not None else [0.0] * 3 for st in steps], np.float64).reshape(M, 3)
+    return present, time, quat, pos
 
 
 class LinsGpu:
@@ -356,6 +371,14 @@ class LinsGpu:
         self._ck(self.L.lins_gpu_mapper_step(self.h, C.byref(d), C.byref(rep)))
         return rep
 
+    def mapper_fuse(self, time, quat_xyzw, pos):
+        """transform_fusion_node's pose (LinsFusedPose) for this odometry message against the mapper's state now: call it
+        before the mapper_step of the same message."""
+        d = LinsMapperDesc(time=float(time), quat=(C.c_double * 4)(*[float(v) for v in quat_xyzw]), pos=(C.c_double * 3)(*[float(v) for v in pos]))
+        out = LinsFusedPose()
+        self._ck(self.L.lins_gpu_mapper_fuse(self.h, C.byref(d), C.byref(out)))
+        return out
+
     def mapper_download(self, rep):
         """Key poses (n x 7: x, y, z, roll, pitch, yaw, time), the window's ids, and the last processed cycle's clouds
         ((n, 4) float32: map_corner_ds, map_surf_ds, corner_ds, surf_ds, outlier_ds, surf_total_ds) whose sizes `rep`,
@@ -402,10 +425,7 @@ class LinsGpu:
         """One lockstep step: steps[s] = (time, quat_xyzw, pos, corner, surf, outlier) of slot s, or None for an absent
         slot.  Returns the list of LinsMapperReport (None for absent slots)."""
         M = len(steps)
-        present = np.array([st is not None for st in steps], np.uint8)
-        time = np.array([float(st[0]) if st is not None else 0.0 for st in steps], np.float64)
-        quat = np.array([[float(v) for v in st[1]] if st is not None else [0.0, 0.0, 0.0, 1.0] for st in steps], np.float64).reshape(M, 4)
-        pos = np.array([[float(v) for v in st[2]] if st is not None else [0.0] * 3 for st in steps], np.float64).reshape(M, 3)
+        present, time, quat, pos = _odometry_arrays(steps)
         clouds = [pack_csr([st[3 + k] if st is not None else None for st in steps]) for k in range(3)]
         d = LinsMappersDesc(n_slots=M, present=ptr(present), time=ptr(time), quat=ptr(quat), pos=ptr(pos),
                             corner=ptr(clouds[0][0]), corner_off=ptr(clouds[0][1]), surf=ptr(clouds[1][0]), surf_off=ptr(clouds[1][1]),
@@ -413,6 +433,16 @@ class LinsGpu:
         reps = (LinsMapperReport * M)()
         self._ck(self.L.lins_gpu_mappers_step(self.h, C.byref(d), C.cast(reps, C.c_void_p)))
         return [reps[s] if present[s] else None for s in range(M)]
+
+    def mappers_fuse(self, steps):
+        """mapper_fuse for every slot of a lockstep step: steps[s] = (time, quat_xyzw, pos, ...) of slot s, or None for an
+        absent slot.  Returns the list of LinsFusedPose (None for absent slots)."""
+        M = len(steps)
+        present, time, quat, pos = _odometry_arrays(steps)
+        d = LinsMappersDesc(n_slots=M, present=ptr(present), time=ptr(time), quat=ptr(quat), pos=ptr(pos))
+        out = (LinsFusedPose * M)()
+        self._ck(self.L.lins_gpu_mappers_fuse(self.h, C.byref(d), C.cast(out, C.c_void_p)))
+        return [out[s] if present[s] else None for s in range(M)]
 
     def mappers_download(self, slot, rep):
         """mapper_download of one slot: (key poses, window, clouds) with the sizes its last processed cycle's report gives."""
@@ -448,6 +478,12 @@ class LinsGpu:
         pose, sizes = np.zeros((self._seq_n, 7)), np.zeros((self._seq_n, 3), np.int32)
         self._ck(self.L.lins_gpu_seq_map_published(self.h, ptr(pose), ptr(sizes)))
         return pose, sizes
+
+    def seq_map_fused(self):
+        """Each slot's LinsFusedPose of the last seq_map_step (valid = 0: the slot did not publish)."""
+        out = (LinsFusedPose * self._seq_n)()
+        self._ck(self.L.lins_gpu_seq_map_fused(self.h, C.cast(out, C.c_void_p)))
+        return list(out)
 
     # ---- batched mode ------------------------------------------------------------------------------------------
     def batch_upload(self, batch):

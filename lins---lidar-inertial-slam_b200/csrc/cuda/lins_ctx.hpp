@@ -144,6 +144,7 @@ struct SeqPubState {
   Buf<double, kPinned> h_glob;         // n x 20: the global states after the last step
   Buf<int, kPinned> h_proj_counts;     // n x 2: the last projection's counts (segmented, outlier)
   CopyList copies;                     // the outlier stash, then the next outlier generation
+  std::vector<lins_fused_pose> fused;  // each slot's fused pose of the last publish step (valid = 0: none)
 };
 
 // One sequence-mode slot's setup on the host.  A slot of a new run, and a restarted one, is this record as constructed.
@@ -658,11 +659,14 @@ int voxel_grid_reserve(lins_ctx* ctx, VgScratch& w, int n, int n_seg);
 // surf, outlier, surf total) and of the loop state st (null: no key frames, or the 10 / 100 gate failed): transformUpdate,
 // saveKeyFramesAndFactor and the loop candidate; commits s into m and fills r.  A saved key frame is left in *save for
 // keyframes_queue, which transforms every listed key frame's DS clouds into its store slot in one launch.
+// mapper_node_fuse: transform_fusion_node's pose for the odometry message (time, quat, pos) against the node as it
+// stands, i.e. with the pair the node published after its last processed cycle (DESIGN.md §4.13).
 struct KfSave { MapperKeyFrame* kf; MapperKeyPose kp; const float4* ds[3]; };
 void mapper_node_reset(MapperNode& m);
 void mapper_node_imu(MapperScalars& s, const double* time, const double* roll, const double* pitch, int n);
 bool mapper_cycle_begin(const MapperNode& m, MapperScalars& s, double time, const double quat[4], const double pos[3], lins_mapper_report& r);
 void mapper_window_sizes(const MapperNode& m, const MapperScalars& s, int& n_corner, int& n_surf);
+void mapper_node_fuse(const MapperNode& m, double time, const double quat[4], const double pos[3], lins_fused_pose& out);
 void mapper_cycle_end(MapperNode& m, MapperScalars& s, double time, double scan_period, const int cnt[6], const lins_map::MapLoopState* st,
                       lins_mapper_report& r, KfSave* save, bool* saved);
 int keyframes_queue(lins_ctx* ctx, const KfSave* saves, int n, Buf<unsigned char>& dev, Buf<unsigned char, kPinned>& host);

@@ -2,8 +2,9 @@
 // lins_mappers.cu runs for one or many drives: a node's host logic, its key-frame store's transform, and the device
 // pcl::VoxelGrid the cycle runs (also behind lins_gpu_voxel_grid).
 //
-// Host, per node (MapperNode): transformAssociateToMap, the window's deque of key-frame ids, transformUpdate with the IMU
-// ring, the 0.3 m key-frame test, the pose's round trip through gtsam's Rot3 and the loop-candidate search, in the
+// Host, per node (MapperNode): transformAssociateToMap (csrc/host/transform_fusion.hpp, which the fusion shares), the
+// fused pose of an odometry message against the node's state, the window's deque of key-frame ids, transformUpdate with
+// the IMU ring, the 0.3 m key-frame test, the pose's round trip through gtsam's Rot3 and the loop-candidate search, in the
 // reference's f32 / f64 types (no multiply-add contraction: this unit is built with -fmad=false and g++ does not
 // contract on x86-64 without -mfma).  Device: the key-frame store, each key frame's DS clouds transformed into the map
 // frame once, at save time, with its PointTypePose (one launch for the key frames a step saves).
@@ -26,6 +27,7 @@
 #include <cstdint>
 #include <cstring>
 
+#include "../host/transform_fusion.hpp"
 #include "lins_ctx.hpp"
 #include "lins_features.cuh"
 
@@ -294,27 +296,6 @@ int keyframes_queue(lins_ctx* ctx, const KfSave* saves, int n, Buf<unsigned char
 namespace {
 
 // ---- host scalar code, typed as the reference types it ---------------------------------------------------------------
-// tf::Matrix3x3(q).getRPY(roll, pitch, yaw) (tf/LinearMath/Matrix3x3.h: setRotation, getEulerYPR with solution 1)
-void tf_get_rpy(double qx, double qy, double qz, double qw, double& roll, double& pitch, double& yaw) {
-  const double d = qx * qx + qy * qy + qz * qz + qw * qw;
-  const double s = 2.0 / d;
-  const double xs = qx * s, ys = qy * s, zs = qz * s;
-  const double wx = qw * xs, wy = qw * ys, wz = qw * zs;
-  const double xx = qx * xs, xy = qx * ys, xz = qx * zs;
-  const double yy = qy * ys, yz = qy * zs, zz = qz * zs;
-  const double m00 = 1.0 - (yy + zz), m10 = xy + wz, m20 = xz - wy, m21 = yz + wx, m22 = 1.0 - (xx + yy);
-  if (std::fabs(m20) >= 1) {
-    yaw = 0;
-    const double delta = std::atan2(m21, m22);
-    if (m20 < 0) { pitch = M_PI / 2.0; roll = delta; }
-    else { pitch = -M_PI / 2.0; roll = delta; }
-  } else {
-    pitch = -std::asin(m20);
-    roll = std::atan2(m21 / std::cos(pitch), m22 / std::cos(pitch));
-    yaw = std::atan2(m10 / std::cos(pitch), m00 / std::cos(pitch));
-  }
-}
-
 // gtsam Rot3::RzRyRx(x, y, z) (the matrix representation) and Rot3::xyz() through RQ; ypr = (z, y, x):
 // roll() = x, pitch() = y, yaw() = z
 void rot3_rzryrx(double x, double y, double z, double R[3][3]) {
@@ -341,59 +322,6 @@ void rot3_xyz(const double A[3][3], double xyz[3]) {
   mat_mul3(B, Qy, Cm);
   const double z = -std::atan2(-Cm[1][0], Cm[1][1]);
   xyz[0] = x; xyz[1] = y; xyz[2] = z;
-}
-
-// transformAssociateToMap (:411-536); cos / sin / asin / atan2 of floats are the f32 overloads (DESIGN.md §4.4)
-void transform_associate_to_map(MapperScalars& s) {
-  const float* Sum = s.transformSum;
-  const float* Bef = s.transformBefMapped;
-  const float* Aft = s.transformAftMapped;
-  float* Inc = s.transformIncre;
-  float* T = s.transformTobeMapped;
-  using std::cos; using std::sin;
-  float x1 = cos(Sum[1]) * (Bef[3] - Sum[3]) - sin(Sum[1]) * (Bef[5] - Sum[5]);
-  float y1 = Bef[4] - Sum[4];
-  float z1 = sin(Sum[1]) * (Bef[3] - Sum[3]) + cos(Sum[1]) * (Bef[5] - Sum[5]);
-  float x2 = x1;
-  float y2 = cos(Sum[0]) * y1 + sin(Sum[0]) * z1;
-  float z2 = -sin(Sum[0]) * y1 + cos(Sum[0]) * z1;
-  Inc[3] = cos(Sum[2]) * x2 + sin(Sum[2]) * y2;
-  Inc[4] = -sin(Sum[2]) * x2 + cos(Sum[2]) * y2;
-  Inc[5] = z2;
-  const float sbcx = sin(Sum[0]), cbcx = cos(Sum[0]), sbcy = sin(Sum[1]), cbcy = cos(Sum[1]), sbcz = sin(Sum[2]), cbcz = cos(Sum[2]);
-  const float sblx = sin(Bef[0]), cblx = cos(Bef[0]), sbly = sin(Bef[1]), cbly = cos(Bef[1]), sblz = sin(Bef[2]), cblz = cos(Bef[2]);
-  const float salx = sin(Aft[0]), calx = cos(Aft[0]), saly = sin(Aft[1]), caly = cos(Aft[1]), salz = sin(Aft[2]), calz = cos(Aft[2]);
-  const float srx = -sbcx * (salx * sblx + calx * cblx * salz * sblz + calx * calz * cblx * cblz) -
-                    cbcx * sbcy * (calx * calz * (cbly * sblz - cblz * sblx * sbly) - calx * salz * (cbly * cblz + sblx * sbly * sblz) + cblx * salx * sbly) -
-                    cbcx * cbcy * (calx * salz * (cblz * sbly - cbly * sblx * sblz) - calx * calz * (sbly * sblz + cbly * cblz * sblx) + cblx * cbly * salx);
-  T[0] = -std::asin(srx);
-  const float srycrx = sbcx * (cblx * cblz * (caly * salz - calz * salx * saly) - cblx * sblz * (caly * calz + salx * saly * salz) + calx * saly * sblx) -
-                       cbcx * cbcy * ((caly * calz + salx * saly * salz) * (cblz * sbly - cbly * sblx * sblz) +
-                                      (caly * salz - calz * salx * saly) * (sbly * sblz + cbly * cblz * sblx) - calx * cblx * cbly * saly) +
-                       cbcx * sbcy * ((caly * calz + salx * saly * salz) * (cbly * cblz + sblx * sbly * sblz) +
-                                      (caly * salz - calz * salx * saly) * (cbly * sblz - cblz * sblx * sbly) + calx * cblx * saly * sbly);
-  const float crycrx = sbcx * (cblx * sblz * (calz * saly - caly * salx * salz) - cblx * cblz * (saly * salz + caly * calz * salx) + calx * caly * sblx) +
-                       cbcx * cbcy * ((saly * salz + caly * calz * salx) * (sbly * sblz + cbly * cblz * sblx) +
-                                      (calz * saly - caly * salx * salz) * (cblz * sbly - cbly * sblx * sblz) + calx * caly * cblx * cbly) -
-                       cbcx * sbcy * ((saly * salz + caly * calz * salx) * (cbly * sblz - cblz * sblx * sbly) +
-                                      (calz * saly - caly * salx * salz) * (cbly * cblz + sblx * sbly * sblz) - calx * caly * cblx * sbly);
-  T[1] = std::atan2(srycrx / cos(T[0]), crycrx / cos(T[0]));
-  const float srzcrx = (cbcz * sbcy - cbcy * sbcx * sbcz) * (calx * salz * (cblz * sbly - cbly * sblx * sblz) - calx * calz * (sbly * sblz + cbly * cblz * sblx) + cblx * cbly * salx) -
-                       (cbcy * cbcz + sbcx * sbcy * sbcz) * (calx * calz * (cbly * sblz - cblz * sblx * sbly) - calx * salz * (cbly * cblz + sblx * sbly * sblz) + cblx * salx * sbly) +
-                       cbcx * sbcz * (salx * sblx + calx * cblx * salz * sblz + calx * calz * cblx * cblz);
-  const float crzcrx = (cbcy * sbcz - cbcz * sbcx * sbcy) * (calx * calz * (cbly * sblz - cblz * sblx * sbly) - calx * salz * (cbly * cblz + sblx * sbly * sblz) + cblx * salx * sbly) -
-                       (sbcy * sbcz + cbcy * cbcz * sbcx) * (calx * salz * (cblz * sbly - cbly * sblx * sblz) - calx * calz * (sbly * sblz + cbly * cblz * sblx) + cblx * cbly * salx) +
-                       cbcx * cbcz * (salx * sblx + calx * cblx * salz * sblz + calx * calz * cblx * cblz);
-  T[2] = std::atan2(srzcrx / cos(T[0]), crzcrx / cos(T[0]));
-  x1 = cos(T[2]) * Inc[3] - sin(T[2]) * Inc[4];
-  y1 = sin(T[2]) * Inc[3] + cos(T[2]) * Inc[4];
-  z1 = Inc[5];
-  x2 = x1;
-  y2 = cos(T[0]) * y1 - sin(T[0]) * z1;
-  z2 = sin(T[0]) * y1 + cos(T[0]) * z1;
-  T[3] = Aft[3] - (cos(T[1]) * x2 + sin(T[1]) * z2);
-  T[4] = Aft[4] - y2;
-  T[5] = Aft[5] - (-sin(T[1]) * x2 + cos(T[1]) * z2);
 }
 
 // transformUpdate (:538-577)
@@ -468,10 +396,7 @@ bool mapper_cycle_begin(const MapperNode& m, MapperScalars& s, double timeLaserO
   std::memset(&r, 0, sizeof(r));
   r.loop_candidate = -1;
   {  // laserOdometryHandler :713-722
-    double roll, pitch, yaw;
-    tf_get_rpy(quat[2], -quat[0], -quat[1], quat[3], roll, pitch, yaw);
-    s.transformSum[0] = -pitch; s.transformSum[1] = -yaw; s.transformSum[2] = roll;
-    s.transformSum[3] = pos[0]; s.transformSum[4] = pos[1]; s.transformSum[5] = pos[2];
+    lins_tf::odometry_transform(quat, pos, s.transformSum);
   }
   if (!(timeLaserOdometry - s.timeLastProcessing >= 0.3)) {  // :1821 (the odometry still replaces transformSum)
     r.skipped_interval = 1;
@@ -481,7 +406,7 @@ bool mapper_cycle_begin(const MapperNode& m, MapperScalars& s, double timeLaserO
     return false;
   }
   s.timeLastProcessing = timeLaserOdometry;
-  transform_associate_to_map(s);
+  lins_tf::transform_associate_to_map(s.transformSum, s.transformBefMapped, s.transformAftMapped, s.transformIncre, s.transformTobeMapped);
   for (int i = 0; i < 6; ++i) r.transform_guess[i] = s.transformTobeMapped[i];
   // extractSurroundingKeyFrames :1201-1246 (the deque of ids)
   const int numPoses = (int)m.poses.size();
@@ -499,6 +424,15 @@ bool mapper_cycle_begin(const MapperNode& m, MapperScalars& s, double timeLaserO
     }
   }
   return true;
+}
+
+void mapper_node_fuse(const MapperNode& m, double time, const double quat[4], const double pos[3], lins_fused_pose& out) {
+  // every processed cycle ends with a key pose (the first one always saves), so a node without key poses has not
+  // published; the pair it holds then is the fusion node's initial zeros, not yet round-tripped through publishTF
+  std::memset(&out, 0, sizeof(out));
+  out.time = time;
+  lins_tf::transform_fusion(quat, pos, !m.poses.empty(), m.s.transformAftMapped, m.s.transformBefMapped, out.transform_mapped, out.pos, out.quat);
+  out.valid = 1;
 }
 
 void mapper_window_sizes(const MapperNode& m, const MapperScalars& s, int& n_corner, int& n_surf) {

@@ -29,6 +29,16 @@ int need_open(lins_ctx* ctx) {
   return ctx->mappers.n > 0 ? LINS_OK : fail(ctx, LINS_E_NOMAP, "lins_gpu_mappers_open has not been called");
 }
 
+// the odometry fields of a lockstep descriptor, as lins_gpu_mappers_step and _fuse check them
+int check_odometry(lins_ctx* ctx, const lins_mappers_desc* d) {
+  if (!ctx) return LINS_E_INVALID;
+  if (!d) return fail(ctx, LINS_E_INVALID, "null desc");
+  if (need_open(ctx) != LINS_OK) return LINS_E_NOMAP;
+  if (d->n_slots != ctx->mappers.n) return fail(ctx, LINS_E_INVALID, "n_slots differs from the open run's");
+  if (!d->time || !d->quat || !d->pos) return fail(ctx, LINS_E_INVALID, "null time / quat / pos");
+  return LINS_OK;
+}
+
 const char* const kBad = "VoxelGrid: the leaf is too small for the cloud's extent (div_x * div_y * div_z > INT32_MAX)";
 
 }  // namespace
@@ -284,17 +294,26 @@ int lins_gpu_mappers_imu(lins_ctx* ctx, const int32_t* off, const double* time, 
 }
 
 int lins_gpu_mappers_step(lins_ctx* ctx, const lins_mappers_desc* d, lins_mapper_report* reps) {
-  if (!ctx) return LINS_E_INVALID;
-  if (!d) return fail(ctx, LINS_E_INVALID, "null desc");
-  if (need_open(ctx) != LINS_OK) return LINS_E_NOMAP;
+  const int rc = check_odometry(ctx, d);
+  if (rc != LINS_OK) return rc;
   const int M = ctx->mappers.n;
-  if (d->n_slots != M) return fail(ctx, LINS_E_INVALID, "n_slots differs from the open run's");
-  if (!d->time || !d->quat || !d->pos) return fail(ctx, LINS_E_INVALID, "null time / quat / pos");
   const lins_point* src[3] = {d->corner, d->surf, d->outlier};
   const int32_t* off[3] = {d->corner_off, d->surf_off, d->outlier_off};
   static const char* const what[3] = {"bad corner offsets / cloud", "bad surf offsets / cloud", "bad outlier offsets / cloud"};
   for (int k = 0; k < 3; ++k) if (check_csr(ctx, off[k], M, src[k], what[k]) != LINS_OK) return LINS_E_INVALID;
   return mappers_step(ctx, ctx->mappers, d, reps, nullptr, nullptr);
+}
+
+int lins_gpu_mappers_fuse(lins_ctx* ctx, const lins_mappers_desc* d, lins_fused_pose* out) {
+  const int rc = check_odometry(ctx, d);
+  if (rc != LINS_OK) return rc;
+  if (!out) return fail(ctx, LINS_E_INVALID, "null out");
+  const MappersState& ms = ctx->mappers;
+  for (int s = 0; s < ms.n; ++s) {
+    if (d->present && !d->present[s]) { std::memset(&out[s], 0, sizeof(out[s])); continue; }
+    mapper_node_fuse(ms.node[s], d->time[s], d->quat + 4 * s, d->pos + 3 * s, out[s]);
+  }
+  return LINS_OK;
 }
 
 int lins_gpu_mappers_download(lins_ctx* ctx, int32_t slot, double* key_poses, int32_t* window, float* map_corner_ds, float* map_surf_ds,
@@ -340,6 +359,15 @@ int lins_gpu_mapper_step(lins_ctx* ctx, const lins_mapper_desc* d, lins_mapper_r
   one.surf = d->surf; one.surf_off = off[1];
   one.outlier = d->outlier; one.outlier_off = off[2];
   return mappers_step(ctx, ctx->mapper, &one, rep, nullptr, nullptr);
+}
+
+int lins_gpu_mapper_fuse(lins_ctx* ctx, const lins_mapper_desc* d, lins_fused_pose* out) {
+  if (!ctx) return LINS_E_INVALID;
+  if (!d || !out) return fail(ctx, LINS_E_INVALID, "null desc / out");
+  const int rc = mapper_open(ctx);
+  if (rc != LINS_OK) return rc;
+  mapper_node_fuse(ctx->mapper.node[0], d->time, d->quat, d->pos, *out);
+  return LINS_OK;
 }
 
 int lins_gpu_mapper_download(lins_ctx* ctx, double* key_poses, int32_t* window, float* map_corner_ds, float* map_surf_ds,

@@ -814,10 +814,12 @@ int seq_map_run(lins_ctx* ctx, const lins_seq_map_desc* d, lins_mapper_report* r
   pb.pending = false;
   if (published) std::copy(pub.begin(), pub.end(), published);
 
-  // the mapping nodes' inputs: scan_last_'s less-sharp / less-flat clouds are the slot's current maps, in XYZ order
+  // the mapping nodes' inputs: scan_last_'s less-sharp / less-flat clouds are the slot's current maps, in XYZ order.
+  // The fusion node handles the odometry before the mapping node's cycle for this scan ends (DESIGN.md §4.13).
   std::vector<MapPiece> dev(3 * (size_t)n);
   std::vector<double> quat(4 * (size_t)n), pos(3 * (size_t)n);
   for (int s = 0; s < n; ++s) {
+    std::memset(&pb.fused[s], 0, sizeof(pb.fused[s]));
     if (!pub[s]) continue;
     const SeqSlot& r = q.slot[s];
     if (r.yzx) {
@@ -827,6 +829,7 @@ int seq_map_run(lins_ctx* ctx, const lins_seq_map_desc* d, lins_mapper_report* r
     }
     std::copy(r.pose, r.pose + 3, &pos[3 * (size_t)s]);
     std::copy(r.pose + 3, r.pose + 7, &quat[4 * (size_t)s]);
+    mapper_node_fuse(ctx->mappers.node[s], d->time[s], r.pose + 3, r.pose, pb.fused[s]);
   }
   lins_mappers_desc md;
   std::memset(&md, 0, sizeof(md));
@@ -953,8 +956,11 @@ int lins_gpu_seq_restart(lins_ctx* ctx, const uint8_t* mask) {
   swap_maps(q);
   for (int s = 0; s < n; ++s)
     if (mask[s]) { q.h_stale_v[s] = 0; q.fusion[s] = FUSION_INIT; q.status[s] = LINS_SEQ_IDLE; }
-  // a new recording is a new LinsFusion with a new mapping node
-  if (q.pub.bound && (rc = mappers_reset(ctx, ctx->mappers, mask)) != LINS_OK) return rc;
+  // a new recording is a new LinsFusion with a new mapping node (and nothing fused yet)
+  if (q.pub.bound) {
+    for (int s = 0; s < n; ++s) if (mask[s]) q.pub.fused[s] = lins_fused_pose{};
+    if ((rc = mappers_reset(ctx, ctx->mappers, mask)) != LINS_OK) return rc;
+  }
   CK(queue_map_state(ctx, q));
   CK(cudaStreamSynchronize(ctx->stream));  // (the two sources above are pageable)
   return LINS_OK;
@@ -1090,6 +1096,7 @@ int lins_gpu_seq_map_open(lins_ctx* ctx) {
   for (SeqSlot& r : q.slot) { r.yzx = fresh.yzx; std::copy(fresh.pose, fresh.pose + 7, r.pose); }
   pb.h_outl_off.assign((size_t)n + 1, 0);
   pb.fusion_before.assign(n, FUSION_INIT);
+  pb.fused.assign(n, lins_fused_pose{});
   pb.pending = false;
   pb.dev_outliers = false;
   pb.bound = true;
@@ -1127,6 +1134,15 @@ int lins_gpu_seq_map_published(lins_ctx* ctx, double* pose, int32_t* sizes) {
     sizes[3 * s + 1] = y ? current_piece(q, 0, s).len : 0;
     sizes[3 * s + 2] = y ? pb.h_outl_off[s + 1] - pb.h_outl_off[s] : 0;
   }
+  return LINS_OK;
+}
+
+int lins_gpu_seq_map_fused(lins_ctx* ctx, lins_fused_pose* out) {
+  if (!ctx) return LINS_E_INVALID;
+  SeqState& q = ctx->seq;
+  if (q.n == 0 || !q.pub.bound) return fail(ctx, LINS_E_NOMAP, "no sequence run bound by lins_gpu_seq_map_open");
+  if (!out) return fail(ctx, LINS_E_INVALID, "null out");
+  std::copy(q.pub.fused.begin(), q.pub.fused.end(), out);
   return LINS_OK;
 }
 

@@ -269,6 +269,7 @@ int load_run(lins_ctx* ctx, const uint8_t* mask, const std::vector<B::View>& v) 
     if (b.h.flags & B::kTuned) { r.tune = SeqSlot::Tuning{sc.tune, {}}; std::copy(sc.align_R, sc.align_R + 9, r.tune->R); }
     any_configured |= r.cfg.has_value();
     if (!pb.bound) continue;
+    pb.fused[s] = lins_fused_pose{};  // (a last-step output: none until the slot's next publish)
     r.yzx = sc.yzx != 0;
     std::copy(sc.pose, sc.pose + 7, r.pose);
     MapperNode& m = ms.node[s];

@@ -89,6 +89,16 @@ class LinsMapperReport(C.Structure):
                 ("transform_aft_mapped", C.c_float * 6), ("map", LinsMapReport)]
 
 
+class LinsFusedPose(C.Structure):
+    """lins_fused_pose (include/lins_gpu.h): transform_fusion_node's pose of one odometry message."""
+    _fields_ = [("time", C.c_double), ("pos", C.c_double * 3), ("quat", C.c_double * 4), ("transform_mapped", C.c_float * 6),
+                ("valid", C.c_int32), ("pad", C.c_int32)]
+
+    def row(self):
+        """(x, y, z, qx, qy, qz, qw)"""
+        return list(self.pos) + list(self.quat)
+
+
 class LinsScanResult(C.Structure):
     _fields_ = [
         ("scan_id", C.c_int32),

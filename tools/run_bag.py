@@ -4,9 +4,11 @@
 BASELINE.json configs[1] runner (GPU box): replays a ROS1 bag through the restated front end (image projection, feature
 extraction, IMU propagation) and the GPU IESKF update, prints the trajectory.  With --map, every odometry output (what
 LinsFusion::publishTopics hands the mapping node: globalStateYZX_ and the YZX clouds) also runs one cycle of the device
-mapper (lins_gpu_mapper_step), and DIR/odometry.txt and DIR/mapped.txt receive the two trajectories, one line per
-published scan: stamp, then x y z qx qy qz qw of the odometry, resp. the processed flag and transformAftMapped (rx ry rz
-tx ty tz, the mapping node's YZX frame).  The replayed IMU messages are not fed to the mapper's roll / pitch queue (the
+mapper (lins_gpu_mapper_step), and DIR/odometry.txt, DIR/mapped.txt and DIR/integrated.txt receive three trajectories,
+one line per published scan: stamp, then x y z qx qy qz qw of the odometry, resp. the processed flag and
+transformAftMapped (rx ry rz tx ty tz, the mapping node's YZX frame), resp. x y z qx qy qz qw of transform_fusion_node's
+pose (/integrated_to_init in /camera_init: the odometry corrected by the last processed cycle before the scan,
+lins_gpu_mapper_fuse).  The replayed IMU messages are not fed to the mapper's roll / pitch queue (the
 front end reads their rates and accelerations only), so transformUpdate runs without the IMU blend.  Uncompressed and lz4-compressed bags
 are read directly; for bz2 run `python tools/bag_tool.py decompress IN.bag OUT.bag` first."""
 import argparse, importlib, os, sys
@@ -16,7 +18,7 @@ ap = argparse.ArgumentParser()
 ap.add_argument("bag"); ap.add_argument("--lidar", default="/velodyne_points"); ap.add_argument("--imu", default="/imu/data")
 ap.add_argument("--max-scans", type=int, default=0); ap.add_argument("--lidar-model", type=int, default=0)
 ap.add_argument("--map", action="store_true", help="run the mapping node's cycle after every odometry output")
-ap.add_argument("--out", default=".", help="with --map: directory for odometry.txt and mapped.txt")
+ap.add_argument("--out", default=".", help="with --map: directory for odometry.txt, mapped.txt and integrated.txt")
 a = ap.parse_args()
 synth = importlib.import_module("lins---lidar-inertial-slam_b200.synth")
 out = synth.run_bag(a.bag, a.lidar, a.imu, a.max_scans, a.lidar_model)
@@ -29,11 +31,14 @@ if a.map:
     g = capi.LinsGpu()
     g.mapper_reset()
     os.makedirs(a.out, exist_ok=True)
-    with open(os.path.join(a.out, "odometry.txt"), "w") as fo, open(os.path.join(a.out, "mapped.txt"), "w") as fm:
+    files = [os.path.join(a.out, f) for f in ("odometry.txt", "mapped.txt", "integrated.txt")]
+    with open(files[0], "w") as fo, open(files[1], "w") as fm, open(files[2], "w") as fi:
         for m in out["map_inputs"]:
+            fused = g.mapper_fuse(m["time"], m["quat"], m["pos"])  # (the fusion node sees the odometry before the cycle ends)
             rep = g.mapper_step(m["time"], m["quat"], m["pos"], m["corner"], m["surf"], m["outlier"])
             fo.write("%.9f %s\n" % (m["time"], " ".join("%.9g" % v for v in list(m["pos"]) + list(m["quat"]))))
             fm.write("%.9f %d %s\n" % (m["time"], rep.processed, " ".join("%.9g" % v for v in rep.transform_aft_mapped)))
+            fi.write("%.9f %s\n" % (m["time"], " ".join("%.9g" % v for v in fused.row())))
             last = rep
     print("mapper:", len(out["map_inputs"]), "odometry outputs,", last.n_keyframes if out["map_inputs"] else 0, "key frames;",
-          "trajectories in", os.path.join(a.out, "odometry.txt"), "and", os.path.join(a.out, "mapped.txt"))
+          "trajectories in", ", ".join(files[:2]), "and", files[2])

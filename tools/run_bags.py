@@ -9,8 +9,9 @@ with one value per bag (e.g. 0,1,1,0): bags of different sensors then run in one
 bag's model (lins_gpu_seq_step_cloud2_mixed).  Prints a summary line and the trajectory per bag, like run_bag.py; with
 --out, writes DIR/<bag name>.npz (stamps, status, scan_status, global_est, iters, flags per scan).  With --map, each
 bag's mapping node runs on what its estimator publishes, in lockstep on the device (lins_gpu_seq_map_step), and
-DIR/<bag name>.odometry.txt and DIR/<bag name>.mapped.txt (DIR: --out, default .) receive the two trajectories in
-tools/run_bag.py --map's line format; like run_bag.py --map, the bags' IMU orientation is not fed to the mappers.
+DIR/<bag name>.odometry.txt, DIR/<bag name>.mapped.txt and DIR/<bag name>.integrated.txt (DIR: --out, default .)
+receive the three trajectories in tools/run_bag.py --map's line format; like run_bag.py --map, the bags' IMU orientation
+is not fed to the mappers.
 --config a.yaml[,b.yaml,...] takes LINS config files (exp_port.yaml, OpenCV YAML): one for every bag or one per bag.
 Each bag's slot is configured with its file's rig (scan period, feature thresholds, extrinsic, IMU noise, init stds and
 biases); the files must agree on the keys every slot shares (num_iter, icp_freq, nearest_feature_search_sq_dist,
@@ -75,16 +76,18 @@ def bag_tunings(spec, n_bags):
 
 
 def write_map(o, out_dir, name):
-    """<name>.odometry.txt and <name>.mapped.txt of one replayed bag, one line per published scan as tools/run_bag.py --map
-    writes odometry.txt and mapped.txt: stamp, then x y z qx qy qz qw of the odometry, resp. the processed flag and
-    transformAftMapped."""
+    """<name>.odometry.txt, <name>.mapped.txt and <name>.integrated.txt of one replayed bag, one line per published scan as
+    tools/run_bag.py --map writes odometry.txt, mapped.txt and integrated.txt: stamp, then x y z qx qy qz qw of the
+    odometry, resp. the processed flag and transformAftMapped, resp. x y z qx qy qz qw of the fused pose."""
     os.makedirs(out_dir, exist_ok=True)
-    with open(os.path.join(out_dir, name + ".odometry.txt"), "w") as fo, open(os.path.join(out_dir, name + ".mapped.txt"), "w") as fm:
-        for t, od, pr, aft in zip(o["map_time"], o["map_odom"], o["map_processed"], o["map_aft_mapped"]):
+    files = [os.path.join(out_dir, name + ext) for ext in (".odometry.txt", ".mapped.txt", ".integrated.txt")]
+    with open(files[0], "w") as fo, open(files[1], "w") as fm, open(files[2], "w") as fi:
+        for t, od, pr, aft, fu in zip(o["map_time"], o["map_odom"], o["map_processed"], o["map_aft_mapped"], o["map_fused"]):
             fo.write("%.9f %s\n" % (t, " ".join("%.9g" % v for v in od)))
             fm.write("%.9f %d %s\n" % (t, pr, " ".join("%.9g" % v for v in aft)))
+            fi.write("%.9f %s\n" % (t, " ".join("%.9g" % v for v in fu)))
     print("mapper:", len(o["map_time"]), "odometry outputs,", len(o["key_poses"]), "key frames;", "trajectories in",
-          os.path.join(out_dir, name + ".odometry.txt"), "and", os.path.join(out_dir, name + ".mapped.txt"))
+          ", ".join(files[:2]), "and", files[2])
 
 
 def main(argv=None):

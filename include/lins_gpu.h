@@ -613,8 +613,9 @@ typedef struct lins_map_report {
 int lins_gpu_map_set(lins_ctx* ctx, const lins_point* corner_from_map, int n_corner, const lins_point* surf_from_map,
                      int n_surf);
 /* ≙ the iteration loop of scan2MapOptimization (:1640-1648): up to 10 x (cornerOptimization, surfOptimization,
-   LMOptimization) against the map set by lins_gpu_map_set; 5-NN search, line / plane fits, coefficients and the
-   A^T A / A^T B reduction on the device, the 6x6 step on the host.  transform_io: transformTobeMapped in / out.
+   LMOptimization) against the map set by lins_gpu_map_set; 5-NN search, line / plane fits, coefficients, the
+   A^T A / A^T B reduction and the 6x6 step on the device, one synchronisation per call.  transform_io:
+   transformTobeMapped in / out.
    (transformUpdate, :538-577, blends IMU roll / pitch afterwards and stays with the caller.) */
 int lins_gpu_scan2map(lins_ctx* ctx, const lins_point* corner_last, int n_corner, const lins_point* surf_last, int n_surf,
                       float* transform_io /*6*/, lins_map_report* rep);

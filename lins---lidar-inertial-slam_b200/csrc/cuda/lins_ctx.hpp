@@ -352,6 +352,24 @@ struct VoxelGridState {
   VgScratch w;
   Buf<VgInfo> info; Buf<VgInfo, kPinned> h_info;
 };
+// The scan-to-map refinement of a table of slots (lins_map.cu): the lockstep mappers' step, the single mapper's, and the
+// one slot of lins_gpu_map_set / scan2map / map_associate.  The layout is that of the table map_fill_table last filled.
+struct ScanToMap {
+  Buf<lins_map::MapLoopState> loop;          // per slot: the loop state (matP / isDegenerate persist)
+  Buf<lins_map::MapLoopState, kPinned> h_loop;
+  Buf<lins_map::PassConsts> consts;          // per slot: sin / cos + translation of the pass being run
+  Buf<lins_map::PassConsts, kPinned> h_consts;
+  Buf<lins_map::MapSlot> mslot;              // per slot: its maps, queries, grids and fit blocks
+  Buf<lins_map::MapSlot, kPinned> h_mslot;
+  Buf<int> blk_slot; Buf<int, kPinned> h_blk_slot;  // per fit block: its slot
+  Buf<int> grid_start, count, cursor;        // every slot's corner and surf buckets
+  Buf<float4> sorted;                        // every slot's map points, bucket-sorted
+  Buf<unsigned char> scan_temp;              // CUB scratch of the buckets' scan
+  Buf<float> part_d; Buf<int> part_i; Buf<double> partial;
+  int n_slots = 0, buckets = 0, points = 0;  // the layout: slots, buckets, map capacity in all
+  int blocks[2] = {0, 0};                    // fit blocks of the corner and the surf launch
+};
+
 // A run of mapping nodes in lockstep (lins_mappers.cu): the lockstep mappers (lins_gpu_mappers_*), or the single
 // mapper (lins_gpu_mapper_*) as a run of one slot.  One MapperNode per slot with its six DS clouds of the last
 // processed cycle (map corner, map surf, corner, surf, outlier, surf total), and the step's shared device buffers
@@ -359,23 +377,13 @@ struct MappersState {
   int n = 0;                                 // slots (0 = not opened)
   std::vector<MapperNode> node;
   std::vector<std::array<Buf<float4>, 6>> ds;
-  Buf<lins_map::MapLoopState> loop;          // per slot: the scan-to-map loop state (matP / isDegenerate persist)
-  Buf<lins_map::MapLoopState, kPinned> h_loop;
-  Buf<lins_map::PassConsts> consts;          // per slot
-  Buf<lins_map::PassConsts, kPinned> h_consts;
-  Buf<lins_map::MapSlot> mslot;              // per slot: the step's scan-to-map view
-  Buf<lins_map::MapSlot, kPinned> h_mslot;
-  Buf<int> blk_slot; Buf<int, kPinned> h_blk_slot;  // per fit block: its slot
+  ScanToMap stm;                             // a slot per mapping node
   Buf<float4> vin[2];                        // the VoxelGrids' inputs: round 1 (maps and scans), round 2 (surf total)
   Buf<float4, kPinned> h_in;
   VgScratch vg;
   Buf<VgInfo> vg_info; Buf<VgInfo, kPinned> h_vg_info, h_vg_init;
   Buf<int> vg_off; Buf<int, kPinned> h_vg_off;      // per round: S + 1 segment offsets
   Buf<float4*> vg_out; Buf<float4*, kPinned> h_vg_out;  // per round: S output clouds
-  Buf<int> grid_start, grid_count, grid_cursor;      // every slot's corner and surf buckets
-  Buf<float4> grid_sorted;
-  Buf<unsigned char> scan_temp;              // CUB scratch of the buckets' scan
-  Buf<float> part_d; Buf<int> part_i; Buf<double> partial;
   Buf<unsigned char> tf; Buf<unsigned char, kPinned> h_tf;  // the key frames' transform jobs
   CopyList copies;                           // the local maps' concatenation, then the surf-total one
 };
@@ -416,24 +424,14 @@ struct lins_ctx {
   Buf<lins_point, kPinned> h_out;  // pinned staging of the update_map read-back
   Buf<double> tmp_lin;
   Buf<float4, kPinned> h_tmp;
-  // row F2 (scan-to-map refinement): the map clouds, the current feature clouds, search / reduction scratch
+  // row F2 (lins_gpu_map_set / scan2map / map_associate): a one-slot scan-to-map table over the map clouds (their sizes on
+  // the device for MapSlot::n_map, on the host -1 before the first map_set) and the current feature clouds, and
+  // map_associate's dense outputs
   struct MapState {
     Buf<float4> map_c, map_s, q_c, q_s;
+    Buf<int> n_map;
     int n_map_c = -1, n_map_s = -1;
-    struct Grid {  // hashed uniform grid of one map cloud (lins_map.cuh: GridIndex)
-      Buf<float4> sorted;
-      Buf<int> start, count, cursor;
-      unsigned mask = 0;                      // buckets - 1
-      float origin[3] = {0.f, 0.f, 0.f};
-      int n = 0;
-    } grid_c, grid_s;
-    Buf<lins_map::MapLoopState> loop;   // device-resident state of one scan2map call
-    Buf<lins_map::MapLoopState, kPinned> h_loop;
-    Buf<lins_map::PassConsts> consts;   // sin / cos + translation of the pass being run
-    Buf<float> part_d;
-    Buf<int> part_i;
-    Buf<double> partial;
-    Buf<double, kPinned> h_partial;
+    lins_capi::ScanToMap stm;
     Buf<int32_t> knn_c, knn_s;
     Buf<float> coeff_c, coeff_s;
     Buf<uint8_t> mask_c, mask_s;
@@ -629,20 +627,18 @@ int upload_bytes(lins_ctx* ctx, void* dst, Buf<unsigned char, kPinned>& staging,
 // decoded and has no points), upload them and queue their decode into ctx->proj.up (qs, qs_off; no synchronisation).
 // off (n + 1) receives the host copy of qs_off.
 int cloud2_run(lins_ctx* ctx, const lins_cloud2_desc* d, const uint8_t* present, std::vector<int32_t>& off);
-// lins_map.cu: the grid origin of a host cloud; bucket-sort n device map points into g; queue the scan-to-map loop on
-// the queries in ctx->mp.q_c / q_s (nc, ns) from transform T, with the loop state's D2H into mp.h_loop (no
-// synchronisation); read a loop state into T and a report
-void map_grid_origin(const lins_point* host_pts, int n, float origin[3]);
-int map_build_grid(lins_ctx* ctx, lins_ctx::MapState::Grid& g, const float4* map, int n, const float origin[3]);
-int map_queue_loop(lins_ctx* ctx, int nc, int ns, const float* T);
+// lins_map.cu: the scan-to-map refinement of a table of n_slots slots in sm.  map_fill_table: sm.h_mslot (pinned,
+// n_slots) holds each slot's map and query clouds, capacities, device map counts, grid origins, start transform and run
+// flag; fills the rest of the table (bucket ranges, point numbering, fit blocks, blk_slot, pass constants), reserves sm's
+// buffers and queues the H2D of the table.  map_queue_grids: every slot's two grids in one bucket array (one count, one
+// CUB scan, one scatter).  map_queue_loop: the start / gate kernel (a slot with run = 0 starts done), LINS_MAP_MAX_ITER
+// passes of one 5-NN and one fit launch per kind over all slots and one LM launch with a warp per slot, then the loop
+// states' D2H into sm.h_loop; sm.loop (n_slots) keeps each slot's matP / isDegenerate.  Nothing is synchronised.
+// map_loop_report: a loop state into T and a report.
+int map_fill_table(lins_ctx* ctx, ScanToMap& sm, int n_slots);
+int map_queue_grids(lins_ctx* ctx, ScanToMap& sm);
+int map_queue_loop(lins_ctx* ctx, ScanToMap& sm);
 void map_loop_report(const lins_map::MapLoopState& st, float* T, lins_map_report* rep);
-// lins_map.cu: the scan-to-map loops of many slots in one queue (the mapping nodes' step).  ms.h_mslot (pinned, n_slots)
-// holds each slot's map and query clouds, capacities, device map counts, start transform and run flag; the rest of the
-// table is filled here.  Queued: every slot's two grids in one bucket array (one count, one CUB scan, one scatter), the
-// start / gate kernel (a slot with run = 0 starts done), and LINS_MAP_MAX_ITER passes of one 5-NN and one fit launch per
-// kind over all slots and one LM launch with a warp per slot; then the loop states' D2H into ms.h_loop.  Nothing is
-// synchronised; ms.loop (n_slots) keeps each slot's matP / isDegenerate.
-int map_queue_slots(lins_ctx* ctx, MappersState& ms, int n_slots);
 // lins_mapper.cu: queue pcl::VoxelGrid of n_seg segments of the device points `in` (segment k: [h_off[k], h_off[k + 1]),
 // leaf[k]) into outputs with room for each segment's points (out for one segment; else the device table d_out, with
 // d_off the device copy of h_off), the records at info (device, n_seg; their initial values staged through h_init, pinned,

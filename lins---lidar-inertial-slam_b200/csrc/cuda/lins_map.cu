@@ -1,5 +1,6 @@
 // lins_map.cu — host side of row F2 (SURVEY.md §8(f)): the mapping node's scan-to-map refinement, whose kernels are in
-// lins_map.cuh.
+// lins_map.cuh.  One driver over a table of slots (ScanToMap): the host fills the table, then queues the grid build and
+// the loop.  The mapping nodes run a slot each; lins_gpu_map_set / scan2map / map_associate run the one slot of ctx->mp.
 #include <cuda_runtime.h>
 #include <cub/device/device_scan.cuh>
 
@@ -26,113 +27,40 @@ lins_map::PassConsts host_pass_consts(const float* T) {  // libm sin / cos in f3
   return pc;
 }
 
-// which 5-NN search a pass uses: the hashed grid (exact for every point that can be accepted) or the brute-force slices
-// (exact for every point).  LINS_MAP_KNN=grid|brute overrides the caller's default.
-bool map_use_grid(bool dflt) {
+// which 5-NN search map_associate's pass uses: the hashed grid (exact for every point that can be accepted) or the
+// brute-force slices (exact for every point, the default).  LINS_MAP_KNN=grid|brute overrides it; the loop always
+// searches the grid.
+bool map_use_grid() {
   const char* e = std::getenv("LINS_MAP_KNN");  // (read per call: tests flip it between calls)
-  return !e || !*e ? dflt : std::strcmp(e, "grid") == 0;
+  return e && std::strcmp(e, "grid") == 0;
 }
-
-// the kernels' view of a grid (lins_ctx.hpp keeps its parts: that header cannot include lins_map.cuh)
-lins_map::GridIndex grid_index(const lins_ctx::MapState::Grid& g) {
-  lins_map::GridIndex gi;
-  gi.pts = g.sorted.p; gi.start = g.start.p; gi.mask = g.mask; gi.ox = g.origin[0]; gi.oy = g.origin[1]; gi.oz = g.origin[2];
-  return gi;
-}
-
-}  // namespace
-
-namespace lins_capi {
 
 // the grid origin of a host cloud: its finite minimum (cells are addressed by hash: the extent does not matter)
-void map_grid_origin(const lins_point* host_pts, int n, float origin[3]) {
+void map_grid_origin(const lins_point* host_pts, int n, lins_map::GridIndex& g) {
   float mn[3] = {3.0e38f, 3.0e38f, 3.0e38f};
   for (int i = 0; i < n; ++i) {
     const float v[3] = {host_pts[i].x, host_pts[i].y, host_pts[i].z};
     for (int k = 0; k < 3; ++k) if (v[k] == v[k] && std::fabs(v[k]) < 1.0e30f && v[k] < mn[k]) mn[k] = v[k];
   }
-  for (int k = 0; k < 3; ++k) origin[k] = mn[k] < 3.0e38f ? mn[k] : 0.f;
+  for (int k = 0; k < 3; ++k) mn[k] = mn[k] < 3.0e38f ? mn[k] : 0.f;
+  g.ox = mn[0]; g.oy = mn[1]; g.oz = mn[2];
 }
 
-// bucket-sort one device-resident map cloud into its grid (≙ kdtree*FromMap->setInputCloud, :1637-1638).  Any finite
-// origin gives the same 5-NN: the cells are exact (lins_map.cuh: grid_cell) and addressed by hash.
-int map_build_grid(lins_ctx* ctx, lins_ctx::MapState::Grid& g, const float4* map, int n, const float origin[3]) {
+// the 5-NN of kind k (0 corner, 1 surf) through every slot's grid, for the table's fit blocks
+void queue_knn_grid(lins_ctx* ctx, const ScanToMap& sm, int k, const lins_map::MapLoopState* st) {
   using namespace lins_map;
-  g.n = n;
-  if (n <= 0) return LINS_OK;
-  unsigned nb = 4096;
-  while (nb < 2u * (unsigned)n && nb < (1u << 24)) nb <<= 1;
-  CK(g.start.reserve((size_t)nb + 2)); CK(g.count.reserve((size_t)nb + 2)); CK(g.cursor.reserve((size_t)nb + 2)); CK(g.sorted.reserve((size_t)n + 1));
-  g.mask = nb - 1;
-  for (int k = 0; k < 3; ++k) g.origin[k] = origin[k];
-  const GridIndex gi = grid_index(g);
-  CK(cudaMemsetAsync(g.count.p, 0, sizeof(int) * nb, ctx->stream));
-  lins_grid_count_kernel<<<(n + 255) / 256, 256, 0, ctx->stream>>>(map, n, gi, g.count.p, nullptr, 0);
-  lins_grid_scan_kernel<<<1, 1024, 0, ctx->stream>>>(g.count.p, g.start.p, g.cursor.p, (int)nb);
-  lins_grid_scatter_kernel<<<(n + 255) / 256, 256, 0, ctx->stream>>>(map, n, gi, g.cursor.p, g.sorted.p, nullptr, 0);
-  CK(cudaGetLastError());
-  ctx->launches += 3;
-  return LINS_OK;
+  lins_map_knn_grid_kernel<<<sm.blocks[k] * kFitThreads / kGridKnnWarps, kGridKnnWarps * 32, 0, ctx->stream>>>(
+      sm.blocks[k] * kFitThreads, sm.consts.p, st, sm.part_d.p, sm.part_i.p, sm.mslot.p, sm.n_slots, sm.blk_slot.p + (k ? sm.blocks[0] : 0), k);
 }
 
-}  // namespace lins_capi
-
-namespace {
-
-// queue one cornerOptimization + surfOptimization pass (5-NN, fits, block partials) that reads its constants from
-// m.consts (device); nothing is synchronised.  Returns the number of partial blocks.
-int map_queue_pass(lins_ctx* ctx, int nc, int ns, bool dense, bool grid, const lins_map::MapLoopState* st, int* nblocks_out) {
+// the fits and block partials of kind k over n_slices partial lists per row, with dense outputs where non-null
+void queue_fit(lins_ctx* ctx, const ScanToMap& sm, int k, int n_slices, const lins_map::MapLoopState* st, int32_t* knn, float* coeff,
+               uint8_t* mask) {
   using namespace lins_map;
-  lins_ctx::MapState& m = ctx->mp;
-  const int qb[2] = {(nc + kKnnThreads - 1) / kKnnThreads, (ns + kKnnThreads - 1) / kKnnThreads};
-  const int nq[2] = {nc, ns}, nm[2] = {std::max(m.n_map_c, 0), std::max(m.n_map_s, 0)};
-  const float4* q[2] = {m.q_c.p, m.q_s.p};
-  const float4* mp[2] = {m.map_c.p, m.map_s.p};
-  const lins_ctx::MapState::Grid* gr[2] = {&m.grid_c, &m.grid_s};
-  int slices[2], slice_len[2];
-  size_t part = 0;
-  for (int k = 0; k < 2; ++k) {
-    // brute force: enough (query block, map slice) pairs for ~8 CTAs per SM (the scan is latency bound: profiles/r01_map_*);
-    // a slice is at least 256 map points.  grid: one list per query
-    int S = qb[k] > 0 ? (8 * ctx->sm_count + qb[k] - 1) / qb[k] : 1;
-    S = std::max(1, std::min(S, std::min(64, (nm[k] + 255) / 256)));
-    if (grid) S = 1;
-    slices[k] = S;
-    slice_len[k] = std::max(1, (nm[k] + S - 1) / S);
-    part = std::max(part, (size_t)nq[k] * S * 5);
-  }
-  CK(m.part_d.reserve(part + 1)); CK(m.part_i.reserve(part + 1));
-  const int nblocks = qb[0] + qb[1];
-  CK(m.partial.reserve((size_t)(nblocks + 1) * (kRowAcc + 1))); CK(m.h_partial.reserve((size_t)(nblocks + 1) * (kRowAcc + 1)));
-  if (dense) {
-    CK(m.knn_c.reserve(5 * (size_t)nc + 1)); CK(m.knn_s.reserve(5 * (size_t)ns + 1)); CK(m.coeff_c.reserve(4 * (size_t)nc + 1));
-    CK(m.coeff_s.reserve(4 * (size_t)ns + 1)); CK(m.mask_c.reserve((size_t)nc + 1)); CK(m.mask_s.reserve((size_t)ns + 1));
-  }
-  for (int k = 0; k < 2; ++k) {
-    if (nq[k] == 0) continue;
-    if (grid && nm[k] > 0)
-      lins_map_knn_grid_kernel<<<(nq[k] + kGridKnnWarps - 1) / kGridKnnWarps, kGridKnnWarps * 32, 0, ctx->stream>>>(q[k], nq[k], grid_index(*gr[k]), m.consts.p, st, m.part_d.p, m.part_i.p, nullptr, nullptr, k);
-    else
-      lins_map_knn_kernel<<<dim3(qb[k], slices[k]), kKnnThreads, 0, ctx->stream>>>(q[k], nq[k], mp[k], nm[k], slice_len[k], m.consts.p, st, m.part_d.p, m.part_i.p);
-    double* partial = m.partial.p + (size_t)(k == 0 ? 0 : qb[0]) * (kRowAcc + 1);
-    if (k == 0)
-      lins_map_fit_kernel<true><<<qb[k], kFitThreads, 0, ctx->stream>>>(q[k], nq[k], mp[k], slices[k], m.part_d.p, m.part_i.p, m.consts.p, st, dense ? m.knn_c.p : nullptr,
-                                                                       dense ? m.coeff_c.p : nullptr, dense ? m.mask_c.p : nullptr, partial, nullptr, nullptr);
-    else
-      lins_map_fit_kernel<false><<<qb[k], kFitThreads, 0, ctx->stream>>>(q[k], nq[k], mp[k], slices[k], m.part_d.p, m.part_i.p, m.consts.p, st, dense ? m.knn_s.p : nullptr,
-                                                                        dense ? m.coeff_s.p : nullptr, dense ? m.mask_s.p : nullptr, partial, nullptr, nullptr);
-    CK(cudaGetLastError());
-    ctx->launches += 2;
-  }
-  *nblocks_out = nblocks;
-  return LINS_OK;
-}
-
-int map_stage_queries(lins_ctx* ctx, const lins_point* corner, int nc, const lins_point* surf, int ns) {
-  if (check_cloud(ctx, corner, nc, "bad corner feature cloud") != LINS_OK || check_cloud(ctx, surf, ns, "bad surf feature cloud") != LINS_OK)
-    return LINS_E_INVALID;
-  if (ctx->mp.n_map_c < 0) return fail(ctx, LINS_E_NOMAP, "lins_gpu_map_set has not been called");
-  return upload2(ctx, ctx->mp.q_c, corner, nc, ctx->mp.q_s, surf, ns);
+  const size_t b0 = k ? sm.blocks[0] : 0;
+  auto* fit = k ? lins_map_fit_kernel<false> : lins_map_fit_kernel<true>;
+  fit<<<sm.blocks[k], kFitThreads, 0, ctx->stream>>>(n_slices, sm.part_d.p, sm.part_i.p, sm.consts.p, st, knn, coeff, mask,
+                                                     sm.partial.p + b0 * (kRowAcc + 1), sm.mslot.p, sm.n_slots, sm.blk_slot.p + b0);
 }
 
 }  // namespace
@@ -154,40 +82,10 @@ __global__ void lins_map_gate_kernel(lins_map::MapLoopState* __restrict__ st, co
 
 namespace lins_capi {
 
-// the iteration loop of scan2MapOptimization (:1640-1648) on the queries in ctx->mp.q_c / q_s and the map set up
-// in ctx->mp, queued up front with the loop state's D2H into mp.h_loop; nothing is synchronised
-int map_queue_loop(lins_ctx* ctx, int nc, int ns, const float* T) {
+int map_fill_table(lins_ctx* ctx, ScanToMap& sm, int n_slots) {
   using namespace lins_map;
-  lins_ctx::MapState& m = ctx->mp;
-  // The whole iteration loop (:1640-1648) is queued up front: transformTobeMapped, matP / isDegenerate and the report live
-  // on the device (MapLoopState); the first pass uses libm sin / cos of the caller's transform (bit-identical to the
-  // reference's first pass), later ones the constants the LM kernel derived on the device.
-  if (!m.loop.p) {  // isDegenerate / matP are members of the reference's mapping node (:226-227, :395-396): they survive the
-    CK(m.loop.reserve(1));  // calls — a call whose first pass selects < 50 points keeps using the previous scan's values
-    CK(cudaMemsetAsync(m.loop.p, 0, sizeof(MapLoopState), ctx->stream));
-  }
-  CK(m.h_loop.reserve(1)); CK(m.consts.reserve(1));
-  const PassConsts pc0 = host_pass_consts(T);
-  CK(cudaMemcpyAsync(m.loop.p, T, sizeof(float) * 6, cudaMemcpyHostToDevice, ctx->stream));  // (pageable sources: staged before the call returns)
-  CK(cudaMemsetAsync(reinterpret_cast<char*>(m.loop.p) + offsetof(MapLoopState, done), 0, sizeof(MapLoopState) - offsetof(MapLoopState, done), ctx->stream));
-  CK(cudaMemcpyAsync(m.consts.p, &pc0, sizeof(pc0), cudaMemcpyHostToDevice, ctx->stream));
-  const bool grid = map_use_grid(true);
-  for (int iter = 0; iter < LINS_MAP_MAX_ITER; ++iter) {
-    int nblocks = 0;
-    const int rc = map_queue_pass(ctx, nc, ns, false, grid, m.loop.p, &nblocks);
-    if (rc != LINS_OK) return rc;
-    lins_map_lm_kernel<<<1, 32, 0, ctx->stream>>>(m.partial.p, nblocks, iter, m.loop.p, m.consts.p, nullptr);
-    CK(cudaGetLastError());
-    ctx->launches += 1;
-  }
-  CK(cudaMemcpyAsync(m.h_loop.p, m.loop.p, sizeof(MapLoopState), cudaMemcpyDeviceToHost, ctx->stream));
-  return LINS_OK;
-}
-
-int map_queue_slots(lins_ctx* ctx, MappersState& ms, int n_slots) {
-  using namespace lins_map;
-  MapSlot* h = ms.h_mslot.p;
-  // per slot: map_build_grid's bucket rule for each map, fit blocks that start with the slot's queries
+  MapSlot* h = sm.h_mslot.p;
+  // per slot: each map's bucket count from its capacity, fit blocks that start with the slot's queries
   int nb_tot = 0, pts = 0, blocks[2] = {0, 0};
   std::vector<int> blk_slot[2];
   for (int s = 0; s < n_slots; ++s) {
@@ -195,7 +93,7 @@ int map_queue_slots(lins_ctx* ctx, MappersState& ms, int n_slots) {
     for (int k = 0; k < 2; ++k) {
       unsigned nb = v.run ? 4096 : 1;  // (a slot that does not run searches nothing)
       while (v.run && nb < 2u * (unsigned)v.cap[k] && nb < (1u << 24)) nb <<= 1;
-      v.g[k].mask = nb - 1; v.g[k].ox = v.g[k].oy = v.g[k].oz = 0.f;  // (any finite origin gives the same 5-NN)
+      v.g[k].mask = nb - 1;
       v.bucket0[k] = nb_tot; nb_tot += (int)nb;
       v.m0[k] = pts; pts += v.cap[k];
       v.blk[k] = blocks[k];
@@ -205,58 +103,61 @@ int map_queue_slots(lins_ctx* ctx, MappersState& ms, int n_slots) {
     }
   }
   size_t scan_bytes = 0;
-  CK(cub::DeviceScan::ExclusiveSum(nullptr, scan_bytes, ms.grid_count.p, ms.grid_start.p, nb_tot + 1, ctx->stream));
-  CK(ms.scan_temp.grow(scan_bytes + 16));
-  CK(ms.grid_start.grow((size_t)nb_tot + 2)); CK(ms.grid_count.grow((size_t)nb_tot + 2)); CK(ms.grid_cursor.grow((size_t)nb_tot + 2));
-  CK(ms.grid_sorted.grow((size_t)pts + 1));
+  CK(cub::DeviceScan::ExclusiveSum(nullptr, scan_bytes, sm.count.p, sm.grid_start.p, nb_tot + 1, ctx->stream));
+  CK(sm.scan_temp.grow(scan_bytes + 16));
+  CK(sm.grid_start.grow((size_t)nb_tot + 2)); CK(sm.count.grow((size_t)nb_tot + 2)); CK(sm.cursor.grow((size_t)nb_tot + 2));
+  CK(sm.sorted.grow((size_t)pts + 1));
   const size_t rows = (size_t)std::max(blocks[0], blocks[1]) * kFitThreads;
-  CK(ms.part_d.grow(5 * rows + 1)); CK(ms.part_i.grow(5 * rows + 1));
-  CK(ms.partial.grow((size_t)(blocks[0] + blocks[1] + 1) * (kRowAcc + 1)));
-  CK(ms.blk_slot.grow((size_t)blocks[0] + blocks[1] + 1)); CK(ms.h_blk_slot.grow((size_t)blocks[0] + blocks[1] + 1));
-  CK(ms.consts.grow(n_slots)); CK(ms.h_consts.grow(n_slots)); CK(ms.mslot.grow(n_slots));
+  CK(sm.part_d.grow(5 * rows + 1)); CK(sm.part_i.grow(5 * rows + 1));
+  CK(sm.partial.grow((size_t)(blocks[0] + blocks[1] + 1) * (kRowAcc + 1)));
+  CK(sm.blk_slot.grow((size_t)blocks[0] + blocks[1] + 1)); CK(sm.h_blk_slot.grow((size_t)blocks[0] + blocks[1] + 1));
+  CK(sm.consts.grow(n_slots)); CK(sm.h_consts.grow(n_slots)); CK(sm.mslot.grow(n_slots));
   for (int s = 0; s < n_slots; ++s) {
-    for (int k = 0; k < 2; ++k) { h[s].g[k].pts = ms.grid_sorted.p; h[s].g[k].start = ms.grid_start.p + h[s].bucket0[k]; }
-    ms.h_consts.p[s] = host_pass_consts(h[s].T);
+    for (int k = 0; k < 2; ++k) { h[s].g[k].pts = sm.sorted.p; h[s].g[k].start = sm.grid_start.p + h[s].bucket0[k]; }
+    sm.h_consts.p[s] = host_pass_consts(h[s].T);
   }
-  std::copy(blk_slot[0].begin(), blk_slot[0].end(), ms.h_blk_slot.p);
-  std::copy(blk_slot[1].begin(), blk_slot[1].end(), ms.h_blk_slot.p + blocks[0]);
-  CK(cudaMemcpyAsync(ms.mslot.p, h, sizeof(MapSlot) * n_slots, cudaMemcpyHostToDevice, ctx->stream));
-  CK(cudaMemcpyAsync(ms.consts.p, ms.h_consts.p, sizeof(PassConsts) * n_slots, cudaMemcpyHostToDevice, ctx->stream));
+  std::copy(blk_slot[0].begin(), blk_slot[0].end(), sm.h_blk_slot.p);
+  std::copy(blk_slot[1].begin(), blk_slot[1].end(), sm.h_blk_slot.p + blocks[0]);
+  CK(cudaMemcpyAsync(sm.mslot.p, h, sizeof(MapSlot) * n_slots, cudaMemcpyHostToDevice, ctx->stream));
+  CK(cudaMemcpyAsync(sm.consts.p, sm.h_consts.p, sizeof(PassConsts) * n_slots, cudaMemcpyHostToDevice, ctx->stream));
   if (blocks[0] + blocks[1])
-    CK(cudaMemcpyAsync(ms.blk_slot.p, ms.h_blk_slot.p, sizeof(int) * (blocks[0] + blocks[1]), cudaMemcpyHostToDevice, ctx->stream));
-  // every slot's two grids: one count, one scan of all buckets, one scatter
-  CK(cudaMemsetAsync(ms.grid_count.p, 0, sizeof(int) * ((size_t)nb_tot + 1), ctx->stream));
-  const GridIndex g0{};
-  if (pts) lins_grid_count_kernel<<<(pts + 255) / 256, 256, 0, ctx->stream>>>(nullptr, pts, g0, ms.grid_count.p, ms.mslot.p, n_slots);
-  size_t bytes = ms.scan_temp.cap;
-  CK(cub::DeviceScan::ExclusiveSum(ms.scan_temp.p, bytes, ms.grid_count.p, ms.grid_start.p, nb_tot + 1, ctx->stream));
-  CK(cudaMemcpyAsync(ms.grid_cursor.p, ms.grid_start.p, sizeof(int) * nb_tot, cudaMemcpyDeviceToDevice, ctx->stream));
-  if (pts) lins_grid_scatter_kernel<<<(pts + 255) / 256, 256, 0, ctx->stream>>>(nullptr, pts, g0, ms.grid_cursor.p, ms.grid_sorted.p, ms.mslot.p, n_slots);
-  lins_map_gate_kernel<<<(n_slots + 127) / 128, 128, 0, ctx->stream>>>(ms.loop.p, ms.mslot.p, n_slots);
+    CK(cudaMemcpyAsync(sm.blk_slot.p, sm.h_blk_slot.p, sizeof(int) * (blocks[0] + blocks[1]), cudaMemcpyHostToDevice, ctx->stream));
+  sm.n_slots = n_slots; sm.buckets = nb_tot; sm.points = pts; sm.blocks[0] = blocks[0]; sm.blocks[1] = blocks[1];
+  return LINS_OK;
+}
+
+int map_queue_grids(lins_ctx* ctx, ScanToMap& sm) {
+  using namespace lins_map;
+  const int pts = sm.points, nb = sm.buckets;
+  CK(cudaMemsetAsync(sm.count.p, 0, sizeof(int) * ((size_t)nb + 1), ctx->stream));
+  if (pts) lins_grid_count_kernel<<<(pts + 255) / 256, 256, 0, ctx->stream>>>(pts, sm.count.p, sm.mslot.p, sm.n_slots);
+  size_t bytes = sm.scan_temp.cap;
+  CK(cub::DeviceScan::ExclusiveSum(sm.scan_temp.p, bytes, sm.count.p, sm.grid_start.p, nb + 1, ctx->stream));
+  CK(cudaMemcpyAsync(sm.cursor.p, sm.grid_start.p, sizeof(int) * nb, cudaMemcpyDeviceToDevice, ctx->stream));
+  if (pts) lins_grid_scatter_kernel<<<(pts + 255) / 256, 256, 0, ctx->stream>>>(pts, sm.cursor.p, sm.sorted.p, sm.mslot.p, sm.n_slots);
   CK(cudaGetLastError());
-  ctx->launches += pts ? 4 : 2;
-  // the loop: per pass one 5-NN and one fit launch per kind over every slot, one LM launch of a warp per slot
-  double* partial_s = ms.partial.p + (size_t)blocks[0] * (kRowAcc + 1);
+  ctx->launches += pts ? 3 : 1;
+  return LINS_OK;
+}
+
+int map_queue_loop(lins_ctx* ctx, ScanToMap& sm) {
+  using namespace lins_map;
+  lins_map_gate_kernel<<<(sm.n_slots + 127) / 128, 128, 0, ctx->stream>>>(sm.loop.p, sm.mslot.p, sm.n_slots);
+  CK(cudaGetLastError());
+  ctx->launches += 1;
+  // per pass one 5-NN and one fit launch per kind over every slot, one LM launch of a warp per slot
   for (int iter = 0; iter < LINS_MAP_MAX_ITER; ++iter) {
-    if (blocks[0]) {
-      lins_map_knn_grid_kernel<<<blocks[0] * kFitThreads / kGridKnnWarps, kGridKnnWarps * 32, 0, ctx->stream>>>(
-          nullptr, blocks[0] * kFitThreads, g0, ms.consts.p, ms.loop.p, ms.part_d.p, ms.part_i.p, ms.mslot.p, ms.blk_slot.p, 0);
-      lins_map_fit_kernel<true><<<blocks[0], kFitThreads, 0, ctx->stream>>>(nullptr, 0, nullptr, 1, ms.part_d.p, ms.part_i.p, ms.consts.p, ms.loop.p,
-                                                                            nullptr, nullptr, nullptr, ms.partial.p, ms.mslot.p, ms.blk_slot.p);
+    for (int k = 0; k < 2; ++k) {
+      if (!sm.blocks[k]) continue;
+      queue_knn_grid(ctx, sm, k, sm.loop.p);
+      queue_fit(ctx, sm, k, 1, sm.loop.p, nullptr, nullptr, nullptr);
       ctx->launches += 2;
     }
-    if (blocks[1]) {
-      lins_map_knn_grid_kernel<<<blocks[1] * kFitThreads / kGridKnnWarps, kGridKnnWarps * 32, 0, ctx->stream>>>(
-          nullptr, blocks[1] * kFitThreads, g0, ms.consts.p, ms.loop.p, ms.part_d.p, ms.part_i.p, ms.mslot.p, ms.blk_slot.p + blocks[0], 1);
-      lins_map_fit_kernel<false><<<blocks[1], kFitThreads, 0, ctx->stream>>>(nullptr, 0, nullptr, 1, ms.part_d.p, ms.part_i.p, ms.consts.p, ms.loop.p,
-                                                                             nullptr, nullptr, nullptr, partial_s, ms.mslot.p, ms.blk_slot.p + blocks[0]);
-      ctx->launches += 2;
-    }
-    lins_map_lm_kernel<<<n_slots, 32, 0, ctx->stream>>>(ms.partial.p, blocks[0], iter, ms.loop.p, ms.consts.p, ms.mslot.p);
+    lins_map_lm_kernel<<<sm.n_slots, 32, 0, ctx->stream>>>(sm.partial.p, sm.blocks[0], iter, sm.loop.p, sm.consts.p, sm.mslot.p);
     CK(cudaGetLastError());
     ctx->launches += 1;
   }
-  CK(cudaMemcpyAsync(ms.h_loop.p, ms.loop.p, sizeof(MapLoopState) * n_slots, cudaMemcpyDeviceToHost, ctx->stream));
+  CK(cudaMemcpyAsync(sm.h_loop.p, sm.loop.p, sizeof(MapLoopState) * sm.n_slots, cudaMemcpyDeviceToHost, ctx->stream));
   return LINS_OK;
 }
 
@@ -274,6 +175,25 @@ void map_loop_report(const lins_map::MapLoopState& st, float* T, lins_map_report
 
 }  // namespace lins_capi
 
+namespace {
+
+// the queries of the one-slot table in ctx->mp (lins_gpu_map_set has set its maps): checked, uploaded and, with the start
+// transform T, in the table, which is filled and uploaded
+int map_stage_queries(lins_ctx* ctx, const lins_point* corner, int nc, const lins_point* surf, int ns, const float* T) {
+  if (check_cloud(ctx, corner, nc, "bad corner feature cloud") != LINS_OK || check_cloud(ctx, surf, ns, "bad surf feature cloud") != LINS_OK)
+    return LINS_E_INVALID;
+  lins_ctx::MapState& m = ctx->mp;
+  if (m.n_map_c < 0) return fail(ctx, LINS_E_NOMAP, "lins_gpu_map_set has not been called");
+  const int rc = upload2(ctx, m.q_c, corner, nc, m.q_s, surf, ns);
+  if (rc != LINS_OK) return rc;
+  lins_map::MapSlot& v = m.stm.h_mslot.p[0];
+  v.q[0] = m.q_c.p; v.q[1] = m.q_s.p; v.nq[0] = nc; v.nq[1] = ns;
+  for (int i = 0; i < 6; ++i) v.T[i] = T[i];
+  return map_fill_table(ctx, m.stm, 1);
+}
+
+}  // namespace
+
 extern "C" {
 
 int lins_gpu_map_set(lins_ctx* ctx, const lins_point* corner, int nc, const lins_point* surf, int ns) {
@@ -281,15 +201,26 @@ int lins_gpu_map_set(lins_ctx* ctx, const lins_point* corner, int nc, const lins
   if (check_cloud(ctx, corner, nc, "bad corner map cloud") != LINS_OK || check_cloud(ctx, surf, ns, "bad surf map cloud") != LINS_OK)
     return LINS_E_INVALID;
   CK(cudaSetDevice(ctx->device));
-  int rc = upload2(ctx, ctx->mp.map_c, corner, nc, ctx->mp.map_s, surf, ns);
+  lins_ctx::MapState& m = ctx->mp;
+  int rc = upload2(ctx, m.map_c, corner, nc, m.map_s, surf, ns);
   if (rc != LINS_OK) return rc;
-  ctx->mp.n_map_c = nc; ctx->mp.n_map_s = ns;
-  float oc[3], os[3];
-  map_grid_origin(corner, nc, oc);
-  map_grid_origin(surf, ns, os);
-  rc = map_build_grid(ctx, ctx->mp.grid_c, ctx->mp.map_c.p, nc, oc);
-  if (rc != LINS_OK) return rc;
-  return map_build_grid(ctx, ctx->mp.grid_s, ctx->mp.map_s.p, ns, os);
+  const int n[2] = {nc, ns};
+  CK(m.n_map.reserve(2));
+  CK(cudaMemcpyAsync(m.n_map.p, n, sizeof(n), cudaMemcpyHostToDevice, ctx->stream));  // (pageable: staged before the call returns)
+  m.n_map_c = nc; m.n_map_s = ns;
+  // a one-slot table whose maps' capacities are their sizes, each grid's origin its cloud's finite minimum
+  CK(m.stm.h_mslot.reserve(1));
+  lins_map::MapSlot& v = m.stm.h_mslot.p[0];
+  std::memset(&v, 0, sizeof(v));
+  v.run = 1;
+  const lins_point* src[2] = {corner, surf};
+  for (int k = 0; k < 2; ++k) {
+    v.map[k] = (k ? m.map_s : m.map_c).p; v.cap[k] = n[k]; v.n_map[k] = m.n_map.p + k;
+    map_grid_origin(src[k], n[k], v.g[k]);
+  }
+  if ((rc = map_fill_table(ctx, m.stm, 1)) != LINS_OK || (rc = map_queue_grids(ctx, m.stm)) != LINS_OK) return rc;
+  CK(cudaStreamSynchronize(ctx->stream));  // (the next call rewrites the table's pinned staging)
+  return LINS_OK;
 }
 
 int lins_gpu_scan2map(lins_ctx* ctx, const lins_point* corner, int nc, const lins_point* surf, int ns, float* T, lins_map_report* rep) {
@@ -305,31 +236,63 @@ int lins_gpu_scan2map(lins_ctx* ctx, const lins_point* corner, int nc, const lin
     if (rep) *rep = r;
     return LINS_OK;
   }
-  int rc = map_stage_queries(ctx, corner, nc, surf, ns);
+  int rc = map_stage_queries(ctx, corner, nc, surf, ns, T);
   if (rc != LINS_OK) return rc;
-  rc = map_queue_loop(ctx, nc, ns, T);
-  if (rc != LINS_OK) return rc;
+  ScanToMap& sm = m.stm;
+  // isDegenerate / matP are members of the reference's mapping node (:226-227, :395-396): they start at 0 and survive the
+  // calls — a call whose first pass selects < 50 points keeps using the previous scan's values
+  if (!sm.loop.p) {
+    CK(sm.loop.reserve(1)); CK(sm.h_loop.reserve(1));
+    CK(cudaMemsetAsync(sm.loop.p, 0, sizeof(lins_map::MapLoopState), ctx->stream));
+  }
+  if ((rc = map_queue_loop(ctx, sm)) != LINS_OK) return rc;
   CK(cudaStreamSynchronize(ctx->stream));
-  map_loop_report(*m.h_loop.p, T, &r);
+  map_loop_report(*sm.h_loop.p, T, &r);
   if (rep) *rep = r;
   return LINS_OK;
 }
 
 int lins_gpu_map_associate(lins_ctx* ctx, const lins_point* corner, int nc, const lins_point* surf, int ns, const float* T,
                            int32_t* cknn, int32_t* sknn, float* ccoeff, float* scoeff, uint8_t* cmask, uint8_t* smask) {
+  using namespace lins_map;
   if (!ctx) return LINS_E_INVALID;
   if (!T) return fail(ctx, LINS_E_INVALID, "null transform");
   CK(cudaSetDevice(ctx->device));
-  int rc = map_stage_queries(ctx, corner, nc, surf, ns);
+  int rc = map_stage_queries(ctx, corner, nc, surf, ns, T);
   if (rc != LINS_OK) return rc;
   lins_ctx::MapState& m = ctx->mp;
-  CK(m.consts.reserve(1));
-  const lins_map::PassConsts pc = host_pass_consts(T);
-  CK(cudaMemcpyAsync(m.consts.p, &pc, sizeof(pc), cudaMemcpyHostToDevice, ctx->stream));
-  int nblocks = 0;
-  // the parity hook: brute force by default (exact neighbours for EVERY point, also those the 1 m gate rejects)
-  rc = map_queue_pass(ctx, nc, ns, true, map_use_grid(false), nullptr, &nblocks);
-  if (rc != LINS_OK) return rc;
+  ScanToMap& sm = m.stm;
+  const MapSlot& v = sm.h_mslot.p[0];
+  // the parity hook: brute force by default (exact neighbours for EVERY point, also those the 1 m gate rejects), over
+  // enough (query block, map slice) pairs for ~8 CTAs per SM (the scan is latency bound: profiles/r01_map_*); a slice is
+  // at least 256 map points.  The grid leaves one list per query.
+  const bool grid = map_use_grid();
+  int slices[2] = {1, 1}, slice_len[2] = {0, 0};
+  size_t part = 0;
+  for (int k = 0; k < 2; ++k) {
+    if (grid || !sm.blocks[k]) continue;
+    const int S = std::max(1, std::min((8 * ctx->sm_count + sm.blocks[k] - 1) / sm.blocks[k], std::min(64, (v.cap[k] + 255) / 256)));
+    slices[k] = S;
+    slice_len[k] = std::max(1, (v.cap[k] + S - 1) / S);
+    part = std::max(part, (size_t)v.nq[k] * S * 5);
+  }
+  CK(sm.part_d.grow(part + 1)); CK(sm.part_i.grow(part + 1));
+  CK(m.knn_c.reserve(5 * (size_t)nc + 1)); CK(m.knn_s.reserve(5 * (size_t)ns + 1)); CK(m.coeff_c.reserve(4 * (size_t)nc + 1));
+  CK(m.coeff_s.reserve(4 * (size_t)ns + 1)); CK(m.mask_c.reserve((size_t)nc + 1)); CK(m.mask_s.reserve((size_t)ns + 1));
+  int32_t* knn[2] = {m.knn_c.p, m.knn_s.p};
+  float* coeff[2] = {m.coeff_c.p, m.coeff_s.p};
+  uint8_t* mask[2] = {m.mask_c.p, m.mask_s.p};
+  for (int k = 0; k < 2; ++k) {
+    if (!sm.blocks[k]) continue;
+    if (grid)
+      queue_knn_grid(ctx, sm, k, nullptr);
+    else
+      lins_map_knn_kernel<<<dim3(sm.blocks[k], slices[k]), kKnnThreads, 0, ctx->stream>>>(v.q[k], v.nq[k], v.map[k], v.cap[k], slice_len[k], sm.consts.p,
+                                                                                          nullptr, sm.part_d.p, sm.part_i.p);
+    queue_fit(ctx, sm, k, slices[k], nullptr, knn[k], coeff[k], mask[k]);
+    CK(cudaGetLastError());
+    ctx->launches += 2;
+  }
   CK(d2h(ctx, cknn, m.knn_c.p, sizeof(int32_t) * 5 * (size_t)nc));
   CK(d2h(ctx, sknn, m.knn_s.p, sizeof(int32_t) * 5 * (size_t)ns));
   CK(d2h(ctx, ccoeff, m.coeff_c.p, sizeof(float) * 4 * (size_t)nc));

@@ -6,13 +6,16 @@
 //                         streamed through shared memory in tiles and cut into slices across the grid so that all
 //                         SMs work (a few thousand queries alone would fill only ~25 CTAs); every (query, slice)
 //                         pair leaves a sorted partial list.  f32 ((dx*dx)+dy*dy)+dz*dz, ascending (distance, index).
+//   lins_map_knn_grid_kernel  the same 5-NN through a hashed uniform grid, for every point that can be accepted.
 //   lins_map_fit_kernel   merges the partial lists, then per point: line fit (covariance + cv::eigen 3x3) or plane
 //                         fit (cv::solve QR 5x3), validity tests, weight, coefficients, the row of matA / matB, and
 //                         the f64 block reduction of A^T A (21) and A^T B (6).
-//   host                  sums the block partials in a fixed order, rounds to f32 and takes the 6x6 LM step
-//                         (lins_map_host.hpp).  sin / cos of the transform are evaluated on the host in f32 (6 values
-//                         per iteration), so everything the device computes is f32 + - * / sqrt, which IEEE fixes bit
-//                         for bit: indices, coefficients and masks equal the CPU oracle exactly.
+//   lins_map_lm_kernel    sums the block partials in a fixed order, rounds to f32, takes the 6x6 LM step and derives
+//                         the next pass's sin / cos.  The first pass's sin / cos are evaluated on the host in f32, so
+//                         everything the device computes for it is f32 + - * / sqrt, which IEEE fixes bit for bit:
+//                         indices, coefficients and masks equal the CPU oracle exactly.
+// Every kernel but the brute force serves a table of slots (MapSlot): the lockstep mappers' many, or the one slot of
+// lins_gpu_map_set / scan2map / map_associate.
 // The small OpenCV kernels (cv::eigen = cyclic Jacobi, cv::solve(DECOMP_QR) = Householder) are restated in
 // lins_cv_small.hpp, shared by host and device.
 #pragma once
@@ -176,27 +179,29 @@ __device__ __forceinline__ void lm_row(const float4 po, const float* c, const Pa
 }
 
 // One thread per feature point.  partial: [gridDim.x][kRowAcc + 1] (the last entry = selected points of the block).
-// Many slots (sl non-null): block b serves slot blk_slot[b], whose queries q[CORNER ? 0 : 1] start at its block
-// blk[...]; a block never straddles two slots, so each slot's partials are those of its own single call.
+// Block b serves slot blk_slot[b] (n_sl slots), whose queries q[CORNER ? 0 : 1] start at its block blk[...]; a block
+// never straddles two slots, so each slot's partials are those of a run of that slot alone.  part_d / part_i:
+// [rows][n_slices][5]
+// (n_slices > 1: the brute-force slices of a one-slot table, whose rows are its query indices).  The dense outputs
+// (knn_out, coeff_out, mask_out; null: not written) are indexed by the slot's query index.
 template <bool CORNER>
-__global__ void __launch_bounds__(kFitThreads) lins_map_fit_kernel(const float4* __restrict__ q, int n_q, const float4* __restrict__ map,
-                                                                   int n_slices, const float* __restrict__ part_d,
+__global__ void __launch_bounds__(kFitThreads) lins_map_fit_kernel(int n_slices, const float* __restrict__ part_d,
                                                                    const int* __restrict__ part_i, const PassConsts* __restrict__ pcp,
                                                                    const MapLoopState* __restrict__ st, int32_t* __restrict__ knn_out,
                                                                    float* __restrict__ coeff_out, uint8_t* __restrict__ mask_out,
-                                                                   double* __restrict__ partial, const MapSlot* __restrict__ sl,
+                                                                   double* __restrict__ partial, const MapSlot* __restrict__ sl, int n_sl,
                                                                    const int* __restrict__ blk_slot) {
+  constexpr int K = CORNER ? 0 : 1;
   const int row = blockIdx.x * kFitThreads + threadIdx.x;
-  int slot = 0, qi = row;
-  if (sl) {
-    constexpr int K = CORNER ? 0 : 1;
-    slot = blk_slot[blockIdx.x];
-    const MapSlot& v = sl[slot];
-    q = v.q[K]; n_q = v.nq[K]; map = v.map[K];
-    qi = (blockIdx.x - v.blk[K]) * kFitThreads + threadIdx.x;
-  }
-  if (st && st[slot].done) return;
+  const int slot = n_sl == 1 ? 0 : blk_slot[blockIdx.x];  // (a one-slot table skips the lookup's latency)
+  // the slot's record, loop state and constants are loaded before any branch on them, so their latencies overlap
+  const MapSlot& v = sl[slot];
+  const bool done = st && st[slot].done;
   const PassConsts pc = pcp[slot];
+  const float4* __restrict__ q = v.q[K];
+  const float4* __restrict__ map = v.map[K];
+  const int n_q = v.nq[K], qi = (blockIdx.x - v.blk[K]) * kFitThreads + threadIdx.x;
+  if (done) return;
   double acc[kRowAcc];
 #pragma unroll
   for (int k = 0; k < kRowAcc; ++k) acc[k] = 0.0;
@@ -275,7 +280,7 @@ __global__ void __launch_bounds__(kFitThreads) lins_map_fit_kernel(const float4*
 // Grid.  The reference accepts a feature point only if its FIFTH neighbour lies within 1 m (pointSearchSqDis[4] < 1.0,
 // lidar_mapping_node.cpp:1374, :1481), so the only neighbours that matter are those within 1 m, and every map point
 // whose f32 distance is < 1 lies in the 3 x 3 x 3 block of 1 m cells around the query's cell (cells of the exact
-// difference: grid_cell, DESIGN.md §4.4).  lins_gpu_map_set bucket-sorts
+// difference: grid_cell, DESIGN.md §4.4).  The grid build bucket-sorts
 // the map by hash(cell) (the role of kdtree*FromMap->setInputCloud, :1637-1638); a query warp gives one cell of the
 // block to each of 27 lanes (cells that hash to the same bucket are visited once), every lane keeps the five smallest
 // (distance, index) keys of its bucket — points of other cells that share the bucket are just extra candidates — and a
@@ -283,7 +288,7 @@ __global__ void __launch_bounds__(kFitThreads) lins_map_fit_kernel(const float4*
 // would have been in the block); otherwise the true fifth distance is >= 1 as well and the point is rejected either
 // way.  Keys are (f32 distance bits, index), so ties resolve to the lower index exactly like the brute-force scan.
 //
-// LM loop.  scan2map keeps transformTobeMapped, matP / isDegenerate and the report on the device (MapLoopState): per
+// LM loop.  The loop keeps transformTobeMapped, matP / isDegenerate and the report on the device (MapLoopState): per
 // iteration the 5-NN kernel, the fit / reduction kernel and a one-warp kernel that sums the block partials in a fixed
 // order, takes the 6 x 6 step (LMOptimization :1598-1632, lins_cv_small.hpp) and prepares the next iteration's sin / cos;
 // once it sets `done`, the launches still queued return at once.  One D2H and one synchronisation per call.
@@ -306,48 +311,32 @@ __device__ __forceinline__ void grid_cell(const GridIndex& g, float x, float y, 
   iy = (unsigned)__double2int_rd((double)y - (double)g.oy);
   iz = (unsigned)__double2int_rd((double)z - (double)g.oz);
 }
-// counting sort of the map by bucket: count, (host-launched) scan, scatter.  Many slots (sl non-null, n_sl slots): point
-// i of the n is point i - m0[k] of slot s's map k, with the slot's grid and its buckets from bucket0[k] on; n counts the
-// maps' capacities, and n_dev points at the device-resident number of a map's real points.
+// counting sort of every slot's maps by bucket: count, (host-launched) scan, scatter.  Point i of the n (n_sl slots) is
+// point i - m0[k] of slot s's map k, with the slot's grid and its buckets from bucket0[k] on; n counts the maps'
+// capacities, and n_dev points at the device-resident number of a map's real points.
 struct GridPoint { const float4* map; int i; const int* n_dev; GridIndex g; int b0; };
-__device__ __forceinline__ GridPoint grid_point(const float4* map, int i, const GridIndex& g, const MapSlot* sl, int n_sl) {
-  if (!sl) return GridPoint{map, i, nullptr, g, 0};
+__device__ __forceinline__ GridPoint grid_point(int i, const MapSlot* sl, int n_sl) {
   int lo = 0, hi = n_sl - 1;  // the last slot whose maps start at or before i
   while (lo < hi) { const int m = (lo + hi + 1) >> 1; if (sl[m].m0[0] <= i) lo = m; else hi = m - 1; }
   const MapSlot& v = sl[lo];
   const int k = i >= v.m0[1];
   return GridPoint{v.map[k], i - v.m0[k], v.n_map[k], v.g[k], v.bucket0[k]};
 }
-__global__ void lins_grid_count_kernel(const float4* __restrict__ map, int n, GridIndex g, int* __restrict__ count,
-                                       const MapSlot* __restrict__ sl, int n_sl) {
+__global__ void lins_grid_count_kernel(int n, int* __restrict__ count, const MapSlot* __restrict__ sl, int n_sl) {
   const int i0 = blockIdx.x * blockDim.x + threadIdx.x;
   if (i0 >= n) return;
-  const GridPoint gp = grid_point(map, i0, g, sl, n_sl);
-  if (gp.n_dev && gp.i >= *gp.n_dev) return;
+  const GridPoint gp = grid_point(i0, sl, n_sl);
+  if (gp.i >= *gp.n_dev) return;
   const float4 p = __ldg(&gp.map[gp.i]);
   unsigned ix, iy, iz;
   grid_cell(gp.g, p.x, p.y, p.z, ix, iy, iz);
   atomicAdd(&count[gp.b0 + (grid_hash(ix, iy, iz) & gp.g.mask)], 1);
 }
-// exclusive scan of count[0..n) -> start[0..n], one CTA (runs once per lins_gpu_map_set)
-__global__ void __launch_bounds__(1024) lins_grid_scan_kernel(const int* __restrict__ count, int* __restrict__ start, int* __restrict__ cursor, int n) {
-  __shared__ int part[1024];
-  const int per = (n + 1023) / 1024, lo = threadIdx.x * per, hi = min(n, lo + per);
-  int s = 0;
-  for (int i = lo; i < hi; ++i) s += count[i];
-  part[threadIdx.x] = s;
-  __syncthreads();
-  if (threadIdx.x == 0) { int run = 0; for (int i = 0; i < 1024; ++i) { const int v = part[i]; part[i] = run; run += v; } start[n] = run; }
-  __syncthreads();
-  int run = part[threadIdx.x];
-  for (int i = lo; i < hi; ++i) { start[i] = run; cursor[i] = run; run += count[i]; }
-}
-__global__ void lins_grid_scatter_kernel(const float4* __restrict__ map, int n, GridIndex g, int* __restrict__ cursor,
-                                         float4* __restrict__ sorted, const MapSlot* __restrict__ sl, int n_sl) {
+__global__ void lins_grid_scatter_kernel(int n, int* __restrict__ cursor, float4* __restrict__ sorted, const MapSlot* __restrict__ sl, int n_sl) {
   const int i0 = blockIdx.x * blockDim.x + threadIdx.x;
   if (i0 >= n) return;
-  const GridPoint gp = grid_point(map, i0, g, sl, n_sl);
-  if (gp.n_dev && gp.i >= *gp.n_dev) return;
+  const GridPoint gp = grid_point(i0, sl, n_sl);
+  if (gp.i >= *gp.n_dev) return;
   const float4 p = __ldg(&gp.map[gp.i]);
   unsigned ix, iy, iz;
   grid_cell(gp.g, p.x, p.y, p.z, ix, iy, iz);
@@ -370,26 +359,26 @@ struct Top5K {  // five smallest (distance bits, index) keys, ascending
   }
 };
 
-// one warp per query; part_d / part_i: [n_q][1][5] (a single "slice" for lins_map_fit_kernel).  Many slots (sl
-// non-null): n_q rows in lins_map_fit_kernel's blocks, row r in block r / kFitThreads of slot blk_slot[that block], map
-// `kind` (0 corner, 1 surf).
-__global__ void __launch_bounds__(kGridKnnWarps * 32) lins_map_knn_grid_kernel(const float4* __restrict__ q, int n_q, GridIndex g,
-                                                                               const PassConsts* __restrict__ pcp, const MapLoopState* __restrict__ st,
+// one warp per query; part_d / part_i: [n_rows][1][5] (a single "slice" for lins_map_fit_kernel).  n_rows rows in
+// lins_map_fit_kernel's blocks, row r in block r / kFitThreads of slot blk_slot[that block] (n_sl slots), map `kind` (0
+// corner, 1 surf).
+__global__ void __launch_bounds__(kGridKnnWarps * 32) lins_map_knn_grid_kernel(int n_rows, const PassConsts* __restrict__ pcp,
+                                                                               const MapLoopState* __restrict__ st,
                                                                                float* __restrict__ part_d, int* __restrict__ part_i,
-                                                                               const MapSlot* __restrict__ sl, const int* __restrict__ blk_slot, int kind) {
+                                                                               const MapSlot* __restrict__ sl, int n_sl, const int* __restrict__ blk_slot,
+                                                                               int kind) {
   const int lane = threadIdx.x & 31;
   const int row = blockIdx.x * kGridKnnWarps + (threadIdx.x >> 5);
-  if (row >= n_q) return;
-  int slot = 0, qi = row;
-  if (sl) {
-    slot = blk_slot[row / kFitThreads];
-    const MapSlot& v = sl[slot];
-    qi = row - v.blk[kind] * kFitThreads;
-    if (qi >= v.nq[kind]) return;
-    q = v.q[kind]; g = v.g[kind];
-  }
-  if (st && st[slot].done) return;
+  if (row >= n_rows) return;
+  const int slot = n_sl == 1 ? 0 : blk_slot[row / kFitThreads];  // (a one-slot table skips the lookup's latency)
+  // the slot's record, loop state and constants are loaded before any branch on them, so their latencies overlap
+  const MapSlot& v = sl[slot];
+  const bool done = st && st[slot].done;
   const PassConsts pc = pcp[slot];
+  const int qi = row - v.blk[kind] * kFitThreads;
+  const float4* __restrict__ q = v.q[kind];
+  const GridIndex g = v.g[kind];
+  if (done || qi >= v.nq[kind]) return;
   const float3 s = associate_to_map(__ldg(&q[qi]), pc);
   unsigned cx, cy, cz;
   grid_cell(g, s.x, s.y, s.z, cx, cy, cz);
@@ -442,20 +431,20 @@ __device__ __forceinline__ void pass_consts_from(const float* T, PassConsts& pc)
 
 // one warp per slot, one block each (the 6 x 6 step itself is one thread): block partials -> matAtA / matAtB (f32), the LM
 // step, the next iteration's constants.  Every matrix lives in shared memory (plain dynamically indexed loads / stores).
-// One slot: partial blocks [0, nblocks).  Many slots (sl non-null): slot s sums its corner blocks [blk[0], blk[0] +
-// nblk[0]) and then its surf blocks, which start at nblocks (the corner launch's block count) + blk[1].
+// Slot s sums its corner blocks [blk[0], blk[0] + nblk[0]) and then its surf blocks, which start at nblocks (the corner
+// launch's block count) + blk[1].
 __global__ void lins_map_lm_kernel(const double* __restrict__ partial, int nblocks, int iter, MapLoopState* __restrict__ st,
                                    PassConsts* __restrict__ pc_next, const MapSlot* __restrict__ sl) {
   st += blockIdx.x; pc_next += blockIdx.x;
+  const MapSlot& m = sl[blockIdx.x];  // (loaded with the done flag)
+  const int c0 = m.blk[0], c1 = c0 + m.nblk[0], s0 = nblocks + m.blk[1], s1 = s0 + m.nblk[1];
   if (st->done) return;
   __shared__ double acc[kRowAcc + 1];
   __shared__ float AtA[36], AtB[6], Aw[36], X[6], Ae[36], E[6], V[36], V2[36], Vc[36], Vinv[36], X2[6];
   if (threadIdx.x <= kRowAcc) {  // lane k sums column k of the block partials, in a fixed order: corner blocks, then surf
     double v = 0.0;               // blocks (laserCloudOri's order)
-    int r[4] = {0, nblocks, 0, 0};
-    if (sl) { const MapSlot& m = sl[blockIdx.x]; r[0] = m.blk[0]; r[1] = m.blk[0] + m.nblk[0]; r[2] = nblocks + m.blk[1]; r[3] = r[2] + m.nblk[1]; }
-    for (int b = r[0]; b < r[1]; ++b) v += partial[(size_t)b * (kRowAcc + 1) + threadIdx.x];
-    for (int b = r[2]; b < r[3]; ++b) v += partial[(size_t)b * (kRowAcc + 1) + threadIdx.x];
+    for (int b = c0; b < c1; ++b) v += partial[(size_t)b * (kRowAcc + 1) + threadIdx.x];
+    for (int b = s0; b < s1; ++b) v += partial[(size_t)b * (kRowAcc + 1) + threadIdx.x];
     acc[threadIdx.x] = v;
   }
   __syncwarp();

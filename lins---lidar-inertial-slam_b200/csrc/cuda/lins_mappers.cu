@@ -6,7 +6,7 @@
 // launch that follows: sequence mode's publish step, lins_seq.cu); one gather launch of every slot's window
 // into its local-map clouds; one segmented VoxelGrid over the five clouds of every slot (map corner 0.2 m, map surf
 // 0.4 m, corner 0.2 m, surf 0.4 m, outlier 0.4 m), one gather of each slot's surf DS + outlier DS and one segmented
-// VoxelGrid of those (0.4 m); every slot's grids and scan-to-map loop (lins_map.cu: map_queue_slots); the read-back of
+// VoxelGrid of those (0.4 m); every slot's grids and scan-to-map loop (lins_map.cu, grid origin 0); the read-back of
 // the VoxelGrid records and loop states.  After it, the host tail of each slot and one transform launch for every key
 // frame saved.  The VoxelGrids' outputs are sized by their inputs and padded with NaN, and the later launches take those
 // capacities.  The segments of a VoxelGrid keep their input ranges and each slot's fit blocks cover its own queries
@@ -51,8 +51,8 @@ int mappers_open(lins_ctx* ctx, MappersState& ms, int n_slots) {
   ms.n = 0;
   ms.node = std::vector<MapperNode>(n_slots);  // (constructed in place: a node is not copyable)
   ms.ds = std::vector<std::array<Buf<float4>, 6>>(n_slots);
-  CK(ms.loop.reserve(n_slots)); CK(ms.h_loop.reserve(n_slots)); CK(ms.h_mslot.reserve(n_slots));
-  CK(cudaMemsetAsync(ms.loop.p, 0, sizeof(lins_map::MapLoopState) * n_slots, ctx->stream));  // matP, isDegenerate
+  CK(ms.stm.loop.reserve(n_slots)); CK(ms.stm.h_loop.reserve(n_slots)); CK(ms.stm.h_mslot.reserve(n_slots));
+  CK(cudaMemsetAsync(ms.stm.loop.p, 0, sizeof(lins_map::MapLoopState) * n_slots, ctx->stream));  // matP, isDegenerate
   ms.n = n_slots;
   return LINS_OK;
 }
@@ -63,7 +63,7 @@ int mappers_reset(lins_ctx* ctx, MappersState& ms, const uint8_t* mask) {
   for (int s = 0; s < ms.n; ++s)
     if (mask[s]) {
       mapper_node_reset(ms.node[s]);
-      CK(cudaMemsetAsync(ms.loop.p + s, 0, sizeof(lins_map::MapLoopState), ctx->stream));
+      CK(cudaMemsetAsync(ms.stm.loop.p + s, 0, sizeof(lins_map::MapLoopState), ctx->stream));
     }
   return LINS_OK;
 }
@@ -207,20 +207,23 @@ int mappers_step(lins_ctx* ctx, MappersState& ms, const lins_mappers_desc* d, li
                              ms.vg_out.p + 5 * P, ms.h_vg_init.p + 5 * P, info + 5 * P)) != LINS_OK)
     return rc;
 
-  // scan2MapOptimization of every slot with key frames (a slot without runs no pass, like the single mapper's host gate)
+  // scan2MapOptimization of every slot with key frames (a slot without runs no pass, like the single mapper's host gate);
+  // every grid's origin is 0 (any finite origin gives the same 5-NN)
   bool any_map = false;
-  for (int s = 0; s < M; ++s) std::memset(&ms.h_mslot.p[s], 0, sizeof(lins_map::MapSlot));
+  for (int s = 0; s < M; ++s) std::memset(&ms.stm.h_mslot.p[s], 0, sizeof(lins_map::MapSlot));
   for (int p = 0; p < P; ++p) {
     const int s = proc[p];
     if (ms.node[s].poses.empty()) continue;
-    lins_map::MapSlot& v = ms.h_mslot.p[s];
+    lins_map::MapSlot& v = ms.stm.h_mslot.p[s];
     v.run = 1; any_map = true;
     for (int k = 0; k < 2; ++k) { v.map[k] = ms.ds[s][k].p; v.cap[k] = mapc[2 * p + k]; v.n_map[k] = &info[3 * P + 2 * p + k].count; }
     v.q[0] = ms.ds[s][2].p; v.nq[0] = h_off1[3 * p + 1] - h_off1[3 * p];
     v.q[1] = ms.ds[s][5].p; v.nq[1] = h_off2[p + 1] - h_off2[p];
     for (int i = 0; i < 6; ++i) v.T[i] = sc[s].transformTobeMapped[i];
   }
-  if (any_map && (rc = map_queue_slots(ctx, ms, M)) != LINS_OK) return rc;
+  if (any_map && ((rc = map_fill_table(ctx, ms.stm, M)) != LINS_OK || (rc = map_queue_grids(ctx, ms.stm)) != LINS_OK ||
+                  (rc = map_queue_loop(ctx, ms.stm)) != LINS_OK))
+    return rc;
   CK(cudaMemcpyAsync(ms.h_vg_info.p, info, sizeof(VgInfo) * 6 * (size_t)P, cudaMemcpyDeviceToHost, ctx->stream));
   CK(cudaStreamSynchronize(ctx->stream));  // the step's one read-back
   for (int s : proc) ms.node[s].last.valid = false;  // (a failed step has overwritten their previous clouds)
@@ -238,7 +241,7 @@ int mappers_step(lins_ctx* ctx, MappersState& ms, const lins_mappers_desc* d, li
     const bool gate = cnt[0] > 10 && cnt[1] > 100;
     KfSave sv;
     bool saved = false;
-    mapper_cycle_end(ms.node[s], sc[s], d->time[s], period ? period[s] : ctx->prm.scan_period, cnt, gate ? &ms.h_loop.p[s] : nullptr, rr[s], &sv, &saved);
+    mapper_cycle_end(ms.node[s], sc[s], d->time[s], period ? period[s] : ctx->prm.scan_period, cnt, gate ? &ms.stm.h_loop.p[s] : nullptr, rr[s], &sv, &saved);
     if (saved) {
       for (int k = 0; k < 3; ++k) sv.ds[k] = ms.ds[s][2 + k].p;
       saves.push_back(sv);

@@ -103,7 +103,7 @@ void save_copies(lins_ctx* ctx, int s, const B::Header& h, float4* dst, const st
   o = at(B::kKfClouds);
   for (const auto& k : kf)
     for (int a = 0; a < 3; ++a) { const MapperKeyFrame& f = m.slots[k.second]; v.push_back(DevCopy{f.c[a].p, o, f.n[a], 0}); o += f.n[a]; }
-  v.push_back(DevCopy{f4(ctx->mappers.loop.p + s), at(B::kLoop), (int)(sizeof(lins_map::MapLoopState) / 16), 0});
+  v.push_back(DevCopy{f4(ctx->mappers.stm.loop.p + s), at(B::kLoop), (int)(sizeof(lins_map::MapLoopState) / 16), 0});
 }
 
 // the host records of slot s's blob into img (its first byte in the pinned image)
@@ -218,7 +218,7 @@ int load_run(lins_ctx* ctx, const uint8_t* mask, const std::vector<B::View>& v) 
     const int row_len[6] = {20, 324, 20, 20, 8, 20};
     for (int i = 0; i < 6; ++i) copies.push_back(DevCopy{at(s, B::kRows) + B::kRowOff[i] / 2, reinterpret_cast<float4*>(rows[i]), row_len[i] / 2, 0});
     if (!pb.bound) continue;
-    copies.push_back(DevCopy{at(s, B::kLoop), reinterpret_cast<float4*>(ms.loop.p + s), (int)(sizeof(lins_map::MapLoopState) / 16), 0});
+    copies.push_back(DevCopy{at(s, B::kLoop), reinterpret_cast<float4*>(ms.stm.loop.p + s), (int)(sizeof(lins_map::MapLoopState) / 16), 0});
     // the key-frame store of a fresh node: a store slot for each key frame (a free one first), its clouds from the staging
     MapperNode& m = ms.node[s];
     const float4* src = at(s, B::kKfClouds);

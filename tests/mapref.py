@@ -132,7 +132,7 @@ def associate_knn(corner_map, surf_map, corner_q, surf_q, T, prune=None):
     return out
 
 
-# ---- the device grid (lins_map.cuh: grid_cell, grid_hash; lins_map.cu: map_build_grid) ----------------------------
+# ---- the device grid (lins_map.cuh: grid_cell, grid_hash; lins_map.cu: map_grid_origin, map_fill_table) ------------
 INT_MIN, INT_MAX = -(1 << 31), (1 << 31) - 1
 
 

@@ -180,10 +180,8 @@ def test_report_over_a_call_sequence_on_a_fresh_context(capi, ob):
     assert degs[0] == 1 and degs[1] == 0  # (the second call selects < 50 points right after a degenerate one)
 
 
-def test_map_set_sequence_leaves_no_stale_grid(capi):
-    """200 k points, then 300, then an empty corner cloud, then 60 k with a shifted origin, on one context: after each
-    map_set the grid pass equals mapref's (stale bucket starts or counts would show as wrong or missing neighbours)."""
-    g = capi.LinsGpu()
+def _map_set_sequence():
+    """200 k points, then 300, then an empty corner cloud, then 60 k with a shifted origin."""
     big = mapcases.plane_scene(5, n_planes=500, n_q=20000)
     small = mapcases.plane_scene(6, n_planes=1, n_q=200)
     small = mapcases.MapCase("300", mapref.xyz(small.corner_map)[:40], mapref.xyz(small.surf_map)[:300],
@@ -192,13 +190,38 @@ def test_map_set_sequence_leaves_no_stale_grid(capi):
                              mapref.xyz(small.surf_q), small.T)
     shifted = mapcases.translated(mapcases.plane_scene(7, n_planes=150, n_q=5000), [-317.25, 1250.5, -40.0])
     assert len(big.surf_map) == 200_000 and len(shifted.surf_map) == 60_000
-    for c in (big, small, empty, shifted):
+    return big, small, empty, shifted
+
+
+def test_map_set_sequence_leaves_no_stale_grid(capi):
+    """The sequence on one context: after each map_set the grid pass equals mapref's (stale bucket starts or counts would
+    show as wrong or missing neighbours)."""
+    g = capi.LinsGpu()
+    for c in _map_set_sequence():
         g.map_set(c.corner_map, c.surf_map)
         with knn_mode("grid"):
             dev = g.map_associate(c.corner_q, c.surf_q, c.T)
         ref = mapref.associate_knn(c.corner_map, c.surf_map, c.corner_q, c.surf_q, c.T)
         grid_rows_ok(dev, ref, _sizes(c), c.name)
         assert (ref["surf_dist"][:, 4] < 1).sum() > len(c.surf_q) // 4, c.name
+
+
+def test_scan2map_after_each_map_set_of_the_sequence(capi, ob):
+    """scan2map after each map_set of the sequence, on one context, equals the oracle taken through the same sequence:
+    the one-slot table's grids, fit blocks and loop state follow every change of the maps' sizes (the empty corner map
+    fails the 10 / 100 gate; matP / isDegenerate persist across the calls)."""
+    g, m = capi.LinsGpu(), ob.MapOracle()
+    ran = []
+    for c in _map_set_sequence():
+        g.map_set(c.corner_map, c.surf_map)
+        m.set_map(c.corner_map, c.surf_map)
+        cq, sq = c.corner_q[:500], c.surf_q[:2000]  # (the oracle's 5-NN is brute force)
+        T, rep = g.scan2map(cq, sq, c.T)
+        To, ro = m.scan2map(cq, sq, c.T)
+        _same_report(rep, ro, c.name)
+        assert _t_close(T, To), (c.name, T, To)
+        ran.append(not rep.skipped and rep.n_sel[0] >= 50)
+    assert ran == [True, True, False, True]
 
 
 def test_large_shape_grid_equals_mapref(gpu):

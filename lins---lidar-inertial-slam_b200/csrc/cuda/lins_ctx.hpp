@@ -126,6 +126,26 @@ struct CopyList {
 // one device range of float4 records: len points at src
 struct MapPiece { const float4* src = nullptr; int len = 0; };
 
+// The map updatePointCloud keeps (StateEstimator.hpp:1116-1161) for n units: each unit's surf and corner map (the clouds
+// the walks and tripods read) and, while it is stale, the surf and corner clouds its 1-NN index was last built on (after
+// a refresh that failed the >= 5 && >= 20 guard; empty elsewhere).  Clouds are CSR over the units in unit order: cloud c
+// (map_s, map_c, tree_s, tree_c) of unit s is [h_off[c (n + 1) + s], h_off[c (n + 1) + s + 1]) of cur[c].  nxt and h_noff
+// hold the next generation while it is built.  Sequence mode keeps one for its slots, the single-scan seam one with one
+// unit; n = 0: no map yet.
+struct MapGen {
+  int n = 0;
+  Buf<float4> cur[4], nxt[4];
+  std::vector<int> h_off, h_noff;
+  std::vector<unsigned char> h_stale;  // 1: the unit's 1-NN clouds are tree_s / tree_c
+  Buf<int> dev;                        // the device copy of h_off, then h_stale's bytes (queue_map_state)
+  // n units without maps (host side only)
+  void reset(int units) { n = units; h_off.assign(4 * (size_t)(n + 1), 0); h_stale.assign(n, 0); }
+  const int* off() const { return dev.p; }
+  const unsigned char* stale() const { return reinterpret_cast<const unsigned char*>(dev.p + 4 * (size_t)(n + 1)); }
+};
+// what a map refresh makes of one unit: its next four clouds and its stale flag
+struct MapRefresh { MapPiece next[4]; unsigned char stale; };
+
 // Sequence mode's publish step (lins_gpu_seq_map_*, lins_seq.cu): what LinsFusion::publishTopics hands each slot's
 // mapping node (scan_last_'s YZX clouds, globalStateYZX_), kept for a run bound to the lockstep mappers (each slot's YZX
 // flag and pose are in its SeqSlot).  Maps and the kept outlier clouds are in XYZ order; the mapper step's gather writes
@@ -161,9 +181,7 @@ struct SeqSlot {
   double pose[7] = {0, 0, 0, 0, 0, 0, 1};     // bound run: the slot's globalStateYZX_ (pos, quat x y z w)
 };
 
-// Sequence mode (lins_gpu_seq_*, lins_seq.cu): the running sequences' filter state and maps.  Maps are CSR over the
-// sequences in sequence order; `tree` holds the cloud a sequence's 1-NN index was last built on where that differs from
-// its map (stale[s] = 1, after a refresh that failed the >=5 && >=20 guard), and is empty elsewhere.
+// Sequence mode (lins_gpu_seq_*, lins_seq.cu): the running sequences' filter state and maps (a unit per sequence).
 struct SeqState {
   int n = 0;                      // sequences (0 = lins_gpu_seq_begin / lins_gpu_seq_open has not run)
   double consts[10];              // lins_seq::Consts of the run's params
@@ -190,12 +208,7 @@ struct SeqState {
   Buf<double> prior_state, prior_cov;                  // the last step's IESKF prior (after the IMU propagation)
   Buf<int> icp_ind_s, icp_ind_c;                       // correspondence IDs of the ICP fallback (the IESKF's stay in run)
   Buf<unsigned char> icp;                              // n IcpState records (lins_icp_step.cuh; icp_state_bytes() each)
-  Buf<float4> map_s, map_c, tree_s, tree_c;            // current generation
-  Buf<float4> nmap_s, nmap_c, ntree_s, ntree_c;        // next generation (built by the step, then swapped in)
-  Buf<int> map_off;                                    // 4 x (n + 1): map_s, map_c, tree_s, tree_c
-  Buf<unsigned char> stale;
-  std::vector<int> h_map_off, h_nmap_off;              // host copies of map_off
-  std::vector<unsigned char> h_stale_v;
+  MapGen map;                                          // the next generation is built by the step, then swapped in
   Resident up;                                         // the step's four uploaded clouds (qs, qc, ts = new less-flat, tc = new less-sharp)
   Resident run;                                        // the IESKF batch: compacted queries of the sequences that run, outputs
   Buf<double> imu; Buf<int> imu_off;
@@ -411,11 +424,7 @@ struct lins_ctx {
   lins_capi::FeatState feat;   // lins_gpu_extract_features, lins_gpu_seq_step_pcl, lins_gpu_seq_step_raw
   lins_capi::ProjState proj;   // lins_gpu_project_scans, lins_gpu_seq_step_raw, lins_gpu_seq_step_cloud2
   lins_capi::Cloud2State c2;   // lins_gpu_decode_cloud2, lins_gpu_seq_step_cloud2
-  // the single-scan map: "last" clouds (walks + tripods) and the clouds the 1-NN index was built on
-  Buf<float4> map_s, map_c, tree_s, tree_c;
-  Buf<int> map_off;  // 4 x 2 ints: [0,ns][0,nc][0,tns][0,tnc]
-  int map_ns = -1, map_nc = -1, tree_ns = -1, tree_nc = -1;
-  bool tree_is_map = true;
+  lins_capi::MapGen map;       // the single-scan map (one unit)
   bool timers_on = false;
   bool verbose = false;  // LINS_VERBOSE: print the launch configuration
   int force_slots = 0;  // tuning knob (LINS_SLOTS): resident units per CTA
@@ -578,14 +587,16 @@ inline int upload2(lins_ctx* ctx, Buf<float4>& dst_a, const lins_point* a, int n
 int upload_clouds(lins_ctx* ctx, Resident& r, int n, const lins_point* const pts[4], const int32_t* const offs[4], int point_format);
 // lins_gpu.cu: the fused kernel's IESKF launch over bv (with r's scratch), its query tile, the estimateTransform loop of
 // bv's device-resident units (pose: 20 doubles, icp: one IcpState per unit, set by the caller; n_iter launches, the largest
-// NUM_ITER of the units), and the CSR transformToEnd
-// of the units with run[u] != 0 (lin: 20 doubles per unit, period: one SCAN_PERIOD per unit, both on the device)
+// NUM_ITER of the units), bv's targets pointed at the maps of g (map_targets), and transformToEnd in place on the CSR
+// clouds of the units with run[u] != 0 (lin: 20 doubles per unit, period: one SCAN_PERIOD per unit, both on the device;
+// a block per unit)
 int fused_ieskf_launch(lins_ctx* ctx, Resident& r, const lins_dev::BatchView& bv);
 int fused_qtile(int max_q);
 size_t icp_state_bytes();
 int icp_loop(lins_ctx* ctx, Resident& r, lins_dev::BatchView bv, double* pose, lins_dev::IcpState* icp, int n_iter);
-int transform_to_end_csr(lins_ctx* ctx, float4* pts, const int* off, int n_units, const double* lin, const unsigned char* run,
-                         const double* period);
+void map_targets(lins_dev::BatchView& bv, const MapGen& g);
+int transform_to_end(lins_ctx* ctx, float4* pts, const int* off, int n_units, const double* lin, const unsigned char* run,
+                     const double* period);
 // device-resident input of one feature extraction: n scans of line_num rings; scan i's points are pts[off[i] ..
 // off[i] + count[count_stride * i]) (off[i] .. off[i + 1] when count is null), its per-point cloud_info at the same
 // offsets; ring: n x 2 x line_num (start, end), ori: n x 3; total = off[n], the length of the per-point outputs
@@ -682,17 +693,20 @@ int mappers_step(lins_ctx* ctx, MappersState& ms, const lins_mappers_desc* d, li
 // (named in its messages) that needs a lins_gpu_seq_open run: LINS_E_NOMAP without a run, LINS_E_INVALID when args_ok is
 // false (a null argument) or for a run of lins_gpu_seq_begin; check_fresh: LINS_E_INVALID unless slot s is fresh.
 // upload_slot_consts: every slot's device constants (its config's, else the run's) for the first n slots, then a
-// synchronisation; queue_map_state: the upload of the host copies of map_off and stale (pageable: the caller
-// synchronises before they change); current_piece: cloud c (map_s, map_c, tree_s, tree_c) of slot s in the current
-// generation; build_next_maps: the next generation from next[4 * s + c] (fills h_nmap_off, reserves nmap_* / ntree_* and
-// appends the copies that fill them to `copies`); swap_maps: the next generation becomes the current one (its copies
-// have been queued)
+// synchronisation
 int check_open_run(lins_ctx* ctx, const char* entry, bool args_ok);
 int check_fresh(lins_ctx* ctx, int s, const char* entry);
 int upload_slot_consts(lins_ctx* ctx, int n);
-cudaError_t queue_map_state(lins_ctx* ctx, SeqState& q);
-MapPiece current_piece(const SeqState& q, int c, int s);
-int build_next_maps(lins_ctx* ctx, SeqState& q, const std::vector<MapPiece>& next, std::vector<DevCopy>& copies);
-void swap_maps(SeqState& q);
+// lins_seq.cu: a MapGen's generations.  reserve_maps: g's device state for n units and current maps of ns / nc points
+// (growth loses the contents); queue_map_state: one H2D of h_off and h_stale into g.dev (a pageable source: staged before
+// it returns); current_piece: cloud c of unit s in the current generation; refresh_maps: unit s's refresh by its new
+// clouds (the guard rule); build_next_maps: the next generation from next[4 * s + c] (fills h_noff, reserves nxt and
+// appends the copies that fill it to `copies`); swap_maps: the next generation becomes the current one
+int reserve_maps(lins_ctx* ctx, MapGen& g, int n, size_t ns, size_t nc);
+cudaError_t queue_map_state(lins_ctx* ctx, MapGen& g);
+MapPiece current_piece(const MapGen& g, int c, int s);
+MapRefresh refresh_maps(const MapGen& g, int s, MapPiece surf, MapPiece corner);
+int build_next_maps(lins_ctx* ctx, MapGen& g, const std::vector<MapPiece>& next, std::vector<DevCopy>& copies);
+void swap_maps(MapGen& g);
 
 }  // namespace lins_capi

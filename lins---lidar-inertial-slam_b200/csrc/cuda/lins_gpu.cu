@@ -344,7 +344,7 @@ __global__ void __launch_bounds__(kThreads, kMinCtas) lins_ieskf_kernel(const __
 
 
 // F1: transformToEnd (StateEstimator.hpp:1083-1101).  The per-scan constants (block-wide, into shared memory) and the
-// per-point body, shared by the single-cloud kernel and the CSR kernel of sequence mode.
+// per-point body.
 __device__ __forceinline__ void to_end_consts(const double* __restrict__ lin, double* sphi, double* srn, double* sq) {
   if (threadIdx.x == 0) {
     q4 q; q.x = lin[6]; q.y = lin[7]; q.z = lin[8]; q.w = lin[9];
@@ -366,31 +366,25 @@ __device__ __forceinline__ float4 to_end_point(float4 p, const double* sphi, con
   return p;
 }
 
-// CSR version: one block per unit u with run[u] != 0, its cloud pts[off[u], off[u+1]) with linState_ lin[20 u ..] and
-// SCAN_PERIOD period[u].
-__global__ void lins_transform_to_end_csr_kernel(float4* __restrict__ pts, const int* __restrict__ off, const double* __restrict__ lin,
-                                                 const unsigned char* __restrict__ run, const double* __restrict__ period) {
+// In place on CSR clouds: unit u = blockIdx.x, its cloud pts[off[u], off[u + 1]) over gridDim.y blocks, with linState_
+// lin[20 u ..] and SCAN_PERIOD period[u] (period null: scan_period).  Units with run[u] == 0 are skipped (run null: none
+// is).  out (optional) receives full PointXYZI records at the same indices, for a straight D2H into a caller's cloud.
+__global__ void lins_transform_to_end_kernel(float4* __restrict__ pts, const int* __restrict__ off, const double* __restrict__ lin,
+                                             const unsigned char* __restrict__ run, const double* __restrict__ period,
+                                             double scan_period, lins_point* __restrict__ out) {
   __shared__ double sphi[3], srn[3], sq[4];
   const int u = blockIdx.x;
-  if (!run[u]) return;
+  if (run && !run[u]) return;
   to_end_consts(lin + (size_t)u * 20, sphi, srn, sq);
-  const double scan_period = period[u];
-  for (int i = off[u] + threadIdx.x; i < off[u + 1]; i += blockDim.x) pts[i] = to_end_point(pts[i], sphi, srn, sq, scan_period);
-}
-
-// in place on a packed cloud; out32 (optional) receives full PointXYZI records
-__global__ void lins_transform_to_end_kernel(float4* __restrict__ pts, int n, const double* __restrict__ lin,
-                                             double scan_period, lins_point* __restrict__ out32) {
-  __shared__ double sphi[3], srn[3], sq[4];
-  to_end_consts(lin, sphi, srn, sq);
-  int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= n) return;
-  float4 p = to_end_point(pts[i], sphi, srn, sq, scan_period);
-  pts[i] = p;
-  if (out32) {  // full pcl::PointXYZI records for a straight D2H into the caller's cloud
-    float4* o = reinterpret_cast<float4*>(out32 + i);
-    o[0] = make_float4(p.x, p.y, p.z, 1.0f);
-    o[1] = make_float4(p.w, 0.f, 0.f, 0.f);
+  if (period) scan_period = period[u];
+  for (int i = off[u] + blockIdx.y * blockDim.x + threadIdx.x; i < off[u + 1]; i += gridDim.y * blockDim.x) {
+    const float4 p = to_end_point(pts[i], sphi, srn, sq, scan_period);
+    pts[i] = p;
+    if (out) {
+      float4* o = reinterpret_cast<float4*>(out + i);
+      o[0] = make_float4(p.x, p.y, p.z, 1.0f);
+      o[1] = make_float4(p.w, 0.f, 0.f, 0.f);
+    }
   }
 }
 
@@ -489,7 +483,7 @@ BatchView view_of(const Resident& r, bool reports, bool trace) {
 // Upload the queries + prior of ONE scan into ctx->single and point its targets at the resident map.
 int stage_single(lins_ctx* ctx, const lins_point* surf_flat, int ns, const lins_point* corner_sharp, int nc,
                  const double* state_in, const double* cov_in, bool trace) {
-  if (ctx->map_ns < 0) return fail(ctx, LINS_E_NOMAP, "lins_gpu_set_map has not been called");
+  if (ctx->map.n == 0) return fail(ctx, LINS_E_NOMAP, "lins_gpu_set_map has not been called");
   if (check_cloud(ctx, surf_flat, ns, "bad surf_flat cloud") != LINS_OK || check_cloud(ctx, corner_sharp, nc, "bad corner_sharp cloud") != LINS_OK)
     return LINS_E_INVALID;
   Resident& r = ctx->single;
@@ -509,28 +503,15 @@ int stage_single(lins_ctx* ctx, const lins_point* surf_flat, int ns, const lins_
   CK(cudaMemcpyAsync(r.qc_off.p, r.h_off.p + 2, sizeof(int) * 2, cudaMemcpyHostToDevice, ctx->stream));
   CK(cudaMemcpyAsync(r.state_in.p, r.h_state.p, sizeof(double) * 20, cudaMemcpyHostToDevice, ctx->stream));
   CK(cudaMemcpyAsync(r.cov_in.p, r.h_cov.p, sizeof(double) * 324, cudaMemcpyHostToDevice, ctx->stream));
-  r.nts = (size_t)std::max(std::max(ctx->map_ns, ctx->tree_ns), 0);
-  r.ntc = (size_t)std::max(std::max(ctx->map_nc, ctx->tree_nc), 0);
+  r.nts = (size_t)ctx->map.h_off[1];  // (the index is built over the map)
+  r.ntc = (size_t)ctx->map.h_off[3];
   return reserve_outputs(ctx, r, true, trace);
 }
 
 BatchView single_view(lins_ctx* ctx, bool trace) {
   BatchView bv = view_of(ctx->single, true, trace);
-  bv.ts = ctx->map_s.p; bv.ts_off = ctx->map_off.p + 0;
-  bv.tc = ctx->map_c.p; bv.tc_off = ctx->map_off.p + 2;
-  if (!ctx->tree_is_map) {
-    bv.nn_s = ctx->tree_s.p; bv.nn_s_off = ctx->map_off.p + 4;
-    bv.nn_c = ctx->tree_c.p; bv.nn_c_off = ctx->map_off.p + 6;
-  }
+  map_targets(bv, ctx->map);
   return bv;
-}
-
-int upload_map_offsets(lins_ctx* ctx) {
-  CK(ctx->map_off.reserve(8));
-  int h[8] = {0, ctx->map_ns, 0, ctx->map_nc, 0, ctx->tree_ns, 0, ctx->tree_nc};
-  // (h is pageable stack memory: cudaMemcpyAsync returns once it has been copied to the driver's staging buffer)
-  CK(cudaMemcpyAsync(ctx->map_off.p, h, sizeof(h), cudaMemcpyHostToDevice, ctx->stream));
-  return LINS_OK;
 }
 
 // r's outputs into the caller's arrays (each may be null; states as ABI rows) through r's pinned staging: one synchronisation
@@ -589,10 +570,18 @@ int icp_loop(lins_ctx* ctx, Resident& r, BatchView bv, double* pose, IcpState* i
   return LINS_OK;
 }
 
-int transform_to_end_csr(lins_ctx* ctx, float4* pts, const int* off, int n_units, const double* lin, const unsigned char* run,
-                         const double* period) {
+// walks and tripods on the maps of g's units, the 1-NN search of a stale unit on its 1-NN clouds
+void map_targets(BatchView& bv, const MapGen& g) {
+  const int N1 = g.n + 1;
+  bv.ts = g.cur[0].p; bv.ts_off = g.off(); bv.tc = g.cur[1].p; bv.tc_off = g.off() + N1;
+  bv.nn_s = g.cur[2].p; bv.nn_s_off = g.off() + 2 * N1; bv.nn_c = g.cur[3].p; bv.nn_c_off = g.off() + 3 * N1;
+  bv.nn_stale = g.stale();
+}
+
+int transform_to_end(lins_ctx* ctx, float4* pts, const int* off, int n_units, const double* lin, const unsigned char* run,
+                     const double* period) {
   if (n_units <= 0) return LINS_OK;
-  lins_transform_to_end_csr_kernel<<<n_units, 256, 0, ctx->stream>>>(pts, off, lin, run, period);
+  lins_transform_to_end_kernel<<<n_units, 256, 0, ctx->stream>>>(pts, off, lin, run, period, 0.0, nullptr);
   CK(cudaGetLastError());
   ctx->launches += 1;
   return LINS_OK;
@@ -659,10 +648,18 @@ int lins_gpu_set_map(lins_ctx* ctx, const lins_point* surf, int ns, const lins_p
   if (check_cloud(ctx, surf, ns, "bad surf map cloud") != LINS_OK || check_cloud(ctx, corner, nc, "bad corner map cloud") != LINS_OK)
     return LINS_E_INVALID;
   CK(cudaSetDevice(ctx->device));
-  const int rc = upload2(ctx, ctx->map_s, surf, ns, ctx->map_c, corner, nc);
+  MapGen& g = ctx->map;
+  // every allocation first: the map only changes once nothing can fail any more
+  int rc = reserve_maps(ctx, g, 1, 0, 0);
+  if (rc == LINS_OK) rc = upload2_reserve(ctx, g.nxt[0], ns, g.nxt[1], nc);
   if (rc != LINS_OK) return rc;
-  ctx->map_ns = ns; ctx->map_nc = nc; ctx->tree_ns = ns; ctx->tree_nc = nc; ctx->tree_is_map = true;
-  return upload_map_offsets(ctx);
+  g.reset(1);
+  g.h_noff = {0, ns, 0, nc, 0, 0, 0, 0};
+  swap_maps(g);
+  rc = upload2_queue(ctx, g.cur[0], surf, ns, g.cur[1], corner, nc);
+  if (rc != LINS_OK) return rc;
+  CK(queue_map_state(ctx, g));
+  return LINS_OK;
 }
 
 int lins_gpu_ieskf(lins_ctx* ctx, const lins_point* surf_flat, int ns, const lins_point* corner_sharp, int nc,
@@ -848,8 +845,8 @@ int lins_gpu_estimate_transform(lins_ctx* ctx, const lins_point* surf_flat, int 
   return LINS_OK;
 }
 
-// ≙ updatePointCloud (StateEstimator.hpp:1116-1161), XYZ part: transformToEnd on the device, then the map swap + the
-// guarded index refresh.  The clouds stay on the device as the next map; copying them back is optional (the reference
+// ≙ updatePointCloud (StateEstimator.hpp:1116-1161), XYZ part: the map swap + the guarded index refresh (refresh_maps),
+// with transformToEnd in place on the new map on the device.  Copying the clouds back is optional (the reference
 // transforms scan_new_'s clouds in place because the mapping node consumes them) and, when asked for, is one D2H of
 // full PointXYZI records straight into the caller's clouds — one stream synchronisation per call, none without read-back.
 int lins_gpu_update_map_ex(lins_ctx* ctx, const lins_point* surf, int ns, const lins_point* corner, int nc, const double* lin_state,
@@ -863,40 +860,45 @@ int lins_gpu_update_map_ex(lins_ctx* ctx, const lins_point* surf, int ns, const 
     if (ctx->single.n != 1 || !ctx->single.state_out.p) return fail(ctx, LINS_E_INVALID, "no device-resident state: call lins_gpu_ieskf first or pass lin_state");
     lin_dev = ctx->single.state_out.p;
   }
-  const bool rebuild = nc >= 5 && ns >= 20;  // :1156-1157
   const bool want_out = (ns > 0 && surf_out) || (nc > 0 && corner_out);
-  // every allocation first: the context is only changed once nothing can fail any more
-  const bool keep_tree = !rebuild && ctx->tree_is_map;  // keep the old map alive as the 1-NN cloud if the guard fails
-  Buf<float4>& dst_s = keep_tree ? ctx->tree_s : ctx->map_s;  // (after the swap below these are the new map buffers)
-  Buf<float4>& dst_c = keep_tree ? ctx->tree_c : ctx->map_c;
-  int rc = upload2_reserve(ctx, dst_s, ns, dst_c, nc);  // (waits until the H2D of a previous call has read the staging)
+  MapGen& g = ctx->map;
+  // every allocation first: the map only changes once nothing can fail any more.  The new clouds go straight into the
+  // next generation's map buffers.
+  int rc = reserve_maps(ctx, g, 1, 0, 0);
+  if (rc == LINS_OK) rc = upload2_reserve(ctx, g.nxt[0], ns, g.nxt[1], nc);  // (waits until the H2D of a previous call has read the staging)
   if (rc != LINS_OK) return rc;
-  CK(ctx->map_s.reserve(1)); CK(ctx->map_c.reserve(1)); CK(ctx->tree_s.reserve(1)); CK(ctx->tree_c.reserve(1));
   CK(ctx->tmp_lin.reserve(20));
   if (want_out) CK(ctx->tmp_out.reserve((size_t)ns + nc + 1));
-  if (keep_tree) {
-    std::swap(ctx->tree_s, ctx->map_s); std::swap(ctx->tree_c, ctx->map_c);
-    ctx->tree_ns = std::max(ctx->map_ns, 0); ctx->tree_nc = std::max(ctx->map_nc, 0);
-    ctx->tree_is_map = false;
-  }
+  if (g.n == 0) g.reset(1);  // (before any set_map: an empty map)
+  const MapRefresh m = refresh_maps(g, 0, MapPiece{g.nxt[0].p, ns}, MapPiece{g.nxt[1].p, nc});
+  // a 1-NN cloud that stays is a whole current buffer (one unit): it moves into the next generation by exchange
+  for (int c = 2; c < 4; ++c)
+    for (Buf<float4>& b : g.cur)
+      if (m.next[c].len && m.next[c].src == b.p) { std::swap(g.nxt[c], b); break; }
+  g.h_noff = {0, ns, 0, nc, 0, m.next[2].len, 0, m.next[3].len};
+  swap_maps(g);
+  g.h_stale[0] = m.stale;
   if (lin_state) {
     double lin[20];
     pad_states(lin, lin_state, 1);
     CK(cudaMemcpyAsync(ctx->tmp_lin.p, lin, sizeof(lin), cudaMemcpyHostToDevice, ctx->stream));  // (pageable source: staged before the call returns)
     lin_dev = ctx->tmp_lin.p;
   }
-  rc = upload2_queue(ctx, ctx->map_s, surf, ns, ctx->map_c, corner, nc);
+  rc = upload2_queue(ctx, g.cur[0], surf, ns, g.cur[1], corner, nc);
   if (rc != LINS_OK) return rc;
+  CK(queue_map_state(ctx, g));
   lins_point* o_s = surf_out && ns ? ctx->tmp_out.p : nullptr;
   lins_point* o_c = corner_out && nc ? ctx->tmp_out.p + ns : nullptr;
-  if (ns) { lins_transform_to_end_kernel<<<(ns + 255) / 256, 256, 0, ctx->stream>>>(ctx->map_s.p, ns, lin_dev, ctx->prm.scan_period, o_s); ctx->launches += 1; }
-  if (nc) { lins_transform_to_end_kernel<<<(nc + 255) / 256, 256, 0, ctx->stream>>>(ctx->map_c.p, nc, lin_dev, ctx->prm.scan_period, o_c); ctx->launches += 1; }
+  const int np[2] = {ns, nc};
+  lins_point* out[2] = {o_s, o_c};
+  for (int k = 0; k < 2; ++k) {  // (cloud k of the unit: offsets off()[2k], off()[2k + 1])
+    if (!np[k]) continue;
+    const dim3 grid(1, std::min((np[k] + 255) / 256, 65535));
+    lins_transform_to_end_kernel<<<grid, 256, 0, ctx->stream>>>(g.cur[k].p, g.off() + 2 * k, lin_dev, nullptr, nullptr, ctx->prm.scan_period, out[k]);
+    ctx->launches += 1;
+  }
   CK(cudaGetLastError());
-  ctx->map_ns = ns; ctx->map_nc = nc;
-  if (rebuild) { ctx->tree_is_map = true; ctx->tree_ns = ns; ctx->tree_nc = nc; }
-  if (map_replaced) *map_replaced = rebuild ? 1 : 0;
-  rc = upload_map_offsets(ctx);
-  if (rc != LINS_OK) return rc;
+  if (map_replaced) *map_replaced = m.stale ? 0 : 1;
   if (want_out) {  // full records through pinned staging (a D2H into pageable memory is staged chunk by chunk by the driver)
     CK(ctx->h_out.reserve((size_t)ns + nc + 1));
     if (o_s) CK(cudaMemcpyAsync(ctx->h_out.p, o_s, sizeof(lins_point) * ns, cudaMemcpyDeviceToHost, ctx->stream));

@@ -51,11 +51,11 @@ struct BatchView {
   const float4* qc; const int* qc_off;   // corner queries (cornerPointsSharp_)
   const float4* ts; const int* ts_off;   // surf targets   (last surfPointsLessFlat_)
   const float4* tc; const int* tc_off;   // corner targets (last cornerPointsLessSharp_)
-  // clouds the 1-NN index was built on; null = same as ts/tc.  They differ only after a map refresh that
-  // failed the >=5 && >=20 guard (StateEstimator.hpp:1156-1157): scan_last_ advanced, the kd-trees did not.
+  // clouds the 1-NN index was built on where they differ from ts/tc: after a map refresh that failed the >=5 && >=20
+  // guard (StateEstimator.hpp:1156-1157) scan_last_ advanced, the kd-trees did not.  Null (with nn_stale) = none.
   const float4* nn_s; const int* nn_s_off;
   const float4* nn_c; const int* nn_c_off;
-  const unsigned char* nn_stale;         // per unit: 1 = nn_s / nn_c hold its 1-NN clouds; null = every unit's do (when nn_s is set)
+  const unsigned char* nn_stale;         // per unit, set with nn_s: 1 = nn_s / nn_c hold its 1-NN clouds
   const double* state_in;                // n x 20 (19 used)
   const double* cov_in;                  // n x 324, column-major
   double* state_out;                     // n x 20
@@ -100,7 +100,7 @@ struct KParams {
 
 // unit `scan` searches a 1-NN cloud of its own (a stale index: brute-force 1-NN over it, then walks over the map)
 __device__ __forceinline__ bool nn_separate(const BatchView& bv, int scan) {
-  return bv.nn_s != nullptr && (bv.nn_stale == nullptr || bv.nn_stale[scan] != 0);
+  return bv.nn_s != nullptr && bv.nn_stale[scan] != 0;
 }
 
 __device__ __forceinline__ unsigned long long pack_key(float d, unsigned int lo) {

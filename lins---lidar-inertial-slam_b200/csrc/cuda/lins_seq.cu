@@ -313,10 +313,8 @@ int launch_fresh(lins_ctx* ctx, SeqState& q, int n, const unsigned char* mask_de
 int reserve_run(lins_ctx* ctx, SeqState& q, int n, size_t ns, size_t nc) {
   CK(q.filt.reserve((size_t)n * 20)); CK(q.cov.reserve((size_t)n * 324)); CK(q.glob.reserve((size_t)n * 20));
   CK(q.lin.reserve((size_t)n * 20)); CK(q.imu_last.reserve((size_t)n * 8)); CK(q.icp_pose.reserve((size_t)n * 20)); CK(q.icp.reserve(icp_state_bytes() * n));
-  CK(q.map_s.reserve(ns + 1)); CK(q.map_c.reserve(nc + 1)); CK(q.tree_s.reserve(1)); CK(q.tree_c.reserve(1));
-  CK(q.map_off.reserve(4 * (size_t)(n + 1))); CK(q.stale.reserve(n));
   CK(q.run.results.reserve(n)); CK(q.run.reports.reserve(n));
-  return LINS_OK;
+  return reserve_maps(ctx, q.map, n, ns, nc);
 }
 
 // the host side of a run whose slots are in place: no step yet, every slot idle in the given fusion status
@@ -333,46 +331,66 @@ void install_run(SeqState& q, int n, bool has_init) {
 
 namespace lins_capi {
 
-// queue the upload of the host copies of map_off and stale (pageable: the caller synchronises before they change)
-cudaError_t queue_map_state(lins_ctx* ctx, SeqState& q) {
-  const cudaError_t e = cudaMemcpyAsync(q.map_off.p, q.h_map_off.data(), sizeof(int) * q.h_map_off.size(), cudaMemcpyHostToDevice, ctx->stream);
-  return e != cudaSuccess ? e : cudaMemcpyAsync(q.stale.p, q.h_stale_v.data(), q.h_stale_v.size(), cudaMemcpyHostToDevice, ctx->stream);
-}
-
 // ---- map generations -----------------------------------------------------------------------------------------------------
-// Where one (cloud, slot) range of the next generation comes from: a MapPiece (lins_ctx.hpp)
+// Where one (cloud, unit) range of the next generation comes from: a MapPiece (lins_ctx.hpp)
 
-// cloud c (map_s, map_c, tree_s, tree_c) of slot s in the current generation
-MapPiece current_piece(const SeqState& q, int c, int s) {
-  const int N1 = q.n + 1;
-  const int* mo = q.h_map_off.data();
-  const float4* srcs[4] = {q.map_s.p, q.map_c.p, q.tree_s.p, q.tree_c.p};
-  return MapPiece{srcs[c] + mo[c * N1 + s], mo[c * N1 + s + 1] - mo[c * N1 + s]};
+// g's device state for n units and current maps of ns / nc points
+int reserve_maps(lins_ctx* ctx, MapGen& g, int n, size_t ns, size_t nc) {
+  CK(g.cur[0].reserve(ns + 1)); CK(g.cur[1].reserve(nc + 1)); CK(g.cur[2].reserve(1)); CK(g.cur[3].reserve(1));
+  for (Buf<float4>& b : g.nxt) CK(b.reserve(1));
+  CK(g.dev.reserve(4 * (size_t)(n + 1) + (n + 3) / 4));
+  return LINS_OK;
 }
 
-// The next generation from next[4 * s + c], slot s's cloud c: fills h_nmap_off, reserves nmap_* / ntree_* and appends the
-// copies that fill them, in slot order, to `copies`
-int build_next_maps(lins_ctx* ctx, SeqState& q, const std::vector<MapPiece>& next, std::vector<DevCopy>& copies) {
-  const int n = q.n, N1 = n + 1;
-  q.h_nmap_off.assign(4 * (size_t)N1, 0);
-  int* no = q.h_nmap_off.data();
+// queue the upload of h_off and h_stale (one H2D from a pageable copy: the driver stages it before the call returns)
+cudaError_t queue_map_state(lins_ctx* ctx, MapGen& g) {
+  std::vector<int> h(g.h_off.size() + (g.n + 3) / 4, 0);
+  std::copy(g.h_off.begin(), g.h_off.end(), h.begin());
+  std::memcpy(h.data() + g.h_off.size(), g.h_stale.data(), g.h_stale.size());
+  return cudaMemcpyAsync(g.dev.p, h.data(), sizeof(int) * h.size(), cudaMemcpyHostToDevice, ctx->stream);
+}
+
+// cloud c (map_s, map_c, tree_s, tree_c) of unit s in the current generation
+MapPiece current_piece(const MapGen& g, int c, int s) {
+  const int N1 = g.n + 1;
+  const int* mo = g.h_off.data();
+  return MapPiece{g.cur[c].p + mo[c * N1 + s], mo[c * N1 + s + 1] - mo[c * N1 + s]};
+}
+
+// the map swap of updatePointCloud (:1151-1160) for unit s and its new clouds: they become its map; its 1-NN index is
+// rebuilt on them iff corner >= 5 && surf >= 20 (not stale), else it stays on the clouds it was built on: the old map,
+// or the older clouds of a unit that is already stale
+MapRefresh refresh_maps(const MapGen& g, int s, MapPiece surf, MapPiece corner) {
+  MapRefresh r{{surf, corner, MapPiece{}, MapPiece{}}, 0};
+  if (corner.len >= 5 && surf.len >= 20) return r;  // :1156-1157
+  const int from = g.h_stale[s] ? 2 : 0;
+  r.next[2] = current_piece(g, from, s);
+  r.next[3] = current_piece(g, from + 1, s);
+  r.stale = 1;
+  return r;
+}
+
+// The next generation from next[4 * s + c], unit s's cloud c: fills h_noff, reserves nxt and appends the copies that fill
+// it, in unit order, to `copies`
+int build_next_maps(lins_ctx* ctx, MapGen& g, const std::vector<MapPiece>& next, std::vector<DevCopy>& copies) {
+  const int n = g.n, N1 = n + 1;
+  g.h_noff.assign(4 * (size_t)N1, 0);
+  int* no = g.h_noff.data();
   for (int s = 0; s < n; ++s)
     for (int c = 0; c < 4; ++c) no[c * N1 + s + 1] = no[c * N1 + s] + next[4 * (size_t)s + c].len;
-  CK(q.nmap_s.reserve((size_t)no[N1 - 1] + 1)); CK(q.nmap_c.reserve((size_t)no[2 * N1 - 1] + 1));
-  CK(q.ntree_s.reserve((size_t)no[3 * N1 - 1] + 1)); CK(q.ntree_c.reserve((size_t)no[4 * N1 - 1] + 1));
-  float4* dst[4] = {q.nmap_s.p, q.nmap_c.p, q.ntree_s.p, q.ntree_c.p};
+  for (int c = 0; c < 4; ++c) CK(g.nxt[c].reserve((size_t)no[(c + 1) * N1 - 1] + 1));
   for (int s = 0; s < n; ++s)
     for (int c = 0; c < 4; ++c) {
       const MapPiece& p = next[4 * (size_t)s + c];
-      if (p.len) copies.push_back(DevCopy{p.src, dst[c] + no[c * N1 + s], p.len, 0});
+      if (p.len) copies.push_back(DevCopy{p.src, g.nxt[c].p + no[c * N1 + s], p.len, 0});
     }
   return LINS_OK;
 }
 
-// the next generation becomes the current one (its copies have been queued)
-void swap_maps(SeqState& q) {
-  std::swap(q.map_s, q.nmap_s); std::swap(q.map_c, q.nmap_c); std::swap(q.tree_s, q.ntree_s); std::swap(q.tree_c, q.ntree_c);
-  q.h_map_off.swap(q.h_nmap_off);
+// the next generation becomes the current one (whatever fills it has been queued)
+void swap_maps(MapGen& g) {
+  for (int c = 0; c < 4; ++c) std::swap(g.cur[c], g.nxt[c]);
+  g.h_off.swap(g.h_noff);
 }
 
 }  // namespace lins_capi
@@ -430,7 +448,7 @@ int seq_step_phases(lins_ctx* ctx, const lins_seq_step_desc* d, const int32_t* c
   const int N1 = n + 1;
   if (q.pub.bound) q.pub.fusion_before = q.fusion;  // (publishTopics' rule reads the status before the scan)
   std::vector<MapPiece> next(4 * (size_t)n);
-  std::vector<unsigned char> new_stale(q.h_stale_v);
+  std::vector<unsigned char> new_stale(q.map.h_stale);
   std::vector<unsigned char> imu_use(n, IMU_IGNORE);
   int n_run = 0, n_init = 0, n_second = 0;
   for (int s = 0; s < n; ++s) {
@@ -448,18 +466,15 @@ int seq_step_phases(lins_ctx* ctx, const lins_seq_step_desc* d, const int32_t* c
     n_run += ran;
     n_init += init;
     n_second += status[s] == LINS_SEQ_SECOND;
-    // map swap (:1151-1160): the new clouds become the map; the 1-NN index is rebuilt iff ncl >= 5 && nsl >= 20, else it
-    // stays on the cloud it was built on (the old map, or an older stale cloud).  A first scan's clouds become the map
-    // as they are (setInputCloud, :363-364) and a second scan's like a running one's: both pass the guard after the init gate.
+    // map swap (refresh_maps).  A first scan's clouds become the map as they are (setInputCloud, :363-364) and a second
+    // scan's like a running one's: both pass the guard after the init gate.
     MapPiece* p = &next[4 * (size_t)s];  // map_s, map_c, tree_s, tree_c
     if (ran || init) {
-      p[0] = MapPiece{q.up.ts.p + offs[2][s], nsl};
-      p[1] = MapPiece{q.up.tc.p + offs[3][s], ncl};
-      if (ncl >= 5 && nsl >= 20) new_stale[s] = 0;
-      else if (!q.h_stale_v[s]) { p[2] = current_piece(q, 0, s); p[3] = current_piece(q, 1, s); new_stale[s] = 1; }
-      else { p[2] = current_piece(q, 2, s); p[3] = current_piece(q, 3, s); }
+      const MapRefresh m = refresh_maps(q.map, s, MapPiece{q.up.ts.p + offs[2][s], nsl}, MapPiece{q.up.tc.p + offs[3][s], ncl});
+      std::copy(m.next, m.next + 4, p);
+      new_stale[s] = m.stale;
     } else {
-      for (int c = 0; c < 4; ++c) p[c] = current_piece(q, c, s);
+      for (int c = 0; c < 4; ++c) p[c] = current_piece(q.map, c, s);
     }
   }
   // the IESKF's queries, then the second scans' after them in the compacted buffers, with offsets of their own (init_off):
@@ -476,14 +491,14 @@ int seq_step_phases(lins_ctx* ctx, const lins_seq_step_desc* d, const int32_t* c
   // ---- allocations ------------------------------------------------------------------------------------------------
   Resident& r = q.run;
   r.n = n; r.nqs = init_off[N1 - 1]; r.nqc = init_off[2 * N1 - 1]; r.max_q = max_q;
-  r.nts = q.h_map_off[N1 - 1]; r.ntc = q.h_map_off[2 * N1 - 1];
+  r.nts = q.map.h_off[N1 - 1]; r.ntc = q.map.h_off[2 * N1 - 1];
   CK(r.qs.reserve(r.nqs + 1)); CK(r.qc.reserve(r.nqc + 1)); CK(r.qs_off.reserve(N1)); CK(r.qc_off.reserve(N1));
   rc = reserve_outputs(ctx, r, true, false);
   if (rc != LINS_OK) return rc;
   CK(r.h_off.reserve(4 * (size_t)N1));
   if (n_init) { CK(q.init_off.reserve(2 * (size_t)N1)); CK(q.scan_imu.reserve((size_t)n * 6)); CK(q.h_scan_imu.reserve((size_t)n * 6)); }
   // (pre and init_icp are lins_gpu_seq_open's: they keep their contents from step to step)
-  rc = build_next_maps(ctx, q, next, copies);
+  rc = build_next_maps(ctx, q.map, next, copies);
   if (rc != LINS_OK) return rc;
   const size_t n_imu = d->imu_off ? (size_t)d->imu_off[n] : 0;
   CK(q.imu.reserve(7 * n_imu + 1)); CK(q.imu_off.reserve(N1)); CK(q.h_imu.reserve(7 * n_imu + 1)); CK(q.h_imu_off.reserve(N1));
@@ -563,9 +578,7 @@ int seq_step_phases(lins_ctx* ctx, const lins_seq_step_desc* d, const int32_t* c
   std::memset(&bv, 0, sizeof(bv));
   bv.n_scans = n;
   bv.qs = r.qs.p; bv.qs_off = r.qs_off.p; bv.qc = r.qc.p; bv.qc_off = r.qc_off.p;
-  bv.ts = q.map_s.p; bv.ts_off = q.map_off.p; bv.tc = q.map_c.p; bv.tc_off = q.map_off.p + N1;
-  bv.nn_s = q.tree_s.p; bv.nn_s_off = q.map_off.p + 2 * N1; bv.nn_c = q.tree_c.p; bv.nn_c_off = q.map_off.p + 3 * N1;
-  bv.nn_stale = q.stale.p;
+  map_targets(bv, q.map);
   bv.unit_period = q.period.p;
   bv.unit_tune = q.unit_tune.p;
   bv.state_in = q.prior_state.p; bv.cov_in = q.prior_cov.p; bv.state_out = r.state_out.p; bv.cov_out = r.cov_out.p;
@@ -645,13 +658,13 @@ int seq_step_phases(lins_ctx* ctx, const lins_seq_step_desc* d, const int32_t* c
   for (int s = 0; s < n; ++s)
     q.h_status.p[n + s] = status[s] == LINS_SEQ_RAN || status[s] == LINS_SEQ_ICP || status[s] == LINS_SEQ_SECOND ? 1 : 0;
   CK(cudaMemcpyAsync(run_mask, q.h_status.p + n, n, cudaMemcpyHostToDevice, ctx->stream));
-  rc = transform_to_end_csr(ctx, q.up.ts.p, q.up.ts_off.p, n, q.lin.p, run_mask, q.period.p);
-  if (rc == LINS_OK) rc = transform_to_end_csr(ctx, q.up.tc.p, q.up.tc_off.p, n, q.lin.p, run_mask, q.period.p);
+  rc = transform_to_end(ctx, q.up.ts.p, q.up.ts_off.p, n, q.lin.p, run_mask, q.period.p);
+  if (rc == LINS_OK) rc = transform_to_end(ctx, q.up.tc.p, q.up.tc_off.p, n, q.lin.p, run_mask, q.period.p);
   if (rc == LINS_OK) rc = q.copies.launch(ctx, n_qcopies, n_copies - n_qcopies);
   if (rc != LINS_OK) return rc;
-  swap_maps(q);
-  q.h_stale_v = new_stale;
-  CK(queue_map_state(ctx, q));
+  swap_maps(q.map);
+  q.map.h_stale = new_stale;
+  CK(queue_map_state(ctx, q.map));
   CK(cudaEventRecord(q.ev[4], ctx->stream));
   if (q.pub.bound) CK(cudaMemcpyAsync(q.pub.h_glob.p, q.glob.p, sizeof(double) * 20 * (size_t)n, cudaMemcpyDeviceToHost, ctx->stream));
   CK(cudaStreamSynchronize(ctx->stream));  // (the two sources above are pageable and change with the next step)
@@ -823,8 +836,8 @@ int seq_map_run(lins_ctx* ctx, const lins_seq_map_desc* d, lins_mapper_report* r
     if (!pub[s]) continue;
     const SeqSlot& r = q.slot[s];
     if (r.yzx) {
-      dev[3 * s + 0] = current_piece(q, 1, s);
-      dev[3 * s + 1] = current_piece(q, 0, s);
+      dev[3 * s + 0] = current_piece(q.map, 1, s);
+      dev[3 * s + 1] = current_piece(q.map, 0, s);
       dev[3 * s + 2] = MapPiece{pb.outl.p + pb.h_outl_off[s], pb.h_outl_off[s + 1] - pb.h_outl_off[s]};
     }
     std::copy(r.pose, r.pose + 3, &pos[3 * (size_t)s]);
@@ -865,22 +878,21 @@ int lins_gpu_seq_begin(lins_ctx* ctx, const lins_seq_params* prm, const lins_seq
   const size_t ns = d->surf_map_off[n], nc = d->corner_map_off[n];
   rc = reserve_run(ctx, q, n, ns, nc);
   if (rc != LINS_OK) return rc;
-  if (ns) CK(cudaMemcpyAsync(q.map_s.p, q.up.ts.p, sizeof(float4) * ns, cudaMemcpyDeviceToDevice, ctx->stream));
-  if (nc) CK(cudaMemcpyAsync(q.map_c.p, q.up.tc.p, sizeof(float4) * nc, cudaMemcpyDeviceToDevice, ctx->stream));
+  if (ns) CK(cudaMemcpyAsync(q.map.cur[0].p, q.up.ts.p, sizeof(float4) * ns, cudaMemcpyDeviceToDevice, ctx->stream));
+  if (nc) CK(cudaMemcpyAsync(q.map.cur[1].p, q.up.tc.p, sizeof(float4) * nc, cudaMemcpyDeviceToDevice, ctx->stream));
   std::vector<double> st((size_t)n * 20), gl((size_t)n * 20), il((size_t)n * 8);
   pad_states(st.data(), d->filter_state, n);
   pad_states(gl.data(), d->global_state, n);
   copy_rows(il.data(), 8, d->imu_last, 6, n);
-  q.h_map_off.assign(4 * (size_t)(n + 1), 0);
-  std::memcpy(&q.h_map_off[0], d->surf_map_off, sizeof(int) * (n + 1));
-  std::memcpy(&q.h_map_off[n + 1], d->corner_map_off, sizeof(int) * (n + 1));
-  q.h_stale_v.assign(n, 0);
+  q.map.reset(n);
+  std::memcpy(&q.map.h_off[0], d->surf_map_off, sizeof(int) * (n + 1));
+  std::memcpy(&q.map.h_off[n + 1], d->corner_map_off, sizeof(int) * (n + 1));
   CK(cudaMemcpyAsync(q.filt.p, st.data(), sizeof(double) * st.size(), cudaMemcpyHostToDevice, ctx->stream));
   CK(cudaMemcpyAsync(q.lin.p, st.data(), sizeof(double) * st.size(), cudaMemcpyHostToDevice, ctx->stream));
   CK(cudaMemcpyAsync(q.glob.p, gl.data(), sizeof(double) * gl.size(), cudaMemcpyHostToDevice, ctx->stream));
   CK(cudaMemcpyAsync(q.imu_last.p, il.data(), sizeof(double) * il.size(), cudaMemcpyHostToDevice, ctx->stream));
   CK(cudaMemcpyAsync(q.cov.p, d->filter_cov, sizeof(double) * 324 * (size_t)n, cudaMemcpyHostToDevice, ctx->stream));
-  CK(queue_map_state(ctx, q));
+  CK(queue_map_state(ctx, q.map));
   CK(cudaStreamSynchronize(ctx->stream));  // (the sources above are pageable host memory)
   consts_of(q.consts, prm);
   std::fill(q.init_consts, q.init_consts + kNInit, 0.0);  // (a hand-over does not initialise)
@@ -908,8 +920,7 @@ int lins_gpu_seq_open(lins_ctx* ctx, const lins_seq_params* prm, const lins_seq_
   init_consts_of(q.init_consts, prm, ip);
   q.slot.assign(n, SeqSlot());
   if ((rc = upload_slot_consts(ctx, n)) != LINS_OK) return rc;
-  q.h_map_off.assign(4 * (size_t)(n + 1), 0);
-  q.h_stale_v.assign(n, 0);
+  q.map.reset(n);
   CK(cudaMemsetAsync(q.lin.p, 0, sizeof(double) * 20 * (size_t)n, ctx->stream));
   CK(cudaMemsetAsync(q.imu_last.p, 0, sizeof(double) * 8 * (size_t)n, ctx->stream));
   CK(cudaMemsetAsync(q.pre.p, 0, sizeof(double) * 20 * (size_t)n, ctx->stream));
@@ -917,7 +928,7 @@ int lins_gpu_seq_open(lins_ctx* ctx, const lins_seq_params* prm, const lins_seq_
   CK(cudaMemsetAsync(q.init_icp.p, 0, icp_state_bytes() * n, ctx->stream));
   CK(cudaMemsetAsync(q.run.results.p, 0, sizeof(lins_scan_result) * n, ctx->stream));
   CK(cudaMemsetAsync(q.run.reports.p, 0, sizeof(lins_report) * n, ctx->stream));
-  CK(queue_map_state(ctx, q));
+  CK(queue_map_state(ctx, q.map));
   rc = launch_fresh(ctx, q, n, nullptr);
   if (rc != LINS_OK) return rc;
   CK(cudaStreamSynchronize(ctx->stream));  // (the sources above are pageable host memory)
@@ -934,9 +945,9 @@ int lins_gpu_seq_restart(lins_ctx* ctx, const uint8_t* mask) {
   // the restarted slots' maps go: the other slots' ranges are copied into the next generation, which is swapped in
   std::vector<MapPiece> next(4 * (size_t)n);
   for (int s = 0; s < n; ++s)
-    if (!mask[s]) for (int c = 0; c < 4; ++c) next[4 * (size_t)s + c] = current_piece(q, c, s);
+    if (!mask[s]) for (int c = 0; c < 4; ++c) next[4 * (size_t)s + c] = current_piece(q.map, c, s);
   std::vector<DevCopy> copies;
-  rc = build_next_maps(ctx, q, next, copies);
+  rc = build_next_maps(ctx, q.map, next, copies);
   if (rc == LINS_OK) rc = q.copies.reserve(ctx, copies.size());
   if (rc != LINS_OK) return rc;
   CK(q.status_d.reserve(3 * (size_t)n)); CK(q.h_status.reserve(3 * (size_t)n));
@@ -953,16 +964,16 @@ int lins_gpu_seq_restart(lins_ctx* ctx, const uint8_t* mask) {
   rc = q.copies.launch(ctx, 0, (int)copies.size());
   if (rc == LINS_OK) rc = launch_fresh(ctx, q, n, q.status_d.p);
   if (rc != LINS_OK) { q.n = 0; return rc; }  // (some slots may have changed: the run ends, as after a failed step)
-  swap_maps(q);
+  swap_maps(q.map);
   for (int s = 0; s < n; ++s)
-    if (mask[s]) { q.h_stale_v[s] = 0; q.fusion[s] = FUSION_INIT; q.status[s] = LINS_SEQ_IDLE; }
+    if (mask[s]) { q.map.h_stale[s] = 0; q.fusion[s] = FUSION_INIT; q.status[s] = LINS_SEQ_IDLE; }
   // a new recording is a new LinsFusion with a new mapping node (and nothing fused yet)
   if (q.pub.bound) {
     for (int s = 0; s < n; ++s) if (mask[s]) q.pub.fused[s] = lins_fused_pose{};
     if ((rc = mappers_reset(ctx, ctx->mappers, mask)) != LINS_OK) return rc;
   }
-  CK(queue_map_state(ctx, q));
-  CK(cudaStreamSynchronize(ctx->stream));  // (the two sources above are pageable)
+  CK(queue_map_state(ctx, q.map));
+  CK(cudaStreamSynchronize(ctx->stream));  // (the source above is pageable)
   return LINS_OK;
 }
 
@@ -1130,8 +1141,8 @@ int lins_gpu_seq_map_published(lins_ctx* ctx, double* pose, int32_t* sizes) {
     const bool y = q.slot[s].yzx;
     if (pose) std::copy(q.slot[s].pose, q.slot[s].pose + 7, pose + 7 * (size_t)s);
     if (!sizes) continue;
-    sizes[3 * s + 0] = y ? current_piece(q, 1, s).len : 0;
-    sizes[3 * s + 1] = y ? current_piece(q, 0, s).len : 0;
+    sizes[3 * s + 0] = y ? current_piece(q.map, 1, s).len : 0;
+    sizes[3 * s + 1] = y ? current_piece(q.map, 0, s).len : 0;
     sizes[3 * s + 2] = y ? pb.h_outl_off[s + 1] - pb.h_outl_off[s] : 0;
   }
   return LINS_OK;
@@ -1240,13 +1251,12 @@ int lins_gpu_seq_download_maps(lins_ctx* ctx, int32_t* off, float* surf_map, flo
   if (q.n == 0) return fail(ctx, LINS_E_NOMAP, "lins_gpu_seq_begin has not been called");
   CK(cudaSetDevice(ctx->device));
   const size_t N1 = q.n + 1;
-  const int* mo = q.h_map_off.data();
+  const int* mo = q.map.h_off.data();
   float* dst[4] = {surf_map, corner_map, surf_tree, corner_tree};
-  const float4* src[4] = {q.map_s.p, q.map_c.p, q.tree_s.p, q.tree_c.p};
-  for (int c = 0; c < 4; ++c) CK(d2h(ctx, dst[c], src[c], sizeof(float4) * mo[c * N1 + N1 - 1]));
+  for (int c = 0; c < 4; ++c) CK(d2h(ctx, dst[c], q.map.cur[c].p, sizeof(float4) * mo[c * N1 + N1 - 1]));
   CK(cudaStreamSynchronize(ctx->stream));
   if (off) std::memcpy(off, mo, sizeof(int32_t) * 4 * N1);
-  if (stale) std::memcpy(stale, q.h_stale_v.data(), q.n);
+  if (stale) std::memcpy(stale, q.map.h_stale.data(), q.n);
   return LINS_OK;
 }
 

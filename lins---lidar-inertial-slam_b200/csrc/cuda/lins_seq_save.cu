@@ -45,7 +45,7 @@ std::vector<std::pair<int, int>> stored_keyframes(const MapperNode& m) {
 B::Counts slot_counts(const lins_ctx* ctx, int s) {
   const SeqState& q = ctx->seq;
   B::Counts c;
-  for (int k = 0; k < 4; ++k) c.n_map[k] = current_piece(q, k, s).len;
+  for (int k = 0; k < 4; ++k) c.n_map[k] = current_piece(q.map, k, s).len;
   c.bound = q.pub.bound;
   if (c.bound) {
     const MapperNode& m = ctx->mappers.node[s];
@@ -95,7 +95,7 @@ void save_copies(lins_ctx* ctx, int s, const B::Header& h, float4* dst, const st
   const int row_len[6] = {20, 324, 20, 20, 8, 20};
   for (int i = 0; i < 6; ++i) v.push_back(DevCopy{f4(rows[i]), at(B::kRows) + B::kRowOff[i] / 2, row_len[i] / 2, 0});
   float4* o = at(B::kMaps);
-  for (int c = 0; c < 4; ++c) { const MapPiece p = current_piece(q, c, s); v.push_back(DevCopy{p.src, o, p.len, 0}); o += p.len; }
+  for (int c = 0; c < 4; ++c) { const MapPiece p = current_piece(q.map, c, s); v.push_back(DevCopy{p.src, o, p.len, 0}); o += p.len; }
   if (!q.pub.bound) return;
   const SeqPubState& pb = q.pub;
   v.push_back(DevCopy{pb.outl.p + pb.h_outl_off[s], at(B::kOutlier), pb.h_outl_off[s + 1] - pb.h_outl_off[s], 0});
@@ -119,7 +119,7 @@ void save_host(lins_ctx* ctx, int s, const B::Counts& c, B::Header h, uint8_t* i
   B::Scalars sc;
   std::memset(&sc, 0, sizeof(sc));
   sc.fusion = q.fusion[s];
-  sc.stale = q.h_stale_v[s];
+  sc.stale = q.map.h_stale[s];
   for (int k = 0; k < 4; ++k) sc.n_map[k] = (int32_t)c.n_map[k];
   sc.n_outlier = (int32_t)c.n_outlier; sc.n_poses = (int32_t)c.n_poses; sc.n_window = (int32_t)c.n_window; sc.n_keyframes = (int32_t)c.n_keyframes;
   std::copy(q.consts, q.consts + 10, sc.consts);
@@ -192,13 +192,13 @@ int load_run(lins_ctx* ctx, const uint8_t* mask, const std::vector<B::View>& v) 
   for (int s = 0; s < n; ++s) {
     const float4* p = mask[s] ? at(s, B::kMaps) : nullptr;
     for (int c = 0; c < 4; ++c) {
-      if (!mask[s]) { next[4 * (size_t)s + c] = current_piece(q, c, s); continue; }
+      if (!mask[s]) { next[4 * (size_t)s + c] = current_piece(q.map, c, s); continue; }
       next[4 * (size_t)s + c] = MapPiece{p, v[s].sc.n_map[c]};
       p += v[s].sc.n_map[c];
     }
   }
   std::vector<DevCopy> copies;
-  int rc = build_next_maps(ctx, q, next, copies);
+  int rc = build_next_maps(ctx, q.map, next, copies);
   if (rc != LINS_OK) return rc;
   std::vector<MapPiece> onext;
   if (pb.bound) {
@@ -246,7 +246,7 @@ int load_run(lins_ctx* ctx, const uint8_t* mask, const std::vector<B::View>& v) 
   if (total) CK(cudaMemcpyAsync(q.blob.p, img, total, cudaMemcpyHostToDevice, ctx->stream));
   if ((rc = q.copies.stage(ctx, copies.data(), (int)copies.size(), 0)) != LINS_OK) return rc;
   if ((rc = q.copies.launch(ctx, 0, (int)copies.size())) != LINS_OK) return rc;
-  swap_maps(q);
+  swap_maps(q.map);
   if (pb.bound) { std::swap(pb.outl, pb.noutl); pb.h_outl_off.swap(pb.h_noutl_off); }
 
   // the host bookkeeping of the loaded slots
@@ -255,7 +255,7 @@ int load_run(lins_ctx* ctx, const uint8_t* mask, const std::vector<B::View>& v) 
     if (!mask[s]) continue;
     const B::View& b = v[s];
     const B::Scalars& sc = b.sc;
-    q.h_stale_v[s] = (unsigned char)sc.stale;
+    q.map.h_stale[s] = (unsigned char)sc.stale;
     q.fusion[s] = sc.fusion;
     q.status[s] = LINS_SEQ_IDLE;
     // the slot's record is the blob's.  The device constants are uploaded again when the slot is configured now or was
@@ -280,7 +280,7 @@ int load_run(lins_ctx* ctx, const uint8_t* mask, const std::vector<B::View>& v) 
     for (int i = 0; i < sc.n_poses; ++i) { const B::PoseRec p = b.pose(i); std::memcpy(&m.poses[i], &p, sizeof(p)); }
     m.last = MapperLast();  // (no DS clouds until the slot's next processed cycle)
   }
-  CK(queue_map_state(ctx, q));
+  CK(queue_map_state(ctx, q.map));
   // (upload_slot_consts ends with a synchronisation; the sources above are pageable)
   if (any_configured) return upload_slot_consts(ctx, n);
   CK(cudaStreamSynchronize(ctx->stream));

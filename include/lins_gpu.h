@@ -635,9 +635,10 @@ int lins_gpu_map_associate(lins_ctx* ctx, const lins_point* corner_last, int n_c
    scan2MapOptimization with its 10 / 100 gate and transformUpdate (:1635-1652, :538-577) and saveKeyFramesAndFactor
    (:1654-1765).  The clouds, the key-frame store, the VoxelGrids and the scan-to-map
    loop are on the device; transformAssociateToMap, transformUpdate, the key-frame test and the pose bookkeeping run on
-   the host in the reference's f32 / f64 types.  Loop closure (loopClosureThread, performLoopClosure) is not performed:
-   without a loop factor the iSAM2 estimate of a new key frame is the pose inserted for it up to f32 rounding (DESIGN.md §4.9), and
-   correctPoses is a no-op.  The reference's constants are fixed: mappingProcessInterval 0.3 s, window 50, key-frame
+   the host in the reference's f32 / f64 types.  Loop closure (loopClosureThread, performLoopClosure) runs only on a slot
+   enabled by lins_gpu_mapper_loops / lins_gpu_mappers_loops, when the caller calls lins_gpu_mapper_close_loop /
+   lins_gpu_mappers_close_loops (below).  On any other slot it is not performed: without a loop factor the iSAM2 estimate
+   of a new key frame is the pose inserted for it up to f32 rounding (DESIGN.md §4.9), and correctPoses is a no-op.  The reference's constants are fixed: mappingProcessInterval 0.3 s, window 50, key-frame
    distance 0.3 m, loop search 5 m / 30 s; SCAN_PERIOD is the context's lins_params.scan_period (a configured slot's
    own on a run bound by lins_gpu_seq_map_open, see lins_slot_config).
    All clouds are in the mapping node's YZX frame convention, like lins_gpu_scan2map's.
@@ -665,7 +666,7 @@ typedef struct lins_mapper_report {
   int32_t window_len;             /* recentCornerCloudKeyFrames.size() used by this cycle's local map */
   int32_t loop_candidate;         /* after a saved key frame: the key pose detectLoopClosure (:1043-1067) would pick (the
                                      nearest within 5 m whose time differs by > 30 s), else -1.  From such a cycle on the
-                                     reference may close a loop this library does not */
+                                     reference may close a loop, which this library closes only on an enabled slot */
   float transform_guess[6];       /* transformTobeMapped after transformAssociateToMap (the scan-to-map start) */
   float transform_aft_mapped[6];  /* transformAftMapped after the cycle */
   lins_map_report map;            /* the scan-to-map loop (map.skipped = 1: the 10 / 100 gate failed, :1636, and
@@ -719,8 +720,8 @@ int lins_gpu_voxel_grid(lins_ctx* ctx, const lins_point* in, int n, float leaf, 
    lins_gpu_mapper_download on a context of its own given the same event sequence (the interval gate, the 10 / 100 gate
    with its stale transformAftMapped, and the duplicated key frame when the window first fills included).  The slots'
    state is a member of the context of its own: lins_gpu_mapper_*, lins_gpu_map_set, lins_gpu_scan2map and
-   lins_gpu_voxel_grid on the same context neither see nor change it.  Loop closure is not performed, as in the single
-   mapper.  A call before lins_gpu_mappers_open returns LINS_E_NOMAP. */
+   lins_gpu_voxel_grid on the same context neither see nor change it.  Loop closure runs on enabled slots only, as in
+   the single mapper.  A call before lins_gpu_mappers_open returns LINS_E_NOMAP. */
 /* opens M mapper slots, each a freshly constructed mapping node (as after lins_gpu_mapper_reset); replaces any open run */
 int lins_gpu_mappers_open(lins_ctx* ctx, int32_t n_slots);
 /* slots with mask[s] != 0 back to the fresh state (hand a slot to a new drive); others untouched */
@@ -751,6 +752,56 @@ int lins_gpu_mappers_download(lins_ctx* ctx, int32_t slot, double* key_poses, in
    out[s].valid = 0 for an absent slot.  Call it with the descriptor of the next lins_gpu_mappers_step, before that step.
    LINS_E_INVALID for a NULL d or out, n_slots != M or a NULL time / quat / pos; LINS_E_NOMAP without a run. */
 int lins_gpu_mappers_fuse(lins_ctx* ctx, const lins_mappers_desc* d, lins_fused_pose* out /*M*/);
+
+/* ---- loop closure: loopClosureThread / performLoopClosure (:1033-1041, :1114-1186) and correctPoses (:1767-1795) ------
+   Opt-in per mapper slot.  An enabled slot keeps every key frame's corner, surf and outlier DS clouds twice, in the map
+   frame and in the body frame (no memory bound: 32 bytes per DS point of every key frame), and keeps the key-pose graph:
+   the prior on key 0 and the chain factors of saveKeyFramesAndFactor (:1673-1705, variances 1e-6 1e-6 1e-6 1e-8 1e-8
+   1e-6, :382-385) and the loop factors close_loops adds.  Until its first loop factor every step of an enabled slot is
+   bit-identical to a plain slot's.  From then on each key-frame save takes latestEstimate from a Gauss-Newton solve of
+   the whole graph to convergence (f64, host; iSAM2's incremental relinearisation only approaches that fixed point, and
+   how far it lags cannot be measured without gtsam: DESIGN.md §4.14), and the next processed cycle after a closure runs
+   correctPoses: every key pose from the estimate of the last save (which predates the loop factor when that cycle saved
+   no key frame, as in the reference), the stored map-frame clouds re-transformed and the window rebuilt.
+   The reference runs performLoopClosure at 1 Hz of wall time in its own thread; here the caller's call is the thread's
+   tick, run between mapping steps (bag_replay.replay(loops=True) and tools/run_bag(s).py --loops call it whenever a
+   slot's odometry stamp has advanced >= 1 s since its last call).
+   lins_gpu_mapper_reset / lins_gpu_mappers_reset (and lins_gpu_seq_restart on a bound run) return a slot to not
+   enabled; lins_gpu_seq_save and lins_gpu_seq_load refuse an enabled slot with LINS_E_INVALID. */
+typedef struct lins_loop_report {
+  int32_t closest_history_frame_id;  /* closestHistoryFrameID: -1 = no candidate (nothing else ran or changed) */
+  int32_t latest_frame_id;           /* latestFrameIDLoopCloure (-1 without a candidate) */
+  int32_t n_source;                  /* latestSurfKeyFrameCloud after the (int)intensity >= 0 filter (a NaN intensity or
+                                        one outside (-1, 2^31) is dropped, as x86's truncation gives INT_MIN) */
+  int32_t n_history_ds;              /* nearHistorySurfKeyFrameCloudDS: key frames closest +- 25 clipped to [0, latest],
+                                        corner + surf in the map frame, VoxelGrid 0.4 m */
+  int32_t icp_iters;                 /* ICP iterations run (<= 100) */
+  int32_t n_corr0;                   /* correspondences of the first iteration (squared distance <= 100^2) */
+  int32_t converged;                 /* icp.hasConverged() */
+  int32_t accepted;                  /* converged && getFitnessScore() <= historyKeyframeFitnessScore (0.3f): a loop factor
+                                        was added and aLoopIsClosed set */
+  double fitness;                    /* getFitnessScore(): mean squared 1-NN distance of the source under the final
+                                        transform (DBL_MAX without a neighbour) */
+  float final_transform[16];         /* getFinalTransformation(), row-major 4 x 4 */
+  double factor[6];                  /* accepted: poseFrom.between(poseTo) as x, y, z, roll, pitch, yaw (Rot3::xyz) */
+  double noise;                      /* accepted: the factor's variance on each of its six components (the f32 score) */
+} lins_loop_report;
+/* enables loop closure on the masked slots, each of which must be fresh (not present in a step since open or its last
+   reset; on a run bound by lins_gpu_seq_map_open, no sequence step since open or the slot's last lins_gpu_seq_restart,
+   as lins_gpu_seq_configure judges it; all or nothing: LINS_E_INVALID and nothing changes otherwise).  Enabling an
+   enabled slot is a no-op.  correctPoses clears the window when it runs, as the reference does: a download before the
+   next processed cycle returns none. */
+int lins_gpu_mappers_loops(lins_ctx* ctx, const uint8_t* mask /*M*/);
+/* one performLoopClosure for every masked slot, all in one device pass with one synchronisation: per slot its
+   candidate (the one lins_mapper_report.loop_candidate reports, around currentRobotPosPoint of its last processed cycle
+   and timeLaserOdometry of its last odometry message), the history sub-map's VoxelGrid, PCL's ICP (100 iterations at
+   most, correspondence distance 100, transformation and fitness epsilon 1e-6) and on acceptance the loop factor.
+   reps[s] is written for masked slots (reps may be NULL).  LINS_E_INVALID before anything changes for a masked slot that
+   is not enabled; LINS_E_TOOBIG when a history VoxelGrid overflows (nothing changes). */
+int lins_gpu_mappers_close_loops(lins_ctx* ctx, const uint8_t* mask /*M*/, lins_loop_report* reps /*M or NULL*/);
+/* the same on the single mapper (a run of one slot of the lockstep code) */
+int lins_gpu_mapper_loops(lins_ctx* ctx);
+int lins_gpu_mapper_close_loop(lins_ctx* ctx, lins_loop_report* rep);
 
 /* ---- sequence mode feeding its mapping nodes: LinsFusion::publishTopics (Estimator.cpp:177-202, :254-320) on the device ---
    A run opened by lins_gpu_seq_open can be bound to the context's lockstep mappers: slot s of the sequence run feeds

@@ -260,7 +260,7 @@ def read_checkpoint(directory):
 
 
 def replay(recordings, slots, model=None, device=0, gpu=None, map=False, checkpoint=None, checkpoint_every=None, stop_after=None,
-           resume=None):
+           resume=None, loops=False):
     """Run the recordings through `slots` slots of one context.  model: one LinsLidarModel for every recording (None =
     VLP-16) or a list with one per recording; a slot is projected with the model of the recording it holds.  Returns per
     recording a dict of per-scan arrays: stamps, status (StateEstimator::status_ after the scan), scan_status (LINS_SEQ_*),
@@ -276,11 +276,20 @@ def replay(recordings, slots, model=None, device=0, gpu=None, map=False, checkpo
     returns None (it returns the outputs as usual when it has fewer steps); with checkpoint_every=N it writes one after
     every N-th step and runs on.  resume: a checkpoint directory written for the same recordings, slot count and map:
     the replay continues from its step in a new context (gpu: one to open it on) and returns what a replay that never
-    stopped returns."""
+    stopped returns.
+    loops=True (with map=True) enables each recording's loop closure (lins_gpu_mappers_loops when a slot takes the
+    recording) and ticks its loop thread after a published scan whenever the recording's stamp has advanced >= 1.0 s
+    since its last tick (one lins_gpu_mappers_close_loops for all slots due): key_poses are then the corrected ones, and
+    loops_accepted counts the recording's closures.  A slot with loop closure cannot be saved, so loops=True takes no
+    checkpoint, stop_after or resume."""
     models, rec_model = model_table(recordings, model)
     lengths = [len(r) for r in recordings]
     if (stop_after is not None or checkpoint_every) and checkpoint is None:
         raise ValueError("stop_after / checkpoint_every need a checkpoint directory")
+    if loops and not map:
+        raise ValueError("loops=True needs map=True")
+    if loops and (checkpoint is not None or stop_after is not None or checkpoint_every or resume is not None):
+        raise ValueError("loops=True cannot checkpoint or resume: a slot with loop closure is not saved")
     start, blobs = 0, None
     if resume is not None:
         st, blobs = read_checkpoint(resume)
@@ -298,6 +307,9 @@ def replay(recordings, slots, model=None, device=0, gpu=None, map=False, checkpo
         for o in out:
             o.update(map_time=[], map_odom=[], map_processed=[], map_aft_mapped=[], map_keyframes=[], map_sizes=[], map_fused=[],
                      key_poses=np.zeros((0, 7)))
+            if loops:
+                o["loops_accepted"] = 0
+    last_tick = [None] * slots  # (loops) the stamp of each slot's last loop-thread tick
     if resume is not None:
         out, held = st["out"], st["held"]
         g.seq_load(np.array([b is not None for b in blobs], np.uint8), blobs)
@@ -318,6 +330,12 @@ def replay(recordings, slots, model=None, device=0, gpu=None, map=False, checkpo
                         finish(j)
             if restart.any():
                 g.seq_restart(restart)
+            if loops:  # a slot taking a recording (after open or its restart) is fresh
+                first = np.array([w is not None and w[1] == 0 for w in who], np.uint8)
+                if first.any():
+                    g.mappers_loops(first)
+                    for j in np.flatnonzero(first):
+                        last_tick[j] = None
             fresh = [w is not None and w[1] == 0 and getattr(recordings[w[0]], "config", None) is not None for w in who]
             if any(fresh):  # a slot taking a recording with a rig of its own (after open or its restart)
                 g.seq_configure(np.array(fresh, np.uint8), [recordings[w[0]].config if f else None for w, f in zip(who, fresh)])
@@ -371,6 +389,15 @@ def replay(recordings, slots, model=None, device=0, gpu=None, map=False, checkpo
                     o["map_aft_mapped"].append(list(r.transform_aft_mapped)); o["map_keyframes"].append(r.n_keyframes)
                     o["map_sizes"].append(sizes[j].copy())
                     o["map_fused"].append(fused[j].row())
+                if loops:  # the loop thread's 1 Hz tick, on each recording's own stamps
+                    due = np.zeros(slots, np.uint8)
+                    for j, w in enumerate(who):
+                        if w is not None and pub[j] and (last_tick[j] is None or time[j] - last_tick[j] >= 1.0):
+                            due[j], last_tick[j] = 1, time[j]
+                    if due.any():
+                        for j, lr in enumerate(g.mappers_close_loops(due)):
+                            if lr is not None and lr.accepted:
+                                out[who[j][0]]["loops_accepted"] += 1
             done = t + 1
             if stop_after is not None and done == stop_after:
                 write_checkpoint(g, checkpoint, done, who, lengths, map, held, out)

@@ -13,7 +13,7 @@ import subprocess
 
 import numpy as np
 
-from .ctypes_defs import (Batch, COV_SIZE, LinsBatchDesc, LinsCloud2Desc, LinsCloud2Layout, LinsFeatureParams, LinsLidarModel, LinsLidarModels, LinsFusedPose, LinsMapperDesc, LinsMapperReport, LinsMappersDesc, LinsMapReport, LinsParams, LinsPclDesc,
+from .ctypes_defs import (Batch, COV_SIZE, LinsBatchDesc, LinsCloud2Desc, LinsCloud2Layout, LinsFeatureParams, LinsLidarModel, LinsLidarModels, LinsFusedPose, LinsLoopReport, LinsMapperDesc, LinsMapperReport, LinsMappersDesc, LinsMapReport, LinsParams, LinsPclDesc,
                           LinsRawDesc, LinsReport, LinsScanResult, LinsSeqBeginDesc, LinsSeqInitParams, LinsSeqParams, LinsSeqPclDesc,
                           LinsSeqCloud2Desc, LinsSeqMapDesc, LinsSeqRawDesc, LinsSeqStepDesc, LinsSlotConfig, LinsSlotTuning, POINT_DTYPE, SCAN_RESULT_DTYPE, STATE_DIM, as_points, make_points, ptr)
 
@@ -40,19 +40,20 @@ EXPORTS = [
     "lins_gpu_mappers_open", "lins_gpu_mappers_reset", "lins_gpu_mappers_imu", "lins_gpu_mappers_step", "lins_gpu_mappers_download",
     "lins_gpu_seq_map_open", "lins_gpu_seq_map_step", "lins_gpu_seq_map_published", "lins_gpu_seq_configure", "lins_gpu_seq_tune",
     "lins_gpu_seq_save_size", "lins_gpu_seq_save", "lins_gpu_seq_load", "lins_gpu_mapper_fuse", "lins_gpu_mappers_fuse",
-    "lins_gpu_seq_map_fused",
+    "lins_gpu_seq_map_fused", "lins_gpu_mappers_loops", "lins_gpu_mappers_close_loops", "lins_gpu_mapper_loops",
+    "lins_gpu_mapper_close_loop",
 ]
 
 NVCC_ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]  # H100 (Hopper)
 NVCC_COMMON = NVCC_ARCH + ["-lineinfo", "-O3", "-std=c++17", "-Xcompiler", "-fPIC"]
 # translation units and their extra flags: lins_gpu.cu (the fused kernel and most of the C-ABI), lins_upload.cu (batch
 # upload), lins_map.cu (row F2's host side), lins_seq.cu (sequence mode), lins_features.cu (feature extraction),
-# lins_projection.cu (image projection), lins_cloud2.cu (PointCloud2 decoding), lins_mapper.cu (the mapping node's cycle), lins_mappers.cu (many mapping nodes in lockstep), lins_seq_save.cu (saving and loading slots) — all bit-exact, so no multiply-add contraction: the association and the map
+# lins_projection.cu (image projection), lins_cloud2.cu (PointCloud2 decoding), lins_mapper.cu (the mapping node's cycle), lins_mappers.cu (many mapping nodes in lockstep), lins_loops.cu (their loop closure), lins_seq_save.cu (saving and loading slots) — all bit-exact, so no multiply-add contraction: the association and the map
 # fits depend on it — and lins_jacobian.cu (the tolerance-checked split Jacobian kernel: contraction allowed)
 UNITS = [("lins_gpu.cu", ["-fmad=false"]), ("lins_upload.cu", ["-fmad=false"]), ("lins_map.cu", ["-fmad=false"]),
          ("lins_seq.cu", ["-fmad=false"]), ("lins_features.cu", ["-fmad=false"]), ("lins_projection.cu", ["-fmad=false"]),
          ("lins_cloud2.cu", ["-fmad=false"]), ("lins_mapper.cu", ["-fmad=false"]), ("lins_mappers.cu", ["-fmad=false"]),
-         ("lins_seq_save.cu", ["-fmad=false"]), ("lins_jacobian.cu", [])]
+         ("lins_loops.cu", ["-fmad=false"]), ("lins_seq_save.cu", ["-fmad=false"]), ("lins_jacobian.cu", [])]
 
 
 def build(force=False, verbose=False):
@@ -156,6 +157,10 @@ def lib():
         L.lins_gpu_seq_load.argtypes = [vp, vp, vp, vp]
         L.lins_gpu_mapper_fuse.argtypes = [vp, C.POINTER(LinsMapperDesc), C.POINTER(LinsFusedPose)]
         L.lins_gpu_mappers_fuse.argtypes = [vp, C.POINTER(LinsMappersDesc), vp]
+        L.lins_gpu_mappers_loops.argtypes = [vp, vp]
+        L.lins_gpu_mappers_close_loops.argtypes = [vp, vp, vp]
+        L.lins_gpu_mapper_loops.argtypes = [vp]
+        L.lins_gpu_mapper_close_loop.argtypes = [vp, C.POINTER(LinsLoopReport)]
         L.lins_gpu_seq_map_fused.argtypes = [vp, vp]
         _LIB = L
     return _LIB
@@ -447,6 +452,32 @@ class LinsGpu:
     def mappers_download(self, slot, rep):
         """mapper_download of one slot: (key poses, window, clouds) with the sizes its last processed cycle's report gives."""
         return self._download_node(lambda *out: self.L.lins_gpu_mappers_download(self.h, int(slot), *out), rep)
+
+    # ---- loop closure of the mapping nodes (lins_gpu_mapper(s)_loops / close_loop(s)) ----------------------------
+    def mapper_loops(self):
+        """Enable loop closure on the single mapper (fresh: before its first step)."""
+        self._ck(self.L.lins_gpu_mapper_loops(self.h))
+
+    def mapper_close_loop(self):
+        """One performLoopClosure of the single mapper: its LinsLoopReport."""
+        rep = LinsLoopReport()
+        self._ck(self.L.lins_gpu_mapper_close_loop(self.h, C.byref(rep)))
+        return rep
+
+    def mappers_loops(self, mask):
+        """Enable loop closure on the masked lockstep slots (each fresh)."""
+        m = np.ascontiguousarray(mask, np.uint8).reshape(-1)
+        assert len(m) == self._mappers_n
+        self._ck(self.L.lins_gpu_mappers_loops(self.h, ptr(m)))
+
+    def mappers_close_loops(self, mask):
+        """performLoopClosure of every masked (enabled) slot in one device pass: a LinsLoopReport per masked slot, None
+        elsewhere."""
+        m = np.ascontiguousarray(mask, np.uint8).reshape(-1)
+        assert len(m) == self._mappers_n
+        reps = (LinsLoopReport * len(m))()
+        self._ck(self.L.lins_gpu_mappers_close_loops(self.h, ptr(m), C.cast(reps, C.c_void_p)))
+        return [reps[s] if m[s] else None for s in range(len(m))]
 
     # ---- sequence mode feeding its mapping nodes (lins_gpu_seq_map_*) ---------------------------------------------
     def seq_map_open(self):

@@ -23,6 +23,7 @@
 
 #include "../../../include/lins_gpu.h"
 #include "../host/host_pool.hpp"
+#include "../host/pose_graph.hpp"
 #include "lins_slot_blob.hpp"
 
 namespace lins_dev { struct IcpState; struct BatchView; struct UnitTuning; }  // lins_kernels.cuh
@@ -329,8 +330,9 @@ struct VgInfo {
 };
 // PointTypePose (:57-65): the f32 pose fields and the f64 time
 struct MapperKeyPose { float x, y, z, roll, pitch, yaw; double time; };
-// one stored key frame: its corner, surf and outlier DS clouds in the map frame
-struct MapperKeyFrame { Buf<float4> c[3]; int n[3] = {0, 0, 0}; };
+// one stored key frame: its corner, surf and outlier DS clouds in the map frame, and on a slot with loop closure the
+// same clouds in the body frame (b), from which correctPoses re-transforms c
+struct MapperKeyFrame { Buf<float4> c[3], b[3]; int n[3] = {0, 0, 0}; };
 // the mapping node's scalar members the cycle reads and writes (lidar_mapping_node.cpp:198-214, :356-408): the slot
 // blob's record of them, and the window
 struct MapperScalars : lins_blob::MapperRec {
@@ -340,6 +342,18 @@ struct MapperScalars : lins_blob::MapperRec {
   MapperScalars() : MapperRec() { imuPointerLast = -1; timeLastProcessing = -1; }
 };
 struct MapperLast { bool valid = false; int n[6] = {0, 0, 0, 0, 0, 0}; };  // the last processed cycle's DS sizes
+// a node's loop closure (lins_loops.cu): the key-pose graph (prior, chain and loop factors), isamCurrentEstimate of the
+// last save, aLoopIsClosed, and what performLoopClosure reads of the node between cycles
+struct MapperLoops {
+  bool enabled = false;
+  bool closed = false;                  // aLoopIsClosed
+  bool rebuild = false;                 // correctPoses ran in this cycle: the stored clouds are re-transformed
+  int n_loop = 0;                       // loop factors in the graph
+  float cur[3] = {0, 0, 0};             // currentRobotPosPoint of the last processed cycle
+  double time = 0;                      // timeLaserOdometry of the last odometry message
+  std::vector<lins_pg::Factor> graph;
+  std::vector<lins_pg::Pose3> est;      // isamCurrentEstimate of the last save
+};
 // one mapping node's host state: its scalars, its key poses, the key-frame store (the window and the newest key frame,
 // each key frame's DS clouds in the map frame) and the sizes of its last processed cycle's clouds
 struct MapperNode {
@@ -349,6 +363,8 @@ struct MapperNode {
   std::unordered_map<int, int> slot_of;      // key-frame id -> slot
   std::vector<int> free_slots;
   MapperLast last;
+  bool stepped = false;                      // present in a step since open / reset (not fresh)
+  MapperLoops loops;
 };
 // the scratch of segmented VoxelGrids (lins_mapper.cu): 32-bit keys for one segment, (segment, key) 64-bit keys for more
 struct VgScratch {
@@ -383,6 +399,27 @@ struct ScanToMap {
   int blocks[2] = {0, 0};                    // fit blocks of the corner and the surf launch
 };
 
+// performLoopClosure of many slots in one device pass (lins_loops.cu).  Per slot with a candidate: its source (the
+// latest key frame's corner + surf cloud) at src0, the running source at src, its history cloud at tin and that
+// cloud's VoxelGrid at tgt (each at the slot's offsets), the 1-NN of every source point (corr, dist) and the ICP state.
+struct LoopSlot { const float4* src0; float4* src; const float4* tgt; const int* n_tgt; int* corr; float* dist; int n_src, pad; };
+struct LoopIcpState {
+  float fin[12];          // final_transformation_ rows 0..2 (row 3 is 0 0 0 1)
+  float inc[12];          // transformation_ of the last iteration
+  double prev_mse, fitness;
+  int iters, done, converged, n_corr0, n_src, n_fit, pad[2];
+};
+struct LoopPass {
+  Buf<float4> src0, src, tin, tgt;
+  Buf<int> corr; Buf<float> dist;
+  Buf<LoopSlot> slot; Buf<LoopSlot, kPinned> h_slot;
+  Buf<int2> blk; Buf<int2, kPinned> h_blk;     // per 1-NN block: (slot, first source point)
+  Buf<LoopIcpState> st; Buf<LoopIcpState, kPinned> h_st;
+  Buf<VgInfo> info; Buf<VgInfo, kPinned> h_info, h_init;
+  Buf<int> off; Buf<int, kPinned> h_off;
+  Buf<float4*> out; Buf<float4*, kPinned> h_out;
+};
+
 // A run of mapping nodes in lockstep (lins_mappers.cu): the lockstep mappers (lins_gpu_mappers_*), or the single
 // mapper (lins_gpu_mapper_*) as a run of one slot.  One MapperNode per slot with its six DS clouds of the last
 // processed cycle (map corner, map surf, corner, surf, outlier, surf total), and the step's shared device buffers
@@ -399,6 +436,7 @@ struct MappersState {
   Buf<float4*> vg_out; Buf<float4*, kPinned> h_vg_out;  // per round: S output clouds
   Buf<unsigned char> tf; Buf<unsigned char, kPinned> h_tf;  // the key frames' transform jobs
   CopyList copies;                           // the local maps' concatenation, then the surf-total one
+  LoopPass lp;                               // lins_gpu_mappers_close_loops
 };
 
 }  // namespace lins_capi
@@ -668,7 +706,11 @@ int voxel_grid_reserve(lins_ctx* ctx, VgScratch& w, int n, int n_seg);
 // keyframes_queue, which transforms every listed key frame's DS clouds into its store slot in one launch.
 // mapper_node_fuse: transform_fusion_node's pose for the odometry message (time, quat, pos) against the node as it
 // stands, i.e. with the pair the node published after its last processed cycle (DESIGN.md §4.13).
-struct KfSave { MapperKeyFrame* kf; MapperKeyPose kp; const float4* ds[3]; };
+// a key frame's clouds ds transformed by kp into kf->c; body: also copied as they are into kf->b
+struct KfSave { MapperKeyFrame* kf; MapperKeyPose kp; const float4* ds[3]; bool body; };
+int loop_candidate(const MapperNode& m, const float cur[3], double time);
+void mapper_loops_save(MapperNode& m, const MapperScalars& s, double R[3][3], double t[3]);
+void mapper_correct_poses(MapperNode& m);
 void mapper_node_reset(MapperNode& m);
 void mapper_node_imu(MapperScalars& s, const double* time, const double* roll, const double* pitch, int n);
 bool mapper_cycle_begin(const MapperNode& m, MapperScalars& s, double time, const double quat[4], const double pos[3], lins_mapper_report& r);
@@ -689,6 +731,7 @@ int mappers_open(lins_ctx* ctx, MappersState& ms, int n_slots);
 int mappers_reset(lins_ctx* ctx, MappersState& ms, const uint8_t* mask);
 int mappers_step(lins_ctx* ctx, MappersState& ms, const lins_mappers_desc* d, lins_mapper_report* reps, const MapPiece* dev,
                  const double* period);
+int mappers_close_loops(lins_ctx* ctx, MappersState& ms, const uint8_t* mask, lins_loop_report* reps);
 // lins_seq.cu: what the slot entries, a step, a restart and a load share.  check_open_run: the preamble of an entry
 // (named in its messages) that needs a lins_gpu_seq_open run: LINS_E_NOMAP without a run, LINS_E_INVALID when args_ok is
 // false (a null argument) or for a run of lins_gpu_seq_begin; check_fresh: LINS_E_INVALID unless slot s is fresh.

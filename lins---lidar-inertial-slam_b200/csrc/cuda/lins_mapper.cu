@@ -275,9 +275,12 @@ int keyframes_queue(lins_ctx* ctx, const KfSave* saves, int n, Buf<unsigned char
     TfConsts c;  // updateTransformPointCloudSinCos: libm's f32 sin / cos of the f32 fields
     c.cr = std::cos(k.roll); c.sr = std::sin(k.roll); c.cp = std::cos(k.pitch); c.sp = std::sin(k.pitch);
     c.cy = std::cos(k.yaw); c.sy = std::sin(k.yaw); c.tx = k.x; c.ty = k.y; c.tz = k.z;
+    const TfConsts id = {1.f, 0.f, 1.f, 0.f, 1.f, 0.f, 0.f, 0.f, 0.f};  // (the identity: each output is its input exactly)
     for (int a = 0; a < 3; ++a) {
       CK(sv.kf->c[a].grow((size_t)sv.kf->n[a] + 1));
+      if (sv.body) CK(sv.kf->b[a].grow((size_t)sv.kf->n[a] + 1));
       if (sv.kf->n[a]) jobs.push_back(TfJob{sv.ds[a], sv.kf->c[a].p, sv.kf->n[a], 0, c});
+      if (sv.kf->n[a] && sv.body) jobs.push_back(TfJob{sv.ds[a], sv.kf->b[a].p, sv.kf->n[a], 0, id});
     }
   }
   if (jobs.empty()) return LINS_OK;
@@ -296,33 +299,8 @@ int keyframes_queue(lins_ctx* ctx, const KfSave* saves, int n, Buf<unsigned char
 namespace {
 
 // ---- host scalar code, typed as the reference types it ---------------------------------------------------------------
-// gtsam Rot3::RzRyRx(x, y, z) (the matrix representation) and Rot3::xyz() through RQ; ypr = (z, y, x):
-// roll() = x, pitch() = y, yaw() = z
-void rot3_rzryrx(double x, double y, double z, double R[3][3]) {
-  const double cx = std::cos(x), sx = std::sin(x), cy = std::cos(y), sy = std::sin(y), cz = std::cos(z), sz = std::sin(z);
-  const double ss_ = sx * sy, cs_ = cx * sy, sc_ = sx * cy, cc_ = cx * cy, c_s = cx * sz, s_s = sx * sz, _cs = cy * sz, _cc = cy * cz,
-               s_c = sx * cz, c_c = cx * cz, ssc = ss_ * cz, csc = cs_ * cz, sss = ss_ * sz, css = cs_ * sz;
-  const double M[3][3] = {{_cc, -c_s + ssc, s_s + csc}, {_cs, c_c + sss, -s_c + css}, {-sy, sc_, cc_}};
-  std::memcpy(R, M, sizeof(M));
-}
-void mat_mul3(const double A[3][3], const double B[3][3], double C[3][3]) {
-  for (int i = 0; i < 3; ++i)
-    for (int j = 0; j < 3; ++j) C[i][j] = A[i][0] * B[0][j] + A[i][1] * B[1][j] + A[i][2] * B[2][j];
-}
-void rot3_xyz(const double A[3][3], double xyz[3]) {
-  const double x = -std::atan2(-A[2][1], A[2][2]);
-  const double cqx = std::cos(-x), sqx = std::sin(-x);
-  const double Qx[3][3] = {{1, 0, 0}, {0, cqx, -sqx}, {0, sqx, cqx}};
-  double B[3][3];
-  mat_mul3(A, Qx, B);
-  const double y = -std::atan2(B[2][0], B[2][2]);
-  const double cqy = std::cos(-y), sqy = std::sin(-y);
-  const double Qy[3][3] = {{cqy, 0, sqy}, {0, 1, 0}, {-sqy, 0, cqy}};
-  double Cm[3][3];
-  mat_mul3(B, Qy, Cm);
-  const double z = -std::atan2(-Cm[1][0], Cm[1][1]);
-  xyz[0] = x; xyz[1] = y; xyz[2] = z;
-}
+using lins_pg::rot3_rzryrx;
+using lins_pg::rot3_xyz;
 
 // transformUpdate (:538-577)
 void transform_update(MapperScalars& s, double timeLaserOdometry, double SCAN_PERIOD) {
@@ -377,6 +355,8 @@ int queue_copies(lins_ctx* ctx, CopyList& l, std::vector<DevCopy> v, int base) {
 
 void mapper_node_reset(MapperNode& m) {
   m.s = MapperScalars();
+  m.stepped = false;
+  m.loops = MapperLoops();
   m.poses.clear();
   for (auto& kv : m.slot_of) m.free_slots.push_back(kv.second);
   m.slot_of.clear();
@@ -463,13 +443,15 @@ void mapper_cycle_end(MapperNode& M, MapperScalars& s, double timeLaserOdometry,
   }
   if (save_kf || M.poses.empty()) {
     for (int k = 0; k < 3; ++k) s.previousRobotPos[k] = cur[k];
-    // the pose inserted into iSAM2, and (no loop factor: DESIGN.md §4.9) its estimate
+    // the pose inserted into iSAM2, and its estimate: without a loop factor the pose itself (DESIGN.md §4.9), else the
+    // solve of the slot's graph (§4.14)
     const float* P = M.poses.empty() ? s.transformTobeMapped : s.transformAftMapped;
-    if (M.poses.empty()) for (int i = 0; i < 6; ++i) s.transformLast[i] = s.transformTobeMapped[i];
     double R[3][3], xyz[3];
     rot3_rzryrx(P[2], P[0], P[1], R);
+    double t[3] = {P[5], P[3], P[4]};  // Point3(x = T[5], y = T[3], z = T[4])
+    if (M.loops.enabled) mapper_loops_save(M, s, R, t);
+    if (M.poses.empty()) for (int i = 0; i < 6; ++i) s.transformLast[i] = s.transformTobeMapped[i];
     rot3_xyz(R, xyz);  // roll() = xyz[0], pitch() = xyz[1], yaw() = xyz[2]
-    const double t[3] = {P[5], P[3], P[4]};  // Point3(x = T[5], y = T[3], z = T[4])
     MapperKeyPose kp;
     kp.x = (float)t[1]; kp.y = (float)t[2]; kp.z = (float)t[0];
     kp.roll = (float)xyz[1]; kp.pitch = (float)xyz[2]; kp.yaw = (float)xyz[0];
@@ -481,24 +463,17 @@ void mapper_cycle_end(MapperNode& M, MapperScalars& s, double timeLaserOdometry,
       s.transformAftMapped[3] = (float)t[1]; s.transformAftMapped[4] = (float)t[2]; s.transformAftMapped[5] = (float)t[0];
       for (int i = 0; i < 6; ++i) { s.transformLast[i] = s.transformAftMapped[i]; s.transformTobeMapped[i] = s.transformAftMapped[i]; }
     }
-    // the key frame's clouds, in the map frame once (its pose never changes without a loop closure)
+    // the key frame's clouds, in the map frame once (its pose changes only in correctPoses)
     MapperKeyFrame& kf = keyframe_slot(M, id);
     kf.n[0] = ndc; kf.n[1] = nds; kf.n[2] = ndo;
     save->kf = &kf;
     save->kp = kp;
     *saved = true;
     r.keyframe_saved = 1;
-    // detectLoopClosure's candidate (:1050-1064): radius 5 m around currentRobotPosPoint, nearest first, |dt| > 30 s
-    float best = 0.f;
-    for (int i = 0; i < (int)M.poses.size(); ++i) {
-      const MapperKeyPose& q = M.poses[i];
-      const float ex = q.x - cur[0], ey = q.y - cur[1], ez = q.z - cur[2];
-      const float d2 = ex * ex + ey * ey + ez * ez;
-      if (!(d2 < 25.0f) || !(std::fabs(q.time - timeLaserOdometry) > 30.0)) continue;
-      if (r.loop_candidate < 0 || d2 < best) { r.loop_candidate = i; best = d2; }
-    }
-    // the store keeps the window and the newest key frame: nothing else can enter a later window
-    for (auto it = M.slot_of.begin(); it != M.slot_of.end();) {
+    r.loop_candidate = loop_candidate(M, cur, timeLaserOdometry);
+    // the store keeps the window and the newest key frame: nothing else can enter a later window (a slot with loop
+    // closure keeps every key frame, for the history sub-maps and correctPoses)
+    for (auto it = M.slot_of.begin(); it != M.slot_of.end() && !M.loops.enabled;) {
       const int kid = it->first;
       if (kid != id && std::find(s.window.begin(), s.window.end(), kid) == s.window.end()) { M.free_slots.push_back(it->second); it = M.slot_of.erase(it); }
       else ++it;
@@ -513,6 +488,25 @@ void mapper_cycle_end(MapperNode& M, MapperScalars& s, double timeLaserOdometry,
   r.n_keyframes = (int)M.poses.size();
   r.window_len = (int)s.window.size();
   for (int i = 0; i < 6; ++i) r.transform_aft_mapped[i] = s.transformAftMapped[i];
+  M.loops.rebuild = false;
+  if (M.loops.enabled) {
+    std::memcpy(M.loops.cur, cur, sizeof(cur));
+    if (M.loops.closed) mapper_correct_poses(M);  // correctPoses :1767-1795 (after the report: window_len is this cycle's)
+  }
+}
+
+// detectLoopClosure's candidate (:1050-1064): radius 5 m around currentRobotPosPoint, nearest first, |dt| > 30 s
+int loop_candidate(const MapperNode& M, const float cur[3], double time) {
+  int id = -1;
+  float best = 0.f;
+  for (int i = 0; i < (int)M.poses.size(); ++i) {
+    const MapperKeyPose& q = M.poses[i];
+    const float ex = q.x - cur[0], ey = q.y - cur[1], ez = q.z - cur[2];
+    const float d2 = ex * ex + ey * ey + ez * ez;
+    if (!(d2 < 25.0f) || !(std::fabs(q.time - time) > 30.0)) continue;
+    if (id < 0 || d2 < best) { id = i; best = d2; }
+  }
+  return id;
 }
 
 int mapper_node_download(lins_ctx* ctx, const MapperNode& M, const float4* const src[6], double* key_poses, int32_t* window, float* const dst[6]) {

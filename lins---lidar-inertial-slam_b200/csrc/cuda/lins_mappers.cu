@@ -98,12 +98,15 @@ int mappers_step(lins_ctx* ctx, MappersState& ms, const lins_mappers_desc* d, li
   std::vector<int> proc, skipped;  // processed slots; interval-skipped slots
   for (int s = 0; s < M; ++s) {
     if (d->present && !d->present[s]) continue;
+    ms.node[s].stepped = true;
     sc[s] = ms.node[s].s;
     (mapper_cycle_begin(ms.node[s], sc[s], d->time[s], d->quat + 4 * s, d->pos + 3 * s, rr[s]) ? proc : skipped).push_back(s);
   }
   const int P = (int)proc.size();
   auto finish = [&]() {
     for (int s : skipped) ms.node[s].s = sc[s];
+    for (int s = 0; s < M; ++s)  // timeLaserOdometry, which a skipped cycle's odometry replaces too
+      if ((!d->present || d->present[s]) && ms.node[s].loops.enabled) ms.node[s].loops.time = d->time[s];
     if (reps) for (int s = 0; s < M; ++s) if (!d->present || d->present[s]) reps[s] = rr[s];
     return LINS_OK;
   };
@@ -239,13 +242,22 @@ int mappers_step(lins_ctx* ctx, MappersState& ms, const lins_mappers_desc* d, li
     const int cnt[6] = {have_map ? hi[3 * P + 2 * p].count : 0, have_map ? hi[3 * P + 2 * p + 1].count : 0, hi[3 * p].count, hi[3 * p + 1].count,
                         hi[3 * p + 2].count, hi[5 * P + p].count};
     const bool gate = cnt[0] > 10 && cnt[1] > 100;
-    KfSave sv;
+    KfSave sv{};
     bool saved = false;
     mapper_cycle_end(ms.node[s], sc[s], d->time[s], period ? period[s] : ctx->prm.scan_period, cnt, gate ? &ms.stm.h_loop.p[s] : nullptr, rr[s], &sv, &saved);
+    MapperNode& m = ms.node[s];
     if (saved) {
       for (int k = 0; k < 3; ++k) sv.ds[k] = ms.ds[s][2 + k].p;
+      sv.body = m.loops.enabled;
+      sv.kp = m.poses.back();  // (correctPoses may have moved it)
       saves.push_back(sv);
     }
+    if (m.loops.rebuild)  // correctPoses: every other stored key frame re-transformed from its body-frame clouds
+      for (const auto& kv : m.slot_of) {
+        if (saved && kv.first == (int)m.poses.size() - 1) continue;
+        MapperKeyFrame& f = m.slots[kv.second];
+        saves.push_back(KfSave{&f, m.poses[kv.first], {f.b[0].p, f.b[1].p, f.b[2].p}, false});
+      }
   }
   if ((rc = keyframes_queue(ctx, saves.data(), (int)saves.size(), ms.tf, ms.h_tf)) != LINS_OK) return rc;
   return finish();
@@ -261,6 +273,17 @@ int mappers_download(lins_ctx* ctx, MappersState& ms, int slot, double* key_pose
   const float4* src[6];
   for (int k = 0; k < 6; ++k) src[k] = ms.ds[slot][k].p;
   return mapper_node_download(ctx, ms.node[slot], src, key_poses, window, dst);
+}
+
+// loop closure on the masked slots, all fresh (checked first: all or nothing).  On a run bound by lins_gpu_seq_map_open
+// a slot is fresh as lins_gpu_seq_configure / _tune judge it: no sequence step since open or its last restart.
+int mappers_loops(lins_ctx* ctx, MappersState& ms, const uint8_t* mask) {
+  const bool bound = &ms == &ctx->mappers && ctx->seq.pub.bound;
+  for (int s = 0; s < ms.n; ++s)
+    if (mask[s] && !ms.node[s].loops.enabled && (ms.node[s].stepped || (bound && !ctx->seq.slot[s].fresh)))
+      return fail(ctx, LINS_E_INVALID, "loop closure: a masked slot is not fresh (present in a step since open / reset)");
+  for (int s = 0; s < ms.n; ++s) if (mask[s]) ms.node[s].loops.enabled = true;
+  return LINS_OK;
 }
 
 // the single mapper: a run of one slot of its own, opened by the first lins_gpu_mapper_* call on the context
@@ -326,6 +349,36 @@ int lins_gpu_mappers_download(lins_ctx* ctx, int32_t slot, double* key_poses, in
   if (slot < 0 || slot >= ctx->mappers.n) return fail(ctx, LINS_E_INVALID, "slot out of range");
   float* const dst[6] = {map_corner_ds, map_surf_ds, corner_ds, surf_ds, outlier_ds, surf_total_ds};
   return mappers_download(ctx, ctx->mappers, slot, key_poses, window, dst);
+}
+
+int lins_gpu_mappers_loops(lins_ctx* ctx, const uint8_t* mask) {
+  if (!ctx) return LINS_E_INVALID;
+  if (need_open(ctx) != LINS_OK) return LINS_E_NOMAP;
+  if (!mask) return fail(ctx, LINS_E_INVALID, "null mask");
+  return mappers_loops(ctx, ctx->mappers, mask);
+}
+
+int lins_gpu_mappers_close_loops(lins_ctx* ctx, const uint8_t* mask, lins_loop_report* reps) {
+  if (!ctx) return LINS_E_INVALID;
+  if (need_open(ctx) != LINS_OK) return LINS_E_NOMAP;
+  if (!mask) return fail(ctx, LINS_E_INVALID, "null mask");
+  return mappers_close_loops(ctx, ctx->mappers, mask, reps);
+}
+
+int lins_gpu_mapper_loops(lins_ctx* ctx) {
+  if (!ctx) return LINS_E_INVALID;
+  const int rc = mapper_open(ctx);
+  if (rc != LINS_OK) return rc;
+  const uint8_t all = 1;
+  return mappers_loops(ctx, ctx->mapper, &all);
+}
+
+int lins_gpu_mapper_close_loop(lins_ctx* ctx, lins_loop_report* rep) {
+  if (!ctx) return LINS_E_INVALID;
+  const int rc = mapper_open(ctx);
+  if (rc != LINS_OK) return rc;
+  const uint8_t all = 1;
+  return mappers_close_loops(ctx, ctx->mapper, &all, rep);
 }
 
 int lins_gpu_mapper_reset(lins_ctx* ctx) {

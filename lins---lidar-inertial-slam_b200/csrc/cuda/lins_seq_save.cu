@@ -65,6 +65,9 @@ int check_run(lins_ctx* ctx, const uint8_t* mask, const char* entry) {
   if (rc != LINS_OK) return rc;
   if (!mask) return fail(ctx, LINS_E_INVALID, "null mask");
   if (ctx->seq.pub.bound && ctx->seq.pub.pending) return fail(ctx, LINS_E_INVALID, "the last step's lins_gpu_seq_map_step has not run");
+  if (ctx->seq.pub.bound)  // (a blob carries the window's map-frame clouds, not an enabled slot's whole body-frame store)
+    for (int s = 0; s < ctx->seq.n; ++s)
+      if (mask[s] && ctx->mappers.node[s].loops.enabled) return fail(ctx, LINS_E_INVALID, (std::string(entry) + ": a masked slot's mapper has loop closure enabled").c_str());
   return LINS_OK;
 }
 
@@ -279,6 +282,7 @@ int load_run(lins_ctx* ctx, const uint8_t* mask, const std::vector<B::View>& v) 
     m.poses.resize(sc.n_poses);
     for (int i = 0; i < sc.n_poses; ++i) { const B::PoseRec p = b.pose(i); std::memcpy(&m.poses[i], &p, sizeof(p)); }
     m.last = MapperLast();  // (no DS clouds until the slot's next processed cycle)
+    m.stepped = true;       // (a loaded node is not fresh: loop closure cannot be enabled on it)
   }
   CK(queue_map_state(ctx, q.map));
   // (upload_slot_consts ends with a synchronisation; the sources above are pageable)

@@ -89,6 +89,14 @@ class LinsMapperReport(C.Structure):
                 ("transform_aft_mapped", C.c_float * 6), ("map", LinsMapReport)]
 
 
+class LinsLoopReport(C.Structure):
+    """lins_loop_report (include/lins_gpu.h): one performLoopClosure of a mapper slot."""
+    _fields_ = [("closest_history_frame_id", C.c_int32), ("latest_frame_id", C.c_int32), ("n_source", C.c_int32),
+                ("n_history_ds", C.c_int32), ("icp_iters", C.c_int32), ("n_corr0", C.c_int32), ("converged", C.c_int32),
+                ("accepted", C.c_int32), ("fitness", C.c_double), ("final_transform", C.c_float * 16), ("factor", C.c_double * 6),
+                ("noise", C.c_double)]
+
+
 class LinsFusedPose(C.Structure):
     """lins_fused_pose (include/lins_gpu.h): transform_fusion_node's pose of one odometry message."""
     _fields_ = [("time", C.c_double), ("pos", C.c_double * 3), ("quat", C.c_double * 4), ("transform_mapped", C.c_float * 6),

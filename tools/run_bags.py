@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""tools/run_bags.py BAG... [--slots S] [--lidar /velodyne_points] [--imu /imu/data] [--max-scans N] [--lidar-model M] [--map]
+"""tools/run_bags.py BAG... [--slots S] [--lidar /velodyne_points] [--imu /imu/data] [--max-scans N] [--lidar-model M] [--map [--loops]]
                    [--config a.yaml[,b.yaml,...] [--tune]] [--checkpoint-every N DIR] [--resume DIR] [--out DIR]
 
 Replays many ROS1 bags through sequence mode in lockstep (bag_replay.py): every bag is scheduled as tools/run_bag.py
@@ -11,7 +11,9 @@ bag's model (lins_gpu_seq_step_cloud2_mixed).  Prints a summary line and the tra
 bag's mapping node runs on what its estimator publishes, in lockstep on the device (lins_gpu_seq_map_step), and
 DIR/<bag name>.odometry.txt, DIR/<bag name>.mapped.txt and DIR/<bag name>.integrated.txt (DIR: --out, default .)
 receive the three trajectories in tools/run_bag.py --map's line format; like run_bag.py --map, the bags' IMU orientation
-is not fed to the mappers.
+is not fed to the mappers.  --loops also closes each bag's loops (bag_replay.replay(loops=True): the loop thread ticked
+when the bag's stamp has advanced >= 1 s), and <bag name>.mapped.txt then holds the final, corrected key poses (stamp,
+x y z roll pitch yaw per key frame); it cannot be combined with --checkpoint-every or --resume.
 --config a.yaml[,b.yaml,...] takes LINS config files (exp_port.yaml, OpenCV YAML): one for every bag or one per bag.
 Each bag's slot is configured with its file's rig (scan period, feature thresholds, extrinsic, IMU noise, init stds and
 biases); the files must agree on the keys every slot shares (num_iter, icp_freq, nearest_feature_search_sq_dist,
@@ -75,17 +77,22 @@ def bag_tunings(spec, n_bags):
     return rc.lins_params(loaded[0][1]), [rc.slot_config(r) for r, _ in loaded], [rc.slot_tuning(t) for _, t in loaded]
 
 
-def write_map(o, out_dir, name):
+def write_map(o, out_dir, name, loops=False):
     """<name>.odometry.txt, <name>.mapped.txt and <name>.integrated.txt of one replayed bag, one line per published scan as
     tools/run_bag.py --map writes odometry.txt, mapped.txt and integrated.txt: stamp, then x y z qx qy qz qw of the
-    odometry, resp. the processed flag and transformAftMapped, resp. x y z qx qy qz qw of the fused pose."""
+    odometry, resp. the processed flag and transformAftMapped, resp. x y z qx qy qz qw of the fused pose.  loops: mapped.txt
+    holds the final (loop-corrected) key poses instead, one line per key frame: stamp, x y z roll pitch yaw."""
     os.makedirs(out_dir, exist_ok=True)
     files = [os.path.join(out_dir, name + ext) for ext in (".odometry.txt", ".mapped.txt", ".integrated.txt")]
     with open(files[0], "w") as fo, open(files[1], "w") as fm, open(files[2], "w") as fi:
         for t, od, pr, aft, fu in zip(o["map_time"], o["map_odom"], o["map_processed"], o["map_aft_mapped"], o["map_fused"]):
             fo.write("%.9f %s\n" % (t, " ".join("%.9g" % v for v in od)))
-            fm.write("%.9f %d %s\n" % (t, pr, " ".join("%.9g" % v for v in aft)))
+            if not loops:
+                fm.write("%.9f %d %s\n" % (t, pr, " ".join("%.9g" % v for v in aft)))
             fi.write("%.9f %s\n" % (t, " ".join("%.9g" % v for v in fu)))
+        if loops:
+            for k in o["key_poses"]:
+                fm.write("%.9f %s\n" % (k[6], " ".join("%.9g" % v for v in k[:6])))
     print("mapper:", len(o["map_time"]), "odometry outputs,", len(o["key_poses"]), "key frames;", "trajectories in",
           ", ".join(files[:2]), "and", files[2])
 
@@ -97,6 +104,7 @@ def main(argv=None):
     ap.add_argument("--max-scans", type=int, default=0)
     ap.add_argument("--lidar-model", default="0", help="0 | 1 for every bag, or one per bag: 0,1,...")
     ap.add_argument("--map", action="store_true", help="run each bag's mapping node on what its estimator publishes")
+    ap.add_argument("--loops", action="store_true", help="with --map: close loops (mapped.txt: the corrected key poses)")
     ap.add_argument("--config", help="LINS config file(s): one for every bag, or one per bag: a.yaml,b.yaml,...")
     ap.add_argument("--tune", action="store_true", help="with --config: each bag also takes its file's tuning and IMU misalignment")
     ap.add_argument("--checkpoint-every", nargs=2, metavar=("N", "DIR"), help="write a checkpoint into DIR after every N-th step")
@@ -109,6 +117,10 @@ def main(argv=None):
             if not a.checkpoint_every[0].isdigit() or int(a.checkpoint_every[0]) < 1:
                 raise ValueError(f"--checkpoint-every: {a.checkpoint_every[0]!r} is not a step count >= 1")
             every, ck_dir = int(a.checkpoint_every[0]), a.checkpoint_every[1]
+        if a.loops and not a.map:
+            raise ValueError("--loops needs --map")
+        if a.loops and (a.checkpoint_every or a.resume):
+            raise ValueError("--loops cannot be combined with --checkpoint-every / --resume: a slot with loop closure is not saved")
         model = lidar_models(a.lidar_model, len(a.bags))
         if a.tune and not a.config:
             raise ValueError("--tune takes the tuning from the --config files")
@@ -123,14 +135,14 @@ def main(argv=None):
     capi = importlib.import_module("lins---lidar-inertial-slam_b200.capi")
     recs = [br.Recording(p, a.lidar, a.imu, a.max_scans, config=c, tuning=t) for p, c, t in zip(a.bags, cfgs, tunes)]
     outs = br.replay(recs, a.slots or len(recs), model=model, map=a.map, gpu=capi.LinsGpu(prm) if prm is not None else None,
-                     checkpoint=ck_dir, checkpoint_every=every, resume=a.resume)
+                     checkpoint=ck_dir, checkpoint_every=every, resume=a.resume, loops=a.loops)
     np.set_printoptions(precision=4, suppress=True)
     for p, o in zip(a.bags, outs):
         print(p, br.summary(o))
         for k, (st, g) in enumerate(zip(o["status"], o["global_est"])):
             print(k, int(st), g)
         if a.map:
-            write_map(o, a.out or ".", os.path.splitext(os.path.basename(p))[0])
+            write_map(o, a.out or ".", os.path.splitext(os.path.basename(p))[0], a.loops)
         if a.out:
             os.makedirs(a.out, exist_ok=True)
             np.savez(os.path.join(a.out, os.path.splitext(os.path.basename(p))[0] + ".npz"),

@@ -803,6 +803,41 @@ int lins_gpu_mappers_close_loops(lins_ctx* ctx, const uint8_t* mask /*M*/, lins_
 int lins_gpu_mapper_loops(lins_ctx* ctx);
 int lins_gpu_mapper_close_loop(lins_ctx* ctx, lins_loop_report* rep);
 
+/* ---- the global map: visualizeGlobalMapThread / publishGlobalMap (:976-1031), the map on /laser_cloud_surround -------
+   For slots with loop closure enabled, whose store keeps every key frame's corner, surf and outlier DS clouds in the map
+   frame (re-transformed by correctPoses).  Per masked slot: the key poses within 500 m of currentRobotPosPoint of its
+   last processed cycle (f32 squared distance < 500^2, non-finite poses never), their pcl::VoxelGrid at 1 m with
+   intensity = key index (each voxel names key frame (int) of its f32 intensity centroid, in ascending voxel index: a
+   voxel may name a key frame it does not contain, and two voxels the same one), the named key frames' clouds
+   concatenated in that order (corner, surf, outlier each; repeats included) and their pcl::VoxelGrid at 0.4 m.  When that
+   VoxelGrid overflows (div_x * div_y * div_z > INT32_MAX, or a box bound of 2^62 or more) the map is the concatenation
+   itself, as PCL 1.7 publishes its input then (unfiltered = 1).  Clouds are in the /camera_init (YZX) frame.
+   The reference ticks this thread at 0.2 Hz of wall time; here the caller's call is the tick, run between mapping steps:
+   it sees the node as its last completed cycle left it (a call between a closure and the next processed cycle sees the
+   poses before correction).  The call changes no mapper state: later steps, reports, closures and downloads are those
+   of a run that never calls it. */
+#define LINS_GLOBAL_MAP_PASS_POINTS (1 << 24) /* gathered points per device pass (a slot above it runs alone) */
+typedef struct lins_global_map_report {
+  int32_t n_key_poses;     /* globalMapKeyPoses: key poses within 500 m of currentRobotPosPoint */
+  int32_t n_key_frames;    /* globalMapKeyPosesDS: key frames concatenated (repeats counted) */
+  int64_t n_points;        /* globalMapKeyFrames: points before down-sampling */
+  int32_t n_map;           /* globalMapKeyFramesDS: points of the published cloud */
+  int32_t unfiltered;      /* 1: the 0.4 m VoxelGrid overflowed and the map is the concatenation itself (n_map == n_points) */
+} lins_global_map_report;
+/* publishGlobalMap of every masked slot: the masked slots' gathered clouds run in device passes of up to
+   LINS_GLOBAL_MAP_PASS_POINTS points, one synchronisation per pass and one after the results' copies; each slot's result
+   is that of a call on it alone.  reps[s] is written for masked slots (reps may be NULL).  A slot's result stays on the
+   device until its next global-map call, its reset or lins_gpu_mappers_open.  LINS_E_INVALID before anything changes
+   for a NULL mask or a masked slot without loop closure; LINS_E_TOOBIG, with nothing changed, when a masked slot's
+   concatenation exceeds INT32_MAX points. */
+int lins_gpu_mappers_global_map(lins_ctx* ctx, const uint8_t* mask /*M*/, lins_global_map_report* reps /*M or NULL*/);
+/* the last global map of a slot: key_ids (n_key_frames: the DS key ids, in order) and cloud (n_map x 4: x, y, z,
+   intensity).  NULL skips.  LINS_E_NOMAP when the slot has none since open or its reset. */
+int lins_gpu_mappers_global_map_download(lins_ctx* ctx, int32_t slot, int32_t* key_ids, float* cloud /*n_map x 4*/);
+/* the same on the single mapper (a run of one slot of the lockstep code) */
+int lins_gpu_mapper_global_map(lins_ctx* ctx, lins_global_map_report* rep);
+int lins_gpu_mapper_global_map_download(lins_ctx* ctx, int32_t* key_ids, float* cloud);
+
 /* ---- sequence mode feeding its mapping nodes: LinsFusion::publishTopics (Estimator.cpp:177-202, :254-320) on the device ---
    A run opened by lins_gpu_seq_open can be bound to the context's lockstep mappers: slot s of the sequence run feeds
    mapper slot s.  After every sequence step (lins_gpu_seq_step, _ex, _pcl, _raw, _cloud2 and the _mixed forms) the run

@@ -260,7 +260,7 @@ def read_checkpoint(directory):
 
 
 def replay(recordings, slots, model=None, device=0, gpu=None, map=False, checkpoint=None, checkpoint_every=None, stop_after=None,
-           resume=None, loops=False):
+           resume=None, loops=False, global_map=False):
     """Run the recordings through `slots` slots of one context.  model: one LinsLidarModel for every recording (None =
     VLP-16) or a list with one per recording; a slot is projected with the model of the recording it holds.  Returns per
     recording a dict of per-scan arrays: stamps, status (StateEstimator::status_ after the scan), scan_status (LINS_SEQ_*),
@@ -281,13 +281,18 @@ def replay(recordings, slots, model=None, device=0, gpu=None, map=False, checkpo
     recording) and ticks its loop thread after a published scan whenever the recording's stamp has advanced >= 1.0 s
     since its last tick (one lins_gpu_mappers_close_loops for all slots due): key_poses are then the corrected ones, and
     loops_accepted counts the recording's closures.  A slot with loop closure cannot be saved, so loops=True takes no
-    checkpoint, stop_after or resume."""
+    checkpoint, stop_after or resume.
+    global_map=True (with loops=True) builds each recording's global map (lins_gpu_mappers_global_map) when it ends,
+    before its slot is handed on, in one call for every slot that finishes at the same step: global_map ((n, 4) float32
+    x y z intensity in /camera_init) and global_map_keys (the key frames it concatenates)."""
     models, rec_model = model_table(recordings, model)
     lengths = [len(r) for r in recordings]
     if (stop_after is not None or checkpoint_every) and checkpoint is None:
         raise ValueError("stop_after / checkpoint_every need a checkpoint directory")
     if loops and not map:
         raise ValueError("loops=True needs map=True")
+    if global_map and not loops:
+        raise ValueError("global_map=True needs loops=True: the global map reads the key frames loop closure keeps")
     if loops and (checkpoint is not None or stop_after is not None or checkpoint_every or resume is not None):
         raise ValueError("loops=True cannot checkpoint or resume: a slot with loop closure is not saved")
     start, blobs = 0, None
@@ -309,25 +314,34 @@ def replay(recordings, slots, model=None, device=0, gpu=None, map=False, checkpo
                      key_poses=np.zeros((0, 7)))
             if loops:
                 o["loops_accepted"] = 0
+            if global_map:
+                o.update(global_map=np.zeros((0, 4), np.float32), global_map_keys=np.zeros(0, np.int32))
     last_tick = [None] * slots  # (loops) the stamp of each slot's last loop-thread tick
     if resume is not None:
         out, held = st["out"], st["held"]
         g.seq_load(np.array([b is not None for b in blobs], np.uint8), blobs)
     blob = _PinnedBlob()
 
-    def finish(j):  # the key poses of the recording slot j held, before the slot is handed on
-        if held[j] is not None and held[j][1] is not None:
-            kp = np.zeros((held[j][1], 7))
-            g._ck(g.L.lins_gpu_mappers_download(g.h, j, _capi.ptr(kp), *[None] * 7))
-            out[held[j][0]]["key_poses"] = kp
-        held[j] = None
+    def finish(js):  # the key poses (and global maps) of the recordings the slots js held, before the slots are handed on
+        js = [j for j in js if held[j] is not None]
+        if global_map and js:
+            mask = np.zeros(slots, np.uint8)
+            mask[js] = 1
+            for j, rep in enumerate(g.mappers_global_map(mask)):
+                if rep is not None:
+                    o = out[held[j][0]]
+                    o["global_map_keys"], o["global_map"] = g.mappers_global_map_download(j, rep)
+        for j in js:
+            if held[j][1] is not None:
+                kp = np.zeros((held[j][1], 7))
+                g._ck(g.L.lins_gpu_mappers_download(g.h, j, _capi.ptr(kp), *[None] * 7))
+                out[held[j][0]]["key_poses"] = kp
+            held[j] = None
 
     try:
         for t, (restart, who) in enumerate(itertools.islice(slot_queue(lengths, slots), start, None), start):
             if map:
-                for j in range(slots):
-                    if held[j] is not None and (who[j] is None or who[j][0] != held[j][0]):
-                        finish(j)
+                finish([j for j in range(slots) if held[j] is not None and (who[j] is None or who[j][0] != held[j][0])])
             if restart.any():
                 g.seq_restart(restart)
             if loops:  # a slot taking a recording (after open or its restart) is fresh
@@ -405,8 +419,7 @@ def replay(recordings, slots, model=None, device=0, gpu=None, map=False, checkpo
             if checkpoint_every and done % checkpoint_every == 0:
                 write_checkpoint(g, checkpoint, done, who, lengths, map, held, out)
         if map:
-            for j in range(slots):
-                finish(j)
+            finish(range(slots))
             out = [_map_arrays(o) for o in out]
     finally:
         blob.release()

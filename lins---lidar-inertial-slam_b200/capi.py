@@ -13,7 +13,7 @@ import subprocess
 
 import numpy as np
 
-from .ctypes_defs import (Batch, COV_SIZE, LinsBatchDesc, LinsCloud2Desc, LinsCloud2Layout, LinsFeatureParams, LinsLidarModel, LinsLidarModels, LinsFusedPose, LinsLoopReport, LinsMapperDesc, LinsMapperReport, LinsMappersDesc, LinsMapReport, LinsParams, LinsPclDesc,
+from .ctypes_defs import (Batch, COV_SIZE, LinsBatchDesc, LinsCloud2Desc, LinsCloud2Layout, LinsFeatureParams, LinsLidarModel, LinsLidarModels, LinsFusedPose, LinsGlobalMapReport, LinsLoopReport, LinsMapperDesc, LinsMapperReport, LinsMappersDesc, LinsMapReport, LinsParams, LinsPclDesc,
                           LinsRawDesc, LinsReport, LinsScanResult, LinsSeqBeginDesc, LinsSeqInitParams, LinsSeqParams, LinsSeqPclDesc,
                           LinsSeqCloud2Desc, LinsSeqMapDesc, LinsSeqRawDesc, LinsSeqStepDesc, LinsSlotConfig, LinsSlotTuning, POINT_DTYPE, SCAN_RESULT_DTYPE, STATE_DIM, as_points, make_points, ptr)
 
@@ -41,7 +41,8 @@ EXPORTS = [
     "lins_gpu_seq_map_open", "lins_gpu_seq_map_step", "lins_gpu_seq_map_published", "lins_gpu_seq_configure", "lins_gpu_seq_tune",
     "lins_gpu_seq_save_size", "lins_gpu_seq_save", "lins_gpu_seq_load", "lins_gpu_mapper_fuse", "lins_gpu_mappers_fuse",
     "lins_gpu_seq_map_fused", "lins_gpu_mappers_loops", "lins_gpu_mappers_close_loops", "lins_gpu_mapper_loops",
-    "lins_gpu_mapper_close_loop",
+    "lins_gpu_mapper_close_loop", "lins_gpu_mappers_global_map", "lins_gpu_mappers_global_map_download",
+    "lins_gpu_mapper_global_map", "lins_gpu_mapper_global_map_download",
 ]
 
 NVCC_ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]  # H100 (Hopper)
@@ -162,6 +163,10 @@ def lib():
         L.lins_gpu_mapper_loops.argtypes = [vp]
         L.lins_gpu_mapper_close_loop.argtypes = [vp, C.POINTER(LinsLoopReport)]
         L.lins_gpu_seq_map_fused.argtypes = [vp, vp]
+        L.lins_gpu_mappers_global_map.argtypes = [vp, vp, vp]
+        L.lins_gpu_mappers_global_map_download.argtypes = [vp, C.c_int32, vp, vp]
+        L.lins_gpu_mapper_global_map.argtypes = [vp, C.POINTER(LinsGlobalMapReport)]
+        L.lins_gpu_mapper_global_map_download.argtypes = [vp, vp, vp]
         _LIB = L
     return _LIB
 
@@ -478,6 +483,34 @@ class LinsGpu:
         reps = (LinsLoopReport * len(m))()
         self._ck(self.L.lins_gpu_mappers_close_loops(self.h, ptr(m), C.cast(reps, C.c_void_p)))
         return [reps[s] if m[s] else None for s in range(len(m))]
+
+    # ---- the global map of the mapping nodes (lins_gpu_mapper(s)_global_map(_download)) ---------------------------
+    def mapper_global_map(self):
+        """publishGlobalMap of the single mapper (loop closure enabled): its LinsGlobalMapReport."""
+        rep = LinsGlobalMapReport()
+        self._ck(self.L.lins_gpu_mapper_global_map(self.h, C.byref(rep)))
+        return rep
+
+    def mapper_global_map_download(self, rep):
+        """(key ids (n_key_frames int32), cloud (n_map, 4) float32 x y z intensity) of the single mapper's last global map,
+        with the sizes its report `rep` gives."""
+        keys, cloud = np.zeros(rep.n_key_frames, np.int32), np.zeros((rep.n_map, 4), np.float32)
+        self._ck(self.L.lins_gpu_mapper_global_map_download(self.h, ptr(keys), ptr(cloud)))
+        return keys, cloud
+
+    def mappers_global_map(self, mask):
+        """publishGlobalMap of every masked (enabled) lockstep slot: a LinsGlobalMapReport per masked slot, None elsewhere."""
+        m = np.ascontiguousarray(mask, np.uint8).reshape(-1)
+        assert len(m) == self._mappers_n
+        reps = (LinsGlobalMapReport * len(m))()
+        self._ck(self.L.lins_gpu_mappers_global_map(self.h, ptr(m), C.cast(reps, C.c_void_p)))
+        return [reps[s] if m[s] else None for s in range(len(m))]
+
+    def mappers_global_map_download(self, slot, rep):
+        """mapper_global_map_download of one lockstep slot."""
+        keys, cloud = np.zeros(rep.n_key_frames, np.int32), np.zeros((rep.n_map, 4), np.float32)
+        self._ck(self.L.lins_gpu_mappers_global_map_download(self.h, int(slot), ptr(keys), ptr(cloud)))
+        return keys, cloud
 
     # ---- sequence mode feeding its mapping nodes (lins_gpu_seq_map_*) ---------------------------------------------
     def seq_map_open(self):

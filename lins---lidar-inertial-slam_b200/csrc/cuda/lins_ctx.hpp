@@ -354,6 +354,14 @@ struct MapperLoops {
   std::vector<lins_pg::Factor> graph;
   std::vector<lins_pg::Pose3> est;      // isamCurrentEstimate of the last save
 };
+// a node's last global map (lins_gpu_mappers_global_map, lins_loops.cu): its report, the DS key ids and the published
+// cloud in a buffer of its own (valid = false: none since open / reset)
+struct MapperGlobalMap {
+  bool valid = false;
+  lins_global_map_report rep{};
+  std::vector<int32_t> keys;
+  Buf<float4> cloud;
+};
 // one mapping node's host state: its scalars, its key poses, the key-frame store (the window and the newest key frame,
 // each key frame's DS clouds in the map frame) and the sizes of its last processed cycle's clouds
 struct MapperNode {
@@ -365,6 +373,7 @@ struct MapperNode {
   MapperLast last;
   bool stepped = false;                      // present in a step since open / reset (not fresh)
   MapperLoops loops;
+  MapperGlobalMap gm;
 };
 // the scratch of segmented VoxelGrids (lins_mapper.cu): 32-bit keys for one segment, (segment, key) 64-bit keys for more
 struct VgScratch {
@@ -732,6 +741,8 @@ int mappers_reset(lins_ctx* ctx, MappersState& ms, const uint8_t* mask);
 int mappers_step(lins_ctx* ctx, MappersState& ms, const lins_mappers_desc* d, lins_mapper_report* reps, const MapPiece* dev,
                  const double* period);
 int mappers_close_loops(lins_ctx* ctx, MappersState& ms, const uint8_t* mask, lins_loop_report* reps);
+// lins_loops.cu: publishGlobalMap of the masked (enabled) slots into each slot's MapperGlobalMap (DESIGN.md §4.15)
+int mappers_global_map(lins_ctx* ctx, MappersState& ms, const uint8_t* mask, lins_global_map_report* reps);
 // lins_seq.cu: what the slot entries, a step, a restart and a load share.  check_open_run: the preamble of an entry
 // (named in its messages) that needs a lins_gpu_seq_open run: LINS_E_NOMAP without a run, LINS_E_INVALID when args_ok is
 // false (a null argument) or for a run of lins_gpu_seq_begin; check_fresh: LINS_E_INVALID unless slot s is fresh.

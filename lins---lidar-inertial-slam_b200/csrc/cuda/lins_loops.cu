@@ -14,15 +14,20 @@
 // DefaultConvergenceCriteria and sets the slot's done flag; then the fitness pass and one read-back.  A 1-NN block
 // covers source points of one slot only and every sum runs in a fixed order, so each slot's result is that of a run
 // of one slot.
+//
+// The global map (publishGlobalMap :976-1031, DESIGN.md §4.15) of the same enabled slots reuses the gather and
+// segmented VoxelGrid of the history sub-maps (gather_voxel_grid) on the key frames csrc/host/global_map.hpp selects.
 #include <cuda_runtime.h>
 
 #include <algorithm>
 #include <cfloat>
+#include <climits>
 #include <cmath>
 #include <cstdint>
 #include <cstring>
 #include <vector>
 
+#include "../host/global_map.hpp"
 #include "lins_ctx.hpp"
 
 using namespace lins_capi;
@@ -263,6 +268,49 @@ void key_pose_from(const lins_pg::Pose3& e, MapperKeyPose& k) {
 
 const lins_pg::Vec6 kOdomVar = {1e-6, 1e-6, 1e-6, 1e-8, 1e-8, 1e-6};  // priorNoise / odometryNoise (:382-385)
 
+// every buffer gather_voxel_grid uses for n points in n_seg segments and n_copies gather copies (grow-only)
+int gather_voxel_grid_reserve(lins_ctx* ctx, MappersState& ms, int n, int n_seg, size_t n_copies) {
+  LoopPass& lp = ms.lp;
+  int rc;
+  if ((rc = voxel_grid_reserve(ctx, ms.vg, n, n_seg)) != LINS_OK) return rc;
+  CK(lp.tin.grow((size_t)n + 1)); CK(lp.tgt.grow((size_t)n + 1));
+  CK(lp.info.reserve(n_seg)); CK(lp.h_info.reserve(n_seg)); CK(lp.h_init.reserve(n_seg));
+  CK(lp.off.reserve(n_seg + 1)); CK(lp.h_off.reserve(n_seg + 1)); CK(lp.out.reserve(n_seg)); CK(lp.h_out.reserve(n_seg));
+  return ms.copies.reserve(ctx, n_copies);
+}
+
+// The history sub-maps of close_loops and the global map: segment p of one segmented 0.4 m VoxelGrid is the
+// concatenation of the device clouds lists[p].  One gather launch (the caller's copies first) into ms.lp.tin at toff[p]
+// (lists.size() + 1 offsets, filled here), then the VoxelGrid into ms.lp.tgt at the same offsets, its records at
+// ms.lp.info for the caller to read back.  Every buffer is reserved before anything is queued.
+int gather_voxel_grid(lins_ctx* ctx, MappersState& ms, const std::vector<std::vector<MapPiece>>& lists, std::vector<DevCopy> copies,
+                      std::vector<int>& toff) {
+  LoopPass& lp = ms.lp;
+  const int A = (int)lists.size();
+  toff.assign(A + 1, 0);
+  for (int p = 0; p < A; ++p) {
+    int n = 0;
+    for (const MapPiece& c : lists[p]) n += c.len;
+    toff[p + 1] = toff[p] + n;
+  }
+  const int nt = toff[A];
+  size_t n_copies = copies.size();
+  for (const auto& l : lists) n_copies += l.size();
+  int rc;
+  if ((rc = gather_voxel_grid_reserve(ctx, ms, nt, A, n_copies)) != LINS_OK) return rc;
+  for (int p = 0; p < A; ++p) {
+    float4* o = lp.tin.p + toff[p];
+    for (const MapPiece& c : lists[p]) { copies.push_back(DevCopy{c.src, o, c.len, 0}); o += c.len; }
+  }
+  if ((rc = queue_copies(ctx, ms.copies, std::move(copies), 0)) != LINS_OK) return rc;
+  std::vector<float> leaf(A, 0.4f);
+  for (int p = 0; p < A; ++p) { lp.h_off.p[p] = toff[p]; lp.h_out.p[p] = lp.tgt.p + toff[p]; }
+  lp.h_off.p[A] = nt;
+  CK(cudaMemcpyAsync(lp.off.p, lp.h_off.p, sizeof(int) * (A + 1), cudaMemcpyHostToDevice, ctx->stream));
+  CK(cudaMemcpyAsync(lp.out.p, lp.h_out.p, sizeof(float4*) * A, cudaMemcpyHostToDevice, ctx->stream));
+  return voxel_grid_queue(ctx, ms.vg, lp.tin.p, A, toff.data(), lp.off.p, leaf.data(), lp.tgt.p, lp.out.p, lp.h_init.p, lp.info.p);
+}
+
 }  // namespace
 
 namespace lins_capi {
@@ -326,54 +374,41 @@ int mappers_close_loops(lins_ctx* ctx, MappersState& ms, const uint8_t* mask, li
   };
   if (A == 0) return finish();
 
-  // the sources (latest corner, surf) and history clouds (closest +- 25: corner, surf per key frame), gathered
+  // the sources (latest corner, surf) and history clouds (closest +- 25: corner, surf per key frame)
   LoopPass& lp = ms.lp;
-  std::vector<int> soff(A + 1, 0), toff(A + 1, 0);
-  std::vector<DevCopy> copies;
+  std::vector<int> soff(A + 1, 0);
+  std::vector<std::vector<MapPiece>> hist(A);
   auto kf = [&](const MapperNode& m, int id) -> const MapperKeyFrame& { return m.slots[m.slot_of.at(id)]; };
   for (int p = 0; p < A; ++p) {
     const MapperNode& m = ms.node[act[p]];
     const int latest = rr[act[p]].latest_frame_id, closest = rr[act[p]].closest_history_frame_id;
     soff[p + 1] = soff[p] + kf(m, latest).n[0] + kf(m, latest).n[1];
-    int nt = 0;
-    for (int j = std::max(0, closest - kHistory); j <= std::min(latest, closest + kHistory); ++j) nt += kf(m, j).n[0] + kf(m, j).n[1];
-    toff[p + 1] = toff[p] + nt;
+    for (int j = std::max(0, closest - kHistory); j <= std::min(latest, closest + kHistory); ++j)
+      for (int a = 0; a < 2; ++a) hist[p].push_back(MapPiece{kf(m, j).c[a].p, kf(m, j).n[a]});
   }
-  const int ns = soff[A], nt = toff[A];
+  const int ns = soff[A];
   std::vector<int2> blocks;
   for (int p = 0; p < A; ++p)
     for (int i = 0; i < soff[p + 1] - soff[p]; i += kNnThreads) blocks.push_back(make_int2(p, i));
   const int nb = (int)blocks.size();
-  // every buffer first (a growth frees memory queued work may still read)
+  // every buffer first (a growth frees memory queued work may still read; gather_voxel_grid reserves its own before it
+  // queues anything)
   int rc;
-  if ((rc = voxel_grid_reserve(ctx, ms.vg, nt, A)) != LINS_OK) return rc;
-  CK(lp.src0.grow((size_t)ns + 1)); CK(lp.src.grow((size_t)ns + 1)); CK(lp.tin.grow((size_t)nt + 1)); CK(lp.tgt.grow((size_t)nt + 1));
+  CK(lp.src0.grow((size_t)ns + 1)); CK(lp.src.grow((size_t)ns + 1));
   CK(lp.corr.grow((size_t)ns + 1)); CK(lp.dist.grow((size_t)ns + 1));
   CK(lp.slot.reserve(A)); CK(lp.h_slot.reserve(A)); CK(lp.st.reserve(A)); CK(lp.h_st.reserve(A));
   CK(lp.blk.reserve(std::max(nb, 1))); CK(lp.h_blk.reserve(std::max(nb, 1)));
-  CK(lp.info.reserve(A)); CK(lp.h_info.reserve(A)); CK(lp.h_init.reserve(A));
-  CK(lp.off.reserve(A + 1)); CK(lp.h_off.reserve(A + 1)); CK(lp.out.reserve(A)); CK(lp.h_out.reserve(A));
+  std::vector<DevCopy> copies;
   for (int p = 0; p < A; ++p) {
     const MapperNode& m = ms.node[act[p]];
-    const int latest = rr[act[p]].latest_frame_id, closest = rr[act[p]].closest_history_frame_id;
+    const int latest = rr[act[p]].latest_frame_id;
     float4* o = lp.src0.p + soff[p];
     for (int a = 0; a < 2; ++a) { copies.push_back(DevCopy{kf(m, latest).c[a].p, o, kf(m, latest).n[a], 0}); o += kf(m, latest).n[a]; }
-    o = lp.tin.p + toff[p];
-    for (int j = std::max(0, closest - kHistory); j <= std::min(latest, closest + kHistory); ++j)
-      for (int a = 0; a < 2; ++a) { copies.push_back(DevCopy{kf(m, j).c[a].p, o, kf(m, j).n[a], 0}); o += kf(m, j).n[a]; }
   }
-  copies.erase(std::remove_if(copies.begin(), copies.end(), [](const DevCopy& c) { return c.n <= 0; }), copies.end());
-  if ((rc = ms.copies.reserve(ctx, copies.size())) != LINS_OK) return rc;
-  if ((rc = queue_copies(ctx, ms.copies, copies, 0)) != LINS_OK) return rc;
+  // nearHistorySurfKeyFrameCloudDS: one segmented VoxelGrid, a segment per slot, gathered with the sources
+  std::vector<int> toff;
+  if ((rc = gather_voxel_grid(ctx, ms, hist, std::move(copies), toff)) != LINS_OK) return rc;
   if (ns) CK(cudaMemcpyAsync(lp.src.p, lp.src0.p, sizeof(float4) * ns, cudaMemcpyDeviceToDevice, ctx->stream));
-  // nearHistorySurfKeyFrameCloudDS: one segmented VoxelGrid, a segment per slot
-  std::vector<float> leaf(A, 0.4f);
-  for (int p = 0; p < A; ++p) { lp.h_off.p[p] = toff[p]; lp.h_out.p[p] = lp.tgt.p + toff[p]; }
-  lp.h_off.p[A] = nt;
-  CK(cudaMemcpyAsync(lp.off.p, lp.h_off.p, sizeof(int) * (A + 1), cudaMemcpyHostToDevice, ctx->stream));
-  CK(cudaMemcpyAsync(lp.out.p, lp.h_out.p, sizeof(float4*) * A, cudaMemcpyHostToDevice, ctx->stream));
-  if ((rc = voxel_grid_queue(ctx, ms.vg, lp.tin.p, A, toff.data(), lp.off.p, leaf.data(), lp.tgt.p, lp.out.p, lp.h_init.p, lp.info.p)) != LINS_OK)
-    return rc;
   // the ICP: the slot table, the block table and the initial states (identity, prev MSE DBL_MAX)
   for (int p = 0; p < A; ++p) {
     lp.h_slot.p[p] = LoopSlot{lp.src0.p + soff[p], lp.src.p + soff[p], lp.tgt.p + toff[p], &lp.info.p[p].count, lp.corr.p + soff[p], lp.dist.p + soff[p],
@@ -438,6 +473,94 @@ int mappers_close_loops(lins_ctx* ctx, MappersState& ms, const uint8_t* mask, li
     r.noise = noise;
   }
   return finish();
+}
+
+// publishGlobalMap (:976-1031) of the masked slots (DESIGN.md §4.15): the key-frame selection on the host
+// (csrc/host/global_map.hpp), then the named key frames' stored map-frame clouds (c = T(b, pose) after every save and
+// correctPoses, so the two-argument transformPointCloud is not run again) gathered and down-sampled in passes of up to
+// LINS_GLOBAL_MAP_PASS_POINTS points, a segment per slot, one synchronisation per pass.  Each result is copied into a
+// buffer of the slot's own; nothing else of the node changes.
+int mappers_global_map(lins_ctx* ctx, MappersState& ms, const uint8_t* mask, lins_global_map_report* reps) {
+  const int M = ms.n;
+  for (int s = 0; s < M; ++s)
+    if (mask[s] && !ms.node[s].loops.enabled)
+      return fail(ctx, LINS_E_INVALID, "lins_gpu_mappers_global_map: a masked slot does not have loop closure enabled");
+  CK(cudaSetDevice(ctx->device));
+  struct Job { int s; lins_global_map_report rep; std::vector<int32_t> keys; std::vector<MapPiece> clouds; };
+  std::vector<Job> jobs;
+  for (int s = 0; s < M; ++s) {
+    if (!mask[s]) continue;
+    const MapperNode& m = ms.node[s];
+    Job j{s, {}, {}, {}};
+    const std::vector<int32_t> sel = lins_gm::select_key_poses(m.poses, m.loops.cur);  // (none without key poses)
+    j.keys = lins_gm::key_poses_ds(m.poses, sel);
+    long long n = 0;
+    for (int32_t id : j.keys) {
+      const MapperKeyFrame& f = m.slots[m.slot_of.at(id)];
+      for (int a = 0; a < 3; ++a) { j.clouds.push_back(MapPiece{f.c[a].p, f.n[a]}); n += f.n[a]; }
+    }
+    if (n > INT_MAX) return fail(ctx, LINS_E_TOOBIG, "lins_gpu_mappers_global_map: a slot's key-frame clouds exceed INT32_MAX points");
+    j.rep.n_key_poses = (int32_t)sel.size();
+    j.rep.n_key_frames = (int32_t)j.keys.size();
+    j.rep.n_points = n;
+    jobs.push_back(std::move(j));
+  }
+  // the passes over the jobs with points, in slot order: a pass takes slots while its points stay within the budget
+  std::vector<std::pair<size_t, size_t>> passes;  // [first, last) job
+  long long in_pass = 0;
+  for (size_t k = 0; k < jobs.size(); ++k) {
+    const long long n = jobs[k].rep.n_points;
+    if (n == 0) continue;
+    if (passes.empty() || in_pass + n > LINS_GLOBAL_MAP_PASS_POINTS) {  // (a slot above the budget runs alone)
+      passes.push_back({k, k});
+      in_pass = 0;
+    }
+    passes.back().second = k + 1;
+    in_pass += n;
+  }
+  // every pass's buffers first: a pass's result copies read them while the next pass is queued
+  for (const auto& ps : passes) {
+    int n = 0, segs = 0;
+    size_t n_copies = 0;
+    for (size_t k = ps.first; k < ps.second; ++k)
+      if (jobs[k].rep.n_points) { n += (int)jobs[k].rep.n_points; segs += 1; n_copies += jobs[k].clouds.size(); }
+    const int rc = gather_voxel_grid_reserve(ctx, ms, n, segs, n_copies);
+    if (rc != LINS_OK) return rc;
+  }
+  std::vector<Buf<float4>> cloud(jobs.size());
+  LoopPass& lp = ms.lp;
+  for (const auto& ps : passes) {
+    std::vector<size_t> seg;
+    std::vector<std::vector<MapPiece>> lists;
+    for (size_t k = ps.first; k < ps.second; ++k)
+      if (jobs[k].rep.n_points) { seg.push_back(k); lists.push_back(jobs[k].clouds); }
+    std::vector<int> toff;
+    int rc;
+    if ((rc = gather_voxel_grid(ctx, ms, lists, {}, toff)) != LINS_OK) return rc;
+    CK(cudaMemcpyAsync(lp.h_info.p, lp.info.p, sizeof(VgInfo) * seg.size(), cudaMemcpyDeviceToHost, ctx->stream));
+    CK(cudaStreamSynchronize(ctx->stream));  // the pass's one read-back
+    for (size_t p = 0; p < seg.size(); ++p) {
+      lins_global_map_report& r = jobs[seg[p]].rep;
+      const VgInfo& v = lp.h_info.p[p];
+      // PCL 1.7's VoxelGrid publishes its input when the leaf is too small (output = *input_): the concatenation
+      r.unfiltered = v.toobig;
+      r.n_map = v.toobig ? (int32_t)r.n_points : v.count;
+      CK(cloud[seg[p]].reserve((size_t)r.n_map));
+      if (r.n_map)
+        CK(cudaMemcpyAsync(cloud[seg[p]].p, (v.toobig ? lp.tin.p : lp.tgt.p) + toff[p], sizeof(float4) * r.n_map, cudaMemcpyDeviceToDevice,
+                           ctx->stream));
+    }
+  }
+  if (!passes.empty()) CK(cudaStreamSynchronize(ctx->stream));  // the results' copies
+  for (size_t k = 0; k < jobs.size(); ++k) {
+    MapperGlobalMap& g = ms.node[jobs[k].s].gm;
+    g.valid = true;
+    g.rep = jobs[k].rep;
+    g.keys = std::move(jobs[k].keys);
+    g.cloud = std::move(cloud[k]);
+    if (reps) reps[jobs[k].s] = g.rep;
+  }
+  return LINS_OK;
 }
 
 }  // namespace lins_capi

@@ -357,6 +357,7 @@ void mapper_node_reset(MapperNode& m) {
   m.s = MapperScalars();
   m.stepped = false;
   m.loops = MapperLoops();
+  m.gm = MapperGlobalMap();  // (frees the last global map's cloud)
   m.poses.clear();
   for (auto& kv : m.slot_of) m.free_slots.push_back(kv.second);
   m.slot_of.clear();

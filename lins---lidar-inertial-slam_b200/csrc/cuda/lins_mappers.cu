@@ -286,6 +286,17 @@ int mappers_loops(lins_ctx* ctx, MappersState& ms, const uint8_t* mask) {
   return LINS_OK;
 }
 
+// a node's last global map: its key ids and cloud (NULL skips)
+int global_map_download(lins_ctx* ctx, const MapperNode& m, int32_t* key_ids, float* cloud) {
+  const MapperGlobalMap& g = m.gm;
+  if (!g.valid) return fail(ctx, LINS_E_NOMAP, "no global map since the slot's open / reset");
+  CK(cudaSetDevice(ctx->device));
+  if (key_ids) std::copy(g.keys.begin(), g.keys.end(), key_ids);
+  CK(d2h(ctx, cloud, g.cloud.p, sizeof(float4) * (size_t)g.rep.n_map));
+  CK(cudaStreamSynchronize(ctx->stream));
+  return LINS_OK;
+}
+
 // the single mapper: a run of one slot of its own, opened by the first lins_gpu_mapper_* call on the context
 int mapper_open(lins_ctx* ctx) {
   return ctx->mapper.n > 0 ? LINS_OK : mappers_open(ctx, ctx->mapper, 1);
@@ -363,6 +374,35 @@ int lins_gpu_mappers_close_loops(lins_ctx* ctx, const uint8_t* mask, lins_loop_r
   if (need_open(ctx) != LINS_OK) return LINS_E_NOMAP;
   if (!mask) return fail(ctx, LINS_E_INVALID, "null mask");
   return mappers_close_loops(ctx, ctx->mappers, mask, reps);
+}
+
+int lins_gpu_mappers_global_map(lins_ctx* ctx, const uint8_t* mask, lins_global_map_report* reps) {
+  if (!ctx) return LINS_E_INVALID;
+  if (need_open(ctx) != LINS_OK) return LINS_E_NOMAP;
+  if (!mask) return fail(ctx, LINS_E_INVALID, "null mask");
+  return mappers_global_map(ctx, ctx->mappers, mask, reps);
+}
+
+int lins_gpu_mappers_global_map_download(lins_ctx* ctx, int32_t slot, int32_t* key_ids, float* cloud) {
+  if (!ctx) return LINS_E_INVALID;
+  if (need_open(ctx) != LINS_OK) return LINS_E_NOMAP;
+  if (slot < 0 || slot >= ctx->mappers.n) return fail(ctx, LINS_E_INVALID, "slot out of range");
+  return global_map_download(ctx, ctx->mappers.node[slot], key_ids, cloud);
+}
+
+int lins_gpu_mapper_global_map(lins_ctx* ctx, lins_global_map_report* rep) {
+  if (!ctx) return LINS_E_INVALID;
+  const int rc = mapper_open(ctx);
+  if (rc != LINS_OK) return rc;
+  const uint8_t all = 1;
+  return mappers_global_map(ctx, ctx->mapper, &all, rep);
+}
+
+int lins_gpu_mapper_global_map_download(lins_ctx* ctx, int32_t* key_ids, float* cloud) {
+  if (!ctx) return LINS_E_INVALID;
+  const int rc = mapper_open(ctx);
+  if (rc != LINS_OK) return rc;
+  return global_map_download(ctx, ctx->mapper.node[0], key_ids, cloud);
 }
 
 int lins_gpu_mapper_loops(lins_ctx* ctx) {

@@ -97,6 +97,15 @@ class LinsLoopReport(C.Structure):
                 ("noise", C.c_double)]
 
 
+GLOBAL_MAP_PASS_POINTS = 1 << 24  # LINS_GLOBAL_MAP_PASS_POINTS: gathered points per device pass of the global map
+
+
+class LinsGlobalMapReport(C.Structure):
+    """lins_global_map_report (include/lins_gpu.h): one publishGlobalMap of a mapper slot."""
+    _fields_ = [("n_key_poses", C.c_int32), ("n_key_frames", C.c_int32), ("n_points", C.c_int64), ("n_map", C.c_int32),
+                ("unfiltered", C.c_int32)]
+
+
 class LinsFusedPose(C.Structure):
     """lins_fused_pose (include/lins_gpu.h): transform_fusion_node's pose of one odometry message."""
     _fields_ = [("time", C.c_double), ("pos", C.c_double * 3), ("quat", C.c_double * 4), ("transform_mapped", C.c_float * 6),

@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""tools/run_bag.py BAG [--lidar /velodyne_points] [--imu /imu/data] [--max-scans N] [--lidar-model 0|1] [--map [--loops] [--out DIR]]
+"""tools/run_bag.py BAG [--lidar /velodyne_points] [--imu /imu/data] [--max-scans N] [--lidar-model 0|1] [--map [--loops [--global-map]] [--out DIR]]
 
 BASELINE.json configs[1] runner (GPU box): replays a ROS1 bag through the restated front end (image projection, feature
 extraction, IMU propagation) and the GPU IESKF update, prints the trajectory.  With --map, every odometry output (what
@@ -9,7 +9,9 @@ one line per published scan: stamp, then x y z qx qy qz qw of the odometry, resp
 transformAftMapped (rx ry rz tx ty tz, the mapping node's YZX frame), resp. x y z qx qy qz qw of transform_fusion_node's
 pose (/integrated_to_init in /camera_init: the odometry corrected by the last processed cycle before the scan,
 lins_gpu_mapper_fuse).  --loops also closes loops (the loop thread ticked after a cycle whenever the stamp has advanced
->= 1 s since its last tick), and mapped.txt then holds the final, corrected key poses (stamp, x y z roll pitch yaw).  The replayed IMU messages are not fed to the mapper's roll / pitch queue (the
+>= 1 s since its last tick), and mapped.txt then holds the final, corrected key poses (stamp, x y z roll pitch yaw).
+--global-map (with --loops) also writes DIR/global_map.pcd after the last cycle: the mapping node's global map
+(publishGlobalMap, lins_gpu_mapper_global_map) as a binary PCD of x y z intensity in /camera_init.  The replayed IMU messages are not fed to the mapper's roll / pitch queue (the
 front end reads their rates and accelerations only), so transformUpdate runs without the IMU blend.  Uncompressed and lz4-compressed bags
 are read directly; for bz2 run `python tools/bag_tool.py decompress IN.bag OUT.bag` first."""
 import argparse, importlib, os, sys
@@ -20,10 +22,13 @@ ap.add_argument("bag"); ap.add_argument("--lidar", default="/velodyne_points"); 
 ap.add_argument("--max-scans", type=int, default=0); ap.add_argument("--lidar-model", type=int, default=0)
 ap.add_argument("--map", action="store_true", help="run the mapping node's cycle after every odometry output")
 ap.add_argument("--loops", action="store_true", help="with --map: close loops; mapped.txt then holds the corrected key poses")
+ap.add_argument("--global-map", action="store_true", help="with --loops: write DIR/global_map.pcd after the last cycle")
 ap.add_argument("--out", default=".", help="with --map: directory for odometry.txt, mapped.txt and integrated.txt")
 a = ap.parse_args()
 if a.loops and not a.map:
     ap.error("--loops needs --map")
+if a.global_map and not a.loops:
+    ap.error("--global-map needs --loops: the global map reads the key frames loop closure keeps")
 synth = importlib.import_module("lins---lidar-inertial-slam_b200.synth")
 out = synth.run_bag(a.bag, a.lidar, a.imu, a.max_scans, a.lidar_model)
 print("scans", len(out["status"]), "IESKF updates", len(out["iters"]), "mean iterations %.2f" % (out["iters"].mean() if len(out["iters"]) else 0), "diverged", int(((out["flags"] & 2) != 0).sum()))
@@ -56,5 +61,11 @@ if a.map:
         if a.loops and last_processed is not None:  # the final, loop-corrected key poses: stamp, x y z roll pitch yaw
             for k in g.mapper_download(last_processed)[0]:
                 fm.write("%.9f %s\n" % (k[6], " ".join("%.9g" % v for v in k[:6])))
+    if a.global_map:
+        pcd = importlib.import_module("lins---lidar-inertial-slam_b200.pcd")
+        grep = g.mapper_global_map()
+        path = os.path.join(a.out, "global_map.pcd")
+        pcd.write_pcd(path, g.mapper_global_map_download(grep)[1])
+        print("global map:", grep.n_map, "points from", grep.n_key_frames, "key frames" + (" (unfiltered)" if grep.unfiltered else "") + ";", path)
     print("mapper:", len(out["map_inputs"]), "odometry outputs,", last.n_keyframes if out["map_inputs"] else 0, "key frames;",
           "trajectories in", ", ".join(files[:2]), "and", files[2])

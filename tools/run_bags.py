@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""tools/run_bags.py BAG... [--slots S] [--lidar /velodyne_points] [--imu /imu/data] [--max-scans N] [--lidar-model M] [--map [--loops]]
+"""tools/run_bags.py BAG... [--slots S] [--lidar /velodyne_points] [--imu /imu/data] [--max-scans N] [--lidar-model M] [--map [--loops [--global-map]]]
                    [--config a.yaml[,b.yaml,...] [--tune]] [--checkpoint-every N DIR] [--resume DIR] [--out DIR]
 
 Replays many ROS1 bags through sequence mode in lockstep (bag_replay.py): every bag is scheduled as tools/run_bag.py
@@ -13,7 +13,9 @@ DIR/<bag name>.odometry.txt, DIR/<bag name>.mapped.txt and DIR/<bag name>.integr
 receive the three trajectories in tools/run_bag.py --map's line format; like run_bag.py --map, the bags' IMU orientation
 is not fed to the mappers.  --loops also closes each bag's loops (bag_replay.replay(loops=True): the loop thread ticked
 when the bag's stamp has advanced >= 1 s), and <bag name>.mapped.txt then holds the final, corrected key poses (stamp,
-x y z roll pitch yaw per key frame); it cannot be combined with --checkpoint-every or --resume.
+x y z roll pitch yaw per key frame); it cannot be combined with --checkpoint-every or --resume.  --global-map (with
+--loops) also writes each bag's global map when the bag ends (bag_replay.replay(global_map=True)) to
+DIR/<bag name>.global_map.pcd, a binary PCD of x y z intensity in /camera_init.
 --config a.yaml[,b.yaml,...] takes LINS config files (exp_port.yaml, OpenCV YAML): one for every bag or one per bag.
 Each bag's slot is configured with its file's rig (scan period, feature thresholds, extrinsic, IMU noise, init stds and
 biases); the files must agree on the keys every slot shares (num_iter, icp_freq, nearest_feature_search_sq_dist,
@@ -105,6 +107,7 @@ def main(argv=None):
     ap.add_argument("--lidar-model", default="0", help="0 | 1 for every bag, or one per bag: 0,1,...")
     ap.add_argument("--map", action="store_true", help="run each bag's mapping node on what its estimator publishes")
     ap.add_argument("--loops", action="store_true", help="with --map: close loops (mapped.txt: the corrected key poses)")
+    ap.add_argument("--global-map", action="store_true", help="with --loops: write DIR/<bag name>.global_map.pcd")
     ap.add_argument("--config", help="LINS config file(s): one for every bag, or one per bag: a.yaml,b.yaml,...")
     ap.add_argument("--tune", action="store_true", help="with --config: each bag also takes its file's tuning and IMU misalignment")
     ap.add_argument("--checkpoint-every", nargs=2, metavar=("N", "DIR"), help="write a checkpoint into DIR after every N-th step")
@@ -119,6 +122,8 @@ def main(argv=None):
             every, ck_dir = int(a.checkpoint_every[0]), a.checkpoint_every[1]
         if a.loops and not a.map:
             raise ValueError("--loops needs --map")
+        if a.global_map and not a.loops:
+            raise ValueError("--global-map needs --loops: the global map reads the key frames loop closure keeps")
         if a.loops and (a.checkpoint_every or a.resume):
             raise ValueError("--loops cannot be combined with --checkpoint-every / --resume: a slot with loop closure is not saved")
         model = lidar_models(a.lidar_model, len(a.bags))
@@ -135,7 +140,8 @@ def main(argv=None):
     capi = importlib.import_module("lins---lidar-inertial-slam_b200.capi")
     recs = [br.Recording(p, a.lidar, a.imu, a.max_scans, config=c, tuning=t) for p, c, t in zip(a.bags, cfgs, tunes)]
     outs = br.replay(recs, a.slots or len(recs), model=model, map=a.map, gpu=capi.LinsGpu(prm) if prm is not None else None,
-                     checkpoint=ck_dir, checkpoint_every=every, resume=a.resume, loops=a.loops)
+                     checkpoint=ck_dir, checkpoint_every=every, resume=a.resume, loops=a.loops,
+                     global_map=a.global_map)
     np.set_printoptions(precision=4, suppress=True)
     for p, o in zip(a.bags, outs):
         print(p, br.summary(o))
@@ -143,6 +149,11 @@ def main(argv=None):
             print(k, int(st), g)
         if a.map:
             write_map(o, a.out or ".", os.path.splitext(os.path.basename(p))[0], a.loops)
+        if a.global_map:
+            pcd = importlib.import_module("lins---lidar-inertial-slam_b200.pcd")
+            path = os.path.join(a.out or ".", os.path.splitext(os.path.basename(p))[0] + ".global_map.pcd")
+            pcd.write_pcd(path, o["global_map"])
+            print("global map:", len(o["global_map"]), "points from", len(o["global_map_keys"]), "key frames;", path)
         if a.out:
             os.makedirs(a.out, exist_ok=True)
             np.savez(os.path.join(a.out, os.path.splitext(os.path.basename(p))[0] + ".npz"),

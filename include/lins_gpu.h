@@ -838,6 +838,50 @@ int lins_gpu_mappers_global_map_download(lins_ctx* ctx, int32_t slot, int32_t* k
 int lins_gpu_mapper_global_map(lins_ctx* ctx, lins_global_map_report* rep);
 int lins_gpu_mapper_global_map_download(lins_ctx* ctx, int32_t* key_ids, float* cloud);
 
+/* ---- saving and loading mapping nodes: checkpoint, resume and move a drive's mapping node ---------------------------
+   A slot of the lockstep mappers (a run not bound by lins_gpu_seq_map_open) or the single mapper is saved as a
+   self-contained byte blob and loaded into a fresh slot of either, in this context or another, on the same GPU or another
+   with the same library build; one format serves both APIs.  The loaded slot then continues bit-identically to the slot
+   it was saved from: every later report, download, fused pose, close_loops report and global map is the source's.
+   A blob carries the node's scalars and IMU queue, its window (as the deque holds it), every key pose, the stored key
+   frames' DS clouds and the scan-to-map loop state.  A plain slot's store is the window and the newest key frame (at most
+   51) with their map-frame clouds.  A slot with loop closure keeps every key frame: its blob carries their body-frame
+   clouds only (16 bytes per DS point), and the load rebuilds the map-frame store from them with the key poses, which
+   gives the same bits the saved store holds; it also carries the key-pose graph (prior, chain and loop factors in order),
+   the estimate of the last save, aLoopIsClosed, the loop count, currentRobotPosPoint and the last odometry stamp.  The
+   loaded slot takes the blob's loop-closure state whatever the fresh slot had; it is not fresh, so loop closure cannot
+   be enabled on it.  A blob does not carry the last cycle's outputs: the download returns key poses and window but no DS
+   clouds until the slot's next processed cycle, and lins_gpu_mappers_global_map_download returns LINS_E_NOMAP until the
+   slot's next global-map call.
+   Every lockstep call takes a slot mask (M entries); slot s's blob is the byte range [off[s], off[s + 1]) of one
+   buffer.  A call stages the masked blobs' total bytes on the device and in pinned host memory: save and load with
+   smaller masks to bound it.  A run bound to sequence mode is refused (LINS_E_INVALID): lins_gpu_seq_save saves its slots
+   with their estimators.  A sequence-mode blob is not a mapper blob, and the other way round. */
+/* The offsets of each masked slot's blob in one buffer (off: M + 1; an unmasked slot's range is empty).  Host bookkeeping
+   only, no synchronisation.  LINS_E_INVALID for a NULL argument or a bound run; LINS_E_NOMAP without an open run. */
+int lins_gpu_mappers_save_size(lins_ctx* ctx, const uint8_t* mask /*M*/, uint64_t* off /*M+1*/);
+/* Writes every masked slot's blob at blob + off[s], off as lins_gpu_mappers_save_size returned it.  One gather launch, one
+   D2H and one synchronisation whatever the mask; the run is unchanged.  LINS_E_INVALID as lins_gpu_mappers_save_size and
+   for other offsets or a NULL blob; a CUDA error ends the run. */
+int lins_gpu_mappers_save(lins_ctx* ctx, const uint8_t* mask /*M*/, void* blob, const uint64_t* off /*M+1*/);
+/* Loads the blob at [off[s], off[s + 1]) of blob into every masked slot, each of which must be fresh (not present in a
+   step since lins_gpu_mappers_open or its last reset).  Every masked blob is validated in full first (format, record
+   sizes of the build, lengths, section bounds, counts, IMU queue pointers, the window's key frames, and on a slot with
+   loop closure the key frames, the factor list's order and keys, finite values and positive variances): all or nothing,
+   LINS_E_INVALID with nothing changed for any rejection, a NULL argument or a bound run.  Then one H2D, at most two
+   launches and one synchronisation.  A CUDA error after the validation ends the run.  LINS_E_NOMAP without an open run. */
+int lins_gpu_mappers_load(lins_ctx* ctx, const uint8_t* mask /*M*/, const void* blob, const uint64_t* off /*M+1*/);
+/* the same on the single mapper (a run of one slot of the lockstep code): its blob's length, the blob (bytes as
+   lins_gpu_mapper_save_size returned them) and a load into the single mapper, fresh since its first call or last reset */
+int lins_gpu_mapper_save_size(lins_ctx* ctx, uint64_t* bytes);
+int lins_gpu_mapper_save(lins_ctx* ctx, void* blob, uint64_t bytes);
+int lins_gpu_mapper_load(lins_ctx* ctx, const void* blob, uint64_t bytes);
+/* diagnostics: the host wall time in ms of the last completed lins_gpu_mappers_load / lins_gpu_mapper_load on the
+   context, by phase: validation, allocation (the key frames' store and the staging), staging (the blobs into pinned
+   memory), device (queueing the H2D and the launches, and the synchronisation that waits for them), bookkeeping.
+   LINS_E_NOMAP before the first. */
+int lins_gpu_mappers_load_phase_ms(lins_ctx* ctx, double* ms /*5*/);
+
 /* ---- sequence mode feeding its mapping nodes: LinsFusion::publishTopics (Estimator.cpp:177-202, :254-320) on the device ---
    A run opened by lins_gpu_seq_open can be bound to the context's lockstep mappers: slot s of the sequence run feeds
    mapper slot s.  After every sequence step (lins_gpu_seq_step, _ex, _pcl, _raw, _cloud2 and the _mixed forms) the run

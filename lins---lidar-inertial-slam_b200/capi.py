@@ -42,19 +42,21 @@ EXPORTS = [
     "lins_gpu_seq_save_size", "lins_gpu_seq_save", "lins_gpu_seq_load", "lins_gpu_mapper_fuse", "lins_gpu_mappers_fuse",
     "lins_gpu_seq_map_fused", "lins_gpu_mappers_loops", "lins_gpu_mappers_close_loops", "lins_gpu_mapper_loops",
     "lins_gpu_mapper_close_loop", "lins_gpu_mappers_global_map", "lins_gpu_mappers_global_map_download",
-    "lins_gpu_mapper_global_map", "lins_gpu_mapper_global_map_download",
+    "lins_gpu_mapper_global_map", "lins_gpu_mapper_global_map_download", "lins_gpu_mappers_save_size", "lins_gpu_mappers_save",
+    "lins_gpu_mappers_load", "lins_gpu_mapper_save_size", "lins_gpu_mapper_save", "lins_gpu_mapper_load", "lins_gpu_mappers_load_phase_ms",
 ]
 
 NVCC_ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]  # H100 (Hopper)
 NVCC_COMMON = NVCC_ARCH + ["-lineinfo", "-O3", "-std=c++17", "-Xcompiler", "-fPIC"]
 # translation units and their extra flags: lins_gpu.cu (the fused kernel and most of the C-ABI), lins_upload.cu (batch
 # upload), lins_map.cu (row F2's host side), lins_seq.cu (sequence mode), lins_features.cu (feature extraction),
-# lins_projection.cu (image projection), lins_cloud2.cu (PointCloud2 decoding), lins_mapper.cu (the mapping node's cycle), lins_mappers.cu (many mapping nodes in lockstep), lins_loops.cu (their loop closure), lins_seq_save.cu (saving and loading slots) — all bit-exact, so no multiply-add contraction: the association and the map
+# lins_projection.cu (image projection), lins_cloud2.cu (PointCloud2 decoding), lins_mapper.cu (the mapping node's cycle), lins_mappers.cu (many mapping nodes in lockstep), lins_loops.cu (their loop closure), lins_seq_save.cu (saving and loading slots), lins_mapper_save.cu (saving and loading mapping nodes) — all bit-exact, so no multiply-add contraction: the association and the map
 # fits depend on it — and lins_jacobian.cu (the tolerance-checked split Jacobian kernel: contraction allowed)
 UNITS = [("lins_gpu.cu", ["-fmad=false"]), ("lins_upload.cu", ["-fmad=false"]), ("lins_map.cu", ["-fmad=false"]),
          ("lins_seq.cu", ["-fmad=false"]), ("lins_features.cu", ["-fmad=false"]), ("lins_projection.cu", ["-fmad=false"]),
          ("lins_cloud2.cu", ["-fmad=false"]), ("lins_mapper.cu", ["-fmad=false"]), ("lins_mappers.cu", ["-fmad=false"]),
-         ("lins_loops.cu", ["-fmad=false"]), ("lins_seq_save.cu", ["-fmad=false"]), ("lins_jacobian.cu", [])]
+         ("lins_loops.cu", ["-fmad=false"]), ("lins_seq_save.cu", ["-fmad=false"]),
+         ("lins_mapper_save.cu", ["-fmad=false"]), ("lins_jacobian.cu", [])]
 
 
 def build(force=False, verbose=False):
@@ -167,6 +169,13 @@ def lib():
         L.lins_gpu_mappers_global_map_download.argtypes = [vp, C.c_int32, vp, vp]
         L.lins_gpu_mapper_global_map.argtypes = [vp, C.POINTER(LinsGlobalMapReport)]
         L.lins_gpu_mapper_global_map_download.argtypes = [vp, vp, vp]
+        L.lins_gpu_mappers_save_size.argtypes = [vp, vp, vp]
+        L.lins_gpu_mappers_save.argtypes = [vp, vp, vp, vp]
+        L.lins_gpu_mappers_load.argtypes = [vp, vp, vp, vp]
+        L.lins_gpu_mapper_save_size.argtypes = [vp, C.POINTER(C.c_uint64)]
+        L.lins_gpu_mapper_save.argtypes = [vp, vp, C.c_uint64]
+        L.lins_gpu_mapper_load.argtypes = [vp, vp, C.c_uint64]
+        L.lins_gpu_mappers_load_phase_ms.argtypes = [vp, vp]
         _LIB = L
     return _LIB
 
@@ -511,6 +520,56 @@ class LinsGpu:
         keys, cloud = np.zeros(rep.n_key_frames, np.int32), np.zeros((rep.n_map, 4), np.float32)
         self._ck(self.L.lins_gpu_mappers_global_map_download(self.h, int(slot), ptr(keys), ptr(cloud)))
         return keys, cloud
+
+    # ---- saving and loading mapping nodes (lins_gpu_mapper(s)_save / _load) ------------------------------------------
+    def mappers_save(self, mask):
+        """Save the lockstep slots with mask[s] != 0: a list of M entries, each slot's blob (bytes, self-contained: it loads
+        into a fresh lockstep slot or a fresh single mapper of any context of this library build) or None where the mask
+        is 0.  The run is unchanged."""
+        m = self._mapper_mask(mask)
+        off = np.zeros(len(m) + 1, np.uint64)
+        self._ck(self.L.lins_gpu_mappers_save_size(self.h, ptr(m), ptr(off)))
+        buf = np.zeros(max(int(off[-1]), 1), np.uint8)
+        self._ck(self.L.lins_gpu_mappers_save(self.h, ptr(m), ptr(buf), ptr(off)))
+        return [buf[int(off[s]): int(off[s + 1])].tobytes() if m[s] else None for s in range(len(m))]
+
+    def mappers_load(self, mask, blobs):
+        """Load blobs[s] (bytes, as mappers_save or mapper_save returned it) into every lockstep slot with mask[s] != 0,
+        each still fresh (no step since open / its last reset); blobs has M entries (None where the mask is 0).  All or
+        nothing."""
+        m = self._mapper_mask(mask)
+        if len(blobs) != len(m):
+            raise ValueError(f"{len(blobs)} blobs, the run has {len(m)} slots")
+        parts = [bytes(blobs[s]) if m[s] else b"" for s in range(len(m))]
+        off = np.zeros(len(m) + 1, np.uint64)
+        off[1:] = np.cumsum([len(p) for p in parts])
+        buf = np.frombuffer(b"".join(parts) or b"\0", np.uint8)
+        self._ck(self.L.lins_gpu_mappers_load(self.h, ptr(m), ptr(buf), ptr(off)))
+
+    def mapper_save(self):
+        """The single mapper's blob (bytes)."""
+        n = C.c_uint64(0)
+        self._ck(self.L.lins_gpu_mapper_save_size(self.h, C.byref(n)))
+        buf = np.zeros(max(n.value, 1), np.uint8)
+        self._ck(self.L.lins_gpu_mapper_save(self.h, ptr(buf), n.value))
+        return buf[:n.value].tobytes()
+
+    def mapper_load(self, blob):
+        """Load a blob (as mapper_save or mappers_save returned it) into the single mapper, still fresh."""
+        buf = np.frombuffer(bytes(blob) or b"\0", np.uint8)
+        self._ck(self.L.lins_gpu_mapper_load(self.h, ptr(buf), len(bytes(blob))))
+
+    def mappers_load_phase_ms(self):
+        """The last mapper load's host phases in ms: (validation, allocation, staging, device, bookkeeping)."""
+        out = np.zeros(5)
+        self._ck(self.L.lins_gpu_mappers_load_phase_ms(self.h, ptr(out)))
+        return out
+
+    def _mapper_mask(self, mask):
+        m = np.ascontiguousarray(mask, dtype=np.uint8).reshape(-1)
+        if len(m) != getattr(self, "_mappers_n", -1):
+            raise ValueError(f"mask has {len(m)} entries, the run {getattr(self, '_mappers_n', 0)}")
+        return m
 
     # ---- sequence mode feeding its mapping nodes (lins_gpu_seq_map_*) ---------------------------------------------
     def seq_map_open(self):

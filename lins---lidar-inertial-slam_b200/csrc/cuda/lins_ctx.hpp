@@ -446,6 +446,8 @@ struct MappersState {
   Buf<unsigned char> tf; Buf<unsigned char, kPinned> h_tf;  // the key frames' transform jobs
   CopyList copies;                           // the local maps' concatenation, then the surf-total one
   LoopPass lp;                               // lins_gpu_mappers_close_loops
+  Buf<float4> blob; Buf<float4, kPinned> h_blob;  // lins_gpu_mapper(s)_save / _load: the slot blobs on the device and
+                                                  // their pinned staging (lins_mapper_save.cu)
 };
 
 }  // namespace lins_capi
@@ -495,6 +497,8 @@ struct lins_ctx {
   lins_capi::MappersState mapper;   // lins_gpu_mapper_*: one slot, opened by the first call
   lins_capi::MappersState mappers;  // lins_gpu_mappers_*
   lins_capi::VoxelGridState vg;     // lins_gpu_voxel_grid
+  double mapper_load_ms[5] = {0, 0, 0, 0, 0};  // the last mapper load's host phases (lins_gpu_mappers_load_phase_ms)
+  bool mapper_load_valid = false;
 };
 
 namespace lins_capi {

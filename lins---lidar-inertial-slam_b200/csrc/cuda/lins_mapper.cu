@@ -30,6 +30,7 @@
 #include "../host/transform_fusion.hpp"
 #include "lins_ctx.hpp"
 #include "lins_features.cuh"
+#include "lins_mapper_tf.cuh"
 
 using namespace lins_capi;
 
@@ -186,21 +187,11 @@ __global__ void __launch_bounds__(kVgThreads) lins_vg_centroid_kernel(const Key*
 }
 
 // transformPointCloud (:624-652) with the constants of updateTransformPointCloudSinCos (:609-622), one block per job
-struct TfConsts { float cr, sr, cp, sp, cy, sy, tx, ty, tz; };
 struct TfJob { const float4* in; float4* out; int n, pad; TfConsts c; };
 __global__ void __launch_bounds__(256) lins_mapper_transform_kernel(const TfJob* __restrict__ jobs) {
   const TfJob& jb = jobs[blockIdx.x];
   const TfConsts c = jb.c;
-  for (int i = threadIdx.x; i < jb.n; i += blockDim.x) {
-    const float4 p = jb.in[i];
-    const float x1 = c.cy * p.x - c.sy * p.y;
-    const float y1 = c.sy * p.x + c.cy * p.y;
-    const float z1 = p.z;
-    const float x2 = x1;
-    const float y2 = c.cr * y1 - c.sr * z1;
-    const float z2 = c.sr * y1 + c.cr * z1;
-    jb.out[i] = make_float4(c.cp * x2 + c.sp * z2 + c.tx, y2 + c.ty, -c.sp * x2 + c.cp * z2 + c.tz, p.w);
-  }
+  for (int i = threadIdx.x; i < jb.n; i += blockDim.x) jb.out[i] = tf_point(c, jb.in[i]);
 }
 
 int ceil_log2(int n) { int b = 0; while ((1 << b) < n) ++b; return b; }
@@ -271,10 +262,7 @@ int keyframes_queue(lins_ctx* ctx, const KfSave* saves, int n, Buf<unsigned char
   std::vector<TfJob> jobs;
   for (int i = 0; i < n; ++i) {
     const KfSave& sv = saves[i];
-    const MapperKeyPose& k = sv.kp;
-    TfConsts c;  // updateTransformPointCloudSinCos: libm's f32 sin / cos of the f32 fields
-    c.cr = std::cos(k.roll); c.sr = std::sin(k.roll); c.cp = std::cos(k.pitch); c.sp = std::sin(k.pitch);
-    c.cy = std::cos(k.yaw); c.sy = std::sin(k.yaw); c.tx = k.x; c.ty = k.y; c.tz = k.z;
+    const TfConsts c = tf_consts(sv.kp);
     const TfConsts id = {1.f, 0.f, 1.f, 0.f, 1.f, 0.f, 0.f, 0.f, 0.f};  // (the identity: each output is its input exactly)
     for (int a = 0; a < 3; ++a) {
       CK(sv.kf->c[a].grow((size_t)sv.kf->n[a] + 1));

@@ -122,6 +122,26 @@ struct View {
   KeyframeRec keyframe(int i) const { KeyframeRec r; std::memcpy(&r, at(kKeyframes) + sizeof(KeyframeRec) * i, sizeof(r)); return r; }
 };
 
+// The mapping-node checks a sequence-mode blob and a mapper blob (lins_mapper_blob.hpp) share, once the key-frame table
+// ids[0..n_keyframes) is known to hold distinct ids of key poses: the IMU queue pointers are in range, every window id
+// names a stored key frame, and so do the newest key pose and every key frame the next window can take.
+template <typename Window>
+inline const char* mapper_state_check(const MapperRec& m, int32_t n_poses, int32_t n_window, Window window, const int32_t* ids, int32_t n_keyframes) {
+  if (m.imuPointerFront < 0 || m.imuPointerFront >= LINS_MAPPER_IMU_QUEUE || m.imuPointerLast < -1 || m.imuPointerLast >= LINS_MAPPER_IMU_QUEUE)
+    return "bad IMU queue pointer in slot blob";
+  auto stored = [&](int32_t id) {
+    for (int i = 0; i < n_keyframes; ++i) if (ids[i] == id) return true;
+    return false;
+  };
+  for (int i = 0; i < n_window; ++i) if (!stored(window(i))) return "slot blob window names no stored key frame";
+  // the key frames a later cycle's window can take: the newest, and while the window is short the last 50
+  if (n_poses > 0 && !stored(n_poses - 1)) return "slot blob lacks its newest key frame";
+  if (n_window < LINS_MAPPER_WINDOW)
+    for (int32_t id = n_poses > LINS_MAPPER_WINDOW ? n_poses - LINS_MAPPER_WINDOW : 0; id < n_poses; ++id)
+      if (!stored(id)) return "slot blob lacks a key frame of its next window";
+  return nullptr;
+}
+
 inline bool finite_all(const double* v, int n, bool nonneg) {
   for (int i = 0; i < n; ++i) if (!std::isfinite(v[i]) || (nonneg && v[i] < 0)) return false;
   return true;
@@ -197,20 +217,7 @@ inline const char* parse(const uint8_t* p, uint64_t len, const BuildSizes& sz, V
   if (want.total != len || std::memcmp(want.sec, h.sec, sizeof(h.sec)) != 0) return "slot blob section table differs from its counts";
   if (!bound) return nullptr;
   std::memcpy(&v.m, v.at(kMapper), sizeof(MapperRec));
-  const MapperRec& m = v.m;
-  if (m.imuPointerFront < 0 || m.imuPointerFront >= LINS_MAPPER_IMU_QUEUE || m.imuPointerLast < -1 || m.imuPointerLast >= LINS_MAPPER_IMU_QUEUE)
-    return "bad IMU queue pointer in slot blob";
-  auto stored = [&](int32_t id) {
-    for (int i = 0; i < s.n_keyframes; ++i) if (ids[i] == id) return true;
-    return false;
-  };
-  for (int i = 0; i < s.n_window; ++i) if (!stored(v.window(i))) return "slot blob window names no stored key frame";
-  // the key frames a later cycle's window can take: the newest, and while the window is short the last 50
-  if (s.n_poses > 0 && !stored(s.n_poses - 1)) return "slot blob lacks its newest key frame";
-  if (s.n_window < LINS_MAPPER_WINDOW)
-    for (int32_t id = s.n_poses > LINS_MAPPER_WINDOW ? s.n_poses - LINS_MAPPER_WINDOW : 0; id < s.n_poses; ++id)
-      if (!stored(id)) return "slot blob lacks a key frame of its next window";
-  return nullptr;
+  return mapper_state_check(v.m, s.n_poses, s.n_window, [&](int i) { return v.window(i); }, ids, s.n_keyframes);
 }
 
 }  // namespace lins_blob

@@ -680,7 +680,9 @@ int lins_gpu_mapper_imu(lins_ctx* ctx, const double* time, const double* roll, c
 /* ≙ laserOdometryHandler (:711-724) + the cloud handlers + one pass of run() (:1806-1855).  LINS_E_TOOBIG when a
    VoxelGrid's div_x * div_y * div_z exceeds INT32_MAX (the leaf is too small for the cloud's extent); the mapper's state
    (transforms, key frames, window, IMU queue) is then unchanged, and lins_gpu_mapper_download returns no clouds until
-   the next cycle completes.  rep may be NULL. */
+   the next cycle completes.  LINS_E_CUDA when a key frame saved by the cycle cannot be stored (pinned host memory for a
+   slot with loop closure, or device memory): the cycle is committed but its key frame is not, so the mapper is
+   discarded and the next lins_gpu_mapper_* call starts a fresh one.  rep may be NULL. */
 int lins_gpu_mapper_step(lins_ctx* ctx, const lins_mapper_desc* desc, lins_mapper_report* rep);
 /* the key poses (cloudKeyPoses6D: n_keyframes x 7 doubles x, y, z, roll, pitch, yaw, time; the first six are the f32
    PointTypePose fields), the window (window_len key-frame ids, oldest first, as used by the last processed cycle) and that
@@ -743,7 +745,9 @@ typedef struct lins_mappers_desc {
    LINS_E_INVALID before anything changes for a bad descriptor (n_slots != M, null time / quat / pos, bad offsets, a
    NULL cloud with points).  LINS_E_TOOBIG when any slot's VoxelGrid overflows: then no slot's state changes (transforms,
    key frames, windows, IMU queues), and lins_gpu_mappers_download returns no clouds for the slots the step processed
-   until their next completed cycle. */
+   until their next completed cycle.  LINS_E_CUDA when a key frame a slot saved cannot be stored (the pinned host store
+   of a slot with loop closure, or device memory): the slots' cycles are committed but not their key frames, so the run
+   ends (LINS_E_NOMAP until lins_gpu_mappers_open). */
 int lins_gpu_mappers_step(lins_ctx* ctx, const lins_mappers_desc* d, lins_mapper_report* reps /*M or NULL*/);
 /* lins_gpu_mapper_download of one slot */
 int lins_gpu_mappers_download(lins_ctx* ctx, int32_t slot, double* key_poses, int32_t* window, float* map_corner_ds,
@@ -754,20 +758,27 @@ int lins_gpu_mappers_download(lins_ctx* ctx, int32_t slot, double* key_poses, in
 int lins_gpu_mappers_fuse(lins_ctx* ctx, const lins_mappers_desc* d, lins_fused_pose* out /*M*/);
 
 /* ---- loop closure: loopClosureThread / performLoopClosure (:1033-1041, :1114-1186) and correctPoses (:1767-1795) ------
-   Opt-in per mapper slot.  An enabled slot keeps every key frame's corner, surf and outlier DS clouds twice, in the map
-   frame and in the body frame (no memory bound: 32 bytes per DS point of every key frame), and keeps the key-pose graph:
+   Opt-in per mapper slot.  An enabled slot keeps every key frame's corner, surf and outlier DS clouds in the body frame
+   in a host store (16 bytes per DS point, in the run's pinned, mapped host memory, taken in 1 MiB chunks of slabs that
+   grow with the run from 4 MiB to 64 MiB; a larger key frame gets a block of its own), while its device store is a plain slot's: the map-frame clouds of
+   the window and the newest key frame.  A key frame's map-frame cloud is the transform of its body cloud by its key
+   pose, computed where it is read (the history sub-map, the global map), with the bits the device store holds for the
+   key frames it keeps.  The slot keeps the key-pose graph:
    the prior on key 0 and the chain factors of saveKeyFramesAndFactor (:1673-1705, variances 1e-6 1e-6 1e-6 1e-8 1e-8
    1e-6, :382-385) and the loop factors close_loops adds.  Until its first loop factor every step of an enabled slot is
    bit-identical to a plain slot's.  From then on each key-frame save takes latestEstimate from a Gauss-Newton solve of
    the whole graph to convergence (f64, host; iSAM2's incremental relinearisation only approaches that fixed point, and
    how far it lags cannot be measured without gtsam: DESIGN.md §4.14), and the next processed cycle after a closure runs
    correctPoses: every key pose from the estimate of the last save (which predates the loop factor when that cycle saved
-   no key frame, as in the reference), the stored map-frame clouds re-transformed and the window rebuilt.
+   no key frame, as in the reference), the device store's map-frame clouds re-transformed from the host store and the
+   window rebuilt.
    The reference runs performLoopClosure at 1 Hz of wall time in its own thread; here the caller's call is the thread's
    tick, run between mapping steps (bag_replay.replay(loops=True) and tools/run_bag(s).py --loops call it whenever a
    slot's odometry stamp has advanced >= 1 s since its last call).
    lins_gpu_mapper_reset / lins_gpu_mappers_reset (and lins_gpu_seq_restart on a bound run) return a slot to not
-   enabled; lins_gpu_seq_save and lins_gpu_seq_load refuse an enabled slot with LINS_E_INVALID. */
+   enabled and hand its host store's chunks back to the run, which keeps its slabs for the slots' later key frames;
+   lins_gpu_mappers_open (and lins_gpu_seq_map_open) and lins_gpu_destroy free them.  lins_gpu_seq_save and
+   lins_gpu_seq_load refuse an enabled slot with LINS_E_INVALID. */
 typedef struct lins_loop_report {
   int32_t closest_history_frame_id;  /* closestHistoryFrameID: -1 = no candidate (nothing else ran or changed) */
   int32_t latest_frame_id;           /* latestFrameIDLoopCloure (-1 without a candidate) */
@@ -802,10 +813,19 @@ int lins_gpu_mappers_close_loops(lins_ctx* ctx, const uint8_t* mask /*M*/, lins_
 /* the same on the single mapper (a run of one slot of the lockstep code) */
 int lins_gpu_mapper_loops(lins_ctx* ctx);
 int lins_gpu_mapper_close_loop(lins_ctx* ctx, lins_loop_report* rep);
+/* The bytes of each masked slot's key-frame stores: device[s] = 16 x the points of its device store's map-frame clouds,
+   host[s] = 16 x the points of its host store's body clouds (0 on a slot without loop closure), and *host_reserved (NULL
+   skips) the pinned memory of the run's host store: its slabs and large blocks.  Host bookkeeping only, no
+   synchronisation.  LINS_E_INVALID for a NULL mask / device / host; LINS_E_NOMAP without an open run. */
+int lins_gpu_mappers_store_bytes(lins_ctx* ctx, const uint8_t* mask /*M*/, uint64_t* device /*M*/, uint64_t* host /*M*/,
+                                 uint64_t* host_reserved /*1 or NULL*/);
+/* the same on the single mapper (a run of one slot of the lockstep code) */
+int lins_gpu_mapper_store_bytes(lins_ctx* ctx, uint64_t* device, uint64_t* host, uint64_t* host_reserved /*NULL skips*/);
 
 /* ---- the global map: visualizeGlobalMapThread / publishGlobalMap (:976-1031), the map on /laser_cloud_surround -------
-   For slots with loop closure enabled, whose store keeps every key frame's corner, surf and outlier DS clouds in the map
-   frame (re-transformed by correctPoses).  Per masked slot: the key poses within 500 m of currentRobotPosPoint of its
+   For slots with loop closure enabled, whose host store keeps every key frame's corner, surf and outlier DS clouds in
+   the body frame; the gather reads them over the host link and transforms them by their key poses (as they stand after
+   the last correctPoses).  Per masked slot: the key poses within 500 m of currentRobotPosPoint of its
    last processed cycle (f32 squared distance < 500^2, non-finite poses never), their pcl::VoxelGrid at 1 m with
    intensity = key index (each voxel names key frame (int) of its f32 intensity centroid, in ascending voxel index: a
    voxel may name a key frame it does not contain, and two voxels the same one), the named key frames' clouds
@@ -845,17 +865,21 @@ int lins_gpu_mapper_global_map_download(lins_ctx* ctx, int32_t* key_ids, float* 
    it was saved from: every later report, download, fused pose, close_loops report and global map is the source's.
    A blob carries the node's scalars and IMU queue, its window (as the deque holds it), every key pose, the stored key
    frames' DS clouds and the scan-to-map loop state.  A plain slot's store is the window and the newest key frame (at most
-   51) with their map-frame clouds.  A slot with loop closure keeps every key frame: its blob carries their body-frame
-   clouds only (16 bytes per DS point), and the load rebuilds the map-frame store from them with the key poses, which
-   gives the same bits the saved store holds; it also carries the key-pose graph (prior, chain and loop factors in order),
+   51) with their map-frame clouds.  A slot with loop closure keeps every key frame in its host store: its blob carries
+   their body-frame clouds (16 bytes per DS point), copied from and into the host store on the host; the load rebuilds
+   the device store of the key frames a later window can take (the window, the newest key frame and, while the window is
+   short, the last 50) from them with the key poses, which gives the same bits the saved store holds (the source's
+   device store can hold a few more: key frames its window dropped since its last key-frame save, which nothing reads
+   again and its next save evicts); it also carries the key-pose graph (prior, chain and loop factors in order),
    the estimate of the last save, aLoopIsClosed, the loop count, currentRobotPosPoint and the last odometry stamp.  The
    loaded slot takes the blob's loop-closure state whatever the fresh slot had; it is not fresh, so loop closure cannot
    be enabled on it.  A blob does not carry the last cycle's outputs: the download returns key poses and window but no DS
    clouds until the slot's next processed cycle, and lins_gpu_mappers_global_map_download returns LINS_E_NOMAP until the
    slot's next global-map call.
    Every lockstep call takes a slot mask (M entries); slot s's blob is the byte range [off[s], off[s + 1]) of one
-   buffer.  A call stages the masked blobs' total bytes on the device and in pinned host memory: save and load with
-   smaller masks to bound it.  A run bound to sequence mode is refused (LINS_E_INVALID): lins_gpu_seq_save saves its slots
+   buffer.  A load stages the masked blobs' total bytes on the device and in pinned host memory, a save the bytes that come
+   from the device (a plain slot's key-frame clouds and every slot's loop state): save and load with smaller masks to
+   bound it.  A run bound to sequence mode is refused (LINS_E_INVALID): lins_gpu_seq_save saves its slots
    with their estimators.  A sequence-mode blob is not a mapper blob, and the other way round. */
 /* The offsets of each masked slot's blob in one buffer (off: M + 1; an unmasked slot's range is empty).  Host bookkeeping
    only, no synchronisation.  LINS_E_INVALID for a NULL argument or a bound run; LINS_E_NOMAP without an open run. */
@@ -877,8 +901,8 @@ int lins_gpu_mapper_save_size(lins_ctx* ctx, uint64_t* bytes);
 int lins_gpu_mapper_save(lins_ctx* ctx, void* blob, uint64_t bytes);
 int lins_gpu_mapper_load(lins_ctx* ctx, const void* blob, uint64_t bytes);
 /* diagnostics: the host wall time in ms of the last completed lins_gpu_mappers_load / lins_gpu_mapper_load on the
-   context, by phase: validation, allocation (the key frames' store and the staging), staging (the blobs into pinned
-   memory), device (queueing the H2D and the launches, and the synchronisation that waits for them), bookkeeping.
+   context, by phase: validation, allocation (the key frames' stores and the staging), staging (the blobs into pinned
+   memory and the loop slots' host stores), device (queueing the H2D and the launches, and the synchronisation that waits for them), bookkeeping.
    LINS_E_NOMAP before the first. */
 int lins_gpu_mappers_load_phase_ms(lins_ctx* ctx, double* ms /*5*/);
 

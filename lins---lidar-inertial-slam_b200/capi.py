@@ -44,6 +44,7 @@ EXPORTS = [
     "lins_gpu_mapper_close_loop", "lins_gpu_mappers_global_map", "lins_gpu_mappers_global_map_download",
     "lins_gpu_mapper_global_map", "lins_gpu_mapper_global_map_download", "lins_gpu_mappers_save_size", "lins_gpu_mappers_save",
     "lins_gpu_mappers_load", "lins_gpu_mapper_save_size", "lins_gpu_mapper_save", "lins_gpu_mapper_load", "lins_gpu_mappers_load_phase_ms",
+    "lins_gpu_mappers_store_bytes", "lins_gpu_mapper_store_bytes",
 ]
 
 NVCC_ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]  # H100 (Hopper)
@@ -176,6 +177,8 @@ def lib():
         L.lins_gpu_mapper_save.argtypes = [vp, vp, C.c_uint64]
         L.lins_gpu_mapper_load.argtypes = [vp, vp, C.c_uint64]
         L.lins_gpu_mappers_load_phase_ms.argtypes = [vp, vp]
+        L.lins_gpu_mappers_store_bytes.argtypes = [vp, vp, vp, vp, vp]
+        L.lins_gpu_mapper_store_bytes.argtypes = [vp, vp, vp, vp]
         _LIB = L
     return _LIB
 
@@ -492,6 +495,22 @@ class LinsGpu:
         reps = (LinsLoopReport * len(m))()
         self._ck(self.L.lins_gpu_mappers_close_loops(self.h, ptr(m), C.cast(reps, C.c_void_p)))
         return [reps[s] if m[s] else None for s in range(len(m))]
+
+    # ---- the key-frame stores' bytes (lins_gpu_mapper(s)_store_bytes) -------------------------------------------------
+    def mappers_store_bytes(self, mask=None):
+        """The masked lockstep slots' key-frame store bytes: (device (M,) uint64, host (M,) uint64, host_reserved int).
+        device: 16 x the points of a slot's device store; host: 16 x the points of its host store (0 on a plain slot);
+        host_reserved: the run's pinned slabs and large blocks.  Unmasked entries are 0.  Host bookkeeping only."""
+        m = self._mapper_mask(np.ones(getattr(self, "_mappers_n", 0), np.uint8) if mask is None else mask)
+        dev, host, res = np.zeros(len(m), np.uint64), np.zeros(len(m), np.uint64), np.zeros(1, np.uint64)
+        self._ck(self.L.lins_gpu_mappers_store_bytes(self.h, ptr(m), ptr(dev), ptr(host), ptr(res)))
+        return dev, host, int(res[0])
+
+    def mapper_store_bytes(self):
+        """The single mapper's key-frame store bytes: (device, host, host_reserved) as mappers_store_bytes gives them."""
+        out = np.zeros(3, np.uint64)
+        self._ck(self.L.lins_gpu_mapper_store_bytes(self.h, ptr(out[0:1]), ptr(out[1:2]), ptr(out[2:3])))
+        return int(out[0]), int(out[1]), int(out[2])
 
     # ---- the global map of the mapping nodes (lins_gpu_mapper(s)_global_map(_download)) ---------------------------
     def mapper_global_map(self):

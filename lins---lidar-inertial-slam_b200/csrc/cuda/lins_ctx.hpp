@@ -24,6 +24,7 @@
 #include "../../../include/lins_gpu.h"
 #include "../host/host_pool.hpp"
 #include "../host/pose_graph.hpp"
+#include "lins_kf_arena.hpp"
 #include "lins_slot_blob.hpp"
 
 namespace lins_dev { struct IcpState; struct BatchView; struct UnitTuning; }  // lins_kernels.cuh
@@ -330,9 +331,12 @@ struct VgInfo {
 };
 // PointTypePose (:57-65): the f32 pose fields and the f64 time
 struct MapperKeyPose { float x, y, z, roll, pitch, yaw; double time; };
-// one stored key frame: its corner, surf and outlier DS clouds in the map frame, and on a slot with loop closure the
-// same clouds in the body frame (b), from which correctPoses re-transforms c
-struct MapperKeyFrame { Buf<float4> c[3], b[3]; int n[3] = {0, 0, 0}; };
+// one key frame of the device store: its corner, surf and outlier DS clouds in the map frame
+struct MapperKeyFrame { Buf<float4> c[3]; int n[3] = {0, 0, 0}; };
+// one key frame of a loop-closure slot's host store: its corner, surf and outlier DS clouds in the body frame, back to
+// back at p in the run's pinned, mapped arena (the device reads and writes them through the same address; nullptr
+// without points).  Its map-frame clouds are T(b, key pose): tf_point(tf_consts(pose), b), computed on demand.
+struct HostKeyFrame { float4* p = nullptr; int n[3] = {0, 0, 0}; };
 // the mapping node's scalar members the cycle reads and writes (lidar_mapping_node.cpp:198-214, :356-408): the slot
 // blob's record of them, and the window
 struct MapperScalars : lins_blob::MapperRec {
@@ -362,14 +366,17 @@ struct MapperGlobalMap {
   std::vector<int32_t> keys;
   Buf<float4> cloud;
 };
-// one mapping node's host state: its scalars, its key poses, the key-frame store (the window and the newest key frame,
-// each key frame's DS clouds in the map frame) and the sizes of its last processed cycle's clouds
+// one mapping node's host state: its scalars, its key poses, the device key-frame store (the window and the newest key
+// frame, each key frame's DS clouds in the map frame), on a slot with loop closure the host store of every key frame,
+// and the sizes of its last processed cycle's clouds
 struct MapperNode {
   MapperScalars s;
   std::vector<MapperKeyPose> poses;          // cloudKeyPoses6D
-  std::vector<MapperKeyFrame> slots;         // the key-frame store
+  std::vector<MapperKeyFrame> slots;         // the device key-frame store
   std::unordered_map<int, int> slot_of;      // key-frame id -> slot
   std::vector<int> free_slots;
+  std::vector<HostKeyFrame> host;            // loop closure: the host store, by key-frame id (every key pose's)
+  lins_arena::Holding held;                  // what the host store holds of the run's arena
   MapperLast last;
   bool stepped = false;                      // present in a step since open / reset (not fresh)
   MapperLoops loops;
@@ -427,13 +434,20 @@ struct LoopPass {
   Buf<VgInfo> info; Buf<VgInfo, kPinned> h_info, h_init;
   Buf<int> off; Buf<int, kPinned> h_off;
   Buf<float4*> out; Buf<float4*, kPinned> h_out;
+  Buf<unsigned char> jobs; Buf<unsigned char, kPinned> h_jobs;  // the gather's jobs (lins_loops.cu: GatherJob)
 };
 
+// The arena of a run's host key-frame stores: 1 MiB chunks of pinned, mapped memory, in slabs of 4 chunks first, then
+// as many as the run holds, up to 64 (lins_mappers.cu: pinned_mapped_allocator)
+constexpr size_t kKfChunkBytes = size_t(1) << 20;
+constexpr int kKfFirstSlabChunks = 4, kKfMaxSlabChunks = 64;
+lins_arena::Allocator pinned_mapped_allocator();
 // A run of mapping nodes in lockstep (lins_mappers.cu): the lockstep mappers (lins_gpu_mappers_*), or the single
 // mapper (lins_gpu_mapper_*) as a run of one slot.  One MapperNode per slot with its six DS clouds of the last
 // processed cycle (map corner, map surf, corner, surf, outlier, surf total), and the step's shared device buffers
 struct MappersState {
   int n = 0;                                 // slots (0 = not opened)
+  lins_arena::Arena store{kKfChunkBytes, kKfFirstSlabChunks, kKfMaxSlabChunks, pinned_mapped_allocator()};  // the slots' host key-frame stores
   std::vector<MapperNode> node;
   std::vector<std::array<Buf<float4>, 6>> ds;
   ScanToMap stm;                             // a slot per mapping node
@@ -710,7 +724,8 @@ int voxel_grid_queue(lins_ctx* ctx, VgScratch& w, const float4* in, int n_seg, c
                      float4* out, float4* const* d_out, VgInfo* h_init, VgInfo* info);
 int voxel_grid_reserve(lins_ctx* ctx, VgScratch& w, int n, int n_seg);
 // lins_mapper.cu: the mapping node's host logic, which lins_mappers.cu runs for every slot.
-// mapper_node_reset: a freshly constructed node (the store's buffers are kept for reuse); mapper_node_imu: imuHandler.
+// mapper_node_reset: a freshly constructed node (the device store's buffers are kept for reuse, the host store's arena
+// holding goes back to the run's store); mapper_node_imu: imuHandler.
 // mapper_cycle_begin: laserOdometryHandler into s (a copy of m.s, committed by the caller) and, unless the 0.3 s gate
 // skips the cycle (false; r reports it), transformAssociateToMap and the window; window_sizes: the local map's corner and
 // surf + outlier point counts.  mapper_cycle_end, after the read-back of the DS counts cnt (map corner, map surf, corner,
@@ -719,12 +734,13 @@ int voxel_grid_reserve(lins_ctx* ctx, VgScratch& w, int n, int n_seg);
 // keyframes_queue, which transforms every listed key frame's DS clouds into its store slot in one launch.
 // mapper_node_fuse: transform_fusion_node's pose for the odometry message (time, quat, pos) against the node as it
 // stands, i.e. with the pair the node published after its last processed cycle (DESIGN.md §4.13).
-// a key frame's clouds ds transformed by kp into kf->c; body: also copied as they are into kf->b
-struct KfSave { MapperKeyFrame* kf; MapperKeyPose kp; const float4* ds[3]; bool body; };
+// a key frame's clouds ds transformed by kp into kf->c; body (a host-store block, or null): also written as they are
+// into body, back to back, through the mapped address
+struct KfSave { MapperKeyFrame* kf; MapperKeyPose kp; const float4* ds[3]; float4* body; };
 int loop_candidate(const MapperNode& m, const float cur[3], double time);
 void mapper_loops_save(MapperNode& m, const MapperScalars& s, double R[3][3], double t[3]);
 void mapper_correct_poses(MapperNode& m);
-void mapper_node_reset(MapperNode& m);
+void mapper_node_reset(MapperNode& m, lins_arena::Arena& store);
 void mapper_node_imu(MapperScalars& s, const double* time, const double* roll, const double* pitch, int n);
 bool mapper_cycle_begin(const MapperNode& m, MapperScalars& s, double time, const double quat[4], const double pos[3], lins_mapper_report& r);
 void mapper_window_sizes(const MapperNode& m, const MapperScalars& s, int& n_corner, int& n_surf);

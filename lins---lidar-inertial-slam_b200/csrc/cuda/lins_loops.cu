@@ -7,7 +7,8 @@
 // ICP's result (pcl's getTranslationAndEulerAngles / getTransformation in f32, gtsam's Pose3 in f64).
 //
 // Device, one pass over every slot with a candidate (one synchronisation): one gather of the sources (the latest key
-// frame's corner + surf cloud in the map frame) and the history clouds (key frames closest +- 25, corner + surf), one
+// frame's corner + surf cloud in the map frame, from the device store) and the history clouds (key frames closest +- 25,
+// corner + surf, read from the host store over the host link and transformed by their key poses on the way), one
 // segmented VoxelGrid (0.4 m, a segment per slot), then up to 100 queued ICP iterations, each one exhaustive 1-NN
 // launch over every active slot's source points and one launch of a CTA per slot that reduces the correspondences in a
 // fixed order, solves the rigid transform (Horn's quaternion form of the Umeyama / SVD optimum), applies PCL's
@@ -17,6 +18,8 @@
 //
 // The global map (publishGlobalMap :976-1031, DESIGN.md §4.15) of the same enabled slots reuses the gather and
 // segmented VoxelGrid of the history sub-maps (gather_voxel_grid) on the key frames csrc/host/global_map.hpp selects.
+// A key frame's map-frame cloud is T(b, key pose) of its host-store body cloud b: the bits the device store holds for
+// the key frames it keeps (every save and correctPoses writes them so, and a load rebuilds them so).
 #include <cuda_runtime.h>
 
 #include <algorithm>
@@ -29,6 +32,7 @@
 
 #include "../host/global_map.hpp"
 #include "lins_ctx.hpp"
+#include "lins_mapper_tf.cuh"
 
 using namespace lins_capi;
 
@@ -229,6 +233,29 @@ __global__ void __launch_bounds__(kRedThreads) lins_loop_icp_kernel(const LoopSl
   if (conv) { S.converged = 1; S.done = 1; }
 }
 
+// one copy of the gather in front of a segmented VoxelGrid: n records from src (device memory, or the host store's
+// mapped memory) to dst, through tf_point(c) when tf != 0 (a host-store body cloud into the map frame)
+struct GatherJob { const float4* src; float4* dst; int n, tf; TfConsts c; };
+
+// one block per job; each source record is read once
+__global__ void __launch_bounds__(256) lins_loop_gather_kernel(const GatherJob* __restrict__ jobs) {
+  const GatherJob& jb = jobs[blockIdx.x];
+  const TfConsts c = jb.c;
+  if (jb.tf)
+    for (int i = threadIdx.x; i < jb.n; i += blockDim.x) jb.dst[i] = tf_point(c, jb.src[i]);
+  else
+    for (int i = threadIdx.x; i < jb.n; i += blockDim.x) jb.dst[i] = jb.src[i];
+}
+
+// the gather jobs of a host-store key frame's clouds a (0 corner, 1 surf, 2 outlier) for a < n_clouds, each transformed
+// by the key pose, appended to v (dst is set by gather_voxel_grid)
+void host_kf_jobs(const MapperNode& m, int id, int n_clouds, std::vector<GatherJob>& v) {
+  const HostKeyFrame& h = m.host[id];
+  const TfConsts c = tf_consts(m.poses[id]);
+  const float4* p = h.p;
+  for (int a = 0; a < n_clouds; ++a) { v.push_back(GatherJob{p, nullptr, h.n[a], 1, c}); p += h.n[a]; }
+}
+
 // pcl::getTransformation(x, y, z, roll, pitch, yaw) as a 3 x 4 f32 matrix
 void pcl_transformation(float x, float y, float z, float roll, float pitch, float yaw, float t[12]) {
   const float A = std::cos(yaw), B = std::sin(yaw), C = std::cos(pitch), D = std::sin(pitch), E = std::cos(roll), F = std::sin(roll);
@@ -268,41 +295,52 @@ void key_pose_from(const lins_pg::Pose3& e, MapperKeyPose& k) {
 
 const lins_pg::Vec6 kOdomVar = {1e-6, 1e-6, 1e-6, 1e-8, 1e-8, 1e-6};  // priorNoise / odometryNoise (:382-385)
 
-// every buffer gather_voxel_grid uses for n points in n_seg segments and n_copies gather copies (grow-only)
-int gather_voxel_grid_reserve(lins_ctx* ctx, MappersState& ms, int n, int n_seg, size_t n_copies) {
+// every buffer gather_voxel_grid uses for n points in n_seg segments and n_jobs gather jobs (grow-only)
+int gather_voxel_grid_reserve(lins_ctx* ctx, MappersState& ms, int n, int n_seg, size_t n_jobs) {
   LoopPass& lp = ms.lp;
   int rc;
   if ((rc = voxel_grid_reserve(ctx, ms.vg, n, n_seg)) != LINS_OK) return rc;
   CK(lp.tin.grow((size_t)n + 1)); CK(lp.tgt.grow((size_t)n + 1));
   CK(lp.info.reserve(n_seg)); CK(lp.h_info.reserve(n_seg)); CK(lp.h_init.reserve(n_seg));
   CK(lp.off.reserve(n_seg + 1)); CK(lp.h_off.reserve(n_seg + 1)); CK(lp.out.reserve(n_seg)); CK(lp.h_out.reserve(n_seg));
-  return ms.copies.reserve(ctx, n_copies);
+  CK(lp.jobs.reserve(sizeof(GatherJob) * (n_jobs + 1))); CK(lp.h_jobs.reserve(sizeof(GatherJob) * (n_jobs + 1)));
+  return LINS_OK;
 }
 
 // The history sub-maps of close_loops and the global map: segment p of one segmented 0.4 m VoxelGrid is the
-// concatenation of the device clouds lists[p].  One gather launch (the caller's copies first) into ms.lp.tin at toff[p]
-// (lists.size() + 1 offsets, filled here), then the VoxelGrid into ms.lp.tgt at the same offsets, its records at
-// ms.lp.info for the caller to read back.  Every buffer is reserved before anything is queued.
-int gather_voxel_grid(lins_ctx* ctx, MappersState& ms, const std::vector<std::vector<MapPiece>>& lists, std::vector<DevCopy> copies,
+// concatenation of the clouds lists[p] (host-store key frames, transformed on the way).  One gather launch (the
+// caller's jobs first, with their own destinations) into ms.lp.tin at toff[p] (lists.size() + 1 offsets, filled
+// here), then the VoxelGrid into ms.lp.tgt at the same offsets, its records at ms.lp.info for the caller to read back.
+// Every buffer is reserved before anything is queued.  The pinned job table is rewritten only after the caller's
+// synchronisation of the previous call (each caller reads its results back before it gathers again).
+int gather_voxel_grid(lins_ctx* ctx, MappersState& ms, const std::vector<std::vector<GatherJob>>& lists, std::vector<GatherJob> jobs,
                       std::vector<int>& toff) {
   LoopPass& lp = ms.lp;
   const int A = (int)lists.size();
   toff.assign(A + 1, 0);
   for (int p = 0; p < A; ++p) {
     int n = 0;
-    for (const MapPiece& c : lists[p]) n += c.len;
+    for (const GatherJob& c : lists[p]) n += c.n;
     toff[p + 1] = toff[p] + n;
   }
   const int nt = toff[A];
-  size_t n_copies = copies.size();
-  for (const auto& l : lists) n_copies += l.size();
+  size_t n_jobs = jobs.size();
+  for (const auto& l : lists) n_jobs += l.size();
   int rc;
-  if ((rc = gather_voxel_grid_reserve(ctx, ms, nt, A, n_copies)) != LINS_OK) return rc;
+  if ((rc = gather_voxel_grid_reserve(ctx, ms, nt, A, n_jobs)) != LINS_OK) return rc;
   for (int p = 0; p < A; ++p) {
     float4* o = lp.tin.p + toff[p];
-    for (const MapPiece& c : lists[p]) { copies.push_back(DevCopy{c.src, o, c.len, 0}); o += c.len; }
+    for (GatherJob c : lists[p]) { c.dst = o; jobs.push_back(c); o += c.n; }
   }
-  if ((rc = queue_copies(ctx, ms.copies, std::move(copies), 0)) != LINS_OK) return rc;
+  jobs.erase(std::remove_if(jobs.begin(), jobs.end(), [](const GatherJob& c) { return c.n <= 0; }), jobs.end());
+  if (!jobs.empty()) {
+    const size_t bytes = sizeof(GatherJob) * jobs.size();
+    std::memcpy(lp.h_jobs.p, jobs.data(), bytes);
+    CK(cudaMemcpyAsync(lp.jobs.p, lp.h_jobs.p, bytes, cudaMemcpyHostToDevice, ctx->stream));
+    lins_loop_gather_kernel<<<(unsigned)jobs.size(), 256, 0, ctx->stream>>>(reinterpret_cast<const GatherJob*>(lp.jobs.p));
+    CK(cudaGetLastError());
+    ctx->launches += 1;
+  }
   std::vector<float> leaf(A, 0.4f);
   for (int p = 0; p < A; ++p) { lp.h_off.p[p] = toff[p]; lp.h_out.p[p] = lp.tgt.p + toff[p]; }
   lp.h_off.p[A] = nt;
@@ -377,14 +415,13 @@ int mappers_close_loops(lins_ctx* ctx, MappersState& ms, const uint8_t* mask, li
   // the sources (latest corner, surf) and history clouds (closest +- 25: corner, surf per key frame)
   LoopPass& lp = ms.lp;
   std::vector<int> soff(A + 1, 0);
-  std::vector<std::vector<MapPiece>> hist(A);
+  std::vector<std::vector<GatherJob>> hist(A);
   auto kf = [&](const MapperNode& m, int id) -> const MapperKeyFrame& { return m.slots[m.slot_of.at(id)]; };
   for (int p = 0; p < A; ++p) {
     const MapperNode& m = ms.node[act[p]];
     const int latest = rr[act[p]].latest_frame_id, closest = rr[act[p]].closest_history_frame_id;
     soff[p + 1] = soff[p] + kf(m, latest).n[0] + kf(m, latest).n[1];
-    for (int j = std::max(0, closest - kHistory); j <= std::min(latest, closest + kHistory); ++j)
-      for (int a = 0; a < 2; ++a) hist[p].push_back(MapPiece{kf(m, j).c[a].p, kf(m, j).n[a]});
+    for (int j = std::max(0, closest - kHistory); j <= std::min(latest, closest + kHistory); ++j) host_kf_jobs(m, j, 2, hist[p]);
   }
   const int ns = soff[A];
   std::vector<int2> blocks;
@@ -398,12 +435,12 @@ int mappers_close_loops(lins_ctx* ctx, MappersState& ms, const uint8_t* mask, li
   CK(lp.corr.grow((size_t)ns + 1)); CK(lp.dist.grow((size_t)ns + 1));
   CK(lp.slot.reserve(A)); CK(lp.h_slot.reserve(A)); CK(lp.st.reserve(A)); CK(lp.h_st.reserve(A));
   CK(lp.blk.reserve(std::max(nb, 1))); CK(lp.h_blk.reserve(std::max(nb, 1)));
-  std::vector<DevCopy> copies;
+  std::vector<GatherJob> copies;  // the sources, from the device store (the newest key frame stays there)
   for (int p = 0; p < A; ++p) {
     const MapperNode& m = ms.node[act[p]];
     const int latest = rr[act[p]].latest_frame_id;
     float4* o = lp.src0.p + soff[p];
-    for (int a = 0; a < 2; ++a) { copies.push_back(DevCopy{kf(m, latest).c[a].p, o, kf(m, latest).n[a], 0}); o += kf(m, latest).n[a]; }
+    for (int a = 0; a < 2; ++a) { copies.push_back(GatherJob{kf(m, latest).c[a].p, o, kf(m, latest).n[a], 0, TfConsts{}}); o += kf(m, latest).n[a]; }
   }
   // nearHistorySurfKeyFrameCloudDS: one segmented VoxelGrid, a segment per slot, gathered with the sources
   std::vector<int> toff;
@@ -476,8 +513,8 @@ int mappers_close_loops(lins_ctx* ctx, MappersState& ms, const uint8_t* mask, li
 }
 
 // publishGlobalMap (:976-1031) of the masked slots (DESIGN.md §4.15): the key-frame selection on the host
-// (csrc/host/global_map.hpp), then the named key frames' stored map-frame clouds (c = T(b, pose) after every save and
-// correctPoses, so the two-argument transformPointCloud is not run again) gathered and down-sampled in passes of up to
+// (csrc/host/global_map.hpp), then the named key frames' map-frame clouds (T(b, pose) of their host-store clouds, the
+// bits the device store holds for its key frames) gathered and down-sampled in passes of up to
 // LINS_GLOBAL_MAP_PASS_POINTS points, a segment per slot, one synchronisation per pass.  Each result is copied into a
 // buffer of the slot's own; nothing else of the node changes.
 int mappers_global_map(lins_ctx* ctx, MappersState& ms, const uint8_t* mask, lins_global_map_report* reps) {
@@ -486,7 +523,7 @@ int mappers_global_map(lins_ctx* ctx, MappersState& ms, const uint8_t* mask, lin
     if (mask[s] && !ms.node[s].loops.enabled)
       return fail(ctx, LINS_E_INVALID, "lins_gpu_mappers_global_map: a masked slot does not have loop closure enabled");
   CK(cudaSetDevice(ctx->device));
-  struct Job { int s; lins_global_map_report rep; std::vector<int32_t> keys; std::vector<MapPiece> clouds; };
+  struct Job { int s; lins_global_map_report rep; std::vector<int32_t> keys; std::vector<GatherJob> clouds; };
   std::vector<Job> jobs;
   for (int s = 0; s < M; ++s) {
     if (!mask[s]) continue;
@@ -496,8 +533,8 @@ int mappers_global_map(lins_ctx* ctx, MappersState& ms, const uint8_t* mask, lin
     j.keys = lins_gm::key_poses_ds(m.poses, sel);
     long long n = 0;
     for (int32_t id : j.keys) {
-      const MapperKeyFrame& f = m.slots[m.slot_of.at(id)];
-      for (int a = 0; a < 3; ++a) { j.clouds.push_back(MapPiece{f.c[a].p, f.n[a]}); n += f.n[a]; }
+      host_kf_jobs(m, id, 3, j.clouds);
+      for (int a = 0; a < 3; ++a) n += m.host[id].n[a];
     }
     if (n > INT_MAX) return fail(ctx, LINS_E_TOOBIG, "lins_gpu_mappers_global_map: a slot's key-frame clouds exceed INT32_MAX points");
     j.rep.n_key_poses = (int32_t)sel.size();
@@ -531,7 +568,7 @@ int mappers_global_map(lins_ctx* ctx, MappersState& ms, const uint8_t* mask, lin
   LoopPass& lp = ms.lp;
   for (const auto& ps : passes) {
     std::vector<size_t> seg;
-    std::vector<std::vector<MapPiece>> lists;
+    std::vector<std::vector<GatherJob>> lists;
     for (size_t k = ps.first; k < ps.second; ++k)
       if (jobs[k].rep.n_points) { seg.push_back(k); lists.push_back(jobs[k].clouds); }
     std::vector<int> toff;

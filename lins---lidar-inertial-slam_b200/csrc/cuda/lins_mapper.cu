@@ -7,7 +7,8 @@
 // the IMU ring, the 0.3 m key-frame test, the pose's round trip through gtsam's Rot3 and the loop-candidate search, in the
 // reference's f32 / f64 types (no multiply-add contraction: this unit is built with -fmad=false and g++ does not
 // contract on x86-64 without -mfma).  Device: the key-frame store, each key frame's DS clouds transformed into the map
-// frame once, at save time, with its PointTypePose (one launch for the key frames a step saves).
+// frame once, at save time, with its PointTypePose (one launch for the key frames a step saves); on a slot with loop
+// closure the same launch writes the body-frame clouds into the host store through their mapped addresses.
 //
 // VoxelGrid (csrc/host/feature_extraction.hpp restates PCL's applyFilter), on one or many clouds (segments) in one pass:
 // each segment's finite points' min / max (ordered-integer atomics: min / max are exact in any order), its min_b =
@@ -263,12 +264,13 @@ int keyframes_queue(lins_ctx* ctx, const KfSave* saves, int n, Buf<unsigned char
   for (int i = 0; i < n; ++i) {
     const KfSave& sv = saves[i];
     const TfConsts c = tf_consts(sv.kp);
-    const TfConsts id = {1.f, 0.f, 1.f, 0.f, 1.f, 0.f, 0.f, 0.f, 0.f};  // (the identity: each output is its input exactly)
+    const TfConsts id = {1.f, 0.f, 1.f, 0.f, 1.f, 0.f, 0.f, 0.f, 0.f};  // (the identity: the bits T(b, pose) is built on)
+    float4* body = sv.body;
     for (int a = 0; a < 3; ++a) {
       CK(sv.kf->c[a].grow((size_t)sv.kf->n[a] + 1));
-      if (sv.body) CK(sv.kf->b[a].grow((size_t)sv.kf->n[a] + 1));
       if (sv.kf->n[a]) jobs.push_back(TfJob{sv.ds[a], sv.kf->c[a].p, sv.kf->n[a], 0, c});
-      if (sv.kf->n[a] && sv.body) jobs.push_back(TfJob{sv.ds[a], sv.kf->b[a].p, sv.kf->n[a], 0, id});
+      if (sv.kf->n[a] && body) jobs.push_back(TfJob{sv.ds[a], body, sv.kf->n[a], 0, id});
+      if (body) body += sv.kf->n[a];
     }
   }
   if (jobs.empty()) return LINS_OK;
@@ -341,7 +343,7 @@ int queue_copies(lins_ctx* ctx, CopyList& l, std::vector<DevCopy> v, int base) {
   return rc != LINS_OK ? rc : l.launch(ctx, base, (int)v.size());
 }
 
-void mapper_node_reset(MapperNode& m) {
+void mapper_node_reset(MapperNode& m, lins_arena::Arena& store) {
   m.s = MapperScalars();
   m.stepped = false;
   m.loops = MapperLoops();
@@ -349,6 +351,8 @@ void mapper_node_reset(MapperNode& m) {
   m.poses.clear();
   for (auto& kv : m.slot_of) m.free_slots.push_back(kv.second);
   m.slot_of.clear();
+  store.give_back(m.held);
+  m.host.clear();
   m.last = MapperLast();
 }
 
@@ -460,9 +464,9 @@ void mapper_cycle_end(MapperNode& M, MapperScalars& s, double timeLaserOdometry,
     *saved = true;
     r.keyframe_saved = 1;
     r.loop_candidate = loop_candidate(M, cur, timeLaserOdometry);
-    // the store keeps the window and the newest key frame: nothing else can enter a later window (a slot with loop
-    // closure keeps every key frame, for the history sub-maps and correctPoses)
-    for (auto it = M.slot_of.begin(); it != M.slot_of.end() && !M.loops.enabled;) {
+    // the device store keeps the window and the newest key frame: nothing else can enter a later window (a slot with
+    // loop closure keeps every key frame in its host store, for the history sub-maps and the global map)
+    for (auto it = M.slot_of.begin(); it != M.slot_of.end();) {
       const int kid = it->first;
       if (kid != id && std::find(s.window.begin(), s.window.end(), kid) == s.window.end()) { M.free_slots.push_back(it->second); it = M.slot_of.erase(it); }
       else ++it;

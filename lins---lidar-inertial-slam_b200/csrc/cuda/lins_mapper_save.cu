@@ -3,14 +3,19 @@
 // _save / _load).  A slot's blob (lins_mapper_blob.hpp) carries what a later step, fuse, download, close_loops or global
 // map of the slot reads: its scalars and IMU queue, window, key poses, stored key frames' clouds and scan-to-map loop
 // state, and on a slot with loop closure the key-pose graph, its estimate and MapperLoops' scalars.
-//   save: one gather launch of every masked slot's device pieces (a plain slot's map-frame key-frame clouds, a loop
-//         slot's body-frame ones, the loop state) into one staging buffer laid out as the caller's buffer, one D2H into
-//         pinned staging, one synchronisation; the host records are written after it.
-//   load: every masked blob validated in full first; then one H2D of the blobs (with the rebuild's job table behind
-//         them), one gather launch that installs the loop states and fills the plain slots' key frames, and one launch of
-//         lins_mapper_rebuild_kernel that writes each loop slot's key frame into its body-frame store and its transform
-//         by the key pose into the map-frame store, c = T(b, pose), as every save and correctPoses leave them
-//         (DESIGN.md §4.15); one synchronisation at the end.
+//   save: one gather launch of every masked slot's device pieces (a plain slot's map-frame key-frame clouds, the loop
+//         state) into one staging buffer of the slots' device ranges back to back, one D2H into pinned staging, one
+//         synchronisation; the host records are written after it, and a loop slot's body-frame clouds are copied from
+//         its host store (the synchronisation orders the copy after the last kernel that wrote them).
+//   load: every masked blob validated in full first; then a synchronisation (a queued kernel may still write a chunk a
+//         reset handed back), a loop slot's body-frame clouds copied into its host store on the host, one H2D of the
+//         blobs (with the rebuild's job table behind them), one gather launch that installs the loop states and fills
+//         the plain slots' key frames, and one launch of lins_mapper_rebuild_kernel that writes the transform by the key
+//         pose of each key frame a loop slot's device store keeps into that store, c = T(b, pose), as every save and
+//         correctPoses leave them (DESIGN.md §4.15); one synchronisation at the end.
+// A loop slot's blob carries every key frame (its host store); the loaded device store is the key frames a later window
+// can take (lins_slot_blob.hpp's mapper_state_check): the window, the newest key frame and, while the window is short,
+// the last 50.
 // A call's device and pinned staging is the masked blobs' total (and the job table on a load): a caller bounds it by
 // saving and loading with smaller masks.
 #include <cuda_runtime.h>
@@ -23,6 +28,7 @@
 #include <vector>
 
 #include "lins_ctx.hpp"
+#include "lins_kf_arena.hpp"
 #include "lins_map_types.cuh"
 #include "lins_mapper_blob.hpp"
 #include "lins_mapper_tf.cuh"
@@ -44,18 +50,14 @@ B::BuildSizes build_sizes() {
                        (uint32_t)sizeof(B::FactorRec)};
 }
 
-// one loaded key-frame cloud of a slot with loop closure: its body-frame points in the staging (in) into b, and their
-// transform by the key pose (k) into c
-struct KfRebuild { const float4* in; float4* b; float4* c; int n, pad; TfConsts k; };
+// one loaded key-frame cloud of a slot with loop closure that its device store keeps: its body-frame points in the
+// staging (in) transformed by the key pose (k) into c
+struct KfRebuild { const float4* in; float4* c; int n, pad; TfConsts k; };
 
 __global__ void __launch_bounds__(256) lins_mapper_rebuild_kernel(const KfRebuild* __restrict__ jobs) {
   const KfRebuild& jb = jobs[blockIdx.x];
   const TfConsts c = jb.k;
-  for (int i = threadIdx.x; i < jb.n; i += blockDim.x) {
-    const float4 p = jb.in[i];
-    jb.b[i] = p;
-    jb.c[i] = tf_point(c, p);
-  }
+  for (int i = threadIdx.x; i < jb.n; i += blockDim.x) jb.c[i] = tf_point(c, jb.in[i]);
 }
 
 double ms_since(std::chrono::steady_clock::time_point& t) {
@@ -65,20 +67,30 @@ double ms_since(std::chrono::steady_clock::time_point& t) {
   return ms;
 }
 
-// the stored key frames of a node as (id, store slot), by id (the blob's order)
+// the stored key frames of a node as (id, device store slot), by id (the blob's order): a plain slot's device store;
+// every key frame of a slot with loop closure (its host store; the slot is -1)
 std::vector<std::pair<int, int>> stored_keyframes(const MapperNode& m) {
-  std::vector<std::pair<int, int>> v(m.slot_of.begin(), m.slot_of.end());
+  std::vector<std::pair<int, int>> v;
+  if (m.loops.enabled) {
+    for (int id = 0; id < (int)m.host.size(); ++id) v.push_back({id, -1});
+    return v;
+  }
+  v.assign(m.slot_of.begin(), m.slot_of.end());
   std::sort(v.begin(), v.end());
   return v;
 }
+
+// the cloud sizes of stored key frame k
+const int* kf_sizes(const MapperNode& m, const std::pair<int, int>& k) { return m.loops.enabled ? m.host[k.first].n : m.slots[k.second].n; }
 
 B::Counts node_counts(const MapperNode& m) {
   B::Counts c;
   c.n_poses = (int64_t)m.poses.size();
   c.n_window = (int64_t)m.s.window.size();
-  c.n_keyframes = (int64_t)m.slot_of.size();
-  for (const auto& kv : m.slot_of)
-    for (int a = 0; a < 3; ++a) c.n_kf_points += m.slots[kv.second].n[a];
+  const std::vector<std::pair<int, int>> kf = stored_keyframes(m);
+  c.n_keyframes = (int64_t)kf.size();
+  for (const auto& k : kf)
+    for (int a = 0; a < 3; ++a) c.n_kf_points += kf_sizes(m, k)[a];
   c.n_factors = (int64_t)m.loops.graph.size();
   c.n_est = (int64_t)m.loops.est.size();
   return c;
@@ -108,21 +120,30 @@ void put(uint8_t* dst, const void* src, size_t bytes) {
   std::memset(dst + bytes, 0, B::align16(bytes) - bytes);
 }
 
-// the device pieces of slot s's blob, as gather copies into dst (the blob's first byte in the device staging): the key
-// frames' clouds (in kf order; body frame on a slot with loop closure) and the loop state
-void save_copies(MappersState& ms, int s, const B::Header& h, float4* dst, const std::vector<std::pair<int, int>>& kf, std::vector<DevCopy>& v) {
+// the bytes [lo, hi) of slot s's blob that come from the device: a plain slot's key frames' clouds and the loop state,
+// which follows them; a slot with loop closure's loop state (its key frames' clouds come from its host store)
+void device_range(const MapperNode& m, const B::Header& h, uint64_t& lo, uint64_t& hi) {
+  lo = m.loops.enabled ? h.sec[B::kLoop].off : h.sec[B::kKfClouds].off;
+  hi = h.sec[B::kLoop].off + h.sec[B::kLoop].bytes;
+}
+
+// the device pieces of slot s's blob, as gather copies into dst (byte lo of the blob's device range in the device
+// staging): a plain slot's key frames' clouds (in kf order) and the loop state
+void save_copies(MappersState& ms, int s, const B::Header& h, float4* dst, uint64_t lo, const std::vector<std::pair<int, int>>& kf, std::vector<DevCopy>& v) {
   const MapperNode& m = ms.node[s];
+  dst -= lo / 16;
   float4* o = dst + h.sec[B::kKfClouds].off / 16;
   for (const auto& k : kf)
-    for (int a = 0; a < 3; ++a) {
+    for (int a = 0; a < 3 && !m.loops.enabled; ++a) {
       const MapperKeyFrame& f = m.slots[k.second];
-      v.push_back(DevCopy{m.loops.enabled ? f.b[a].p : f.c[a].p, o, f.n[a], 0});
+      v.push_back(DevCopy{f.c[a].p, o, f.n[a], 0});
       o += f.n[a];
     }
   v.push_back(DevCopy{reinterpret_cast<const float4*>(ms.stm.loop.p + s), dst + h.sec[B::kLoop].off / 16, (int)(sizeof(lins_map::MapLoopState) / 16), 0});
 }
 
-// the host records of slot s's blob into img (its first byte in the pinned image)
+// the host records of slot s's blob into img (its first byte in the caller's buffer), and a loop slot's key-frame clouds
+// from its host store
 void save_host(const MapperNode& m, const B::Counts& c, B::Header h, uint8_t* img, const std::vector<std::pair<int, int>>& kf) {
   const MapperLoops& L = m.loops;
   h.magic = B::kMagic;
@@ -146,10 +167,19 @@ void save_host(const MapperNode& m, const B::Counts& c, B::Header h, uint8_t* im
   put(img + h.sec[B::kWindow].off, win.data(), sizeof(int32_t) * win.size());
   std::vector<B::KeyframeRec> tab;
   for (const auto& k : kf) {
-    const MapperKeyFrame& f = m.slots[k.second];
-    tab.push_back(B::KeyframeRec{k.first, {f.n[0], f.n[1], f.n[2]}});
+    const int* n = kf_sizes(m, k);
+    tab.push_back(B::KeyframeRec{k.first, {n[0], n[1], n[2]}});
   }
   put(img + h.sec[B::kKeyframes].off, tab.data(), sizeof(B::KeyframeRec) * tab.size());
+  if (L.enabled) {  // the host store's body-frame clouds, in table order (the caller has synchronised the stream)
+    uint8_t* o = img + h.sec[B::kKfClouds].off;
+    for (const auto& k : kf) {
+      const HostKeyFrame& f = m.host[k.first];
+      const size_t bytes = sizeof(float4) * ((size_t)f.n[0] + f.n[1] + f.n[2]);
+      if (bytes) std::memcpy(o, f.p, bytes);
+      o += bytes;
+    }
+  }
   std::vector<B::FactorRec> fac(L.graph.size());
   for (size_t i = 0; i < L.graph.size(); ++i) {
     const lins_pg::Factor& f = L.graph[i];
@@ -166,31 +196,38 @@ void save_host(const MapperNode& m, const B::Counts& c, B::Header h, uint8_t* im
 // the device part of a save on checked arguments (a failure ends the run)
 int save_run(lins_ctx* ctx, MappersState& ms, const uint8_t* mask, uint8_t* blob, const uint64_t* off) {
   const int n = ms.n;
-  const uint64_t total = off[n];
   CK(cudaSetDevice(ctx->device));
-  CK(ms.blob.reserve(total / 16 + 1)); CK(ms.h_blob.reserve(total / 16 + 1));
   std::vector<B::Counts> counts(n);
   std::vector<B::Header> hdr(n);
   std::vector<std::vector<std::pair<int, int>>> kf(n);
-  std::vector<DevCopy> copies;
+  std::vector<uint64_t> lo(n, 0), hi(n, 0), doff(n + 1, 0);  // each slot's device range, and its place in the staging
   for (int s = 0; s < n; ++s) {
+    doff[s + 1] = doff[s];
     if (!mask[s]) continue;
     counts[s] = node_counts(ms.node[s]);
     B::layout(counts[s], build_sizes(), hdr[s]);
     kf[s] = stored_keyframes(ms.node[s]);
-    save_copies(ms, s, hdr[s], ms.blob.p + off[s] / 16, kf[s], copies);
+    device_range(ms.node[s], hdr[s], lo[s], hi[s]);
+    doff[s + 1] += hi[s] - lo[s];
   }
+  const uint64_t total = doff[n];
+  CK(ms.blob.reserve(total / 16 + 1)); CK(ms.h_blob.reserve(total / 16 + 1));
+  std::vector<DevCopy> copies;
+  for (int s = 0; s < n; ++s)
+    if (mask[s]) save_copies(ms, s, hdr[s], ms.blob.p + doff[s] / 16, lo[s], kf[s], copies);
   copies.erase(std::remove_if(copies.begin(), copies.end(), [](const DevCopy& c) { return c.n <= 0; }), copies.end());
   int rc = ms.copies.reserve(ctx, copies.size());
   if (rc == LINS_OK) rc = ms.copies.stage(ctx, copies.data(), (int)copies.size(), 0);
   if (rc == LINS_OK) rc = ms.copies.launch(ctx, 0, (int)copies.size());
   if (rc != LINS_OK) return rc;
-  uint8_t* img = reinterpret_cast<uint8_t*>(ms.h_blob.p);
-  CK(cudaMemcpyAsync(img, ms.blob.p, total, cudaMemcpyDeviceToHost, ctx->stream));
+  const uint8_t* img = reinterpret_cast<const uint8_t*>(ms.h_blob.p);
+  CK(cudaMemcpyAsync(ms.h_blob.p, ms.blob.p, total, cudaMemcpyDeviceToHost, ctx->stream));
   CK(cudaStreamSynchronize(ctx->stream));
-  for (int s = 0; s < n; ++s)
-    if (mask[s]) save_host(ms.node[s], counts[s], hdr[s], img + off[s], kf[s]);
-  std::memcpy(blob, img, total);
+  for (int s = 0; s < n; ++s) {
+    if (!mask[s]) continue;
+    std::memcpy(blob + off[s] + lo[s], img + doff[s], hi[s] - lo[s]);
+    save_host(ms.node[s], counts[s], hdr[s], blob + off[s], kf[s]);
+  }
   return LINS_OK;
 }
 
@@ -200,6 +237,7 @@ int load_run(lins_ctx* ctx, MappersState& ms, const uint8_t* mask, const std::ve
   auto t = std::chrono::steady_clock::now();
   const int n = ms.n;
   CK(cudaSetDevice(ctx->device));
+  CK(cudaStreamSynchronize(ctx->stream));  // (before the host writes the host stores' chunks)
   // the blobs back to back in the staging, each at a 16-byte boundary (its length is a multiple of 16), then the
   // rebuild's job table
   std::vector<uint64_t> base(n, 0);
@@ -212,23 +250,48 @@ int load_run(lins_ctx* ctx, MappersState& ms, const uint8_t* mask, const std::ve
     if (v[s].loops())
       for (int i = 0; i < v[s].sc.n_keyframes; ++i) {
         const B::KeyframeRec k = v[s].keyframe(i);
-        for (int a = 0; a < 3; ++a) n_jobs += k.n[a] > 0;
+        for (int a = 0; a < 3; ++a) n_jobs += k.n[a] > 0;  // (a bound: only the device store's key frames get jobs)
       }
   }
   const uint64_t job_off = B::align16(total), staged = job_off + sizeof(KfRebuild) * n_jobs;
   CK(ms.blob.reserve(staged / 16 + 1)); CK(ms.h_blob.reserve(staged / 16 + 1));
   auto at = [&](int s, int sec) { return ms.blob.p + (base[s] + v[s].h.sec[sec].off) / 16; };
-  // every buffer first: each key frame's store slot (a free one first) and its clouds
+  // every buffer first: each device-store key frame's slot (a free one first) and its clouds, and each loop slot's host
+  // store blocks
   std::vector<DevCopy> copies;
   std::vector<KfRebuild> jobs;
+  std::vector<std::pair<float4*, const uint8_t*>> host_fill;  // (host-store block, its clouds in the caller's blob)
+  std::vector<size_t> host_bytes;
   for (int s = 0; s < n; ++s) {
     if (!mask[s]) continue;
     const B::View& b = v[s];
     MapperNode& m = ms.node[s];
     copies.push_back(DevCopy{at(s, B::kLoop), reinterpret_cast<float4*>(ms.stm.loop.p + s), (int)(sizeof(lins_map::MapLoopState) / 16), 0});
     const float4* src = at(s, B::kKfClouds);
+    const uint8_t* hsrc = b.at(B::kKfClouds);
+    std::vector<unsigned char> keep;  // a loop slot: the key frames its device store keeps
+    if (b.loops()) {
+      const int np = b.sc.n_poses;
+      keep.assign(np, 0);
+      for (int i = 0; i < b.sc.n_window; ++i) keep[b.window(i)] = 1;
+      if (np > 0) keep[np - 1] = 1;
+      if (b.sc.n_window < LINS_MAPPER_WINDOW)
+        for (int id = std::max(0, np - LINS_MAPPER_WINDOW); id < np; ++id) keep[id] = 1;
+      m.host.assign(np, HostKeyFrame());
+    }
     for (int i = 0; i < b.sc.n_keyframes; ++i) {
       const B::KeyframeRec k = b.keyframe(i);
+      if (b.loops()) {
+        HostKeyFrame& hk = m.host[k.id];
+        std::copy(k.n, k.n + 3, hk.n);
+        const size_t bytes = sizeof(float4) * ((size_t)k.n[0] + k.n[1] + k.n[2]);
+        void* p = nullptr;
+        if (!ms.store.take(m.held, bytes, &p)) return fail(ctx, LINS_E_CUDA, "the host key-frame store could not allocate pinned memory");
+        hk.p = static_cast<float4*>(p);
+        if (bytes) { host_fill.push_back({hk.p, hsrc}); host_bytes.push_back(bytes); }
+        hsrc += bytes;
+        if (!keep[k.id]) { src += k.n[0] + k.n[1] + k.n[2]; continue; }
+      }
       int slot;
       if (!m.free_slots.empty()) { slot = m.free_slots.back(); m.free_slots.pop_back(); }
       else { slot = (int)m.slots.size(); m.slots.emplace_back(); }
@@ -242,8 +305,7 @@ int load_run(lins_ctx* ctx, MappersState& ms, const uint8_t* mask, const std::ve
         f.n[a] = k.n[a];
         CK(f.c[a].grow((size_t)k.n[a] + 1));
         if (b.loops()) {
-          CK(f.b[a].grow((size_t)k.n[a] + 1));
-          if (k.n[a]) jobs.push_back(KfRebuild{src, f.b[a].p, f.c[a].p, k.n[a], 0, tc});
+          if (k.n[a]) jobs.push_back(KfRebuild{src, f.c[a].p, k.n[a], 0, tc});
         } else {
           copies.push_back(DevCopy{src, f.c[a].p, k.n[a], 0});
         }
@@ -256,7 +318,8 @@ int load_run(lins_ctx* ctx, MappersState& ms, const uint8_t* mask, const std::ve
   if ((rc = ms.copies.reserve(ctx, copies.size())) != LINS_OK) return rc;
   ph[1] = ms_since(t);
 
-  // the blobs and the job table into the pinned image
+  // the loop slots' host stores, the blobs and the job table into the pinned image
+  for (size_t i = 0; i < host_fill.size(); ++i) std::memcpy(host_fill[i].first, host_fill[i].second, host_bytes[i]);
   uint8_t* img = reinterpret_cast<uint8_t*>(ms.h_blob.p);
   for (int s = 0; s < n; ++s) if (mask[s]) std::memcpy(img + base[s], v[s].p, v[s].h.total);
   if (!jobs.empty()) std::memcpy(img + job_off, jobs.data(), sizeof(KfRebuild) * jobs.size());

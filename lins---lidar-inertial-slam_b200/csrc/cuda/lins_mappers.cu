@@ -8,7 +8,14 @@
 // 0.4 m, corner 0.2 m, surf 0.4 m, outlier 0.4 m), one gather of each slot's surf DS + outlier DS and one segmented
 // VoxelGrid of those (0.4 m); every slot's grids and scan-to-map loop (lins_map.cu, grid origin 0); the read-back of
 // the VoxelGrid records and loop states.  After it, the host tail of each slot and one transform launch for every key
-// frame saved.  The VoxelGrids' outputs are sized by their inputs and padded with NaN, and the later launches take those
+// frame saved (and, on a slot with loop closure, for its body-frame clouds into the host store and, after correctPoses,
+// for its device store re-transformed from the host store).
+//
+// The host store (DESIGN.md §4.14) is the run's arena of pinned, mapped memory (lins_kf_arena.hpp).  Device work reads
+// and writes it only on the context's stream, and host code touches a chunk only where the stream is idle: a save
+// reads it after its synchronisation, a load writes it after a synchronisation at its start, and open and destroy free
+// the slabs after one.  A reset hands its chunks back without touching them; the next writer of a chunk is a later
+// kernel on the stream or a load.  The VoxelGrids' outputs are sized by their inputs and padded with NaN, and the later launches take those
 // capacities.  The segments of a VoxelGrid keep their input ranges and each slot's fit blocks cover its own queries
 // only, so every slot's clouds, sums and steps are those of a run of one slot.
 #include <cuda_runtime.h>
@@ -45,11 +52,26 @@ const char* const kBad = "VoxelGrid: the leaf is too small for the cloud's exten
 
 namespace lins_capi {
 
+// the host store's slabs: pinned and mapped, at one address for the host and the device (UVA; anything else fails)
+lins_arena::Allocator pinned_mapped_allocator() {
+  auto alloc = [](size_t bytes, void*) -> void* {
+    void* p = nullptr;
+    if (cudaHostAlloc(&p, bytes, cudaHostAllocMapped) != cudaSuccess) return nullptr;
+    void* d = nullptr;
+    if (cudaHostGetDevicePointer(&d, p, 0) != cudaSuccess || d != p) { cudaFreeHost(p); return nullptr; }
+    return p;
+  };
+  auto release = [](void* p, void*) { cudaFreeHost(p); };
+  return lins_arena::Allocator{alloc, release, nullptr};
+}
+
 // n_slots fresh mapping nodes in ms, replacing any open run
 int mappers_open(lins_ctx* ctx, MappersState& ms, int n_slots) {
   CK(cudaSetDevice(ctx->device));
+  CK(cudaStreamSynchronize(ctx->stream));  // (queued work may still write the host stores' slabs)
   ms.n = 0;
   ms.node = std::vector<MapperNode>(n_slots);  // (constructed in place: a node is not copyable)
+  ms.store.release();
   ms.ds = std::vector<std::array<Buf<float4>, 6>>(n_slots);
   CK(ms.stm.loop.reserve(n_slots)); CK(ms.stm.h_loop.reserve(n_slots)); CK(ms.stm.h_mslot.reserve(n_slots));
   CK(cudaMemsetAsync(ms.stm.loop.p, 0, sizeof(lins_map::MapLoopState) * n_slots, ctx->stream));  // matP, isDegenerate
@@ -62,7 +84,7 @@ int mappers_reset(lins_ctx* ctx, MappersState& ms, const uint8_t* mask) {
   CK(cudaSetDevice(ctx->device));
   for (int s = 0; s < ms.n; ++s)
     if (mask[s]) {
-      mapper_node_reset(ms.node[s]);
+      mapper_node_reset(ms.node[s], ms.store);
       CK(cudaMemsetAsync(ms.stm.loop.p + s, 0, sizeof(lins_map::MapLoopState), ctx->stream));
     }
   return LINS_OK;
@@ -248,18 +270,34 @@ int mappers_step(lins_ctx* ctx, MappersState& ms, const lins_mappers_desc* d, li
     MapperNode& m = ms.node[s];
     if (saved) {
       for (int k = 0; k < 3; ++k) sv.ds[k] = ms.ds[s][2 + k].p;
-      sv.body = m.loops.enabled;
       sv.kp = m.poses.back();  // (correctPoses may have moved it)
+      sv.body = nullptr;
+      if (m.loops.enabled) {  // its block of the host store, by id (ids are saved in order)
+        HostKeyFrame h;
+        std::copy(sv.kf->n, sv.kf->n + 3, h.n);
+        void* p = nullptr;
+        if (!ms.store.take(m.held, sizeof(float4) * ((size_t)h.n[0] + h.n[1] + h.n[2]), &p)) {
+          ms.n = 0;  // (this slot and the ones before it have committed their cycles: the run ends, as after a failed load)
+          return fail(ctx, LINS_E_CUDA, "the host key-frame store could not allocate pinned memory (the run has ended)");
+        }
+        h.p = static_cast<float4*>(p);
+        m.host.push_back(h);
+        sv.body = h.p;
+      }
       saves.push_back(sv);
     }
-    if (m.loops.rebuild)  // correctPoses: every other stored key frame re-transformed from its body-frame clouds
+    if (m.loops.rebuild)  // correctPoses: every other key frame of the device store re-transformed from the host store
       for (const auto& kv : m.slot_of) {
         if (saved && kv.first == (int)m.poses.size() - 1) continue;
         MapperKeyFrame& f = m.slots[kv.second];
-        saves.push_back(KfSave{&f, m.poses[kv.first], {f.b[0].p, f.b[1].p, f.b[2].p}, false});
+        const HostKeyFrame& h = m.host[kv.first];
+        saves.push_back(KfSave{&f, m.poses[kv.first], {h.p, h.p + h.n[0], h.p + h.n[0] + h.n[1]}, nullptr});
       }
   }
-  if ((rc = keyframes_queue(ctx, saves.data(), (int)saves.size(), ms.tf, ms.h_tf)) != LINS_OK) return rc;
+  if ((rc = keyframes_queue(ctx, saves.data(), (int)saves.size(), ms.tf, ms.h_tf)) != LINS_OK) {
+    ms.n = 0;  // (the slots' cycles are committed, their key frames not stored: the run ends)
+    return rc;
+  }
   return finish();
 }
 
@@ -283,6 +321,24 @@ int mappers_loops(lins_ctx* ctx, MappersState& ms, const uint8_t* mask) {
     if (mask[s] && !ms.node[s].loops.enabled && (ms.node[s].stepped || (bound && !ctx->seq.slot[s].fresh)))
       return fail(ctx, LINS_E_INVALID, "loop closure: a masked slot is not fresh (present in a step since open / reset)");
   for (int s = 0; s < ms.n; ++s) if (mask[s]) ms.node[s].loops.enabled = true;
+  return LINS_OK;
+}
+
+// the bytes of the masked slots' key-frame stores (host bookkeeping only)
+int store_bytes(lins_ctx* ctx, const MappersState& ms, const uint8_t* mask, uint64_t* device, uint64_t* host, uint64_t* host_reserved) {
+  if (!mask || !device || !host) return fail(ctx, LINS_E_INVALID, "null mask / device / host");
+  for (int s = 0; s < ms.n; ++s) {
+    if (!mask[s]) continue;
+    const MapperNode& m = ms.node[s];
+    uint64_t d = 0, h = 0;
+    for (const auto& kv : m.slot_of)
+      for (int a = 0; a < 3; ++a) d += (uint64_t)m.slots[kv.second].n[a];
+    for (const HostKeyFrame& k : m.host)
+      for (int a = 0; a < 3; ++a) h += (uint64_t)k.n[a];
+    device[s] = sizeof(float4) * d;
+    host[s] = sizeof(float4) * h;
+  }
+  if (host_reserved) *host_reserved = ms.store.reserved();
   return LINS_OK;
 }
 
@@ -388,6 +444,20 @@ int lins_gpu_mappers_global_map_download(lins_ctx* ctx, int32_t slot, int32_t* k
   if (need_open(ctx) != LINS_OK) return LINS_E_NOMAP;
   if (slot < 0 || slot >= ctx->mappers.n) return fail(ctx, LINS_E_INVALID, "slot out of range");
   return global_map_download(ctx, ctx->mappers.node[slot], key_ids, cloud);
+}
+
+int lins_gpu_mappers_store_bytes(lins_ctx* ctx, const uint8_t* mask, uint64_t* device, uint64_t* host, uint64_t* host_reserved) {
+  if (!ctx) return LINS_E_INVALID;
+  if (need_open(ctx) != LINS_OK) return LINS_E_NOMAP;
+  return store_bytes(ctx, ctx->mappers, mask, device, host, host_reserved);
+}
+
+int lins_gpu_mapper_store_bytes(lins_ctx* ctx, uint64_t* device, uint64_t* host, uint64_t* host_reserved) {
+  if (!ctx) return LINS_E_INVALID;
+  const int rc = mapper_open(ctx);
+  if (rc != LINS_OK) return rc;
+  const uint8_t all = 1;
+  return store_bytes(ctx, ctx->mapper, &all, device, host, host_reserved);
 }
 
 int lins_gpu_mapper_global_map(lins_ctx* ctx, lins_global_map_report* rep) {

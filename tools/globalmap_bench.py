@@ -11,7 +11,9 @@ whatever moved its poses):
   stays within LINS_GLOBAL_MAP_PASS_POINTS), and the device memory the first call adds (its grow-only scratch plus the
   results, from cudaMemGetInfo before and after), with the results' own bytes;
 - a long single drive (--long-trips round trips of the same road, >= 1000 key frames) at M = 1.
-M = 1000 is skipped when the slots' key-frame store would not fit in the free device memory.
+M = 1000 is skipped when the slots' host key-frame stores would not fit in a quarter of the host's MemAvailable (the
+host is shared; a slot's need is its host store's bytes after the M = 1 run rounded up to whole 1 MiB chunks, plus one
+chunk for the chunks' unused tails), or their device stores in the free device memory.
 Prints one JSON line with the GPU's name and power limit."""
 import argparse
 import importlib
@@ -97,6 +99,23 @@ def measure(g, M, stream):
                 device_bytes_added_by_first_call=int(free0 - free1), result_bytes=int(16 * sum(r.n_map for r in reps)))
 
 
+CHUNK = 1 << 20  # the host store's chunk (lins_ctx.hpp: kKfChunkBytes)
+
+
+def host_need_per_slot(g):
+    """pinned bytes one slot of run g needs: its host store's bytes in whole chunks, plus one chunk of unused tails"""
+    return (-(-int(g.mappers_store_bytes()[1][0]) // CHUNK) + 1) * CHUNK
+
+
+def mem_available():
+    """MemAvailable of /proc/meminfo in bytes"""
+    with open("/proc/meminfo") as f:
+        for line in f:
+            if line.startswith("MemAvailable:"):
+                return int(line.split()[1]) * 1024
+    raise RuntimeError("no MemAvailable in /proc/meminfo")
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--slots", default="1,132,1000")
@@ -107,15 +126,17 @@ def main():
     ev = drive(a.seed)
     res = {"what": "lins_gpu_mappers_global_map, tools/loops_bench.py's drifted out-and-back drive in every slot",
            "pass_points": defs.GLOBAL_MAP_PASS_POINTS}
-    store = None
+    store = host = None  # per slot: the device memory a run adds, the host store's pinned bytes
+    res["host_mem_available"] = mem_available()
     for M in [int(x) for x in a.slots.split(",")]:
-        if store is not None and M * store > 0.8 * torch.cuda.mem_get_info()[0]:
+        if store is not None and (M * host > 0.25 * mem_available() or M * store > 0.8 * torch.cuda.mem_get_info()[0]):
             res[f"M={M}"] = "skipped: the store does not fit"
             continue
         free0 = torch.cuda.mem_get_info()[0]
         g, reps = run(ev, M, stream)
         if store is None:
             store = (free0 - torch.cuda.mem_get_info()[0]) / M
+            host = host_need_per_slot(g)
         res[f"M={M}"] = measure(g, M, stream)
         del g
     g, reps = run(long_drive(a.seed, a.long_trips), 1, stream)

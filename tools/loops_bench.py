@@ -11,8 +11,10 @@ whose odometry drifts, copied into every slot, so that every slot has a candidat
 - the host cost of a key-frame save once a slot has a loop factor (the Gauss-Newton solve of the key-pose graph and
   correctPoses): the single mapper's step time after its first closure minus a plain mapper's at the same step, against
   the key-frame count;
-- the store's bytes per key frame: an enabled slot keeps every key frame's three DS clouds twice (map and body frame, 16 B
-  per point each), a plain slot its window once.
+- the key-frame stores' bytes after the drive, from lins_gpu_mappers_store_bytes: an enabled slot's device store (the
+  window and the newest key frame in the map frame, as a plain slot's) and its host store (every key frame's three DS
+  clouds in the body frame, 16 B per point, in pinned host memory), per slot and per key frame, and the run's pinned
+  slabs.
 Prints one JSON line with the GPU's name and power limit."""
 import argparse
 import importlib
@@ -101,8 +103,9 @@ def main():
                    icp_iters_mean=float(it.mean()), icp_iters_max=int(it.max()), n_source_mean=float(np.mean([lr.n_source for lr in lrs])),
                    n_history_ds_mean=float(np.mean([lr.n_history_ds for lr in lrs])), accepted=int(sum(lr.accepted for lr in lrs)))
         nk = reps[0].n_keyframes
-        pts = [r.n_corner_ds + r.n_surf_ds + r.n_outlier_ds for r in [reps[0]]]
-        row["store_bytes_per_key_frame_enabled_last_cycle"] = 2 * 16 * pts[0]
+        dev, host, reserved = g.mappers_store_bytes()
+        row.update(store_device_bytes_per_slot=int(dev[0]), store_host_bytes_per_slot=int(host[0]),
+                   store_host_bytes_per_key_frame=round(int(host[0]) / max(nk, 1), 1), store_host_reserved_bytes=reserved)
         row["key_frames"] = nk
         res[f"M={M}"] = row
         del g

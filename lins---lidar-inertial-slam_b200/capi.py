@@ -51,13 +51,12 @@ NVCC_ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]  # H100 (Hopper)
 NVCC_COMMON = NVCC_ARCH + ["-lineinfo", "-O3", "-std=c++17", "-Xcompiler", "-fPIC"]
 # translation units and their extra flags: lins_gpu.cu (the fused kernel and most of the C-ABI), lins_upload.cu (batch
 # upload), lins_map.cu (row F2's host side), lins_seq.cu (sequence mode), lins_features.cu (feature extraction),
-# lins_projection.cu (image projection), lins_cloud2.cu (PointCloud2 decoding), lins_mapper.cu (the mapping node's cycle), lins_mappers.cu (many mapping nodes in lockstep), lins_loops.cu (their loop closure), lins_seq_save.cu (saving and loading slots), lins_mapper_save.cu (saving and loading mapping nodes) — all bit-exact, so no multiply-add contraction: the association and the map
+# lins_projection.cu (image projection), lins_cloud2.cu (PointCloud2 decoding), lins_mapper.cu (the mapping node's cycle), lins_mappers.cu (many mapping nodes in lockstep), lins_loops.cu (their loop closure), lins_checkpoint.cu (saving and loading sequence-mode slots and mapping nodes) — all bit-exact, so no multiply-add contraction: the association and the map
 # fits depend on it — and lins_jacobian.cu (the tolerance-checked split Jacobian kernel: contraction allowed)
 UNITS = [("lins_gpu.cu", ["-fmad=false"]), ("lins_upload.cu", ["-fmad=false"]), ("lins_map.cu", ["-fmad=false"]),
          ("lins_seq.cu", ["-fmad=false"]), ("lins_features.cu", ["-fmad=false"]), ("lins_projection.cu", ["-fmad=false"]),
          ("lins_cloud2.cu", ["-fmad=false"]), ("lins_mapper.cu", ["-fmad=false"]), ("lins_mappers.cu", ["-fmad=false"]),
-         ("lins_loops.cu", ["-fmad=false"]), ("lins_seq_save.cu", ["-fmad=false"]),
-         ("lins_mapper_save.cu", ["-fmad=false"]), ("lins_jacobian.cu", [])]
+         ("lins_loops.cu", ["-fmad=false"]), ("lins_checkpoint.cu", ["-fmad=false"]), ("lins_jacobian.cu", [])]
 
 
 def build(force=False, verbose=False):
@@ -545,25 +544,13 @@ class LinsGpu:
         """Save the lockstep slots with mask[s] != 0: a list of M entries, each slot's blob (bytes, self-contained: it loads
         into a fresh lockstep slot or a fresh single mapper of any context of this library build) or None where the mask
         is 0.  The run is unchanged."""
-        m = self._mapper_mask(mask)
-        off = np.zeros(len(m) + 1, np.uint64)
-        self._ck(self.L.lins_gpu_mappers_save_size(self.h, ptr(m), ptr(off)))
-        buf = np.zeros(max(int(off[-1]), 1), np.uint8)
-        self._ck(self.L.lins_gpu_mappers_save(self.h, ptr(m), ptr(buf), ptr(off)))
-        return [buf[int(off[s]): int(off[s + 1])].tobytes() if m[s] else None for s in range(len(m))]
+        return self._save_blobs(self.L.lins_gpu_mappers_save_size, self.L.lins_gpu_mappers_save, self._mapper_mask(mask))
 
     def mappers_load(self, mask, blobs):
         """Load blobs[s] (bytes, as mappers_save or mapper_save returned it) into every lockstep slot with mask[s] != 0,
         each still fresh (no step since open / its last reset); blobs has M entries (None where the mask is 0).  All or
         nothing."""
-        m = self._mapper_mask(mask)
-        if len(blobs) != len(m):
-            raise ValueError(f"{len(blobs)} blobs, the run has {len(m)} slots")
-        parts = [bytes(blobs[s]) if m[s] else b"" for s in range(len(m))]
-        off = np.zeros(len(m) + 1, np.uint64)
-        off[1:] = np.cumsum([len(p) for p in parts])
-        buf = np.frombuffer(b"".join(parts) or b"\0", np.uint8)
-        self._ck(self.L.lins_gpu_mappers_load(self.h, ptr(m), ptr(buf), ptr(off)))
+        self._load_blobs(self.L.lins_gpu_mappers_load, self._mapper_mask(mask), blobs)
 
     def mapper_save(self):
         """The single mapper's blob (bytes)."""
@@ -730,24 +717,30 @@ class LinsGpu:
         """Save the slots with mask[s] != 0: a list of S entries, each slot's blob (bytes, self-contained: it can be
         written to a file alone and loaded into a fresh slot of any seq_open run of this library build) or None where the
         mask is 0.  The run is unchanged."""
-        m = self._slot_mask(mask)
-        off = np.zeros(self._seq_n + 1, np.uint64)
-        self._ck(self.L.lins_gpu_seq_save_size(self.h, ptr(m), ptr(off)))
-        buf = np.zeros(max(int(off[-1]), 1), np.uint8)
-        self._ck(self.L.lins_gpu_seq_save(self.h, ptr(m), ptr(buf), ptr(off)))
-        return [buf[int(off[s]): int(off[s + 1])].tobytes() if m[s] else None for s in range(self._seq_n)]
+        return self._save_blobs(self.L.lins_gpu_seq_save_size, self.L.lins_gpu_seq_save, self._slot_mask(mask))
 
     def seq_load(self, mask, blobs):
         """Load blobs[s] (bytes, as seq_save returned it) into every slot with mask[s] != 0, each still fresh (no step
         since seq_open / its last seq_restart); blobs has S entries (None where the mask is 0).  All or nothing."""
-        m = self._slot_mask(mask)
-        if len(blobs) != self._seq_n:
-            raise ValueError(f"{len(blobs)} blobs, the run has {self._seq_n} slots")
-        parts = [bytes(blobs[s]) if m[s] else b"" for s in range(self._seq_n)]
-        off = np.zeros(self._seq_n + 1, np.uint64)
+        self._load_blobs(self.L.lins_gpu_seq_load, self._slot_mask(mask), blobs)
+
+    def _save_blobs(self, save_size, save, m):
+        """seq_save / mappers_save through their C entries: each slot's blob, None where m is 0"""
+        off = np.zeros(len(m) + 1, np.uint64)
+        self._ck(save_size(self.h, ptr(m), ptr(off)))
+        buf = np.zeros(max(int(off[-1]), 1), np.uint8)
+        self._ck(save(self.h, ptr(m), ptr(buf), ptr(off)))
+        return [buf[int(off[s]): int(off[s + 1])].tobytes() if m[s] else None for s in range(len(m))]
+
+    def _load_blobs(self, load, m, blobs):
+        """seq_load / mappers_load through their C entry"""
+        if len(blobs) != len(m):
+            raise ValueError(f"{len(blobs)} blobs, the run has {len(m)} slots")
+        parts = [bytes(blobs[s]) if m[s] else b"" for s in range(len(m))]
+        off = np.zeros(len(m) + 1, np.uint64)
         off[1:] = np.cumsum([len(p) for p in parts])
         buf = np.frombuffer(b"".join(parts) or b"\0", np.uint8)
-        self._ck(self.L.lins_gpu_seq_load(self.h, ptr(m), ptr(buf), ptr(off)))
+        self._ck(load(self.h, ptr(m), ptr(buf), ptr(off)))
 
     def _slot_mask(self, mask):
         m = np.ascontiguousarray(mask, dtype=np.uint8)

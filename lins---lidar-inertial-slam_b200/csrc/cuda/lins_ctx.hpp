@@ -226,7 +226,7 @@ struct SeqState {
   std::vector<int> h_run_off;                          // 2 x (n + 1): the last step's compacted query offsets (surf, corner)
   SeqPubState pub;                                     // the publish step of a run bound to the lockstep mappers
   Buf<float4> blob; Buf<float4, kPinned> h_blob;       // lins_gpu_seq_save / _load: the slot blobs on the device and
-                                                       // their pinned staging (lins_seq_save.cu)
+                                                       // their pinned staging (lins_checkpoint.cu)
   ~SeqState() { for (cudaEvent_t e : ev) if (e) cudaEventDestroy(e); }
 };
 
@@ -461,7 +461,7 @@ struct MappersState {
   CopyList copies;                           // the local maps' concatenation, then the surf-total one
   LoopPass lp;                               // lins_gpu_mappers_close_loops
   Buf<float4> blob; Buf<float4, kPinned> h_blob;  // lins_gpu_mapper(s)_save / _load: the slot blobs on the device and
-                                                  // their pinned staging (lins_mapper_save.cu)
+                                                  // their pinned staging (lins_checkpoint.cu)
 };
 
 }  // namespace lins_capi
@@ -748,6 +748,9 @@ void mapper_node_fuse(const MapperNode& m, double time, const double quat[4], co
 void mapper_cycle_end(MapperNode& m, MapperScalars& s, double time, double scan_period, const int cnt[6], const lins_map::MapLoopState* st,
                       lins_mapper_report& r, KfSave* save, bool* saved);
 int keyframes_queue(lins_ctx* ctx, const KfSave* saves, int n, Buf<unsigned char>& dev, Buf<unsigned char, kPinned>& host);
+// lins_mapper.cu: the device store's slot of key frame id (its own, a free one, or a new one), sized for n points of each
+// cloud (a step's new key frame, a loaded one)
+MapperKeyFrame& store_keyframe(MapperNode& m, int id, const int n[3]);
 // lins_mapper.cu: a node's key poses, window and last cycle's clouds (src: its six DS clouds on the device; NULL skips)
 int mapper_node_download(lins_ctx* ctx, const MapperNode& m, const float4* const src[6], double* key_poses, int32_t* window, float* const dst[6]);
 // lins_mapper.cu: the non-empty copies of v through the gather list l, staged at entries base.. and run in one launch

@@ -321,20 +321,21 @@ void transform_update(MapperScalars& s, double timeLaserOdometry, double SCAN_PE
   }
 }
 
-// the slot of key frame id (a free one, or a new one)
-MapperKeyFrame& keyframe_slot(MapperNode& M, int id) {
-  auto it = M.slot_of.find(id);
-  if (it != M.slot_of.end()) return M.slots[it->second];
-  int s;
-  if (!M.free_slots.empty()) { s = M.free_slots.back(); M.free_slots.pop_back(); }
-  else { s = (int)M.slots.size(); M.slots.emplace_back(); }
-  M.slot_of[id] = s;
-  return M.slots[s];
-}
-
 }  // namespace
 
 namespace lins_capi {
+
+MapperKeyFrame& store_keyframe(MapperNode& M, int id, const int n[3]) {
+  auto it = M.slot_of.find(id);
+  int s;
+  if (it != M.slot_of.end()) s = it->second;
+  else if (!M.free_slots.empty()) { s = M.free_slots.back(); M.free_slots.pop_back(); }
+  else { s = (int)M.slots.size(); M.slots.emplace_back(); }
+  M.slot_of[id] = s;
+  MapperKeyFrame& f = M.slots[s];
+  std::copy(n, n + 3, f.n);
+  return f;
+}
 
 // the non-empty copies of a batch through the gather list, at entries base.. (two batches of one cycle do not overlap)
 int queue_copies(lins_ctx* ctx, CopyList& l, std::vector<DevCopy> v, int base) {
@@ -457,9 +458,8 @@ void mapper_cycle_end(MapperNode& M, MapperScalars& s, double timeLaserOdometry,
       for (int i = 0; i < 6; ++i) { s.transformLast[i] = s.transformAftMapped[i]; s.transformTobeMapped[i] = s.transformAftMapped[i]; }
     }
     // the key frame's clouds, in the map frame once (its pose changes only in correctPoses)
-    MapperKeyFrame& kf = keyframe_slot(M, id);
-    kf.n[0] = ndc; kf.n[1] = nds; kf.n[2] = ndo;
-    save->kf = &kf;
+    const int n[3] = {ndc, nds, ndo};
+    save->kf = &store_keyframe(M, id, n);
     save->kp = kp;
     *saved = true;
     r.keyframe_saved = 1;

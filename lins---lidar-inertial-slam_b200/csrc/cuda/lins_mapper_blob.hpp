@@ -1,40 +1,25 @@
 // lins_mapper_blob.hpp — the byte format of one saved mapping-node slot of the lockstep mappers or the single mapper
-// (lins_gpu_mappers_save / _load, lins_gpu_mapper_save / _load, lins_mapper_save.cu): its records, its layout and its
-// validation.  Plain C++ with no CUDA, so the CPU suite compiles it with g++ (tests/test_mapper_checkpoint_cpu.py).
-// One format for both APIs: a blob of either loads into the other.
-//
-// A blob is a header, then sections at 16-byte offsets in a fixed order, each sized by the counts of the scalar section
-// (so the section table is fully determined by them, and a loader checks it is exactly that):
-//   scalars   Scalars: the counts, then MapperLoops' closed, n_loop, cur and time
-//   mapper    lins_blob::MapperRec: the node's scalars and IMU queue
-//   poses     lins_blob::PoseRec per key pose
-//   window    int32 key-frame ids, oldest first (the deque as it is, its duplicate id included)
-//   keyframes lins_blob::KeyframeRec per stored key frame, by id
-//   kfclouds  each stored key frame's corner, surf and outlier clouds, in table order, as float4 runs: in the map frame
-//             (c) on a plain slot, in the body frame (b) on a slot with loop closure, whose loader rebuilds c = T(b, pose)
-//   loop      the scan-to-map loop state (the build's MapLoopState bytes)
-//   factors   FactorRec per factor of the key-pose graph, in its order (slots with loop closure)
-//   est       EstRec per key pose: isamCurrentEstimate of the last save (slots with loop closure)
-// The blob records the build's record sizes, and a build whose sizes differ rejects it.  The factor, estimate and
-// body-frame store sections are the graph and store of lins_capi::MapperLoops / MapperKeyFrame as they are, so that a
-// later sequence-mode format could carry a slot with loop closure in the same records.
+// (lins_gpu_mappers_save / _load, lins_gpu_mapper_save / _load, lins_checkpoint.cu): its records, its layout and its
+// validation, on the core of lins_blob.hpp.  One format for both APIs: a blob of either loads into the other.  Plain C++
+// with no CUDA, so the CPU suite compiles it with g++ (tests/test_mapper_checkpoint_cpu.py).
 #pragma once
-#include <cmath>
-#include <cstddef>
-#include <cstdint>
-#include <cstring>
-#include <vector>
-
-#include "../../../include/lins_gpu.h"
-#include "lins_slot_blob.hpp"
+#include "lins_blob.hpp"
 
 namespace lins_mblob {
 
-using lins_blob::align16;
+// Sections: scalars (Scalars: the counts, then MapperLoops' closed, n_loop, cur and time), the node's sections, factors
+// (a FactorRec per factor of the key-pose graph, in its order) and est (an EstRec per key pose: isamCurrentEstimate of
+// the last save).  A plain slot's kfclouds are in the map frame (c); a slot with loop closure keeps every key frame, in
+// the body frame (b), and its loader rebuilds c = T(b, pose) for those a later window can take.  The graph, estimate and
+// body-frame store sections are those of lins_capi::MapperLoops / HostKeyFrame as they are, so that a later
+// sequence-mode format could carry a slot with loop closure in the same records.
 using lins_blob::KeyframeRec;
 using lins_blob::MapperRec;
+using lins_blob::NodeSecs;
+using lins_blob::NodeView;
 using lins_blob::PoseRec;
 using lins_blob::SectionRec;
+using lins_blob::rec;
 
 constexpr uint64_t kMagic = 0x5250414d534e494cull;  // "LINSMAPR" in little-endian byte order
 constexpr uint32_t kVersion = 1;
@@ -90,29 +75,20 @@ inline void layout(const Counts& c, const BuildSizes& sz, Header& h) {
       sz.loop_state,
       sizeof(FactorRec) * uint64_t(c.n_factors),
       sizeof(EstRec) * uint64_t(c.n_est)};
-  uint64_t o = align16(sizeof(Header));
-  for (int i = 0; i < kNumSections; ++i) {
-    h.sec[i].off = o;
-    h.sec[i].bytes = bytes[i];
-    o = align16(o + bytes[i]);
-  }
-  h.total = o;
+  h.total = lins_blob::section_table(sizeof(Header), bytes, kNumSections, h.sec);
+}
+inline NodeSecs node_secs(const Header& h) {
+  return {h.sec[kMapper].off, h.sec[kPoses].off, h.sec[kWindow].off, h.sec[kKeyframes].off, h.sec[kKfClouds].off, h.sec[kLoop].off};
 }
 
-// a parsed blob: the header and scalar records copied out, the rest left in place (p: the blob's first byte; it need
-// not be aligned, so records are read with memcpy)
-struct View {
-  const uint8_t* p = nullptr;
+// a parsed blob: the header and scalar records copied out
+struct View : NodeView {
   Header h;
   Scalars sc;
-  MapperRec m;
   bool loops() const { return h.flags & kLoops; }
   const uint8_t* at(int section) const { return p + h.sec[section].off; }
-  PoseRec pose(int i) const { PoseRec r; std::memcpy(&r, at(kPoses) + sizeof(PoseRec) * i, sizeof(r)); return r; }
-  int32_t window(int i) const { int32_t r; std::memcpy(&r, at(kWindow) + sizeof(int32_t) * i, sizeof(r)); return r; }
-  KeyframeRec keyframe(int i) const { KeyframeRec r; std::memcpy(&r, at(kKeyframes) + sizeof(KeyframeRec) * i, sizeof(r)); return r; }
-  FactorRec factor(int i) const { FactorRec r; std::memcpy(&r, at(kFactors) + sizeof(FactorRec) * i, sizeof(r)); return r; }
-  EstRec est(int i) const { EstRec r; std::memcpy(&r, at(kEst) + sizeof(EstRec) * i, sizeof(r)); return r; }
+  FactorRec factor(int i) const { return rec<FactorRec>(at(kFactors), i); }
+  EstRec est(int i) const { return rec<EstRec>(at(kEst), i); }
 };
 
 inline bool finite_n(const double* v, int n) {
@@ -128,17 +104,9 @@ inline const char* parse(const uint8_t* p, uint64_t len, const BuildSizes& sz, V
   if (!p || len < sizeof(Header)) return "blob shorter than its header";
   std::memcpy(&v.h, p, sizeof(Header));
   const Header& h = v.h;
-  if (h.magic != kMagic) return "not a mapper blob (bad magic)";
-  if (h.version != kVersion) return "mapper blob of another format version";
-  if (std::memcmp(&h.sizes, &sz, sizeof(sz)) != 0) return "mapper blob of another library build (record sizes differ)";
-  if (h.flags & ~uint32_t(kLoops)) return "bad mapper blob flags";
-  if (h.n_sections != kNumSections || h.pad != 0) return "bad mapper blob section count";
-  if (h.total != len) return "mapper blob length differs from its header's";
-  for (int i = 0; i < kNumSections; ++i)
-    if (h.sec[i].off % 16 || h.sec[i].off < sizeof(Header) || h.sec[i].off > len || h.sec[i].bytes > len - h.sec[i].off)
-      return "mapper blob section outside the blob";
-  if (h.sec[kScalars].bytes != sizeof(Scalars)) return "bad mapper blob scalar section";
-  std::memcpy(&v.sc, v.at(kScalars), sizeof(Scalars));
+  if (const char* bad = lins_blob::check_envelope(h, len, "mapper", kMagic, kVersion, kLoops, sz, h.n_sections == kNumSections && h.pad == 0, sizeof(Scalars)))
+    return bad;
+  v.sc = rec<Scalars>(v.at(kScalars), 0);
   const Scalars& s = v.sc;
   const bool loops = v.loops();
   if (s.n_poses < 0 || s.n_window < 0 || s.n_keyframes < 0 || s.n_factors < 0 || s.n_est < 0 || s.n_loop < 0)
@@ -153,28 +121,17 @@ inline const char* parse(const uint8_t* p, uint64_t len, const BuildSizes& sz, V
   if (h.sec[kPoses].bytes != sizeof(PoseRec) * (uint64_t)s.n_poses || h.sec[kKeyframes].bytes != sizeof(KeyframeRec) * (uint64_t)s.n_keyframes ||
       h.sec[kFactors].bytes != sizeof(FactorRec) * (uint64_t)s.n_factors)
     return "bad mapper blob pose, key-frame or factor section";
+  v.node = node_secs(h);
+  v.n_poses = s.n_poses; v.n_window = s.n_window; v.n_keyframes = s.n_keyframes;
   Counts c;
   c.n_poses = s.n_poses; c.n_window = s.n_window; c.n_keyframes = s.n_keyframes; c.n_factors = s.n_factors; c.n_est = s.n_est;
-  std::vector<int32_t> ids(s.n_keyframes);
-  std::vector<unsigned char> seen(s.n_poses, 0);
-  for (int i = 0; i < s.n_keyframes; ++i) {
-    const KeyframeRec k = v.keyframe(i);
-    if (k.id < 0 || k.id >= s.n_poses) return "mapper blob key frame of no key pose";
-    if (seen[k.id]) return "mapper blob stores a key frame twice";
-    seen[k.id] = 1;
-    ids[i] = k.id;
-    for (int a = 0; a < 3; ++a) {
-      if (k.n[a] < 0) return "negative key-frame cloud count in mapper blob";
-      c.n_kf_points += k.n[a];
-    }
-  }
-  if (c.n_kf_points > INT32_MAX) return "mapper blob key-frame clouds too large";
+  std::vector<int32_t> ids;
+  if (const char* bad = lins_blob::check_keyframes(v, "mapper", ids, c.n_kf_points)) return bad;
   Header want;
   layout(c, sz, want);
   if (want.total != len || std::memcmp(want.sec, h.sec, sizeof(h.sec)) != 0) return "mapper blob section table differs from its counts";
-  std::memcpy(&v.m, v.at(kMapper), sizeof(MapperRec));
-  const char* bad = lins_blob::mapper_state_check(v.m, s.n_poses, s.n_window, [&](int i) { return v.window(i); }, ids.data(), s.n_keyframes);
-  if (bad) return bad;
+  v.m = rec<MapperRec>(v.at(kMapper), 0);
+  if (const char* bad = lins_blob::mapper_state_check(v, ids)) return bad;
   if (!loops) return nullptr;
   // a slot with loop closure keeps every key frame (correctPoses re-transforms them all), and an estimate per key pose
   if (s.n_keyframes != s.n_poses) return "mapper blob with loop closure lacks a key pose's key frame";

@@ -1,6 +1,6 @@
 // lins_mapper_tf.cuh — the key-frame store's transform (transformPointCloud :624-652 with the constants of
 // updateTransformPointCloudSinCos :609-622), shared by the units that fill the store and those that read a key frame's
-// map-frame clouds from its body-frame ones: lins_mapper.cu (a step's saved and corrected key frames), lins_mapper_save.cu
+// map-frame clouds from its body-frame ones: lins_mapper.cu (a step's saved and corrected key frames), lins_checkpoint.cu
 // (a loaded slot's device store rebuilt from its body-frame clouds) and lins_loops.cu (the history sub-maps and global
 // maps gathered from the host store).  All three are built with -fmad=false, so a point's transform is the same bits in
 // each: the invariant c = T(b, pose) that the device store, the loads and the gathers rely on.

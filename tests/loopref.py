@@ -3,7 +3,8 @@ detectLoopClosure :1043-1112, performLoopClosure :1114-1186, correctPoses :1767-
 library solves in place of iSAM2 (DESIGN.md §4.14).
 
 Rotation exponentials and logarithms come from scipy's Rotation, the 1-NN from scipy's cKDTree (its candidates
-re-ranked by the f32 distance the library computes, ties to the lower index), the rigid transform from Umeyama's SVD,
+re-ranked by the f32 distance the library computes, ties to the lower index) or, exactly, by brute force (nn1_exact),
+the rigid transform from Umeyama's SVD (or Horn's quaternion, for stability checks),
 and the graph's solve is a dense Gauss-Newton with central-difference Jacobians, so none of it shares
 code with the library's kernels or its host solver."""
 import math
@@ -148,6 +149,36 @@ def nn1(tree, tgt, p):
     return idx[rows, order], d[rows, order]
 
 
+def nn1_exact(tgt, p, chunk=1 << 22):
+    """Brute-force exact f32 1-NN of every point of p over all of tgt: ((dx^2 + dy^2) + dz^2) in f32, ties to the lower
+    target index, a distance that is not below FLT_MAX never taken (as the device's strict d < best from FLT_MAX).
+    -> (idx (-1: none), d (FLT_MAX: none), gap: sqrt(second best) - sqrt(best) in f64 (inf with fewer than two))."""
+    n, m = len(p), len(tgt)
+    idx, d, gap = np.full(n, -1, np.int64), np.full(n, F(np.finfo(F).max), F), np.full(n, np.inf)
+    if m == 0 or n == 0:
+        return idx, d, gap
+    q = np.asarray(tgt, F)[:, :3]
+    step = max(1, chunk // m)
+    for a in range(0, n, step):
+        s = np.asarray(p[a:a + step, :3], F)
+        dx, dy, dz = (q[None, :, k] - s[:, None, k] for k in range(3))
+        with np.errstate(over="ignore", invalid="ignore"):
+            dd = (dx * dx + dy * dy) + dz * dz
+            dd = np.where(dd < np.finfo(F).max, dd, F(np.inf))
+        i = np.argmin(dd, axis=1)  # (the first of equal minima: the lower index)
+        rows = np.arange(len(s))
+        b = dd[rows, i]
+        ok = np.isfinite(b)
+        idx[a:a + step] = np.where(ok, i, -1)
+        d[a:a + step] = np.where(ok, b, F(np.finfo(F).max))
+        if m > 1:
+            dd[rows, i] = np.inf
+            b2 = dd.min(1).astype(np.float64)
+            with np.errstate(invalid="ignore"):
+                gap[a:a + step] = np.where(ok, np.sqrt(b2) - np.sqrt(b.astype(np.float64)), np.inf)
+    return idx, d, gap
+
+
 def umeyama(s, t):
     ms, mt = s.mean(0), t.mean(0)
     Sg = (t - mt).T @ (s - ms) / len(s)
@@ -159,27 +190,61 @@ def umeyama(s, t):
     return R, mt - R @ ms
 
 
-def icp(src, tgt):
-    """-> dict(iters, converged, n_corr0, fitness, final (4 x 4 f32), corr0 (first iteration's 1-NN indices))."""
+def horn(s, t, reverse=False):
+    """The same optimum by Horn's quaternion (numpy.linalg.eigh of the 4 x 4 form) on the one-pass cross-covariance
+    sum s t^T - n ms mt^T, summed in reverse point order: a second solver and summation order for stability checks."""
+    if reverse:
+        s, t = s[::-1], t[::-1]
+    n = len(s)
+    ms, mt = np.sum(s, 0) / n, np.sum(t, 0) / n
+    H = np.einsum("ij,ik->jk", s, t) - n * np.outer(ms, mt)
+    (Sxx, Sxy, Sxz), (Syx, Syy, Syz), (Szx, Szy, Szz) = H
+    N = np.array([[Sxx + Syy + Szz, Syz - Szy, Szx - Sxz, Sxy - Syx],
+                  [Syz - Szy, Sxx - Syy - Szz, Sxy + Syx, Szx + Sxz],
+                  [Szx - Sxz, Sxy + Syx, -Sxx + Syy - Szz, Syz + Szy],
+                  [Sxy - Syx, Szx + Sxz, Syz + Szy, -Sxx - Syy + Szz]])
+    w, x, y, z = np.linalg.eigh(N)[1][:, -1]
+    R = Rotation.from_quat([x, y, z, w]).as_matrix()
+    return R, mt - R @ ms
+
+
+def icp(src, tgt, exact=False, solver="svd", reverse=False, trace=False):
+    """-> dict(iters, converged, n_corr0, fitness, final (4 x 4 f32), corr0 (first iteration's 1-NN indices)).
+    exact: the 1-NN by nn1_exact (else cKDTree's 8 nearest re-ranked, which can miss the f32 nearest among more than 8
+    near-equidistant targets); solver "svd" (Umeyama) or "horn"; reverse: the sums in reverse point order.  trace: also
+    "trace", per iteration dict(n_corr, mse, cos (the rotation criterion's cos_angle), tsq (the translation
+    criterion's squared norm), gap (per used correspondence: sqrt(second best) - sqrt(best) f32 distance, exact only),
+    near_limit (the distinct 1-NN distances within 1 m^2 of the 1e4 m^2 correspondence limit)),
+    and "stop": "ncorr" (fewer than 3 correspondences), "cap", "transform" or "mse"."""
     src = np.asarray(src, F)[keep_mask(np.asarray(src, F)[:, 3])]
     tgt = np.asarray(tgt, F)
-    out = dict(iters=0, converged=0, n_corr0=0, n_source=len(src), fitness=np.finfo(np.float64).max, final=np.eye(4, dtype=F), corr0=None)
+    out = dict(iters=0, converged=0, n_corr0=0, n_source=len(src), fitness=np.finfo(np.float64).max, final=np.eye(4, dtype=F), corr0=None,
+               trace=[], stop="ncorr")
     if len(tgt) == 0 or len(src) == 0:
         return out
-    tree = cKDTree(tgt[:, :3].astype(np.float64))
+    if exact:
+        nn = lambda p: nn1_exact(tgt, p)  # noqa: E731
+    else:
+        tree = cKDTree(tgt[:, :3].astype(np.float64))
+        nn = lambda p: nn1(tree, tgt, p) + (None,)  # noqa: E731
     fin = np.eye(4, dtype=F)[:3]
     cur = src.copy()
     prev_mse = np.finfo(np.float64).max
     it = 0
     while True:
-        idx, d = nn1(tree, tgt, cur)
-        ok = d <= F(1e4)
+        idx, d, gap = nn(cur)
+        ok = (idx >= 0) & (d <= F(1e4))
         if it == 0:
             out["n_corr0"], out["corr0"] = int(ok.sum()), np.where(ok, idx, -1)
+        found = d[idx >= 0]
+        rec = dict(n_corr=int(ok.sum()), gap=None if gap is None else gap[ok], near_limit=np.unique(found[np.abs(found.astype(np.float64) - 1e4) < 1.0]))
+        if trace:
+            out["trace"].append(rec)
         if ok.sum() < 3:
-            out["converged"] = 0
+            out["converged"], out["stop"] = 0, "ncorr"
             break
-        R, t = umeyama(cur[ok, :3].astype(np.float64), tgt[idx[ok], :3].astype(np.float64))
+        s64, t64 = cur[ok, :3].astype(np.float64), tgt[idx[ok], :3].astype(np.float64)
+        R, t = umeyama(s64, t64) if solver == "svd" else horn(s64, t64, reverse)
         T = np.concatenate([R, t[:, None]], 1).astype(F)
         cur = xf(T, cur)
         nf = np.zeros((3, 4), F)
@@ -191,16 +256,29 @@ def icp(src, tgt):
         it += 1
         cos_angle = 0.5 * float(F(F(F(T[0, 0] + T[1, 1]) + T[2, 2]) - F(1)))
         tsq = float(F(F(F(T[0, 3] * T[0, 3]) + F(T[1, 3] * T[1, 3])) + F(T[2, 3] * T[2, 3])))
-        mse = float(np.sum(d[ok].astype(np.float64))) / ok.sum()
-        if it >= MAX_ITER or (cos_angle >= 0.99999 and tsq <= 1e-6) or abs(mse - prev_mse) < 1e-12 or abs(mse - prev_mse) / prev_mse < 1e-6:
-            out["converged"] = 1
+        dk = d[ok].astype(np.float64)
+        mse = float(np.sum(dk[::-1] if reverse else dk)) / ok.sum()
+        rec.update(mse=mse, prev_mse=prev_mse, cos=cos_angle, tsq=tsq)
+        stop = "cap" if it >= MAX_ITER else "transform" if (cos_angle >= 0.99999 and tsq <= 1e-6) else \
+            "mse" if (abs(mse - prev_mse) < 1e-12 or abs(mse - prev_mse) / prev_mse < 1e-6) else None
+        if stop:
+            out["converged"], out["stop"] = 1, stop
             break
         prev_mse = mse
     out["iters"] = it
     out["final"] = np.concatenate([fin, np.array([[0, 0, 0, 1]], F)])
-    _, d = nn1(tree, tgt, xf(fin, src))
-    out["fitness"] = float(np.sum(d.astype(np.float64))) / len(d)
+    idx, d, _ = nn(xf(fin, src))
+    d = d[idx >= 0].astype(np.float64)
+    out["fitness"] = float(np.sum(d[::-1] if reverse else d)) / len(d) if len(d) else np.finfo(np.float64).max
     return out
+
+
+def fitness_of(final, src, tgt):
+    """getFitnessScore of a given final transform: the mean exact f32 1-NN distance of the kept source under it"""
+    src = np.asarray(src, F)[keep_mask(np.asarray(src, F)[:, 3])]
+    idx, d, _ = nn1_exact(np.asarray(tgt, F), xf(np.asarray(final, F)[:3], src))
+    d = d[idx >= 0].astype(np.float64)
+    return float(np.sum(d)) / len(d) if len(d) else np.finfo(np.float64).max
 
 
 # ---- detectLoopClosure's inputs and the loop factor ------------------------------------------------------------------
